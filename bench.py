@@ -1,8 +1,9 @@
 #!/usr/bin/env python
 """bench.py -- ICP scans/sec on BASELINE.json's headline configuration (cfg2), plus the other measured rows of SURVEY 8(d/e).
 
-    python bench.py --gpus N --steps K --warmup W            # this repo's sm_100a path (one process per GPU)
+    python bench.py --gpus N --steps K --warmup W            # this repo's sm_90a path (one process per GPU)
     python bench.py --impl reference --gpus N ...            # the reference's CPU path (oracle port + verbatim octree)
+    python bench.py ... --dump-outputs DIR                   # also write the last timed step's results as DIR/<name>.npy
 
 A "step" registers SUB x B independent OS1-128 scans per GPU (default 4 x 256 = 1024; 131 072 points each, drawn from 512
 distinct scans per GPU, consecutive sub-batches never repeat an input) against the 1 M-point warehouse map with up to 20 ICP
@@ -13,7 +14,7 @@ so_register_batch with HOST (pinned) scan buffers, H2D of the scans and D2H of t
 Ranks shard the scan list (no data-path collective): weak scaling.
 
 Extra blocks on the same JSON line (rank 0; all measured in this run):
-  roofline   k-NN kernel of the ICP step against the measured HBM peak, algorithmic bytes as SURVEY 8(d) defines them
+  roofline   k-NN kernel of the ICP step against the HBM peak (MEASURED_PEAKS.json, else the H100 data sheet), algorithmic bytes as SURVEY 8(d) defines them
   knn_cfg5   BASELINE configs[4]: 10 M queries, k = 5, 5 M-point map, queries split over the N GPUs: GB/s, fraction of peak
   cfg4       BASELINE configs[3] literally: 1024 distinct scans, fixed total, sharded over the N GPUs, one gather (strong scaling)
   wide_prior the same batch kernel path with +-0.5 m / +-5 deg priors (ICP iterations 4+ exercised)
@@ -42,9 +43,9 @@ CFG4_TOTAL = 1024
 DISTINCT = 512                                   # distinct scans per GPU behind the weak-scaling step (two calls' worth: consecutive calls never repeat an input)
 # SURVEY 8(d): algorithmic bytes of the k-NN = 16 B query read + k * 8 B result (u32 id + f32 d2) per query, + the map once.
 KNN_BYTES_PER_QUERY = 16 + 5 * 8
-# ncu --set full, dram__bytes_read.sum + dram__bytes_write.sum of ONE k_knn_scan launch / its queries (profiles/README.md says
-# which capture; None where no capture of the current kernel is committed)
-NCU_DRAM_BYTES_PER_QUERY = {"k_knn_scan": 76.8, "k_knn_fit": None}      # profiles/ncu_prof_r2t_metrics.csv: (26.78 MB read + 53.74 MB written) / 1 048 576 queries
+# measured DRAM bytes (read + written) of ONE launch / its queries; None: not measured on the H100 (no hardware-counter
+# profiler there), so the roofline reports algorithmic bytes only
+NCU_DRAM_BYTES_PER_QUERY = {"k_knn_scan": None, "k_knn_fit": None}
 
 
 def _peaks():
@@ -52,7 +53,7 @@ def _peaks():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "H100 SXM data sheet (HBM3 3.35 TB/s), not a measured figure"
 
 
 class ClockSampler(threading.Thread):
@@ -167,6 +168,17 @@ def make_inputs(first_scan: int, n_scans: int):
         except Exception as e:                                 # read-only or full /tmp: the cache is only a convenience
             print(f"[bench] input cache not written ({type(e).__name__}: {e})", file=sys.stderr)
     return map_xyzi, scans, np.stack(priors), np.stack(truths)
+
+
+def dump_outputs(path: str, res, gathered: np.ndarray) -> None:
+    """What the timed path hands its caller in the last timed step, as float64 .npy files (about 0.5 MB for 1024 scans):
+    the per-scan result structs of this rank in call order and the all-gathered result rows of every rank."""
+    rs = [r for rk in res for r in rk]
+    arrays = {"pose": [list(r.pose) for r in rs], "pose_opt": [list(r.pose_opt) for r in rs], "cov": [list(r.cov) for r in rs],
+              "status": [r.status for r in rs], "n_iterations": [r.n_iterations for r in rs], "gathered_rows": gathered}
+    os.makedirs(path, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(path, name + ".npy"), np.asarray(a, np.float64))
 
 
 def cfg5_queries(map_xyzi: np.ndarray, first: int, count: int, block: int = 125_000) -> np.ndarray:
@@ -351,6 +363,8 @@ def run_ours(args):
     if sampler:
         sampler.close()
     launches = ctx.kernel_launches()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, res, gathered.cpu().numpy())
     n_total = per_step * world
     value = n_total * args.steps / (ms * 1e-3)
 
@@ -447,7 +461,7 @@ def run_ours(args):
         per_q = NCU_DRAM_BYTES_PER_QUERY.get(kname)
         roofline = {"bound": "hbm", "kernel": kname, "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
                     "traffic": per_q * queries / max(n_k, 1) if per_q else None,
-                    "traffic_source": f"profiles/ (ncu --set full: dram__bytes_read.sum + dram__bytes_write.sum of one {kname} launch per query, scaled to this launch size)",
+                    "traffic_source": "measured DRAM bytes per query x queries of the launch" if per_q else "not measured",
                     "peak_source": peak_src, "launches_profiled": int(n_k), "avg_launch_ms": ms_k / max(n_k, 1),
                     "algorithmic_bytes_per_launch": alg_bytes / max(n_k, 1),
                     "algorithmic_bytes": "SURVEY 8(d): (16 B query + 5 x 8 B result) x queries of the launch + 16 B x map points once per launch",
@@ -672,7 +686,10 @@ def main():
     ap.add_argument("--no-cfg4", action="store_true")
     ap.add_argument("--no-cfg5", action="store_true")
     ap.add_argument("--no-live", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's per-scan results to DIR/<name>.npy (float64)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.impl == "reference":
         run_reference(args)
     else:

@@ -1,5 +1,5 @@
 /* =============================================================================
- * superodom_b200.h -- C ABI of the B200-native ICP registration hot path.
+ * superodom_b200.h -- C ABI of the H100-native (sm_90a) ICP registration hot path.
  *
  * This is the drop-in boundary for ONE path of superxslam/SuperOdom: the per-scan
  * registration in LidarSLAM::performLocalizationAndMapping.  The reference has no
@@ -22,7 +22,7 @@
  *   - one host thread per context, one context per GPU (the reference is
  *     non-reentrant: file-scope pose globals, LidarSlam.cpp:7-9).
  *   - there is NO CPU fallback: every entry point fails with SO_ERR_CUDA when no
- *     sm_100 device / kernel image is available.
+ *     sm_90 device / kernel image is available.
  * ============================================================================= */
 #ifndef SUPERODOM_B200_H
 #define SUPERODOM_B200_H
@@ -140,7 +140,7 @@ typedef struct {
 so_ctx* so_create(const so_config* cfg);
 void so_destroy(so_ctx* ctx);
 const char* so_last_error(void);
-/* 1 when a CUDA device of compute capability 10.x is usable by this library */
+/* 1 when a CUDA device of compute capability 9.x is usable by this library */
 int so_device_available(void);
 /* Use an externally owned CUDA stream (cudaStream_t as void*) for all work of this context; NULL = own stream. */
 int so_set_stream(so_ctx* ctx, void* cuda_stream);

@@ -3,7 +3,7 @@
 Used by the parity tests and bench.py; the reference's own host language is C++, whose binding is the header-only
 shim include/superodom_b200/LidarSlam.hpp.  No torch types cross this boundary: numpy arrays for host buffers,
 raw device pointers (ints) for the *_device entry points.  There is no CPU fallback: `Context()` raises if the
-shared library is missing or no sm_100 device is present.
+shared library is missing or no sm_90 device is present.
 """
 from __future__ import annotations
 

@@ -1,4 +1,4 @@
-"""Build the sm_100a shared library IN-TREE: superodom_b200/libsuperodom_b200.so (C ABI, no torch types)."""
+"""Build the sm_90a shared library IN-TREE: superodom_b200/libsuperodom_b200.so (C ABI, no torch types)."""
 from __future__ import annotations
 
 import os
@@ -9,7 +9,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.environ.get("SO_LIB_OUT") or os.path.join(HERE, "libsuperodom_b200.so")
 SOURCES = ["so_icp.cu", "so_map.cu", "so_scan.cu", "so_api.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 
 
@@ -41,7 +41,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         if p.returncode:
             raise RuntimeError(f"nvcc failed on {src}")
     # the arch flag also goes to the link step: without it nvcc adds an (empty) device-link stub for its default architecture
-    subprocess.check_call([nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB, *objs, "-lcudart"])
+    subprocess.check_call([nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", LIB, *objs, "-lcudart"])
     return LIB
 
 

@@ -621,7 +621,7 @@ int so_device_available(void) {
     if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) { cudaGetLastError(); return 0; }
     cudaDeviceProp p;
     if (cudaGetDeviceProperties(&p, 0) != cudaSuccess) { cudaGetLastError(); return 0; }
-    return p.major == 10 ? 1 : 0;
+    return p.major == 9 ? 1 : 0;
 }
 
 so_ctx* so_create(const so_config* cfg_in) {
@@ -635,7 +635,7 @@ so_ctx* so_create(const so_config* cfg_in) {
     if (cfg.device < 0 || cfg.device >= n) { set_error("bad device ordinal"); return nullptr; }
     cudaDeviceProp p;
     cudaGetDeviceProperties(&p, cfg.device);
-    if (p.major != 10) { set_error("device is not compute capability 10.x (kernels are built for sm_100a only)"); return nullptr; }
+    if (p.major != 9) { set_error("device is not compute capability 9.x (kernels are built for sm_90a only)"); return nullptr; }
     Ctx* c = new Ctx();
     c->device = cfg.device;
     c->cfg = cfg;

@@ -16,10 +16,9 @@ constexpr size_t kMaxChunks = 16;        // one upload event per chunk (Ctx::ev_
 //   chunk_override : that many equal chunks (SO_CHUNKS, tuning aid)
 //   host scans     : chunks that GROW -- 8, 16, 40, 64, then doubling (cumulative bounds 8, 24, 64, 128, 256, ...).  The one upload
 //                    nothing can hide is chunk 0's, so it is short; every later chunk is uploaded (copy stream, back to back) while
-//                    the chunks before it compute, and it can be large because that computing takes longer than its copy (a scan
-//                    costs ~90 us of kernels and ~40 us of PCIe).  Large chunks matter: the wide kernels of an 8- or 16-scan chunk
-//                    leave the GPU launch-bound (measured: 128 scans in 16 / 8 / 4 / 2 equal chunks run at 9 476 / ~10 400 /
-//                    10 775 / 11 027 scans/s device-resident).  No chunk but the first two is shorter than 8 scans.
+//                    the chunks before it compute, and it can be large because that computing takes longer than its copy.  On an
+//                    H100 80GB HBM3 (700 W limit, scripts/ab_step.py, 256-scan calls) this rule gives 7 805 scans/s end to end,
+//                    one chunk 6 078, 4 / 8 equal chunks 7 394 / 7 478.  No chunk but the first two is shorter than 8 scans.
 //   device scans   : two chunks (one per stream) from 16 scans on, else one.
 inline std::vector<uint32_t> chunk_bounds(size_t n_scans, bool host_input, bool profiling, int chunk_override) {
     std::vector<uint32_t> b;

@@ -1,4 +1,4 @@
-// so_icp.cu -- sm_100a kernels of the per-scan ICP registration path.
+// so_icp.cu -- sm_90a kernels of the per-scan ICP registration path.
 //
 //   k_scan_keys / k_scan_gather : order the scan by map cell once per registration (warp-coherent cell walks).
 //   k_knn_scan   : per scan point -- pose transform, block lookup, radius-bounded 5-NN in the sorted hash grid
@@ -1261,7 +1261,12 @@ __device__ __forceinline__ void evaluate_body_tma(const BatchView& bv, const Cor
             nd = sg.nd[threadIdx.x];
             sp = sg.sp[threadIdx.x];
             __syncthreads();                               // every thread holds its point: the stage may be refilled
-            if (threadIdx.x == 0 && r + kEvalStages < full) issue(r + kEvalStages);
+            if (threadIdx.x == 0 && r + kEvalStages < full) {
+                // the stage was just read through the generic proxy and is rewritten through the async (TMA) proxy:
+                // the two are ordered only by a proxy fence
+                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+                issue(r + kEvalStages);
+            }
         } else {
             if (cta0 + uint32_t(r) * kThreads >= n) break;
             if (i < n) {

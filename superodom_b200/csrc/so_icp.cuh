@@ -85,9 +85,9 @@ constexpr int kFitPts = SO_FIT_PTS;      // points per thread in k_fit
 #endif
 constexpr int kFitThreads = SO_FIT_THREADS;
 // 1: search and fit of a point run in one kernel (k_knn_fit); 0: k_knn_scan hands the neighbours to k_fit through HBM.
-// Measured on B200 (cfg2, 64 scans): fused 1.907 ms per matching stage vs 1.833 ms split (8 224 vs 8 508 scans/s) -- the stage
-// is issue-bound on the SUM of both halves' instructions (ncu: 223 M = 149 M + 82 M warp-instructions, 64 % issue-active either
-// way), so sharing an SM between search and fit warps buys nothing and the fused kernel spills a little more.  Split stays the
+// The stage is issue-bound on the SUM of both halves' instructions, so sharing an SM between search and fit warps buys little:
+// on an H100 80GB HBM3 (700 W limit, scripts/ab_knn.py, 64 cfg2 scans) fused 1.72 ms vs split 1.05 + 0.70 ms per matching stage
+// (2 %), and so_register_injected (the reference-octree parity proof) needs the split form.  Split stays the
 // default; the fused form saves 105 B/point of HBM traffic and the 80 B/point neighbour buffer.
 #ifndef SO_FUSE_KNN_FIT
 #define SO_FUSE_KNN_FIT 0

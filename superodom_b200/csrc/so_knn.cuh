@@ -157,9 +157,9 @@ struct GlobalGrid {
 };
 
 // SO_KNN_TILE = 1 builds the TMA-tiled search (brick query order, 128 queries per CTA, tile with global fallback); 0 (default) the
-// global-memory search (cell-linear query order, 256 queries per CTA).  MEASURED on B200 (cfg2, 16 scans = 2.1 M queries per launch;
-// cfg5 10 M queries): tiled 0.339 ms / 3.84 ms, same brick-ordered kernel without the tile 0.303 / 3.03 ms, cell-linear global
-// kernel 0.282 / 2.72 ms -- results bit-identical in all three.  The search is bound by per-candidate instructions (distance,
+// global-memory search (cell-linear query order, 256 queries per CTA).  Both give bit-identical results.  Measured on an H100 80GB HBM3
+// (700 W limit, scripts/ab_knn.py, 64 cfg2 scans = 8.4 M queries per launch): tiled 1.45 ms, global 1.05-1.07 ms per launch.
+// The search is bound by per-candidate instructions (distance,
 // min/max network, record), which a tile does not remove; what it removes (row headers: index arithmetic + two cell-table loads,
 // ~30 % of the instructions) is paid back by the tile build (box reduction, row scan, cell table, ~250 warp-instructions and eight
 // barriers per 128 queries, with the bulk-copy latency exposed at 6 CTAs per SM) and by the brick order, whose 8-cell runs
@@ -168,7 +168,7 @@ struct GlobalGrid {
 #define SO_KNN_TILE 0
 #endif
 #ifndef SO_KNN_THREADS
-#define SO_KNN_THREADS 64          // measured on B200: 256 -> 0.2825, 128 -> 0.2749, 64 -> 0.2729, 32 -> 0.2758 ms per 2.1 M scan queries; cfg5 2.718 / 2.587 / 2.585 / 2.650 ms
+#define SO_KNN_THREADS 64          // H100 (as above): 32 -> 1.08, 64 -> 1.05-1.07, 128 -> 1.07, 256 -> 1.11 ms per launch
 #endif
 constexpr int kTileThreads = SO_KNN_TILE ? 128 : SO_KNN_THREADS;      // queries per CTA of the search kernels
 #ifndef SO_TILE_PTS

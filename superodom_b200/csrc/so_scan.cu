@@ -1,4 +1,4 @@
-// so_scan.cu -- scan preparation in front of the registration path (SURVEY 8f row 2), sm_100a:
+// so_scan.cu -- scan preparation in front of the registration path (SURVEY 8f row 2), sm_90a:
 //   k_deskew          featureExtraction::removePointDistortion<BufferType> (src/FeatureExtraction/featureExtraction.cpp:222-314)
 //   k_uniform_flags / k_uniform_scatter
 //                     featureExtraction::uniformFeatureExtraction (:504-525)

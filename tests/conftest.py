@@ -10,7 +10,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run by the driver with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a real H100 (sm_90a); select with -m gpu")
 
 
 _cases = {}
@@ -40,7 +40,7 @@ def oracle_mod():
 def gpu_api():
     from superodom_b200 import api
     lib = api.load_library()          # raises if the extension is missing: no silent fallback
-    assert lib.so_device_available(), "no sm_100 device visible"
+    assert lib.so_device_available(), "no sm_90 device visible"
     return api
 
 

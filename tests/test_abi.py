@@ -1,4 +1,4 @@
-"""CPU-side checks of the drop-in boundary: the in-tree shared library builds for sm_100a, loads, exports every
+"""CPU-side checks of the drop-in boundary: the in-tree shared library builds for sm_90a, loads, exports every
 symbol include/superodom_b200.h declares, and refuses to work (loudly) without a GPU -- there is no CPU fallback."""
 import ctypes as C
 import os
@@ -35,9 +35,9 @@ def test_library_builds_and_exports_every_declared_symbol():
     for name in decl:
         assert hasattr(L, name), f"{name} declared in the header but not exported"
     assert sorted(api.EXPORTS) == decl, "python binding and header disagree on the ABI surface"
-    # SASS is sm_100a
+    # SASS is sm_90a
     out = subprocess.run(["cuobjdump", "--list-elf", lib_path], capture_output=True, text=True).stdout
-    assert "sm_100a" in out
+    assert "sm_90a" in out
 
 
 def test_struct_layouts_match_header(tmp_path):
@@ -72,8 +72,8 @@ def test_product_never_imports_the_oracle():
                     assert "so_oracle" not in txt and "from oracle" not in txt and "import oracle" not in txt, fn
 
 
-def test_library_holds_only_sm_100a_images():
-    """Write for B200 only: every device ELF inside the shared library is an sm_100a image (no other architecture, no PTX)."""
+def test_library_holds_only_sm_90a_images():
+    """Write for H100 only: every device ELF inside the shared library is an sm_90a image (no other architecture, no PTX)."""
     import shutil
     import subprocess
     from superodom_b200 import build
@@ -82,7 +82,7 @@ def test_library_holds_only_sm_100a_images():
         pytest.skip("cuobjdump not available")
     lib = build.build()
     elfs = [ln for ln in subprocess.run([tool, "-lelf", lib], capture_output=True, text=True).stdout.splitlines() if "ELF file" in ln]
-    assert elfs and all("sm_100a" in ln for ln in elfs), elfs
+    assert elfs and all("sm_90a" in ln for ln in elfs), elfs
     ptx = [ln for ln in subprocess.run([tool, "-lptx", lib], capture_output=True, text=True).stdout.splitlines() if "PTX file" in ln]
     assert not ptx, ptx
 

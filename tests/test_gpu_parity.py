@@ -1,4 +1,4 @@
-"""GPU parity tests: the sm_100a path, called through the C ABI, against the CPU oracle on identical inputs.
+"""GPU parity tests: the sm_90a path, called through the C ABI, against the CPU oracle on identical inputs.
 
 Bars (task section 3): bit-exact for integer / index work (neighbour ids, float d2, status codes, histograms,
 iteration counts); FP64 quantities within the stated tolerances (normal equations 1e-10 relative, pose 1e-4 m /
@@ -8,6 +8,7 @@ import ctypes as C
 import numpy as np
 import pytest
 
+import ref_octree_golden
 from conftest import get_case, quat_angle
 
 pytestmark = pytest.mark.gpu
@@ -56,8 +57,8 @@ def test_knn_bit_exact(gpu_api, oracle_mod, name):
         gi, gd = ctx.knn(q[:2000], k, 0.0)
         oi, od, of = om.knn(q[:2000], k, 0)
         assert np.array_equal(_gi(gi)[of], oi[of]) and np.array_equal(gd[of], od[of])
-    if name == "hall" and oracle_mod.has_ref_octree():    # reference's own octree (verbatim) agrees here
-        ri, rd, rf = om.knn(q[:-500], 5, 2)
+    if name == "hall":                                    # reference's own octree (verbatim, stored output) agrees here
+        ri, rd = ref_octree_golden.knn(om, "hall", q[:-500])
         gi, gd = ctx.knn(q[:-500], 5, 0.0)
         assert np.array_equal(_gi(gi), ri) and np.array_equal(gd, rd)
     ctx.close()
@@ -125,11 +126,11 @@ def test_register_pose_parity(gpu_api, oracle_mod, name, cap):
     assert np.linalg.norm(np.array(r.pose)[:3] - case["pose_true"][:3]) < 0.02
     r2 = ctx.register(case["scan_xyzi"], case["pose_prior"], cfg["max_iterations"], cap)
     assert np.array_equal(np.array(r.pose), np.array(r2.pose)) and np.array_equal(np.array(r.cov), np.array(r2.cov))
-    if name == "hall" and oracle_mod.has_ref_octree():
-        # the reference's own (verbatim) octree in the loop: same pose, because on this layout the octree is exact
-        rr = om.register(case["scan_xyzi"], case["pose_prior"], cfg["plane_res"], cfg["max_iterations"], cap, knn_mode=2)
-        _assert_pose_close(np.array(r.pose), np.array(rr.pose))
-        assert rr.n_iterations == r.n_iterations
+    if name == "hall":
+        # the reference's own (verbatim) octree in the loop (stored result): same pose, because on this layout the octree is exact
+        g = ref_octree_golden.load()
+        _assert_pose_close(np.array(r.pose), g["hall.pose"])
+        assert int(g["hall.n_iterations"]) == r.n_iterations
     ctx.close()
 
 

@@ -6,6 +6,7 @@ import os
 import numpy as np
 import pytest
 
+import ref_octree_golden
 from conftest import get_case, quat_angle
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
@@ -107,14 +108,12 @@ def test_reference_octree_pins_the_knn_restatement(oracle_mod):
     """Parity pin for SURVEY 8(c): where the verbatim reference octree is exact, the oracle's exact k-NN must equal
     it bit for bit (indices AND float distances).  Elsewhere the mismatch rate is reported."""
     O = oracle_mod
-    if not O.has_ref_octree():
-        pytest.skip("oracle/_ref not built (no /root/reference on this box and no prebuilt _ref)")
     xyzi = _x_dominant_map()
     m = O.OracleMap(xyzi)
     rng = np.random.default_rng(2)
     q = xyzi[::13, :3] + rng.normal(0, 0.1, size=xyzi[::13, :3].shape).astype(np.float32)
     i0, d0, _ = m.knn(q, 5, 0)
-    i2, d2, _ = m.knn(q, 5, 2)
+    i2, d2 = ref_octree_golden.knn(m, "xdom", q)           # the reference octree's output, stored
     assert np.array_equal(d0, d2)
     assert np.array_equal(i0, i2)
     # on the warehouse scene the octree is NOT exact (two reference bugs): report, and bound, the rate
@@ -122,7 +121,7 @@ def test_reference_octree_pins_the_knn_restatement(oracle_mod):
     m = O.OracleMap(c["map_xyzi"])
     q = c["map_xyzi"][::37, :3] + rng.normal(0, 0.1, size=c["map_xyzi"][::37, :3].shape).astype(np.float32)
     i0, d0, _ = m.knn(q, 5, 0)
-    i2, d2, _ = m.knn(q, 5, 2)
+    i2, d2 = ref_octree_golden.knn(m, "cfg1_warehouse", q)
     bad = int((np.sort(i0, 1) != np.sort(i2, 1)).any(1).sum())
     print(f"reference octree vs exact on cfg1 warehouse: {bad}/{len(q)} queries differ")
     assert bad < 0.02 * len(q)

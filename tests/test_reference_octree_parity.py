@@ -1,5 +1,6 @@
 """Parity against the reference's REAL k-NN path: nanoflann::Octree::knnNeighbors (flann/octree.h:1004-1055, called from
 LocalMap::nearestKSearchSurf, LocalMap.h:509-521), compiled verbatim into oracle/_ref, on the BASELINE configurations.
+Its outputs are stored under tests/golden (tests/ref_octree_golden.py), so these tests need no reference tree.
 
 The reference octree is not an exact k-NN (`inside()` tests x on all three axes, the root bbox update compares x against
 the y/z maxima and writes min[2] for max[2]: octree.h:383-385,984-1001); this library searches exactly inside the block
@@ -10,20 +11,17 @@ the y/z maxima and writes min[2] for max[2]: octree.h:383-385,984-1001); this li
       within the north-star tolerance (1e-4 m / 1e-4 rad; observed ~1e-12).  Hence the k-NN is the ONLY deviation.
   (B) BOUND: the deviation the exact search causes -- GPU exact vs octree-in-the-loop -- is recorded (mismatching queries,
       |dpos|, |drot|) and bounded (<= 5e-4 m / 5e-4 rad), and the exact result is not farther from ground truth than the
-      octree result beyond that bound.  The numbers are written to gpurun_out/octree_parity.json and printed.
+      octree result beyond that bound.  The numbers are printed.
 """
 import json
-import os
 
 import numpy as np
 import pytest
 
+import ref_octree_golden as R
 from conftest import get_case, quat_angle
 
 pytestmark = pytest.mark.gpu
-
-CASES = [("cfg1", 2000), ("cfg1", 0), ("cfg2", 0), ("cfg3", 0)]
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def _ctx(api, case):
@@ -33,80 +31,61 @@ def _ctx(api, case):
 
 
 def _record(key, row):
-    out = os.path.join(ROOT, "gpurun_out")
-    try:
-        os.makedirs(out, exist_ok=True)
-        path = os.path.join(out, "octree_parity.json")
-        data = {}
-        if os.path.exists(path):
-            with open(path) as f:
-                data = json.load(f)
-        data[key] = row
-        with open(path, "w") as f:
-            json.dump(data, f, indent=1, sort_keys=True)
-    except OSError:
-        pass
     print(f"[octree-parity] {key}: {json.dumps(row)}")
 
 
-@pytest.mark.parametrize("name,cap", CASES)
+@pytest.mark.parametrize("name,cap", R.TRACE_CASES)
 def test_injected_reference_octree_neighbours_reproduce_the_reference_path(gpu_api, oracle_mod, name, cap):
-    if not oracle_mod.has_ref_octree():
-        pytest.skip("oracle/_ref (reference octree compiled verbatim) not present")
     case = get_case(name)
     cfg = case["cfg"]
     scan, prior = case["scan_xyzi"], case["pose_prior"]
-    om = oracle_mod.OracleMap(case["map_xyzi"], ref_octree=True)
-    trace = np.zeros((cfg["max_iterations"], len(scan), 5), np.int64)
-    ro = om.register(scan, prior, cfg["plane_res"], cfg["max_iterations"], cap, knn_mode=2, n_threads=8, nn_trace=trace)
-    assert ro.status == 0
-    n = ro.n_iterations
+    om = oracle_mod.OracleMap(case["map_xyzi"])
+    ro, _, _, _ = R.register_result(om, name, case, cap)             # reference octree in the loop (stored)
+    trace = R.register_trace(om, name, case, cap)
+    assert ro["status"] == 0
+    n = ro["n_iterations"]
     ctx = _ctx(gpu_api, case)
     r = ctx.register_injected(scan, prior, cfg["max_iterations"], trace[:n], cap)
     assert r.status == 0
     # (A) identical control flow and counts, pose far inside the tolerance
     assert r.n_iterations == n
-    assert list(r.iter_n_surf[:n]) == list(ro.iter_n_surf[:n])
-    assert list(r.iter_lm_steps[:n]) == list(ro.iter_lm_steps[:n])
-    assert list(r.iter_lm_successful[:n]) == list(ro.iter_lm_successful[:n])
-    assert list(r.iter_lm_termination[:n]) == list(ro.iter_lm_termination[:n])
-    assert list(r.hist_obs) == list(ro.hist_obs) and list(r.hist_reject_plane) == list(ro.hist_reject_plane)
-    pg, po = np.array(r.pose), np.array(ro.pose)
+    assert list(r.iter_n_surf[:n]) == list(ro["iter_n_surf"])
+    assert list(r.iter_lm_steps[:n]) == list(ro["iter_lm_steps"])
+    assert list(r.iter_lm_successful[:n]) == list(ro["iter_lm_successful"])
+    assert list(r.iter_lm_termination[:n]) == list(ro["iter_lm_termination"])
+    assert list(r.hist_obs) == list(ro["hist_obs"]) and list(r.hist_reject_plane) == list(ro["hist_reject_plane"])
+    pg, po = np.array(r.pose), ro["pose"]
     dpos, drot = float(np.abs(pg[:3] - po[:3]).max()), float(quat_angle(pg[3:], po[3:]))
     assert dpos <= 1e-4 and drot <= 1e-4, (dpos, drot)
     assert dpos <= 1e-9 and drot <= 1e-7, ("expected ~1e-12: the stages after the search are the same arithmetic", dpos, drot)
-    assert np.allclose(r.iter_cost[:n], ro.iter_cost[:n], rtol=1e-9)
-    cg, co = np.array(r.cov).reshape(6, 6), np.array(ro.cov).reshape(6, 6)
+    assert np.allclose(r.iter_cost[:n], ro["iter_cost"], rtol=1e-9)
+    cg, co = np.array(r.cov).reshape(6, 6), ro["cov"].reshape(6, 6)
     assert np.abs(cg - co).max() <= 1e-6 * np.abs(co).max()
-    _record(f"{name}_cap{cap}_injected", {"icp_iterations": n, "dpos_m": dpos, "drot_rad": drot, "n_ok_last": int(ro.iter_n_surf[n - 1])})
+    _record(f"{name}_cap{cap}_injected", {"icp_iterations": n, "dpos_m": dpos, "drot_rad": drot, "n_ok_last": int(ro["iter_n_surf"][n - 1])})
     ctx.close()
 
 
-@pytest.mark.parametrize("name,cap", CASES)
+@pytest.mark.parametrize("name,cap", R.REGISTER_CASES)
 def test_exact_knn_deviation_from_reference_octree_is_bounded(gpu_api, oracle_mod, name, cap):
-    if not oracle_mod.has_ref_octree():
-        pytest.skip("oracle/_ref (reference octree compiled verbatim) not present")
     case = get_case(name)
     cfg = case["cfg"]
     scan, prior, truth = case["scan_xyzi"], case["pose_prior"], case["pose_true"]
-    om = oracle_mod.OracleMap(case["map_xyzi"], ref_octree=True)
-    ro = om.register(scan, prior, cfg["plane_res"], cfg["max_iterations"], cap, knn_mode=2, n_threads=8)      # reference octree in the loop
+    om = oracle_mod.OracleMap(case["map_xyzi"])
+    ro, status2, mism_rows, oc0 = R.register_result(om, name, case, cap)                                          # reference octree in the loop (stored)
     ctx = _ctx(gpu_api, case)
     r = ctx.register(scan, prior, cfg["max_iterations"], cap)                                                # exact in-block k-NN
-    assert r.status == 0 and ro.status == 0
-    pg, po = np.array(r.pose), np.array(ro.pose)
+    assert r.status == 0 and ro["status"] == 0
+    pg, po = np.array(r.pose), ro["pose"]
     dpos, drot = float(np.linalg.norm(pg[:3] - po[:3])), float(quat_angle(pg[3:], po[3:]))
     eg = float(np.linalg.norm(pg[:3] - truth[:3]))
     eo = float(np.linalg.norm(po[:3] - truth[:3]))
     # mismatch rate of the neighbour sets at the prior pose (first ICP iteration)
-    oc2, _, _ = om.correspond(scan, prior, cfg["plane_res"], cap, 2, n_threads=8)
-    oc0, _, _ = om.correspond(scan, prior, cfg["plane_res"], cap, 0, n_threads=8)
     searched = (oc0["status"] >= 0) & (oc0["status"] != 1)
-    mism = searched & (np.sort(oc2["nn"], 1) != np.sort(oc0["nn"], 1)).any(1)
-    gates = searched & (oc2["status"] != oc0["status"])
+    mism = searched & np.isin(np.arange(len(scan)), mism_rows)
+    gates = searched & (status2 != oc0["status"])
     row = {"queries": int(searched.sum()), "octree_wrong_neighbour_sets": int(mism.sum()), "mismatch_rate": float(mism.sum() / max(1, searched.sum())),
            "gate_flips": int(gates.sum()), "dpos_gpu_exact_vs_octree_m": dpos, "drot_rad": drot, "err_vs_truth_gpu_exact_m": eg,
-           "err_vs_truth_octree_m": eo, "icp_iterations_gpu": int(r.n_iterations), "icp_iterations_octree": int(ro.n_iterations)}
+           "err_vs_truth_octree_m": eo, "icp_iterations_gpu": int(r.n_iterations), "icp_iterations_octree": ro["n_iterations"]}
     _record(f"{name}_cap{cap}_exact_vs_octree", row)
     assert dpos <= 5e-4 and drot <= 5e-4, row
     assert eg <= eo + 5e-4, row
