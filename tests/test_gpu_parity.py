@@ -35,28 +35,96 @@ def _assert_pose_close(pg, po, tol_m=POSE_TOL_M, tol_r=POSE_TOL_RAD):
     assert quat_angle(pg[3:], po[3:]) <= tol_r, (pg, po)
 
 
-@pytest.mark.parametrize("name", ["tiny", "cfg1", "hall"])
-def test_knn_bit_exact(gpu_api, oracle_mod, name):
-    case = get_case(name)
-    ctx = _ctx(gpu_api, case)
-    om = oracle_mod.OracleMap(case["map_xyzi"])
+def _cell_faces(plane_res, lo, hi):
+    """float32 coordinates in [lo, hi) of the k-NN grid's cell faces (cell edge 50 / nb, nb = min(192, floor(100 / sqrt(3 planeRes)))
+    cells per 50 m block, DESIGN section 2), with the float32 neighbours on either side of each."""
+    nb = min(192, int(100.0 / np.sqrt(3.0 * np.float64(np.float32(plane_res)))))
+    j = np.arange(int(np.floor((lo + 25.0) * nb / 50.0)), int(np.ceil((hi + 25.0) * nb / 50.0)) + 1)
+    f = (-25.0 + j * (50.0 / nb)).astype(np.float32)
+    f = f[(f >= lo) & (f < hi)]
+    return f, np.nextafter(f, np.float32(-np.inf)), np.nextafter(f, np.float32(np.inf))
+
+
+def _knn_case(name):
+    """(map_xyzi, plane_res, queries) for test_knn_bit_exact.  lattice: voxel centres at planeRes spacing, a second lattice
+    whose planes lie on the grid's cell faces (and one float32 step either side), exact distance ties everywhere; queries on lattice
+    points, midpoints, faces and at random.  dense: clusters of 6-64 coincident or nearly coincident points, so that far more than
+    the 24 candidates the search buffers fall inside its bound."""
     rng = np.random.default_rng(0)
-    base = case["map_xyzi"][::7, :3]
-    q = base + rng.normal(0, 0.12, size=base.shape).astype(np.float32)
-    q = np.concatenate([q, rng.uniform(-30, 30, size=(500, 3)).astype(np.float32) + q.mean(0)])     # incl. far-away queries
+    if name not in ("lattice", "dense"):
+        case = get_case(name)
+        base = case["map_xyzi"][::7, :3]
+        q = base + rng.normal(0, 0.12, size=base.shape).astype(np.float32)
+        q = np.concatenate([q, rng.uniform(-30, 30, size=(500, 3)).astype(np.float32) + q.mean(0)])     # incl. far-away queries
+        return case["map_xyzi"], case["cfg"]["plane_res"], q
+    pr = 0.2
+    if name == "lattice":
+        g = (np.arange(-30, 30) + 0.5) * pr
+        a = np.stack(np.meshgrid(g, g, (np.arange(-3, 3) + 0.5) * pr, indexing="ij"), -1).reshape(-1, 3)
+        fx, fxm, fxp = _cell_faces(pr, 8.0, 12.0)
+        fz, fzm, fzp = _cell_faces(pr, -1.0, 1.0)
+        xs = np.concatenate([fx, fxm[::3], fxp[1::3]])
+        zs = np.concatenate([fz, fzm[::2], fzp[1::2]])
+        b = np.stack(np.meshgrid(xs, np.float32(fx - 20.0), zs, indexing="ij"), -1).reshape(-1, 3)
+        pts = np.concatenate([a.astype(np.float32), b.astype(np.float32)])
+        q = np.concatenate([pts[rng.choice(len(pts), 3000, replace=False)],
+                            (pts[rng.choice(len(a), 2000)] + np.float32(pr / 2) * rng.integers(0, 2, size=(2000, 3))).astype(np.float32),
+                            np.stack([rng.choice(fx, 2000), rng.uniform(-6, 6, 2000), rng.choice(fz, 2000)], 1).astype(np.float32),
+                            np.stack([rng.uniform(8, 12, 2000), rng.choice(np.float32(fx - 20.0), 2000), rng.uniform(-1, 1, 2000)], 1).astype(np.float32),
+                            rng.uniform(-7, 13, size=(2000, 3)).astype(np.float32) * np.float32([1, 1, 0.2])])
+    else:
+        cen = rng.uniform(-5, 5, size=(600, 3)) * [1, 1, 0.3]
+        pts = []
+        for i, c in enumerate(cen):
+            n = int(rng.integers(6, 65))
+            jit = [0.0, 1e-6, 1e-4, 1e-2][i % 4]
+            pts.append(c + rng.normal(0, jit, size=(n, 3)) if jit else np.repeat(c[None], n, 0))
+        pts = np.concatenate(pts).astype(np.float32)
+        q = np.concatenate([cen.astype(np.float32), (cen + rng.normal(0, 0.1, size=cen.shape)).astype(np.float32),
+                            ((cen[:-1] + cen[1:]) / 2).astype(np.float32), rng.uniform(-6, 6, size=(2000, 3)).astype(np.float32) * np.float32([1, 1, 0.3])])
+    xyzi = np.concatenate([pts, np.ones((len(pts), 1), np.float32)], 1)
+    return xyzi, pr, q
+
+
+@pytest.mark.parametrize("name", ["tiny", "cfg1", "hall", "lattice", "dense"])
+def test_knn_bit_exact(gpu_api, oracle_mod, name):
+    map_xyzi, pr, q = _knn_case(name)
+    ctx = gpu_api.Context(max_map_points=max(1 << 20, len(map_xyzi) + 1024), max_scan_points=262144, plane_res=pr)
+    ctx.map_set_points(map_xyzi)
+    om = oracle_mod.OracleMap(map_xyzi)
     gi, gd = ctx.knn(q, 5, 0.0)                           # exact, unbounded
     oi, od, of = om.knn(q, 5, 0)
     assert np.array_equal(_gi(gi)[of], oi[of]) and np.array_equal(gd[of], od[of])
     assert (gi[~of] == 0xFFFFFFFF).all()
-    bound = np.float32(3 * np.float32(case["cfg"]["plane_res"]))
+    bound = np.float32(3 * np.float32(pr))
     gi, gd = ctx.knn(q, 5, float(bound))                  # radius-bounded: same neighbours up to the bound
     keep = od <= bound
     assert np.array_equal(_gi(gi)[keep & of[:, None]], oi[keep & of[:, None]])
     assert (gi[~keep | ~of[:, None]] == 0xFFFFFFFF).all()
-    for k in (1, 3, 8):
-        gi, gd = ctx.knn(q[:2000], k, 0.0)
-        oi, od, of = om.knn(q[:2000], k, 0)
-        assert np.array_equal(_gi(gi)[of], oi[of]) and np.array_equal(gd[of], od[of])
+    import torch
+    qs = q if name in ("lattice", "dense") else q[:2000]
+    for k in range(1, 9):
+        gi, gd = ctx.knn(qs, k, 0.0)
+        oi, od, of = om.knn(qs, k, 0)
+        assert np.array_equal(_gi(gi)[of], oi[of]) and np.array_equal(gd[of], od[of]), k
+        if name in ("lattice", "dense"):
+            assert of.all()
+            gi, gd = ctx.knn(qs, k, float(bound))
+            keep = od <= bound
+            assert np.array_equal(_gi(gi)[keep], oi[keep]) and np.array_equal(gd[keep], od[keep]) and (gi[~keep] == 0xFFFFFFFF).all(), k
+        # so_knn_device (device-resident queries and results) returns the same bits as so_knn
+        for b in (0.0, float(bound)):
+            hi, hd = ctx.knn(qs, k, b)
+            dq = torch.from_numpy(np.concatenate([qs, np.ones((len(qs), 1), np.float32)], 1)).cuda()      # float4 queries
+            di = torch.empty((len(qs), k), dtype=torch.int32, device="cuda")
+            dd = torch.empty((len(qs), k), dtype=torch.float32, device="cuda")
+            ctx.knn_device(dq.data_ptr(), len(qs), k, b, di.data_ptr(), dd.data_ptr())
+            torch.cuda.synchronize()
+            assert np.array_equal(di.cpu().numpy().view(np.uint32), hi) and np.array_equal(dd.cpu().numpy(), hd), (k, b)
+    if name == "dense":                # the search buffers 24 candidates inside its bound and inserts the rest directly: reached here
+        _, od5, _ = om.knn(q[:600], 5, 0)
+        inside = ((map_xyzi[None, :, :3].astype(np.float64) - q[:600, None, :]) ** 2).sum(-1) <= od5[:, 4:5] * 1.001
+        assert (inside.sum(1) > 24).sum() > 100
     if name == "hall":                                    # reference's own octree (verbatim, stored output) agrees here
         ri, rd = ref_octree_golden.knn(om, "hall", q[:-500])
         gi, gd = ctx.knn(q[:-500], 5, 0.0)
@@ -267,6 +335,72 @@ def test_batch_equals_singles(gpu_api):
     for a, b in zip(singles, res2):
         assert np.array_equal(np.array(a.pose), np.array(b.pose))
     ctx.close()
+
+
+# Scan sizes of the boundary-size batch: 1 / 4 / 16 points per evaluation thread switch at 4 096 / 65 536 points, a TMA ring stage
+# is refilled above 4 096 points per CTA, and a scan whose first point sits at an odd offset takes the generic-load fallback.
+# Eighteen scans form two chunks of nine, so both chunks evaluate through the TMA ring, while a single registration takes the fused
+# plain-load kernel.  Offsets alternate in parity; 65 536 and 100 001 sit behind odd-sized scans at odd offsets; one scan is empty.
+_BATCH_SIZES = [1, 4097, 256, 65537, 255, 4096, 257, 65536, 0, 4095, 3, 100001, 2, 65535, 1000, 7, 131072, 511]
+
+
+def _result_bits(r):
+    """pose, pose_opt, cov, status, iteration count, the per-iteration arrays and the histograms as raw bytes (NaN-safe)"""
+    return np.array(list(r.pose) + list(r.pose_opt) + list(r.cov) + [r.status, r.n_iterations] + list(r.iter_n_surf) + list(r.iter_dtrans)
+                    + list(r.iter_drot) + list(r.iter_lm_steps) + list(r.iter_lm_successful) + list(r.iter_lm_termination)
+                    + list(r.iter_cost) + list(r.hist_obs) + list(r.hist_reject_plane), np.float64).tobytes()
+
+
+def test_batch_equals_singles_at_boundary_sizes(gpu_api, oracle_mod, monkeypatch):
+    """test_batch_equals_singles at every evaluation granularity: 18 scans cut from the cfg2 scan (_BATCH_SIZES), each bit-equal to
+    its single so_register in every recorded field -- host batch, device batch, repeated calls, a fresh context, one stream."""
+    case0 = get_case("cfg2")
+    full = case0["scan_xyzi"]
+    scans, poses = [], []
+    for i, n in enumerate(_BATCH_SIZES):
+        start = (i * 7919) % (len(full) - n + 1)
+        scans.append(full[start:start + n])
+        poses.append(case0["pose_prior"])
+    offs = np.cumsum([0] + _BATCH_SIZES[:-1])
+    big = np.array(_BATCH_SIZES) > 4096
+    assert (offs[big] % 2 == 1).any() and (offs[big] % 2 == 0).any()
+    ctx = _ctx(gpu_api, case0, max_batch=len(scans))
+    singles = [ctx.register(s, p, 5, skip_map_checks=True) for s, p in zip(scans, poses)]
+    want = [_result_bits(a) for a in singles]
+    assert sum(a.status == 0 for a in singles) >= 8
+    flat = np.ascontiguousarray(np.concatenate(scans, 0))
+    res = ctx.register_batch(flat, [len(s) for s in scans], np.stack(poses), 5, skip_map_checks=True)
+    for i, b in enumerate(res):
+        assert _result_bits(b) == want[i], ("host batch", i, _BATCH_SIZES[i])
+    import torch
+    d = torch.from_numpy(flat).cuda()
+    res2 = ctx.register_batch_device(d.data_ptr(), [len(s) for s in scans], np.stack(poses), 5, skip_map_checks=True)
+    for i, b in enumerate(res2):
+        assert _result_bits(b) == want[i], ("device batch", i, _BATCH_SIZES[i])
+    for rep in range(2):
+        res3 = ctx.register_batch(flat, [len(s) for s in scans], np.stack(poses), 5, skip_map_checks=True)
+        assert [_result_bits(b) for b in res3] == want, ("repeat", rep)
+    # the single-scan normal equations at the ring's boundary sizes against the oracle
+    om = oracle_mod.OracleMap(case0["map_xyzi"], ref_octree=False)
+    pr = case0["cfg"]["plane_res"]
+    for i in (_BATCH_SIZES.index(4097), _BATCH_SIZES.index(65537), _BATCH_SIZES.index(131072)):
+        ctx.correspond(scans[i], poses[i], 0)
+        H, g, cost = ctx.evaluate(poses[i])
+        oc, _, _ = om.correspond(scans[i], poses[i], pr, 0, 0, n_threads=8)
+        oH, og, ocost, _ = oracle_mod.evaluate(oc, poses[i], pr)
+        assert np.abs(H - oH).max() <= 1e-10 * np.abs(oH).max(), _BATCH_SIZES[i]
+        assert np.abs(g - og).max() <= 1e-10 * max(np.abs(og).max(), 1e-3 * np.abs(oH).max()), _BATCH_SIZES[i]
+        assert abs(cost - ocost) <= 1e-10 * ocost, _BATCH_SIZES[i]
+    ctx.close()
+    for env in (None, "SO_SINGLE_STREAM"):              # a fresh context, then a fresh one scheduling both chunks on one stream
+        if env:
+            monkeypatch.setenv(env, "1")
+        ctx = _ctx(gpu_api, case0, max_batch=len(scans))
+        res4 = ctx.register_batch(flat, [len(s) for s in scans], np.stack(poses), 5, skip_map_checks=True)
+        ctx.close()
+        assert [_result_bits(b) for b in res4] == want, env
+        if env:
+            monkeypatch.delenv(env)
 
 
 def test_full_size_properties_cfg2(gpu_api, oracle_mod):
