@@ -890,8 +890,8 @@ __global__ void __launch_bounds__(kThreads) k_knn_inject(MapView m, const float4
     for (int j = 0; j < 5; ++j) nb.pos[size_t(j) * nb.cap + gi] = 0xFFFFFFFFu;
 }
 
-// A 16-byte global load the compiler may neither merge with an earlier load of the same address nor hoist: k_fit re-reads
-// its neighbours (L1 hits) rather than keeping them live in registers.
+// A 16-byte global load the compiler may neither merge with an earlier load of the same address nor hoist: k_knn_fit (and
+// k_fit built with SO_FIT_NBD_SMEM=0) re-reads its neighbours (L1 hits) rather than keeping them live in registers.
 __device__ __forceinline__ float4 ld_f4_again(const float4* p) {
     float4 v;
     asm volatile("ld.global.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p));
@@ -903,13 +903,32 @@ __device__ __forceinline__ float4 ld_f4_again(const float4* p) {
 // neighbours k_knn_scan handed over: fit_point() below + the per-scan histograms.  The first residual/Jacobian evaluation of
 // the following ceres::Solve is a separate k_evaluate<PH_CORR> launch, which keeps this kernel at 64 registers.
 // ------------------------------------------------------------------------------------------------------------------
+// Shared-memory load the compiler may not replace by the value stored earlier: k_fit keeps its neighbours' FP64 coordinates
+// in shared memory rather than live in registers across the eigen-solve.
+__device__ __forceinline__ double ld_shared_again(const double* p) {
+    double v;
+    asm volatile("ld.shared.f64 %0, [%1];" : "=d"(v) : "r"(uint32_t(__cvta_generic_to_shared(p))));
+    return v;
+}
+
 // The rest of LidarSLAM::ComputePlaneDistanceParameters (LidarSlam.cpp:536-572) for one scan point whose k-NN outcome is
 // `status`: PCA, plane fit, gates, observability labels, fit weight; writes the correspondence record and counts the
-// histograms.  nbr(j) re-reads neighbour j (a volatile, L1-hit load: the neighbours are read three times rather than held in
-// 30 FP64 registers across the eigen-solve).  FP64 throughout.
-template <class NbrLoad>
+// histograms.  FP64 throughout.  nbr(j) loads neighbour j.  The fit reads the neighbours three more times after the mean
+// (scatter, QR, plane distances) and does not hold them in 30 FP64 registers across the eigen-solve: with STRIDE > 0 the first
+// pass widens each coordinate once and parks it in shared memory (nbd[(3 j + k) * STRIDE], this thread's column), and the
+// later passes load it from there; with STRIDE == 0 every pass calls nbr(j) again and widens afresh (float -> double
+// conversions run at a quarter of the FP64 rate).
+template <int STRIDE, class NbrLoad>
 __device__ __forceinline__ void fit_point(const MapView& m, const CorrBuf& cb, const NnBuf& nb, size_t gi, const float4 sp, const double* s_pose,
-                                          int status, NbrLoad nbr, int* s_hist) {
+                                          int status, NbrLoad nbr, double* nbd, int* s_hist) {
+    auto nbr_d = [&](int j, double& x, double& y, double& z) {
+        if constexpr (STRIDE > 0) {
+            x = ld_shared_again(nbd + (3 * j + 0) * STRIDE); y = ld_shared_again(nbd + (3 * j + 1) * STRIDE); z = ld_shared_again(nbd + (3 * j + 2) * STRIDE);
+        } else {
+            const float4 c = nbr(j);
+            x = double(c.x); y = double(c.y); z = double(c.z);
+        }
+    };
     int o0 = 0, o1 = 0, o2 = 0;
     double nrm[3] = {0, 0, 0}, dpl = 0.0, wq = 0.0;
     if (status == SO_MATCH_SUCCESS) {
@@ -919,26 +938,30 @@ __device__ __forceinline__ void fit_point(const MapView& m, const CorrBuf& cb, c
         qrot(s_pose + 3, pin, pf);
         pf[0] += s_pose[0]; pf[1] += s_pose[1]; pf[2] += s_pose[2];
         const float qx = float(pf[0]), qy = float(pf[1]), qz = float(pf[2]);
-        // computePCAForFeature (:749-790) + utils::ComputePCA (superodom_utils.h:143-151).  The five neighbours are read
-        // three times (here, for the QR, for the distances) through nbr() instead of being held in 30 FP64 registers across
-        // the eigen-solve: the re-reads hit L1 and the kernel fits 4 CTAs per SM.
+        // computePCAForFeature (:749-790) + utils::ComputePCA (superodom_utils.h:143-151)
         double mean[3] = {0, 0, 0};
 #pragma unroll
         for (int j = 0; j < 5; ++j) {
             const float4 c = nbr(j);
-            mean[0] += double(c.x); mean[1] += double(c.y); mean[2] += double(c.z);
+            const double x = double(c.x), y = double(c.y), z = double(c.z);
+            if constexpr (STRIDE > 0) { nbd[(3 * j + 0) * STRIDE] = x; nbd[(3 * j + 1) * STRIDE] = y; nbd[(3 * j + 2) * STRIDE] = z; }
+            mean[0] += x; mean[1] += y; mean[2] += z;
             if (cb.nn) {
                 const float dx = qx - c.x, dy = qy - c.y, dz = qz - c.z;
                 cb.nn[gi * 5 + j] = __float_as_uint(c.w);
                 cb.nn_d2[gi * 5 + j] = float(double(dx) * double(dx) + double(dy) * double(dy) + double(dz) * double(dz));
             }
         }
-        mean[0] /= 5.0; mean[1] /= 5.0; mean[2] /= 5.0;        // utils::ComputePCA divides (superodom_utils.h:146): the eigenvalue gates below read this
+        // mean /= 5, as utils::ComputePCA divides (superodom_utils.h:146): the eigenvalue gates below read it.  The division by
+        // the reciprocal 0.2 = RN(1/5) gives the same bits (div_rcp): a sum of five floats is +0 (exact through div_rcp) or in
+        // [2^-149, 2^131], inside div_rcp_ok's range.
+        mean[0] = div_rcp(mean[0], 5.0, 0.2); mean[1] = div_rcp(mean[1], 5.0, 0.2); mean[2] = div_rcp(mean[2], 5.0, 0.2);
         double S[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
 #pragma unroll
         for (int j = 0; j < 5; ++j) {
-            const float4 c = nbr(j);
-            const double c0 = double(c.x) - mean[0], c1 = double(c.y) - mean[1], c2 = double(c.z) - mean[2];
+            double x, y, z;
+            nbr_d(j, x, y, z);
+            const double c0 = x - mean[0], c1 = y - mean[1], c2 = z - mean[2];
             S[0] += c0 * c0; S[1] += c0 * c1; S[2] += c0 * c2; S[4] += c1 * c1; S[5] += c1 * c2; S[8] += c2 * c2;
         }
         S[3] = S[1]; S[6] = S[2]; S[7] = S[5];
@@ -978,33 +1001,35 @@ __device__ __forceinline__ void fit_point(const MapView& m, const CorrBuf& cb, c
                 double A[5][3], b[5];
 #pragma unroll
                 for (int j = 0; j < 5; ++j) {
-                    const float4 c = nbr(j);
-                    A[j][0] = double(c.x); A[j][1] = double(c.y); A[j][2] = double(c.z); b[j] = -1.0;
+                    nbr_d(j, A[j][0], A[j][1], A[j][2]);
+                    b[j] = -1.0;
                 }
                 colpiv_qr_solve_5x3(A, b, x);
             }
             if (!(isfinite(x[0]) && isfinite(x[1]) && isfinite(x[2]))) status = SO_MATCH_INVALID_NUMERICAL;
             else {
                 // negative_OA_dot_norm = 1 / norm.norm(); norm.normalize()  (:812-816): square root and divisions as written there,
-                // because the planeRes/2 gate below reads both
+                // because the planeRes/2 gate below reads both.  dd is RN(1/nn), so x / nn may be taken as div_rcp(x, nn, dd).
                 const double nn = sqrt(x[0] * x[0] + x[1] * x[1] + x[2] * x[2]);
                 const double dd = 1.0 / nn;
-                x[0] /= nn; x[1] /= nn; x[2] /= nn;
+#pragma unroll
+                for (int k = 0; k < 3; ++k) x[k] = div_rcp_ok(x[k], nn) ? div_rcp(x[k], nn, dd) : x[k] / nn;
                 const double maxd = double(m.plane_res) / 2.0;
                 double msum = 0.0;
                 bool ok = true;
 #pragma unroll
                 for (int j = 0; j < 5; ++j) {
-                    const float4 c = nbr(j);
-                    const double dist = fabs(x[0] * double(c.x) + x[1] * double(c.y) + x[2] * double(c.z) + dd);
+                    double cx, cy, cz;
+                    nbr_d(j, cx, cy, cz);
+                    const double dist = fabs(x[0] * cx + x[1] * cy + x[2] * cz + dd);
                     if (ok && dist > maxd) ok = false;
                     msum += dist;
                 }
                 if (!ok) status = SO_MATCH_MSE_TOO_LARGE;
                 else {
-                    const double mean_dist = msum / 5.0;
+                    const double mean_dist = div_rcp_ok(msum, 5.0) ? div_rcp(msum, 5.0, 0.2) : msum / 5.0;
                     const float fq[4] = {float(s_pose[3]), float(s_pose[4]), float(s_pose[5]), float(s_pose[6])};
-                    float rotq[6], trq[3];
+                    float rcq[3], trq[3];          // rotation scores +rc_a / -rc_a, translation scores; indexed by constants only
 #pragma unroll
                     for (int a = 0; a < 3; ++a) {
                         // computeRotatedAxes (:624-638): float quaternion * e_a, no FMA contraction (host code is plain IEEE)
@@ -1018,7 +1043,7 @@ __device__ __forceinline__ void fit_point(const MapView& m, const CorrBuf& cb, c
                         const float az = __fadd_rn(__fadd_rn(v2, __fmul_rn(fq[3], uz)), __fsub_rn(__fmul_rn(fq[0], uy), __fmul_rn(fq[1], ux)));
                         // Eigen's unrolled 3-vector dot associates as a0*b0 + (a1*b1 + a2*b2)
                         const float rc = __fadd_rn(__fmul_rn(cr[0], ax), __fadd_rn(__fmul_rn(cr[1], ay), __fmul_rn(cr[2], az)));
-                        rotq[2 * a] = rc; rotq[2 * a + 1] = -rc;
+                        rcq[a] = rc;
                         const float dn = __fadd_rn(__fmul_rn(nf[0], ax), __fadd_rn(__fmul_rn(nf[1], ay), __fmul_rn(nf[2], az)));
                         trq[a] = __fmul_rn(planar_sq, fabsf(dn));
                     }
@@ -1026,21 +1051,26 @@ __device__ __forceinline__ void fit_point(const MapView& m, const CorrBuf& cb, c
                     // scores are {+rc_a, -rc_a}, a = 0..2, so the largest is +|rc_a| of the axis with the largest magnitude (first axis
                     // on ties, as the stable sort keeps index order; index 2a for rc_a >= 0, 2a+1 below) and the runner-up the same
                     // among the other two axes -- unless every score is zero (or the winner's is NaN), when index order decides: 0, 1.
-                    const float m0 = fabsf(rotq[0]), m1 = fabsf(rotq[2]), m2 = fabsf(rotq[4]);
+                    // (Scores picked by selects, not by a computed index: an array indexed at run time lives in local memory.)
+                    const float m0 = fabsf(rcq[0]), m1 = fabsf(rcq[1]), m2 = fabsf(rcq[2]);
                     int a0 = 0; float mb = m0;
                     if (m1 > mb) { a0 = 1; mb = m1; }
                     if (m2 > mb) { a0 = 2; mb = m2; }
                     const int b0 = a0 == 0 ? 1 : 0, b1 = a0 == 2 ? 1 : 2;             // the other two axes, ascending
                     const float mb0 = a0 == 0 ? m1 : m0, mb1 = a0 == 2 ? m1 : m2;
                     const int a1 = mb1 > mb0 ? b1 : b0;
-                    const int r0 = 2 * a0 + (rotq[2 * a0] < 0.f ? 1 : 0);
-                    const int r1 = (mb > 0.f) ? 2 * a1 + (rotq[2 * a1] < 0.f ? 1 : 0) : 1;
+                    const float rc_a0 = a0 == 0 ? rcq[0] : (a0 == 1 ? rcq[1] : rcq[2]), rc_a1 = a1 == 0 ? rcq[0] : (a1 == 1 ? rcq[1] : rcq[2]);
+                    const int r0 = 2 * a0 + (rc_a0 < 0.f ? 1 : 0);
+                    const int r1 = (mb > 0.f) ? 2 * a1 + (rc_a1 < 0.f ? 1 : 0) : 1;
                     int t0 = 0;
-#pragma unroll
-                    for (int q = 1; q < 3; ++q) if (trq[q] > trq[t0]) t0 = q;
+                    float tb = trq[0];
+                    if (trq[1] > tb) { t0 = 1; tb = trq[1]; }
+                    if (trq[2] > tb) t0 = 2;
                     o0 = r0; o1 = r1; o2 = 6 + t0;
                     nrm[0] = x[0]; nrm[1] = x[1]; nrm[2] = x[2]; dpl = dd;
-                    wq = 1.0 - sqrt(mean_dist / double(m.bound_d2));     // fitQualityCoeff = 1 - sqrt(meanDist / (3*planeRes_)) (:568)
+                    // fitQualityCoeff = 1 - sqrt(meanDist / (3*planeRes_)) (:568); the map's inv_bound_d2 is RN(1 / bound_d2)
+                    const double bd2 = double(m.bound_d2);
+                    wq = 1.0 - sqrt(div_rcp_ok(mean_dist, bd2) ? div_rcp(mean_dist, bd2, m.inv_bound_d2) : mean_dist / bd2);
                     status = SO_MATCH_SUCCESS;
                 }
             }
@@ -1068,6 +1098,9 @@ __global__ void __launch_bounds__(kFitThreads, SO_FIT_MINB) k_fit(MapView m, Bat
     if (st->phase != PH_CORR) return;
     __shared__ double s_pose[7];
     __shared__ int s_hist[16];
+#if SO_FIT_NBD_SMEM
+    __shared__ double s_nbd[15 * kFitThreads];      // the five neighbours in FP64, one column per thread (15 x 8 B x 256 = 30 KB)
+#endif
     if (threadIdx.x < 7) s_pose[threadIdx.x] = st->x[threadIdx.x];
     if (threadIdx.x < 16) s_hist[threadIdx.x] = 0;
     __syncthreads();
@@ -1078,7 +1111,13 @@ __global__ void __launch_bounds__(kFitThreads, SO_FIT_MINB) k_fit(MapView m, Bat
         const size_t gi = size_t(bv.offset[s]) + i;
         if (i < n) {
             const float4* npts = nb.pts + gi;
-            fit_point(m, cb, nb, gi, __ldg(&bv.scan[gi]), s_pose, int(nb.pre[gi]), [&](int j) { return ld_f4_again(npts + size_t(j) * nb.cap); }, s_hist);
+#if SO_FIT_NBD_SMEM
+            fit_point<kFitThreads>(m, cb, nb, gi, __ldg(&bv.scan[gi]), s_pose, int(nb.pre[gi]), [&](int j) { return __ldcs(npts + size_t(j) * nb.cap); },
+                                   s_nbd + threadIdx.x, s_hist);
+#else
+            fit_point<0>(m, cb, nb, gi, __ldg(&bv.scan[gi]), s_pose, int(nb.pre[gi]), [&](int j) { return ld_f4_again(npts + size_t(j) * nb.cap); },
+                         nullptr, s_hist);
+#endif
         }
     }
     __syncthreads();
@@ -1134,7 +1173,7 @@ __global__ void __launch_bounds__(kThreads, 4) k_knn_fit(MapView m, BatchView bv
             pos[j] = tk.id[j] != 0xFFFFFFFFu ? tk.pos[j] : 0xFFFFFFFFu;
             nb.pos[size_t(j) * nb.cap + gi] = pos[j];
         }
-        fit_point(m, cb, nb, gi, sp, s_pose, pre, [&](int j) { return ld_f4_again(m.pts + pos[j]); }, s_hist);
+        fit_point<0>(m, cb, nb, gi, sp, s_pose, pre, [&](int j) { return ld_f4_again(m.pts + pos[j]); }, nullptr, s_hist);
     }
     __syncthreads();
     if (threadIdx.x < 16 && s_hist[threadIdx.x]) atomicAdd(&bv.hist[s * kHistStride + threadIdx.x], s_hist[threadIdx.x]);

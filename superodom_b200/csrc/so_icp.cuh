@@ -68,6 +68,10 @@ __host__ inline uint32_t eval_grid(uint32_t n_max) {
     const uint32_t per = uint32_t(kEvalPts) * 256u, g = (n_max + per - 1u) / per;
     return g > 64u ? g : 64u;
 }
+// k_fit launch shape, re-measured on an H100 80GB HBM3 (700 W limit; scripts/ab_knn.py, 64 cfg2 scans = 8.4 M points per launch,
+// two alternating rounds, ms per launch): 2 points x 256 threads x 4 CTAs/SM 0.554-0.560; 1 point per thread 0.544-0.545;
+// 128 threads x 8 CTAs/SM 0.552-0.554; neighbours re-read and re-converted per pass (SO_FIT_NBD_SMEM=0) 0.594-0.609.  The
+// defaults are kept: the other shapes are within 3 % and were not carried through the full suite.
 #ifndef SO_FIT_PTS
 #define SO_FIT_PTS 2
 #endif
@@ -84,6 +88,11 @@ constexpr int kFitPts = SO_FIT_PTS;      // points per thread in k_fit
 #define SO_FIT_MINB 4
 #endif
 constexpr int kFitThreads = SO_FIT_THREADS;
+// 1: k_fit widens each neighbour coordinate to FP64 once and keeps it in shared memory for the later passes (15 doubles per
+// thread); 0: every pass re-reads the neighbour (L1 hit) and converts it again.
+#ifndef SO_FIT_NBD_SMEM
+#define SO_FIT_NBD_SMEM 1
+#endif
 // 1: search and fit of a point run in one kernel (k_knn_fit); 0: k_knn_scan hands the neighbours to k_fit through HBM.
 // The stage is issue-bound on the SUM of both halves' instructions, so sharing an SM between search and fit warps buys little:
 // on an H100 80GB HBM3 (700 W limit, scripts/ab_knn.py, 64 cfg2 scans) fused 1.72 ms vs split 1.05 + 0.70 ms per matching stage
