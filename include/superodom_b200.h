@@ -107,8 +107,8 @@ typedef struct {
     int32_t prediction_source;    /* stats.prediction_source: 1 when the pose prior rows were added (LidarSlam.cpp:278,297) */
     double time_ms;               /* stats.time_elapsed: the ICP loop, device time measured with CUDA events */
     double time_total_ms;         /* whole so_register call incl. H2D / D2H (host clock) */
-    int32_t knn_searched;         /* telemetry, summed over the ICP iterations: queries that ran the neighbour search ... */
-    int32_t knn_verified;         /* ... and queries whose previous five neighbours were proven to still be their 5-NN (no search) */
+    int32_t knn_searched;         /* reserved, always 0 */
+    int32_t knn_verified;         /* reserved, always 0 */
 } so_icp_result;
 
 /* One accepted/rejected plane correspondence, for stage-level parity tests
@@ -297,11 +297,12 @@ uint64_t so_kernel_launches(so_ctx* ctx, int reset);
  * last reset (bench.py e2e accounting). */
 int so_bytes_copied(so_ctx* ctx, uint64_t* h2d, uint64_t* d2h, int reset);
 /* Accumulated device time (ms, CUDA events on the context stream) and launch count of a kernel class since the last
- * reset; classes: 0 k_knn_scan (scan k-NN; k_knn_fit = k-NN + plane fit in a SO_BUILD_FUSED_MATCH build), 1 k_evaluate +
+ * reset; classes: 0 k_knn_scan (scan k-NN), 1 k_evaluate +
  * k_lm_step (LM step), 2 k_knn (so_knn*), 3 scan ordering / map build / map insert / scan preparation, 4 first evaluation of
- * a solve (k_evaluate + k_lm_step iteration zero), 5 k_fit (plane fit; empty in a fused build).
+ * a solve (k_evaluate + k_lm_step iteration zero), 5 k_fit (plane fit).
  * Profiling mode serialises kernels; enable only for roofline runs. */
-/* Build-time switches of the loaded library: bit 0 (SO_BUILD_FUSED_MATCH) = search and fit run as one kernel. */
+/* Build-time switches of the loaded library.  Bit 0 (SO_BUILD_FUSED_MATCH, search and fit as one kernel) is reserved: this
+ * library always runs them as two kernels and returns 0. */
 #define SO_BUILD_FUSED_MATCH 1
 int so_build_flags(void);
 int so_profile_enable(so_ctx* ctx, int on);

@@ -44,8 +44,6 @@ for k, nm in names.items():
     out[nm + "_launches"] = int(n)
 out["err_vs_truth"] = float(np.abs(np.array([list(r.pose) for r in res])[:, :3] - truths[:, :3]).max())
 out["icp_iters_mean"] = float(np.mean([r.n_iterations for r in res]))
-ver, sea = sum(r.knn_verified for r in res), sum(r.knn_searched for r in res)
-out["knn_verified_frac"] = ver / max(ver + sea, 1)
 ctx.close()
 
 if "--parity" in sys.argv:

@@ -94,7 +94,6 @@ static int ctx_alloc(Ctx* c) {
     SO_CUDA_TRY(cudaMalloc(&c->nn.pts, c->scan_cap * 5 * sizeof(float4)));
     SO_CUDA_TRY(cudaMalloc(&c->nn.d5, c->scan_cap * sizeof(float)));
     SO_CUDA_TRY(cudaMalloc(&c->nn.pre, c->scan_cap));
-    SO_CUDA_TRY(cudaMalloc(&c->nn.vq, c->scan_cap * sizeof(float4)));
     c->nn.cap = c->scan_cap;
     { int rc2 = scan_sort_alloc(c); if (rc2) return rc2; }
     SO_CUDA_TRY(cudaMalloc(&c->d_offset, c->max_batch * sizeof(uint32_t)));
@@ -138,7 +137,7 @@ static void ctx_free(Ctx* c) {
     for (auto& e : c->ev_copy) if (e) cudaEventDestroy(e);
     map_free(c);
     cudaFree(c->d_scan_sorted); cudaFree(c->d_skeys); cudaFree(c->d_skeys_out); cudaFree(c->d_svals); cudaFree(c->d_svals_out);
-    cudaFree(c->d_sort_tmp); cudaFree(c->d_sort_tmp2); cudaFree(c->nn.pos); cudaFree(c->nn.pts); cudaFree(c->nn.d5); cudaFree(c->nn.pre); cudaFree(c->nn.vq);
+    cudaFree(c->d_sort_tmp); cudaFree(c->d_sort_tmp2); cudaFree(c->nn.pos); cudaFree(c->nn.pts); cudaFree(c->nn.d5); cudaFree(c->nn.pre);
     cudaFree(c->d_scan); cudaFree(c->d_offset); cudaFree(c->d_state); cudaFreeHost(c->h_state); cudaFreeHost(c->h_offset);
     cudaFree(c->d_partials); cudaFree(c->d_counters); cudaFree(c->d_hist);
     cudaFree(c->d_escan); cudaFree(c->d_eoffset); cudaFree(c->ebuf.a); cudaFree(c->ebuf.b); cudaFree(c->ebuf.flags); cudaFree(c->ebuf.nn); cudaFree(c->ebuf.selmask);
@@ -275,7 +274,7 @@ static int prepare_scans(Ctx* c, const float4* d_scan_in, const Chunk& ch, cudaS
     const BatchView bv = batch_view(c, d_scan_in, ch.first);
     timed_launch_begin(c);
     // key layout: [scan inside the chunk | dropped (compact only) | cell]; 32-bit keys whenever everything fits
-    const uint64_t n_cells = scan_key_space(c->surf.n_slots, mv.nb);       // cell / brick-order keys (so_knn.cuh)
+    const uint64_t n_cells = scan_key_space(c->surf.n_slots, mv.nb);       // cell-order keys (so_knn.cuh)
     int cell_bits = 1, scan_bits = 0;
     while (cell_bits < 32 && (uint64_t(1) << cell_bits) <= n_cells) ++cell_bits;       // cells 0..n_cells-1 < mask = 2^cell_bits - 1
     if (compact && ch.small && !c->no_small_prepare) {
@@ -323,7 +322,6 @@ static int run_schedule(Ctx* c, const Chunk& ch, int iters, int lm, bool with_nn
     eb.offset = c->d_eoffset + ch.first;                  // like bv.offset: indexed by the scan's position inside the chunk
     if (!with_nn) { eb.nn = nullptr; eb.selmask = nullptr; }
     *was_loop = false;
-    if (d_inject && kCorrLaunches != 2) return fail(SO_ERR_ARG, "so_register_injected needs the split k_knn_scan / k_fit build");
     if (c->profiling || with_nn || d_inject) {
         // profiling mode: one launch at a time, timed with events, and only launches that have work (the host peeks
         // at the phases) so that the per-class average is the duration of a kernel that actually ran
@@ -336,14 +334,11 @@ static int run_schedule(Ctx* c, const Chunk& ch, int iters, int lm, bool with_nn
         };
         for (int it = 0; it < iters; ++it) {
             if (any_in(PH_CORR)) {
-                if (kCorrLaunches == 1) { timed_launch_begin(c); launch_match(mv, bv, cb, c->nn, grid_x, n_scans, c->stream); timed_launch_end(c, 0); }
-                else {
-                    timed_launch_begin(c);
-                    if (d_inject) launch_inject(mv, c->surf.d_xyzi, c->surf.n, bv, c->nn, d_inject, inject_iters, grid_x, n_scans, c->stream);
-                    else launch_match(mv, bv, cb, c->nn, grid_x, n_scans, c->stream, 1);                                               // k_knn_scan
-                    timed_launch_end(c, 0);
-                    timed_launch_begin(c); launch_match(mv, bv, cb, c->nn, grid_x, n_scans, c->stream, 2); timed_launch_end(c, 5);      // k_fit
-                }
+                timed_launch_begin(c);
+                if (d_inject) launch_inject(mv, c->surf.d_xyzi, c->surf.n, bv, c->nn, d_inject, inject_iters, grid_x, n_scans, c->stream);
+                else launch_match(mv, bv, cb, c->nn, grid_x, n_scans, c->stream, 1);                                               // k_knn_scan
+                timed_launch_end(c, 0);
+                timed_launch_begin(c); launch_match(mv, bv, cb, c->nn, grid_x, n_scans, c->stream, 2); timed_launch_end(c, 5);      // k_fit
                 timed_launch_begin(c); launch_first_eval(bv, cb, grid_x, n_scans, c->stream, &me, &eb, grid_e); c->launches += 1 + (grid_e ? 1 : 0); timed_launch_end(c, 4);
             }
             for (int k = 0; k < lm; ++k)
@@ -411,7 +406,7 @@ static int run_schedule(Ctx* c, const Chunk& ch, int iters, int lm, bool with_nn
     slot->used = ++c->graph_clock;
     SO_CUDA_TRY(cudaGraphLaunch(slot->exec, run_stream));
     *was_loop = slot->is_loop;
-    if (!slot->is_loop) c->launches += uint64_t(iters) * (bv.counters && !grid_e ? kCorrLaunches + 1 + lm : kCorrLaunches + 2 + 2 * lm + (grid_e ? 1 + lm : 0));      // loop form: counted from the iterations executed
+    if (!slot->is_loop) c->launches += uint64_t(iters) * (bv.counters && !grid_e ? 2 + 1 + lm : 2 + 2 + 2 * lm + (grid_e ? 1 + lm : 0));      // 2: k_knn_scan + k_fit; loop form: counted from the iterations executed
     return SO_OK;
 }
 
@@ -447,7 +442,7 @@ static void fill_result(const Ctx* c, const IcpState& s, const double pose_in[7]
     r->pos_err = s.pos_err; r->pos_inv_cond = s.pos_inv_cond; r->ori_err_deg = s.ori_err_deg; r->ori_inv_cond = s.ori_inv_cond;
     for (int i = 0; i < 3; ++i) { r->pos_dir[i] = s.pos_dir[i]; r->ori_dir[i] = s.ori_dir[i]; }
     if (s.status) r->status = s.status;
-    r->knn_searched = s.knn_searched; r->knn_verified = s.knn_verified;
+    r->knn_searched = 0; r->knn_verified = 0;             // reserved
     r->prediction_source = s.use_prior ? 1 : 0;
     double T[7];
     std::memcpy(T, s.x, sizeof(T));
@@ -594,8 +589,8 @@ static int register_core(Ctx* c, const float4* d_scan, const uint32_t* n_points,
             int max_it = 0;
             for (uint32_t s = chunks[k].first; s < chunks[k].first + chunks[k].count; ++s) max_it = std::max(max_it, int(c->h_state[s].n_iterations));
             const bool fused = chunks[k].count <= 2 && !chunks[k].grid_e && !c->no_fused_lm;
-            c->launches += uint64_t(max_it) * uint64_t(fused ? kCorrLaunches + 2 + o.lm_max_iterations
-                                                             : kCorrLaunches + 3 + 2 * o.lm_max_iterations + (chunks[k].grid_e ? 1 + o.lm_max_iterations : 0));
+            c->launches += uint64_t(max_it) * uint64_t(fused ? 2 + 2 + o.lm_max_iterations
+                                                             : 2 + 3 + 2 * o.lm_max_iterations + (chunks[k].grid_e ? 1 + o.lm_max_iterations : 0));
         }
         for (size_t s = 0; s < n_scans; ++s) {
             if (results[s].status == SO_STATUS_NOT_ENOUGH_FEATURES || n_points[s] == 0) continue;
@@ -1224,7 +1219,7 @@ int so_correspond(so_ctx* ctx, const void* surf, size_t n, size_t stride, size_t
     const MapView mv = map_view(c, c->surf);
     BatchView bv = batch_view(c, c->d_scan_sorted);
     bv.coop_knn = grid_x <= kCoopMaxGrid && !c->no_coop_knn;            // as a single small registration would search
-    timed_launch_begin(c); launch_correspond(mv, bv, c->corr, c->nn, grid_x, 1, c->stream); c->launches += kCorrLaunches + 2; timed_launch_end(c, 0);
+    timed_launch_begin(c); launch_correspond(mv, bv, c->corr, c->nn, grid_x, 1, c->stream); c->launches += 2 + 2; timed_launch_end(c, 0);
     SO_CUDA_TRY(cudaGetLastError());
     std::vector<double4> nd(n); std::vector<double> w(n); std::vector<uchar4> fl(n); std::vector<uint32_t> nn(n * 5); std::vector<float> d2(n * 5);
     std::vector<float4> sorted(n);
@@ -1394,7 +1389,7 @@ int so_bytes_copied(so_ctx* ctx, uint64_t* h2d, uint64_t* d2h, int reset) {
     return SO_OK;
 }
 
-int so_build_flags(void) { return SO_FUSE_KNN_FIT ? SO_BUILD_FUSED_MATCH : 0; }
+int so_build_flags(void) { return 0; }
 
 int so_profile_enable(so_ctx* ctx, int on) {
     Ctx* c = reinterpret_cast<Ctx*>(ctx);

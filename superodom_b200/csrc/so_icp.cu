@@ -5,7 +5,6 @@
 //                  (three-round select: bound, gather, refine); hands the five neighbours to k_fit.         [a5-a7]
 //   k_fit        : 3x3 PCA + 5x3 column-pivoted QR plane fit with the reference's accept/reject gates, observability
 //                  labels + histograms, fit weight; writes the correspondence record.                     [a8-a11]
-//   k_knn_fit    : optional fusion of the two (SO_FUSE_KNN_FIT; measured slower, see so_icp.cuh).
 //   k_evaluate   : per correspondence -- residual, 1x6 Jacobian, Tukey/Scaled robust weight at the matched pose (first
 //                  evaluation of a solve) or at the LM candidate, warp/CTA-reduced in FP64 (21+6+1 accumulators). [a12-a13]
 //   k_edge_fit / k_edge_evaluate : the edge / line branch (10-NN in the edge map, best-line selection, line factor).   [a19]
@@ -78,43 +77,13 @@ __device__ __noinline__ double grad_max_norm(const double x[7], const double g[6
     return m;
 }
 
-__device__ __noinline__ void covariance_and_errors(IcpState& st) {
-    // ceres::Covariance{apply_loss_function, DENSE_SVD, null_space_rank=-1} in tangent space (LidarSlam.cpp:854-871):
-    // pseudo-inverse of J^T J dropping singular directions with s_i/s_max < sqrt(1e-14) (covariance_impl.cc).
-    double A[36], V[36], w[6];
-    _Pragma("unroll") for (int i = 0; i < 6; ++i) _Pragma("unroll") for (int j = 0; j < 6; ++j) A[i * 6 + j] = st.H[i <= j ? tri(i, j) : tri(j, i)];
-    jacobi_eig6_rr<30>(A, V, w);
-    const double lmax = w[5];
-    double inv[6];
-    bool cut = false;
-    _Pragma("unroll") for (int k = 5; k >= 0; --k) {          // descending singular values = descending eigenvalues
-        const double ratio = (w[k] > 0.0 && lmax > 0.0) ? sqrt(w[k] / lmax) : 0.0;
-        if (cut || ratio < 1e-7) { cut = true; inv[k] = 0.0; } else inv[k] = 1.0 / w[k];
-    }
-    _Pragma("unroll") for (int i = 0; i < 6; ++i) _Pragma("unroll") for (int j = 0; j < 6; ++j) {
-        double t = 0.0;
-        _Pragma("unroll") for (int k = 0; k < 6; ++k) t += V[i * 6 + k] * inv[k] * V[j * 6 + k];
-        st.cov[i * 6 + j] = t;
-    }
-    // EstimateRegistrationError (LidarSlam.cpp:873-884): 3x3 eigen of the position / orientation blocks
-    double P[9], O[9], E[9], e[3];
-    _Pragma("unroll") for (int i = 0; i < 3; ++i) _Pragma("unroll") for (int j = 0; j < 3; ++j) { P[i * 3 + j] = st.cov[i * 6 + j]; O[i * 3 + j] = st.cov[(i + 3) * 6 + (j + 3)]; }
-    jacobi_eig<3, 20>(P, E, e);
-    st.pos_err = sqrt(e[2]); st.pos_dir[0] = E[2]; st.pos_dir[1] = E[5]; st.pos_dir[2] = E[8];
-    st.pos_inv_cond = sqrt(e[0]) / sqrt(e[2]);
-    jacobi_eig<3, 20>(O, E, e);
-    st.ori_err_deg = sqrt(e[2]) / M_PI * 180.0; st.ori_dir[0] = E[2]; st.ori_dir[1] = E[5]; st.ori_dir[2] = E[8];
-    st.ori_inv_cond = sqrt(e[0]) / sqrt(e[2]);
-}
-
-#ifndef SO_COV_SERIAL
-#define SO_COV_SERIAL 0           // 1: the covariance step on the one thread that runs the optimiser (A/B aid)
-#endif
-// The same computation spread over the 32 lanes of one warp (S and sc in shared memory).  The 6x6 Jacobi takes its rotations in the
-// round-robin order of jacobi_eig6_rr: the three angles of a round are computed by three lanes at once, and each rotation updates
-// its 8 off-diagonal entries, 12 eigenvector entries and 2x2 block on 15 lanes in one step instead of ~110 dependent FP64
-// instructions on one thread (the covariance was 38 of the ~50 us the last optimiser step of a registration took).  Per element
-// the arithmetic and its order are those of the serial routine.
+// ceres::Covariance + EstimateRegistrationError at the end of a registration, on the 32 lanes of the CTA's first warp (S and sc in
+// shared memory).  The 6x6 cyclic Jacobi (at most 30 sweeps, convergence test and FP32 angle of jacobi_eig) takes its rotations in
+// ROUND-ROBIN order: five rounds of three pairs with disjoint indices -- (0,5)(1,4)(2,3) / (0,4)(3,5)(1,2) / (0,3)(2,4)(1,5) /
+// (0,2)(1,3)(4,5) / (0,1)(2,5)(3,4).  The angle of a pair depends only on its own 2x2 block, which the other two rotations of the
+// round do not touch, so the three angles of a round are computed by three lanes at once; each rotation then updates its 8
+// off-diagonal entries, 12 eigenvector entries and 2x2 block on 15 lanes in one step instead of ~110 dependent FP64 instructions
+// on one thread (on one thread the covariance was 38 of the ~50 us the last optimiser step of a registration took).
 __constant__ int c_rr_p[15] = {0, 1, 2, 0, 3, 1, 0, 2, 1, 0, 1, 4, 0, 2, 3};
 __constant__ int c_rr_q[15] = {5, 4, 3, 4, 5, 2, 3, 4, 5, 2, 3, 5, 1, 5, 4};
 struct CovScratch { double a[36], v[36], w[6], inv[6], t[3], c[3], s[3]; int perm[6]; };
@@ -139,7 +108,7 @@ __device__ __noinline__ void covariance_and_errors_warp(IcpState& S, CovScratch&
 #pragma unroll
                 for (int q = p + 1; q < 6; ++q) off += sc.a[p * 6 + q] * sc.a[p * 6 + q];
             }
-            stop = (off <= SO_JACOBI_OFF_TOL * dia || off == 0.0) ? 1 : 0;
+            stop = (off <= kJacobiOffTol * dia || off == 0.0) ? 1 : 0;
         }
         if (__shfl_sync(full, stop, 0)) break;
 #pragma unroll 1
@@ -248,11 +217,7 @@ __device__ __noinline__ void end_solve(IcpState& st) {
         st.status = SO_STATUS_NO_CORRESPONDENCES; st.phase = PH_DONE; return;
     }
     if (st.num_successful == 1 || it == st.max_icp_iters - 1) {      // (:141)
-#if SO_COV_SERIAL
-        covariance_and_errors(st);
-#else
         st.need_cov = 1;                          // lm_step_body: first warp of the CTA, right after this serial step
-#endif
         st.phase = PH_DONE;
     } else {
         st.icp_iter = it + 1;
@@ -426,47 +391,6 @@ __device__ __forceinline__ void accumulate(double acc[kAcc], const double n[3], 
     acc[27] += 0.5 * rho0;
 }
 
-#ifndef SO_KNN_VERIFY
-#define SO_KNN_VERIFY 0           // 1: try to PROVE the previous five neighbours still exact before searching again.  Off: measured slower
-                                  // on every BASELINE workload (3.6 % of the queries verify on cfg2; DESIGN.md section 4, tried-and-measured)
-#endif
-// ICP iterations after the first, before any walk: the record of the query's last FULL search (nb.vq: where the query was, q0, and a
-// lower bound D on the squared distance from q0 to every point of the block outside the five found) proves the five still ARE the
-// 5-NN at the new position q1 whenever   max_i |q1 - s_i| < sqrt(D) - |q1 - q0|   -- any other point x has
-// |q1 - x| >= |q0 - x| - |q1 - q0| >= sqrt(D) - |q1 - q0| (triangle inequality), strictly beyond all five, so neither membership nor
-// ties with outsiders can differ from what a fresh search returns.  Then only their distances (the reference's rounding) and their
-// (d2, id) order are renewed -- ~150 instructions instead of the ~3 700 of a walk.  Margins cover the float evaluation of the norms.
-// Requires the five to lie in the block the query is in NOW (the search is block-local, LocalMap.h:488-507).  On success tk holds
-// the five in order (tk.pos = positions in the sorted map) and true is returned.
-__device__ __forceinline__ bool verify_neighbours(const MapView& m, const QueryCell& qc, const NnBuf& nb, size_t gi, float qx, float qy, float qz,
-                                                  TopK<5>& tk) {
-    const float4 rec = nb.vq[gi];
-    if (!(rec.w > 0.f)) return false;
-    const uint32_t cells = uint32_t(m.nb) * uint32_t(m.nb) * uint32_t(m.nb);
-    const uint32_t lo = __ldg(&m.cell_start[uint32_t(qc.slot) * cells]), hi = __ldg(&m.cell_start[uint32_t(qc.slot) * cells + cells]);
-    const float mx = qx - rec.x, my = qy - rec.y, mz = qz - rec.z;
-    const float moved = sqrtf(fmaf(mx, mx, fmaf(my, my, mz * mz))) * 1.000002f + 1e-6f;
-    const float reach = sqrtf(rec.w) * 0.999998f - moved - 1e-6f;           // every outsider is at least this far from q1
-    if (!(reach > 0.f)) return false;
-    bool ok = true;
-    float4 c[5]; uint32_t pos[5];
-#pragma unroll
-    for (int j = 0; j < 5; ++j) {
-        pos[j] = nb.pos[size_t(j) * nb.cap + gi];
-        ok = ok && pos[j] >= lo && pos[j] < hi;
-        c[j] = __ldg(&m.pts[ok ? pos[j] : lo]);
-    }
-    if (!ok) return false;
-    float far2 = 0.f;
-#pragma unroll
-    for (int j = 0; j < 5; ++j) far2 = fmaxf(far2, exact_d2(c[j], qx, qy, qz));
-    if (!(sqrtf(far2) * 1.000002f < reach)) return false;
-    tk.init(FLT_MAX);
-#pragma unroll
-    for (int j = 0; j < 5; ++j) tk.offer(exact_d2(c[j], qx, qy, qz), __float_as_uint(c[j].w), pos[j]);
-    return true;
-}
-
 // ICP iterations after the first: the previous iteration's five neighbours still exist, so the largest of their (exact)
 // distances to the moved query bounds the new 5th-neighbour distance -- provided they lie in the block the query is in NOW
 // (the search is block-local, LocalMap.h:488-507: after a pose update that carries the point across a 50 m block face the old
@@ -500,11 +424,11 @@ __device__ __forceinline__ bool should_process(uint32_t i, double rate) {
 }
 
 // ------------------------------------------------------------------------------------------------------------------
-// Scan preparation (once per registration): order the scan points by the map cell they fall into at the PRIOR pose, cells
-// grouped into 8x8x8 bricks (scan_order_key), so that the 128 queries of a CTA sit in a compact box of cells (one shared,
-// bulk-copied candidate tile) and the 32 lanes of a warp walk the same cell rows.  Pose updates inside one registration are a
-// few cm against 0.39 m cells, so the order stays coherent for all ICP iterations.  The sorted copy carries the point's original index in .w (the reference's
-// shouldProcessPoint() decimation is defined on the original index, LidarSlam.cpp:353-359).
+// Scan preparation (once per registration): order the scan points by the map cell they fall into at the PRIOR pose
+// (scan_order_key: cell-linear, x fastest), so that the 32 lanes of a warp walk the same cell rows.  Pose updates inside one
+// registration are a few cm against 0.39 m cells, so the order stays coherent for all ICP iterations.  The sorted copy carries
+// the point's original index in .w (the reference's shouldProcessPoint() decimation is defined on the original index,
+// LidarSlam.cpp:353-359).
 // ------------------------------------------------------------------------------------------------------------------
 // Key = (scan index inside the chunk) << cell_bits | cell; cells beyond the mask and off-map points sort last inside their scan.
 // KeyT = uint32_t when cell_bits + scan bits fit (the usual case: 4 radix passes over 8-byte pairs instead of 5 over 12-byte ones).
@@ -530,7 +454,7 @@ __global__ void __launch_bounds__(kThreads) k_scan_keys(MapView m, BatchView bv,
     qrot(st->x + 3, pin, pf);
     QueryCell qc;
     locate(m, float(pf[0] + st->x[0]), float(pf[1] + st->x[1]), float(pf[2] + st->x[2]), qc);
-    const uint32_t cell = qc.slot >= 0 ? scan_order_key(m, qc) : 0xFFFFFFFFu;      // brick order (so_knn.cuh)
+    const uint32_t cell = qc.slot >= 0 ? scan_order_key(m, qc) : 0xFFFFFFFFu;      // cell order (so_knn.cuh)
     const uint32_t mask = cell_bits >= 32 ? 0xFFFFFFFFu : ((1u << cell_bits) - 1u);
     keys[gi] = KeyT((KeyT(s) << (cell_bits + (COMPACT ? 1 : 0))) | KeyT(cell < mask ? cell : mask));
     vals[gi] = uint32_t(gi);
@@ -633,89 +557,42 @@ __global__ void __launch_bounds__(kSmallThreads) k_prepare_small(MapView m, Batc
 // k_knn_scan: findNearestNeighbors (LidarSlam.cpp:720-747) for every processed scan point at the current pose: the select k-NN of
 // so_knn.cuh, one query per thread, queries consecutive in scan order.  Light on registers (FP32 search, FP64 only for the pose
 // transform and the exact d2 of real contenders) so that many warps per SM hide the latency of the cell walks.
-// SO_KNN_TILE build: 128 queries per CTA in brick order; the CTA stages the candidate tile of its queries' cell box (build_tile:
-// one cp.async.bulk per map row onto an mbarrier, a 16-bit local cell table) and searches shared memory; CTAs whose box does not
-// fit search global memory.  Measured slower than the global search (so_knn.cuh), so it is not the default.
 // ------------------------------------------------------------------------------------------------------------------
-#ifndef SO_KNN_MINB
-#define SO_KNN_MINB (SO_KNN_TILE ? 6 : 1024 / SO_KNN_THREADS)      // 64 registers per thread either way
-#endif
-__global__ void __launch_bounds__(kTileThreads, SO_KNN_MINB) k_knn_scan(MapView m, BatchView bv, NnBuf nb) {
+// Queries per CTA, measured on an H100 80GB HBM3 (700 W limit, scripts/ab_knn.py, 64 cfg2 scans = 8.4 M queries per launch):
+// 32 -> 1.08, 64 -> 1.05-1.07, 128 -> 1.07, 256 -> 1.11 ms per launch.  1024 / kKnnThreads CTAs per SM = 64 registers per thread.
+constexpr int kKnnThreads = 64;
+__global__ void __launch_bounds__(kKnnThreads, 1024 / kKnnThreads) k_knn_scan(MapView m, BatchView bv, NnBuf nb) {
     const int s = blockIdx.y;
     IcpState* st = bv.st + s;
     if (st->phase != PH_CORR) return;
     __shared__ double s_pose[7];
-    __shared__ uint32_t s_buf[kBufCap * kTileThreads];
-#if SO_KNN_TILE
-    __shared__ TileSmem s_tile;
-#endif
+    __shared__ uint32_t s_buf[kBufCap * kKnnThreads];
     if (threadIdx.x < 7) s_pose[threadIdx.x] = st->x[threadIdx.x];
     __syncthreads();
     const uint32_t n = uint32_t(st->n_points);
-    const uint32_t i = blockIdx.x * kTileThreads + threadIdx.x;
-    if (blockIdx.x * kTileThreads >= n) return;           // whole CTA past the end; partial CTAs stay together for the tile build
+    const uint32_t i = blockIdx.x * kKnnThreads + threadIdx.x;
+    if (blockIdx.x * kKnnThreads >= n) return;            // whole CTA past the end
     const bool in_range = i < n;
     const size_t gi = size_t(bv.offset[s]) + (in_range ? i : 0);
     const float4 sp = __ldg(&bv.scan[gi]);
     int pre = SO_MATCH_SKIPPED;
     TopK<5> tk;
     tk.init(m.bound_d2);
-    bool searchable = false, verified = false;
-    float qx = 0.f, qy = 0.f, qz = 0.f, u_seed = -1.f;
-    QueryCell qc;
-    qc.slot = -1; qc.nblock = 0; qc.c[0] = qc.c[1] = qc.c[2] = 0; qc.f[0] = qc.f[1] = qc.f[2] = 0.f;
     if (in_range && should_process(__float_as_uint(sp.w), st->sampling_rate)) {
         const double pin[3] = {double(sp.x), double(sp.y), double(sp.z)};
         double pf[3];
         qrot(s_pose + 3, pin, pf);
-        qx = float(pf[0] + s_pose[0]); qy = float(pf[1] + s_pose[1]); qz = float(pf[2] + s_pose[2]);
+        const float qx = float(pf[0] + s_pose[0]), qy = float(pf[1] + s_pose[1]), qz = float(pf[2] + s_pose[2]);
+        QueryCell qc;
         locate(m, qx, qy, qz, qc);
         if (qc.slot < 0 || qc.nblock < 5) pre = SO_MATCH_NOT_ENOUGH_NEIGHBORS;
         else {
-            searchable = true;
-            if (st->icp_iter > 0) {
-                verified = SO_KNN_VERIFY && verify_neighbours(m, qc, nb, gi, qx, qy, qz, tk);
-                if (!verified && nb.pre[gi] == SO_MATCH_SUCCESS) u_seed = seed_bound(m, qc, nb, gi, qx, qy, qz);
-            }
+            const float u_seed = st->icp_iter > 0 && nb.pre[gi] == SO_MATCH_SUCCESS ? seed_bound(m, qc, nb, gi, qx, qy, qz) : -1.f;
+            knn_select<5, true>(BlockGrid(m, qc.slot), m, qc, qx, qy, qz, u_seed, m.bound_d2, s_buf, tk);
+            pre = tk.count() < 5 ? SO_MATCH_NEIGHBORS_TOO_FAR : SO_MATCH_SUCCESS;       // d2[4] > 3*planeRes_ (:741-744)
         }
-    }
-    if (verified) {                                       // the stored five are still the 5-NN: distances and order renewed, no walk
-        searchable = false;
-        pre = tk.d2[4] > m.bound_d2 ? SO_MATCH_NEIGHBORS_TOO_FAR : SO_MATCH_SUCCESS;       // d2[4] > 3*planeRes_ (:741-744)
-    }
-    if (SO_KNN_VERIFY) {                                  // telemetry: one atomic pair per warp
-        const unsigned ms = __ballot_sync(0xffffffffu, searchable), mv = __ballot_sync(0xffffffffu, verified);
-        if ((threadIdx.x & 31) == 0) { if (ms) atomicAdd(&st->knn_searched, __popc(ms)); if (mv) atomicAdd(&st->knn_verified, __popc(mv)); }
-    }
-#if SO_KNN_TILE
-    TileGrid tg;
-    const bool tiled = build_tile(m, s_tile, searchable, qc, tg);
-#else
-    const bool tiled = false;
-#endif
-    float next_lb = -1.f;
-    if (searchable) {
-#if SO_KNN_TILE
-        if (tiled) {
-            knn_select<5, SO_R1_OCTANT != 0>(tg, m, qc, qx, qy, qz, u_seed, m.bound_d2, s_buf, tk, SO_KNN_VERIFY ? &next_lb : nullptr);
-#pragma unroll
-            for (int j = 0; j < 5; ++j) if (tk.id[j] != 0xFFFFFFFFu) tk.pos[j] = tg.pos_of(tk.pos[j]);
-        } else
-#endif
-        {
-            const GlobalGrid gg(m, qc.slot);
-            knn_select<5, SO_R1_OCTANT != 0>(gg, m, qc, qx, qy, qz, u_seed, m.bound_d2, s_buf, tk, SO_KNN_VERIFY ? &next_lb : nullptr);
-        }
-        pre = tk.count() < 5 ? SO_MATCH_NEIGHBORS_TOO_FAR : SO_MATCH_SUCCESS;       // d2[4] > 3*planeRes_ (:741-744)
-        if (pre != SO_MATCH_SUCCESS) next_lb = -1.f;
     }
     if (!in_range) return;
-    if (SO_KNN_VERIFY && !verified) nb.vq[gi] = make_float4(qx, qy, qz, next_lb);       // a verified query keeps the record of its last full search
-    if (verified && pre != SO_MATCH_SUCCESS) {             // the fifth of the stored neighbours moved beyond the gate: the set stays on record
-        nb.pre[gi] = (unsigned char)pre;
-        nb.d5[gi] = m.bound_d2;
-        return;
-    }
     nb.pre[gi] = (unsigned char)pre;
     nb.d5[gi] = tk.d2[4];
 #pragma unroll
@@ -764,7 +641,7 @@ __global__ void __launch_bounds__(kThreads) k_knn_scan_coop(MapView m, BatchView
         locate(m, qx, qy, qz, qc);
         if (qc.slot < 0 || qc.nblock < 5) pre = SO_MATCH_NOT_ENOUGH_NEIGHBORS;
         else {
-            const GlobalGrid g(m, qc.slot);
+            const BlockGrid g(m, qc.slot);
             const int nbc = m.nb, R = m.R;
             const float cs = m.cs, U = m.bound_d2 * 1.000004f, Um = U * 1.0001f;
             // ---- lane l: row (oz, oy) of the cube, its candidate span
@@ -781,8 +658,8 @@ __global__ void __launch_bounds__(kThreads) k_knn_scan_coop(MapView m, BatchView
                     const bool l2 = l1 && R >= 2 && cx >= 2 && fmaf(fx + cs, fx + cs, lb) <= Um;
                     const bool r1 = cx + 1 < nbc && fmaf(gx, gx, lb) <= Um;
                     const bool r2 = r1 && R >= 2 && cx + 2 < nbc && fmaf(gx + cs, gx + cs, lb) <= Um;
-                    uint32_t end, tag;
-                    g.row(zz, yy, cx - int(l1) - int(l2), cx + int(r1) + int(r2), t, end, tag);
+                    uint32_t end;
+                    g.row(zz, yy, cx - int(l1) - int(l2), cx + int(r1) + int(r2), t, end);
                     len = end - t;
                 }
             }
@@ -890,14 +767,6 @@ __global__ void __launch_bounds__(kThreads) k_knn_inject(MapView m, const float4
     for (int j = 0; j < 5; ++j) nb.pos[size_t(j) * nb.cap + gi] = 0xFFFFFFFFu;
 }
 
-// A 16-byte global load the compiler may neither merge with an earlier load of the same address nor hoist: k_knn_fit (and
-// k_fit built with SO_FIT_NBD_SMEM=0) re-reads its neighbours (L1 hits) rather than keeping them live in registers.
-__device__ __forceinline__ float4 ld_f4_again(const float4* p) {
-    float4 v;
-    asm volatile("ld.global.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p));
-    return v;
-}
-
 // ------------------------------------------------------------------------------------------------------------------
 // k_fit: the rest of LidarSLAM::ComputePlaneDistanceParameters (LidarSlam.cpp:536-572) for every scan point, from the
 // neighbours k_knn_scan handed over: fit_point() below + the per-scan histograms.  The first residual/Jacobian evaluation of
@@ -913,21 +782,15 @@ __device__ __forceinline__ double ld_shared_again(const double* p) {
 
 // The rest of LidarSLAM::ComputePlaneDistanceParameters (LidarSlam.cpp:536-572) for one scan point whose k-NN outcome is
 // `status`: PCA, plane fit, gates, observability labels, fit weight; writes the correspondence record and counts the
-// histograms.  FP64 throughout.  nbr(j) loads neighbour j.  The fit reads the neighbours three more times after the mean
-// (scatter, QR, plane distances) and does not hold them in 30 FP64 registers across the eigen-solve: with STRIDE > 0 the first
-// pass widens each coordinate once and parks it in shared memory (nbd[(3 j + k) * STRIDE], this thread's column), and the
-// later passes load it from there; with STRIDE == 0 every pass calls nbr(j) again and widens afresh (float -> double
-// conversions run at a quarter of the FP64 rate).
-template <int STRIDE, class NbrLoad>
+// histograms.  FP64 throughout.  The neighbours come from k_knn_scan's hand-over (nb.pts).  The fit reads them three more times
+// after the mean (scatter, QR, plane distances) and does not hold them in 30 FP64 registers across the eigen-solve: the first
+// pass widens each coordinate once and parks it in shared memory (nbd[(3 j + k) * kFitThreads], this thread's column), and the
+// later passes load it from there instead of re-reading and widening afresh (float -> double conversions run at a quarter of
+// the FP64 rate).
 __device__ __forceinline__ void fit_point(const MapView& m, const CorrBuf& cb, const NnBuf& nb, size_t gi, const float4 sp, const double* s_pose,
-                                          int status, NbrLoad nbr, double* nbd, int* s_hist) {
+                                          int status, double* nbd, int* s_hist) {
     auto nbr_d = [&](int j, double& x, double& y, double& z) {
-        if constexpr (STRIDE > 0) {
-            x = ld_shared_again(nbd + (3 * j + 0) * STRIDE); y = ld_shared_again(nbd + (3 * j + 1) * STRIDE); z = ld_shared_again(nbd + (3 * j + 2) * STRIDE);
-        } else {
-            const float4 c = nbr(j);
-            x = double(c.x); y = double(c.y); z = double(c.z);
-        }
+        x = ld_shared_again(nbd + (3 * j + 0) * kFitThreads); y = ld_shared_again(nbd + (3 * j + 1) * kFitThreads); z = ld_shared_again(nbd + (3 * j + 2) * kFitThreads);
     };
     int o0 = 0, o1 = 0, o2 = 0;
     double nrm[3] = {0, 0, 0}, dpl = 0.0, wq = 0.0;
@@ -942,9 +805,9 @@ __device__ __forceinline__ void fit_point(const MapView& m, const CorrBuf& cb, c
         double mean[3] = {0, 0, 0};
 #pragma unroll
         for (int j = 0; j < 5; ++j) {
-            const float4 c = nbr(j);
+            const float4 c = __ldcs(nb.pts + gi + size_t(j) * nb.cap);
             const double x = double(c.x), y = double(c.y), z = double(c.z);
-            if constexpr (STRIDE > 0) { nbd[(3 * j + 0) * STRIDE] = x; nbd[(3 * j + 1) * STRIDE] = y; nbd[(3 * j + 2) * STRIDE] = z; }
+            nbd[(3 * j + 0) * kFitThreads] = x; nbd[(3 * j + 1) * kFitThreads] = y; nbd[(3 * j + 2) * kFitThreads] = z;
             mean[0] += x; mean[1] += y; mean[2] += z;
             if (cb.nn) {
                 const float dx = qx - c.x, dy = qy - c.y, dz = qz - c.z;
@@ -970,16 +833,11 @@ __device__ __forceinline__ void fit_point(const MapView& m, const CorrBuf& cb, c
         // eigenvector from its eigenvalue, then the smallest eigenvalue once more as the Rayleigh quotient of that vector (full
         // double precision where the lambda0 < 1e-6 gate reads it)
         double ev[3], no[3];
-#if SO_FIT_JACOBI
-        jacobi_eig<3, 12, false>(S, nullptr, ev);
-        eigvec3_from_value(sxx, sxy, sxz, syy, syz, szz, ev[0], no);
-#else
         sym3_eigenvalues(sxx, sxy, sxz, syy, syz, szz, ev);
         eigvec3_from_value(sxx, sxy, sxz, syy, syz, szz, ev[0], no);
         ev[0] = no[0] * (sxx * no[0] + sxy * no[1] + sxz * no[2]) + no[1] * (sxy * no[0] + syy * no[1] + syz * no[2]) +
                 no[2] * (sxz * no[0] + syz * no[1] + szz * no[2]);
         ev[1] = (sxx + syy + szz) - ev[0] - ev[2];
-#endif
         if (ev[0] < 1e-6 || ev[1] / ev[2] < 0.1) status = SO_MATCH_BAD_PCA_STRUCTURE;      // the reference's quotient, literally (:772)
         else {
             // What FeatureObservabilityAnalysis (:574-693) needs from the PCA -- the oriented normal (:553-561) and the
@@ -1092,15 +950,13 @@ __device__ __forceinline__ void fit_point(const MapView& m, const CorrBuf& cb, c
     cb.flags[gi] = make_uchar4((unsigned char)status, (unsigned char)o0, (unsigned char)o1, (unsigned char)o2);
 }
 
-__global__ void __launch_bounds__(kFitThreads, SO_FIT_MINB) k_fit(MapView m, BatchView bv, CorrBuf cb, NnBuf nb) {
+__global__ void __launch_bounds__(kFitThreads, kFitMinBlocks) k_fit(MapView m, BatchView bv, CorrBuf cb, NnBuf nb) {
     const int s = blockIdx.y;
     IcpState* st = bv.st + s;
     if (st->phase != PH_CORR) return;
     __shared__ double s_pose[7];
     __shared__ int s_hist[16];
-#if SO_FIT_NBD_SMEM
     __shared__ double s_nbd[15 * kFitThreads];      // the five neighbours in FP64, one column per thread (15 x 8 B x 256 = 30 KB)
-#endif
     if (threadIdx.x < 7) s_pose[threadIdx.x] = st->x[threadIdx.x];
     if (threadIdx.x < 16) s_hist[threadIdx.x] = 0;
     __syncthreads();
@@ -1109,71 +965,7 @@ __global__ void __launch_bounds__(kFitThreads, SO_FIT_MINB) k_fit(MapView m, Bat
     for (int rr = 0; rr < kFitPts; ++rr) {          // kFitPts points per thread
         const uint32_t i = (blockIdx.x * kFitPts + rr) * kFitThreads + threadIdx.x;
         const size_t gi = size_t(bv.offset[s]) + i;
-        if (i < n) {
-            const float4* npts = nb.pts + gi;
-#if SO_FIT_NBD_SMEM
-            fit_point<kFitThreads>(m, cb, nb, gi, __ldg(&bv.scan[gi]), s_pose, int(nb.pre[gi]), [&](int j) { return __ldcs(npts + size_t(j) * nb.cap); },
-                                   s_nbd + threadIdx.x, s_hist);
-#else
-            fit_point<0>(m, cb, nb, gi, __ldg(&bv.scan[gi]), s_pose, int(nb.pre[gi]), [&](int j) { return ld_f4_again(npts + size_t(j) * nb.cap); },
-                         nullptr, s_hist);
-#endif
-        }
-    }
-    __syncthreads();
-    if (threadIdx.x < 16 && s_hist[threadIdx.x]) atomicAdd(&bv.hist[s * kHistStride + threadIdx.x], s_hist[threadIdx.x]);
-}
-
-// ------------------------------------------------------------------------------------------------------------------
-// k_knn_fit: k_knn_scan and k_fit for the same point in one thread.  Both halves fit 64 registers, so fusing costs no
-// occupancy, and it (a) drops the 80 B/point neighbour hand-over through HBM (write + read back) and the second read of the
-// scan, (b) removes a kernel boundary per ICP iteration, and (c) lets warps that are in the integer-heavy search and warps
-// that are in the FP64-heavy fit share an SM, so both pipes stay busy.  The fit reads its neighbours straight from the
-// search-ordered map at the positions the search just visited (L1/L2 hits).
-// ------------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kThreads, 4) k_knn_fit(MapView m, BatchView bv, CorrBuf cb, NnBuf nb) {
-    const int s = blockIdx.y;
-    const IcpState* st = bv.st + s;
-    if (st->phase != PH_CORR) return;
-    __shared__ double s_pose[7];
-    __shared__ int s_hist[16];
-    __shared__ uint32_t s_buf[kBufCap * kThreads];
-    if (threadIdx.x < 7) s_pose[threadIdx.x] = st->x[threadIdx.x];
-    if (threadIdx.x < 16) s_hist[threadIdx.x] = 0;
-    __syncthreads();
-    const uint32_t n = uint32_t(st->n_points);
-    const uint32_t i = blockIdx.x * kThreads + threadIdx.x;
-    if (i < n) {
-        const size_t gi = size_t(bv.offset[s]) + i;
-        const float4 sp = __ldg(&bv.scan[gi]);
-        int pre = SO_MATCH_SKIPPED;
-        TopK<5> tk;
-        tk.init(m.bound_d2);
-        if (should_process(__float_as_uint(sp.w), st->sampling_rate)) {
-            const double pin[3] = {double(sp.x), double(sp.y), double(sp.z)};
-            double pf[3];
-            qrot(s_pose + 3, pin, pf);
-            const float qx = float(pf[0] + s_pose[0]), qy = float(pf[1] + s_pose[1]), qz = float(pf[2] + s_pose[2]);
-            QueryCell qc;
-            locate(m, qx, qy, qz, qc);
-            if (qc.slot < 0 || qc.nblock < 5) pre = SO_MATCH_NOT_ENOUGH_NEIGHBORS;
-            else {
-                float u_seed = -1.f;
-                if (st->icp_iter > 0 && nb.pre[gi] == SO_MATCH_SUCCESS) u_seed = seed_bound(m, qc, nb, gi, qx, qy, qz);        // see k_knn_scan
-                const GlobalGrid gg(m, qc.slot);
-                knn_select<5, SO_R1_OCTANT != 0>(gg, m, qc, qx, qy, qz, u_seed, m.bound_d2, s_buf, tk);
-                pre = tk.count() < 5 ? SO_MATCH_NEIGHBORS_TOO_FAR : SO_MATCH_SUCCESS;       // d2[4] > 3*planeRes_ (:741-744)
-            }
-        }
-        nb.pre[gi] = (unsigned char)pre;
-        nb.d5[gi] = tk.d2[4];
-        uint32_t pos[5];
-#pragma unroll
-        for (int j = 0; j < 5; ++j) {
-            pos[j] = tk.id[j] != 0xFFFFFFFFu ? tk.pos[j] : 0xFFFFFFFFu;
-            nb.pos[size_t(j) * nb.cap + gi] = pos[j];
-        }
-        fit_point<0>(m, cb, nb, gi, sp, s_pose, pre, [&](int j) { return ld_f4_again(m.pts + pos[j]); }, nullptr, s_hist);
+        if (i < n) fit_point(m, cb, nb, gi, __ldg(&bv.scan[gi]), s_pose, int(nb.pre[gi]), s_nbd + threadIdx.x, s_hist);
     }
     __syncthreads();
     if (threadIdx.x < 16 && s_hist[threadIdx.x]) atomicAdd(&bv.hist[s * kHistStride + threadIdx.x], s_hist[threadIdx.x]);
@@ -1235,9 +1027,33 @@ __device__ __forceinline__ void evaluate_body(const BatchView& bv, const CorrBuf
     reduce_to_partials(acc, bv, s);
 }
 
-#ifndef SO_EVAL_TMA
-#define SO_EVAL_TMA 1             // 0: k_evaluate streams its correspondences with per-thread loads (evaluate_body)
-#endif
+// ---- mbarrier / bulk-copy primitives (PTX ISA: mbarrier, cp.async.bulk) ----------------------------------------------------------
+__device__ __forceinline__ uint32_t smem_addr(const void* p) { return uint32_t(__cvta_generic_to_shared(p)); }
+__device__ __forceinline__ void mbar_init(unsigned long long* bar, uint32_t arrivals) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_addr(bar)), "r"(arrivals) : "memory");
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+}
+__device__ __forceinline__ void mbar_arrive_expect_tx(unsigned long long* bar, uint32_t bytes) {
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_addr(bar)), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_wait(unsigned long long* bar, uint32_t parity) {
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "SO_MBAR_WAIT:\n"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
+        "@p bra SO_MBAR_DONE;\n"
+        "bra SO_MBAR_WAIT;\n"
+        "SO_MBAR_DONE:\n"
+        "}\n" ::"r"(smem_addr(bar)), "r"(parity) : "memory");
+}
+// 1-D TMA: `bytes` (multiple of 16) from global to shared memory, completion counted on the mbarrier
+__device__ __forceinline__ void bulk_copy_g2s(void* dst_smem, const void* src_global, uint32_t bytes, unsigned long long* bar) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_addr(dst_smem)),
+                 "l"(src_global), "r"(bytes), "r"(smem_addr(bar))
+                 : "memory");
+}
+
 // The same evaluation with the 56 B/point stream staged by the TMA engine.  A CTA's points are eval_pts(n) consecutive tiles of
 // kThreads points, and a tile is three contiguous spans (normals+offset 32 B/pt, scan point 16 B/pt, weight 8 B/pt): one elected
 // thread enqueues three cp.async.bulk copies per tile into a kEvalStages-deep shared-memory ring, each stage completing on its
@@ -1330,11 +1146,7 @@ template <int PHASE>
 __global__ void __launch_bounds__(kThreads, 2) k_evaluate(BatchView bv, CorrBuf cb) {
     const int s = blockIdx.y;
     if (bv.st[s].phase != PHASE) return;
-#if SO_EVAL_TMA
     evaluate_body_tma<PHASE>(bv, cb, s);
-#else
-    evaluate_body<PHASE>(bv, cb, s);
-#endif
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -1408,7 +1220,7 @@ __global__ void __launch_bounds__(kThreads) k_edge_fit(MapView m, BatchView bv, 
         locate(m, qx, qy, qz, qc);
         // "<10 points in the block": the reference indexes with size_t(-1) (LocalMap.h:404-419); treated as NOT_ENOUGH_NEIGHBORS
         if (qc.slot >= 0 && qc.nblock >= 10) {
-            knn_search<10>(GlobalGrid(m, qc.slot), m, qc, qx, qy, qz, 0.f, s_buf, tk);
+            knn_search<10>(BlockGrid(m, qc.slot), m, qc, qx, qy, qz, 0.f, s_buf, tk);
             float P[10][3];
 #pragma unroll
             for (int j = 0; j < 10; ++j) { const float4 c = __ldg(&m.pts[tk.pos[j]]); P[j][0] = c.x; P[j][1] = c.y; P[j][2] = c.z; }
@@ -1644,7 +1456,7 @@ __global__ void k_loop_cond(const IcpState* __restrict__ st, uint32_t n_scans, c
 // ------------------------------------------------------------------------------------------------------------------
 // k_knn: LocalMap::nearestKSearchSurf for a batch of world-frame queries (so_knn / so_knn_device)
 // ------------------------------------------------------------------------------------------------------------------
-// brick-order key of every query (so_knn* orders large query sets first, for the same reason scans are ordered)
+// cell-order key of every query (so_knn* orders large query sets first, for the same reason scans are ordered)
 __global__ void __launch_bounds__(kThreads) k_query_keys(MapView m, const float4* __restrict__ q, size_t nq, uint32_t* __restrict__ keys,
                                                          uint32_t* __restrict__ vals) {
     const size_t i = size_t(blockIdx.x) * kThreads + threadIdx.x;
@@ -1656,37 +1468,23 @@ __global__ void __launch_bounds__(kThreads) k_query_keys(MapView m, const float4
     vals[i] = uint32_t(i);
 }
 
-// 128 queries per CTA.  ORDERED: the queries arrive in brick order (`order`), so the CTA first tries the shared candidate tile.
-template <int K, bool ORDERED>
-__global__ void __launch_bounds__(kTileThreads) k_knn(MapView m, const float4* __restrict__ q, const uint32_t* __restrict__ order, size_t nq,
-                                                      float max_d2, uint32_t* __restrict__ idx, float* __restrict__ d2) {
-    __shared__ uint32_t s_buf[kBufCap * kTileThreads];
-#if SO_KNN_TILE
-    __shared__ TileSmem s_tile;
-#endif
-    const size_t j0 = size_t(blockIdx.x) * kTileThreads;
+// kKnnThreads queries per CTA; `order` (optional): the queries in cell order, thread j takes the j-th of them.
+template <int K>
+__global__ void __launch_bounds__(kKnnThreads) k_knn(MapView m, const float4* __restrict__ q, const uint32_t* __restrict__ order, size_t nq,
+                                                     float max_d2, uint32_t* __restrict__ idx, float* __restrict__ d2) {
+    __shared__ uint32_t s_buf[kBufCap * kKnnThreads];
+    const size_t j0 = size_t(blockIdx.x) * kKnnThreads;
     if (j0 >= nq) return;
     const size_t j = j0 + threadIdx.x;
     const bool in_range = j < nq;
-    const size_t i = in_range ? (order ? size_t(order[j]) : j) : 0;        // thread j handles the j-th query in brick order, answers in caller order
+    const size_t i = in_range ? (order ? size_t(order[j]) : j) : 0;        // thread j handles the j-th query in cell order, answers in caller order
     const float4 p = __ldg(&q[i]);
     TopK<K> tk;
     tk.init(max_d2 > 0.f ? max_d2 : FLT_MAX);
     QueryCell qc;
     qc.slot = -1; qc.nblock = 0; qc.c[0] = qc.c[1] = qc.c[2] = 0; qc.f[0] = qc.f[1] = qc.f[2] = 0.f;
     if (in_range) locate(m, p.x, p.y, p.z, qc);
-    const bool searchable = in_range && qc.slot >= 0;
-#if SO_KNN_TILE
-    TileGrid tg;
-    const bool tiled = ORDERED && build_tile(m, s_tile, searchable, qc, tg);        // every thread takes part in the build
-#endif
-    if (searchable) {
-#if SO_KNN_TILE
-        if (tiled) knn_search<K>(tg, m, qc, p.x, p.y, p.z, max_d2, s_buf, tk);
-        else
-#endif
-            knn_search<K>(GlobalGrid(m, qc.slot), m, qc, p.x, p.y, p.z, max_d2, s_buf, tk);
-    }
+    if (in_range && qc.slot >= 0) knn_search<K>(BlockGrid(m, qc.slot), m, qc, p.x, p.y, p.z, max_d2, s_buf, tk);
     if (!in_range) return;
 #pragma unroll
     for (int jj = 0; jj < K; ++jj) {
@@ -1738,17 +1536,12 @@ void launch_scan_gather(const float4* in, const uint32_t* vals, const uint64_t* 
 // medge / eb / grid_e: edge branch (grid_e == 0: idle); k_lm_step sums the partials of both branches.
 void launch_match(const MapView& m, const BatchView& bv, const CorrBuf& cb, const NnBuf& nb, uint32_t grid_x, uint32_t n_scans, cudaStream_t st, int part) {
     if (!grid_x) return;
-#if SO_FUSE_KNN_FIT
-    (void)part;
-    k_knn_fit<<<dim3(grid_x, n_scans), kThreads, 0, st>>>(m, bv, cb, nb);
-#else
     if (part != 2) {
         if (bv.coop_knn) k_knn_scan_coop<<<dim3(grid_x * (kThreads / kCoopWarps), n_scans), kThreads, 0, st>>>(m, bv, nb);
-        else k_knn_scan<<<dim3(grid_x * (kThreads / kTileThreads), n_scans), kTileThreads, 0, st>>>(m, bv, nb);
+        else k_knn_scan<<<dim3(grid_x * (kThreads / kKnnThreads), n_scans), kKnnThreads, 0, st>>>(m, bv, nb);
     }
     const uint32_t gf = (grid_x * kThreads + kFitPts * kFitThreads - 1) / (kFitPts * kFitThreads);
     if (part != 1) k_fit<<<dim3(gf, n_scans), kFitThreads, 0, st>>>(m, bv, cb, nb);
-#endif
 }
 void launch_inject(const MapView& m, const float4* by_id, uint32_t n_map, const BatchView& bv, const NnBuf& nb, const uint32_t* ids, int n_trace_iters,
                    uint32_t grid_x, uint32_t n_scans, cudaStream_t st) {
@@ -1785,9 +1578,7 @@ void launch_query_keys(const MapView& m, const float4* q, size_t nq, uint32_t* k
 }
 template <int K>
 static void launch_knn_k(const MapView& m, const float4* q, const uint32_t* order, size_t nq, float max_d2, uint32_t* idx, float* d2, cudaStream_t st) {
-    const uint32_t grid = uint32_t((nq + kTileThreads - 1) / kTileThreads);
-    if (order) k_knn<K, true><<<grid, kTileThreads, 0, st>>>(m, q, order, nq, max_d2, idx, d2);
-    else k_knn<K, false><<<grid, kTileThreads, 0, st>>>(m, q, order, nq, max_d2, idx, d2);
+    k_knn<K><<<uint32_t((nq + kKnnThreads - 1) / kKnnThreads), kKnnThreads, 0, st>>>(m, q, order, nq, max_d2, idx, d2);
 }
 int launch_knn(const MapView& m, const float4* q, const uint32_t* order, size_t nq, int k, float max_d2, uint32_t* idx, float* d2, cudaStream_t st) {
     switch (k) {

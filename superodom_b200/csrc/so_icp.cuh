@@ -45,17 +45,11 @@ struct NnBuf {
     float4* pts;         // [5][cap] the neighbours themselves {x,y,z,bitcast(id)}: k_fit streams them instead of gathering
     float* d5;           // [cap] exact 5th-neighbour d2 of the last search (decides whether its neighbours seed the next one)
     unsigned char* pre;  // [cap] SO_MATCH_SKIPPED / NOT_ENOUGH_NEIGHBORS / NEIGHBORS_TOO_FAR / SUCCESS (= has 5 neighbours)
-    float4* vq;          // [cap] record of the last FULL search that found 5 neighbours: the query position {x,y,z} and, in w, a lower
-                         //       bound on the squared distance to every other point of the block (w < 0: no record).  While the query
-                         //       stays close enough to that position the stored five provably remain its 5-NN (k_knn_scan).
     size_t cap;
 };
 
-#ifndef SO_EVAL_PTS
-#define SO_EVAL_PTS 16
-#endif
 constexpr uint32_t kCoopMaxGrid = 32;     // k_knn_scan_coop serves scans of up to 32 x 256 queries (a decimated live scan is ~2 000)
-constexpr int kEvalPts = SO_EVAL_PTS;     // points per thread in k_evaluate (large scans)
+constexpr int kEvalPts = 16;              // points per thread in k_evaluate (large scans); part of the partial-sum layout, so of the result bits
 // Points per thread of the evaluation kernels as a function of the scan's own size (never of the batch it is in, so that a scan's
 // partial sums -- and with them its result, bit for bit -- do not depend on its neighbours): small scans spread over more CTAs,
 // because ONE CTA looping over 16 points per thread was most of a latency-bound optimiser step.
@@ -70,38 +64,13 @@ __host__ inline uint32_t eval_grid(uint32_t n_max) {
 }
 // k_fit launch shape, re-measured on an H100 80GB HBM3 (700 W limit; scripts/ab_knn.py, 64 cfg2 scans = 8.4 M points per launch,
 // two alternating rounds, ms per launch): 2 points x 256 threads x 4 CTAs/SM 0.554-0.560; 1 point per thread 0.544-0.545;
-// 128 threads x 8 CTAs/SM 0.552-0.554; neighbours re-read and re-converted per pass (SO_FIT_NBD_SMEM=0) 0.594-0.609.  The
-// defaults are kept: the other shapes are within 3 % and were not carried through the full suite.
-#ifndef SO_FIT_PTS
-#define SO_FIT_PTS 2
-#endif
-constexpr int kFitPts = SO_FIT_PTS;      // points per thread in k_fit
+// 128 threads x 8 CTAs/SM 0.552-0.554; neighbours re-read and re-converted per pass instead of kept in shared memory 0.594-0.609.
+// The defaults are kept: the other shapes are within 3 % and were not carried through the full suite.
 // k_fit only matches / fits; the first evaluation of the solve is a k_evaluate<PH_CORR> launch, so k_fit carries no
 // normal-equation accumulators (64 registers, 4 CTAs per SM).
-#ifndef SO_FIT_JACOBI
-#define SO_FIT_JACOBI 0          // 1: eigenvalues of the 3x3 scatter by cyclic Jacobi (round-1 kernel; A/B aid)
-#endif
-#ifndef SO_FIT_THREADS
-#define SO_FIT_THREADS 256
-#endif
-#ifndef SO_FIT_MINB
-#define SO_FIT_MINB 4
-#endif
-constexpr int kFitThreads = SO_FIT_THREADS;
-// 1: k_fit widens each neighbour coordinate to FP64 once and keeps it in shared memory for the later passes (15 doubles per
-// thread); 0: every pass re-reads the neighbour (L1 hit) and converts it again.
-#ifndef SO_FIT_NBD_SMEM
-#define SO_FIT_NBD_SMEM 1
-#endif
-// 1: search and fit of a point run in one kernel (k_knn_fit); 0: k_knn_scan hands the neighbours to k_fit through HBM.
-// The stage is issue-bound on the SUM of both halves' instructions, so sharing an SM between search and fit warps buys little:
-// on an H100 80GB HBM3 (700 W limit, scripts/ab_knn.py, 64 cfg2 scans) fused 1.72 ms vs split 1.05 + 0.70 ms per matching stage
-// (2 %), and so_register_injected (the reference-octree parity proof) needs the split form.  Split stays the
-// default; the fused form saves 105 B/point of HBM traffic and the 80 B/point neighbour buffer.
-#ifndef SO_FUSE_KNN_FIT
-#define SO_FUSE_KNN_FIT 0
-#endif
-constexpr int kCorrLaunches = SO_FUSE_KNN_FIT ? 1 : 2;      // launches of the correspondence stage before the first evaluation
+constexpr int kFitPts = 2;               // points per thread in k_fit
+constexpr int kFitThreads = 256;
+constexpr int kFitMinBlocks = 4;
 
 void launch_scan_keys(const MapView& m, const BatchView& bv, uint64_t* keys, uint32_t* vals, uint32_t grid_x, uint32_t n_scans, int cell_bits, bool key32,
                       bool compact, cudaStream_t st);
@@ -110,7 +79,7 @@ constexpr uint32_t kPrepareSmallCap = 4096;    // survivors k_prepare_small can 
 void launch_prepare_small(const MapView& m, const BatchView& bv, float4* out, uint32_t n_scans, int key_bits, uint32_t max_kept, cudaStream_t st);
 void launch_scan_gather(const float4* in, const uint32_t* vals, const uint64_t* keys, size_t first, const uint32_t* offset, size_t total, float4* out,
                         int cell_bits, bool key32, cudaStream_t st);
-// part: 0 = the whole stage; split build only: 1 = k_knn_scan alone, 2 = k_fit alone (profiling)
+// part: 0 = the whole stage; 1 = k_knn_scan alone, 2 = k_fit alone (profiling)
 void launch_match(const MapView& m, const BatchView& bv, const CorrBuf& cb, const NnBuf& nb, uint32_t grid_x, uint32_t n_scans, cudaStream_t st, int part = 0);
 void launch_inject(const MapView& m, const float4* by_id, uint32_t n_map, const BatchView& bv, const NnBuf& nb, const uint32_t* ids, int n_trace_iters,
                    uint32_t grid_x, uint32_t n_scans, cudaStream_t st);
