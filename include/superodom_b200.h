@@ -290,6 +290,68 @@ int so_knn_device(so_ctx* ctx, const void* d_q_xyzw, size_t nq, int k, float max
  * *n_out.  Returns SO_OK or SO_ERR_ARG. */
 int so_sampling_indices(uint32_t n, int32_t max_surface_features, uint32_t* out, size_t cap, size_t* n_out);
 
+/* ---- global localization against the prior map ------------------------------------------------------------------ */
+/* extends: localization mode (laserMapping.cpp:163-173 loads the prior map, :306-313 takes the start pose from init_x ... init_yaw
+ * unchanged).  Instead of an exact start pose, search a region around a rough centre: every x/y/z voxel shift and yaw step of the
+ * scan is scored against an occupancy bitmap of the surf map, the best hypotheses (after non-maximum suppression) are registered
+ * with the ordinary ICP path, and the registration with the most accepted plane correspondences wins.  Roll and pitch are taken
+ * from the centre (IMU gravity, as initializeFirstFrame does, laserMapping.cpp:281-298).  Zero fields take the defaults shown. */
+typedef struct {
+    double half_x, half_y, half_z;  /* search half-extents (m) around the centre; 0 = that axis is not searched */
+    double yaw_half;                /* yaw half-range (rad) around the centre's yaw; >= pi = the full circle */
+    double res;                     /* voxel edge of the bitmap and translation step (m), default 0.25 */
+    double yaw_step;                /* yaw step (rad), default 2 deg */
+    double max_range;               /* scan points farther than this are not scored (m), default 40 */
+    int32_t score_points;           /* scan points scored (shouldProcessPoint decimation), default 1024, at most 4096 */
+    int32_t dilate;                 /* bitmap dilation (voxels, cube neighbourhood), default 1, at most 8 */
+    int32_t k;                      /* candidates refined, default 16, at most 64 */
+    int32_t pad_;
+    double nms_xy;                  /* suppression radius in x/y (m), default 1.0 */
+    double nms_yaw;                 /* suppression half-width in yaw (rad), default 10 deg */
+} so_global_opts;
+
+/* One refined candidate, in rank order (score descending, hypothesis index ascending). */
+typedef struct {
+    double prior[7];        /* hypothesis pose the registration started from */
+    int32_t score;          /* occupied bitmap cells hit by the score points */
+    int32_t n_success;      /* SO_MATCH_SUCCESS correspondences of the final ICP iteration */
+    double cost;            /* final cost of the last ICP iteration */
+    double pose[7];         /* so_icp_result.pose of its registration */
+    int32_t status;         /* so_icp_result.status */
+    int32_t pad_;
+} so_global_candidate;
+
+typedef struct {
+    double pose[7];         /* the winner's refined pose; the centre when status != SO_OK */
+    int32_t status;         /* SO_OK / SO_STATUS_NO_CORRESPONDENCES / SO_STATUS_NOT_ENOUGH_FEATURES */
+    int32_t winner;         /* index into the candidate list, -1 when none */
+    int32_t n_candidates;   /* candidates kept by the suppression and registered */
+    int32_t best_score;     /* score of the best hypothesis */
+    uint64_t n_hypotheses;  /* NX * NY * NZ * NYAW */
+    int32_t n_score_points; /* scan points scored */
+    int32_t pad_;
+    double time_raster_ms, time_dilate_ms, time_score_ms, time_sort_ms;  /* device time of each search stage (CUDA events) */
+    double time_refine_ms;  /* candidate read-back, suppression and registrations (host clock) */
+    double time_total_ms;   /* whole call (host clock) */
+    so_icp_result icp;      /* the winner's registration (zeroed when there is none) */
+} so_global_result;
+
+/* Global localization of a sensor-frame surf cloud (layout as so_register) around center_pose7.  Writes up to cap candidates to
+ * cands (may be NULL with cap 0).  The map is not modified and not shifted, an attached pose sink gets no rows; afterwards
+ * so_map_add_registered_scan inserts this cloud.  Returns SO_OK, a soft status, or an error (argument errors before any device
+ * work; SO_ERR_CAPACITY above 2^24 hypotheses, a bitmap above 2^32 bits or a cloud above max_scan_points). */
+int so_localize_global(so_ctx* ctx, const void* xyzi, size_t n, size_t stride_bytes, size_t intensity_offset, const double center_pose7[7],
+                       const so_global_opts* gopts, const so_icp_opts* opts, so_global_candidate* cands, size_t cap,
+                       so_global_result* out);
+/* Stage hook of so_localize_global: the uint16 score of every hypothesis, index ((yaw * NZ + z) * NY + y) * NX + x, and
+ * dims = {NX, NY, NZ, NYAW}.  Needs cap >= the hypothesis count; *n_score_points (optional) receives the points scored. */
+int so_localize_scores(so_ctx* ctx, const void* xyzi, size_t n, size_t stride_bytes, size_t intensity_offset, const double center_pose7[7],
+                       const so_global_opts* gopts, uint16_t* scores, size_t cap, int32_t dims[4], int32_t* n_score_points);
+/* Host-only (needs no device): the argument checks of so_localize_global's options, dims = {NX, NY, NZ, NYAW}, the hypothesis
+ * count and the size of one occupancy bitmap.  Returns SO_OK, SO_ERR_ARG or SO_ERR_CAPACITY (dims and counts are filled for the
+ * capacity error too). */
+int so_localize_global_size(const so_global_opts* gopts, int32_t dims[4], uint64_t* n_hypotheses, uint64_t* bitmap_bytes);
+
 /* ---- instrumentation ------------------------------------------------------------------------------ */
 /* Number of this library's kernels launched since the last reset (bench.py gpu_launches). */
 uint64_t so_kernel_launches(so_ctx* ctx, int reset);
@@ -299,7 +361,8 @@ int so_bytes_copied(so_ctx* ctx, uint64_t* h2d, uint64_t* d2h, int reset);
 /* Accumulated device time (ms, CUDA events on the context stream) and launch count of a kernel class since the last
  * reset; classes: 0 k_knn_scan (scan k-NN), 1 k_evaluate +
  * k_lm_step (LM step), 2 k_knn (so_knn*), 3 scan ordering / map build / map insert / scan preparation, 4 first evaluation of
- * a solve (k_evaluate + k_lm_step iteration zero), 5 k_fit (plane fit).
+ * a solve (k_evaluate + k_lm_step iteration zero), 5 k_fit (plane fit), 6 global localization search (bitmap raster, dilation,
+ * hypothesis scoring, key sort).
  * Profiling mode serialises kernels; enable only for roofline runs. */
 /* Build-time switches of the loaded library.  Bit 0 (SO_BUILD_FUSED_MATCH, search and fit as one kernel) is reserved: this
  * library always runs them as two kernels and returns 0. */

@@ -316,6 +316,32 @@ public:
         lasttimeLaserOdometry = timeLaserOdometry;
     }
 
+    // Global localization against the prior map (so_localize_global; extends localization mode, laserMapping.cpp:163-173,306-313):
+    // call once after the prior map is loaded and before the first Localization(), with a rough start pose whose roll and pitch are
+    // trusted (IMU gravity).  Sets T_w_lidar and last_T_w_lidar as initializeFirstFrame does in localization mode -- to the refined
+    // pose, or to the centre when nothing was found.  Returns the status; last_global holds the whole result.
+    so_global_result last_global{};
+    template <class CloudPtr>
+    int globalLocalize(const CloudPtr& planner_point, const Transformd& centre, const so_global_opts& opts) {
+        localMap.sync_resolution();
+        size_t stride, ioff;
+        using PointT = typename std::decay<decltype(planner_point->points[0])>::type;
+        point_layout<PointT>(&stride, &ioff);
+        so_icp_opts o{};
+        o.max_icp_iters = int32_t(LocalizationICPMaxIter);
+        o.max_surface_features = OptSet.max_surface_features;
+        o.lm_max_iterations = 4;
+        o.yaw_ratio = OptSet.yaw_ratio;
+        double c[7];
+        centre.to_pose7(c);
+        const void* surf = planner_point->size() ? planner_point->points.data() : nullptr;
+        const int rc = so_localize_global(context.h, surf, planner_point->size(), stride, ioff, c, &opts, &o, nullptr, 0, &last_global);
+        check(rc, "so_localize_global");
+        T_w_lidar = Transformd::from_pose7(last_global.pose);
+        last_T_w_lidar = T_w_lidar;
+        return rc;
+    }
+
     // LidarSLAM::EstimateLidarUncertainty (LidarSlam.cpp:915-975)
     void EstimateLidarUncertainty() {
         const auto& h = PlaneFeatureHistogramObs;

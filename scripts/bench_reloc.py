@@ -1,0 +1,114 @@
+#!/usr/bin/env python3
+"""bench_reloc.py -- global localization (so_localize_global) on the cfg2 map (1 M points) with one OS1-128 scan and the default
+search: half 10 m in x and y at 0.25 m, the full circle at 2 deg = 81 x 81 x 180 = 1 180 980 hypotheses x 1024 score points.
+
+Prints one JSON line: median whole-call wall time over --calls calls after --warmup calls, the per-stage device times (CUDA events
+in the call; profile class 6 from one extra profiled call), hypotheses/s and bitmap lookups/s of the scoring kernel, the bitmap
+size, the recovery error against the truth, and the card name and power limit read in the same run.  --cpu adds one single-thread
+run of the numpy restatement of the search (tests/global_localization_numpy.py) for a speed-up figure.  Writes nothing.
+"""
+import argparse
+import json
+import math
+import os
+import sys
+import time
+
+for v in ("OMP_NUM_THREADS", "OPENBLAS_NUM_THREADS", "MKL_NUM_THREADS"):
+    os.environ.setdefault(v, "1")
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
+
+import numpy as np  # noqa: E402
+
+
+def card():
+    name, limit = None, None
+    try:
+        import torch
+        name = torch.cuda.get_device_name(0)
+    except Exception:
+        pass
+    try:
+        import pynvml as nv
+        nv.nvmlInit()
+        h = nv.nvmlDeviceGetHandleByIndex(0)
+        limit = nv.nvmlDeviceGetPowerManagementLimit(h) / 1000.0
+        if name is None:
+            name = nv.nvmlDeviceGetName(h)
+            name = name.decode() if isinstance(name, bytes) else name
+    except Exception:
+        pass
+    return name, limit
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--calls", type=int, default=20)
+    ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--scan", type=int, default=0, help="cfg2 scan index")
+    ap.add_argument("--cpu", action="store_true")
+    a = ap.parse_args()
+    from superodom_b200 import api, synth
+    import global_localization_numpy as GN
+    scene, map_xyzi = synth.make_map_for("cfg2")
+    case = synth.make_case_on(scene, map_xyzi, "cfg2", a.scan)
+    truth = case["pose_true"]
+    rng = np.random.default_rng(7100 + a.scan)
+    d = rng.uniform(-8.0, 8.0, 2)
+    dyaw = rng.uniform(-math.pi, math.pi)
+    q = synth.quat_mul(np.array([0.0, 0.0, math.sin(dyaw / 2), math.cos(dyaw / 2)]), truth[3:])
+    center = np.r_[truth[0] + d[0], truth[1] + d[1], truth[2], q / np.linalg.norm(q)]
+    region = dict(half_x=10.0, half_y=10.0, yaw_half=math.pi)
+    g = api.global_opts(**region)
+    dims, n_hyp, bitmap_bytes = api.localize_global_size(g)
+    ctx = api.Context(max_map_points=len(map_xyzi) + (1 << 18), max_scan_points=262144, plane_res=0.2, max_batch=16)
+    ctx.map_set_points(map_xyzi)
+    scan = case["scan_xyzi"]
+    for _ in range(a.warmup):
+        ctx.localize_global(scan, center, 20, g)
+    wall, st = [], {k: [] for k in ("raster", "dilate", "score", "sort", "refine")}
+    for _ in range(a.calls):
+        t0 = time.perf_counter()
+        pose, res, cands = ctx.localize_global(scan, center, 20, g)      # returns after a device synchronise
+        wall.append((time.perf_counter() - t0) * 1e3)
+        for k in st:
+            st[k].append(getattr(res, f"time_{k}_ms"))
+    ctx.profile_get(6, reset=True)
+    ctx.profile_enable(True)
+    ctx.localize_global(scan, center, 20, g)
+    ctx.profile_enable(False)
+    prof_ms, prof_n = ctx.profile_get(6, reset=True)
+    med = {k: float(np.median(v)) for k, v in st.items()}
+    ns = sorted((c.n_success for c in cands if c.status == 0), reverse=True)
+    name, limit = card()
+    out = {
+        "workload": f"cfg2 map ({len(map_xyzi)} pts), OS1-128 scan {a.scan} ({len(scan)} pts), centre {np.linalg.norm(d):.2f} m / "
+                    f"{math.degrees(dyaw):.1f} deg off, default search {dims} = {n_hyp} hypotheses x {res.n_score_points} score points",
+        "card": name, "power_limit_w": limit,
+        "calls": a.calls, "warmup": a.warmup,
+        "wall_ms_median": float(np.median(wall)), "wall_ms_min": float(np.min(wall)), "wall_ms_max": float(np.max(wall)),
+        "stage_ms_median": med,
+        "profile_class6_ms": prof_ms, "profile_class6_launches": prof_n,
+        "hypotheses_per_s": n_hyp / (med["score"] * 1e-3),
+        "lookups_per_s": n_hyp * res.n_score_points / (med["score"] * 1e-3),
+        "bitmap_bytes": bitmap_bytes,
+        "status": res.status, "n_candidates": res.n_candidates, "best_score": res.best_score,
+        "winner_success": ns[0] if ns else 0, "runner_up_success": ns[1] if len(ns) > 1 else 0,
+        "err_m": float(np.linalg.norm(pose[:3] - truth[:3])),
+        "err_deg": math.degrees(2.0 * math.acos(min(1.0, abs(float(np.dot(pose[3:], truth[3:])))))),
+    }
+    if a.cpu:
+        t0 = time.perf_counter()
+        GN.localize_scores_numpy(scan, center, ctx.map_download(0)[:, :3], **region)
+        cpu_ms = (time.perf_counter() - t0) * 1e3
+        out["cpu_numpy_search_ms"] = cpu_ms
+        out["speedup_search_vs_cpu"] = cpu_ms / (med["raster"] + med["dilate"] + med["score"] + med["sort"])
+    ctx.close()
+    print(json.dumps(out))
+
+
+if __name__ == "__main__":
+    main()

@@ -21,7 +21,7 @@ EXPORTS = [
     "so_map_set_resolution", "so_map_set_origin", "so_map_get_origin", "so_map_shift", "so_map_set_points",
     "so_map_set_edge_points", "so_map_add_surf", "so_map_add_edge", "so_map_add_scan", "so_map_add_registered_scan", "so_map_add_scan_edge", "so_map_counts_5x5", "so_map_download", "so_map_size",
     "so_scan_prefilter", "so_scan_deskew", "so_scan_extract_uniform", "so_register", "so_register_prefiltered", "so_register_injected", "so_set_pose_sink", "so_register_batch", "so_register_batch_edges", "so_register_batch_device", "so_correspond", "so_correspond_edge", "so_evaluate",
-    "so_knn", "so_knn_device", "so_sampling_indices", "so_kernel_launches", "so_bytes_copied", "so_build_flags", "so_profile_enable", "so_profile_get",
+    "so_knn", "so_knn_device", "so_sampling_indices", "so_localize_global", "so_localize_scores", "so_localize_global_size", "so_kernel_launches", "so_bytes_copied", "so_build_flags", "so_profile_enable", "so_profile_get",
 ]
 
 
@@ -51,6 +51,31 @@ class IcpResult(C.Structure):
                 ("map_surf_5x5", C.c_int32), ("map_edge_5x5", C.c_int32), ("scan_surf_num", C.c_int32), ("scan_edge_num", C.c_int32),
                 ("pos_in_localmap", C.c_int32 * 3), ("prediction_source", C.c_int32),
                 ("time_ms", C.c_double), ("time_total_ms", C.c_double), ("knn_searched", C.c_int32), ("knn_verified", C.c_int32)]
+
+
+class GlobalOpts(C.Structure):
+    """so_global_opts: zero fields take the defaults (res 0.25 m, yaw_step 2 deg, max_range 40 m, score_points 1024, dilate 1,
+    k 16, nms_xy 1 m, nms_yaw 10 deg)."""
+    _fields_ = [("half_x", C.c_double), ("half_y", C.c_double), ("half_z", C.c_double), ("yaw_half", C.c_double),
+                ("res", C.c_double), ("yaw_step", C.c_double), ("max_range", C.c_double), ("score_points", C.c_int32),
+                ("dilate", C.c_int32), ("k", C.c_int32), ("pad_", C.c_int32), ("nms_xy", C.c_double), ("nms_yaw", C.c_double)]
+
+
+class GlobalCandidate(C.Structure):
+    _fields_ = [("prior", C.c_double * 7), ("score", C.c_int32), ("n_success", C.c_int32), ("cost", C.c_double),
+                ("pose", C.c_double * 7), ("status", C.c_int32), ("pad_", C.c_int32)]
+
+
+class GlobalResult(C.Structure):
+    _fields_ = [("pose", C.c_double * 7), ("status", C.c_int32), ("winner", C.c_int32), ("n_candidates", C.c_int32),
+                ("best_score", C.c_int32), ("n_hypotheses", C.c_uint64), ("n_score_points", C.c_int32), ("pad_", C.c_int32),
+                ("time_raster_ms", C.c_double), ("time_dilate_ms", C.c_double), ("time_score_ms", C.c_double),
+                ("time_sort_ms", C.c_double), ("time_refine_ms", C.c_double), ("time_total_ms", C.c_double), ("icp", IcpResult)]
+
+
+def global_opts(half_x=0.0, half_y=0.0, half_z=0.0, yaw_half=0.0, res=0.0, yaw_step=0.0, max_range=0.0, score_points=0, dilate=0,
+                k=0, nms_xy=0.0, nms_yaw=0.0) -> GlobalOpts:
+    return GlobalOpts(half_x, half_y, half_z, yaw_half, res, yaw_step, max_range, score_points, dilate, k, 0, nms_xy, nms_yaw)
 
 
 CORR_DTYPE = np.dtype([("n", "<f8", 3), ("d", "<f8"), ("w", "<f8"), ("nn", "<u4", 5), ("nn_d2", "<f4", 5),
@@ -113,6 +138,11 @@ def load_library():
     L.so_knn.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_int, C.c_float, C.c_void_p, C.c_void_p]
     L.so_knn_device.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_float, C.c_void_p, C.c_void_p]
     L.so_sampling_indices.argtypes = [C.c_uint32, C.c_int32, C.c_void_p, C.c_size_t, C.c_void_p]
+    L.so_localize_global.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p,
+                                     C.c_void_p, C.c_size_t, C.c_void_p]
+    L.so_localize_scores.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p,
+                                     C.c_size_t, C.c_void_p, C.c_void_p]
+    L.so_localize_global_size.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     L.so_kernel_launches.restype = C.c_uint64
     L.so_kernel_launches.argtypes = [C.c_void_p, C.c_int]
     L.so_bytes_copied.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
@@ -135,6 +165,21 @@ def sampling_indices(n: int, max_surface_features: int) -> np.ndarray:
     if L.so_sampling_indices(n, max_surface_features, out.ctypes.data_as(C.c_void_p), n, C.byref(cnt)) != 0:
         raise SuperOdomError("so_sampling_indices failed")
     return out[:cnt.value].copy()
+
+
+def localize_global_size(opts: GlobalOpts | None = None, **kw):
+    """Host-only: (dims (NX, NY, NZ, NYAW), hypothesis count, bitmap bytes) of a global localization search; raises SuperOdomError
+    with .code = SO_ERR_ARG (-1) / SO_ERR_CAPACITY (-3) on invalid or too large searches."""
+    L = load_library()
+    o = opts if opts is not None else global_opts(**kw)
+    dims = np.zeros(4, np.int32)
+    nh, nb = C.c_uint64(), C.c_uint64()
+    rc = L.so_localize_global_size(C.byref(o), _p(dims), C.byref(nh), C.byref(nb))
+    if rc < 0:
+        e = SuperOdomError(f"so_localize_global_size failed ({rc}): " + L.so_last_error().decode())
+        e.code = rc
+        raise e
+    return tuple(int(v) for v in dims), nh.value, nb.value
 
 
 def device_available() -> bool:
@@ -436,6 +481,37 @@ class Context:
         cost = C.c_double()
         self._chk(self.L.so_evaluate(self.h, _p(pose), _p(H), _p(g), C.byref(cost)), "so_evaluate")
         return H, g, cost.value
+
+    # ---- global localization
+    def localize_global(self, scan_xyzi: np.ndarray, center_pose7, max_icp_iters: int, opts: GlobalOpts | None = None,
+                        max_surface_features: int = 0, **kw):
+        """Global localization of a sensor-frame surf cloud around center_pose7 -> (pose [7], GlobalResult, [GlobalCandidate]).
+        Soft statuses are in result.status; errors raise."""
+        s = np.ascontiguousarray(scan_xyzi, dtype=np.float32)
+        c = np.ascontiguousarray(center_pose7, dtype=np.float64)
+        g = opts if opts is not None else global_opts()
+        o = self._opts(max_icp_iters, max_surface_features, **kw)
+        cands = (GlobalCandidate * 64)()
+        r = GlobalResult()
+        stride = s.shape[1] * 4
+        self._chk(self.L.so_localize_global(self.h, _p(s) if len(s) else None, s.shape[0], stride, 12 if s.shape[1] >= 4 else stride, _p(c),
+                                            C.byref(g), C.byref(o), cands, 64, C.byref(r)), "so_localize_global")
+        return np.array(r.pose), r, [cands[i] for i in range(min(r.n_candidates, 64))]
+
+    def localize_scores(self, scan_xyzi: np.ndarray, center_pose7, opts: GlobalOpts | None = None):
+        """Score of every hypothesis -> (uint16 [NYAW, NZ, NY, NX], number of score points)."""
+        s = np.ascontiguousarray(scan_xyzi, dtype=np.float32)
+        c = np.ascontiguousarray(center_pose7, dtype=np.float64)
+        g = opts if opts is not None else global_opts()
+        (nx, ny, nz, nyaw), nh, _ = localize_global_size(g)
+        scores = np.zeros(max(nh, 1), np.uint16)
+        dims = np.zeros(4, np.int32)
+        npts = C.c_int32()
+        stride = s.shape[1] * 4
+        self._chk(self.L.so_localize_scores(self.h, _p(s) if len(s) else None, s.shape[0], stride, 12 if s.shape[1] >= 4 else stride, _p(c),
+                                            C.byref(g), _p(scores), nh, _p(dims), C.byref(npts)), "so_localize_scores")
+        assert tuple(dims) == (nx, ny, nz, nyaw)
+        return scores[:nh].reshape(nyaw, nz, ny, nx), npts.value
 
     # ---- k-NN
     def knn(self, q_xyz: np.ndarray, k: int = 5, max_d2: float = 0.0):

@@ -19,12 +19,9 @@ void set_error(const std::string& s) { g_err = s; }
 static int fail(int code, const std::string& msg) { set_error(msg); return code; }
 
 // ---------------------------------------------------------------------------------------------- host pose helpers
-// tf2 Matrix3x3(q).getRPY + Quaternion::setRPY round trip: LidarSLAM::MannualYawCorrection (LidarSlam.cpp:891-913)
-static void manual_yaw_correction(const double last[7], double T[7], double yaw_ratio) {
-    double tn, rn;
-    rel_motion(last, T, &tn, &rn);
-    const float translation_norm = float(tn);
-    const double x = T[3], y = T[4], z = T[5], w = T[6];
+// tf2 Matrix3x3(q).getRPY of the quaternion {x, y, z, w}
+static void tf2_get_rpy(const double q[4], double* roll_out, double* pitch_out, double* yaw_out) {
+    const double x = q[0], y = q[1], z = q[2], w = q[3];
     const double d = x * x + y * y + z * z + w * w, s = 2.0 / d;
     const double xs = x * s, ys = y * s, zs = z * s, wx = w * xs, wy = w * ys, wz = w * zs;
     const double xx = x * xs, xy = x * ys, xz = x * zs, yy = y * ys, yz = y * zs, zz = z * zs;
@@ -39,6 +36,16 @@ static void manual_yaw_correction(const double last[7], double T[7], double yaw_
         roll = std::atan2(m21 / std::cos(pitch), m22 / std::cos(pitch));
         yaw = std::atan2(m10 / std::cos(pitch), m00 / std::cos(pitch));
     }
+    *roll_out = roll; *pitch_out = pitch; *yaw_out = yaw;
+}
+
+// tf2 Matrix3x3(q).getRPY + Quaternion::setRPY round trip: LidarSLAM::MannualYawCorrection (LidarSlam.cpp:891-913)
+static void manual_yaw_correction(const double last[7], double T[7], double yaw_ratio) {
+    double tn, rn;
+    rel_motion(last, T, &tn, &rn);
+    const float translation_norm = float(tn);
+    double roll, pitch, yaw;
+    tf2_get_rpy(T + 3, &roll, &pitch, &yaw);
     const double cyaw = yaw + double(translation_norm) * yaw_ratio * M_PI / 180;
     const double hy = cyaw * 0.5, hp = pitch * 0.5, hr = roll * 0.5;
     const double cy = std::cos(hy), sy = std::sin(hy), cp = std::cos(hp), sp = std::sin(hp), cr = std::cos(hr), sr = std::sin(hr);
@@ -146,6 +153,9 @@ static void ctx_free(Ctx* c) {
     cudaFree(c->d_qkeys); cudaFree(c->d_qkeys_out); cudaFree(c->d_qvals); cudaFree(c->d_qvals_out); cudaFree(c->d_qsort_tmp);
     if (c->h_stage) cudaFreeHost(c->h_stage);
     cudaFree(c->d_dec);
+    cudaFree(c->reloc.d_bits[0]); cudaFree(c->reloc.d_bits[1]); cudaFree(c->reloc.d_keys); cudaFree(c->reloc.d_keys_out);
+    cudaFree(c->reloc.d_tmp); cudaFree(c->reloc.d_pts); cudaFree(c->reloc.d_q);
+    for (auto& e : c->reloc.ev) if (e) cudaEventDestroy(e);
     if (c->ev_dec) cudaEventDestroy(c->ev_dec);
     if (c->ev0) cudaEventDestroy(c->ev0);
     if (c->ev1) cudaEventDestroy(c->ev1);
@@ -601,6 +611,217 @@ static int register_core(Ctx* c, const float4* d_scan, const uint32_t* n_points,
     if (c->d_pose_sink) c->sink_cursor += n_scans;
     return SO_OK;
 }
+
+// ---------------------------------------------------------------------------------------------- global localization
+// The score of so_localize_global is an integer function of a few double-precision expressions evaluated on the host (score-point
+// ranges, the yaw quaternions) and on the device (voxel of every point).  The host ones are compiled without FMA contraction so that
+// a numpy restatement, which never contracts, reproduces them bit for bit on any host architecture.
+#if defined(__GNUC__) && !defined(__clang__)
+#define SO_NO_FP_CONTRACT __attribute__((optimize("fp-contract=off")))
+#else
+#define SO_NO_FP_CONTRACT
+#endif
+
+struct GlobalPlan {
+    so_global_opts o{};                    // defaults applied
+    RelocGrid g{};
+    int32_t I = 0, J = 0, K = 0;           // index of the centre along each shift axis
+    int32_t m_off = 0;                     // yaw index of the centre's yaw (0 for the full circle)
+    double dpsi = 0.0;                     // yaw step actually used
+    uint64_t n_hyp = 0, bitmap_words = 0;
+};
+
+// Defaults, argument checks and the grid of so_localize_global (host only).  Capacity errors return with the plan filled in.
+static int global_plan(const so_global_opts* in, GlobalPlan* P) {
+    if (!in) return fail(SO_ERR_ARG, "null so_global_opts");
+    so_global_opts o = *in;
+    if (o.res == 0) o.res = 0.25;
+    if (o.yaw_step == 0) o.yaw_step = 2.0 * M_PI / 180.0;
+    if (o.max_range == 0) o.max_range = 40.0;
+    if (o.score_points == 0) o.score_points = 1024;
+    if (o.dilate == 0) o.dilate = 1;
+    if (o.k == 0) o.k = 16;
+    if (o.nms_xy == 0) o.nms_xy = 1.0;
+    if (o.nms_yaw == 0) o.nms_yaw = 10.0 * M_PI / 180.0;
+    auto nonneg = [](double v) { return std::isfinite(v) && v >= 0.0; };
+    auto pos = [](double v) { return std::isfinite(v) && v > 0.0; };
+    if (!nonneg(o.half_x) || !nonneg(o.half_y) || !nonneg(o.half_z)) return fail(SO_ERR_ARG, "search half-extents must be finite and >= 0");
+    if (!nonneg(o.yaw_half)) return fail(SO_ERR_ARG, "yaw_half must be finite and >= 0");
+    if (!pos(o.res) || !pos(o.yaw_step) || !pos(o.max_range)) return fail(SO_ERR_ARG, "res, yaw_step and max_range must be finite and > 0");
+    if (!nonneg(o.nms_xy) || !nonneg(o.nms_yaw)) return fail(SO_ERR_ARG, "nms_xy and nms_yaw must be finite and >= 0");
+    if (o.score_points < 1 || o.score_points > 4096) return fail(SO_ERR_ARG, "score_points must be in [1, 4096]");
+    if (o.k < 1 || o.k > 64) return fail(SO_ERR_ARG, "k must be in [1, 64]");
+    if (o.dilate < 1 || o.dilate > 8) return fail(SO_ERR_ARG, "dilate must be in [1, 8]");
+    P->o = o;
+    const double Id = std::floor(o.half_x / o.res), Jd = std::floor(o.half_y / o.res), Kd = std::floor(o.half_z / o.res);
+    const double ed = std::ceil(o.max_range / o.res);
+    const bool full = o.yaw_half >= M_PI;
+    const double Md = full ? 0.0 : std::floor(o.yaw_half / o.yaw_step);
+    double nyaw = full ? std::floor(2.0 * M_PI / o.yaw_step + 0.5) : 2.0 * Md + 1.0;
+    if (nyaw < 1.0) nyaw = 1.0;
+    const double lim = double(1 << 24);
+    if (Id > lim || Jd > lim || Kd > lim || ed > lim || nyaw > lim) return fail(SO_ERR_CAPACITY, "search region too large (more than 2^24 hypotheses)");
+    RelocGrid& g = P->g;
+    P->I = int32_t(Id); P->J = int32_t(Jd); P->K = int32_t(Kd); P->m_off = int32_t(Md);
+    g.nx = 2 * P->I + 1; g.ny = 2 * P->J + 1; g.nz = 2 * P->K + 1; g.nyaw = int32_t(nyaw);
+    g.e = int32_t(ed);
+    g.res = o.res;
+    P->dpsi = full ? 2.0 * M_PI / nyaw : o.yaw_step;
+    const double hyp = double(g.nx) * g.ny * g.nz * g.nyaw;
+    const double words = std::ceil((double(g.nx) + 2.0 * g.e) / 32.0) * (double(g.ny) + 2.0 * g.e) * (double(g.nz) + 2.0 * g.e);
+    P->n_hyp = hyp < 1.8e19 ? uint64_t(hyp) : UINT64_MAX;
+    P->bitmap_words = words < 1.8e19 ? uint64_t(words) : UINT64_MAX;
+    if (hyp > lim) return fail(SO_ERR_CAPACITY, "more than 2^24 hypotheses");
+    if (words * 32.0 > 4294967296.0) return fail(SO_ERR_CAPACITY, "occupancy bitmap above 2^32 bits");
+    g.bx = g.nx + 2 * g.e; g.by = g.ny + 2 * g.e; g.bz = g.nz + 2 * g.e; g.wpr = (g.bx + 31) / 32;
+    return SO_OK;
+}
+
+static void plan_dims(const GlobalPlan& P, int32_t dims[4]) { dims[0] = P.g.nx; dims[1] = P.g.ny; dims[2] = P.g.nz; dims[3] = P.g.nyaw; }
+
+// The scan side of the search: the points that are scored, the centre's rotation split into yaw and roll/pitch, one quaternion per
+// hypothesis yaw.
+struct GlobalScan {
+    std::vector<float4> pts;               // score points, cloud order
+    double t[3], lo[3], yaw_c, q_rp[4];     // centre position, bitmap corner (RelocGrid::lo)
+    std::vector<double> q;                 // [nyaw][4] q_z(yaw_m) (x) q_rp
+    std::vector<double> yaw;               // [nyaw] yaw_m
+};
+
+// finite, within max_range (double squared range), then shouldProcessPoint capped at score_points (so_sampling_indices' rule)
+SO_NO_FP_CONTRACT static void select_score_points(const void* xyzi, size_t n, size_t stride, size_t ioff, const so_global_opts& o, GlobalScan* S) {
+    std::vector<float4> near;
+    near.reserve(n);
+    const double r2max = o.max_range * o.max_range;
+    const unsigned char* p = static_cast<const unsigned char*>(xyzi);
+    for (size_t i = 0; i < n; ++i, p += stride) {
+        const float4 v = read_point(p, stride, ioff);
+        if (!std::isfinite(v.x) || !std::isfinite(v.y) || !std::isfinite(v.z)) continue;
+        const double x = v.x, y = v.y, z = v.z;
+        const double xx = x * x, yy = y * y, zz = z * z;
+        if ((xx + yy) + zz > r2max) continue;
+        near.push_back(v);
+    }
+    std::vector<uint32_t> idx(near.size());
+    size_t k = 0;
+    so_sampling_indices(uint32_t(near.size()), o.score_points, idx.data(), idx.size(), &k);
+    S->pts.resize(k);
+    for (size_t j = 0; j < k; ++j) S->pts[j] = near[idx[j]];
+}
+
+SO_NO_FP_CONTRACT static void qmul_nc(const double a[4], const double b[4], double o[4]) {    // qmul (so_internal.cuh), uncontracted
+    const double a3b0 = a[3] * b[0], a0b3 = a[0] * b[3], a1b2 = a[1] * b[2], a2b1 = a[2] * b[1];
+    const double a3b1 = a[3] * b[1], a1b3 = a[1] * b[3], a2b0 = a[2] * b[0], a0b2 = a[0] * b[2];
+    const double a3b2 = a[3] * b[2], a2b3 = a[2] * b[3], a0b1 = a[0] * b[1], a1b0 = a[1] * b[0];
+    const double a3b3 = a[3] * b[3], a0b0 = a[0] * b[0], a1b1 = a[1] * b[1], a2b2 = a[2] * b[2];
+    o[0] = ((a3b0 + a0b3) + a1b2) - a2b1;
+    o[1] = ((a3b1 + a1b3) + a2b0) - a0b2;
+    o[2] = ((a3b2 + a2b3) + a0b1) - a1b0;
+    o[3] = ((a3b3 - a0b0) - a1b1) - a2b2;
+}
+
+// q_c = q_z(yaw_c) (x) q_rp with yaw_c tf2's getRPY yaw of the normalised centre rotation; hypothesis yaw m is yaw_c + (m - m_off) dpsi
+SO_NO_FP_CONTRACT static void yaw_quaternions(const GlobalPlan& P, const double center[7], GlobalScan* S) {
+    const double x = center[3], y = center[4], z = center[5], w = center[6];
+    const double xx = x * x, yy = y * y, zz = z * z, ww = w * w;
+    const double nrm = std::sqrt(((xx + yy) + zz) + ww);
+    const double qc[4] = {x / nrm, y / nrm, z / nrm, w / nrm};
+    double roll, pitch;
+    tf2_get_rpy(qc, &roll, &pitch, &S->yaw_c);
+    const double h = -S->yaw_c * 0.5;
+    const double qz_inv[4] = {0.0, 0.0, std::sin(h), std::cos(h)};
+    qmul_nc(qz_inv, qc, S->q_rp);
+    const int32_t shift[3] = {P.I, P.J, P.K};
+    for (int a = 0; a < 3; ++a) {
+        S->t[a] = center[a];
+        const double reach = double(shift[a] + P.g.e) * P.g.res;
+        S->lo[a] = center[a] - reach;
+    }
+    S->q.resize(size_t(P.g.nyaw) * 4);
+    S->yaw.resize(P.g.nyaw);
+    for (int32_t m = 0; m < P.g.nyaw; ++m) {
+        const double psi = S->yaw_c + double(m - P.m_off) * P.dpsi;
+        const double hm = psi * 0.5;
+        const double qz[4] = {0.0, 0.0, std::sin(hm), std::cos(hm)};
+        S->yaw[m] = psi;
+        qmul_nc(qz, S->q_rp, S->q.data() + 4 * m);
+    }
+}
+
+// Allocate / grow the search buffers, upload the score points and yaw quaternions, and run raster -> dilate -> score (-> sort) on
+// the context stream.  The keys end in reloc.d_keys (hypothesis order) and, sorted, in reloc.d_keys_out.
+static int global_search(Ctx* c, const GlobalPlan& P, const GlobalScan& S, bool sort) {
+    Ctx::Reloc& R = c->reloc;
+    if (!R.ev[0]) for (auto& e : R.ev) SO_CUDA_TRY(cudaEventCreate(&e));
+    if (!R.d_pts) SO_CUDA_TRY(cudaMalloc(&R.d_pts, size_t(kRelocMaxPoints) * sizeof(float4)));
+    if (P.bitmap_words > R.bit_words) {
+        cudaFree(R.d_bits[0]); cudaFree(R.d_bits[1]); R.d_bits[0] = R.d_bits[1] = nullptr; R.bit_words = 0;
+        SO_CUDA_TRY(cudaMalloc(&R.d_bits[0], P.bitmap_words * sizeof(uint32_t)));
+        SO_CUDA_TRY(cudaMalloc(&R.d_bits[1], P.bitmap_words * sizeof(uint32_t)));
+        R.bit_words = P.bitmap_words;
+    }
+    if (P.n_hyp > R.key_cap) {
+        cudaFree(R.d_keys); cudaFree(R.d_keys_out); cudaFree(R.d_tmp);
+        R.d_keys = R.d_keys_out = nullptr; R.d_tmp = nullptr; R.key_cap = 0; R.tmp_bytes = 0;
+        SO_CUDA_TRY(cudaMalloc(&R.d_keys, P.n_hyp * sizeof(uint64_t)));
+        SO_CUDA_TRY(cudaMalloc(&R.d_keys_out, P.n_hyp * sizeof(uint64_t)));
+        R.tmp_bytes = reloc_sort_bytes(P.n_hyp) + 256;
+        SO_CUDA_TRY(cudaMalloc(&R.d_tmp, R.tmp_bytes));
+        R.key_cap = P.n_hyp;
+    }
+    if (S.q.size() > R.q_cap) {
+        cudaFree(R.d_q); R.d_q = nullptr; R.q_cap = 0;
+        SO_CUDA_TRY(cudaMalloc(&R.d_q, S.q.size() * sizeof(double)));
+        R.q_cap = S.q.size();
+    }
+    { int rc = ensure_maps(c); if (rc) return rc; }
+    RelocGrid g = P.g;
+    for (int a = 0; a < 3; ++a) g.lo[a] = S.lo[a];
+    cudaStream_t st = c->stream;
+    if (!S.pts.empty()) SO_CUDA_TRY(cudaMemcpyAsync(R.d_pts, S.pts.data(), S.pts.size() * sizeof(float4), cudaMemcpyHostToDevice, st));
+    SO_CUDA_TRY(cudaMemcpyAsync(R.d_q, S.q.data(), S.q.size() * sizeof(double), cudaMemcpyHostToDevice, st));
+    count_h2d(c, S.pts.size() * sizeof(float4) + S.q.size() * sizeof(double));
+    SO_CUDA_TRY(cudaEventRecord(R.ev[0], st));
+    timed_launch_begin(c);
+    SO_CUDA_TRY(cudaMemsetAsync(R.d_bits[0], 0, P.bitmap_words * sizeof(uint32_t), st));
+    launch_reloc_raster(c->surf.d_xyzi, c->surf.n, g, R.d_bits[0], st);
+    timed_launch_end(c, 6);
+    SO_CUDA_TRY(cudaEventRecord(R.ev[1], st));
+    timed_launch_begin(c);
+    const uint32_t* bits = launch_reloc_dilate(g, P.o.dilate, R.d_bits[0], R.d_bits[1], st);
+    c->launches += 2;
+    timed_launch_end(c, 6);
+    SO_CUDA_TRY(cudaEventRecord(R.ev[2], st));
+    timed_launch_begin(c);
+    { int rc = launch_reloc_score(R.d_pts, int(S.pts.size()), R.d_q, g, bits, R.d_keys, st); if (rc) return rc; }
+    timed_launch_end(c, 6);
+    SO_CUDA_TRY(cudaEventRecord(R.ev[3], st));
+    if (sort) {
+        timed_launch_begin(c);
+        { int rc = reloc_sort(R.d_tmp, R.tmp_bytes, R.d_keys, R.d_keys_out, P.n_hyp, st); if (rc) return rc; }
+        timed_launch_end(c, 6);
+    }
+    SO_CUDA_TRY(cudaEventRecord(R.ev[4], st));
+    SO_CUDA_TRY(cudaGetLastError());
+    return SO_OK;
+}
+
+static int global_check_args(Ctx* c, const void* xyzi, size_t n, size_t stride, const double center[7], const so_global_opts* gopts, GlobalPlan* P) {
+    if (!c || !center || !gopts || (!xyzi && n) || stride < 12) return fail(SO_ERR_ARG, "bad args");
+    for (int a = 0; a < 7; ++a) if (!std::isfinite(center[a])) return fail(SO_ERR_ARG, "centre pose is not finite");
+    if (center[3] == 0 && center[4] == 0 && center[5] == 0 && center[6] == 0) return fail(SO_ERR_ARG, "centre quaternion is zero");
+    int rc = global_plan(gopts, P);
+    if (rc) return rc;
+    if (n > c->cfg.max_scan_points) return fail(SO_ERR_CAPACITY, "scan larger than so_config.max_scan_points");
+    return SO_OK;
+}
+
+// Detaches the pose sink for the candidate registrations (they are internal to one call) and puts it back on every return path.
+struct SinkDetach {
+    Ctx* c; double* rows; size_t cap, cursor;
+    explicit SinkDetach(Ctx* cc) : c(cc), rows(cc->d_pose_sink), cap(cc->sink_cap), cursor(cc->sink_cursor) { c->d_pose_sink = nullptr; }
+    ~SinkDetach() { c->d_pose_sink = rows; c->sink_cap = cap; c->sink_cursor = cursor; }
+};
 
 }  // namespace so
 
@@ -1358,6 +1579,159 @@ int so_knn(so_ctx* ctx, const float* q_xyz, size_t nq, size_t stride, int k, flo
     return SO_OK;
 }
 
+// ---- global localization -------------------------------------------------------------------------------------------
+int so_localize_global_size(const so_global_opts* gopts, int32_t dims[4], uint64_t* n_hyp, uint64_t* bitmap_bytes) {
+    GlobalPlan P;
+    const int rc = global_plan(gopts, &P);
+    if (rc == SO_ERR_ARG) return rc;
+    if (dims) plan_dims(P, dims);
+    if (n_hyp) *n_hyp = P.n_hyp;
+    if (bitmap_bytes) *bitmap_bytes = P.bitmap_words < UINT64_MAX / 4 ? P.bitmap_words * 4 : UINT64_MAX;
+    return rc;
+}
+
+int so_localize_scores(so_ctx* ctx, const void* xyzi, size_t n, size_t stride, size_t ioff, const double center[7], const so_global_opts* gopts,
+                       uint16_t* scores, size_t cap, int32_t dims[4], int32_t* n_score_points) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    GlobalPlan P;
+    int rc = global_check_args(c, xyzi, n, stride, center, gopts, &P);
+    if (rc) return rc;
+    if (!scores || !dims) return fail(SO_ERR_ARG, "bad args");
+    if (cap < P.n_hyp) return fail(SO_ERR_CAPACITY, "score array smaller than the hypothesis count");
+    SO_CUDA_TRY(cudaSetDevice(c->device));
+    GlobalScan S;
+    select_score_points(xyzi, n, stride, ioff, P.o, &S);
+    yaw_quaternions(P, center, &S);
+    rc = global_search(c, P, S, false);
+    if (rc) return rc;
+    std::vector<uint64_t> keys(P.n_hyp);
+    SO_CUDA_TRY(cudaMemcpyAsync(keys.data(), c->reloc.d_keys, P.n_hyp * sizeof(uint64_t), cudaMemcpyDeviceToHost, c->stream));
+    count_d2h(c, P.n_hyp * sizeof(uint64_t));
+    SO_CUDA_TRY(cudaStreamSynchronize(c->stream));
+    for (size_t h = 0; h < P.n_hyp; ++h) scores[h] = uint16_t(65535u - uint32_t(keys[h] >> 32));
+    plan_dims(P, dims);
+    if (n_score_points) *n_score_points = int32_t(S.pts.size());
+    return SO_OK;
+}
+
+int so_localize_global(so_ctx* ctx, const void* xyzi, size_t n, size_t stride, size_t ioff, const double center[7], const so_global_opts* gopts,
+                       const so_icp_opts* opts, so_global_candidate* cands, size_t cap, so_global_result* out) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    GlobalPlan P;
+    int rc = global_check_args(c, xyzi, n, stride, center, gopts, &P);
+    if (rc) return rc;
+    if (!opts || !out || (!cands && cap)) return fail(SO_ERR_ARG, "bad args");
+    if (opts->max_icp_iters <= 0 || opts->max_icp_iters > SO_MAX_ICP_ITERS) return fail(SO_ERR_ARG, "max_icp_iters must be in [1,32]");
+    if (opts->lm_max_iterations > 16) return fail(SO_ERR_ARG, "lm_max_iterations must be <= 16");
+    SO_CUDA_TRY(cudaSetDevice(c->device));
+    const auto t0 = std::chrono::steady_clock::now();
+    std::memset(out, 0, sizeof(*out));
+    std::memcpy(out->pose, center, 7 * sizeof(double));
+    out->winner = -1;
+    out->n_hypotheses = P.n_hyp;
+    GlobalScan S;
+    select_score_points(xyzi, n, stride, ioff, P.o, &S);
+    yaw_quaternions(P, center, &S);
+    out->n_score_points = int32_t(S.pts.size());
+    rc = global_search(c, P, S, true);
+    if (rc) return rc;
+    // sorted prefix: 64 entries per candidate asked for leaves room for the hypotheses the suppression drops around each kept one
+    const size_t n_pref = std::min<size_t>(P.n_hyp, size_t(64) * P.o.k);
+    std::vector<uint64_t> pref(n_pref);
+    SO_CUDA_TRY(cudaMemcpyAsync(pref.data(), c->reloc.d_keys_out, n_pref * sizeof(uint64_t), cudaMemcpyDeviceToHost, c->stream));
+    count_d2h(c, n_pref * sizeof(uint64_t));
+    SO_CUDA_TRY(cudaStreamSynchronize(c->stream));
+    const auto t1 = std::chrono::steady_clock::now();
+    double* stage[4] = {&out->time_raster_ms, &out->time_dilate_ms, &out->time_score_ms, &out->time_sort_ms};
+    for (int s = 0; s < 4; ++s) { float ms = 0.f; cudaEventElapsedTime(&ms, c->reloc.ev[s], c->reloc.ev[s + 1]); *stage[s] = double(ms); }
+    out->best_score = n_pref ? int32_t(65535u - uint32_t(pref[0] >> 32)) : 0;
+    // greedy suppression in rank order: drop a hypothesis within nms_xy (x/y distance) AND nms_yaw (wrapped) of a kept one
+    struct Cand { double prior[7]; double yaw; int32_t score; };
+    std::vector<Cand> kept;
+    const RelocGrid& g = P.g;
+    for (size_t r = 0; r < n_pref && int32_t(kept.size()) < P.o.k; ++r) {
+        const int32_t score = int32_t(65535u - uint32_t(pref[r] >> 32));
+        if (score == 0) break;
+        uint32_t lin = uint32_t(pref[r] & 0xffffffffu);
+        const int32_t i = int32_t(lin % uint32_t(g.nx)); lin /= uint32_t(g.nx);
+        const int32_t j = int32_t(lin % uint32_t(g.ny)); lin /= uint32_t(g.ny);
+        const int32_t k = int32_t(lin % uint32_t(g.nz));
+        const int32_t m = int32_t(lin / uint32_t(g.nz));
+        Cand cd;
+        cd.prior[0] = S.t[0] + double(i - P.I) * g.res;
+        cd.prior[1] = S.t[1] + double(j - P.J) * g.res;
+        cd.prior[2] = S.t[2] + double(k - P.K) * g.res;
+        std::memcpy(cd.prior + 3, S.q.data() + 4 * m, 4 * sizeof(double));
+        cd.yaw = S.yaw[m];
+        cd.score = score;
+        bool suppressed = false;
+        for (const Cand& o : kept) {
+            const double dx = cd.prior[0] - o.prior[0], dy = cd.prior[1] - o.prior[1];
+            const double dyaw = std::fabs(std::remainder(cd.yaw - o.yaw, 2.0 * M_PI));
+            if (dx * dx + dy * dy <= P.o.nms_xy * P.o.nms_xy && dyaw <= P.o.nms_yaw) { suppressed = true; break; }
+        }
+        if (!suppressed) kept.push_back(cd);
+    }
+    // the whole cloud goes to the scan buffer (so_map_add_registered_scan inserts it afterwards), once per batch slot
+    c->prefiltered_n = SIZE_MAX;
+    rc = upload_cloud(c, xyzi, n, stride, ioff, c->d_scan);
+    if (rc) return rc;
+    c->last_scan_n = uint32_t(n);
+    const size_t n_cand = kept.size();
+    out->n_candidates = int32_t(n_cand);
+    std::vector<so_icp_result> res(n_cand);
+    if (n_cand) {
+        const size_t B = std::min<size_t>(c->max_batch, n_cand);
+        for (size_t s = 1; s < B && n; ++s)
+            SO_CUDA_TRY(cudaMemcpyAsync(c->d_scan + s * n, c->d_scan, n * sizeof(float4), cudaMemcpyDeviceToDevice, c->stream));
+        std::vector<uint32_t> npts(B, uint32_t(n));
+        std::vector<double> priors(7 * n_cand);
+        for (size_t q = 0; q < n_cand; ++q) std::memcpy(priors.data() + 7 * q, kept[q].prior, 7 * sizeof(double));
+        SinkDetach sink(c);                                   // the candidate registrations leave no rows in a pose sink
+        for (size_t s0 = 0; s0 < n_cand; s0 += B) {
+            const size_t nb = std::min(B, n_cand - s0);
+            rc = register_core(c, c->d_scan, npts.data(), nb, priors.data() + 7 * s0, opts, res.data() + s0, false);
+            if (rc) return rc;
+        }
+    }
+    // winner: most SUCCESS correspondences in the final ICP iteration, then the lower final cost, then the better rank
+    int32_t winner = -1;
+    bool all_nef = n_cand > 0;
+    auto final_cost = [](const so_icp_result& r) { return r.n_iterations > 0 ? r.iter_cost[r.n_iterations - 1] : HUGE_VAL; };
+    for (size_t q = 0; q < n_cand; ++q) {
+        const so_icp_result& r = res[q];
+        all_nef &= r.status == SO_STATUS_NOT_ENOUGH_FEATURES;
+        if (r.status != SO_OK) continue;
+        if (winner < 0) { winner = int32_t(q); continue; }
+        const so_icp_result& b = res[winner];
+        if (r.hist_reject_plane[SO_MATCH_SUCCESS] > b.hist_reject_plane[SO_MATCH_SUCCESS] ||
+            (r.hist_reject_plane[SO_MATCH_SUCCESS] == b.hist_reject_plane[SO_MATCH_SUCCESS] && final_cost(r) < final_cost(b)))
+            winner = int32_t(q);
+    }
+    for (size_t q = 0; q < std::min(n_cand, cap); ++q) {
+        so_global_candidate& o = cands[q];
+        std::memset(&o, 0, sizeof(o));
+        std::memcpy(o.prior, kept[q].prior, sizeof(o.prior));
+        o.score = kept[q].score;
+        o.n_success = res[q].hist_reject_plane[SO_MATCH_SUCCESS];
+        o.cost = res[q].n_iterations > 0 ? res[q].iter_cost[res[q].n_iterations - 1] : 0.0;
+        std::memcpy(o.pose, res[q].pose, sizeof(o.pose));
+        o.status = res[q].status;
+    }
+    out->winner = winner;
+    if (winner >= 0) {
+        out->status = SO_OK;
+        out->icp = res[winner];
+        std::memcpy(out->pose, res[winner].pose, sizeof(out->pose));
+    } else {
+        out->status = all_nef ? SO_STATUS_NOT_ENOUGH_FEATURES : SO_STATUS_NO_CORRESPONDENCES;
+    }
+    const auto t2 = std::chrono::steady_clock::now();
+    out->time_refine_ms = std::chrono::duration<double, std::milli>(t2 - t1).count();
+    out->time_total_ms = std::chrono::duration<double, std::milli>(t2 - t0).count();
+    return out->status;
+}
+
 // ---- instrumentation -----------------------------------------------------------------------------------------------
 uint64_t so_kernel_launches(so_ctx* ctx, int reset) {
     Ctx* c = reinterpret_cast<Ctx*>(ctx);
@@ -1400,7 +1774,7 @@ int so_profile_enable(so_ctx* ctx, int on) {
 
 int so_profile_get(so_ctx* ctx, int cls, double* ms, uint64_t* launches, int reset) {
     Ctx* c = reinterpret_cast<Ctx*>(ctx);
-    if (!c || cls < 0 || cls > 5) return fail(SO_ERR_ARG, "bad args");
+    if (!c || cls < 0 || cls > 6) return fail(SO_ERR_ARG, "bad args");
     if (ms) *ms = c->prof[cls].ms;
     if (launches) *launches = c->prof[cls].launches;
     if (reset) c->prof[cls] = ProfileSlot{};

@@ -128,11 +128,21 @@ struct Ctx {
     cudaStream_t copy_stream = nullptr;            // H2D of batch chunks overlaps the previous chunk's kernels
     cudaEvent_t ev_copy[17] = {};           // [0..15]: per upload chunk; [16]: guard
 
+    // ---- global localization (so_localize_global): allocated on first use, grown on demand --------------------------
+    struct Reloc {
+        uint32_t* d_bits[2] = {nullptr, nullptr}; size_t bit_words = 0;     // occupancy bitmap, ping-pong for the dilation passes
+        uint64_t* d_keys = nullptr; uint64_t* d_keys_out = nullptr; size_t key_cap = 0;
+        void* d_tmp = nullptr; size_t tmp_bytes = 0;                        // radix-sort scratch
+        float4* d_pts = nullptr;                                           // [kRelocMaxPoints] score points
+        double* d_q = nullptr; size_t q_cap = 0;                           // one quaternion per yaw
+        cudaEvent_t ev[5] = {};                                            // stage boundaries
+    } reloc;
+
     // ---- instrumentation ----------------------------------------------------------------------------------------
     uint64_t launches = 0;
     uint64_t bytes_h2d = 0, bytes_d2h = 0;         // host<->device bytes moved by registration / k-NN calls
     bool profiling = false;
-    ProfileSlot prof[6];
+    ProfileSlot prof[7];
     cudaEvent_t ev0 = nullptr, ev1 = nullptr, evp0 = nullptr, evp1 = nullptr;
 };
 
@@ -162,5 +172,20 @@ int scan_sort_alloc(Ctx* c);             // temp storage for the per-registratio
 int query_sort(Ctx* c, size_t n);         // d_qkeys/d_qvals -> *_out (allocates on growth)
 int query_sort_reserve(Ctx* c, size_t n);
 int scan_sort(Ctx* c, size_t first, size_t n, int n_scans, int cell_bits, bool key32, cudaStream_t st);   // d_skeys/d_svals[first..first+n) -> *_out
+// so_reloc.cu (global localization search)
+struct RelocGrid {
+    int32_t nx, ny, nz, nyaw;              // hypotheses per axis: 2I+1, 2J+1, 2K+1, yaw steps
+    int32_t e;                             // ceil(max_range / res): the scan's reach in voxels
+    int32_t bx, by, bz, wpr;               // bitmap voxels per axis (nx + 2e, ...), 32-bit words per x row
+    double lo[3];                          // world position of bitmap voxel (0, 0, 0): t_c - (I + e, J + e, K + e) * res
+    double res;
+};
+constexpr int kRelocMaxPoints = 4097;      // score_points <= 4096; shouldProcessPoint keeps at most one more
+constexpr int kRelocThreads = 256, kRelocRows = 8;   // k_reloc_score: CTA size, y shifts per CTA
+void launch_reloc_raster(const float4* pts, uint32_t n, const RelocGrid& g, uint32_t* bits, cudaStream_t st);
+uint32_t* launch_reloc_dilate(const RelocGrid& g, int d, uint32_t* a, uint32_t* b, cudaStream_t st);   // 3 passes; returns the result buffer
+int launch_reloc_score(const float4* spts, int n_pts, const double* d_q, const RelocGrid& g, const uint32_t* bits, uint64_t* keys, cudaStream_t st);
+size_t reloc_sort_bytes(size_t n);
+int reloc_sort(void* tmp, size_t tmp_bytes, const uint64_t* in, uint64_t* out, size_t n, cudaStream_t st);
 
 }  // namespace so
