@@ -98,7 +98,6 @@ static int ctx_alloc(Ctx* c) {
     SO_CUDA_TRY(cudaMalloc(&c->d_svals, c->scan_cap * sizeof(uint32_t)));
     SO_CUDA_TRY(cudaMalloc(&c->d_svals_out, c->scan_cap * sizeof(uint32_t)));
     SO_CUDA_TRY(cudaMalloc(&c->nn.pos, c->scan_cap * 5 * sizeof(uint32_t)));
-    SO_CUDA_TRY(cudaMalloc(&c->nn.pts, c->scan_cap * 5 * sizeof(float4)));
     SO_CUDA_TRY(cudaMalloc(&c->nn.d5, c->scan_cap * sizeof(float)));
     SO_CUDA_TRY(cudaMalloc(&c->nn.pre, c->scan_cap));
     c->nn.cap = c->scan_cap;
@@ -144,7 +143,7 @@ static void ctx_free(Ctx* c) {
     for (auto& e : c->ev_copy) if (e) cudaEventDestroy(e);
     map_free(c);
     cudaFree(c->d_scan_sorted); cudaFree(c->d_skeys); cudaFree(c->d_skeys_out); cudaFree(c->d_svals); cudaFree(c->d_svals_out);
-    cudaFree(c->d_sort_tmp); cudaFree(c->d_sort_tmp2); cudaFree(c->nn.pos); cudaFree(c->nn.pts); cudaFree(c->nn.d5); cudaFree(c->nn.pre);
+    cudaFree(c->d_sort_tmp); cudaFree(c->d_sort_tmp2); cudaFree(c->nn.pos); cudaFree(c->nn.d5); cudaFree(c->nn.pre);
     cudaFree(c->d_scan); cudaFree(c->d_offset); cudaFree(c->d_state); cudaFreeHost(c->h_state); cudaFreeHost(c->h_offset);
     cudaFree(c->d_partials); cudaFree(c->d_counters); cudaFree(c->d_hist);
     cudaFree(c->d_escan); cudaFree(c->d_eoffset); cudaFree(c->ebuf.a); cudaFree(c->ebuf.b); cudaFree(c->ebuf.flags); cudaFree(c->ebuf.nn); cudaFree(c->ebuf.selmask);

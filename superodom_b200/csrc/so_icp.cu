@@ -599,8 +599,6 @@ __global__ void __launch_bounds__(kKnnThreads, 1024 / kKnnThreads) k_knn_scan(Ma
     for (int j = 0; j < 5; ++j) {
         const bool ok = tk.id[j] != 0xFFFFFFFFu;
         nb.pos[size_t(j) * nb.cap + gi] = ok ? tk.pos[j] : 0xFFFFFFFFu;
-        // the five points are L1-hot here; handing them on as coalesced 16-byte stores saves k_fit five scattered gathers
-        if (pre == SO_MATCH_SUCCESS) nb.pts[size_t(j) * nb.cap + gi] = __ldg(&m.pts[tk.pos[j]]);
     }
 }
 
@@ -709,7 +707,6 @@ __global__ void __launch_bounds__(kThreads) k_knn_scan_coop(MapView m, BatchView
         if (lane == j) {
             const bool ok = tk.id[j] != 0xFFFFFFFFu;
             nb.pos[size_t(j) * nb.cap + gi] = ok ? tk.pos[j] : 0xFFFFFFFFu;
-            if (pre == SO_MATCH_SUCCESS) nb.pts[size_t(j) * nb.cap + gi] = __ldg(&m.pts[tk.pos[j]]);
         }
     }
 }
@@ -721,6 +718,19 @@ __global__ void __launch_bounds__(kThreads) k_knn_scan_coop(MapView m, BatchView
 // the neighbour sets of the reference's own octree (oracle knn_mode 2) isolates the one known deviation of this library from the
 // reference path: exact in-block k-NN instead of the octree's data-dependent misses (flann/octree.h:383-385,984-1001).
 // ------------------------------------------------------------------------------------------------------------------
+// Position of map point `id` (coordinates c) in the sorted map: locate() bins a point exactly as the index build does (k_keys,
+// k_keys_dev: the same double expressions), so the point lies in the cell its own coordinates locate and one scan of that cell
+// finds it.  0xFFFFFFFF when the index does not hold it (outside the grid).
+__device__ __forceinline__ uint32_t sorted_pos_of(const MapView& m, const float4 c, uint32_t id) {
+    QueryCell qc;
+    locate(m, c.x, c.y, c.z, qc);
+    if (qc.slot < 0) return 0xFFFFFFFFu;
+    const uint32_t key = scan_order_key(m, qc);
+    for (uint32_t t = __ldg(&m.cell_start[key]), e = __ldg(&m.cell_start[key + 1]); t < e; ++t)
+        if (__float_as_uint(__ldg(&m.pts[t]).w) == id) return t;
+    return 0xFFFFFFFFu;
+}
+
 __global__ void __launch_bounds__(kThreads) k_knn_inject(MapView m, const float4* __restrict__ by_id, uint32_t n_map, BatchView bv, NnBuf nb,
                                                          const uint32_t* __restrict__ ids, int n_trace_iters) {
     const int s = blockIdx.y;
@@ -737,6 +747,9 @@ __global__ void __launch_bounds__(kThreads) k_knn_inject(MapView m, const float4
     const uint32_t orig = __float_as_uint(sp.w);
     int pre = SO_MATCH_SKIPPED;
     float d5 = m.bound_d2;
+    uint32_t pos[5];
+#pragma unroll
+    for (int j = 0; j < 5; ++j) pos[j] = 0xFFFFFFFFu;
     if (should_process(orig, st->sampling_rate)) {
         pre = SO_MATCH_NOT_ENOUGH_NEIGHBORS;
         const int it = st->icp_iter;
@@ -745,6 +758,12 @@ __global__ void __launch_bounds__(kThreads) k_knn_inject(MapView m, const float4
             bool ok = true;
 #pragma unroll
             for (int j = 0; j < 5; ++j) ok = ok && p[j] < n_map;
+            // k_fit takes positions in the sorted map; a neighbour the index does not hold counts as no result
+#pragma unroll
+            for (int j = 0; j < 5; ++j) {
+                if (ok) pos[j] = sorted_pos_of(m, __ldg(&by_id[p[j]]), p[j]);
+                ok = ok && pos[j] != 0xFFFFFFFFu;
+            }
             if (ok) {
                 const double pin[3] = {double(sp.x), double(sp.y), double(sp.z)};
                 double pf[3];
@@ -755,7 +774,6 @@ __global__ void __launch_bounds__(kThreads) k_knn_inject(MapView m, const float4
                     const float4 c = __ldg(&by_id[p[j]]);
                     const float dx = qx - c.x, dy = qy - c.y, dz = qz - c.z;
                     d5 = float(double(dx) * double(dx) + double(dy) * double(dy) + double(dz) * double(dz));
-                    nb.pts[size_t(j) * nb.cap + gi] = make_float4(c.x, c.y, c.z, __uint_as_float(p[j]));
                 }
                 pre = double(d5) > double(m.bound_d2) ? SO_MATCH_NEIGHBORS_TOO_FAR : SO_MATCH_SUCCESS;      // pointSearchSqDis[4] > 3*planeRes_ (:741-744)
             }
@@ -763,8 +781,9 @@ __global__ void __launch_bounds__(kThreads) k_knn_inject(MapView m, const float4
     }
     nb.pre[gi] = (unsigned char)pre;
     nb.d5[gi] = d5;
+    // positions only for a full neighbour set: the stage outputs (cb.nn) of a rejected point carry no ids on this path
 #pragma unroll
-    for (int j = 0; j < 5; ++j) nb.pos[size_t(j) * nb.cap + gi] = 0xFFFFFFFFu;
+    for (int j = 0; j < 5; ++j) nb.pos[size_t(j) * nb.cap + gi] = pre == SO_MATCH_SUCCESS ? pos[j] : 0xFFFFFFFFu;
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -782,7 +801,9 @@ __device__ __forceinline__ double ld_shared_again(const double* p) {
 
 // The rest of LidarSLAM::ComputePlaneDistanceParameters (LidarSlam.cpp:536-572) for one scan point whose k-NN outcome is
 // `status`: PCA, plane fit, gates, observability labels, fit weight; writes the correspondence record and counts the
-// histograms.  FP64 throughout.  The neighbours come from k_knn_scan's hand-over (nb.pts).  The fit reads them three more times
+// histograms.  FP64 throughout.  k_knn_scan hands over the neighbours' positions (nb.pos) and the points are gathered from the
+// sorted map: it fits in L2 (16 MB at the bench shape) and the queries are cell-ordered, so neighbouring lanes mostly load the
+// same points.  The fit reads them three more times
 // after the mean (scatter, QR, plane distances) and does not hold them in 30 FP64 registers across the eigen-solve: the first
 // pass widens each coordinate once and parks it in shared memory (nbd[(3 j + k) * kFitThreads], this thread's column), and the
 // later passes load it from there instead of re-reading and widening afresh (float -> double conversions run at a quarter of
@@ -805,7 +826,7 @@ __device__ __forceinline__ void fit_point(const MapView& m, const CorrBuf& cb, c
         double mean[3] = {0, 0, 0};
 #pragma unroll
         for (int j = 0; j < 5; ++j) {
-            const float4 c = __ldcs(nb.pts + gi + size_t(j) * nb.cap);
+            const float4 c = __ldg(&m.pts[__ldg(&nb.pos[size_t(j) * nb.cap + gi])]);
             const double x = double(c.x), y = double(c.y), z = double(c.z);
             nbd[(3 * j + 0) * kFitThreads] = x; nbd[(3 * j + 1) * kFitThreads] = y; nbd[(3 * j + 2) * kFitThreads] = z;
             mean[0] += x; mean[1] += y; mean[2] += z;

@@ -39,10 +39,10 @@ struct BatchView {
     bool coop_knn = false;    // small registration: one warp per query (k_knn_scan_coop)
 };
 
-// neighbour hand-off between k_knn_scan and k_fit
+// neighbour hand-off between k_knn_scan and k_fit: positions only.  k_fit gathers the five points from the sorted map, which
+// (16 B per map point, 16 MB at the bench shape) fits in L2; handing over the points would send 160 B per query through HBM.
 struct NnBuf {
-    uint32_t* pos;       // [5][cap] positions of the 5 neighbours in the sorted map (0xFFFFFFFF = none); seeds the next iteration
-    float4* pts;         // [5][cap] the neighbours themselves {x,y,z,bitcast(id)}: k_fit streams them instead of gathering
+    uint32_t* pos;       // [5][cap] positions of the 5 neighbours in the sorted map (0xFFFFFFFF = none); k_fit's input, seeds the next iteration
     float* d5;           // [cap] exact 5th-neighbour d2 of the last search (decides whether its neighbours seed the next one)
     unsigned char* pre;  // [cap] SO_MATCH_SKIPPED / NOT_ENOUGH_NEIGHBORS / NEIGHBORS_TOO_FAR / SUCCESS (= has 5 neighbours)
     size_t cap;
@@ -65,7 +65,8 @@ __host__ inline uint32_t eval_grid(uint32_t n_max) {
 // k_fit launch shape, re-measured on an H100 80GB HBM3 (700 W limit; scripts/ab_knn.py, 64 cfg2 scans = 8.4 M points per launch,
 // two alternating rounds, ms per launch): 2 points x 256 threads x 4 CTAs/SM 0.554-0.560; 1 point per thread 0.544-0.545;
 // 128 threads x 8 CTAs/SM 0.552-0.554; neighbours re-read and re-converted per pass instead of kept in shared memory 0.594-0.609.
-// The defaults are kept: the other shapes are within 3 % and were not carried through the full suite.
+// The defaults are kept: the other shapes are within 3 % and were not carried through the full suite.  These times are with the
+// neighbour points handed over through HBM; with positions handed over (NnBuf) the default shape takes 0.487-0.489 ms.
 // k_fit only matches / fits; the first evaluation of the solve is a k_evaluate<PH_CORR> launch, so k_fit carries no
 // normal-equation accumulators (64 registers, 4 CTAs per SM).
 constexpr int kFitPts = 2;               // points per thread in k_fit
