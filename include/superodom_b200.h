@@ -352,6 +352,47 @@ int so_localize_scores(so_ctx* ctx, const void* xyzi, size_t n, size_t stride_by
  * capacity error too). */
 int so_localize_global_size(const so_global_opts* gopts, int32_t dims[4], uint64_t* n_hypotheses, uint64_t* bitmap_bytes);
 
+/* ---- global localization over the whole map: exact branch-and-bound ---------------------------------------------------- */
+/* so_localize_global_bnb searches the same hypotheses with the same scores and returns exactly what so_localize_global returns
+ * (every field but the time_* ones, and the candidate list), but finds the sorted key prefix by branch-and-bound over an occupancy
+ * pyramid instead of scoring every hypothesis.  Its memory scales with the map, not with the search region, so it accepts up to
+ * 2^32 hypotheses: a region covering a whole prior map (so_map_bounds gives the extent).  Level L of the pyramid is
+ * B_L(x, y, z) = OR over a, b in [0, 2^L) of B(x+a, y+b, z); the bound of a level-L node (yaw m, z shift k, x/y shifts
+ * [i0, i0+2^L) x [j0, j0+2^L)) is U = sum over score points of B_L at the point's voxel shifted by (i0, j0), at least the score of
+ * every hypothesis in the node. */
+#define SO_BNB_LEVELS 32
+typedef struct {
+    int32_t lmax;                           /* coarsest level: the smallest L >= 1 whose root fits 65 536 nodes (DESIGN.md §4) */
+    int32_t kstar_score;                    /* score of the last key of the prefix (the final K*) */
+    uint64_t root_nodes;                    /* NYAW * NZ * ceil(NX / 2^lmax) * ceil(NY / 2^lmax) */
+    uint64_t scored[SO_BNB_LEVELS];         /* per level: nodes whose bound was computed (level 0: hypotheses scored) */
+    uint64_t discarded[SO_BNB_LEVELS];      /* per level: nodes discarded by the pruning rule */
+    uint64_t leaves_scored;                 /* scored[0] */
+    uint64_t steps;                         /* traversal steps (one small read-back each) */
+    uint64_t pyramid_bytes;                 /* device bytes of all pyramid levels */
+    double time_build_ms;                   /* device time: map bounds, raster, dilation, levels, offset table (CUDA events) */
+    double time_search_ms;                  /* device time of the traversal (CUDA events) */
+} so_bnb_stats;
+
+/* Arguments as so_localize_global, plus optional statistics.  The result's time_raster_ms covers the map bounds and the raster,
+ * time_dilate_ms the dilation, pyramid levels and offset table, time_score_ms the traversal; time_sort_ms is 0.  Errors before any
+ * device work: argument errors as so_localize_global, SO_ERR_CAPACITY above 2^32 hypotheses or an offset table (NYAW * NZ * score
+ * points * 16 B) above 1 GiB; after the map bounds: SO_ERR_CAPACITY for a pyramid level above 2^32 bits. */
+int so_localize_global_bnb(so_ctx* ctx, const void* xyzi, size_t n, size_t stride_bytes, size_t intensity_offset, const double center_pose7[7],
+                           const so_global_opts* gopts, const so_icp_opts* opts, so_global_candidate* cands, size_t cap,
+                           so_global_result* out, so_bnb_stats* stats);
+/* Stage hook: the first min(NX*NY*NZ*NYAW, 64 k) keys (65535 - score) << 32 | index of the ascending order of every hypothesis'
+ * key, i.e. so_localize_global's sorted prefix.  Writes min(*n_keys, cap) keys; *n_keys = the prefix length. */
+int so_localize_bnb_keys(so_ctx* ctx, const void* xyzi, size_t n, size_t stride_bytes, size_t intensity_offset, const double center_pose7[7],
+                         const so_global_opts* gopts, uint64_t* keys, size_t cap, size_t* n_keys, so_bnb_stats* stats);
+/* Stage hook: U of every node of pyramid level `level` (0 .. lmax), index ((yaw * NZ + z) * NBY + by) * NBX + bx with
+ * NBX = ceil(NX / 2^level), NBY = ceil(NY / 2^level); dims = {NBX, NBY, NZ, NYAW}.  Level 0 equals so_localize_scores.  dims are
+ * also filled when cap is below the node count (SO_ERR_CAPACITY, returned before any device work; out may then be NULL). */
+int so_localize_bnb_bounds(so_ctx* ctx, const void* xyzi, size_t n, size_t stride_bytes, size_t intensity_offset, const double center_pose7[7],
+                           const so_global_opts* gopts, int level, uint16_t* out, size_t cap, int32_t dims[4]);
+/* Bounding box of the surf map, reduced on the device; *n = its point count (lo and hi are zero for an empty map). */
+int so_map_bounds(so_ctx* ctx, float lo[3], float hi[3], size_t* n);
+
 /* ---- instrumentation ------------------------------------------------------------------------------ */
 /* Number of this library's kernels launched since the last reset (bench.py gpu_launches). */
 uint64_t so_kernel_launches(so_ctx* ctx, int reset);
@@ -362,7 +403,7 @@ int so_bytes_copied(so_ctx* ctx, uint64_t* h2d, uint64_t* d2h, int reset);
  * reset; classes: 0 k_knn_scan (scan k-NN), 1 k_evaluate +
  * k_lm_step (LM step), 2 k_knn (so_knn*), 3 scan ordering / map build / map insert / scan preparation, 4 first evaluation of
  * a solve (k_evaluate + k_lm_step iteration zero), 5 k_fit (plane fit), 6 global localization search (bitmap raster, dilation,
- * hypothesis scoring, key sort).
+ * hypothesis scoring, key sort; for the branch-and-bound also map bounds, pyramid levels, offset table and traversal steps).
  * Profiling mode serialises kernels; enable only for roofline runs. */
 /* Build-time switches of the loaded library.  Bit 0 (SO_BUILD_FUSED_MATCH, search and fit as one kernel) is reserved: this
  * library always runs them as two kernels and returns 0. */

@@ -342,6 +342,39 @@ public:
         return rc;
     }
 
+    // globalLocalize over the whole prior map, for a robot that restarts with no idea where it is (so_localize_global_bnb, same
+    // result as so_localize_global on the same region): half_x / half_y are set from so_map_bounds so that the region covers the
+    // surf map, so the centre supplies only z, roll/pitch and the yaw origin.  The other options (yaw_half, res, ...) are used as
+    // given.  Sets T_w_lidar and last_T_w_lidar as globalLocalize does; last_bnb holds the search statistics.
+    so_bnb_stats last_bnb{};
+    template <class CloudPtr>
+    int globalLocalizeInMap(const CloudPtr& planner_point, const Transformd& centre, so_global_opts opts) {
+        localMap.sync_resolution();
+        size_t stride, ioff;
+        using PointT = typename std::decay<decltype(planner_point->points[0])>::type;
+        point_layout<PointT>(&stride, &ioff);
+        so_icp_opts o{};
+        o.max_icp_iters = int32_t(LocalizationICPMaxIter);
+        o.max_surface_features = OptSet.max_surface_features;
+        o.lm_max_iterations = 4;
+        o.yaw_ratio = OptSet.yaw_ratio;
+        double c[7];
+        centre.to_pose7(c);
+        float lo[3], hi[3];
+        size_t n_map = 0;
+        check(so_map_bounds(context.h, lo, hi, &n_map), "so_map_bounds");
+        auto half = [](double l, double h, double x) { const double a = h - x, b = x - l; return a > b ? (a > 0.0 ? a : 0.0) : (b > 0.0 ? b : 0.0); };
+        opts.half_x = half(lo[0], hi[0], c[0]);
+        opts.half_y = half(lo[1], hi[1], c[1]);
+        const void* surf = planner_point->size() ? planner_point->points.data() : nullptr;
+        const int rc = so_localize_global_bnb(context.h, surf, planner_point->size(), stride, ioff, c, &opts, &o, nullptr, 0, &last_global,
+                                             &last_bnb);
+        check(rc, "so_localize_global_bnb");
+        T_w_lidar = Transformd::from_pose7(last_global.pose);
+        last_T_w_lidar = T_w_lidar;
+        return rc;
+    }
+
     // LidarSLAM::EstimateLidarUncertainty (LidarSlam.cpp:915-975)
     void EstimateLidarUncertainty() {
         const auto& h = PlaneFeatureHistogramObs;

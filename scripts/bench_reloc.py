@@ -6,6 +6,11 @@ Prints one JSON line: median whole-call wall time over --calls calls after --war
 in the call; profile class 6 from one extra profiled call), hypotheses/s and bitmap lookups/s of the scoring kernel, the bitmap
 size, the recovery error against the truth, and the card name and power limit read in the same run.  --cpu adds one single-thread
 run of the numpy restatement of the search (tests/global_localization_numpy.py) for a speed-up figure.  Writes nothing.
+
+--bnb adds so_localize_global_bnb on the same search, timed in alternation with the exhaustive call (whole call and search stage).
+--whole-map adds branch-and-bound searches over whole maps: the cfg2 map (0.25 m, 2 deg, centre at the map centre with the true z
+and a seeded yaw) and a 300 m x 300 m synthetic map (synth.make_map(150.0, 0.2)), each with its per-level statistics, the share of
+hypotheses whose leaves were scored and the recovery error.  Either flag prints one more JSON line per workload.
 """
 import argparse
 import json
@@ -50,6 +55,8 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--scan", type=int, default=0, help="cfg2 scan index")
     ap.add_argument("--cpu", action="store_true")
+    ap.add_argument("--bnb", action="store_true", help="also time so_localize_global_bnb against the exhaustive call")
+    ap.add_argument("--whole-map", action="store_true", help="also run branch-and-bound searches over the whole cfg2 and 300 m maps")
     a = ap.parse_args()
     from superodom_b200 import api, synth
     import global_localization_numpy as GN
@@ -106,8 +113,90 @@ def main():
         cpu_ms = (time.perf_counter() - t0) * 1e3
         out["cpu_numpy_search_ms"] = cpu_ms
         out["speedup_search_vs_cpu"] = cpu_ms / (med["raster"] + med["dilate"] + med["score"] + med["sort"])
+    if a.bnb:
+        bnb_out = bnb_vs_exhaustive(ctx, scan, center, truth, g, a.calls, a.warmup)
     ctx.close()
     print(json.dumps(out))
+    if a.bnb:
+        print(json.dumps(dict(bnb_out, card=name, power_limit_w=limit)))
+    if a.whole_map:
+        ctx = api.Context(max_map_points=len(map_xyzi) + (1 << 18), max_scan_points=262144, plane_res=0.2, max_batch=16)
+        ctx.map_set_points(map_xyzi)
+        print(json.dumps(dict(whole_map(ctx, "cfg2 map", case, a.calls, a.warmup, out["hypotheses_per_s"]), card=name, power_limit_w=limit)))
+        ctx.close()
+        t0 = time.perf_counter()
+        scene3, map3 = synth.make_map(150.0, 0.2)
+        gen_s = time.perf_counter() - t0
+        case3 = synth.make_case_on(scene3, map3, "cfg2", a.scan)
+        ctx = api.Context(max_map_points=len(map3) + (1 << 18), max_scan_points=262144, plane_res=0.2, max_batch=16)
+        ctx.map_set_points(map3)
+        r = whole_map(ctx, f"300 m x 300 m synthetic map ({len(map3)} pts, generated in {gen_s:.1f} s)", case3, max(3, a.calls // 4), 1, out["hypotheses_per_s"])
+        print(json.dumps(dict(r, card=name, power_limit_w=limit)))
+        ctx.close()
+
+
+def _stats(st):
+    L = st.lmax
+    return {"lmax": L, "root_nodes": st.root_nodes, "scored": list(st.scored)[:L + 1], "discarded": list(st.discarded)[:L + 1],
+            "leaves_scored": st.leaves_scored, "steps": st.steps, "kstar_score": st.kstar_score, "pyramid_bytes": st.pyramid_bytes,
+            "build_ms": st.time_build_ms, "search_ms": st.time_search_ms}
+
+
+def bnb_vs_exhaustive(ctx, scan, center, truth, g, calls, warmup):
+    """The default search both ways, alternating call by call; the two results must be bit-identical apart from timings."""
+    for _ in range(warmup):
+        ctx.localize_global(scan, center, 20, g)
+        ctx.localize_global_bnb(scan, center, 20, g)
+    wall = {"exhaustive": [], "bnb": []}
+    search = {"exhaustive": [], "bnb": []}
+    same = True
+    for _ in range(calls):
+        t0 = time.perf_counter()
+        pose, res, _ = ctx.localize_global(scan, center, 20, g)
+        wall["exhaustive"].append((time.perf_counter() - t0) * 1e3)
+        search["exhaustive"].append(res.time_raster_ms + res.time_dilate_ms + res.time_score_ms + res.time_sort_ms)
+        t0 = time.perf_counter()
+        pose_b, res_b, _, st = ctx.localize_global_bnb(scan, center, 20, g)
+        wall["bnb"].append((time.perf_counter() - t0) * 1e3)
+        search["bnb"].append(res_b.time_raster_ms + res_b.time_dilate_ms + res_b.time_score_ms)
+        same &= bool(np.array_equal(pose, pose_b)) and res.winner == res_b.winner and res.best_score == res_b.best_score
+    return {"workload": "default cfg2 search, exhaustive vs branch-and-bound, alternating", "calls": calls,
+            "wall_ms_median": {k: float(np.median(v)) for k, v in wall.items()},
+            "wall_ms_range": {k: [float(np.min(v)), float(np.max(v))] for k, v in wall.items()},
+            "search_ms_median": {k: float(np.median(v)) for k, v in search.items()},
+            "search_ms_range": {k: [float(np.min(v)), float(np.max(v))] for k, v in search.items()},
+            "same_result": same, "n_hypotheses": res.n_hypotheses, "leaf_fraction": st.leaves_scored / res.n_hypotheses,
+            "stats": _stats(st)}
+
+
+def whole_map(ctx, label, case, calls, warmup, exhaustive_rate):
+    """Branch-and-bound over the whole map from its centre (true z, seeded yaw), 0.25 m and 2 deg.  exhaustive_rate: hypotheses/s of
+    the exhaustive scoring kernel in this run, for the time an exhaustive search of the same region would take if it were allowed."""
+    from superodom_b200 import api
+    truth = case["pose_true"]
+    lo, hi, n_map = ctx.map_bounds()
+    yaw = np.random.default_rng(9100).uniform(-math.pi, math.pi)
+    center = np.r_[0.5 * (float(lo[0]) + float(hi[0])), 0.5 * (float(lo[1]) + float(hi[1])), truth[2],
+                   0.0, 0.0, math.sin(yaw / 2), math.cos(yaw / 2)]
+    g = api.whole_map_opts(lo, hi, center, yaw_half=math.pi)
+    for _ in range(warmup):
+        ctx.localize_global_bnb(case["scan_xyzi"], center, 20, g)
+    wall, search = [], []
+    for _ in range(calls):
+        t0 = time.perf_counter()
+        pose, res, cands, st = ctx.localize_global_bnb(case["scan_xyzi"], center, 20, g)
+        wall.append((time.perf_counter() - t0) * 1e3)
+        search.append(st.time_build_ms + st.time_search_ms)
+    return {"workload": f"{label}: whole-map search {g.half_x:.2f} x {g.half_y:.2f} m half-extents = {res.n_hypotheses} hypotheses x "
+                        f"{res.n_score_points} score points", "calls": calls,
+            "wall_ms_median": float(np.median(wall)), "wall_ms_range": [float(np.min(wall)), float(np.max(wall))],
+            "bnb_ms_median": float(np.median(search)), "bnb_ms_range": [float(np.min(search)), float(np.max(search))],
+            "exhaustive_rate_equivalent_ms": res.n_hypotheses / exhaustive_rate * 1e3,
+            "leaf_fraction": st.leaves_scored / res.n_hypotheses, "stats": _stats(st),
+            "status": res.status, "best_score": res.best_score, "n_candidates": res.n_candidates,
+            "true_offset_m": float(np.linalg.norm(center[:2] - truth[:2])),
+            "err_m": float(np.linalg.norm(pose[:3] - truth[:3])),
+            "err_deg": math.degrees(2.0 * math.acos(min(1.0, abs(float(np.dot(pose[3:], truth[3:]))))))}
 
 
 if __name__ == "__main__":

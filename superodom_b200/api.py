@@ -21,7 +21,7 @@ EXPORTS = [
     "so_map_set_resolution", "so_map_set_origin", "so_map_get_origin", "so_map_shift", "so_map_set_points",
     "so_map_set_edge_points", "so_map_add_surf", "so_map_add_edge", "so_map_add_scan", "so_map_add_registered_scan", "so_map_add_scan_edge", "so_map_counts_5x5", "so_map_download", "so_map_size",
     "so_scan_prefilter", "so_scan_deskew", "so_scan_extract_uniform", "so_register", "so_register_prefiltered", "so_register_injected", "so_set_pose_sink", "so_register_batch", "so_register_batch_edges", "so_register_batch_device", "so_correspond", "so_correspond_edge", "so_evaluate",
-    "so_knn", "so_knn_device", "so_sampling_indices", "so_localize_global", "so_localize_scores", "so_localize_global_size", "so_kernel_launches", "so_bytes_copied", "so_build_flags", "so_profile_enable", "so_profile_get",
+    "so_knn", "so_knn_device", "so_sampling_indices", "so_localize_global", "so_localize_scores", "so_localize_global_size", "so_localize_global_bnb", "so_localize_bnb_keys", "so_localize_bnb_bounds", "so_map_bounds", "so_kernel_launches", "so_bytes_copied", "so_build_flags", "so_profile_enable", "so_profile_get",
 ]
 
 
@@ -76,6 +76,25 @@ class GlobalResult(C.Structure):
 def global_opts(half_x=0.0, half_y=0.0, half_z=0.0, yaw_half=0.0, res=0.0, yaw_step=0.0, max_range=0.0, score_points=0, dilate=0,
                 k=0, nms_xy=0.0, nms_yaw=0.0) -> GlobalOpts:
     return GlobalOpts(half_x, half_y, half_z, yaw_half, res, yaw_step, max_range, score_points, dilate, k, 0, nms_xy, nms_yaw)
+
+
+BNB_LEVELS = 32
+
+
+class BnbStats(C.Structure):
+    """so_bnb_stats: where the branch-and-bound search spent its work (per level: bounds computed and nodes discarded)."""
+    _fields_ = [("lmax", C.c_int32), ("kstar_score", C.c_int32), ("root_nodes", C.c_uint64),
+                ("scored", C.c_uint64 * BNB_LEVELS), ("discarded", C.c_uint64 * BNB_LEVELS), ("leaves_scored", C.c_uint64),
+                ("steps", C.c_uint64), ("pyramid_bytes", C.c_uint64), ("time_build_ms", C.c_double), ("time_search_ms", C.c_double)]
+
+
+def whole_map_opts(map_lo, map_hi, center_pose7, **kw) -> GlobalOpts:
+    """global_opts whose x/y region around the centre covers the map's bounding box (Context.map_bounds): half_x / half_y are the
+    largest distance from the centre to the box along each axis.  The centre then supplies only z, roll/pitch and the yaw origin;
+    the remaining options (yaw_half, res, ...) are passed through."""
+    hx = max(float(map_hi[0]) - float(center_pose7[0]), float(center_pose7[0]) - float(map_lo[0]), 0.0)
+    hy = max(float(map_hi[1]) - float(center_pose7[1]), float(center_pose7[1]) - float(map_lo[1]), 0.0)
+    return global_opts(half_x=hx, half_y=hy, **kw)
 
 
 CORR_DTYPE = np.dtype([("n", "<f8", 3), ("d", "<f8"), ("w", "<f8"), ("nn", "<u4", 5), ("nn_d2", "<f4", 5),
@@ -143,6 +162,13 @@ def load_library():
     L.so_localize_scores.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p,
                                      C.c_size_t, C.c_void_p, C.c_void_p]
     L.so_localize_global_size.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.so_localize_global_bnb.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p,
+                                         C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
+    L.so_localize_bnb_keys.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p,
+                                       C.c_size_t, C.c_void_p, C.c_void_p]
+    L.so_localize_bnb_bounds.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p, C.c_void_p, C.c_int,
+                                         C.c_void_p, C.c_size_t, C.c_void_p]
+    L.so_map_bounds.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     L.so_kernel_launches.restype = C.c_uint64
     L.so_kernel_launches.argtypes = [C.c_void_p, C.c_int]
     L.so_bytes_copied.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
@@ -512,6 +538,60 @@ class Context:
                                             C.byref(g), _p(scores), nh, _p(dims), C.byref(npts)), "so_localize_scores")
         assert tuple(dims) == (nx, ny, nz, nyaw)
         return scores[:nh].reshape(nyaw, nz, ny, nx), npts.value
+
+    def localize_global_bnb(self, scan_xyzi: np.ndarray, center_pose7, max_icp_iters: int, opts: GlobalOpts | None = None,
+                            max_surface_features: int = 0, **kw):
+        """so_localize_global by branch-and-bound (same results, up to 2^32 hypotheses) -> (pose [7], GlobalResult,
+        [GlobalCandidate], BnbStats)."""
+        s = np.ascontiguousarray(scan_xyzi, dtype=np.float32)
+        c = np.ascontiguousarray(center_pose7, dtype=np.float64)
+        g = opts if opts is not None else global_opts()
+        o = self._opts(max_icp_iters, max_surface_features, **kw)
+        cands = (GlobalCandidate * 64)()
+        r = GlobalResult()
+        st = BnbStats()
+        stride = s.shape[1] * 4
+        self._chk(self.L.so_localize_global_bnb(self.h, _p(s) if len(s) else None, s.shape[0], stride, 12 if s.shape[1] >= 4 else stride,
+                                                _p(c), C.byref(g), C.byref(o), cands, 64, C.byref(r), C.byref(st)), "so_localize_global_bnb")
+        return np.array(r.pose), r, [cands[i] for i in range(min(r.n_candidates, 64))], st
+
+    def localize_bnb_keys(self, scan_xyzi: np.ndarray, center_pose7, opts: GlobalOpts | None = None):
+        """The sorted key prefix the branch-and-bound finds -> (uint64 keys [min(n_hyp, 64 k)], BnbStats)."""
+        s = np.ascontiguousarray(scan_xyzi, dtype=np.float32)
+        c = np.ascontiguousarray(center_pose7, dtype=np.float64)
+        g = opts if opts is not None else global_opts()
+        keys = np.zeros(64 * 64, np.uint64)
+        n = C.c_size_t()
+        st = BnbStats()
+        stride = s.shape[1] * 4
+        self._chk(self.L.so_localize_bnb_keys(self.h, _p(s) if len(s) else None, s.shape[0], stride, 12 if s.shape[1] >= 4 else stride,
+                                              _p(c), C.byref(g), _p(keys), len(keys), C.byref(n), C.byref(st)), "so_localize_bnb_keys")
+        return keys[:n.value].copy(), st
+
+    def localize_bnb_bounds(self, scan_xyzi: np.ndarray, center_pose7, level: int, opts: GlobalOpts | None = None):
+        """Bound U of every node of pyramid level `level` -> uint16 [NYAW, NZ, ceil(NY / 2^level), ceil(NX / 2^level)]."""
+        s = np.ascontiguousarray(scan_xyzi, dtype=np.float32)
+        c = np.ascontiguousarray(center_pose7, dtype=np.float64)
+        g = opts if opts is not None else global_opts()
+        dims = np.zeros(4, np.int32)
+        stride = s.shape[1] * 4
+        args = (self.h, _p(s) if len(s) else None, s.shape[0], stride, 12 if s.shape[1] >= 4 else stride, _p(c), C.byref(g), level)
+        rc = self.L.so_localize_bnb_bounds(*args, None, 0, _p(dims))          # host-only: the level's dims with a capacity error
+        if rc != -3:
+            self._chk(rc, "so_localize_bnb_bounds")
+        nbx, nby, nz, nyaw = (int(v) for v in dims)
+        n = nbx * nby * nz * nyaw
+        out = np.zeros(max(n, 1), np.uint16)
+        self._chk(self.L.so_localize_bnb_bounds(*args, _p(out), n, _p(dims)), "so_localize_bnb_bounds")
+        assert tuple(dims) == (nbx, nby, nz, nyaw)
+        return out[:n].reshape(nyaw, nz, nby, nbx)
+
+    def map_bounds(self):
+        """Bounding box of the surf map, reduced on the device -> (lo float32 [3], hi float32 [3], point count)."""
+        lo, hi = np.zeros(3, np.float32), np.zeros(3, np.float32)
+        n = C.c_size_t()
+        self._chk(self.L.so_map_bounds(self.h, _p(lo), _p(hi), C.byref(n)), "so_map_bounds")
+        return lo, hi, n.value
 
     # ---- k-NN
     def knn(self, q_xyz: np.ndarray, k: int = 5, max_d2: float = 0.0):

@@ -137,6 +137,19 @@ struct Ctx {
         double* d_q = nullptr; size_t q_cap = 0;                           // one quaternion per yaw
         cudaEvent_t ev[5] = {};                                            // stage boundaries
     } reloc;
+    // ---- branch-and-bound search (so_localize_global_bnb): allocated on first use, grown on demand ---------------------
+    struct Bnb {
+        uint32_t* d_pyr = nullptr; size_t pyr_words = 0;                   // every level of the clipped pyramid, back to back
+        uint32_t* d_scratch = nullptr; size_t scratch_words = 0;           // raster / dilation ping-pong partner of level 0
+        int4* d_off = nullptr; size_t off_cap = 0;                         // [nyaw][nz][n_pts] voxel offsets of the score points
+        uint64_t* d_nodes = nullptr;                                       // level buffers: [kBnbRoot] root chunk + [4C] per finer level
+        uint64_t* d_unsorted = nullptr;                                    // [kBnbRoot] scored nodes before the sort
+        uint64_t* d_merge[2] = {nullptr, nullptr};                         // [kBnbMerge] running top-P + new leaves, sorted copy
+        void* d_tmp = nullptr; size_t tmp_bytes = 0;                       // radix-sort scratch
+        struct BnbCtl* d_ctl = nullptr; struct BnbCtl* h_ctl = nullptr;    // K*, level counts and statistics (pinned mirror)
+        uint32_t* d_bounds = nullptr;                                      // [6] map bounding box (ordered float bits)
+        cudaEvent_t ev[4] = {};                                            // build start, build end / search start, search end, spare
+    } bnb;
 
     // ---- instrumentation ----------------------------------------------------------------------------------------
     uint64_t launches = 0;
@@ -187,5 +200,42 @@ uint32_t* launch_reloc_dilate(const RelocGrid& g, int d, uint32_t* a, uint32_t* 
 int launch_reloc_score(const float4* spts, int n_pts, const double* d_q, const RelocGrid& g, const uint32_t* bits, uint64_t* keys, cudaStream_t st);
 size_t reloc_sort_bytes(size_t n);
 int reloc_sort(void* tmp, size_t tmp_bytes, const uint64_t* in, uint64_t* out, size_t n, cudaStream_t st);
+
+// so_reloc.cu (branch-and-bound search over an occupancy pyramid)
+constexpr int kBnbLevels = 32;             // levels 0..31 (nx <= 2^25 + 1 needs at most 26)
+constexpr int kBnbBatch = 1 << 14;         // C: nodes expanded per step, so a finer level buffer holds at most 4C
+constexpr int kBnbRoot = 1 << 16;          // root nodes scored per chunk, and the root size the Lmax rule aims for
+constexpr int kBnbMaxKeys = 64 * 64;       // P <= 64 k with k <= 64
+constexpr int kBnbMerge = kBnbMaxKeys + 4 * kBnbBatch;
+constexpr uint64_t kBnbNone = ~0ull;       // a discarded node: sorts after every valid key (bit 48 set, sorted bits 0..48)
+// The clipped pyramid.  Level L stores B_L(x, y, z) = OR_{a,b in [0,2^L)} B(x+a, y+b, z) for box voxels x in [x0 - (2^L-1), x0 + wx),
+// y in [y0 - (2^L-1), y0 + wy), z in [z0, z0 + wz), where [x0, x0+wx) x [y0, y0+wy) x [z0, z0+wz) is the window W of the search box
+// that the surf map's voxel bounding box, grown by the dilation, covers.  B is 0 outside W, so so is B_L outside its array.
+struct BnbPyramid {
+    int32_t x0, y0, z0, wx, wy, wz;
+    int32_t lmax;
+    int32_t wpr[kBnbLevels];               // 32-bit words per row of each level
+    uint64_t off[kBnbLevels];              // first word of each level in Ctx::Bnb::d_pyr
+};
+struct BnbCtl {                            // device control block, read back after every step
+    uint64_t kstar;                        // P-th smallest leaf key found so far (kBnbNone while fewer than P are known)
+    uint64_t cnt[kBnbLevels];              // per level: end of the nodes still admitted by K*
+    unsigned long long scored[kBnbLevels], discarded[kBnbLevels];
+};
+void launch_map_bounds(const float4* pts, uint32_t n, uint32_t* d_bounds, cudaStream_t st);   // d_bounds: min xyz, max xyz (ordered bits)
+void launch_bnb_raster(const float4* pts, uint32_t n, const RelocGrid& g, const BnbPyramid& p, uint32_t* bits, cudaStream_t st);
+void launch_bnb_levels(const BnbPyramid& p, uint32_t* pyr, cudaStream_t st);                  // levels 1..lmax from level 0
+void launch_bnb_offsets(const float4* spts, int n_pts, const double* d_q, const RelocGrid& g, const BnbPyramid& p, int4* off,
+                        cudaStream_t st);
+// Bound of level-`level` nodes: parents == nullptr scores nodes first .. first+n-1 of the level in (m, k, tile y, tile x) order;
+// otherwise node c is child (c & 3) of parents[c >> 2] (key order).  out[c] = the node key, or kBnbNone when it is clipped away,
+// its parent is above K* or its own key is above K*.
+void launch_bnb_score(const RelocGrid& g, const BnbPyramid& p, const uint32_t* pyr, const int4* off, int n_pts, int level,
+                      const uint64_t* parents, uint64_t first, uint32_t n, BnbCtl* ctl, uint64_t* out, cudaStream_t st);
+// cnt[l] for l in 1..lmax: the end of the keys <= K* among nodes[l][head[l], cnt_in[l]) (sorted); the rest are counted as discarded
+struct BnbTrim { uint64_t head[kBnbLevels], cnt[kBnbLevels], base[kBnbLevels]; int32_t lmax; };
+void launch_bnb_trim(const BnbTrim& t, const uint64_t* nodes, BnbCtl* ctl, cudaStream_t st);
+size_t bnb_sort_bytes(size_t n);
+int bnb_sort(void* tmp, size_t tmp_bytes, const uint64_t* in, uint64_t* out, size_t n, cudaStream_t st);
 
 }  // namespace so
