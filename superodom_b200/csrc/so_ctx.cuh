@@ -1,6 +1,8 @@
 // so_ctx.cuh -- the context behind the C ABI: owns every device buffer, the stream, CUDA graphs and host mirrors.
 #pragma once
+#include <cstring>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "so_icp.cuh"
@@ -17,6 +19,21 @@ namespace so {
     } while (0)
 
 void set_error(const std::string& s);
+
+// Grow-only device buffer: when n elements (bytes for void) exceed cap, free the old buffer and allocate n; the contents are not
+// kept.  A failed allocation leaves cap at 0, so the next call retries.
+template <class T>
+int grow_buffer(T*& p, size_t& cap, size_t n) {
+    if (n <= cap) return SO_OK;
+    cudaFree(p);
+    p = nullptr;
+    cap = 0;
+    size_t bytes = n;
+    if constexpr (!std::is_void_v<T>) bytes *= sizeof(T);
+    SO_CUDA_TRY(cudaMalloc(&p, bytes));
+    cap = n;
+    return SO_OK;
+}
 
 struct ProfileSlot { double ms = 0.0; uint64_t launches = 0; };
 
@@ -96,9 +113,11 @@ struct Ctx {
     bool no_dec_upload = false;                    // SO_NO_DEC_UPLOAD: A/B aid, always upload the whole cloud first
 
     // ---- k-NN scratch -------------------------------------------------------------------------------------------
-    float4* d_q = nullptr; uint32_t* d_knn_idx = nullptr; float* d_knn_d2 = nullptr; size_t knn_cap = 0;
-    uint32_t* d_qkeys = nullptr; uint32_t* d_qkeys_out = nullptr; uint32_t* d_qvals = nullptr; uint32_t* d_qvals_out = nullptr;
-    void* d_qsort_tmp = nullptr; size_t qsort_tmp_bytes = 0; size_t qsort_cap = 0;      // cell ordering of so_knn* queries
+    float4* d_q = nullptr; uint32_t* d_knn_idx = nullptr; float* d_knn_d2 = nullptr;
+    size_t q_cap = 0, knn_idx_cap = 0, knn_d2_cap = 0;
+    uint32_t* d_qkeys = nullptr; uint32_t* d_qkeys_out = nullptr; uint32_t* d_qvals = nullptr; uint32_t* d_qvals_out = nullptr;   // cell ordering of so_knn* queries
+    size_t qkeys_cap = 0, qkeys_out_cap = 0, qvals_cap = 0, qvals_out_cap = 0;
+    void* d_qsort_tmp = nullptr; size_t qsort_tmp_bytes = 0;
 
     // ---- CUDA graph cache for the ICP schedule (one entry per batch chunk shape) ------------------------------------
     // Everything a captured schedule bakes into its kernel arguments: the chunk shape and both MapViews (pointers, origin, grid,
@@ -130,8 +149,8 @@ struct Ctx {
 
     // ---- global localization (so_localize_global): allocated on first use, grown on demand --------------------------
     struct Reloc {
-        uint32_t* d_bits[2] = {nullptr, nullptr}; size_t bit_words = 0;     // occupancy bitmap, ping-pong for the dilation passes
-        uint64_t* d_keys = nullptr; uint64_t* d_keys_out = nullptr; size_t key_cap = 0;
+        uint32_t* d_bits[2] = {nullptr, nullptr}; size_t bit_words[2] = {0, 0};     // occupancy bitmap, ping-pong for the dilation passes
+        uint64_t* d_keys = nullptr; uint64_t* d_keys_out = nullptr; size_t key_cap = 0, key_out_cap = 0;
         void* d_tmp = nullptr; size_t tmp_bytes = 0;                        // radix-sort scratch
         float4* d_pts = nullptr;                                           // [kRelocMaxPoints] score points
         double* d_q = nullptr; size_t q_cap = 0;                           // one quaternion per yaw
@@ -159,6 +178,28 @@ struct Ctx {
     cudaEvent_t ev0 = nullptr, ev1 = nullptr, evp0 = nullptr, evp1 = nullptr;
 };
 
+// so_api.cu
+int fail(int code, const std::string& msg);                 // set_error(msg), return code
+void tf2_get_rpy(const double q[4], double* roll, double* pitch, double* yaw);
+int ensure_maps(Ctx* c);                                    // rebuild dirty map stores
+int upload_cloud(Ctx* c, const void* src, size_t n, size_t stride, size_t ioff, float4* dst);
+void count_h2d(Ctx* c, size_t b);
+void count_d2h(Ctx* c, size_t b);
+void timed_launch_begin(Ctx* c);
+void timed_launch_end(Ctx* c, int cls);                     // counts one launch; profile class cls when profiling
+int icp_opts_check(const so_icp_opts& o);                   // max_icp_iters and lm_max_iterations in the supported range
+// Registration of n_scans scans at d_scan (packed, back to back), or of host_src's packed scans uploaded chunk by chunk.
+int register_core(Ctx* c, const float4* d_scan, const uint32_t* n_points, size_t n_scans, const double* poses,
+                  const so_icp_opts* opts_in, so_icp_result* results, bool allow_shift, const void* host_src = nullptr,
+                  const uint32_t* n_edge = nullptr, const uint32_t* d_inject = nullptr, int inject_iters = 0);
+inline float4 read_point(const unsigned char* p, size_t stride, size_t ioff) {     // one point of a strided host cloud
+    float xyz[3], it = 0.f;
+    std::memcpy(xyz, p, 12);
+    if (ioff + 4 <= stride) std::memcpy(&it, p + ioff, 4);
+    return make_float4(xyz[0], xyz[1], xyz[2], it);
+}
+// so_global.cu
+void global_free(Ctx* c);                                   // the search buffers and events of Ctx::reloc / Ctx::bnb
 // so_map.cu
 int map_alloc(Ctx* c);
 void map_free(Ctx* c);
@@ -195,7 +236,6 @@ struct RelocGrid {
 };
 constexpr int kRelocMaxPoints = 4097;      // score_points <= 4096; shouldProcessPoint keeps at most one more
 constexpr int kRelocThreads = 256, kRelocRows = 8;   // k_reloc_score: CTA size, y shifts per CTA
-void launch_reloc_raster(const float4* pts, uint32_t n, const RelocGrid& g, uint32_t* bits, cudaStream_t st);
 uint32_t* launch_reloc_dilate(const RelocGrid& g, int d, uint32_t* a, uint32_t* b, cudaStream_t st);   // 3 passes; returns the result buffer
 int launch_reloc_score(const float4* spts, int n_pts, const double* d_q, const RelocGrid& g, const uint32_t* bits, uint64_t* keys, cudaStream_t st);
 size_t reloc_sort_bytes(size_t n);
@@ -223,6 +263,7 @@ struct BnbCtl {                            // device control block, read back af
     unsigned long long scored[kBnbLevels], discarded[kBnbLevels];
 };
 void launch_map_bounds(const float4* pts, uint32_t n, uint32_t* d_bounds, cudaStream_t st);   // d_bounds: min xyz, max xyz (ordered bits)
+// Raster of the surf store into the window W of p (the whole box: x0 = y0 = z0 = 0, wx/wy/wz = bx/by/bz, wpr[0] = g.wpr)
 void launch_bnb_raster(const float4* pts, uint32_t n, const RelocGrid& g, const BnbPyramid& p, uint32_t* bits, cudaStream_t st);
 void launch_bnb_levels(const BnbPyramid& p, uint32_t* pyr, cudaStream_t st);                  // levels 1..lmax from level 0
 void launch_bnb_offsets(const float4* spts, int n_pts, const double* d_q, const RelocGrid& g, const BnbPyramid& p, int4* off,

@@ -199,17 +199,12 @@ int map_rebuild(Ctx* c, MapStore& ms) {
     }
     if (cells + 1 > ms.cell_cap) {
         SO_CUDA_TRY(cudaStreamSynchronize(st));
-        cudaFree(ms.d_cell_start);
-        ms.d_cell_start = nullptr;
-        ms.cell_cap = cells + 1 + cells / 4;
-        SO_CUDA_TRY(cudaMalloc(&ms.d_cell_start, ms.cell_cap * sizeof(uint32_t)));
+        int rc = grow_buffer(ms.d_cell_start, ms.cell_cap, cells + 1 + cells / 4);
+        if (rc) return rc;
         size_t need = 0;
         cub::DeviceScan::ExclusiveSum(nullptr, need, ms.d_cell_start, ms.d_cell_start, int(ms.cell_cap));
-        if (need > c->cub_tmp_bytes) {
-            cudaFree(c->d_cub_tmp);
-            c->cub_tmp_bytes = need + 256;
-            SO_CUDA_TRY(cudaMalloc(&c->d_cub_tmp, c->cub_tmp_bytes));
-        }
+        rc = grow_buffer(c->d_cub_tmp, c->cub_tmp_bytes, need + 256);
+        if (rc) return rc;
     }
     SO_CUDA_TRY(cudaMemsetAsync(ms.d_cell_start, 0, (cells + 1) * sizeof(uint32_t), st));
     const uint32_t g2 = (m + 255) / 256;
@@ -237,19 +232,14 @@ int scan_sort_alloc(Ctx* c) {
 }
 
 int query_sort_reserve(Ctx* c, size_t n) {
-    if (n <= c->qsort_cap) return SO_OK;
-    cudaFree(c->d_qkeys); cudaFree(c->d_qkeys_out); cudaFree(c->d_qvals); cudaFree(c->d_qvals_out); cudaFree(c->d_qsort_tmp);
-    c->d_qkeys = c->d_qkeys_out = c->d_qvals = c->d_qvals_out = nullptr; c->d_qsort_tmp = nullptr; c->qsort_cap = 0;
-    SO_CUDA_TRY(cudaMalloc(&c->d_qkeys, n * sizeof(uint32_t)));
-    SO_CUDA_TRY(cudaMalloc(&c->d_qkeys_out, n * sizeof(uint32_t)));
-    SO_CUDA_TRY(cudaMalloc(&c->d_qvals, n * sizeof(uint32_t)));
-    SO_CUDA_TRY(cudaMalloc(&c->d_qvals_out, n * sizeof(uint32_t)));
+    int rc = grow_buffer(c->d_qkeys, c->qkeys_cap, n);
+    if (!rc) rc = grow_buffer(c->d_qkeys_out, c->qkeys_out_cap, n);
+    if (!rc) rc = grow_buffer(c->d_qvals, c->qvals_cap, n);
+    if (!rc) rc = grow_buffer(c->d_qvals_out, c->qvals_out_cap, n);
+    if (rc) return rc;
     size_t need = 0;
     cub::DeviceRadixSort::SortPairs(nullptr, need, c->d_qkeys, c->d_qkeys_out, c->d_qvals, c->d_qvals_out, int(n), 0, 32);
-    c->qsort_tmp_bytes = need + 256;
-    SO_CUDA_TRY(cudaMalloc(&c->d_qsort_tmp, c->qsort_tmp_bytes));
-    c->qsort_cap = n;
-    return SO_OK;
+    return grow_buffer(c->d_qsort_tmp, c->qsort_tmp_bytes, need + 256);
 }
 
 int query_sort(Ctx* c, size_t n) {
@@ -595,17 +585,12 @@ int map_add_points(Ctx* c, MapStore& ms, uint32_t n_new) {
             while (slots > want_slots && slots * cells_per_slot + 1 >= (size_t(1) << 31)) --slots;
             if (slots * cells_per_slot + 1 >= (size_t(1) << 31)) return map_add_points_sync(c, ms, n_new);
             SO_CUDA_TRY(cudaStreamSynchronize(st));
-            cudaFree(ms.d_cell_start);
-            ms.d_cell_start = nullptr;
-            ms.cell_cap = slots * cells_per_slot + 1;
-            SO_CUDA_TRY(cudaMalloc(&ms.d_cell_start, ms.cell_cap * sizeof(uint32_t)));
+            int rc = grow_buffer(ms.d_cell_start, ms.cell_cap, slots * cells_per_slot + 1);
+            if (rc) return rc;
             size_t need = 0;
             cub::DeviceScan::ExclusiveSum(nullptr, need, ms.d_cell_start, ms.d_cell_start, int(ms.cell_cap));
-            if (need > c->cub_tmp_bytes) {
-                cudaFree(c->d_cub_tmp);
-                c->cub_tmp_bytes = need + 256;
-                SO_CUDA_TRY(cudaMalloc(&c->d_cub_tmp, c->cub_tmp_bytes));
-            }
+            rc = grow_buffer(c->d_cub_tmp, c->cub_tmp_bytes, need + 256);
+            if (rc) return rc;
         }
     }
     // this insert indexes at most the current slots + 4 new ones (more: error flag -> synchronous rebuild); table work is sized for that

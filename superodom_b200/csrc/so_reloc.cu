@@ -1,6 +1,6 @@
 // so_reloc.cu -- global localization search (so_localize_global): occupancy bitmap of the surf map, cube dilation, exhaustive
 // scoring of x/y/z voxel shifts x yaw steps of the scan, and the key sort that ranks the hypotheses.  The host side (score-point
-// selection, suppression, refinement through register_core) lives in so_api.cu.
+// selection, suppression, refinement through register_core) lives in so_global.cu.
 //
 // Everything here is integer-valued once a point has been put into a voxel, and the voxel of a point is computed with
 // explicitly rounded FP64 operations (__dmul_rn / __dadd_rn / __dsub_rn / __ddiv_rn: no FMA contraction), so a numpy
@@ -32,19 +32,6 @@ __device__ __forceinline__ int3 reloc_voxel(const float4 v, const double q[4], d
     double r[3];
     qrot_rn(q, vd, r);
     return make_int3(int(floor(__ddiv_rn(r[0], res))), int(floor(__ddiv_rn(r[1], res))), int(floor(__ddiv_rn(r[2], res))));
-}
-
-// One thread per surf-store point: w = floor((m - lo) / res) per axis; points inside the box set their bit.
-__global__ void __launch_bounds__(256) k_reloc_raster(const float4* __restrict__ pts, uint32_t n, RelocGrid g, uint32_t* __restrict__ bits) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const float4 p = pts[i];
-    const double fx = floor(__ddiv_rn(__dsub_rn(double(p.x), g.lo[0]), g.res));
-    const double fy = floor(__ddiv_rn(__dsub_rn(double(p.y), g.lo[1]), g.res));
-    const double fz = floor(__ddiv_rn(__dsub_rn(double(p.z), g.lo[2]), g.res));
-    if (!(fx >= 0.0 && fx < double(g.bx) && fy >= 0.0 && fy < double(g.by) && fz >= 0.0 && fz < double(g.bz))) return;
-    const uint32_t x = uint32_t(fx), y = uint32_t(fy), z = uint32_t(fz);
-    atomicOr(bits + (size_t(z) * g.by + y) * g.wpr + (x >> 5), 1u << (x & 31));
 }
 
 // One pass of the separable cube dilation, one thread per bitmap word: axis 0 ORs the word shifted by 1..d bits both ways (with the
@@ -137,7 +124,8 @@ __global__ void __launch_bounds__(256) k_map_bounds(const float4* __restrict__ p
         for (int a = 0; a < 3; ++a) { atomicMin(b + a, lo[a]); atomicMax(b + 3 + a, hi[a]); }
 }
 
-// k_reloc_raster into the window W only: the same voxel expression against the same lo, then shifted to W's origin.
+// One thread per surf-store point: the box voxel floor((m - lo) / res) per axis; points inside the window W set their bit, shifted
+// to W's origin.  Both searches raster through it: the exhaustive one with W = the whole box.
 __global__ void __launch_bounds__(256) k_bnb_raster(const float4* __restrict__ pts, uint32_t n, RelocGrid g, BnbPyramid w, uint32_t* __restrict__ bits) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
@@ -272,10 +260,6 @@ __global__ void k_bnb_trim(BnbTrim t, const uint64_t* __restrict__ nodes, BnbCtl
 }
 
 }  // namespace
-
-void launch_reloc_raster(const float4* pts, uint32_t n, const RelocGrid& g, uint32_t* bits, cudaStream_t st) {
-    if (n) k_reloc_raster<<<(n + 255) / 256, 256, 0, st>>>(pts, n, g, bits);
-}
 
 uint32_t* launch_reloc_dilate(const RelocGrid& g, int d, uint32_t* a, uint32_t* b, cudaStream_t st) {
     const size_t total = size_t(g.by) * g.bz * g.wpr;

@@ -1,6 +1,6 @@
 """numpy restatement of the search stage of so_localize_global (score points, hypotheses, occupancy bitmap, dilation, scores).
 
-Every floating-point expression is evaluated in the same order as the library (superodom_b200/csrc/so_api.cu for the host part,
+Every floating-point expression is evaluated in the same order as the library (superodom_b200/csrc/so_global.cu for the host part,
 so_reloc.cu for the device part, whose operations are explicitly rounded), and numpy never contracts a multiply-add, so the
 scores are reproduced exactly, element for element.  Scalars go through Python's `math`, which calls the same libm as the host
 library.  Shared by tests/test_global_localization.py and scripts/bench_reloc.py.
