@@ -245,6 +245,33 @@ int so_register_batch_edges(so_ctx* ctx, const void* surf_xyzi, const uint32_t* 
 int so_register_batch_device(so_ctx* ctx, const void* d_scans_xyzi, const uint32_t* n_points, size_t n_scans,
                              const double* poses_in, const so_icp_opts* opts, so_icp_result* results);
 
+/* ---- within-scan motion compensation (LidarSlam.h:65-82 UndistortionMode; empty upstream, LidarSlam.cpp:382-400) ------------
+ * A constant body-velocity model, re-estimated at the start of every ICP iteration from the current estimate T_cur:
+ *   D = T_prev^-1 * T_cur,  alpha_i = double(time_i) / dt (0 for a non-finite time),  q_i = slerp(identity, q_D, alpha_i),
+ *   pInit_i = float3(qrot(q_i, p_i) + alpha_i * t_D)
+ * and the iteration runs on pInit (rounded to float) in place of the sensor-frame point.  time_i is the float at byte time_offset of
+ * each record, in seconds after the instant the pose describes (the shipped pipeline: the scan start, time stored in intensity by
+ * uniformFeatureExtraction, so time_offset == intensity_offset).  Surf cloud only.  Argument errors (mode 2, a bad dt, a
+ * non-finite prev_pose) are returned before any device work.  After so_register_undistort / so_register_prefiltered_undistort,
+ * so_map_add_registered_scan(pose) inserts the whole cloud undistorted with the D that pose gives: world = T(pose) * pInit. */
+typedef struct {
+    int32_t mode;          /* 0 NONE (the scan registers exactly as so_register), 1 APPROXIMATED; 2 (OPTIMIZED) -> SO_ERR_ARG */
+    int32_t rotation;      /* 1 rotation + translation, 0 translation only (cloud already rotation-deskewed by so_scan_deskew imu_only) */
+    double prev_pose[7];   /* previous registration's pose7 */
+    double dt;             /* seconds from prev_pose to the pose being estimated, finite and > 0 */
+} so_undistort;
+int so_register_undistort(so_ctx* ctx, const void* surf_xyzi, size_t n, size_t stride_bytes, size_t intensity_offset, size_t time_offset,
+                          const double pose_in[7], const so_undistort* u, const so_icp_opts* opts, so_icp_result* out);
+/* ... of the cloud the last so_scan_prefilter left on the device; the time is the filtered cloud's intensity (w). */
+int so_register_prefiltered_undistort(so_ctx* ctx, const double pose_in[7], const so_undistort* u, const so_icp_opts* opts, so_icp_result* out);
+/* ... of a batch as so_register_batch, u[n_scans]: one so_undistort per scan (mode 0 and 1 may be mixed). */
+int so_register_batch_undistort(so_ctx* ctx, const void* surf_xyzi, const uint32_t* n_points, size_t n_scans, size_t stride_bytes,
+                                size_t intensity_offset, size_t time_offset, const double* poses_in, const so_undistort* u,
+                                const so_icp_opts* opts, so_icp_result* results);
+/* Stage hook: pInit of a cloud at T_cur = pose, as packed float4 {x, y, z, intensity} in input order (mode 0: the cloud as is). */
+int so_undistort_points(so_ctx* ctx, const void* xyzi, size_t n, size_t stride_bytes, size_t intensity_offset, size_t time_offset,
+                        const double pose[7], const so_undistort* u, float* out_xyzi);
+
 /* Sharded-replay plumbing (BASELINE cfg4; SURVEY 8e "K8"): a caller-owned DEVICE buffer of cap_rows x 8 doubles.  Every following
  * so_register / so_register_batch* call appends one row per scan, starting at first_row and advancing: {pose_opt[7] (the
  * optimiser output, so_icp_result.pose_opt), status + 256 * n_iterations}; scans that were not registered (soft statuses) carry
@@ -403,7 +430,8 @@ int so_bytes_copied(so_ctx* ctx, uint64_t* h2d, uint64_t* d2h, int reset);
  * reset; classes: 0 k_knn_scan (scan k-NN), 1 k_evaluate +
  * k_lm_step (LM step), 2 k_knn (so_knn*), 3 scan ordering / map build / map insert / scan preparation, 4 first evaluation of
  * a solve (k_evaluate + k_lm_step iteration zero), 5 k_fit (plane fit), 6 global localization search (bitmap raster, dilation,
- * hypothesis scoring, key sort; for the branch-and-bound also map bounds, pyramid levels, offset table and traversal steps).
+ * hypothesis scoring, key sort; for the branch-and-bound also map bounds, pyramid levels, offset table and traversal steps),
+ * 7 k_undistort (within-scan motion compensation: per ICP iteration, and the undistorted map insert / so_undistort_points).
  * Profiling mode serialises kernels; enable only for roofline runs. */
 /* Build-time switches of the loaded library.  Bit 0 (SO_BUILD_FUSED_MATCH, search and fit as one kernel) is reserved: this
  * library always runs them as two kernels and returns 0. */

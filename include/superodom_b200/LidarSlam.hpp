@@ -204,6 +204,7 @@ private:
 class LidarSLAM {
 public:
     enum class PredictionSource { IMU_ORIENTATION, LIO_ODOM, VIO_ODOM, NEURAL_IMU_ODOM, CONSTANT_VELOCITY };
+    enum UndistortionMode { NONE = 0, APPROXIMATED = 1, OPTIMIZED = 2 };                         // LidarSlam.h:65-82
     enum MatchingResult : uint8_t { SUCCESS = 0, NOT_ENOUGH_NEIGHBORS = 1, NEIGHBORS_TOO_FAR = 2, BAD_PCA_STRUCTURE = 3,
                                     INVAVLID_NUMERICAL = 4, MSE_TOO_LARGE = 5, UNKNON = 6, nRejectionCauses = 7 };
     enum Feature_observability : uint8_t { rx_cross = 0, neg_rx_cross = 1, ry_cross = 2, neg_ry_cross = 3, rz_cross = 4, neg_rz_cross = 5,
@@ -240,6 +241,11 @@ public:
     std::array<int, nFeatureObs> PlaneFeatureHistogramObs{};
     std::array<int, nRejectionCauses> MatchRejectionHistogramLine{}, MatchRejectionHistogramPlane{};
     size_t LocalizationICPMaxIter = 4;                           // LidarSlam.h:273
+    UndistortionMode Undistortion = NONE;                        // LidarSlam.h:266; APPROXIMATED: so_register_undistort, time in intensity
+    bool UndistortRotation = true;                               // shim only: false when the cloud's rotation was already removed
+                                                                 // (featureExtraction's IMU branch, so_scan_deskew imu_only)
+    Transformd undistort_prev_pose;                              // pose of the previous scan (last_T_w_lidar is the prior by then)
+    bool undistort_has_prev = false;
     so_icp_result last_result{};                                 // everything the device reported for the last scan
 
     explicit LidarSLAM(int device = 0, uint32_t max_map_points = 0, uint32_t max_scan_points = 0) : localMap(&context) {
@@ -251,6 +257,7 @@ public:
     template <class CloudPtr>
     void Localization(bool initialization, PredictionSource predictodom, const Transformd& position, const CloudPtr& edge_point,
                       const CloudPtr& planner_point, double timeLaserOdometry) {
+        if (Undistortion == OPTIMIZED) throw Error("UndistortionMode::OPTIMIZED is not implemented");
         T_w_lidar = position; T_w_initial_guess = position; last_T_w_lidar = position;          // initializeState (:53-57)
         localMap.sync_resolution();
         size_t stride, ioff;
@@ -264,6 +271,7 @@ public:
             if (edge_point && edge_point->size()) check(so_map_add_scan_edge(context.h, edge_point->points.data(), edge_point->size(), stride, ioff, pose), "so_map_add_scan_edge");
             if (planner_point->size()) check(so_map_add_scan(context.h, surf, planner_point->size(), stride, ioff, pose), "so_map_add_scan");
             lasttimeLaserOdometry = timeLaserOdometry;
+            undistort_prev_pose = T_w_lidar; undistort_has_prev = true;
             return;
         }
         EstimateLidarUncertainty();                                                              // (:915-986), from the PREVIOUS scan's histogram
@@ -281,9 +289,19 @@ public:
             o.prior_uncertainty[2] = float(lidarOdomUncer.uncertainty_z);
         }
         position.to_pose7(pose);
-        const int rc = so_register(context.h, surf, planner_point->size(), edge_point ? (const void*)edge_point->points.data() : nullptr,
-                                   edge_point ? edge_point->size() : 0, stride, ioff, pose, &o, &last_result);
-        check(rc, "so_register");
+        const double dt = timeLaserOdometry - lasttimeLaserOdometry;
+        int rc;
+        if (Undistortion == APPROXIMATED && undistort_has_prev && dt > 0 && !(edge_point && edge_point->size())) {
+            so_undistort u{};                                      // the surf cloud only; the edge cloud is empty upstream
+            u.mode = 1; u.rotation = UndistortRotation ? 1 : 0; u.dt = dt;
+            undistort_prev_pose.to_pose7(u.prev_pose);
+            rc = so_register_undistort(context.h, surf, planner_point->size(), stride, ioff, ioff, pose, &u, &o, &last_result);
+            check(rc, "so_register_undistort");
+        } else {
+            rc = so_register(context.h, surf, planner_point->size(), edge_point ? (const void*)edge_point->points.data() : nullptr,
+                             edge_point ? edge_point->size() : 0, stride, ioff, pose, &o, &last_result);
+            check(rc, "so_register");
+        }
         const so_icp_result& r = last_result;
         pos_in_localmap.v[0] = r.pos_in_localmap[0]; pos_in_localmap.v[1] = r.pos_in_localmap[1]; pos_in_localmap.v[2] = r.pos_in_localmap[2];
         check(so_map_get_origin(context.h, localMap.origin_.v), "so_map_get_origin");
@@ -314,6 +332,7 @@ public:
         if (edge_point && edge_point->size()) check(so_map_add_scan_edge(context.h, edge_point->points.data(), edge_point->size(), stride, ioff, r.pose), "so_map_add_scan_edge");
         if (planner_point->size()) check(so_map_add_registered_scan(context.h, r.pose), "so_map_add_registered_scan");   // the scan is still on the device
         lasttimeLaserOdometry = timeLaserOdometry;
+        undistort_prev_pose = T_w_lidar; undistort_has_prev = true;
     }
 
     // Global localization against the prior map (so_localize_global; extends localization mode, laserMapping.cpp:163-173,306-313):

@@ -20,7 +20,8 @@ EXPORTS = [
     "so_create", "so_destroy", "so_last_error", "so_device_available", "so_set_stream",
     "so_map_set_resolution", "so_map_set_origin", "so_map_get_origin", "so_map_shift", "so_map_set_points",
     "so_map_set_edge_points", "so_map_add_surf", "so_map_add_edge", "so_map_add_scan", "so_map_add_registered_scan", "so_map_add_scan_edge", "so_map_counts_5x5", "so_map_download", "so_map_size",
-    "so_scan_prefilter", "so_scan_deskew", "so_scan_extract_uniform", "so_register", "so_register_prefiltered", "so_register_injected", "so_set_pose_sink", "so_register_batch", "so_register_batch_edges", "so_register_batch_device", "so_correspond", "so_correspond_edge", "so_evaluate",
+    "so_scan_prefilter", "so_scan_deskew", "so_scan_extract_uniform", "so_register", "so_register_prefiltered", "so_register_injected", "so_set_pose_sink", "so_register_batch", "so_register_batch_edges", "so_register_batch_device",
+    "so_register_undistort", "so_register_prefiltered_undistort", "so_register_batch_undistort", "so_undistort_points", "so_correspond", "so_correspond_edge", "so_evaluate",
     "so_knn", "so_knn_device", "so_sampling_indices", "so_localize_global", "so_localize_scores", "so_localize_global_size", "so_localize_global_bnb", "so_localize_bnb_keys", "so_localize_bnb_bounds", "so_map_bounds", "so_kernel_launches", "so_bytes_copied", "so_build_flags", "so_profile_enable", "so_profile_get",
 ]
 
@@ -51,6 +52,15 @@ class IcpResult(C.Structure):
                 ("map_surf_5x5", C.c_int32), ("map_edge_5x5", C.c_int32), ("scan_surf_num", C.c_int32), ("scan_edge_num", C.c_int32),
                 ("pos_in_localmap", C.c_int32 * 3), ("prediction_source", C.c_int32),
                 ("time_ms", C.c_double), ("time_total_ms", C.c_double), ("knn_searched", C.c_int32), ("knn_verified", C.c_int32)]
+
+
+class Undistort(C.Structure):
+    """so_undistort: within-scan motion compensation of one scan (mode 0 NONE, 1 APPROXIMATED)."""
+    _fields_ = [("mode", C.c_int32), ("rotation", C.c_int32), ("prev_pose", C.c_double * 7), ("dt", C.c_double)]
+
+
+def undistort(prev_pose7, dt: float, rotation: bool = True, mode: int = 1) -> Undistort:
+    return Undistort(int(mode), int(rotation), (C.c_double * 7)(*[float(v) for v in prev_pose7]), float(dt))
 
 
 class GlobalOpts(C.Structure):
@@ -145,6 +155,13 @@ def load_library():
                               C.c_void_p, C.c_void_p, C.c_void_p]
     L.so_register_prefiltered.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     L.so_register_injected.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]
+    L.so_register_undistort.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p, C.c_void_p,
+                                        C.c_void_p, C.c_void_p]
+    L.so_register_prefiltered_undistort.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.so_register_batch_undistort.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t,
+                                              C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.so_undistort_points.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p, C.c_void_p,
+                                      C.c_void_p]
     L.so_set_pose_sink.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t]
     L.so_register_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t,
                                     C.c_void_p, C.c_void_p, C.c_void_p]
@@ -449,6 +466,51 @@ class Context:
         if rc < 0:
             self._chk(rc, "so_register_prefiltered")
         return res
+
+    # ---- within-scan motion compensation (u: an Undistort, see undistort()); time_col: the column holding each point's time
+    def register_undistort(self, scan_xyzi: np.ndarray, pose7, u: Undistort, max_icp_iters: int, max_surface_features: int = 0,
+                           time_col: int = 3, **kw) -> IcpResult:
+        s = np.ascontiguousarray(scan_xyzi, dtype=np.float32)
+        pose = np.ascontiguousarray(pose7, dtype=np.float64)
+        o = self._opts(max_icp_iters, max_surface_features, **kw)
+        r = IcpResult()
+        stride = s.shape[1] * 4
+        rc = self.L.so_register_undistort(self.h, _p(s), s.shape[0], stride, 12 if s.shape[1] >= 4 else stride, time_col * 4, _p(pose),
+                                          C.byref(u), C.byref(o), C.byref(r))
+        self._chk(rc, "so_register_undistort")
+        return r
+
+    def register_prefiltered_undistort(self, pose7, u: Undistort, max_icp_iters: int, max_surface_features: int = 0, **kw) -> IcpResult:
+        pose = np.ascontiguousarray(pose7, dtype=np.float64)
+        o = self._opts(max_icp_iters, max_surface_features, **kw)
+        r = IcpResult()
+        self._chk(self.L.so_register_prefiltered_undistort(self.h, _p(pose), C.byref(u), C.byref(o), C.byref(r)), "so_register_prefiltered_undistort")
+        return r
+
+    def register_batch_undistort(self, scans_xyzi: np.ndarray, n_points, poses, us, max_icp_iters: int, max_surface_features: int = 0,
+                                 time_col: int = 3, **kw):
+        """us: one Undistort per scan."""
+        n_points = np.ascontiguousarray(n_points, dtype=np.uint32)
+        poses = np.ascontiguousarray(poses, dtype=np.float64)
+        ns = len(n_points)
+        ua = (Undistort * ns)(*us)
+        o = self._opts(max_icp_iters, max_surface_features, **kw)
+        res = (IcpResult * ns)()
+        a = np.ascontiguousarray(scans_xyzi, dtype=np.float32)
+        stride = a.shape[1] * 4
+        self._chk(self.L.so_register_batch_undistort(self.h, _p(a), _p(n_points), ns, stride, 12, time_col * 4, _p(poses), ua, C.byref(o), res),
+                  "so_register_batch_undistort")
+        return res
+
+    def undistort_points(self, xyzi: np.ndarray, pose7, u: Undistort, time_col: int = 3) -> np.ndarray:
+        """pInit of every point at T_cur = pose7 -> float32 [n, 4] {x, y, z, intensity}."""
+        a = np.ascontiguousarray(xyzi, dtype=np.float32)
+        pose = np.ascontiguousarray(pose7, dtype=np.float64)
+        out = np.zeros((max(len(a), 1), 4), np.float32)
+        stride = a.shape[1] * 4
+        self._chk(self.L.so_undistort_points(self.h, _p(a), a.shape[0], stride, 12 if a.shape[1] >= 4 else stride, time_col * 4, _p(pose),
+                                             C.byref(u), _p(out)), "so_undistort_points")
+        return out[: len(a)]
 
     def register_batch(self, scans_xyzi: np.ndarray, n_points, poses, max_icp_iters: int, max_surface_features: int = 0, **kw):
         """scans_xyzi: float32 [sum(n_points), 4] host array (pinned or pageable)."""

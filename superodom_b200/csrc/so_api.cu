@@ -154,6 +154,7 @@ static void ctx_free(Ctx* c) {
     if (c->h_stage) cudaFreeHost(c->h_stage);
     cudaFree(c->d_dec);
     global_free(c);
+    undistort_free(c);
     if (c->ev_dec) cudaEventDestroy(c->ev_dec);
     if (c->ev0) cudaEventDestroy(c->ev0);
     if (c->ev1) cudaEventDestroy(c->ev1);
@@ -306,8 +307,9 @@ static int prepare_scans(Ctx* c, const float4* d_scan_in, const Chunk& ch, cudaS
 // scan is not in the matching phase, so a fixed schedule follows whatever path the device-side state machine takes.
 // Preferred form: a CUDA-graph WHILE node around ONE iteration (k_loop_cond ends the loop when every scan of the chunk
 // is done); fallback: the schedule unrolled max_icp_iters times.  Returns whether the loop form ran.
+// undistort: k_undistort (the scans' pInit at the current pose, so_undistort.cu) heads every iteration.
 static int run_schedule(Ctx* c, const Chunk& ch, int iters, int lm, bool with_nn, bool* was_loop, cudaStream_t run_stream = nullptr,
-                        const uint32_t* d_inject = nullptr, int inject_iters = 0) {
+                        const uint32_t* d_inject = nullptr, int inject_iters = 0, bool undistort = false) {
     if (!run_stream) run_stream = c->stream;
     const float4* d_scan = c->d_scan_sorted;
     const MapView mv = map_view(c, c->surf);
@@ -323,6 +325,9 @@ static int run_schedule(Ctx* c, const Chunk& ch, int iters, int lm, bool with_nn
     eb.offset = c->d_eoffset + ch.first;                  // like bv.offset: indexed by the scan's position inside the chunk
     if (!with_nn) { eb.nn = nullptr; eb.selmask = nullptr; }
     *was_loop = false;
+    auto undistort_step = [&](cudaStream_t s) {
+        launch_undistort(bv, c->d_scan_sorted, c->d_scan, c->und.d_time, c->und.d_par + ch.first, grid_x, n_scans, s);
+    };
     if (c->profiling || with_nn || d_inject) {
         // profiling mode: one launch at a time, timed with events, and only launches that have work (the host peeks
         // at the phases) so that the per-class average is the duration of a kernel that actually ran
@@ -335,6 +340,7 @@ static int run_schedule(Ctx* c, const Chunk& ch, int iters, int lm, bool with_nn
         };
         for (int it = 0; it < iters; ++it) {
             if (any_in(PH_CORR)) {
+                if (undistort) { timed_launch_begin(c); undistort_step(c->stream); timed_launch_end(c, 7); }
                 timed_launch_begin(c);
                 if (d_inject) launch_inject(mv, c->surf.d_xyzi, c->surf.n, bv, c->nn, d_inject, inject_iters, grid_x, n_scans, c->stream);
                 else launch_match(mv, bv, cb, c->nn, grid_x, n_scans, c->stream, 1);                                               // k_knn_scan
@@ -355,6 +361,7 @@ static int run_schedule(Ctx* c, const Chunk& ch, int iters, int lm, bool with_nn
     key.ptrs[4] = me.pts; key.ptrs[5] = me.cell_start; key.ptrs[6] = me.block_slot; key.ptrs[7] = me.block_count;
     for (int a = 0; a < 3; ++a) key.origin[a] = mv.origin[a];
     key.nb[0] = mv.nb; key.nb[1] = me.nb; key.res[0] = mv.plane_res; key.res[1] = me.plane_res;
+    if (undistort) { key.undistort = 1; key.und_time = c->und.d_time; }
     Ctx::GraphSlot* slot = nullptr;
     for (auto& g : c->graphs)
         if (g.exec && std::memcmp(&g.key, &key, sizeof(key)) == 0) slot = &g;
@@ -378,6 +385,7 @@ static int run_schedule(Ctx* c, const Chunk& ch, int iters, int lm, bool with_nn
                 cudaGraph_t body = p.conditional.phGraph_out[0];
                 ok = cudaStreamBeginCaptureToGraph(c->stream, body, nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal) == cudaSuccess;
                 if (ok) {
+                    if (undistort) undistort_step(c->stream);
                     launch_correspond(mv, bv, cb, c->nn, grid_x, n_scans, c->stream, &me, &eb, grid_e);
                     for (int k = 0; k < lm; ++k) launch_evaluate(bv, cb, grid_x, n_scans, c->stream, &eb, grid_e);
                     launch_loop_cond(bv, n_scans, handle, c->stream);
@@ -394,6 +402,7 @@ static int run_schedule(Ctx* c, const Chunk& ch, int iters, int lm, bool with_nn
             cudaGraph_t g = nullptr;
             SO_CUDA_TRY(cudaStreamBeginCapture(c->stream, cudaStreamCaptureModeThreadLocal));
             for (int it = 0; it < iters; ++it) {
+                if (undistort) undistort_step(c->stream);
                 launch_correspond(mv, bv, cb, c->nn, grid_x, n_scans, c->stream, &me, &eb, grid_e);
                 for (int k = 0; k < lm; ++k) launch_evaluate(bv, cb, grid_x, n_scans, c->stream, &eb, grid_e);
             }
@@ -407,7 +416,7 @@ static int run_schedule(Ctx* c, const Chunk& ch, int iters, int lm, bool with_nn
     slot->used = ++c->graph_clock;
     SO_CUDA_TRY(cudaGraphLaunch(slot->exec, run_stream));
     *was_loop = slot->is_loop;
-    if (!slot->is_loop) c->launches += uint64_t(iters) * (bv.counters && !grid_e ? 2 + 1 + lm : 2 + 2 + 2 * lm + (grid_e ? 1 + lm : 0));      // 2: k_knn_scan + k_fit; loop form: counted from the iterations executed
+    if (!slot->is_loop) c->launches += uint64_t(iters) * ((bv.counters && !grid_e ? 2 + 1 + lm : 2 + 2 + 2 * lm + (grid_e ? 1 + lm : 0)) + (undistort ? 1 : 0));      // 2: k_knn_scan + k_fit; loop form: counted from the iterations executed
     return SO_OK;
 }
 
@@ -466,7 +475,8 @@ int icp_opts_check(const so_icp_opts& o) {
 // d_scan: device scans (packed, back to back).  host_src != nullptr: the scans are still on the host (packed float4); this
 // function uploads them into d_scan chunk by chunk on the copy stream.
 int register_core(Ctx* c, const float4* d_scan, const uint32_t* n_points, size_t n_scans, const double* poses, const so_icp_opts* opts_in,
-                  so_icp_result* results, bool allow_shift, const void* host_src, const uint32_t* n_edge, const uint32_t* d_inject, int inject_iters) {
+                  so_icp_result* results, bool allow_shift, const void* host_src, const uint32_t* n_edge, const uint32_t* d_inject, int inject_iters,
+                  bool undistort) {
     so_icp_opts o = *opts_in;
     if (o.lm_max_iterations <= 0) o.lm_max_iterations = 4;
     { int rc = icp_opts_check(o); if (rc) return rc; }
@@ -569,7 +579,7 @@ int register_core(Ctx* c, const float4* d_scan, const uint32_t* n_points, size_t
             if (ch.grid_x == 0) continue;
             int rc = prepare_scans(c, d_scan, ch, st, true);
             bool was_loop = false;
-            if (!rc) rc = run_schedule(c, ch, o.max_icp_iters, o.lm_max_iterations, false, &was_loop, st, d_inject, inject_iters);
+            if (!rc) rc = run_schedule(c, ch, o.max_icp_iters, o.lm_max_iterations, false, &was_loop, st, d_inject, inject_iters, undistort);
             if (rc) {                                       // leave no work behind on the side streams before reporting the error
                 cudaStreamSynchronize(c->aux_stream);
                 cudaStreamSynchronize(c->copy_stream);
@@ -594,8 +604,8 @@ int register_core(Ctx* c, const float4* d_scan, const uint32_t* n_points, size_t
             int max_it = 0;
             for (uint32_t s = chunks[k].first; s < chunks[k].first + chunks[k].count; ++s) max_it = std::max(max_it, int(c->h_state[s].n_iterations));
             const bool fused = chunks[k].count <= 2 && !chunks[k].grid_e && !c->no_fused_lm;
-            c->launches += uint64_t(max_it) * uint64_t(fused ? 2 + 2 + o.lm_max_iterations
-                                                             : 2 + 3 + 2 * o.lm_max_iterations + (chunks[k].grid_e ? 1 + o.lm_max_iterations : 0));
+            c->launches += uint64_t(max_it) * uint64_t((fused ? 2 + 2 + o.lm_max_iterations
+                                                              : 2 + 3 + 2 * o.lm_max_iterations + (chunks[k].grid_e ? 1 + o.lm_max_iterations : 0)) + (undistort ? 1 : 0));
         }
         for (size_t s = 0; s < n_scans; ++s) {
             if (results[s].status == SO_STATUS_NOT_ENOUGH_FEATURES || n_points[s] == 0) continue;
@@ -749,6 +759,7 @@ static int store_add(Ctx* c, MapStore& ms, const void* xyzi, size_t n, size_t st
     if (xyzi) rc = upload_cloud(c, xyzi, n, stride, ioff, ms.d_xyzi + ms.n);
     else SO_CUDA_TRY(cudaMemcpyAsync(ms.d_xyzi + ms.n, c->d_scan, n * sizeof(float4), cudaMemcpyDeviceToDevice, c->stream));   // the registered scan, still on the device
     if (rc) return rc;
+    if (!xyzi && pose && c->und.last.on) { rc = undistort_tail(c, ms, uint32_t(n), pose); if (rc) return rc; }   // after so_register_undistort*
     if (pose) { rc = map_transform_tail(c, ms, uint32_t(n), pose); if (rc) return rc; }
     timed_launch_begin(c);
     rc = map_add_points(c, ms, uint32_t(n));
@@ -1071,6 +1082,7 @@ int so_register(so_ctx* ctx, const void* surf, size_t n_surf, const void* edge, 
         c->bytes_h2d += size_t(kept) * sizeof(float4);
         c->defer.src = surf; c->defer.n = n_surf; c->defer.stride = stride; c->defer.ioff = ioff; c->defer.stage_off = kPrepareSmallCap;
         c->last_scan_n = n;
+        c->und.last.on = 0;
         so_icp_opts o2 = *opts;
         o2.max_surface_features = 0;                                     // the decimation has been applied
         rc = register_core(c, c->d_dec, &kept, 1, pose_in, &o2, out, true, nullptr, &ne);
@@ -1083,6 +1095,7 @@ int so_register(so_ctx* ctx, const void* surf, size_t n_surf, const void* edge, 
         rc = upload_cloud(c, surf, n_surf, stride, ioff, c->d_scan);
         if (rc) return rc;
         c->last_scan_n = n;                                             // so_map_add_registered_scan inserts it without a second upload
+        c->und.last.on = 0;
         rc = upload_cloud(c, edge, n_edge, stride, ioff, c->d_escan);   // edge branch input (empty upstream: featureExtraction.cpp:429-436)
         if (rc) return rc;
         rc = register_core(c, c->d_scan, &n, 1, pose_in, opts, out, true, nullptr, &ne);
@@ -1103,6 +1116,7 @@ int so_register_prefiltered(so_ctx* ctx, const double pose_in[7], const so_icp_o
     c->prefiltered_n = SIZE_MAX;
     if (n) SO_CUDA_TRY(cudaMemcpyAsync(c->d_scan, c->d_scan_sorted, size_t(n) * sizeof(float4), cudaMemcpyDeviceToDevice, c->stream));
     c->last_scan_n = n;
+    c->und.last.on = 0;
     int rc = register_core(c, c->d_scan, &n, 1, pose_in, opts, out, true);
     if (rc) return rc;
     out->scan_edge_num = 0;
@@ -1398,7 +1412,7 @@ int so_profile_enable(so_ctx* ctx, int on) {
 
 int so_profile_get(so_ctx* ctx, int cls, double* ms, uint64_t* launches, int reset) {
     Ctx* c = reinterpret_cast<Ctx*>(ctx);
-    if (!c || cls < 0 || cls > 6) return fail(SO_ERR_ARG, "bad args");
+    if (!c || cls < 0 || cls > 7) return fail(SO_ERR_ARG, "bad args");
     if (ms) *ms = c->prof[cls].ms;
     if (launches) *launches = c->prof[cls].launches;
     if (reset) c->prof[cls] = ProfileSlot{};

@@ -37,6 +37,16 @@ int grow_buffer(T*& p, size_t& cap, size_t n) {
 
 struct ProfileSlot { double ms = 0.0; uint64_t launches = 0; };
 
+// Within-scan motion compensation of one scan (so_undistort, mode APPROXIMATED): everything k_undistort needs besides the
+// current pose.  Kept out of IcpState so that the other kernels do not change.
+struct UndistortParams {
+    double q_prev_conj[4];                         // conj(q_prev), xyzw
+    double t_prev[3];
+    double dt;                                     // seconds from prev_pose to the pose being estimated, > 0
+    int32_t on;                                    // 0: the scan registers exactly as so_register
+    int32_t rotation;                              // 1: slerp the rotation too; 0: translation only
+};
+
 // One per-block cloud family of the LocalMap (surf or edge): points in id order, the sorted hash grid, block tables.
 struct MapStore {
     float res = 0.4f;                              // planeRes_ (surf) / lineRes_ (edge): voxel leaf and gate / search radius
@@ -126,6 +136,7 @@ struct Ctx {
     struct GraphKey {
         uint32_t first, count, grid_x, grid_e; int32_t iters, lm;
         const void* ptrs[8]; int32_t origin[3]; int32_t nb[2]; float res[2];
+        int32_t undistort; const void* und_time;   // k_undistort heads every iteration (0 / nullptr otherwise)
     };
     struct GraphSlot {
         cudaGraphExec_t exec = nullptr;
@@ -169,12 +180,20 @@ struct Ctx {
         uint32_t* d_bounds = nullptr;                                      // [6] map bounding box (ordered float bits)
         cudaEvent_t ev[4] = {};                                            // build start, build end / search start, search end, spare
     } bnb;
+    // ---- within-scan motion compensation (so_register_undistort*): allocated on first use, grown on demand ------------
+    struct Und {
+        UndistortParams* d_par = nullptr; size_t par_cap = 0;              // [max_batch] per-scan parameters of the registration
+        float* d_time = nullptr; size_t time_cap = 0;                      // per-point times of the scans in d_scan (upload order)
+        float4* d_hook = nullptr; size_t hook_cap = 0;                     // so_undistort_points: the cloud and its times
+        float* d_hook_time = nullptr; size_t hook_time_cap = 0;
+        UndistortParams last{};                                            // of the scan so_map_add_registered_scan inserts (on == 0: none)
+    } und;
 
     // ---- instrumentation ----------------------------------------------------------------------------------------
     uint64_t launches = 0;
     uint64_t bytes_h2d = 0, bytes_d2h = 0;         // host<->device bytes moved by registration / k-NN calls
     bool profiling = false;
-    ProfileSlot prof[7];
+    ProfileSlot prof[8];
     cudaEvent_t ev0 = nullptr, ev1 = nullptr, evp0 = nullptr, evp1 = nullptr;
 };
 
@@ -191,7 +210,7 @@ int icp_opts_check(const so_icp_opts& o);                   // max_icp_iters and
 // Registration of n_scans scans at d_scan (packed, back to back), or of host_src's packed scans uploaded chunk by chunk.
 int register_core(Ctx* c, const float4* d_scan, const uint32_t* n_points, size_t n_scans, const double* poses,
                   const so_icp_opts* opts_in, so_icp_result* results, bool allow_shift, const void* host_src = nullptr,
-                  const uint32_t* n_edge = nullptr, const uint32_t* d_inject = nullptr, int inject_iters = 0);
+                  const uint32_t* n_edge = nullptr, const uint32_t* d_inject = nullptr, int inject_iters = 0, bool undistort = false);
 inline float4 read_point(const unsigned char* p, size_t stride, size_t ioff) {     // one point of a strided host cloud
     float xyz[3], it = 0.f;
     std::memcpy(xyz, p, 12);
@@ -200,6 +219,13 @@ inline float4 read_point(const unsigned char* p, size_t stride, size_t ioff) {  
 }
 // so_global.cu
 void global_free(Ctx* c);                                   // the search buffers and events of Ctx::reloc / Ctx::bnb
+// so_undistort.cu
+void undistort_free(Ctx* c);                                // the buffers of Ctx::und
+// k_undistort: pInit of every active point of the chunk's scans (bv.st / bv.offset / par already offset to the chunk), from the
+// raw points in upload order (raw, times: indexed offset + original index) into the ordered copy `sorted`, w kept
+void launch_undistort(const BatchView& bv, float4* sorted, const float4* raw, const float* times, const UndistortParams* par,
+                      uint32_t grid_x, uint32_t n_scans, cudaStream_t st);
+int undistort_tail(Ctx* c, MapStore& ms, uint32_t n_new, const double pose[7]);   // ms tail = the registered scan: pInit at pose, in place
 // so_map.cu
 int map_alloc(Ctx* c);
 void map_free(Ctx* c);

@@ -263,6 +263,7 @@ static int global_refine(Ctx* c, const GlobalPlan& P, const GlobalScan& S, const
     int rc = upload_cloud(c, xyzi, n, stride, ioff, c->d_scan);
     if (rc) return rc;
     c->last_scan_n = uint32_t(n);
+    c->und.last.on = 0;
     const size_t n_cand = kept.size();
     out->n_candidates = int32_t(n_cand);
     std::vector<so_icp_result> res(n_cand);

@@ -1,0 +1,301 @@
+// so_undistort.cu -- within-scan motion compensation inside the registration: the reference's UndistortionMode::APPROXIMATED
+// (LidarSlam.h:65-82; its branch of ComputePointInitAndFinalPose, LidarSlam.cpp:382-400, is empty upstream), sm_90a.
+//
+// A constant body-velocity model.  At the start of every ICP iteration, with T_cur the scan's current estimate:
+//   D       = T_prev^-1 * T_cur                 q_D = normalise(conj(q_prev) * q_cur), t_D = qrot(conj(q_prev), t_cur - t_prev)
+//   alpha_i = double(tau_i) / dt                (a non-finite tau_i gives 0)
+//   q_i     = slerp(identity, q_D, alpha_i)     (Eigen's QuaternionBase::slerp; identity when rotation == 0)
+//   pInit_i = float3(qrot(q_i, p_i) + alpha_i * t_D)
+// and the iteration runs on pInit in place of p.  Every product and sum is rounded on its own (no FMA contraction), so that
+// tests/undistort_numpy.py restates the bits; only the FP64 acos / sin are the device's.
+//   k_undistort        the ICP form: one thread per active point of the ordered scans, writes d_scan_sorted (w kept)
+//   k_undistort_cloud  a contiguous cloud at a given pose: the map insert after an undistorted registration, so_undistort_points
+#include <chrono>
+#include <cmath>
+#include <vector>
+
+#include "so_ctx.cuh"
+
+namespace so {
+
+__device__ __forceinline__ void qmul_rn(const double a[4], const double b[4], double o[4]) {
+    o[0] = __dsub_rn(__dadd_rn(__dadd_rn(__dmul_rn(a[3], b[0]), __dmul_rn(a[0], b[3])), __dmul_rn(a[1], b[2])), __dmul_rn(a[2], b[1]));
+    o[1] = __dsub_rn(__dadd_rn(__dadd_rn(__dmul_rn(a[3], b[1]), __dmul_rn(a[1], b[3])), __dmul_rn(a[2], b[0])), __dmul_rn(a[0], b[2]));
+    o[2] = __dsub_rn(__dadd_rn(__dadd_rn(__dmul_rn(a[3], b[2]), __dmul_rn(a[2], b[3])), __dmul_rn(a[0], b[1])), __dmul_rn(a[1], b[0]));
+    o[3] = __dsub_rn(__dsub_rn(__dsub_rn(__dmul_rn(a[3], b[3]), __dmul_rn(a[0], b[0])), __dmul_rn(a[1], b[1])), __dmul_rn(a[2], b[2]));
+}
+// qrot of so_internal.cuh (v + 2w (q x v) + 2 q x (q x v)) with every operation rounded
+__device__ __forceinline__ void qrot_rn(const double q[4], const double v[3], double o[3]) {
+    double ux = __dsub_rn(__dmul_rn(q[1], v[2]), __dmul_rn(q[2], v[1]));
+    double uy = __dsub_rn(__dmul_rn(q[2], v[0]), __dmul_rn(q[0], v[2]));
+    double uz = __dsub_rn(__dmul_rn(q[0], v[1]), __dmul_rn(q[1], v[0]));
+    ux = __dadd_rn(ux, ux); uy = __dadd_rn(uy, uy); uz = __dadd_rn(uz, uz);
+    o[0] = __dadd_rn(__dadd_rn(v[0], __dmul_rn(q[3], ux)), __dsub_rn(__dmul_rn(q[1], uz), __dmul_rn(q[2], uy)));
+    o[1] = __dadd_rn(__dadd_rn(v[1], __dmul_rn(q[3], uy)), __dsub_rn(__dmul_rn(q[2], ux), __dmul_rn(q[0], uz)));
+    o[2] = __dadd_rn(__dadd_rn(v[2], __dmul_rn(q[3], uz)), __dsub_rn(__dmul_rn(q[0], uy), __dmul_rn(q[1], ux)));
+}
+
+// Per-scan part, once per CTA: sh = {q_D[4], t_D[3], theta, 1 / sin(theta)}; theta < 0 marks Eigen's linear branch (|d| >= 1 - eps,
+// d = dot(identity, q_D) = q_D.w).
+__device__ __forceinline__ void und_setup(const UndistortParams& P, const double x[7], double sh[9]) {
+    double q[4];
+    qmul_rn(P.q_prev_conj, x + 3, q);
+    const double n2 = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(q[0], q[0]), __dmul_rn(q[1], q[1])), __dmul_rn(q[2], q[2])), __dmul_rn(q[3], q[3]));
+    const double s = 1.0 / sqrt(n2);
+    for (int k = 0; k < 4; ++k) sh[k] = __dmul_rn(q[k], s);
+    const double d[3] = {__dsub_rn(x[0], P.t_prev[0]), __dsub_rn(x[1], P.t_prev[1]), __dsub_rn(x[2], P.t_prev[2])};
+    qrot_rn(P.q_prev_conj, d, sh + 4);
+    const double ad = fabs(sh[3]);
+    if (ad >= 1.0 - 2.220446049250313e-16) { sh[7] = -1.0; sh[8] = 0.0; }
+    else { sh[7] = acos(ad); sh[8] = 1.0 / sin(sh[7]); }
+}
+
+__device__ __forceinline__ float4 und_point(const UndistortParams& P, const double sh[9], float4 p, float tau) {
+    const double a = isfinite(tau) ? double(tau) / P.dt : 0.0;
+    const double v[3] = {double(p.x), double(p.y), double(p.z)};
+    double o[3] = {v[0], v[1], v[2]};
+    if (P.rotation) {
+        double s0, s1;
+        if (sh[7] < 0.0) { s0 = __dsub_rn(1.0, a); s1 = a; }
+        else {
+            s0 = __dmul_rn(sin(__dmul_rn(__dsub_rn(1.0, a), sh[7])), sh[8]);
+            s1 = __dmul_rn(sin(__dmul_rn(a, sh[7])), sh[8]);
+        }
+        if (sh[3] < 0.0) s1 = -s1;
+        const double qi[4] = {__dadd_rn(__dmul_rn(s0, 0.0), __dmul_rn(s1, sh[0])), __dadd_rn(__dmul_rn(s0, 0.0), __dmul_rn(s1, sh[1])),
+                              __dadd_rn(__dmul_rn(s0, 0.0), __dmul_rn(s1, sh[2])), __dadd_rn(s0, __dmul_rn(s1, sh[3]))};
+        qrot_rn(qi, v, o);
+    }
+    return make_float4(float(__dadd_rn(o[0], __dmul_rn(a, sh[4]))), float(__dadd_rn(o[1], __dmul_rn(a, sh[5]))),
+                       float(__dadd_rn(o[2], __dmul_rn(a, sh[6]))), p.w);
+}
+
+// One thread per active point, CTAs laid out per scan like the other per-point kernels; exits at once for scans that are not in
+// PH_CORR or not undistorted.  The raw point and its time are gathered from the upload buffers by the original index that scan
+// ordering left in w (no ordered raw copy, so the ordering kernels stay as they are): ~52 B per point -- the ordered slot
+// (16 B read for w), the raw point and its time (20 B, gathered), the store (16 B).
+__global__ void __launch_bounds__(kThreads) k_undistort(BatchView bv, float4* __restrict__ sorted, const float4* __restrict__ raw,
+                                                        const float* __restrict__ times, const UndistortParams* __restrict__ par) {
+    const int s = blockIdx.y;
+    const IcpState* st = bv.st + s;
+    if (st->phase != PH_CORR) return;
+    const UndistortParams P = par[s];
+    if (!P.on) return;
+    const uint32_t n = uint32_t(st->n_points);
+    if (blockIdx.x * kThreads >= n) return;
+    __shared__ double sh[9];
+    if (threadIdx.x == 0) und_setup(P, st->x, sh);
+    __syncthreads();
+    const uint32_t i = blockIdx.x * kThreads + threadIdx.x;
+    if (i >= n) return;
+    const size_t base = size_t(bv.offset[s]), gi = base + i;
+    const float w = sorted[gi].w;
+    const size_t src = base + __float_as_uint(w);                        // original index (k_scan_gather / k_prepare_small)
+    float4 o = und_point(P, sh, __ldg(&raw[src]), __ldg(&times[src]));
+    o.w = w;
+    sorted[gi] = o;
+}
+
+void launch_undistort(const BatchView& bv, float4* sorted, const float4* raw, const float* times, const UndistortParams* par,
+                      uint32_t grid_x, uint32_t n_scans, cudaStream_t st) {
+    k_undistort<<<dim3(grid_x, n_scans), kThreads, 0, st>>>(bv, sorted, raw, times, par);
+}
+
+struct UndPose { double v[7]; };
+__global__ void __launch_bounds__(256) k_undistort_cloud(float4* __restrict__ pts, const float* __restrict__ times, uint32_t n,
+                                                         UndistortParams P, UndPose x) {
+    __shared__ double sh[9];
+    if (threadIdx.x == 0) und_setup(P, x.v, sh);
+    __syncthreads();
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    pts[i] = und_point(P, sh, pts[i], times[i]);
+}
+
+static void launch_undistort_cloud(Ctx* c, float4* pts, const float* times, uint32_t n, const UndistortParams& P, const double pose[7]) {
+    UndPose x;
+    for (int k = 0; k < 7; ++k) x.v[k] = pose[k];
+    if (!n) return;
+    timed_launch_begin(c);
+    k_undistort_cloud<<<(n + 255) / 256, 256, 0, c->stream>>>(pts, times, n, P, x);
+    timed_launch_end(c, 7);                                               // counts the launch
+}
+
+int undistort_tail(Ctx* c, MapStore& ms, uint32_t n_new, const double pose[7]) {
+    launch_undistort_cloud(c, ms.d_xyzi + ms.n, c->und.d_time, n_new, c->und.last, pose);
+    SO_CUDA_TRY(cudaGetLastError());
+    return SO_OK;
+}
+
+void undistort_free(Ctx* c) {
+    cudaFree(c->und.d_par); cudaFree(c->und.d_time); cudaFree(c->und.d_hook); cudaFree(c->und.d_hook_time);
+}
+
+// ------------------------------------------------------------------------------------------------------------------ host side
+static bool finite_pose(const double p[7]) {
+    for (int k = 0; k < 7; ++k) if (!std::isfinite(p[k])) return false;
+    return p[3] * p[3] + p[4] * p[4] + p[5] * p[5] + p[6] * p[6] > 0.0;
+}
+
+static int check_undistort(const so_undistort* u) {
+    if (!u) return fail(SO_ERR_ARG, "bad args");
+    if (u->mode == 2) return fail(SO_ERR_ARG, "so_undistort.mode 2 (OPTIMIZED) is not implemented");
+    if (u->mode != 0 && u->mode != 1) return fail(SO_ERR_ARG, "so_undistort.mode must be 0 (NONE) or 1 (APPROXIMATED)");
+    if (u->mode == 0) return SO_OK;
+    if (u->rotation != 0 && u->rotation != 1) return fail(SO_ERR_ARG, "so_undistort.rotation must be 0 or 1");
+    if (!(std::isfinite(u->dt) && u->dt > 0.0)) return fail(SO_ERR_ARG, "so_undistort.dt must be finite and > 0");
+    if (!finite_pose(u->prev_pose)) return fail(SO_ERR_ARG, "so_undistort.prev_pose must be finite with a non-zero quaternion");
+    return SO_OK;
+}
+
+static UndistortParams make_params(const so_undistort& u) {
+    UndistortParams P{};
+    P.on = u.mode == 1 ? 1 : 0;
+    if (!P.on) return P;
+    P.q_prev_conj[0] = -u.prev_pose[3]; P.q_prev_conj[1] = -u.prev_pose[4]; P.q_prev_conj[2] = -u.prev_pose[5]; P.q_prev_conj[3] = u.prev_pose[6];
+    for (int a = 0; a < 3; ++a) P.t_prev[a] = u.prev_pose[a];
+    P.dt = u.dt;
+    P.rotation = u.rotation;
+    return P;
+}
+
+// The float at byte time_offset of every record -> dst (device)
+static int upload_times(Ctx* c, const void* src, size_t n, size_t stride, size_t toff, float* dst) {
+    if (n == 0) return SO_OK;
+    std::vector<float> h(n);
+    const unsigned char* p = static_cast<const unsigned char*>(src) + toff;
+    for (size_t i = 0; i < n; ++i, p += stride) std::memcpy(&h[i], p, 4);
+    SO_CUDA_TRY(cudaMemcpyAsync(dst, h.data(), n * sizeof(float), cudaMemcpyHostToDevice, c->stream));   // pageable: staged before return
+    count_h2d(c, n * sizeof(float));
+    return SO_OK;
+}
+
+static int reserve(Ctx* c, size_t n_points) {
+    int rc = grow_buffer(c->und.d_par, c->und.par_cap, size_t(c->max_batch));
+    if (!rc) rc = grow_buffer(c->und.d_time, c->und.time_cap, std::max<size_t>(n_points, 1));
+    return rc;
+}
+
+static int upload_params(Ctx* c, const UndistortParams* P, size_t n) {
+    SO_CUDA_TRY(cudaMemcpyAsync(c->und.d_par, P, n * sizeof(UndistortParams), cudaMemcpyHostToDevice, c->stream));
+    count_h2d(c, n * sizeof(UndistortParams));
+    return SO_OK;
+}
+
+// The single-scan tail: the cloud (n points) is in d_scan, its times in und.d_time
+static int register_one(Ctx* c, uint32_t n, const double pose_in[7], const so_undistort* u, const so_icp_opts* opts, so_icp_result* out,
+                        std::chrono::steady_clock::time_point t0) {
+    const UndistortParams P = make_params(*u);
+    int rc = upload_params(c, &P, 1);
+    if (rc) return rc;
+    c->last_scan_n = n;
+    c->und.last = P;
+    rc = register_core(c, c->d_scan, &n, 1, pose_in, opts, out, true, nullptr, nullptr, nullptr, 0, true);
+    if (rc) return rc;
+    out->scan_edge_num = 0;
+    out->time_total_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    return out->status;
+}
+
+}  // namespace so
+
+using namespace so;
+
+extern "C" {
+
+int so_register_undistort(so_ctx* ctx, const void* surf, size_t n_surf, size_t stride, size_t ioff, size_t toff, const double pose_in[7],
+                          const so_undistort* u, const so_icp_opts* opts, so_icp_result* out) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c || !pose_in || !opts || !out || (!surf && n_surf) || stride < 12 || toff + 4 > stride) return fail(SO_ERR_ARG, "bad args");
+    int rc = check_undistort(u);
+    if (rc) return rc;
+    if (u->mode == 0) return so_register(ctx, surf, n_surf, nullptr, 0, stride, ioff, pose_in, opts, out);
+    if (n_surf > c->cfg.max_scan_points) return fail(SO_ERR_CAPACITY, "scan larger than so_config.max_scan_points");
+    SO_CUDA_TRY(cudaSetDevice(c->device));
+    const auto t0 = std::chrono::steady_clock::now();
+    rc = reserve(c, n_surf);
+    if (!rc) rc = upload_cloud(c, surf, n_surf, stride, ioff, c->d_scan);
+    if (!rc) rc = upload_times(c, surf, n_surf, stride, toff, c->und.d_time);
+    if (rc) return rc;
+    return register_one(c, uint32_t(n_surf), pose_in, u, opts, out, t0);
+}
+
+int so_register_prefiltered_undistort(so_ctx* ctx, const double pose_in[7], const so_undistort* u, const so_icp_opts* opts, so_icp_result* out) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c || !pose_in || !opts || !out) return fail(SO_ERR_ARG, "bad args");
+    int rc = check_undistort(u);
+    if (rc) return rc;
+    if (u->mode == 0) return so_register_prefiltered(ctx, pose_in, opts, out);
+    if (c->prefiltered_n == SIZE_MAX) return fail(SO_ERR_ARG, "so_register_prefiltered_undistort needs a preceding so_scan_prefilter (and nothing that reuses the scan buffers in between)");
+    SO_CUDA_TRY(cudaSetDevice(c->device));
+    const auto t0 = std::chrono::steady_clock::now();
+    const size_t n = c->prefiltered_n;
+    rc = reserve(c, n);
+    if (rc) return rc;
+    c->prefiltered_n = SIZE_MAX;
+    if (n) {
+        SO_CUDA_TRY(cudaMemcpyAsync(c->d_scan, c->d_scan_sorted, n * sizeof(float4), cudaMemcpyDeviceToDevice, c->stream));
+        // the filtered cloud's w (the VoxelGrid average of the time the extraction stored in intensity) is the time
+        SO_CUDA_TRY(cudaMemcpy2DAsync(c->und.d_time, sizeof(float), reinterpret_cast<const char*>(c->d_scan_sorted) + 12, sizeof(float4),
+                                      sizeof(float), n, cudaMemcpyDeviceToDevice, c->stream));
+    }
+    return register_one(c, uint32_t(n), pose_in, u, opts, out, t0);
+}
+
+int so_register_batch_undistort(so_ctx* ctx, const void* surf, const uint32_t* n_points, size_t n_scans, size_t stride, size_t ioff, size_t toff,
+                                const double* poses_in, const so_undistort* u, const so_icp_opts* opts, so_icp_result* results) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c || !surf || !n_points || !poses_in || !u || !opts || !results || stride < 12 || toff + 4 > stride) return fail(SO_ERR_ARG, "bad args");
+    if (n_scans == 0 || n_scans > c->max_batch) return fail(SO_ERR_CAPACITY, "n_scans exceeds so_config.max_batch");
+    size_t total = 0;
+    for (size_t s = 0; s < n_scans; ++s) { if (n_points[s] > c->cfg.max_scan_points) return fail(SO_ERR_CAPACITY, "scan too large"); total += n_points[s]; }
+    std::vector<UndistortParams> P(n_scans);
+    bool any = false;
+    for (size_t s = 0; s < n_scans; ++s) {
+        int rc = check_undistort(u + s);
+        if (rc) return rc;
+        P[s] = make_params(u[s]);
+        any |= P[s].on != 0;
+    }
+    SO_CUDA_TRY(cudaSetDevice(c->device));
+    const auto t0 = std::chrono::steady_clock::now();
+    c->und.last.on = 0;                                                  // d_scan and the times no longer hold the last single scan
+    int rc = reserve(c, total);
+    if (!rc && any) rc = upload_times(c, surf, total, stride, toff, c->und.d_time);
+    if (!rc && any) rc = upload_params(c, P.data(), n_scans);
+    if (rc) return rc;
+    if (stride == 16 && ioff == 12) {                                   // packed: chunked upload overlapped with the kernels, as so_register_batch
+        rc = register_core(c, c->d_scan, n_points, n_scans, poses_in, opts, results, false, surf, nullptr, nullptr, 0, any);
+    } else {
+        rc = upload_cloud(c, surf, total, stride, ioff, c->d_scan);
+        if (!rc) rc = register_core(c, c->d_scan, n_points, n_scans, poses_in, opts, results, false, nullptr, nullptr, nullptr, 0, any);
+    }
+    if (rc) return rc;
+    const double ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    for (size_t s = 0; s < n_scans; ++s) results[s].time_total_ms = ms;
+    return SO_OK;
+}
+
+int so_undistort_points(so_ctx* ctx, const void* xyzi, size_t n, size_t stride, size_t ioff, size_t toff, const double pose[7],
+                        const so_undistort* u, float* out_xyzi) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c || !pose || (n && (!xyzi || !out_xyzi)) || stride < 12 || toff + 4 > stride || !finite_pose(pose)) return fail(SO_ERR_ARG, "bad args");
+    int rc = check_undistort(u);
+    if (rc) return rc;
+    if (n > c->scan_cap) return fail(SO_ERR_CAPACITY, "cloud larger than the context's scan capacity");
+    SO_CUDA_TRY(cudaSetDevice(c->device));
+    if (n == 0) return SO_OK;
+    rc = grow_buffer(c->und.d_hook, c->und.hook_cap, n);
+    if (!rc) rc = grow_buffer(c->und.d_hook_time, c->und.hook_time_cap, n);
+    if (!rc) rc = upload_cloud(c, xyzi, n, stride, ioff, c->und.d_hook);
+    if (!rc) rc = upload_times(c, xyzi, n, stride, toff, c->und.d_hook_time);
+    if (rc) return rc;
+    if (u->mode == 1) launch_undistort_cloud(c, c->und.d_hook, c->und.d_hook_time, uint32_t(n), make_params(*u), pose);
+    SO_CUDA_TRY(cudaGetLastError());
+    SO_CUDA_TRY(cudaMemcpyAsync(out_xyzi, c->und.d_hook, n * sizeof(float4), cudaMemcpyDeviceToHost, c->stream));
+    count_d2h(c, n * sizeof(float4));
+    SO_CUDA_TRY(cudaStreamSynchronize(c->stream));
+    return SO_OK;
+}
+
+}  // extern "C"

@@ -563,3 +563,45 @@ def make_raw_sweep(n: int = 50_000, seed: int = 4000, sweep_s: float = 0.1, star
                      w1 * w2 - x1 * x2 - y1 * y2 - z1 * z2]
     T_i_l = np.r_[0.05, -0.02, 0.11, _quat_axis_angle([0.2, 1.0, -0.1], 0.35)]
     return dict(points=pts, start_time=start_time, sample_times=st, sample_poses=sp, T_i_l=T_i_l)
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# Motion-distorted scans (within-scan motion compensation, so_register_undistort)
+# ---------------------------------------------------------------------------------------------------------------
+def make_moving_scan(scene: Scene, sensor: str, pose_start: np.ndarray, speed: float, yaw_rate: float, seed: int,
+                     sweep_s: float = 0.1, dt: float = 0.1, imu_deskewed: bool = False, range_noise: float = 0.01,
+                     rmin: float = 0.2, rmax: float = 130.0):
+    """A spinning-lidar sweep taken while the sensor moves: constant forward body velocity `speed` (m/s, along the start pose's
+    x axis) and yaw rate `yaw_rate` (rad/s).  Column c fires at t = c / n_cols * sweep_s and is ray-cast from the pose at t; its
+    points are expressed in the sensor frame at t, with t stored in intensity.  imu_deskewed rotates every point into the start
+    orientation (what so_scan_deskew with imu_only leaves: rotation removed, translation kept).
+    -> dict(scan_xyzi float32 [n,4], pose_true (the pose at the sweep start), pose_prev / pose_next (the same motion at -dt / +dt),
+    prior)."""
+    vlp = sensor == "vlp16"
+    n_cols, n_rings = (1800, 16) if vlp else (1024, 128)
+    if sensor not in ("vlp16", "os1_128"):
+        raise ValueError(sensor)
+    rng = np.random.default_rng(seed)
+    dirs = sensor_dirs(sensor).reshape(n_cols, n_rings, 3)
+    q0 = np.asarray(pose_start[3:], np.float64)
+    R0 = quat_to_R(q0)
+    v_w = R0 @ np.array([speed, 0.0, 0.0])
+
+    def pose_at(t):
+        q = quat_mul(q0, quat_from_rotvec(np.array([0.0, 0.0, yaw_rate * t])))
+        return np.concatenate([pose_start[:3] + v_w * t, q / np.linalg.norm(q)])
+
+    out = []
+    for c in range(n_cols):
+        t = c / n_cols * sweep_s
+        P = pose_at(t)
+        d = dirs[c]
+        r = raycast(scene, P[:3], d @ quat_to_R(P[3:]).T) + rng.normal(0.0, range_noise, size=len(d))
+        ok = np.isfinite(r) & (r > rmin) & (r < rmax)
+        pts = d[ok] * r[ok, None]
+        if imu_deskewed:
+            pts = pts @ quat_to_R(quat_from_rotvec(np.array([0.0, 0.0, yaw_rate * t]))).T
+        out.append(np.concatenate([pts, np.full((len(pts), 1), t)], 1))
+    scan = np.concatenate(out).astype(np.float32)
+    prior = perturb_pose(pose_start, seed + 7, dt=0.05, dth_deg=0.5)
+    return dict(scan_xyzi=scan, pose_true=np.asarray(pose_start, np.float64), pose_prev=pose_at(-dt), pose_next=pose_at(dt), prior=prior)
