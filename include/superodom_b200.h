@@ -255,7 +255,8 @@ int so_register_batch_device(so_ctx* ctx, const void* d_scans_xyzi, const uint32
  * non-finite prev_pose) are returned before any device work.  After so_register_undistort / so_register_prefiltered_undistort,
  * so_map_add_registered_scan(pose) inserts the whole cloud undistorted with the D that pose gives: world = T(pose) * pInit. */
 typedef struct {
-    int32_t mode;          /* 0 NONE (the scan registers exactly as so_register), 1 APPROXIMATED; 2 (OPTIMIZED) -> SO_ERR_ARG */
+    int32_t mode;          /* 0 NONE (the scan registers exactly as so_register), 1 APPROXIMATED; 2 (OPTIMIZED) -> SO_ERR_ARG:
+                              OPTIMIZED estimates a second pose, see so_register_optimized */
     int32_t rotation;      /* 1 rotation + translation, 0 translation only (cloud already rotation-deskewed by so_scan_deskew imu_only) */
     double prev_pose[7];   /* previous registration's pose7 */
     double dt;             /* seconds from prev_pose to the pose being estimated, finite and > 0 */
@@ -271,6 +272,40 @@ int so_register_batch_undistort(so_ctx* ctx, const void* surf_xyzi, const uint32
 /* Stage hook: pInit of a cloud at T_cur = pose, as packed float4 {x, y, z, intensity} in input order (mode 0: the cloud as is). */
 int so_undistort_points(so_ctx* ctx, const void* xyzi, size_t n, size_t stride_bytes, size_t intensity_offset, size_t time_offset,
                         const double pose[7], const so_undistort* u, float* out_xyzi);
+
+/* ---- within-scan motion estimated by the registration (LidarSlam.h:77-81 UndistortionMode::OPTIMIZED; empty upstream) ---------
+ * Two pose7 unknowns per scan: T, the pose at time 0 (what every registration estimates), and D, the motion over dt, so that the
+ * pose at time dt is T * D.  With alpha_i = double(time_i) / dt (0 for a non-finite time) the solve's point is
+ *   u_i(D) = qrot(slerp(identity, q_D, alpha_i), p_i) + alpha_i * t_D
+ * and its rows are so_register's plane rows at T on u_i(D), plus six rows of SE3AbsolutatePoseFactor on D (measurement
+ * motion_prior, row k multiplied by sqrt(n_ok * motion_info[k]), n_ok the accepted correspondences of the ICP iteration).  Every ICP
+ * iteration searches and fits at T on float(u(D)) at the current D.  Surf cloud only; use_pose_prior must be 0.  Argument errors (a
+ * bad dt, a non-finite motion_prior or one with a zero quaternion, a negative or non-finite motion_info, use_pose_prior) are returned
+ * before any device work.  icp.cov and the error fields describe T.  After so_register_optimized /
+ * so_register_prefiltered_optimized, so_map_add_registered_scan(pose) inserts T(pose) * u_i(D_opt) for the whole cloud. */
+typedef struct {
+    double dt;               /* seconds the motion spans, finite and > 0 */
+    double motion_prior[7];  /* D0, e.g. T_prev^-1 * pose_in; identity {0,0,0, 0,0,0,1} when unknown */
+    double motion_info[6];   /* information of D0 per accepted correspondence (translation xyz, rotation xyz), >= 0 */
+} so_motion;
+typedef struct {
+    so_icp_result icp;       /* icp.pose_opt = T */
+    double motion[7];        /* D */
+    double pose_end[7];      /* T * D, the pose at time dt */
+} so_motion_result;
+int so_register_optimized(so_ctx* ctx, const void* surf_xyzi, size_t n, size_t stride_bytes, size_t intensity_offset, size_t time_offset,
+                          const double pose_in[7], const so_motion* m, const so_icp_opts* opts, so_motion_result* out);
+/* ... of the cloud the last so_scan_prefilter left on the device; the time is the filtered cloud's intensity (w). */
+int so_register_prefiltered_optimized(so_ctx* ctx, const double pose_in[7], const so_motion* m, const so_icp_opts* opts, so_motion_result* out);
+/* ... of a batch as so_register_batch, m[n_scans]: one so_motion per scan. */
+int so_register_batch_optimized(so_ctx* ctx, const void* surf_xyzi, const uint32_t* n_points, size_t n_scans, size_t stride_bytes,
+                                size_t intensity_offset, size_t time_offset, const double* poses_in, const so_motion* m,
+                                const so_icp_opts* opts, so_motion_result* results);
+/* Stage hook: the correspondences at T = pose for float(u(motion)), then the plane rows' normal equations at (T, motion) over the
+ * 12 tangent columns (T's translation, rotation, D's translation, rotation): H (row-major 12x12), g, cost; prior rows excluded. */
+int so_evaluate_optimized(so_ctx* ctx, const void* xyzi, size_t n, size_t stride_bytes, size_t intensity_offset, size_t time_offset,
+                          const double pose[7], const double motion[7], double dt, int32_t max_surface_features, double H[144],
+                          double g[12], double* cost);
 
 /* Sharded-replay plumbing (BASELINE cfg4; SURVEY 8e "K8"): a caller-owned DEVICE buffer of cap_rows x 8 doubles.  Every following
  * so_register / so_register_batch* call appends one row per scan, starting at first_row and advancing: {pose_opt[7] (the
@@ -431,7 +466,8 @@ int so_bytes_copied(so_ctx* ctx, uint64_t* h2d, uint64_t* d2h, int reset);
  * k_lm_step (LM step), 2 k_knn (so_knn*), 3 scan ordering / map build / map insert / scan preparation, 4 first evaluation of
  * a solve (k_evaluate + k_lm_step iteration zero), 5 k_fit (plane fit), 6 global localization search (bitmap raster, dilation,
  * hypothesis scoring, key sort; for the branch-and-bound also map bounds, pyramid levels, offset table and traversal steps),
- * 7 k_undistort (within-scan motion compensation: per ICP iteration, and the undistorted map insert / so_undistort_points).
+ * 7 k_undistort (within-scan motion compensation: per ICP iteration, and the undistorted map insert / so_undistort_points; the
+ * per-iteration warp and the map insert of so_register_optimized*), 8 evaluation + trust-region step of so_register_optimized*.
  * Profiling mode serialises kernels; enable only for roofline runs. */
 /* Build-time switches of the loaded library.  Bit 0 (SO_BUILD_FUSED_MATCH, search and fit as one kernel) is reserved: this
  * library always runs them as two kernels and returns 0. */

@@ -241,7 +241,13 @@ public:
     std::array<int, nFeatureObs> PlaneFeatureHistogramObs{};
     std::array<int, nRejectionCauses> MatchRejectionHistogramLine{}, MatchRejectionHistogramPlane{};
     size_t LocalizationICPMaxIter = 4;                           // LidarSlam.h:273
-    UndistortionMode Undistortion = NONE;                        // LidarSlam.h:266; APPROXIMATED: so_register_undistort, time in intensity
+    UndistortionMode Undistortion = NONE;                        // LidarSlam.h:266; APPROXIMATED: so_register_undistort, OPTIMIZED:
+                                                                 // so_register_optimized; time in intensity
+    // OPTIMIZED: information per accepted correspondence of the motion prior D0 = undistort_prev_pose^-1 * position (translation
+    // xyz, rotation xyz).  0, a free motion, has the smallest worst-case pose error of the accuracy sweep in DESIGN.md §4; a larger
+    // value helps only while the velocity stays what the previous registration saw
+    double OptimizedMotionInformation[6] = {0, 0, 0, 0, 0, 0};
+    Transformd LastMotion;                                       // OPTIMIZED: the motion D the last registration estimated (identity otherwise)
     bool UndistortRotation = true;                               // shim only: false when the cloud's rotation was already removed
                                                                  // (featureExtraction's IMU branch, so_scan_deskew imu_only)
     Transformd undistort_prev_pose;                              // pose of the previous scan (last_T_w_lidar is the prior by then)
@@ -257,7 +263,6 @@ public:
     template <class CloudPtr>
     void Localization(bool initialization, PredictionSource predictodom, const Transformd& position, const CloudPtr& edge_point,
                       const CloudPtr& planner_point, double timeLaserOdometry) {
-        if (Undistortion == OPTIMIZED) throw Error("UndistortionMode::OPTIMIZED is not implemented");
         T_w_lidar = position; T_w_initial_guess = position; last_T_w_lidar = position;          // initializeState (:53-57)
         localMap.sync_resolution();
         size_t stride, ioff;
@@ -291,7 +296,19 @@ public:
         position.to_pose7(pose);
         const double dt = timeLaserOdometry - lasttimeLaserOdometry;
         int rc;
-        if (Undistortion == APPROXIMATED && undistort_has_prev && dt > 0 && !(edge_point && edge_point->size())) {
+        LastMotion = Transformd();
+        if (Undistortion == OPTIMIZED && dt > 0 && !(edge_point && edge_point->size()) && !o.use_pose_prior) {
+            so_motion m{};                                         // the surf cloud only; so_register_optimized refuses the pose prior
+            m.dt = dt;
+            const Transformd D0 = undistort_has_prev ? undistort_prev_pose.inverse() * position : Transformd();
+            D0.to_pose7(m.motion_prior);
+            for (int k = 0; k < 6; ++k) m.motion_info[k] = OptimizedMotionInformation[k];
+            so_motion_result mr{};
+            rc = so_register_optimized(context.h, surf, planner_point->size(), stride, ioff, ioff, pose, &m, &o, &mr);
+            check(rc, "so_register_optimized");
+            last_result = mr.icp;
+            LastMotion = Transformd::from_pose7(mr.motion);
+        } else if (Undistortion == APPROXIMATED && undistort_has_prev && dt > 0 && !(edge_point && edge_point->size())) {
             so_undistort u{};                                      // the surf cloud only; the edge cloud is empty upstream
             u.mode = 1; u.rotation = UndistortRotation ? 1 : 0; u.dt = dt;
             undistort_prev_pose.to_pose7(u.prev_pose);

@@ -21,7 +21,7 @@ EXPORTS = [
     "so_map_set_resolution", "so_map_set_origin", "so_map_get_origin", "so_map_shift", "so_map_set_points",
     "so_map_set_edge_points", "so_map_add_surf", "so_map_add_edge", "so_map_add_scan", "so_map_add_registered_scan", "so_map_add_scan_edge", "so_map_counts_5x5", "so_map_download", "so_map_size",
     "so_scan_prefilter", "so_scan_deskew", "so_scan_extract_uniform", "so_register", "so_register_prefiltered", "so_register_injected", "so_set_pose_sink", "so_register_batch", "so_register_batch_edges", "so_register_batch_device",
-    "so_register_undistort", "so_register_prefiltered_undistort", "so_register_batch_undistort", "so_undistort_points", "so_correspond", "so_correspond_edge", "so_evaluate",
+    "so_register_undistort", "so_register_prefiltered_undistort", "so_register_batch_undistort", "so_undistort_points", "so_register_optimized", "so_register_prefiltered_optimized", "so_register_batch_optimized", "so_evaluate_optimized", "so_correspond", "so_correspond_edge", "so_evaluate",
     "so_knn", "so_knn_device", "so_sampling_indices", "so_localize_global", "so_localize_scores", "so_localize_global_size", "so_localize_global_bnb", "so_localize_bnb_keys", "so_localize_bnb_bounds", "so_map_bounds", "so_kernel_launches", "so_bytes_copied", "so_build_flags", "so_profile_enable", "so_profile_get",
 ]
 
@@ -61,6 +61,25 @@ class Undistort(C.Structure):
 
 def undistort(prev_pose7, dt: float, rotation: bool = True, mode: int = 1) -> Undistort:
     return Undistort(int(mode), int(rotation), (C.c_double * 7)(*[float(v) for v in prev_pose7]), float(dt))
+
+
+class Motion(C.Structure):
+    """so_motion: the motion prior of so_register_optimized* (D0 over dt seconds, information per accepted correspondence)."""
+    _fields_ = [("dt", C.c_double), ("motion_prior", C.c_double * 7), ("motion_info", C.c_double * 6)]
+
+
+class MotionResult(C.Structure):
+    """so_motion_result: icp.pose_opt = T (the pose at time 0), motion = D, pose_end = T * D (the pose at time dt)."""
+    _fields_ = [("icp", IcpResult), ("motion", C.c_double * 7), ("pose_end", C.c_double * 7)]
+
+
+# motion_info per accepted correspondence that the accuracy sweep of scripts/bench_undistort.py chose (DESIGN.md §4); the C++ shim's
+# LidarSLAM::OptimizedMotionInformation defaults to the same value
+DEFAULT_MOTION_INFO = 0.0
+
+
+def motion(dt: float, prior7=(0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 1.0), info=(DEFAULT_MOTION_INFO,) * 6) -> Motion:
+    return Motion(float(dt), (C.c_double * 7)(*[float(v) for v in prior7]), (C.c_double * 6)(*[float(v) for v in info]))
 
 
 class GlobalOpts(C.Structure):
@@ -162,6 +181,13 @@ def load_library():
                                               C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     L.so_undistort_points.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p, C.c_void_p,
                                       C.c_void_p]
+    L.so_register_optimized.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p, C.c_void_p,
+                                        C.c_void_p, C.c_void_p]
+    L.so_register_prefiltered_optimized.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.so_register_batch_optimized.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t,
+                                              C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.so_evaluate_optimized.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p, C.c_void_p,
+                                        C.c_double, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
     L.so_set_pose_sink.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t]
     L.so_register_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t,
                                     C.c_void_p, C.c_void_p, C.c_void_p]
@@ -511,6 +537,55 @@ class Context:
         self._chk(self.L.so_undistort_points(self.h, _p(a), a.shape[0], stride, 12 if a.shape[1] >= 4 else stride, time_col * 4, _p(pose),
                                              C.byref(u), _p(out)), "so_undistort_points")
         return out[: len(a)]
+
+    # ---- within-scan motion estimated by the registration (m: a Motion, see motion()); time_col: the column holding each point's time
+    def register_optimized(self, scan_xyzi: np.ndarray, pose7, m: Motion, max_icp_iters: int, max_surface_features: int = 0,
+                           time_col: int = 3, **kw) -> MotionResult:
+        s = np.ascontiguousarray(scan_xyzi, dtype=np.float32)
+        pose = np.ascontiguousarray(pose7, dtype=np.float64)
+        o = self._opts(max_icp_iters, max_surface_features, **kw)
+        r = MotionResult()
+        stride = s.shape[1] * 4
+        rc = self.L.so_register_optimized(self.h, _p(s), s.shape[0], stride, 12 if s.shape[1] >= 4 else stride, time_col * 4, _p(pose),
+                                          C.byref(m), C.byref(o), C.byref(r))
+        self._chk(rc, "so_register_optimized")
+        return r
+
+    def register_prefiltered_optimized(self, pose7, m: Motion, max_icp_iters: int, max_surface_features: int = 0, **kw) -> MotionResult:
+        pose = np.ascontiguousarray(pose7, dtype=np.float64)
+        o = self._opts(max_icp_iters, max_surface_features, **kw)
+        r = MotionResult()
+        self._chk(self.L.so_register_prefiltered_optimized(self.h, _p(pose), C.byref(m), C.byref(o), C.byref(r)), "so_register_prefiltered_optimized")
+        return r
+
+    def register_batch_optimized(self, scans_xyzi: np.ndarray, n_points, poses, ms, max_icp_iters: int, max_surface_features: int = 0,
+                                 time_col: int = 3, **kw):
+        """ms: one Motion per scan."""
+        n_points = np.ascontiguousarray(n_points, dtype=np.uint32)
+        poses = np.ascontiguousarray(poses, dtype=np.float64)
+        ns = len(n_points)
+        ma = (Motion * ns)(*ms)
+        o = self._opts(max_icp_iters, max_surface_features, **kw)
+        res = (MotionResult * ns)()
+        a = np.ascontiguousarray(scans_xyzi, dtype=np.float32)
+        stride = a.shape[1] * 4
+        self._chk(self.L.so_register_batch_optimized(self.h, _p(a), _p(n_points), ns, stride, 12, time_col * 4, _p(poses), ma, C.byref(o), res),
+                  "so_register_batch_optimized")
+        return res
+
+    def evaluate_optimized(self, xyzi: np.ndarray, pose7, motion7, dt: float, max_surface_features: int = 0, time_col: int = 3):
+        """Plane rows' (H [12, 12], g [12], cost) at (T = pose7, D = motion7) over the correspondences at T of float(u(D))."""
+        a = np.ascontiguousarray(xyzi, dtype=np.float32)
+        pose = np.ascontiguousarray(pose7, dtype=np.float64)
+        mot = np.ascontiguousarray(motion7, dtype=np.float64)
+        H = np.zeros((12, 12))
+        g = np.zeros(12)
+        cost = C.c_double()
+        stride = a.shape[1] * 4
+        self._chk(self.L.so_evaluate_optimized(self.h, _p(a), a.shape[0], stride, 12 if a.shape[1] >= 4 else stride, time_col * 4, _p(pose),
+                                               _p(mot), float(dt), int(max_surface_features), _p(H), _p(g), C.byref(cost)),
+                  "so_evaluate_optimized")
+        return H, g, cost.value
 
     def register_batch(self, scans_xyzi: np.ndarray, n_points, poses, max_icp_iters: int, max_surface_features: int = 0, **kw):
         """scans_xyzi: float32 [sum(n_points), 4] host array (pinned or pageable)."""

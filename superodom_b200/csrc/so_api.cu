@@ -155,6 +155,7 @@ static void ctx_free(Ctx* c) {
     cudaFree(c->d_dec);
     global_free(c);
     undistort_free(c);
+    motion_free(c);
     if (c->ev_dec) cudaEventDestroy(c->ev_dec);
     if (c->ev0) cudaEventDestroy(c->ev0);
     if (c->ev1) cudaEventDestroy(c->ev1);
@@ -307,9 +308,11 @@ static int prepare_scans(Ctx* c, const float4* d_scan_in, const Chunk& ch, cudaS
 // scan is not in the matching phase, so a fixed schedule follows whatever path the device-side state machine takes.
 // Preferred form: a CUDA-graph WHILE node around ONE iteration (k_loop_cond ends the loop when every scan of the chunk
 // is done); fallback: the schedule unrolled max_icp_iters times.  Returns whether the loop form ran.
-// undistort: k_undistort (the scans' pInit at the current pose, so_undistort.cu) heads every iteration.
+// undistort 1: k_undistort (the scans' pInit at the current pose, so_undistort.cu) heads every iteration.
+// undistort 2 (so_motion.cu): [k_motion_warp, k_knn_scan, k_fit, k_motion_eval<PH_CORR>, k_motion_step, (k_motion_eval<PH_EVAL>,
+// k_motion_step) x lm] per iteration: the motion is a second parameter block of the solve.
 static int run_schedule(Ctx* c, const Chunk& ch, int iters, int lm, bool with_nn, bool* was_loop, cudaStream_t run_stream = nullptr,
-                        const uint32_t* d_inject = nullptr, int inject_iters = 0, bool undistort = false) {
+                        const uint32_t* d_inject = nullptr, int inject_iters = 0, int undistort = 0) {
     if (!run_stream) run_stream = c->stream;
     const float4* d_scan = c->d_scan_sorted;
     const MapView mv = map_view(c, c->surf);
@@ -318,7 +321,7 @@ static int run_schedule(Ctx* c, const Chunk& ch, int iters, int lm, bool with_nn
     if (!with_nn) { cb.nn = nullptr; cb.nn_d2 = nullptr; }
     const uint32_t grid_x = ch.grid_x, n_scans = ch.count, grid_e = ch.grid_e;
     // one or two scans in flight: launch-latency bound -> optimiser step folded into the evaluation kernels (k_evaluate_lm)
-    if (n_scans <= 2 && !c->profiling && !c->no_fused_lm) bv.counters = c->d_counters + ch.first;
+    if (n_scans <= 2 && !c->profiling && !c->no_fused_lm && undistort != 2) bv.counters = c->d_counters + ch.first;
     bv.coop_knn = n_scans <= 2 && grid_x <= kCoopMaxGrid && !c->no_coop_knn;      // latency-bound search: a warp per query
     const MapView me = map_view(c, c->edge);
     EdgeBuf eb = c->ebuf;
@@ -326,7 +329,23 @@ static int run_schedule(Ctx* c, const Chunk& ch, int iters, int lm, bool with_nn
     if (!with_nn) { eb.nn = nullptr; eb.selmask = nullptr; }
     *was_loop = false;
     auto undistort_step = [&](cudaStream_t s) {
-        launch_undistort(bv, c->d_scan_sorted, c->d_scan, c->und.d_time, c->und.d_par + ch.first, grid_x, n_scans, s);
+        if (undistort == 2) launch_motion_warp(bv, c->d_scan_sorted, c->d_scan, c->und.d_time, c->mot.d_st, ch.first, grid_x, n_scans, s);
+        else launch_undistort(bv, c->d_scan_sorted, c->d_scan, c->und.d_time, c->und.d_par + ch.first, grid_x, n_scans, s);
+    };
+    double* const mot_partials = c->mot.d_partials ? c->mot.d_partials + size_t(ch.first) * c->mot.stride * kMotionAcc : nullptr;
+    auto motion_solve = [&](int phase, cudaStream_t s) {
+        launch_motion_solve(phase, bv, cb, c->d_scan, c->und.d_time, c->mot.d_st, ch.first, mot_partials, c->mot.stride, grid_x, n_scans, s);
+    };
+    // one ICP iteration after the (optional) undistortion head: correspondences, the first evaluation and lm candidate evaluations
+    auto iteration = [&](cudaStream_t s) {
+        if (undistort == 2) {
+            launch_match(mv, bv, cb, c->nn, grid_x, n_scans, s);
+            motion_solve(PH_CORR, s);
+            for (int k = 0; k < lm; ++k) motion_solve(PH_EVAL, s);
+            return;
+        }
+        launch_correspond(mv, bv, cb, c->nn, grid_x, n_scans, s, &me, &eb, grid_e);
+        for (int k = 0; k < lm; ++k) launch_evaluate(bv, cb, grid_x, n_scans, s, &eb, grid_e);
     };
     if (c->profiling || with_nn || d_inject) {
         // profiling mode: one launch at a time, timed with events, and only launches that have work (the host peeks
@@ -339,6 +358,16 @@ static int run_schedule(Ctx* c, const Chunk& ch, int iters, int lm, bool with_nn
             return false;
         };
         for (int it = 0; it < iters; ++it) {
+            if (undistort == 2) {                                // every scan is in PH_CORR or PH_DONE when an iteration starts
+                if (!any_in(PH_CORR)) continue;
+                timed_launch_begin(c); undistort_step(c->stream); timed_launch_end(c, 7);
+                timed_launch_begin(c); launch_match(mv, bv, cb, c->nn, grid_x, n_scans, c->stream, 1); timed_launch_end(c, 0);
+                timed_launch_begin(c); launch_match(mv, bv, cb, c->nn, grid_x, n_scans, c->stream, 2); timed_launch_end(c, 5);
+                timed_launch_begin(c); motion_solve(PH_CORR, c->stream); c->launches++; timed_launch_end(c, 8);
+                for (int k = 0; k < lm; ++k)
+                    if (any_in(PH_EVAL)) { timed_launch_begin(c); motion_solve(PH_EVAL, c->stream); c->launches++; timed_launch_end(c, 8); }
+                continue;
+            }
             if (any_in(PH_CORR)) {
                 if (undistort) { timed_launch_begin(c); undistort_step(c->stream); timed_launch_end(c, 7); }
                 timed_launch_begin(c);
@@ -361,7 +390,7 @@ static int run_schedule(Ctx* c, const Chunk& ch, int iters, int lm, bool with_nn
     key.ptrs[4] = me.pts; key.ptrs[5] = me.cell_start; key.ptrs[6] = me.block_slot; key.ptrs[7] = me.block_count;
     for (int a = 0; a < 3; ++a) key.origin[a] = mv.origin[a];
     key.nb[0] = mv.nb; key.nb[1] = me.nb; key.res[0] = mv.plane_res; key.res[1] = me.plane_res;
-    if (undistort) { key.undistort = 1; key.und_time = c->und.d_time; }
+    if (undistort) { key.undistort = undistort; key.und_time = c->und.d_time; }
     Ctx::GraphSlot* slot = nullptr;
     for (auto& g : c->graphs)
         if (g.exec && std::memcmp(&g.key, &key, sizeof(key)) == 0) slot = &g;
@@ -386,8 +415,7 @@ static int run_schedule(Ctx* c, const Chunk& ch, int iters, int lm, bool with_nn
                 ok = cudaStreamBeginCaptureToGraph(c->stream, body, nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal) == cudaSuccess;
                 if (ok) {
                     if (undistort) undistort_step(c->stream);
-                    launch_correspond(mv, bv, cb, c->nn, grid_x, n_scans, c->stream, &me, &eb, grid_e);
-                    for (int k = 0; k < lm; ++k) launch_evaluate(bv, cb, grid_x, n_scans, c->stream, &eb, grid_e);
+                    iteration(c->stream);
                     launch_loop_cond(bv, n_scans, handle, c->stream);
                     cudaGraph_t dummy = nullptr;
                     ok = cudaStreamEndCapture(c->stream, &dummy) == cudaSuccess;
@@ -403,8 +431,7 @@ static int run_schedule(Ctx* c, const Chunk& ch, int iters, int lm, bool with_nn
             SO_CUDA_TRY(cudaStreamBeginCapture(c->stream, cudaStreamCaptureModeThreadLocal));
             for (int it = 0; it < iters; ++it) {
                 if (undistort) undistort_step(c->stream);
-                launch_correspond(mv, bv, cb, c->nn, grid_x, n_scans, c->stream, &me, &eb, grid_e);
-                for (int k = 0; k < lm; ++k) launch_evaluate(bv, cb, grid_x, n_scans, c->stream, &eb, grid_e);
+                iteration(c->stream);
             }
             SO_CUDA_TRY(cudaStreamEndCapture(c->stream, &g));
             cudaError_t e = cudaGraphInstantiate(&slot->exec, g, 0);
@@ -416,7 +443,9 @@ static int run_schedule(Ctx* c, const Chunk& ch, int iters, int lm, bool with_nn
     slot->used = ++c->graph_clock;
     SO_CUDA_TRY(cudaGraphLaunch(slot->exec, run_stream));
     *was_loop = slot->is_loop;
-    if (!slot->is_loop) c->launches += uint64_t(iters) * ((bv.counters && !grid_e ? 2 + 1 + lm : 2 + 2 + 2 * lm + (grid_e ? 1 + lm : 0)) + (undistort ? 1 : 0));      // 2: k_knn_scan + k_fit; loop form: counted from the iterations executed
+    if (!slot->is_loop)
+        c->launches += uint64_t(iters) * (undistort == 2 ? 1 + 2 + 2 + 2 * lm
+                                                         : (bv.counters && !grid_e ? 2 + 1 + lm : 2 + 2 + 2 * lm + (grid_e ? 1 + lm : 0)) + (undistort ? 1 : 0));      // 2: k_knn_scan + k_fit; loop form: counted from the iterations executed
     return SO_OK;
 }
 
@@ -476,7 +505,7 @@ int icp_opts_check(const so_icp_opts& o) {
 // function uploads them into d_scan chunk by chunk on the copy stream.
 int register_core(Ctx* c, const float4* d_scan, const uint32_t* n_points, size_t n_scans, const double* poses, const so_icp_opts* opts_in,
                   so_icp_result* results, bool allow_shift, const void* host_src, const uint32_t* n_edge, const uint32_t* d_inject, int inject_iters,
-                  bool undistort) {
+                  int undistort) {
     so_icp_opts o = *opts_in;
     if (o.lm_max_iterations <= 0) o.lm_max_iterations = 4;
     { int rc = icp_opts_check(o); if (rc) return rc; }
@@ -604,6 +633,7 @@ int register_core(Ctx* c, const float4* d_scan, const uint32_t* n_points, size_t
             int max_it = 0;
             for (uint32_t s = chunks[k].first; s < chunks[k].first + chunks[k].count; ++s) max_it = std::max(max_it, int(c->h_state[s].n_iterations));
             const bool fused = chunks[k].count <= 2 && !chunks[k].grid_e && !c->no_fused_lm;
+            if (undistort == 2) { c->launches += uint64_t(max_it) * uint64_t(1 + 2 + 3 + 2 * o.lm_max_iterations); continue; }
             c->launches += uint64_t(max_it) * uint64_t((fused ? 2 + 2 + o.lm_max_iterations
                                                               : 2 + 3 + 2 * o.lm_max_iterations + (chunks[k].grid_e ? 1 + o.lm_max_iterations : 0)) + (undistort ? 1 : 0));
         }
@@ -1412,7 +1442,7 @@ int so_profile_enable(so_ctx* ctx, int on) {
 
 int so_profile_get(so_ctx* ctx, int cls, double* ms, uint64_t* launches, int reset) {
     Ctx* c = reinterpret_cast<Ctx*>(ctx);
-    if (!c || cls < 0 || cls > 7) return fail(SO_ERR_ARG, "bad args");
+    if (!c || cls < 0 || cls > 8) return fail(SO_ERR_ARG, "bad args");
     if (ms) *ms = c->prof[cls].ms;
     if (launches) *launches = c->prof[cls].launches;
     if (reset) c->prof[cls] = ProfileSlot{};

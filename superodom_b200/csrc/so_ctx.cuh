@@ -36,6 +36,8 @@ int grow_buffer(T*& p, size_t& cap, size_t n) {
 }
 
 struct ProfileSlot { double ms = 0.0; uint64_t launches = 0; };
+struct MotionState;                                // so_motion.cu: per-scan motion block of mode OPTIMIZED
+constexpr int kMotionAcc = 91;                     // 78 (upper triangle of the 12x12 H) + 12 (g) + 1 (cost)
 
 // Within-scan motion compensation of one scan (so_undistort, mode APPROXIMATED): everything k_undistort needs besides the
 // current pose.  Kept out of IcpState so that the other kernels do not change.
@@ -186,14 +188,22 @@ struct Ctx {
         float* d_time = nullptr; size_t time_cap = 0;                      // per-point times of the scans in d_scan (upload order)
         float4* d_hook = nullptr; size_t hook_cap = 0;                     // so_undistort_points: the cloud and its times
         float* d_hook_time = nullptr; size_t hook_time_cap = 0;
-        UndistortParams last{};                                            // of the scan so_map_add_registered_scan inserts (on == 0: none)
+        UndistortParams last{};                                            // of the scan so_map_add_registered_scan inserts (on == 0: none,
+                                                                           // 2: so_register_optimized*, the motion is mot.last_D)
     } und;
+    // ---- within-scan motion estimated by the registration (so_register_optimized*): allocated on first use ------------------
+    struct Mot {
+        MotionState* d_st = nullptr; size_t st_cap = 0;                    // [max_batch] per-scan motion blocks
+        double* d_partials = nullptr; size_t partials_cap = 0;             // [max_batch][stride][kMotionAcc] per-CTA sums
+        uint32_t stride = 0;                                               // CTAs per scan the partials are laid out for
+        double last_D[7] = {0, 0, 0, 0, 0, 0, 1};                          // D_opt of the last single-scan registration (und.last.on == 2)
+    } mot;
 
     // ---- instrumentation ----------------------------------------------------------------------------------------
     uint64_t launches = 0;
     uint64_t bytes_h2d = 0, bytes_d2h = 0;         // host<->device bytes moved by registration / k-NN calls
     bool profiling = false;
-    ProfileSlot prof[8];
+    ProfileSlot prof[9];
     cudaEvent_t ev0 = nullptr, ev1 = nullptr, evp0 = nullptr, evp1 = nullptr;
 };
 
@@ -208,9 +218,10 @@ void timed_launch_begin(Ctx* c);
 void timed_launch_end(Ctx* c, int cls);                     // counts one launch; profile class cls when profiling
 int icp_opts_check(const so_icp_opts& o);                   // max_icp_iters and lm_max_iterations in the supported range
 // Registration of n_scans scans at d_scan (packed, back to back), or of host_src's packed scans uploaded chunk by chunk.
+// undistort: 0 none, 1 APPROXIMATED (Ctx::und.d_par), 2 OPTIMIZED (Ctx::mot.d_st; every scan of the call).
 int register_core(Ctx* c, const float4* d_scan, const uint32_t* n_points, size_t n_scans, const double* poses,
                   const so_icp_opts* opts_in, so_icp_result* results, bool allow_shift, const void* host_src = nullptr,
-                  const uint32_t* n_edge = nullptr, const uint32_t* d_inject = nullptr, int inject_iters = 0, bool undistort = false);
+                  const uint32_t* n_edge = nullptr, const uint32_t* d_inject = nullptr, int inject_iters = 0, int undistort = 0);
 inline float4 read_point(const unsigned char* p, size_t stride, size_t ioff) {     // one point of a strided host cloud
     float xyz[3], it = 0.f;
     std::memcpy(xyz, p, 12);
@@ -221,11 +232,23 @@ inline float4 read_point(const unsigned char* p, size_t stride, size_t ioff) {  
 void global_free(Ctx* c);                                   // the search buffers and events of Ctx::reloc / Ctx::bnb
 // so_undistort.cu
 void undistort_free(Ctx* c);                                // the buffers of Ctx::und
+bool finite_pose(const double p[7]);                        // finite, with a non-zero quaternion
+int upload_times(Ctx* c, const void* src, size_t n, size_t stride, size_t toff, float* dst);   // the float at toff of every record -> dst
 // k_undistort: pInit of every active point of the chunk's scans (bv.st / bv.offset / par already offset to the chunk), from the
 // raw points in upload order (raw, times: indexed offset + original index) into the ordered copy `sorted`, w kept
 void launch_undistort(const BatchView& bv, float4* sorted, const float4* raw, const float* times, const UndistortParams* par,
                       uint32_t grid_x, uint32_t n_scans, cudaStream_t st);
 int undistort_tail(Ctx* c, MapStore& ms, uint32_t n_new, const double pose[7]);   // ms tail = the registered scan: pInit at pose, in place
+// so_motion.cu
+void motion_free(Ctx* c);                                   // the buffers of Ctx::mot
+int motion_tail(Ctx* c, MapStore& ms, uint32_t n_new);      // ms tail = the registered scan: u(mot.last_D), in place
+// One ICP iteration's kernels of mode OPTIMIZED for the chunk's scans (bv.st / bv.offset / partials already offset to the chunk, ms
+// the whole array and `first` the chunk's first scan): the warp u(D) into `sorted`, and one evaluation + trust-region step (phase
+// PH_CORR: the first of a solve)
+void launch_motion_warp(const BatchView& bv, float4* sorted, const float4* raw, const float* times, const MotionState* ms, uint32_t first,
+                        uint32_t grid_x, uint32_t n_scans, cudaStream_t st);
+void launch_motion_solve(int phase, const BatchView& bv, const CorrBuf& cb, const float4* raw, const float* times, MotionState* ms, uint32_t first,
+                         double* partials, uint32_t stride, uint32_t grid_x, uint32_t n_scans, cudaStream_t st);
 // so_map.cu
 int map_alloc(Ctx* c);
 void map_free(Ctx* c);

@@ -1,0 +1,767 @@
+// so_motion.cu -- within-scan motion estimated by the registration itself: the reference's UndistortionMode::OPTIMIZED (LidarSlam.h:77-81,
+// "both begin and end scan are optimized using registration of undistorted scan and map; scan is linearly undistorted between begin
+// and end poses"; its branch of ComputePointInitAndFinalPose, LidarSlam.cpp:390-392, is empty upstream), sm_90a.
+//
+// Two pose7 parameter blocks per scan: T, the pose at tau = 0, and D, the motion over dt (the pose at tau = dt is T * D).  With
+// alpha_i = double(tau_i) / dt (0 for a non-finite tau_i):
+//   u_i(D) = qrot(slerp(identity, q_D, alpha_i), p_i) + alpha_i * t_D          (und_point's formula with D from the state)
+//   r_i    = n_i . (R(q) u_i(D) + t) + d_i                                      under ScaledLoss(TukeyLoss), as so_register
+// plus six rows of SE3AbsolutatePoseFactor on D (measurement D0, multiplier sqrt(n_ok * info_k)).  Each ICP iteration rounds u(D) to
+// float and runs the unchanged search and fit at T on it (k_motion_warp -> d_scan_sorted); the solve evaluates u in double at the
+// candidate D.  Both blocks use PoseLocalParameterization; the D rotation columns are the exact derivative
+//   dr/d(dtheta_D) = alpha (p x b)^T J_r(alpha phi) J_r(phi)^-1,  b = R(q_alpha)^T R(q)^T n,  phi = Log(q_D) on the shortest path.
+//   k_motion_warp        float(u(D)) of every active point into the ordered scan (w kept), like k_undistort
+//   k_motion_eval<PH>    residual and 12-column row per correspondence, 91 per-CTA sums (78 + 12 + 1) through shared memory
+//   k_motion_step<PH>    fixed-order cross-CTA sum, then the 12-parameter trust-region step; the 12x12 covariance at the end
+//   k_motion_cloud       u(D_opt) of a contiguous cloud: the map insert after a single-scan registration
+#include <chrono>
+#include <cmath>
+#include <vector>
+
+#include "so_undistort.cuh"
+
+namespace so {
+
+struct MotionState {
+    double D0[7];              // motion prior (quaternion normalised)
+    double info[6];            // its information diagonal per accepted correspondence
+    double dt;                 // seconds the motion spans, > 0
+    double D[7], Dc[7];        // accepted / candidate motion
+    double H[78], g[12];       // at (x, D): upper triangle of the 12x12, gradient; prior rows included
+    double cost;               // so_evaluate_optimized: the plane rows' cost
+    double scale[12], diag[12], sqrt_info[6];
+    int32_t stage;             // so_evaluate_optimized: the first evaluation reports H, g, cost and ends the registration
+    int32_t pad;
+};
+static_assert(sizeof(MotionState) % 8 == 0, "copied as 8-byte words");
+
+__host__ __device__ inline int tri12(int i, int j) { return i * 12 - (i * (i - 1)) / 2 + (j - i); }
+
+// sh = {q_D[4] normalised, t_D[3], theta, 1 / sin(theta)} of a motion D, rounded as und_setup rounds
+__device__ __forceinline__ void motion_setup(const double D[7], double sh[9]) {
+    const double n2 = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(D[3], D[3]), __dmul_rn(D[4], D[4])), __dmul_rn(D[5], D[5])), __dmul_rn(D[6], D[6]));
+    const double s = 1.0 / sqrt(n2);
+    for (int k = 0; k < 4; ++k) sh[k] = __dmul_rn(D[3 + k], s);
+    for (int k = 0; k < 3; ++k) sh[4 + k] = D[k];
+    und_angle(sh);
+}
+
+// ------------------------------------------------------------------------------------------------------------------ warp
+__global__ void __launch_bounds__(kThreads) k_motion_warp(BatchView bv, float4* __restrict__ sorted, const float4* __restrict__ raw,
+                                                          const float* __restrict__ times, const MotionState* __restrict__ ms) {
+    const int s = blockIdx.y;
+    const IcpState* st = bv.st + s;
+    if (st->phase != PH_CORR) return;
+    const uint32_t n = uint32_t(st->n_points);
+    if (blockIdx.x * kThreads >= n) return;
+    __shared__ double sh[9];
+    if (threadIdx.x == 0) motion_setup(ms[s].D, sh);
+    __syncthreads();
+    UndistortParams P{};
+    P.dt = ms[s].dt; P.on = 1; P.rotation = 1;
+    const uint32_t i = blockIdx.x * kThreads + threadIdx.x;
+    if (i >= n) return;
+    const size_t base = size_t(bv.offset[s]), gi = base + i;
+    const float w = sorted[gi].w;
+    const size_t src = base + __float_as_uint(w);                        // original index (scan ordering)
+    float4 o = und_point(P, sh, __ldg(&raw[src]), __ldg(&times[src]));
+    o.w = w;
+    sorted[gi] = o;
+}
+
+struct MotionD { double v[7]; };
+__global__ void __launch_bounds__(256) k_motion_cloud(float4* __restrict__ pts, const float* __restrict__ times, uint32_t n, MotionD D, double dt) {
+    __shared__ double sh[9];
+    if (threadIdx.x == 0) motion_setup(D.v, sh);
+    __syncthreads();
+    UndistortParams P{};
+    P.dt = dt; P.on = 1; P.rotation = 1;
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    pts[i] = und_point(P, sh, pts[i], times[i]);
+}
+
+// ------------------------------------------------------------------------------------------------------------------ evaluation
+// Coefficients of J_r(v) = I - c1 [v]x + c2 [v]x^2 and J_r(v)^-1 = I + [v]x / 2 + c3 [v]x^2 at |v| = th.  Below th = 1e-2 their
+// Taylor series to th^4 (truncation < 3e-17, where the closed forms lose ~eps / th^2 to cancellation).
+__host__ __device__ inline void jr_coeffs(double th, double* c1, double* c2) {
+    if (th < 1e-2) {
+        const double t2 = th * th;
+        *c1 = 0.5 - t2 / 24.0 + t2 * t2 / 720.0;
+        *c2 = 1.0 / 6.0 - t2 / 120.0 + t2 * t2 / 5040.0;
+    } else {
+        *c1 = (1.0 - cos(th)) / (th * th);
+        *c2 = (th - sin(th)) / (th * th * th);
+    }
+}
+__host__ __device__ inline double jrinv_coeff(double th) {
+    if (th < 1e-2) { const double t2 = th * th; return 1.0 / 12.0 + t2 / 720.0 + t2 * t2 / 30240.0; }
+    return 1.0 / (th * th) - 1.0 / (2.0 * th * tan(0.5 * th));                // 1/th^2 - (1 + cos th) / (2 th sin th)
+}
+__device__ __forceinline__ void cross3(const double a[3], const double b[3], double o[3]) {
+    o[0] = a[1] * b[2] - a[2] * b[1]; o[1] = a[2] * b[0] - a[0] * b[2]; o[2] = a[0] * b[1] - a[1] * b[0];
+}
+
+// per CTA: pose T, R(q), the motion's slerp setup, phi = Log(q_D) (shortest path), its angle, and c3(|phi|)
+struct MotionCta { double T[7], R[9], sh[9], phi[3], th, c3, dt; };
+
+__device__ __forceinline__ void motion_cta_setup(const double T[7], const double D[7], double dt, MotionCta& m) {
+    for (int k = 0; k < 7; ++k) m.T[k] = T[k];
+    qtoR(T + 3, m.R);
+    double q[4];
+    const double n = sqrt(D[3] * D[3] + D[4] * D[4] + D[5] * D[5] + D[6] * D[6]);
+    for (int k = 0; k < 4; ++k) q[k] = D[3 + k] / n;
+    for (int k = 0; k < 4; ++k) m.sh[k] = q[k];
+    for (int k = 0; k < 3; ++k) m.sh[4 + k] = D[k];
+    und_angle(m.sh);
+    const double sg = q[3] < 0.0 ? -1.0 : 1.0;
+    const double vn = sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2]);
+    m.th = 2.0 * atan2(vn, sg * q[3]);
+    const double f = vn > 0.0 ? sg * m.th / vn : 0.0;
+    for (int k = 0; k < 3; ++k) m.phi[k] = f * q[k];
+    m.c3 = jrinv_coeff(m.th);
+    m.dt = dt;
+}
+
+// One correspondence: the row sqrt(rho') [J (12), r] and rho / 2 (ScaledLoss(TukeyLoss) through Ceres' corrector, as accumulate())
+__device__ __forceinline__ void motion_row(const MotionCta& m, const double nd[4], double wc, float4 p, float tau, double a2, double row[14]) {
+    const double al = isfinite(tau) ? double(tau) / m.dt : 0.0;
+    const double pv[3] = {double(p.x), double(p.y), double(p.z)};
+    double s0, s1;                                                       // Eigen's slerp(identity, q_D, alpha)
+    if (m.sh[7] < 0.0) { s0 = 1.0 - al; s1 = al; }
+    else { s0 = sin((1.0 - al) * m.sh[7]) * m.sh[8]; s1 = sin(al * m.sh[7]) * m.sh[8]; }
+    if (m.sh[3] < 0.0) s1 = -s1;
+    const double qa[4] = {s1 * m.sh[0], s1 * m.sh[1], s1 * m.sh[2], s0 + s1 * m.sh[3]};
+    double u[3];
+    qrot(qa, pv, u);
+    for (int k = 0; k < 3; ++k) u[k] += al * m.sh[4 + k];
+    double pw[3];
+    qrot(m.T + 3, u, pw);
+    for (int k = 0; k < 3; ++k) pw[k] += m.T[k];
+    const double r = nd[0] * pw[0] + nd[1] * pw[1] + nd[2] * pw[2] + nd[3];
+    const double sr = r * r;
+    double rho0, rho1;
+    if (sr <= a2) { const double v = 1.0 - sr / a2, v2 = v * v; rho0 = a2 / 6.0 * (1.0 - v2 * v); rho1 = 0.5 * v2; }
+    else { rho0 = a2 / 6.0; rho1 = 0.0; }
+    rho0 *= wc; rho1 *= wc;
+    const double* R = m.R;
+    const double av[3] = {R[0] * nd[0] + R[3] * nd[1] + R[6] * nd[2], R[1] * nd[0] + R[4] * nd[1] + R[7] * nd[2],
+                          R[2] * nd[0] + R[5] * nd[1] + R[8] * nd[2]};            // R^T n
+    double J[12];
+    J[0] = nd[0]; J[1] = nd[1]; J[2] = nd[2];
+    cross3(u, av, J + 3);                                                // -n^T R [u]x
+    for (int k = 0; k < 3; ++k) J[6 + k] = al * av[k];                   // alpha n^T R
+    const double qc[4] = {-qa[0], -qa[1], -qa[2], qa[3]};
+    double b[3], w[3], t1[3], t2[3];
+    qrot(qc, av, b);                                                     // R(q_alpha)^T R^T n
+    cross3(pv, b, w);                                                    // p x b
+    // J_r(alpha phi)^T w = w + c1 (v x w) + c2 v x (v x w), v = alpha phi
+    const double v[3] = {al * m.phi[0], al * m.phi[1], al * m.phi[2]};
+    double c1, c2;
+    jr_coeffs(fabs(al) * m.th, &c1, &c2);
+    cross3(v, w, t1); cross3(v, t1, t2);
+    for (int k = 0; k < 3; ++k) w[k] = w[k] + c1 * t1[k] + c2 * t2[k];
+    // J_r(phi)^-T w = w - (phi x w) / 2 + c3 phi x (phi x w)
+    cross3(m.phi, w, t1); cross3(m.phi, t1, t2);
+    for (int k = 0; k < 3; ++k) J[9 + k] = al * (w[k] - 0.5 * t1[k] + m.c3 * t2[k]);
+    const double sc = sqrt(rho1);
+#pragma unroll
+    for (int k = 0; k < 12; ++k) row[k] = sc * J[k];
+    row[12] = sc * r;
+    row[13] = 0.5 * rho0;
+}
+
+constexpr int kRowStride = 14;
+// Tiles of kThreads points (the per-CTA layout of k_evaluate: eval_pts(n) tiles per CTA, eval_ctas(n) CTAs per scan): every thread
+// stages its row in shared memory, then thread e < 91 adds component e of the tile's 256 rows in index order.  One register
+// accumulator per thread instead of 91.
+template <int PHASE>
+__global__ void __launch_bounds__(kThreads) k_motion_eval(BatchView bv, CorrBuf cb, const float4* __restrict__ raw, const float* __restrict__ times,
+                                                          const MotionState* __restrict__ ms, double* __restrict__ partials, uint32_t stride) {
+    const int s = blockIdx.y;
+    const IcpState* st = bv.st + s;
+    if (st->phase != PHASE) return;
+    const uint32_t n = uint32_t(st->n_points);
+    const int pts = eval_pts(n);
+    if (blockIdx.x >= eval_ctas(n)) return;
+    __shared__ MotionCta m;
+    __shared__ double rows[kThreads * kRowStride];
+    if (threadIdx.x == 0) motion_cta_setup(PHASE == PH_EVAL ? st->cand : st->x, PHASE == PH_EVAL ? ms[s].Dc : ms[s].D, ms[s].dt, m);
+    const int e = threadIdx.x;
+    int ei = 0, ej = 0;                                                  // component e: H(ei, ej) for e < 78, g(e - 78), cost
+    if (e < 78) { int k = e; while (k >= 12 - ei) { k -= 12 - ei; ++ei; } ej = ei + k; }
+    else if (e < 90) { ei = e - 78; ej = 12; }
+    else { ei = 13; ej = -1; }
+    double acc = 0.0;
+    const size_t base = size_t(bv.offset[s]);
+    __syncthreads();
+#pragma unroll 1
+    for (int r = 0; r < pts; ++r) {
+        const uint32_t i = (blockIdx.x * uint32_t(pts) + uint32_t(r)) * kThreads + threadIdx.x;
+        double row[14];
+#pragma unroll
+        for (int k = 0; k < 14; ++k) row[k] = 0.0;
+        if (i < n) {
+            const double wc = cb.w[base + i];
+            if (wc != 0.0) {
+                const double4 nd4 = cb.nd[base + i];
+                const double nd[4] = {nd4.x, nd4.y, nd4.z, nd4.w};
+                const size_t src = base + __float_as_uint(bv.scan[base + i].w);
+                motion_row(m, nd, wc, __ldg(&raw[src]), __ldg(&times[src]), bv.tukey_a2, row);
+            }
+        }
+#pragma unroll
+        for (int k = 0; k < 14; ++k) rows[threadIdx.x * kRowStride + k] = row[k];
+        __syncthreads();
+        if (e < kMotionAcc) {
+            if (ej >= 0) { for (int t = 0; t < kThreads; ++t) acc += rows[t * kRowStride + ei] * rows[t * kRowStride + ej]; }
+            else { for (int t = 0; t < kThreads; ++t) acc += rows[t * kRowStride + ei]; }
+        }
+        __syncthreads();
+    }
+    if (e < kMotionAcc) partials[(size_t(s) * stride + blockIdx.x) * kMotionAcc + e] = acc;
+}
+
+// ------------------------------------------------------------------------------------------------------------------ step
+// The trust-region loop of so_icp.cu (lm_begin_solve / lm_continue / lm_after_eval / end_solve) over the 12 tangent columns of
+// (T, D): Jacobi scaling and the LM diagonal over 12 columns, x_norm and the step norm over the 14 ambient values, the gradient
+// max-norm through Plus of both blocks.  Runs on one thread, on shared-memory copies of the two states.
+__device__ __noinline__ void m_end_solve(IcpState& st) {
+    const int it = st.icp_iter;
+    st.iter_n_surf[it] = st.n_ok - st.n_ok_edge;
+    st.iter_n_edge[it] = st.n_ok_edge;
+    rel_motion(st.x_iter_start, st.x, &st.iter_dtrans[it], &st.iter_drot[it]);
+    st.iter_lm_steps[it] = st.lm_iter;
+    st.iter_lm_successful[it] = st.num_successful;
+    st.iter_lm_termination[it] = st.termination;
+    st.iter_cost[it] = st.cost;
+    st.n_iterations = it + 1;
+    if (st.n_ok == 0) { st.status = SO_STATUS_NO_CORRESPONDENCES; st.phase = PH_DONE; return; }     // the prior rows are zero then
+    if (st.num_successful == 1 || it == st.max_icp_iters - 1) { st.need_cov = 1; st.phase = PH_DONE; }
+    else { st.icp_iter = it + 1; st.phase = PH_CORR; }
+}
+
+__device__ __noinline__ double m_gmax(const IcpState& S, const MotionState& M) {
+    double nt[6], nd[6], xp[7], dp[7];
+    for (int j = 0; j < 6; ++j) { nt[j] = -M.g[j]; nd[j] = -M.g[6 + j]; }
+    pose_plus(S.x, nt, xp);
+    pose_plus(M.D, nd, dp);
+    double m = 0.0;
+    for (int i = 0; i < 7; ++i) m = fmax(m, fmax(fabs(S.x[i] - xp[i]), fabs(M.D[i] - dp[i])));
+    return m;
+}
+
+// SE3AbsolutatePoseFactor on D (add_pose_prior's rows, columns 6..11)
+__device__ __noinline__ void m_add_prior(const MotionState& M, const double D[7], double a[kMotionAcc]) {
+    const double qm[4] = {-M.D0[3], -M.D0[4], -M.D0[5], M.D0[6]};
+    double e[4];
+    qmul(qm, D + 3, e);
+    double r[6] = {D[0] - M.D0[0], D[1] - M.D0[1], D[2] - M.D0[2], 2.0 * e[0], 2.0 * e[1], 2.0 * e[2]};
+    double J[36];
+    for (int i = 0; i < 36; ++i) J[i] = 0.0;
+    J[0] = J[7] = J[14] = 1.0;
+    J[3 * 6 + 3] = e[3];  J[3 * 6 + 4] = -e[2]; J[3 * 6 + 5] = e[1];
+    J[4 * 6 + 3] = e[2];  J[4 * 6 + 4] = e[3];  J[4 * 6 + 5] = -e[0];
+    J[5 * 6 + 3] = -e[1]; J[5 * 6 + 4] = e[0];  J[5 * 6 + 5] = e[3];
+    for (int i = 0; i < 6; ++i) { r[i] *= M.sqrt_info[i]; for (int j = 0; j < 6; ++j) J[i * 6 + j] *= M.sqrt_info[i]; }
+    for (int i = 0; i < 6; ++i) {
+        for (int j = i; j < 6; ++j) { double t = 0.0; for (int k = 0; k < 6; ++k) t += J[k * 6 + i] * J[k * 6 + j]; a[tri12(6 + i, 6 + j)] += t; }
+        double t = 0.0; for (int k = 0; k < 6; ++k) t += J[k * 6 + i] * r[k];
+        a[78 + 6 + i] += t;
+    }
+    double sq = 0.0; for (int k = 0; k < 6; ++k) sq += r[k] * r[k];
+    a[90] += 0.5 * sq;
+}
+
+// Cholesky solve of the SPD 12x12 M y = r (M full row-major, destroyed); false on a non-positive pivot
+__device__ __noinline__ bool chol12_solve(double* M, const double* r, double* y) {
+    double inv[12], z[12];
+#pragma unroll 1
+    for (int j = 0; j < 12; ++j) {
+        double s = M[j * 12 + j];
+        for (int k = 0; k < j; ++k) s -= M[j * 12 + k] * M[j * 12 + k];
+        if (!(s > 0.0)) return false;
+        const double il = rsqrt(s);
+        inv[j] = il;
+        M[j * 12 + j] = s * il;
+#pragma unroll 1
+        for (int i = j + 1; i < 12; ++i) {
+            double t = M[i * 12 + j];
+            for (int k = 0; k < j; ++k) t -= M[i * 12 + k] * M[j * 12 + k];
+            M[i * 12 + j] = t * il;
+        }
+    }
+#pragma unroll 1
+    for (int i = 0; i < 12; ++i) { double t = r[i]; for (int k = 0; k < i; ++k) t -= M[i * 12 + k] * z[k]; z[i] = t * inv[i]; }
+#pragma unroll 1
+    for (int i = 11; i >= 0; --i) { double t = z[i]; for (int k = i + 1; k < 12; ++k) t -= M[k * 12 + i] * y[k]; y[i] = t * inv[i]; }
+    return true;
+}
+
+__device__ __noinline__ void m_lm_continue(IcpState& st, MotionState& M, bool step_successful) {
+    for (;;) {
+        if (step_successful) st.num_successful++; else st.num_unsuccessful++;
+        if (st.lm_iter >= st.lm_max_iterations) { st.termination = 0; m_end_solve(st); return; }
+        if (st.gmax <= 1e-10) { st.termination = 1; m_end_solve(st); return; }
+        if (st.radius <= 1e-32) { st.termination = 4; m_end_solve(st); return; }
+        st.lm_iter++;
+        step_successful = false;
+        double Hs[144], gs[12], A[144], y[12];
+        for (int i = 0; i < 12; ++i) {
+            gs[i] = M.g[i] * M.scale[i];
+            for (int j = 0; j < 12; ++j) Hs[i * 12 + j] = M.H[i <= j ? tri12(i, j) : tri12(j, i)] * M.scale[i] * M.scale[j];
+        }
+        if (!st.reuse_diagonal) for (int j = 0; j < 12; ++j) M.diag[j] = fmin(fmax(Hs[j * 12 + j], 1e-6), 1e32);
+        st.reuse_diagonal = 1;
+        for (int i = 0; i < 144; ++i) A[i] = Hs[i];
+        for (int j = 0; j < 12; ++j) A[j * 12 + j] += M.diag[j] / st.radius;
+        bool valid = chol12_solve(A, gs, y);
+        double step[12], mcc = 0.0;
+        if (valid) {
+            double sg = 0.0, sHs = 0.0;
+            for (int j = 0; j < 12; ++j) { step[j] = -y[j]; valid = valid && isfinite(step[j]); }
+            for (int i = 0; i < 12; ++i) { sg += step[i] * gs[i]; double t = 0.0; for (int j = 0; j < 12; ++j) t += Hs[i * 12 + j] * step[j]; sHs += step[i] * t; }
+            mcc = -sg - 0.5 * sHs;
+        }
+        if (!valid || !(mcc > 0.0)) {
+            if (++st.consecutive_invalid >= 5) { st.termination = 5; m_end_solve(st); return; }
+            st.radius *= 0.5; st.reuse_diagonal = 1;
+            continue;
+        }
+        st.consecutive_invalid = 0;
+        st.model_cost_change = mcc;
+        double dT[6], dD[6];
+        for (int j = 0; j < 6; ++j) { dT[j] = step[j] * M.scale[j]; dD[j] = step[6 + j] * M.scale[6 + j]; }
+        pose_plus(st.x, dT, st.cand);
+        pose_plus(M.D, dD, M.Dc);
+        st.phase = PH_EVAL;
+        return;
+    }
+}
+
+__device__ __noinline__ void m_begin_solve(IcpState& st, MotionState& M, const double* acc_in, int n_ok) {
+    double acc[kMotionAcc];
+    for (int k = 0; k < kMotionAcc; ++k) acc[k] = acc_in[k];
+    for (int k = 0; k < 6; ++k) M.sqrt_info[k] = sqrt(double(n_ok) * M.info[k]);
+    m_add_prior(M, M.D, acc);
+    for (int k = 0; k < 78; ++k) M.H[k] = acc[k];
+    for (int k = 0; k < 12; ++k) M.g[k] = acc[78 + k];
+    st.cost = acc[90];
+    st.n_ok = n_ok;
+    for (int i = 0; i < 7; ++i) st.x_iter_start[i] = st.x[i];
+    st.lm_iter = 0; st.num_successful = 0; st.num_unsuccessful = 0; st.consecutive_invalid = 0; st.termination = 0;
+    if (n_ok == 0) { st.termination = 6; m_end_solve(st); return; }
+    for (int j = 0; j < 12; ++j) M.scale[j] = 1.0 / (1.0 + sqrt(M.H[tri12(j, j)]));
+    double xn = 0.0;
+    for (int i = 0; i < 7; ++i) xn += st.x[i] * st.x[i] + M.D[i] * M.D[i];
+    st.x_norm = sqrt(xn);
+    st.gmax = m_gmax(st, M);
+    st.radius = 1e4; st.decrease_factor = 2.0; st.reuse_diagonal = 0;
+    m_lm_continue(st, M, false);
+}
+
+__device__ __noinline__ void m_after_eval(IcpState& st, MotionState& M, const double* acc_in) {
+    double acc[kMotionAcc];
+    for (int k = 0; k < kMotionAcc; ++k) acc[k] = acc_in[k];
+    m_add_prior(M, M.Dc, acc);
+    const double cand_cost = acc[90];
+    double sn = 0.0;
+    for (int i = 0; i < 7; ++i) { const double a = st.x[i] - st.cand[i], b = M.D[i] - M.Dc[i]; sn += a * a + b * b; }
+    sn = sqrt(sn);
+    if (sn <= 1e-8 * (st.x_norm + 1e-8)) { st.termination = 2; m_end_solve(st); return; }
+    const double cost_change = st.cost - cand_cost;
+    if (fabs(cost_change) <= 1e-6 * st.cost) { st.termination = 3; m_end_solve(st); return; }
+    const double rd = cost_change / st.model_cost_change;
+    if (rd > 1e-3) {
+        double xn = 0.0;
+        for (int i = 0; i < 7; ++i) { st.x[i] = st.cand[i]; M.D[i] = M.Dc[i]; xn += st.x[i] * st.x[i] + M.D[i] * M.D[i]; }
+        st.x_norm = sqrt(xn);
+        for (int k = 0; k < 78; ++k) M.H[k] = acc[k];
+        for (int k = 0; k < 12; ++k) M.g[k] = acc[78 + k];
+        st.cost = cand_cost;
+        st.gmax = m_gmax(st, M);
+        const double t = 2.0 * rd - 1.0;
+        st.radius = fmin(1e16, st.radius / fmax(1.0 / 3.0, 1.0 - t * t * t));
+        st.decrease_factor = 2.0; st.reuse_diagonal = 0;
+        m_lm_continue(st, M, true);
+    } else {
+        st.radius = st.radius / st.decrease_factor; st.decrease_factor *= 2.0; st.reuse_diagonal = 1;
+        m_lm_continue(st, M, false);
+    }
+}
+
+// ceres::Covariance{apply_loss_function, DENSE_SVD} over the 12 tangent columns on the CTA's first warp: cyclic Jacobi of H (each
+// rotation's angle on lane 0, the rows of H on lanes 0-11, of the eigenvectors on lanes 12-23, the 2x2 block on lane 24), the
+// pseudo-inverse dropping directions with s_i / s_max < sqrt(1e-14), and T's 6x6 block with EstimateRegistrationError's 3x3
+// analyses into the scan's state, as covariance_and_errors_warp does for the 6-column solve.
+struct Cov12 { double a[144], v[144], w[12], inv[12], t, c, s; int perm[12]; };
+
+__device__ __noinline__ void cov12_warp(IcpState& S, const MotionState& M, Cov12& sc) {
+    const unsigned full = 0xffffffffu;
+    const int lane = threadIdx.x & 31;
+    for (int e = lane; e < 144; e += 32) {
+        const int i = e / 12, j = e % 12;
+        sc.a[e] = M.H[i <= j ? tri12(i, j) : tri12(j, i)];
+        sc.v[e] = i == j ? 1.0 : 0.0;
+    }
+    __syncwarp();
+#pragma unroll 1
+    for (int sweep = 0; sweep < 30; ++sweep) {
+        int stop = 0;
+        if (lane == 0) {
+            double off = 0.0, dia = 0.0;
+            for (int p = 0; p < 12; ++p) { dia += sc.a[p * 12 + p] * sc.a[p * 12 + p]; for (int q = p + 1; q < 12; ++q) off += sc.a[p * 12 + q] * sc.a[p * 12 + q]; }
+            stop = (off <= kJacobiOffTol * dia || off == 0.0) ? 1 : 0;
+        }
+        if (__shfl_sync(full, stop, 0)) break;
+#pragma unroll 1
+        for (int p = 0; p < 11; ++p) {
+#pragma unroll 1
+            for (int q = p + 1; q < 12; ++q) {
+                if (lane == 0) {
+                    const double apq = sc.a[p * 12 + q];
+                    double t = 0.0;
+                    if (apq != 0.0) {
+                        const double dlt = sc.a[q * 12 + q] - sc.a[p * 12 + p], b2 = 2.0 * apq;
+                        t = b2 / (fabs(dlt) + sqrt(dlt * dlt + b2 * b2));
+                        if (dlt < 0.0) t = -t;
+                    }
+                    const double c = 1.0 / sqrt(t * t + 1.0);
+                    sc.t = t; sc.c = c; sc.s = t * c;
+                }
+                __syncwarp();
+                const double t = sc.t, c = sc.c, sn = sc.s;
+                if (t != 0.0) {
+                    const int r = lane < 12 ? lane : lane - 12;
+                    const bool do_a = lane < 12 && r != p && r != q, do_v = lane >= 12 && lane < 24, do_d = lane == 24;
+                    double n0 = 0.0, n1 = 0.0;
+                    if (do_a) { const double arp = sc.a[r * 12 + p], arq = sc.a[r * 12 + q]; n0 = c * arp - sn * arq; n1 = sn * arp + c * arq; }
+                    if (do_v) { const double vrp = sc.v[r * 12 + p], vrq = sc.v[r * 12 + q]; n0 = c * vrp - sn * vrq; n1 = sn * vrp + c * vrq; }
+                    if (do_d) { const double apq = sc.a[p * 12 + q]; n0 = sc.a[p * 12 + p] - t * apq; n1 = sc.a[q * 12 + q] + t * apq; }
+                    __syncwarp();
+                    if (do_a) { sc.a[r * 12 + p] = sc.a[p * 12 + r] = n0; sc.a[r * 12 + q] = sc.a[q * 12 + r] = n1; }
+                    if (do_v) { sc.v[r * 12 + p] = n0; sc.v[r * 12 + q] = n1; }
+                    if (do_d) { sc.a[p * 12 + p] = n0; sc.a[q * 12 + q] = n1; sc.a[p * 12 + q] = 0.0; sc.a[q * 12 + p] = 0.0; }
+                }
+                __syncwarp();
+            }
+        }
+    }
+    if (lane == 0) {
+        double w[12];
+        int pm[12];
+        for (int i = 0; i < 12; ++i) { w[i] = sc.a[i * 12 + i]; pm[i] = i; }
+        for (int i = 0; i < 11; ++i)
+            for (int j = i + 1; j < 12; ++j)
+                if (w[j] < w[i]) { const double tw = w[i]; w[i] = w[j]; w[j] = tw; const int tp = pm[i]; pm[i] = pm[j]; pm[j] = tp; }
+        const double lmax = w[11];
+        bool cut = false;
+        for (int i = 11; i >= 0; --i) {                                   // a cut direction cuts every smaller one
+            const double ratio = (w[i] > 0.0 && lmax > 0.0) ? sqrt(w[i] / lmax) : 0.0;
+            cut = cut || ratio < 1e-7;
+            sc.inv[i] = cut ? 0.0 : 1.0 / w[i];
+            sc.w[i] = w[i]; sc.perm[i] = pm[i];
+        }
+    }
+    __syncwarp();
+    for (int e = lane; e < 36; e += 32) {
+        const int i = e / 6, j = e % 6;
+        double t = 0.0;
+        for (int k = 0; k < 12; ++k) t += sc.v[i * 12 + sc.perm[k]] * sc.inv[k] * sc.v[j * 12 + sc.perm[k]];
+        S.cov[e] = t;
+    }
+    __syncwarp();
+    if (lane < 2) {
+        double Mx[9], E[9], ev[3];
+        const int o = lane * 3;
+        for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) Mx[i * 3 + j] = S.cov[(i + o) * 6 + (j + o)];
+        jacobi_eig<3, 20>(Mx, E, ev);
+        const double err = sqrt(ev[2]), inv_cond = sqrt(ev[0]) / sqrt(ev[2]);
+        if (lane == 0) { S.pos_err = err; S.pos_dir[0] = E[2]; S.pos_dir[1] = E[5]; S.pos_dir[2] = E[8]; S.pos_inv_cond = inv_cond; }
+        else { S.ori_err_deg = err / M_PI * 180.0; S.ori_dir[0] = E[2]; S.ori_dir[1] = E[5]; S.ori_dir[2] = E[8]; S.ori_inv_cond = inv_cond; }
+    }
+    __syncwarp();
+}
+
+template <int AFTER>
+__global__ void __launch_bounds__(128) k_motion_step(BatchView bv, MotionState* __restrict__ ms, const double* __restrict__ partials, uint32_t stride) {
+    const int s = blockIdx.x;
+    IcpState* st = bv.st + s;
+    if (st->phase != AFTER) return;
+    __shared__ IcpState s_st;
+    __shared__ MotionState s_m;
+    __shared__ double s_sum[kMotionAcc];
+    {
+        const unsigned long long* a = reinterpret_cast<const unsigned long long*>(st);
+        unsigned long long* b = reinterpret_cast<unsigned long long*>(&s_st);
+        for (uint32_t k = threadIdx.x; k < sizeof(IcpState) / 8; k += blockDim.x) b[k] = a[k];
+        const unsigned long long* c = reinterpret_cast<const unsigned long long*>(ms + s);
+        unsigned long long* d = reinterpret_cast<unsigned long long*>(&s_m);
+        for (uint32_t k = threadIdx.x; k < sizeof(MotionState) / 8; k += blockDim.x) d[k] = c[k];
+    }
+    if (threadIdx.x < kMotionAcc) {                                      // the scan's CTAs in index order
+        const uint32_t np = eval_ctas(uint32_t(st->n_points));
+        const double* base = partials + size_t(s) * stride * kMotionAcc + threadIdx.x;
+        double v = 0.0;
+        for (uint32_t b = 0; b < np; ++b) v += base[size_t(b) * kMotionAcc];
+        s_sum[threadIdx.x] = v;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        IcpState& S = s_st;
+        MotionState& M = s_m;
+        if (AFTER == PH_CORR) {
+            for (int k = 0; k < 9; ++k) S.hist_obs[k] = bv.hist[s * kHistStride + k];
+            for (int k = 0; k < 7; ++k) S.hist_rej[k] = bv.hist[s * kHistStride + 9 + k];
+            for (int k = 0; k < 7; ++k) S.hist_rej_line[k] = bv.hist[s * kHistStride + 16 + k];
+            S.n_ok_edge = 0;
+            const int n_ok = S.hist_rej[0];
+            for (int k = 0; k < kHistStride; ++k) bv.hist[s * kHistStride + k] = 0;
+            if (M.stage) {                                               // so_evaluate_optimized: report the plane rows and stop
+                for (int k = 0; k < 78; ++k) M.H[k] = s_sum[k];
+                for (int k = 0; k < 12; ++k) M.g[k] = s_sum[78 + k];
+                M.cost = s_sum[90]; S.n_ok = n_ok; S.n_iterations = 1; S.phase = PH_DONE;
+            } else m_begin_solve(S, M, s_sum, n_ok);
+        } else m_after_eval(S, M, s_sum);
+    }
+    __syncthreads();
+    if (s_st.need_cov) {
+        __shared__ Cov12 s_cov;
+        if (threadIdx.x < 32) cov12_warp(s_st, s_m, s_cov);
+        __syncthreads();
+    }
+    {
+        const unsigned long long* a = reinterpret_cast<const unsigned long long*>(&s_st);
+        unsigned long long* b = reinterpret_cast<unsigned long long*>(st);
+        for (uint32_t k = threadIdx.x; k < sizeof(IcpState) / 8; k += blockDim.x) b[k] = a[k];
+        const unsigned long long* c = reinterpret_cast<const unsigned long long*>(&s_m);
+        unsigned long long* d = reinterpret_cast<unsigned long long*>(ms + s);
+        for (uint32_t k = threadIdx.x; k < sizeof(MotionState) / 8; k += blockDim.x) d[k] = c[k];
+    }
+}
+
+void launch_motion_warp(const BatchView& bv, float4* sorted, const float4* raw, const float* times, const MotionState* ms, uint32_t first,
+                        uint32_t grid_x, uint32_t n_scans, cudaStream_t st) {
+    k_motion_warp<<<dim3(grid_x, n_scans), kThreads, 0, st>>>(bv, sorted, raw, times, ms + first);
+}
+
+void launch_motion_solve(int phase, const BatchView& bv, const CorrBuf& cb, const float4* raw, const float* times, MotionState* ms, uint32_t first,
+                         double* partials, uint32_t stride, uint32_t grid_x, uint32_t n_scans, cudaStream_t st) {
+    ms += first;
+    const uint32_t gx = eval_grid(grid_x * kThreads);
+    if (phase == PH_CORR) {
+        k_motion_eval<PH_CORR><<<dim3(gx, n_scans), kThreads, 0, st>>>(bv, cb, raw, times, ms, partials, stride);
+        k_motion_step<PH_CORR><<<n_scans, 128, 0, st>>>(bv, ms, partials, stride);
+    } else {
+        k_motion_eval<PH_EVAL><<<dim3(gx, n_scans), kThreads, 0, st>>>(bv, cb, raw, times, ms, partials, stride);
+        k_motion_step<PH_EVAL><<<n_scans, 128, 0, st>>>(bv, ms, partials, stride);
+    }
+}
+
+int motion_tail(Ctx* c, MapStore& ms, uint32_t n_new) {
+    if (!n_new) return SO_OK;
+    MotionD D;
+    for (int k = 0; k < 7; ++k) D.v[k] = c->mot.last_D[k];
+    timed_launch_begin(c);
+    k_motion_cloud<<<(n_new + 255) / 256, 256, 0, c->stream>>>(ms.d_xyzi + ms.n, c->und.d_time, n_new, D, c->und.last.dt);
+    timed_launch_end(c, 7);
+    SO_CUDA_TRY(cudaGetLastError());
+    return SO_OK;
+}
+
+void motion_free(Ctx* c) { cudaFree(c->mot.d_st); cudaFree(c->mot.d_partials); }
+
+// ------------------------------------------------------------------------------------------------------------------ host side
+static int check_motion(const so_motion* m, const so_icp_opts* o) {
+    if (!m || !o) return fail(SO_ERR_ARG, "bad args");
+    if (!(std::isfinite(m->dt) && m->dt > 0.0)) return fail(SO_ERR_ARG, "so_motion.dt must be finite and > 0");
+    if (!finite_pose(m->motion_prior)) return fail(SO_ERR_ARG, "so_motion.motion_prior must be finite with a non-zero quaternion");
+    for (int k = 0; k < 6; ++k)
+        if (!(std::isfinite(m->motion_info[k]) && m->motion_info[k] >= 0.0)) return fail(SO_ERR_ARG, "so_motion.motion_info must be finite and >= 0");
+    if (o->use_pose_prior) return fail(SO_ERR_ARG, "use_pose_prior is not supported by so_register_optimized");
+    return icp_opts_check(*o);
+}
+
+static MotionState make_state(const so_motion& m) {
+    MotionState M;
+    std::memset(&M, 0, sizeof(M));
+    const double* p = m.motion_prior;
+    const double n = std::sqrt(p[3] * p[3] + p[4] * p[4] + p[5] * p[5] + p[6] * p[6]);
+    for (int k = 0; k < 3; ++k) M.D0[k] = p[k];
+    for (int k = 3; k < 7; ++k) M.D0[k] = p[k] / n;
+    for (int k = 0; k < 7; ++k) M.D[k] = M.Dc[k] = M.D0[k];
+    for (int k = 0; k < 6; ++k) M.info[k] = m.motion_info[k];
+    M.dt = m.dt;
+    return M;
+}
+
+static int reserve(Ctx* c, size_t n_points) {
+    c->mot.stride = eval_grid(c->grid_x_cap * kThreads);
+    int rc = grow_buffer(c->mot.d_st, c->mot.st_cap, size_t(c->max_batch));
+    if (!rc) rc = grow_buffer(c->mot.d_partials, c->mot.partials_cap, size_t(c->max_batch) * c->mot.stride * kMotionAcc);
+    if (!rc) rc = grow_buffer(c->und.d_time, c->und.time_cap, std::max<size_t>(n_points, 1));
+    return rc;
+}
+
+static int upload_states(Ctx* c, const MotionState* M, size_t n) {
+    SO_CUDA_TRY(cudaMemcpyAsync(c->mot.d_st, M, n * sizeof(MotionState), cudaMemcpyHostToDevice, c->stream));
+    count_h2d(c, n * sizeof(MotionState));
+    return SO_OK;
+}
+
+static int download_states(Ctx* c, MotionState* M, size_t n) {
+    SO_CUDA_TRY(cudaMemcpyAsync(M, c->mot.d_st, n * sizeof(MotionState), cudaMemcpyDeviceToHost, c->stream));
+    count_d2h(c, n * sizeof(MotionState));
+    SO_CUDA_TRY(cudaStreamSynchronize(c->stream));
+    return SO_OK;
+}
+
+// so_motion_result from the registration's result and the motion block: pose_end = T * D with T = pose_opt
+static void fill_motion(const so_icp_result& icp, const MotionState& M, so_motion_result* out) {
+    out->icp = icp;
+    for (int k = 0; k < 7; ++k) out->motion[k] = M.D[k];
+    const double* T = icp.pose_opt;
+    double t[3];
+    qrot(T + 3, M.D, t);
+    for (int k = 0; k < 3; ++k) out->pose_end[k] = T[k] + t[k];
+    qmul(T + 3, M.D + 3, out->pose_end + 3);
+}
+
+// The single-scan tail: the cloud (n points) is in d_scan, its times in und.d_time
+static int register_one(Ctx* c, uint32_t n, const double pose_in[7], const so_motion* m, const so_icp_opts* opts, so_motion_result* out,
+                        std::chrono::steady_clock::time_point t0) {
+    MotionState M = make_state(*m);
+    int rc = upload_states(c, &M, 1);
+    if (rc) return rc;
+    so_icp_result icp;
+    rc = register_core(c, c->d_scan, &n, 1, pose_in, opts, &icp, true, nullptr, nullptr, nullptr, 0, 2);
+    if (!rc) rc = download_states(c, &M, 1);
+    if (rc) return rc;
+    c->last_scan_n = n;
+    c->und.last = UndistortParams{};
+    c->und.last.on = 2; c->und.last.dt = m->dt;
+    for (int k = 0; k < 7; ++k) c->mot.last_D[k] = M.D[k];
+    icp.scan_edge_num = 0;
+    icp.time_total_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    fill_motion(icp, M, out);
+    return icp.status;
+}
+
+}  // namespace so
+
+using namespace so;
+
+extern "C" {
+
+int so_register_optimized(so_ctx* ctx, const void* surf, size_t n_surf, size_t stride, size_t ioff, size_t toff, const double pose_in[7],
+                          const so_motion* m, const so_icp_opts* opts, so_motion_result* out) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c || !pose_in || !opts || !out || (!surf && n_surf) || stride < 12 || toff + 4 > stride) return fail(SO_ERR_ARG, "bad args");
+    int rc = check_motion(m, opts);
+    if (rc) return rc;
+    if (n_surf > c->cfg.max_scan_points) return fail(SO_ERR_CAPACITY, "scan larger than so_config.max_scan_points");
+    SO_CUDA_TRY(cudaSetDevice(c->device));
+    const auto t0 = std::chrono::steady_clock::now();
+    rc = reserve(c, n_surf);
+    if (!rc) rc = upload_cloud(c, surf, n_surf, stride, ioff, c->d_scan);
+    if (!rc) rc = upload_times(c, surf, n_surf, stride, toff, c->und.d_time);
+    if (rc) return rc;
+    return register_one(c, uint32_t(n_surf), pose_in, m, opts, out, t0);
+}
+
+int so_register_prefiltered_optimized(so_ctx* ctx, const double pose_in[7], const so_motion* m, const so_icp_opts* opts, so_motion_result* out) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c || !pose_in || !opts || !out) return fail(SO_ERR_ARG, "bad args");
+    int rc = check_motion(m, opts);
+    if (rc) return rc;
+    if (c->prefiltered_n == SIZE_MAX) return fail(SO_ERR_ARG, "so_register_prefiltered_optimized needs a preceding so_scan_prefilter (and nothing that reuses the scan buffers in between)");
+    SO_CUDA_TRY(cudaSetDevice(c->device));
+    const auto t0 = std::chrono::steady_clock::now();
+    const size_t n = c->prefiltered_n;
+    rc = reserve(c, n);
+    if (rc) return rc;
+    c->prefiltered_n = SIZE_MAX;
+    if (n) {
+        SO_CUDA_TRY(cudaMemcpyAsync(c->d_scan, c->d_scan_sorted, n * sizeof(float4), cudaMemcpyDeviceToDevice, c->stream));
+        // the filtered cloud's w (the VoxelGrid average of the time the extraction stored in intensity) is the time
+        SO_CUDA_TRY(cudaMemcpy2DAsync(c->und.d_time, sizeof(float), reinterpret_cast<const char*>(c->d_scan_sorted) + 12, sizeof(float4),
+                                      sizeof(float), n, cudaMemcpyDeviceToDevice, c->stream));
+    }
+    return register_one(c, uint32_t(n), pose_in, m, opts, out, t0);
+}
+
+int so_register_batch_optimized(so_ctx* ctx, const void* surf, const uint32_t* n_points, size_t n_scans, size_t stride, size_t ioff, size_t toff,
+                                const double* poses_in, const so_motion* m, const so_icp_opts* opts, so_motion_result* results) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c || !surf || !n_points || !poses_in || !m || !opts || !results || stride < 12 || toff + 4 > stride) return fail(SO_ERR_ARG, "bad args");
+    if (n_scans == 0 || n_scans > c->max_batch) return fail(SO_ERR_CAPACITY, "n_scans exceeds so_config.max_batch");
+    size_t total = 0;
+    for (size_t s = 0; s < n_scans; ++s) { if (n_points[s] > c->cfg.max_scan_points) return fail(SO_ERR_CAPACITY, "scan too large"); total += n_points[s]; }
+    std::vector<MotionState> M(n_scans);
+    for (size_t s = 0; s < n_scans; ++s) {
+        int rc = check_motion(m + s, opts);
+        if (rc) return rc;
+        M[s] = make_state(m[s]);
+    }
+    SO_CUDA_TRY(cudaSetDevice(c->device));
+    const auto t0 = std::chrono::steady_clock::now();
+    c->und.last.on = 0;                                                  // d_scan and the times no longer hold the last single scan
+    int rc = reserve(c, total);
+    if (!rc) rc = upload_times(c, surf, total, stride, toff, c->und.d_time);
+    if (!rc) rc = upload_states(c, M.data(), n_scans);
+    if (rc) return rc;
+    std::vector<so_icp_result> icp(n_scans);
+    if (stride == 16 && ioff == 12) {                                   // packed: chunked upload overlapped with the kernels
+        rc = register_core(c, c->d_scan, n_points, n_scans, poses_in, opts, icp.data(), false, surf, nullptr, nullptr, 0, 2);
+    } else {
+        rc = upload_cloud(c, surf, total, stride, ioff, c->d_scan);
+        if (!rc) rc = register_core(c, c->d_scan, n_points, n_scans, poses_in, opts, icp.data(), false, nullptr, nullptr, nullptr, 0, 2);
+    }
+    if (!rc) rc = download_states(c, M.data(), n_scans);
+    if (rc) return rc;
+    const double ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    for (size_t s = 0; s < n_scans; ++s) {
+        icp[s].time_total_ms = ms;
+        fill_motion(icp[s], M[s], results + s);
+    }
+    return SO_OK;
+}
+
+int so_evaluate_optimized(so_ctx* ctx, const void* xyzi, size_t n, size_t stride, size_t ioff, size_t toff, const double pose[7],
+                          const double motion[7], double dt, int32_t max_surface_features, double H[144], double g[12], double* cost) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c || !pose || !motion || !xyzi || n == 0 || stride < 12 || toff + 4 > stride || !finite_pose(pose)) return fail(SO_ERR_ARG, "bad args");
+    so_motion m{};
+    m.dt = dt;
+    for (int k = 0; k < 7; ++k) m.motion_prior[k] = motion[k];
+    so_icp_opts o{};
+    o.max_icp_iters = 1; o.lm_max_iterations = 1; o.max_surface_features = max_surface_features; o.skip_map_checks = 1;
+    int rc = check_motion(&m, &o);
+    if (rc) return rc;
+    if (n > c->cfg.max_scan_points) return fail(SO_ERR_CAPACITY, "scan larger than so_config.max_scan_points");
+    SO_CUDA_TRY(cudaSetDevice(c->device));
+    rc = reserve(c, n);
+    if (!rc) rc = upload_cloud(c, xyzi, n, stride, ioff, c->d_scan);
+    if (!rc) rc = upload_times(c, xyzi, n, stride, toff, c->und.d_time);
+    if (rc) return rc;
+    c->last_scan_n = 0;                                                  // the stage hook leaves no registered scan behind
+    c->und.last.on = 0;
+    MotionState M = make_state(m);
+    M.stage = 1;
+    rc = upload_states(c, &M, 1);
+    if (rc) return rc;
+    double* sink = c->d_pose_sink;                                       // a stage evaluation appends no pose row
+    c->d_pose_sink = nullptr;
+    so_icp_result r;
+    uint32_t nn = uint32_t(n);
+    rc = register_core(c, c->d_scan, &nn, 1, pose, &o, &r, false, nullptr, nullptr, nullptr, 0, 2);
+    c->d_pose_sink = sink;
+    if (!rc) rc = download_states(c, &M, 1);
+    if (rc) return rc;
+    if (H) for (int i = 0; i < 12; ++i) for (int j = 0; j < 12; ++j) H[i * 12 + j] = M.H[i <= j ? tri12(i, j) : tri12(j, i)];
+    if (g) for (int i = 0; i < 12; ++i) g[i] = M.g[i];
+    if (cost) *cost = M.cost;
+    return SO_OK;
+}
+
+}  // extern "C"

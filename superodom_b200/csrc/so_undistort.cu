@@ -6,69 +6,16 @@
 //   alpha_i = double(tau_i) / dt                (a non-finite tau_i gives 0)
 //   q_i     = slerp(identity, q_D, alpha_i)     (Eigen's QuaternionBase::slerp; identity when rotation == 0)
 //   pInit_i = float3(qrot(q_i, p_i) + alpha_i * t_D)
-// and the iteration runs on pInit in place of p.  Every product and sum is rounded on its own (no FMA contraction), so that
-// tests/undistort_numpy.py restates the bits; only the FP64 acos / sin are the device's.
+// and the iteration runs on pInit in place of p (und_point, so_undistort.cuh; tests/undistort_numpy.py restates its bits).
 //   k_undistort        the ICP form: one thread per active point of the ordered scans, writes d_scan_sorted (w kept)
 //   k_undistort_cloud  a contiguous cloud at a given pose: the map insert after an undistorted registration, so_undistort_points
 #include <chrono>
 #include <cmath>
 #include <vector>
 
-#include "so_ctx.cuh"
+#include "so_undistort.cuh"
 
 namespace so {
-
-__device__ __forceinline__ void qmul_rn(const double a[4], const double b[4], double o[4]) {
-    o[0] = __dsub_rn(__dadd_rn(__dadd_rn(__dmul_rn(a[3], b[0]), __dmul_rn(a[0], b[3])), __dmul_rn(a[1], b[2])), __dmul_rn(a[2], b[1]));
-    o[1] = __dsub_rn(__dadd_rn(__dadd_rn(__dmul_rn(a[3], b[1]), __dmul_rn(a[1], b[3])), __dmul_rn(a[2], b[0])), __dmul_rn(a[0], b[2]));
-    o[2] = __dsub_rn(__dadd_rn(__dadd_rn(__dmul_rn(a[3], b[2]), __dmul_rn(a[2], b[3])), __dmul_rn(a[0], b[1])), __dmul_rn(a[1], b[0]));
-    o[3] = __dsub_rn(__dsub_rn(__dsub_rn(__dmul_rn(a[3], b[3]), __dmul_rn(a[0], b[0])), __dmul_rn(a[1], b[1])), __dmul_rn(a[2], b[2]));
-}
-// qrot of so_internal.cuh (v + 2w (q x v) + 2 q x (q x v)) with every operation rounded
-__device__ __forceinline__ void qrot_rn(const double q[4], const double v[3], double o[3]) {
-    double ux = __dsub_rn(__dmul_rn(q[1], v[2]), __dmul_rn(q[2], v[1]));
-    double uy = __dsub_rn(__dmul_rn(q[2], v[0]), __dmul_rn(q[0], v[2]));
-    double uz = __dsub_rn(__dmul_rn(q[0], v[1]), __dmul_rn(q[1], v[0]));
-    ux = __dadd_rn(ux, ux); uy = __dadd_rn(uy, uy); uz = __dadd_rn(uz, uz);
-    o[0] = __dadd_rn(__dadd_rn(v[0], __dmul_rn(q[3], ux)), __dsub_rn(__dmul_rn(q[1], uz), __dmul_rn(q[2], uy)));
-    o[1] = __dadd_rn(__dadd_rn(v[1], __dmul_rn(q[3], uy)), __dsub_rn(__dmul_rn(q[2], ux), __dmul_rn(q[0], uz)));
-    o[2] = __dadd_rn(__dadd_rn(v[2], __dmul_rn(q[3], uz)), __dsub_rn(__dmul_rn(q[0], uy), __dmul_rn(q[1], ux)));
-}
-
-// Per-scan part, once per CTA: sh = {q_D[4], t_D[3], theta, 1 / sin(theta)}; theta < 0 marks Eigen's linear branch (|d| >= 1 - eps,
-// d = dot(identity, q_D) = q_D.w).
-__device__ __forceinline__ void und_setup(const UndistortParams& P, const double x[7], double sh[9]) {
-    double q[4];
-    qmul_rn(P.q_prev_conj, x + 3, q);
-    const double n2 = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(q[0], q[0]), __dmul_rn(q[1], q[1])), __dmul_rn(q[2], q[2])), __dmul_rn(q[3], q[3]));
-    const double s = 1.0 / sqrt(n2);
-    for (int k = 0; k < 4; ++k) sh[k] = __dmul_rn(q[k], s);
-    const double d[3] = {__dsub_rn(x[0], P.t_prev[0]), __dsub_rn(x[1], P.t_prev[1]), __dsub_rn(x[2], P.t_prev[2])};
-    qrot_rn(P.q_prev_conj, d, sh + 4);
-    const double ad = fabs(sh[3]);
-    if (ad >= 1.0 - 2.220446049250313e-16) { sh[7] = -1.0; sh[8] = 0.0; }
-    else { sh[7] = acos(ad); sh[8] = 1.0 / sin(sh[7]); }
-}
-
-__device__ __forceinline__ float4 und_point(const UndistortParams& P, const double sh[9], float4 p, float tau) {
-    const double a = isfinite(tau) ? double(tau) / P.dt : 0.0;
-    const double v[3] = {double(p.x), double(p.y), double(p.z)};
-    double o[3] = {v[0], v[1], v[2]};
-    if (P.rotation) {
-        double s0, s1;
-        if (sh[7] < 0.0) { s0 = __dsub_rn(1.0, a); s1 = a; }
-        else {
-            s0 = __dmul_rn(sin(__dmul_rn(__dsub_rn(1.0, a), sh[7])), sh[8]);
-            s1 = __dmul_rn(sin(__dmul_rn(a, sh[7])), sh[8]);
-        }
-        if (sh[3] < 0.0) s1 = -s1;
-        const double qi[4] = {__dadd_rn(__dmul_rn(s0, 0.0), __dmul_rn(s1, sh[0])), __dadd_rn(__dmul_rn(s0, 0.0), __dmul_rn(s1, sh[1])),
-                              __dadd_rn(__dmul_rn(s0, 0.0), __dmul_rn(s1, sh[2])), __dadd_rn(s0, __dmul_rn(s1, sh[3]))};
-        qrot_rn(qi, v, o);
-    }
-    return make_float4(float(__dadd_rn(o[0], __dmul_rn(a, sh[4]))), float(__dadd_rn(o[1], __dmul_rn(a, sh[5]))),
-                       float(__dadd_rn(o[2], __dmul_rn(a, sh[6]))), p.w);
-}
 
 // One thread per active point, CTAs laid out per scan like the other per-point kernels; exits at once for scans that are not in
 // PH_CORR or not undistorted.  The raw point and its time are gathered from the upload buffers by the original index that scan
@@ -122,6 +69,7 @@ static void launch_undistort_cloud(Ctx* c, float4* pts, const float* times, uint
 }
 
 int undistort_tail(Ctx* c, MapStore& ms, uint32_t n_new, const double pose[7]) {
+    if (c->und.last.on == 2) return motion_tail(c, ms, n_new);       // after so_register_optimized*: u(D_opt), whatever the pose
     launch_undistort_cloud(c, ms.d_xyzi + ms.n, c->und.d_time, n_new, c->und.last, pose);
     SO_CUDA_TRY(cudaGetLastError());
     return SO_OK;
@@ -132,14 +80,14 @@ void undistort_free(Ctx* c) {
 }
 
 // ------------------------------------------------------------------------------------------------------------------ host side
-static bool finite_pose(const double p[7]) {
+bool finite_pose(const double p[7]) {
     for (int k = 0; k < 7; ++k) if (!std::isfinite(p[k])) return false;
     return p[3] * p[3] + p[4] * p[4] + p[5] * p[5] + p[6] * p[6] > 0.0;
 }
 
 static int check_undistort(const so_undistort* u) {
     if (!u) return fail(SO_ERR_ARG, "bad args");
-    if (u->mode == 2) return fail(SO_ERR_ARG, "so_undistort.mode 2 (OPTIMIZED) is not implemented");
+    if (u->mode == 2) return fail(SO_ERR_ARG, "so_undistort.mode 2 (OPTIMIZED) estimates a second pose: use so_register_optimized");
     if (u->mode != 0 && u->mode != 1) return fail(SO_ERR_ARG, "so_undistort.mode must be 0 (NONE) or 1 (APPROXIMATED)");
     if (u->mode == 0) return SO_OK;
     if (u->rotation != 0 && u->rotation != 1) return fail(SO_ERR_ARG, "so_undistort.rotation must be 0 or 1");
@@ -160,7 +108,7 @@ static UndistortParams make_params(const so_undistort& u) {
 }
 
 // The float at byte time_offset of every record -> dst (device)
-static int upload_times(Ctx* c, const void* src, size_t n, size_t stride, size_t toff, float* dst) {
+int upload_times(Ctx* c, const void* src, size_t n, size_t stride, size_t toff, float* dst) {
     if (n == 0) return SO_OK;
     std::vector<float> h(n);
     const unsigned char* p = static_cast<const unsigned char*>(src) + toff;
