@@ -168,8 +168,13 @@ int so_map_add_edge(so_ctx* ctx, const void* xyzi, size_t n, size_t stride_bytes
 /* replaces: LidarSLAM::transformAndAddToMap(cloud, world_cloud, false) (LidarSlam.cpp:60-80): transform the
  * sensor-frame scan by pose (utils::TransformPoint: double math, float store) on the device, then so_map_add_surf. */
 int so_map_add_scan(so_ctx* ctx, const void* xyzi, size_t n, size_t stride_bytes, size_t intensity_offset, const double pose[7]);
-/* Same insert for the surf cloud most recently passed to so_register, which is still in device memory: the live loop
- * Localization() -> transformAndAddToMap() (LidarSlam.cpp:155-171) without uploading the scan a second time. */
+/* Same insert for the surf cloud of the last single-scan registration (so_register, so_register_prefiltered, so_register_undistort,
+ * so_register_optimized and their prefiltered forms, so_localize_global*), which is still in device memory: the live loop
+ * Localization() -> transformAndAddToMap() (LidarSlam.cpp:155-171) without uploading the scan a second time.  Fails with SO_ERR_ARG,
+ * before any device work, when a call that reuses the scan buffers ran in between: so_scan_prefilter, so_scan_deskew,
+ * so_scan_extract_uniform, so_correspond, so_register_injected, the host batches so_register_batch*, so_evaluate_optimized (not
+ * so_register_batch_device, the k-NN, the other map calls, so_undistort_points or so_correspond_edge).  SO_OK and nothing inserted
+ * before the first registration. */
 int so_map_add_registered_scan(so_ctx* ctx, const double pose[7]);
 /* ... and transformAndAddToMap(cloud, world_cloud, true) for the edge cloud. */
 int so_map_add_scan_edge(so_ctx* ctx, const void* xyzi, size_t n, size_t stride_bytes, size_t intensity_offset, const double pose[7]);

@@ -304,50 +304,62 @@ static int prepare_scans(Ctx* c, const float4* d_scan_in, const Chunk& ch, cudaS
     return SO_OK;
 }
 
-// [k_knn_scan, k_fit, k_evaluate<PH_CORR>, k_lm_step, (k_evaluate<PH_EVAL>, k_lm_step) x lm] per ICP iteration; every kernel exits at once when its
-// scan is not in the matching phase, so a fixed schedule follows whatever path the device-side state machine takes.
-// Preferred form: a CUDA-graph WHILE node around ONE iteration (k_loop_cond ends the loop when every scan of the chunk
-// is done); fallback: the schedule unrolled max_icp_iters times.  Returns whether the loop form ran.
-// undistort 1: k_undistort (the scans' pInit at the current pose, so_undistort.cu) heads every iteration.
-// undistort 2 (so_motion.cu): [k_motion_warp, k_knn_scan, k_fit, k_motion_eval<PH_CORR>, k_motion_step, (k_motion_eval<PH_EVAL>,
-// k_motion_step) x lm] per iteration: the motion is a second parameter block of the solve.
-static int run_schedule(Ctx* c, const Chunk& ch, int iters, int lm, bool with_nn, bool* was_loop, cudaStream_t run_stream = nullptr,
-                        const uint32_t* d_inject = nullptr, int inject_iters = 0, int undistort = 0) {
-    if (!run_stream) run_stream = c->stream;
-    const float4* d_scan = c->d_scan_sorted;
+// One or two scans in flight are launch-latency bound: the optimiser step is folded into the evaluation kernels (k_evaluate_lm, which
+// launch_first_eval / launch_evaluate take when the chunk has no edge cloud).  Mode OPTIMIZED has its own solve.
+static bool fused_lm(const Ctx* c, uint32_t n_scans, UndistortionMode mode) {
+    return n_scans <= 2 && !c->profiling && !c->no_fused_lm && mode != UndistortionMode::OPTIMIZED;
+}
+
+// Kernels one ICP iteration of a captured schedule launches: the unrolled graph runs `iters` of them, the loop graph one per
+// iteration executed plus its k_loop_cond.  2: k_knn_scan + k_fit.
+static uint64_t iteration_launches(UndistortionMode mode, bool fused, uint32_t grid_e, int lm) {
+    if (mode == UndistortionMode::OPTIMIZED) return 1 + 2 + 2 + 2 * uint64_t(lm);         // warp, search + fit, (eval + step) x (1 + lm)
+    const uint64_t head = mode == UndistortionMode::APPROXIMATED ? 1 : 0;                  // k_undistort
+    if (fused && !grid_e) return head + 2 + 1 + uint64_t(lm);
+    return head + 2 + 2 + 2 * uint64_t(lm) + (grid_e ? 1 + uint64_t(lm) : 0);
+}
+
+// One ICP iteration: [head, k_knn_scan, k_fit, first solve, lm solves].  Every kernel exits at once when its scan is not in the
+// matching phase, so a fixed schedule follows whatever path the device-side state machine takes.
+//   head         mode APPROXIMATED: k_undistort (the scans' pInit at the current pose); OPTIMIZED: k_motion_warp (u(D)); NONE: none
+//   first solve  k_evaluate<PH_CORR> (+ k_edge_fit) + k_lm_step; OPTIMIZED: k_motion_eval<PH_CORR> + k_motion_step
+//   lm solves    k_evaluate<PH_EVAL> (+ k_edge_evaluate) + k_lm_step; OPTIMIZED: k_motion_eval<PH_EVAL> + k_motion_step
+// Preferred form: a CUDA-graph WHILE node around ONE iteration (k_loop_cond ends the loop when every scan of the chunk is done);
+// fallback: the schedule unrolled `iters` times.  Sets *was_loop to whether the loop form ran.  Profiling or injected neighbours:
+// launched one kernel at a time instead.
+static int run_schedule(Ctx* c, const Chunk& ch, int iters, int lm, UndistortionMode mode, const uint32_t* d_inject, int inject_iters,
+                        cudaStream_t run_stream, bool* was_loop) {
     const MapView mv = map_view(c, c->surf);
-    BatchView bv = batch_view(c, d_scan, ch.first);
+    BatchView bv = batch_view(c, c->d_scan_sorted, ch.first);
     CorrBuf cb = c->corr;
-    if (!with_nn) { cb.nn = nullptr; cb.nn_d2 = nullptr; }
+    cb.nn = nullptr; cb.nn_d2 = nullptr;
     const uint32_t grid_x = ch.grid_x, n_scans = ch.count, grid_e = ch.grid_e;
-    // one or two scans in flight: launch-latency bound -> optimiser step folded into the evaluation kernels (k_evaluate_lm)
-    if (n_scans <= 2 && !c->profiling && !c->no_fused_lm && undistort != 2) bv.counters = c->d_counters + ch.first;
+    const bool fused = fused_lm(c, n_scans, mode);
+    if (fused) bv.counters = c->d_counters + ch.first;
     bv.coop_knn = n_scans <= 2 && grid_x <= kCoopMaxGrid && !c->no_coop_knn;      // latency-bound search: a warp per query
     const MapView me = map_view(c, c->edge);
     EdgeBuf eb = c->ebuf;
     eb.offset = c->d_eoffset + ch.first;                  // like bv.offset: indexed by the scan's position inside the chunk
-    if (!with_nn) { eb.nn = nullptr; eb.selmask = nullptr; }
+    eb.nn = nullptr; eb.selmask = nullptr;
     *was_loop = false;
-    auto undistort_step = [&](cudaStream_t s) {
-        if (undistort == 2) launch_motion_warp(bv, c->d_scan_sorted, c->d_scan, c->und.d_time, c->mot.d_st, ch.first, grid_x, n_scans, s);
+    const bool optimized = mode == UndistortionMode::OPTIMIZED;
+    double* const mot_partials = c->mot.d_partials ? c->mot.d_partials + size_t(ch.first) * c->mot.stride * kMotionAcc : nullptr;
+    auto head = [&](cudaStream_t s) {
+        if (optimized) launch_motion_warp(bv, c->d_scan_sorted, c->d_scan, c->und.d_time, c->mot.d_st, ch.first, grid_x, n_scans, s);
         else launch_undistort(bv, c->d_scan_sorted, c->d_scan, c->und.d_time, c->und.d_par + ch.first, grid_x, n_scans, s);
     };
-    double* const mot_partials = c->mot.d_partials ? c->mot.d_partials + size_t(ch.first) * c->mot.stride * kMotionAcc : nullptr;
-    auto motion_solve = [&](int phase, cudaStream_t s) {
-        launch_motion_solve(phase, bv, cb, c->d_scan, c->und.d_time, c->mot.d_st, ch.first, mot_partials, c->mot.stride, grid_x, n_scans, s);
+    auto solve = [&](int phase, cudaStream_t s) {
+        if (optimized) launch_motion_solve(phase, bv, cb, c->d_scan, c->und.d_time, c->mot.d_st, ch.first, mot_partials, c->mot.stride, grid_x, n_scans, s);
+        else if (phase == PH_CORR) launch_first_eval(bv, cb, grid_x, n_scans, s, &me, &eb, grid_e);
+        else launch_evaluate(bv, cb, grid_x, n_scans, s, &eb, grid_e);
     };
-    // one ICP iteration after the (optional) undistortion head: correspondences, the first evaluation and lm candidate evaluations
     auto iteration = [&](cudaStream_t s) {
-        if (undistort == 2) {
-            launch_match(mv, bv, cb, c->nn, grid_x, n_scans, s);
-            motion_solve(PH_CORR, s);
-            for (int k = 0; k < lm; ++k) motion_solve(PH_EVAL, s);
-            return;
-        }
-        launch_correspond(mv, bv, cb, c->nn, grid_x, n_scans, s, &me, &eb, grid_e);
-        for (int k = 0; k < lm; ++k) launch_evaluate(bv, cb, grid_x, n_scans, s, &eb, grid_e);
+        if (mode != UndistortionMode::NONE) head(s);
+        launch_match(mv, bv, cb, c->nn, grid_x, n_scans, s);
+        solve(PH_CORR, s);
+        for (int k = 0; k < lm; ++k) solve(PH_EVAL, s);
     };
-    if (c->profiling || with_nn || d_inject) {
+    if (c->profiling || d_inject) {
         // profiling mode: one launch at a time, timed with events, and only launches that have work (the host peeks
         // at the phases) so that the per-class average is the duration of a kernel that actually ran
         std::vector<IcpState> peek(n_scans);
@@ -357,28 +369,19 @@ static int run_schedule(Ctx* c, const Chunk& ch, int iters, int lm, bool with_nn
             for (uint32_t s = 0; s < n_scans; ++s) if (peek[s].phase == ph) return true;
             return false;
         };
+        const uint64_t solve_extra = 1 + (grid_e ? 1 : 0);          // launches of a solve besides the one timed_launch_end counts
         for (int it = 0; it < iters; ++it) {
-            if (undistort == 2) {                                // every scan is in PH_CORR or PH_DONE when an iteration starts
-                if (!any_in(PH_CORR)) continue;
-                timed_launch_begin(c); undistort_step(c->stream); timed_launch_end(c, 7);
-                timed_launch_begin(c); launch_match(mv, bv, cb, c->nn, grid_x, n_scans, c->stream, 1); timed_launch_end(c, 0);
-                timed_launch_begin(c); launch_match(mv, bv, cb, c->nn, grid_x, n_scans, c->stream, 2); timed_launch_end(c, 5);
-                timed_launch_begin(c); motion_solve(PH_CORR, c->stream); c->launches++; timed_launch_end(c, 8);
-                for (int k = 0; k < lm; ++k)
-                    if (any_in(PH_EVAL)) { timed_launch_begin(c); motion_solve(PH_EVAL, c->stream); c->launches++; timed_launch_end(c, 8); }
-                continue;
-            }
             if (any_in(PH_CORR)) {
-                if (undistort) { timed_launch_begin(c); undistort_step(c->stream); timed_launch_end(c, 7); }
+                if (mode != UndistortionMode::NONE) { timed_launch_begin(c); head(c->stream); timed_launch_end(c, 7); }
                 timed_launch_begin(c);
                 if (d_inject) launch_inject(mv, c->surf.d_xyzi, c->surf.n, bv, c->nn, d_inject, inject_iters, grid_x, n_scans, c->stream);
                 else launch_match(mv, bv, cb, c->nn, grid_x, n_scans, c->stream, 1);                                               // k_knn_scan
                 timed_launch_end(c, 0);
                 timed_launch_begin(c); launch_match(mv, bv, cb, c->nn, grid_x, n_scans, c->stream, 2); timed_launch_end(c, 5);      // k_fit
-                timed_launch_begin(c); launch_first_eval(bv, cb, grid_x, n_scans, c->stream, &me, &eb, grid_e); c->launches += 1 + (grid_e ? 1 : 0); timed_launch_end(c, 4);
+                timed_launch_begin(c); solve(PH_CORR, c->stream); c->launches += solve_extra; timed_launch_end(c, optimized ? 8 : 4);
             }
             for (int k = 0; k < lm; ++k)
-                if (any_in(PH_EVAL)) { timed_launch_begin(c); launch_evaluate(bv, cb, grid_x, n_scans, c->stream, &eb, grid_e); c->launches += 1 + (grid_e ? 1 : 0); timed_launch_end(c, 1); }
+                if (any_in(PH_EVAL)) { timed_launch_begin(c); solve(PH_EVAL, c->stream); c->launches += solve_extra; timed_launch_end(c, optimized ? 8 : 1); }
         }
         SO_CUDA_TRY(cudaGetLastError());
         return SO_OK;
@@ -390,7 +393,7 @@ static int run_schedule(Ctx* c, const Chunk& ch, int iters, int lm, bool with_nn
     key.ptrs[4] = me.pts; key.ptrs[5] = me.cell_start; key.ptrs[6] = me.block_slot; key.ptrs[7] = me.block_count;
     for (int a = 0; a < 3; ++a) key.origin[a] = mv.origin[a];
     key.nb[0] = mv.nb; key.nb[1] = me.nb; key.res[0] = mv.plane_res; key.res[1] = me.plane_res;
-    if (undistort) { key.undistort = undistort; key.und_time = c->und.d_time; }
+    if (mode != UndistortionMode::NONE) { key.mode = mode; key.und_time = c->und.d_time; }
     Ctx::GraphSlot* slot = nullptr;
     for (auto& g : c->graphs)
         if (g.exec && std::memcmp(&g.key, &key, sizeof(key)) == 0) slot = &g;
@@ -414,7 +417,6 @@ static int run_schedule(Ctx* c, const Chunk& ch, int iters, int lm, bool with_nn
                 cudaGraph_t body = p.conditional.phGraph_out[0];
                 ok = cudaStreamBeginCaptureToGraph(c->stream, body, nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal) == cudaSuccess;
                 if (ok) {
-                    if (undistort) undistort_step(c->stream);
                     iteration(c->stream);
                     launch_loop_cond(bv, n_scans, handle, c->stream);
                     cudaGraph_t dummy = nullptr;
@@ -429,10 +431,7 @@ static int run_schedule(Ctx* c, const Chunk& ch, int iters, int lm, bool with_nn
         if (!slot->exec) {
             cudaGraph_t g = nullptr;
             SO_CUDA_TRY(cudaStreamBeginCapture(c->stream, cudaStreamCaptureModeThreadLocal));
-            for (int it = 0; it < iters; ++it) {
-                if (undistort) undistort_step(c->stream);
-                iteration(c->stream);
-            }
+            for (int it = 0; it < iters; ++it) iteration(c->stream);
             SO_CUDA_TRY(cudaStreamEndCapture(c->stream, &g));
             cudaError_t e = cudaGraphInstantiate(&slot->exec, g, 0);
             cudaGraphDestroy(g);
@@ -443,9 +442,7 @@ static int run_schedule(Ctx* c, const Chunk& ch, int iters, int lm, bool with_nn
     slot->used = ++c->graph_clock;
     SO_CUDA_TRY(cudaGraphLaunch(slot->exec, run_stream));
     *was_loop = slot->is_loop;
-    if (!slot->is_loop)
-        c->launches += uint64_t(iters) * (undistort == 2 ? 1 + 2 + 2 + 2 * lm
-                                                         : (bv.counters && !grid_e ? 2 + 1 + lm : 2 + 2 + 2 * lm + (grid_e ? 1 + lm : 0)) + (undistort ? 1 : 0));      // 2: k_knn_scan + k_fit; loop form: counted from the iterations executed
+    if (!slot->is_loop) c->launches += uint64_t(iters) * iteration_launches(mode, fused, grid_e, lm);   // loop form: counted by register_core
     return SO_OK;
 }
 
@@ -500,13 +497,19 @@ int icp_opts_check(const so_icp_opts& o) {
     return SO_OK;
 }
 
-// Shared tail of so_register / so_register_batch*: scans are on the device at d_scan (packed, back to back).
-// d_scan: device scans (packed, back to back).  host_src != nullptr: the scans are still on the host (packed float4); this
-// function uploads them into d_scan chunk by chunk on the copy stream.
-int register_core(Ctx* c, const float4* d_scan, const uint32_t* n_points, size_t n_scans, const double* poses, const so_icp_opts* opts_in,
-                  so_icp_result* results, bool allow_shift, const void* host_src, const uint32_t* n_edge, const uint32_t* d_inject, int inject_iters,
-                  int undistort) {
-    so_icp_opts o = *opts_in;
+// The registration of q's scans once they are on the device: at q.scans for Source::DEVICE, else at d_scan, where Source::HOST_PACKED
+// scans are uploaded here chunk by chunk on the copy stream.  Mode APPROXIMATED / OPTIMIZED: the scans' times, parameters or motion
+// blocks are on the device too.
+static int register_core(Ctx* c, const RegisterRequest& q) {
+    const float4* const d_scan = q.src == RegisterRequest::Source::DEVICE ? static_cast<const float4*>(q.scans) : c->d_scan;
+    const void* const host_src = q.src == RegisterRequest::Source::HOST_PACKED ? q.scans : nullptr;
+    const uint32_t* const n_points = q.n_points;
+    const uint32_t* const n_edge = q.n_edge;
+    const size_t n_scans = q.n_scans;
+    const double* const poses = q.poses;
+    so_icp_result* const results = q.results;
+    double* const sink = q.sink_rows ? c->d_pose_sink : nullptr;
+    so_icp_opts o = *q.opts;
     if (o.lm_max_iterations <= 0) o.lm_max_iterations = 4;
     { int rc = icp_opts_check(o); if (rc) return rc; }
     { int rc = ensure_maps(c); if (rc) return rc; }
@@ -521,7 +524,7 @@ int register_core(Ctx* c, const float4* d_scan, const uint32_t* n_points, size_t
         r->scan_surf_num = int32_t(n_points[s]);
         // prepareOptimizationState (LidarSlam.cpp:361-369)
         int32_t ijk[3];
-        if (allow_shift && !o.skip_map_checks) { int rc = so_map_shift(reinterpret_cast<so_ctx*>(c), pose, ijk); if (rc < 0) return rc; }
+        if (q.allow_shift && !o.skip_map_checks) { int rc = so_map_shift(reinterpret_cast<so_ctx*>(c), pose, ijk); if (rc < 0) return rc; }
         else for (int a = 0; a < 3; ++a) ijk[a] = block_coord_h(pose[a] + kHalfBlock, c->origin[a]);
         for (int a = 0; a < 3; ++a) r->pos_in_localmap[a] = ijk[a];
         r->map_surf_5x5 = counts_5x5(c, c->surf, ijk);
@@ -539,10 +542,10 @@ int register_core(Ctx* c, const float4* d_scan, const uint32_t* n_points, size_t
             c->h_state[s].phase = PH_DONE; c->h_state[s].status = r->status;
         } else { any = true; max_n = std::max(max_n, n_points[s]); }
     }
-    if (c->d_pose_sink && c->sink_cursor + n_scans > c->sink_cap) return fail(SO_ERR_CAPACITY, "pose sink full (so_set_pose_sink)");
-    if (!any && c->d_pose_sink) {                               // nothing to register: the rows are the priors
+    if (sink && c->sink_cursor + n_scans > c->sink_cap) return fail(SO_ERR_CAPACITY, "pose sink full (so_set_pose_sink)");
+    if (!any && sink) {                                         // nothing to register: the rows are the priors
         SO_CUDA_TRY(cudaMemcpyAsync(c->d_state, c->h_state, n_scans * sizeof(IcpState), cudaMemcpyHostToDevice, c->stream));
-        launch_pack_poses(c->d_state, uint32_t(n_scans), c->d_pose_sink + c->sink_cursor * 8, c->stream);
+        launch_pack_poses(c->d_state, uint32_t(n_scans), sink + c->sink_cursor * 8, c->stream);
         SO_CUDA_TRY(cudaStreamSynchronize(c->stream));
     }
     if (any) {
@@ -608,7 +611,7 @@ int register_core(Ctx* c, const float4* d_scan, const uint32_t* n_points, size_t
             if (ch.grid_x == 0) continue;
             int rc = prepare_scans(c, d_scan, ch, st, true);
             bool was_loop = false;
-            if (!rc) rc = run_schedule(c, ch, o.max_icp_iters, o.lm_max_iterations, false, &was_loop, st, d_inject, inject_iters, undistort);
+            if (!rc) rc = run_schedule(c, ch, o.max_icp_iters, o.lm_max_iterations, q.mode, q.inject ? c->d_inject : nullptr, q.inject_iters, st, &was_loop);
             if (rc) {                                       // leave no work behind on the side streams before reporting the error
                 cudaStreamSynchronize(c->aux_stream);
                 cudaStreamSynchronize(c->copy_stream);
@@ -622,7 +625,7 @@ int register_core(Ctx* c, const float4* d_scan, const uint32_t* n_points, size_t
         }
         SO_CUDA_TRY(cudaEventRecord(c->ev1, c->stream));
         { int rc = run_deferred_upload(c); if (rc) return rc; }      // host-side staging of the whole cloud while the registration runs
-        if (c->d_pose_sink) { launch_pack_poses(c->d_state, uint32_t(n_scans), c->d_pose_sink + c->sink_cursor * 8, c->stream); c->launches++; }
+        if (sink) { launch_pack_poses(c->d_state, uint32_t(n_scans), sink + c->sink_cursor * 8, c->stream); c->launches++; }
         SO_CUDA_TRY(cudaMemcpyAsync(c->h_state, c->d_state, n_scans * sizeof(IcpState), cudaMemcpyDeviceToHost, c->stream));
         count_d2h(c, n_scans * sizeof(IcpState));
         SO_CUDA_TRY(cudaStreamSynchronize(c->stream));
@@ -632,10 +635,8 @@ int register_core(Ctx* c, const float4* d_scan, const uint32_t* n_points, size_t
             if (!loop_flags[k]) continue;
             int max_it = 0;
             for (uint32_t s = chunks[k].first; s < chunks[k].first + chunks[k].count; ++s) max_it = std::max(max_it, int(c->h_state[s].n_iterations));
-            const bool fused = chunks[k].count <= 2 && !chunks[k].grid_e && !c->no_fused_lm;
-            if (undistort == 2) { c->launches += uint64_t(max_it) * uint64_t(1 + 2 + 3 + 2 * o.lm_max_iterations); continue; }
-            c->launches += uint64_t(max_it) * uint64_t((fused ? 2 + 2 + o.lm_max_iterations
-                                                              : 2 + 3 + 2 * o.lm_max_iterations + (chunks[k].grid_e ? 1 + o.lm_max_iterations : 0)) + (undistort ? 1 : 0));
+            const bool fused = fused_lm(c, chunks[k].count, q.mode);
+            c->launches += uint64_t(max_it) * (iteration_launches(q.mode, fused, chunks[k].grid_e, o.lm_max_iterations) + 1);   // + k_loop_cond
         }
         for (size_t s = 0; s < n_scans; ++s) {
             if (results[s].status == SO_STATUS_NOT_ENOUGH_FEATURES || n_points[s] == 0) continue;
@@ -643,14 +644,138 @@ int register_core(Ctx* c, const float4* d_scan, const uint32_t* n_points, size_t
             results[s].time_ms = double(ms);
         }
     }
-    if (c->d_pose_sink) c->sink_cursor += n_scans;
+    if (sink) c->sink_cursor += n_scans;
     return SO_OK;
+}
+
+// A capped so_register scan (the shipped configurations cap a 28 800-point scan at 2 000 features): the registration reads only the
+// points shouldProcessPoint keeps, so only those go up in front of it, into d_dec (32 KB instead of 460 KB).  The whole cloud -- needed
+// by so_map_add_registered_scan, not by the registration -- is staged and copied on the copy stream while the registration runs.
+static int upload_kept(Ctx* c, const RegisterRequest& q, size_t n_edge, uint32_t* kept_out) {
+    const uint32_t n = q.n_points[0];
+    const std::vector<uint32_t>& keep = decimation_list(c, n, q.opts->max_surface_features);
+    const uint32_t kept = uint32_t(keep.size());
+    if (kept == 0 || kept > kPrepareSmallCap) return fail(SO_ERR_ARG, "decimation list out of range");
+    const bool packed = q.stride == 16 && q.ioff == 12;
+    if (n_edge && !packed) SO_CUDA_TRY(cudaStreamSynchronize(c->stream));     // a strided edge cloud has to have left the staging buffer
+    SO_CUDA_TRY(cudaEventSynchronize(c->ev_dec));                              // so has the previous call's deferred copy
+    int rc = ensure_stage(c, (size_t(kPrepareSmallCap) + (packed ? 0 : n)) * sizeof(float4));
+    if (rc) return rc;
+    float4* h = static_cast<float4*>(c->h_stage);
+    const unsigned char* p = static_cast<const unsigned char*>(q.scans);
+    for (uint32_t j = 0; j < kept; ++j) h[j] = read_point(p + size_t(keep[j]) * q.stride, q.stride, q.ioff);
+    SO_CUDA_TRY(cudaEventRecord(c->ev_copy[16], c->stream));                  // the whole-cloud copy must not overtake earlier readers of d_scan
+    SO_CUDA_TRY(cudaStreamWaitEvent(c->copy_stream, c->ev_copy[16], 0));
+    SO_CUDA_TRY(cudaMemcpyAsync(c->d_dec, h, size_t(kept) * sizeof(float4), cudaMemcpyHostToDevice, c->stream));
+    c->bytes_h2d += size_t(kept) * sizeof(float4);
+    c->defer.src = q.scans; c->defer.n = n; c->defer.stride = q.stride; c->defer.ioff = q.ioff; c->defer.stage_off = kPrepareSmallCap;
+    *kept_out = kept;
+    return SO_OK;
+}
+
+int register_scans(Ctx* c, const RegisterRequest& q) {
+    using Source = RegisterRequest::Source;
+    SO_CUDA_TRY(cudaSetDevice(c->device));
+    const auto t0 = std::chrono::steady_clock::now();
+    size_t total = 0, total_e = 0;
+    for (size_t s = 0; s < q.n_scans; ++s) { total += q.n_points[s]; if (q.n_edge) total_e += q.n_edge[s]; }
+    const bool host = q.src == Source::HOST || q.src == Source::HOST_PACKED;
+    const bool with_times = q.mode != UndistortionMode::NONE;
+    if (q.src != Source::DEVICE) c->reg.valid = false;                         // d_scan is overwritten; valid again below if insertable
+    int rc = SO_OK;
+    if (q.mode == UndistortionMode::APPROXIMATED) rc = undistort_reserve(c, total);
+    if (q.mode == UndistortionMode::OPTIMIZED) rc = motion_reserve(c, total);
+    if (!rc && q.inject) {
+        const size_t words = size_t(q.inject_iters) * total * 5;
+        rc = grow_buffer(c->d_inject, c->inject_cap, words);
+        if (!rc) SO_CUDA_TRY(cudaMemcpyAsync(c->d_inject, q.inject, words * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
+    }
+    if (!rc && q.edge) rc = upload_cloud(c, q.edge, total_e, q.stride, q.ioff, c->d_escan);   // first: it may use the staging buffer
+    if (rc) return rc;
+    RegisterRequest core = q;                      // what register_core registers: a capped so_register scan, its kept points
+    const so_icp_opts& o = *q.opts;
+    so_icp_opts o_kept = o;
+    uint32_t kept = 0;
+    const bool decimated = q.src == Source::HOST && q.insertable && q.mode == UndistortionMode::NONE && !c->no_dec_upload &&
+                           o.max_surface_features > 0 && total > size_t(o.max_surface_features) && uint32_t(o.max_surface_features) + 1 <= kPrepareSmallCap;
+    if (decimated) {
+        rc = upload_kept(c, q, total_e, &kept);
+        o_kept.max_surface_features = 0;                                         // the decimation has been applied
+        core.src = Source::DEVICE; core.scans = c->d_dec; core.n_points = &kept; core.opts = &o_kept;
+    } else if (q.src == Source::HOST) {
+        rc = upload_cloud(c, q.scans, total, q.stride, q.ioff, c->d_scan);
+    } else if (q.src == Source::PREFILTERED) {
+        c->prefiltered_n = SIZE_MAX;
+        if (total) SO_CUDA_TRY(cudaMemcpyAsync(c->d_scan, c->d_scan_sorted, total * sizeof(float4), cudaMemcpyDeviceToDevice, c->stream));
+        // the filtered cloud's w (the VoxelGrid average of the time the extraction stored in intensity) is the time
+        if (total && with_times)
+            SO_CUDA_TRY(cudaMemcpy2DAsync(c->und.d_time, sizeof(float), reinterpret_cast<const char*>(c->d_scan_sorted) + 12, sizeof(float4),
+                                          sizeof(float), total, cudaMemcpyDeviceToDevice, c->stream));
+    }
+    if (!rc && host && with_times) rc = upload_times(c, q.scans, total, q.stride, q.toff, c->und.d_time);
+    if (!rc && q.mode == UndistortionMode::APPROXIMATED) {
+        SO_CUDA_TRY(cudaMemcpyAsync(c->und.d_par, q.und, q.n_scans * sizeof(UndistortParams), cudaMemcpyHostToDevice, c->stream));
+        count_h2d(c, q.n_scans * sizeof(UndistortParams));
+    }
+    if (!rc && q.mode == UndistortionMode::OPTIMIZED) {
+        SO_CUDA_TRY(cudaMemcpyAsync(c->mot.d_st, q.motion, q.n_scans * sizeof(MotionState), cudaMemcpyHostToDevice, c->stream));
+        count_h2d(c, q.n_scans * sizeof(MotionState));
+    }
+    if (rc) return rc;
+    rc = register_core(c, core);
+    if (decimated) {
+        const int rc2 = run_deferred_upload(c);                                  // not yet run when nothing was launched (soft statuses) or on errors
+        SO_CUDA_TRY(cudaStreamWaitEvent(c->stream, c->ev_dec, 0));               // later work on the context stream (the insert) sees the whole cloud
+        if (!rc) rc = rc2;
+        if (!rc) q.results[0].scan_surf_num = int32_t(total);
+    }
+    if (!rc && q.mode == UndistortionMode::OPTIMIZED) {
+        SO_CUDA_TRY(cudaMemcpyAsync(q.motion, c->mot.d_st, q.n_scans * sizeof(MotionState), cudaMemcpyDeviceToHost, c->stream));
+        count_d2h(c, q.n_scans * sizeof(MotionState));
+        SO_CUDA_TRY(cudaStreamSynchronize(c->stream));
+    }
+    if (rc) return rc;
+    const double ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    for (size_t s = 0; s < q.n_scans; ++s) {
+        q.results[s].time_total_ms = ms;
+        if (q.motion_results) fill_motion(q.results[s], q.motion[s], q.motion_results + s);
+    }
+    if (q.insertable) {
+        c->reg = RegisteredScan{};
+        c->reg.n = uint32_t(total); c->reg.mode = q.mode;
+        if (q.mode == UndistortionMode::APPROXIMATED) c->reg.par = q.und[0];
+        if (q.mode == UndistortionMode::OPTIMIZED) { std::memcpy(c->reg.D, q.motion[0].D, sizeof(c->reg.D)); c->reg.dt = q.motion[0].dt; }
+    }
+    return SO_OK;
+}
+
+// ---------------------------------------------------------------------------------------------- the so_register* family
+// A single scan as the live loop registers it: the map may shift to the prior, the scan stays for so_map_add_registered_scan
+static RegisterRequest single_scan(const uint32_t* n, const double* pose, const so_icp_opts* opts, so_icp_result* out) {
+    RegisterRequest q;
+    q.n_points = n; q.poses = pose; q.opts = opts; q.results = out; q.allow_shift = true; q.insertable = true;
+    return q;
+}
+static int status_of(int rc, const so_icp_result& r) { return rc ? rc : r.status; }
+static int check_batch(const Ctx* c, const uint32_t* n_points, size_t n_scans) {
+    if (n_scans == 0 || n_scans > c->max_batch) return fail(SO_ERR_CAPACITY, "n_scans exceeds so_config.max_batch");
+    for (size_t s = 0; s < n_scans; ++s) if (n_points[s] > c->cfg.max_scan_points) return fail(SO_ERR_CAPACITY, "scan too large");
+    return SO_OK;
+}
+// A batch of host clouds: packed float4 ones go up chunk by chunk beside the kernels, strided ones whole first
+static RegisterRequest batch_request(const void* surf, const uint32_t* n_points, size_t n_scans, size_t stride, size_t ioff, const double* poses,
+                                     const so_icp_opts* opts, so_icp_result* results) {
+    RegisterRequest q;
+    q.src = stride == 16 && ioff == 12 ? RegisterRequest::Source::HOST_PACKED : RegisterRequest::Source::HOST;
+    q.scans = surf; q.stride = stride; q.ioff = ioff; q.n_points = n_points; q.n_scans = n_scans; q.poses = poses; q.opts = opts; q.results = results;
+    return q;
 }
 
 }  // namespace so
 
 // =================================================================================================== C ABI
 using namespace so;
+using Source = RegisterRequest::Source;
 
 extern "C" {
 
@@ -778,7 +903,18 @@ static int store_set_points(Ctx* c, MapStore& ms, const void* xyzi, size_t n, si
     ms.n = uint32_t(n);
     return map_rebuild(c, ms);
 }
-// xyzi == nullptr with n != 0: the n points of the scan last uploaded by so_register (c->d_scan)
+// ms tail = the registered scan (Ctx::reg), still in d_scan, compensated for its motion as it was registered
+static int put_registered_scan(Ctx* c, MapStore& ms, const double pose[7]) {
+    const RegisteredScan& r = c->reg;
+    SO_CUDA_TRY(cudaMemcpyAsync(ms.d_xyzi + ms.n, c->d_scan, size_t(r.n) * sizeof(float4), cudaMemcpyDeviceToDevice, c->stream));
+    switch (r.mode) {
+        case UndistortionMode::APPROXIMATED: return undistort_tail(c, ms, r, pose);
+        case UndistortionMode::OPTIMIZED: return motion_tail(c, ms, r);      // u(D_opt), whatever the pose
+        default: return SO_OK;
+    }
+}
+
+// xyzi == nullptr with n != 0: the registered scan (put_registered_scan)
 static int store_add(Ctx* c, MapStore& ms, const void* xyzi, size_t n, size_t stride, size_t ioff, const double* pose) {
     if (!c || stride < 12) return fail(SO_ERR_ARG, "bad args");
     if (size_t(ms.n) + n > c->cfg.max_map_points) return fail(SO_ERR_CAPACITY, "map + new points exceed so_config.max_map_points");
@@ -786,10 +922,8 @@ static int store_add(Ctx* c, MapStore& ms, const void* xyzi, size_t n, size_t st
     if (n == 0) return SO_OK;
     int rc = SO_OK;
     if (ms.dirty) { rc = map_rebuild(c, ms); if (rc) return rc; }           // pending origin / resolution change first: it may compact the cloud
-    if (xyzi) rc = upload_cloud(c, xyzi, n, stride, ioff, ms.d_xyzi + ms.n);
-    else SO_CUDA_TRY(cudaMemcpyAsync(ms.d_xyzi + ms.n, c->d_scan, n * sizeof(float4), cudaMemcpyDeviceToDevice, c->stream));   // the registered scan, still on the device
+    rc = xyzi ? upload_cloud(c, xyzi, n, stride, ioff, ms.d_xyzi + ms.n) : put_registered_scan(c, ms, pose);
     if (rc) return rc;
-    if (!xyzi && pose && c->und.last.on) { rc = undistort_tail(c, ms, uint32_t(n), pose); if (rc) return rc; }   // after so_register_undistort*
     if (pose) { rc = map_transform_tail(c, ms, uint32_t(n), pose); if (rc) return rc; }
     timed_launch_begin(c);
     rc = map_add_points(c, ms, uint32_t(n));
@@ -823,8 +957,9 @@ int so_map_add_scan(so_ctx* ctx, const void* xyzi, size_t n, size_t stride, size
 int so_map_add_registered_scan(so_ctx* ctx, const double pose[7]) {
     Ctx* c = reinterpret_cast<Ctx*>(ctx);
     if (!c || !pose) return fail(SO_ERR_ARG, "bad args");
-    if (c->last_scan_n == 0) return SO_OK;
-    return store_add(c, c->surf, nullptr, c->last_scan_n, 16, 12, pose);
+    if (!c->reg.valid) return fail(SO_ERR_ARG, "so_map_add_registered_scan needs a preceding single-scan so_register* (and nothing that reuses the scan buffers in between)");
+    if (c->reg.n == 0) return SO_OK;
+    return store_add(c, c->surf, nullptr, c->reg.n, 16, 12, pose);
 }
 int so_map_add_scan_edge(so_ctx* ctx, const void* xyzi, size_t n, size_t stride, size_t ioff, const double pose[7]) {
     Ctx* c = reinterpret_cast<Ctx*>(ctx);
@@ -910,6 +1045,7 @@ int so_scan_prefilter(so_ctx* ctx, const void* xyzi, size_t n, size_t stride, si
     }
     int rc = so_map_set_resolution(ctx, *line_res, *plane_res);   // slam.localMap.lineRes_/planeRes_ = config_ (:648-649)
     if (rc) return rc;
+    c->reg.valid = false;
     rc = upload_cloud(c, xyzi, n, stride, ioff, c->d_scan);
     if (rc) return rc;
     uint32_t m = 0;
@@ -1019,6 +1155,7 @@ int so_scan_deskew(so_ctx* ctx, void* points, size_t n, size_t stride, size_t ti
     if (start_pose_out) std::memcpy(start_pose_out, out7, sizeof(out7));
     if (n_past_end) *n_past_end = 0;
     if (n == 0) return SO_OK;
+    c->reg.valid = false;
     int rc = upload_cloud(c, points, n, stride, time_offset, c->d_scan);          // float4 {x, y, z, time}
     if (rc) return rc;
     // pose samples into device scratch (the scan-sort key buffer): [times n][poses 7n]; IMU samples lose their translation here
@@ -1058,6 +1195,7 @@ int so_scan_extract_uniform(so_ctx* ctx, const void* points, size_t n, size_t st
     if (n > c->scan_cap) return fail(SO_ERR_CAPACITY, "cloud larger than the scan buffers");
     SO_CUDA_TRY(cudaSetDevice(c->device));
     *n_out = 0;
+    c->reg.valid = false;
     int rc = upload_cloud(c, points, n, stride, time_offset, c->d_scan);
     if (rc) return rc;
     uint32_t m = 0;
@@ -1075,83 +1213,29 @@ int so_scan_extract_uniform(so_ctx* ctx, const void* points, size_t n, size_t st
     return SO_OK;
 }
 
-// ---- registration ----------------------------------------------------------------------------------------------
+// ---- registration: the so_register* family.  Each entry point checks its own arguments, in its own order and with its own messages,
+// describes the call and hands it to register_scans.  Single-scan calls return the registration's status, batches SO_OK.
 int so_register(so_ctx* ctx, const void* surf, size_t n_surf, const void* edge, size_t n_edge, size_t stride, size_t ioff,
                 const double pose_in[7], const so_icp_opts* opts, so_icp_result* out) {
     Ctx* c = reinterpret_cast<Ctx*>(ctx);
     if (!c || !pose_in || !opts || !out || (!surf && n_surf) || (!edge && n_edge) || stride < 12) return fail(SO_ERR_ARG, "bad args");
     if (n_edge > c->edge_cap) return fail(SO_ERR_CAPACITY, "edge cloud larger than so_config.max_scan_points");
     if (n_surf > c->cfg.max_scan_points) return fail(SO_ERR_CAPACITY, "scan larger than so_config.max_scan_points");
-    SO_CUDA_TRY(cudaSetDevice(c->device));
-    const auto t0 = std::chrono::steady_clock::now();
-    const uint32_t n = uint32_t(n_surf);
-    const uint32_t ne = uint32_t(n_edge);
-    int rc;
-    // Decimated scan (the shipped configurations cap a 28 800-point scan at 2 000 features): the registration reads only the points
-    // shouldProcessPoint keeps, so only those go up in front of it (32 KB instead of 460 KB); the whole cloud -- needed by
-    // so_map_add_registered_scan, not by the registration -- is staged and copied on the copy stream while the registration runs.
-    const bool decimated = !c->no_dec_upload && opts->max_surface_features > 0 && n > uint32_t(opts->max_surface_features) &&
-                           uint32_t(opts->max_surface_features) + 1 <= kPrepareSmallCap;
-    if (decimated) {
-        const std::vector<uint32_t>& keep = decimation_list(c, n, opts->max_surface_features);
-        const uint32_t kept = uint32_t(keep.size());
-        if (kept == 0 || kept > kPrepareSmallCap) return fail(SO_ERR_ARG, "decimation list out of range");
-        const bool packed = stride == 16 && ioff == 12;
-        rc = upload_cloud(c, edge, n_edge, stride, ioff, c->d_escan);   // first: a strided edge cloud goes through the same staging buffer
-        if (rc) return rc;
-        if (n_edge && !packed) SO_CUDA_TRY(cudaStreamSynchronize(c->stream));       // ... and has to have left it
-        SO_CUDA_TRY(cudaEventSynchronize(c->ev_dec));                    // so has the previous call's deferred copy
-        rc = ensure_stage(c, (size_t(kPrepareSmallCap) + (packed ? 0 : n_surf)) * sizeof(float4));
-        if (rc) return rc;
-        float4* h = static_cast<float4*>(c->h_stage);
-        const unsigned char* p = static_cast<const unsigned char*>(surf);
-        for (uint32_t j = 0; j < kept; ++j) h[j] = read_point(p + size_t(keep[j]) * stride, stride, ioff);
-        SO_CUDA_TRY(cudaEventRecord(c->ev_copy[16], c->stream));        // the whole-cloud copy must not overtake earlier readers of d_scan
-        SO_CUDA_TRY(cudaStreamWaitEvent(c->copy_stream, c->ev_copy[16], 0));
-        SO_CUDA_TRY(cudaMemcpyAsync(c->d_dec, h, size_t(kept) * sizeof(float4), cudaMemcpyHostToDevice, c->stream));
-        c->bytes_h2d += size_t(kept) * sizeof(float4);
-        c->defer.src = surf; c->defer.n = n_surf; c->defer.stride = stride; c->defer.ioff = ioff; c->defer.stage_off = kPrepareSmallCap;
-        c->last_scan_n = n;
-        c->und.last.on = 0;
-        so_icp_opts o2 = *opts;
-        o2.max_surface_features = 0;                                     // the decimation has been applied
-        rc = register_core(c, c->d_dec, &kept, 1, pose_in, &o2, out, true, nullptr, &ne);
-        const int rc2 = run_deferred_upload(c);                          // not yet run when nothing was launched (soft statuses) or on errors
-        SO_CUDA_TRY(cudaStreamWaitEvent(c->stream, c->ev_dec, 0));       // later work on the context stream (the insert) sees the whole cloud
-        if (rc) return rc;
-        if (rc2) return rc2;
-        out->scan_surf_num = int32_t(n_surf);
-    } else {
-        rc = upload_cloud(c, surf, n_surf, stride, ioff, c->d_scan);
-        if (rc) return rc;
-        c->last_scan_n = n;                                             // so_map_add_registered_scan inserts it without a second upload
-        c->und.last.on = 0;
-        rc = upload_cloud(c, edge, n_edge, stride, ioff, c->d_escan);   // edge branch input (empty upstream: featureExtraction.cpp:429-436)
-        if (rc) return rc;
-        rc = register_core(c, c->d_scan, &n, 1, pose_in, opts, out, true, nullptr, &ne);
-        if (rc) return rc;
-    }
-    out->scan_edge_num = int32_t(n_edge);
-    out->time_total_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-    return out->status;
+    const uint32_t n = uint32_t(n_surf), ne = uint32_t(n_edge);
+    RegisterRequest q = single_scan(&n, pose_in, opts, out);
+    q.scans = surf; q.stride = stride; q.ioff = ioff;
+    q.edge = edge; q.n_edge = &ne;                                       // edge branch input (empty upstream: featureExtraction.cpp:429-436)
+    return status_of(register_scans(c, q), *out);
 }
 
 int so_register_prefiltered(so_ctx* ctx, const double pose_in[7], const so_icp_opts* opts, so_icp_result* out) {
     Ctx* c = reinterpret_cast<Ctx*>(ctx);
     if (!c || !pose_in || !opts || !out) return fail(SO_ERR_ARG, "bad args");
     if (c->prefiltered_n == SIZE_MAX) return fail(SO_ERR_ARG, "so_register_prefiltered needs a preceding so_scan_prefilter (and nothing that reuses the scan buffers in between)");
-    SO_CUDA_TRY(cudaSetDevice(c->device));
-    const auto t0 = std::chrono::steady_clock::now();
     const uint32_t n = uint32_t(c->prefiltered_n);
-    c->prefiltered_n = SIZE_MAX;
-    if (n) SO_CUDA_TRY(cudaMemcpyAsync(c->d_scan, c->d_scan_sorted, size_t(n) * sizeof(float4), cudaMemcpyDeviceToDevice, c->stream));
-    c->last_scan_n = n;
-    c->und.last.on = 0;
-    int rc = register_core(c, c->d_scan, &n, 1, pose_in, opts, out, true);
-    if (rc) return rc;
-    out->scan_edge_num = 0;
-    out->time_total_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-    return out->status;
+    RegisterRequest q = single_scan(&n, pose_in, opts, out);
+    q.src = Source::PREFILTERED;
+    return status_of(register_scans(c, q), *out);
 }
 
 int so_register_injected(so_ctx* ctx, const void* surf, size_t n_surf, size_t stride, size_t ioff, const double pose_in[7], const so_icp_opts* opts,
@@ -1159,80 +1243,141 @@ int so_register_injected(so_ctx* ctx, const void* surf, size_t n_surf, size_t st
     Ctx* c = reinterpret_cast<Ctx*>(ctx);
     if (!c || !pose_in || !opts || !out || !surf || !nn_ids || n_surf == 0 || n_trace_iters <= 0 || stride < 12) return fail(SO_ERR_ARG, "bad args");
     if (n_surf > c->cfg.max_scan_points) return fail(SO_ERR_CAPACITY, "scan larger than so_config.max_scan_points");
-    SO_CUDA_TRY(cudaSetDevice(c->device));
-    const size_t words = size_t(n_trace_iters) * n_surf * 5;
-    int rc = grow_buffer(c->d_inject, c->inject_cap, words);
-    if (rc) return rc;
-    SO_CUDA_TRY(cudaMemcpyAsync(c->d_inject, nn_ids, words * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
-    rc = upload_cloud(c, surf, n_surf, stride, ioff, c->d_scan);
-    if (rc) return rc;
     const uint32_t n = uint32_t(n_surf);
-    rc = register_core(c, c->d_scan, &n, 1, pose_in, opts, out, true, nullptr, nullptr, c->d_inject, int(n_trace_iters));
-    if (rc) return rc;
-    return out->status;
+    RegisterRequest q = single_scan(&n, pose_in, opts, out);
+    q.scans = surf; q.stride = stride; q.ioff = ioff; q.inject = nn_ids; q.inject_iters = n_trace_iters;
+    q.insertable = false;                                                // a test hook: its scan is not the live loop's
+    return status_of(register_scans(c, q), *out);
 }
 
 int so_register_batch(so_ctx* ctx, const void* surf, const uint32_t* n_points, size_t n_scans, size_t stride, size_t ioff,
                       const double* poses_in, const so_icp_opts* opts, so_icp_result* results) {
     Ctx* c = reinterpret_cast<Ctx*>(ctx);
     if (!c || !surf || !n_points || !poses_in || !opts || !results || stride < 12) return fail(SO_ERR_ARG, "bad args");
-    if (n_scans == 0 || n_scans > c->max_batch) return fail(SO_ERR_CAPACITY, "n_scans exceeds so_config.max_batch");
-    size_t total = 0;
-    for (size_t s = 0; s < n_scans; ++s) { if (n_points[s] > c->cfg.max_scan_points) return fail(SO_ERR_CAPACITY, "scan too large"); total += n_points[s]; }
-    SO_CUDA_TRY(cudaSetDevice(c->device));
-    const auto t0 = std::chrono::steady_clock::now();
-    int rc;
-    if (stride == 16 && ioff == 12) {
-        rc = register_core(c, c->d_scan, n_points, n_scans, poses_in, opts, results, false, surf);      // chunked, overlapped upload
-    } else {
-        rc = upload_cloud(c, surf, total, stride, ioff, c->d_scan);
-        if (rc) return rc;
-        rc = register_core(c, c->d_scan, n_points, n_scans, poses_in, opts, results, false);
-    }
-    if (rc) return rc;
-    const double ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-    for (size_t s = 0; s < n_scans; ++s) results[s].time_total_ms = ms;
-    return SO_OK;
+    int rc = check_batch(c, n_points, n_scans);
+    return rc ? rc : register_scans(c, batch_request(surf, n_points, n_scans, stride, ioff, poses_in, opts, results));
 }
 
 int so_register_batch_edges(so_ctx* ctx, const void* surf, const uint32_t* n_points, const void* edge, const uint32_t* n_edge, size_t n_scans,
                             size_t stride, size_t ioff, const double* poses_in, const so_icp_opts* opts, so_icp_result* results) {
     Ctx* c = reinterpret_cast<Ctx*>(ctx);
     if (!c || !surf || !n_points || !n_edge || !poses_in || !opts || !results || stride < 12) return fail(SO_ERR_ARG, "bad args");
-    if (n_scans == 0 || n_scans > c->max_batch) return fail(SO_ERR_CAPACITY, "n_scans exceeds so_config.max_batch");
-    size_t total = 0, total_e = 0;
-    for (size_t s = 0; s < n_scans; ++s) {
-        if (n_points[s] > c->cfg.max_scan_points) return fail(SO_ERR_CAPACITY, "scan too large");
-        total += n_points[s]; total_e += n_edge[s];
-    }
+    int rc = check_batch(c, n_points, n_scans);
+    if (rc) return rc;
+    size_t total_e = 0;
+    for (size_t s = 0; s < n_scans; ++s) total_e += n_edge[s];
     if (total_e > c->edge_cap) return fail(SO_ERR_CAPACITY, "edge clouds of the batch exceed so_config.max_scan_points points in total");
     if (total_e && !edge) return fail(SO_ERR_ARG, "bad args");
-    SO_CUDA_TRY(cudaSetDevice(c->device));
-    const auto t0 = std::chrono::steady_clock::now();
-    int rc = upload_cloud(c, edge, total_e, stride, ioff, c->d_escan);
-    if (rc) return rc;
-    rc = upload_cloud(c, surf, total, stride, ioff, c->d_scan);
-    if (rc) return rc;
-    rc = register_core(c, c->d_scan, n_points, n_scans, poses_in, opts, results, false, nullptr, n_edge);
-    if (rc) return rc;
-    const double ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-    for (size_t s = 0; s < n_scans; ++s) results[s].time_total_ms = ms;
-    return SO_OK;
+    RegisterRequest q = batch_request(surf, n_points, n_scans, stride, ioff, poses_in, opts, results);
+    q.src = Source::HOST;                                                // uploaded whole, packed or not
+    q.edge = edge; q.n_edge = n_edge;
+    return register_scans(c, q);
 }
 
 int so_register_batch_device(so_ctx* ctx, const void* d_scans, const uint32_t* n_points, size_t n_scans, const double* poses_in,
                              const so_icp_opts* opts, so_icp_result* results) {
     Ctx* c = reinterpret_cast<Ctx*>(ctx);
     if (!c || !d_scans || !n_points || !poses_in || !opts || !results) return fail(SO_ERR_ARG, "bad args");
-    if (n_scans == 0 || n_scans > c->max_batch) return fail(SO_ERR_CAPACITY, "n_scans exceeds so_config.max_batch");
-    for (size_t s = 0; s < n_scans; ++s) if (n_points[s] > c->cfg.max_scan_points) return fail(SO_ERR_CAPACITY, "scan too large");
-    SO_CUDA_TRY(cudaSetDevice(c->device));
-    const auto t0 = std::chrono::steady_clock::now();
-    int rc = register_core(c, static_cast<const float4*>(d_scans), n_points, n_scans, poses_in, opts, results, false);
+    int rc = check_batch(c, n_points, n_scans);
     if (rc) return rc;
-    const double ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-    for (size_t s = 0; s < n_scans; ++s) results[s].time_total_ms = ms;
-    return SO_OK;
+    RegisterRequest q = batch_request(d_scans, n_points, n_scans, 16, 12, poses_in, opts, results);
+    q.src = Source::DEVICE;
+    return register_scans(c, q);
+}
+
+int so_register_undistort(so_ctx* ctx, const void* surf, size_t n_surf, size_t stride, size_t ioff, size_t toff, const double pose_in[7],
+                          const so_undistort* u, const so_icp_opts* opts, so_icp_result* out) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c || !pose_in || !opts || !out || (!surf && n_surf) || stride < 12 || toff + 4 > stride) return fail(SO_ERR_ARG, "bad args");
+    int rc = check_undistort(u);
+    if (rc) return rc;
+    if (u->mode == 0) return so_register(ctx, surf, n_surf, nullptr, 0, stride, ioff, pose_in, opts, out);
+    if (n_surf > c->cfg.max_scan_points) return fail(SO_ERR_CAPACITY, "scan larger than so_config.max_scan_points");
+    const uint32_t n = uint32_t(n_surf);
+    const UndistortParams P = make_params(*u);
+    RegisterRequest q = single_scan(&n, pose_in, opts, out);
+    q.scans = surf; q.stride = stride; q.ioff = ioff; q.toff = toff; q.mode = UndistortionMode::APPROXIMATED; q.und = &P;
+    return status_of(register_scans(c, q), *out);
+}
+
+int so_register_prefiltered_undistort(so_ctx* ctx, const double pose_in[7], const so_undistort* u, const so_icp_opts* opts, so_icp_result* out) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c || !pose_in || !opts || !out) return fail(SO_ERR_ARG, "bad args");
+    int rc = check_undistort(u);
+    if (rc) return rc;
+    if (u->mode == 0) return so_register_prefiltered(ctx, pose_in, opts, out);
+    if (c->prefiltered_n == SIZE_MAX) return fail(SO_ERR_ARG, "so_register_prefiltered_undistort needs a preceding so_scan_prefilter (and nothing that reuses the scan buffers in between)");
+    const uint32_t n = uint32_t(c->prefiltered_n);
+    const UndistortParams P = make_params(*u);
+    RegisterRequest q = single_scan(&n, pose_in, opts, out);
+    q.src = Source::PREFILTERED; q.mode = UndistortionMode::APPROXIMATED; q.und = &P;
+    return status_of(register_scans(c, q), *out);
+}
+
+int so_register_batch_undistort(so_ctx* ctx, const void* surf, const uint32_t* n_points, size_t n_scans, size_t stride, size_t ioff, size_t toff,
+                                const double* poses_in, const so_undistort* u, const so_icp_opts* opts, so_icp_result* results) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c || !surf || !n_points || !poses_in || !u || !opts || !results || stride < 12 || toff + 4 > stride) return fail(SO_ERR_ARG, "bad args");
+    int rc = check_batch(c, n_points, n_scans);
+    if (rc) return rc;
+    std::vector<UndistortParams> P(n_scans);
+    bool any = false;
+    for (size_t s = 0; s < n_scans; ++s) {
+        if ((rc = check_undistort(u + s))) return rc;
+        P[s] = make_params(u[s]);
+        any |= P[s].on != 0;
+    }
+    RegisterRequest q = batch_request(surf, n_points, n_scans, stride, ioff, poses_in, opts, results);
+    q.toff = toff; q.und = P.data();
+    q.mode = any ? UndistortionMode::APPROXIMATED : UndistortionMode::NONE;   // mode 0 scans in an APPROXIMATED batch: k_undistort skips them
+    return register_scans(c, q);
+}
+
+int so_register_optimized(so_ctx* ctx, const void* surf, size_t n_surf, size_t stride, size_t ioff, size_t toff, const double pose_in[7],
+                          const so_motion* m, const so_icp_opts* opts, so_motion_result* out) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c || !pose_in || !opts || !out || (!surf && n_surf) || stride < 12 || toff + 4 > stride) return fail(SO_ERR_ARG, "bad args");
+    int rc = check_motion(m, opts);
+    if (rc) return rc;
+    if (n_surf > c->cfg.max_scan_points) return fail(SO_ERR_CAPACITY, "scan larger than so_config.max_scan_points");
+    const uint32_t n = uint32_t(n_surf);
+    MotionState M = make_state(*m);
+    so_icp_result icp;
+    RegisterRequest q = single_scan(&n, pose_in, opts, &icp);
+    q.scans = surf; q.stride = stride; q.ioff = ioff; q.toff = toff;
+    q.mode = UndistortionMode::OPTIMIZED; q.motion = &M; q.motion_results = out;
+    return status_of(register_scans(c, q), icp);
+}
+
+int so_register_prefiltered_optimized(so_ctx* ctx, const double pose_in[7], const so_motion* m, const so_icp_opts* opts, so_motion_result* out) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c || !pose_in || !opts || !out) return fail(SO_ERR_ARG, "bad args");
+    int rc = check_motion(m, opts);
+    if (rc) return rc;
+    if (c->prefiltered_n == SIZE_MAX) return fail(SO_ERR_ARG, "so_register_prefiltered_optimized needs a preceding so_scan_prefilter (and nothing that reuses the scan buffers in between)");
+    const uint32_t n = uint32_t(c->prefiltered_n);
+    MotionState M = make_state(*m);
+    so_icp_result icp;
+    RegisterRequest q = single_scan(&n, pose_in, opts, &icp);
+    q.src = Source::PREFILTERED; q.mode = UndistortionMode::OPTIMIZED; q.motion = &M; q.motion_results = out;
+    return status_of(register_scans(c, q), icp);
+}
+
+int so_register_batch_optimized(so_ctx* ctx, const void* surf, const uint32_t* n_points, size_t n_scans, size_t stride, size_t ioff, size_t toff,
+                                const double* poses_in, const so_motion* m, const so_icp_opts* opts, so_motion_result* results) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c || !surf || !n_points || !poses_in || !m || !opts || !results || stride < 12 || toff + 4 > stride) return fail(SO_ERR_ARG, "bad args");
+    int rc = check_batch(c, n_points, n_scans);
+    if (rc) return rc;
+    std::vector<MotionState> M(n_scans);
+    for (size_t s = 0; s < n_scans; ++s) {
+        if ((rc = check_motion(m + s, opts))) return rc;
+        M[s] = make_state(m[s]);
+    }
+    std::vector<so_icp_result> icp(n_scans);
+    RegisterRequest q = batch_request(surf, n_points, n_scans, stride, ioff, poses_in, opts, icp.data());
+    q.toff = toff; q.mode = UndistortionMode::OPTIMIZED; q.motion = M.data(); q.motion_results = results;
+    return register_scans(c, q);
 }
 
 int so_set_pose_sink(so_ctx* ctx, void* d_rows, size_t cap_rows, size_t first_row) {
@@ -1251,6 +1396,7 @@ int so_correspond(so_ctx* ctx, const void* surf, size_t n, size_t stride, size_t
     if (n > c->cfg.max_scan_points) return fail(SO_ERR_CAPACITY, "scan larger than so_config.max_scan_points");
     SO_CUDA_TRY(cudaSetDevice(c->device));
     { int rc0 = ensure_maps(c); if (rc0) return rc0; }
+    c->reg.valid = false;
     int rc = upload_cloud(c, surf, n, stride, ioff, c->d_scan);
     if (rc) return rc;
     so_icp_opts o{}; o.max_icp_iters = -1; o.lm_max_iterations = 4; o.max_surface_features = max_surface_features;

@@ -36,8 +36,11 @@ int grow_buffer(T*& p, size_t& cap, size_t n) {
 }
 
 struct ProfileSlot { double ms = 0.0; uint64_t launches = 0; };
-struct MotionState;                                // so_motion.cu: per-scan motion block of mode OPTIMIZED
 constexpr int kMotionAcc = 91;                     // 78 (upper triangle of the 12x12 H) + 12 (g) + 1 (cost)
+
+// Within-scan motion compensation of a registration (the reference's UndistortionMode, LidarSlam.h:65-82): NONE, APPROXIMATED
+// (so_undistort.cu: k_undistort heads every ICP iteration), OPTIMIZED (so_motion.cu: the motion is a second parameter block).
+enum class UndistortionMode : int32_t { NONE = 0, APPROXIMATED = 1, OPTIMIZED = 2 };
 
 // Within-scan motion compensation of one scan (so_undistort, mode APPROXIMATED): everything k_undistort needs besides the
 // current pose.  Kept out of IcpState so that the other kernels do not change.
@@ -47,6 +50,59 @@ struct UndistortParams {
     double dt;                                     // seconds from prev_pose to the pose being estimated, > 0
     int32_t on;                                    // 0: the scan registers exactly as so_register
     int32_t rotation;                              // 1: slerp the rotation too; 0: translation only
+};
+
+// Per-scan motion block of mode OPTIMIZED (so_motion.cu), next to the scan's IcpState
+struct MotionState {
+    double D0[7];              // motion prior (quaternion normalised)
+    double info[6];            // its information diagonal per accepted correspondence
+    double dt;                 // seconds the motion spans, > 0
+    double D[7], Dc[7];        // accepted / candidate motion
+    double H[78], g[12];       // at (x, D): upper triangle of the 12x12, gradient; prior rows included
+    double cost;               // so_evaluate_optimized: the plane rows' cost
+    double scale[12], diag[12], sqrt_info[6];
+    int32_t stage;             // so_evaluate_optimized: the first evaluation reports H, g, cost and ends the registration
+    int32_t pad;
+};
+static_assert(sizeof(MotionState) % 8 == 0, "copied as 8-byte words");
+
+// The scan so_map_add_registered_scan inserts: d_scan[0..n) in upload order and, unless mode NONE, its times in und.d_time[0..n)
+struct RegisteredScan {
+    bool valid = true;                             // false: a call has overwritten d_scan or the times since that scan registered
+    uint32_t n = 0;                                // 0: no scan registered yet, nothing to insert
+    UndistortionMode mode = UndistortionMode::NONE;
+    UndistortParams par{};                         // APPROXIMATED: the parameters it registered with
+    double D[7] = {0, 0, 0, 0, 0, 0, 1}, dt = 0;   // OPTIMIZED: the estimated motion D_opt and the time it spans
+};
+
+// One registration call (register_scans, so_api.cu): where the scans come from, what they are, how they register, where the
+// results go.  Serves every so_register* entry point, so_evaluate_optimized and the candidate refinement of so_localize_global*.
+struct RegisterRequest {
+    enum class Source {
+        HOST,                                      // host cloud(s) in the stride / ioff layout, uploaded whole first
+        HOST_PACKED,                               // host batch of packed float4, uploaded chunk by chunk beside the kernels
+        DEVICE,                                    // packed float4 scans in device memory (d_scan and its record untouched)
+        PREFILTERED,                               // the cloud so_scan_prefilter left in d_scan_sorted; its w is the time
+    };
+    Source src = Source::HOST;
+    const void* scans = nullptr;                   // HOST*: the host cloud; DEVICE: the device scans
+    size_t stride = 16, ioff = 12, toff = 12;      // host layout: bytes per point, offsets of the intensity and of the time
+    const uint32_t* n_points = nullptr;            // [n_scans], scans back to back
+    size_t n_scans = 1;
+    const void* edge = nullptr;                    // optional host edge clouds (host layout), n_edge[s] points each, back to back
+    const uint32_t* n_edge = nullptr;
+    const double* poses = nullptr;                 // [n_scans][7] priors
+    const so_icp_opts* opts = nullptr;
+    UndistortionMode mode = UndistortionMode::NONE;
+    const UndistortParams* und = nullptr;          // APPROXIMATED: [n_scans]
+    MotionState* motion = nullptr;                 // OPTIMIZED: [n_scans], uploaded first and read back after the registration
+    const uint32_t* inject = nullptr;              // host neighbour ids [inject_iters][n][5] in place of the search
+    int inject_iters = 0;
+    bool allow_shift = false;                      // the map may shift to the priors (single-scan registration)
+    bool sink_rows = true;                         // an attached pose sink gets a row per scan
+    bool insertable = false;                       // the scan stays for so_map_add_registered_scan
+    so_icp_result* results = nullptr;              // [n_scans]
+    so_motion_result* motion_results = nullptr;    // OPTIMIZED, optional: [n_scans] results with the motion
 };
 
 // One per-block cloud family of the LocalMap (surf or edge): points in id order, the sorted hash grid, block tables.
@@ -89,7 +145,7 @@ struct Ctx {
     uint32_t max_batch = 1;
     size_t scan_cap = 0;                           // points over the whole batch
     size_t prefiltered_n = SIZE_MAX;               // points so_scan_prefilter left in d_scan_sorted (SIZE_MAX: none / overwritten since)
-    uint32_t last_scan_n = 0;                      // points of the scan so_register uploaded last (d_scan[0..n), original order)
+    RegisteredScan reg;                            // what d_scan (and und.d_time) hold for so_map_add_registered_scan
     float4* d_scan = nullptr;                      // upload target for host scans (original order)
     float4* d_scan_sorted = nullptr;               // cell-ordered copy the kernels read; w = original index
     uint64_t* d_skeys = nullptr; uint64_t* d_skeys_out = nullptr;   // scan sort keys (scan id << 32 | cell)
@@ -138,7 +194,7 @@ struct Ctx {
     struct GraphKey {
         uint32_t first, count, grid_x, grid_e; int32_t iters, lm;
         const void* ptrs[8]; int32_t origin[3]; int32_t nb[2]; float res[2];
-        int32_t undistort; const void* und_time;   // k_undistort heads every iteration (0 / nullptr otherwise)
+        UndistortionMode mode; const void* und_time;   // the head of every iteration (NONE / nullptr: none)
     };
     struct GraphSlot {
         cudaGraphExec_t exec = nullptr;
@@ -188,15 +244,12 @@ struct Ctx {
         float* d_time = nullptr; size_t time_cap = 0;                      // per-point times of the scans in d_scan (upload order)
         float4* d_hook = nullptr; size_t hook_cap = 0;                     // so_undistort_points: the cloud and its times
         float* d_hook_time = nullptr; size_t hook_time_cap = 0;
-        UndistortParams last{};                                            // of the scan so_map_add_registered_scan inserts (on == 0: none,
-                                                                           // 2: so_register_optimized*, the motion is mot.last_D)
     } und;
     // ---- within-scan motion estimated by the registration (so_register_optimized*): allocated on first use ------------------
     struct Mot {
         MotionState* d_st = nullptr; size_t st_cap = 0;                    // [max_batch] per-scan motion blocks
         double* d_partials = nullptr; size_t partials_cap = 0;             // [max_batch][stride][kMotionAcc] per-CTA sums
         uint32_t stride = 0;                                               // CTAs per scan the partials are laid out for
-        double last_D[7] = {0, 0, 0, 0, 0, 0, 1};                          // D_opt of the last single-scan registration (und.last.on == 2)
     } mot;
 
     // ---- instrumentation ----------------------------------------------------------------------------------------
@@ -217,11 +270,9 @@ void count_d2h(Ctx* c, size_t b);
 void timed_launch_begin(Ctx* c);
 void timed_launch_end(Ctx* c, int cls);                     // counts one launch; profile class cls when profiling
 int icp_opts_check(const so_icp_opts& o);                   // max_icp_iters and lm_max_iterations in the supported range
-// Registration of n_scans scans at d_scan (packed, back to back), or of host_src's packed scans uploaded chunk by chunk.
-// undistort: 0 none, 1 APPROXIMATED (Ctx::und.d_par), 2 OPTIMIZED (Ctx::mot.d_st; every scan of the call).
-int register_core(Ctx* c, const float4* d_scan, const uint32_t* n_points, size_t n_scans, const double* poses,
-                  const so_icp_opts* opts_in, so_icp_result* results, bool allow_shift, const void* host_src = nullptr,
-                  const uint32_t* n_edge = nullptr, const uint32_t* d_inject = nullptr, int inject_iters = 0, int undistort = 0);
+// Serves one request: puts the scans, their times and the mode's parameters on the device, registers, reads the motion back, fills
+// results (time_total_ms included) and keeps the record of the scan left in d_scan.  The caller has checked the arguments.
+int register_scans(Ctx* c, const RegisterRequest& q);
 inline float4 read_point(const unsigned char* p, size_t stride, size_t ioff) {     // one point of a strided host cloud
     float xyz[3], it = 0.f;
     std::memcpy(xyz, p, 12);
@@ -232,16 +283,24 @@ inline float4 read_point(const unsigned char* p, size_t stride, size_t ioff) {  
 void global_free(Ctx* c);                                   // the search buffers and events of Ctx::reloc / Ctx::bnb
 // so_undistort.cu
 void undistort_free(Ctx* c);                                // the buffers of Ctx::und
+int undistort_reserve(Ctx* c, size_t n_points);             // Ctx::und's parameters (max_batch) and times (n_points)
+int check_undistort(const so_undistort* u);                 // argument errors of one so_undistort
+UndistortParams make_params(const so_undistort& u);
 bool finite_pose(const double p[7]);                        // finite, with a non-zero quaternion
 int upload_times(Ctx* c, const void* src, size_t n, size_t stride, size_t toff, float* dst);   // the float at toff of every record -> dst
 // k_undistort: pInit of every active point of the chunk's scans (bv.st / bv.offset / par already offset to the chunk), from the
 // raw points in upload order (raw, times: indexed offset + original index) into the ordered copy `sorted`, w kept
 void launch_undistort(const BatchView& bv, float4* sorted, const float4* raw, const float* times, const UndistortParams* par,
                       uint32_t grid_x, uint32_t n_scans, cudaStream_t st);
-int undistort_tail(Ctx* c, MapStore& ms, uint32_t n_new, const double pose[7]);   // ms tail = the registered scan: pInit at pose, in place
+// ms tail = the registered scan r (APPROXIMATED): pInit at pose, in place
+int undistort_tail(Ctx* c, MapStore& ms, const RegisteredScan& r, const double pose[7]);
 // so_motion.cu
 void motion_free(Ctx* c);                                   // the buffers of Ctx::mot
-int motion_tail(Ctx* c, MapStore& ms, uint32_t n_new);      // ms tail = the registered scan: u(mot.last_D), in place
+int motion_reserve(Ctx* c, size_t n_points);                // Ctx::mot's blocks and partials (max_batch), Ctx::und's times (n_points)
+int check_motion(const so_motion* m, const so_icp_opts* o); // argument errors of one so_motion and the options it registers with
+MotionState make_state(const so_motion& m);
+void fill_motion(const so_icp_result& icp, const MotionState& M, so_motion_result* out);   // out = icp + motion, pose_end = T * D
+int motion_tail(Ctx* c, MapStore& ms, const RegisteredScan& r);   // ms tail = the registered scan r (OPTIMIZED): u(r.D), in place
 // One ICP iteration's kernels of mode OPTIMIZED for the chunk's scans (bv.st / bv.offset / partials already offset to the chunk, ms
 // the whole array and `first` the chunk's first scan): the warp u(D) into `sorted`, and one evaluation + trust-region step (phase
 // PH_CORR: the first of a solve)

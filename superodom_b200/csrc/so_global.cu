@@ -1,6 +1,6 @@
 // so_global.cu -- global localization against the prior map, host side: defaults and limits of the search, score points and yaw
 // quaternions, the exhaustive and the branch-and-bound searches (kernels in so_reloc.cu), suppression and refinement of the best
-// hypotheses through register_core, and the so_localize_* / so_map_bounds entry points of the C ABI.
+// hypotheses through register_scans, and the so_localize_* / so_map_bounds entry points of the C ABI.
 #include <algorithm>
 #include <chrono>
 #include <cmath>
@@ -218,13 +218,6 @@ static int global_check_args(Ctx* c, const void* xyzi, size_t n, size_t stride, 
     return SO_OK;
 }
 
-// Detaches the pose sink for the candidate registrations (they are internal to one call) and puts it back on every return path.
-struct SinkDetach {
-    Ctx* c; double* rows; size_t cap, cursor;
-    explicit SinkDetach(Ctx* cc) : c(cc), rows(cc->d_pose_sink), cap(cc->sink_cap), cursor(cc->sink_cursor) { c->d_pose_sink = nullptr; }
-    ~SinkDetach() { c->d_pose_sink = rows; c->sink_cap = cap; c->sink_cursor = cursor; }
-};
-
 // Everything after the search: suppression over the sorted key prefix pref[0..n_pref), refinement of the kept candidates, winner
 // selection.  Shared by so_localize_global and so_localize_global_bnb, which produce the same prefix.
 static int global_refine(Ctx* c, const GlobalPlan& P, const GlobalScan& S, const uint64_t* pref, size_t n_pref, const void* xyzi, size_t n,
@@ -260,10 +253,11 @@ static int global_refine(Ctx* c, const GlobalPlan& P, const GlobalScan& S, const
     }
     // the whole cloud goes to the scan buffer (so_map_add_registered_scan inserts it afterwards), once per batch slot
     c->prefiltered_n = SIZE_MAX;
+    c->reg.valid = false;
     int rc = upload_cloud(c, xyzi, n, stride, ioff, c->d_scan);
     if (rc) return rc;
-    c->last_scan_n = uint32_t(n);
-    c->und.last.on = 0;
+    c->reg = RegisteredScan{};
+    c->reg.n = uint32_t(n);
     const size_t n_cand = kept.size();
     out->n_candidates = int32_t(n_cand);
     std::vector<so_icp_result> res(n_cand);
@@ -274,10 +268,11 @@ static int global_refine(Ctx* c, const GlobalPlan& P, const GlobalScan& S, const
         std::vector<uint32_t> npts(B, uint32_t(n));
         std::vector<double> priors(7 * n_cand);
         for (size_t q = 0; q < n_cand; ++q) std::memcpy(priors.data() + 7 * q, kept[q].prior, 7 * sizeof(double));
-        SinkDetach sink(c);                                   // the candidate registrations leave no rows in a pose sink
+        RegisterRequest q;                                    // the candidate registrations leave no rows in a pose sink
+        q.src = RegisterRequest::Source::DEVICE; q.scans = c->d_scan; q.n_points = npts.data(); q.opts = opts; q.sink_rows = false;
         for (size_t s0 = 0; s0 < n_cand; s0 += B) {
-            const size_t nb = std::min(B, n_cand - s0);
-            rc = register_core(c, c->d_scan, npts.data(), nb, priors.data() + 7 * s0, opts, res.data() + s0, false);
+            q.n_scans = std::min(B, n_cand - s0); q.poses = priors.data() + 7 * s0; q.results = res.data() + s0;
+            rc = register_scans(c, q);
             if (rc) return rc;
         }
     }

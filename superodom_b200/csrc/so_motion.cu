@@ -14,26 +14,12 @@
 //   k_motion_eval<PH>    residual and 12-column row per correspondence, 91 per-CTA sums (78 + 12 + 1) through shared memory
 //   k_motion_step<PH>    fixed-order cross-CTA sum, then the 12-parameter trust-region step; the 12x12 covariance at the end
 //   k_motion_cloud       u(D_opt) of a contiguous cloud: the map insert after a single-scan registration
-#include <chrono>
 #include <cmath>
 #include <vector>
 
 #include "so_undistort.cuh"
 
 namespace so {
-
-struct MotionState {
-    double D0[7];              // motion prior (quaternion normalised)
-    double info[6];            // its information diagonal per accepted correspondence
-    double dt;                 // seconds the motion spans, > 0
-    double D[7], Dc[7];        // accepted / candidate motion
-    double H[78], g[12];       // at (x, D): upper triangle of the 12x12, gradient; prior rows included
-    double cost;               // so_evaluate_optimized: the plane rows' cost
-    double scale[12], diag[12], sqrt_info[6];
-    int32_t stage;             // so_evaluate_optimized: the first evaluation reports H, g, cost and ends the registration
-    int32_t pad;
-};
-static_assert(sizeof(MotionState) % 8 == 0, "copied as 8-byte words");
 
 __host__ __device__ inline int tri12(int i, int j) { return i * 12 - (i * (i - 1)) / 2 + (j - i); }
 
@@ -558,12 +544,12 @@ void launch_motion_solve(int phase, const BatchView& bv, const CorrBuf& cb, cons
     }
 }
 
-int motion_tail(Ctx* c, MapStore& ms, uint32_t n_new) {
-    if (!n_new) return SO_OK;
+int motion_tail(Ctx* c, MapStore& ms, const RegisteredScan& r) {
+    if (!r.n) return SO_OK;
     MotionD D;
-    for (int k = 0; k < 7; ++k) D.v[k] = c->mot.last_D[k];
+    for (int k = 0; k < 7; ++k) D.v[k] = r.D[k];
     timed_launch_begin(c);
-    k_motion_cloud<<<(n_new + 255) / 256, 256, 0, c->stream>>>(ms.d_xyzi + ms.n, c->und.d_time, n_new, D, c->und.last.dt);
+    k_motion_cloud<<<(r.n + 255) / 256, 256, 0, c->stream>>>(ms.d_xyzi + ms.n, c->und.d_time, r.n, D, r.dt);
     timed_launch_end(c, 7);
     SO_CUDA_TRY(cudaGetLastError());
     return SO_OK;
@@ -572,7 +558,7 @@ int motion_tail(Ctx* c, MapStore& ms, uint32_t n_new) {
 void motion_free(Ctx* c) { cudaFree(c->mot.d_st); cudaFree(c->mot.d_partials); }
 
 // ------------------------------------------------------------------------------------------------------------------ host side
-static int check_motion(const so_motion* m, const so_icp_opts* o) {
+int check_motion(const so_motion* m, const so_icp_opts* o) {
     if (!m || !o) return fail(SO_ERR_ARG, "bad args");
     if (!(std::isfinite(m->dt) && m->dt > 0.0)) return fail(SO_ERR_ARG, "so_motion.dt must be finite and > 0");
     if (!finite_pose(m->motion_prior)) return fail(SO_ERR_ARG, "so_motion.motion_prior must be finite with a non-zero quaternion");
@@ -582,7 +568,7 @@ static int check_motion(const so_motion* m, const so_icp_opts* o) {
     return icp_opts_check(*o);
 }
 
-static MotionState make_state(const so_motion& m) {
+MotionState make_state(const so_motion& m) {
     MotionState M;
     std::memset(&M, 0, sizeof(M));
     const double* p = m.motion_prior;
@@ -595,7 +581,7 @@ static MotionState make_state(const so_motion& m) {
     return M;
 }
 
-static int reserve(Ctx* c, size_t n_points) {
+int motion_reserve(Ctx* c, size_t n_points) {
     c->mot.stride = eval_grid(c->grid_x_cap * kThreads);
     int rc = grow_buffer(c->mot.d_st, c->mot.st_cap, size_t(c->max_batch));
     if (!rc) rc = grow_buffer(c->mot.d_partials, c->mot.partials_cap, size_t(c->max_batch) * c->mot.stride * kMotionAcc);
@@ -603,21 +589,8 @@ static int reserve(Ctx* c, size_t n_points) {
     return rc;
 }
 
-static int upload_states(Ctx* c, const MotionState* M, size_t n) {
-    SO_CUDA_TRY(cudaMemcpyAsync(c->mot.d_st, M, n * sizeof(MotionState), cudaMemcpyHostToDevice, c->stream));
-    count_h2d(c, n * sizeof(MotionState));
-    return SO_OK;
-}
-
-static int download_states(Ctx* c, MotionState* M, size_t n) {
-    SO_CUDA_TRY(cudaMemcpyAsync(M, c->mot.d_st, n * sizeof(MotionState), cudaMemcpyDeviceToHost, c->stream));
-    count_d2h(c, n * sizeof(MotionState));
-    SO_CUDA_TRY(cudaStreamSynchronize(c->stream));
-    return SO_OK;
-}
-
 // so_motion_result from the registration's result and the motion block: pose_end = T * D with T = pose_opt
-static void fill_motion(const so_icp_result& icp, const MotionState& M, so_motion_result* out) {
+void fill_motion(const so_icp_result& icp, const MotionState& M, so_motion_result* out) {
     out->icp = icp;
     for (int k = 0; k < 7; ++k) out->motion[k] = M.D[k];
     const double* T = icp.pose_opt;
@@ -627,105 +600,11 @@ static void fill_motion(const so_icp_result& icp, const MotionState& M, so_motio
     qmul(T + 3, M.D + 3, out->pose_end + 3);
 }
 
-// The single-scan tail: the cloud (n points) is in d_scan, its times in und.d_time
-static int register_one(Ctx* c, uint32_t n, const double pose_in[7], const so_motion* m, const so_icp_opts* opts, so_motion_result* out,
-                        std::chrono::steady_clock::time_point t0) {
-    MotionState M = make_state(*m);
-    int rc = upload_states(c, &M, 1);
-    if (rc) return rc;
-    so_icp_result icp;
-    rc = register_core(c, c->d_scan, &n, 1, pose_in, opts, &icp, true, nullptr, nullptr, nullptr, 0, 2);
-    if (!rc) rc = download_states(c, &M, 1);
-    if (rc) return rc;
-    c->last_scan_n = n;
-    c->und.last = UndistortParams{};
-    c->und.last.on = 2; c->und.last.dt = m->dt;
-    for (int k = 0; k < 7; ++k) c->mot.last_D[k] = M.D[k];
-    icp.scan_edge_num = 0;
-    icp.time_total_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-    fill_motion(icp, M, out);
-    return icp.status;
-}
-
 }  // namespace so
 
 using namespace so;
 
 extern "C" {
-
-int so_register_optimized(so_ctx* ctx, const void* surf, size_t n_surf, size_t stride, size_t ioff, size_t toff, const double pose_in[7],
-                          const so_motion* m, const so_icp_opts* opts, so_motion_result* out) {
-    Ctx* c = reinterpret_cast<Ctx*>(ctx);
-    if (!c || !pose_in || !opts || !out || (!surf && n_surf) || stride < 12 || toff + 4 > stride) return fail(SO_ERR_ARG, "bad args");
-    int rc = check_motion(m, opts);
-    if (rc) return rc;
-    if (n_surf > c->cfg.max_scan_points) return fail(SO_ERR_CAPACITY, "scan larger than so_config.max_scan_points");
-    SO_CUDA_TRY(cudaSetDevice(c->device));
-    const auto t0 = std::chrono::steady_clock::now();
-    rc = reserve(c, n_surf);
-    if (!rc) rc = upload_cloud(c, surf, n_surf, stride, ioff, c->d_scan);
-    if (!rc) rc = upload_times(c, surf, n_surf, stride, toff, c->und.d_time);
-    if (rc) return rc;
-    return register_one(c, uint32_t(n_surf), pose_in, m, opts, out, t0);
-}
-
-int so_register_prefiltered_optimized(so_ctx* ctx, const double pose_in[7], const so_motion* m, const so_icp_opts* opts, so_motion_result* out) {
-    Ctx* c = reinterpret_cast<Ctx*>(ctx);
-    if (!c || !pose_in || !opts || !out) return fail(SO_ERR_ARG, "bad args");
-    int rc = check_motion(m, opts);
-    if (rc) return rc;
-    if (c->prefiltered_n == SIZE_MAX) return fail(SO_ERR_ARG, "so_register_prefiltered_optimized needs a preceding so_scan_prefilter (and nothing that reuses the scan buffers in between)");
-    SO_CUDA_TRY(cudaSetDevice(c->device));
-    const auto t0 = std::chrono::steady_clock::now();
-    const size_t n = c->prefiltered_n;
-    rc = reserve(c, n);
-    if (rc) return rc;
-    c->prefiltered_n = SIZE_MAX;
-    if (n) {
-        SO_CUDA_TRY(cudaMemcpyAsync(c->d_scan, c->d_scan_sorted, n * sizeof(float4), cudaMemcpyDeviceToDevice, c->stream));
-        // the filtered cloud's w (the VoxelGrid average of the time the extraction stored in intensity) is the time
-        SO_CUDA_TRY(cudaMemcpy2DAsync(c->und.d_time, sizeof(float), reinterpret_cast<const char*>(c->d_scan_sorted) + 12, sizeof(float4),
-                                      sizeof(float), n, cudaMemcpyDeviceToDevice, c->stream));
-    }
-    return register_one(c, uint32_t(n), pose_in, m, opts, out, t0);
-}
-
-int so_register_batch_optimized(so_ctx* ctx, const void* surf, const uint32_t* n_points, size_t n_scans, size_t stride, size_t ioff, size_t toff,
-                                const double* poses_in, const so_motion* m, const so_icp_opts* opts, so_motion_result* results) {
-    Ctx* c = reinterpret_cast<Ctx*>(ctx);
-    if (!c || !surf || !n_points || !poses_in || !m || !opts || !results || stride < 12 || toff + 4 > stride) return fail(SO_ERR_ARG, "bad args");
-    if (n_scans == 0 || n_scans > c->max_batch) return fail(SO_ERR_CAPACITY, "n_scans exceeds so_config.max_batch");
-    size_t total = 0;
-    for (size_t s = 0; s < n_scans; ++s) { if (n_points[s] > c->cfg.max_scan_points) return fail(SO_ERR_CAPACITY, "scan too large"); total += n_points[s]; }
-    std::vector<MotionState> M(n_scans);
-    for (size_t s = 0; s < n_scans; ++s) {
-        int rc = check_motion(m + s, opts);
-        if (rc) return rc;
-        M[s] = make_state(m[s]);
-    }
-    SO_CUDA_TRY(cudaSetDevice(c->device));
-    const auto t0 = std::chrono::steady_clock::now();
-    c->und.last.on = 0;                                                  // d_scan and the times no longer hold the last single scan
-    int rc = reserve(c, total);
-    if (!rc) rc = upload_times(c, surf, total, stride, toff, c->und.d_time);
-    if (!rc) rc = upload_states(c, M.data(), n_scans);
-    if (rc) return rc;
-    std::vector<so_icp_result> icp(n_scans);
-    if (stride == 16 && ioff == 12) {                                   // packed: chunked upload overlapped with the kernels
-        rc = register_core(c, c->d_scan, n_points, n_scans, poses_in, opts, icp.data(), false, surf, nullptr, nullptr, 0, 2);
-    } else {
-        rc = upload_cloud(c, surf, total, stride, ioff, c->d_scan);
-        if (!rc) rc = register_core(c, c->d_scan, n_points, n_scans, poses_in, opts, icp.data(), false, nullptr, nullptr, nullptr, 0, 2);
-    }
-    if (!rc) rc = download_states(c, M.data(), n_scans);
-    if (rc) return rc;
-    const double ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-    for (size_t s = 0; s < n_scans; ++s) {
-        icp[s].time_total_ms = ms;
-        fill_motion(icp[s], M[s], results + s);
-    }
-    return SO_OK;
-}
 
 int so_evaluate_optimized(so_ctx* ctx, const void* xyzi, size_t n, size_t stride, size_t ioff, size_t toff, const double pose[7],
                           const double motion[7], double dt, int32_t max_surface_features, double H[144], double g[12], double* cost) {
@@ -739,24 +618,14 @@ int so_evaluate_optimized(so_ctx* ctx, const void* xyzi, size_t n, size_t stride
     int rc = check_motion(&m, &o);
     if (rc) return rc;
     if (n > c->cfg.max_scan_points) return fail(SO_ERR_CAPACITY, "scan larger than so_config.max_scan_points");
-    SO_CUDA_TRY(cudaSetDevice(c->device));
-    rc = reserve(c, n);
-    if (!rc) rc = upload_cloud(c, xyzi, n, stride, ioff, c->d_scan);
-    if (!rc) rc = upload_times(c, xyzi, n, stride, toff, c->und.d_time);
-    if (rc) return rc;
-    c->last_scan_n = 0;                                                  // the stage hook leaves no registered scan behind
-    c->und.last.on = 0;
     MotionState M = make_state(m);
     M.stage = 1;
-    rc = upload_states(c, &M, 1);
-    if (rc) return rc;
-    double* sink = c->d_pose_sink;                                       // a stage evaluation appends no pose row
-    c->d_pose_sink = nullptr;
+    const uint32_t nn = uint32_t(n);
     so_icp_result r;
-    uint32_t nn = uint32_t(n);
-    rc = register_core(c, c->d_scan, &nn, 1, pose, &o, &r, false, nullptr, nullptr, nullptr, 0, 2);
-    c->d_pose_sink = sink;
-    if (!rc) rc = download_states(c, &M, 1);
+    RegisterRequest q;                                                   // a stage evaluation leaves no registered scan and no pose row
+    q.scans = xyzi; q.stride = stride; q.ioff = ioff; q.toff = toff; q.n_points = &nn; q.poses = pose; q.opts = &o;
+    q.mode = UndistortionMode::OPTIMIZED; q.motion = &M; q.sink_rows = false; q.results = &r;
+    rc = register_scans(c, q);
     if (rc) return rc;
     if (H) for (int i = 0; i < 12; ++i) for (int j = 0; j < 12; ++j) H[i * 12 + j] = M.H[i <= j ? tri12(i, j) : tri12(j, i)];
     if (g) for (int i = 0; i < 12; ++i) g[i] = M.g[i];

@@ -9,7 +9,6 @@
 // and the iteration runs on pInit in place of p (und_point, so_undistort.cuh; tests/undistort_numpy.py restates its bits).
 //   k_undistort        the ICP form: one thread per active point of the ordered scans, writes d_scan_sorted (w kept)
 //   k_undistort_cloud  a contiguous cloud at a given pose: the map insert after an undistorted registration, so_undistort_points
-#include <chrono>
 #include <cmath>
 #include <vector>
 
@@ -68,9 +67,8 @@ static void launch_undistort_cloud(Ctx* c, float4* pts, const float* times, uint
     timed_launch_end(c, 7);                                               // counts the launch
 }
 
-int undistort_tail(Ctx* c, MapStore& ms, uint32_t n_new, const double pose[7]) {
-    if (c->und.last.on == 2) return motion_tail(c, ms, n_new);       // after so_register_optimized*: u(D_opt), whatever the pose
-    launch_undistort_cloud(c, ms.d_xyzi + ms.n, c->und.d_time, n_new, c->und.last, pose);
+int undistort_tail(Ctx* c, MapStore& ms, const RegisteredScan& r, const double pose[7]) {
+    launch_undistort_cloud(c, ms.d_xyzi + ms.n, c->und.d_time, r.n, r.par, pose);
     SO_CUDA_TRY(cudaGetLastError());
     return SO_OK;
 }
@@ -85,7 +83,7 @@ bool finite_pose(const double p[7]) {
     return p[3] * p[3] + p[4] * p[4] + p[5] * p[5] + p[6] * p[6] > 0.0;
 }
 
-static int check_undistort(const so_undistort* u) {
+int check_undistort(const so_undistort* u) {
     if (!u) return fail(SO_ERR_ARG, "bad args");
     if (u->mode == 2) return fail(SO_ERR_ARG, "so_undistort.mode 2 (OPTIMIZED) estimates a second pose: use so_register_optimized");
     if (u->mode != 0 && u->mode != 1) return fail(SO_ERR_ARG, "so_undistort.mode must be 0 (NONE) or 1 (APPROXIMATED)");
@@ -96,7 +94,7 @@ static int check_undistort(const so_undistort* u) {
     return SO_OK;
 }
 
-static UndistortParams make_params(const so_undistort& u) {
+UndistortParams make_params(const so_undistort& u) {
     UndistortParams P{};
     P.on = u.mode == 1 ? 1 : 0;
     if (!P.on) return P;
@@ -118,31 +116,10 @@ int upload_times(Ctx* c, const void* src, size_t n, size_t stride, size_t toff, 
     return SO_OK;
 }
 
-static int reserve(Ctx* c, size_t n_points) {
+int undistort_reserve(Ctx* c, size_t n_points) {
     int rc = grow_buffer(c->und.d_par, c->und.par_cap, size_t(c->max_batch));
     if (!rc) rc = grow_buffer(c->und.d_time, c->und.time_cap, std::max<size_t>(n_points, 1));
     return rc;
-}
-
-static int upload_params(Ctx* c, const UndistortParams* P, size_t n) {
-    SO_CUDA_TRY(cudaMemcpyAsync(c->und.d_par, P, n * sizeof(UndistortParams), cudaMemcpyHostToDevice, c->stream));
-    count_h2d(c, n * sizeof(UndistortParams));
-    return SO_OK;
-}
-
-// The single-scan tail: the cloud (n points) is in d_scan, its times in und.d_time
-static int register_one(Ctx* c, uint32_t n, const double pose_in[7], const so_undistort* u, const so_icp_opts* opts, so_icp_result* out,
-                        std::chrono::steady_clock::time_point t0) {
-    const UndistortParams P = make_params(*u);
-    int rc = upload_params(c, &P, 1);
-    if (rc) return rc;
-    c->last_scan_n = n;
-    c->und.last = P;
-    rc = register_core(c, c->d_scan, &n, 1, pose_in, opts, out, true, nullptr, nullptr, nullptr, 0, true);
-    if (rc) return rc;
-    out->scan_edge_num = 0;
-    out->time_total_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-    return out->status;
 }
 
 }  // namespace so
@@ -150,79 +127,6 @@ static int register_one(Ctx* c, uint32_t n, const double pose_in[7], const so_un
 using namespace so;
 
 extern "C" {
-
-int so_register_undistort(so_ctx* ctx, const void* surf, size_t n_surf, size_t stride, size_t ioff, size_t toff, const double pose_in[7],
-                          const so_undistort* u, const so_icp_opts* opts, so_icp_result* out) {
-    Ctx* c = reinterpret_cast<Ctx*>(ctx);
-    if (!c || !pose_in || !opts || !out || (!surf && n_surf) || stride < 12 || toff + 4 > stride) return fail(SO_ERR_ARG, "bad args");
-    int rc = check_undistort(u);
-    if (rc) return rc;
-    if (u->mode == 0) return so_register(ctx, surf, n_surf, nullptr, 0, stride, ioff, pose_in, opts, out);
-    if (n_surf > c->cfg.max_scan_points) return fail(SO_ERR_CAPACITY, "scan larger than so_config.max_scan_points");
-    SO_CUDA_TRY(cudaSetDevice(c->device));
-    const auto t0 = std::chrono::steady_clock::now();
-    rc = reserve(c, n_surf);
-    if (!rc) rc = upload_cloud(c, surf, n_surf, stride, ioff, c->d_scan);
-    if (!rc) rc = upload_times(c, surf, n_surf, stride, toff, c->und.d_time);
-    if (rc) return rc;
-    return register_one(c, uint32_t(n_surf), pose_in, u, opts, out, t0);
-}
-
-int so_register_prefiltered_undistort(so_ctx* ctx, const double pose_in[7], const so_undistort* u, const so_icp_opts* opts, so_icp_result* out) {
-    Ctx* c = reinterpret_cast<Ctx*>(ctx);
-    if (!c || !pose_in || !opts || !out) return fail(SO_ERR_ARG, "bad args");
-    int rc = check_undistort(u);
-    if (rc) return rc;
-    if (u->mode == 0) return so_register_prefiltered(ctx, pose_in, opts, out);
-    if (c->prefiltered_n == SIZE_MAX) return fail(SO_ERR_ARG, "so_register_prefiltered_undistort needs a preceding so_scan_prefilter (and nothing that reuses the scan buffers in between)");
-    SO_CUDA_TRY(cudaSetDevice(c->device));
-    const auto t0 = std::chrono::steady_clock::now();
-    const size_t n = c->prefiltered_n;
-    rc = reserve(c, n);
-    if (rc) return rc;
-    c->prefiltered_n = SIZE_MAX;
-    if (n) {
-        SO_CUDA_TRY(cudaMemcpyAsync(c->d_scan, c->d_scan_sorted, n * sizeof(float4), cudaMemcpyDeviceToDevice, c->stream));
-        // the filtered cloud's w (the VoxelGrid average of the time the extraction stored in intensity) is the time
-        SO_CUDA_TRY(cudaMemcpy2DAsync(c->und.d_time, sizeof(float), reinterpret_cast<const char*>(c->d_scan_sorted) + 12, sizeof(float4),
-                                      sizeof(float), n, cudaMemcpyDeviceToDevice, c->stream));
-    }
-    return register_one(c, uint32_t(n), pose_in, u, opts, out, t0);
-}
-
-int so_register_batch_undistort(so_ctx* ctx, const void* surf, const uint32_t* n_points, size_t n_scans, size_t stride, size_t ioff, size_t toff,
-                                const double* poses_in, const so_undistort* u, const so_icp_opts* opts, so_icp_result* results) {
-    Ctx* c = reinterpret_cast<Ctx*>(ctx);
-    if (!c || !surf || !n_points || !poses_in || !u || !opts || !results || stride < 12 || toff + 4 > stride) return fail(SO_ERR_ARG, "bad args");
-    if (n_scans == 0 || n_scans > c->max_batch) return fail(SO_ERR_CAPACITY, "n_scans exceeds so_config.max_batch");
-    size_t total = 0;
-    for (size_t s = 0; s < n_scans; ++s) { if (n_points[s] > c->cfg.max_scan_points) return fail(SO_ERR_CAPACITY, "scan too large"); total += n_points[s]; }
-    std::vector<UndistortParams> P(n_scans);
-    bool any = false;
-    for (size_t s = 0; s < n_scans; ++s) {
-        int rc = check_undistort(u + s);
-        if (rc) return rc;
-        P[s] = make_params(u[s]);
-        any |= P[s].on != 0;
-    }
-    SO_CUDA_TRY(cudaSetDevice(c->device));
-    const auto t0 = std::chrono::steady_clock::now();
-    c->und.last.on = 0;                                                  // d_scan and the times no longer hold the last single scan
-    int rc = reserve(c, total);
-    if (!rc && any) rc = upload_times(c, surf, total, stride, toff, c->und.d_time);
-    if (!rc && any) rc = upload_params(c, P.data(), n_scans);
-    if (rc) return rc;
-    if (stride == 16 && ioff == 12) {                                   // packed: chunked upload overlapped with the kernels, as so_register_batch
-        rc = register_core(c, c->d_scan, n_points, n_scans, poses_in, opts, results, false, surf, nullptr, nullptr, 0, any);
-    } else {
-        rc = upload_cloud(c, surf, total, stride, ioff, c->d_scan);
-        if (!rc) rc = register_core(c, c->d_scan, n_points, n_scans, poses_in, opts, results, false, nullptr, nullptr, nullptr, 0, any);
-    }
-    if (rc) return rc;
-    const double ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-    for (size_t s = 0; s < n_scans; ++s) results[s].time_total_ms = ms;
-    return SO_OK;
-}
 
 int so_undistort_points(so_ctx* ctx, const void* xyzi, size_t n, size_t stride, size_t ioff, size_t toff, const double pose[7],
                         const so_undistort* u, float* out_xyzi) {
