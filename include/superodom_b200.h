@@ -156,12 +156,17 @@ int so_map_get_origin(so_ctx* ctx, int32_t out_origin[3]);
  * [3,17]x[3,17]x[3,7]; blocks rolled off the grid are dropped.  Returns the sensor block in out_ijk. */
 int so_map_shift(so_ctx* ctx, const double t_w_cur[3], int32_t out_ijk[3]);
 /* Load an ALREADY voxel-filtered world-frame surf cloud as the whole map (no filtering): replay / localization
- * mode with a prebuilt map.  Point ids (so_corr.nn) are indices into this array. */
+ * mode with a prebuilt map.  Point ids (so_corr.nn) are indices into this array.
+ * A store counts as built only once its neighbour index is: when a map change cannot build it (SO_ERR_CAPACITY: the map spans
+ * too many 50 m blocks for the cell table at this planeRes; SO_ERR_CUDA), every later call that reads the map (registration,
+ * k-NN, global localization, so_map_counts_5x5, so_map_download, so_map_shift, the inserts) returns the same error until a
+ * later change lets the index build, e.g. so_map_set_points of a smaller cloud. */
 int so_map_set_points(so_ctx* ctx, const void* xyzi, size_t n, size_t stride_bytes, size_t intensity_offset);
 /* Same for the edge clouds (MapBlock::pedge_pc_): an already lineRes-filtered world-frame edge cloud as the whole edge map. */
 int so_map_set_edge_points(so_ctx* ctx, const void* xyzi, size_t n, size_t stride_bytes, size_t intensity_offset);
 /* replaces: LocalMap::addSurfPointCloud (LocalMap.h:591-645): bin world-frame points into blocks, voxel-centroid
- * filter every touched block at leaf planeRes (pcl::VoxelGrid semantics), rebuild the neighbour index. */
+ * filter every touched block at leaf planeRes (pcl::VoxelGrid semantics), rebuild the neighbour index.  When the index cannot
+ * be built, the filtered points stay in the store and it stays unbuilt, with the rule of so_map_set_points. */
 int so_map_add_surf(so_ctx* ctx, const void* xyzi, size_t n, size_t stride_bytes, size_t intensity_offset);
 /* replaces: LocalMap::addEdgePointCloud (LocalMap.h:529-589): the same insert at leaf lineRes into the edge clouds. */
 int so_map_add_edge(so_ctx* ctx, const void* xyzi, size_t n, size_t stride_bytes, size_t intensity_offset);

@@ -94,7 +94,7 @@ static int ctx_alloc(Ctx* c) {
     SO_CUDA_TRY(cudaMalloc(&c->d_dec, size_t(kPrepareSmallCap) * sizeof(float4)));
     SO_CUDA_TRY(cudaEventCreateWithFlags(&c->ev_dec, cudaEventDisableTiming));
     SO_CUDA_TRY(cudaMalloc(&c->d_scan_sorted, c->scan_cap * sizeof(float4)));
-    SO_CUDA_TRY(cudaMalloc(&c->d_skeys, c->scan_cap * sizeof(uint64_t) + 64));      // + slack: scan_voxel_filter lays [count 16 B][heads][ranks] over it
+    SO_CUDA_TRY(cudaMalloc(&c->d_skeys, c->scan_cap * sizeof(uint64_t)));
     SO_CUDA_TRY(cudaMalloc(&c->d_skeys_out, c->scan_cap * sizeof(uint64_t)));
     SO_CUDA_TRY(cudaMalloc(&c->d_svals, c->scan_cap * sizeof(uint32_t)));
     SO_CUDA_TRY(cudaMalloc(&c->d_svals_out, c->scan_cap * sizeof(uint32_t)));
@@ -842,13 +842,11 @@ int so_map_set_resolution(so_ctx* ctx, float line_res, float plane_res) {
     if (line_res > 0 && line_res != c->edge.res) {
         const int nb_old = c->edge.nb;
         c->edge.res = line_res;
-        c->map_epoch++;
         if (map_cells_per_block(line_res) != nb_old) c->edge.dirty = true;
     }
     if (plane_res != c->surf.res) {
         const int nb_old = c->surf.nb;
         c->surf.res = plane_res;
-        c->map_epoch++;                                     // bound_d2 / plane_res live in the captured MapView
         if (map_cells_per_block(plane_res) != nb_old) c->surf.dirty = true;
     }
     return SO_OK;

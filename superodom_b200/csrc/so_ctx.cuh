@@ -118,7 +118,7 @@ struct MapStore {
     std::vector<int32_t> h_block_count, h_block_slot;   // host mirrors
     int n_slots = 0;
     int nb = 64;                                   // cells per block axis
-    bool dirty = true;
+    bool dirty = true;                             // the index is not built for the current cloud, origin and resolution
 };
 
 struct Ctx {
@@ -135,11 +135,10 @@ struct Ctx {
     uint64_t* d_keys_out = nullptr;                // [max_map]
     uint32_t* d_vals = nullptr;                    // [max_map] ids (in)
     uint32_t* d_vals_out = nullptr;                // [max_map]
-    int32_t* d_block_of_point = nullptr;           // [max_map] grid block of each raw point or -1
     void* d_cub_tmp = nullptr;
     size_t cub_tmp_bytes = 0;
-    void* d_insert_info = nullptr;                 // device-side bookkeeping of a map insert (InsertInfo + touched-block flags)
-    void* h_insert_info = nullptr;                 // pinned read-back target
+    struct MapScratch* d_map_scratch = nullptr;    // device-side bookkeeping of a store change or a scan pre-filter (so_map.cu)
+    struct InsertInfo* h_map_info = nullptr;       // pinned read-back target of its InsertInfo
 
     // ---- scans / correspondences / optimiser state -------------------------------------------------------------
     uint32_t max_batch = 1;
@@ -202,7 +201,6 @@ struct Ctx {
     };
     GraphSlot graphs[20];
     uint64_t graph_clock = 0;
-    uint64_t map_epoch = 1;
     bool force_key64 = false;                      // SO_FORCE_KEY64: test aid, take the 64-bit scan-order key path even when 32 bits suffice
     bool no_coop_knn = false;                      // SO_NO_COOP_KNN: A/B aid, always one query per thread
     bool no_small_prepare = false;                 // SO_NO_SMALL_PREPARE: A/B aid, always the device-wide scan ordering
@@ -311,7 +309,7 @@ void launch_motion_solve(int phase, const BatchView& bv, const CorrBuf& cb, cons
 // so_map.cu
 int map_alloc(Ctx* c);
 void map_free(Ctx* c);
-int map_add_points(Ctx* c, MapStore& ms, uint32_t n_new);   // ms.d_xyzi[n .. n+n_new) holds the new points: voxel-filter touched blocks, rebuild
+int map_add_points(Ctx* c, MapStore& ms, uint32_t n_new);   // ms.d_xyzi[n .. n+n_new) holds the new points: voxel-filter touched blocks, index
 int map_transform_tail(Ctx* c, MapStore& ms, uint32_t n_new, const double pose[7]);   // sensor-frame tail points -> world frame
 int scan_voxel_filter(Ctx* c, uint32_t n, float leaf, uint32_t* n_out);
 // so_scan.cu
@@ -327,7 +325,7 @@ struct DeskewParams {
 };
 void launch_deskew(float4* pts, uint32_t n, const DeskewParams& P, cudaStream_t st);
 int scan_extract_uniform(Ctx* c, uint32_t n, uint32_t skip, float block_range, int int_abs, uint32_t* n_out);   // d_scan -> d_scan_sorted   // d_scan -> d_scan_sorted (VoxelGrid on a scan)
-int map_rebuild(Ctx* c, MapStore& ms);    // (re)bin, drop off-grid points, sort, build cell table
+int map_rebuild(Ctx* c, MapStore& ms);    // (re)bin, drop off-grid points, index; the store stays dirty when it fails
 MapView map_view(const Ctx* c, const MapStore& ms);
 int map_cells_per_block(float plane_res);
 int scan_sort_alloc(Ctx* c);             // temp storage for the per-registration scan sort

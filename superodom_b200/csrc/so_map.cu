@@ -5,12 +5,16 @@
 // built by histogram + exclusive scan.  Cells have edge cs = 50/nb >= sqrt(3*planeRes): every neighbour that can
 // pass the NEIGHBORS_TOO_FAR gate lies in the 27 cells around the query's cell, and because nb divides the 50 m
 // block exactly, "same block" (LocalMap.h:488-507) is "same slot".
+//
+// Every change to a store goes through one pipeline: an optional filter stage (voxel filter of the touched blocks, drop of
+// off-grid points; filter_stage) and one index stage (block counts, slots, cell table; count_blocks + index_cells).
 #include <algorithm>
 #include <cmath>
 
 #include <cub/cub.cuh>
 
 #include "so_ctx.cuh"
+#include "so_knn.cuh"
 
 namespace so {
 
@@ -33,65 +37,36 @@ static int map_rings(float plane_res, int nb) {
     return R < 1 ? 1 : R;
 }
 
+// Device-side bookkeeping of a store change or a scan pre-filter: everything the host would otherwise read back between launches.
+struct InsertInfo {
+    uint32_t begin, end;        // sorted filter keys: [0, begin) kept in order, [begin, end) voxel-filtered, [end, total) dropped
+    uint32_t n_out;             // points of the filtered cloud (the cloud the index stage indexes)
+    uint32_t n_slots;           // non-empty blocks of that cloud
+    uint32_t n_kept;            // its points on the grid
+    uint32_t error;             // 1: more slots than the cell table was sized for
+    uint32_t overflow;          // scan pre-filter: a voxel index beyond the narrow key
+    uint32_t pad;
+};
+struct MapScratch {
+    InsertInfo info;
+    uint8_t touched[kNumBlocks];                                     // blocks the new points of an insert reach
+};
+
+constexpr size_t kMaxCells = size_t(1) << 31;      // cell indices are 32-bit in the kernels and the scan length is an int
+
 __device__ __forceinline__ int block_coord(double v, int origin) {   // LocalMap.h:594-605
     int c = int(v / kBlock);
     if (v < 0) c--;
     return c + origin;
 }
 
-__global__ void k_block_of(const float4* __restrict__ raw, uint32_t n, int3 origin, int32_t* __restrict__ block_of_point,
-                           int32_t* __restrict__ block_count) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const float4 p = raw[i];
-    const int gx = block_coord(double(p.x) + kHalfBlock, origin.x);
-    const int gy = block_coord(double(p.y) + kHalfBlock, origin.y);
-    const int gz = block_coord(double(p.z) + kHalfBlock, origin.z);
-    int lin = -1;
-    if (gx >= 0 && gx < kW && gy >= 0 && gy < kH && gz >= 0 && gz < kD && isfinite(p.x) && isfinite(p.y) && isfinite(p.z)) {
-        lin = gx + kW * gy + kW * kH * gz;
-        atomicAdd(&block_count[lin], 1);
-    }
-    block_of_point[i] = lin;
-}
-
-__global__ void k_flags(const int32_t* __restrict__ block_of_point, uint32_t n, uint8_t* __restrict__ flags) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) flags[i] = block_of_point[i] >= 0;
-}
-
-__global__ void k_keys(const float4* __restrict__ raw, uint32_t n, int3 origin, const int32_t* __restrict__ block_slot,
-                       int nb, double inv_cs, uint64_t* __restrict__ keys, uint32_t* __restrict__ vals,
-                       uint32_t* __restrict__ cell_count) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const float4 p = raw[i];
-    const float q[3] = {p.x, p.y, p.z};
-    const int o[3] = {origin.x, origin.y, origin.z};
-    int g[3], c[3];
-#pragma unroll
-    for (int a = 0; a < 3; ++a) {
-        const double v = double(q[a]) + kHalfBlock;
-        int b = int(v / kBlock);
-        if (v < 0) b--;
-        g[a] = b + o[a];
-        int cc = int((v - kBlock * double(b)) * inv_cs);
-        c[a] = cc < 0 ? 0 : (cc > nb - 1 ? nb - 1 : cc);
-    }
-    const int lin = g[0] + kW * g[1] + kW * kH * g[2];
-    const uint64_t slot = uint64_t(block_slot[lin]);
-    const uint64_t key = slot * uint64_t(nb) * uint64_t(nb) * uint64_t(nb) + uint64_t((c[2] * nb + c[1]) * nb + c[0]);
-    keys[i] = key;
-    vals[i] = i;
-    atomicAdd(&cell_count[key], 1u);
-}
-
-__global__ void k_gather(const float4* __restrict__ raw, const uint32_t* __restrict__ vals, uint32_t n, float4* __restrict__ sorted) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const uint32_t id = vals[i];
-    const float4 p = raw[id];
-    sorted[i] = make_float4(p.x, p.y, p.z, __uint_as_float(id));
+// Linear grid block of a point under `origin`, or -1 when the block is off the 21 x 21 x 11 grid or the point is not finite
+__device__ __forceinline__ int grid_block(const float4 p, int3 origin) {
+    const int gx = block_coord(double(p.x) + kHalfBlock, origin.x), gy = block_coord(double(p.y) + kHalfBlock, origin.y),
+              gz = block_coord(double(p.z) + kHalfBlock, origin.z);
+    if (gx >= 0 && gx < kW && gy >= 0 && gy < kH && gz >= 0 && gz < kD && isfinite(p.x) && isfinite(p.y) && isfinite(p.z))
+        return gx + kW * gy + kW * kH * gz;
+    return -1;
 }
 
 static int store_alloc(Ctx* c, MapStore& ms) {
@@ -117,17 +92,15 @@ int map_alloc(Ctx* c) {
     SO_CUDA_TRY(cudaMalloc(&c->d_keys_out, M * sizeof(uint64_t)));
     SO_CUDA_TRY(cudaMalloc(&c->d_vals, M * sizeof(uint32_t)));
     SO_CUDA_TRY(cudaMalloc(&c->d_vals_out, M * sizeof(uint32_t)));
-    SO_CUDA_TRY(cudaMalloc(&c->d_block_of_point, M * sizeof(int32_t)));
-    // cub temp: the larger of sort / scan / select requirements at full capacity
-    size_t a = 0, b = 0, d = 0;
+    // cub temp: the 64-bit filter sort (the 32-bit cell sort needs less) and the scan of its voxel heads at full capacity;
+    // reserve_cells grows it for the scan of the cell table
+    size_t a = 0, b = 0;
     cub::DeviceRadixSort::SortPairs(nullptr, a, c->d_keys, c->d_keys_out, c->d_vals, c->d_vals_out, int(M), 0, 64);
-    cub::DeviceSelect::Flagged(nullptr, d, c->surf.d_xyzi, (uint8_t*)nullptr, c->surf.d_sorted, (uint32_t*)nullptr, int(M));
-    const size_t max_cells = size_t(64) * 128 * 128 * 128 + 1;     // scan temp is tiny; size for a generous table
-    cub::DeviceScan::ExclusiveSum(nullptr, b, (uint32_t*)nullptr, (uint32_t*)nullptr, int(std::min<size_t>(max_cells, size_t(1) << 30)));
-    c->cub_tmp_bytes = std::max(a, std::max(b, d)) + 256;
+    cub::DeviceScan::ExclusiveSum(nullptr, b, (uint32_t*)nullptr, (uint32_t*)nullptr, int(M));
+    c->cub_tmp_bytes = std::max(a, b) + 256;
     SO_CUDA_TRY(cudaMalloc(&c->d_cub_tmp, c->cub_tmp_bytes));
-    SO_CUDA_TRY(cudaMalloc(&c->d_insert_info, 8192));
-    SO_CUDA_TRY(cudaMallocHost(&c->h_insert_info, 256));
+    SO_CUDA_TRY(cudaMalloc(&c->d_map_scratch, sizeof(MapScratch)));
+    SO_CUDA_TRY(cudaMallocHost(&c->h_map_info, sizeof(InsertInfo)));
     return SO_OK;
 }
 
@@ -135,9 +108,9 @@ void map_free(Ctx* c) {
     for (MapStore* ms : {&c->surf, &c->edge}) {
         cudaFree(ms->d_xyzi); cudaFree(ms->d_sorted); cudaFree(ms->d_block_slot); cudaFree(ms->d_block_count); cudaFree(ms->d_cell_start);
     }
-    cudaFree(c->d_keys); cudaFree(c->d_keys_out); cudaFree(c->d_vals); cudaFree(c->d_vals_out); cudaFree(c->d_block_of_point); cudaFree(c->d_cub_tmp);
-    cudaFree(c->d_insert_info);
-    if (c->h_insert_info) cudaFreeHost(c->h_insert_info);
+    cudaFree(c->d_keys); cudaFree(c->d_keys_out); cudaFree(c->d_vals); cudaFree(c->d_vals_out); cudaFree(c->d_cub_tmp);
+    cudaFree(c->d_map_scratch);
+    if (c->h_map_info) cudaFreeHost(c->h_map_info);
 }
 
 MapView map_view(const Ctx* c, const MapStore& ms) {
@@ -150,76 +123,6 @@ MapView map_view(const Ctx* c, const MapStore& ms) {
     m.plane_res = ms.res;
     m.R = map_rings(ms.res, ms.nb);
     return m;
-}
-
-// (Re)build the index from d_map_xyzi[0..map_n): bin to blocks under the current origin, drop off-grid points
-// (what LocalMap::shiftMap does to blocks rolled off the grid, LocalMap.h:169-287), sort, build the cell table.
-int map_rebuild(Ctx* c, MapStore& ms) {
-    cudaStream_t st = c->stream;
-    ms.nb = map_cells_per_block(ms.res);
-    c->map_epoch++;
-    ms.dirty = false;
-    const int3 origin = make_int3(c->origin[0], c->origin[1], c->origin[2]);
-    SO_CUDA_TRY(cudaMemsetAsync(ms.d_block_count, 0, kNumBlocks * sizeof(int32_t), st));
-    std::fill(ms.h_block_count.begin(), ms.h_block_count.end(), 0);
-    std::fill(ms.h_block_slot.begin(), ms.h_block_slot.end(), -1);
-    ms.n_slots = 0;
-    if (ms.n == 0) {
-        SO_CUDA_TRY(cudaMemsetAsync(ms.d_block_slot, 0xFF, kNumBlocks * sizeof(int32_t), st));
-        SO_CUDA_TRY(cudaStreamSynchronize(st));
-        return SO_OK;
-    }
-    const uint32_t n = ms.n;
-    const uint32_t grid = (n + 255) / 256;
-    k_block_of<<<grid, 256, 0, st>>>(ms.d_xyzi, n, origin, c->d_block_of_point, ms.d_block_count);
-    c->launches++;
-    SO_CUDA_TRY(cudaMemcpyAsync(ms.h_block_count.data(), ms.d_block_count, kNumBlocks * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-    SO_CUDA_TRY(cudaStreamSynchronize(st));
-    uint64_t kept = 0;
-    for (int b = 0; b < kNumBlocks; ++b) if (ms.h_block_count[b] > 0) { ms.h_block_slot[b] = ms.n_slots++; kept += uint64_t(ms.h_block_count[b]); }
-    SO_CUDA_TRY(cudaMemcpyAsync(ms.d_block_slot, ms.h_block_slot.data(), kNumBlocks * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-    if (kept < n) {
-        // compact away the points whose block rolled off the grid, preserving order (ids are ranks in this order)
-        uint8_t* flags = reinterpret_cast<uint8_t*>(c->d_vals_out);
-        uint32_t* d_num = reinterpret_cast<uint32_t*>(c->d_keys_out);
-        k_flags<<<grid, 256, 0, st>>>(c->d_block_of_point, n, flags);
-        size_t tmp = c->cub_tmp_bytes;
-        SO_CUDA_TRY(cub::DeviceSelect::Flagged(c->d_cub_tmp, tmp, ms.d_xyzi, flags, ms.d_sorted, d_num, int(n), st));
-        SO_CUDA_TRY(cudaMemcpyAsync(ms.d_xyzi, ms.d_sorted, kept * sizeof(float4), cudaMemcpyDeviceToDevice, st));
-        c->launches += 3;
-        ms.n = uint32_t(kept);
-    }
-    if (kept == 0) { SO_CUDA_TRY(cudaStreamSynchronize(st)); return SO_OK; }
-    const uint32_t m = ms.n;
-    const size_t cells = size_t(ms.n_slots) * ms.nb * ms.nb * ms.nb;
-    if (cells + 1 >= (size_t(1) << 31)) {          // cell indices are 32-bit in the kernels and the scan length is an int
-        SO_CUDA_TRY(cudaStreamSynchronize(st));
-        set_error("map spans too many 50 m blocks for the dense cell table (n_slots * nb^3 >= 2^31)");
-        return SO_ERR_CAPACITY;
-    }
-    if (cells + 1 > ms.cell_cap) {
-        SO_CUDA_TRY(cudaStreamSynchronize(st));
-        int rc = grow_buffer(ms.d_cell_start, ms.cell_cap, cells + 1 + cells / 4);
-        if (rc) return rc;
-        size_t need = 0;
-        cub::DeviceScan::ExclusiveSum(nullptr, need, ms.d_cell_start, ms.d_cell_start, int(ms.cell_cap));
-        rc = grow_buffer(c->d_cub_tmp, c->cub_tmp_bytes, need + 256);
-        if (rc) return rc;
-    }
-    SO_CUDA_TRY(cudaMemsetAsync(ms.d_cell_start, 0, (cells + 1) * sizeof(uint32_t), st));
-    const uint32_t g2 = (m + 255) / 256;
-    k_keys<<<g2, 256, 0, st>>>(ms.d_xyzi, m, origin, ms.d_block_slot, ms.nb, double(ms.nb) / kBlock, c->d_keys, c->d_vals, ms.d_cell_start);
-    int bits = 1;
-    while ((uint64_t(1) << bits) < uint64_t(cells)) ++bits;
-    size_t tmp = c->cub_tmp_bytes;
-    SO_CUDA_TRY(cub::DeviceRadixSort::SortPairs(c->d_cub_tmp, tmp, c->d_keys, c->d_keys_out, c->d_vals, c->d_vals_out, int(m), 0, bits, st));
-    k_gather<<<g2, 256, 0, st>>>(ms.d_xyzi, c->d_vals_out, m, ms.d_sorted);
-    tmp = c->cub_tmp_bytes;
-    SO_CUDA_TRY(cub::DeviceScan::ExclusiveSum(c->d_cub_tmp, tmp, ms.d_cell_start, ms.d_cell_start, int(cells + 1), st));
-    c->launches += 8;
-    SO_CUDA_TRY(cudaGetLastError());
-    SO_CUDA_TRY(cudaStreamSynchronize(st));
-    return SO_OK;
 }
 
 int scan_sort_alloc(Ctx* c) {
@@ -264,71 +167,6 @@ int scan_sort(Ctx* c, size_t first, size_t n, int n_scans, int cell_bits, bool k
     return SO_OK;
 }
 
-// ------------------------------------------------------------------------------------------------------------------
-// Map insert: LocalMap::addSurfPointCloud (LocalMap.h:591-645).  New world-frame points are appended, every block they
-// touch is re-filtered as a whole by a voxel-centroid filter of leaf planeRes_ (pcl::VoxelGrid semantics: voxel =
-// floor(coord * (1.0f/leaf)) in float32, centroid of all four fields accumulated in float32 and divided by
-// float(count), output ordered by voxel index (k, j, i)), untouched blocks keep their clouds.  PCL leaves the in-voxel
-// accumulation order unspecified (std::sort on the voxel index); here it is ascending cloud order (old points, then
-// new points in input order), the order the stable radix sort preserves.
-// ------------------------------------------------------------------------------------------------------------------
-__global__ void k_mark_touched(const int32_t* __restrict__ block_of_point, uint32_t first_new, uint32_t n, uint8_t* __restrict__ touched) {
-    const uint32_t i = first_new + blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n && block_of_point[i] >= 0) touched[block_of_point[i]] = 1;
-}
-
-// Sort key of the insert: [63] touched flag | [48..60] grid block (13 bits: 0..4850) | 3 x 16 bits of BLOCK-LOCAL voxel index (k, j, i).
-// PCL orders a block's output by the voxel index relative to the block cloud's bounding box; subtracting any per-block constant
-// keeps that order, so the index is taken relative to the block's minimum corner (minus a 2-voxel guard for the float rounding of
-// x * inv_leaf at the faces): 50 m / leaf + 4 values per axis -- 16 bits hold leaf >= 1 mm, wherever the block is in the world.
-__global__ void k_voxel_keys(const float4* __restrict__ raw, const int32_t* __restrict__ block_of_point, const uint8_t* __restrict__ touched,
-                             uint32_t n, float inv_leaf, int3 origin, uint64_t* __restrict__ keys, uint32_t* __restrict__ vals) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const int32_t b = block_of_point[i];
-    uint64_t key;
-    if (b < 0) key = ~uint64_t(0);                                  // off-grid: dropped
-    else if (!touched[b]) key = 0;                                  // untouched block: keep, in place (stable sort)
-    else {
-        const float4 p = raw[i];
-        const int gx = b % kW, gy = (b / kW) % kH, gz = b / (kW * kH);
-        const double il = double(inv_leaf);
-        const int64_t bx = int64_t(floor((double(gx - origin.x) * kBlock - kHalfBlock) * il)) - 2;
-        const int64_t by = int64_t(floor((double(gy - origin.y) * kBlock - kHalfBlock) * il)) - 2;
-        const int64_t bz = int64_t(floor((double(gz - origin.z) * kBlock - kHalfBlock) * il)) - 2;
-        auto local = [](int64_t v) { return uint64_t(v < 0 ? 0 : (v > 65535 ? 65535 : v)); };
-        const uint64_t vi = local(int64_t(floorf(__fmul_rn(p.x, inv_leaf))) - bx);      // pcl::VoxelGrid: floor(coord * inverse_leaf_size) in float
-        const uint64_t vj = local(int64_t(floorf(__fmul_rn(p.y, inv_leaf))) - by);
-        const uint64_t vk = local(int64_t(floorf(__fmul_rn(p.z, inv_leaf))) - bz);
-        key = (uint64_t(1) << 63) | (uint64_t(b) << 48) | (vk << 32) | (vj << 16) | vi;
-    }
-    keys[i] = key;
-    vals[i] = i;
-}
-
-__global__ void k_voxel_heads(const uint64_t* __restrict__ keys, uint32_t begin, uint32_t end, uint32_t* __restrict__ head) {
-    const uint32_t i = begin + blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < end) head[i - begin] = (i == begin || keys[i] != keys[i - 1]) ? 1u : 0u;
-}
-
-__global__ void k_voxel_centroid(const float4* __restrict__ raw, const uint64_t* __restrict__ keys, const uint32_t* __restrict__ vals,
-                                 const uint32_t* __restrict__ rank, uint32_t begin, uint32_t end, float4* __restrict__ out) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < begin) { out[i] = raw[vals[i]]; return; }               // untouched blocks: copied through in order
-    if (i >= end) return;
-    if (!(i == begin || keys[i] != keys[i - 1])) return;             // not a voxel head
-    const uint64_t key = keys[i];
-    float ax = 0.f, ay = 0.f, az = 0.f, aw = 0.f;
-    uint32_t cnt = 0;
-    for (uint32_t j = i; j < end && keys[j] == key; ++j) {           // pcl::CentroidPoint: float accumulators, cloud order
-        const float4 p = raw[vals[j]];
-        ax = __fadd_rn(ax, p.x); ay = __fadd_rn(ay, p.y); az = __fadd_rn(az, p.z); aw = __fadd_rn(aw, p.w);
-        ++cnt;
-    }
-    const float nf = float(cnt);
-    out[begin + rank[i - begin]] = make_float4(__fdiv_rn(ax, nf), __fdiv_rn(ay, nf), __fdiv_rn(az, nf), __fdiv_rn(aw, nf));
-}
-
 struct Pose7 { double v[7]; };
 __global__ void k_transform_points(float4* __restrict__ pts, uint32_t n, Pose7 pose) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -349,90 +187,98 @@ int map_transform_tail(Ctx* c, MapStore& ms, uint32_t n_new, const double pose[7
     return SO_OK;
 }
 
-static int map_add_points_sync(Ctx* c, MapStore& ms, uint32_t n_new) {
-    cudaStream_t st = c->stream;
-    const uint32_t total = ms.n + n_new;
-    if (n_new == 0) return SO_OK;
-    const int3 origin = make_int3(c->origin[0], c->origin[1], c->origin[2]);
-    const uint32_t grid = (total + 255) / 256;
-    uint8_t* d_touched = reinterpret_cast<uint8_t*>(c->d_vals_out);          // scratch: 4851 bytes
-    SO_CUDA_TRY(cudaMemsetAsync(ms.d_block_count, 0, kNumBlocks * sizeof(int32_t), st));
-    SO_CUDA_TRY(cudaMemsetAsync(d_touched, 0, kNumBlocks, st));
-    k_block_of<<<grid, 256, 0, st>>>(ms.d_xyzi, total, origin, c->d_block_of_point, ms.d_block_count);
-    k_mark_touched<<<(n_new + 255) / 256, 256, 0, st>>>(c->d_block_of_point, ms.n, total, d_touched);
-    std::vector<uint8_t> h_touched(kNumBlocks);
-    SO_CUDA_TRY(cudaMemcpyAsync(ms.h_block_count.data(), ms.d_block_count, kNumBlocks * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-    SO_CUDA_TRY(cudaMemcpyAsync(h_touched.data(), d_touched, kNumBlocks, cudaMemcpyDeviceToHost, st));
-    SO_CUDA_TRY(cudaStreamSynchronize(st));
-    uint64_t n_untouched = 0, n_touched = 0;
-    for (int b = 0; b < kNumBlocks; ++b) (h_touched[b] ? n_touched : n_untouched) += uint64_t(ms.h_block_count[b]);
-    // keys need the touched flags: keep them in a scratch that the sort does not use
-    uint8_t* d_touched2 = reinterpret_cast<uint8_t*>(c->d_cub_tmp);
-    SO_CUDA_TRY(cudaMemcpyAsync(d_touched2, h_touched.data(), kNumBlocks, cudaMemcpyHostToDevice, st));
-    const float inv_leaf = 1.0f / ms.res;                               // Eigen::Array4f::Ones() / leaf_size_
-    k_voxel_keys<<<grid, 256, 0, st>>>(ms.d_xyzi, c->d_block_of_point, d_touched2, total, inv_leaf, origin, c->d_keys, c->d_vals);
-    SO_CUDA_TRY(cudaStreamSynchronize(st));                                   // d_cub_tmp is reused by the sort next
-    size_t tmp = c->cub_tmp_bytes;
-    SO_CUDA_TRY(cub::DeviceRadixSort::SortPairs(c->d_cub_tmp, tmp, c->d_keys, c->d_keys_out, c->d_vals, c->d_vals_out, int(total), 0, 64, st));
-    const uint32_t begin = uint32_t(n_untouched), end = uint32_t(n_untouched + n_touched);
-    uint32_t n_vox = 0;
-    uint32_t* d_head = reinterpret_cast<uint32_t*>(c->d_keys);               // keys_in is free after the sort
-    if (n_touched) {
-        k_voxel_heads<<<(uint32_t(n_touched) + 255) / 256, 256, 0, st>>>(c->d_keys_out, begin, end, d_head);
-        uint32_t last_flag = 0, last_rank = 0;
-        tmp = c->cub_tmp_bytes;
-        uint32_t* d_rank = d_head + n_touched;                                // second half of the same scratch (8 B/pt available)
-        SO_CUDA_TRY(cub::DeviceScan::ExclusiveSum(c->d_cub_tmp, tmp, d_head, d_rank, int(n_touched), st));
-        SO_CUDA_TRY(cudaMemcpyAsync(&last_flag, d_head + n_touched - 1, 4, cudaMemcpyDeviceToHost, st));
-        SO_CUDA_TRY(cudaMemcpyAsync(&last_rank, d_rank + n_touched - 1, 4, cudaMemcpyDeviceToHost, st));
-        SO_CUDA_TRY(cudaStreamSynchronize(st));
-        n_vox = last_rank + last_flag;
-        k_voxel_centroid<<<(end + 255) / 256, 256, 0, st>>>(ms.d_xyzi, c->d_keys_out, c->d_vals_out, d_rank, begin, end, ms.d_sorted);
-    } else if (begin) {
-        k_voxel_centroid<<<(begin + 255) / 256, 256, 0, st>>>(ms.d_xyzi, c->d_keys_out, c->d_vals_out, nullptr, begin, begin, ms.d_sorted);
-    }
-    ms.n = begin + n_vox;
-    if (ms.n) SO_CUDA_TRY(cudaMemcpyAsync(ms.d_xyzi, ms.d_sorted, size_t(ms.n) * sizeof(float4), cudaMemcpyDeviceToDevice, st));
-    c->launches += 12;
-    SO_CUDA_TRY(cudaGetLastError());
-    return map_rebuild(c, ms);
+// ------------------------------------------------------------------------------------------------------------------
+// Voxel reduction shared by the map's filter stage and the scan pre-filter: pcl::VoxelGrid semantics (voxel =
+// floor(coord * (1.0f/leaf)) in float32, centroid of all four fields accumulated in float32 and divided by float(count), output
+// ordered by voxel index).  PCL leaves the in-voxel accumulation order unspecified (std::sort on the voxel index); here it is
+// ascending cloud order, the order the stable radix sort preserves.  Sorted keys below t_voxel are copied through in order, keys
+// in [t_voxel, t_drop) are averaged voxel by voxel, keys from t_drop on are dropped.
+// ------------------------------------------------------------------------------------------------------------------
+// boundaries of the three key classes in the sorted keys, by binary search (one thread)
+__global__ void k_voxel_bounds(const uint64_t* __restrict__ keys, uint32_t total, uint64_t t_voxel, uint64_t t_drop, InsertInfo* __restrict__ info) {
+    if (threadIdx.x || blockIdx.x) return;
+    uint32_t lo = 0, hi = total;
+    while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (keys[mid] >= t_voxel) hi = mid; else lo = mid + 1; }      // first filtered key
+    info->begin = lo;
+    hi = total;
+    while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (keys[mid] >= t_drop) hi = mid; else lo = mid + 1; }       // first dropped key
+    info->end = lo;
 }
 
-// Device-side bookkeeping of an insert: everything the host used to read back between launches.
-struct InsertInfo {
-    uint32_t begin, end;        // sorted insert keys: [0, begin) untouched blocks, [begin, end) touched blocks, [end, total) dropped
-    uint32_t n_out;             // points of the new cloud
-    uint32_t n_slots;           // non-empty blocks of the new cloud
-    uint32_t error;             // 1: cell table capacity exceeded
-    uint32_t pad[3];
-};
+__global__ void k_voxel_heads(const uint64_t* __restrict__ keys, uint32_t total, const InsertInfo* __restrict__ info, uint32_t* __restrict__ head) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= total) return;
+    head[i] = (i >= info->begin && i < info->end && (i == info->begin || keys[i] != keys[i - 1])) ? 1u : 0u;
+}
 
+// rank[] = exclusive scan of head[] over [0, total): rank[i] counts the voxels before sorted position i
+__global__ void k_voxel_centroid(const float4* __restrict__ raw, const uint64_t* __restrict__ keys, const uint32_t* __restrict__ vals,
+                                 const uint32_t* __restrict__ head, const uint32_t* __restrict__ rank, uint32_t total, InsertInfo* __restrict__ info,
+                                 float4* __restrict__ out) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= total) return;
+    const uint32_t begin = info->begin, end = info->end;
+    if (i == total - 1) info->n_out = begin + rank[i] + head[i];      // voxels in total
+    if (i < begin) { out[i] = raw[vals[i]]; return; }                   // kept points: copied through in order
+    if (i >= end || !head[i]) return;
+    const uint64_t key = keys[i];
+    float ax = 0.f, ay = 0.f, az = 0.f, aw = 0.f;
+    uint32_t cnt = 0;
+    for (uint32_t j = i; j < end && keys[j] == key; ++j) {             // pcl::CentroidPoint: float accumulators, cloud order
+        const float4 p = raw[vals[j]];
+        ax = __fadd_rn(ax, p.x); ay = __fadd_rn(ay, p.y); az = __fadd_rn(az, p.z); aw = __fadd_rn(aw, p.w);
+        ++cnt;
+    }
+    const float nf = float(cnt);
+    out[begin + rank[i]] = make_float4(__fdiv_rn(ax, nf), __fdiv_rn(ay, nf), __fdiv_rn(az, nf), __fdiv_rn(aw, nf));
+}
+
+// raw[0..total) sorted by keys / vals -> out[0..info->n_out); head: scratch of 2 * total words (heads, then ranks)
+static int voxel_reduce(Ctx* c, const float4* raw, const uint64_t* keys, const uint32_t* vals, uint32_t total, uint64_t t_voxel, uint64_t t_drop,
+                        uint32_t* head, void* tmp, size_t tmp_bytes, float4* out) {
+    cudaStream_t st = c->stream;
+    InsertInfo* d_info = &c->d_map_scratch->info;
+    const uint32_t grid = (total + 255) / 256;
+    uint32_t* rank = head + total;
+    k_voxel_bounds<<<1, 32, 0, st>>>(keys, total, t_voxel, t_drop, d_info);
+    k_voxel_heads<<<grid, 256, 0, st>>>(keys, total, d_info, head);
+    SO_CUDA_TRY(cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, head, rank, int(total), st));
+    k_voxel_centroid<<<grid, 256, 0, st>>>(raw, keys, vals, head, rank, total, d_info, out);
+    c->launches += 5;
+    return SO_OK;
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// Filter stage: LocalMap::addSurfPointCloud (LocalMap.h:591-645).  New world-frame points are appended, every block they
+// touch is re-filtered as a whole by a voxel-centroid filter of leaf planeRes_ (output ordered by voxel index (k, j, i)),
+// untouched blocks keep their clouds, points off the grid (what LocalMap::shiftMap does to blocks rolled off it,
+// LocalMap.h:169-287) are dropped.  The in-voxel accumulation order is old points, then new points in input order.
+// ------------------------------------------------------------------------------------------------------------------
 __global__ void k_mark_touched_new(const float4* __restrict__ pts, uint32_t n_new, int3 origin, uint8_t* __restrict__ touched) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n_new) return;
-    const float4 p = pts[i];
-    const int gx = block_coord(double(p.x) + kHalfBlock, origin.x), gy = block_coord(double(p.y) + kHalfBlock, origin.y),
-              gz = block_coord(double(p.z) + kHalfBlock, origin.z);
-    if (gx >= 0 && gx < kW && gy >= 0 && gy < kH && gz >= 0 && gz < kD && isfinite(p.x) && isfinite(p.y) && isfinite(p.z))
-        touched[gx + kW * gy + kW * kH * gz] = 1;
+    const int b = grid_block(pts[i], origin);
+    if (b >= 0) touched[b] = 1;
 }
 
 // insert key of every point (old cloud followed by the new points), the block recomputed from the coordinates:
 // [class: 0 untouched block, 1 touched, 2 dropped][block 13 bits][vk][vj][vi], vb bits per block-local voxel index (50 m / leaf + 5
-// values: 8 bits at leaf 0.2) -- 39 key bits = 5 radix passes instead of the 8 of a full 64-bit key
+// values: 8 bits at leaf 0.2) -- 39 key bits = 5 radix passes instead of the 8 of a full 64-bit key.
+// PCL orders a block's output by the voxel index relative to the block cloud's bounding box; subtracting any per-block constant
+// keeps that order, so the index is taken relative to the block's minimum corner (minus a 2-voxel guard for the float rounding of
+// x * inv_leaf at the faces).
 __global__ void k_insert_keys(const float4* __restrict__ raw, uint32_t n, float inv_leaf, int3 origin, const uint8_t* __restrict__ touched,
                               int vb, uint64_t* __restrict__ keys, uint32_t* __restrict__ vals) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const float4 p = raw[i];
-    const int gx = block_coord(double(p.x) + kHalfBlock, origin.x), gy = block_coord(double(p.y) + kHalfBlock, origin.y),
-              gz = block_coord(double(p.z) + kHalfBlock, origin.z);
+    const int b = grid_block(p, origin);
     const int cls_shift = 13 + 3 * vb;
     uint64_t key = uint64_t(2) << cls_shift;                              // off-grid / non-finite: dropped
-    if (gx >= 0 && gx < kW && gy >= 0 && gy < kH && gz >= 0 && gz < kD && isfinite(p.x) && isfinite(p.y) && isfinite(p.z)) {
-        const int b = gx + kW * gy + kW * kH * gz;
+    if (b >= 0) {
         if (!touched[b]) key = 0;                                         // untouched block: kept in place (stable sort)
         else {
+            const int gx = b % kW, gy = (b / kW) % kH, gz = b / (kW * kH);
             const double il = double(inv_leaf);
             const int64_t bx = int64_t(floor((double(gx - origin.x) * kBlock - kHalfBlock) * il)) - 2;
             const int64_t by = int64_t(floor((double(gy - origin.y) * kBlock - kHalfBlock) * il)) - 2;
@@ -449,72 +295,57 @@ __global__ void k_insert_keys(const float4* __restrict__ raw, uint32_t n, float 
     vals[i] = i;
 }
 
-// boundaries of the three key classes in the sorted keys, by binary search (one thread)
-__global__ void k_insert_bounds(const uint64_t* __restrict__ keys, uint32_t total, int cls_shift, InsertInfo* __restrict__ info) {
-    if (threadIdx.x || blockIdx.x) return;
-    uint32_t lo = 0, hi = total;
-    while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if ((keys[mid] >> cls_shift) >= 1) hi = mid; else lo = mid + 1; }      // first touched key
-    info->begin = lo;
-    hi = total;
-    while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if ((keys[mid] >> cls_shift) >= 2) hi = mid; else lo = mid + 1; }      // first dropped key
-    info->end = lo;
-    info->error = 0;
+// d_xyzi[0..ms.n + n_new) (the store's cloud, then n_new new points) -> the filtered cloud in d_xyzi[0..info->n_out); the two cloud
+// buffers swap roles (no device-to-device copy of the map).  n_new == 0: nothing is touched, only the off-grid points are dropped
+// (the sort then runs over the two class bits alone).
+static int filter_stage(Ctx* c, MapStore& ms, uint32_t n_new) {
+    cudaStream_t st = c->stream;
+    const uint32_t total = ms.n + n_new;
+    const int3 origin = make_int3(c->origin[0], c->origin[1], c->origin[2]);
+    uint8_t* d_touched = c->d_map_scratch->touched;
+    SO_CUDA_TRY(cudaMemsetAsync(d_touched, 0, kNumBlocks, st));
+    if (n_new) k_mark_touched_new<<<(n_new + 255) / 256, 256, 0, st>>>(ms.d_xyzi + ms.n, n_new, origin, d_touched);
+    const float inv_leaf = 1.0f / ms.res;                               // Eigen::Array4f::Ones() / leaf_size_
+    int vb = 1;                                                         // bits of a block-local voxel index: 50 m / leaf + 5 values
+    while (vb < 16 && double(1 << vb) < kBlock * double(inv_leaf) + 5.0) ++vb;
+    const int cls_shift = 13 + 3 * vb;
+    k_insert_keys<<<(total + 255) / 256, 256, 0, st>>>(ms.d_xyzi, total, inv_leaf, origin, d_touched, vb, c->d_keys, c->d_vals);
+    size_t tmp = c->cub_tmp_bytes;
+    SO_CUDA_TRY(cub::DeviceRadixSort::SortPairs(c->d_cub_tmp, tmp, c->d_keys, c->d_keys_out, c->d_vals, c->d_vals_out, int(total),
+                                                n_new ? 0 : cls_shift, cls_shift + 2, st));
+    c->launches += 8;
+    const int rc = voxel_reduce(c, ms.d_xyzi, c->d_keys_out, c->d_vals_out, total, uint64_t(1) << cls_shift, uint64_t(2) << cls_shift,
+                                reinterpret_cast<uint32_t*>(c->d_keys), c->d_cub_tmp, c->cub_tmp_bytes, ms.d_sorted);   // keys_in is free after the sort
+    std::swap(ms.d_xyzi, ms.d_sorted);                                  // d_xyzi: the new cloud in id order; d_sorted: free for the new index
+    return rc;
 }
 
-__global__ void k_voxel_heads_dev(const uint64_t* __restrict__ keys, uint32_t total, const InsertInfo* __restrict__ info, uint32_t* __restrict__ head) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= total) return;
-    head[i] = (i >= info->begin && i < info->end && (i == info->begin || keys[i] != keys[i - 1])) ? 1u : 0u;
-}
-
-// rank[] = exclusive scan of head[] over [0, total): rank[i] counts the voxels before sorted position i
-__global__ void k_voxel_centroid_dev(const float4* __restrict__ raw, const uint64_t* __restrict__ keys, const uint32_t* __restrict__ vals,
-                                     const uint32_t* __restrict__ head, const uint32_t* __restrict__ rank, uint32_t total, InsertInfo* __restrict__ info,
-                                     float4* __restrict__ out) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= total) return;
-    const uint32_t begin = info->begin, end = info->end;
-    if (i == total - 1) info->n_out = begin + rank[i] + head[i];      // voxels in total
-    if (i < begin) { out[i] = raw[vals[i]]; return; }                   // untouched blocks: copied through in order
-    if (i >= end || !head[i]) return;
-    const uint64_t key = keys[i];
-    float ax = 0.f, ay = 0.f, az = 0.f, aw = 0.f;
-    uint32_t cnt = 0;
-    for (uint32_t j = i; j < end && keys[j] == key; ++j) {             // pcl::CentroidPoint: float accumulators, cloud order
-        const float4 p = raw[vals[j]];
-        ax = __fadd_rn(ax, p.x); ay = __fadd_rn(ay, p.y); az = __fadd_rn(az, p.z); aw = __fadd_rn(aw, p.w);
-        ++cnt;
-    }
-    const float nf = float(cnt);
-    out[begin + rank[i]] = make_float4(__fdiv_rn(ax, nf), __fdiv_rn(ay, nf), __fdiv_rn(az, nf), __fdiv_rn(aw, nf));
-}
-
-// ---- index of a cloud whose size lives on the device (every point on-grid): block counts, slots, cell keys, cell table ------------
+// ------------------------------------------------------------------------------------------------------------------
+// Index stage: the search index of d_xyzi[0..info->n_out) (every point on the grid): block counts, slots in block order, cell
+// keys through locate() -- the searches bin a point with the same code -- a 32-bit sort, the gather and the cell table.
+// ------------------------------------------------------------------------------------------------------------------
 // One atomic per (warp, block) instead of one per point: the cloud is ordered block by block, so a warp almost always holds a
-// single block (1.1 M same-address atomics took 660 us; aggregated they take a few).
-__global__ void k_block_count_dev(const float4* __restrict__ raw, const InsertInfo* __restrict__ info, int3 origin, int32_t* __restrict__ block_count) {
+// single block (1.1 M same-address atomics took 660 us; aggregated they take a few).  Off-grid points are counted nowhere.
+__global__ void k_block_count(const float4* __restrict__ raw, const InsertInfo* __restrict__ info, int3 origin, int32_t* __restrict__ block_count) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    int lin = -1;
-    if (i < info->n_out) {
-        const float4 p = raw[i];
-        const int gx = block_coord(double(p.x) + kHalfBlock, origin.x), gy = block_coord(double(p.y) + kHalfBlock, origin.y),
-                  gz = block_coord(double(p.z) + kHalfBlock, origin.z);
-        if (gx >= 0 && gx < kW && gy >= 0 && gy < kH && gz >= 0 && gz < kD) lin = gx + kW * gy + kW * kH * gz;
-    }
+    const int lin = i < info->n_out ? grid_block(raw[i], origin) : -1;
     const unsigned peers = __match_any_sync(0xffffffffu, lin);
     if (lin >= 0 && (threadIdx.x & 31) == __ffs(peers) - 1) atomicAdd(&block_count[lin], __popc(peers));
 }
 
-// slots of the non-empty blocks in block order (what the host loop of map_rebuild does), one CTA
+// slots of the non-empty blocks in block order, the points they hold, and the error flag of a slot count above slot_cap (one CTA)
 __global__ void __launch_bounds__(1024) k_assign_slots(const int32_t* __restrict__ block_count, int32_t* __restrict__ block_slot, InsertInfo* __restrict__ info,
                                                        uint32_t slot_cap) {
     __shared__ uint32_t s_part[1024];
+    __shared__ uint32_t s_kept;
     const int per = (kNumBlocks + 1023) / 1024;
     const int b0 = threadIdx.x * per;
-    uint32_t mine = 0;
-    for (int k = 0; k < per; ++k) { const int b = b0 + k; if (b < kNumBlocks && block_count[b] > 0) ++mine; }
+    uint32_t mine = 0, kept = 0;
+    for (int k = 0; k < per; ++k) { const int b = b0 + k; if (b < kNumBlocks && block_count[b] > 0) { ++mine; kept += uint32_t(block_count[b]); } }
     s_part[threadIdx.x] = mine;
+    if (threadIdx.x == 0) s_kept = 0;
     __syncthreads();
+    if (kept) atomicAdd(&s_kept, kept);
     for (int o = 1; o < 1024; o <<= 1) {                                // Hillis-Steele inclusive scan
         const uint32_t v = threadIdx.x >= o ? s_part[threadIdx.x - o] : 0;
         __syncthreads();
@@ -526,37 +357,27 @@ __global__ void __launch_bounds__(1024) k_assign_slots(const int32_t* __restrict
         const int b = b0 + k;
         if (b < kNumBlocks) block_slot[b] = block_count[b] > 0 ? int32_t(slot++) : -1;
     }
-    if (threadIdx.x == 1023) { info->n_slots = s_part[1023]; if (s_part[1023] > slot_cap) info->error = 1; }
+    if (threadIdx.x == 1023) { info->n_slots = s_part[1023]; info->n_kept = s_kept; info->error = s_part[1023] > slot_cap; }
 }
 
-// cell key + histogram; positions >= n_out get the largest key so that they sort behind every real point
-__global__ void k_keys_dev(const float4* __restrict__ raw, uint32_t total, const InsertInfo* __restrict__ info, int3 origin, const int32_t* __restrict__ block_slot,
-                           int nb, double inv_cs, uint32_t* __restrict__ keys, uint32_t* __restrict__ vals, uint32_t* __restrict__ cell_count) {
+// cell key + histogram; positions >= n_out (and every position after a slot overflow) get the largest key and sort behind every
+// real point
+__global__ void k_cell_keys(const float4* __restrict__ raw, uint32_t total, const InsertInfo* __restrict__ info, MapView m,
+                            uint32_t* __restrict__ keys, uint32_t* __restrict__ vals, uint32_t* __restrict__ cell_count) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= total) return;
     vals[i] = i;
     if (i >= info->n_out || info->error) { keys[i] = 0xFFFFFFFFu; return; }
     const float4 p = raw[i];
-    const float q[3] = {p.x, p.y, p.z};
-    const int o[3] = {origin.x, origin.y, origin.z};
-    int g[3], c[3];
-#pragma unroll
-    for (int a = 0; a < 3; ++a) {
-        const double v = double(q[a]) + kHalfBlock;
-        int b = int(v / kBlock);
-        if (v < 0) b--;
-        g[a] = b + o[a];
-        int cc = int((v - kBlock * double(b)) * inv_cs);
-        c[a] = cc < 0 ? 0 : (cc > nb - 1 ? nb - 1 : cc);
-    }
-    const uint32_t slot = uint32_t(block_slot[g[0] + kW * g[1] + kW * kH * g[2]]);
-    const uint32_t key = slot * uint32_t(nb) * uint32_t(nb) * uint32_t(nb) + uint32_t((c[2] * nb + c[1]) * nb + c[0]);
+    QueryCell qc;
+    locate(m, p.x, p.y, p.z, qc);
+    const uint32_t key = scan_order_key(m, qc);
     keys[i] = key;
     atomicAdd(&cell_count[key], 1u);
 }
 
-__global__ void k_gather_dev(const float4* __restrict__ raw, const uint32_t* __restrict__ vals, uint32_t total, const InsertInfo* __restrict__ info,
-                             float4* __restrict__ sorted) {
+__global__ void k_gather(const float4* __restrict__ raw, const uint32_t* __restrict__ vals, uint32_t total, const InsertInfo* __restrict__ info,
+                         float4* __restrict__ sorted) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= total || i >= info->n_out) return;
     const uint32_t id = vals[i];
@@ -564,89 +385,117 @@ __global__ void k_gather_dev(const float4* __restrict__ raw, const uint32_t* __r
     sorted[i] = make_float4(p.x, p.y, p.z, __uint_as_float(id));
 }
 
-// LocalMap::addSurfPointCloud without a host round trip between its steps: mark touched blocks, one stable sort by
-// (touched, block, voxel), voxel heads + scan + centroids into the other cloud buffer, then the search index of the new cloud
-// (block counts and slots on the device, cell keys + histogram, sort, gather, scan).  The host reads the sizes, block tables and
-// the error flag back ONCE, at the end.  The two cloud buffers swap roles (no device-to-device copy of the map).
-int map_add_points(Ctx* c, MapStore& ms, uint32_t n_new) {
-    cudaStream_t st = c->stream;
-    if (n_new == 0) return SO_OK;
-    const uint32_t total = ms.n + n_new;                                // the caller rebuilt a dirty store BEFORE appending the new points
-    const int3 origin = make_int3(c->origin[0], c->origin[1], c->origin[2]);
-    const uint32_t grid = (total + 255) / 256;
-    const int nb = map_cells_per_block(ms.res);
-    const uint32_t cells_per_slot = uint32_t(nb) * uint32_t(nb) * uint32_t(nb);
-    // cell table capacity for the slots this insert can need: the current ones plus every block a new point may open
-    {
-        const size_t want_slots = size_t(ms.n_slots) + 4;
-        const size_t want = want_slots * cells_per_slot + 1;
-        if (want > ms.cell_cap || ms.nb != nb) {
-            size_t slots = want_slots + 4;
-            while (slots > want_slots && slots * cells_per_slot + 1 >= (size_t(1) << 31)) --slots;
-            if (slots * cells_per_slot + 1 >= (size_t(1) << 31)) return map_add_points_sync(c, ms, n_new);
-            SO_CUDA_TRY(cudaStreamSynchronize(st));
-            int rc = grow_buffer(ms.d_cell_start, ms.cell_cap, slots * cells_per_slot + 1);
-            if (rc) return rc;
-            size_t need = 0;
-            cub::DeviceScan::ExclusiveSum(nullptr, need, ms.d_cell_start, ms.d_cell_start, int(ms.cell_cap));
-            rc = grow_buffer(c->d_cub_tmp, c->cub_tmp_bytes, need + 256);
-            if (rc) return rc;
-        }
+// Cell table for `slots` slots, with up to `spare` slots of headroom where the limit allows, and the cub scratch to scan it.
+// SO_ERR_CAPACITY, before anything grows, when `slots` alone reach the limit.
+static int reserve_cells(Ctx* c, MapStore& ms, size_t slots, size_t spare) {
+    const size_t cells_per_slot = size_t(ms.nb) * ms.nb * ms.nb;
+    const size_t max_slots = (kMaxCells - 2) / cells_per_slot;         // slots * cells_per_slot + 1 < 2^31
+    if (slots > max_slots) {
+        set_error("map spans too many 50 m blocks for the dense cell table (n_slots * nb^3 >= 2^31)");
+        return SO_ERR_CAPACITY;
     }
-    // this insert indexes at most the current slots + 4 new ones (more: error flag -> synchronous rebuild); table work is sized for that
-    const uint32_t slot_cap = uint32_t(std::min<size_t>((ms.cell_cap - 1) / cells_per_slot, size_t(ms.n_slots) + 4));
-    const size_t cells_used = size_t(slot_cap) * cells_per_slot + 1;
-    ms.nb = nb;
-    InsertInfo* d_info = reinterpret_cast<InsertInfo*>(c->d_insert_info);
-    uint8_t* d_touched = reinterpret_cast<uint8_t*>(c->d_insert_info) + 64;         // 4851 bytes behind the info struct
-    SO_CUDA_TRY(cudaMemsetAsync(d_touched, 0, kNumBlocks, st));
-    k_mark_touched_new<<<(n_new + 255) / 256, 256, 0, st>>>(ms.d_xyzi + ms.n, n_new, origin, d_touched);
-    const float inv_leaf = 1.0f / ms.res;                               // Eigen::Array4f::Ones() / leaf_size_
-    int vb = 1;                                                         // bits of a block-local voxel index: 50 m / leaf + 5 values
-    while (vb < 16 && double(1 << vb) < kBlock * double(inv_leaf) + 5.0) ++vb;
-    const int cls_shift = 13 + 3 * vb;
-    k_insert_keys<<<grid, 256, 0, st>>>(ms.d_xyzi, total, inv_leaf, origin, d_touched, vb, c->d_keys, c->d_vals);
-    size_t tmp = c->cub_tmp_bytes;
-    SO_CUDA_TRY(cub::DeviceRadixSort::SortPairs(c->d_cub_tmp, tmp, c->d_keys, c->d_keys_out, c->d_vals, c->d_vals_out, int(total), 0, cls_shift + 2, st));
-    k_insert_bounds<<<1, 32, 0, st>>>(c->d_keys_out, total, cls_shift, d_info);
-    uint32_t* d_head = reinterpret_cast<uint32_t*>(c->d_keys);          // keys_in is free after the sort: [heads total][ranks total]
-    uint32_t* d_rank = d_head + total;
-    k_voxel_heads_dev<<<grid, 256, 0, st>>>(c->d_keys_out, total, d_info, d_head);
-    tmp = c->cub_tmp_bytes;
-    SO_CUDA_TRY(cub::DeviceScan::ExclusiveSum(c->d_cub_tmp, tmp, d_head, d_rank, int(total), st));
-    k_voxel_centroid_dev<<<grid, 256, 0, st>>>(ms.d_xyzi, c->d_keys_out, c->d_vals_out, d_head, d_rank, total, d_info, ms.d_sorted);
-    std::swap(ms.d_xyzi, ms.d_sorted);                                  // d_xyzi: the new cloud in id order; d_sorted: free for the new index
-    // ---- search index of the new cloud
+    if (slots * cells_per_slot + 1 <= ms.cell_cap) return SO_OK;
+    SO_CUDA_TRY(cudaStreamSynchronize(c->stream));
+    int rc = grow_buffer(ms.d_cell_start, ms.cell_cap, std::min(slots + spare, max_slots) * cells_per_slot + 1);
+    if (rc) return rc;
+    size_t need = 0;
+    cub::DeviceScan::ExclusiveSum(nullptr, need, ms.d_cell_start, ms.d_cell_start, int(ms.cell_cap));
+    return grow_buffer(c->d_cub_tmp, c->cub_tmp_bytes, need + 256);
+}
+
+// block counts and slots of d_xyzi[0..info->n_out); more than slot_cap slots raise info->error
+static int count_blocks(Ctx* c, MapStore& ms, uint32_t n_max, uint32_t slot_cap) {
+    cudaStream_t st = c->stream;
+    InsertInfo* d_info = &c->d_map_scratch->info;
     SO_CUDA_TRY(cudaMemsetAsync(ms.d_block_count, 0, kNumBlocks * sizeof(int32_t), st));
-    k_block_count_dev<<<grid, 256, 0, st>>>(ms.d_xyzi, d_info, origin, ms.d_block_count);
+    k_block_count<<<(n_max + 255) / 256, 256, 0, st>>>(ms.d_xyzi, d_info, make_int3(c->origin[0], c->origin[1], c->origin[2]), ms.d_block_count);
     k_assign_slots<<<1, 1024, 0, st>>>(ms.d_block_count, ms.d_block_slot, d_info, slot_cap);
+    c->launches += 3;
+    return SO_OK;
+}
+
+// The cell table of slot_cap slots over the slots count_blocks assigned, then the one read-back of the sizes, the error flag and
+// the host mirrors.  The store is clean (its index built) when no slot overflowed.
+static int index_cells(Ctx* c, MapStore& ms, uint32_t n_max, uint32_t slot_cap) {
+    cudaStream_t st = c->stream;
+    InsertInfo* d_info = &c->d_map_scratch->info;
+    InsertInfo* h_info = c->h_map_info;
+    const uint32_t grid = (n_max + 255) / 256;
+    const size_t cells_used = size_t(slot_cap) * ms.nb * ms.nb * ms.nb + 1;
     SO_CUDA_TRY(cudaMemsetAsync(ms.d_cell_start, 0, cells_used * sizeof(uint32_t), st));
-    uint32_t* keys32 = reinterpret_cast<uint32_t*>(c->d_keys);          // heads / ranks are dead now
+    uint32_t* keys32 = reinterpret_cast<uint32_t*>(c->d_keys);
     uint32_t* keys32_out = reinterpret_cast<uint32_t*>(c->d_keys_out);
-    k_keys_dev<<<grid, 256, 0, st>>>(ms.d_xyzi, total, d_info, origin, ms.d_block_slot, nb, double(nb) / kBlock, keys32, c->d_vals, ms.d_cell_start);
-    int bits = 1;
-    while (bits < 32 && (uint64_t(1) << bits) < uint64_t(ms.cell_cap)) ++bits;
-    tmp = c->cub_tmp_bytes;
-    SO_CUDA_TRY(cub::DeviceRadixSort::SortPairs(c->d_cub_tmp, tmp, keys32, keys32_out, c->d_vals, c->d_vals_out, int(total), 0, 32, st));
-    (void)bits;
-    k_gather_dev<<<grid, 256, 0, st>>>(ms.d_xyzi, c->d_vals_out, total, d_info, ms.d_sorted);
+    k_cell_keys<<<grid, 256, 0, st>>>(ms.d_xyzi, n_max, d_info, map_view(c, ms), keys32, c->d_vals, ms.d_cell_start);
+    size_t tmp = c->cub_tmp_bytes;
+    SO_CUDA_TRY(cub::DeviceRadixSort::SortPairs(c->d_cub_tmp, tmp, keys32, keys32_out, c->d_vals, c->d_vals_out, int(n_max), 0, 32, st));
+    k_gather<<<grid, 256, 0, st>>>(ms.d_xyzi, c->d_vals_out, n_max, d_info, ms.d_sorted);
     tmp = c->cub_tmp_bytes;
     SO_CUDA_TRY(cub::DeviceScan::ExclusiveSum(c->d_cub_tmp, tmp, ms.d_cell_start, ms.d_cell_start, int(cells_used), st));
-    // ---- the one read-back
-    InsertInfo* h_info = reinterpret_cast<InsertInfo*>(c->h_insert_info);
     SO_CUDA_TRY(cudaMemcpyAsync(h_info, d_info, sizeof(InsertInfo), cudaMemcpyDeviceToHost, st));
     SO_CUDA_TRY(cudaMemcpyAsync(ms.h_block_count.data(), ms.d_block_count, kNumBlocks * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
     SO_CUDA_TRY(cudaMemcpyAsync(ms.h_block_slot.data(), ms.d_block_slot, kNumBlocks * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-    c->launches += 26;
+    c->launches += 10;
     SO_CUDA_TRY(cudaGetLastError());
     SO_CUDA_TRY(cudaStreamSynchronize(st));
     ms.n = h_info->n_out;
     ms.n_slots = int(h_info->n_slots);
-    if (h_info->error) {                                                // more new blocks than the table was sized for: index again, synchronously
-        ms.dirty = true;
-        return map_rebuild(c, ms);
-    }
+    ms.dirty = h_info->error != 0;
     return SO_OK;
+}
+
+// (Re)build the index of d_xyzi[0..n) under the current origin and resolution: count blocks and assign slots over the raw cloud,
+// size the cell table, drop off-grid points (filter stage, nothing touched) when there are any, index.
+int map_rebuild(Ctx* c, MapStore& ms) {
+    cudaStream_t st = c->stream;
+    ms.nb = map_cells_per_block(ms.res);
+    ms.dirty = true;
+    if (ms.n == 0) {
+        SO_CUDA_TRY(cudaMemsetAsync(ms.d_block_count, 0, kNumBlocks * sizeof(int32_t), st));
+        SO_CUDA_TRY(cudaMemsetAsync(ms.d_block_slot, 0xFF, kNumBlocks * sizeof(int32_t), st));
+        SO_CUDA_TRY(cudaStreamSynchronize(st));
+        std::fill(ms.h_block_count.begin(), ms.h_block_count.end(), 0);
+        std::fill(ms.h_block_slot.begin(), ms.h_block_slot.end(), -1);
+        ms.n_slots = 0;
+        ms.dirty = false;
+        return SO_OK;
+    }
+    const uint32_t n = ms.n;
+    InsertInfo* h_info = c->h_map_info;
+    *h_info = InsertInfo{};
+    h_info->n_out = n;
+    SO_CUDA_TRY(cudaMemcpyAsync(&c->d_map_scratch->info, h_info, sizeof(InsertInfo), cudaMemcpyHostToDevice, st));
+    int rc = count_blocks(c, ms, n, kNumBlocks);
+    if (rc) return rc;
+    SO_CUDA_TRY(cudaMemcpyAsync(h_info, &c->d_map_scratch->info, sizeof(InsertInfo), cudaMemcpyDeviceToHost, st));
+    SO_CUDA_TRY(cudaGetLastError());
+    SO_CUDA_TRY(cudaStreamSynchronize(st));
+    const uint32_t n_slots = h_info->n_slots;
+    rc = reserve_cells(c, ms, n_slots, n_slots / 4);
+    if (rc) return rc;
+    if (h_info->n_kept < n) { rc = filter_stage(c, ms, 0); if (rc) return rc; }
+    return index_cells(c, ms, n, n_slots);
+}
+
+// LocalMap::addSurfPointCloud without a host round trip between its steps: the filter stage, then the index stage bounded to the
+// current slots plus 4 new ones.  The host reads the sizes, block tables and the error flag back ONCE, at the end; when the new
+// cloud opened more blocks, the table grows to the slot count read back and the index stage runs again (not the filter).
+int map_add_points(Ctx* c, MapStore& ms, uint32_t n_new) {
+    if (n_new == 0) return SO_OK;
+    const uint32_t total = ms.n + n_new;                                // the caller rebuilt a dirty store BEFORE appending the new points
+    ms.nb = map_cells_per_block(ms.res);
+    const size_t cells_per_slot = size_t(ms.nb) * ms.nb * ms.nb;
+    const uint32_t slot_cap = uint32_t(std::min<size_t>(size_t(ms.n_slots) + 4, (kMaxCells - 2) / cells_per_slot));
+    int rc = reserve_cells(c, ms, slot_cap, 4);
+    if (rc) return rc;
+    ms.dirty = true;
+    rc = filter_stage(c, ms, n_new);
+    if (!rc) rc = count_blocks(c, ms, total, slot_cap);
+    if (!rc) rc = index_cells(c, ms, total, slot_cap);
+    if (rc || !ms.dirty) return rc;
+    const uint32_t n_slots = uint32_t(ms.n_slots);                      // more new blocks than the table was sized for
+    rc = reserve_cells(c, ms, n_slots, 4);
+    if (!rc) rc = count_blocks(c, ms, total, n_slots);
+    return rc ? rc : index_cells(c, ms, total, n_slots);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -676,50 +525,31 @@ __global__ void k_voxel_keys_cloud(const float4* __restrict__ raw, uint32_t n, f
     vals[i] = i;
 }
 
-__global__ void k_count_valid(const uint64_t* __restrict__ keys, uint32_t n, uint64_t skipped_key, uint32_t* __restrict__ count) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n && keys[i] != skipped_key && (i + 1 == n || keys[i + 1] == skipped_key)) *count = i + 1;   // sorted: last valid key
-}
-
 int scan_voxel_filter(Ctx* c, uint32_t n, float leaf, uint32_t* n_out) {
     cudaStream_t st = c->stream;
     *n_out = 0;
     if (n == 0) return SO_OK;
     const uint32_t grid = (n + 255) / 256;
     const float inv_leaf = 1.0f / leaf;
-    uint32_t* d_flag = reinterpret_cast<uint32_t*>(c->d_insert_info) + 2000;     // scratch word behind the insert bookkeeping
-    uint32_t* d_cnt = reinterpret_cast<uint32_t*>(c->d_skeys);      // keys_in is free after the sort: [count][heads...][ranks...]
-    uint32_t n_valid = 0;
+    InsertInfo* d_info = &c->d_map_scratch->info;
+    InsertInfo* h_info = c->h_map_info;
     for (int wide = 0; wide < 2; ++wide) {
         const int vb = wide ? 17 : 13;
-        SO_CUDA_TRY(cudaMemsetAsync(d_flag, 0, 4, st));
-        if (wide) k_voxel_keys_cloud<17><<<grid, 256, 0, st>>>(c->d_scan, n, inv_leaf, c->d_skeys, c->d_svals, d_flag);
-        else k_voxel_keys_cloud<13><<<grid, 256, 0, st>>>(c->d_scan, n, inv_leaf, c->d_skeys, c->d_svals, d_flag);
+        SO_CUDA_TRY(cudaMemsetAsync(&d_info->overflow, 0, sizeof(uint32_t), st));
+        if (wide) k_voxel_keys_cloud<17><<<grid, 256, 0, st>>>(c->d_scan, n, inv_leaf, c->d_skeys, c->d_svals, &d_info->overflow);
+        else k_voxel_keys_cloud<13><<<grid, 256, 0, st>>>(c->d_scan, n, inv_leaf, c->d_skeys, c->d_svals, &d_info->overflow);
         size_t tmp = c->sort_tmp_bytes;
         SO_CUDA_TRY(cub::DeviceRadixSort::SortPairs(c->d_sort_tmp, tmp, c->d_skeys, c->d_skeys_out, c->d_svals, c->d_svals_out, int(n), 0, 3 * vb + 1, st));
-        SO_CUDA_TRY(cudaMemsetAsync(d_cnt, 0, 4, st));
-        k_count_valid<<<grid, 256, 0, st>>>(c->d_skeys_out, n, uint64_t(1) << (3 * vb), d_cnt);
-        uint32_t h[2] = {0, 0};
-        SO_CUDA_TRY(cudaMemcpyAsync(&h[0], d_cnt, 4, cudaMemcpyDeviceToHost, st));
-        SO_CUDA_TRY(cudaMemcpyAsync(&h[1], d_flag, 4, cudaMemcpyDeviceToHost, st));
+        c->launches += 7;
+        const int rc = voxel_reduce(c, c->d_scan, c->d_skeys_out, c->d_svals_out, n, 0, uint64_t(1) << (3 * vb),
+                                    reinterpret_cast<uint32_t*>(c->d_skeys), c->d_sort_tmp, c->sort_tmp_bytes, c->d_scan_sorted);   // keys_in is free after the sort
+        if (rc) return rc;
+        SO_CUDA_TRY(cudaMemcpyAsync(h_info, d_info, sizeof(InsertInfo), cudaMemcpyDeviceToHost, st));
+        SO_CUDA_TRY(cudaGetLastError());
         SO_CUDA_TRY(cudaStreamSynchronize(st));
-        n_valid = h[0];
-        if (!h[1]) break;                                           // every voxel index fitted the narrow key
+        if (!h_info->overflow) break;                               // every voxel index fitted the narrow key
     }
-    if (n_valid == 0) return SO_OK;
-    uint32_t* d_head = d_cnt + 4;
-    uint32_t* d_rank = d_head + n_valid;
-    k_voxel_heads<<<(n_valid + 255) / 256, 256, 0, st>>>(c->d_skeys_out, 0, n_valid, d_head);
-    size_t tmp = c->sort_tmp_bytes;
-    SO_CUDA_TRY(cub::DeviceScan::ExclusiveSum(c->d_sort_tmp, tmp, d_head, d_rank, int(n_valid), st));
-    uint32_t last_flag = 0, last_rank = 0;
-    SO_CUDA_TRY(cudaMemcpyAsync(&last_flag, d_head + n_valid - 1, 4, cudaMemcpyDeviceToHost, st));
-    SO_CUDA_TRY(cudaMemcpyAsync(&last_rank, d_rank + n_valid - 1, 4, cudaMemcpyDeviceToHost, st));
-    k_voxel_centroid<<<(n_valid + 255) / 256, 256, 0, st>>>(c->d_scan, c->d_skeys_out, c->d_svals_out, d_rank, 0, n_valid, c->d_scan_sorted);
-    SO_CUDA_TRY(cudaStreamSynchronize(st));
-    *n_out = last_rank + last_flag;
-    c->launches += 10;
-    SO_CUDA_TRY(cudaGetLastError());
+    *n_out = h_info->n_out;
     return SO_OK;
 }
 
