@@ -219,6 +219,31 @@ int so_scan_deskew(so_ctx* ctx, void* points, size_t n, size_t stride_bytes, siz
  * *n_out = points produced (may exceed cap_points; only cap_points are written). */
 int so_scan_extract_uniform(so_ctx* ctx, const void* points, size_t n, size_t stride_bytes, size_t time_offset, int skip_num,
                             float block_range, int int_abs, float* out_xyzi, size_t cap_points, size_t* n_out);
+/* fills: the edgePoints cloud featureExtraction::extractFeatures publishes empty (featureExtraction.cpp:429-436), so that the line
+ * branch of so_register gets real input.  LOAM edge selection (Zhang & Singh, RSS 2014, §V-A, as A-LOAM's scanRegistration, with
+ * LOAM's occlusion and parallel-beam rejection; DESIGN.md §9 is the full definition), float32, each operation rounded on its own:
+ *   - valid points: x, y, z, time finite and (x*x + y*y) + z*z > min_range^2; ordered by (ring, time, input index);
+ *   - per ring of m points, 5 <= k <= m-6: curvature |sum of q_{k-5..k+5} except q_k, minus 10 q_k|^2;
+ *   - excluded before selection: the occluded side of a gap (|q_{k+1}-q_k|^2 > 0.1, relative distance < 0.1) and points whose
+ *     both neighbour gaps exceed 0.0002 |q_k|^2;
+ *   - six sectors per ring (rings below 17 points give nothing); in each, curvature descending (ties by position), up to
+ *     max_per_sector points with curvature > edge_threshold that are not excluded are accepted, each excluding itself and up to 5
+ *     neighbours per side until a gap |dq|^2 > 0.05;
+ *   - output: packed float4 {x, y, z, intensity = time} ordered by (ring, position); with voxel_leaf > 0 then pcl::VoxelGrid(voxel_leaf)
+ *     on the sensor frame (laserMapping's corner filter at lineRes, laserMapping.cpp:635-640), bit-equal to so_scan_prefilter's filter.
+ * points: n records of stride_bytes, float x, y, z at bytes 0, 4, 8, float time at time_offset, uint16 ring at ring_offset
+ * (point_os::PointcloudXYZITR: stride 32, time at 20, ring at 24).  Does not touch the scan buffers: so_register_prefiltered and
+ * so_map_add_registered_scan stay valid across this call.  *n_out = points produced (may exceed cap_points; only cap_points are
+ * written).  SO_ERR_ARG before any device work: a NULL with n > 0, a stride that does not hold the fields, a time or ring overlapping
+ * x, y, z or each other, a negative or non-finite option; SO_ERR_CAPACITY: n > max_scan_points.  opts may be NULL (all defaults). */
+typedef struct {
+    float min_range;          /* points at or inside this range are dropped (default 0: zero returns only) */
+    float edge_threshold;     /* curvature a point must exceed (default 0.1) */
+    float voxel_leaf;         /* > 0: voxel-centroid filter of the edge cloud at this leaf (default 0: off) */
+    int32_t max_per_sector;   /* points accepted per sector (default 20, A-LOAM's less-sharp set) */
+} so_edge_opts;
+int so_scan_extract_edges(so_ctx* ctx, const void* points, size_t n, size_t stride_bytes, size_t time_offset, size_t ring_offset,
+                          const so_edge_opts* opts, float* out_xyzi, size_t cap_points, size_t* n_out);
 
 /* ---- registration (LidarSLAM) --------------------------------------------------------------------- */
 /* replaces: LidarSLAM::Localization(true, predictodom, position, edge, planner, t) -> performLocalizationAndMapping
@@ -473,7 +498,7 @@ uint64_t so_kernel_launches(so_ctx* ctx, int reset);
 int so_bytes_copied(so_ctx* ctx, uint64_t* h2d, uint64_t* d2h, int reset);
 /* Accumulated device time (ms, CUDA events on the context stream) and launch count of a kernel class since the last
  * reset; classes: 0 k_knn_scan (scan k-NN), 1 k_evaluate +
- * k_lm_step (LM step), 2 k_knn (so_knn*), 3 scan ordering / map build / map insert / scan preparation, 4 first evaluation of
+ * k_lm_step (LM step), 2 k_knn (so_knn*), 3 scan ordering / map build / map insert / scan preparation (pre-filter, deskew, uniform and edge extraction), 4 first evaluation of
  * a solve (k_evaluate + k_lm_step iteration zero), 5 k_fit (plane fit), 6 global localization search (bitmap raster, dilation,
  * hypothesis scoring, key sort; for the branch-and-bound also map bounds, pyramid levels, offset table and traversal steps),
  * 7 k_undistort (within-scan motion compensation: per ICP iteration, and the undistorted map insert / so_undistort_points; the

@@ -7,6 +7,7 @@
 //       super_odometry/src/FeatureExtraction/featureExtraction.cpp:222-314
 //   featureExtraction::uniformFeatureExtraction(pc_in, pc_out_surf, skip_num, block_range)
 //       super_odometry/src/FeatureExtraction/featureExtraction.cpp:504-525
+// and the edge cloud featureExtraction::extractFeatures publishes empty (:429-436): extractEdgeFeatures.
 //
 // Same argument meaning as upstream; the node's members they read or write
 // (T_i_l, q_w_original_l, t_w_original_l) are explicit arguments here.  The pose
@@ -82,6 +83,38 @@ inline void uniformFeatureExtraction(Context& ctx, const RawCloudPtr& pc_in, Clo
         OutT p{};
         p.x = out[4 * i]; p.y = out[4 * i + 1]; p.z = out[4 * i + 2]; p.intensity = out[4 * i + 3];
         pc_out_surf->points[base + i] = p;
+    }
+}
+
+// ... and the offset of the uint16 `ring` field (byte 24 in point_os::PointcloudXYZITR)
+template <class PointT>
+inline void raw_point_layout(size_t* stride, size_t* time_off, size_t* ring_off) {
+    raw_point_layout<PointT>(stride, time_off);
+    PointT p{};
+    *ring_off = size_t(reinterpret_cast<const char*>(&p.ring) - reinterpret_cast<const char*>(&p));
+}
+
+// The edgePoints cloud extractFeatures leaves empty (featureExtraction.cpp:429-436): LOAM edge selection over the rings of *pc_in
+// (so_scan_extract_edges), appended to *pc_out_edge with intensity = the raw point's time.  opts.voxel_leaf = lineRes applies
+// laserMapping's corner filter (downSizeFilterCorner, laserMapping.cpp:635-640) on the device.
+template <class RawCloudPtr, class CloudPtr>
+inline void extractEdgeFeatures(Context& ctx, const RawCloudPtr& pc_in, CloudPtr& pc_out_edge, const so_edge_opts& opts = so_edge_opts{}) {
+    using RawT = typename std::decay<decltype(pc_in->points[0])>::type;
+    using OutT = typename std::decay<decltype(pc_out_edge->points[0])>::type;
+    if (!ctx.h) throw Error("extractEdgeFeatures: context not created");
+    size_t stride = 0, toff = 0, roff = 0;
+    raw_point_layout<RawT>(&stride, &toff, &roff);
+    const size_t n = pc_in->size();
+    std::vector<float> out(4 * (n ? n : 1));
+    size_t m = 0;
+    const int rc = so_scan_extract_edges(ctx.h, pc_in->points.data(), n, stride, toff, roff, &opts, out.data(), n ? n : 1, &m);
+    if (rc < 0) throw Error(std::string("so_scan_extract_edges: ") + so_last_error());
+    const size_t base = pc_out_edge->points.size();
+    pc_out_edge->points.resize(base + m);
+    for (size_t i = 0; i < m; ++i) {
+        OutT p{};
+        p.x = out[4 * i]; p.y = out[4 * i + 1]; p.z = out[4 * i + 2]; p.intensity = out[4 * i + 3];
+        pc_out_edge->points[base + i] = p;
     }
 }
 

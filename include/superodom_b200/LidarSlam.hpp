@@ -309,7 +309,8 @@ public:
             last_result = mr.icp;
             LastMotion = Transformd::from_pose7(mr.motion);
         } else if (Undistortion == APPROXIMATED && undistort_has_prev && dt > 0 && !(edge_point && edge_point->size())) {
-            so_undistort u{};                                      // the surf cloud only; the edge cloud is empty upstream
+            so_undistort u{};                                      // the surf cloud only: a non-empty edge cloud (extractEdgeFeatures)
+                                                                   // turns within-scan compensation off and takes so_register below
             u.mode = 1; u.rotation = UndistortRotation ? 1 : 0; u.dt = dt;
             undistort_prev_pose.to_pose7(u.prev_pose);
             rc = so_register_undistort(context.h, surf, planner_point->size(), stride, ioff, ioff, pose, &u, &o, &last_result);

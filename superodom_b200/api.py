@@ -20,7 +20,7 @@ EXPORTS = [
     "so_create", "so_destroy", "so_last_error", "so_device_available", "so_set_stream",
     "so_map_set_resolution", "so_map_set_origin", "so_map_get_origin", "so_map_shift", "so_map_set_points",
     "so_map_set_edge_points", "so_map_add_surf", "so_map_add_edge", "so_map_add_scan", "so_map_add_registered_scan", "so_map_add_scan_edge", "so_map_counts_5x5", "so_map_download", "so_map_size",
-    "so_scan_prefilter", "so_scan_deskew", "so_scan_extract_uniform", "so_register", "so_register_prefiltered", "so_register_injected", "so_set_pose_sink", "so_register_batch", "so_register_batch_edges", "so_register_batch_device",
+    "so_scan_prefilter", "so_scan_deskew", "so_scan_extract_uniform", "so_scan_extract_edges", "so_register", "so_register_prefiltered", "so_register_injected", "so_set_pose_sink", "so_register_batch", "so_register_batch_edges", "so_register_batch_device",
     "so_register_undistort", "so_register_prefiltered_undistort", "so_register_batch_undistort", "so_undistort_points", "so_register_optimized", "so_register_prefiltered_optimized", "so_register_batch_optimized", "so_evaluate_optimized", "so_correspond", "so_correspond_edge", "so_evaluate",
     "so_knn", "so_knn_device", "so_sampling_indices", "so_localize_global", "so_localize_scores", "so_localize_global_size", "so_localize_global_bnb", "so_localize_bnb_keys", "so_localize_bnb_bounds", "so_map_bounds", "so_kernel_launches", "so_bytes_copied", "so_build_flags", "so_profile_enable", "so_profile_get",
 ]
@@ -126,6 +126,11 @@ def whole_map_opts(map_lo, map_hi, center_pose7, **kw) -> GlobalOpts:
     return global_opts(half_x=hx, half_y=hy, **kw)
 
 
+class EdgeOpts(C.Structure):
+    """so_edge_opts: zero fields take the defaults (min_range 0, edge_threshold 0.1, voxel_leaf 0 = no filter, max_per_sector 20)."""
+    _fields_ = [("min_range", C.c_float), ("edge_threshold", C.c_float), ("voxel_leaf", C.c_float), ("max_per_sector", C.c_int32)]
+
+
 CORR_DTYPE = np.dtype([("n", "<f8", 3), ("d", "<f8"), ("w", "<f8"), ("nn", "<u4", 5), ("nn_d2", "<f4", 5),
                        ("status", "u1"), ("obs", "u1", 3), ("pad_", "u1", 4)], align=True)
 
@@ -170,6 +175,8 @@ def load_library():
                                  C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
     L.so_scan_extract_uniform.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_int, C.c_float, C.c_int,
                                           C.c_void_p, C.c_size_t, C.c_void_p]
+    L.so_scan_extract_edges.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p, C.c_void_p,
+                                        C.c_size_t, C.c_void_p]
     L.so_register.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t,
                               C.c_void_p, C.c_void_p, C.c_void_p]
     L.so_register_prefiltered.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -426,6 +433,21 @@ class Context:
         self._chk(self.L.so_scan_extract_uniform(self.h, _p(a), a.shape[0], a.shape[1] * 4, time_col * 4, int(skip_num), float(block_range), int(int_abs),
                                                  _p(out), len(out), C.byref(n)), "so_scan_extract_uniform")
         return out[: n.value]
+
+    def scan_extract_edges(self, records: np.ndarray, time_offset: int = 20, ring_offset: int = 24, min_range: float = 0.0,
+                           edge_threshold: float = 0.0, voxel_leaf: float = 0.0, max_per_sector: int = 0) -> np.ndarray:
+        """LOAM edge features of a raw scan -> float32 [m, 4] {x, y, z, intensity = time}, ordered by (ring, position), or by voxel
+        with voxel_leaf > 0.  records: one row per point (point_os::PointcloudXYZITR: float32 [n, 8], time at byte 20, uint16 ring
+        at byte 24); zero options take the defaults of so_edge_opts."""
+        a = np.ascontiguousarray(records)
+        n = a.shape[0] if a.ndim else 0
+        stride = a.nbytes // n if n else max(a.itemsize * (a.shape[1] if a.ndim == 2 else 1), 1)
+        o = EdgeOpts(float(min_range), float(edge_threshold), float(voxel_leaf), int(max_per_sector))
+        out = np.zeros((max(n, 1), 4), np.float32)
+        m = C.c_size_t()
+        self._chk(self.L.so_scan_extract_edges(self.h, _p(a), n, stride, int(time_offset), int(ring_offset), C.byref(o), _p(out), len(out),
+                                               C.byref(m)), "so_scan_extract_edges")
+        return out[: m.value]
 
     # ---- registration
     @staticmethod

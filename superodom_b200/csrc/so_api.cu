@@ -156,6 +156,7 @@ static void ctx_free(Ctx* c) {
     global_free(c);
     undistort_free(c);
     motion_free(c);
+    features_free(c);
     if (c->ev_dec) cudaEventDestroy(c->ev_dec);
     if (c->ev0) cudaEventDestroy(c->ev0);
     if (c->ev1) cudaEventDestroy(c->ev1);

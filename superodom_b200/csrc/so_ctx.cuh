@@ -249,6 +249,19 @@ struct Ctx {
         double* d_partials = nullptr; size_t partials_cap = 0;             // [max_batch][stride][kMotionAcc] per-CTA sums
         uint32_t stride = 0;                                               // CTAs per scan the partials are laid out for
     } mot;
+    // ---- edge extraction (so_scan_extract_edges): allocated on first use, grown on demand; never touches the scan buffers ----
+    struct Feat {
+        unsigned char* d_raw = nullptr; size_t raw_cap = 0;                // the caller's records as given
+        size_t cap = 0;                                                    // points every per-point buffer below holds
+        uint64_t* d_keys[2] = {nullptr, nullptr};                          // sort keys in / out: (ring, time), then (ring, sector, curvature)
+        uint32_t* d_vals[2] = {nullptr, nullptr};
+        float4* d_pts = nullptr;                                           // valid points in (ring, time, index) order, w = time
+        uint8_t* d_excl = nullptr; uint8_t* d_reach = nullptr;             // excluded marks; neighbour-mark reach of each candidate
+        uint32_t* d_sel = nullptr; uint32_t* d_rank = nullptr;             // accepted flags and their exclusive scan
+        float4* d_out = nullptr; float4* d_vout = nullptr;                 // edge cloud; after the voxel filter
+        void* d_tmp = nullptr; size_t tmp_bytes = 0;                       // radix-sort / scan scratch
+        uint32_t* d_ring = nullptr;                                        // [65536] first position, [65536] end, [65536] ring list, [4] control
+    } feat;
 
     // ---- instrumentation ----------------------------------------------------------------------------------------
     uint64_t launches = 0;
@@ -311,7 +324,12 @@ int map_alloc(Ctx* c);
 void map_free(Ctx* c);
 int map_add_points(Ctx* c, MapStore& ms, uint32_t n_new);   // ms.d_xyzi[n .. n+n_new) holds the new points: voxel-filter touched blocks, index
 int map_transform_tail(Ctx* c, MapStore& ms, uint32_t n_new, const double pose[7]);   // sensor-frame tail points -> world frame
-int scan_voxel_filter(Ctx* c, uint32_t n, float leaf, uint32_t* n_out);
+int scan_voxel_filter(Ctx* c, uint32_t n, float leaf, uint32_t* n_out);   // d_scan -> d_scan_sorted (VoxelGrid on a scan)
+// The same filter on any packed cloud in[0..n) -> out, with the caller's sort buffers (keys: 2n words of head scratch after the sort)
+struct VoxelBufs { uint64_t* keys; uint64_t* keys_out; uint32_t* vals; uint32_t* vals_out; void* tmp; size_t tmp_bytes; };
+int cloud_voxel_filter(Ctx* c, const float4* in, uint32_t n, float leaf, const VoxelBufs& b, float4* out, uint32_t* n_out);
+// so_features.cu
+void features_free(Ctx* c);                                 // the buffers of Ctx::feat
 // so_scan.cu
 struct DeskewParams {
     double start_time;                     // lidar_start_time

@@ -525,7 +525,7 @@ __global__ void k_voxel_keys_cloud(const float4* __restrict__ raw, uint32_t n, f
     vals[i] = i;
 }
 
-int scan_voxel_filter(Ctx* c, uint32_t n, float leaf, uint32_t* n_out) {
+int cloud_voxel_filter(Ctx* c, const float4* in, uint32_t n, float leaf, const VoxelBufs& b, float4* out, uint32_t* n_out) {
     cudaStream_t st = c->stream;
     *n_out = 0;
     if (n == 0) return SO_OK;
@@ -536,13 +536,13 @@ int scan_voxel_filter(Ctx* c, uint32_t n, float leaf, uint32_t* n_out) {
     for (int wide = 0; wide < 2; ++wide) {
         const int vb = wide ? 17 : 13;
         SO_CUDA_TRY(cudaMemsetAsync(&d_info->overflow, 0, sizeof(uint32_t), st));
-        if (wide) k_voxel_keys_cloud<17><<<grid, 256, 0, st>>>(c->d_scan, n, inv_leaf, c->d_skeys, c->d_svals, &d_info->overflow);
-        else k_voxel_keys_cloud<13><<<grid, 256, 0, st>>>(c->d_scan, n, inv_leaf, c->d_skeys, c->d_svals, &d_info->overflow);
-        size_t tmp = c->sort_tmp_bytes;
-        SO_CUDA_TRY(cub::DeviceRadixSort::SortPairs(c->d_sort_tmp, tmp, c->d_skeys, c->d_skeys_out, c->d_svals, c->d_svals_out, int(n), 0, 3 * vb + 1, st));
+        if (wide) k_voxel_keys_cloud<17><<<grid, 256, 0, st>>>(in, n, inv_leaf, b.keys, b.vals, &d_info->overflow);
+        else k_voxel_keys_cloud<13><<<grid, 256, 0, st>>>(in, n, inv_leaf, b.keys, b.vals, &d_info->overflow);
+        size_t tmp = b.tmp_bytes;
+        SO_CUDA_TRY(cub::DeviceRadixSort::SortPairs(b.tmp, tmp, b.keys, b.keys_out, b.vals, b.vals_out, int(n), 0, 3 * vb + 1, st));
         c->launches += 7;
-        const int rc = voxel_reduce(c, c->d_scan, c->d_skeys_out, c->d_svals_out, n, 0, uint64_t(1) << (3 * vb),
-                                    reinterpret_cast<uint32_t*>(c->d_skeys), c->d_sort_tmp, c->sort_tmp_bytes, c->d_scan_sorted);   // keys_in is free after the sort
+        const int rc = voxel_reduce(c, in, b.keys_out, b.vals_out, n, 0, uint64_t(1) << (3 * vb),
+                                    reinterpret_cast<uint32_t*>(b.keys), b.tmp, b.tmp_bytes, out);   // keys_in is free after the sort
         if (rc) return rc;
         SO_CUDA_TRY(cudaMemcpyAsync(h_info, d_info, sizeof(InsertInfo), cudaMemcpyDeviceToHost, st));
         SO_CUDA_TRY(cudaGetLastError());
@@ -551,6 +551,11 @@ int scan_voxel_filter(Ctx* c, uint32_t n, float leaf, uint32_t* n_out) {
     }
     *n_out = h_info->n_out;
     return SO_OK;
+}
+
+int scan_voxel_filter(Ctx* c, uint32_t n, float leaf, uint32_t* n_out) {
+    const VoxelBufs b{c->d_skeys, c->d_skeys_out, c->d_svals, c->d_svals_out, c->d_sort_tmp, c->sort_tmp_bytes};
+    return cloud_voxel_filter(c, c->d_scan, n, leaf, b, c->d_scan_sorted, n_out);
 }
 
 }  // namespace so

@@ -605,3 +605,49 @@ def make_moving_scan(scene: Scene, sensor: str, pose_start: np.ndarray, speed: f
     scan = np.concatenate(out).astype(np.float32)
     prior = perturb_pose(pose_start, seed + 7, dt=0.05, dth_deg=0.5)
     return dict(scan_xyzi=scan, pose_true=np.asarray(pose_start, np.float64), pose_prev=pose_at(-dt), pose_next=pose_at(dt), prior=prior)
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# Ring-ordered raw scans (edge extraction, so_scan_extract_edges)
+# ---------------------------------------------------------------------------------------------------------------
+RING_STRIDE, RING_TIME_OFFSET, RING_RING_OFFSET = 32, 20, 24     # point_os::PointcloudXYZITR: time at byte 20, uint16 ring at byte 24
+
+
+def make_ring_scan(scene: Scene, sensor: str, pose7: np.ndarray, seed: int, order: str = "column", sweep_s: float = 0.1,
+                   range_noise: float = 0.01, rmin: float = 0.2, rmax: float = 130.0) -> np.ndarray:
+    """A spinning-lidar scan as the driver delivers it: float32 [n, 8] point_os::PointcloudXYZITR records {x, y, z, pad, intensity,
+    time, ring (uint16 in the low half of float 6), pad}, sensor frame, ray-cast from the static pose7.  Ring r is the r-th lowest
+    beam; column c fires at t = c / n_cols * sweep_s, so (ring, time) is unique per point.  order "column" lists the points column
+    by column (the firing order), "ring" ring by ring.  Returns outside (rmin, rmax) are dropped."""
+    n_cols, n_rings = {"vlp16": (1800, 16), "os1_128": (1024, 128)}[sensor]
+    if order not in ("column", "ring"):
+        raise ValueError(order)
+    rng = np.random.default_rng(seed)
+    dirs = sensor_dirs(sensor)                                        # column-major, rings inner
+    rr = raycast(scene, pose7[:3], dirs @ quat_to_R(pose7[3:]).T)
+    rr = rr + rng.normal(0.0, range_noise, size=rr.shape)
+    col = np.repeat(np.arange(n_cols), n_rings)
+    ring = np.tile(np.arange(n_rings), n_cols)
+    if order == "ring":
+        perm = np.lexsort((col, ring))
+        dirs, rr, col, ring = dirs[perm], rr[perm], col[perm], ring[perm]
+    ok = np.isfinite(rr) & (rr > rmin) & (rr < rmax)
+    n = int(ok.sum())
+    rec = np.zeros((n, 8), np.float32)
+    rec[:, :3] = dirs[ok] * rr[ok, None]
+    rec[:, 4] = rng.uniform(0.0, 255.0, n)
+    rec[:, 5] = (col[ok] / n_cols * sweep_s).astype(np.float32)
+    rec.view(np.uint16)[:, 12] = ring[ok].astype(np.uint16)
+    return rec
+
+
+def make_corridor_scene() -> Scene:
+    """A 400 m x 6 m corridor (x along it, walls at y = +-3, floor -1.8, ceiling 3.2; the end walls at x = +-200 lie beyond the
+    130 m range) with free-standing 0.1 m square floor-to-ceiling poles every 4 m, 1 m off each wall.  Pole centres sit at
+    x = 2 + 4i, so no face plane comes within 1 m of the origin."""
+    room = np.array([-200.0, 200.0, -3.0, 3.0, -1.8, 3.2])
+    boxes = []
+    for cx in np.arange(-198.0, 199.0, 4.0):
+        for cy in (-2.0, 2.0):
+            boxes.append([cx - 0.05, cx + 0.05, cy - 0.05, cy + 0.05, -1.8, 3.2])
+    return Scene(room=room, boxes=np.array(boxes, np.float64))
