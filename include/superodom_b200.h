@@ -40,6 +40,9 @@ extern "C" {
 #define SO_OK 0
 #define SO_STATUS_NOT_ENOUGH_FEATURES 1 /* hasEnoughFeatures() false: pose = prior (LidarSlam.cpp:113-116,379-381) */
 #define SO_STATUS_NO_CORRESPONDENCES 2  /* every scan point was rejected; reference would CHECK-fail in ceres::Covariance */
+#define SO_STATUS_INVALID_EVALUATION 3  /* the first evaluation of an ICP iteration's solve has a non-finite cost: an edge row weighted NaN
+                                           (line fit on an exactly collinear neighbourhood); the reference CHECK-fails in ceres::Corrector.
+                                           pose = the pose that ICP iteration started from, its iter_cost NaN, cov and errors zero */
 #define SO_ERR_ARG (-1)
 #define SO_ERR_CUDA (-2)
 #define SO_ERR_CAPACITY (-3)
@@ -99,7 +102,8 @@ typedef struct {
     int32_t hist_reject_plane[7]; /* MatchRejectionHistogramPlane of the last ICP iteration */
     int32_t hist_reject_line[7];  /* MatchRejectionHistogramLine of the last ICP iteration (all 0 without an edge cloud) */
     double cov[36];               /* RegistrationError::Covariance, row-major, order x,y,z,rx,ry,rz */
-    double pos_err, pos_dir[3], pos_inv_cond;     /* PositionError, PositionErrorDirection, PosInverseConditionNum */
+    double pos_err, pos_dir[3], pos_inv_cond;     /* PositionError, PositionErrorDirection, PosInverseConditionNum (a negative
+                                                     rounding of the smallest eigenvalue below a cut direction reads as 0, not NaN) */
     double ori_err_deg, ori_dir[3], ori_inv_cond; /* OrientationError (degrees), ...Direction, OriInverseConditionNum */
     double total_translation, total_rotation, translation_from_last, rotation_from_last; /* stats.* (LidarSlam.cpp:198-210) */
     int32_t map_surf_5x5, map_edge_5x5, scan_surf_num, scan_edge_num; /* stats.laser_cloud_* (LidarSlam.cpp:371-377) */
@@ -370,6 +374,13 @@ int so_correspond_edge(so_ctx* ctx, const void* edge_xyzi, size_t n, size_t stri
 /* Robustified normal equations at `pose` over the correspondences of the last so_correspond call:
  * H = sum rho' J^T J (row-major 6x6), g = sum rho' J^T r, cost = 1/2 sum rho (lidarOptimization.cpp:55-80 + Ceres corrector). */
 int so_evaluate(so_ctx* ctx, const double pose[7], double H[36], double g[6], double* cost);
+/* Test hook: the end of a registration on a given normal matrix -- ceres::Covariance's pseudo-inverse (directions with
+ * sqrt(w_i / w_max) < 1e-7 cut, and every smaller one with them) and EstimateRegistrationError's 3x3 analyses (LidarSlam.cpp:854-884),
+ * by the device code a registration ends with, in a one-CTA launch.  H: symmetric n x n, row-major, upper triangle read; n = 6
+ * (so_register*) or 12 (so_register_optimized*: T's columns first, T's 6x6 block reported).  Fills out->cov, pos_err, pos_dir,
+ * pos_inv_cond, ori_err_deg, ori_dir, ori_inv_cond and zeroes the rest.  Replaces the state a preceding so_correspond* left for
+ * so_evaluate. */
+int so_covariance(so_ctx* ctx, const double* H, int32_t n, so_icp_result* out);
 
 /* ---- neighbour search (LocalMap::nearestKSearchSurf, LocalMap.h:481-525) --------------------------- */
 /* k nearest map points IN THE QUERY'S OWN 50 m BLOCK for nq world-frame queries (packed xyz floats, 12 B stride or

@@ -9,6 +9,7 @@ compiled verbatim) and falls back to oracle/libso_oracle.so (restatement only).
 from __future__ import annotations
 
 import ctypes as C
+import hashlib
 import os
 import subprocess
 
@@ -54,15 +55,30 @@ EDGE_CORR_DTYPE = np.dtype([("p", "<f8", 3), ("a", "<f8", 3), ("b", "<f8", 3), (
                             ("n_sel", "<i4"), ("status", "<i4")], align=True)
 
 
+def _source_id() -> str:
+    """First 16 hex digits of so_oracle.cpp's SHA-256 (what the Makefile compiles into the library)."""
+    with open(os.path.join(_HERE, "so_oracle.cpp"), "rb") as f:
+        return hashlib.sha256(f.read()).hexdigest()[:16]
+
+
+def _built_from_source(path: str) -> bool:
+    """path exists and was compiled from the so_oracle.cpp beside this file (file times cannot tell: a checkout or a copy
+    sets them)."""
+    if not os.path.exists(path):
+        return False
+    with open(path, "rb") as f:
+        return b"so_oracle source id " + _source_id().encode() + b";" in f.read()
+
+
 def build(force: bool = False) -> None:
     """Compile the oracle (plain lib always; _ref lib when /root/reference exists)."""
     lib = os.path.join(_HERE, "libso_oracle.so")
-    src = os.path.join(_HERE, "so_oracle.cpp")
-    if force or not os.path.exists(lib) or os.path.getmtime(lib) < os.path.getmtime(src):
-        subprocess.check_call(["make", "-C", _HERE, "libso_oracle.so"], stdout=subprocess.DEVNULL)
+    sid = "SRC_ID=" + _source_id()
+    if force or not _built_from_source(lib):
+        subprocess.check_call(["make", "-B", "-C", _HERE, sid, "libso_oracle.so"], stdout=subprocess.DEVNULL)
     ref = os.path.join(_HERE, "_ref", "libso_oracle_ref.so")
-    if os.path.isdir("/root/reference") and (force or not os.path.exists(ref) or os.path.getmtime(ref) < os.path.getmtime(src)):
-        subprocess.check_call(["make", "-C", _HERE, "ref"], stdout=subprocess.DEVNULL)
+    if os.path.isdir("/root/reference") and (force or not _built_from_source(ref)):
+        subprocess.check_call(["make", "-C", _HERE, sid, "ref"], stdout=subprocess.DEVNULL)
 
 
 _lib = None
@@ -74,9 +90,11 @@ def lib():
         return _lib
     ref = os.path.join(_HERE, "_ref", "libso_oracle_ref.so")
     plain = os.path.join(_HERE, "libso_oracle.so")
-    if not os.path.exists(plain) and not os.path.exists(ref):
+    # a _ref library compiled from another version of so_oracle.cpp (it is rebuilt only where the reference tree exists) is not used
+    if not _built_from_source(ref) and not _built_from_source(plain):
         build()
-    path = ref if os.path.exists(ref) else plain
+    path = ref if _built_from_source(ref) else plain
+    assert _built_from_source(path), f"{path} was not compiled from {os.path.join(_HERE, 'so_oracle.cpp')}"
     L = C.CDLL(path)
     L.orc_map_create.restype = C.c_void_p
     L.orc_map_destroy.argtypes = [C.c_void_p]

@@ -852,6 +852,7 @@ struct Evaluator {
 
 struct SolveSummary { int num_successful_steps = 0, num_unsuccessful_steps = 0, iterations = 0, termination = 0; double initial_cost = 0, final_cost = 0; };
 // termination: 0 NO_CONVERGENCE(max iters) 1 gradient tol 2 parameter tol 3 function tol 4 radius 5 invalid steps 6 no residuals
+//              7 non-finite cost at the start (the reference aborts)
 
 // ceres::Solve with options {max_num_iterations=4, DENSE_QR} (LidarSlam.cpp:230-240), everything else default:
 // TrustRegionMinimizer::Minimize + LevenbergMarquardtStrategy + TrustRegionStepEvaluator(monotonic).
@@ -876,6 +877,9 @@ static SolveSummary ceres_solve(const Evaluator& E, double params[7], int max_nu
     auto scale_columns = [&]() { for (int j = 0; j < 6; ++j) { double* c = &J[size_t(j) * n]; for (size_t i = 0; i < n; ++i) c[i] *= scale[j]; } };
     // IterationZero
     E.full(x, &x_cost, res, J, g);
+    // a non-finite loss weight (ScaledLoss(TukeyLoss, w), w = NaN) makes the cost NaN: Ceres 2.0 CHECK-fails in the Corrector of that
+    // residual block (corrector.cc: neither rho'' <= 0 nor rho' > 0 holds) and ends the process; reported as termination 7
+    if (!std::isfinite(x_cost)) { S.termination = 7; S.initial_cost = S.final_cost = x_cost; return S; }
     for (int j = 0; j < 6; ++j) { double s = 0; const double* c = &J[size_t(j) * n]; for (size_t i = 0; i < n; ++i) s += c[i] * c[i]; scale[j] = 1.0 / (1.0 + std::sqrt(s)); }
     scale_columns();
     double gmax = grad_max_norm(x, g);
@@ -983,6 +987,13 @@ static void manual_yaw_correction(const double last[7], double T[7], double yaw_
 }  // namespace orc
 
 // ============================================================================= C API (ctypes)
+// Which source this library was compiled from (oracle.py reads it out of the file): a library left from another version of this
+// file, e.g. a prebuilt _ref/ that cannot be rebuilt where the reference tree is absent, is then not loaded.
+#ifndef SO_ORACLE_SOURCE_ID
+#define SO_ORACLE_SOURCE_ID "unknown"
+#endif
+__attribute__((used)) static const char kOracleSourceId[] = "so_oracle source id " SO_ORACLE_SOURCE_ID ";";
+
 extern "C" {
 
 #define ORC_MAX_ICP_ITERS 32
@@ -1278,6 +1289,11 @@ int orc_register_full(void* m, const float* scan_xyzi, size_t n, const float* ed
         rel_motion(prev, T, &out->iter_dtrans[it], &out->iter_drot[it]);
         out->iter_lm_steps[it] = S.iterations; out->iter_lm_successful[it] = S.num_successful_steps; out->iter_lm_termination[it] = S.termination; out->iter_cost[it] = S.final_cost;
         out->n_iterations = it + 1;
+        if (S.termination == 7) {                                 // SO_STATUS_INVALID_EVALUATION: no step, no covariance
+            out->iter_lm_steps[it] = out->iter_lm_successful[it] = out->iter_lm_termination[it] = 0;
+            out->status = 3;
+            break;
+        }
         if (S.num_successful_steps == 1 || it == max_iters - 1) {     // (:141-146)
             if (!E.blocks.empty() || !E.edges.empty()) {
                 ceres_covariance(E, T, out->cov); have_cov = true;

@@ -21,7 +21,7 @@ EXPORTS = [
     "so_map_set_resolution", "so_map_set_origin", "so_map_get_origin", "so_map_shift", "so_map_set_points",
     "so_map_set_edge_points", "so_map_add_surf", "so_map_add_edge", "so_map_add_scan", "so_map_add_registered_scan", "so_map_add_scan_edge", "so_map_counts_5x5", "so_map_download", "so_map_size",
     "so_scan_prefilter", "so_scan_deskew", "so_scan_extract_uniform", "so_scan_extract_edges", "so_register", "so_register_prefiltered", "so_register_injected", "so_set_pose_sink", "so_register_batch", "so_register_batch_edges", "so_register_batch_device",
-    "so_register_undistort", "so_register_prefiltered_undistort", "so_register_batch_undistort", "so_undistort_points", "so_register_optimized", "so_register_prefiltered_optimized", "so_register_batch_optimized", "so_evaluate_optimized", "so_correspond", "so_correspond_edge", "so_evaluate",
+    "so_register_undistort", "so_register_prefiltered_undistort", "so_register_batch_undistort", "so_undistort_points", "so_register_optimized", "so_register_prefiltered_optimized", "so_register_batch_optimized", "so_evaluate_optimized", "so_correspond", "so_correspond_edge", "so_evaluate", "so_covariance",
     "so_knn", "so_knn_device", "so_sampling_indices", "so_localize_global", "so_localize_scores", "so_localize_global_size", "so_localize_global_bnb", "so_localize_bnb_keys", "so_localize_bnb_bounds", "so_map_bounds", "so_kernel_launches", "so_bytes_copied", "so_build_flags", "so_profile_enable", "so_profile_get",
 ]
 
@@ -204,6 +204,7 @@ def load_library():
     L.so_correspond.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p, C.c_int32,
                                 C.c_void_p, C.c_void_p, C.c_void_p]
     L.so_evaluate.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.so_covariance.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]
     L.so_knn.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_int, C.c_float, C.c_void_p, C.c_void_p]
     L.so_knn_device.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_float, C.c_void_p, C.c_void_p]
     L.so_sampling_indices.argtypes = [C.c_uint32, C.c_int32, C.c_void_p, C.c_size_t, C.c_void_p]
@@ -666,6 +667,14 @@ class Context:
         cost = C.c_double()
         self._chk(self.L.so_evaluate(self.h, _p(pose), _p(H), _p(g), C.byref(cost)), "so_evaluate")
         return H, g, cost.value
+
+    def covariance(self, H) -> IcpResult:
+        """The covariance step that ends a registration, on a symmetric H [6, 6] or [12, 12]: cov and the error fields of the result."""
+        a = np.ascontiguousarray(H, dtype=np.float64)
+        assert a.ndim == 2 and a.shape[0] == a.shape[1] and a.shape[0] in (6, 12)
+        r = IcpResult()
+        self._chk(self.L.so_covariance(self.h, _p(a), a.shape[0], C.byref(r)), "so_covariance")
+        return r
 
     # ---- global localization
     def localize_global(self, scan_xyzi: np.ndarray, center_pose7, max_icp_iters: int, opts: GlobalOpts | None = None,

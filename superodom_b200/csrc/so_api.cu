@@ -1500,6 +1500,37 @@ int so_evaluate(so_ctx* ctx, const double pose[7], double H[36], double g[6], do
     return SO_OK;
 }
 
+int so_covariance(so_ctx* ctx, const double* H, int32_t n, so_icp_result* out) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c || !H || !out || (n != 6 && n != 12)) return fail(SO_ERR_ARG, "bad args");
+    SO_CUDA_TRY(cudaSetDevice(c->device));
+    IcpState& s = c->h_state[0];                              // the state of a preceding so_correspond* is replaced
+    std::memset(&s, 0, sizeof(s));
+    timed_launch_begin(c);
+    if (n == 6) {
+        for (int i = 0; i < 6; ++i) for (int j = i; j < 6; ++j) s.H[tri(i, j)] = H[i * 6 + j];
+        SO_CUDA_TRY(cudaMemcpyAsync(c->d_state, c->h_state, sizeof(IcpState), cudaMemcpyHostToDevice, c->stream));
+        launch_covariance(c->d_state, c->stream);
+    } else {
+        { int rc = grow_buffer(c->mot.d_st, c->mot.st_cap, std::max<size_t>(c->max_batch, 1)); if (rc) return rc; }
+        MotionState M{};
+        for (int i = 0; i < 12; ++i) for (int j = i; j < 12; ++j) M.H[i * 12 - (i * (i - 1)) / 2 + (j - i)] = H[i * 12 + j];
+        SO_CUDA_TRY(cudaMemcpyAsync(c->d_state, c->h_state, sizeof(IcpState), cudaMemcpyHostToDevice, c->stream));
+        SO_CUDA_TRY(cudaMemcpyAsync(c->mot.d_st, &M, sizeof(MotionState), cudaMemcpyHostToDevice, c->stream));
+        launch_covariance12(c->d_state, c->mot.d_st, c->stream);
+    }
+    c->launches++;
+    timed_launch_end(c, 1);
+    SO_CUDA_TRY(cudaGetLastError());
+    SO_CUDA_TRY(cudaMemcpyAsync(c->h_state, c->d_state, sizeof(IcpState), cudaMemcpyDeviceToHost, c->stream));
+    SO_CUDA_TRY(cudaStreamSynchronize(c->stream));
+    std::memset(out, 0, sizeof(*out));
+    std::memcpy(out->cov, s.cov, sizeof(out->cov));
+    out->pos_err = s.pos_err; out->pos_inv_cond = s.pos_inv_cond; out->ori_err_deg = s.ori_err_deg; out->ori_inv_cond = s.ori_inv_cond;
+    for (int i = 0; i < 3; ++i) { out->pos_dir[i] = s.pos_dir[i]; out->ori_dir[i] = s.ori_dir[i]; }
+    return SO_OK;
+}
+
 // ---- k-NN --------------------------------------------------------------------------------------------------------
 int so_knn_device(so_ctx* ctx, const void* d_q, size_t nq, int k, float max_d2, uint32_t* d_idx, float* d_d2) {
     Ctx* c = reinterpret_cast<Ctx*>(ctx);

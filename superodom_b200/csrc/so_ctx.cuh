@@ -319,6 +319,8 @@ void launch_motion_warp(const BatchView& bv, float4* sorted, const float4* raw, 
                         uint32_t grid_x, uint32_t n_scans, cudaStream_t st);
 void launch_motion_solve(int phase, const BatchView& bv, const CorrBuf& cb, const float4* raw, const float* times, MotionState* ms, uint32_t first,
                          double* partials, uint32_t stride, uint32_t grid_x, uint32_t n_scans, cudaStream_t st);
+// so_covariance: cov12_warp on ms->H into st's covariance and error fields (device memory)
+void launch_covariance12(IcpState* st, const MotionState* ms, cudaStream_t stream);
 // so_map.cu
 int map_alloc(Ctx* c);
 void map_free(Ctx* c);

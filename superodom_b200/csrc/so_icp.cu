@@ -78,7 +78,7 @@ __device__ __noinline__ double grad_max_norm(const double x[7], const double g[6
 }
 
 // ceres::Covariance + EstimateRegistrationError at the end of a registration, on the 32 lanes of the CTA's first warp (S and sc in
-// shared memory).  The 6x6 cyclic Jacobi (at most 30 sweeps, convergence test and FP32 angle of jacobi_eig) takes its rotations in
+// shared memory).  The 6x6 cyclic Jacobi (at most 30 sweeps, convergence test of jacobi_eig, FP64 angles) takes its rotations in
 // ROUND-ROBIN order: five rounds of three pairs with disjoint indices -- (0,5)(1,4)(2,3) / (0,4)(3,5)(1,2) / (0,3)(2,4)(1,5) /
 // (0,2)(1,3)(4,5) / (0,1)(2,5)(3,4).  The angle of a pair depends only on its own 2x2 block, which the other two rotations of the
 // round do not touch, so the three angles of a round are computed by three lanes at once; each rotation then updates its 8
@@ -115,11 +115,15 @@ __device__ __noinline__ void covariance_and_errors_warp(IcpState& S, CovScratch&
         for (int round = 0; round < 5; ++round) {
             if (lane < 3) {                                  // the three angles of the round (disjoint 2x2 blocks)
                 const int p = c_rr_p[round * 3 + lane], q = c_rr_q[round * 3 + lane];
+                // the angle in FP64: the update below (a_pp - t a_pq, a_qq + t a_pq, a_pq := 0) is exact only for the exact angle, and
+                // an FP32 one left a backward error of 1e-7 |a_pq| per rotation -- cov off by ~1e-8 kappa(H) relative
                 const double apq = sc.a[p * 6 + q];
-                const float dlt = float(sc.a[q * 6 + q] - sc.a[p * 6 + p]), b2 = float(2.0 * apq);
-                float tf = __fdividef(b2, fabsf(dlt) + sqrtf(fmaf(dlt, dlt, b2 * b2)));
-                if (!(fabsf(tf) <= 1.0f)) tf = 0.0f;         // apq == 0 after the cast (or inf / nan): no rotation
-                const double t = apq != 0.0 ? double(dlt < 0.0f ? -tf : tf) : 0.0;
+                double t = 0.0;
+                if (apq != 0.0) {
+                    const double dlt = sc.a[q * 6 + q] - sc.a[p * 6 + p], b2 = 2.0 * apq;
+                    t = b2 / (fabs(dlt) + sqrt(dlt * dlt + b2 * b2));
+                    if (dlt < 0.0) t = -t;
+                }
                 const double c = rsqrt(t * t + 1.0);
                 sc.t[lane] = t; sc.c[lane] = c; sc.s[lane] = t * c;
             }
@@ -194,8 +198,10 @@ __device__ __noinline__ void covariance_and_errors_warp(IcpState& S, CovScratch&
         for (int i = 0; i < 3; ++i)
 #pragma unroll
             for (int j = 0; j < 3; ++j) M[i * 3 + j] = S.cov[(i + o) * 6 + (j + o)];
-        jacobi_eig<3, 20>(M, E, e);
-        const double err = sqrt(e[2]), inv_cond = sqrt(e[0]) / sqrt(e[2]);
+        jacobi_eig<3, 20, true>(M, E, e);
+        // the block is positive semi-definite: below a cut direction its smallest eigenvalue is zero and comes out as +-rounding,
+        // read as 0 (the reference's sqrt of a negative rounding gives NaN; DESIGN.md section 3)
+        const double err = sqrt(e[2]), inv_cond = sqrt(fmax(e[0], 0.0)) / sqrt(e[2]);
         if (lane == 0) { S.pos_err = err; S.pos_dir[0] = E[2]; S.pos_dir[1] = E[5]; S.pos_dir[2] = E[8]; S.pos_inv_cond = inv_cond; }
         else { S.ori_err_deg = err / M_PI * 180.0; S.ori_dir[0] = E[2]; S.ori_dir[1] = E[5]; S.ori_dir[2] = E[8]; S.ori_inv_cond = inv_cond; }
     }
@@ -319,6 +325,17 @@ __device__ __noinline__ void lm_begin_solve(IcpState& st, const double* acc_in, 
     _Pragma("unroll") for (int i = 0; i < 7; ++i) st.x_iter_start[i] = st.x[i];
     st.lm_iter = 0; st.num_successful = 0; st.num_unsuccessful = 0; st.consecutive_invalid = 0; st.termination = 0;
     if (n_ok == 0 && !st.use_prior) { st.termination = 6; end_solve(st); return; }
+    if (!isfinite(st.cost)) {
+        // A row's loss weight is not finite (ScaledLoss(TukeyLoss, w) with w = NaN: a line fit on an exactly collinear neighbourhood,
+        // whose mean squared distance is rounding noise of either sign).  The reference CHECK-fails in ceres::Corrector here (Ceres
+        // 2.0 corrector.cc: neither rho'' <= 0 nor rho' > 0 holds for NaN) and ends the process; the registration stops with a status
+        // and the pose this ICP iteration started from (DESIGN.md section 3).
+        const int it = st.icp_iter;
+        st.iter_n_surf[it] = n_ok - st.n_ok_edge; st.iter_n_edge[it] = st.n_ok_edge; st.iter_cost[it] = st.cost;
+        st.n_iterations = it + 1;
+        st.status = SO_STATUS_INVALID_EVALUATION; st.phase = PH_DONE;
+        return;
+    }
     _Pragma("unroll") for (int j = 0; j < 6; ++j) st.scale[j] = 1.0 / (1.0 + sqrt(st.H[tri(j, j)]));      // jacobi_scaling at iteration 0
     double xn = 0.0; _Pragma("unroll") for (int i = 0; i < 7; ++i) xn += st.x[i] * st.x[i];
     st.x_norm = sqrt(xn);
@@ -1441,6 +1458,22 @@ __global__ void __launch_bounds__(128) k_lm_step(BatchView bv, uint32_t n_partia
     if (bv.st[s].phase != AFTER) return;
     lm_step_body<AFTER>(bv, s, n_partials, edge_partial_offset);
 }
+
+// so_covariance (6 columns): the covariance step that ends a registration, on st->H, in one 32-thread CTA and a shared copy of the
+// state as lm_step_body runs it
+__global__ void __launch_bounds__(32) k_covariance(IcpState* st) {
+    __shared__ IcpState s_st;
+    __shared__ CovScratch s_cov;
+    unsigned long long* sh = reinterpret_cast<unsigned long long*>(&s_st);
+    unsigned long long* gl = reinterpret_cast<unsigned long long*>(st);
+    for (uint32_t k = threadIdx.x; k < sizeof(IcpState) / 8; k += blockDim.x) sh[k] = gl[k];
+    __syncthreads();
+    covariance_and_errors_warp(s_st, s_cov);
+    __syncthreads();
+    for (uint32_t k = threadIdx.x; k < sizeof(IcpState) / 8; k += blockDim.x) gl[k] = sh[k];
+}
+
+void launch_covariance(IcpState* st, cudaStream_t stream) { k_covariance<<<1, 32, 0, stream>>>(st); }
 
 
 // ------------------------------------------------------------------------------------------------------------------

@@ -91,6 +91,8 @@ void launch_correspond(const MapView& m, const BatchView& bv, const CorrBuf& cb,
 void launch_evaluate(const BatchView& bv, const CorrBuf& cb, uint32_t grid_x, uint32_t n_scans, cudaStream_t st, const EdgeBuf* eb = nullptr, uint32_t grid_e = 0);
 void launch_loop_cond(const BatchView& bv, uint32_t n_scans, cudaGraphConditionalHandle handle, cudaStream_t st);
 void launch_pack_poses(const IcpState* st, uint32_t n_scans, double* rows, cudaStream_t stream);
+// so_covariance: covariance_and_errors_warp on st->H (one scan's state, device memory)
+void launch_covariance(IcpState* st, cudaStream_t stream);
 void launch_query_keys(const MapView& m, const float4* q, size_t nq, uint32_t* keys, uint32_t* vals, cudaStream_t st);
 int launch_knn(const MapView& m, const float4* q, const uint32_t* order, size_t nq, int k, float max_d2, uint32_t* idx, float* d2, cudaStream_t st);
 

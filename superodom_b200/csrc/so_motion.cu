@@ -461,13 +461,32 @@ __device__ __noinline__ void cov12_warp(IcpState& S, const MotionState& M, Cov12
         double Mx[9], E[9], ev[3];
         const int o = lane * 3;
         for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) Mx[i * 3 + j] = S.cov[(i + o) * 6 + (j + o)];
-        jacobi_eig<3, 20>(Mx, E, ev);
-        const double err = sqrt(ev[2]), inv_cond = sqrt(ev[0]) / sqrt(ev[2]);
+        jacobi_eig<3, 20, true>(Mx, E, ev);
+        const double err = sqrt(ev[2]), inv_cond = sqrt(fmax(ev[0], 0.0)) / sqrt(ev[2]);     // as covariance_and_errors_warp
         if (lane == 0) { S.pos_err = err; S.pos_dir[0] = E[2]; S.pos_dir[1] = E[5]; S.pos_dir[2] = E[8]; S.pos_inv_cond = inv_cond; }
         else { S.ori_err_deg = err / M_PI * 180.0; S.ori_dir[0] = E[2]; S.ori_dir[1] = E[5]; S.ori_dir[2] = E[8]; S.ori_inv_cond = inv_cond; }
     }
     __syncwarp();
 }
+
+// so_covariance (12 columns): cov12_warp on ms->H, in one 32-thread CTA and shared copies of both blocks as k_motion_step runs it
+__global__ void __launch_bounds__(32) k_covariance12(IcpState* st, const MotionState* ms) {
+    __shared__ IcpState s_st;
+    __shared__ MotionState s_m;
+    __shared__ Cov12 s_cov;
+    unsigned long long* sh = reinterpret_cast<unsigned long long*>(&s_st);
+    unsigned long long* gl = reinterpret_cast<unsigned long long*>(st);
+    for (uint32_t k = threadIdx.x; k < sizeof(IcpState) / 8; k += blockDim.x) sh[k] = gl[k];
+    const unsigned long long* gm = reinterpret_cast<const unsigned long long*>(ms);
+    unsigned long long* sm = reinterpret_cast<unsigned long long*>(&s_m);
+    for (uint32_t k = threadIdx.x; k < sizeof(MotionState) / 8; k += blockDim.x) sm[k] = gm[k];
+    __syncthreads();
+    cov12_warp(s_st, s_m, s_cov);
+    __syncthreads();
+    for (uint32_t k = threadIdx.x; k < sizeof(IcpState) / 8; k += blockDim.x) gl[k] = sh[k];
+}
+
+void launch_covariance12(IcpState* st, const MotionState* ms, cudaStream_t stream) { k_covariance12<<<1, 32, 0, stream>>>(st, ms); }
 
 template <int AFTER>
 __global__ void __launch_bounds__(128) k_motion_step(BatchView bv, MotionState* __restrict__ ms, const double* __restrict__ partials, uint32_t stride) {

@@ -9,6 +9,7 @@ import numpy as np
 import pytest
 
 import ref_octree_golden
+import solve_numerics_ref
 from conftest import get_case, quat_angle
 
 pytestmark = pytest.mark.gpu
@@ -622,10 +623,15 @@ def test_edge_line_branch_correspondences(gpu_api, oracle_mod):
     swap = np.abs(gc["a"][ok] - oc["b"][ok]).max(1) + np.abs(gc["b"][ok] - oc["a"][ok]).max(1)
     assert (np.minimum(same, swap) < 1e-7).all()          # eigenvector of a 2-10 point scatter: conditioning-limited
     assert np.allclose(gc["w"][ok], oc["w"][ok], rtol=1e-9)
-    # normal equations of the edge rows alone
+    # normal equations of the edge rows alone, against the restated line rows on the device's own (a, b, w)
+    # (tests/test_solve_numerics.py covers more poses and inputs)
+    a2 = solve_numerics_ref.tukey_a2(0.1)
     for pose in (case["pose_prior"], case["pose_true"]):
         H, g, cost = ctx.evaluate(pose)
-        r = om.register(np.zeros((0, 4), np.float32), pose, 0.2, 1, edge_xyzi=es, line_res=0.1, skip_map_checks=True)   # noqa: F841 (smoke)
+        rH, rg, rcost, _ = solve_numerics_ref.line_normal_equations(es[ok, :3].astype(np.float64), gc["a"][ok], gc["b"][ok], gc["w"][ok], pose, a2)
+        assert np.abs(H - rH).max() <= 1e-10 * np.abs(rH).max()
+        assert np.abs(g - rg).max() <= 1e-10 * max(np.abs(rg).max(), 1e-3 * np.abs(rH).max())
+        assert abs(cost - rcost) <= 1e-10 * rcost
     ctx.close()
 
 
