@@ -181,7 +181,7 @@ int so_map_add_scan(so_ctx* ctx, const void* xyzi, size_t n, size_t stride_bytes
  * so_register_optimized and their prefiltered forms, so_localize_global*), which is still in device memory: the live loop
  * Localization() -> transformAndAddToMap() (LidarSlam.cpp:155-171) without uploading the scan a second time.  Fails with SO_ERR_ARG,
  * before any device work, when a call that reuses the scan buffers ran in between: so_scan_prefilter, so_scan_deskew,
- * so_scan_extract_uniform, so_correspond, so_register_injected, the host batches so_register_batch*, so_evaluate_optimized (not
+ * so_scan_extract_uniform, so_correspond, so_correspond_seeded, so_register_injected, the host batches so_register_batch*, so_evaluate_optimized (not
  * so_register_batch_device, the k-NN, the other map calls, so_undistort_points or so_correspond_edge).  SO_OK and nothing inserted
  * before the first registration. */
 int so_map_add_registered_scan(so_ctx* ctx, const double pose[7]);
@@ -368,6 +368,14 @@ int so_register_injected(so_ctx* ctx, const void* surf_xyzi, size_t n_surf, size
 /* processPlannerFeatures at a fixed pose (LidarSlam.cpp:323-344): fills corr[n], hist_obs[9], hist_rej[7]. */
 int so_correspond(so_ctx* ctx, const void* surf_xyzi, size_t n, size_t stride_bytes, size_t intensity_offset,
                   const double pose[7], int32_t max_surface_features, so_corr* corr, int32_t hist_obs[9], int32_t hist_rej[7]);
+/* Test hook: the correspondences of ICP iteration 1 -- the search that takes its bound from the previous iteration's neighbours.
+ * The scan is ordered at pose_prev, as a registration starting there orders it; iteration 0's search and fit run at pose_prev
+ * unreported; then iteration 1's search and fit run at `pose` on the neighbour records iteration 0 left, and fill corr[n],
+ * hist_obs[9] and hist_rej[7] as so_correspond does.  The seed only prunes: the result equals so_correspond at `pose`.  so_evaluate
+ * then uses iteration 1's correspondences.  Argument errors and side effects are those of so_correspond. */
+int so_correspond_seeded(so_ctx* ctx, const void* surf_xyzi, size_t n, size_t stride_bytes, size_t intensity_offset,
+                         const double pose[7], int32_t max_surface_features, so_corr* corr, int32_t hist_obs[9], int32_t hist_rej[7],
+                         const double pose_prev[7]);
 /* processEdgeFeatures at a fixed pose (LidarSlam.cpp:310-321): fills corr[n], hist_rej_line[7]. */
 int so_correspond_edge(so_ctx* ctx, const void* edge_xyzi, size_t n, size_t stride_bytes, size_t intensity_offset, const double pose[7],
                        so_edge_corr* corr, int32_t hist_rej_line[7]);

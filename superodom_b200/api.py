@@ -21,7 +21,7 @@ EXPORTS = [
     "so_map_set_resolution", "so_map_set_origin", "so_map_get_origin", "so_map_shift", "so_map_set_points",
     "so_map_set_edge_points", "so_map_add_surf", "so_map_add_edge", "so_map_add_scan", "so_map_add_registered_scan", "so_map_add_scan_edge", "so_map_counts_5x5", "so_map_download", "so_map_size",
     "so_scan_prefilter", "so_scan_deskew", "so_scan_extract_uniform", "so_scan_extract_edges", "so_register", "so_register_prefiltered", "so_register_injected", "so_set_pose_sink", "so_register_batch", "so_register_batch_edges", "so_register_batch_device",
-    "so_register_undistort", "so_register_prefiltered_undistort", "so_register_batch_undistort", "so_undistort_points", "so_register_optimized", "so_register_prefiltered_optimized", "so_register_batch_optimized", "so_evaluate_optimized", "so_correspond", "so_correspond_edge", "so_evaluate", "so_covariance",
+    "so_register_undistort", "so_register_prefiltered_undistort", "so_register_batch_undistort", "so_undistort_points", "so_register_optimized", "so_register_prefiltered_optimized", "so_register_batch_optimized", "so_evaluate_optimized", "so_correspond", "so_correspond_seeded", "so_correspond_edge", "so_evaluate", "so_covariance",
     "so_knn", "so_knn_device", "so_sampling_indices", "so_localize_global", "so_localize_scores", "so_localize_global_size", "so_localize_global_bnb", "so_localize_bnb_keys", "so_localize_bnb_bounds", "so_map_bounds", "so_kernel_launches", "so_bytes_copied", "so_build_flags", "so_profile_enable", "so_profile_get",
 ]
 
@@ -203,6 +203,7 @@ def load_library():
     L.so_register_batch_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p]
     L.so_correspond.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p, C.c_int32,
                                 C.c_void_p, C.c_void_p, C.c_void_p]
+    L.so_correspond_seeded.argtypes = list(L.so_correspond.argtypes) + [C.c_void_p]
     L.so_evaluate.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     L.so_covariance.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]
     L.so_knn.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_int, C.c_float, C.c_void_p, C.c_void_p]
@@ -649,15 +650,21 @@ class Context:
                   "so_register_batch_device")
         return res
 
-    def correspond(self, scan_xyzi: np.ndarray, pose7, max_surface_features: int = 0):
+    def correspond(self, scan_xyzi: np.ndarray, pose7, max_surface_features: int = 0, seed_pose=None):
+        """Correspondences at pose7 -> (corr, hist_obs, hist_rej).  seed_pose: run them as ICP iteration 1 of a registration that
+        started at seed_pose, searching with the bound iteration 0's neighbours give (so_correspond_seeded)."""
         s = np.ascontiguousarray(scan_xyzi, dtype=np.float32)
         pose = np.ascontiguousarray(pose7, dtype=np.float64)
         corr = np.zeros(s.shape[0], CORR_DTYPE)
         ho = np.zeros(9, np.int32)
         hr = np.zeros(7, np.int32)
         stride = s.shape[1] * 4
-        self._chk(self.L.so_correspond(self.h, _p(s), s.shape[0], stride, 12 if s.shape[1] >= 4 else stride, _p(pose),
-                                       max_surface_features, _p(corr), _p(ho), _p(hr)), "so_correspond")
+        args = (self.h, _p(s), s.shape[0], stride, 12 if s.shape[1] >= 4 else stride, _p(pose), max_surface_features, _p(corr), _p(ho), _p(hr))
+        if seed_pose is None:
+            self._chk(self.L.so_correspond(*args), "so_correspond")
+        else:
+            prev = np.ascontiguousarray(seed_pose, dtype=np.float64)
+            self._chk(self.L.so_correspond_seeded(*args, _p(prev)), "so_correspond_seeded")
         return corr, ho, hr
 
     def evaluate(self, pose7):

@@ -1388,10 +1388,10 @@ int so_set_pose_sink(so_ctx* ctx, void* d_rows, size_t cap_rows, size_t first_ro
 }
 
 // ---- stage-level entry points ------------------------------------------------------------------------------------
-int so_correspond(so_ctx* ctx, const void* surf, size_t n, size_t stride, size_t ioff, const double pose[7], int32_t max_surface_features,
-                  so_corr* corr, int32_t hist_obs[9], int32_t hist_rej[7]) {
-    Ctx* c = reinterpret_cast<Ctx*>(ctx);
-    if (!c || !surf || !pose || !corr || n == 0 || stride < 12) return fail(SO_ERR_ARG, "bad args");
+// so_correspond / so_correspond_seeded: pose_prev == nullptr -> the search and fit of iteration 0 at `pose`; otherwise the scan is
+// ordered at pose_prev, iteration 0 runs there unreported, and iteration 1 runs at `pose` on the neighbour records it left.
+static int correspond_stage(Ctx* c, const void* surf, size_t n, size_t stride, size_t ioff, const double pose[7], const double* pose_prev,
+                            int32_t max_surface_features, so_corr* corr, int32_t hist_obs[9], int32_t hist_rej[7]) {
     if (n > c->cfg.max_scan_points) return fail(SO_ERR_CAPACITY, "scan larger than so_config.max_scan_points");
     SO_CUDA_TRY(cudaSetDevice(c->device));
     { int rc0 = ensure_maps(c); if (rc0) return rc0; }
@@ -1399,7 +1399,7 @@ int so_correspond(so_ctx* ctx, const void* surf, size_t n, size_t stride, size_t
     int rc = upload_cloud(c, surf, n, stride, ioff, c->d_scan);
     if (rc) return rc;
     so_icp_opts o{}; o.max_icp_iters = -1; o.lm_max_iterations = 4; o.max_surface_features = max_surface_features;
-    init_state(c->h_state[0], pose, uint32_t(n), o);
+    init_state(c->h_state[0], pose_prev ? pose_prev : pose, uint32_t(n), o);
     c->h_offset[0] = 0;
     SO_CUDA_TRY(cudaMemcpyAsync(c->d_state, c->h_state, sizeof(IcpState), cudaMemcpyHostToDevice, c->stream));
     SO_CUDA_TRY(cudaMemcpyAsync(c->d_offset, c->h_offset, sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
@@ -1412,6 +1412,14 @@ int so_correspond(so_ctx* ctx, const void* surf, size_t n, size_t stride, size_t
     bv.coop_knn = grid_x <= kCoopMaxGrid && !c->no_coop_knn;            // as a single small registration would search
     timed_launch_begin(c); launch_correspond(mv, bv, c->corr, c->nn, grid_x, 1, c->stream); c->launches += 2 + 2; timed_launch_end(c, 0);
     SO_CUDA_TRY(cudaGetLastError());
+    if (pose_prev) {
+        // iteration 1 at `pose`: same scan order, the neighbour records (pre, d5, pos) of iteration 0 are what seed_bound reads
+        init_state(c->h_state[0], pose, uint32_t(n), o);
+        c->h_state[0].icp_iter = 1;
+        SO_CUDA_TRY(cudaMemcpyAsync(c->d_state, c->h_state, sizeof(IcpState), cudaMemcpyHostToDevice, c->stream));
+        timed_launch_begin(c); launch_correspond(mv, bv, c->corr, c->nn, grid_x, 1, c->stream); c->launches += 2 + 2; timed_launch_end(c, 0);
+        SO_CUDA_TRY(cudaGetLastError());
+    }
     std::vector<double4> nd(n); std::vector<double> w(n); std::vector<uchar4> fl(n); std::vector<uint32_t> nn(n * 5); std::vector<float> d2(n * 5);
     std::vector<float4> sorted(n);
     SO_CUDA_TRY(cudaMemcpyAsync(nd.data(), c->corr.nd, n * sizeof(double4), cudaMemcpyDeviceToHost, c->stream));
@@ -1434,6 +1442,20 @@ int so_correspond(so_ctx* ctx, const void* surf, size_t n, size_t stride, size_t
     if (hist_obs) std::memcpy(hist_obs, c->h_state[0].hist_obs, 9 * sizeof(int32_t));
     if (hist_rej) std::memcpy(hist_rej, c->h_state[0].hist_rej, 7 * sizeof(int32_t));
     return SO_OK;
+}
+
+int so_correspond(so_ctx* ctx, const void* surf, size_t n, size_t stride, size_t ioff, const double pose[7], int32_t max_surface_features,
+                  so_corr* corr, int32_t hist_obs[9], int32_t hist_rej[7]) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c || !surf || !pose || !corr || n == 0 || stride < 12) return fail(SO_ERR_ARG, "bad args");
+    return correspond_stage(c, surf, n, stride, ioff, pose, nullptr, max_surface_features, corr, hist_obs, hist_rej);
+}
+
+int so_correspond_seeded(so_ctx* ctx, const void* surf, size_t n, size_t stride, size_t ioff, const double pose[7], int32_t max_surface_features,
+                         so_corr* corr, int32_t hist_obs[9], int32_t hist_rej[7], const double pose_prev[7]) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c || !surf || !pose || !corr || n == 0 || stride < 12 || !pose_prev) return fail(SO_ERR_ARG, "bad args");
+    return correspond_stage(c, surf, n, stride, ioff, pose, pose_prev, max_surface_features, corr, hist_obs, hist_rej);
 }
 
 int so_correspond_edge(so_ctx* ctx, const void* edge, size_t n, size_t stride, size_t ioff, const double pose[7], so_edge_corr* corr,

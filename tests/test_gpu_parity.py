@@ -11,6 +11,7 @@ import pytest
 import ref_octree_golden
 import solve_numerics_ref
 from conftest import get_case, quat_angle
+from search_sets import knn_case as _knn_case
 
 pytestmark = pytest.mark.gpu
 
@@ -34,57 +35,6 @@ def _gi(idx):
 def _assert_pose_close(pg, po, tol_m=POSE_TOL_M, tol_r=POSE_TOL_RAD):
     assert np.abs(pg[:3] - po[:3]).max() <= tol_m, (pg, po)
     assert quat_angle(pg[3:], po[3:]) <= tol_r, (pg, po)
-
-
-def _cell_faces(plane_res, lo, hi):
-    """float32 coordinates in [lo, hi) of the k-NN grid's cell faces (cell edge 50 / nb, nb = min(192, floor(100 / sqrt(3 planeRes)))
-    cells per 50 m block, DESIGN section 2), with the float32 neighbours on either side of each."""
-    nb = min(192, int(100.0 / np.sqrt(3.0 * np.float64(np.float32(plane_res)))))
-    j = np.arange(int(np.floor((lo + 25.0) * nb / 50.0)), int(np.ceil((hi + 25.0) * nb / 50.0)) + 1)
-    f = (-25.0 + j * (50.0 / nb)).astype(np.float32)
-    f = f[(f >= lo) & (f < hi)]
-    return f, np.nextafter(f, np.float32(-np.inf)), np.nextafter(f, np.float32(np.inf))
-
-
-def _knn_case(name):
-    """(map_xyzi, plane_res, queries) for test_knn_bit_exact.  lattice: voxel centres at planeRes spacing, a second lattice
-    whose planes lie on the grid's cell faces (and one float32 step either side), exact distance ties everywhere; queries on lattice
-    points, midpoints, faces and at random.  dense: clusters of 6-64 coincident or nearly coincident points, so that far more than
-    the 24 candidates the search buffers fall inside its bound."""
-    rng = np.random.default_rng(0)
-    if name not in ("lattice", "dense"):
-        case = get_case(name)
-        base = case["map_xyzi"][::7, :3]
-        q = base + rng.normal(0, 0.12, size=base.shape).astype(np.float32)
-        q = np.concatenate([q, rng.uniform(-30, 30, size=(500, 3)).astype(np.float32) + q.mean(0)])     # incl. far-away queries
-        return case["map_xyzi"], case["cfg"]["plane_res"], q
-    pr = 0.2
-    if name == "lattice":
-        g = (np.arange(-30, 30) + 0.5) * pr
-        a = np.stack(np.meshgrid(g, g, (np.arange(-3, 3) + 0.5) * pr, indexing="ij"), -1).reshape(-1, 3)
-        fx, fxm, fxp = _cell_faces(pr, 8.0, 12.0)
-        fz, fzm, fzp = _cell_faces(pr, -1.0, 1.0)
-        xs = np.concatenate([fx, fxm[::3], fxp[1::3]])
-        zs = np.concatenate([fz, fzm[::2], fzp[1::2]])
-        b = np.stack(np.meshgrid(xs, np.float32(fx - 20.0), zs, indexing="ij"), -1).reshape(-1, 3)
-        pts = np.concatenate([a.astype(np.float32), b.astype(np.float32)])
-        q = np.concatenate([pts[rng.choice(len(pts), 3000, replace=False)],
-                            (pts[rng.choice(len(a), 2000)] + np.float32(pr / 2) * rng.integers(0, 2, size=(2000, 3))).astype(np.float32),
-                            np.stack([rng.choice(fx, 2000), rng.uniform(-6, 6, 2000), rng.choice(fz, 2000)], 1).astype(np.float32),
-                            np.stack([rng.uniform(8, 12, 2000), rng.choice(np.float32(fx - 20.0), 2000), rng.uniform(-1, 1, 2000)], 1).astype(np.float32),
-                            rng.uniform(-7, 13, size=(2000, 3)).astype(np.float32) * np.float32([1, 1, 0.2])])
-    else:
-        cen = rng.uniform(-5, 5, size=(600, 3)) * [1, 1, 0.3]
-        pts = []
-        for i, c in enumerate(cen):
-            n = int(rng.integers(6, 65))
-            jit = [0.0, 1e-6, 1e-4, 1e-2][i % 4]
-            pts.append(c + rng.normal(0, jit, size=(n, 3)) if jit else np.repeat(c[None], n, 0))
-        pts = np.concatenate(pts).astype(np.float32)
-        q = np.concatenate([cen.astype(np.float32), (cen + rng.normal(0, 0.1, size=cen.shape)).astype(np.float32),
-                            ((cen[:-1] + cen[1:]) / 2).astype(np.float32), rng.uniform(-6, 6, size=(2000, 3)).astype(np.float32) * np.float32([1, 1, 0.3])])
-    xyzi = np.concatenate([pts, np.ones((len(pts), 1), np.float32)], 1)
-    return xyzi, pr, q
 
 
 @pytest.mark.parametrize("name", ["tiny", "cfg1", "hall", "lattice", "dense"])
