@@ -376,6 +376,10 @@ int so_correspond(so_ctx* ctx, const void* surf_xyzi, size_t n, size_t stride_by
 int so_correspond_seeded(so_ctx* ctx, const void* surf_xyzi, size_t n, size_t stride_bytes, size_t intensity_offset,
                          const double pose[7], int32_t max_surface_features, so_corr* corr, int32_t hist_obs[9], int32_t hist_rej[7],
                          const double pose_prev[7]);
+/* Test hook: the first n points of the cell-ordered scan buffer the kernels read, as the last registration left it: packed float4
+ * {x, y, z, w} per point, scans at their batch offsets, w = the point's index inside its scan (uint32 bit pattern).  Meaningful after
+ * a so_register_batch* call of mode 0 (modes 1 and 2 rewrite x, y, z every ICP iteration); n <= so_config.max_scan_points * max_batch. */
+int so_ordered_scans(so_ctx* ctx, float* out_xyzw, size_t n);
 /* processEdgeFeatures at a fixed pose (LidarSlam.cpp:310-321): fills corr[n], hist_rej_line[7]. */
 int so_correspond_edge(so_ctx* ctx, const void* edge_xyzi, size_t n, size_t stride_bytes, size_t intensity_offset, const double pose[7],
                        so_edge_corr* corr, int32_t hist_rej_line[7]);

@@ -21,7 +21,7 @@ EXPORTS = [
     "so_map_set_resolution", "so_map_set_origin", "so_map_get_origin", "so_map_shift", "so_map_set_points",
     "so_map_set_edge_points", "so_map_add_surf", "so_map_add_edge", "so_map_add_scan", "so_map_add_registered_scan", "so_map_add_scan_edge", "so_map_counts_5x5", "so_map_download", "so_map_size",
     "so_scan_prefilter", "so_scan_deskew", "so_scan_extract_uniform", "so_scan_extract_edges", "so_register", "so_register_prefiltered", "so_register_injected", "so_set_pose_sink", "so_register_batch", "so_register_batch_edges", "so_register_batch_device",
-    "so_register_undistort", "so_register_prefiltered_undistort", "so_register_batch_undistort", "so_undistort_points", "so_register_optimized", "so_register_prefiltered_optimized", "so_register_batch_optimized", "so_evaluate_optimized", "so_correspond", "so_correspond_seeded", "so_correspond_edge", "so_evaluate", "so_covariance",
+    "so_register_undistort", "so_register_prefiltered_undistort", "so_register_batch_undistort", "so_undistort_points", "so_register_optimized", "so_register_prefiltered_optimized", "so_register_batch_optimized", "so_evaluate_optimized", "so_correspond", "so_correspond_seeded", "so_ordered_scans", "so_correspond_edge", "so_evaluate", "so_covariance",
     "so_knn", "so_knn_device", "so_sampling_indices", "so_localize_global", "so_localize_scores", "so_localize_global_size", "so_localize_global_bnb", "so_localize_bnb_keys", "so_localize_bnb_bounds", "so_map_bounds", "so_kernel_launches", "so_bytes_copied", "so_build_flags", "so_profile_enable", "so_profile_get",
 ]
 
@@ -204,6 +204,7 @@ def load_library():
     L.so_correspond.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p, C.c_int32,
                                 C.c_void_p, C.c_void_p, C.c_void_p]
     L.so_correspond_seeded.argtypes = list(L.so_correspond.argtypes) + [C.c_void_p]
+    L.so_ordered_scans.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     L.so_evaluate.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     L.so_covariance.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]
     L.so_knn.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_int, C.c_float, C.c_void_p, C.c_void_p]
@@ -649,6 +650,13 @@ class Context:
         self._chk(self.L.so_register_batch_device(self.h, C.c_void_p(d_scans_ptr), _p(n_points), ns, _p(poses), C.byref(o), res),
                   "so_register_batch_device")
         return res
+
+    def ordered_scans(self, n: int) -> np.ndarray:
+        """Test hook: the first n points of the cell-ordered scan buffer the last batch registration left (n x 4 float32;
+        column 3 holds the point's index inside its scan as a uint32 bit pattern)."""
+        out = np.empty((n, 4), np.float32)
+        self._chk(self.L.so_ordered_scans(self.h, _p(out), n), "so_ordered_scans")
+        return out
 
     def correspond(self, scan_xyzi: np.ndarray, pose7, max_surface_features: int = 0, seed_pose=None):
         """Correspondences at pose7 -> (corr, hist_obs, hist_rej).  seed_pose: run them as ICP iteration 1 of a registration that

@@ -272,6 +272,9 @@ struct Chunk { uint32_t first, count, pt_first, pt_count, grid_x, grid_e = 0, gr
 
 // Once per registration: order every scan by map cell at its prior pose (k_scan_keys -> radix sort -> k_scan_gather, or the one-CTA
 // k_prepare_small for small registrations).  compact: drop the points the decimation skips here, once, instead of in every kernel.
+// The dropped bit is only carried when a scan of the chunk is capped: without one it is zero in every key and k_scan_finish changes
+// nothing, and leaving it out keeps 128-scan chunks of the 1 M-point map at 25 + 7 = 32 bits -- 32-bit keys, 4 radix passes over
+// 8-byte pairs instead of 5 over 12-byte ones -- for the same permutation.
 static int prepare_scans(Ctx* c, const float4* d_scan_in, const Chunk& ch, cudaStream_t st, bool compact) {
     c->prefiltered_n = SIZE_MAX;                                   // d_scan_sorted is about to be overwritten
     const MapView mv = map_view(c, c->surf);
@@ -289,6 +292,11 @@ static int prepare_scans(Ctx* c, const float4* d_scan_in, const Chunk& ch, cudaS
         return SO_OK;
     }
     while ((1u << scan_bits) < ch.count) ++scan_bits;
+    if (compact && !c->force_drop_bit) {
+        bool capped = false;
+        for (uint32_t s = ch.first; s < ch.first + ch.count; ++s) capped |= c->h_state[s].sampling_rate >= 0.0;     // init_state: -1 = no cap
+        compact = capped;
+    }
     const int extra = compact ? 1 : 0;
     const bool key32 = !c->force_key64 && cell_bits < 32 && cell_bits + extra + scan_bits <= 32;
     if (!key32) cell_bits = 32;
@@ -813,6 +821,7 @@ so_ctx* so_create(const so_config* cfg_in) {
     if (std::getenv("SO_NO_SMALL_PREPARE")) c->no_small_prepare = true;
     if (std::getenv("SO_NO_COOP_KNN")) c->no_coop_knn = true;
     if (std::getenv("SO_FORCE_KEY64")) c->force_key64 = true;
+    if (std::getenv("SO_FORCE_DROP_BIT")) c->force_drop_bit = true;
     if (std::getenv("SO_NO_DEC_UPLOAD")) c->no_dec_upload = true;
     if (const char* e = std::getenv("SO_CHUNKS")) c->chunk_override = std::max(0, std::min(16, std::atoi(e)));      // profiling aid: ncu cannot see inside conditional-node bodies
     if (ctx_alloc(c) != SO_OK) { ctx_free(c); return nullptr; }
@@ -1449,6 +1458,17 @@ int so_correspond(so_ctx* ctx, const void* surf, size_t n, size_t stride, size_t
     Ctx* c = reinterpret_cast<Ctx*>(ctx);
     if (!c || !surf || !pose || !corr || n == 0 || stride < 12) return fail(SO_ERR_ARG, "bad args");
     return correspond_stage(c, surf, n, stride, ioff, pose, nullptr, max_surface_features, corr, hist_obs, hist_rej);
+}
+
+int so_ordered_scans(so_ctx* ctx, float* out, size_t n) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c || (!out && n)) return fail(SO_ERR_ARG, "bad args");
+    if (n > c->scan_cap) return fail(SO_ERR_CAPACITY, "more points than the scan buffer holds");
+    SO_CUDA_TRY(cudaSetDevice(c->device));
+    SO_CUDA_TRY(cudaStreamSynchronize(c->aux_stream));
+    SO_CUDA_TRY(cudaMemcpyAsync(out, c->d_scan_sorted, n * sizeof(float4), cudaMemcpyDeviceToHost, c->stream));
+    SO_CUDA_TRY(cudaStreamSynchronize(c->stream));
+    return SO_OK;
 }
 
 int so_correspond_seeded(so_ctx* ctx, const void* surf, size_t n, size_t stride, size_t ioff, const double pose[7], int32_t max_surface_features,

@@ -202,6 +202,7 @@ struct Ctx {
     GraphSlot graphs[20];
     uint64_t graph_clock = 0;
     bool force_key64 = false;                      // SO_FORCE_KEY64: test aid, take the 64-bit scan-order key path even when 32 bits suffice
+    bool force_drop_bit = false;                   // SO_FORCE_DROP_BIT: test aid, carry the scan-order key's dropped bit even when no scan of the chunk is capped
     bool no_coop_knn = false;                      // SO_NO_COOP_KNN: A/B aid, always one query per thread
     bool no_small_prepare = false;                 // SO_NO_SMALL_PREPARE: A/B aid, always the device-wide scan ordering
     bool no_fused_lm = false;                      // SO_NO_FUSED_LM: A/B aid, always the two-kernel evaluation + optimiser step
