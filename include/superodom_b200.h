@@ -187,6 +187,13 @@ int so_map_add_scan(so_ctx* ctx, const void* xyzi, size_t n, size_t stride_bytes
 int so_map_add_registered_scan(so_ctx* ctx, const double pose[7]);
 /* ... and transformAndAddToMap(cloud, world_cloud, true) for the edge cloud. */
 int so_map_add_scan_edge(so_ctx* ctx, const void* xyzi, size_t n, size_t stride_bytes, size_t intensity_offset, const double pose[7]);
+/* The same insert for the edge cloud of the last single-scan registration, which is still in device memory.  After so_register it
+ * inserts exactly what so_map_add_scan_edge of the same cloud inserts; after so_register_undistort_edges it inserts the edge cloud
+ * undistorted with the D that pose gives, world = T(pose) * pInit, and after so_register_optimized_edges T(pose) * u_e(D_opt), as
+ * so_map_add_registered_scan does for the surf cloud.  Fails
+ * with SO_ERR_ARG, before any device work, whenever so_map_add_registered_scan would, and after so_correspond_edge.  SO_OK and
+ * nothing inserted when that registration had no edge cloud (every other so_register* entry point). */
+int so_map_add_registered_edges(so_ctx* ctx, const double pose[7]);
 /* replaces: LocalMap::get5x5LocalMapFeatureSize (LocalMap.h:291-318) */
 int so_map_counts_5x5(so_ctx* ctx, const int32_t ijk[3], int32_t* n_edge, int32_t* n_surf);
 /* replaces: LocalMap::getAllLocalMap (mode 0, LocalMap.h:647-658) / get5x5LocalMap(pos) (mode 1, :660-687).
@@ -290,7 +297,8 @@ int so_register_batch_device(so_ctx* ctx, const void* d_scans_xyzi, const uint32
  *   pInit_i = float3(qrot(q_i, p_i) + alpha_i * t_D)
  * and the iteration runs on pInit (rounded to float) in place of the sensor-frame point.  time_i is the float at byte time_offset of
  * each record, in seconds after the instant the pose describes (the shipped pipeline: the scan start, time stored in intensity by
- * uniformFeatureExtraction, so time_offset == intensity_offset).  Surf cloud only.  Argument errors (mode 2, a bad dt, a
+ * uniformFeatureExtraction, so time_offset == intensity_offset).  Surf cloud only (so_register_undistort_edges adds the edge
+ * cloud).  Argument errors (mode 2, a bad dt, a
  * non-finite prev_pose) are returned before any device work.  After so_register_undistort / so_register_prefiltered_undistort,
  * so_map_add_registered_scan(pose) inserts the whole cloud undistorted with the D that pose gives: world = T(pose) * pInit. */
 typedef struct {
@@ -302,6 +310,15 @@ typedef struct {
 } so_undistort;
 int so_register_undistort(so_ctx* ctx, const void* surf_xyzi, size_t n, size_t stride_bytes, size_t intensity_offset, size_t time_offset,
                           const double pose_in[7], const so_undistort* u, const so_icp_opts* opts, so_icp_result* out);
+/* ... with an edge cloud for the line branch (so_register's edge_xyzi): every ICP iteration warps the edge cloud with the same D as
+ * the surf cloud, and the line fit and evaluation run on its pInit (rounded to float) in place of the sensor-frame edge points.  Both
+ * clouds share stride, intensity offset and time offset (so_scan_extract_uniform and so_scan_extract_edges both store the time in
+ * intensity).  n_edge == 0: exactly so_register_undistort; mode 0: exactly so_register with the edge cloud.  Argument errors (those of
+ * so_register_undistort, a NULL edge_xyzi with n_edge > 0; SO_ERR_CAPACITY for n_edge > max_scan_points) come before any device
+ * work.  so_map_add_registered_edges(pose) afterwards inserts the edge cloud undistorted at pose. */
+int so_register_undistort_edges(so_ctx* ctx, const void* surf_xyzi, size_t n_surf, const void* edge_xyzi, size_t n_edge, size_t stride_bytes,
+                                size_t intensity_offset, size_t time_offset, const double pose_in[7], const so_undistort* u,
+                                const so_icp_opts* opts, so_icp_result* out);
 /* ... of the cloud the last so_scan_prefilter left on the device; the time is the filtered cloud's intensity (w). */
 int so_register_prefiltered_undistort(so_ctx* ctx, const double pose_in[7], const so_undistort* u, const so_icp_opts* opts, so_icp_result* out);
 /* ... of a batch as so_register_batch, u[n_scans]: one so_undistort per scan (mode 0 and 1 may be mixed). */
@@ -318,7 +335,8 @@ int so_undistort_points(so_ctx* ctx, const void* xyzi, size_t n, size_t stride_b
  *   u_i(D) = qrot(slerp(identity, q_D, alpha_i), p_i) + alpha_i * t_D
  * and its rows are so_register's plane rows at T on u_i(D), plus six rows of SE3AbsolutatePoseFactor on D (measurement
  * motion_prior, row k multiplied by sqrt(n_ok * motion_info[k]), n_ok the accepted correspondences of the ICP iteration).  Every ICP
- * iteration searches and fits at T on float(u(D)) at the current D.  Surf cloud only; use_pose_prior must be 0.  Argument errors (a
+ * iteration searches and fits at T on float(u(D)) at the current D.  Surf cloud only (so_register_optimized_edges adds the edge
+ * cloud); use_pose_prior must be 0.  Argument errors (a
  * bad dt, a non-finite motion_prior or one with a zero quaternion, a negative or non-finite motion_info, use_pose_prior) are returned
  * before any device work.  icp.cov and the error fields describe T.  After so_register_optimized /
  * so_register_prefiltered_optimized, so_map_add_registered_scan(pose) inserts T(pose) * u_i(D_opt) for the whole cloud. */
@@ -334,6 +352,17 @@ typedef struct {
 } so_motion_result;
 int so_register_optimized(so_ctx* ctx, const void* surf_xyzi, size_t n, size_t stride_bytes, size_t intensity_offset, size_t time_offset,
                           const double pose_in[7], const so_motion* m, const so_icp_opts* opts, so_motion_result* out);
+/* ... with an edge cloud for the line branch: every ICP iteration searches and fits the edge cloud at T on float(u_e(D)), and its line
+ * rows join the solve over the 12 columns: r = (lp - a) x (lp - b) / |a - b| with lp = R(q) u(D) + t (EdgeAnalyticCostFunction),
+ * under ScaledLoss(TukeyLoss(sqrt(3 lineRes))).  The motion prior's multiplier counts accepted planes plus accepted lines;
+ * icp.iter_n_edge and icp.hist_reject_line are filled; a NaN-weighted line row ends the registration with
+ * SO_STATUS_INVALID_EVALUATION, as in so_register.  Both clouds share stride, intensity offset and time offset.  n_edge == 0: exactly
+ * so_register_optimized.  Argument errors (those of so_register_optimized, a NULL edge_xyzi with n_edge > 0; SO_ERR_CAPACITY for
+ * n_edge > max_scan_points) come before any device work.  so_map_add_registered_edges(pose) afterwards inserts
+ * T(pose) * u_e(D_opt). */
+int so_register_optimized_edges(so_ctx* ctx, const void* surf_xyzi, size_t n_surf, const void* edge_xyzi, size_t n_edge, size_t stride_bytes,
+                                size_t intensity_offset, size_t time_offset, const double pose_in[7], const so_motion* m,
+                                const so_icp_opts* opts, so_motion_result* out);
 /* ... of the cloud the last so_scan_prefilter left on the device; the time is the filtered cloud's intensity (w). */
 int so_register_prefiltered_optimized(so_ctx* ctx, const double pose_in[7], const so_motion* m, const so_icp_opts* opts, so_motion_result* out);
 /* ... of a batch as so_register_batch, m[n_scans]: one so_motion per scan. */
@@ -345,6 +374,10 @@ int so_register_batch_optimized(so_ctx* ctx, const void* surf_xyzi, const uint32
 int so_evaluate_optimized(so_ctx* ctx, const void* xyzi, size_t n, size_t stride_bytes, size_t intensity_offset, size_t time_offset,
                           const double pose[7], const double motion[7], double dt, int32_t max_surface_features, double H[144],
                           double g[12], double* cost);
+/* Stage hook: the same with the edge cloud's line rows added (its lines fitted at T on float(u_e(motion))). */
+int so_evaluate_optimized_edges(so_ctx* ctx, const void* xyzi, size_t n, const void* edge_xyzi, size_t n_edge, size_t stride_bytes,
+                                size_t intensity_offset, size_t time_offset, const double pose[7], const double motion[7], double dt,
+                                int32_t max_surface_features, double H[144], double g[12], double* cost);
 
 /* Sharded-replay plumbing (BASELINE cfg4; SURVEY 8e "K8"): a caller-owned DEVICE buffer of cap_rows x 8 doubles.  Every following
  * so_register / so_register_batch* call appends one row per scan, starting at first_row and advancing: {pose_opt[7] (the

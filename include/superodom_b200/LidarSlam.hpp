@@ -297,24 +297,39 @@ public:
         const double dt = timeLaserOdometry - lasttimeLaserOdometry;
         int rc;
         LastMotion = Transformd();
-        if (Undistortion == OPTIMIZED && dt > 0 && !(edge_point && edge_point->size()) && !o.use_pose_prior) {
-            so_motion m{};                                         // the surf cloud only; so_register_optimized refuses the pose prior
+        const bool has_edges = edge_point && edge_point->size();
+        bool edges_registered = false;                             // the edge cloud is still on the device (so_map_add_registered_edges)
+        if (Undistortion == OPTIMIZED && dt > 0 && !o.use_pose_prior) {
+            so_motion m{};                                         // so_register_optimized* refuses the pose prior
             m.dt = dt;
             const Transformd D0 = undistort_has_prev ? undistort_prev_pose.inverse() * position : Transformd();
             D0.to_pose7(m.motion_prior);
             for (int k = 0; k < 6; ++k) m.motion_info[k] = OptimizedMotionInformation[k];
             so_motion_result mr{};
-            rc = so_register_optimized(context.h, surf, planner_point->size(), stride, ioff, ioff, pose, &m, &o, &mr);
-            check(rc, "so_register_optimized");
+            if (has_edges) {
+                rc = so_register_optimized_edges(context.h, surf, planner_point->size(), edge_point->points.data(), edge_point->size(), stride,
+                                                 ioff, ioff, pose, &m, &o, &mr);
+                check(rc, "so_register_optimized_edges");
+                edges_registered = true;
+            } else {
+                rc = so_register_optimized(context.h, surf, planner_point->size(), stride, ioff, ioff, pose, &m, &o, &mr);
+                check(rc, "so_register_optimized");
+            }
             last_result = mr.icp;
             LastMotion = Transformd::from_pose7(mr.motion);
-        } else if (Undistortion == APPROXIMATED && undistort_has_prev && dt > 0 && !(edge_point && edge_point->size())) {
-            so_undistort u{};                                      // the surf cloud only: a non-empty edge cloud (extractEdgeFeatures)
-                                                                   // turns within-scan compensation off and takes so_register below
+        } else if (Undistortion == APPROXIMATED && undistort_has_prev && dt > 0) {
+            so_undistort u{};                                      // both clouds carry their time in intensity
             u.mode = 1; u.rotation = UndistortRotation ? 1 : 0; u.dt = dt;
             undistort_prev_pose.to_pose7(u.prev_pose);
-            rc = so_register_undistort(context.h, surf, planner_point->size(), stride, ioff, ioff, pose, &u, &o, &last_result);
-            check(rc, "so_register_undistort");
+            if (has_edges) {
+                rc = so_register_undistort_edges(context.h, surf, planner_point->size(), edge_point->points.data(), edge_point->size(), stride,
+                                                 ioff, ioff, pose, &u, &o, &last_result);
+                check(rc, "so_register_undistort_edges");
+                edges_registered = true;
+            } else {
+                rc = so_register_undistort(context.h, surf, planner_point->size(), stride, ioff, ioff, pose, &u, &o, &last_result);
+                check(rc, "so_register_undistort");
+            }
         } else {
             rc = so_register(context.h, surf, planner_point->size(), edge_point ? (const void*)edge_point->points.data() : nullptr,
                              edge_point ? edge_point->size() : 0, stride, ioff, pose, &o, &last_result);
@@ -347,7 +362,8 @@ public:
         stats.n_iterations = r.n_iterations;
         last_T_w_lidar = T_w_lidar;
         // checkMotionThresholds always accepts (:193) -> transformAndAddToMap (:163-167)
-        if (edge_point && edge_point->size()) check(so_map_add_scan_edge(context.h, edge_point->points.data(), edge_point->size(), stride, ioff, r.pose), "so_map_add_scan_edge");
+        if (edges_registered) check(so_map_add_registered_edges(context.h, r.pose), "so_map_add_registered_edges");    // compensated, at r.pose
+        else if (has_edges) check(so_map_add_scan_edge(context.h, edge_point->points.data(), edge_point->size(), stride, ioff, r.pose), "so_map_add_scan_edge");
         if (planner_point->size()) check(so_map_add_registered_scan(context.h, r.pose), "so_map_add_registered_scan");   // the scan is still on the device
         lasttimeLaserOdometry = timeLaserOdometry;
         undistort_prev_pose = T_w_lidar; undistort_has_prev = true;

@@ -19,9 +19,9 @@ MAX_ICP_ITERS = 32
 EXPORTS = [
     "so_create", "so_destroy", "so_last_error", "so_device_available", "so_set_stream",
     "so_map_set_resolution", "so_map_set_origin", "so_map_get_origin", "so_map_shift", "so_map_set_points",
-    "so_map_set_edge_points", "so_map_add_surf", "so_map_add_edge", "so_map_add_scan", "so_map_add_registered_scan", "so_map_add_scan_edge", "so_map_counts_5x5", "so_map_download", "so_map_size",
+    "so_map_set_edge_points", "so_map_add_surf", "so_map_add_edge", "so_map_add_scan", "so_map_add_registered_scan", "so_map_add_registered_edges", "so_map_add_scan_edge", "so_map_counts_5x5", "so_map_download", "so_map_size",
     "so_scan_prefilter", "so_scan_deskew", "so_scan_extract_uniform", "so_scan_extract_edges", "so_register", "so_register_prefiltered", "so_register_injected", "so_set_pose_sink", "so_register_batch", "so_register_batch_edges", "so_register_batch_device",
-    "so_register_undistort", "so_register_prefiltered_undistort", "so_register_batch_undistort", "so_undistort_points", "so_register_optimized", "so_register_prefiltered_optimized", "so_register_batch_optimized", "so_evaluate_optimized", "so_correspond", "so_correspond_seeded", "so_ordered_scans", "so_correspond_edge", "so_evaluate", "so_covariance",
+    "so_register_undistort", "so_register_undistort_edges", "so_register_prefiltered_undistort", "so_register_batch_undistort", "so_undistort_points", "so_register_optimized", "so_register_optimized_edges", "so_register_prefiltered_optimized", "so_register_batch_optimized", "so_evaluate_optimized", "so_evaluate_optimized_edges", "so_correspond", "so_correspond_seeded", "so_ordered_scans", "so_correspond_edge", "so_evaluate", "so_covariance",
     "so_knn", "so_knn_device", "so_sampling_indices", "so_localize_global", "so_localize_scores", "so_localize_global_size", "so_localize_global_bnb", "so_localize_bnb_keys", "so_localize_bnb_bounds", "so_map_bounds", "so_kernel_launches", "so_bytes_copied", "so_build_flags", "so_profile_enable", "so_profile_get",
 ]
 
@@ -161,6 +161,7 @@ def load_library():
     L.so_map_add_surf.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t]
     L.so_map_add_scan.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p]
     L.so_map_add_registered_scan.argtypes = [C.c_void_p, C.c_void_p]
+    L.so_map_add_registered_edges.argtypes = [C.c_void_p, C.c_void_p]
     L.so_map_add_scan_edge.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p]
     L.so_map_set_edge_points.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t]
     L.so_map_add_edge.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t]
@@ -183,6 +184,8 @@ def load_library():
     L.so_register_injected.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]
     L.so_register_undistort.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p, C.c_void_p,
                                         C.c_void_p, C.c_void_p]
+    L.so_register_undistort_edges.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t,
+                                              C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     L.so_register_prefiltered_undistort.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     L.so_register_batch_undistort.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t,
                                               C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -190,6 +193,10 @@ def load_library():
                                       C.c_void_p]
     L.so_register_optimized.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p, C.c_void_p,
                                         C.c_void_p, C.c_void_p]
+    L.so_register_optimized_edges.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t,
+                                              C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.so_evaluate_optimized_edges.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t,
+                                              C.c_void_p, C.c_void_p, C.c_double, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
     L.so_register_prefiltered_optimized.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     L.so_register_batch_optimized.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t,
                                               C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -366,6 +373,11 @@ class Context:
         pose = np.ascontiguousarray(pose7, dtype=np.float64)
         self._chk(self.L.so_map_add_registered_scan(self.h, _p(pose)), "so_map_add_registered_scan")
 
+    def map_add_registered_edges(self, pose7):
+        """Insert the edge cloud last passed to register() / register_undistort_edges() (still on the device) at pose7."""
+        pose = np.ascontiguousarray(pose7, dtype=np.float64)
+        self._chk(self.L.so_map_add_registered_edges(self.h, _p(pose)), "so_map_add_registered_edges")
+
     def map_set_origin(self, t):
         t = np.ascontiguousarray(t, dtype=np.float64)
         o = np.zeros(3, np.int32)
@@ -531,6 +543,24 @@ class Context:
         self._chk(rc, "so_register_undistort")
         return r
 
+    def register_undistort_edges(self, scan_xyzi: np.ndarray, edge_xyzi, pose7, u: Undistort, max_icp_iters: int,
+                                 max_surface_features: int = 0, time_col: int = 3, **kw) -> IcpResult:
+        """register_undistort with an edge cloud (same columns as the scan, its time in the same column) for the line branch."""
+        s = np.ascontiguousarray(scan_xyzi, dtype=np.float32)
+        pose = np.ascontiguousarray(pose7, dtype=np.float64)
+        o = self._opts(max_icp_iters, max_surface_features, **kw)
+        r = IcpResult()
+        stride = s.shape[1] * 4
+        e, ne = None, 0
+        if edge_xyzi is not None and len(edge_xyzi):
+            ea = np.ascontiguousarray(edge_xyzi, dtype=np.float32)
+            assert ea.shape[1] == s.shape[1]
+            e, ne = _p(ea), ea.shape[0]
+        rc = self.L.so_register_undistort_edges(self.h, _p(s), s.shape[0], e, ne, stride, 12 if s.shape[1] >= 4 else stride, time_col * 4,
+                                                _p(pose), C.byref(u), C.byref(o), C.byref(r))
+        self._chk(rc, "so_register_undistort_edges")
+        return r
+
     def register_prefiltered_undistort(self, pose7, u: Undistort, max_icp_iters: int, max_surface_features: int = 0, **kw) -> IcpResult:
         pose = np.ascontiguousarray(pose7, dtype=np.float64)
         o = self._opts(max_icp_iters, max_surface_features, **kw)
@@ -611,6 +641,43 @@ class Context:
                                                _p(mot), float(dt), int(max_surface_features), _p(H), _p(g), C.byref(cost)),
                   "so_evaluate_optimized")
         return H, g, cost.value
+
+    def register_optimized_edges(self, scan_xyzi: np.ndarray, edge_xyzi, pose7, m: Motion, max_icp_iters: int, max_surface_features: int = 0,
+                                 time_col: int = 3, **kw) -> MotionResult:
+        """register_optimized with an edge cloud (same columns as the scan, its time in the same column) for the line branch."""
+        s = np.ascontiguousarray(scan_xyzi, dtype=np.float32)
+        pose = np.ascontiguousarray(pose7, dtype=np.float64)
+        o = self._opts(max_icp_iters, max_surface_features, **kw)
+        r = MotionResult()
+        stride = s.shape[1] * 4
+        e, ne = self._edge_arg(edge_xyzi, s)
+        rc = self.L.so_register_optimized_edges(self.h, _p(s), s.shape[0], e, ne, stride, 12 if s.shape[1] >= 4 else stride, time_col * 4,
+                                                _p(pose), C.byref(m), C.byref(o), C.byref(r))
+        self._chk(rc, "so_register_optimized_edges")
+        return r
+
+    def evaluate_optimized_edges(self, xyzi: np.ndarray, edge_xyzi, pose7, motion7, dt: float, max_surface_features: int = 0, time_col: int = 3):
+        """evaluate_optimized with the edge cloud's line rows added."""
+        a = np.ascontiguousarray(xyzi, dtype=np.float32)
+        pose = np.ascontiguousarray(pose7, dtype=np.float64)
+        mot = np.ascontiguousarray(motion7, dtype=np.float64)
+        H = np.zeros((12, 12))
+        g = np.zeros(12)
+        cost = C.c_double()
+        stride = a.shape[1] * 4
+        e, ne = self._edge_arg(edge_xyzi, a)
+        self._chk(self.L.so_evaluate_optimized_edges(self.h, _p(a), a.shape[0], e, ne, stride, 12 if a.shape[1] >= 4 else stride, time_col * 4,
+                                                     _p(pose), _p(mot), float(dt), int(max_surface_features), _p(H), _p(g), C.byref(cost)),
+                  "so_evaluate_optimized_edges")
+        return H, g, cost.value
+
+    @staticmethod
+    def _edge_arg(edge_xyzi, s):
+        """(pointer, count) of an optional edge cloud laid out like s; the array is kept alive by the caller's reference"""
+        if edge_xyzi is None or not len(edge_xyzi):
+            return None, 0
+        assert edge_xyzi.dtype == np.float32 and edge_xyzi.flags.c_contiguous and edge_xyzi.shape[1] == s.shape[1]
+        return _p(edge_xyzi), edge_xyzi.shape[0]
 
     def register_batch(self, scans_xyzi: np.ndarray, n_points, poses, max_icp_iters: int, max_surface_features: int = 0, **kw):
         """scans_xyzi: float32 [sum(n_points), 4] host array (pinned or pageable)."""

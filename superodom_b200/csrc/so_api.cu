@@ -322,17 +322,20 @@ static bool fused_lm(const Ctx* c, uint32_t n_scans, UndistortionMode mode) {
 // Kernels one ICP iteration of a captured schedule launches: the unrolled graph runs `iters` of them, the loop graph one per
 // iteration executed plus its k_loop_cond.  2: k_knn_scan + k_fit.
 static uint64_t iteration_launches(UndistortionMode mode, bool fused, uint32_t grid_e, int lm) {
-    if (mode == UndistortionMode::OPTIMIZED) return 1 + 2 + 2 + 2 * uint64_t(lm);         // warp, search + fit, (eval + step) x (1 + lm)
-    const uint64_t head = mode == UndistortionMode::APPROXIMATED ? 1 : 0;                  // k_undistort
+    if (mode == UndistortionMode::OPTIMIZED)                                                // warp, search + fit, (eval + step) x (1 + lm);
+        return 1 + 2 + 2 + 2 * uint64_t(lm) + (grid_e ? 1 + 2 + uint64_t(lm) : 0);       // edges: their warp, k_edge_fit + line rows, line rows x lm
+    const uint64_t head = mode == UndistortionMode::APPROXIMATED ? (grid_e ? 2 : 1) : 0;  // k_undistort (+ k_undistort_edges)
     if (fused && !grid_e) return head + 2 + 1 + uint64_t(lm);
     return head + 2 + 2 + 2 * uint64_t(lm) + (grid_e ? 1 + uint64_t(lm) : 0);
 }
 
 // One ICP iteration: [head, k_knn_scan, k_fit, first solve, lm solves].  Every kernel exits at once when its scan is not in the
 // matching phase, so a fixed schedule follows whatever path the device-side state machine takes.
-//   head         mode APPROXIMATED: k_undistort (the scans' pInit at the current pose); OPTIMIZED: k_motion_warp (u(D)); NONE: none
-//   first solve  k_evaluate<PH_CORR> (+ k_edge_fit) + k_lm_step; OPTIMIZED: k_motion_eval<PH_CORR> + k_motion_step
-//   lm solves    k_evaluate<PH_EVAL> (+ k_edge_evaluate) + k_lm_step; OPTIMIZED: k_motion_eval<PH_EVAL> + k_motion_step
+//   head         mode APPROXIMATED: k_undistort (the scans' pInit at the current pose) + k_undistort_edges when the chunk has an edge
+//                cloud; OPTIMIZED: k_motion_warp (u(D)) + k_motion_warp_edges likewise; NONE: none
+//   first solve  k_evaluate<PH_CORR> (+ k_edge_fit) + k_lm_step; OPTIMIZED: k_motion_eval<PH_CORR> (+ k_edge_fit + k_motion_eval_edge)
+//                + k_motion_step
+//   lm solves    k_evaluate<PH_EVAL> (+ k_edge_evaluate) + k_lm_step; OPTIMIZED: k_motion_eval<PH_EVAL> (+ k_motion_eval_edge) + k_motion_step
 // Preferred form: a CUDA-graph WHILE node around ONE iteration (k_loop_cond ends the loop when every scan of the chunk is done);
 // fallback: the schedule unrolled `iters` times.  Sets *was_loop to whether the loop form ran.  Profiling or injected neighbours:
 // launched one kernel at a time instead.
@@ -352,13 +355,19 @@ static int run_schedule(Ctx* c, const Chunk& ch, int iters, int lm, Undistortion
     eb.nn = nullptr; eb.selmask = nullptr;
     *was_loop = false;
     const bool optimized = mode == UndistortionMode::OPTIMIZED;
+    const bool warp_edges = mode != UndistortionMode::NONE && grid_e;     // the line branch runs on the edge cloud's pInit / float(u(D))
+    if (warp_edges) eb.scan = c->und.d_ewarp;
     double* const mot_partials = c->mot.d_partials ? c->mot.d_partials + size_t(ch.first) * c->mot.stride * kMotionAcc : nullptr;
+    const MotionEdges med{me, eb, c->d_escan, c->und.d_etime, c->mot.d_epartials, grid_e};
+    const MotionEdges* const mep = optimized && warp_edges ? &med : nullptr;
     auto head = [&](cudaStream_t s) {
-        if (optimized) launch_motion_warp(bv, c->d_scan_sorted, c->d_scan, c->und.d_time, c->mot.d_st, ch.first, grid_x, n_scans, s);
+        if (optimized) launch_motion_warp(bv, c->d_scan_sorted, c->d_scan, c->und.d_time, c->mot.d_st, ch.first, grid_x, n_scans, s, mep);
         else launch_undistort(bv, c->d_scan_sorted, c->d_scan, c->und.d_time, c->und.d_par + ch.first, grid_x, n_scans, s);
+        if (warp_edges && !optimized)
+            launch_undistort_edges(bv, eb.offset, c->und.d_ewarp, c->d_escan, c->und.d_etime, c->und.d_par + ch.first, grid_e, n_scans, s);
     };
     auto solve = [&](int phase, cudaStream_t s) {
-        if (optimized) launch_motion_solve(phase, bv, cb, c->d_scan, c->und.d_time, c->mot.d_st, ch.first, mot_partials, c->mot.stride, grid_x, n_scans, s);
+        if (optimized) launch_motion_solve(phase, bv, cb, c->d_scan, c->und.d_time, c->mot.d_st, ch.first, mot_partials, c->mot.stride, grid_x, n_scans, s, mep);
         else if (phase == PH_CORR) launch_first_eval(bv, cb, grid_x, n_scans, s, &me, &eb, grid_e);
         else launch_evaluate(bv, cb, grid_x, n_scans, s, &eb, grid_e);
     };
@@ -379,15 +388,16 @@ static int run_schedule(Ctx* c, const Chunk& ch, int iters, int lm, Undistortion
             return false;
         };
         const uint64_t solve_extra = 1 + (grid_e ? 1 : 0);          // launches of a solve besides the one timed_launch_end counts
+        const uint64_t corr_extra = solve_extra + (optimized && grid_e ? 1 : 0);   // OPTIMIZED: k_edge_fit + k_motion_eval_edge
         for (int it = 0; it < iters; ++it) {
             if (any_in(PH_CORR)) {
-                if (mode != UndistortionMode::NONE) { timed_launch_begin(c); head(c->stream); timed_launch_end(c, 7); }
+                if (mode != UndistortionMode::NONE) { timed_launch_begin(c); head(c->stream); c->launches += warp_edges ? 1 : 0; timed_launch_end(c, 7); }
                 timed_launch_begin(c);
                 if (d_inject) launch_inject(mv, c->surf.d_xyzi, c->surf.n, bv, c->nn, d_inject, inject_iters, grid_x, n_scans, c->stream);
                 else launch_match(mv, bv, cb, c->nn, grid_x, n_scans, c->stream, 1);                                               // k_knn_scan
                 timed_launch_end(c, 0);
                 timed_launch_begin(c); launch_match(mv, bv, cb, c->nn, grid_x, n_scans, c->stream, 2); timed_launch_end(c, 5);      // k_fit
-                timed_launch_begin(c); solve(PH_CORR, c->stream); c->launches += solve_extra; timed_launch_end(c, optimized ? 8 : 4);
+                timed_launch_begin(c); solve(PH_CORR, c->stream); c->launches += corr_extra; timed_launch_end(c, optimized ? 8 : 4);
             }
             for (int k = 0; k < lm; ++k)
                 if (any_in(PH_EVAL)) { timed_launch_begin(c); solve(PH_EVAL, c->stream); c->launches += solve_extra; timed_launch_end(c, optimized ? 8 : 1); }
@@ -403,6 +413,7 @@ static int run_schedule(Ctx* c, const Chunk& ch, int iters, int lm, Undistortion
     for (int a = 0; a < 3; ++a) key.origin[a] = mv.origin[a];
     key.nb[0] = mv.nb; key.nb[1] = me.nb; key.res[0] = mv.plane_res; key.res[1] = me.plane_res;
     if (mode != UndistortionMode::NONE) { key.mode = mode; key.und_time = c->und.d_time; }
+    if (warp_edges) key.und_edge = c->und.d_ewarp;
     Ctx::GraphSlot* slot = nullptr;
     for (auto& g : c->graphs)
         if (g.exec && std::memcmp(&g.key, &key, sizeof(key)) == 0) slot = &g;
@@ -699,7 +710,11 @@ int register_scans(Ctx* c, const RegisterRequest& q) {
         rc = grow_buffer(c->d_inject, c->inject_cap, words);
         if (!rc) SO_CUDA_TRY(cudaMemcpyAsync(c->d_inject, q.inject, words * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
     }
+    const bool edge_times = q.mode != UndistortionMode::NONE && q.edge && total_e;    // so_register_undistort_edges / _optimized_edges
+    if (!rc && edge_times) rc = undistort_edge_reserve(c);
+    if (!rc && edge_times && q.mode == UndistortionMode::OPTIMIZED) rc = motion_edge_reserve(c);
     if (!rc && q.edge) rc = upload_cloud(c, q.edge, total_e, q.stride, q.ioff, c->d_escan);   // first: it may use the staging buffer
+    if (!rc && edge_times) rc = upload_times(c, q.edge, total_e, q.stride, q.toff, c->und.d_etime);
     if (rc) return rc;
     RegisterRequest core = q;                      // what register_core registers: a capped so_register scan, its kept points
     const so_icp_opts& o = *q.opts;
@@ -752,6 +767,7 @@ int register_scans(Ctx* c, const RegisterRequest& q) {
     if (q.insertable) {
         c->reg = RegisteredScan{};
         c->reg.n = uint32_t(total); c->reg.mode = q.mode;
+        if (q.edge) c->reg.n_edge = uint32_t(total_e);
         if (q.mode == UndistortionMode::APPROXIMATED) c->reg.par = q.und[0];
         if (q.mode == UndistortionMode::OPTIMIZED) { std::memcpy(c->reg.D, q.motion[0].D, sizeof(c->reg.D)); c->reg.dt = q.motion[0].dt; }
     }
@@ -911,18 +927,21 @@ static int store_set_points(Ctx* c, MapStore& ms, const void* xyzi, size_t n, si
     ms.n = uint32_t(n);
     return map_rebuild(c, ms);
 }
-// ms tail = the registered scan (Ctx::reg), still in d_scan, compensated for its motion as it was registered
+// ms tail = the registered scan (Ctx::reg), still in d_scan, compensated for its motion as it was registered; for the edge store, its
+// edge cloud, still in d_escan (left by so_register, so_register_undistort_edges and so_register_optimized_edges)
 static int put_registered_scan(Ctx* c, MapStore& ms, const double pose[7]) {
     const RegisteredScan& r = c->reg;
-    SO_CUDA_TRY(cudaMemcpyAsync(ms.d_xyzi + ms.n, c->d_scan, size_t(r.n) * sizeof(float4), cudaMemcpyDeviceToDevice, c->stream));
+    const bool edges = &ms == &c->edge;
+    SO_CUDA_TRY(cudaMemcpyAsync(ms.d_xyzi + ms.n, edges ? c->d_escan : c->d_scan, size_t(edges ? r.n_edge : r.n) * sizeof(float4),
+                                cudaMemcpyDeviceToDevice, c->stream));
     switch (r.mode) {
-        case UndistortionMode::APPROXIMATED: return undistort_tail(c, ms, r, pose);
-        case UndistortionMode::OPTIMIZED: return motion_tail(c, ms, r);      // u(D_opt), whatever the pose
+        case UndistortionMode::APPROXIMATED: return edges ? undistort_edge_tail(c, ms, r, pose) : undistort_tail(c, ms, r, pose);
+        case UndistortionMode::OPTIMIZED: return edges ? motion_edge_tail(c, ms, r) : motion_tail(c, ms, r);   // u(D_opt), whatever the pose
         default: return SO_OK;
     }
 }
 
-// xyzi == nullptr with n != 0: the registered scan (put_registered_scan)
+// xyzi == nullptr with n != 0: the registered scan or its edge cloud (put_registered_scan)
 static int store_add(Ctx* c, MapStore& ms, const void* xyzi, size_t n, size_t stride, size_t ioff, const double* pose) {
     if (!c || stride < 12) return fail(SO_ERR_ARG, "bad args");
     if (size_t(ms.n) + n > c->cfg.max_map_points) return fail(SO_ERR_CAPACITY, "map + new points exceed so_config.max_map_points");
@@ -968,6 +987,14 @@ int so_map_add_registered_scan(so_ctx* ctx, const double pose[7]) {
     if (!c->reg.valid) return fail(SO_ERR_ARG, "so_map_add_registered_scan needs a preceding single-scan so_register* (and nothing that reuses the scan buffers in between)");
     if (c->reg.n == 0) return SO_OK;
     return store_add(c, c->surf, nullptr, c->reg.n, 16, 12, pose);
+}
+int so_map_add_registered_edges(so_ctx* ctx, const double pose[7]) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c || !pose) return fail(SO_ERR_ARG, "bad args");
+    if (!c->reg.valid || !c->reg.edge_valid)
+        return fail(SO_ERR_ARG, "so_map_add_registered_edges needs a preceding single-scan so_register* (and nothing that reuses the scan or edge buffers in between)");
+    if (c->reg.n_edge == 0) return SO_OK;
+    return store_add(c, c->edge, nullptr, c->reg.n_edge, 16, 12, pose);
 }
 int so_map_add_scan_edge(so_ctx* ctx, const void* xyzi, size_t n, size_t stride, size_t ioff, const double pose[7]) {
     Ctx* c = reinterpret_cast<Ctx*>(ctx);
@@ -1293,19 +1320,32 @@ int so_register_batch_device(so_ctx* ctx, const void* d_scans, const uint32_t* n
     return register_scans(c, q);
 }
 
-int so_register_undistort(so_ctx* ctx, const void* surf, size_t n_surf, size_t stride, size_t ioff, size_t toff, const double pose_in[7],
-                          const so_undistort* u, const so_icp_opts* opts, so_icp_result* out) {
+// so_register_undistort (edge == nullptr, n_edge == 0) and so_register_undistort_edges: both clouds share the layout and the time offset
+static int register_undistort(so_ctx* ctx, const void* surf, size_t n_surf, const void* edge, size_t n_edge, size_t stride, size_t ioff,
+                              size_t toff, const double pose_in[7], const so_undistort* u, const so_icp_opts* opts, so_icp_result* out) {
     Ctx* c = reinterpret_cast<Ctx*>(ctx);
-    if (!c || !pose_in || !opts || !out || (!surf && n_surf) || stride < 12 || toff + 4 > stride) return fail(SO_ERR_ARG, "bad args");
+    if (!c || !pose_in || !opts || !out || (!surf && n_surf) || (!edge && n_edge) || stride < 12 || toff + 4 > stride) return fail(SO_ERR_ARG, "bad args");
+    if (n_edge > c->edge_cap) return fail(SO_ERR_CAPACITY, "edge cloud larger than so_config.max_scan_points");
     int rc = check_undistort(u);
     if (rc) return rc;
-    if (u->mode == 0) return so_register(ctx, surf, n_surf, nullptr, 0, stride, ioff, pose_in, opts, out);
+    if (u->mode == 0) return so_register(ctx, surf, n_surf, n_edge ? edge : nullptr, n_edge, stride, ioff, pose_in, opts, out);
     if (n_surf > c->cfg.max_scan_points) return fail(SO_ERR_CAPACITY, "scan larger than so_config.max_scan_points");
-    const uint32_t n = uint32_t(n_surf);
+    const uint32_t n = uint32_t(n_surf), ne = uint32_t(n_edge);
     const UndistortParams P = make_params(*u);
     RegisterRequest q = single_scan(&n, pose_in, opts, out);
     q.scans = surf; q.stride = stride; q.ioff = ioff; q.toff = toff; q.mode = UndistortionMode::APPROXIMATED; q.und = &P;
+    if (ne) { q.edge = edge; q.n_edge = &ne; }
     return status_of(register_scans(c, q), *out);
+}
+
+int so_register_undistort(so_ctx* ctx, const void* surf, size_t n_surf, size_t stride, size_t ioff, size_t toff, const double pose_in[7],
+                          const so_undistort* u, const so_icp_opts* opts, so_icp_result* out) {
+    return register_undistort(ctx, surf, n_surf, nullptr, 0, stride, ioff, toff, pose_in, u, opts, out);
+}
+
+int so_register_undistort_edges(so_ctx* ctx, const void* surf, size_t n_surf, const void* edge, size_t n_edge, size_t stride, size_t ioff,
+                                size_t toff, const double pose_in[7], const so_undistort* u, const so_icp_opts* opts, so_icp_result* out) {
+    return register_undistort(ctx, surf, n_surf, edge, n_edge, stride, ioff, toff, pose_in, u, opts, out);
 }
 
 int so_register_prefiltered_undistort(so_ctx* ctx, const double pose_in[7], const so_undistort* u, const so_icp_opts* opts, so_icp_result* out) {
@@ -1341,20 +1381,33 @@ int so_register_batch_undistort(so_ctx* ctx, const void* surf, const uint32_t* n
     return register_scans(c, q);
 }
 
-int so_register_optimized(so_ctx* ctx, const void* surf, size_t n_surf, size_t stride, size_t ioff, size_t toff, const double pose_in[7],
-                          const so_motion* m, const so_icp_opts* opts, so_motion_result* out) {
+// so_register_optimized (edge == nullptr, n_edge == 0) and so_register_optimized_edges: both clouds share the layout and the time offset
+static int register_optimized(so_ctx* ctx, const void* surf, size_t n_surf, const void* edge, size_t n_edge, size_t stride, size_t ioff,
+                              size_t toff, const double pose_in[7], const so_motion* m, const so_icp_opts* opts, so_motion_result* out) {
     Ctx* c = reinterpret_cast<Ctx*>(ctx);
-    if (!c || !pose_in || !opts || !out || (!surf && n_surf) || stride < 12 || toff + 4 > stride) return fail(SO_ERR_ARG, "bad args");
+    if (!c || !pose_in || !opts || !out || (!surf && n_surf) || (!edge && n_edge) || stride < 12 || toff + 4 > stride) return fail(SO_ERR_ARG, "bad args");
+    if (n_edge > c->edge_cap) return fail(SO_ERR_CAPACITY, "edge cloud larger than so_config.max_scan_points");
     int rc = check_motion(m, opts);
     if (rc) return rc;
     if (n_surf > c->cfg.max_scan_points) return fail(SO_ERR_CAPACITY, "scan larger than so_config.max_scan_points");
-    const uint32_t n = uint32_t(n_surf);
+    const uint32_t n = uint32_t(n_surf), ne = uint32_t(n_edge);
     MotionState M = make_state(*m);
     so_icp_result icp;
     RegisterRequest q = single_scan(&n, pose_in, opts, &icp);
     q.scans = surf; q.stride = stride; q.ioff = ioff; q.toff = toff;
     q.mode = UndistortionMode::OPTIMIZED; q.motion = &M; q.motion_results = out;
+    if (ne) { q.edge = edge; q.n_edge = &ne; }
     return status_of(register_scans(c, q), icp);
+}
+
+int so_register_optimized(so_ctx* ctx, const void* surf, size_t n_surf, size_t stride, size_t ioff, size_t toff, const double pose_in[7],
+                          const so_motion* m, const so_icp_opts* opts, so_motion_result* out) {
+    return register_optimized(ctx, surf, n_surf, nullptr, 0, stride, ioff, toff, pose_in, m, opts, out);
+}
+
+int so_register_optimized_edges(so_ctx* ctx, const void* surf, size_t n_surf, const void* edge, size_t n_edge, size_t stride, size_t ioff,
+                                size_t toff, const double pose_in[7], const so_motion* m, const so_icp_opts* opts, so_motion_result* out) {
+    return register_optimized(ctx, surf, n_surf, edge, n_edge, stride, ioff, toff, pose_in, m, opts, out);
 }
 
 int so_register_prefiltered_optimized(so_ctx* ctx, const double pose_in[7], const so_motion* m, const so_icp_opts* opts, so_motion_result* out) {
@@ -1485,6 +1538,7 @@ int so_correspond_edge(so_ctx* ctx, const void* edge, size_t n, size_t stride, s
     if (n > c->edge_cap) return fail(SO_ERR_CAPACITY, "edge cloud larger than so_config.max_scan_points");
     SO_CUDA_TRY(cudaSetDevice(c->device));
     { int rc0 = ensure_maps(c); if (rc0) return rc0; }
+    c->reg.edge_valid = false;                                           // d_escan is overwritten below
     int rc = upload_cloud(c, edge, n, stride, ioff, c->d_escan);
     if (rc) return rc;
     so_icp_opts o{}; o.max_icp_iters = -1; o.lm_max_iterations = 4;

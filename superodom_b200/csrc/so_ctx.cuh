@@ -66,10 +66,13 @@ struct MotionState {
 };
 static_assert(sizeof(MotionState) % 8 == 0, "copied as 8-byte words");
 
-// The scan so_map_add_registered_scan inserts: d_scan[0..n) in upload order and, unless mode NONE, its times in und.d_time[0..n)
+// The scan so_map_add_registered_scan inserts: d_scan[0..n) in upload order and, unless mode NONE, its times in und.d_time[0..n);
+// the edge cloud so_map_add_registered_edges inserts: d_escan[0..n_edge) and, unless mode NONE, its times in und.d_etime
 struct RegisteredScan {
     bool valid = true;                             // false: a call has overwritten d_scan or the times since that scan registered
+    bool edge_valid = true;                        // false: so_correspond_edge has overwritten d_escan since
     uint32_t n = 0;                                // 0: no scan registered yet, nothing to insert
+    uint32_t n_edge = 0;                           // 0: the registration had no edge cloud, nothing to insert
     UndistortionMode mode = UndistortionMode::NONE;
     UndistortParams par{};                         // APPROXIMATED: the parameters it registered with
     double D[7] = {0, 0, 0, 0, 0, 0, 1}, dt = 0;   // OPTIMIZED: the estimated motion D_opt and the time it spans
@@ -194,6 +197,7 @@ struct Ctx {
         uint32_t first, count, grid_x, grid_e; int32_t iters, lm;
         const void* ptrs[8]; int32_t origin[3]; int32_t nb[2]; float res[2];
         UndistortionMode mode; const void* und_time;   // the head of every iteration (NONE / nullptr: none)
+        const void* und_edge;                          // APPROXIMATED with an edge cloud: the warped edge cloud the line branch reads
     };
     struct GraphSlot {
         cudaGraphExec_t exec = nullptr;
@@ -243,12 +247,15 @@ struct Ctx {
         float* d_time = nullptr; size_t time_cap = 0;                      // per-point times of the scans in d_scan (upload order)
         float4* d_hook = nullptr; size_t hook_cap = 0;                     // so_undistort_points: the cloud and its times
         float* d_hook_time = nullptr; size_t hook_time_cap = 0;
+        float* d_etime = nullptr; size_t etime_cap = 0;                    // [edge_cap] times of the edge cloud in d_escan
+        float4* d_ewarp = nullptr; size_t ewarp_cap = 0;                   // [edge_cap] its pInit at the current pose (EdgeBuf::scan)
     } und;
     // ---- within-scan motion estimated by the registration (so_register_optimized*): allocated on first use ------------------
     struct Mot {
         MotionState* d_st = nullptr; size_t st_cap = 0;                    // [max_batch] per-scan motion blocks
         double* d_partials = nullptr; size_t partials_cap = 0;             // [max_batch][stride][kMotionAcc] per-CTA sums
         uint32_t stride = 0;                                               // CTAs per scan the partials are laid out for
+        double* d_epartials = nullptr; size_t epartials_cap = 0;           // the edge clouds' per-CTA sums (so_register_optimized_edges)
     } mot;
     // ---- edge extraction (so_scan_extract_edges): allocated on first use, grown on demand; never touches the scan buffers ----
     struct Feat {
@@ -296,6 +303,7 @@ void global_free(Ctx* c);                                   // the search buffer
 // so_undistort.cu
 void undistort_free(Ctx* c);                                // the buffers of Ctx::und
 int undistort_reserve(Ctx* c, size_t n_points);             // Ctx::und's parameters (max_batch) and times (n_points)
+int undistort_edge_reserve(Ctx* c);                         // Ctx::und's edge times and warped edge cloud (edge_cap, fixed once allocated)
 int check_undistort(const so_undistort* u);                 // argument errors of one so_undistort
 UndistortParams make_params(const so_undistort& u);
 bool finite_pose(const double p[7]);                        // finite, with a non-zero quaternion
@@ -304,8 +312,14 @@ int upload_times(Ctx* c, const void* src, size_t n, size_t stride, size_t toff, 
 // raw points in upload order (raw, times: indexed offset + original index) into the ordered copy `sorted`, w kept
 void launch_undistort(const BatchView& bv, float4* sorted, const float4* raw, const float* times, const UndistortParams* par,
                       uint32_t grid_x, uint32_t n_scans, cudaStream_t st);
+// k_undistort_edges: pInit of every edge point of the chunk's scans (eoffset already offset to the chunk), from the raw edge cloud
+// and its times (indexed eoffset + i) into `out` at the same index, w kept
+void launch_undistort_edges(const BatchView& bv, const uint32_t* eoffset, float4* out, const float4* raw, const float* times,
+                            const UndistortParams* par, uint32_t grid_e, uint32_t n_scans, cudaStream_t st);
 // ms tail = the registered scan r (APPROXIMATED): pInit at pose, in place
 int undistort_tail(Ctx* c, MapStore& ms, const RegisteredScan& r, const double pose[7]);
+// ms tail = the registered edge cloud r (APPROXIMATED): pInit at pose, in place
+int undistort_edge_tail(Ctx* c, MapStore& ms, const RegisteredScan& r, const double pose[7]);
 // so_motion.cu
 void motion_free(Ctx* c);                                   // the buffers of Ctx::mot
 int motion_reserve(Ctx* c, size_t n_points);                // Ctx::mot's blocks and partials (max_batch), Ctx::und's times (n_points)
@@ -313,13 +327,20 @@ int check_motion(const so_motion* m, const so_icp_opts* o); // argument errors o
 MotionState make_state(const so_motion& m);
 void fill_motion(const so_icp_result& icp, const MotionState& M, so_motion_result* out);   // out = icp + motion, pose_end = T * D
 int motion_tail(Ctx* c, MapStore& ms, const RegisteredScan& r);   // ms tail = the registered scan r (OPTIMIZED): u(r.D), in place
+int motion_edge_tail(Ctx* c, MapStore& ms, const RegisteredScan& r);   // ms tail = its edge cloud: u(r.D) with the edge times, in place
+int motion_edge_reserve(Ctx* c);                             // Ctx::mot's edge partials
+// The edge cloud of an OPTIMIZED chunk: the edge map, the line buffers (eb.scan: where the warp puts float(u(D)) of the edge points,
+// eb.offset: the chunk's edge offsets), the raw edge points and their times, the edge partials and the CTAs covering the largest cloud
+struct MotionEdges { MapView map; EdgeBuf eb; const float4* raw; const float* times; double* partials; uint32_t grid_e; };
 // One ICP iteration's kernels of mode OPTIMIZED for the chunk's scans (bv.st / bv.offset / partials already offset to the chunk, ms
 // the whole array and `first` the chunk's first scan): the warp u(D) into `sorted`, and one evaluation + trust-region step (phase
 // PH_CORR: the first of a solve)
+// me (optional): the chunk's edge clouds -- the warp also writes float(u(D)) of the edge points, the solve adds k_edge_fit (PH_CORR)
+// and the line rows (k_motion_eval_edge) to the sums k_motion_step reduces
 void launch_motion_warp(const BatchView& bv, float4* sorted, const float4* raw, const float* times, const MotionState* ms, uint32_t first,
-                        uint32_t grid_x, uint32_t n_scans, cudaStream_t st);
+                        uint32_t grid_x, uint32_t n_scans, cudaStream_t st, const MotionEdges* me = nullptr);
 void launch_motion_solve(int phase, const BatchView& bv, const CorrBuf& cb, const float4* raw, const float* times, MotionState* ms, uint32_t first,
-                         double* partials, uint32_t stride, uint32_t grid_x, uint32_t n_scans, cudaStream_t st);
+                         double* partials, uint32_t stride, uint32_t grid_x, uint32_t n_scans, cudaStream_t st, const MotionEdges* me = nullptr);
 // so_covariance: cov12_warp on ms->H into st's covariance and error fields (device memory)
 void launch_covariance12(IcpState* st, const MotionState* ms, cudaStream_t stream);
 // so_map.cu

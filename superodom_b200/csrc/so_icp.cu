@@ -1609,6 +1609,9 @@ void launch_first_eval(const BatchView& bv, const CorrBuf& cb, uint32_t grid_x, 
     if (grid_e) k_edge_fit<<<dim3(grid_e, n_scans), kThreads, 0, st>>>(*medge, bv, *eb, bv.edge_partial_offset);
     k_lm_step<PH_CORR><<<n_scans, 128, 0, st>>>(bv, gp, bv.edge_partial_offset);
 }
+void launch_edge_fit(const MapView& medge, const BatchView& bv, const EdgeBuf& eb, uint32_t grid_e, uint32_t n_scans, cudaStream_t st) {
+    if (grid_e) k_edge_fit<<<dim3(grid_e, n_scans), kThreads, 0, st>>>(medge, bv, eb, bv.edge_partial_offset);
+}
 void launch_correspond(const MapView& m, const BatchView& bv, const CorrBuf& cb, const NnBuf& nb, uint32_t grid_x, uint32_t n_scans, cudaStream_t st,
                        const MapView* medge, const EdgeBuf* eb, uint32_t grid_e) {
     launch_match(m, bv, cb, nb, grid_x, n_scans, st);

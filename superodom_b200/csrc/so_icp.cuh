@@ -86,6 +86,8 @@ void launch_inject(const MapView& m, const float4* by_id, uint32_t n_map, const 
                    uint32_t grid_x, uint32_t n_scans, cudaStream_t st);
 void launch_first_eval(const BatchView& bv, const CorrBuf& cb, uint32_t grid_x, uint32_t n_scans, cudaStream_t st, const MapView* medge = nullptr,
                        const EdgeBuf* eb = nullptr, uint32_t grid_e = 0);
+// k_edge_fit alone (mode OPTIMIZED: the line correspondences and histogram; its 6-column sums are not read there)
+void launch_edge_fit(const MapView& medge, const BatchView& bv, const EdgeBuf& eb, uint32_t grid_e, uint32_t n_scans, cudaStream_t st);
 void launch_correspond(const MapView& m, const BatchView& bv, const CorrBuf& cb, const NnBuf& nb, uint32_t grid_x, uint32_t n_scans, cudaStream_t st,
                        const MapView* medge = nullptr, const EdgeBuf* eb = nullptr, uint32_t grid_e = 0);
 void launch_evaluate(const BatchView& bv, const CorrBuf& cb, uint32_t grid_x, uint32_t n_scans, cudaStream_t st, const EdgeBuf* eb = nullptr, uint32_t grid_e = 0);

@@ -14,6 +14,9 @@
 //   k_motion_eval<PH>    residual and 12-column row per correspondence, 91 per-CTA sums (78 + 12 + 1) through shared memory
 //   k_motion_step<PH>    fixed-order cross-CTA sum, then the 12-parameter trust-region step; the 12x12 covariance at the end
 //   k_motion_cloud       u(D_opt) of a contiguous cloud: the map insert after a single-scan registration
+// With an edge cloud (so_register_optimized_edges): k_motion_warp_edges writes float(u_e(D)) for k_edge_fit's search and fit at T, and
+//   k_motion_eval_edge<PH> adds the line rows' 91 per-CTA sums (three rows per line, motion_line_rows) into a partial buffer of their
+//   own, which k_motion_step adds after the planes' in the same fixed order
 #include <cmath>
 #include <vector>
 
@@ -53,6 +56,26 @@ __global__ void __launch_bounds__(kThreads) k_motion_warp(BatchView bv, float4* 
     float4 o = und_point(P, sh, __ldg(&raw[src]), __ldg(&times[src]));
     o.w = w;
     sorted[gi] = o;
+}
+
+// The same warp for the edge cloud (so_register_optimized_edges): one thread per edge point, raw point, time and output at one index
+__global__ void __launch_bounds__(kThreads) k_motion_warp_edges(BatchView bv, const uint32_t* __restrict__ eoffset, float4* __restrict__ out,
+                                                                const float4* __restrict__ raw, const float* __restrict__ times,
+                                                                const MotionState* __restrict__ ms) {
+    const int s = blockIdx.y;
+    const IcpState* st = bv.st + s;
+    if (st->phase != PH_CORR) return;
+    const uint32_t n = uint32_t(st->n_edge);
+    if (blockIdx.x * kThreads >= n) return;
+    __shared__ double sh[9];
+    if (threadIdx.x == 0) motion_setup(ms[s].D, sh);
+    __syncthreads();
+    UndistortParams P{};
+    P.dt = ms[s].dt; P.on = 1; P.rotation = 1;
+    const uint32_t i = blockIdx.x * kThreads + threadIdx.x;
+    if (i >= n) return;
+    const size_t gi = size_t(eoffset[s]) + i;
+    out[gi] = und_point(P, sh, __ldg(&raw[gi]), __ldg(&times[gi]));
 }
 
 struct MotionD { double v[7]; };
@@ -157,6 +180,64 @@ __device__ __forceinline__ void motion_row(const MotionCta& m, const double nd[4
     row[13] = 0.5 * rho0;
 }
 
+// One line correspondence (EdgeAnalyticCostFunction, lidarOptimization.cpp:12-47, at lp = R(q) u(D) + t): r = (lp - a) x (lp - b) / |a - b|,
+// dr/dlp = skew(b - a) / |a - b|.  Row k is motion_row's 12 columns with n replaced by the k-th row of that matrix (the T columns
+// are the reference's Jacobian at u(D), the D columns the plane row's chain rule); ScaledLoss(TukeyLoss) at a2 through Ceres'
+// corrector for a 3-dimensional residual, as accumulate_edge: rows[k] = sqrt(rho') [J_k (12), r_k], *half_rho = rho / 2.
+__device__ __forceinline__ void motion_line_rows(const MotionCta& m, const double a[3], const double bb[3], double wc, float4 p, float tau,
+                                                 double a2, double rows[3][13], double* half_rho) {
+    const double al = isfinite(tau) ? double(tau) / m.dt : 0.0;
+    const double pv[3] = {double(p.x), double(p.y), double(p.z)};
+    double s0, s1;                                                       // Eigen's slerp(identity, q_D, alpha)
+    if (m.sh[7] < 0.0) { s0 = 1.0 - al; s1 = al; }
+    else { s0 = sin((1.0 - al) * m.sh[7]) * m.sh[8]; s1 = sin(al * m.sh[7]) * m.sh[8]; }
+    if (m.sh[3] < 0.0) s1 = -s1;
+    const double qa[4] = {s1 * m.sh[0], s1 * m.sh[1], s1 * m.sh[2], s0 + s1 * m.sh[3]};
+    double u[3];
+    qrot(qa, pv, u);
+    for (int k = 0; k < 3; ++k) u[k] += al * m.sh[4 + k];
+    double pw[3];
+    qrot(m.T + 3, u, pw);
+    for (int k = 0; k < 3; ++k) pw[k] += m.T[k];
+    const double de[3] = {a[0] - bb[0], a[1] - bb[1], a[2] - bb[2]};
+    const double den = sqrt(de[0] * de[0] + de[1] * de[1] + de[2] * de[2]);
+    const double x[3] = {pw[0] - a[0], pw[1] - a[1], pw[2] - a[2]}, y[3] = {pw[0] - bb[0], pw[1] - bb[1], pw[2] - bb[2]};
+    const double r[3] = {(x[1] * y[2] - x[2] * y[1]) / den, (x[2] * y[0] - x[0] * y[2]) / den, (x[0] * y[1] - x[1] * y[0]) / den};
+    const double sr = r[0] * r[0] + r[1] * r[1] + r[2] * r[2];
+    double rho0, rho1;
+    if (sr <= a2) { const double v = 1.0 - sr / a2, v2 = v * v; rho0 = a2 / 6.0 * (1.0 - v2 * v); rho1 = 0.5 * v2; }
+    else { rho0 = a2 / 6.0; rho1 = 0.0; }
+    rho0 *= wc; rho1 *= wc;
+    const double sc = sqrt(rho1);
+    const double re[3] = {-de[0], -de[1], -de[2]};
+    const double K[9] = {0, -re[2], re[1], re[2], 0, -re[0], -re[1], re[0], 0};     // skew(b - a)
+    const double* R = m.R;
+    const double qc[4] = {-qa[0], -qa[1], -qa[2], qa[3]};
+    const double v[3] = {al * m.phi[0], al * m.phi[1], al * m.phi[2]};
+    double c1, c2;
+    jr_coeffs(fabs(al) * m.th, &c1, &c2);
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        const double nd[3] = {K[3 * k] / den, K[3 * k + 1] / den, K[3 * k + 2] / den};
+        const double av[3] = {R[0] * nd[0] + R[3] * nd[1] + R[6] * nd[2], R[1] * nd[0] + R[4] * nd[1] + R[7] * nd[2],
+                              R[2] * nd[0] + R[5] * nd[1] + R[8] * nd[2]};        // R^T n_k
+        double J[12];
+        J[0] = nd[0]; J[1] = nd[1]; J[2] = nd[2];
+        cross3(u, av, J + 3);
+        for (int j = 0; j < 3; ++j) J[6 + j] = al * av[j];
+        double b[3], w[3], t1[3], t2[3];
+        qrot(qc, av, b);
+        cross3(pv, b, w);
+        cross3(v, w, t1); cross3(v, t1, t2);
+        for (int j = 0; j < 3; ++j) w[j] = w[j] + c1 * t1[j] + c2 * t2[j];
+        cross3(m.phi, w, t1); cross3(m.phi, t1, t2);
+        for (int j = 0; j < 3; ++j) J[9 + j] = al * (w[j] - 0.5 * t1[j] + m.c3 * t2[j]);
+        for (int j = 0; j < 12; ++j) rows[k][j] = sc * J[j];
+        rows[k][12] = sc * r[k];
+    }
+    *half_rho = 0.5 * rho0;
+}
+
 constexpr int kRowStride = 14;
 // Tiles of kThreads points (the per-CTA layout of k_evaluate: eval_pts(n) tiles per CTA, eval_ctas(n) CTAs per scan): every thread
 // stages its row in shared memory, then thread e < 91 adds component e of the tile's 256 rows in index order.  One register
@@ -206,6 +287,62 @@ __global__ void __launch_bounds__(kThreads) k_motion_eval(BatchView bv, CorrBuf 
         __syncthreads();
     }
     if (e < kMotionAcc) partials[(size_t(s) * stride + blockIdx.x) * kMotionAcc + e] = acc;
+}
+
+// First edge-partial slot of chunk scan s (global scan first + s): edge clouds lie back to back, so slots s + eoffset / kThreads + b,
+// b < ceil(n_edge / kThreads), never overlap and stay below the edge capacity's CTAs + max_batch
+__device__ __forceinline__ size_t edge_slot(const uint32_t* eoffset, int s, uint32_t first) {
+    return size_t(first) + size_t(s) + size_t(eoffset[s] / kThreads);
+}
+
+// The line rows of the edge cloud (so_register_optimized_edges): one edge point per thread from k_edge_fit's lines (EdgeBuf a / b, weight
+// in a.w) and the raw edge point and time; the three rows of every point go through the same shared-memory reduction as k_motion_eval's
+// one, row k of all the CTA's points before row k + 1.  91 sums per CTA into epartials.
+template <int PHASE>
+__global__ void __launch_bounds__(kThreads) k_motion_eval_edge(BatchView bv, EdgeBuf eb, const float4* __restrict__ raw, const float* __restrict__ times,
+                                                               const MotionState* __restrict__ ms, double* __restrict__ epartials, uint32_t first) {
+    const int s = blockIdx.y;
+    const IcpState* st = bv.st + s;
+    if (st->phase != PHASE) return;
+    const uint32_t n = uint32_t(st->n_edge);
+    if (blockIdx.x * kThreads >= n) return;
+    __shared__ MotionCta m;
+    __shared__ double rows[kThreads * kRowStride];
+    if (threadIdx.x == 0) motion_cta_setup(PHASE == PH_EVAL ? st->cand : st->x, PHASE == PH_EVAL ? ms[s].Dc : ms[s].D, ms[s].dt, m);
+    const int e = threadIdx.x;
+    int ei = 0, ej = 0;
+    if (e < 78) { int k = e; while (k >= 12 - ei) { k -= 12 - ei; ++ei; } ej = ei + k; }
+    else if (e < 90) { ei = e - 78; ej = 12; }
+    else { ei = 13; ej = -1; }
+    __syncthreads();
+    double lr[3][13], half = 0.0;
+#pragma unroll
+    for (int k = 0; k < 3; ++k)
+#pragma unroll
+        for (int j = 0; j < 13; ++j) lr[k][j] = 0.0;
+    const uint32_t i = blockIdx.x * kThreads + threadIdx.x;
+    if (i < n) {
+        const size_t gi = size_t(eb.offset[s]) + i;
+        const double4 a = eb.a[gi];
+        if (a.w != 0.0) {                                                 // rejected points carry weight 0; NaN weights take part
+            const double4 b = eb.b[gi];
+            const double aa[3] = {a.x, a.y, a.z}, bb[3] = {b.x, b.y, b.z};
+            motion_line_rows(m, aa, bb, a.w, __ldg(&raw[gi]), __ldg(&times[gi]), bv.tukey_a2_line, lr, &half);
+        }
+    }
+    double acc = 0.0;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        for (int j = 0; j < 13; ++j) rows[threadIdx.x * kRowStride + j] = lr[k][j];
+        rows[threadIdx.x * kRowStride + 13] = k == 0 ? half : 0.0;
+        __syncthreads();
+        if (e < kMotionAcc) {
+            if (ej >= 0) { for (int t = 0; t < kThreads; ++t) acc += rows[t * kRowStride + ei] * rows[t * kRowStride + ej]; }
+            else { for (int t = 0; t < kThreads; ++t) acc += rows[t * kRowStride + ei]; }
+        }
+        __syncthreads();
+    }
+    if (e < kMotionAcc) epartials[(edge_slot(eb.offset, s, first) + blockIdx.x) * kMotionAcc + e] = acc;
 }
 
 // ------------------------------------------------------------------------------------------------------------------ step
@@ -337,6 +474,15 @@ __device__ __noinline__ void m_begin_solve(IcpState& st, MotionState& M, const d
     for (int i = 0; i < 7; ++i) st.x_iter_start[i] = st.x[i];
     st.lm_iter = 0; st.num_successful = 0; st.num_unsuccessful = 0; st.consecutive_invalid = 0; st.termination = 0;
     if (n_ok == 0) { st.termination = 6; m_end_solve(st); return; }
+    if (st.n_ok_edge > 0 && !isfinite(st.cost)) {
+        // a NaN-weighted line row: the rule of lm_begin_solve (so_icp.cu) -- the registration stops with a status and the pose this
+        // ICP iteration started from
+        const int it = st.icp_iter;
+        st.iter_n_surf[it] = n_ok - st.n_ok_edge; st.iter_n_edge[it] = st.n_ok_edge; st.iter_cost[it] = st.cost;
+        st.n_iterations = it + 1;
+        st.status = SO_STATUS_INVALID_EVALUATION; st.phase = PH_DONE;
+        return;
+    }
     for (int j = 0; j < 12; ++j) M.scale[j] = 1.0 / (1.0 + sqrt(M.H[tri12(j, j)]));
     double xn = 0.0;
     for (int i = 0; i < 7; ++i) xn += st.x[i] * st.x[i] + M.D[i] * M.D[i];
@@ -489,7 +635,8 @@ __global__ void __launch_bounds__(32) k_covariance12(IcpState* st, const MotionS
 void launch_covariance12(IcpState* st, const MotionState* ms, cudaStream_t stream) { k_covariance12<<<1, 32, 0, stream>>>(st, ms); }
 
 template <int AFTER>
-__global__ void __launch_bounds__(128) k_motion_step(BatchView bv, MotionState* __restrict__ ms, const double* __restrict__ partials, uint32_t stride) {
+__global__ void __launch_bounds__(128) k_motion_step(BatchView bv, MotionState* __restrict__ ms, const double* __restrict__ partials, uint32_t stride,
+                                                      const double* __restrict__ epartials, const uint32_t* __restrict__ eoffset, uint32_t first) {
     const int s = blockIdx.x;
     IcpState* st = bv.st + s;
     if (st->phase != AFTER) return;
@@ -509,6 +656,11 @@ __global__ void __launch_bounds__(128) k_motion_step(BatchView bv, MotionState* 
         const double* base = partials + size_t(s) * stride * kMotionAcc + threadIdx.x;
         double v = 0.0;
         for (uint32_t b = 0; b < np; ++b) v += base[size_t(b) * kMotionAcc];
+        const uint32_t ne = (uint32_t(st->n_edge) + kThreads - 1) / kThreads;          // the edge cloud's CTAs after the planes' (0: none)
+        if (ne) {
+            const double* eb = epartials + edge_slot(eoffset, s, first) * kMotionAcc + threadIdx.x;
+            for (uint32_t b = 0; b < ne; ++b) v += eb[size_t(b) * kMotionAcc];
+        }
         s_sum[threadIdx.x] = v;
     }
     __syncthreads();
@@ -519,8 +671,8 @@ __global__ void __launch_bounds__(128) k_motion_step(BatchView bv, MotionState* 
             for (int k = 0; k < 9; ++k) S.hist_obs[k] = bv.hist[s * kHistStride + k];
             for (int k = 0; k < 7; ++k) S.hist_rej[k] = bv.hist[s * kHistStride + 9 + k];
             for (int k = 0; k < 7; ++k) S.hist_rej_line[k] = bv.hist[s * kHistStride + 16 + k];
-            S.n_ok_edge = 0;
-            const int n_ok = S.hist_rej[0];
+            S.n_ok_edge = S.hist_rej_line[0];                            // 0 without an edge cloud
+            const int n_ok = S.hist_rej[0] + S.n_ok_edge;                // features_corres.size(): planes plus lines
             for (int k = 0; k < kHistStride; ++k) bv.hist[s * kHistStride + k] = 0;
             if (M.stage) {                                               // so_evaluate_optimized: report the plane rows and stop
                 for (int k = 0; k < 78; ++k) M.H[k] = s_sum[k];
@@ -546,20 +698,30 @@ __global__ void __launch_bounds__(128) k_motion_step(BatchView bv, MotionState* 
 }
 
 void launch_motion_warp(const BatchView& bv, float4* sorted, const float4* raw, const float* times, const MotionState* ms, uint32_t first,
-                        uint32_t grid_x, uint32_t n_scans, cudaStream_t st) {
+                        uint32_t grid_x, uint32_t n_scans, cudaStream_t st, const MotionEdges* me) {
     k_motion_warp<<<dim3(grid_x, n_scans), kThreads, 0, st>>>(bv, sorted, raw, times, ms + first);
+    if (me && me->grid_e)
+        k_motion_warp_edges<<<dim3(me->grid_e, n_scans), kThreads, 0, st>>>(bv, me->eb.offset, const_cast<float4*>(me->eb.scan), me->raw, me->times, ms + first);
 }
 
 void launch_motion_solve(int phase, const BatchView& bv, const CorrBuf& cb, const float4* raw, const float* times, MotionState* ms, uint32_t first,
-                         double* partials, uint32_t stride, uint32_t grid_x, uint32_t n_scans, cudaStream_t st) {
+                         double* partials, uint32_t stride, uint32_t grid_x, uint32_t n_scans, cudaStream_t st, const MotionEdges* me) {
     ms += first;
     const uint32_t gx = eval_grid(grid_x * kThreads);
+    const uint32_t ge = me ? me->grid_e : 0;
+    const uint32_t* eoff = me ? me->eb.offset : nullptr;
+    double* ep = me ? me->partials : nullptr;
     if (phase == PH_CORR) {
         k_motion_eval<PH_CORR><<<dim3(gx, n_scans), kThreads, 0, st>>>(bv, cb, raw, times, ms, partials, stride);
-        k_motion_step<PH_CORR><<<n_scans, 128, 0, st>>>(bv, ms, partials, stride);
+        if (ge) {
+            launch_edge_fit(me->map, bv, me->eb, ge, n_scans, st);
+            k_motion_eval_edge<PH_CORR><<<dim3(ge, n_scans), kThreads, 0, st>>>(bv, me->eb, me->raw, me->times, ms, ep, first);
+        }
+        k_motion_step<PH_CORR><<<n_scans, 128, 0, st>>>(bv, ms, partials, stride, ep, eoff, first);
     } else {
         k_motion_eval<PH_EVAL><<<dim3(gx, n_scans), kThreads, 0, st>>>(bv, cb, raw, times, ms, partials, stride);
-        k_motion_step<PH_EVAL><<<n_scans, 128, 0, st>>>(bv, ms, partials, stride);
+        if (ge) k_motion_eval_edge<PH_EVAL><<<dim3(ge, n_scans), kThreads, 0, st>>>(bv, me->eb, me->raw, me->times, ms, ep, first);
+        k_motion_step<PH_EVAL><<<n_scans, 128, 0, st>>>(bv, ms, partials, stride, ep, eoff, first);
     }
 }
 
@@ -574,7 +736,18 @@ int motion_tail(Ctx* c, MapStore& ms, const RegisteredScan& r) {
     return SO_OK;
 }
 
-void motion_free(Ctx* c) { cudaFree(c->mot.d_st); cudaFree(c->mot.d_partials); }
+int motion_edge_tail(Ctx* c, MapStore& ms, const RegisteredScan& r) {
+    if (!r.n_edge) return SO_OK;
+    MotionD D;
+    for (int k = 0; k < 7; ++k) D.v[k] = r.D[k];
+    timed_launch_begin(c);
+    k_motion_cloud<<<(r.n_edge + 255) / 256, 256, 0, c->stream>>>(ms.d_xyzi + ms.n, c->und.d_etime, r.n_edge, D, r.dt);
+    timed_launch_end(c, 7);
+    SO_CUDA_TRY(cudaGetLastError());
+    return SO_OK;
+}
+
+void motion_free(Ctx* c) { cudaFree(c->mot.d_st); cudaFree(c->mot.d_partials); cudaFree(c->mot.d_epartials); }
 
 // ------------------------------------------------------------------------------------------------------------------ host side
 int check_motion(const so_motion* m, const so_icp_opts* o) {
@@ -608,6 +781,12 @@ int motion_reserve(Ctx* c, size_t n_points) {
     return rc;
 }
 
+// The edge cloud's partials (edge_slot: at most the edge capacity's CTAs + max_batch slots), sized once, so that a captured schedule's
+// pointer stays valid
+int motion_edge_reserve(Ctx* c) {
+    return grow_buffer(c->mot.d_epartials, c->mot.epartials_cap, (size_t(c->edge_grid_cap) + c->max_batch) * kMotionAcc);
+}
+
 // so_motion_result from the registration's result and the motion block: pose_end = T * D with T = pose_opt
 void fill_motion(const so_icp_result& icp, const MotionState& M, so_motion_result* out) {
     out->icp = icp;
@@ -625,10 +804,14 @@ using namespace so;
 
 extern "C" {
 
-int so_evaluate_optimized(so_ctx* ctx, const void* xyzi, size_t n, size_t stride, size_t ioff, size_t toff, const double pose[7],
-                          const double motion[7], double dt, int32_t max_surface_features, double H[144], double g[12], double* cost) {
+// so_evaluate_optimized (edge == nullptr, n_edge == 0) and so_evaluate_optimized_edges
+static int evaluate_optimized(so_ctx* ctx, const void* xyzi, size_t n, const void* edge, size_t n_edge, size_t stride, size_t ioff, size_t toff,
+                              const double pose[7], const double motion[7], double dt, int32_t max_surface_features, double H[144], double g[12],
+                              double* cost) {
     Ctx* c = reinterpret_cast<Ctx*>(ctx);
-    if (!c || !pose || !motion || !xyzi || n == 0 || stride < 12 || toff + 4 > stride || !finite_pose(pose)) return fail(SO_ERR_ARG, "bad args");
+    if (!c || !pose || !motion || !xyzi || n == 0 || (!edge && n_edge) || stride < 12 || toff + 4 > stride || !finite_pose(pose))
+        return fail(SO_ERR_ARG, "bad args");
+    if (n_edge > c->edge_cap) return fail(SO_ERR_CAPACITY, "edge cloud larger than so_config.max_scan_points");
     so_motion m{};
     m.dt = dt;
     for (int k = 0; k < 7; ++k) m.motion_prior[k] = motion[k];
@@ -644,12 +827,25 @@ int so_evaluate_optimized(so_ctx* ctx, const void* xyzi, size_t n, size_t stride
     RegisterRequest q;                                                   // a stage evaluation leaves no registered scan and no pose row
     q.scans = xyzi; q.stride = stride; q.ioff = ioff; q.toff = toff; q.n_points = &nn; q.poses = pose; q.opts = &o;
     q.mode = UndistortionMode::OPTIMIZED; q.motion = &M; q.sink_rows = false; q.results = &r;
+    const uint32_t ne = uint32_t(n_edge);
+    if (ne) { q.edge = edge; q.n_edge = &ne; }
     rc = register_scans(c, q);
     if (rc) return rc;
     if (H) for (int i = 0; i < 12; ++i) for (int j = 0; j < 12; ++j) H[i * 12 + j] = M.H[i <= j ? tri12(i, j) : tri12(j, i)];
     if (g) for (int i = 0; i < 12; ++i) g[i] = M.g[i];
     if (cost) *cost = M.cost;
     return SO_OK;
+}
+
+int so_evaluate_optimized(so_ctx* ctx, const void* xyzi, size_t n, size_t stride, size_t ioff, size_t toff, const double pose[7],
+                          const double motion[7], double dt, int32_t max_surface_features, double H[144], double g[12], double* cost) {
+    return evaluate_optimized(ctx, xyzi, n, nullptr, 0, stride, ioff, toff, pose, motion, dt, max_surface_features, H, g, cost);
+}
+
+int so_evaluate_optimized_edges(so_ctx* ctx, const void* xyzi, size_t n, const void* edge, size_t n_edge, size_t stride, size_t ioff, size_t toff,
+                                const double pose[7], const double motion[7], double dt, int32_t max_surface_features, double H[144],
+                                double g[12], double* cost) {
+    return evaluate_optimized(ctx, xyzi, n, edge, n_edge, stride, ioff, toff, pose, motion, dt, max_surface_features, H, g, cost);
 }
 
 }  // extern "C"

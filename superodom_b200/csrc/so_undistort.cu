@@ -8,6 +8,7 @@
 //   pInit_i = float3(qrot(q_i, p_i) + alpha_i * t_D)
 // and the iteration runs on pInit in place of p (und_point, so_undistort.cuh; tests/undistort_numpy.py restates its bits).
 //   k_undistort        the ICP form: one thread per active point of the ordered scans, writes d_scan_sorted (w kept)
+//   k_undistort_edges  the ICP form for the edge cloud (so_register_undistort_edges): d_escan -> und.d_ewarp, same index
 //   k_undistort_cloud  a contiguous cloud at a given pose: the map insert after an undistorted registration, so_undistort_points
 #include <cmath>
 #include <vector>
@@ -47,6 +48,32 @@ void launch_undistort(const BatchView& bv, float4* sorted, const float4* raw, co
     k_undistort<<<dim3(grid_x, n_scans), kThreads, 0, st>>>(bv, sorted, raw, times, par);
 }
 
+// The same warp for the edge cloud (so_register_undistort_edges): one thread per edge point; the edge cloud is not reordered, so
+// raw point, time and output share the index.  k_edge_fit / k_edge_evaluate then read `out` as their sensor-frame cloud.
+__global__ void __launch_bounds__(kThreads) k_undistort_edges(BatchView bv, const uint32_t* __restrict__ eoffset, float4* __restrict__ out,
+                                                              const float4* __restrict__ raw, const float* __restrict__ times,
+                                                              const UndistortParams* __restrict__ par) {
+    const int s = blockIdx.y;
+    const IcpState* st = bv.st + s;
+    if (st->phase != PH_CORR) return;
+    const UndistortParams P = par[s];
+    if (!P.on) return;
+    const uint32_t n = uint32_t(st->n_edge);
+    if (blockIdx.x * kThreads >= n) return;
+    __shared__ double sh[9];
+    if (threadIdx.x == 0) und_setup(P, st->x, sh);
+    __syncthreads();
+    const uint32_t i = blockIdx.x * kThreads + threadIdx.x;
+    if (i >= n) return;
+    const size_t gi = size_t(eoffset[s]) + i;
+    out[gi] = und_point(P, sh, __ldg(&raw[gi]), __ldg(&times[gi]));
+}
+
+void launch_undistort_edges(const BatchView& bv, const uint32_t* eoffset, float4* out, const float4* raw, const float* times,
+                            const UndistortParams* par, uint32_t grid_e, uint32_t n_scans, cudaStream_t st) {
+    k_undistort_edges<<<dim3(grid_e, n_scans), kThreads, 0, st>>>(bv, eoffset, out, raw, times, par);
+}
+
 struct UndPose { double v[7]; };
 __global__ void __launch_bounds__(256) k_undistort_cloud(float4* __restrict__ pts, const float* __restrict__ times, uint32_t n,
                                                          UndistortParams P, UndPose x) {
@@ -73,8 +100,15 @@ int undistort_tail(Ctx* c, MapStore& ms, const RegisteredScan& r, const double p
     return SO_OK;
 }
 
+int undistort_edge_tail(Ctx* c, MapStore& ms, const RegisteredScan& r, const double pose[7]) {
+    launch_undistort_cloud(c, ms.d_xyzi + ms.n, c->und.d_etime, r.n_edge, r.par, pose);
+    SO_CUDA_TRY(cudaGetLastError());
+    return SO_OK;
+}
+
 void undistort_free(Ctx* c) {
     cudaFree(c->und.d_par); cudaFree(c->und.d_time); cudaFree(c->und.d_hook); cudaFree(c->und.d_hook_time);
+    cudaFree(c->und.d_etime); cudaFree(c->und.d_ewarp);
 }
 
 // ------------------------------------------------------------------------------------------------------------------ host side
@@ -119,6 +153,13 @@ int upload_times(Ctx* c, const void* src, size_t n, size_t stride, size_t toff, 
 int undistort_reserve(Ctx* c, size_t n_points) {
     int rc = grow_buffer(c->und.d_par, c->und.par_cap, size_t(c->max_batch));
     if (!rc) rc = grow_buffer(c->und.d_time, c->und.time_cap, std::max<size_t>(n_points, 1));
+    return rc;
+}
+
+// Sized to the edge capacity on first use and never regrown, so that a captured schedule's pointer to d_ewarp stays valid
+int undistort_edge_reserve(Ctx* c) {
+    int rc = grow_buffer(c->und.d_etime, c->und.etime_cap, std::max<size_t>(c->edge_cap, 1));
+    if (!rc) rc = grow_buffer(c->und.d_ewarp, c->und.ewarp_cap, std::max<size_t>(c->edge_cap, 1));
     return rc;
 }
 

@@ -641,6 +641,40 @@ def make_ring_scan(scene: Scene, sensor: str, pose7: np.ndarray, seed: int, orde
     return rec
 
 
+def make_moving_ring_scan(scene: Scene, sensor: str, pose_start: np.ndarray, speed: float, yaw_rate: float, seed: int,
+                          sweep_s: float = 0.1, dt: float = 0.1, range_noise: float = 0.01, rmin: float = 0.2, rmax: float = 130.0):
+    """make_moving_scan's sweep (constant forward body velocity `speed` along the start pose's x axis, yaw rate `yaw_rate`; column c
+    fires at t = c / n_cols * sweep_s from the pose at t, its points in the sensor frame at t) delivered as make_ring_scan's
+    point_os::PointcloudXYZITR records {x, y, z, pad, intensity, time, ring, pad}, in firing order.
+    -> dict(points float32 [n, 8], pose_true (the pose at the sweep start), pose_prev / pose_next (the same motion at -dt / +dt), prior)."""
+    n_cols, n_rings = {"vlp16": (1800, 16), "os1_128": (1024, 128)}[sensor]
+    rng = np.random.default_rng(seed)
+    dirs = sensor_dirs(sensor).reshape(n_cols, n_rings, 3)
+    q0 = np.asarray(pose_start[3:], np.float64)
+    v_w = quat_to_R(q0) @ np.array([speed, 0.0, 0.0])
+
+    def pose_at(t):
+        q = quat_mul(q0, quat_from_rotvec(np.array([0.0, 0.0, yaw_rate * t])))
+        return np.concatenate([pose_start[:3] + v_w * t, q / np.linalg.norm(q)])
+
+    out = []
+    for c in range(n_cols):
+        t = c / n_cols * sweep_s
+        P = pose_at(t)
+        d = dirs[c]
+        r = raycast(scene, P[:3], d @ quat_to_R(P[3:]).T) + rng.normal(0.0, range_noise, size=len(d))
+        ok = np.isfinite(r) & (r > rmin) & (r < rmax)
+        rec = np.zeros((int(ok.sum()), 8), np.float32)
+        rec[:, :3] = d[ok] * r[ok, None]
+        rec[:, 5] = np.float32(t)
+        rec.view(np.uint16)[:, 12] = np.arange(n_rings)[ok].astype(np.uint16)
+        out.append(rec)
+    rec = np.concatenate(out)
+    rec[:, 4] = rng.uniform(0.0, 255.0, len(rec))
+    prior = perturb_pose(pose_start, seed + 7, dt=0.05, dth_deg=0.5)
+    return dict(points=rec, pose_true=np.asarray(pose_start, np.float64), pose_prev=pose_at(-dt), pose_next=pose_at(dt), prior=prior)
+
+
 def make_corridor_scene() -> Scene:
     """A 400 m x 6 m corridor (x along it, walls at y = +-3, floor -1.8, ceiling 3.2; the end walls at x = +-200 lie beyond the
     130 m range) with free-standing 0.1 m square floor-to-ceiling poles every 4 m, 1 m off each wall.  Pole centres sit at
