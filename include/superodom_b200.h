@@ -379,6 +379,42 @@ int so_evaluate_optimized_edges(so_ctx* ctx, const void* xyzi, size_t n, const v
                                 size_t intensity_offset, size_t time_offset, const double pose[7], const double motion[7], double dt,
                                 int32_t max_surface_features, double H[144], double g[12], double* cost);
 
+/* ---- degeneracy-aware registration (the reference's isDegenerate, LidarSlam.h:264; its rule is commented out upstream) -----------
+ * Once per ICP iteration, at the start of its solve, the 6x6 normal matrix H at the iteration's start pose (plane rows, line rows,
+ * pose-prior rows when use_pose_prior is set; order t, theta) is analysed block by block:
+ *   I_t = H_tt - H_tr H_rr^+ H_rt,   I_theta = H_rr - H_rt H_tt^+ H_tr
+ * (^+ the pseudo-inverse with ceres::Covariance's cut, sqrt(w_k / w_max) < 1e-7).  These are the inverses of the covariance blocks
+ * EstimateRegistrationError analyses, so sqrt(i_min / i_max) of I_t is PosInverseConditionNum when H is invertible (and likewise for
+ * theta).  Eigenpair (i_k, u_k) of a block, ascending, is flagged when i_k <= threshold^2 * max(i_max, 0).  constrain = 1 and
+ * something flagged: that iteration's solve is Ceres' trust-region solve on the same cost with the local parameterisation
+ * x [+] B y, B = the unflagged eigenvectors (6 x m, translation ones first), so the pose does not move along a flagged direction.
+ * Otherwise the registration is so_register's, bit for bit.  Combining it with undistortion (so_register_undistort*,
+ * so_register_optimized*) is not supported.  Argument errors (a NaN or negative threshold, a threshold >= 1, constrain not 0 or 1) come
+ * before any device work.  so_map_add_registered_scan / so_map_add_registered_edges work afterwards as after so_register. */
+typedef struct {
+    double pos_threshold, ori_threshold;   /* on sqrt(i_k / i_max), each in [0, 1) */
+    int32_t constrain;                     /* 0: report only (the registration is so_register's, bit for bit); 1: reduced solve */
+    int32_t pad_;
+} so_degeneracy;
+typedef struct {
+    so_icp_result icp;
+    int32_t iter_n_flag_pos[SO_MAX_ICP_ITERS], iter_n_flag_ori[SO_MAX_ICP_ITERS];   /* directions flagged per ICP iteration */
+    double pos_info[3], pos_axes[9], ori_info[3], ori_axes[9];   /* last ICP iteration: eigenpairs of I_t, I_theta, ascending;
+                                                                    axes[3k..3k+2] = eigenvector k */
+    int32_t flags_pos, flags_ori;                                 /* bit k: eigenvector k flagged, last ICP iteration */
+} so_degeneracy_result;
+int so_register_degeneracy(so_ctx* ctx, const void* surf_xyzi, size_t n_surf, const void* edge_xyzi, size_t n_edge, size_t stride_bytes,
+                           size_t intensity_offset, const double pose_in[7], const so_degeneracy* d, const so_icp_opts* opts,
+                           so_degeneracy_result* out);
+/* ... of a batch as so_register_batch (edge_xyzi / n_edge: optional, as so_register_batch_edges), d[n_scans]: one per scan. */
+int so_register_batch_degeneracy(so_ctx* ctx, const void* surf_xyzi, const uint32_t* n_points, const void* edge_xyzi, const uint32_t* n_edge,
+                                 size_t n_scans, size_t stride_bytes, size_t intensity_offset, const double* poses_in, const so_degeneracy* d,
+                                 const so_icp_opts* opts, so_degeneracy_result* results);
+/* Test hook: the analysis above on a given symmetric H (row-major 6x6, upper triangle read), by the device code a solve begins with,
+ * in a one-thread launch.  Fills pos_info, pos_axes, ori_info, ori_axes and the flags; zeroes the rest.  Replaces the state a
+ * preceding so_correspond* left for so_evaluate. */
+int so_degeneracy_analysis(so_ctx* ctx, const double* H, const so_degeneracy* d, so_degeneracy_result* out);
+
 /* Sharded-replay plumbing (BASELINE cfg4; SURVEY 8e "K8"): a caller-owned DEVICE buffer of cap_rows x 8 doubles.  Every following
  * so_register / so_register_batch* call appends one row per scan, starting at first_row and advancing: {pose_opt[7] (the
  * optimiser output, so_icp_result.pose_opt), status + 256 * n_iterations}; scans that were not registered (soft statuses) carry

@@ -237,7 +237,13 @@ public:
     std::string map_dir;
     float init_x = 0, init_y = 0, init_z = 0, init_roll = 0, init_pitch = 0, init_yaw = 0, localization_mode = 0, update_map = 0;
     double lasttimeLaserOdometry = 0;
-    bool bInitialization = false, isDegenerate = false;          // isDegenerate is never set by the reference (LidarSlam.cpp:976-985)
+    // isDegenerate: set after every registration by the reference's commented-out rule (LidarSlam.cpp:976-985) on the final covariance,
+    // pos_inv_cond < Pos_degeneracy_threshold || ori_inv_cond < Ori_degeneracy_threshold (never with the default thresholds of 0)
+    bool bInitialization = false, isDegenerate = false;
+    // shim only: with Undistortion == NONE, register through so_register_degeneracy (constrain = 1, the degeneracy thresholds above):
+    // each ICP iteration's solve leaves the directions the scan does not constrain alone
+    bool DegeneracyAware = false;
+    so_degeneracy_result last_degeneracy{};                      // DegeneracyAware: what the analysis reported for the last scan
     std::array<int, nFeatureObs> PlaneFeatureHistogramObs{};
     std::array<int, nRejectionCauses> MatchRejectionHistogramLine{}, MatchRejectionHistogramPlane{};
     size_t LocalizationICPMaxIter = 4;                           // LidarSlam.h:273
@@ -330,6 +336,13 @@ public:
                 rc = so_register_undistort(context.h, surf, planner_point->size(), stride, ioff, ioff, pose, &u, &o, &last_result);
                 check(rc, "so_register_undistort");
             }
+        } else if (DegeneracyAware && Undistortion == NONE) {
+            so_degeneracy d{};
+            d.pos_threshold = Pos_degeneracy_threshold; d.ori_threshold = Ori_degeneracy_threshold; d.constrain = 1;
+            rc = so_register_degeneracy(context.h, surf, planner_point->size(), edge_point ? (const void*)edge_point->points.data() : nullptr,
+                                        edge_point ? edge_point->size() : 0, stride, ioff, pose, &d, &o, &last_degeneracy);
+            check(rc, "so_register_degeneracy");
+            last_result = last_degeneracy.icp;
         } else {
             rc = so_register(context.h, surf, planner_point->size(), edge_point ? (const void*)edge_point->points.data() : nullptr,
                              edge_point ? edge_point->size() : 0, stride, ioff, pose, &o, &last_result);
@@ -355,6 +368,7 @@ public:
         LocalizationUncertainty.PositionErrorDirection = Vector3d(r.pos_dir[0], r.pos_dir[1], r.pos_dir[2]);
         LocalizationUncertainty.OrientationErrorDirection = Vector3d(r.ori_dir[0], r.ori_dir[1], r.ori_dir[2]);
         std::memcpy(LocalizationUncertainty.Covariance.data(), r.cov, sizeof(r.cov));
+        isDegenerate = r.pos_inv_cond < Pos_degeneracy_threshold || r.ori_inv_cond < Ori_degeneracy_threshold;
         T_w_lidar = Transformd::from_pose7(r.pose);                                              // after MannualYawCorrection (:891-913)
         stats.time_elapsed = r.time_ms;                                                          // updateOptimizationStats (:198-210)
         stats.total_translation = r.total_translation; stats.total_rotation = r.total_rotation;

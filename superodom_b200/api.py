@@ -22,6 +22,7 @@ EXPORTS = [
     "so_map_set_edge_points", "so_map_add_surf", "so_map_add_edge", "so_map_add_scan", "so_map_add_registered_scan", "so_map_add_registered_edges", "so_map_add_scan_edge", "so_map_counts_5x5", "so_map_download", "so_map_size",
     "so_scan_prefilter", "so_scan_deskew", "so_scan_extract_uniform", "so_scan_extract_edges", "so_register", "so_register_prefiltered", "so_register_injected", "so_set_pose_sink", "so_register_batch", "so_register_batch_edges", "so_register_batch_device",
     "so_register_undistort", "so_register_undistort_edges", "so_register_prefiltered_undistort", "so_register_batch_undistort", "so_undistort_points", "so_register_optimized", "so_register_optimized_edges", "so_register_prefiltered_optimized", "so_register_batch_optimized", "so_evaluate_optimized", "so_evaluate_optimized_edges", "so_correspond", "so_correspond_seeded", "so_ordered_scans", "so_correspond_edge", "so_evaluate", "so_covariance",
+    "so_register_degeneracy", "so_register_batch_degeneracy", "so_degeneracy_analysis",
     "so_knn", "so_knn_device", "so_sampling_indices", "so_localize_global", "so_localize_scores", "so_localize_global_size", "so_localize_global_bnb", "so_localize_bnb_keys", "so_localize_bnb_bounds", "so_map_bounds", "so_kernel_launches", "so_bytes_copied", "so_build_flags", "so_profile_enable", "so_profile_get",
 ]
 
@@ -80,6 +81,24 @@ DEFAULT_MOTION_INFO = 0.0
 
 def motion(dt: float, prior7=(0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 1.0), info=(DEFAULT_MOTION_INFO,) * 6) -> Motion:
     return Motion(float(dt), (C.c_double * 7)(*[float(v) for v in prior7]), (C.c_double * 6)(*[float(v) for v in info]))
+
+
+class Degeneracy(C.Structure):
+    """so_degeneracy: thresholds on sqrt(i_k / i_max) of the translation / rotation information (each in [0, 1)); constrain = 1 keeps
+    the solve off the flagged directions, 0 only reports them."""
+    _fields_ = [("pos_threshold", C.c_double), ("ori_threshold", C.c_double), ("constrain", C.c_int32), ("pad_", C.c_int32)]
+
+
+def degeneracy(pos_threshold: float, ori_threshold: float, constrain: bool = True) -> Degeneracy:
+    return Degeneracy(float(pos_threshold), float(ori_threshold), int(constrain), 0)
+
+
+class DegeneracyResult(C.Structure):
+    """so_degeneracy_result: the registration, flagged directions per ICP iteration, and the last iteration's eigenpairs of I_t and
+    I_theta (ascending; axes[3k:3k+3] = eigenvector k) with their flags (bit k: eigenvector k flagged)."""
+    _fields_ = [("icp", IcpResult), ("iter_n_flag_pos", C.c_int32 * MAX_ICP_ITERS), ("iter_n_flag_ori", C.c_int32 * MAX_ICP_ITERS),
+                ("pos_info", C.c_double * 3), ("pos_axes", C.c_double * 9), ("ori_info", C.c_double * 3), ("ori_axes", C.c_double * 9),
+                ("flags_pos", C.c_int32), ("flags_ori", C.c_int32)]
 
 
 class GlobalOpts(C.Structure):
@@ -214,6 +233,11 @@ def load_library():
     L.so_ordered_scans.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     L.so_evaluate.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     L.so_covariance.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]
+    L.so_register_degeneracy.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t,
+                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.so_register_batch_degeneracy.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t,
+                                               C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.so_degeneracy_analysis.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     L.so_knn.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_int, C.c_float, C.c_void_p, C.c_void_p]
     L.so_knn_device.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_float, C.c_void_p, C.c_void_p]
     L.so_sampling_indices.argtypes = [C.c_uint32, C.c_int32, C.c_void_p, C.c_size_t, C.c_void_p]
@@ -756,6 +780,49 @@ class Context:
         assert a.ndim == 2 and a.shape[0] == a.shape[1] and a.shape[0] in (6, 12)
         r = IcpResult()
         self._chk(self.L.so_covariance(self.h, _p(a), a.shape[0], C.byref(r)), "so_covariance")
+        return r
+
+    # ---- degeneracy-aware registration (d: a Degeneracy, see degeneracy())
+    def register_degeneracy(self, scan_xyzi: np.ndarray, pose7, d: Degeneracy, max_icp_iters: int, max_surface_features: int = 0,
+                            edge_xyzi=None, **kw) -> DegeneracyResult:
+        s = np.ascontiguousarray(scan_xyzi, dtype=np.float32)
+        pose = np.ascontiguousarray(pose7, dtype=np.float64)
+        o = self._opts(max_icp_iters, max_surface_features, **kw)
+        r = DegeneracyResult()
+        stride = s.shape[1] * 4
+        ea = None if edge_xyzi is None or not len(edge_xyzi) else np.ascontiguousarray(edge_xyzi, dtype=np.float32)
+        e, ne = self._edge_arg(ea, s)
+        rc = self.L.so_register_degeneracy(self.h, _p(s), s.shape[0], e, ne, stride, 12 if s.shape[1] >= 4 else stride, _p(pose),
+                                           C.byref(d), C.byref(o), C.byref(r))
+        self._chk(rc, "so_register_degeneracy")
+        return r
+
+    def register_batch_degeneracy(self, scans_xyzi: np.ndarray, n_points, poses, ds, max_icp_iters: int, max_surface_features: int = 0,
+                                  edges_xyzi=None, n_edge=None, **kw):
+        """ds: one Degeneracy per scan; edges_xyzi / n_edge (optional): one edge cloud per scan, back to back."""
+        n_points = np.ascontiguousarray(n_points, dtype=np.uint32)
+        poses = np.ascontiguousarray(poses, dtype=np.float64)
+        ns = len(n_points)
+        da = (Degeneracy * ns)(*ds)
+        o = self._opts(max_icp_iters, max_surface_features, **kw)
+        res = (DegeneracyResult * ns)()
+        a = np.ascontiguousarray(scans_xyzi, dtype=np.float32)
+        e, ne = None, None
+        if n_edge is not None:
+            ne = np.ascontiguousarray(n_edge, dtype=np.uint32)
+            assert len(ne) == ns
+            ea = np.ascontiguousarray(edges_xyzi, dtype=np.float32).reshape(-1, a.shape[1])
+            e = _p(ea) if len(ea) else None
+        self._chk(self.L.so_register_batch_degeneracy(self.h, _p(a), _p(n_points), e, None if ne is None else _p(ne), ns, a.shape[1] * 4, 12,
+                                                      _p(poses), da, C.byref(o), res), "so_register_batch_degeneracy")
+        return res
+
+    def degeneracy_analysis(self, H, d: Degeneracy) -> DegeneracyResult:
+        """The analysis a degeneracy-aware solve begins with, on a symmetric H [6, 6]: eigenpairs and flags of I_t and I_theta."""
+        a = np.ascontiguousarray(H, dtype=np.float64)
+        assert a.shape == (6, 6)
+        r = DegeneracyResult()
+        self._chk(self.L.so_degeneracy_analysis(self.h, _p(a), C.byref(d), C.byref(r)), "so_degeneracy_analysis")
         return r
 
     # ---- global localization

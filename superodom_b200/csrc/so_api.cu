@@ -156,6 +156,7 @@ static void ctx_free(Ctx* c) {
     global_free(c);
     undistort_free(c);
     motion_free(c);
+    cudaFree(c->deg.d_st);
     features_free(c);
     if (c->ev_dec) cudaEventDestroy(c->ev_dec);
     if (c->ev0) cudaEventDestroy(c->ev0);
@@ -314,9 +315,10 @@ static int prepare_scans(Ctx* c, const float4* d_scan_in, const Chunk& ch, cudaS
 }
 
 // One or two scans in flight are launch-latency bound: the optimiser step is folded into the evaluation kernels (k_evaluate_lm, which
-// launch_first_eval / launch_evaluate take when the chunk has no edge cloud).  Mode OPTIMIZED has its own solve.
-static bool fused_lm(const Ctx* c, uint32_t n_scans, UndistortionMode mode) {
-    return n_scans <= 2 && !c->profiling && !c->no_fused_lm && mode != UndistortionMode::OPTIMIZED;
+// launch_first_eval / launch_evaluate take when the chunk has no edge cloud).  Mode OPTIMIZED and the degeneracy-aware registration
+// have their own step kernels.
+static bool fused_lm(const Ctx* c, uint32_t n_scans, UndistortionMode mode, bool degen) {
+    return n_scans <= 2 && !c->profiling && !c->no_fused_lm && mode != UndistortionMode::OPTIMIZED && !degen;
 }
 
 // Kernels one ICP iteration of a captured schedule launches: the unrolled graph runs `iters` of them, the loop graph one per
@@ -338,15 +340,16 @@ static uint64_t iteration_launches(UndistortionMode mode, bool fused, uint32_t g
 //   lm solves    k_evaluate<PH_EVAL> (+ k_edge_evaluate) + k_lm_step; OPTIMIZED: k_motion_eval<PH_EVAL> (+ k_motion_eval_edge) + k_motion_step
 // Preferred form: a CUDA-graph WHILE node around ONE iteration (k_loop_cond ends the loop when every scan of the chunk is done);
 // fallback: the schedule unrolled `iters` times.  Sets *was_loop to whether the loop form ran.  Profiling or injected neighbours:
-// launched one kernel at a time instead.
+// launched one kernel at a time instead.  dg: the chunk's DegenState array of a degeneracy-aware registration (k_lm_step_deg steps
+// its solves), else nullptr.
 static int run_schedule(Ctx* c, const Chunk& ch, int iters, int lm, UndistortionMode mode, const uint32_t* d_inject, int inject_iters,
-                        cudaStream_t run_stream, bool* was_loop) {
+                        cudaStream_t run_stream, bool* was_loop, DegenState* dg) {
     const MapView mv = map_view(c, c->surf);
     BatchView bv = batch_view(c, c->d_scan_sorted, ch.first);
     CorrBuf cb = c->corr;
     cb.nn = nullptr; cb.nn_d2 = nullptr;
     const uint32_t grid_x = ch.grid_x, n_scans = ch.count, grid_e = ch.grid_e;
-    const bool fused = fused_lm(c, n_scans, mode);
+    const bool fused = fused_lm(c, n_scans, mode, dg != nullptr);
     if (fused) bv.counters = c->d_counters + ch.first;
     bv.coop_knn = n_scans <= 2 && grid_x <= kCoopMaxGrid && !c->no_coop_knn;      // latency-bound search: a warp per query
     const MapView me = map_view(c, c->edge);
@@ -368,8 +371,8 @@ static int run_schedule(Ctx* c, const Chunk& ch, int iters, int lm, Undistortion
     };
     auto solve = [&](int phase, cudaStream_t s) {
         if (optimized) launch_motion_solve(phase, bv, cb, c->d_scan, c->und.d_time, c->mot.d_st, ch.first, mot_partials, c->mot.stride, grid_x, n_scans, s, mep);
-        else if (phase == PH_CORR) launch_first_eval(bv, cb, grid_x, n_scans, s, &me, &eb, grid_e);
-        else launch_evaluate(bv, cb, grid_x, n_scans, s, &eb, grid_e);
+        else if (phase == PH_CORR) launch_first_eval(bv, cb, grid_x, n_scans, s, &me, &eb, grid_e, dg);
+        else launch_evaluate(bv, cb, grid_x, n_scans, s, &eb, grid_e, dg);
     };
     auto iteration = [&](cudaStream_t s) {
         if (mode != UndistortionMode::NONE) head(s);
@@ -414,6 +417,7 @@ static int run_schedule(Ctx* c, const Chunk& ch, int iters, int lm, Undistortion
     key.nb[0] = mv.nb; key.nb[1] = me.nb; key.res[0] = mv.plane_res; key.res[1] = me.plane_res;
     if (mode != UndistortionMode::NONE) { key.mode = mode; key.und_time = c->und.d_time; }
     if (warp_edges) key.und_edge = c->und.d_ewarp;
+    key.degen = dg;
     Ctx::GraphSlot* slot = nullptr;
     for (auto& g : c->graphs)
         if (g.exec && std::memcmp(&g.key, &key, sizeof(key)) == 0) slot = &g;
@@ -631,7 +635,8 @@ static int register_core(Ctx* c, const RegisterRequest& q) {
             if (ch.grid_x == 0) continue;
             int rc = prepare_scans(c, d_scan, ch, st, true);
             bool was_loop = false;
-            if (!rc) rc = run_schedule(c, ch, o.max_icp_iters, o.lm_max_iterations, q.mode, q.inject ? c->d_inject : nullptr, q.inject_iters, st, &was_loop);
+            if (!rc) rc = run_schedule(c, ch, o.max_icp_iters, o.lm_max_iterations, q.mode, q.inject ? c->d_inject : nullptr, q.inject_iters, st, &was_loop,
+                                       q.degen ? c->deg.d_st + ch.first : nullptr);
             if (rc) {                                       // leave no work behind on the side streams before reporting the error
                 cudaStreamSynchronize(c->aux_stream);
                 cudaStreamSynchronize(c->copy_stream);
@@ -655,7 +660,7 @@ static int register_core(Ctx* c, const RegisterRequest& q) {
             if (!loop_flags[k]) continue;
             int max_it = 0;
             for (uint32_t s = chunks[k].first; s < chunks[k].first + chunks[k].count; ++s) max_it = std::max(max_it, int(c->h_state[s].n_iterations));
-            const bool fused = fused_lm(c, chunks[k].count, q.mode);
+            const bool fused = fused_lm(c, chunks[k].count, q.mode, q.degen != nullptr);
             c->launches += uint64_t(max_it) * (iteration_launches(q.mode, fused, chunks[k].grid_e, o.lm_max_iterations) + 1);   // + k_loop_cond
         }
         for (size_t s = 0; s < n_scans; ++s) {
@@ -705,6 +710,7 @@ int register_scans(Ctx* c, const RegisterRequest& q) {
     int rc = SO_OK;
     if (q.mode == UndistortionMode::APPROXIMATED) rc = undistort_reserve(c, total);
     if (q.mode == UndistortionMode::OPTIMIZED) rc = motion_reserve(c, total);
+    if (!rc && q.degen) rc = grow_buffer(c->deg.d_st, c->deg.st_cap, size_t(c->max_batch));
     if (!rc && q.inject) {
         const size_t words = size_t(q.inject_iters) * total * 5;
         rc = grow_buffer(c->d_inject, c->inject_cap, words);
@@ -745,6 +751,10 @@ int register_scans(Ctx* c, const RegisterRequest& q) {
         SO_CUDA_TRY(cudaMemcpyAsync(c->mot.d_st, q.motion, q.n_scans * sizeof(MotionState), cudaMemcpyHostToDevice, c->stream));
         count_h2d(c, q.n_scans * sizeof(MotionState));
     }
+    if (!rc && q.degen) {
+        SO_CUDA_TRY(cudaMemcpyAsync(c->deg.d_st, q.degen, q.n_scans * sizeof(DegenState), cudaMemcpyHostToDevice, c->stream));
+        count_h2d(c, q.n_scans * sizeof(DegenState));
+    }
     if (rc) return rc;
     rc = register_core(c, core);
     if (decimated) {
@@ -756,6 +766,11 @@ int register_scans(Ctx* c, const RegisterRequest& q) {
     if (!rc && q.mode == UndistortionMode::OPTIMIZED) {
         SO_CUDA_TRY(cudaMemcpyAsync(q.motion, c->mot.d_st, q.n_scans * sizeof(MotionState), cudaMemcpyDeviceToHost, c->stream));
         count_d2h(c, q.n_scans * sizeof(MotionState));
+        SO_CUDA_TRY(cudaStreamSynchronize(c->stream));
+    }
+    if (!rc && q.degen) {
+        SO_CUDA_TRY(cudaMemcpyAsync(q.degen, c->deg.d_st, q.n_scans * sizeof(DegenState), cudaMemcpyDeviceToHost, c->stream));
+        count_d2h(c, q.n_scans * sizeof(DegenState));
         SO_CUDA_TRY(cudaStreamSynchronize(c->stream));
     }
     if (rc) return rc;
@@ -1320,6 +1335,75 @@ int so_register_batch_device(so_ctx* ctx, const void* d_scans, const uint32_t* n
     return register_scans(c, q);
 }
 
+// ---- degeneracy-aware registration: so_register's schedule with k_lm_step_deg stepping the solves (DESIGN.md section 3)
+static int check_degeneracy(const so_degeneracy* d, size_t n) {
+    for (size_t s = 0; s < n; ++s) {
+        if (!(d[s].pos_threshold >= 0.0 && d[s].pos_threshold < 1.0) || !(d[s].ori_threshold >= 0.0 && d[s].ori_threshold < 1.0))
+            return fail(SO_ERR_ARG, "degeneracy thresholds must be in [0, 1)");
+        if (d[s].constrain != 0 && d[s].constrain != 1) return fail(SO_ERR_ARG, "so_degeneracy.constrain must be 0 or 1");
+    }
+    return SO_OK;
+}
+static DegenState degen_state(const so_degeneracy& d) {
+    DegenState s{};
+    s.pos_thr2 = d.pos_threshold * d.pos_threshold;
+    s.ori_thr2 = d.ori_threshold * d.ori_threshold;
+    s.constrain = d.constrain;
+    s.m = 6;
+    return s;
+}
+static void fill_degeneracy(const DegenState& s, so_degeneracy_result* out) {
+    std::memcpy(out->iter_n_flag_pos, s.iter_n_flag_pos, sizeof(out->iter_n_flag_pos));
+    std::memcpy(out->iter_n_flag_ori, s.iter_n_flag_ori, sizeof(out->iter_n_flag_ori));
+    std::memcpy(out->pos_info, s.pos_info, sizeof(out->pos_info)); std::memcpy(out->pos_axes, s.pos_axes, sizeof(out->pos_axes));
+    std::memcpy(out->ori_info, s.ori_info, sizeof(out->ori_info)); std::memcpy(out->ori_axes, s.ori_axes, sizeof(out->ori_axes));
+    out->flags_pos = s.flags_pos; out->flags_ori = s.flags_ori;
+}
+
+int so_register_degeneracy(so_ctx* ctx, const void* surf, size_t n_surf, const void* edge, size_t n_edge, size_t stride, size_t ioff,
+                           const double pose_in[7], const so_degeneracy* d, const so_icp_opts* opts, so_degeneracy_result* out) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c || !pose_in || !d || !opts || !out || (!surf && n_surf) || (!edge && n_edge) || stride < 12) return fail(SO_ERR_ARG, "bad args");
+    int rc = check_degeneracy(d, 1);
+    if (rc) return rc;
+    if (n_edge > c->edge_cap) return fail(SO_ERR_CAPACITY, "edge cloud larger than so_config.max_scan_points");
+    if (n_surf > c->cfg.max_scan_points) return fail(SO_ERR_CAPACITY, "scan larger than so_config.max_scan_points");
+    const uint32_t n = uint32_t(n_surf), ne = uint32_t(n_edge);
+    DegenState S = degen_state(*d);
+    RegisterRequest q = single_scan(&n, pose_in, opts, &out->icp);
+    q.scans = surf; q.stride = stride; q.ioff = ioff;
+    q.edge = edge; q.n_edge = &ne;
+    q.degen = &S;
+    rc = register_scans(c, q);
+    if (rc) return rc;
+    fill_degeneracy(S, out);
+    return out->icp.status;
+}
+
+int so_register_batch_degeneracy(so_ctx* ctx, const void* surf, const uint32_t* n_points, const void* edge, const uint32_t* n_edge, size_t n_scans,
+                                 size_t stride, size_t ioff, const double* poses_in, const so_degeneracy* d, const so_icp_opts* opts,
+                                 so_degeneracy_result* results) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c || !surf || !n_points || !poses_in || !d || !opts || !results || stride < 12) return fail(SO_ERR_ARG, "bad args");
+    int rc = check_batch(c, n_points, n_scans);
+    if (!rc) rc = check_degeneracy(d, n_scans);
+    if (rc) return rc;
+    size_t total_e = 0;
+    if (n_edge) for (size_t s = 0; s < n_scans; ++s) total_e += n_edge[s];
+    if (total_e > c->edge_cap) return fail(SO_ERR_CAPACITY, "edge clouds of the batch exceed so_config.max_scan_points points in total");
+    if (total_e && !edge) return fail(SO_ERR_ARG, "bad args");
+    std::vector<so_icp_result> icp(n_scans);
+    std::vector<DegenState> S(n_scans);
+    for (size_t s = 0; s < n_scans; ++s) S[s] = degen_state(d[s]);
+    RegisterRequest q = batch_request(surf, n_points, n_scans, stride, ioff, poses_in, opts, icp.data());
+    if (n_edge) { q.src = Source::HOST; q.edge = edge; q.n_edge = n_edge; }      // as so_register_batch_edges
+    q.degen = S.data();
+    rc = register_scans(c, q);
+    if (rc) return rc;
+    for (size_t s = 0; s < n_scans; ++s) { results[s].icp = icp[s]; fill_degeneracy(S[s], results + s); }
+    return SO_OK;
+}
+
 // so_register_undistort (edge == nullptr, n_edge == 0) and so_register_undistort_edges: both clouds share the layout and the time offset
 static int register_undistort(so_ctx* ctx, const void* surf, size_t n_surf, const void* edge, size_t n_edge, size_t stride, size_t ioff,
                               size_t toff, const double pose_in[7], const so_undistort* u, const so_icp_opts* opts, so_icp_result* out) {
@@ -1624,6 +1708,30 @@ int so_covariance(so_ctx* ctx, const double* H, int32_t n, so_icp_result* out) {
     std::memcpy(out->cov, s.cov, sizeof(out->cov));
     out->pos_err = s.pos_err; out->pos_inv_cond = s.pos_inv_cond; out->ori_err_deg = s.ori_err_deg; out->ori_inv_cond = s.ori_inv_cond;
     for (int i = 0; i < 3; ++i) { out->pos_dir[i] = s.pos_dir[i]; out->ori_dir[i] = s.ori_dir[i]; }
+    return SO_OK;
+}
+
+int so_degeneracy_analysis(so_ctx* ctx, const double* H, const so_degeneracy* d, so_degeneracy_result* out) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c || !H || !d || !out) return fail(SO_ERR_ARG, "bad args");
+    { int rc = check_degeneracy(d, 1); if (rc) return rc; }
+    SO_CUDA_TRY(cudaSetDevice(c->device));
+    { int rc = grow_buffer(c->deg.d_st, c->deg.st_cap, std::max<size_t>(c->max_batch, 1)); if (rc) return rc; }
+    IcpState& s = c->h_state[0];                              // the state of a preceding so_correspond* is replaced
+    std::memset(&s, 0, sizeof(s));
+    for (int i = 0; i < 6; ++i) for (int j = i; j < 6; ++j) s.H[tri(i, j)] = H[i * 6 + j];
+    DegenState S = degen_state(*d);
+    timed_launch_begin(c);
+    SO_CUDA_TRY(cudaMemcpyAsync(c->d_state, c->h_state, sizeof(IcpState), cudaMemcpyHostToDevice, c->stream));
+    SO_CUDA_TRY(cudaMemcpyAsync(c->deg.d_st, &S, sizeof(DegenState), cudaMemcpyHostToDevice, c->stream));
+    launch_degeneracy_analysis(c->d_state, c->deg.d_st, c->stream);
+    c->launches++;
+    timed_launch_end(c, 1);
+    SO_CUDA_TRY(cudaGetLastError());
+    SO_CUDA_TRY(cudaMemcpyAsync(&S, c->deg.d_st, sizeof(DegenState), cudaMemcpyDeviceToHost, c->stream));
+    SO_CUDA_TRY(cudaStreamSynchronize(c->stream));
+    std::memset(out, 0, sizeof(*out));
+    fill_degeneracy(S, out);
     return SO_OK;
 }
 

@@ -99,6 +99,7 @@ struct RegisterRequest {
     UndistortionMode mode = UndistortionMode::NONE;
     const UndistortParams* und = nullptr;          // APPROXIMATED: [n_scans]
     MotionState* motion = nullptr;                 // OPTIMIZED: [n_scans], uploaded first and read back after the registration
+    DegenState* degen = nullptr;                   // degeneracy-aware registration (mode NONE): [n_scans], uploaded first and read back
     const uint32_t* inject = nullptr;              // host neighbour ids [inject_iters][n][5] in place of the search
     int inject_iters = 0;
     bool allow_shift = false;                      // the map may shift to the priors (single-scan registration)
@@ -198,6 +199,7 @@ struct Ctx {
         const void* ptrs[8]; int32_t origin[3]; int32_t nb[2]; float res[2];
         UndistortionMode mode; const void* und_time;   // the head of every iteration (NONE / nullptr: none)
         const void* und_edge;                          // APPROXIMATED with an edge cloud: the warped edge cloud the line branch reads
+        const void* degen;                             // degeneracy-aware registration: the DegenState array (nullptr: off)
     };
     struct GraphSlot {
         cudaGraphExec_t exec = nullptr;
@@ -257,6 +259,10 @@ struct Ctx {
         uint32_t stride = 0;                                               // CTAs per scan the partials are laid out for
         double* d_epartials = nullptr; size_t epartials_cap = 0;           // the edge clouds' per-CTA sums (so_register_optimized_edges)
     } mot;
+    // ---- degeneracy-aware registration (so_register_degeneracy*, so_degeneracy_analysis): allocated on first use --------------
+    struct Deg {
+        DegenState* d_st = nullptr; size_t st_cap = 0;                     // [max_batch] per-scan analysis and solve columns
+    } deg;
     // ---- edge extraction (so_scan_extract_edges): allocated on first use, grown on demand; never touches the scan buffers ----
     struct Feat {
         unsigned char* d_raw = nullptr; size_t raw_cap = 0;                // the caller's records as given

@@ -231,8 +231,45 @@ __device__ __noinline__ void end_solve(IcpState& st) {
     }
 }
 
-// TrustRegionMinimizer loop from FinalizeIterationAndCheckIfMinimizerCanContinue up to the next cost evaluation.
-__device__ __noinline__ void lm_continue(IcpState& st, bool step_successful) {
+// Reduced system of a degeneracy-aware solve: Hr = B^T H B and gr = B^T g over the columns of B (zero beyond dg.m, so Hr and gr are
+// zero-padded to 6).
+__device__ __forceinline__ void reduced_system(const IcpState& st, const DegenState& dg, double Hr[36], double gr[6]) {
+    double HB[36];
+    _Pragma("unroll") for (int i = 0; i < 6; ++i)
+        _Pragma("unroll") for (int k = 0; k < 6; ++k) {
+            double t = 0.0;
+            _Pragma("unroll") for (int j = 0; j < 6; ++j) t += st.H[i <= j ? tri(i, j) : tri(j, i)] * dg.B[j * 6 + k];
+            HB[i * 6 + k] = t;
+        }
+    _Pragma("unroll") for (int k = 0; k < 6; ++k) {
+        double t = 0.0;
+        _Pragma("unroll") for (int i = 0; i < 6; ++i) t += dg.B[i * 6 + k] * st.g[i];
+        gr[k] = t;
+        _Pragma("unroll") for (int l = 0; l < 6; ++l) {
+            double u = 0.0;
+            _Pragma("unroll") for (int i = 0; i < 6; ++i) u += dg.B[i * 6 + k] * HB[i * 6 + l];
+            Hr[k * 6 + l] = u;
+        }
+    }
+}
+
+// ||x - Plus(x, -B B^T g)||_inf: the gradient max-norm of the solve on B's columns.  (Not through grad_max_norm: a caller with a
+// local-memory g would change the code of the ambient solve, whose callers all pass shared memory.)
+__device__ __noinline__ double grad_max_norm_red(const double x[7], const double g[6], const DegenState& dg) {
+    double gr[6], neg[6], xp[7];
+    _Pragma("unroll") for (int k = 0; k < 6; ++k) { double t = 0.0; _Pragma("unroll") for (int i = 0; i < 6; ++i) t += dg.B[i * 6 + k] * g[i]; gr[k] = t; }
+    _Pragma("unroll") for (int i = 0; i < 6; ++i) { double t = 0.0; _Pragma("unroll") for (int k = 0; k < 6; ++k) t += dg.B[i * 6 + k] * gr[k]; neg[i] = -t; }
+    pose_plus(x, neg, xp);
+    double m = 0.0;
+    _Pragma("unroll") for (int i = 0; i < 7; ++i) m = fmax(m, fabs(x[i] - xp[i]));
+    return m;
+}
+
+// TrustRegionMinimizer loop from FinalizeIterationAndCheckIfMinimizerCanContinue up to the next cost evaluation.  RED: the solve on the
+// m columns of dg.B (local parameterisation x [+] B y): Jacobi scaling, LM diagonal and model cost change of the reduced system, which is
+// padded to 6 with identity rows and zero right-hand sides for chol6_solve.
+template <bool RED>
+__device__ __forceinline__ void lm_continue_t(IcpState& st, const DegenState* dg, bool step_successful) {
     for (;;) {
         if (step_successful) st.num_successful++; else st.num_unsuccessful++;
         if (st.lm_iter >= st.lm_max_iterations) { st.termination = 0; end_solve(st); return; }
@@ -242,9 +279,18 @@ __device__ __noinline__ void lm_continue(IcpState& st, bool step_successful) {
         step_successful = false;
         // LevenbergMarquardtStrategy::ComputeStep on the Jacobi-scaled system
         double Hs[36], gs[6];
-        _Pragma("unroll") for (int i = 0; i < 6; ++i) {
-            gs[i] = st.g[i] * st.scale[i];
-            _Pragma("unroll") for (int j = 0; j < 6; ++j) Hs[i * 6 + j] = st.H[i <= j ? tri(i, j) : tri(j, i)] * st.scale[i] * st.scale[j];
+        if constexpr (RED) {
+            double Hr[36], gr[6];
+            reduced_system(st, *dg, Hr, gr);
+            _Pragma("unroll") for (int i = 0; i < 6; ++i) {
+                gs[i] = gr[i] * st.scale[i];
+                _Pragma("unroll") for (int j = 0; j < 6; ++j) Hs[i * 6 + j] = Hr[i * 6 + j] * st.scale[i] * st.scale[j];
+            }
+        } else {
+            _Pragma("unroll") for (int i = 0; i < 6; ++i) {
+                gs[i] = st.g[i] * st.scale[i];
+                _Pragma("unroll") for (int j = 0; j < 6; ++j) Hs[i * 6 + j] = st.H[i <= j ? tri(i, j) : tri(j, i)] * st.scale[i] * st.scale[j];
+            }
         }
         if (!st.reuse_diagonal)
             _Pragma("unroll") for (int j = 0; j < 6; ++j) st.diag[j] = fmin(fmax(Hs[j * 6 + j], 1e-6), 1e32);
@@ -252,6 +298,7 @@ __device__ __noinline__ void lm_continue(IcpState& st, bool step_successful) {
         double M[36], y[6];
         _Pragma("unroll") for (int i = 0; i < 36; ++i) M[i] = Hs[i];
         _Pragma("unroll") for (int j = 0; j < 6; ++j) M[j * 6 + j] += st.diag[j] / st.radius;       // lm_diagonal^2 = diagonal / radius
+        if constexpr (RED) _Pragma("unroll") for (int j = 0; j < 6; ++j) if (j >= dg->m) M[j * 6 + j] = 1.0;
         bool valid = chol6_solve(M, gs, y);
         double step[6], mcc = 0.0;
         if (valid) {
@@ -270,11 +317,19 @@ __device__ __noinline__ void lm_continue(IcpState& st, bool step_successful) {
         st.model_cost_change = mcc;
         double delta[6];
         _Pragma("unroll") for (int j = 0; j < 6; ++j) delta[j] = step[j] * st.scale[j];
-        pose_plus(st.x, delta, st.cand);
+        if constexpr (RED) {                    // the ambient step B y
+            double d6[6];
+            _Pragma("unroll") for (int i = 0; i < 6; ++i) { double t = 0.0; _Pragma("unroll") for (int k = 0; k < 6; ++k) t += dg->B[i * 6 + k] * delta[k]; d6[i] = t; }
+            pose_plus(st.x, d6, st.cand);
+        } else {
+            pose_plus(st.x, delta, st.cand);
+        }
         st.phase = PH_EVAL;
         return;
     }
 }
+__device__ __noinline__ void lm_continue(IcpState& st, bool step_successful) { lm_continue_t<false>(st, nullptr, step_successful); }
+__device__ __noinline__ void lm_continue_red(IcpState& st, const DegenState& dg, bool step_successful) { lm_continue_t<true>(st, &dg, step_successful); }
 
 // SE3AbsolutatePoseFactor (factor/SE3AbsolutatePoseFactor.cpp:9-51) added by addAbsolutePoseConstraints (LidarSlam.cpp:285-298):
 // residual [p - p_meas ; 2 vec(q_meas^* q)] times sqrt_information (diagonal here), no loss function; local Jacobian
@@ -301,8 +356,85 @@ __device__ __noinline__ void add_pose_prior(const IcpState& st, const double x[7
     a[27] += 0.5 * sq;
 }
 
-// IterationZero of a new solve, fed by k_fit's reduction.
-__device__ __noinline__ void lm_begin_solve(IcpState& st, const double* acc_in, int n_ok) {
+// Pseudo-inverse of a symmetric 3x3 with ceres::Covariance's cut rule (covariance_and_errors_warp): eigen-directions with
+// sqrt(w_k / w_max) < 1e-7 or w_k <= 0 are dropped.
+__device__ __forceinline__ void pinv3_cut(const double A[9], double P[9]) {
+    double a[9], v[9], w[3];
+    _Pragma("unroll") for (int i = 0; i < 9; ++i) a[i] = A[i];
+    jacobi_eig<3, 20, true>(a, v, w);
+    double inv[3];
+    _Pragma("unroll") for (int k = 0; k < 3; ++k) {
+        const double ratio = (w[k] > 0.0 && w[2] > 0.0) ? sqrt(w[k] / w[2]) : 0.0;
+        inv[k] = ratio < 1e-7 ? 0.0 : 1.0 / w[k];
+    }
+    _Pragma("unroll") for (int i = 0; i < 3; ++i)
+        _Pragma("unroll") for (int j = 0; j < 3; ++j) {
+            double t = 0.0;
+            _Pragma("unroll") for (int k = 0; k < 3; ++k) t += v[i * 3 + k] * inv[k] * v[j * 3 + k];
+            P[i * 3 + j] = t;
+        }
+}
+
+// Information of one block: the Schur complement I = A - C P C^T (P the cut pseudo-inverse of the other block), its eigenpairs
+// (ascending) and the flagged ones (i_k <= thr2 * max(i_max, 0)).  C: the 3x3 coupling, rows this block, columns the other one.
+__device__ __forceinline__ int block_information(const double A[9], const double C[9], const double Other[9], double thr2, double info[3], double axes[9]) {
+    double P[9], CP[9], I[9], v[9];
+    pinv3_cut(Other, P);
+    _Pragma("unroll") for (int i = 0; i < 3; ++i)
+        _Pragma("unroll") for (int j = 0; j < 3; ++j) {
+            double t = 0.0;
+            _Pragma("unroll") for (int k = 0; k < 3; ++k) t += C[i * 3 + k] * P[k * 3 + j];
+            CP[i * 3 + j] = t;
+        }
+    _Pragma("unroll") for (int i = 0; i < 3; ++i)
+        _Pragma("unroll") for (int j = i; j < 3; ++j) {
+            double t = 0.0;
+            _Pragma("unroll") for (int k = 0; k < 3; ++k) t += CP[i * 3 + k] * C[j * 3 + k];
+            I[i * 3 + j] = I[j * 3 + i] = A[i * 3 + j] - t;      // symmetric by construction
+        }
+    jacobi_eig<3, 20, true>(I, v, info);
+    int flags = 0;
+    const double cut = thr2 * fmax(info[2], 0.0);
+    _Pragma("unroll") for (int k = 0; k < 3; ++k) {
+        _Pragma("unroll") for (int i = 0; i < 3; ++i) axes[k * 3 + i] = v[i * 3 + k];
+        if (info[k] <= cut) flags |= 1 << k;
+    }
+    return flags;
+}
+
+// The degeneracy analysis of a solve (DESIGN.md section 3) on the normal matrix H (upper triangle, order t, theta): I_t and I_theta,
+// their eigenpairs and flags, and B = the unflagged eigenvectors (translation ones first).  m = 6 unless constrain and something is
+// flagged; B is then the identity.
+__device__ __noinline__ void degeneracy_analysis(const double Hu[21], DegenState& dg) {
+    double Htt[9], Htr[9], Hrt[9], Hrr[9];
+    _Pragma("unroll") for (int i = 0; i < 3; ++i)
+        _Pragma("unroll") for (int j = 0; j < 3; ++j) {
+            Htt[i * 3 + j] = Hu[i <= j ? tri(i, j) : tri(j, i)];
+            Hrr[i * 3 + j] = Hu[i <= j ? tri(i + 3, j + 3) : tri(j + 3, i + 3)];
+            Htr[i * 3 + j] = Hu[tri(i, j + 3)];
+            Hrt[j * 3 + i] = Hu[tri(i, j + 3)];
+        }
+    dg.flags_pos = block_information(Htt, Htr, Hrr, dg.pos_thr2, dg.pos_info, dg.pos_axes);
+    dg.flags_ori = block_information(Hrr, Hrt, Htt, dg.ori_thr2, dg.ori_info, dg.ori_axes);
+    _Pragma("unroll") for (int i = 0; i < 36; ++i) dg.B[i] = 0.0;
+    const bool reduce = dg.constrain && (dg.flags_pos | dg.flags_ori);
+    int m = 0;
+    _Pragma("unroll") for (int k = 0; k < 6; ++k) {
+        const bool pos = k < 3;
+        const int e = pos ? k : k - 3;
+        if (!reduce) { dg.B[k * 6 + k] = 1.0; ++m; continue; }
+        if (((pos ? dg.flags_pos : dg.flags_ori) >> e) & 1) continue;
+        const double* ax = (pos ? dg.pos_axes : dg.ori_axes) + 3 * e;
+        _Pragma("unroll") for (int i = 0; i < 3; ++i) dg.B[(i + (pos ? 0 : 3)) * 6 + m] = ax[i];
+        ++m;
+    }
+    dg.m = m;
+}
+
+// IterationZero of a new solve, fed by k_fit's reduction.  DEG: the degeneracy-aware solve -- the analysis on H at x_iter_start, then
+// the solve on B's columns when it has fewer than 6 (otherwise exactly the ambient solve).
+template <bool DEG>
+__device__ __forceinline__ void lm_begin_solve_t(IcpState& st, DegenState* dg, const double* acc_in, int n_ok) {
     double acc[kAcc];
     _Pragma("unroll") for (int k = 0; k < kAcc; ++k) acc[k] = acc_in[k];
     if (st.use_prior) {
@@ -336,16 +468,33 @@ __device__ __noinline__ void lm_begin_solve(IcpState& st, const double* acc_in, 
         st.status = SO_STATUS_INVALID_EVALUATION; st.phase = PH_DONE;
         return;
     }
-    _Pragma("unroll") for (int j = 0; j < 6; ++j) st.scale[j] = 1.0 / (1.0 + sqrt(st.H[tri(j, j)]));      // jacobi_scaling at iteration 0
+    bool red = false;
+    if constexpr (DEG) {
+        degeneracy_analysis(st.H, *dg);
+        dg->iter_n_flag_pos[st.icp_iter] = __popc(dg->flags_pos);
+        dg->iter_n_flag_ori[st.icp_iter] = __popc(dg->flags_ori);
+        red = dg->m < 6;
+    }
+    if (red) {
+        double Hr[36], gr[6];
+        reduced_system(st, *dg, Hr, gr);
+        _Pragma("unroll") for (int j = 0; j < 6; ++j) st.scale[j] = 1.0 / (1.0 + sqrt(Hr[j * 6 + j]));      // over B's columns
+    } else {
+        _Pragma("unroll") for (int j = 0; j < 6; ++j) st.scale[j] = 1.0 / (1.0 + sqrt(st.H[tri(j, j)]));      // jacobi_scaling at iteration 0
+    }
     double xn = 0.0; _Pragma("unroll") for (int i = 0; i < 7; ++i) xn += st.x[i] * st.x[i];
     st.x_norm = sqrt(xn);
-    st.gmax = grad_max_norm(st.x, st.g);
+    st.gmax = red ? grad_max_norm_red(st.x, st.g, *dg) : grad_max_norm(st.x, st.g);
     st.radius = 1e4; st.decrease_factor = 2.0; st.reuse_diagonal = 0;
-    lm_continue(st, false);
+    if (red) lm_continue_red(st, *dg, false);
+    else lm_continue(st, false);
 }
+__device__ __noinline__ void lm_begin_solve(IcpState& st, const double* acc_in, int n_ok) { lm_begin_solve_t<false>(st, nullptr, acc_in, n_ok); }
+__device__ __noinline__ void lm_begin_solve_deg(IcpState& st, DegenState& dg, const double* acc_in, int n_ok) { lm_begin_solve_t<true>(st, &dg, acc_in, n_ok); }
 
-// After the cost (and H, g) at the candidate are known.
-__device__ __noinline__ void lm_after_eval(IcpState& st, const double* acc_in) {
+// After the cost (and H, g) at the candidate are known.  RED: of a solve on B's columns.
+template <bool RED>
+__device__ __forceinline__ void lm_after_eval_t(IcpState& st, const DegenState* dg, const double* acc_in) {
     double acc[kAcc];
     _Pragma("unroll") for (int k = 0; k < kAcc; ++k) acc[k] = acc_in[k];
     if (st.use_prior) add_pose_prior(st, st.cand, acc);
@@ -365,16 +514,26 @@ __device__ __noinline__ void lm_after_eval(IcpState& st, const double* acc_in) {
         _Pragma("unroll") for (int k = 0; k < 21; ++k) st.H[k] = acc[k];
         _Pragma("unroll") for (int k = 0; k < 6; ++k) st.g[k] = acc[21 + k];
         st.cost = cand_cost;
-        st.gmax = grad_max_norm(st.x, st.g);
+        if constexpr (RED) st.gmax = grad_max_norm_red(st.x, st.g, *dg);
+        else st.gmax = grad_max_norm(st.x, st.g);
         const double t = 2.0 * rd - 1.0;
         st.radius = st.radius / fmax(1.0 / 3.0, 1.0 - t * t * t);
         st.radius = fmin(1e16, st.radius);
         st.decrease_factor = 2.0; st.reuse_diagonal = 0;
-        lm_continue(st, true);
+        if constexpr (RED) lm_continue_red(st, *dg, true);
+        else lm_continue(st, true);
     } else {                // StepRejected
         st.radius = st.radius / st.decrease_factor; st.decrease_factor *= 2.0; st.reuse_diagonal = 1;
-        lm_continue(st, false);
+        if constexpr (RED) lm_continue_red(st, *dg, false);
+        else lm_continue(st, false);
     }
+}
+__device__ __noinline__ void lm_after_eval(IcpState& st, const double* acc_in) { lm_after_eval_t<false>(st, nullptr, acc_in); }
+// the degeneracy-aware solve's: on B's columns when it has fewer than 6, else the ambient step (its own copy: a third caller of
+// lm_after_eval changes that function's code in the other kernels)
+__device__ __noinline__ void lm_after_eval_deg(IcpState& st, const DegenState& dg, const double* acc_in) {
+    if (dg.m < 6) lm_after_eval_t<true>(st, &dg, acc_in);
+    else lm_after_eval_t<false>(st, nullptr, acc_in);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -1386,9 +1545,10 @@ __global__ void __launch_bounds__(kThreads) k_edge_evaluate(BatchView bv, EdgeBu
 // k_lm_step: one CTA per scan.  Sums the per-CTA partials of the preceding k_fit (AFTER == PH_CORR) or k_evaluate
 // (AFTER == PH_EVAL) in a fixed order, then one thread advances the optimiser / ICP state machine.
 // ------------------------------------------------------------------------------------------------------------------
-// Called by >= 128 threads of one CTA (all of them: it synchronises the CTA); the first 128 do the work.
-template <int AFTER>
-__device__ __forceinline__ void lm_step_body(const BatchView& bv, int s, uint32_t n_partials, uint32_t edge_partial_offset) {
+// Called by >= 128 threads of one CTA (all of them: it synchronises the CTA); the first 128 do the work.  DEG: the step of the
+// degeneracy-aware registration, with the scan's DegenState (dg: the chunk's array) beside its IcpState.
+template <int AFTER, bool DEG = false>
+__device__ __forceinline__ void lm_step_body(const BatchView& bv, int s, uint32_t n_partials, uint32_t edge_partial_offset, DegenState* dg = nullptr) {
     IcpState* st = bv.st + s;
     __shared__ double s_red[4][kAcc];
     __shared__ double s_sum[kAcc];
@@ -1413,6 +1573,14 @@ __device__ __forceinline__ void lm_step_body(const BatchView& bv, int s, uint32_
         unsigned long long* dst = reinterpret_cast<unsigned long long*>(&s_st);
         for (uint32_t k = threadIdx.x; k < sizeof(IcpState) / 8; k += blockDim.x) dst[k] = src[k];
     }
+    DegenState* sdg = nullptr;                             // the DegenState's shared copy, the same way
+    if constexpr (DEG) {
+        __shared__ DegenState s_dg;
+        sdg = &s_dg;
+        const unsigned long long* src = reinterpret_cast<const unsigned long long*>(dg + s);
+        unsigned long long* dst = reinterpret_cast<unsigned long long*>(&s_dg);
+        for (uint32_t k = threadIdx.x; k < sizeof(DegenState) / 8; k += blockDim.x) dst[k] = src[k];
+    }
     __syncthreads();
     if (threadIdx.x < kAcc) s_sum[threadIdx.x] = (s_red[0][threadIdx.x] + s_red[1][threadIdx.x]) + (s_red[2][threadIdx.x] + s_red[3][threadIdx.x]);
     __syncthreads();
@@ -1430,13 +1598,15 @@ __device__ __forceinline__ void lm_step_body(const BatchView& bv, int s, uint32_
                 for (int k = 0; k < 21; ++k) S.H[k] = s_sum[k];
                 for (int k = 0; k < 6; ++k) S.g[k] = s_sum[21 + k];
                 S.cost = s_sum[27]; S.n_ok = n_ok; S.phase = PH_DONE;
-            } else lm_begin_solve(S, s_sum, n_ok);
+            } else if constexpr (DEG) lm_begin_solve_deg(S, *sdg, s_sum, n_ok);
+            else lm_begin_solve(S, s_sum, n_ok);
         } else {
             if (S.max_icp_iters < 0) {          // stage mode (so_evaluate): report and stop
                 for (int k = 0; k < 21; ++k) S.H[k] = s_sum[k];
                 for (int k = 0; k < 6; ++k) S.g[k] = s_sum[21 + k];
                 S.cost = s_sum[27]; S.phase = PH_DONE;
-            } else lm_after_eval(S, s_sum);
+            } else if constexpr (DEG) lm_after_eval_deg(S, *sdg, s_sum);
+            else lm_after_eval(S, s_sum);
         }
     }
     __syncthreads();
@@ -1450,6 +1620,11 @@ __device__ __forceinline__ void lm_step_body(const BatchView& bv, int s, uint32_
         unsigned long long* dst = reinterpret_cast<unsigned long long*>(st);
         for (uint32_t k = threadIdx.x; k < sizeof(IcpState) / 8; k += blockDim.x) dst[k] = src[k];
     }
+    if constexpr (DEG) {
+        const unsigned long long* src = reinterpret_cast<const unsigned long long*>(sdg);
+        unsigned long long* dst = reinterpret_cast<unsigned long long*>(dg + s);
+        for (uint32_t k = threadIdx.x; k < sizeof(DegenState) / 8; k += blockDim.x) dst[k] = src[k];
+    }
 }
 
 template <int AFTER>
@@ -1458,6 +1633,18 @@ __global__ void __launch_bounds__(128) k_lm_step(BatchView bv, uint32_t n_partia
     if (bv.st[s].phase != AFTER) return;
     lm_step_body<AFTER>(bv, s, n_partials, edge_partial_offset);
 }
+
+// k_lm_step of the degeneracy-aware registration (so_register_degeneracy*); dg: the chunk's DegenState array
+template <int AFTER>
+__global__ void __launch_bounds__(128) k_lm_step_deg(BatchView bv, uint32_t n_partials, uint32_t edge_partial_offset, DegenState* __restrict__ dg) {
+    const int s = blockIdx.x;
+    if (bv.st[s].phase != AFTER) return;
+    lm_step_body<AFTER, true>(bv, s, n_partials, edge_partial_offset, dg);
+}
+
+// so_degeneracy_analysis: degeneracy_analysis on st->H, one thread
+__global__ void k_degeneracy_analysis(const IcpState* __restrict__ st, DegenState* __restrict__ dg) { degeneracy_analysis(st->H, *dg); }
+void launch_degeneracy_analysis(const IcpState* st, DegenState* dg, cudaStream_t stream) { k_degeneracy_analysis<<<1, 1, 0, stream>>>(st, dg); }
 
 // so_covariance (6 columns): the covariance step that ends a registration, on st->H, in one 32-thread CTA and a shared copy of the
 // state as lm_step_body runs it
@@ -1602,12 +1789,13 @@ void launch_inject(const MapView& m, const float4* by_id, uint32_t n_map, const 
     if (grid_x) k_knn_inject<<<dim3(grid_x, n_scans), kThreads, 0, st>>>(m, by_id, n_map, bv, nb, ids, n_trace_iters);
 }
 void launch_first_eval(const BatchView& bv, const CorrBuf& cb, uint32_t grid_x, uint32_t n_scans, cudaStream_t st, const MapView* medge, const EdgeBuf* eb,
-                       uint32_t grid_e) {
+                       uint32_t grid_e, DegenState* dg) {
     const uint32_t gp = grid_x ? eval_grid(grid_x * kThreads) : 0;
-    if (bv.counters && gp && !grid_e) { k_evaluate_lm<PH_CORR><<<dim3(gp, n_scans), kThreads, 0, st>>>(bv, cb, bv.counters); return; }
+    if (bv.counters && gp && !grid_e && !dg) { k_evaluate_lm<PH_CORR><<<dim3(gp, n_scans), kThreads, 0, st>>>(bv, cb, bv.counters); return; }
     if (gp) k_evaluate<PH_CORR><<<dim3(gp, n_scans), kThreads, 0, st>>>(bv, cb);
     if (grid_e) k_edge_fit<<<dim3(grid_e, n_scans), kThreads, 0, st>>>(*medge, bv, *eb, bv.edge_partial_offset);
-    k_lm_step<PH_CORR><<<n_scans, 128, 0, st>>>(bv, gp, bv.edge_partial_offset);
+    if (dg) k_lm_step_deg<PH_CORR><<<n_scans, 128, 0, st>>>(bv, gp, bv.edge_partial_offset, dg);
+    else k_lm_step<PH_CORR><<<n_scans, 128, 0, st>>>(bv, gp, bv.edge_partial_offset);
 }
 void launch_edge_fit(const MapView& medge, const BatchView& bv, const EdgeBuf& eb, uint32_t grid_e, uint32_t n_scans, cudaStream_t st) {
     if (grid_e) k_edge_fit<<<dim3(grid_e, n_scans), kThreads, 0, st>>>(medge, bv, eb, bv.edge_partial_offset);
@@ -1617,12 +1805,14 @@ void launch_correspond(const MapView& m, const BatchView& bv, const CorrBuf& cb,
     launch_match(m, bv, cb, nb, grid_x, n_scans, st);
     launch_first_eval(bv, cb, grid_x, n_scans, st, medge, eb, grid_e);
 }
-void launch_evaluate(const BatchView& bv, const CorrBuf& cb, uint32_t grid_x, uint32_t n_scans, cudaStream_t st, const EdgeBuf* eb, uint32_t grid_e) {
+void launch_evaluate(const BatchView& bv, const CorrBuf& cb, uint32_t grid_x, uint32_t n_scans, cudaStream_t st, const EdgeBuf* eb, uint32_t grid_e,
+                     DegenState* dg) {
     const uint32_t gx = grid_x ? eval_grid(grid_x * kThreads) : 0;
-    if (bv.counters && gx && !grid_e) { k_evaluate_lm<PH_EVAL><<<dim3(gx, n_scans), kThreads, 0, st>>>(bv, cb, bv.counters); return; }
+    if (bv.counters && gx && !grid_e && !dg) { k_evaluate_lm<PH_EVAL><<<dim3(gx, n_scans), kThreads, 0, st>>>(bv, cb, bv.counters); return; }
     if (gx) k_evaluate<PH_EVAL><<<dim3(gx, n_scans), kThreads, 0, st>>>(bv, cb);
     if (grid_e) k_edge_evaluate<<<dim3(grid_e, n_scans), kThreads, 0, st>>>(bv, *eb, bv.edge_partial_offset);
-    k_lm_step<PH_EVAL><<<n_scans, 128, 0, st>>>(bv, gx, bv.edge_partial_offset);
+    if (dg) k_lm_step_deg<PH_EVAL><<<n_scans, 128, 0, st>>>(bv, gx, bv.edge_partial_offset, dg);
+    else k_lm_step<PH_EVAL><<<n_scans, 128, 0, st>>>(bv, gx, bv.edge_partial_offset);
 }
 void launch_loop_cond(const BatchView& bv, uint32_t n_scans, cudaGraphConditionalHandle handle, cudaStream_t st) {
     k_loop_cond<<<1, 32, 0, st>>>(bv.st, n_scans, handle);

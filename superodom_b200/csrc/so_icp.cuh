@@ -84,17 +84,21 @@ void launch_scan_gather(const float4* in, const uint32_t* vals, const uint64_t* 
 void launch_match(const MapView& m, const BatchView& bv, const CorrBuf& cb, const NnBuf& nb, uint32_t grid_x, uint32_t n_scans, cudaStream_t st, int part = 0);
 void launch_inject(const MapView& m, const float4* by_id, uint32_t n_map, const BatchView& bv, const NnBuf& nb, const uint32_t* ids, int n_trace_iters,
                    uint32_t grid_x, uint32_t n_scans, cudaStream_t st);
+// dg: the chunk's DegenState array of a degeneracy-aware registration (k_lm_step_deg in place of k_lm_step, no fused form)
 void launch_first_eval(const BatchView& bv, const CorrBuf& cb, uint32_t grid_x, uint32_t n_scans, cudaStream_t st, const MapView* medge = nullptr,
-                       const EdgeBuf* eb = nullptr, uint32_t grid_e = 0);
+                       const EdgeBuf* eb = nullptr, uint32_t grid_e = 0, DegenState* dg = nullptr);
 // k_edge_fit alone (mode OPTIMIZED: the line correspondences and histogram; its 6-column sums are not read there)
 void launch_edge_fit(const MapView& medge, const BatchView& bv, const EdgeBuf& eb, uint32_t grid_e, uint32_t n_scans, cudaStream_t st);
 void launch_correspond(const MapView& m, const BatchView& bv, const CorrBuf& cb, const NnBuf& nb, uint32_t grid_x, uint32_t n_scans, cudaStream_t st,
                        const MapView* medge = nullptr, const EdgeBuf* eb = nullptr, uint32_t grid_e = 0);
-void launch_evaluate(const BatchView& bv, const CorrBuf& cb, uint32_t grid_x, uint32_t n_scans, cudaStream_t st, const EdgeBuf* eb = nullptr, uint32_t grid_e = 0);
+void launch_evaluate(const BatchView& bv, const CorrBuf& cb, uint32_t grid_x, uint32_t n_scans, cudaStream_t st, const EdgeBuf* eb = nullptr, uint32_t grid_e = 0,
+                     DegenState* dg = nullptr);
 void launch_loop_cond(const BatchView& bv, uint32_t n_scans, cudaGraphConditionalHandle handle, cudaStream_t st);
 void launch_pack_poses(const IcpState* st, uint32_t n_scans, double* rows, cudaStream_t stream);
 // so_covariance: covariance_and_errors_warp on st->H (one scan's state, device memory)
 void launch_covariance(IcpState* st, cudaStream_t stream);
+// so_degeneracy_analysis: the analysis a degeneracy-aware solve begins with, on st->H, into *dg (device memory, thresholds set)
+void launch_degeneracy_analysis(const IcpState* st, DegenState* dg, cudaStream_t stream);
 void launch_query_keys(const MapView& m, const float4* q, size_t nq, uint32_t* keys, uint32_t* vals, cudaStream_t st);
 int launch_knn(const MapView& m, const float4* q, const uint32_t* order, size_t nq, int k, float max_d2, uint32_t* idx, float* d2, cudaStream_t st);
 

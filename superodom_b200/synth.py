@@ -675,13 +675,13 @@ def make_moving_ring_scan(scene: Scene, sensor: str, pose_start: np.ndarray, spe
     return dict(points=rec, pose_true=np.asarray(pose_start, np.float64), pose_prev=pose_at(-dt), pose_next=pose_at(dt), prior=prior)
 
 
-def make_corridor_scene() -> Scene:
+def make_corridor_scene(poles: bool = True) -> Scene:
     """A 400 m x 6 m corridor (x along it, walls at y = +-3, floor -1.8, ceiling 3.2; the end walls at x = +-200 lie beyond the
     130 m range) with free-standing 0.1 m square floor-to-ceiling poles every 4 m, 1 m off each wall.  Pole centres sit at
-    x = 2 + 4i, so no face plane comes within 1 m of the origin."""
+    x = 2 + 4i, so no face plane comes within 1 m of the origin.  poles=False: the bare corridor, which constrains nothing along x."""
     room = np.array([-200.0, 200.0, -3.0, 3.0, -1.8, 3.2])
     boxes = []
-    for cx in np.arange(-198.0, 199.0, 4.0):
+    for cx in np.arange(-198.0, 199.0, 4.0) if poles else ():
         for cy in (-2.0, 2.0):
             boxes.append([cx - 0.05, cx + 0.05, cy - 0.05, cy + 0.05, -1.8, 3.2])
-    return Scene(room=room, boxes=np.array(boxes, np.float64))
+    return Scene(room=room, boxes=np.array(boxes, np.float64).reshape(-1, 6))
