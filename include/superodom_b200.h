@@ -200,6 +200,40 @@ int so_map_counts_5x5(so_ctx* ctx, const int32_t ijk[3], int32_t* n_edge, int32_
  * Writes packed float4 {x,y,z,intensity} in block order then point-id order; *n_out = points available. */
 int so_map_download(so_ctx* ctx, int mode, const int32_t ijk[3], float* out_xyzi, size_t cap_points, size_t* n_out);
 size_t so_map_size(so_ctx* ctx);
+/* ---- block archive: the map beyond the 21x21x11 window ------------------------------------------------------------------------
+ * Off by default; while it is off every call above behaves as LocalMap does and nothing is allocated for it.  With it on, each store
+ * behaves like a LocalMap over an UNBOUNDED block grid that every search sees through the window.  A block is named by its world
+ * block coordinate w = g - origin (g: the grid index LocalMap.h:594-605 gives a point; w does not depend on the origin).
+ *   - Eviction: when an origin change (so_map_shift, so_map_set_origin, the shift inside a single-scan registration) moves a
+ *     non-empty block out of the window, the rebuild that applies it moves the block's cloud to the archive unchanged: the same
+ *     points in the same order.  Non-finite points are still dropped, and so are points more than 2^19 blocks (26 214 km) from the
+ *     world origin.
+ *   - Restore: when an origin change moves an archived block back into the window, its cloud comes back unchanged and leaves the
+ *     archive.  A block's point order is its k-NN tie-break and its voxel-filter order, so registrations against restored blocks
+ *     give what they gave before the blocks left, bit for bit (only so_corr.nn ids, positions in the store, may differ).
+ *   - Loading: so_map_set_points / so_map_set_edge_points replace the window and the archive together; points outside the window go
+ *     to the archive, so setOrigin(start) followed by the prior-map load keeps the whole map.  They accept up to max_map_points +
+ *     cap_points points; SO_ERR_CAPACITY, before any change, when the part inside the window exceeds max_map_points or the rest
+ *     exceeds cap_points.
+ *   - Inserts are unchanged: so_map_add_* and the registered-scan inserts filter the window blocks they touch and drop points
+ *     outside the window.  This is the one place where a store differs from an unbounded map.
+ *   - Every read (registration, k-NN, so_map_counts_5x5, so_map_download, so_map_bounds, global localization) sees the window only.
+ *   - Nothing is lost silently: an eviction the archive has no room for fails the call that applies it with SO_ERR_CAPACITY and
+ *     leaves the store unbuilt, with the rule of so_map_set_points; growing the archive recovers it with nothing lost, turning it off
+ *     recovers it by dropping the blocks.
+ * so_map_archive: turn the archive on with room for cap_points points per store; again with another value to resize it (contents
+ * kept; SO_ERR_CAPACITY when the value is below what a store holds; both stores change or neither); 0 turns it off and frees it
+ * with its contents.
+ * Host cost: with the archive on, so_map_set_points / so_map_set_edge_points classify and stably sort the cloud on the host (a host
+ * copy of the whole cloud, O(n log n)), and so_map_download_all copies the window and the whole pool to the host; both are meant for
+ * one-time loads and saves.  Shifts and origin changes run on the device and cost the blocks that move. */
+int so_map_archive(so_ctx* ctx, size_t cap_points);
+/* Points and blocks held in the archive of store 0 (surf) or 1 (edge), and its capacity; any pointer may be NULL. */
+int so_map_archive_info(so_ctx* ctx, int store, size_t* n_points, size_t* n_blocks, size_t* cap_points);
+/* The whole map of store 0 (surf) or 1 (edge): the window plus the archive as packed float4 {x,y,z,intensity}, ordered by world
+ * block (z, then y, then x) and by the order within the block.  *n_out = points available (only cap_points are written).  Saved and
+ * loaded with so_map_set_points, it is the next session's prior map. */
+int so_map_download_all(so_ctx* ctx, int store, float* out_xyzi, size_t cap_points, size_t* n_out);
 
 /* ---- scan pre-filter (the step right before the path; SURVEY 8f row 2) ------------------------------------------ */
 /* replaces: laserMapping::adjustVoxelSize (src/LaserMapping/laserMapping.cpp:600-651) for the surf cloud: with

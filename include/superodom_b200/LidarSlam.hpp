@@ -174,6 +174,36 @@ public:
     template <class Cloud> Cloud getAllLocalMap() { return download<Cloud>(0, nullptr); }
     template <class Cloud> Cloud get5x5LocalMap(const Vector3i& position) { return download<Cloud>(1, position.v); }
     size_t size() const { return ctx_->h ? so_map_size(ctx_->h) : 0; }
+    // Shim only: the block archive (so_map_archive).  Keeps the blocks the window drops, with room for cap points per store; 0 turns
+    // it off.  In localization mode, call it before setOrigin and the prior-map load so that the whole prior map is kept.
+    void setArchive(size_t cap) {
+        sync_resolution();
+        check(so_map_archive(ctx_->h, cap), "so_map_archive");
+    }
+    // Shim only: load an already voxel-filtered world-frame surf map as the whole map (so_map_set_points), e.g. a map saved with
+    // getWholeMap + writePointCloud.  With the archive on, the blocks outside the window go to the archive instead of being dropped
+    // (addSurfPointCloud, the reference's load, filters the cloud and keeps only the window).
+    template <class Cloud> void loadPriorMap(const Cloud& cloud) {
+        sync_resolution();
+        size_t stride, ioff;
+        point_layout<typename std::decay<decltype(cloud.points[0])>::type>(&stride, &ioff);
+        check(so_map_set_points(ctx_->h, cloud.points.data(), cloud.points.size(), stride, ioff), "so_map_set_points");
+    }
+    // Points held in the archive (surf and edge stores together)
+    size_t archiveSize() const {
+        size_t s = 0, e = 0;
+        if (ctx_->h) { so_map_archive_info(ctx_->h, 0, &s, nullptr, nullptr); so_map_archive_info(ctx_->h, 1, &e, nullptr, nullptr); }
+        return s + e;
+    }
+    // The whole surf map, window plus archive, ordered by world block (so_map_download_all): a session's map as the next one's prior map
+    template <class Cloud> Cloud getWholeMap() {
+        sync_resolution();
+        size_t n = 0;
+        check(so_map_download_all(ctx_->h, 0, nullptr, 0, &n), "so_map_download_all");
+        std::vector<float> buf(4 * (n ? n : 1));
+        check(so_map_download_all(ctx_->h, 0, buf.data(), n, &n), "so_map_download_all");
+        return to_cloud<Cloud>(buf, n);
+    }
 
     void sync_resolution() {
         ctx_->ensure(lineRes_, planeRes_);
@@ -190,6 +220,13 @@ private:
         const size_t cap = so_map_size(ctx_->h);
         std::vector<float> buf(4 * (cap ? cap : 1));
         check(so_map_download(ctx_->h, mode, ijk, buf.data(), cap, &n), "so_map_download");
+        if (n > cap) {                     // a pending origin change restored archived blocks: the window grew in this call
+            buf.assign(4 * n, 0.f);
+            check(so_map_download(ctx_->h, mode, ijk, buf.data(), n, &n), "so_map_download");
+        }
+        return to_cloud<Cloud>(buf, n);
+    }
+    template <class Cloud> static Cloud to_cloud(const std::vector<float>& buf, size_t n) {
         Cloud out;
         out.points.resize(n);
         for (size_t i = 0; i < n; ++i) { auto& p = out.points[i]; p.x = buf[4 * i]; p.y = buf[4 * i + 1]; p.z = buf[4 * i + 2]; p.intensity = buf[4 * i + 3]; }

@@ -183,5 +183,26 @@ inline bool readPointCloud(const std::string& file_path, CloudPtr cloud_out) {
     return true;
 }
 
+// Writes `cloud` (anything with .points, a std::vector of a point holding float x, y, z, intensity) to `file_path` as an
+// unorganised binary PCD v0.7 file of float fields x y z intensity -- what pcl::io::savePCDFileBinary writes for pcl::PointXYZI, and
+// what readPointCloud reads back bit for bit (non-finite points included).  With LocalMap::getWholeMap it saves a session's map as
+// the next session's prior map.  true / false + a message on stderr, never throws.
+template <class Cloud>
+inline bool writePointCloud(const std::string& file_path, const Cloud& cloud) {
+    std::ofstream f(file_path.c_str(), std::ios::binary | std::ios::trunc);
+    if (!f.good()) { std::cerr << "Error: cannot open for writing: " << file_path << std::endl; return false; }
+    const size_t n = cloud.points.size();
+    f << "# .PCD v0.7 - Point Cloud Data file format\nVERSION 0.7\nFIELDS x y z intensity\nSIZE 4 4 4 4\nTYPE F F F F\nCOUNT 1 1 1 1\n"
+      << "WIDTH " << n << "\nHEIGHT 1\nVIEWPOINT 0 0 0 1 0 0 0\nPOINTS " << n << "\nDATA binary\n";
+    std::vector<float> rec(4 * n);
+    for (size_t i = 0; i < n; ++i) {
+        const auto& p = cloud.points[i];
+        rec[4 * i] = p.x; rec[4 * i + 1] = p.y; rec[4 * i + 2] = p.z; rec[4 * i + 3] = p.intensity;
+    }
+    f.write(reinterpret_cast<const char*>(rec.data()), std::streamsize(rec.size() * sizeof(float)));
+    if (!f.good()) { std::cerr << "Error writing PCD file: " << file_path << std::endl; return false; }
+    return true;
+}
+
 }  // namespace b200
 }  // namespace super_odometry

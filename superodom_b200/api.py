@@ -20,6 +20,7 @@ EXPORTS = [
     "so_create", "so_destroy", "so_last_error", "so_device_available", "so_set_stream",
     "so_map_set_resolution", "so_map_set_origin", "so_map_get_origin", "so_map_shift", "so_map_set_points",
     "so_map_set_edge_points", "so_map_add_surf", "so_map_add_edge", "so_map_add_scan", "so_map_add_registered_scan", "so_map_add_registered_edges", "so_map_add_scan_edge", "so_map_counts_5x5", "so_map_download", "so_map_size",
+    "so_map_archive", "so_map_archive_info", "so_map_download_all",
     "so_scan_prefilter", "so_scan_deskew", "so_scan_extract_uniform", "so_scan_extract_edges", "so_register", "so_register_prefiltered", "so_register_injected", "so_set_pose_sink", "so_register_batch", "so_register_batch_edges", "so_register_batch_device",
     "so_register_undistort", "so_register_undistort_edges", "so_register_prefiltered_undistort", "so_register_batch_undistort", "so_undistort_points", "so_register_optimized", "so_register_optimized_edges", "so_register_prefiltered_optimized", "so_register_batch_optimized", "so_evaluate_optimized", "so_evaluate_optimized_edges", "so_correspond", "so_correspond_seeded", "so_ordered_scans", "so_correspond_edge", "so_evaluate", "so_covariance",
     "so_register_degeneracy", "so_register_batch_degeneracy", "so_degeneracy_analysis",
@@ -189,6 +190,9 @@ def load_library():
     L.so_map_download.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
     L.so_map_size.restype = C.c_size_t
     L.so_map_size.argtypes = [C.c_void_p]
+    L.so_map_archive.argtypes = [C.c_void_p, C.c_size_t]
+    L.so_map_archive_info.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.so_map_download_all.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p]
     L.so_scan_prefilter.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_int, C.c_void_p, C.c_void_p,
                                     C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
     L.so_scan_deskew.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_double, C.c_void_p, C.c_void_p, C.c_size_t,
@@ -434,6 +438,33 @@ class Context:
         out = np.zeros((max(cap, 1), 4), np.float32)
         ij = np.ascontiguousarray(ijk if ijk is not None else [0, 0, 0], dtype=np.int32)
         self._chk(self.L.so_map_download(self.h, mode, _p(ij), _p(out), cap, C.byref(n)), "so_map_download")
+        if n.value > cap:                  # a pending origin change restored archived blocks: the window grew in this call
+            cap = n.value
+            out = np.zeros((cap, 4), np.float32)
+            self._chk(self.L.so_map_download(self.h, mode, _p(ij), _p(out), cap, C.byref(n)), "so_map_download")
+        return out[: n.value]
+
+    # ---- block archive (the map beyond the 21 x 21 x 11 window; off by default)
+    def map_archive(self, cap_points: int):
+        """Turn the block archive on with room for cap_points points per store, resize it (contents kept), or 0: off and freed."""
+        self._chk(self.L.so_map_archive(self.h, int(cap_points)), "so_map_archive")
+
+    def map_archive_info(self, store: int = 0):
+        """-> (points, blocks, capacity) of the archive of store 0 (surf) or 1 (edge)."""
+        p, b, c = C.c_size_t(), C.c_size_t(), C.c_size_t()
+        self._chk(self.L.so_map_archive_info(self.h, store, C.byref(p), C.byref(b), C.byref(c)), "so_map_archive_info")
+        return p.value, b.value, c.value
+
+    def map_download_all(self, store: int = 0) -> np.ndarray:
+        """Window plus archive of store 0 (surf) or 1 (edge), ordered by world block (z, y, x), then by the order within the block."""
+        n = C.c_size_t()
+        cap = self.map_size() + self.map_archive_info(store)[0]       # the whole map, unless a pending origin change drops points
+        out = np.zeros((max(cap, 1), 4), np.float32)
+        self._chk(self.L.so_map_download_all(self.h, store, _p(out), cap, C.byref(n)), "so_map_download_all")
+        if n.value > cap:
+            cap = n.value
+            out = np.zeros((cap, 4), np.float32)
+            self._chk(self.L.so_map_download_all(self.h, store, _p(out), cap, C.byref(n)), "so_map_download_all")
         return out[: n.value]
 
     # ---- scan pre-filter

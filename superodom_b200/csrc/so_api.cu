@@ -935,8 +935,15 @@ int so_map_shift(so_ctx* ctx, const double t[3], int32_t out_ijk[3]) {
 
 static int store_set_points(Ctx* c, MapStore& ms, const void* xyzi, size_t n, size_t stride, size_t ioff) {
     if (!c || (!xyzi && n) || stride < 12) return fail(SO_ERR_ARG, "bad args");
-    if (n > c->cfg.max_map_points) return fail(SO_ERR_CAPACITY, "map larger than so_config.max_map_points");
+    if (n > c->cfg.max_map_points + ms.arc.cap) return fail(SO_ERR_CAPACITY, "map larger than so_config.max_map_points (plus the block archive)");
     SO_CUDA_TRY(cudaSetDevice(c->device));
+    if (ms.arc.cap) {                                        // window and archive replaced together; the checks come before any change
+        std::vector<float4> pts(n);
+        const unsigned char* p = static_cast<const unsigned char*>(xyzi);
+        for (size_t i = 0; i < n; ++i) pts[i] = read_point(p + i * stride, stride, ioff);
+        int rc = archive_load(c, ms, pts.data(), n);
+        return rc ? rc : map_rebuild(c, ms);
+    }
     int rc = upload_cloud(c, xyzi, n, stride, ioff, ms.d_xyzi);
     if (rc) return rc;
     ms.n = uint32_t(n);
@@ -964,6 +971,8 @@ static int store_add(Ctx* c, MapStore& ms, const void* xyzi, size_t n, size_t st
     if (n == 0) return SO_OK;
     int rc = SO_OK;
     if (ms.dirty) { rc = map_rebuild(c, ms); if (rc) return rc; }           // pending origin / resolution change first: it may compact the cloud
+    // ... or, with the block archive on, grow it by the blocks it restores: the new points must still fit behind it
+    if (size_t(ms.n) + n > c->cfg.max_map_points) return fail(SO_ERR_CAPACITY, "map + new points exceed so_config.max_map_points");
     rc = xyzi ? upload_cloud(c, xyzi, n, stride, ioff, ms.d_xyzi + ms.n) : put_registered_scan(c, ms, pose);
     if (rc) return rc;
     if (pose) { rc = map_transform_tail(c, ms, uint32_t(n), pose); if (rc) return rc; }
@@ -1027,6 +1036,31 @@ int so_map_counts_5x5(so_ctx* ctx, const int32_t ijk[3], int32_t* n_edge, int32_
 }
 
 size_t so_map_size(so_ctx* ctx) { Ctx* c = reinterpret_cast<Ctx*>(ctx); return c ? size_t(c->surf.n) + size_t(c->edge.n) : 0; }
+
+int so_map_archive(so_ctx* ctx, size_t cap_points) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c) return fail(SO_ERR_ARG, "null ctx");
+    SO_CUDA_TRY(cudaSetDevice(c->device));
+    return archive_set_cap(c, cap_points);
+}
+
+int so_map_archive_info(so_ctx* ctx, int store, size_t* n_points, size_t* n_blocks, size_t* cap_points) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c || (store != 0 && store != 1)) return fail(SO_ERR_ARG, "bad args");
+    const BlockArchive& a = (store ? c->edge : c->surf).arc;
+    if (n_points) *n_points = a.live;
+    if (n_blocks) *n_blocks = a.dir.size();
+    if (cap_points) *cap_points = a.cap;
+    return SO_OK;
+}
+
+int so_map_download_all(so_ctx* ctx, int store, float* out, size_t cap, size_t* n_out) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c || !n_out || (store != 0 && store != 1)) return fail(SO_ERR_ARG, "bad args");
+    SO_CUDA_TRY(cudaSetDevice(c->device));
+    { int rc = ensure_maps(c); if (rc) return rc; }
+    return archive_download_all(c, store ? c->edge : c->surf, out, cap, n_out);
+}
 
 int so_map_download(so_ctx* ctx, int mode, const int32_t ijk[3], float* out, size_t cap, size_t* n_out) {
     Ctx* c = reinterpret_cast<Ctx*>(ctx);

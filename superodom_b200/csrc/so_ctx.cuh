@@ -1,6 +1,7 @@
 // so_ctx.cuh -- the context behind the C ABI: owns every device buffer, the stream, CUDA graphs and host mirrors.
 #pragma once
 #include <cstring>
+#include <map>
 #include <string>
 #include <type_traits>
 #include <vector>
@@ -109,6 +110,18 @@ struct RegisterRequest {
     so_motion_result* motion_results = nullptr;    // OPTIMIZED, optional: [n_scans] results with the motion
 };
 
+// Block archive of one store (so_map_archive; so_archive.h): the clouds of blocks the window dropped, each kept as one segment of a
+// point pool in its in-block order, found through a directory sorted by world key.  cap == 0: off, nothing allocated.
+struct GatherSeg { uint64_t src, dst; uint32_t n, pad; };      // one block cloud copied src[0..n) -> dst[0..n) (k_seg_gather)
+struct BlockArchive {
+    struct Seg { uint64_t off; uint32_t n; };
+    size_t cap = 0;                                // points the pool holds
+    float4* d_pool = nullptr;                      // [cap]: segments in [0, used), holes where blocks were restored
+    size_t used = 0, live = 0;                     // pool tail; points in live segments
+    std::map<uint64_t, Seg> dir;                   // world key -> segment, key order (host: every origin change goes through the host)
+    GatherSeg* d_segs = nullptr; size_t segs_cap = 0;   // segment lists of the gathers
+};
+
 // One per-block cloud family of the LocalMap (surf or edge): points in id order, the sorted hash grid, block tables.
 struct MapStore {
     float res = 0.4f;                              // planeRes_ (surf) / lineRes_ (edge): voxel leaf and gate / search radius
@@ -123,6 +136,7 @@ struct MapStore {
     int n_slots = 0;
     int nb = 64;                                   // cells per block axis
     bool dirty = true;                             // the index is not built for the current cloud, origin and resolution
+    BlockArchive arc;
 };
 
 struct Ctx {
@@ -374,6 +388,11 @@ struct DeskewParams {
 void launch_deskew(float4* pts, uint32_t n, const DeskewParams& P, cudaStream_t st);
 int scan_extract_uniform(Ctx* c, uint32_t n, uint32_t skip, float block_range, int int_abs, uint32_t* n_out);   // d_scan -> d_scan_sorted   // d_scan -> d_scan_sorted (VoxelGrid on a scan)
 int map_rebuild(Ctx* c, MapStore& ms);    // (re)bin, drop off-grid points, index; the store stays dirty when it fails
+// Block archive (so_map.cu): off-window points go to the archive and archived blocks the window reaches come back inside map_rebuild
+int archive_set_cap(Ctx* c, size_t cap);                  // both stores: on / resize (contents kept) / 0: off and freed; all or nothing
+// so_map_set_points with the archive on: pts[0..n) (finite, host) -> window part in d_xyzi, the rest in the archive; no rebuild
+int archive_load(Ctx* c, MapStore& ms, const float4* pts, size_t n);
+int archive_download_all(Ctx* c, MapStore& ms, float* out, size_t cap, size_t* n_out);   // window + archive by world key
 MapView map_view(const Ctx* c, const MapStore& ms);
 int map_cells_per_block(float plane_res);
 int scan_sort_alloc(Ctx* c);             // temp storage for the per-registration scan sort

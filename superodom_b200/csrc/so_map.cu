@@ -10,9 +10,11 @@
 // off-grid points; filter_stage) and one index stage (block counts, slots, cell table; count_blocks + index_cells).
 #include <algorithm>
 #include <cmath>
+#include <set>
 
 #include <cub/cub.cuh>
 
+#include "so_archive.h"
 #include "so_ctx.cuh"
 #include "so_knn.cuh"
 
@@ -50,6 +52,7 @@ struct InsertInfo {
 struct MapScratch {
     InsertInfo info;
     uint8_t touched[kNumBlocks];                                     // blocks the new points of an insert reach
+    uint32_t runs;                                                   // eviction: blocks (and the dropped run) of the off-window points
 };
 
 constexpr size_t kMaxCells = size_t(1) << 31;      // cell indices are 32-bit in the kernels and the scan length is an int
@@ -107,6 +110,7 @@ int map_alloc(Ctx* c) {
 void map_free(Ctx* c) {
     for (MapStore* ms : {&c->surf, &c->edge}) {
         cudaFree(ms->d_xyzi); cudaFree(ms->d_sorted); cudaFree(ms->d_block_slot); cudaFree(ms->d_block_count); cudaFree(ms->d_cell_start);
+        cudaFree(ms->arc.d_pool); cudaFree(ms->arc.d_segs);
     }
     cudaFree(c->d_keys); cudaFree(c->d_keys_out); cudaFree(c->d_vals); cudaFree(c->d_vals_out); cudaFree(c->d_cub_tmp);
     cudaFree(c->d_map_scratch);
@@ -443,22 +447,29 @@ static int index_cells(Ctx* c, MapStore& ms, uint32_t n_max, uint32_t slot_cap) 
     return SO_OK;
 }
 
+static int map_rebuild_archive(Ctx* c, MapStore& ms);
+
+static int set_empty_index(Ctx* c, MapStore& ms) {
+    cudaStream_t st = c->stream;
+    SO_CUDA_TRY(cudaMemsetAsync(ms.d_block_count, 0, kNumBlocks * sizeof(int32_t), st));
+    SO_CUDA_TRY(cudaMemsetAsync(ms.d_block_slot, 0xFF, kNumBlocks * sizeof(int32_t), st));
+    SO_CUDA_TRY(cudaStreamSynchronize(st));
+    std::fill(ms.h_block_count.begin(), ms.h_block_count.end(), 0);
+    std::fill(ms.h_block_slot.begin(), ms.h_block_slot.end(), -1);
+    ms.n_slots = 0;
+    ms.dirty = false;
+    return SO_OK;
+}
+
 // (Re)build the index of d_xyzi[0..n) under the current origin and resolution: count blocks and assign slots over the raw cloud,
-// size the cell table, drop off-grid points (filter stage, nothing touched) when there are any, index.
+// size the cell table, drop off-grid points (filter stage, nothing touched) when there are any, index.  With the block archive on,
+// off-grid points move to the archive and archived blocks the grid covers come back instead (map_rebuild_archive).
 int map_rebuild(Ctx* c, MapStore& ms) {
     cudaStream_t st = c->stream;
     ms.nb = map_cells_per_block(ms.res);
     ms.dirty = true;
-    if (ms.n == 0) {
-        SO_CUDA_TRY(cudaMemsetAsync(ms.d_block_count, 0, kNumBlocks * sizeof(int32_t), st));
-        SO_CUDA_TRY(cudaMemsetAsync(ms.d_block_slot, 0xFF, kNumBlocks * sizeof(int32_t), st));
-        SO_CUDA_TRY(cudaStreamSynchronize(st));
-        std::fill(ms.h_block_count.begin(), ms.h_block_count.end(), 0);
-        std::fill(ms.h_block_slot.begin(), ms.h_block_slot.end(), -1);
-        ms.n_slots = 0;
-        ms.dirty = false;
-        return SO_OK;
-    }
+    if (ms.arc.cap) return map_rebuild_archive(c, ms);
+    if (ms.n == 0) return set_empty_index(c, ms);
     const uint32_t n = ms.n;
     InsertInfo* h_info = c->h_map_info;
     *h_info = InsertInfo{};
@@ -496,6 +507,273 @@ int map_add_points(Ctx* c, MapStore& ms, uint32_t n_new) {
     rc = reserve_cells(c, ms, n_slots, 4);
     if (!rc) rc = count_blocks(c, ms, total, n_slots);
     return rc ? rc : index_cells(c, ms, total, n_slots);
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// Block archive (so_archive.h): with it on, the rebuild that applies an origin change moves every block the window drops to the
+// archive, unchanged, and brings back every archived block the window now covers.  Per store: one float4 point pool holding one
+// segment per block (its cloud in store order) and a host directory {world key -> segment} in key order.  Evicted segments are
+// appended at the pool's tail; restored ones leave a hole, and the pool is compacted (stably, in pool order) only when an eviction
+// does not fit behind the tail -- so a shift costs the blocks that move, not the size of the archive.
+// ------------------------------------------------------------------------------------------------------------------
+constexpr int kEvictShift = 60;                   // eviction key: class above the 60-bit world key
+static_assert(archive::kWinW == kW && archive::kWinH == kH && archive::kWinD == kD, "the archive's window is the block grid");
+static_assert(3 * archive::kKeyBits <= kEvictShift, "world key fits below the class bits");
+
+// Eviction key of every point of the store's cloud under the new origin: 0 in the window (kept in place by the stable sort);
+// [1][world key] off the window (to the archive: grouped by block, cloud order inside each); [2] not finite or beyond the key
+// range (dropped, as the filter stage drops them)
+__global__ void k_evict_keys(const float4* __restrict__ raw, uint32_t n, int3 origin, uint64_t* __restrict__ keys, uint32_t* __restrict__ vals) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const float4 p = raw[i];
+    uint64_t key = 0;
+    if (grid_block(p, origin) < 0) {
+        const uint64_t w = archive::point_key(p.x, p.y, p.z);
+        key = w == archive::kKeyNone ? uint64_t(2) << kEvictShift : (uint64_t(1) << kEvictShift) | w;
+    }
+    keys[i] = key;
+    vals[i] = i;
+}
+
+// sorted positions [0, n_kept): the window's points, in order -> window; [n_kept, n_kept + n_evict): the evicted blocks -> pool tail
+__global__ void k_evict_gather(const float4* __restrict__ raw, const uint32_t* __restrict__ vals, uint32_t n_kept, uint32_t n_evict,
+                               float4* __restrict__ window, float4* __restrict__ pool_tail) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n_kept) window[i] = raw[vals[i]];
+    else if (i < n_kept + n_evict) pool_tail[i - n_kept] = raw[vals[i]];
+}
+
+// one CTA per block cloud: src[s.src .. +s.n) -> dst[s.dst .. +s.n)
+__global__ void k_seg_gather(const float4* __restrict__ src, float4* __restrict__ dst, const GatherSeg* __restrict__ segs) {
+    const GatherSeg s = segs[blockIdx.x];
+    for (uint32_t j = threadIdx.x; j < s.n; j += blockDim.x) dst[s.dst + j] = src[s.src + j];
+}
+
+static int seg_gather(Ctx* c, BlockArchive& a, const std::vector<GatherSeg>& segs, const float4* src, float4* dst) {
+    if (segs.empty()) return SO_OK;
+    int rc = grow_buffer(a.d_segs, a.segs_cap, segs.size());
+    if (rc) return rc;
+    SO_CUDA_TRY(cudaMemcpyAsync(a.d_segs, segs.data(), segs.size() * sizeof(GatherSeg), cudaMemcpyHostToDevice, c->stream));
+    k_seg_gather<<<unsigned(segs.size()), 256, 0, c->stream>>>(src, dst, a.d_segs);
+    c->launches++;
+    return SO_OK;
+}
+
+// Every live segment but those in `skip`, in pool order, packed from the front of dst.  The directory is not touched: the segments'
+// new offsets go to *moved, for the caller to apply once everything it depends on has succeeded.  Returns the points packed.
+using SegMoves = std::vector<std::pair<BlockArchive::Seg*, uint64_t>>;
+static void apply_moves(const SegMoves& m) { for (const auto& x : m) x.first->off = x.second; }
+static int repack(Ctx* c, BlockArchive& a, float4* dst, size_t* packed, SegMoves* moved, const std::set<const BlockArchive::Seg*>& skip = {}) {
+    std::vector<BlockArchive::Seg*> order;
+    order.reserve(a.dir.size());
+    for (auto& kv : a.dir) if (!skip.count(&kv.second)) order.push_back(&kv.second);
+    std::sort(order.begin(), order.end(), [](const BlockArchive::Seg* x, const BlockArchive::Seg* y) { return x->off < y->off; });
+    std::vector<GatherSeg> segs;
+    segs.reserve(order.size());
+    uint64_t o = 0;
+    for (const BlockArchive::Seg* s : order) { segs.push_back(GatherSeg{s->off, o, s->n, 0}); o += s->n; }
+    int rc = seg_gather(c, a, segs, a.d_pool, dst);
+    if (rc) return rc;
+    moved->clear();
+    for (size_t k = 0; k < order.size(); ++k) moved->emplace_back(order[k], segs[k].dst);
+    *packed = size_t(o);
+    return SO_OK;
+}
+
+// Both stores at once: every new pool is allocated before either store changes, so a failure leaves both as they were
+int archive_set_cap(Ctx* c, size_t cap) {
+    MapStore* stores[2] = {&c->surf, &c->edge};
+    SO_CUDA_TRY(cudaStreamSynchronize(c->stream));
+    if (cap == 0) {
+        for (MapStore* ms : stores) { cudaFree(ms->arc.d_pool); cudaFree(ms->arc.d_segs); ms->arc = BlockArchive{}; }
+        return SO_OK;
+    }
+    for (MapStore* ms : stores)
+        if (cap < ms->arc.live) { set_error("so_map_archive: capacity below the points the archive holds"); return SO_ERR_CAPACITY; }
+    float4* pool[2] = {nullptr, nullptr};
+    for (int k = 0; k < 2; ++k) {
+        if (cap == stores[k]->arc.cap) continue;
+        if (cudaMalloc(&pool[k], cap * sizeof(float4)) != cudaSuccess) {
+            cudaGetLastError();
+            cudaFree(pool[0]);
+            set_error("so_map_archive: cudaMalloc of the archive pool failed");
+            return SO_ERR_CUDA;
+        }
+    }
+    size_t packed[2] = {0, 0};
+    SegMoves moved[2];
+    int rc = SO_OK;
+    for (int k = 0; k < 2 && !rc; ++k) if (pool[k]) rc = repack(c, stores[k]->arc, pool[k], &packed[k], &moved[k]);
+    if (!rc && cudaStreamSynchronize(c->stream) != cudaSuccess) rc = SO_ERR_CUDA;
+    if (rc) { cudaFree(pool[0]); cudaFree(pool[1]); return rc; }          // both directories as they were
+    for (int k = 0; k < 2; ++k) {
+        if (!pool[k]) continue;
+        BlockArchive& a = stores[k]->arc;
+        apply_moves(moved[k]);
+        cudaFree(a.d_pool);
+        a.d_pool = pool[k]; a.cap = cap; a.used = packed[k];
+    }
+    return SO_OK;
+}
+
+int archive_load(Ctx* c, MapStore& ms, const float4* pts, size_t n) {
+    BlockArchive& a = ms.arc;
+    std::vector<float4> win;
+    std::vector<std::pair<uint64_t, uint32_t>> off;                  // (world key, index) of the points outside the window
+    for (size_t i = 0; i < n; ++i) {
+        const uint64_t key = archive::point_key(pts[i].x, pts[i].y, pts[i].z);
+        if (key == archive::kKeyNone) continue;                         // not finite: dropped, as the rebuild drops it
+        int w[3];
+        archive::unpack_key(key, w);
+        if (archive::in_window(w, c->origin)) win.push_back(pts[i]);
+        else off.emplace_back(key, uint32_t(i));
+    }
+    if (win.size() > c->cfg.max_map_points) { set_error("map points inside the window exceed so_config.max_map_points"); return SO_ERR_CAPACITY; }
+    if (off.size() > a.cap) { set_error("map points outside the window exceed the block archive (so_map_archive)"); return SO_ERR_CAPACITY; }
+    std::stable_sort(off.begin(), off.end(), [](const auto& x, const auto& y) { return x.first < y.first; });
+    std::vector<float4> arc(off.size());
+    for (size_t i = 0; i < off.size(); ++i) arc[i] = pts[off[i].second];
+    SO_CUDA_TRY(cudaStreamSynchronize(c->stream));
+    if (!win.empty()) SO_CUDA_TRY(cudaMemcpy(ms.d_xyzi, win.data(), win.size() * sizeof(float4), cudaMemcpyHostToDevice));
+    if (!arc.empty()) SO_CUDA_TRY(cudaMemcpy(a.d_pool, arc.data(), arc.size() * sizeof(float4), cudaMemcpyHostToDevice));
+    a.dir.clear();
+    for (size_t i = 0; i < off.size();) {
+        size_t j = i;
+        while (j < off.size() && off[j].first == off[i].first) ++j;
+        a.dir[off[i].first] = BlockArchive::Seg{uint64_t(i), uint32_t(j - i)};
+        i = j;
+    }
+    a.used = a.live = off.size();
+    ms.n = uint32_t(win.size());
+    ms.dirty = true;
+    return SO_OK;
+}
+
+int archive_download_all(Ctx* c, MapStore& ms, float* out, size_t cap, size_t* n_out) {
+    const BlockArchive& a = ms.arc;
+    std::vector<float4> win(ms.n), pool(a.used);
+    if (ms.n) SO_CUDA_TRY(cudaMemcpy(win.data(), ms.d_xyzi, size_t(ms.n) * sizeof(float4), cudaMemcpyDeviceToHost));
+    if (a.used) SO_CUDA_TRY(cudaMemcpy(pool.data(), a.d_pool, a.used * sizeof(float4), cudaMemcpyDeviceToHost));
+    std::vector<std::pair<uint64_t, uint32_t>> wk(win.size());
+    for (size_t i = 0; i < win.size(); ++i) wk[i] = {archive::point_key(win[i].x, win[i].y, win[i].z), uint32_t(i)};
+    std::stable_sort(wk.begin(), wk.end(), [](const auto& x, const auto& y) { return x.first < y.first; });
+    size_t k = 0, i = 0;
+    auto put = [&](const float4& p) { if (out && k < cap) std::memcpy(out + 4 * k, &p, sizeof(float4)); ++k; };
+    for (auto it = a.dir.begin(); it != a.dir.end() || i < wk.size();) {        // window and archive hold different blocks
+        if (it == a.dir.end() || (i < wk.size() && wk[i].first < it->first)) { put(win[wk[i].second]); ++i; }
+        else { for (uint32_t j = 0; j < it->second.n; ++j) put(pool[it->second.off + j]); ++it; }
+    }
+    *n_out = k;
+    return SO_OK;
+}
+
+static int map_rebuild_archive(Ctx* c, MapStore& ms) {
+    cudaStream_t st = c->stream;
+    BlockArchive& a = ms.arc;
+    InsertInfo* d_info = &c->d_map_scratch->info;
+    InsertInfo* h_info = c->h_map_info;
+    const int3 origin = make_int3(c->origin[0], c->origin[1], c->origin[2]);
+    // blocks to restore: the directory's entries inside the window, one lookup per row of blocks
+    std::vector<std::map<uint64_t, BlockArchive::Seg>::iterator> back;
+    size_t n_back = 0;
+    archive::window_rows(c->origin, [&](uint64_t lo, uint64_t hi) {
+        for (auto it = a.dir.lower_bound(lo); it != a.dir.end() && it->first <= hi; ++it) { back.push_back(it); n_back += it->second.n; }
+    });
+    // points of the store that stay: block counts and slots of the cloud under the new origin (one read-back, as map_rebuild)
+    const uint32_t n = ms.n;
+    uint32_t n_kept = 0, n_slots = 0;
+    if (n) {
+        *h_info = InsertInfo{};
+        h_info->n_out = n;
+        SO_CUDA_TRY(cudaMemcpyAsync(d_info, h_info, sizeof(InsertInfo), cudaMemcpyHostToDevice, st));
+        int rc = count_blocks(c, ms, n, kNumBlocks);
+        if (rc) return rc;
+        SO_CUDA_TRY(cudaMemcpyAsync(h_info, d_info, sizeof(InsertInfo), cudaMemcpyDeviceToHost, st));
+        SO_CUDA_TRY(cudaGetLastError());
+        SO_CUDA_TRY(cudaStreamSynchronize(st));
+        n_kept = h_info->n_kept; n_slots = h_info->n_slots;
+    }
+    // points that leave: sorted by (class, world key), stable, and the runs of that order (one per block, one for the dropped)
+    std::vector<uint64_t> run_key;
+    std::vector<uint32_t> run_n;
+    size_t n_evict = 0;
+    if (n_kept < n) {
+        const uint32_t m = n - n_kept;
+        uint32_t* d_runs = &c->d_map_scratch->runs;
+        size_t need = 0;
+        cub::DeviceRunLengthEncode::Encode(nullptr, need, c->d_keys_out, c->d_keys, c->d_vals, d_runs, int(m));
+        int rc = grow_buffer(c->d_cub_tmp, c->cub_tmp_bytes, need + 256);
+        if (rc) return rc;
+        k_evict_keys<<<(n + 255) / 256, 256, 0, st>>>(ms.d_xyzi, n, origin, c->d_keys, c->d_vals);
+        size_t tmp = c->cub_tmp_bytes;
+        SO_CUDA_TRY(cub::DeviceRadixSort::SortPairs(c->d_cub_tmp, tmp, c->d_keys, c->d_keys_out, c->d_vals, c->d_vals_out, int(n), 0,
+                                                    kEvictShift + 2, st));
+        tmp = c->cub_tmp_bytes;           // run keys and counts into the sort's inputs, free now
+        SO_CUDA_TRY(cub::DeviceRunLengthEncode::Encode(c->d_cub_tmp, tmp, c->d_keys_out + n_kept, c->d_keys, c->d_vals, d_runs, int(m), st));
+        uint32_t runs = 0;
+        SO_CUDA_TRY(cudaMemcpyAsync(&h_info->pad, d_runs, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+        SO_CUDA_TRY(cudaGetLastError());
+        SO_CUDA_TRY(cudaStreamSynchronize(st));
+        runs = h_info->pad;
+        run_key.resize(runs); run_n.resize(runs);
+        SO_CUDA_TRY(cudaMemcpyAsync(run_key.data(), c->d_keys, runs * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+        SO_CUDA_TRY(cudaMemcpyAsync(run_n.data(), c->d_vals, runs * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+        SO_CUDA_TRY(cudaStreamSynchronize(st));
+        c->launches += 1 + 5 + 3;
+        for (uint32_t r = 0; r < runs; ++r) if ((run_key[r] >> kEvictShift) == 1) n_evict += run_n[r];
+    }
+    // every check before the first change: the store stays as it was (and unbuilt) when one fails
+    if (size_t(n_kept) + n_back > c->cfg.max_map_points) {
+        set_error("restoring archived blocks would exceed so_config.max_map_points");
+        return SO_ERR_CAPACITY;
+    }
+    if (a.live - n_back + n_evict > a.cap) { set_error("block archive full: grow it with so_map_archive"); return SO_ERR_CAPACITY; }
+    n_slots += uint32_t(back.size());                                   // restored blocks are not in the window's cloud
+    if (n_kept + n_back) { int rc = reserve_cells(c, ms, n_slots, n_slots / 4); if (rc) return rc; }
+    const bool compact = a.used + n_evict > a.cap;
+    float4* scratch = nullptr;
+    if (compact) SO_CUDA_TRY(cudaMalloc(&scratch, std::max<size_t>(a.live - n_back, 1) * sizeof(float4)));
+    // restore: the blocks' clouds behind the window's points, then out of the directory
+    float4* dst = n_kept < n ? ms.d_sorted : ms.d_xyzi;
+    std::vector<GatherSeg> segs;
+    uint64_t at = n_kept;
+    for (const auto& it : back) { segs.push_back(GatherSeg{it->second.off, at, it->second.n, 0}); at += it->second.n; }
+    int rc = seg_gather(c, a, segs, a.d_pool, dst);
+    size_t packed = 0;
+    SegMoves moved;
+    if (!rc && compact) {                                               // the other segments, stably, through the scratch
+        std::set<const BlockArchive::Seg*> skip;
+        for (const auto& it : back) skip.insert(&it->second);
+        rc = repack(c, a, scratch, &packed, &moved, skip);
+        if (!rc && packed && cudaMemcpyAsync(a.d_pool, scratch, packed * sizeof(float4), cudaMemcpyDeviceToDevice, st) != cudaSuccess) rc = SO_ERR_CUDA;
+        if (!rc && cudaStreamSynchronize(st) != cudaSuccess) rc = SO_ERR_CUDA;
+    }
+    cudaFree(scratch);
+    if (rc) return rc;            // the directory and the store still describe what they held: nothing restored, nothing lost
+    if (compact) { apply_moves(moved); a.used = packed; }
+    for (const auto& it : back) a.dir.erase(it);
+    a.live -= n_back;
+    // evict: the window's points to the front of dst, the leaving blocks behind the pool's tail
+    if (n_kept < n) {
+        const uint32_t total = n_kept + uint32_t(n_evict);
+        if (total) k_evict_gather<<<(total + 255) / 256, 256, 0, st>>>(ms.d_xyzi, c->d_vals_out, n_kept, uint32_t(n_evict), ms.d_sorted, a.d_pool + a.used);
+        c->launches++;
+        for (size_t r = 0; r < run_key.size(); ++r) {
+            if ((run_key[r] >> kEvictShift) != 1) continue;
+            a.dir[run_key[r] & ((uint64_t(1) << kEvictShift) - 1)] = BlockArchive::Seg{uint64_t(a.used), run_n[r]};
+            a.used += run_n[r];
+        }
+        a.live += n_evict;
+        std::swap(ms.d_xyzi, ms.d_sorted);
+    }
+    ms.n = n_kept + uint32_t(n_back);
+    if (ms.n == 0) return set_empty_index(c, ms);
+    *h_info = InsertInfo{};
+    h_info->n_out = ms.n;
+    SO_CUDA_TRY(cudaMemcpyAsync(d_info, h_info, sizeof(InsertInfo), cudaMemcpyHostToDevice, st));
+    rc = count_blocks(c, ms, ms.n, n_slots);
+    return rc ? rc : index_cells(c, ms, ms.n, n_slots);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
