@@ -217,7 +217,8 @@ size_t so_map_size(so_ctx* ctx);
  *     exceeds cap_points.
  *   - Inserts are unchanged: so_map_add_* and the registered-scan inserts filter the window blocks they touch and drop points
  *     outside the window.  This is the one place where a store differs from an unbounded map.
- *   - Every read (registration, k-NN, so_map_counts_5x5, so_map_download, so_map_bounds, global localization) sees the window only.
+ *   - Every read (registration, k-NN, so_map_counts_5x5, so_map_download, so_map_bounds) sees the window only.  Global localization
+ *     sees the window only unless so_global_opts.whole_map is 1; so_map_bounds_all covers the window and the archive.
  *   - Nothing is lost silently: an eviction the archive has no room for fails the call that applies it with SO_ERR_CAPACITY and
  *     leaves the store unbuilt, with the rule of so_map_set_points; growing the archive recovers it with nothing lost, turning it off
  *     recovers it by dropping the blocks.
@@ -528,7 +529,7 @@ typedef struct {
     int32_t score_points;           /* scan points scored (shouldProcessPoint decimation), default 1024, at most 4096 */
     int32_t dilate;                 /* bitmap dilation (voxels, cube neighbourhood), default 1, at most 8 */
     int32_t k;                      /* candidates refined, default 16, at most 64 */
-    int32_t pad_;
+    int32_t whole_map;              /* 0: search and refine in the window; 1: the window plus the surf archive (see below); else SO_ERR_ARG */
     double nms_xy;                  /* suppression radius in x/y (m), default 1.0 */
     double nms_yaw;                 /* suppression half-width in yaw (rad), default 10 deg */
 } so_global_opts;
@@ -552,7 +553,7 @@ typedef struct {
     int32_t best_score;     /* score of the best hypothesis */
     uint64_t n_hypotheses;  /* NX * NY * NZ * NYAW */
     int32_t n_score_points; /* scan points scored */
-    int32_t pad_;
+    int32_t n_windows;      /* whole_map = 1 with the archive on: distinct windows the candidates were registered in; else 0 */
     double time_raster_ms, time_dilate_ms, time_score_ms, time_sort_ms;  /* device time of each search stage (CUDA events) */
     double time_refine_ms;  /* candidate read-back, suppression and registrations (host clock) */
     double time_total_ms;   /* whole call (host clock) */
@@ -615,6 +616,27 @@ int so_localize_bnb_bounds(so_ctx* ctx, const void* xyzi, size_t n, size_t strid
                            const so_global_opts* gopts, int level, uint16_t* out, size_t cap, int32_t dims[4]);
 /* Bounding box of the surf map, reduced on the device; *n = its point count (lo and hi are zero for an empty map). */
 int so_map_bounds(so_ctx* ctx, float lo[3], float hi[3], size_t* n);
+/* The same over the surf window plus the surf archive (so_map_archive), read in place on the device; with the archive off it equals
+ * so_map_bounds. */
+int so_map_bounds_all(so_ctx* ctx, float lo[3], float hi[3], size_t* n);
+
+/* ---- global localization over the whole archived map (so_global_opts.whole_map = 1) ----------------------------------------------
+ * Accepted by so_localize_global, so_localize_global_bnb, so_localize_scores, so_localize_bnb_keys and so_localize_bnb_bounds.  With
+ * the archive off the call is the whole_map = 0 call, bit for bit (n_windows = 0, the window does not move).  With it on:
+ *   - Any pending origin change is applied first; call that origin O0.
+ *   - Search: the occupancy bitmap (level 0 of the pyramid) is rastered from the window's points and every point of the archive's
+ *     live segments, read in place.  The raster ORs bits and the bounds reduce with min / max, so the scores are a function of the
+ *     whole map's point set only; the branch-and-bound clips its window with so_map_bounds_all's box.  Everything after the raster is
+ *     unchanged.
+ *   - Refinement: O(c) is the origin so_map_shift(c.prior) would leave when called at O0.  The candidates are grouped by O(c), the
+ *     groups ordered by their best-ranked member; for each group the window moves to O(c) (the archive evicts and restores blocks)
+ *     and the group registers in rank order, max_batch at a time.  Each candidate's registration equals so_map_shift(prior) followed
+ *     by so_register_batch(scan, prior) on the same map at O0, bit for bit.  The winner rule is unchanged.
+ *   - On return the origin is O(winner), with the window built there, so so_map_add_registered_scan(pose) inserts where the robot
+ *     is; with no winner it is O0 again.  Both stores move together (the origin is shared).  A move the archive has no room for fails
+ *     the call with SO_ERR_CAPACITY under the archive's rule (the store is left unbuilt; growing the archive recovers it).
+ * The limits are unchanged: 2^32 hypotheses, 2^32 bits per pyramid level, the 1 GiB offset table.  A strip 2 km x 100 m at 0.25 m and
+ * 2 deg (about 5.8e8 hypotheses) fits; a 1.5 km x 1.5 km square needs a coarser res or yaw_step. */
 
 /* ---- instrumentation ------------------------------------------------------------------------------ */
 /* Number of this library's kernels launched since the last reset (bench.py gpu_launches). */

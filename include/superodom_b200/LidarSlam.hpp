@@ -453,30 +453,16 @@ public:
     so_bnb_stats last_bnb{};
     template <class CloudPtr>
     int globalLocalizeInMap(const CloudPtr& planner_point, const Transformd& centre, so_global_opts opts) {
-        localMap.sync_resolution();
-        size_t stride, ioff;
-        using PointT = typename std::decay<decltype(planner_point->points[0])>::type;
-        point_layout<PointT>(&stride, &ioff);
-        so_icp_opts o{};
-        o.max_icp_iters = int32_t(LocalizationICPMaxIter);
-        o.max_surface_features = OptSet.max_surface_features;
-        o.lm_max_iterations = 4;
-        o.yaw_ratio = OptSet.yaw_ratio;
-        double c[7];
-        centre.to_pose7(c);
-        float lo[3], hi[3];
-        size_t n_map = 0;
-        check(so_map_bounds(context.h, lo, hi, &n_map), "so_map_bounds");
-        auto half = [](double l, double h, double x) { const double a = h - x, b = x - l; return a > b ? (a > 0.0 ? a : 0.0) : (b > 0.0 ? b : 0.0); };
-        opts.half_x = half(lo[0], hi[0], c[0]);
-        opts.half_y = half(lo[1], hi[1], c[1]);
-        const void* surf = planner_point->size() ? planner_point->points.data() : nullptr;
-        const int rc = so_localize_global_bnb(context.h, surf, planner_point->size(), stride, ioff, c, &opts, &o, nullptr, 0, &last_global,
-                                             &last_bnb);
-        check(rc, "so_localize_global_bnb");
-        T_w_lidar = Transformd::from_pose7(last_global.pose);
-        last_T_w_lidar = T_w_lidar;
-        return rc;
+        return localizeInBox(planner_point, centre, opts, false);
+    }
+
+    // globalLocalizeInMap over the whole prior map held in the window AND the block archive (setArchive -> setOrigin -> loadPriorMap
+    // first): the region is taken from so_map_bounds_all and whole_map is set, so the candidates are registered window by window and
+    // the window is left where the winner is (so_global_opts.whole_map, superodom_b200.h).  Sets T_w_lidar, last_T_w_lidar, last_global
+    // and last_bnb as globalLocalizeInMap does.
+    template <class CloudPtr>
+    int globalLocalizeInWholeMap(const CloudPtr& planner_point, const Transformd& centre, so_global_opts opts) {
+        return localizeInBox(planner_point, centre, opts, true);
     }
 
     // LidarSLAM::EstimateLidarUncertainty (LidarSlam.cpp:915-975)
@@ -494,6 +480,40 @@ public:
     }
 
 private:
+    // globalLocalizeInMap (whole = false) / globalLocalizeInWholeMap (whole = true)
+    template <class CloudPtr>
+    int localizeInBox(const CloudPtr& planner_point, const Transformd& centre, so_global_opts opts, bool whole) {
+        localMap.sync_resolution();
+        size_t stride, ioff;
+        using PointT = typename std::decay<decltype(planner_point->points[0])>::type;
+        point_layout<PointT>(&stride, &ioff);
+        so_icp_opts o{};
+        o.max_icp_iters = int32_t(LocalizationICPMaxIter);
+        o.max_surface_features = OptSet.max_surface_features;
+        o.lm_max_iterations = 4;
+        o.yaw_ratio = OptSet.yaw_ratio;
+        double c[7];
+        centre.to_pose7(c);
+        float lo[3], hi[3];
+        size_t n_map = 0;
+        if (whole) {
+            check(so_map_bounds_all(context.h, lo, hi, &n_map), "so_map_bounds_all");
+            opts.whole_map = 1;
+        } else {
+            check(so_map_bounds(context.h, lo, hi, &n_map), "so_map_bounds");
+        }
+        auto half = [](double l, double h, double x) { const double a = h - x, b = x - l; return a > b ? (a > 0.0 ? a : 0.0) : (b > 0.0 ? b : 0.0); };
+        opts.half_x = half(lo[0], hi[0], c[0]);
+        opts.half_y = half(lo[1], hi[1], c[1]);
+        const void* surf = planner_point->size() ? planner_point->points.data() : nullptr;
+        const int rc = so_localize_global_bnb(context.h, surf, planner_point->size(), stride, ioff, c, &opts, &o, nullptr, 0, &last_global,
+                                             &last_bnb);
+        check(rc, "so_localize_global_bnb");
+        T_w_lidar = Transformd::from_pose7(last_global.pose);
+        last_T_w_lidar = T_w_lidar;
+        return rc;
+    }
+
     static void check(int rc, const char* what) { if (rc < 0) throw Error(std::string(what) + ": " + so_last_error()); }
 };
 

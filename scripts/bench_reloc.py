@@ -11,6 +11,10 @@ run of the numpy restatement of the search (tests/global_localization_numpy.py) 
 --whole-map adds branch-and-bound searches over whole maps: the cfg2 map (0.25 m, 2 deg, centre at the map centre with the true z
 and a seeded yaw) and a 300 m x 300 m synthetic map (synth.make_map(150.0, 0.2)), each with its per-level statistics, the share of
 hypotheses whose leaves were scored and the recovery error.  Either flag prints one more JSON line per workload.
+--archive adds whole-map searches (so_global_opts.whole_map = 1) over three cfg2-sized rooms at x = -800, 0 and +800 m (1.70 km,
+about 3 M points) held in the window and the block archive, window in room A: a scan in room C (the refinement moves the window)
+and a scan in room A (no move).  Per case, medians over --calls calls of the build device time (bounds, segment raster, dilation,
+levels, offsets), the traversal, the refinement wall time and n_windows, and the whole call; one JSON line per case.
 """
 import argparse
 import json
@@ -57,6 +61,7 @@ def main():
     ap.add_argument("--cpu", action="store_true")
     ap.add_argument("--bnb", action="store_true", help="also time so_localize_global_bnb against the exhaustive call")
     ap.add_argument("--whole-map", action="store_true", help="also run branch-and-bound searches over the whole cfg2 and 300 m maps")
+    ap.add_argument("--archive", action="store_true", help="also run whole-map searches over a 1.7 km three-room map in the block archive")
     a = ap.parse_args()
     from superodom_b200 import api, synth
     import global_localization_numpy as GN
@@ -133,6 +138,9 @@ def main():
         r = whole_map(ctx, f"300 m x 300 m synthetic map ({len(map3)} pts, generated in {gen_s:.1f} s)", case3, max(3, a.calls // 4), 1, out["hypotheses_per_s"])
         print(json.dumps(dict(r, card=name, power_limit_w=limit)))
         ctx.close()
+    if a.archive:
+        for r in archive_cases(a.calls, a.warmup):
+            print(json.dumps(dict(r, card=name, power_limit_w=limit)))
 
 
 def _stats(st):
@@ -197,6 +205,65 @@ def whole_map(ctx, label, case, calls, warmup, exhaustive_rate):
             "true_offset_m": float(np.linalg.norm(center[:2] - truth[:2])),
             "err_m": float(np.linalg.norm(pose[:3] - truth[:3])),
             "err_deg": math.degrees(2.0 * math.acos(min(1.0, abs(float(np.dot(pose[3:], truth[3:]))))))}
+
+
+def three_rooms():
+    """Three cfg2-sized rooms at x = -800, 0, +800 m (synth.make_map with the block filter's grid on each room): scenes and the
+    whole cloud."""
+    from superodom_b200 import synth
+    scenes, maps = [], []
+    for k, x in enumerate((-800.0, 0.0, 800.0)):
+        sc = synth.make_scene(52.0, seed=611 + k, center=(x, 0.0))
+        raw = synth.sample_surfaces(sc, 0.2, seed=1234)
+        xyzi = np.concatenate([raw, np.ones((len(raw), 1), np.float32)], 1)
+        scenes.append(sc)
+        maps.append(synth.voxel_filter_blocks(xyzi, 0.2, origin=(10 - int(round(x / 50.0)), 10, 5)))
+    return scenes, np.ascontiguousarray(np.concatenate(maps), np.float32)
+
+
+def archive_cases(calls, warmup):
+    """Whole-map search over the three rooms, window in room A (so_map_set_origin, the load, so_map_shift there).  Before every call
+    the window is put back in room A and rebuilt (untimed), so each call starts from the same state."""
+    from superodom_b200 import api, synth
+    scenes, cloud = three_rooms()
+    cap = 1 << 22
+    ctx = api.Context(max_map_points=cap, max_scan_points=262144, plane_res=0.2, max_batch=16)
+    ctx.map_archive(cap)
+    ctx.map_set_origin([-800.0, 0.0, 0.0])
+    ctx.map_set_points(cloud)
+    ctx.map_shift([-800.0, 0.0, 0.0])
+    o0 = [int(v) for v in ctx.map_origin()]
+    lo, hi, n_map = ctx.map_bounds_all()
+    out = []
+    for room, label in ((2, "room C: the window moves"), (0, "room A: no move")):
+        truth = synth.random_sensor_pose(scenes[room], 900 + 10 * room, 20.0)
+        scan = synth.make_scan(scenes[room], "os1_128", truth, 1000 + 10 * room)
+        yaw = np.random.default_rng(9300 + room).uniform(-math.pi, math.pi)
+        center = np.r_[0.5 * (float(lo[0]) + float(hi[0])), 0.5 * (float(lo[1]) + float(hi[1])), truth[2], 0.0, 0.0,
+                       math.sin(yaw / 2), math.cos(yaw / 2)]
+        g = api.whole_map_opts(lo, hi, center, yaw_half=math.pi, whole_map=True)
+        rec = {k: [] for k in ("build", "search", "refine", "wall")}
+        for it in range(warmup + calls):
+            ctx.map_set_origin([-50.0 * v for v in o0])
+            ctx.map_counts_5x5([10, 10, 5])                               # applies the origin change outside the timed call
+            t0 = time.perf_counter()
+            pose, res, cands, st = ctx.localize_global_bnb(scan, center, 20, g)
+            wall = (time.perf_counter() - t0) * 1e3
+            if it >= warmup:
+                for k, v in (("build", st.time_build_ms), ("search", st.time_search_ms), ("refine", res.time_refine_ms), ("wall", wall)):
+                    rec[k].append(v)
+        out.append({"workload": f"three-room map ({n_map} pts, {hi[0] - lo[0]:.0f} m x {hi[1] - lo[1]:.0f} m), whole-map search "
+                                f"{res.n_hypotheses} hypotheses x {res.n_score_points} score points, scan in {label}",
+                    "calls": calls, "build_device_ms_median": float(np.median(rec["build"])),
+                    "traversal_device_ms_median": float(np.median(rec["search"])),
+                    "refine_wall_ms_median": float(np.median(rec["refine"])), "wall_ms_median": float(np.median(rec["wall"])),
+                    "wall_ms_range": [float(np.min(rec["wall"])), float(np.max(rec["wall"]))],
+                    "n_windows": res.n_windows, "n_candidates": res.n_candidates, "status": res.status,
+                    "err_m": float(np.linalg.norm(pose[:3] - truth[:3])),
+                    "err_deg": math.degrees(2.0 * math.acos(min(1.0, abs(float(np.dot(pose[3:], truth[3:])))))),
+                    "best_ranked_err_m": float(np.linalg.norm(np.array(cands[0].pose[:3]) - truth[:3]))})
+    ctx.close()
+    return out
 
 
 if __name__ == "__main__":

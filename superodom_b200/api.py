@@ -24,7 +24,7 @@ EXPORTS = [
     "so_scan_prefilter", "so_scan_deskew", "so_scan_extract_uniform", "so_scan_extract_edges", "so_register", "so_register_prefiltered", "so_register_injected", "so_set_pose_sink", "so_register_batch", "so_register_batch_edges", "so_register_batch_device",
     "so_register_undistort", "so_register_undistort_edges", "so_register_prefiltered_undistort", "so_register_batch_undistort", "so_undistort_points", "so_register_optimized", "so_register_optimized_edges", "so_register_prefiltered_optimized", "so_register_batch_optimized", "so_evaluate_optimized", "so_evaluate_optimized_edges", "so_correspond", "so_correspond_seeded", "so_ordered_scans", "so_correspond_edge", "so_evaluate", "so_covariance",
     "so_register_degeneracy", "so_register_batch_degeneracy", "so_degeneracy_analysis",
-    "so_knn", "so_knn_device", "so_sampling_indices", "so_localize_global", "so_localize_scores", "so_localize_global_size", "so_localize_global_bnb", "so_localize_bnb_keys", "so_localize_bnb_bounds", "so_map_bounds", "so_kernel_launches", "so_bytes_copied", "so_build_flags", "so_profile_enable", "so_profile_get",
+    "so_knn", "so_knn_device", "so_sampling_indices", "so_localize_global", "so_localize_scores", "so_localize_global_size", "so_localize_global_bnb", "so_localize_bnb_keys", "so_localize_bnb_bounds", "so_map_bounds", "so_map_bounds_all", "so_kernel_launches", "so_bytes_copied", "so_build_flags", "so_profile_enable", "so_profile_get",
 ]
 
 
@@ -104,10 +104,10 @@ class DegeneracyResult(C.Structure):
 
 class GlobalOpts(C.Structure):
     """so_global_opts: zero fields take the defaults (res 0.25 m, yaw_step 2 deg, max_range 40 m, score_points 1024, dilate 1,
-    k 16, nms_xy 1 m, nms_yaw 10 deg)."""
+    k 16, nms_xy 1 m, nms_yaw 10 deg).  whole_map 1: search and refine over the window plus the block archive."""
     _fields_ = [("half_x", C.c_double), ("half_y", C.c_double), ("half_z", C.c_double), ("yaw_half", C.c_double),
                 ("res", C.c_double), ("yaw_step", C.c_double), ("max_range", C.c_double), ("score_points", C.c_int32),
-                ("dilate", C.c_int32), ("k", C.c_int32), ("pad_", C.c_int32), ("nms_xy", C.c_double), ("nms_yaw", C.c_double)]
+                ("dilate", C.c_int32), ("k", C.c_int32), ("whole_map", C.c_int32), ("nms_xy", C.c_double), ("nms_yaw", C.c_double)]
 
 
 class GlobalCandidate(C.Structure):
@@ -117,14 +117,15 @@ class GlobalCandidate(C.Structure):
 
 class GlobalResult(C.Structure):
     _fields_ = [("pose", C.c_double * 7), ("status", C.c_int32), ("winner", C.c_int32), ("n_candidates", C.c_int32),
-                ("best_score", C.c_int32), ("n_hypotheses", C.c_uint64), ("n_score_points", C.c_int32), ("pad_", C.c_int32),
+                ("best_score", C.c_int32), ("n_hypotheses", C.c_uint64), ("n_score_points", C.c_int32), ("n_windows", C.c_int32),
                 ("time_raster_ms", C.c_double), ("time_dilate_ms", C.c_double), ("time_score_ms", C.c_double),
                 ("time_sort_ms", C.c_double), ("time_refine_ms", C.c_double), ("time_total_ms", C.c_double), ("icp", IcpResult)]
 
 
 def global_opts(half_x=0.0, half_y=0.0, half_z=0.0, yaw_half=0.0, res=0.0, yaw_step=0.0, max_range=0.0, score_points=0, dilate=0,
-                k=0, nms_xy=0.0, nms_yaw=0.0) -> GlobalOpts:
-    return GlobalOpts(half_x, half_y, half_z, yaw_half, res, yaw_step, max_range, score_points, dilate, k, 0, nms_xy, nms_yaw)
+                k=0, nms_xy=0.0, nms_yaw=0.0, whole_map=False) -> GlobalOpts:
+    """whole_map: True / False, or an int passed through as given (the library accepts 0 and 1)."""
+    return GlobalOpts(half_x, half_y, half_z, yaw_half, res, yaw_step, max_range, score_points, dilate, k, int(whole_map), nms_xy, nms_yaw)
 
 
 BNB_LEVELS = 32
@@ -257,6 +258,7 @@ def load_library():
     L.so_localize_bnb_bounds.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p, C.c_void_p, C.c_int,
                                          C.c_void_p, C.c_size_t, C.c_void_p]
     L.so_map_bounds.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.so_map_bounds_all.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     L.so_kernel_launches.restype = C.c_uint64
     L.so_kernel_launches.argtypes = [C.c_void_p, C.c_int]
     L.so_bytes_copied.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
@@ -939,6 +941,13 @@ class Context:
         lo, hi = np.zeros(3, np.float32), np.zeros(3, np.float32)
         n = C.c_size_t()
         self._chk(self.L.so_map_bounds(self.h, _p(lo), _p(hi), C.byref(n)), "so_map_bounds")
+        return lo, hi, n.value
+
+    def map_bounds_all(self):
+        """map_bounds over the surf window plus the surf block archive (so_map_bounds_all) -> (lo, hi, point count)."""
+        lo, hi = np.zeros(3, np.float32), np.zeros(3, np.float32)
+        n = C.c_size_t()
+        self._chk(self.L.so_map_bounds_all(self.h, _p(lo), _p(hi), C.byref(n)), "so_map_bounds_all")
         return lo, hi, n.value
 
     # ---- k-NN

@@ -74,6 +74,25 @@ int ensure_maps(Ctx* c) {
     return SO_OK;
 }
 
+void shift_origin(const int32_t o[3], const double t[3], int32_t out[3], int32_t cc_out[3]) {
+    const int dims[3] = {kW, kH, kD};
+    for (int a = 0; a < 3; ++a) {                           // LocalMap::shiftMap (LocalMap.h:169-287)
+        int cc = block_coord_h(t[a] + kHalfBlock, o[a]), shift = 0;
+        while (cc < 3) { cc++; shift++; }
+        while (cc >= dims[a] - 3) { cc--; shift--; }
+        out[a] = o[a] + shift;
+        if (cc_out) cc_out[a] = cc;
+    }
+}
+
+int move_window(Ctx* c, const int32_t o[3]) {
+    if (o[0] != c->origin[0] || o[1] != c->origin[1] || o[2] != c->origin[2]) {
+        for (int a = 0; a < 3; ++a) c->origin[a] = o[a];
+        c->surf.dirty = true; c->edge.dirty = true;
+    }
+    return ensure_maps(c);
+}
+
 // ---------------------------------------------------------------------------------------------- allocation
 static int ctx_alloc(Ctx* c) {
     SO_CUDA_TRY(cudaSetDevice(c->device));
@@ -917,18 +936,9 @@ int so_map_shift(so_ctx* ctx, const double t[3], int32_t out_ijk[3]) {
     Ctx* c = reinterpret_cast<Ctx*>(ctx);
     if (!c || !t || !out_ijk) return fail(SO_ERR_ARG, "bad args");
     SO_CUDA_TRY(cudaSetDevice(c->device));
-    int cc[3], shift[3] = {0, 0, 0};
-    const int dims[3] = {kW, kH, kD};
-    for (int a = 0; a < 3; ++a) {                           // LocalMap::shiftMap (LocalMap.h:169-287)
-        cc[a] = block_coord_h(t[a] + kHalfBlock, c->origin[a]);
-        while (cc[a] < 3) { cc[a]++; shift[a]++; }
-        while (cc[a] >= dims[a] - 3) { cc[a]--; shift[a]--; }
-    }
-    if (shift[0] || shift[1] || shift[2]) {
-        for (int a = 0; a < 3; ++a) c->origin[a] += shift[a];
-        c->surf.dirty = true; c->edge.dirty = true;
-    }
-    { int rc = ensure_maps(c); if (rc) return rc; }
+    int32_t o[3], cc[3];
+    shift_origin(c->origin, t, o, cc);
+    { int rc = move_window(c, o); if (rc) return rc; }
     for (int a = 0; a < 3; ++a) out_ijk[a] = cc[a];
     return SO_OK;
 }

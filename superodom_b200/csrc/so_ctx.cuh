@@ -393,6 +393,12 @@ int archive_set_cap(Ctx* c, size_t cap);                  // both stores: on / r
 // so_map_set_points with the archive on: pts[0..n) (finite, host) -> window part in d_xyzi, the rest in the archive; no rebuild
 int archive_load(Ctx* c, MapStore& ms, const float4* pts, size_t n);
 int archive_download_all(Ctx* c, MapStore& ms, float* out, size_t cap, size_t* n_out);   // window + archive by world key
+// The live segments of ms's archive as {pool offset, -, points} in ms.arc.d_segs (host directory walk, no point copied): *n_segs of
+// them, the largest holding *max_n points
+int archive_segments(Ctx* c, MapStore& ms, uint32_t* n_segs, uint32_t* max_n);
+// LocalMap::shiftMap's rule: the origin so_map_shift(t) leaves when called at origin o, and t's block under it (cc, may be NULL)
+void shift_origin(const int32_t o[3], const double t[3], int32_t out[3], int32_t cc[3]);
+int move_window(Ctx* c, const int32_t o[3]);                // origin = o (both stores dirty when it changes), then ensure_maps
 MapView map_view(const Ctx* c, const MapStore& ms);
 int map_cells_per_block(float plane_res);
 int scan_sort_alloc(Ctx* c);             // temp storage for the per-registration scan sort
@@ -438,6 +444,10 @@ struct BnbCtl {                            // device control block, read back af
 void launch_map_bounds(const float4* pts, uint32_t n, uint32_t* d_bounds, cudaStream_t st);   // d_bounds: min xyz, max xyz (ordered bits)
 // Raster of the surf store into the window W of p (the whole box: x0 = y0 = z0 = 0, wx/wy/wz = bx/by/bz, wpr[0] = g.wpr)
 void launch_bnb_raster(const float4* pts, uint32_t n, const RelocGrid& g, const BnbPyramid& p, uint32_t* bits, cudaStream_t st);
+// The same two over the live segments of an archive pool (segs[s].src: first point, .n: points; max_n: the largest .n), read in place
+void launch_seg_bounds(const float4* pool, const GatherSeg* segs, uint32_t n_segs, uint32_t max_n, uint32_t* d_bounds, cudaStream_t st);
+void launch_seg_raster(const float4* pool, const GatherSeg* segs, uint32_t n_segs, uint32_t max_n, const RelocGrid& g, const BnbPyramid& p,
+                       uint32_t* bits, cudaStream_t st);
 void launch_bnb_levels(const BnbPyramid& p, uint32_t* pyr, cudaStream_t st);                  // levels 1..lmax from level 0
 void launch_bnb_offsets(const float4* spts, int n_pts, const double* d_q, const RelocGrid& g, const BnbPyramid& p, int4* off,
                         cudaStream_t st);

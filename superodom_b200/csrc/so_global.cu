@@ -1,7 +1,9 @@
 // so_global.cu -- global localization against the prior map, host side: defaults and limits of the search, score points and yaw
 // quaternions, the exhaustive and the branch-and-bound searches (kernels in so_reloc.cu), suppression and refinement of the best
-// hypotheses through register_scans, and the so_localize_* / so_map_bounds entry points of the C ABI.
+// hypotheses through register_scans (window by window over the block archive for whole_map searches), and the so_localize_* /
+// so_map_bounds* entry points of the C ABI.
 #include <algorithm>
+#include <array>
 #include <chrono>
 #include <cmath>
 #include <cstring>
@@ -26,6 +28,7 @@ struct GlobalPlan {
     int32_t m_off = 0;                     // yaw index of the centre's yaw (0 for the full circle)
     double dpsi = 0.0;                     // yaw step actually used
     uint64_t n_hyp = 0, bitmap_words = 0;
+    bool whole = false;                    // whole_map = 1 with the archive on: search the archive too, refine window by window
 };
 
 // Defaults, argument checks and the grid of so_localize_global (host only).  Capacity errors return with the plan filled in.
@@ -50,6 +53,7 @@ static int global_plan(const so_global_opts* in, GlobalPlan* P, bool bnb = false
     if (o.score_points < 1 || o.score_points > 4096) return fail(SO_ERR_ARG, "score_points must be in [1, 4096]");
     if (o.k < 1 || o.k > 64) return fail(SO_ERR_ARG, "k must be in [1, 64]");
     if (o.dilate < 1 || o.dilate > 8) return fail(SO_ERR_ARG, "dilate must be in [1, 8]");
+    if (o.whole_map != 0 && o.whole_map != 1) return fail(SO_ERR_ARG, "whole_map must be 0 or 1");
     P->o = o;
     const double Id = std::floor(o.half_x / o.res), Jd = std::floor(o.half_y / o.res), Kd = std::floor(o.half_z / o.res);
     const double ed = std::ceil(o.max_range / o.res);
@@ -168,6 +172,16 @@ static int global_upload(Ctx* c, const GlobalScan& S) {
     return SO_OK;
 }
 
+// The surf archive's live segments into the same raster (whole_map searches; after ensure_maps, which may change the directory)
+static int archive_raster(Ctx* c, const RelocGrid& g, const BnbPyramid& w, uint32_t* bits) {
+    uint32_t n_segs = 0, max_n = 0;
+    int rc = archive_segments(c, c->surf, &n_segs, &max_n);
+    if (rc) return rc;
+    launch_seg_raster(c->surf.arc.d_pool, c->surf.arc.d_segs, n_segs, max_n, g, w, bits, c->stream);
+    c->launches += n_segs ? 1 : 0;
+    return SO_OK;
+}
+
 static int global_search(Ctx* c, const GlobalPlan& P, const GlobalScan& S, bool sort) {
     Ctx::Reloc& R = c->reloc;
     if (!R.ev[0]) for (auto& e : R.ev) SO_CUDA_TRY(cudaEventCreate(&e));
@@ -186,6 +200,7 @@ static int global_search(Ctx* c, const GlobalPlan& P, const GlobalScan& S, bool 
     timed_launch_begin(c);
     SO_CUDA_TRY(cudaMemsetAsync(R.d_bits[0], 0, P.bitmap_words * sizeof(uint32_t), st));
     launch_bnb_raster(c->surf.d_xyzi, c->surf.n, g, box, R.d_bits[0], st);
+    if (P.whole) { int rc = archive_raster(c, g, box, R.d_bits[0]); if (rc) return rc; }
     timed_launch_end(c, 6);
     SO_CUDA_TRY(cudaEventRecord(R.ev[1], st));
     timed_launch_begin(c);
@@ -215,11 +230,15 @@ static int global_check_args(Ctx* c, const void* xyzi, size_t n, size_t stride, 
     int rc = global_plan(gopts, P, bnb);
     if (rc) return rc;
     if (n > c->cfg.max_scan_points) return fail(SO_ERR_CAPACITY, "scan larger than so_config.max_scan_points");
+    P->whole = P->o.whole_map == 1 && c->surf.arc.cap != 0;        // archive off: the window is the whole map
     return SO_OK;
 }
 
 // Everything after the search: suppression over the sorted key prefix pref[0..n_pref), refinement of the kept candidates, winner
-// selection.  Shared by so_localize_global and so_localize_global_bnb, which produce the same prefix.
+// selection.  Shared by so_localize_global and so_localize_global_bnb, which produce the same prefix.  The candidates register in
+// groups of one window each: for whole_map searches the window so_map_shift(prior) would leave from the current origin O0 (groups
+// ordered by their best-ranked member, the window moved to each in turn, and on return left at the winner's, or at O0 when there is
+// none); otherwise the current window, one group in rank order.
 static int global_refine(Ctx* c, const GlobalPlan& P, const GlobalScan& S, const uint64_t* pref, size_t n_pref, const void* xyzi, size_t n,
                          size_t stride, size_t ioff, const so_icp_opts* opts, so_global_candidate* cands, size_t cap, so_global_result* out,
                          std::chrono::steady_clock::time_point t0, std::chrono::steady_clock::time_point t1) {
@@ -261,21 +280,37 @@ static int global_refine(Ctx* c, const GlobalPlan& P, const GlobalScan& S, const
     const size_t n_cand = kept.size();
     out->n_candidates = int32_t(n_cand);
     std::vector<so_icp_result> res(n_cand);
+    const int32_t o0[3] = {c->origin[0], c->origin[1], c->origin[2]};       // the search applied any pending origin change
+    std::vector<std::array<int32_t, 3>> win(n_cand, std::array<int32_t, 3>{o0[0], o0[1], o0[2]});
+    if (P.whole) for (size_t k = 0; k < n_cand; ++k) shift_origin(o0, kept[k].prior, win[k].data(), nullptr);
+    std::vector<std::vector<size_t>> groups;                                 // candidate indices per window, rank order
+    for (size_t k = 0; k < n_cand; ++k) {
+        size_t gi = 0;
+        while (gi < groups.size() && win[groups[gi][0]] != win[k]) ++gi;
+        if (gi == groups.size()) groups.emplace_back();
+        groups[gi].push_back(k);
+    }
     if (n_cand) {
         const size_t B = std::min<size_t>(c->max_batch, n_cand);
         for (size_t s = 1; s < B && n; ++s)
             SO_CUDA_TRY(cudaMemcpyAsync(c->d_scan + s * n, c->d_scan, n * sizeof(float4), cudaMemcpyDeviceToDevice, c->stream));
         std::vector<uint32_t> npts(B, uint32_t(n));
-        std::vector<double> priors(7 * n_cand);
-        for (size_t q = 0; q < n_cand; ++q) std::memcpy(priors.data() + 7 * q, kept[q].prior, 7 * sizeof(double));
         RegisterRequest q;                                    // the candidate registrations leave no rows in a pose sink
         q.src = RegisterRequest::Source::DEVICE; q.scans = c->d_scan; q.n_points = npts.data(); q.opts = opts; q.sink_rows = false;
-        for (size_t s0 = 0; s0 < n_cand; s0 += B) {
-            q.n_scans = std::min(B, n_cand - s0); q.poses = priors.data() + 7 * s0; q.results = res.data() + s0;
-            rc = register_scans(c, q);
-            if (rc) return rc;
+        for (const std::vector<size_t>& grp : groups) {
+            if (P.whole) { rc = move_window(c, win[grp[0]].data()); if (rc) return rc; }   // the map moves; d_scan does not
+            std::vector<double> priors(7 * grp.size());
+            std::vector<so_icp_result> gres(grp.size());
+            for (size_t j = 0; j < grp.size(); ++j) std::memcpy(priors.data() + 7 * j, kept[grp[j]].prior, 7 * sizeof(double));
+            for (size_t s0 = 0; s0 < grp.size(); s0 += B) {
+                q.n_scans = std::min(B, grp.size() - s0); q.poses = priors.data() + 7 * s0; q.results = gres.data() + s0;
+                rc = register_scans(c, q);
+                if (rc) return rc;
+            }
+            for (size_t j = 0; j < grp.size(); ++j) res[grp[j]] = gres[j];
         }
     }
+    if (P.whole) out->n_windows = int32_t(groups.size());
     // winner: most SUCCESS correspondences in the final ICP iteration, then the lower final cost, then the better rank
     int32_t winner = -1;
     bool all_nef = n_cand > 0;
@@ -290,6 +325,7 @@ static int global_refine(Ctx* c, const GlobalPlan& P, const GlobalScan& S, const
             (r.hist_reject_plane[SO_MATCH_SUCCESS] == b.hist_reject_plane[SO_MATCH_SUCCESS] && final_cost(r) < final_cost(b)))
             winner = int32_t(q);
     }
+    if (P.whole) { rc = move_window(c, winner >= 0 ? win[winner].data() : o0); if (rc) return rc; }
     for (size_t q = 0; q < std::min(n_cand, cap); ++q) {
         so_global_candidate& o = cands[q];
         std::memset(&o, 0, sizeof(o));
@@ -366,17 +402,25 @@ static float float_from_order(uint32_t o) {
     return f;
 }
 
-// Bounding box of the surf store, reduced on the device; lo / hi are left alone for an empty map.
-static int map_bounds(Ctx* c, float lo[3], float hi[3], size_t* n) {
+// Bounding box of the surf store (whole: and of its archive's live segments), reduced on the device; lo / hi are left alone for an
+// empty map.
+static int map_bounds(Ctx* c, float lo[3], float hi[3], size_t* n, bool whole = false) {
     { int rc = bnb_alloc(c); if (rc) return rc; }
     { int rc = ensure_maps(c); if (rc) return rc; }
-    *n = c->surf.n;
-    if (!c->surf.n) return SO_OK;
+    const bool arc = whole && c->surf.arc.live;
+    *n = c->surf.n + (arc ? c->surf.arc.live : 0);
+    if (!*n) return SO_OK;
     cudaStream_t st = c->stream;
     SO_CUDA_TRY(cudaMemsetAsync(c->bnb.d_bounds, 0xff, 3 * sizeof(uint32_t), st));
     SO_CUDA_TRY(cudaMemsetAsync(c->bnb.d_bounds + 3, 0, 3 * sizeof(uint32_t), st));
     timed_launch_begin(c);
     launch_map_bounds(c->surf.d_xyzi, c->surf.n, c->bnb.d_bounds, st);
+    if (arc) {
+        uint32_t n_segs = 0, max_n = 0;
+        { int rc = archive_segments(c, c->surf, &n_segs, &max_n); if (rc) return rc; }
+        launch_seg_bounds(c->surf.arc.d_pool, c->surf.arc.d_segs, n_segs, max_n, c->bnb.d_bounds, st);
+        c->launches += c->surf.n ? 1 : 0;                               // one launch is counted by timed_launch_end
+    }
     timed_launch_end(c, 6);
     uint32_t h[6];
     SO_CUDA_TRY(cudaMemcpyAsync(h, c->bnb.d_bounds, sizeof(h), cudaMemcpyDeviceToHost, st));
@@ -425,7 +469,7 @@ static int bnb_build(Ctx* c, const GlobalPlan& P, const GlobalScan& S, RelocGrid
     SO_CUDA_TRY(cudaEventRecord(B.ev[0], st));
     float mlo[3] = {0, 0, 0}, mhi[3] = {0, 0, 0};
     size_t n_map = 0;
-    { int rc = map_bounds(c, mlo, mhi, &n_map); if (rc) return rc; }
+    { int rc = map_bounds(c, mlo, mhi, &n_map, P.whole); if (rc) return rc; }
     RelocGrid g = P.g;
     for (int a = 0; a < 3; ++a) g.lo[a] = S.lo[a];
     BnbPyramid p;
@@ -440,6 +484,7 @@ static int bnb_build(Ctx* c, const GlobalPlan& P, const GlobalScan& S, RelocGrid
     timed_launch_begin(c);
     SO_CUDA_TRY(cudaMemsetAsync(B.d_scratch, 0, w0 * sizeof(uint32_t), st));
     launch_bnb_raster(c->surf.d_xyzi, c->surf.n, g, p, B.d_scratch, st);
+    if (P.whole) { int rc = archive_raster(c, g, p, B.d_scratch); if (rc) return rc; }
     timed_launch_end(c, 6);
     SO_CUDA_TRY(cudaEventRecord(B.ev[1], st));
     RelocGrid gw{};                                                 // level 0 as k_reloc_dilate sees it: the window, same dilation
@@ -728,6 +773,14 @@ int so_map_bounds(so_ctx* ctx, float lo[3], float hi[3], size_t* n) {
     SO_CUDA_TRY(cudaSetDevice(c->device));
     for (int a = 0; a < 3; ++a) lo[a] = hi[a] = 0.f;
     return map_bounds(c, lo, hi, n);
+}
+
+int so_map_bounds_all(so_ctx* ctx, float lo[3], float hi[3], size_t* n) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c || !lo || !hi || !n) return fail(SO_ERR_ARG, "bad args");
+    SO_CUDA_TRY(cudaSetDevice(c->device));
+    for (int a = 0; a < 3; ++a) lo[a] = hi[a] = 0.f;
+    return map_bounds(c, lo, hi, n, true);
 }
 
 }  // extern "C"

@@ -650,6 +650,21 @@ int archive_load(Ctx* c, MapStore& ms, const float4* pts, size_t n) {
     return SO_OK;
 }
 
+int archive_segments(Ctx* c, MapStore& ms, uint32_t* n_segs, uint32_t* max_n) {
+    BlockArchive& a = ms.arc;
+    std::vector<GatherSeg> segs;
+    segs.reserve(a.dir.size());
+    uint32_t m = 0;
+    for (const auto& kv : a.dir) { segs.push_back(GatherSeg{kv.second.off, 0, kv.second.n, 0}); m = std::max(m, kv.second.n); }
+    *n_segs = uint32_t(segs.size());
+    *max_n = m;
+    if (segs.empty()) return SO_OK;
+    int rc = grow_buffer(a.d_segs, a.segs_cap, segs.size());
+    if (rc) return rc;
+    SO_CUDA_TRY(cudaMemcpyAsync(a.d_segs, segs.data(), segs.size() * sizeof(GatherSeg), cudaMemcpyHostToDevice, c->stream));
+    return SO_OK;
+}
+
 int archive_download_all(Ctx* c, MapStore& ms, float* out, size_t cap, size_t* n_out) {
     const BlockArchive& a = ms.arc;
     std::vector<float4> win(ms.n), pool(a.used);

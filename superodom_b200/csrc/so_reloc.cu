@@ -1,4 +1,5 @@
-// so_reloc.cu -- global localization search (so_localize_global): occupancy bitmap of the surf map, cube dilation, exhaustive
+// so_reloc.cu -- global localization search (so_localize_global): occupancy bitmap of the surf map (and of its block archive, read
+// in place, for whole_map searches), cube dilation, exhaustive
 // scoring of x/y/z voxel shifts x yaw steps of the scan, and the key sort that ranks the hypotheses.  The host side (score-point
 // selection, suppression, refinement through register_core) lives in so_global.cu.
 //
@@ -124,19 +125,58 @@ __global__ void __launch_bounds__(256) k_map_bounds(const float4* __restrict__ p
         for (int a = 0; a < 3; ++a) { atomicMin(b + a, lo[a]); atomicMax(b + 3 + a, hi[a]); }
 }
 
-// One thread per surf-store point: the box voxel floor((m - lo) / res) per axis; points inside the window W set their bit, shifted
-// to W's origin.  Both searches raster through it: the exhaustive one with W = the whole box.
+// The box voxel of a map coordinate along one axis, floor((m - lo) / res), every operation rounded on its own.  Every raster goes
+// through it, so the window's points and the archive's land in the same voxels.
+__device__ __forceinline__ double box_voxel(float m, double lo, double res) { return floor(__ddiv_rn(__dsub_rn(double(m), lo), res)); }
+
+// One thread per surf-store point: the box voxel per axis; points inside the window W set their bit, shifted to W's origin.  Both
+// searches raster through it: the exhaustive one with W = the whole box.
 __global__ void __launch_bounds__(256) k_bnb_raster(const float4* __restrict__ pts, uint32_t n, RelocGrid g, BnbPyramid w, uint32_t* __restrict__ bits) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const float4 p = pts[i];
-    const double fx = floor(__ddiv_rn(__dsub_rn(double(p.x), g.lo[0]), g.res));
-    const double fy = floor(__ddiv_rn(__dsub_rn(double(p.y), g.lo[1]), g.res));
-    const double fz = floor(__ddiv_rn(__dsub_rn(double(p.z), g.lo[2]), g.res));
+    const double fx = box_voxel(p.x, g.lo[0], g.res);
+    const double fy = box_voxel(p.y, g.lo[1], g.res);
+    const double fz = box_voxel(p.z, g.lo[2], g.res);
     if (!(fx >= double(w.x0) && fx < double(w.x0 + w.wx) && fy >= double(w.y0) && fy < double(w.y0 + w.wy) &&
           fz >= double(w.z0) && fz < double(w.z0 + w.wz))) return;
     const uint32_t x = uint32_t(fx) - uint32_t(w.x0), y = uint32_t(fy) - uint32_t(w.y0), z = uint32_t(fz) - uint32_t(w.z0);
     atomicOr(bits + (size_t(z) * w.wy + y) * w.wpr[0] + (x >> 5), 1u << (x & 31));
+}
+
+// The archive's pool read in place, segment by segment (the walk of k_seg_gather): CTA (s, y) takes every gridDim.y-th run of
+// blockDim.x points of live segment s, so that a large block spreads over several CTAs.  The pool's holes (restored blocks, stale
+// points) are never read.  Bounds: k_map_bounds' reduction over those points.
+__global__ void __launch_bounds__(256) k_seg_bounds(const float4* __restrict__ pool, const GatherSeg* __restrict__ segs, uint32_t* __restrict__ b) {
+    const GatherSeg s = segs[blockIdx.x];
+    uint32_t lo[3] = {~0u, ~0u, ~0u}, hi[3] = {0u, 0u, 0u};
+    for (uint32_t j = blockIdx.y * blockDim.x + threadIdx.x; j < s.n; j += gridDim.y * blockDim.x) {
+        const float4 p = pool[s.src + j];
+        const uint32_t v[3] = {float_order(p.x), float_order(p.y), float_order(p.z)};
+        for (int a = 0; a < 3; ++a) { lo[a] = min(lo[a], v[a]); hi[a] = max(hi[a], v[a]); }
+    }
+    for (int a = 0; a < 3; ++a) {
+        lo[a] = __reduce_min_sync(0xffffffffu, lo[a]);
+        hi[a] = __reduce_max_sync(0xffffffffu, hi[a]);
+    }
+    if ((threadIdx.x & 31) == 0)
+        for (int a = 0; a < 3; ++a) { atomicMin(b + a, lo[a]); atomicMax(b + 3 + a, hi[a]); }
+}
+
+// Raster: k_bnb_raster's voxel and window test for every point of the live segments
+__global__ void __launch_bounds__(256) k_seg_raster(const float4* __restrict__ pool, const GatherSeg* __restrict__ segs, RelocGrid g, BnbPyramid w,
+                                                    uint32_t* __restrict__ bits) {
+    const GatherSeg s = segs[blockIdx.x];
+    for (uint32_t j = blockIdx.y * blockDim.x + threadIdx.x; j < s.n; j += gridDim.y * blockDim.x) {
+        const float4 p = pool[s.src + j];
+        const double fx = box_voxel(p.x, g.lo[0], g.res);
+        const double fy = box_voxel(p.y, g.lo[1], g.res);
+        const double fz = box_voxel(p.z, g.lo[2], g.res);
+        if (!(fx >= double(w.x0) && fx < double(w.x0 + w.wx) && fy >= double(w.y0) && fy < double(w.y0 + w.wy) &&
+              fz >= double(w.z0) && fz < double(w.z0 + w.wz))) continue;
+        const uint32_t x = uint32_t(fx) - uint32_t(w.x0), y = uint32_t(fy) - uint32_t(w.y0), z = uint32_t(fz) - uint32_t(w.z0);
+        atomicOr(bits + (size_t(z) * w.wy + y) * w.wpr[0] + (x >> 5), 1u << (x & 31));
+    }
 }
 
 // Bits x .. x+31 of a row of wpr words (x may be negative); bits outside the row read 0.
@@ -296,6 +336,18 @@ void launch_map_bounds(const float4* pts, uint32_t n, uint32_t* d_bounds, cudaSt
 
 void launch_bnb_raster(const float4* pts, uint32_t n, const RelocGrid& g, const BnbPyramid& p, uint32_t* bits, cudaStream_t st) {
     if (n) k_bnb_raster<<<(n + 255) / 256, 256, 0, st>>>(pts, n, g, p, bits);
+}
+
+// CTAs per segment: enough for the largest one at 8 points per thread, at most 64
+static dim3 seg_grid(uint32_t n_segs, uint32_t max_n) { return dim3(n_segs, std::min<uint32_t>(64, std::max<uint32_t>(1, (max_n + 2047) / 2048))); }
+
+void launch_seg_bounds(const float4* pool, const GatherSeg* segs, uint32_t n_segs, uint32_t max_n, uint32_t* d_bounds, cudaStream_t st) {
+    if (n_segs) k_seg_bounds<<<seg_grid(n_segs, max_n), 256, 0, st>>>(pool, segs, d_bounds);
+}
+
+void launch_seg_raster(const float4* pool, const GatherSeg* segs, uint32_t n_segs, uint32_t max_n, const RelocGrid& g, const BnbPyramid& p,
+                       uint32_t* bits, cudaStream_t st) {
+    if (n_segs) k_seg_raster<<<seg_grid(n_segs, max_n), 256, 0, st>>>(pool, segs, g, p, bits);
 }
 
 void launch_bnb_levels(const BnbPyramid& p, uint32_t* pyr, cudaStream_t st) {
