@@ -240,7 +240,12 @@ int so_map_download_all(so_ctx* ctx, int store, float* out_xyzi, size_t cap_poin
 /* replaces: laserMapping::adjustVoxelSize (src/LaserMapping/laserMapping.cpp:600-651) for the surf cloud: with
  * auto_voxel_size, pick config_.lineRes/planeRes from the scan statistics (mean|x| * mean|y| * mean|z| < 25 -> 0.1/0.2,
  * > 65 -> 0.4/0.8, else unchanged), then pcl::VoxelGrid(planeRes) on the sensor-frame cloud, then push the resolutions
- * into the map (slam.localMap.lineRes_/planeRes_ = config_, :648-649).  line_res/plane_res are in/out.  Writes up to cap
+ * into the map (slam.localMap.lineRes_/planeRes_ = config_, :648-649).  line_res/plane_res are in/out.  The VoxelGrid is PCL 1.12's
+ * applyFilter for a cloud that is not dense: points with a non-finite x, y or z are skipped; the voxel index is taken relative to the
+ * bounding box of the finite points (idx = i + j div_x + k div_x div_y, 32-bit); when that box spans more than INT32_MAX voxels
+ * (dx dy dz, dx = int64((max_x - min_x) * (1/leaf)) + 1, float arithmetic) the cloud is returned verbatim, non-finite points included, as PCL does; one
+ * centroid per voxel, float sums in cloud order.  Covered: |coordinate / leaf| < 2^20 - 1 on every axis (about 210 km at leaf 0.2);
+ * beyond it PCL's conversions are undefined and the output is not specified (nothing is written past *n_out <= n).  Writes up to cap
  * packed float4 {x,y,z,intensity} points ordered by voxel index; *n_out = points produced. */
 int so_scan_prefilter(so_ctx* ctx, const void* xyzi, size_t n, size_t stride_bytes, size_t intensity_offset, int auto_voxel_size,
                       float* line_res, float* plane_res, float* out_xyzi, size_t cap_points, size_t* n_out, double* average_distance);
@@ -276,7 +281,8 @@ int so_scan_extract_uniform(so_ctx* ctx, const void* points, size_t n, size_t st
  *     max_per_sector points with curvature > edge_threshold that are not excluded are accepted, each excluding itself and up to 5
  *     neighbours per side until a gap |dq|^2 > 0.05;
  *   - output: packed float4 {x, y, z, intensity = time} ordered by (ring, position); with voxel_leaf > 0 then pcl::VoxelGrid(voxel_leaf)
- *     on the sensor frame (laserMapping's corner filter at lineRes, laserMapping.cpp:635-640), bit-equal to so_scan_prefilter's filter.
+ *     on the sensor frame (laserMapping's corner filter at lineRes, laserMapping.cpp:635-640), bit-equal to so_scan_prefilter's filter
+ *     (PCL's bounding-box index and verbatim fall-back included: a small leaf can return the edge cloud unfiltered).
  * points: n records of stride_bytes, float x, y, z at bytes 0, 4, 8, float time at time_offset, uint16 ring at ring_offset
  * (point_os::PointcloudXYZITR: stride 32, time at 20, ring at 24).  Does not touch the scan buffers: so_register_prefiltered and
  * so_map_add_registered_scan stay valid across this call.  *n_out = points produced (may exceed cap_points; only cap_points are
@@ -285,7 +291,7 @@ int so_scan_extract_uniform(so_ctx* ctx, const void* points, size_t n, size_t st
 typedef struct {
     float min_range;          /* points at or inside this range are dropped (default 0: zero returns only) */
     float edge_threshold;     /* curvature a point must exceed (default 0.1) */
-    float voxel_leaf;         /* > 0: voxel-centroid filter of the edge cloud at this leaf (default 0: off) */
+    float voxel_leaf;         /* > 0: pcl::VoxelGrid of the edge cloud at this leaf, as so_scan_prefilter's (default 0: off) */
     int32_t max_per_sector;   /* points accepted per sector (default 20, A-LOAM's less-sharp set) */
 } so_edge_opts;
 int so_scan_extract_edges(so_ctx* ctx, const void* points, size_t n, size_t stride_bytes, size_t time_offset, size_t ring_offset,

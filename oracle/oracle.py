@@ -391,38 +391,15 @@ def map_insert_numpy(old_xyzi, new_xyzi, leaf, origin=(10, 10, 5)):
 
 def adjust_voxel_size_numpy(scan_xyzi, line_res, plane_res, auto_voxel_size=True):
     """laserMapping::adjustVoxelSize (laserMapping.cpp:600-651) for the surf cloud: float32 sequential statistics, leaf
-    selection, pcl::VoxelGrid(planeRes) over the whole cloud.  -> (filtered, line_res, plane_res, average_distance)."""
+    selection, pcl::VoxelGrid(planeRes) over the whole cloud (oracle/voxel_grid_numpy.py, PCL's bounding-box index and its
+    verbatim fall-back).  -> (filtered, line_res, plane_res, average_distance)."""
+    from . import voxel_grid_numpy as vg
     s = np.ascontiguousarray(scan_xyzi, dtype=np.float32)
     avg = 0.0
     if auto_voxel_size and len(s):
-        a = np.zeros(3, np.float32)
-        ab = np.abs(s[:, :3])
-        for i in range(len(s)):               # float accumulators in cloud order, as the reference loop does
-            a = a + ab[i]
-        a = a / np.float32(len(s))
-        avg = float(a[0] * a[1] * a[2])
-        if avg < 25:
-            line_res, plane_res = 0.1, 0.2
-        elif avg > 65:
-            line_res, plane_res = 0.4, 0.8
-    inv = np.float32(1.0) / np.float32(plane_res)
-    fin = np.isfinite(s[:, :3]).all(1)
-    s = s[fin]
-    ijk = np.floor(s[:, :3] * inv).astype(np.int64)
-    order = np.lexsort((ijk[:, 0], ijk[:, 1], ijk[:, 2]))
-    s, ijk = s[order], ijk[order]
-    new = np.ones(len(s), dtype=bool)
-    new[1:] = (ijk[1:] != ijk[:-1]).any(1)
-    seg = np.cumsum(new) - 1
-    nseg = int(seg[-1]) + 1 if len(seg) else 0
-    start = np.flatnonzero(new)
-    rank = np.arange(len(s)) - start[seg]
-    acc = np.zeros((nseg, 4), np.float32)
-    for r in range(int(rank.max()) + 1 if len(rank) else 0):
-        m = rank == r
-        acc[seg[m]] = acc[seg[m]] + s[m]
-    cnt = np.bincount(seg, minlength=nseg).astype(np.float32)
-    return (acc / cnt[:, None]).astype(np.float32), float(np.float32(line_res)), float(np.float32(plane_res)), avg
+        avg = vg.adjust_statistic(s)
+        line_res, plane_res = vg.adjust_leaves(avg, line_res, plane_res)
+    return vg.voxel_grid(s, plane_res), float(np.float32(line_res)), float(np.float32(plane_res)), avg
 
 
 def cube_order(xyzi, origin=(10, 10, 5)):

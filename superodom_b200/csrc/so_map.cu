@@ -46,11 +46,12 @@ struct InsertInfo {
     uint32_t n_slots;           // non-empty blocks of that cloud
     uint32_t n_kept;            // its points on the grid
     uint32_t error;             // 1: more slots than the cell table was sized for
-    uint32_t overflow;          // scan pre-filter: a voxel index beyond the narrow key
+    uint32_t fallback;          // cloud voxel filter: PCL's voxel index would overflow, the output is the input
     uint32_t pad;
 };
 struct MapScratch {
     InsertInfo info;
+    uint32_t bounds[6];                                              // cloud voxel filter: float_order min, ~max per axis (atomicMin)
     uint8_t touched[kNumBlocks];                                     // blocks the new points of an insert reach
     uint32_t runs;                                                   // eviction: blocks (and the dropped run) of the off-window points
 };
@@ -793,26 +794,65 @@ static int map_rebuild_archive(Ctx* c, MapStore& ms) {
 
 // ------------------------------------------------------------------------------------------------------------------
 // Scan pre-filter: the pcl::VoxelGrid(planeRes) that laserMapping::adjustVoxelSize applies to the sensor-frame surf
-// cloud before Localization (laserMapping.cpp:639-645).  Same voxel/centroid semantics as the map insert, one grid
-// for the whole cloud.  In: d_scan[0..n); out: d_scan_sorted[0..*n_out) ordered by voxel index (k, j, i).
+// cloud before Localization (laserMapping.cpp:639-645), and the corner filter of the edge extraction.  One grid for the
+// whole cloud, indexed as VoxelGrid<PointT>::applyFilter (PCL 1.12, filters/impl/voxel_grid.hpp) indexes it: relative to
+// the bounding box of the finite points, and the cloud returned verbatim when dx * dy * dz would overflow an int32.
+// In: in[0..n); out: out[0..*n_out) ordered by PCL's voxel index.
 // ------------------------------------------------------------------------------------------------------------------
-// VB bits per voxel index (offset 2^(VB-1)); the key of a skipped point has bit 3*VB set and sorts last.  VB = 13 covers +-4096
-// voxels around the sensor (819 m at leaf 0.2) in 40 key bits = 5 radix passes; a point beyond that raises *overflow and the caller
-// repeats the filter with VB = 17 (the layout every cloud fits).
-template <int VB>
-__global__ void k_voxel_keys_cloud(const float4* __restrict__ raw, uint32_t n, float inv_leaf, uint64_t* __restrict__ keys, uint32_t* __restrict__ vals,
-                                   uint32_t* __restrict__ overflow) {
+constexpr int kCloudKeyBits = 33;                     // uint32 voxel index, non-finite points at bit 32: five 8-bit radix passes
+
+// Bounding box of the finite points (getMinMax3D of a cloud that is not dense): k_map_bounds' reduction with the non-finite points
+// left out, the maximum stored as ~max (one atomicMin and one 0xFF fill serve both), and the warps of a CTA combined in shared
+// memory first: a few CTAs, 6 atomics each, instead of 6 same-address atomics per warp of the cloud.
+constexpr uint32_t kBoundsCtas = 256;
+__global__ void __launch_bounds__(256) k_cloud_bounds(const float4* __restrict__ pts, uint32_t n, uint32_t* __restrict__ b) {
+    __shared__ uint32_t s[8][6];
+    uint32_t v6[6] = {~0u, ~0u, ~0u, ~0u, ~0u, ~0u};                   // min x, y, z; ~max x, y, z
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const float4 p = pts[i];
+        if (!(isfinite(p.x) && isfinite(p.y) && isfinite(p.z))) continue;
+        const uint32_t v[3] = {float_order(p.x), float_order(p.y), float_order(p.z)};
+        for (int a = 0; a < 3; ++a) { v6[a] = min(v6[a], v[a]); v6[3 + a] = min(v6[3 + a], ~v[a]); }
+    }
+    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    for (int a = 0; a < 6; ++a) v6[a] = __reduce_min_sync(0xffffffffu, v6[a]);
+    if (lane == 0)
+        for (int a = 0; a < 6; ++a) s[w][a] = v6[a];
+    __syncthreads();
+    if (threadIdx.x < 6) {
+        uint32_t m = ~0u;
+        for (int k = 0; k < 8; ++k) m = min(m, s[k][threadIdx.x]);
+        atomicMin(b + threadIdx.x, m);
+    }
+}
+
+// PCL's voxel index of every point: ijk = int(floor(p * inv) - float(min_b)) per axis, idx = ijk0 + ijk1 div0 + ijk2 div0 div1 in
+// 32-bit arithmetic (PCL's int products, mod 2^32).  Non-finite points get bit 32 and sort last.  Every thread derives the grid
+// from the bounds; thread 0 stores PCL's overflow test, dx dy dz > INT32_MAX with dx = int64((max - min) * inv) + 1, decided
+// exactly in double (inside the contract dx dy < 2^44 is exact, and the rounding of the last product is monotone, so it cannot
+// cross INT32_MAX); the float -> int conversions saturate outside the contract.
+__global__ void k_voxel_keys_cloud(const float4* __restrict__ raw, uint32_t n, float inv_leaf, const uint32_t* __restrict__ bounds,
+                                   uint64_t* __restrict__ keys, uint32_t* __restrict__ vals, uint32_t* __restrict__ fallback) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
+    float lo[3];
+    uint32_t min_b[3], div[3];
+    double cells = 1.0;
+    for (int a = 0; a < 3; ++a) {
+        lo[a] = float_unorder(bounds[a]);
+        const float hi = float_unorder(~bounds[3 + a]);
+        cells *= double(int64_t(__fmul_rn(__fsub_rn(hi, lo[a]), inv_leaf)) + 1);
+        min_b[a] = uint32_t(int(floorf(__fmul_rn(lo[a], inv_leaf))));
+        div[a] = uint32_t(int(floorf(__fmul_rn(hi, inv_leaf)))) - min_b[a] + 1u;
+    }
+    if (i == 0) *fallback = bounds[0] != ~0u && cells > 2147483647.0;        // no finite point: no fall-back, nothing out
     const float4 p = raw[i];
-    constexpr int64_t kOff = int64_t(1) << (VB - 1), kMask = (int64_t(1) << VB) - 1;
-    uint64_t key = uint64_t(1) << (3 * VB);                          // non-finite points are skipped, as PCL does
+    uint64_t key = uint64_t(1) << 32;                                // non-finite points are skipped, as PCL does
     if (isfinite(p.x) && isfinite(p.y) && isfinite(p.z)) {
-        const int64_t vi = int64_t(floorf(__fmul_rn(p.x, inv_leaf))) + kOff;
-        const int64_t vj = int64_t(floorf(__fmul_rn(p.y, inv_leaf))) + kOff;
-        const int64_t vk = int64_t(floorf(__fmul_rn(p.z, inv_leaf))) + kOff;
-        if (((vi | vj | vk) & ~kMask) != 0) *overflow = 1;           // outside the VB-bit range (negative values have high bits set)
-        key = (uint64_t(vk & kMask) << (2 * VB)) | (uint64_t(vj & kMask) << VB) | uint64_t(vi & kMask);
+        const float v[3] = {p.x, p.y, p.z};
+        uint32_t ijk[3];
+        for (int a = 0; a < 3; ++a) ijk[a] = uint32_t(int(__fsub_rn(floorf(__fmul_rn(v[a], inv_leaf)), float(int(min_b[a])))));
+        key = ijk[0] + ijk[1] * div[0] + ijk[2] * (div[0] * div[1]);
     }
     keys[i] = key;
     vals[i] = i;
@@ -826,21 +866,24 @@ int cloud_voxel_filter(Ctx* c, const float4* in, uint32_t n, float leaf, const V
     const float inv_leaf = 1.0f / leaf;
     InsertInfo* d_info = &c->d_map_scratch->info;
     InsertInfo* h_info = c->h_map_info;
-    for (int wide = 0; wide < 2; ++wide) {
-        const int vb = wide ? 17 : 13;
-        SO_CUDA_TRY(cudaMemsetAsync(&d_info->overflow, 0, sizeof(uint32_t), st));
-        if (wide) k_voxel_keys_cloud<17><<<grid, 256, 0, st>>>(in, n, inv_leaf, b.keys, b.vals, &d_info->overflow);
-        else k_voxel_keys_cloud<13><<<grid, 256, 0, st>>>(in, n, inv_leaf, b.keys, b.vals, &d_info->overflow);
-        size_t tmp = b.tmp_bytes;
-        SO_CUDA_TRY(cub::DeviceRadixSort::SortPairs(b.tmp, tmp, b.keys, b.keys_out, b.vals, b.vals_out, int(n), 0, 3 * vb + 1, st));
-        c->launches += 7;
-        const int rc = voxel_reduce(c, in, b.keys_out, b.vals_out, n, 0, uint64_t(1) << (3 * vb),
-                                    reinterpret_cast<uint32_t*>(b.keys), b.tmp, b.tmp_bytes, out);   // keys_in is free after the sort
-        if (rc) return rc;
-        SO_CUDA_TRY(cudaMemcpyAsync(h_info, d_info, sizeof(InsertInfo), cudaMemcpyDeviceToHost, st));
-        SO_CUDA_TRY(cudaGetLastError());
+    uint32_t* d_bounds = c->d_map_scratch->bounds;
+    SO_CUDA_TRY(cudaMemsetAsync(d_bounds, 0xFF, 6 * sizeof(uint32_t), st));
+    k_cloud_bounds<<<std::min(grid, kBoundsCtas), 256, 0, st>>>(in, n, d_bounds);
+    k_voxel_keys_cloud<<<grid, 256, 0, st>>>(in, n, inv_leaf, d_bounds, b.keys, b.vals, &d_info->fallback);
+    size_t tmp = b.tmp_bytes;
+    SO_CUDA_TRY(cub::DeviceRadixSort::SortPairs(b.tmp, tmp, b.keys, b.keys_out, b.vals, b.vals_out, int(n), 0, kCloudKeyBits, st));
+    c->launches += 8;
+    const int rc = voxel_reduce(c, in, b.keys_out, b.vals_out, n, 0, uint64_t(1) << 32,
+                                reinterpret_cast<uint32_t*>(b.keys), b.tmp, b.tmp_bytes, out);   // keys_in is free after the sort
+    if (rc) return rc;
+    SO_CUDA_TRY(cudaMemcpyAsync(h_info, d_info, sizeof(InsertInfo), cudaMemcpyDeviceToHost, st));
+    SO_CUDA_TRY(cudaGetLastError());
+    SO_CUDA_TRY(cudaStreamSynchronize(st));
+    if (h_info->fallback) {                                         // PCL: "Integer indices would overflow", output = input
+        SO_CUDA_TRY(cudaMemcpyAsync(out, in, size_t(n) * sizeof(float4), cudaMemcpyDeviceToDevice, st));
         SO_CUDA_TRY(cudaStreamSynchronize(st));
-        if (!h_info->overflow) break;                               // every voxel index fitted the narrow key
+        *n_out = n;
+        return SO_OK;
     }
     *n_out = h_info->n_out;
     return SO_OK;

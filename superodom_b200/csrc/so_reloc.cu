@@ -103,12 +103,6 @@ __global__ void __launch_bounds__(kRelocThreads) k_reloc_score(const float4* __r
 }
 
 // ---------------------------------------------------------------------------------------------- branch and bound
-// float -> uint32 with the same order (negative values flipped), so that min / max reduce with integer atomics
-__device__ __forceinline__ uint32_t float_order(float f) {
-    const uint32_t u = __float_as_uint(f);
-    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-
 // Bounding box of the surf store: per-thread min / max, a warp reduction, one atomic per warp and axis.
 __global__ void __launch_bounds__(256) k_map_bounds(const float4* __restrict__ pts, uint32_t n, uint32_t* __restrict__ b) {
     uint32_t lo[3] = {~0u, ~0u, ~0u}, hi[3] = {0u, 0u, 0u};

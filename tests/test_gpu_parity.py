@@ -529,12 +529,19 @@ def test_scan_prefilter_adjust_voxel_size(gpu_api, oracle_mod):
     ctx.map_add_registered_scan(np.array(r2.pose))
     assert np.array_equal(ctx.map_download(0), ref.map_download(0))
     ref.close()
-    # returns beyond the 13-bit voxel range of the narrow sort key (+-4096 voxels) take the wide-key path: same result as numpy
+    # returns far out on every axis: 69 964 x 67 904 x 14 529 voxels at leaf 0.2 pass PCL's int32 test, the cloud comes back verbatim
     far = s.copy()
     far[5::997, :3] *= np.float32(400.0)
     out2, _, _, _ = ctx.scan_prefilter(far, 0.2, 0.2, False)
     ref2, _, _, _ = oracle_mod.adjust_voxel_size_numpy(far, 0.2, 0.2, False)
-    assert np.abs(far[np.isfinite(far).all(1), :3]).max() > 4096 * 0.2 and np.array_equal(out2, ref2)
+    assert out2.shape == far.shape and np.array_equal(out2.view(np.uint32), far.view(np.uint32))
+    assert np.array_equal(out2.view(np.uint32), ref2.view(np.uint32))
+    # far out along x alone (69 964 x 240 x 43 voxels): PCL filters it, with voxel indices beyond +-4096
+    far = s.copy()
+    far[5::997, 0] *= np.float32(400.0)
+    out2, _, _, _ = ctx.scan_prefilter(far, 0.2, 0.2, False)
+    ref2, _, _, _ = oracle_mod.adjust_voxel_size_numpy(far, 0.2, 0.2, False)
+    assert np.abs(far[np.isfinite(far).all(1), 0]).max() > 4096 * 0.2 and len(out2) < len(far) and np.array_equal(out2, ref2)
     ctx.close()
 
 
