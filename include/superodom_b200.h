@@ -456,6 +456,39 @@ int so_register_batch_degeneracy(so_ctx* ctx, const void* surf_xyzi, const uint3
  * preceding so_correspond* left for so_evaluate. */
 int so_degeneracy_analysis(so_ctx* ctx, const double* H, const so_degeneracy* d, so_degeneracy_result* out);
 
+/* Test hook: one ICP iteration's solve (Ceres' trust-region LM, LidarSlam.cpp:213-240) on caller-given correspondences, for a batch of
+ * n_problems problems, by the device code and the launch sequence a registration of n_problems scans runs -- the fused evaluation +
+ * step kernel for one or two problems (unless SO_NO_FUSED_LM is set), evaluation + step kernels otherwise, the degeneracy-aware step
+ * kernel when d is given -- without the neighbour search and the plane fit.  The rows of problem b follow those of problem b - 1 in
+ * `rows`; every row counts as an accepted plane correspondence (also with w = 0: it then adds nothing but counts towards the prior's
+ * information, as features_corres.size() does).  The registration's plane_res sets the Tukey loss.  n_rows <= so_config.max_scan_points,
+ * n_problems <= max_batch.  d: NULL or one so_degeneracy per problem.  Replaces the state a preceding so_correspond* left for
+ * so_evaluate and the scan buffer so_ordered_scans reads. */
+typedef struct {
+    float p[3];                /* scan point, sensor frame */
+    float pad_;
+    double n[3], d, w;         /* plane n.x + d = 0 and its residualCoefficient */
+} so_solve_row;
+typedef struct {
+    uint32_t n_rows;
+    int32_t lm_max_iterations; /* <= 0: 4; at most 16 */
+    double pose[7];            /* start of the solve */
+    int32_t use_pose_prior;    /* SE3 prior rows (addAbsolutePoseConstraints) with measurement x0 */
+    float visual_confidence_factor, prior_uncertainty[3];
+    int32_t pad_;
+    double x0[7];
+} so_solve_problem;
+typedef struct {
+    double pose[7];
+    double initial_cost, final_cost;
+    int32_t lm_iterations, successful, unsuccessful, termination;   /* termination: as so_icp_result.iter_lm_termination */
+    double radius, decrease_factor, gmax;                           /* the trust-region state the solve ended in */
+    int32_t n_flag_pos, n_flag_ori;                                 /* flagged directions (degeneracy-aware solves) */
+    int32_t status, pad_;                                           /* so_icp_result.status */
+} so_solve_result;
+int so_solve(so_ctx* ctx, const so_solve_row* rows, const so_solve_problem* problems, size_t n_problems, const so_degeneracy* d,
+             so_solve_result* out);
+
 /* Sharded-replay plumbing (BASELINE cfg4; SURVEY 8e "K8"): a caller-owned DEVICE buffer of cap_rows x 8 doubles.  Every following
  * so_register / so_register_batch* call appends one row per scan, starting at first_row and advancing: {pose_opt[7] (the
  * optimiser output, so_icp_result.pose_opt), status + 256 * n_iterations}; scans that were not registered (soft statuses) carry

@@ -109,7 +109,7 @@ def lib():
     L.orc_correspond.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, C.c_float, C.c_int, C.c_int, C.c_int,
                                  C.c_void_p, C.c_void_p, C.c_void_p]
     L.orc_evaluate.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-    L.orc_solve.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_float, C.c_int, C.c_void_p, C.c_void_p]
+    L.orc_solve.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_float, C.c_int, C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]
     L.orc_covariance.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_float, C.c_void_p]
     L.orc_register.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p]
     L.orc_set_nn_trace.argtypes = [C.c_void_p, C.c_size_t, C.c_int]
@@ -265,14 +265,21 @@ def evaluate(corr: np.ndarray, pose7, plane_res):
     return H, g, cost.value, nok.value
 
 
-def solve(corr: np.ndarray, pose7, plane_res, lm_max_iterations=4):
+def solve(corr: np.ndarray, pose7, plane_res, lm_max_iterations=4, pose_prior=None):
+    """One ceres::Solve on the status-0 rows of corr from pose7.  pose_prior = (measurement pose7, visual_confidence_factor,
+    (ux, uy, uz)) adds the SE3AbsolutatePoseFactor rows, their information from the number of those rows."""
     L = lib()
     pose = np.array(pose7, dtype=np.float64)
     summ = np.zeros(4, np.int32)
-    costs = np.zeros(2)
-    L.orc_solve(_p(corr), corr.shape[0], _p(pose), C.c_float(plane_res), lm_max_iterations, _p(summ), _p(costs))
+    costs = np.zeros(5)
+    meas, vcf, unc = None, 0.0, None
+    if pose_prior is not None:
+        meas = np.ascontiguousarray(pose_prior[0], dtype=np.float64)
+        vcf, unc = float(pose_prior[1]), np.ascontiguousarray(pose_prior[2], dtype=np.float32)
+    L.orc_solve(_p(corr), corr.shape[0], _p(pose), C.c_float(plane_res), lm_max_iterations, None if meas is None else _p(meas),
+                C.c_float(vcf), None if unc is None else _p(unc), _p(summ), _p(costs))
     return pose, dict(successful=int(summ[0]), unsuccessful=int(summ[1]), iterations=int(summ[2]), termination=int(summ[3]),
-                      initial_cost=costs[0], final_cost=costs[1])
+                      initial_cost=costs[0], final_cost=costs[1], radius=costs[2], decrease_factor=costs[3], gmax=costs[4])
 
 
 def covariance(corr: np.ndarray, pose7, plane_res):

@@ -776,6 +776,18 @@ struct PosePrior {
     }
 };
 
+// addAbsolutePoseConstraints (LidarSlam.cpp:285-298): the information diagonal from features_corres.size() = good
+static void set_pose_prior(PosePrior& P, const double meas[7], int good, float visual_confidence_factor, const float prior_uncertainty[3]) {
+    const double vcf = double(visual_confidence_factor);
+    double info[6];
+    for (int a = 0; a < 3; ++a) info[a] = (1 - double(prior_uncertainty[a])) * std::max(50, int(good * 0.1)) * vcf;
+    info[3] = info[4] = std::max(10, int(good * 0.01)) * vcf;
+    info[5] = std::max(5, int(good * 0.001)) * 0;
+    P.on = true;
+    std::memcpy(P.meas, meas, sizeof(P.meas));
+    P.set_information(info);
+}
+
 struct Evaluator {
     std::vector<const EdgeCorr*> edges; // accepted edge correspondences (added BEFORE the planes, LidarSlam.cpp:304-307)
     double a2_line = 0;                 // Tukey a^2 for edges, a = double(sqrtf(3*lineRes)) (LidarSlam.cpp:263)
@@ -850,7 +862,10 @@ struct Evaluator {
     }
 };
 
-struct SolveSummary { int num_successful_steps = 0, num_unsuccessful_steps = 0, iterations = 0, termination = 0; double initial_cost = 0, final_cost = 0; };
+struct SolveSummary {
+    int num_successful_steps = 0, num_unsuccessful_steps = 0, iterations = 0, termination = 0; double initial_cost = 0, final_cost = 0;
+    double radius = 0, decrease_factor = 0, gmax = 0;      // the trust-region state the loop ended in
+};
 // termination: 0 NO_CONVERGENCE(max iters) 1 gradient tol 2 parameter tol 3 function tol 4 radius 5 invalid steps 6 no residuals
 //              7 non-finite cost at the start (the reference aborts)
 
@@ -937,6 +952,7 @@ static SolveSummary ceres_solve(const Evaluator& E, double params[7], int max_nu
         }
     }
     S.iterations = iteration; S.final_cost = x_cost;
+    S.radius = radius; S.decrease_factor = decrease_factor; S.gmax = gmax;
     // parameters_ hold the best (last accepted, monotonic) iterate
     if (S.termination == 2 || S.termination == 3) { /* tolerance returns skip Finalize; best already == x (last accepted) */ std::memcpy(best, x, sizeof(x)); }
     std::memcpy(params, best, sizeof(best));
@@ -1194,13 +1210,17 @@ int orc_evaluate(const orc_corr* corr, size_t n, const double pose[7], float pla
     return 0;
 }
 
-// One ceres::Solve on fixed correspondences (stage parity for the LM state machine).
-int orc_solve(const orc_corr* corr, size_t n, double pose[7], float plane_res, int lm_max_iterations, int32_t summary[4], double costs[2]) {
+// One ceres::Solve on fixed correspondences (stage parity for the LM state machine).  prior_meas (optional): the SE3 prior rows with
+// that measurement, their information from the accepted correspondences as a registration computes it.
+// costs: initial and final cost, then the final radius, decrease factor and gradient max-norm.
+int orc_solve(const orc_corr* corr, size_t n, double pose[7], float plane_res, int lm_max_iterations, const double* prior_meas,
+              float visual_confidence_factor, const float* prior_uncertainty, int32_t summary[4], double costs[5]) {
     orc::Evaluator E; const double a = double(std::sqrt(3 * plane_res)); E.a2 = a * a;
     for (size_t i = 0; i < n; ++i) if (corr[i].status == orc::SUCCESS) E.blocks.push_back(&corr[i]);
+    if (prior_meas) orc::set_pose_prior(E.prior, prior_meas, int(E.blocks.size()), visual_confidence_factor, prior_uncertainty);
     orc::SolveSummary S = orc::ceres_solve(E, pose, lm_max_iterations);
     summary[0] = S.num_successful_steps; summary[1] = S.num_unsuccessful_steps; summary[2] = S.iterations; summary[3] = S.termination;
-    costs[0] = S.initial_cost; costs[1] = S.final_cost;
+    costs[0] = S.initial_cost; costs[1] = S.final_cost; costs[2] = S.radius; costs[3] = S.decrease_factor; costs[4] = S.gmax;
     return 0;
 }
 
@@ -1270,17 +1290,8 @@ int orc_register_full(void* m, const float* scan_xyzi, size_t n, const float* ed
         E.blocks.clear();
         for (size_t i = 0; i < n; ++i) if (corr[i].status == SUCCESS) E.blocks.push_back(&corr[i]);
         E.prior.on = false;
-        if (opt->use_pose_prior) {                                // addAbsolutePoseConstraints (:285-298), position = T_w_initial_guess
-            const int good = int(E.blocks.size() + E.edges.size());      // features_corres.size()
-            const double vcf = double(opt->visual_confidence_factor);
-            double info[6];
-            for (int a = 0; a < 3; ++a) info[a] = (1 - double(opt->prior_uncertainty[a])) * std::max(50, int(good * 0.1)) * vcf;
-            info[3] = info[4] = std::max(10, int(good * 0.01)) * vcf;
-            info[5] = std::max(5, int(good * 0.001)) * 0;
-            E.prior.on = true;
-            std::memcpy(E.prior.meas, T0, sizeof(T0));
-            E.prior.set_information(info);
-        }
+        if (opt->use_pose_prior)                                  // position = T_w_initial_guess
+            set_pose_prior(E.prior, T0, int(E.blocks.size() + E.edges.size()), opt->visual_confidence_factor, opt->prior_uncertainty);
         double prev[7]; std::memcpy(prev, T, sizeof(T));
         double params[7]; std::memcpy(params, T, sizeof(T));     // pose_parameters were set in prepareOptimizationState and by the previous solve
         SolveSummary S = ceres_solve(E, params, opt->lm_max_iterations);

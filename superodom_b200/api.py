@@ -23,7 +23,7 @@ EXPORTS = [
     "so_map_archive", "so_map_archive_info", "so_map_download_all",
     "so_scan_prefilter", "so_scan_deskew", "so_scan_extract_uniform", "so_scan_extract_edges", "so_register", "so_register_prefiltered", "so_register_injected", "so_set_pose_sink", "so_register_batch", "so_register_batch_edges", "so_register_batch_device",
     "so_register_undistort", "so_register_undistort_edges", "so_register_prefiltered_undistort", "so_register_batch_undistort", "so_undistort_points", "so_register_optimized", "so_register_optimized_edges", "so_register_prefiltered_optimized", "so_register_batch_optimized", "so_evaluate_optimized", "so_evaluate_optimized_edges", "so_correspond", "so_correspond_seeded", "so_ordered_scans", "so_correspond_edge", "so_evaluate", "so_covariance",
-    "so_register_degeneracy", "so_register_batch_degeneracy", "so_degeneracy_analysis",
+    "so_register_degeneracy", "so_register_batch_degeneracy", "so_degeneracy_analysis", "so_solve",
     "so_knn", "so_knn_device", "so_sampling_indices", "so_localize_global", "so_localize_scores", "so_localize_global_size", "so_localize_global_bnb", "so_localize_bnb_keys", "so_localize_bnb_bounds", "so_map_bounds", "so_map_bounds_all", "so_kernel_launches", "so_bytes_copied", "so_build_flags", "so_profile_enable", "so_profile_get",
 ]
 
@@ -158,6 +158,16 @@ CORR_DTYPE = np.dtype([("n", "<f8", 3), ("d", "<f8"), ("w", "<f8"), ("nn", "<u4"
 EDGE_CORR_DTYPE = np.dtype([("a", "<f8", 3), ("b", "<f8", 3), ("w", "<f8"), ("nn", "<u4", 10), ("selected_mask", "<u4"),
                             ("status", "u1"), ("n_selected", "u1"), ("pad_", "u1", 2)], align=True)
 
+# so_solve's rows, problems and results
+SOLVE_ROW_DTYPE = np.dtype([("p", "<f4", 3), ("pad_", "<f4"), ("n", "<f8", 3), ("d", "<f8"), ("w", "<f8")], align=True)
+SOLVE_PROBLEM_DTYPE = np.dtype([("n_rows", "<u4"), ("lm_max_iterations", "<i4"), ("pose", "<f8", 7), ("use_pose_prior", "<i4"),
+                                ("visual_confidence_factor", "<f4"), ("prior_uncertainty", "<f4", 3), ("pad_", "<i4"), ("x0", "<f8", 7)],
+                               align=True)
+SOLVE_RESULT_DTYPE = np.dtype([("pose", "<f8", 7), ("initial_cost", "<f8"), ("final_cost", "<f8"), ("lm_iterations", "<i4"),
+                               ("successful", "<i4"), ("unsuccessful", "<i4"), ("termination", "<i4"), ("radius", "<f8"),
+                               ("decrease_factor", "<f8"), ("gmax", "<f8"), ("n_flag_pos", "<i4"), ("n_flag_ori", "<i4"),
+                               ("status", "<i4"), ("pad_", "<i4")], align=True)
+
 _lib = None
 
 
@@ -243,6 +253,7 @@ def load_library():
     L.so_register_batch_degeneracy.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t,
                                                C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     L.so_degeneracy_analysis.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.so_solve.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
     L.so_knn.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_int, C.c_float, C.c_void_p, C.c_void_p]
     L.so_knn_device.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_float, C.c_void_p, C.c_void_p]
     L.so_sampling_indices.argtypes = [C.c_uint32, C.c_int32, C.c_void_p, C.c_size_t, C.c_void_p]
@@ -857,6 +868,18 @@ class Context:
         r = DegeneracyResult()
         self._chk(self.L.so_degeneracy_analysis(self.h, _p(a), C.byref(d), C.byref(r)), "so_degeneracy_analysis")
         return r
+
+    def solve(self, rows: np.ndarray, problems: np.ndarray, ds=None) -> np.ndarray:
+        """One ICP iteration's solve per problem on given correspondences (so_solve): rows [sum n_rows] of SOLVE_ROW_DTYPE, problem
+        b's after problem b - 1's; problems [B] of SOLVE_PROBLEM_DTYPE; ds: None or one Degeneracy per problem.
+        -> [B] of SOLVE_RESULT_DTYPE."""
+        rows = np.ascontiguousarray(rows, dtype=SOLVE_ROW_DTYPE)
+        problems = np.ascontiguousarray(problems, dtype=SOLVE_PROBLEM_DTYPE)
+        assert int(problems["n_rows"].sum()) == len(rows)
+        out = np.zeros(len(problems), SOLVE_RESULT_DTYPE)
+        da = None if ds is None else (Degeneracy * len(problems))(*ds)
+        self._chk(self.L.so_solve(self.h, _p(rows) if len(rows) else None, _p(problems), len(problems), da, _p(out)), "so_solve")
+        return out
 
     # ---- global localization
     def localize_global(self, scan_xyzi: np.ndarray, center_pose7, max_icp_iters: int, opts: GlobalOpts | None = None,

@@ -1779,6 +1779,102 @@ int so_degeneracy_analysis(so_ctx* ctx, const double* H, const so_degeneracy* d,
     return SO_OK;
 }
 
+// The buffers k_fit fills (scan point with its index in w, {n, d}, weight, flags, the accepted-row histogram) are written from the
+// caller's rows; then the first evaluation and lm_max evaluations run as one ICP iteration of a registration launches them.
+int so_solve(so_ctx* ctx, const so_solve_row* rows, const so_solve_problem* pr, size_t n_problems, const so_degeneracy* d, so_solve_result* out) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c || !pr || !out || n_problems == 0) return fail(SO_ERR_ARG, "bad args");
+    if (n_problems > size_t(c->max_batch)) return fail(SO_ERR_CAPACITY, "more problems than so_config.max_batch");
+    if (d) { int rc = check_degeneracy(d, n_problems); if (rc) return rc; }
+    size_t total = 0;
+    uint32_t max_n = 0;
+    int lm = 0;
+    for (size_t b = 0; b < n_problems; ++b) {
+        if (pr[b].n_rows > c->cfg.max_scan_points) return fail(SO_ERR_CAPACITY, "problem larger than so_config.max_scan_points");
+        if (pr[b].lm_max_iterations > 16) return fail(SO_ERR_ARG, "lm_max_iterations must be <= 16");
+        total += pr[b].n_rows;
+        max_n = std::max(max_n, pr[b].n_rows);
+        lm = std::max(lm, pr[b].lm_max_iterations <= 0 ? 4 : pr[b].lm_max_iterations);
+    }
+    if (total && !rows) return fail(SO_ERR_ARG, "bad args");
+    SO_CUDA_TRY(cudaSetDevice(c->device));
+    if (d) { int rc = grow_buffer(c->deg.d_st, c->deg.st_cap, size_t(c->max_batch)); if (rc) return rc; }
+    c->prefiltered_n = SIZE_MAX;                                  // d_scan_sorted is overwritten
+    std::vector<float4> sp(total);
+    std::vector<double4> nd(total);
+    std::vector<double> w(total);
+    std::vector<int32_t> hist(n_problems * kHistStride, 0);
+    std::vector<DegenState> dg(d ? n_problems : 0);
+    uint32_t off = 0;
+    for (size_t b = 0; b < n_problems; ++b) {
+        so_icp_opts o{};
+        o.max_icp_iters = 1; o.lm_max_iterations = pr[b].lm_max_iterations <= 0 ? 4 : pr[b].lm_max_iterations;
+        o.use_pose_prior = pr[b].use_pose_prior; o.visual_confidence_factor = pr[b].visual_confidence_factor;
+        for (int a = 0; a < 3; ++a) o.prior_uncertainty[a] = pr[b].prior_uncertainty[a];
+        init_state(c->h_state[b], pr[b].pose, pr[b].n_rows, o);
+        std::memcpy(c->h_state[b].x0, pr[b].x0, sizeof(c->h_state[b].x0));      // the prior's measurement, apart from the start
+        c->h_offset[b] = off;
+        for (uint32_t i = 0; i < pr[b].n_rows; ++i) {
+            const so_solve_row& r = rows[off + i];
+            float4 p = make_float4(r.p[0], r.p[1], r.p[2], 0.f);
+            std::memcpy(&p.w, &i, 4);                             // the point's index inside its scan, as k_scan_gather writes it
+            sp[off + i] = p;
+            nd[off + i] = make_double4(r.n[0], r.n[1], r.n[2], r.d);
+            w[off + i] = r.w;
+        }
+        hist[b * kHistStride + 9] = int32_t(pr[b].n_rows);       // hist_rej[SUCCESS]: every row is accepted
+        if (d) dg[b] = degen_state(d[b]);
+        off += pr[b].n_rows;
+    }
+    cudaStream_t st = c->stream;
+    SO_CUDA_TRY(cudaMemcpyAsync(c->d_state, c->h_state, n_problems * sizeof(IcpState), cudaMemcpyHostToDevice, st));
+    SO_CUDA_TRY(cudaMemcpyAsync(c->d_offset, c->h_offset, n_problems * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+    SO_CUDA_TRY(cudaMemcpyAsync(c->d_hist, hist.data(), hist.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    if (total) {
+        SO_CUDA_TRY(cudaMemcpyAsync(c->d_scan_sorted, sp.data(), total * sizeof(float4), cudaMemcpyHostToDevice, st));
+        SO_CUDA_TRY(cudaMemcpyAsync(c->corr.nd, nd.data(), total * sizeof(double4), cudaMemcpyHostToDevice, st));
+        SO_CUDA_TRY(cudaMemcpyAsync(c->corr.w, w.data(), total * sizeof(double), cudaMemcpyHostToDevice, st));
+        SO_CUDA_TRY(cudaMemsetAsync(c->corr.flags, 0, total * sizeof(uchar4), st));
+    }
+    if (d) SO_CUDA_TRY(cudaMemcpyAsync(c->deg.d_st, dg.data(), n_problems * sizeof(DegenState), cudaMemcpyHostToDevice, st));
+    // the chunk's CTA count as register_core rounds it
+    uint32_t grid_x = (max_n + kThreads - 1) / kThreads;
+    if (grid_x) grid_x = std::min<uint32_t>(c->grid_x_cap, (grid_x + 15u) & ~15u);
+    BatchView bv = batch_view(c, c->d_scan_sorted);
+    if (fused_lm(c, uint32_t(n_problems), UndistortionMode::NONE, d != nullptr)) bv.counters = c->d_counters;
+    CorrBuf cb = c->corr;
+    cb.nn = nullptr; cb.nn_d2 = nullptr;
+    DegenState* const ddg = d ? c->deg.d_st : nullptr;
+    const uint32_t nb = uint32_t(n_problems);
+    timed_launch_begin(c);
+    launch_first_eval(bv, cb, grid_x, nb, st, nullptr, nullptr, 0, ddg);
+    timed_launch_end(c, 4);
+    SO_CUDA_TRY(cudaGetLastError());
+    std::vector<double> cost0(n_problems);                        // the cost IterationZero evaluated (the state's cost moves with the steps)
+    SO_CUDA_TRY(cudaMemcpyAsync(c->h_state, c->d_state, n_problems * sizeof(IcpState), cudaMemcpyDeviceToHost, st));
+    SO_CUDA_TRY(cudaStreamSynchronize(st));
+    for (size_t b = 0; b < n_problems; ++b) cost0[b] = c->h_state[b].cost;
+    for (int k = 0; k < lm; ++k) {
+        timed_launch_begin(c); launch_evaluate(bv, cb, grid_x, nb, st, nullptr, 0, ddg); timed_launch_end(c, 1);
+    }
+    SO_CUDA_TRY(cudaGetLastError());
+    SO_CUDA_TRY(cudaMemcpyAsync(c->h_state, c->d_state, n_problems * sizeof(IcpState), cudaMemcpyDeviceToHost, st));
+    if (d) SO_CUDA_TRY(cudaMemcpyAsync(dg.data(), c->deg.d_st, n_problems * sizeof(DegenState), cudaMemcpyDeviceToHost, st));
+    SO_CUDA_TRY(cudaStreamSynchronize(st));
+    for (size_t b = 0; b < n_problems; ++b) {
+        const IcpState& s = c->h_state[b];
+        so_solve_result& r = out[b];
+        std::memset(&r, 0, sizeof(r));
+        std::memcpy(r.pose, s.x, sizeof(r.pose));
+        r.initial_cost = cost0[b]; r.final_cost = s.cost;
+        r.lm_iterations = s.lm_iter; r.successful = s.num_successful; r.unsuccessful = s.num_unsuccessful; r.termination = s.termination;
+        r.radius = s.radius; r.decrease_factor = s.decrease_factor; r.gmax = s.gmax;
+        if (d) { r.n_flag_pos = dg[b].iter_n_flag_pos[0]; r.n_flag_ori = dg[b].iter_n_flag_ori[0]; }
+        r.status = s.status;
+    }
+    return SO_OK;
+}
+
 // ---- k-NN --------------------------------------------------------------------------------------------------------
 int so_knn_device(so_ctx* ctx, const void* d_q, size_t nq, int k, float max_d2, uint32_t* d_idx, float* d_d2) {
     Ctx* c = reinterpret_cast<Ctx*>(ctx);

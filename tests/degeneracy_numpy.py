@@ -61,74 +61,15 @@ def with_spectrum(rng, info_t, info_r, coupling=0.0, rot_t=None, rot_r=None):
 
 
 # ---------------------------------------------------------------------------------------------------------------- reduced solve
-def solve_reduced(prob, x0, B, max_iterations=4):
+def solve_reduced(prob, x0, B, max_iterations=4, full=False):
     """Ceres' trust-region LM (restated in tests/test_ceres_restatement.py) on prob with the local parameterisation x [+] B y:
     Jacobian J B, Jacobi scaling and LM diagonal over B's m columns, model cost change of the reduced step, gradient max-norm
     through Plus(x, -B B^T g); x_norm and the parameter / function tolerances ambient.
-    -> (x, iterations, successful_steps, unsuccessful_steps, termination) with the termination codes of that restatement."""
+    -> (x, iterations, successful_steps, unsuccessful_steps, termination) with the termination codes of that restatement; full: the
+    dict of test_ceres_restatement.solve_full (costs, the final radius, decrease factor and gradient max-norm, decision margins)."""
     import test_ceres_restatement as CR
-    x = np.array(x0, float)
-    m = B.shape[1]
-    cost, res, J = prob.linearise(x)
-    Jr = J @ B
-    scale = 1.0 / (1.0 + np.linalg.norm(Jr, axis=0))
-    Js = Jr * scale
-
-    def gmax_of(xx, JJ, rr):
-        return np.abs(xx - CR._plus(xx, -(B @ (B.T @ (JJ.T @ rr))))).max()
-    gmax = gmax_of(x, J, res)
-    radius, decrease, reuse = 1e4, 2.0, False
-    diag = None
-    it = succ = unsucc = invalid = 0
-    step_ok = False
-    while True:
-        if step_ok:
-            succ += 1
-        else:
-            unsucc += 1
-        if it >= max_iterations:
-            return x, it, succ, unsucc, 0
-        if gmax <= CR.GRADIENT_TOL:
-            return x, it, succ, unsucc, 1
-        if radius <= CR.MIN_RADIUS:
-            return x, it, succ, unsucc, 4
-        it += 1
-        step_ok = False
-        if not reuse:
-            diag = np.clip((Js * Js).sum(0), CR.MIN_LM_DIAG, CR.MAX_LM_DIAG)
-        reuse = True
-        A = np.concatenate([Js, np.diag(np.sqrt(diag / radius))], 0)
-        b = np.concatenate([res, np.zeros(m)])
-        step = -np.linalg.lstsq(A, b, rcond=None)[0]
-        mr = Js @ step
-        model_change = -(mr * (res + mr / 2.0)).sum()
-        if not (np.isfinite(step).all() and model_change > 0.0):
-            invalid += 1
-            if invalid >= 5:
-                return x, it, succ, unsucc, 5
-            radius *= 0.5
-            continue
-        invalid = 0
-        cand = CR._plus(x, B @ (step * scale))
-        cand_cost = prob.cost(cand)
-        if np.linalg.norm(x - cand) <= CR.PARAMETER_TOL * (np.linalg.norm(x) + CR.PARAMETER_TOL):
-            return x, it, succ, unsucc, 2
-        change = cost - cand_cost
-        if abs(change) <= CR.FUNCTION_TOL * cost:
-            return x, it, succ, unsucc, 3
-        rel = change / model_change
-        if rel > CR.MIN_REL_DECREASE:
-            x = cand
-            cost, res, J = prob.linearise(x)
-            Js = (J @ B) * scale
-            gmax = gmax_of(x, J, res)
-            step_ok = True
-            radius = min(CR.MAX_RADIUS, radius / max(1.0 / 3.0, 1.0 - (2.0 * rel - 1.0) ** 3))
-            decrease, reuse = 2.0, False
-        else:
-            radius /= decrease
-            decrease *= 2.0
-            reuse = True
+    r = CR.solve_full(prob, x0, max_iterations, B=B)
+    return r if full else (r["x"], r["iterations"], r["successful"], r["unsuccessful"], r["termination"])
 
 
 def register(ctx, scan, x0, pos_threshold, ori_threshold, iters, mf, a2, lm=4, constrain=1):

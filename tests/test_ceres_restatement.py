@@ -36,10 +36,13 @@ def _plus(x, d):              # PoseLocalParameterization::Plus (pose_local_para
 
 
 class Problem:
-    """n point-to-plane blocks {p, n, d, w} under ScaledLoss(TukeyLoss(a), w) (LidarSlam.cpp:268-274)."""
+    """n point-to-plane blocks {p, n, d, w} under ScaledLoss(TukeyLoss(a), w) (LidarSlam.cpp:268-274), and optionally the 6 rows of
+    SE3AbsolutatePoseFactor (factor/SE3AbsolutatePoseFactor.cpp: [p - p_m ; 2 vec(q_m^* q)] times a diagonal sqrt-information, no
+    loss), prior = (measurement pose7, sqrt_info[6]) as prior_sqrt_info gives it."""
 
-    def __init__(self, P, N, D, W, a2):
+    def __init__(self, P, N, D, W, a2, prior=None):
         self.P, self.N, self.D, self.W, self.a2 = P, N, D, W, a2
+        self.prior = prior
 
     def _residuals(self, x):
         R = _rot(x[3:])
@@ -52,9 +55,25 @@ class Problem:
         rho1 = np.where(inside, 0.5 * v * v, 0.0) * self.W
         return rho0, rho1
 
+    def _prior_rows(self, x):
+        """residual [6] and local Jacobian [6, 6] of the prior rows: d(2 vec(e))/d(dtheta) = w I + [v]x of e = q_m^* q
+        (Utility::Qleft's bottom-right block)."""
+        meas, si = self.prior
+        qm = np.array([-meas[3], -meas[4], -meas[5], meas[6]])
+        e = _qmul(qm, x[3:])
+        r = np.concatenate([x[:3] - meas[:3], 2.0 * e[:3]])
+        ex, ey, ez, ew = e
+        J = np.zeros((6, 6))
+        J[:3, :3] = np.eye(3)
+        J[3:, 3:] = [[ew, -ez, ey], [ez, ew, -ex], [-ey, ex, ew]]
+        return r * si, J * si[:, None]
+
     def cost(self, x):
         r, _ = self._residuals(x)
-        return 0.5 * self._rho(r * r)[0].sum()
+        c = 0.5 * self._rho(r * r)[0].sum()
+        if self.prior is not None:
+            c += 0.5 * (self._prior_rows(x)[0] ** 2).sum()
+        return c
 
     def linearise(self, x):
         """cost, corrected residuals, corrected local Jacobian [n, 6] (Corrector with rho'' <= 0: both scaled by sqrt(rho'))."""
@@ -63,73 +82,135 @@ class Problem:
         a = self.N @ R                                     # rows: R^T n
         J = np.concatenate([self.N, np.cross(self.P, a)], 1)      # [n^T, -n^T R [p]x] = [n, p x (R^T n)]
         sc = np.sqrt(rho1)
-        return 0.5 * rho0.sum(), r * sc, J * sc[:, None]
+        cost, res, J = 0.5 * rho0.sum(), r * sc, J * sc[:, None]
+        if self.prior is not None:
+            rp, Jp = self._prior_rows(x)
+            cost, res, J = cost + 0.5 * (rp * rp).sum(), np.concatenate([res, rp]), np.concatenate([J, Jp])
+        return cost, res, J
 
 
-def solve(prob, x0, max_iterations=4):
-    """-> (x, iterations, successful_steps, unsuccessful_steps, termination)  termination codes as oracle/so_oracle.cpp."""
+def prior_sqrt_info(n_ok, prior_uncertainty, visual_confidence_factor):
+    """addAbsolutePoseConstraints' information diagonal (LidarSlam.cpp:287-294) from the number of accepted correspondences, with the
+    float inputs widened as the device widens them, and its square root by Eigen's unblocked LLT: the first non-positive pivot and
+    everything after it stay as they are (the yaw weight is 0, so yaw is never square-rooted)."""
+    vcf = float(np.float32(visual_confidence_factor))
+    m1, m2 = max(50, int(n_ok * 0.1)), max(10, int(n_ok * 0.01))
+    info = [(1 - float(np.float32(u))) * m1 * vcf for u in prior_uncertainty] + [m2 * vcf, m2 * vcf, max(5, int(n_ok * 0.001)) * 0]
+    out, failed = np.zeros(6), False
+    for k in range(6):
+        failed = failed or info[k] <= 0.0
+        out[k] = info[k] if failed else np.sqrt(info[k])
+    return out
+
+
+def _rel_margin(value, threshold):
+    """How far a decision `value <= threshold` (or `>`) is from flipping, relative to the threshold."""
+    return abs(value - threshold) / abs(threshold) if threshold != 0.0 else (np.inf if value != 0.0 else 0.0)
+
+
+def solve_full(prob, x0, max_iterations=4, B=None):
+    """Ceres' trust-region LM on prob from x0; B (6 x m, optional): the solve on B's columns, local parameterisation x [+] B y
+    (Jacobian J B, Jacobi scaling and LM diagonal over the m columns, gradient max-norm through Plus(x, -B B^T g); x_norm and the
+    parameter / function tolerances ambient).  -> dict: x, iterations, successful, unsuccessful, termination (codes as
+    oracle/so_oracle.cpp), initial_cost, final_cost, and the trust-region state the solve ends in (radius, decrease_factor, gmax);
+    steps: 'a' accepted / 'r' rejected / 'i' invalid per LM iteration; margin: the smallest relative distance of any decision the
+    solve took from its threshold (gradient, radius, parameter and function tolerances, step quality, model cost change);
+    radius_error: an estimate of the relative error of the final radius that rounding alone leaves.  A step is only known to about
+    cond x machine epsilon (cond: of the damped least-squares system it is solved from), and so is the model cost change; the cost
+    change is a difference of sums rounded at the scale of the initial cost.  Both carry into the step quality rd, and every accepted
+    step multiplies the radius by 1 / max(1/3, 1 - (2 rd - 1)^3), whose relative sensitivity to rd is summed over the steps."""
+    B = np.eye(6) if B is None else np.asarray(B, float)
+    m = B.shape[1]
     x = np.array(x0, float)
     cost, res, J = prob.linearise(x)
-    scale = 1.0 / (1.0 + np.linalg.norm(J, axis=0))        # Jacobi scaling, fixed at iteration 0
-    Js = J * scale
-    g = J.T @ res
+    initial_cost = cost
+    Jr = J @ B
+    scale = 1.0 / (1.0 + np.linalg.norm(Jr, axis=0))       # Jacobi scaling, fixed at iteration 0
+    Js = Jr * scale
 
-    def gmax_of(xx, gg):
-        return np.abs(xx - _plus(xx, -gg)).max()
-    gmax = gmax_of(x, g)
+    def gmax_of(xx, JJ, rr):
+        return np.abs(xx - _plus(xx, -(B @ (B.T @ (JJ.T @ rr))))).max()
+    gmax = gmax_of(x, J, res)
     radius, decrease, reuse = 1e4, 2.0, False
     diag = None
     it = succ = unsucc = invalid = 0
     step_ok = False
+    steps, margins = [], []
+    eps, radius_error = np.finfo(float).eps, 0.0
+
+    def done(term):
+        return dict(x=x, iterations=it, successful=succ, unsuccessful=unsucc, termination=term, initial_cost=initial_cost,
+                    final_cost=cost, radius=radius, decrease_factor=decrease, gmax=gmax, steps="".join(steps),
+                    margin=min(margins) if margins else np.inf, radius_error=radius_error)
     while True:
         if step_ok:
             succ += 1
         else:
             unsucc += 1
         if it >= max_iterations:
-            return x, it, succ, unsucc, 0
+            return done(0)
+        margins.append(_rel_margin(gmax, GRADIENT_TOL))
         if gmax <= GRADIENT_TOL:
-            return x, it, succ, unsucc, 1
+            return done(1)
+        margins.append(_rel_margin(radius, MIN_RADIUS))
         if radius <= MIN_RADIUS:
-            return x, it, succ, unsucc, 4
+            return done(4)
         it += 1
         step_ok = False
         if not reuse:
             diag = np.clip((Js * Js).sum(0), MIN_LM_DIAG, MAX_LM_DIAG)
         reuse = True
         A = np.concatenate([Js, np.diag(np.sqrt(diag / radius))], 0)
-        b = np.concatenate([res, np.zeros(6)])
-        y = np.linalg.lstsq(A, b, rcond=None)[0]
-        step = -y
+        b = np.concatenate([res, np.zeros(m)])
+        step = -np.linalg.lstsq(A, b, rcond=None)[0]
+        cond = np.linalg.cond(A)
         mr = Js @ step
         model_change = -(mr * (res + mr / 2.0)).sum()
+        if np.isfinite(step).all():
+            margins.append(abs(model_change) / max(abs(mr * res).sum() + 0.5 * (mr * mr).sum(), np.finfo(float).tiny))
         if not (np.isfinite(step).all() and model_change > 0.0):
+            steps.append("i")
             invalid += 1
             if invalid >= 5:
-                return x, it, succ, unsucc, 5
+                return done(5)
             radius *= 0.5
             continue
         invalid = 0
-        cand = _plus(x, step * scale)
+        cand = _plus(x, B @ (step * scale))
         cand_cost = prob.cost(cand)
-        if np.linalg.norm(x - cand) <= PARAMETER_TOL * (np.linalg.norm(x) + PARAMETER_TOL):
-            return x, it, succ, unsucc, 2
+        sn, tol = np.linalg.norm(x - cand), PARAMETER_TOL * (np.linalg.norm(x) + PARAMETER_TOL)
+        margins.append(_rel_margin(sn, tol))
+        if sn <= tol:
+            return done(2)
         change = cost - cand_cost
+        margins.append(_rel_margin(abs(change), FUNCTION_TOL * cost))
         if abs(change) <= FUNCTION_TOL * cost:
-            return x, it, succ, unsucc, 3
+            return done(3)
         rel = change / model_change
+        margins.append(_rel_margin(rel, MIN_REL_DECREASE))
         if rel > MIN_REL_DECREASE:
+            steps.append("a")
+            t = 2.0 * rel - 1.0
+            if 1.0 - t ** 3 > 1.0 / 3.0 and radius / (1.0 - t ** 3) < MAX_RADIUS:      # d ln(factor) / d ln(rd), 0 where capped
+                radius_error += abs(6.0 * t * t * rel / (1.0 - t ** 3)) * (cond * eps + eps * initial_cost / abs(change))
             x = cand
             cost, res, J = prob.linearise(x)
-            Js = J * scale
-            gmax = gmax_of(x, J.T @ res)
+            Js = (J @ B) * scale
+            gmax = gmax_of(x, J, res)
             step_ok = True
             radius = min(MAX_RADIUS, radius / max(1.0 / 3.0, 1.0 - (2.0 * rel - 1.0) ** 3))
             decrease, reuse = 2.0, False
         else:
+            steps.append("r")
             radius /= decrease
             decrease *= 2.0
             reuse = True
+
+
+def solve(prob, x0, max_iterations=4):
+    """-> (x, iterations, successful_steps, unsuccessful_steps, termination)  termination codes as oracle/so_oracle.cpp."""
+    r = solve_full(prob, x0, max_iterations)
+    return r["x"], r["iterations"], r["successful"], r["unsuccessful"], r["termination"]
 
 
 def _random_problem(rng, n):
@@ -172,5 +253,5 @@ def test_numpy_and_cpp_restatements_of_the_ceres_solve_agree():
             seen_terms.add(term)
             seen_unsucc += unsucc > 1
     # the sample exercises the max-iterations exit and the function / parameter tolerance exits (rejected steps do not occur with this
-    # bounded loss from any start tried here: the rejection branch is only cross-read, not cross-run)
+    # bounded loss from these starts; tests/test_trust_region_cpu.py runs the rejection branch on problem families that reach it)
     assert {0, 2, 3} <= seen_terms, (seen_terms, seen_unsucc)
