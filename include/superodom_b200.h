@@ -236,6 +236,49 @@ int so_map_archive_info(so_ctx* ctx, int store, size_t* n_points, size_t* n_bloc
  * loaded with so_map_set_points, it is the next session's prior map. */
 int so_map_download_all(so_ctx* ctx, int store, float* out_xyzi, size_t cap_points, size_t* n_out);
 
+/* ---- free-space clearing: take out the map points a scan sees through (moving objects) ---------------------------------------
+ * No reference counterpart (LocalMap::addSurfPointCloud only adds points).  Off unless called; nothing else calls it.
+ * Rule (DESIGN.md §2): the scan, in the frame of pose with the sensor at the pose's origin, is projected to a range image in FP64 --
+ * column floor((az + pi) / az_res), az = atan2(y, x) in [-pi, pi), W = ceil(360 / az_res_deg) columns that wrap; row
+ * floor((el - el_min) / el_res), el = atan2(z, hypot(x, y)), points with el outside [el_min, el_max) left out -- and each pixel keeps
+ * the minimum float range of its finite points with r > 0.  A window map point m, at q = R^T (m - t) (FP64, quaternion normalised),
+ * range r_m, is a candidate when min_range <= r_m <= max_range, its (2 dilate + 1)^2 pixel neighbourhood lies inside the elevation
+ * span and every pixel of it has a return; it is removed when the neighbourhood minimum exceeds r_m + max(margin, margin_rel r_m).
+ * Pixels without a return never remove anything, and a point behind something the scan saw is never removed.
+ * Removal keeps the order of the points left (a block's k-NN tie-break and voxel-filter order) and rebuilds the index; when nothing
+ * is removed the store is left bit for bit as it was.  With the block archive on only the window is carved. */
+typedef struct {
+    float az_res_deg, el_res_deg;   /* pixel size; el_res at least the sensor's beam spacing (VLP-16 2.0, OS1-128 0.4) */
+    float el_min_deg, el_max_deg;   /* elevation span of the image */
+    int32_t dilate;                 /* neighbourhood half-width in pixels, 0..4 (default 2: 5x5) */
+    float margin, margin_rel;       /* metres, fraction of range */
+    float min_range, max_range;     /* map points considered (sensor distance, metres) */
+} so_free_space;
+typedef struct {
+    uint64_t n_image_points;        /* scan points that went into the range image */
+    uint64_t n_pixels_hit;          /* pixels with a return */
+    uint64_t n_candidates;          /* map points tested against a fully observed neighbourhood, over the stores carved */
+    uint64_t n_removed;             /* map points removed, over the stores carved */
+    uint64_t n_after[2];            /* points in the surf and the edge window afterwards */
+} so_free_space_result;
+/* The defaults: the OS1-128 image geometry (az_res 0.4, el_res 0.4, el span [-23, 23]), dilate 2, margin 0.3 m, margin_rel 0.02,
+ * ranges [0.5, 60] m.  Set el_res and the span for the sensor at hand (VLP-16: el_res 2, span [-16, 16]). */
+void so_free_space_defaults(so_free_space* opts);
+/* Clear the map against a host cloud in the frame of pose (already motion-compensated if it needs it); stores: bit 0 surf, bit 1 edge.
+ * One range image per call serves every store selected.  SO_ERR_ARG before any device work, both stores as they were: NULL opts or
+ * pose, a pose that is not finite, a NULL cloud with n > 0, a resolution that is not finite or not positive, el_max <= el_min (or not
+ * finite), W * H > 2^24, dilate outside 0..4, a negative or non-finite margin, min_range >= max_range, stores outside 1..3.
+ * SO_ERR_CAPACITY: n > max_scan_points.  A pending origin or resolution change is applied first; an unbuilt store returns its error.
+ * result may be NULL. */
+int so_map_clear_free_space(so_ctx* ctx, int stores, const void* xyzi, size_t n, size_t stride_bytes, size_t intensity_offset,
+                            const double pose[7], const so_free_space* opts, so_free_space_result* result);
+/* The same against the surf cloud of the last single-scan registration, exactly as so_map_add_registered_scan(pose) would insert it
+ * (compensated under APPROXIMATED / OPTIMIZED), without uploading it again: it is placed in the surf store's tail as the insert
+ * places it.  The registration's record stays valid, so the insert can follow.  Fails as so_map_add_registered_scan does for a missing
+ * or overwritten record (SO_ERR_ARG), and with SO_ERR_CAPACITY when the scan does not fit behind the surf window; SO_OK and nothing
+ * removed before the first registration. */
+int so_map_clear_free_space_registered(so_ctx* ctx, int stores, const double pose[7], const so_free_space* opts, so_free_space_result* result);
+
 /* ---- scan pre-filter (the step right before the path; SURVEY 8f row 2) ------------------------------------------ */
 /* replaces: laserMapping::adjustVoxelSize (src/LaserMapping/laserMapping.cpp:600-651) for the surf cloud: with
  * auto_voxel_size, pick config_.lineRes/planeRes from the scan statistics (mean|x| * mean|y| * mean|z| < 25 -> 0.1/0.2,
@@ -685,7 +728,7 @@ uint64_t so_kernel_launches(so_ctx* ctx, int reset);
 int so_bytes_copied(so_ctx* ctx, uint64_t* h2d, uint64_t* d2h, int reset);
 /* Accumulated device time (ms, CUDA events on the context stream) and launch count of a kernel class since the last
  * reset; classes: 0 k_knn_scan (scan k-NN), 1 k_evaluate +
- * k_lm_step (LM step), 2 k_knn (so_knn*), 3 scan ordering / map build / map insert / scan preparation (pre-filter, deskew, uniform and edge extraction), 4 first evaluation of
+ * k_lm_step (LM step), 2 k_knn (so_knn*), 3 scan ordering / map build / map insert / free-space clearing / scan preparation (pre-filter, deskew, uniform and edge extraction), 4 first evaluation of
  * a solve (k_evaluate + k_lm_step iteration zero), 5 k_fit (plane fit), 6 global localization search (bitmap raster, dilation,
  * hypothesis scoring, key sort; for the branch-and-bound also map bounds, pyramid levels, offset table and traversal steps),
  * 7 k_undistort (within-scan motion compensation: per ICP iteration, and the undistorted map insert / so_undistort_points; the

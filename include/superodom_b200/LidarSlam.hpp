@@ -195,6 +195,21 @@ public:
         if (ctx_->h) { so_map_archive_info(ctx_->h, 0, &s, nullptr, nullptr); so_map_archive_info(ctx_->h, 1, &e, nullptr, nullptr); }
         return s + e;
     }
+    // Shim only, no reference counterpart: remove the map points the sensor-frame cloud (at pose) saw clearly past, e.g. what a moving
+    // object left (so_map_clear_free_space; stores: 1 surf, 2 edge, 3 both).  Give it the full-resolution cloud: it leaves fewer
+    // pixels without a return near the sensor than the voxel-filtered surf stack.
+    template <class Cloud> so_free_space_result clearFreeSpace(const Cloud& cloud, const Transformd& pose, const so_free_space& opts, int stores = 3) {
+        sync_resolution();
+        size_t stride, ioff;
+        point_layout<typename std::decay<decltype(cloud.points[0])>::type>(&stride, &ioff);
+        double p[7];
+        pose.to_pose7(p);
+        so_free_space_result r{};
+        check(so_map_clear_free_space(ctx_->h, stores, cloud.size() ? cloud.points.data() : nullptr, cloud.size(), stride, ioff, p, &opts, &r),
+              "so_map_clear_free_space");
+        return r;
+    }
+    static so_free_space defaultFreeSpace() { so_free_space o{}; so_free_space_defaults(&o); return o; }
     // The whole surf map, window plus archive, ordered by world block (so_map_download_all): a session's map as the next one's prior map
     template <class Cloud> Cloud getWholeMap() {
         sync_resolution();
@@ -296,6 +311,11 @@ public:
     Transformd undistort_prev_pose;                              // pose of the previous scan (last_T_w_lidar is the prior by then)
     bool undistort_has_prev = false;
     so_icp_result last_result{};                                 // everything the device reported for the last scan
+    // shim only: before its inserts, Localization removes from both stores the map points the registered scan saw clearly past
+    // (so_map_clear_free_space_registered with FreeSpaceOpts; set its image geometry for the sensor).  Off by default.
+    bool ClearFreeSpace = false;
+    so_free_space FreeSpaceOpts = LocalMap::defaultFreeSpace();
+    so_free_space_result last_free_space{};                      // ClearFreeSpace: what the last clearing removed
 
     explicit LidarSLAM(int device = 0, uint32_t max_map_points = 0, uint32_t max_scan_points = 0) : localMap(&context) {
         context.cfg.device = device; context.cfg.max_map_points = max_map_points; context.cfg.max_scan_points = max_scan_points;
@@ -413,6 +433,8 @@ public:
         stats.n_iterations = r.n_iterations;
         last_T_w_lidar = T_w_lidar;
         // checkMotionThresholds always accepts (:193) -> transformAndAddToMap (:163-167)
+        if (ClearFreeSpace && planner_point->size())
+            check(so_map_clear_free_space_registered(context.h, 3, r.pose, &FreeSpaceOpts, &last_free_space), "so_map_clear_free_space_registered");
         if (edges_registered) check(so_map_add_registered_edges(context.h, r.pose), "so_map_add_registered_edges");    // compensated, at r.pose
         else if (has_edges) check(so_map_add_scan_edge(context.h, edge_point->points.data(), edge_point->size(), stride, ioff, r.pose), "so_map_add_scan_edge");
         if (planner_point->size()) check(so_map_add_registered_scan(context.h, r.pose), "so_map_add_registered_scan");   // the scan is still on the device

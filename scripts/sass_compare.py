@@ -22,6 +22,8 @@ CUDA = os.environ.get("CUDA_HOME", "/usr/local/cuda")
 def cubins(tree, out):
     procs = []
     for src in SOURCES:
+        if not os.path.exists(os.path.join(tree, "superodom_b200", "csrc", src)):      # a source REV does not have yet
+            continue
         cmd = [os.path.join(CUDA, "bin", "nvcc"), *[f for f in NVCC_FLAGS if f not in ("-Xcompiler", "-fPIC")], "-cubin",
                os.path.join(tree, "superodom_b200", "csrc", src), "-o", os.path.join(out, src.replace(".cu", ".cubin"))]
         procs.append(subprocess.Popen(cmd))
@@ -55,6 +57,9 @@ def main():
         bad = 0
         for src in SOURCES:
             name = src.replace(".cu", ".cubin")
+            if not os.path.exists(os.path.join(old_out, name)):
+                print(f"{src}: new source, functions {sorted(functions(os.path.join(new_out, name)))}")
+                continue
             old, new = functions(os.path.join(old_out, name)), functions(os.path.join(new_out, name))
             for f, body in old.items():
                 if new.get(f) != body:

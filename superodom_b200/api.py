@@ -21,6 +21,7 @@ EXPORTS = [
     "so_map_set_resolution", "so_map_set_origin", "so_map_get_origin", "so_map_shift", "so_map_set_points",
     "so_map_set_edge_points", "so_map_add_surf", "so_map_add_edge", "so_map_add_scan", "so_map_add_registered_scan", "so_map_add_registered_edges", "so_map_add_scan_edge", "so_map_counts_5x5", "so_map_download", "so_map_size",
     "so_map_archive", "so_map_archive_info", "so_map_download_all",
+    "so_free_space_defaults", "so_map_clear_free_space", "so_map_clear_free_space_registered",
     "so_scan_prefilter", "so_scan_deskew", "so_scan_extract_uniform", "so_scan_extract_edges", "so_register", "so_register_prefiltered", "so_register_injected", "so_set_pose_sink", "so_register_batch", "so_register_batch_edges", "so_register_batch_device",
     "so_register_undistort", "so_register_undistort_edges", "so_register_prefiltered_undistort", "so_register_batch_undistort", "so_undistort_points", "so_register_optimized", "so_register_optimized_edges", "so_register_prefiltered_optimized", "so_register_batch_optimized", "so_evaluate_optimized", "so_evaluate_optimized_edges", "so_correspond", "so_correspond_seeded", "so_ordered_scans", "so_correspond_edge", "so_evaluate", "so_covariance",
     "so_register_degeneracy", "so_register_batch_degeneracy", "so_degeneracy_analysis", "so_solve",
@@ -147,6 +148,28 @@ def whole_map_opts(map_lo, map_hi, center_pose7, **kw) -> GlobalOpts:
     return global_opts(half_x=hx, half_y=hy, **kw)
 
 
+class FreeSpace(C.Structure):
+    """so_free_space: range-image geometry (degrees) and decision constants of free-space clearing."""
+    _fields_ = [("az_res_deg", C.c_float), ("el_res_deg", C.c_float), ("el_min_deg", C.c_float), ("el_max_deg", C.c_float),
+                ("dilate", C.c_int32), ("margin", C.c_float), ("margin_rel", C.c_float), ("min_range", C.c_float), ("max_range", C.c_float)]
+
+
+class FreeSpaceResult(C.Structure):
+    _fields_ = [("n_image_points", C.c_uint64), ("n_pixels_hit", C.c_uint64), ("n_candidates", C.c_uint64), ("n_removed", C.c_uint64),
+                ("n_after", C.c_uint64 * 2)]
+
+
+def free_space(**kw) -> FreeSpace:
+    """so_free_space_defaults, then the given fields (e.g. el_res_deg=2.0, el_min_deg=-16, el_max_deg=16 for a VLP-16)."""
+    o = FreeSpace()
+    load_library().so_free_space_defaults(C.byref(o))
+    for k, v in kw.items():
+        if not hasattr(o, k):
+            raise TypeError(f"so_free_space has no field {k}")
+        setattr(o, k, v)
+    return o
+
+
 class EdgeOpts(C.Structure):
     """so_edge_opts: zero fields take the defaults (min_range 0, edge_threshold 0.1, voxel_leaf 0 = no filter, max_per_sector 20)."""
     _fields_ = [("min_range", C.c_float), ("edge_threshold", C.c_float), ("voxel_leaf", C.c_float), ("max_per_sector", C.c_int32)]
@@ -204,6 +227,11 @@ def load_library():
     L.so_map_archive.argtypes = [C.c_void_p, C.c_size_t]
     L.so_map_archive_info.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
     L.so_map_download_all.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p]
+    L.so_free_space_defaults.restype = None
+    L.so_free_space_defaults.argtypes = [C.c_void_p]
+    L.so_map_clear_free_space.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p, C.c_void_p,
+                                          C.c_void_p]
+    L.so_map_clear_free_space_registered.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
     L.so_scan_prefilter.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_int, C.c_void_p, C.c_void_p,
                                     C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
     L.so_scan_deskew.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_double, C.c_void_p, C.c_void_p, C.c_size_t,
@@ -479,6 +507,32 @@ class Context:
             out = np.zeros((cap, 4), np.float32)
             self._chk(self.L.so_map_download_all(self.h, store, _p(out), cap, C.byref(n)), "so_map_download_all")
         return out[: n.value]
+
+    # ---- free-space clearing (off unless called)
+    @staticmethod
+    def _free_result(r: FreeSpaceResult) -> dict:
+        return dict(n_image_points=r.n_image_points, n_pixels_hit=r.n_pixels_hit, n_candidates=r.n_candidates, n_removed=r.n_removed,
+                    n_after=(r.n_after[0], r.n_after[1]))
+
+    def map_clear_free_space(self, scan_xyzi: np.ndarray, pose7, opts: FreeSpace | None = None, stores: int = 1) -> dict:
+        """Remove the window map points that the sensor-frame scan (at pose7) saw clearly past; stores: 1 surf, 2 edge, 3 both."""
+        a = np.ascontiguousarray(scan_xyzi, dtype=np.float32)
+        pose = np.ascontiguousarray(pose7, dtype=np.float64)
+        o = opts if opts is not None else free_space()
+        r = FreeSpaceResult()
+        stride = a.shape[1] * 4
+        self._chk(self.L.so_map_clear_free_space(self.h, int(stores), _p(a), a.shape[0], stride, 12 if a.shape[1] >= 4 else stride, _p(pose),
+                                                 C.byref(o), C.byref(r)), "so_map_clear_free_space")
+        return self._free_result(r)
+
+    def map_clear_free_space_registered(self, pose7, opts: FreeSpace | None = None, stores: int = 1) -> dict:
+        """The same against the scan last passed to a single-scan register*(), as map_add_registered_scan(pose7) would insert it."""
+        pose = np.ascontiguousarray(pose7, dtype=np.float64)
+        o = opts if opts is not None else free_space()
+        r = FreeSpaceResult()
+        self._chk(self.L.so_map_clear_free_space_registered(self.h, int(stores), _p(pose), C.byref(o), C.byref(r)),
+                  "so_map_clear_free_space_registered")
+        return self._free_result(r)
 
     # ---- scan pre-filter
     def scan_prefilter(self, scan_xyzi: np.ndarray, line_res: float, plane_res: float, auto_voxel_size: bool = True, download: bool = True):

@@ -177,6 +177,7 @@ static void ctx_free(Ctx* c) {
     motion_free(c);
     cudaFree(c->deg.d_st);
     features_free(c);
+    free_space_free(c);
     if (c->ev_dec) cudaEventDestroy(c->ev_dec);
     if (c->ev0) cudaEventDestroy(c->ev0);
     if (c->ev1) cudaEventDestroy(c->ev1);
@@ -1034,6 +1035,41 @@ int so_map_add_scan_edge(so_ctx* ctx, const void* xyzi, size_t n, size_t stride,
     Ctx* c = reinterpret_cast<Ctx*>(ctx);
     if (!pose || (!xyzi && n)) return fail(SO_ERR_ARG, "bad args");
     return c ? store_add(c, c->edge, xyzi, n, stride, ioff, pose) : fail(SO_ERR_ARG, "null ctx");
+}
+
+void so_free_space_defaults(so_free_space* opts) { if (opts) free_space_defaults(opts); }
+
+int so_map_clear_free_space(so_ctx* ctx, int stores, const void* xyzi, size_t n, size_t stride, size_t ioff, const double pose[7],
+                            const so_free_space* opts, so_free_space_result* result) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c || (!xyzi && n) || stride < 12) return fail(SO_ERR_ARG, "bad args");
+    { int rc = free_space_check(opts, stores, pose); if (rc) return rc; }
+    if (n > c->cfg.max_scan_points) return fail(SO_ERR_CAPACITY, "so_map_clear_free_space: cloud larger than so_config.max_scan_points");
+    SO_CUDA_TRY(cudaSetDevice(c->device));
+    int rc = free_space_prepare(c, stores);
+    if (!rc) rc = free_space_reserve_points(c, n);
+    if (!rc) rc = upload_cloud(c, xyzi, n, stride, ioff, c->fs.d_pts);
+    return rc ? rc : free_space_clear(c, stores, c->fs.d_pts, uint32_t(n), pose, *opts, result);
+}
+
+// The image comes from the surf store's tail, where put_registered_scan leaves the scan as so_map_add_registered_scan would insert it
+// (before the transform to the world frame); d_scan, the times and the record are only read
+int so_map_clear_free_space_registered(so_ctx* ctx, int stores, const double pose[7], const so_free_space* opts, so_free_space_result* result) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c) return fail(SO_ERR_ARG, "null ctx");
+    { int rc = free_space_check(opts, stores, pose); if (rc) return rc; }
+    if (!c->reg.valid) return fail(SO_ERR_ARG, "so_map_clear_free_space_registered needs a preceding single-scan so_register* (and nothing that reuses the scan buffers in between)");
+    SO_CUDA_TRY(cudaSetDevice(c->device));
+    if (c->reg.n == 0) {
+        if (result) { *result = so_free_space_result{}; result->n_after[0] = c->surf.n; result->n_after[1] = c->edge.n; }
+        return SO_OK;
+    }
+    int rc = free_space_prepare(c, stores | 1);
+    if (rc) return rc;
+    MapStore& ms = c->surf;
+    if (size_t(ms.n) + c->reg.n > c->cfg.max_map_points) return fail(SO_ERR_CAPACITY, "map + registered scan exceed so_config.max_map_points");
+    rc = put_registered_scan(c, ms, pose);
+    return rc ? rc : free_space_clear(c, stores, ms.d_xyzi + ms.n, c->reg.n, pose, *opts, result);
 }
 
 int so_map_counts_5x5(so_ctx* ctx, const int32_t ijk[3], int32_t* n_edge, int32_t* n_surf) {

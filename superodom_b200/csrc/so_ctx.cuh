@@ -291,6 +291,14 @@ struct Ctx {
         uint32_t* d_ring = nullptr;                                        // [65536] first position, [65536] end, [65536] ring list, [4] control
     } feat;
 
+    // ---- free-space clearing (so_map_clear_free_space*, so_free.cu): allocated on first use, grown on demand ---------------------
+    struct FreeSpace {
+        uint32_t* d_img = nullptr; size_t img_cap = 0;                     // range image: float bits of the minimum range per pixel
+        float4* d_pts = nullptr; size_t pts_cap = 0;                       // the host form's cloud
+        uint8_t* d_keep = nullptr; size_t keep_cap = 0;                    // [2][max_map_points] keep flags of the surf and edge windows
+        struct FreeCounters* d_cnt = nullptr; struct FreeCounters* h_cnt = nullptr;   // counters of one call (pinned mirror)
+    } fs;
+
     // ---- instrumentation ----------------------------------------------------------------------------------------
     uint64_t launches = 0;
     uint64_t bytes_h2d = 0, bytes_d2h = 0;         // host<->device bytes moved by registration / k-NN calls
@@ -372,6 +380,17 @@ int scan_voxel_filter(Ctx* c, uint32_t n, float leaf, uint32_t* n_out);   // d_s
 // The same filter on any packed cloud in[0..n) -> out, with the caller's sort buffers (keys: 2n words of head scratch after the sort)
 struct VoxelBufs { uint64_t* keys; uint64_t* keys_out; uint32_t* vals; uint32_t* vals_out; void* tmp; size_t tmp_bytes; };
 int cloud_voxel_filter(Ctx* c, const float4* in, uint32_t n, float leaf, const VoxelBufs& b, float4* out, uint32_t* n_out);
+// Removal of the points whose keep flag is 0 from the built store ms (stable), then its index: n_keep points are left
+int map_compact(Ctx* c, MapStore& ms, const uint8_t* keep, uint32_t n_keep, uint32_t* d_num_selected);
+// so_free.cu (free-space clearing)
+void free_space_defaults(so_free_space* o);
+int free_space_check(const so_free_space* o, int stores, const double pose[7]);   // SO_ERR_ARG cases of so_map_clear_free_space*
+int free_space_prepare(Ctx* c, int stores);                 // rebuild the selected stores that are dirty
+int free_space_reserve_points(Ctx* c, size_t n);            // Ctx::fs.d_pts for a host cloud of n points
+void free_space_free(Ctx* c);
+// The range image of d_pts[0..n_pts) (sensor frame at pose), then every selected store carved against it; the stores are built
+int free_space_clear(Ctx* c, int stores, const float4* d_pts, uint32_t n_pts, const double pose[7], const so_free_space& o,
+                     so_free_space_result* out);
 // so_features.cu
 void features_free(Ctx* c);                                 // the buffers of Ctx::feat
 // so_scan.cu

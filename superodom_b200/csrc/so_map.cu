@@ -449,6 +449,32 @@ static int index_cells(Ctx* c, MapStore& ms, uint32_t n_max, uint32_t slot_cap) 
 }
 
 static int map_rebuild_archive(Ctx* c, MapStore& ms);
+static int set_empty_index(Ctx* c, MapStore& ms);
+
+// Removal of flagged points from a built store: the id-order cloud compacted stably (cub::DeviceSelect::Flagged keeps input order)
+// into the other cloud buffer, the two swapped, then the index stage over the n_keep points left.  Removal empties slots but never
+// opens one, so the cell table of the current slot count holds the new index.
+int map_compact(Ctx* c, MapStore& ms, const uint8_t* keep, uint32_t n_keep, uint32_t* d_num_selected) {
+    cudaStream_t st = c->stream;
+    size_t need = 0;
+    cub::DeviceSelect::Flagged(nullptr, need, ms.d_xyzi, keep, ms.d_sorted, d_num_selected, int(ms.n));
+    int rc = grow_buffer(c->d_cub_tmp, c->cub_tmp_bytes, need + 256);
+    if (rc) return rc;
+    ms.dirty = true;
+    size_t tmp = c->cub_tmp_bytes;
+    SO_CUDA_TRY(cub::DeviceSelect::Flagged(c->d_cub_tmp, tmp, ms.d_xyzi, keep, ms.d_sorted, d_num_selected, int(ms.n), st));
+    c->launches += 2;
+    std::swap(ms.d_xyzi, ms.d_sorted);                                  // d_xyzi: the kept cloud in id order; d_sorted: free for the index
+    const uint32_t slots = uint32_t(ms.n_slots);
+    ms.n = n_keep;
+    if (n_keep == 0) return set_empty_index(c, ms);
+    InsertInfo* h_info = c->h_map_info;
+    *h_info = InsertInfo{};
+    h_info->n_out = n_keep;
+    SO_CUDA_TRY(cudaMemcpyAsync(&c->d_map_scratch->info, h_info, sizeof(InsertInfo), cudaMemcpyHostToDevice, st));
+    rc = count_blocks(c, ms, n_keep, slots);
+    return rc ? rc : index_cells(c, ms, n_keep, slots);
+}
 
 static int set_empty_index(Ctx* c, MapStore& ms) {
     cudaStream_t st = c->stream;
