@@ -28,7 +28,7 @@ def _pose_error(pose, seed):
 
 def _max_excess(map_xyz, scan, pose, o):
     """Largest (neighbourhood minimum - r_m) over the candidates: the smallest margin (margin_rel 0) that removes nothing."""
-    img, _, _ = F.range_image(scan, o)
+    img, hit, _, _ = F.range_image(scan, o)
     H, W = img.shape
     g = F._geom(o)
     q = F.to_sensor(map_xyz, pose)
@@ -37,7 +37,7 @@ def _max_excess(map_xyz, scan, pose, o):
     cu, ru = F._pixel_coords(az, el, g)
     col = np.minimum(np.floor(cu).astype(np.int64), W - 1)
     row = np.clip(np.floor(ru), -1e6, 1e6).astype(np.int64)
-    known, mn, ok = F._neigh(img, row, col, o.dilate)
+    known, mn, ok = F._neigh(img, hit, row, col, o.dilate)
     c = known & ok & (el >= g["el_min"]) & (el < g["el_max"]) & (rm >= o.min_range) & (rm <= o.max_range)
     return float((mn[c] - rm[c]).max())
 
@@ -191,14 +191,14 @@ def test_azimuth_wraps_and_pixels_follow_the_floor_rule():
                min_range=0.0, max_range=100.0)
     assert F.dims(o) == (4, 3)
     pts = np.array([[-10.0, 0.0, 0.0], [-10.0, -1e-12, 0.0], [0.0, 10.0, 0.0], [10.0, 0.0, 0.0], [0.0, -10.0, 0.0]])
-    img, n, hit = F.range_image(np.c_[pts, np.ones(len(pts))].astype(np.float32), o)
-    assert n == 5 and hit == 4
+    img, hit, n, n_hit = F.range_image(np.c_[pts, np.ones(len(pts))].astype(np.float32), o)
+    assert n == 5 and n_hit == 4 and np.array_equal(hit, np.isfinite(img))
     assert img[1, 0] == np.float32(10.0) and np.isfinite(img[1]).all() and not np.isfinite(img[0]).any()
     # every pixel of row 1 known but rows 0 and 2 unknown: a 3x3 neighbourhood never fits, dilate 0 does
     o0 = dataclasses_replace(o, dilate=0)
-    rem, cand = F.removal_mask(np.array([[-5.0, 0.0, 0.0], [5.0, 0.0, 0.0]]), [0, 0, 0, 0, 0, 0, 1], img, o0)
+    rem, cand = F.removal_mask(np.array([[-5.0, 0.0, 0.0], [5.0, 0.0, 0.0]]), [0, 0, 0, 0, 0, 0, 1], img, hit, o0)
     assert cand.all() and rem.all()
-    rem, cand = F.removal_mask(np.array([[-5.0, 0.0, 0.0]]), [0, 0, 0, 0, 0, 0, 1], img, o)
+    rem, cand = F.removal_mask(np.array([[-5.0, 0.0, 0.0]]), [0, 0, 0, 0, 0, 0, 1], img, hit, o)
     assert not cand.any() and not rem.any()
 
 
