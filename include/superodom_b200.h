@@ -599,8 +599,9 @@ int so_sampling_indices(uint32_t n, int32_t max_surface_features, uint32_t* out,
 /* ---- global localization against the prior map ------------------------------------------------------------------ */
 /* extends: localization mode (laserMapping.cpp:163-173 loads the prior map, :306-313 takes the start pose from init_x ... init_yaw
  * unchanged).  Instead of an exact start pose, search a region around a rough centre: every x/y/z voxel shift and yaw step of the
- * scan is scored against an occupancy bitmap of the surf map, the best hypotheses (after non-maximum suppression) are registered
- * with the ordinary ICP path, and the registration with the most accepted plane correspondences wins.  Roll and pitch are taken
+ * scan is a hypothesis, scored against an occupancy bitmap of the surf map; the best hypotheses, found by branch-and-bound (below),
+ * are registered with the ordinary ICP path after non-maximum suppression, and the registration with the most accepted plane
+ * correspondences wins.  Roll and pitch are taken
  * from the centre (IMU gravity, as initializeFirstFrame does, laserMapping.cpp:281-298).  Zero fields take the defaults shown. */
 typedef struct {
     double half_x, half_y, half_z;  /* search half-extents (m) around the centre; 0 = that axis is not searched */
@@ -636,7 +637,10 @@ typedef struct {
     uint64_t n_hypotheses;  /* NX * NY * NZ * NYAW */
     int32_t n_score_points; /* scan points scored */
     int32_t n_windows;      /* whole_map = 1 with the archive on: distinct windows the candidates were registered in; else 0 */
-    double time_raster_ms, time_dilate_ms, time_score_ms, time_sort_ms;  /* device time of each search stage (CUDA events) */
+    double time_raster_ms;  /* device time (CUDA events) of the map bounds and the raster, */
+    double time_dilate_ms;  /* of the dilation, pyramid levels and offset table, */
+    double time_score_ms;   /* of the branch-and-bound traversal; */
+    double time_sort_ms;    /* 0 (the traversal yields the keys in order) */
     double time_refine_ms;  /* candidate read-back, suppression and registrations (host clock) */
     double time_total_ms;   /* whole call (host clock) */
     so_icp_result icp;      /* the winner's registration (zeroed when there is none) */
@@ -644,25 +648,32 @@ typedef struct {
 
 /* Global localization of a sensor-frame surf cloud (layout as so_register) around center_pose7.  Writes up to cap candidates to
  * cands (may be NULL with cap 0).  The map is not modified and not shifted, an attached pose sink gets no rows; afterwards
- * so_map_add_registered_scan inserts this cloud.  Returns SO_OK, a soft status, or an error (argument errors before any device
- * work; SO_ERR_CAPACITY above 2^24 hypotheses, a bitmap above 2^32 bits or a cloud above max_scan_points). */
+ * so_map_add_registered_scan inserts this cloud.  Returns SO_OK, a soft status, or an error.  Before any device work: argument
+ * errors; SO_ERR_CAPACITY above 2^24 hypotheses, a whole-box bitmap ((NX + 2e) * (NY + 2e) * (NZ + 2e) voxels, e =
+ * ceil(max_range / res), rows padded to 32 bits) above 2^32 bits, a cloud above max_scan_points, or an offset table (NYAW * score
+ * points * 16 B) above 1 GiB, i.e. NYAW * score points > 2^26 (yaw steps finer than about 0.02 deg at 4096 points).  After the
+ * map bounds: SO_ERR_CAPACITY for a pyramid level above 2^32 bits, which takes a box near the bitmap limit with a map filling it. */
 int so_localize_global(so_ctx* ctx, const void* xyzi, size_t n, size_t stride_bytes, size_t intensity_offset, const double center_pose7[7],
                        const so_global_opts* gopts, const so_icp_opts* opts, so_global_candidate* cands, size_t cap,
                        so_global_result* out);
 /* Stage hook of so_localize_global: the uint16 score of every hypothesis, index ((yaw * NZ + z) * NY + y) * NX + x, and
- * dims = {NX, NY, NZ, NYAW}.  Needs cap >= the hypothesis count; *n_score_points (optional) receives the points scored. */
+ * dims = {NX, NY, NZ, NYAW}: level 0 of the pyramid scored densely, with no pruning.  Needs cap >= the hypothesis count
+ * (SO_ERR_CAPACITY before any device work); *n_score_points (optional) receives the points scored.  Other errors as
+ * so_localize_global. */
 int so_localize_scores(so_ctx* ctx, const void* xyzi, size_t n, size_t stride_bytes, size_t intensity_offset, const double center_pose7[7],
                        const so_global_opts* gopts, uint16_t* scores, size_t cap, int32_t dims[4], int32_t* n_score_points);
 /* Host-only (needs no device): the argument checks of so_localize_global's options, dims = {NX, NY, NZ, NYAW}, the hypothesis
- * count and the size of one occupancy bitmap.  Returns SO_OK, SO_ERR_ARG or SO_ERR_CAPACITY (dims and counts are filled for the
- * capacity error too). */
+ * count, and the bytes of an occupancy bitmap over the whole search box, the quantity so_localize_global's bitmap limit bounds
+ * (2^32 bits = 512 MiB; the search itself allocates only the pyramid clipped to the map).  Returns SO_OK, SO_ERR_ARG or
+ * SO_ERR_CAPACITY for the hypothesis and bitmap limits (dims and counts are filled for the capacity error too). */
 int so_localize_global_size(const so_global_opts* gopts, int32_t dims[4], uint64_t* n_hypotheses, uint64_t* bitmap_bytes);
 
-/* ---- global localization over the whole map: exact branch-and-bound ---------------------------------------------------- */
-/* so_localize_global_bnb searches the same hypotheses with the same scores and returns exactly what so_localize_global returns
- * (every field but the time_* ones, and the candidate list), but finds the sorted key prefix by branch-and-bound over an occupancy
- * pyramid instead of scoring every hypothesis.  Its memory scales with the map, not with the search region, so it accepts up to
- * 2^32 hypotheses: a region covering a whole prior map (so_map_bounds gives the extent).  Level L of the pyramid is
+/* ---- the search: exact branch-and-bound ------------------------------------------------------------------------------------ */
+/* Every so_localize_global* call finds the sorted key prefix (the best hypotheses, score descending, index ascending) by
+ * branch-and-bound over an occupancy pyramid instead of scoring every hypothesis.  Its memory scales with the map, not with the
+ * search region.  so_localize_global_bnb is so_localize_global with the limits this allows: up to 2^32 hypotheses, no bitmap
+ * limit, so a region may cover a whole prior map (so_map_bounds gives the extent); within so_localize_global's limits the two
+ * return the same result bit for bit (every field but the time_* ones, and the candidate list).  Level L of the pyramid is
  * B_L(x, y, z) = OR over a, b in [0, 2^L) of B(x+a, y+b, z); the bound of a level-L node (yaw m, z shift k, x/y shifts
  * [i0, i0+2^L) x [j0, j0+2^L)) is U = sum over score points of B_L at the point's voxel shifted by (i0, j0), at least the score of
  * every hypothesis in the node. */
@@ -680,15 +691,14 @@ typedef struct {
     double time_search_ms;                  /* device time of the traversal (CUDA events) */
 } so_bnb_stats;
 
-/* Arguments as so_localize_global, plus optional statistics.  The result's time_raster_ms covers the map bounds and the raster,
- * time_dilate_ms the dilation, pyramid levels and offset table, time_score_ms the traversal; time_sort_ms is 0.  Errors before any
- * device work: argument errors as so_localize_global, SO_ERR_CAPACITY above 2^32 hypotheses or an offset table (NYAW * NZ * score
- * points * 16 B) above 1 GiB; after the map bounds: SO_ERR_CAPACITY for a pyramid level above 2^32 bits. */
+/* Arguments and stage times as so_localize_global, plus optional statistics.  Errors before any device work: argument errors as
+ * so_localize_global, SO_ERR_CAPACITY above 2^32 hypotheses or an offset table (NYAW * score points * 16 B) above 1 GiB; after the
+ * map bounds: SO_ERR_CAPACITY for a pyramid level above 2^32 bits. */
 int so_localize_global_bnb(so_ctx* ctx, const void* xyzi, size_t n, size_t stride_bytes, size_t intensity_offset, const double center_pose7[7],
                            const so_global_opts* gopts, const so_icp_opts* opts, so_global_candidate* cands, size_t cap,
                            so_global_result* out, so_bnb_stats* stats);
 /* Stage hook: the first min(NX*NY*NZ*NYAW, 64 k) keys (65535 - score) << 32 | index of the ascending order of every hypothesis'
- * key, i.e. so_localize_global's sorted prefix.  Writes min(*n_keys, cap) keys; *n_keys = the prefix length. */
+ * key: the prefix so_localize_global refines.  Writes min(*n_keys, cap) keys; *n_keys = the prefix length. */
 int so_localize_bnb_keys(so_ctx* ctx, const void* xyzi, size_t n, size_t stride_bytes, size_t intensity_offset, const double center_pose7[7],
                          const so_global_opts* gopts, uint64_t* keys, size_t cap, size_t* n_keys, so_bnb_stats* stats);
 /* Stage hook: U of every node of pyramid level `level` (0 .. lmax), index ((yaw * NZ + z) * NBY + by) * NBX + bx with
@@ -729,8 +739,8 @@ int so_bytes_copied(so_ctx* ctx, uint64_t* h2d, uint64_t* d2h, int reset);
 /* Accumulated device time (ms, CUDA events on the context stream) and launch count of a kernel class since the last
  * reset; classes: 0 k_knn_scan (scan k-NN), 1 k_evaluate +
  * k_lm_step (LM step), 2 k_knn (so_knn*), 3 scan ordering / map build / map insert / free-space clearing / scan preparation (pre-filter, deskew, uniform and edge extraction), 4 first evaluation of
- * a solve (k_evaluate + k_lm_step iteration zero), 5 k_fit (plane fit), 6 global localization search (bitmap raster, dilation,
- * hypothesis scoring, key sort; for the branch-and-bound also map bounds, pyramid levels, offset table and traversal steps),
+ * a solve (k_evaluate + k_lm_step iteration zero), 5 k_fit (plane fit), 6 global localization search (map bounds, bitmap raster,
+ * dilation, pyramid levels, offset table, traversal steps and dense scoring),
  * 7 k_undistort (within-scan motion compensation: per ICP iteration, and the undistorted map insert / so_undistort_points; the
  * per-iteration warp and the map insert of so_register_optimized*), 8 evaluation + trust-region step of so_register_optimized*.
  * Profiling mode serialises kernels; enable only for roofline runs. */

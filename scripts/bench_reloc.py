@@ -1,16 +1,21 @@
 #!/usr/bin/env python3
-"""bench_reloc.py -- global localization (so_localize_global) on the cfg2 map (1 M points) with one OS1-128 scan and the default
-search: half 10 m in x and y at 0.25 m, the full circle at 2 deg = 81 x 81 x 180 = 1 180 980 hypotheses x 1024 score points.
+"""bench_reloc.py -- global localization (so_localize_global) on synthetic maps, one JSON line per workload:
 
-Prints one JSON line: median whole-call wall time over --calls calls after --warmup calls, the per-stage device times (CUDA events
-in the call; profile class 6 from one extra profiled call), hypotheses/s and bitmap lookups/s of the scoring kernel, the bitmap
-size, the recovery error against the truth, and the card name and power limit read in the same run.  --cpu adds one single-thread
-run of the numpy restatement of the search (tests/global_localization_numpy.py) for a speed-up figure.  Writes nothing.
+  default  the cfg2 map (1 M points), one OS1-128 scan, half 10 m in x and y at 0.25 m, the full circle at 2 deg
+           = 81 x 81 x 180 = 1 180 980 hypotheses x 1024 score points;
+  small    the cfg1 map, one VLP-16 scan, half 1 m in x and y, 0.25 m in z, the full circle at 15 deg, max_range 15 m
+           = 9 x 9 x 3 x 24 = 5 832 hypotheses (where the search's per-step read-backs weigh most);
+  z        the default scan and centre with half 5 m in x and y and 2 m in z = 41 x 41 x 17 x 180 = 5 143 860 hypotheses.
 
---bnb adds so_localize_global_bnb on the same search, timed in alternation with the exhaustive call (whole call and search stage).
---whole-map adds branch-and-bound searches over whole maps: the cfg2 map (0.25 m, 2 deg, centre at the map centre with the true z
-and a seeded yaw) and a 300 m x 300 m synthetic map (synth.make_map(150.0, 0.2)), each with its per-level statistics, the share of
-hypotheses whose leaves were scored and the recovery error.  Either flag prints one more JSON line per workload.
+Per workload: median whole-call wall time over --calls calls after --warmup calls, the per-stage device times (CUDA events in the
+call; profile class 6 from one extra profiled call), the search statistics of so_localize_global_bnb on the same call, the
+recovery error against the truth, and the card name and power limit read in the same run.  --cpu adds one single-thread run of
+the numpy restatement of the default search's scoring (tests/global_localization_numpy.py) for a speed-up figure.  Writes nothing.
+The library is the in-tree build, or the one SO_LIB_PATH names.
+
+--whole-map adds so_localize_global_bnb searches over whole maps: the cfg2 map (0.25 m, 2 deg, centre at the map centre with the
+true z and a seeded yaw) and a 300 m x 300 m synthetic map (synth.make_map(150.0, 0.2)), each with its per-level statistics, the
+share of hypotheses whose leaves were scored and the recovery error.  One more JSON line per map.
 --archive adds whole-map searches (so_global_opts.whole_map = 1) over three cfg2-sized rooms at x = -800, 0 and +800 m (1.70 km,
 about 3 M points) held in the window and the block archive, window in room A: a scan in room C (the refinement moves the window)
 and a scan in room A (no move).  Per case, medians over --calls calls of the build device time (bounds, segment raster, dilation,
@@ -57,14 +62,14 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--calls", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
-    ap.add_argument("--scan", type=int, default=0, help="cfg2 scan index")
+    ap.add_argument("--scan", type=int, default=0, help="scan index of every workload")
     ap.add_argument("--cpu", action="store_true")
-    ap.add_argument("--bnb", action="store_true", help="also time so_localize_global_bnb against the exhaustive call")
-    ap.add_argument("--whole-map", action="store_true", help="also run branch-and-bound searches over the whole cfg2 and 300 m maps")
+    ap.add_argument("--whole-map", action="store_true", help="also run so_localize_global_bnb over the whole cfg2 and 300 m maps")
     ap.add_argument("--archive", action="store_true", help="also run whole-map searches over a 1.7 km three-room map in the block archive")
     a = ap.parse_args()
     from superodom_b200 import api, synth
     import global_localization_numpy as GN
+    name, limit = card()
     scene, map_xyzi = synth.make_map_for("cfg2")
     case = synth.make_case_on(scene, map_xyzi, "cfg2", a.scan)
     truth = case["pose_true"]
@@ -73,16 +78,60 @@ def main():
     dyaw = rng.uniform(-math.pi, math.pi)
     q = synth.quat_mul(np.array([0.0, 0.0, math.sin(dyaw / 2), math.cos(dyaw / 2)]), truth[3:])
     center = np.r_[truth[0] + d[0], truth[1] + d[1], truth[2], q / np.linalg.norm(q)]
-    region = dict(half_x=10.0, half_y=10.0, yaw_half=math.pi)
+    off = f"centre {np.linalg.norm(d):.2f} m / {math.degrees(dyaw):.1f} deg off"
+    scene1, map1 = synth.make_map_for("cfg1")
+    case1 = synth.make_case_on(scene1, map1, "cfg1", a.scan)
+    t1 = case1["pose_true"]
+    center1 = np.r_[t1[:3] + np.array([0.37, -0.21, 0.05]), t1[3:]]
+    work = (("default", map_xyzi, case, center, off, dict(half_x=10.0, half_y=10.0, yaw_half=math.pi)),
+            ("small", map1, case1, center1, "centre 0.43 m off", dict(half_x=1.0, half_y=1.0, half_z=0.25, yaw_half=math.pi,
+                                                                     yaw_step=15 * math.pi / 180, max_range=15.0)),
+            ("z", map_xyzi, case, center, off, dict(half_x=5.0, half_y=5.0, half_z=2.0, yaw_half=math.pi)))
+    for label, m, cs, c, where, region in work:
+        out = localize_workload(m, cs, c, region, a.calls, a.warmup)
+        out["workload"] = f"{label}: {out['workload']}, {where}"
+        if a.cpu and label == "default":
+            ctx = api.Context(max_map_points=len(m) + (1 << 18), max_scan_points=262144, plane_res=0.2)
+            ctx.map_set_points(m)
+            t0 = time.perf_counter()
+            GN.localize_scores_numpy(cs["scan_xyzi"], c, ctx.map_download(0)[:, :3], **region)
+            cpu_ms = (time.perf_counter() - t0) * 1e3
+            ctx.close()
+            out["cpu_numpy_scoring_ms"] = cpu_ms
+            out["speedup_search_vs_cpu"] = cpu_ms / sum(out["stage_ms_median"][k] for k in ("raster", "dilate", "score"))
+        print(json.dumps(dict(out, card=name, power_limit_w=limit)))
+    if a.whole_map:
+        ctx = api.Context(max_map_points=len(map_xyzi) + (1 << 18), max_scan_points=262144, plane_res=0.2, max_batch=16)
+        ctx.map_set_points(map_xyzi)
+        print(json.dumps(dict(whole_map(ctx, "cfg2 map", case, a.calls, a.warmup), card=name, power_limit_w=limit)))
+        ctx.close()
+        t0 = time.perf_counter()
+        scene3, map3 = synth.make_map(150.0, 0.2)
+        gen_s = time.perf_counter() - t0
+        case3 = synth.make_case_on(scene3, map3, "cfg2", a.scan)
+        ctx = api.Context(max_map_points=len(map3) + (1 << 18), max_scan_points=262144, plane_res=0.2, max_batch=16)
+        ctx.map_set_points(map3)
+        r = whole_map(ctx, f"300 m x 300 m synthetic map ({len(map3)} pts, generated in {gen_s:.1f} s)", case3, max(3, a.calls // 4), 1)
+        print(json.dumps(dict(r, card=name, power_limit_w=limit)))
+        ctx.close()
+    if a.archive:
+        for r in archive_cases(a.calls, a.warmup):
+            print(json.dumps(dict(r, card=name, power_limit_w=limit)))
+
+
+def localize_workload(map_xyzi, case, center, region, calls, warmup):
+    """so_localize_global on one region: whole-call wall times, stage times, class-6 profile, and one so_localize_global_bnb call
+    for the search statistics."""
+    from superodom_b200 import api
     g = api.global_opts(**region)
-    dims, n_hyp, bitmap_bytes = api.localize_global_size(g)
-    ctx = api.Context(max_map_points=len(map_xyzi) + (1 << 18), max_scan_points=262144, plane_res=0.2, max_batch=16)
+    dims, n_hyp, _ = api.localize_global_size(g)
+    ctx = api.Context(max_map_points=len(map_xyzi) + (1 << 18), max_scan_points=262144, plane_res=case["cfg"]["plane_res"], max_batch=16)
     ctx.map_set_points(map_xyzi)
-    scan = case["scan_xyzi"]
-    for _ in range(a.warmup):
+    scan, truth = case["scan_xyzi"], case["pose_true"]
+    for _ in range(warmup):
         ctx.localize_global(scan, center, 20, g)
-    wall, st = [], {k: [] for k in ("raster", "dilate", "score", "sort", "refine")}
-    for _ in range(a.calls):
+    wall, st = [], {k: [] for k in ("raster", "dilate", "score", "refine")}
+    for _ in range(calls):
         t0 = time.perf_counter()
         pose, res, cands = ctx.localize_global(scan, center, 20, g)      # returns after a device synchronise
         wall.append((time.perf_counter() - t0) * 1e3)
@@ -93,54 +142,20 @@ def main():
     ctx.localize_global(scan, center, 20, g)
     ctx.profile_enable(False)
     prof_ms, prof_n = ctx.profile_get(6, reset=True)
-    med = {k: float(np.median(v)) for k, v in st.items()}
-    ns = sorted((c.n_success for c in cands if c.status == 0), reverse=True)
-    name, limit = card()
-    out = {
-        "workload": f"cfg2 map ({len(map_xyzi)} pts), OS1-128 scan {a.scan} ({len(scan)} pts), centre {np.linalg.norm(d):.2f} m / "
-                    f"{math.degrees(dyaw):.1f} deg off, default search {dims} = {n_hyp} hypotheses x {res.n_score_points} score points",
-        "card": name, "power_limit_w": limit,
-        "calls": a.calls, "warmup": a.warmup,
-        "wall_ms_median": float(np.median(wall)), "wall_ms_min": float(np.min(wall)), "wall_ms_max": float(np.max(wall)),
-        "stage_ms_median": med,
-        "profile_class6_ms": prof_ms, "profile_class6_launches": prof_n,
-        "hypotheses_per_s": n_hyp / (med["score"] * 1e-3),
-        "lookups_per_s": n_hyp * res.n_score_points / (med["score"] * 1e-3),
-        "bitmap_bytes": bitmap_bytes,
-        "status": res.status, "n_candidates": res.n_candidates, "best_score": res.best_score,
-        "winner_success": ns[0] if ns else 0, "runner_up_success": ns[1] if len(ns) > 1 else 0,
-        "err_m": float(np.linalg.norm(pose[:3] - truth[:3])),
-        "err_deg": math.degrees(2.0 * math.acos(min(1.0, abs(float(np.dot(pose[3:], truth[3:])))))),
-    }
-    if a.cpu:
-        t0 = time.perf_counter()
-        GN.localize_scores_numpy(scan, center, ctx.map_download(0)[:, :3], **region)
-        cpu_ms = (time.perf_counter() - t0) * 1e3
-        out["cpu_numpy_search_ms"] = cpu_ms
-        out["speedup_search_vs_cpu"] = cpu_ms / (med["raster"] + med["dilate"] + med["score"] + med["sort"])
-    if a.bnb:
-        bnb_out = bnb_vs_exhaustive(ctx, scan, center, truth, g, a.calls, a.warmup)
+    _, _, _, bst = ctx.localize_global_bnb(scan, center, 20, g)
     ctx.close()
-    print(json.dumps(out))
-    if a.bnb:
-        print(json.dumps(dict(bnb_out, card=name, power_limit_w=limit)))
-    if a.whole_map:
-        ctx = api.Context(max_map_points=len(map_xyzi) + (1 << 18), max_scan_points=262144, plane_res=0.2, max_batch=16)
-        ctx.map_set_points(map_xyzi)
-        print(json.dumps(dict(whole_map(ctx, "cfg2 map", case, a.calls, a.warmup, out["hypotheses_per_s"]), card=name, power_limit_w=limit)))
-        ctx.close()
-        t0 = time.perf_counter()
-        scene3, map3 = synth.make_map(150.0, 0.2)
-        gen_s = time.perf_counter() - t0
-        case3 = synth.make_case_on(scene3, map3, "cfg2", a.scan)
-        ctx = api.Context(max_map_points=len(map3) + (1 << 18), max_scan_points=262144, plane_res=0.2, max_batch=16)
-        ctx.map_set_points(map3)
-        r = whole_map(ctx, f"300 m x 300 m synthetic map ({len(map3)} pts, generated in {gen_s:.1f} s)", case3, max(3, a.calls // 4), 1, out["hypotheses_per_s"])
-        print(json.dumps(dict(r, card=name, power_limit_w=limit)))
-        ctx.close()
-    if a.archive:
-        for r in archive_cases(a.calls, a.warmup):
-            print(json.dumps(dict(r, card=name, power_limit_w=limit)))
+    ns = sorted((c.n_success for c in cands if c.status == 0), reverse=True)
+    return {"workload": f"{len(map_xyzi)}-point map, scan of {len(scan)} pts, search {dims} = {n_hyp} hypotheses x "
+                        f"{res.n_score_points} score points",
+            "calls": calls, "warmup": warmup,
+            "wall_ms_median": float(np.median(wall)), "wall_ms_min": float(np.min(wall)), "wall_ms_max": float(np.max(wall)),
+            "stage_ms_median": {k: float(np.median(v)) for k, v in st.items()},
+            "profile_class6_ms": prof_ms, "profile_class6_launches": prof_n,
+            "leaf_fraction": bst.leaves_scored / n_hyp, "stats": _stats(bst),
+            "status": res.status, "n_candidates": res.n_candidates, "best_score": res.best_score,
+            "winner_success": ns[0] if ns else 0, "runner_up_success": ns[1] if len(ns) > 1 else 0,
+            "err_m": float(np.linalg.norm(pose[:3] - truth[:3])),
+            "err_deg": math.degrees(2.0 * math.acos(min(1.0, abs(float(np.dot(pose[3:], truth[3:]))))))}
 
 
 def _stats(st):
@@ -150,36 +165,8 @@ def _stats(st):
             "build_ms": st.time_build_ms, "search_ms": st.time_search_ms}
 
 
-def bnb_vs_exhaustive(ctx, scan, center, truth, g, calls, warmup):
-    """The default search both ways, alternating call by call; the two results must be bit-identical apart from timings."""
-    for _ in range(warmup):
-        ctx.localize_global(scan, center, 20, g)
-        ctx.localize_global_bnb(scan, center, 20, g)
-    wall = {"exhaustive": [], "bnb": []}
-    search = {"exhaustive": [], "bnb": []}
-    same = True
-    for _ in range(calls):
-        t0 = time.perf_counter()
-        pose, res, _ = ctx.localize_global(scan, center, 20, g)
-        wall["exhaustive"].append((time.perf_counter() - t0) * 1e3)
-        search["exhaustive"].append(res.time_raster_ms + res.time_dilate_ms + res.time_score_ms + res.time_sort_ms)
-        t0 = time.perf_counter()
-        pose_b, res_b, _, st = ctx.localize_global_bnb(scan, center, 20, g)
-        wall["bnb"].append((time.perf_counter() - t0) * 1e3)
-        search["bnb"].append(res_b.time_raster_ms + res_b.time_dilate_ms + res_b.time_score_ms)
-        same &= bool(np.array_equal(pose, pose_b)) and res.winner == res_b.winner and res.best_score == res_b.best_score
-    return {"workload": "default cfg2 search, exhaustive vs branch-and-bound, alternating", "calls": calls,
-            "wall_ms_median": {k: float(np.median(v)) for k, v in wall.items()},
-            "wall_ms_range": {k: [float(np.min(v)), float(np.max(v))] for k, v in wall.items()},
-            "search_ms_median": {k: float(np.median(v)) for k, v in search.items()},
-            "search_ms_range": {k: [float(np.min(v)), float(np.max(v))] for k, v in search.items()},
-            "same_result": same, "n_hypotheses": res.n_hypotheses, "leaf_fraction": st.leaves_scored / res.n_hypotheses,
-            "stats": _stats(st)}
-
-
-def whole_map(ctx, label, case, calls, warmup, exhaustive_rate):
-    """Branch-and-bound over the whole map from its centre (true z, seeded yaw), 0.25 m and 2 deg.  exhaustive_rate: hypotheses/s of
-    the exhaustive scoring kernel in this run, for the time an exhaustive search of the same region would take if it were allowed."""
+def whole_map(ctx, label, case, calls, warmup):
+    """so_localize_global_bnb over the whole map from its centre (true z, seeded yaw), 0.25 m and 2 deg."""
     from superodom_b200 import api
     truth = case["pose_true"]
     lo, hi, n_map = ctx.map_bounds()
@@ -199,7 +186,6 @@ def whole_map(ctx, label, case, calls, warmup, exhaustive_rate):
                         f"{res.n_score_points} score points", "calls": calls,
             "wall_ms_median": float(np.median(wall)), "wall_ms_range": [float(np.min(wall)), float(np.max(wall))],
             "bnb_ms_median": float(np.median(search)), "bnb_ms_range": [float(np.min(search)), float(np.max(search))],
-            "exhaustive_rate_equivalent_ms": res.n_hypotheses / exhaustive_rate * 1e3,
             "leaf_fraction": st.leaves_scored / res.n_hypotheses, "stats": _stats(st),
             "status": res.status, "best_score": res.best_score, "n_candidates": res.n_candidates,
             "true_offset_m": float(np.linalg.norm(center[:2] - truth[:2])),

@@ -235,20 +235,13 @@ struct Ctx {
     cudaStream_t copy_stream = nullptr;            // H2D of batch chunks overlaps the previous chunk's kernels
     cudaEvent_t ev_copy[17] = {};           // [0..15]: per upload chunk; [16]: guard
 
-    // ---- global localization (so_localize_global): allocated on first use, grown on demand --------------------------
-    struct Reloc {
-        uint32_t* d_bits[2] = {nullptr, nullptr}; size_t bit_words[2] = {0, 0};     // occupancy bitmap, ping-pong for the dilation passes
-        uint64_t* d_keys = nullptr; uint64_t* d_keys_out = nullptr; size_t key_cap = 0, key_out_cap = 0;
-        void* d_tmp = nullptr; size_t tmp_bytes = 0;                        // radix-sort scratch
+    // ---- global localization (so_localize_global*): allocated on first use, grown on demand ---------------------------
+    struct Bnb {
         float4* d_pts = nullptr;                                           // [kRelocMaxPoints] score points
         double* d_q = nullptr; size_t q_cap = 0;                           // one quaternion per yaw
-        cudaEvent_t ev[5] = {};                                            // stage boundaries
-    } reloc;
-    // ---- branch-and-bound search (so_localize_global_bnb): allocated on first use, grown on demand ---------------------
-    struct Bnb {
         uint32_t* d_pyr = nullptr; size_t pyr_words = 0;                   // every level of the clipped pyramid, back to back
         uint32_t* d_scratch = nullptr; size_t scratch_words = 0;           // raster / dilation ping-pong partner of level 0
-        int4* d_off = nullptr; size_t off_cap = 0;                         // [nyaw][nz][n_pts] voxel offsets of the score points
+        int4* d_off = nullptr; size_t off_cap = 0;                         // [nyaw][n_pts] voxel offsets of the score points
         uint64_t* d_nodes = nullptr;                                       // level buffers: [kBnbRoot] root chunk + [4C] per finer level
         uint64_t* d_unsorted = nullptr;                                    // [kBnbRoot] scored nodes before the sort
         uint64_t* d_merge[2] = {nullptr, nullptr};                         // [kBnbMerge] running top-P + new leaves, sorted copy
@@ -327,7 +320,7 @@ inline float4 read_point(const unsigned char* p, size_t stride, size_t ioff) {  
     return make_float4(xyz[0], xyz[1], xyz[2], it);
 }
 // so_global.cu
-void global_free(Ctx* c);                                   // the search buffers and events of Ctx::reloc / Ctx::bnb
+void global_free(Ctx* c);                                   // the search buffers and events of Ctx::bnb
 // so_undistort.cu
 void undistort_free(Ctx* c);                                // the buffers of Ctx::und
 int undistort_reserve(Ctx* c, size_t n_points);             // Ctx::und's parameters (max_batch) and times (n_points)
@@ -424,7 +417,7 @@ int scan_sort_alloc(Ctx* c);             // temp storage for the per-registratio
 int query_sort(Ctx* c, size_t n);         // d_qkeys/d_qvals -> *_out (allocates on growth)
 int query_sort_reserve(Ctx* c, size_t n);
 int scan_sort(Ctx* c, size_t first, size_t n, int n_scans, int cell_bits, bool key32, cudaStream_t st);   // d_skeys/d_svals[first..first+n) -> *_out
-// so_reloc.cu (global localization search)
+// so_reloc.cu (global localization: branch-and-bound search over an occupancy pyramid)
 struct RelocGrid {
     int32_t nx, ny, nz, nyaw;              // hypotheses per axis: 2I+1, 2J+1, 2K+1, yaw steps
     int32_t e;                             // ceil(max_range / res): the scan's reach in voxels
@@ -433,13 +426,7 @@ struct RelocGrid {
     double res;
 };
 constexpr int kRelocMaxPoints = 4097;      // score_points <= 4096; shouldProcessPoint keeps at most one more
-constexpr int kRelocThreads = 256, kRelocRows = 8;   // k_reloc_score: CTA size, y shifts per CTA
 uint32_t* launch_reloc_dilate(const RelocGrid& g, int d, uint32_t* a, uint32_t* b, cudaStream_t st);   // 3 passes; returns the result buffer
-int launch_reloc_score(const float4* spts, int n_pts, const double* d_q, const RelocGrid& g, const uint32_t* bits, uint64_t* keys, cudaStream_t st);
-size_t reloc_sort_bytes(size_t n);
-int reloc_sort(void* tmp, size_t tmp_bytes, const uint64_t* in, uint64_t* out, size_t n, cudaStream_t st);
-
-// so_reloc.cu (branch-and-bound search over an occupancy pyramid)
 constexpr int kBnbLevels = 32;             // levels 0..31 (nx <= 2^25 + 1 needs at most 26)
 constexpr int kBnbBatch = 1 << 14;         // C: nodes expanded per step, so a finer level buffer holds at most 4C
 constexpr int kBnbRoot = 1 << 16;          // root nodes scored per chunk, and the root size the Lmax rule aims for
@@ -461,13 +448,14 @@ struct BnbCtl {                            // device control block, read back af
     unsigned long long scored[kBnbLevels], discarded[kBnbLevels];
 };
 void launch_map_bounds(const float4* pts, uint32_t n, uint32_t* d_bounds, cudaStream_t st);   // d_bounds: min xyz, max xyz (ordered bits)
-// Raster of the surf store into the window W of p (the whole box: x0 = y0 = z0 = 0, wx/wy/wz = bx/by/bz, wpr[0] = g.wpr)
+// Raster of the surf store into level 0 of p's window W
 void launch_bnb_raster(const float4* pts, uint32_t n, const RelocGrid& g, const BnbPyramid& p, uint32_t* bits, cudaStream_t st);
 // The same two over the live segments of an archive pool (segs[s].src: first point, .n: points; max_n: the largest .n), read in place
 void launch_seg_bounds(const float4* pool, const GatherSeg* segs, uint32_t n_segs, uint32_t max_n, uint32_t* d_bounds, cudaStream_t st);
 void launch_seg_raster(const float4* pool, const GatherSeg* segs, uint32_t n_segs, uint32_t max_n, const RelocGrid& g, const BnbPyramid& p,
                        uint32_t* bits, cudaStream_t st);
 void launch_bnb_levels(const BnbPyramid& p, uint32_t* pyr, cudaStream_t st);                  // levels 1..lmax from level 0
+// off[m][p]: box voxel {x, y} of score point p at yaw m and shift (0, 0, 0), and its z relative to W's first plane
 void launch_bnb_offsets(const float4* spts, int n_pts, const double* d_q, const RelocGrid& g, const BnbPyramid& p, int4* off,
                         cudaStream_t st);
 // Bound of level-`level` nodes: parents == nullptr scores nodes first .. first+n-1 of the level in (m, k, tile y, tile x) order;

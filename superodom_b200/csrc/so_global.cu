@@ -1,7 +1,7 @@
 // so_global.cu -- global localization against the prior map, host side: defaults and limits of the search, score points and yaw
-// quaternions, the exhaustive and the branch-and-bound searches (kernels in so_reloc.cu), suppression and refinement of the best
-// hypotheses through register_scans (window by window over the block archive for whole_map searches), and the so_localize_* /
-// so_map_bounds* entry points of the C ABI.
+// quaternions, the branch-and-bound search (kernels in so_reloc.cu), suppression and refinement of the best hypotheses through
+// register_scans (window by window over the block archive for whole_map searches), and the so_localize_* / so_map_bounds* entry
+// points of the C ABI.
 #include <algorithm>
 #include <array>
 #include <chrono>
@@ -32,7 +32,8 @@ struct GlobalPlan {
 };
 
 // Defaults, argument checks and the grid of so_localize_global (host only).  Capacity errors return with the plan filled in.
-// bnb: the limits of so_localize_global_bnb instead (2^32 hypotheses; no whole-box bitmap, so no bitmap limit here).
+// Limits: 2^24 hypotheses and a whole-box bitmap of at most 2^32 bits; bnb: those of so_localize_global_bnb instead (2^32
+// hypotheses, no bitmap limit).
 static int global_plan(const so_global_opts* in, GlobalPlan* P, bool bnb = false) {
     if (!in) return fail(SO_ERR_ARG, "null so_global_opts");
     so_global_opts o = *in;
@@ -85,7 +86,7 @@ static int global_plan(const so_global_opts* in, GlobalPlan* P, bool bnb = false
 
 static void plan_dims(const GlobalPlan& P, int32_t dims[4]) { dims[0] = P.g.nx; dims[1] = P.g.ny; dims[2] = P.g.nz; dims[3] = P.g.nyaw; }
 
-// A hypothesis key, as both searches write it: (65535 - score) << 32 | linear index, so that the ascending order is score
+// A hypothesis key, as the search writes it: (65535 - score) << 32 | linear index, so that the ascending order is score
 // descending, then index ascending.
 static int32_t key_score(uint64_t key) { return int32_t(65535u - uint32_t(key >> 32)); }
 static uint32_t key_index(uint64_t key) { return uint32_t(key & 0xffffffffu); }
@@ -159,10 +160,9 @@ SO_NO_FP_CONTRACT static void yaw_quaternions(const GlobalPlan& P, const double 
     }
 }
 
-// Allocate / grow the search buffers, upload the score points and yaw quaternions, and run raster -> dilate -> score (-> sort) on
-// the context stream.  The keys end in reloc.d_keys (hypothesis order) and, sorted, in reloc.d_keys_out.
+// Upload the score points and yaw quaternions on the context stream (the buffers allocated or grown on demand)
 static int global_upload(Ctx* c, const GlobalScan& S) {
-    Ctx::Reloc& R = c->reloc;
+    Ctx::Bnb& R = c->bnb;
     if (!R.d_pts) SO_CUDA_TRY(cudaMalloc(&R.d_pts, size_t(kRelocMaxPoints) * sizeof(float4)));
     { int rc = grow_buffer(R.d_q, R.q_cap, S.q.size()); if (rc) return rc; }
     cudaStream_t st = c->stream;
@@ -182,46 +182,6 @@ static int archive_raster(Ctx* c, const RelocGrid& g, const BnbPyramid& w, uint3
     return SO_OK;
 }
 
-static int global_search(Ctx* c, const GlobalPlan& P, const GlobalScan& S, bool sort) {
-    Ctx::Reloc& R = c->reloc;
-    if (!R.ev[0]) for (auto& e : R.ev) SO_CUDA_TRY(cudaEventCreate(&e));
-    for (int b = 0; b < 2; ++b) { int rc = grow_buffer(R.d_bits[b], R.bit_words[b], P.bitmap_words); if (rc) return rc; }
-    { int rc = grow_buffer(R.d_keys, R.key_cap, P.n_hyp); if (rc) return rc; }
-    { int rc = grow_buffer(R.d_keys_out, R.key_out_cap, P.n_hyp); if (rc) return rc; }
-    { int rc = grow_buffer(R.d_tmp, R.tmp_bytes, reloc_sort_bytes(P.n_hyp) + 256); if (rc) return rc; }
-    { int rc = ensure_maps(c); if (rc) return rc; }
-    RelocGrid g = P.g;
-    for (int a = 0; a < 3; ++a) g.lo[a] = S.lo[a];
-    BnbPyramid box{};                                               // raster window: the whole box
-    box.wx = g.bx; box.wy = g.by; box.wz = g.bz; box.wpr[0] = g.wpr;
-    cudaStream_t st = c->stream;
-    { int rc = global_upload(c, S); if (rc) return rc; }
-    SO_CUDA_TRY(cudaEventRecord(R.ev[0], st));
-    timed_launch_begin(c);
-    SO_CUDA_TRY(cudaMemsetAsync(R.d_bits[0], 0, P.bitmap_words * sizeof(uint32_t), st));
-    launch_bnb_raster(c->surf.d_xyzi, c->surf.n, g, box, R.d_bits[0], st);
-    if (P.whole) { int rc = archive_raster(c, g, box, R.d_bits[0]); if (rc) return rc; }
-    timed_launch_end(c, 6);
-    SO_CUDA_TRY(cudaEventRecord(R.ev[1], st));
-    timed_launch_begin(c);
-    const uint32_t* bits = launch_reloc_dilate(g, P.o.dilate, R.d_bits[0], R.d_bits[1], st);
-    c->launches += 2;
-    timed_launch_end(c, 6);
-    SO_CUDA_TRY(cudaEventRecord(R.ev[2], st));
-    timed_launch_begin(c);
-    { int rc = launch_reloc_score(R.d_pts, int(S.pts.size()), R.d_q, g, bits, R.d_keys, st); if (rc) return rc; }
-    timed_launch_end(c, 6);
-    SO_CUDA_TRY(cudaEventRecord(R.ev[3], st));
-    if (sort) {
-        timed_launch_begin(c);
-        { int rc = reloc_sort(R.d_tmp, R.tmp_bytes, R.d_keys, R.d_keys_out, P.n_hyp, st); if (rc) return rc; }
-        timed_launch_end(c, 6);
-    }
-    SO_CUDA_TRY(cudaEventRecord(R.ev[4], st));
-    SO_CUDA_TRY(cudaGetLastError());
-    return SO_OK;
-}
-
 static int global_check_args(Ctx* c, const void* xyzi, size_t n, size_t stride, const double center[7], const so_global_opts* gopts, GlobalPlan* P,
                              bool bnb = false) {
     if (!c || !center || !gopts || (!xyzi && n) || stride < 12) return fail(SO_ERR_ARG, "bad args");
@@ -235,10 +195,9 @@ static int global_check_args(Ctx* c, const void* xyzi, size_t n, size_t stride, 
 }
 
 // Everything after the search: suppression over the sorted key prefix pref[0..n_pref), refinement of the kept candidates, winner
-// selection.  Shared by so_localize_global and so_localize_global_bnb, which produce the same prefix.  The candidates register in
-// groups of one window each: for whole_map searches the window so_map_shift(prior) would leave from the current origin O0 (groups
-// ordered by their best-ranked member, the window moved to each in turn, and on return left at the winner's, or at O0 when there is
-// none); otherwise the current window, one group in rank order.
+// selection.  The candidates register in groups of one window each: for whole_map searches the window so_map_shift(prior) would
+// leave from the current origin O0 (groups ordered by their best-ranked member, the window moved to each in turn, and on return
+// left at the winner's, or at O0 when there is none); otherwise the current window, one group in rank order.
 static int global_refine(Ctx* c, const GlobalPlan& P, const GlobalScan& S, const uint64_t* pref, size_t n_pref, const void* xyzi, size_t n,
                          size_t stride, size_t ioff, const so_icp_opts* opts, so_global_candidate* cands, size_t cap, so_global_result* out,
                          std::chrono::steady_clock::time_point t0, std::chrono::steady_clock::time_point t1) {
@@ -351,9 +310,9 @@ static int global_refine(Ctx* c, const GlobalPlan& P, const GlobalScan& S, const
 }
 
 // ---------------------------------------------------------------------------------------------- branch and bound
-// The search of so_localize_global_bnb yields the same sorted key prefix as so_localize_global's exhaustive scoring and sort, from
-// an occupancy pyramid of the map (memory: the map's window of the search box, per level) and a batched depth-first traversal
-// (memory: kBnbRoot + 4C keys per level), so neither grows with the hypothesis count.  See DESIGN.md §4.
+// The search yields the P smallest keys of every hypothesis, ascending (the sorted prefix of a dense scoring), from an occupancy
+// pyramid of the map (memory: the map's window of the search box, per level) and a batched depth-first traversal (memory:
+// kBnbRoot + 4C keys per level), so neither grows with the hypothesis count.  See DESIGN.md §4.
 
 // Lmax: the smallest L >= 1 whose root level fits kBnbRoot nodes, or at which one root tile covers every x/y shift (the root is
 // then scored in chunks of kBnbRoot).
@@ -371,11 +330,11 @@ static int bnb_lmax(const RelocGrid& g) {
 
 static_assert(SO_BNB_LEVELS == kBnbLevels, "so_bnb_stats holds one entry per pyramid level");
 
-// 16-byte offset entries for every (yaw, z shift, score point): a host-decidable cap
+// 16-byte offset entries for every (yaw, score point): a host-decidable cap
 constexpr double kBnbTableBytes = double(1u << 30);
 
 static int bnb_check_table(const GlobalPlan& P, const GlobalScan& S) {
-    if (double(P.g.nyaw) * P.g.nz * double(S.pts.size()) * 16.0 > kBnbTableBytes) return fail(SO_ERR_CAPACITY, "offset table above 1 GiB");
+    if (double(P.g.nyaw) * double(S.pts.size()) * 16.0 > kBnbTableBytes) return fail(SO_ERR_CAPACITY, "offset table above 1 GiB");
     return SO_OK;
 }
 
@@ -478,7 +437,7 @@ static int bnb_build(Ctx* c, const GlobalPlan& P, const GlobalScan& S, RelocGrid
     const uint64_t w0 = p.off[1];                                   // level 0 words
     { int rc = grow_buffer(B.d_pyr, B.pyr_words, words); if (rc) return rc; }
     { int rc = grow_buffer(B.d_scratch, B.scratch_words, w0); if (rc) return rc; }
-    const size_t n_off = std::max<size_t>(1, size_t(g.nyaw) * g.nz * S.pts.size());
+    const size_t n_off = std::max<size_t>(1, size_t(g.nyaw) * S.pts.size());
     { int rc = grow_buffer(B.d_off, B.off_cap, n_off); if (rc) return rc; }
     { int rc = global_upload(c, S); if (rc) return rc; }
     timed_launch_begin(c);
@@ -498,7 +457,7 @@ static int bnb_build(Ctx* c, const GlobalPlan& P, const GlobalScan& S, RelocGrid
     c->launches += p.lmax > 0 ? p.lmax - 1 : 0;
     timed_launch_end(c, 6);
     timed_launch_begin(c);
-    launch_bnb_offsets(c->reloc.d_pts, int(S.pts.size()), c->reloc.d_q, g, p, B.d_off, st);
+    launch_bnb_offsets(B.d_pts, int(S.pts.size()), B.d_q, g, p, B.d_off, st);
     timed_launch_end(c, 6);
     SO_CUDA_TRY(cudaEventRecord(B.ev[2], st));
     SO_CUDA_TRY(cudaGetLastError());
@@ -574,7 +533,8 @@ static int bnb_search(Ctx* c, const RelocGrid& g, const BnbPyramid& p, int n_pts
     return SO_OK;
 }
 
-// Build + search: the first min(n_hyp, 64 k) keys of the ascending order of every hypothesis' key, and the statistics.
+// Build + search: the first min(n_hyp, 64 k) keys of the ascending order of every hypothesis' key, and the statistics.  64 keys per
+// candidate asked for leave room for the hypotheses the suppression drops around each kept one.
 static int bnb_run(Ctx* c, const GlobalPlan& P, const GlobalScan& S, std::vector<uint64_t>* keys, so_bnb_stats* stats) {
     RelocGrid g;
     BnbPyramid p;
@@ -600,9 +560,7 @@ static int bnb_run(Ctx* c, const GlobalPlan& P, const GlobalScan& S, std::vector
 }
 
 void global_free(Ctx* c) {
-    cudaFree(c->reloc.d_bits[0]); cudaFree(c->reloc.d_bits[1]); cudaFree(c->reloc.d_keys); cudaFree(c->reloc.d_keys_out);
-    cudaFree(c->reloc.d_tmp); cudaFree(c->reloc.d_pts); cudaFree(c->reloc.d_q);
-    for (auto& e : c->reloc.ev) if (e) cudaEventDestroy(e);
+    cudaFree(c->bnb.d_pts); cudaFree(c->bnb.d_q);
     cudaFree(c->bnb.d_pyr); cudaFree(c->bnb.d_scratch); cudaFree(c->bnb.d_off); cudaFree(c->bnb.d_nodes); cudaFree(c->bnb.d_unsorted);
     cudaFree(c->bnb.d_merge[0]); cudaFree(c->bnb.d_merge[1]); cudaFree(c->bnb.d_tmp); cudaFree(c->bnb.d_ctl); cudaFree(c->bnb.d_bounds);
     if (c->bnb.h_ctl) cudaFreeHost(c->bnb.h_ctl);
@@ -610,20 +568,20 @@ void global_free(Ctx* c) {
 }
 
 // ---------------------------------------------------------------------------------------------- entry points
-// The rest of every entry point's prologue, after its own argument checks: the score points, the offset-table cap of the B&B
-// search (so that its capacity error comes before any device work), the device, the yaw quaternions.
+// The rest of every entry point's prologue, after its own argument checks: the score points, the offset-table cap (so that its
+// capacity error comes before any device work), the device, the yaw quaternions.
 static int global_prologue(Ctx* c, const GlobalPlan& P, const void* xyzi, size_t n, size_t stride, size_t ioff, const double center[7],
-                           bool bnb, GlobalScan* S) {
+                           GlobalScan* S) {
     select_score_points(xyzi, n, stride, ioff, P.o, S);
-    if (bnb) { int rc = bnb_check_table(P, *S); if (rc) return rc; }
+    { int rc = bnb_check_table(P, *S); if (rc) return rc; }
     SO_CUDA_TRY(cudaSetDevice(c->device));
     yaw_quaternions(P, center, S);
     return SO_OK;
 }
 
-// so_localize_global (bnb = false) and so_localize_global_bnb: the sorted key prefix from the search, then global_refine.  Stage
-// times: the exhaustive search's raster, dilation, scoring and sort; the B&B build up to the raster, the rest of the build, and
-// the traversal, with no sort (time_sort_ms = 0).
+// so_localize_global (bnb = false) and so_localize_global_bnb, which differ in their limits only: the sorted key prefix from the
+// search, then global_refine.  Stage times: the build up to the raster, the rest of the build, and the traversal, with no sort
+// (time_sort_ms = 0).
 static int localize(Ctx* c, bool bnb, const void* xyzi, size_t n, size_t stride, size_t ioff, const double center[7], const so_global_opts* gopts,
                     const so_icp_opts* opts, so_global_candidate* cands, size_t cap, so_global_result* out, so_bnb_stats* stats) {
     GlobalPlan P;
@@ -634,7 +592,7 @@ static int localize(Ctx* c, bool bnb, const void* xyzi, size_t n, size_t stride,
     if (rc) return rc;
     const auto t0 = std::chrono::steady_clock::now();
     GlobalScan S;
-    rc = global_prologue(c, P, xyzi, n, stride, ioff, center, bnb, &S);
+    rc = global_prologue(c, P, xyzi, n, stride, ioff, center, &S);
     if (rc) return rc;
     std::memset(out, 0, sizeof(*out));
     std::memcpy(out->pose, center, 7 * sizeof(double));
@@ -642,23 +600,36 @@ static int localize(Ctx* c, bool bnb, const void* xyzi, size_t n, size_t stride,
     out->n_hypotheses = P.n_hyp;
     out->n_score_points = int32_t(S.pts.size());
     std::vector<uint64_t> pref;
-    if (bnb) {
-        rc = bnb_run(c, P, S, &pref, stats);
-        if (rc) return rc;
-    } else {
-        rc = global_search(c, P, S, true);
-        if (rc) return rc;
-        // sorted prefix: 64 entries per candidate asked for leaves room for the hypotheses the suppression drops around each kept one
-        pref.resize(std::min<size_t>(P.n_hyp, size_t(64) * P.o.k));
-        SO_CUDA_TRY(cudaMemcpyAsync(pref.data(), c->reloc.d_keys_out, pref.size() * sizeof(uint64_t), cudaMemcpyDeviceToHost, c->stream));
-        count_d2h(c, pref.size() * sizeof(uint64_t));
-        SO_CUDA_TRY(cudaStreamSynchronize(c->stream));
-    }
+    rc = bnb_run(c, P, S, &pref, stats);
+    if (rc) return rc;
     const auto t1 = std::chrono::steady_clock::now();
-    cudaEvent_t* ev = bnb ? c->bnb.ev : c->reloc.ev;
-    double* stage[4] = {&out->time_raster_ms, &out->time_dilate_ms, &out->time_score_ms, &out->time_sort_ms};
-    for (int s = 0; s < (bnb ? 3 : 4); ++s) { float ms = 0.f; cudaEventElapsedTime(&ms, ev[s], ev[s + 1]); *stage[s] = double(ms); }
+    double* stage[3] = {&out->time_raster_ms, &out->time_dilate_ms, &out->time_score_ms};
+    for (int s = 0; s < 3; ++s) { float ms = 0.f; cudaEventElapsedTime(&ms, c->bnb.ev[s], c->bnb.ev[s + 1]); *stage[s] = double(ms); }
     return global_refine(c, P, S, pref.data(), pref.size(), xyzi, n, stride, ioff, opts, cands, cap, out, t0, t1);
+}
+
+// so_localize_scores (level 0: the score of every hypothesis) and so_localize_bnb_bounds: every node bound of one level, with no
+// pruning, in (yaw, z shift, tile y, tile x) order.
+static int bnb_dense(Ctx* c, const GlobalPlan& P, const GlobalScan& S, int level, uint16_t* bounds) {
+    RelocGrid g;
+    BnbPyramid p;
+    uint64_t words = 0;
+    { int rc = bnb_build(c, P, S, &g, &p, &words); if (rc) return rc; }
+    { int rc = bnb_reset_ctl(c); if (rc) return rc; }
+    const uint64_t total = bnb_level_nodes(g, level);
+    std::vector<uint64_t> buf(kBnbRoot);
+    for (uint64_t r0 = 0; r0 < total; r0 += kBnbRoot) {
+        const uint32_t nr = uint32_t(std::min<uint64_t>(kBnbRoot, total - r0));
+        timed_launch_begin(c);
+        launch_bnb_score(g, p, c->bnb.d_pyr, c->bnb.d_off, int(S.pts.size()), level, nullptr, r0, nr, c->bnb.d_ctl, c->bnb.d_unsorted, c->stream);
+        timed_launch_end(c, 6);
+        SO_CUDA_TRY(cudaMemcpyAsync(buf.data(), c->bnb.d_unsorted, nr * sizeof(uint64_t), cudaMemcpyDeviceToHost, c->stream));
+        count_d2h(c, nr * sizeof(uint64_t));
+        SO_CUDA_TRY(cudaStreamSynchronize(c->stream));
+        for (uint32_t i = 0; i < nr; ++i) bounds[r0 + i] = uint16_t(key_score(buf[i]));
+    }
+    SO_CUDA_TRY(cudaGetLastError());
+    return SO_OK;
 }
 
 }  // namespace so
@@ -687,15 +658,10 @@ int so_localize_scores(so_ctx* ctx, const void* xyzi, size_t n, size_t stride, s
     if (!scores || !dims) return fail(SO_ERR_ARG, "bad args");
     if (cap < P.n_hyp) return fail(SO_ERR_CAPACITY, "score array smaller than the hypothesis count");
     GlobalScan S;
-    rc = global_prologue(c, P, xyzi, n, stride, ioff, center, false, &S);
+    rc = global_prologue(c, P, xyzi, n, stride, ioff, center, &S);
     if (rc) return rc;
-    rc = global_search(c, P, S, false);
+    rc = bnb_dense(c, P, S, 0, scores);
     if (rc) return rc;
-    std::vector<uint64_t> keys(P.n_hyp);
-    SO_CUDA_TRY(cudaMemcpyAsync(keys.data(), c->reloc.d_keys, P.n_hyp * sizeof(uint64_t), cudaMemcpyDeviceToHost, c->stream));
-    count_d2h(c, P.n_hyp * sizeof(uint64_t));
-    SO_CUDA_TRY(cudaStreamSynchronize(c->stream));
-    for (size_t h = 0; h < P.n_hyp; ++h) scores[h] = uint16_t(key_score(keys[h]));
     plan_dims(P, dims);
     if (n_score_points) *n_score_points = int32_t(S.pts.size());
     return SO_OK;
@@ -719,7 +685,7 @@ int so_localize_bnb_keys(so_ctx* ctx, const void* xyzi, size_t n, size_t stride,
     if (rc) return rc;
     if ((!keys && cap) || !n_keys) return fail(SO_ERR_ARG, "bad args");
     GlobalScan S;
-    rc = global_prologue(c, P, xyzi, n, stride, ioff, center, true, &S);
+    rc = global_prologue(c, P, xyzi, n, stride, ioff, center, &S);
     if (rc) return rc;
     std::vector<uint64_t> pref;
     rc = bnb_run(c, P, S, &pref, stats);
@@ -740,31 +706,11 @@ int so_localize_bnb_bounds(so_ctx* ctx, const void* xyzi, size_t n, size_t strid
     const int32_t s = 1 << level;
     dims[0] = int32_t((int64_t(P.g.nx) + s - 1) >> level); dims[1] = int32_t((int64_t(P.g.ny) + s - 1) >> level);
     dims[2] = P.g.nz; dims[3] = P.g.nyaw;
-    const uint64_t total = bnb_level_nodes(P.g, level);
-    if (cap < total) return fail(SO_ERR_CAPACITY, "bound array smaller than the level's node count");
+    if (cap < bnb_level_nodes(P.g, level)) return fail(SO_ERR_CAPACITY, "bound array smaller than the level's node count");
     GlobalScan S;
-    rc = global_prologue(c, P, xyzi, n, stride, ioff, center, true, &S);
+    rc = global_prologue(c, P, xyzi, n, stride, ioff, center, &S);
     if (rc) return rc;
-    RelocGrid g;
-    BnbPyramid p;
-    uint64_t words = 0;
-    rc = bnb_build(c, P, S, &g, &p, &words);
-    if (rc) return rc;
-    rc = bnb_reset_ctl(c);
-    if (rc) return rc;
-    std::vector<uint64_t> buf(kBnbRoot);
-    for (uint64_t r0 = 0; r0 < total; r0 += kBnbRoot) {
-        const uint32_t nr = uint32_t(std::min<uint64_t>(kBnbRoot, total - r0));
-        timed_launch_begin(c);
-        launch_bnb_score(g, p, c->bnb.d_pyr, c->bnb.d_off, int(S.pts.size()), level, nullptr, r0, nr, c->bnb.d_ctl, c->bnb.d_unsorted, c->stream);
-        timed_launch_end(c, 6);
-        SO_CUDA_TRY(cudaMemcpyAsync(buf.data(), c->bnb.d_unsorted, nr * sizeof(uint64_t), cudaMemcpyDeviceToHost, c->stream));
-        count_d2h(c, nr * sizeof(uint64_t));
-        SO_CUDA_TRY(cudaStreamSynchronize(c->stream));
-        for (uint32_t i = 0; i < nr; ++i) bounds[r0 + i] = uint16_t(key_score(buf[i]));
-    }
-    SO_CUDA_TRY(cudaGetLastError());
-    return SO_OK;
+    return bnb_dense(c, P, S, level, bounds);
 }
 
 int so_map_bounds(so_ctx* ctx, float lo[3], float hi[3], size_t* n) {

@@ -1,7 +1,7 @@
-// so_reloc.cu -- global localization search (so_localize_global): occupancy bitmap of the surf map (and of its block archive, read
-// in place, for whole_map searches), cube dilation, exhaustive
-// scoring of x/y/z voxel shifts x yaw steps of the scan, and the key sort that ranks the hypotheses.  The host side (score-point
-// selection, suppression, refinement through register_core) lives in so_global.cu.
+// so_reloc.cu -- global localization search (so_localize_global*): occupancy bitmap of the surf map (and of its block archive, read
+// in place, for whole_map searches), cube dilation, the occupancy pyramid, and the branch-and-bound scoring and traversal of x/y/z
+// voxel shifts x yaw steps of the scan.  The host side (score-point selection, suppression, refinement through register_core)
+// lives in so_global.cu.
 //
 // Everything here is integer-valued once a point has been put into a voxel, and the voxel of a point is computed with
 // explicitly rounded FP64 operations (__dmul_rn / __dadd_rn / __dsub_rn / __ddiv_rn: no FMA contraction), so a numpy
@@ -26,8 +26,7 @@ __device__ __forceinline__ void qrot_rn(const double q[4], const double v[3], do
 }
 
 // The voxel of a score point rotated by a hypothesis yaw's quaternion, relative to the hypothesis translation:
-// floor(qrot(q, v) / res) per axis.  Shared by k_reloc_score's prologue and the branch-and-bound offset table, so both searches
-// see the same voxels.
+// floor(qrot(q, v) / res) per axis: the entries of the branch-and-bound offset table.
 __device__ __forceinline__ int3 reloc_voxel(const float4 v, const double q[4], double res) {
     const double vd[3] = {double(v.x), double(v.y), double(v.z)};
     double r[3];
@@ -60,48 +59,6 @@ __global__ void __launch_bounds__(256) k_reloc_dilate(const uint32_t* __restrict
     out[idx] = r;
 }
 
-// One CTA per (tile of kRelocRows y shifts, z shift, yaw).  Prologue: every score point rotated by the yaw's quaternion and put
-// into its voxel, stored as {x0, y0, z row base} so that hypothesis (i, j) reads bit x0 + i of row (zbase + y0 + j).  Main loop:
-// a warp takes 32 consecutive x shifts of one y shift, so each step reads one or two bitmap words (L1 / L2 resident).  Output:
-// the sort key (65535 - score) << 32 | linear index, which orders hypotheses by score descending, then index ascending.
-__global__ void __launch_bounds__(kRelocThreads) k_reloc_score(const float4* __restrict__ spts, int n_pts, const double* __restrict__ q_yaw,
-                                                                RelocGrid g, const uint32_t* __restrict__ bits, uint64_t* __restrict__ keys) {
-    extern __shared__ int4 s_off[];
-    const int j0 = blockIdx.x * kRelocRows, k = blockIdx.y, m = blockIdx.z;
-    const double q[4] = {q_yaw[4 * m], q_yaw[4 * m + 1], q_yaw[4 * m + 2], q_yaw[4 * m + 3]};
-    for (int p = threadIdx.x; p < n_pts; p += blockDim.x) {
-        const int3 w = reloc_voxel(spts[p], q, g.res);
-        const int z = w.z + k + g.e;
-        int4 o;
-        o.x = w.x + g.e;
-        o.y = (z >= 0 && z < g.bz) ? w.y + g.e : -(1 << 29);        // a z outside the box: every lookup of this point misses
-        o.z = (z >= 0 && z < g.bz) ? z * g.by : 0;
-        o.w = 0;
-        s_off[p] = o;
-    }
-    __syncthreads();
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int nxc = (g.nx + 31) >> 5;
-    for (int item = warp; item < nxc * kRelocRows; item += kRelocThreads / 32) {
-        const int j = j0 + item / nxc, i = (item % nxc) * 32 + lane;
-        if (j >= g.ny) continue;                                    // warp-uniform
-        uint32_t cnt = 0;
-#pragma unroll 4
-        for (int p = 0; p < n_pts; ++p) {
-            const int4 o = s_off[p];
-            const int y = o.y + j, x = o.x + i;
-            if (uint32_t(y) < uint32_t(g.by) && uint32_t(x) < uint32_t(g.bx)) {
-                const uint32_t w = __ldg(bits + size_t(o.z + y) * g.wpr + uint32_t(x >> 5));
-                cnt += (w >> (x & 31)) & 1u;
-            }
-        }
-        if (i < g.nx) {
-            const uint32_t lin = ((uint32_t(m) * g.nz + k) * g.ny + j) * g.nx + i;
-            keys[lin] = (uint64_t(65535u - cnt) << 32) | lin;
-        }
-    }
-}
-
 // ---------------------------------------------------------------------------------------------- branch and bound
 // Bounding box of the surf store: per-thread min / max, a warp reduction, one atomic per warp and axis.
 __global__ void __launch_bounds__(256) k_map_bounds(const float4* __restrict__ pts, uint32_t n, uint32_t* __restrict__ b) {
@@ -123,8 +80,7 @@ __global__ void __launch_bounds__(256) k_map_bounds(const float4* __restrict__ p
 // through it, so the window's points and the archive's land in the same voxels.
 __device__ __forceinline__ double box_voxel(float m, double lo, double res) { return floor(__ddiv_rn(__dsub_rn(double(m), lo), res)); }
 
-// One thread per surf-store point: the box voxel per axis; points inside the window W set their bit, shifted to W's origin.  Both
-// searches raster through it: the exhaustive one with W = the whole box.
+// One thread per surf-store point: the box voxel per axis; points inside the window W set their bit, shifted to W's origin.
 __global__ void __launch_bounds__(256) k_bnb_raster(const float4* __restrict__ pts, uint32_t n, RelocGrid g, BnbPyramid w, uint32_t* __restrict__ bits) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
@@ -203,19 +159,16 @@ __global__ void __launch_bounds__(256) k_bnb_level(BnbPyramid p, int L, uint32_t
     pyr[p.off[L + 1] + idx] = r;
 }
 
-// Offset table, one thread per (yaw m, z shift k, score point): {x, y} box voxel of hypothesis shift (0, 0) as in k_reloc_score,
-// and the plane of W it reads (-1: outside W, every lookup misses).
+// Offset table, one thread per (yaw m, score point): the box voxel {x, y} of hypothesis shift (0, 0, 0), and its z relative to W's
+// first plane (z shift k reads plane z + k of W).
 __global__ void __launch_bounds__(256) k_bnb_offsets(const float4* __restrict__ spts, int n_pts, const double* __restrict__ q_yaw, RelocGrid g,
-                                                     int z0, int wz, int4* __restrict__ off) {
+                                                     int z0, int4* __restrict__ off) {
     const size_t t = size_t(blockIdx.x) * blockDim.x + threadIdx.x;
-    if (t >= size_t(g.nyaw) * g.nz * n_pts) return;
-    const int p = int(t % n_pts);
-    const size_t mk = t / n_pts;
-    const int k = int(mk % g.nz), m = int(mk / g.nz);
+    if (t >= size_t(g.nyaw) * n_pts) return;
+    const int p = int(t % n_pts), m = int(t / n_pts);
     const double q[4] = {q_yaw[4 * m], q_yaw[4 * m + 1], q_yaw[4 * m + 2], q_yaw[4 * m + 3]};
     const int3 w = reloc_voxel(spts[p], q, g.res);
-    const int z = w.z + k + g.e - z0;
-    off[t] = make_int4(w.x + g.e, w.y + g.e, (z >= 0 && z < wz) ? z : -1, 0);
+    off[t] = make_int4(w.x + g.e, w.y + g.e, w.z + g.e - z0, 0);
 }
 
 // Node bound, one warp per node, lanes striding over the score points, one integer warp sum:
@@ -252,13 +205,13 @@ __global__ void __launch_bounds__(256) k_bnb_score(RelocGrid g, BnbPyramid p, co
         }
         uint64_t key = kBnbNone;
         if (live) {                                                 // warp-uniform
-            const int4* o = off + (size_t(m) * nz + k) * size_t(n_pts);
+            const int4* o = off + size_t(m) * size_t(n_pts);
             uint32_t cnt = 0;
             for (int q = lane; q < n_pts; q += 32) {
                 const int4 v = __ldg(o + q);
-                const int x = v.x + int(i0) - ox, y = v.y + int(j0) - oy;
-                if (v.z >= 0 && uint32_t(x) < uint32_t(xw) && uint32_t(y) < uint32_t(yw))
-                    cnt += (__ldg(bits + (size_t(v.z) * yw + y) * wpr + (x >> 5)) >> (x & 31)) & 1u;
+                const int x = v.x + int(i0) - ox, y = v.y + int(j0) - oy, z = v.z + int(k);
+                if (uint32_t(z) < uint32_t(p.wz) && uint32_t(x) < uint32_t(xw) && uint32_t(y) < uint32_t(yw))
+                    cnt += (__ldg(bits + (size_t(z) * yw + y) * wpr + (x >> 5)) >> (x & 31)) & 1u;
             }
             cnt = __reduce_add_sync(0xffffffffu, cnt);
             const uint64_t lin = ((uint64_t(m) * nz + k) * ny + j0) * nx + i0;
@@ -304,26 +257,6 @@ uint32_t* launch_reloc_dilate(const RelocGrid& g, int d, uint32_t* a, uint32_t* 
     return b;
 }
 
-int launch_reloc_score(const float4* spts, int n_pts, const double* d_q, const RelocGrid& g, const uint32_t* bits, uint64_t* keys, cudaStream_t st) {
-    const size_t smem = size_t(n_pts > 0 ? n_pts : 1) * sizeof(int4);
-    SO_CUDA_TRY(cudaFuncSetAttribute(k_reloc_score, cudaFuncAttributeMaxDynamicSharedMemorySize, int(kRelocMaxPoints * sizeof(int4))));
-    const dim3 grid((g.ny + kRelocRows - 1) / kRelocRows, g.nz, g.nyaw);
-    k_reloc_score<<<grid, kRelocThreads, smem, st>>>(spts, n_pts, d_q, g, bits, keys);
-    return SO_OK;
-}
-
-// cub radix sort of the keys: score bits 32..47 and index bits 0..23 (the keys are unique, so the order is fully determined)
-size_t reloc_sort_bytes(size_t n) {
-    size_t b = 0;
-    cub::DeviceRadixSort::SortKeys(nullptr, b, (const uint64_t*)nullptr, (uint64_t*)nullptr, int(n), 0, 48);
-    return b;
-}
-
-int reloc_sort(void* tmp, size_t tmp_bytes, const uint64_t* in, uint64_t* out, size_t n, cudaStream_t st) {
-    SO_CUDA_TRY(cub::DeviceRadixSort::SortKeys(tmp, tmp_bytes, in, out, int(n), 0, 48, st));
-    return SO_OK;
-}
-
 void launch_map_bounds(const float4* pts, uint32_t n, uint32_t* d_bounds, cudaStream_t st) {
     if (n) k_map_bounds<<<std::min<uint32_t>((n + 255) / 256, 1024), 256, 0, st>>>(pts, n, d_bounds);
 }
@@ -352,8 +285,8 @@ void launch_bnb_levels(const BnbPyramid& p, uint32_t* pyr, cudaStream_t st) {
 }
 
 void launch_bnb_offsets(const float4* spts, int n_pts, const double* d_q, const RelocGrid& g, const BnbPyramid& p, int4* off, cudaStream_t st) {
-    const size_t total = size_t(g.nyaw) * g.nz * size_t(n_pts);
-    if (total) k_bnb_offsets<<<uint32_t((total + 255) / 256), 256, 0, st>>>(spts, n_pts, d_q, g, p.z0, p.wz, off);
+    const size_t total = size_t(g.nyaw) * size_t(n_pts);
+    if (total) k_bnb_offsets<<<uint32_t((total + 255) / 256), 256, 0, st>>>(spts, n_pts, d_q, g, p.z0, off);
 }
 
 void launch_bnb_score(const RelocGrid& g, const BnbPyramid& p, const uint32_t* pyr, const int4* off, int n_pts, int level,

@@ -1,10 +1,12 @@
-"""Global localization by branch-and-bound (so_localize_global_bnb): the same sorted key prefix, and so the same result, as the
-exhaustive so_localize_global, from an occupancy pyramid whose memory scales with the map, up to 2^32 hypotheses.
+"""Global localization by branch-and-bound (the search of every so_localize_global* call): the sorted key prefix of every
+hypothesis' score, from an occupancy pyramid whose memory scales with the map; so_localize_global_bnb takes up to 2^32 hypotheses.
 
 CPU: the numpy restatement of the bounds is a bound (every node's U >= its children's U and >= every exact score in it), the
 stats struct layout, the C++ shim builds.
-GPU: bounds equal the numpy restatement at every level; keys equal the exhaustive prefix (also beyond the exhaustive path's cap);
-results equal so_localize_global bit for bit; whole-map recovery; determinism; no side effects; soft statuses; map bounds; shim."""
+GPU: bounds equal the numpy restatement at every level; keys equal the prefix of the dense scores (so_localize_scores, or numpy
+beyond so_localize_global's cap and for tall regions); so_localize_global equals so_localize_global_bnb bit for bit; the offset
+table's capacity error comes before any device work; whole-map recovery; determinism; no side effects; soft statuses; map
+bounds; shim."""
 import ctypes as C
 import math
 import os
@@ -167,9 +169,6 @@ def test_bounds_equal_numpy_at_every_level(gpu_api, name):
         assert n_pts > 0 and got.shape == want.shape
         bad = np.argwhere(got != want)
         assert len(bad) == 0, (L, len(bad), bad[:5])
-        if L == 0:
-            scores, _ = ctx.localize_scores(case["scan_xyzi"], center, g)
-            assert np.array_equal(got, scores)
     with pytest.raises(gpu_api.SuperOdomError):
         ctx.localize_bnb_bounds(case["scan_xyzi"], center, lmax + 1, g)
     ctx.close()
@@ -217,7 +216,7 @@ def test_keys_equal_exhaustive_prefix(gpu_api, name):
 
 @pytest.mark.gpu
 def test_keys_whole_cfg2_map_at_6_deg(gpu_api):
-    """The whole cfg2 map at 0.25 m and 6 deg (about 10^7 hypotheses, under the exhaustive path's cap)."""
+    """The whole cfg2 map at 0.25 m and 6 deg (about 10^7 hypotheses, under so_localize_scores' 2^24 cap)."""
     case = get_case("cfg2")
     ctx = _ctx(gpu_api, case, max_batch=1)
     lo, hi, _ = ctx.map_bounds()
@@ -274,21 +273,66 @@ def test_keys_beyond_the_exhaustive_cap(gpu_api):
 
 
 @pytest.mark.gpu
+def test_keys_z_heavy_region(gpu_api):
+    """A tall region with small x/y at 4096 score points: NYAW * NZ * points * 16 B is above 1 GiB, so a table of score-point
+    offsets per z shift would not fit; one per yaw does.  The dense scores equal the numpy restatement, the keys their prefix."""
+    case = get_case("cfg2")
+    ctx = _ctx(gpu_api, case, max_batch=1)
+    region = dict(half_x=0.25, half_y=0.25, half_z=15.0, yaw_half=math.pi, score_points=4096)
+    t = case["pose_true"]
+    center = np.r_[t[0] + 0.1, t[1] - 0.05, t[2] + 0.3, t[3:]]
+    P = GN.plan(**region)
+    want, n_pts = GN.localize_scores_numpy(case["scan_xyzi"], center, ctx.map_download(0)[:, :3], **region)
+    assert P["nz"] == 121 and P["nyaw"] * P["nz"] * n_pts * 16 > 1 << 30
+    keys, st, scores = _keys_case(gpu_api, ctx, case["scan_xyzi"], center, gpu_api.global_opts(**region), **region)
+    bad = np.argwhere(scores != want)
+    assert len(bad) == 0, (len(bad), bad[:5])
+    assert scores.max() > 0
+    print(f"z-heavy: {scores.size} hypotheses x {n_pts} points, leaves scored {st.leaves_scored}, steps {st.steps}")
+    ctx.close()
+
+
+@pytest.mark.gpu
+def test_offset_table_capacity_error_before_device_work(gpu_api):
+    """NYAW * score points > 2^26 (20 000 yaw steps at 4096 points) is within so_localize_global_size's limits, but the offset table
+    is above 1 GiB: so_localize_global, so_localize_global_bnb and so_localize_scores return SO_ERR_CAPACITY with no kernel launched
+    and no byte copied."""
+    case = get_case("cfg2")
+    ctx = _ctx(gpu_api, case, max_batch=1)
+    g = gpu_api.global_opts(yaw_half=math.pi, yaw_step=2 * math.pi / 20000, score_points=4096)
+    dims, n_hyp, _ = gpu_api.localize_global_size(g)
+    assert dims[3] == 20000 and n_hyp == 20000
+    assert 20000 * len(GN.score_points(case["scan_xyzi"], 4096, 40.0)) > 1 << 26
+    scan, center = case["scan_xyzi"], case["pose_true"]
+    ctx.kernel_launches(reset=True)
+    ctx.bytes_copied(reset=True)
+    for call in (lambda: ctx.localize_global(scan, center, 5, g), lambda: ctx.localize_global_bnb(scan, center, 5, g),
+                 lambda: ctx.localize_scores(scan, center, g)):
+        with pytest.raises(gpu_api.SuperOdomError) as ei:
+            call()
+        assert f"({SO_ERR_CAPACITY})" in str(ei.value) and "offset table" in str(ei.value)
+    assert ctx.kernel_launches() == 0 and ctx.bytes_copied() == (0, 0)
+    ctx.close()
+
+
+@pytest.mark.gpu
 def test_result_equals_exhaustive_on_recovery_cases(gpu_api):
-    """so_localize_global_bnb == so_localize_global bit for bit (timings zeroed), result and candidate list, on the eight recovery
-    cases of the exhaustive path's test."""
+    """On the eight recovery cases of so_localize_global's test: the keys equal the prefix of the dense scores, and
+    so_localize_global == so_localize_global_bnb bit for bit (timings zeroed), result and candidate list."""
     case0 = get_case("cfg2")
     ctx = _ctx(gpu_api, case0)
-    g = gpu_api.global_opts(half_x=10.0, half_y=10.0, yaw_half=math.pi)
+    region = dict(half_x=10.0, half_y=10.0, yaw_half=math.pi)
+    g = gpu_api.global_opts(**region)
     for i in range(8):
         case = get_case("cfg2", i)
         center = _recovery_center(case, i)
+        keys, _, _ = _keys_case(gpu_api, ctx, case["scan_xyzi"], center, g, **region)
         pose, res, cands = ctx.localize_global(case["scan_xyzi"], center, 20, g)
         pose_b, res_b, cands_b, st = ctx.localize_global_bnb(case["scan_xyzi"], center, 20, g)
         assert _global_bits(res, cands) == _global_bits(res_b, cands_b), i
-        assert np.array_equal(pose, pose_b) and res_b.time_sort_ms == 0.0
-        print(f"scan {i}: bnb leaves {st.leaves_scored} of {res.n_hypotheses}, steps {st.steps}, search {st.time_search_ms:.2f} ms "
-              f"vs exhaustive score+sort {res.time_score_ms + res.time_sort_ms:.2f} ms")
+        assert np.array_equal(pose, pose_b) and res.time_sort_ms == res_b.time_sort_ms == 0.0
+        assert res.best_score == 65535 - int(keys[0] >> np.uint64(32))
+        print(f"scan {i}: leaves {st.leaves_scored} of {res.n_hypotheses}, steps {st.steps}, search {st.time_search_ms:.2f} ms")
     ctx.close()
 
 
@@ -423,7 +467,7 @@ def test_map_bounds_equal_downloaded_map(gpu_api):
 @pytest.mark.gpu
 def test_shim_global_localize_in_map_matches_abi(tmp_path, gpu_api):
     """LidarSLAM::globalLocalizeInMap returns the C ABI's pose bit for bit (whole-map region from so_map_bounds) and sets
-    T_w_lidar and last_T_w_lidar; on that region the exhaustive path gives the same result."""
+    T_w_lidar and last_T_w_lidar; on that region so_localize_global gives the same result."""
     exe = _build_shim(tmp_path)
     case = get_case("cfg1", 1)
     center = _recovery_center(case, 1)
