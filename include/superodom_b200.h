@@ -750,6 +750,16 @@ int so_bytes_copied(so_ctx* ctx, uint64_t* h2d, uint64_t* d2h, int reset);
 int so_build_flags(void);
 int so_profile_enable(so_ctx* ctx, int on);
 int so_profile_get(so_ctx* ctx, int kernel_class, double* ms, uint64_t* launches, int reset);
+/* Neighbour graph of the surf store, which so_register_batch* builds by itself when a call's queries number at least 8 times the
+ * store's points and answers most neighbour searches from (same results, fewer candidates).  Builds it for the current map when
+ * none is valid, then, when the buffers are given, writes for each point of the store in search order its id (point_id[t]), the
+ * ids of its *k nearest points of the same 50 m block (nbr_id[t * k + j], ascending (d2, id), 0xFFFFFFFF when the block holds fewer)
+ * and radius[t]: 0.99999 x the distance to the last of them, +inf when the block holds at most *k other points, 0 when unused.
+ * *n_out = points of the store; cap_points < *n_out is SO_ERR_CAPACITY. */
+int so_knn_graph(so_ctx* ctx, uint32_t* point_id, uint32_t* nbr_id, float* radius, size_t cap_points, uint32_t* k, size_t* n_out);
+/* Counters of the searches of k_knn_scan per ICP iteration: counts[2 i] = queries searched in iteration i, counts[2 i + 1] = those
+ * the neighbour graph answered (counts may be NULL).  Reads them, then on != 0 resets and keeps counting, on == 0 stops. */
+int so_knn_graph_stats(so_ctx* ctx, int on, uint64_t* counts);
 
 #ifdef __cplusplus
 }

@@ -26,6 +26,7 @@ EXPORTS = [
     "so_register_undistort", "so_register_undistort_edges", "so_register_prefiltered_undistort", "so_register_batch_undistort", "so_undistort_points", "so_register_optimized", "so_register_optimized_edges", "so_register_prefiltered_optimized", "so_register_batch_optimized", "so_evaluate_optimized", "so_evaluate_optimized_edges", "so_correspond", "so_correspond_seeded", "so_ordered_scans", "so_correspond_edge", "so_evaluate", "so_covariance",
     "so_register_degeneracy", "so_register_batch_degeneracy", "so_degeneracy_analysis", "so_solve",
     "so_knn", "so_knn_device", "so_sampling_indices", "so_localize_global", "so_localize_scores", "so_localize_global_size", "so_localize_global_bnb", "so_localize_bnb_keys", "so_localize_bnb_bounds", "so_map_bounds", "so_map_bounds_all", "so_kernel_launches", "so_bytes_copied", "so_build_flags", "so_profile_enable", "so_profile_get",
+    "so_knn_graph", "so_knn_graph_stats",
 ]
 
 
@@ -303,6 +304,8 @@ def load_library():
     L.so_bytes_copied.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
     L.so_profile_enable.argtypes = [C.c_void_p, C.c_int]
     L.so_profile_get.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int]
+    L.so_knn_graph.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
+    L.so_knn_graph_stats.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
     _lib = L
     return L
 
@@ -398,6 +401,26 @@ class Context:
         n = C.c_uint64()
         self._chk(self.L.so_profile_get(self.h, cls, C.byref(ms), C.byref(n), int(reset)), "so_profile_get")
         return ms.value, n.value
+
+    def knn_graph(self):
+        """The surf store's neighbour graph (built when none is valid): (point ids [n] in search order, neighbour ids [n, k],
+        radius [n]) -- see so_knn_graph."""
+        k = C.c_uint32()
+        n = C.c_size_t()
+        self._chk(self.L.so_knn_graph(self.h, None, None, None, 0, C.byref(k), C.byref(n)), "so_knn_graph")
+        ids = np.zeros(n.value, np.uint32)
+        nbr = np.zeros((n.value, k.value), np.uint32)
+        rad = np.zeros(n.value, np.float32)
+        if n.value:
+            self._chk(self.L.so_knn_graph(self.h, _p(ids), _p(nbr), _p(rad), n.value, C.byref(k), C.byref(n)), "so_knn_graph")
+        return ids, nbr, rad
+
+    def knn_graph_stats(self, on: bool = True) -> np.ndarray:
+        """[MAX_ICP_ITERS, 2] counts since the last call (queries searched, queries the neighbour graph answered) per ICP
+        iteration; on: reset and keep counting, else stop."""
+        out = np.zeros(2 * MAX_ICP_ITERS, np.uint64)
+        self._chk(self.L.so_knn_graph_stats(self.h, int(on), _p(out)), "so_knn_graph_stats")
+        return out.reshape(MAX_ICP_ITERS, 2)
 
     # ---- map
     def map_set_resolution(self, line_res: float, plane_res: float):

@@ -162,8 +162,9 @@ static void ctx_free(Ctx* c) {
     if (c->ev_join) cudaEventDestroy(c->ev_join);
     for (auto& e : c->ev_copy) if (e) cudaEventDestroy(e);
     map_free(c);
+    cudaFree(c->d_graph_stats);
     cudaFree(c->d_scan_sorted); cudaFree(c->d_skeys); cudaFree(c->d_skeys_out); cudaFree(c->d_svals); cudaFree(c->d_svals_out);
-    cudaFree(c->d_sort_tmp); cudaFree(c->d_sort_tmp2); cudaFree(c->nn.pos); cudaFree(c->nn.d5); cudaFree(c->nn.pre);
+    cudaFree(c->d_sort_tmp); cudaFree(c->d_sort_tmp2); cudaFree(c->nn.pos); cudaFree(c->nn.d5); cudaFree(c->nn.pre); cudaFree(c->nn.queue); cudaFree(c->nn.qcount);
     cudaFree(c->d_scan); cudaFree(c->d_offset); cudaFree(c->d_state); cudaFreeHost(c->h_state); cudaFreeHost(c->h_offset);
     cudaFree(c->d_partials); cudaFree(c->d_counters); cudaFree(c->d_hist);
     cudaFree(c->d_escan); cudaFree(c->d_eoffset); cudaFree(c->ebuf.a); cudaFree(c->ebuf.b); cudaFree(c->ebuf.flags); cudaFree(c->ebuf.nn); cudaFree(c->ebuf.selmask);
@@ -286,6 +287,17 @@ void timed_launch_end(Ctx* c, int cls) {
     c->prof[cls].ms += ms; c->prof[cls].launches++;
 }
 
+// With a valid neighbour graph the searches of a call queue the queries it does not answer (k_knn_scan<true>): the queue and the
+// per-scan, per-iteration queue lengths of the call's n_scans scans, zeroed.
+static int graph_queue_begin(Ctx* c, size_t n_scans) {
+    if (!knn_graph_valid(c)) return SO_OK;
+    int rc = grow_buffer(c->nn.queue, c->queue_cap, c->scan_cap);
+    if (!rc) rc = grow_buffer(c->nn.qcount, c->qcount_cap, size_t(c->max_batch) * SO_MAX_ICP_ITERS);
+    if (rc) return rc;
+    SO_CUDA_TRY(cudaMemsetAsync(c->nn.qcount, 0, n_scans * SO_MAX_ICP_ITERS * sizeof(uint32_t), c->stream));
+    return SO_OK;
+}
+
 // A contiguous run of scans of the batch that is uploaded, ordered and registered together.
 // grid_in: CTAs covering the longest scan as uploaded (scan ordering); grid_x: CTAs covering the longest scan once it is reduced to the
 // points shouldProcessPoint keeps (the ICP kernels); small: every scan's survivors fit k_prepare_small
@@ -364,7 +376,9 @@ static uint64_t iteration_launches(UndistortionMode mode, bool fused, uint32_t g
 // its solves), else nullptr.
 static int run_schedule(Ctx* c, const Chunk& ch, int iters, int lm, UndistortionMode mode, const uint32_t* d_inject, int inject_iters,
                         cudaStream_t run_stream, bool* was_loop, DegenState* dg) {
-    const MapView mv = map_view(c, c->surf);
+    const MapView mv = search_view(c);
+    NnBuf nn = c->nn;                                     // queue lengths: indexed by the scan's position inside the chunk
+    if (nn.qcount) nn.qcount += size_t(ch.first) * SO_MAX_ICP_ITERS;
     BatchView bv = batch_view(c, c->d_scan_sorted, ch.first);
     CorrBuf cb = c->corr;
     cb.nn = nullptr; cb.nn_d2 = nullptr;
@@ -396,7 +410,7 @@ static int run_schedule(Ctx* c, const Chunk& ch, int iters, int lm, Undistortion
     };
     auto iteration = [&](cudaStream_t s) {
         if (mode != UndistortionMode::NONE) head(s);
-        launch_match(mv, bv, cb, c->nn, grid_x, n_scans, s);
+        launch_match(mv, bv, cb, nn, grid_x, n_scans, s);
         solve(PH_CORR, s);
         for (int k = 0; k < lm; ++k) solve(PH_EVAL, s);
     };
@@ -417,9 +431,9 @@ static int run_schedule(Ctx* c, const Chunk& ch, int iters, int lm, Undistortion
                 if (mode != UndistortionMode::NONE) { timed_launch_begin(c); head(c->stream); c->launches += warp_edges ? 1 : 0; timed_launch_end(c, 7); }
                 timed_launch_begin(c);
                 if (d_inject) launch_inject(mv, c->surf.d_xyzi, c->surf.n, bv, c->nn, d_inject, inject_iters, grid_x, n_scans, c->stream);
-                else launch_match(mv, bv, cb, c->nn, grid_x, n_scans, c->stream, 1);                                               // k_knn_scan
+                else launch_match(mv, bv, cb, nn, grid_x, n_scans, c->stream, 1);                                               // k_knn_scan
                 timed_launch_end(c, 0);
-                timed_launch_begin(c); launch_match(mv, bv, cb, c->nn, grid_x, n_scans, c->stream, 2); timed_launch_end(c, 5);      // k_fit
+                timed_launch_begin(c); launch_match(mv, bv, cb, nn, grid_x, n_scans, c->stream, 2); timed_launch_end(c, 5);      // k_fit
                 timed_launch_begin(c); solve(PH_CORR, c->stream); c->launches += corr_extra; timed_launch_end(c, optimized ? 8 : 4);
             }
             for (int k = 0; k < lm; ++k)
@@ -438,6 +452,7 @@ static int run_schedule(Ctx* c, const Chunk& ch, int iters, int lm, Undistortion
     if (mode != UndistortionMode::NONE) { key.mode = mode; key.und_time = c->und.d_time; }
     if (warp_edges) key.und_edge = c->und.d_ewarp;
     key.degen = dg;
+    key.graph[0] = mv.graph; key.graph[1] = mv.graph_radius; key.graph[2] = mv.graph_stats; key.graph[3] = nn.queue; key.graph[4] = nn.qcount;
     Ctx::GraphSlot* slot = nullptr;
     for (auto& g : c->graphs)
         if (g.exec && std::memcmp(&g.key, &key, sizeof(key)) == 0) slot = &g;
@@ -600,6 +615,15 @@ static int register_core(Ctx* c, const RegisterRequest& q) {
             c->eoffset_dirty = any_edge;
         }
         count_h2d(c, n_scans * (sizeof(IcpState) + sizeof(uint32_t)));
+        {                                                           // the neighbour graph, when this call's searches pay for it
+            size_t queries = 0;
+            for (size_t s = 0; s < n_scans; ++s)
+                if (c->h_state[s].phase == PH_CORR)
+                    queries += c->h_state[s].sampling_rate < 0.0 ? n_points[s] : std::min<uint32_t>(n_points[s], uint32_t(o.max_surface_features) + 1);
+            int rc = knn_graph_prepare(c, queries);
+            if (!rc) rc = graph_queue_begin(c, n_scans);
+            if (rc) return rc;
+        }
         // Chunk the batch.  Even chunks run on `stream`, odd ones on aux_stream, so that one chunk's serial stretches (the
         // one-CTA optimiser steps, kernel tails, the loop condition) sit under the other's wide kernels; with host input
         // the H2D of chunk k+1 (copy stream) also overlaps the kernels of chunk k.
@@ -681,7 +705,9 @@ static int register_core(Ctx* c, const RegisterRequest& q) {
             int max_it = 0;
             for (uint32_t s = chunks[k].first; s < chunks[k].first + chunks[k].count; ++s) max_it = std::max(max_it, int(c->h_state[s].n_iterations));
             const bool fused = fused_lm(c, chunks[k].count, q.mode, q.degen != nullptr);
-            c->launches += uint64_t(max_it) * (iteration_launches(q.mode, fused, chunks[k].grid_e, o.lm_max_iterations) + 1);   // + k_loop_cond
+            const bool coop = chunks[k].count <= 2 && chunks[k].grid_x <= kCoopMaxGrid && !c->no_coop_knn;
+            const uint64_t round2 = knn_graph_valid(c) && !coop ? 1 : 0;     // k_knn_round2
+            c->launches += uint64_t(max_it) * (iteration_launches(q.mode, fused, chunks[k].grid_e, o.lm_max_iterations) + 1 + round2);   // + k_loop_cond
         }
         for (size_t s = 0; s < n_scans; ++s) {
             if (results[s].status == SO_STATUS_NOT_ENOUGH_FEATURES || n_points[s] == 0) continue;
@@ -874,6 +900,7 @@ so_ctx* so_create(const so_config* cfg_in) {
     if (std::getenv("SO_FORCE_KEY64")) c->force_key64 = true;
     if (std::getenv("SO_FORCE_DROP_BIT")) c->force_drop_bit = true;
     if (std::getenv("SO_NO_DEC_UPLOAD")) c->no_dec_upload = true;
+    if (const char* e = std::getenv("SO_KNN_GRAPH")) c->knn_graph_mode = std::strcmp(e, "on") == 0 ? 1 : (std::strcmp(e, "off") == 0 ? -1 : 0);
     if (const char* e = std::getenv("SO_CHUNKS")) c->chunk_override = std::max(0, std::min(16, std::atoi(e)));      // profiling aid: ncu cannot see inside conditional-node bodies
     if (ctx_alloc(c) != SO_OK) { ctx_free(c); return nullptr; }
     return reinterpret_cast<so_ctx*>(c);
@@ -1633,7 +1660,10 @@ static int correspond_stage(Ctx* c, const void* surf, size_t n, size_t stride, s
     const Chunk ch{0, 1, 0, uint32_t(n), grid_x};
     rc = prepare_scans(c, c->d_scan, ch, c->stream, false);              // stage API reports every point: decimation stays inside the kernels
     if (rc) return rc;
-    const MapView mv = map_view(c, c->surf);
+    rc = knn_graph_prepare(c, 0);                                       // a stage call builds the neighbour graph only when it is forced on
+    if (!rc) rc = graph_queue_begin(c, 1);
+    if (rc) return rc;
+    const MapView mv = search_view(c);
     BatchView bv = batch_view(c, c->d_scan_sorted);
     bv.coop_knn = grid_x <= kCoopMaxGrid && !c->no_coop_knn;            // as a single small registration would search
     timed_launch_begin(c); launch_correspond(mv, bv, c->corr, c->nn, grid_x, 1, c->stream); c->launches += 2 + 2; timed_launch_end(c, 0);
@@ -2002,6 +2032,65 @@ int so_profile_get(so_ctx* ctx, int cls, double* ms, uint64_t* launches, int res
     if (ms) *ms = c->prof[cls].ms;
     if (launches) *launches = c->prof[cls].launches;
     if (reset) c->prof[cls] = ProfileSlot{};
+    return SO_OK;
+}
+
+int so_knn_graph(so_ctx* ctx, uint32_t* point_id, uint32_t* nbr_id, float* radius, size_t cap_points, uint32_t* k, size_t* n_out) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c || !n_out) return fail(SO_ERR_ARG, "null argument");
+    SO_CUDA_TRY(cudaSetDevice(c->device));
+    if (k) *k = uint32_t(kGraphK);
+    { int rc = ensure_maps(c); if (rc) return rc; }
+    MapStore& ms = c->surf;
+    *n_out = ms.n;
+    if (ms.n == 0) return SO_OK;
+    if (!knn_graph_valid(c)) {
+        const int mode = c->knn_graph_mode;
+        c->knn_graph_mode = 1;
+        const int rc = knn_graph_prepare(c, 0);
+        c->knn_graph_mode = mode;
+        if (rc) return rc;
+    }
+    if (!point_id || !nbr_id || !radius) return SO_OK;
+    if (cap_points < ms.n) return fail(SO_ERR_CAPACITY, "so_knn_graph: cap_points below the store's points");
+    std::vector<float4> sorted(ms.n);
+    std::vector<uint32_t> pos(size_t(ms.n) * kGraphK);
+    SO_CUDA_TRY(cudaMemcpyAsync(sorted.data(), ms.d_sorted, sorted.size() * sizeof(float4), cudaMemcpyDeviceToHost, c->stream));
+    SO_CUDA_TRY(cudaMemcpyAsync(pos.data(), ms.d_graph, pos.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
+    SO_CUDA_TRY(cudaMemcpyAsync(radius, ms.d_graph_radius, size_t(ms.n) * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+    SO_CUDA_TRY(cudaStreamSynchronize(c->stream));
+    for (size_t t = 0; t < ms.n; ++t) {
+        std::memcpy(&point_id[t], &sorted[t].w, 4);
+        for (int j = 0; j < kGraphK; ++j) {
+            const uint32_t p = pos[t * kGraphK + j];
+            uint32_t id = 0xFFFFFFFFu;
+            if (p != 0xFFFFFFFFu) std::memcpy(&id, &sorted[p].w, 4);
+            nbr_id[t * kGraphK + j] = id;
+        }
+    }
+    return SO_OK;
+}
+
+int so_knn_graph_stats(so_ctx* ctx, int on, uint64_t* counts) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c) return fail(SO_ERR_ARG, "null ctx");
+    SO_CUDA_TRY(cudaSetDevice(c->device));
+    const size_t bytes = 2 * SO_MAX_ICP_ITERS * sizeof(uint32_t);
+    if (counts) {
+        uint32_t h[2 * SO_MAX_ICP_ITERS] = {};
+        if (c->d_graph_stats) {
+            SO_CUDA_TRY(cudaMemcpyAsync(h, c->d_graph_stats, bytes, cudaMemcpyDeviceToHost, c->stream));
+            SO_CUDA_TRY(cudaStreamSynchronize(c->stream));
+        }
+        for (int i = 0; i < 2 * SO_MAX_ICP_ITERS; ++i) counts[i] = h[i];
+    }
+    if (on && !c->d_graph_stats) SO_CUDA_TRY(cudaMalloc(&c->d_graph_stats, bytes));
+    if (on) SO_CUDA_TRY(cudaMemsetAsync(c->d_graph_stats, 0, bytes, c->stream));
+    if (!on && c->d_graph_stats) {
+        SO_CUDA_TRY(cudaStreamSynchronize(c->stream));
+        cudaFree(c->d_graph_stats);
+        c->d_graph_stats = nullptr;
+    }
     return SO_OK;
 }
 

@@ -136,6 +136,12 @@ struct MapStore {
     int n_slots = 0;
     int nb = 64;                                   // cells per block axis
     bool dirty = true;                             // the index is not built for the current cloud, origin and resolution
+    uint64_t index_gen = 0;                        // bumped by every index build: a neighbour graph is valid for one index only
+    // neighbour graph of the sorted cloud (surf store; knn_graph_prepare): kGraphK positions per point, AoS, and the radius below
+    // which a row is complete.  Valid while graph_gen == index_gen and the store is clean.
+    uint32_t* d_graph = nullptr; size_t graph_cap = 0;      // [graph_cap][kGraphK]
+    float* d_graph_radius = nullptr; size_t radius_cap = 0;
+    uint64_t graph_gen = ~uint64_t(0);
     BlockArchive arc;
 };
 
@@ -170,6 +176,7 @@ struct Ctx {
     void* d_sort_tmp = nullptr; size_t sort_tmp_bytes = 0;
     void* d_sort_tmp2 = nullptr;                   // second radix-sort scratch: scan ordering of the chunks that run on aux_stream
     NnBuf nn{};
+    size_t queue_cap = 0, qcount_cap = 0;         // nn.queue / nn.qcount (allocated with the first neighbour graph a search uses)
     uint32_t* d_offset = nullptr;
     IcpState* d_state = nullptr;
     IcpState* h_state = nullptr;                   // pinned
@@ -196,6 +203,9 @@ struct Ctx {
     cudaEvent_t ev_dec = nullptr;                  // the deferred upload of the whole cloud has landed in d_scan
     struct { const void* src = nullptr; size_t n = 0, stride = 0, ioff = 0, stage_off = 0; } defer;      // pending whole-cloud upload (src == nullptr: none)
     bool no_dec_upload = false;                    // SO_NO_DEC_UPLOAD: A/B aid, always upload the whole cloud first
+    int knn_graph_mode = 0;                        // SO_KNN_GRAPH: test / A/B aid; 0 = built by the rule, 1 (on) = built for every search call,
+                                                   // -1 (off) = never used
+    uint32_t* d_graph_stats = nullptr;             // so_knn_graph_stats: [SO_MAX_ICP_ITERS][2] counters while on, else nullptr
 
     // ---- k-NN scratch -------------------------------------------------------------------------------------------
     float4* d_q = nullptr; uint32_t* d_knn_idx = nullptr; float* d_knn_d2 = nullptr;
@@ -214,6 +224,7 @@ struct Ctx {
         UndistortionMode mode; const void* und_time;   // the head of every iteration (NONE / nullptr: none)
         const void* und_edge;                          // APPROXIMATED with an edge cloud: the warped edge cloud the line branch reads
         const void* degen;                             // degeneracy-aware registration: the DegenState array (nullptr: off)
+        const void* graph[5];                          // MapView::graph, graph_radius, graph_stats of the surf view (nullptr: none), NnBuf::queue, qcount
     };
     struct GraphSlot {
         cudaGraphExec_t exec = nullptr;
@@ -412,6 +423,11 @@ int archive_segments(Ctx* c, MapStore& ms, uint32_t* n_segs, uint32_t* max_n);
 void shift_origin(const int32_t o[3], const double t[3], int32_t out[3], int32_t cc[3]);
 int move_window(Ctx* c, const int32_t o[3]);                // origin = o (both stores dirty when it changes), then ensure_maps
 MapView map_view(const Ctx* c, const MapStore& ms);
+// Neighbour graph of the surf store (so_knn.cuh): built for the current index when a search call of `queries` queries pays for it
+// (queries >= kGraphQueriesPerPoint x the store's points) or the graph is forced on, and none is valid
+int knn_graph_prepare(Ctx* c, size_t queries);
+bool knn_graph_valid(const Ctx* c);
+MapView search_view(const Ctx* c);      // map_view of the surf store with its graph when one is valid and the graph is not off
 int map_cells_per_block(float plane_res);
 int scan_sort_alloc(Ctx* c);             // temp storage for the per-registration scan sort
 int query_sort(Ctx* c, size_t n);         // d_qkeys/d_qvals -> *_out (allocates on growth)

@@ -570,8 +570,9 @@ __device__ __forceinline__ void accumulate(double acc[kAcc], const double n[3], 
 // ICP iterations after the first: the previous iteration's five neighbours still exist, so the largest of their (exact)
 // distances to the moved query bounds the new 5th-neighbour distance -- provided they lie in the block the query is in NOW
 // (the search is block-local, LocalMap.h:488-507: after a pose update that carries the point across a 50 m block face the old
-// neighbours belong to another block and bound nothing).  Returns the bound or -1 (no usable seed).
-__device__ __forceinline__ float seed_bound(const MapView& m, const QueryCell& qc, const NnBuf& nb, size_t gi, float qx, float qy, float qz) {
+// neighbours belong to another block and bound nothing).  Returns the bound or -1 (no usable seed); *pos0: the previous nearest
+// neighbour's position (in the query's block whenever the bound is returned).
+__device__ __forceinline__ float seed_bound(const MapView& m, const QueryCell& qc, const NnBuf& nb, size_t gi, float qx, float qy, float qz, uint32_t* pos0 = nullptr) {
     const uint32_t cells = uint32_t(m.nb) * uint32_t(m.nb) * uint32_t(m.nb);
     const uint32_t lo = __ldg(&m.cell_start[uint32_t(qc.slot) * cells]), hi = __ldg(&m.cell_start[uint32_t(qc.slot) * cells + cells]);
     float u = 0.f;
@@ -579,6 +580,7 @@ __device__ __forceinline__ float seed_bound(const MapView& m, const QueryCell& q
 #pragma unroll
     for (int j = 0; j < 5; ++j) {
         const uint32_t pos = nb.pos[size_t(j) * nb.cap + gi];
+        if (j == 0 && pos0) *pos0 = pos;
         same_block = same_block && pos >= lo && pos < hi;
         const float4 c = __ldg(&m.pts[same_block ? pos : lo]);
         const float dx = qx - c.x, dy = qy - c.y, dz = qz - c.z;
@@ -737,12 +739,17 @@ __global__ void __launch_bounds__(kSmallThreads) k_prepare_small(MapView m, Batc
 // Queries per CTA, measured on an H100 80GB HBM3 (700 W limit, scripts/ab_knn.py, 64 cfg2 scans = 8.4 M queries per launch):
 // 32 -> 1.08, 64 -> 1.05-1.07, 128 -> 1.07, 256 -> 1.11 ms per launch.  1024 / kKnnThreads CTAs per SM = 64 registers per thread.
 constexpr int kKnnThreads = 64;
+// GRAPH (the map has a neighbour graph, so_knn.cuh): a query the graph certifies is ranked from its anchor's row; any other goes to
+// nb.queue with its round-1 bound, and k_knn_round2 runs round 2 for the queue.  Round 2 in this kernel would cost a warp its full
+// length whenever one of its 32 lanes is not certified (at 82-91 % certified per lane almost every warp has one); the queue gathers
+// those queries into warps of their own, in roughly the scan's cell order (each warp appends its lanes in order).
+template <bool GRAPH>
 __global__ void __launch_bounds__(kKnnThreads, 1024 / kKnnThreads) k_knn_scan(MapView m, BatchView bv, NnBuf nb) {
     const int s = blockIdx.y;
     IcpState* st = bv.st + s;
     if (st->phase != PH_CORR) return;
     __shared__ double s_pose[7];
-    __shared__ uint32_t s_buf[kBufCap * kKnnThreads];
+    __shared__ uint32_t s_buf[GRAPH ? 1 : kBufCap * kKnnThreads];
     if (threadIdx.x < 7) s_pose[threadIdx.x] = st->x[threadIdx.x];
     __syncthreads();
     const uint32_t n = uint32_t(st->n_points);
@@ -754,6 +761,8 @@ __global__ void __launch_bounds__(kKnnThreads, 1024 / kKnnThreads) k_knn_scan(Ma
     int pre = SO_MATCH_SKIPPED;
     TopK<5> tk;
     tk.init(m.bound_d2);
+    bool searched = false, by_graph = false;
+    float U = 0.f;
     if (in_range && should_process(__float_as_uint(sp.w), st->sampling_rate)) {
         const double pin[3] = {double(sp.x), double(sp.y), double(sp.z)};
         double pf[3];
@@ -762,19 +771,86 @@ __global__ void __launch_bounds__(kKnnThreads, 1024 / kKnnThreads) k_knn_scan(Ma
         QueryCell qc;
         locate(m, qx, qy, qz, qc);
         if (qc.slot < 0 || qc.nblock < 5) pre = SO_MATCH_NOT_ENOUGH_NEIGHBORS;
-        else {
+        else if (!GRAPH) {
             const float u_seed = st->icp_iter > 0 && nb.pre[gi] == SO_MATCH_SUCCESS ? seed_bound(m, qc, nb, gi, qx, qy, qz) : -1.f;
             knn_select<5, true>(BlockGrid(m, qc.slot), m, qc, qx, qy, qz, u_seed, m.bound_d2, s_buf, tk);
             pre = tk.count() < 5 ? SO_MATCH_NEIGHBORS_TOO_FAR : SO_MATCH_SUCCESS;       // d2[4] > 3*planeRes_ (:741-744)
+        } else {
+            // anchor of the graph certificate: the previous iteration's nearest neighbour when it seeds the bound, else the nearest
+            // candidate round 1 saw
+            uint32_t anchor = 0xFFFFFFFFu;
+            const float u_seed = st->icp_iter > 0 && nb.pre[gi] == SO_MATCH_SUCCESS ? seed_bound(m, qc, nb, gi, qx, qy, qz, &anchor) : -1.f;
+            U = knn_bound<5, true>(BlockGrid(m, qc.slot), m, qc, qx, qy, qz, u_seed, m.bound_d2, &anchor);
+            searched = true;
+            by_graph = anchor != 0xFFFFFFFFu && graph_certified(m, anchor, qx, qy, qz, U);
+            if (by_graph) {
+                knn_graph_rank<5>(m, anchor, qx, qy, qz, U, tk);
+                pre = tk.count() < 5 ? SO_MATCH_NEIGHBORS_TOO_FAR : SO_MATCH_SUCCESS;
+            }
         }
     }
-    if (!in_range) return;
+    const bool defer = searched && !by_graph;
+    if (GRAPH) {                                       // every lane of the warp is still here
+        const int it = min(st->icp_iter, SO_MAX_ICP_ITERS - 1);
+        const uint32_t lane = threadIdx.x & 31;
+        const uint32_t dm = __ballot_sync(0xFFFFFFFFu, defer);
+        if (dm) {
+            const uint32_t lead = __ffs(dm) - 1;
+            uint32_t base = 0;
+            if (lane == lead) base = atomicAdd(&nb.qcount[s * SO_MAX_ICP_ITERS + it], uint32_t(__popc(dm)));
+            base = __shfl_sync(0xFFFFFFFFu, base, lead);
+            if (defer) {
+                nb.queue[bv.offset[s] + base + __popc(dm & ((1u << lane) - 1u))] = uint32_t(gi);
+                nb.d5[gi] = U;
+            }
+        }
+        if (m.graph_stats) {                           // so_knn_graph_stats
+            const uint32_t ns = __popc(__ballot_sync(0xFFFFFFFFu, searched)), ng = __popc(__ballot_sync(0xFFFFFFFFu, by_graph));
+            if (lane == 0) { atomicAdd(&m.graph_stats[2 * it], ns); atomicAdd(&m.graph_stats[2 * it + 1], ng); }
+        }
+    }
+    if (!in_range || defer) return;                    // a queued query's results come from k_knn_round2
     nb.pre[gi] = (unsigned char)pre;
     nb.d5[gi] = tk.d2[4];
 #pragma unroll
     for (int j = 0; j < 5; ++j) {
         const bool ok = tk.id[j] != 0xFFFFFFFFu;
         nb.pos[size_t(j) * nb.cap + gi] = ok ? tk.pos[j] : 0xFFFFFFFFu;
+    }
+}
+
+// k_knn_round2: round 2 of the select search for the queries k_knn_scan<true> queued, one per thread in queue order, with the bound
+// round 1 left in d5: the query, its cell and its bound are those k_knn_scan computed, so the result is the one it would have found.
+__global__ void __launch_bounds__(kKnnThreads, 1024 / kKnnThreads) k_knn_round2(MapView m, BatchView bv, NnBuf nb) {
+    const int s = blockIdx.y;
+    const IcpState* st = bv.st + s;
+    if (st->phase != PH_CORR) return;
+    const uint32_t cnt = nb.qcount[s * SO_MAX_ICP_ITERS + min(st->icp_iter, SO_MAX_ICP_ITERS - 1)];
+    if (blockIdx.x * kKnnThreads >= cnt) return;
+    __shared__ double s_pose[7];
+    __shared__ uint32_t s_buf[kBufCap * kKnnThreads];
+    if (threadIdx.x < 7) s_pose[threadIdx.x] = st->x[threadIdx.x];
+    __syncthreads();
+    const uint32_t j = blockIdx.x * kKnnThreads + threadIdx.x;
+    if (j >= cnt) return;
+    const size_t gi = nb.queue[bv.offset[s] + j];
+    const float U = nb.d5[gi];
+    const float4 sp = __ldg(&bv.scan[gi]);
+    const double pin[3] = {double(sp.x), double(sp.y), double(sp.z)};
+    double pf[3];
+    qrot(s_pose + 3, pin, pf);
+    const float qx = float(pf[0] + s_pose[0]), qy = float(pf[1] + s_pose[1]), qz = float(pf[2] + s_pose[2]);
+    QueryCell qc;
+    locate(m, qx, qy, qz, qc);
+    TopK<5> tk;
+    tk.init(m.bound_d2);
+    knn_gather<5>(BlockGrid(m, qc.slot), m, qc, qx, qy, qz, U, s_buf, tk);
+    nb.pre[gi] = (unsigned char)(tk.count() < 5 ? SO_MATCH_NEIGHBORS_TOO_FAR : SO_MATCH_SUCCESS);
+    nb.d5[gi] = tk.d2[4];
+#pragma unroll
+    for (int k = 0; k < 5; ++k) {
+        const bool ok = tk.id[k] != 0xFFFFFFFFu;
+        nb.pos[size_t(k) * nb.cap + gi] = ok ? tk.pos[k] : 0xFFFFFFFFu;
     }
 }
 
@@ -1779,7 +1855,10 @@ void launch_match(const MapView& m, const BatchView& bv, const CorrBuf& cb, cons
     if (!grid_x) return;
     if (part != 2) {
         if (bv.coop_knn) k_knn_scan_coop<<<dim3(grid_x * (kThreads / kCoopWarps), n_scans), kThreads, 0, st>>>(m, bv, nb);
-        else k_knn_scan<<<dim3(grid_x * (kThreads / kKnnThreads), n_scans), kKnnThreads, 0, st>>>(m, bv, nb);
+        else if (m.graph && nb.queue) {
+            k_knn_scan<true><<<dim3(grid_x * (kThreads / kKnnThreads), n_scans), kKnnThreads, 0, st>>>(m, bv, nb);
+            k_knn_round2<<<dim3(grid_x * (kThreads / kKnnThreads), n_scans), kKnnThreads, 0, st>>>(m, bv, nb);
+        } else k_knn_scan<false><<<dim3(grid_x * (kThreads / kKnnThreads), n_scans), kKnnThreads, 0, st>>>(m, bv, nb);
     }
     const uint32_t gf = (grid_x * kThreads + kFitPts * kFitThreads - 1) / (kFitPts * kFitThreads);
     if (part != 1) k_fit<<<dim3(gf, n_scans), kFitThreads, 0, st>>>(m, bv, cb, nb);

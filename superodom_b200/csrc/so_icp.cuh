@@ -46,6 +46,9 @@ struct NnBuf {
     float* d5;           // [cap] exact 5th-neighbour d2 of the last search (decides whether its neighbours seed the next one)
     unsigned char* pre;  // [cap] SO_MATCH_SKIPPED / NOT_ENOUGH_NEIGHBORS / NEIGHBORS_TOO_FAR / SUCCESS (= has 5 neighbours)
     size_t cap;
+    // with the neighbour graph (MapView::graph): the queries it did not answer, handed from k_knn_scan to k_knn_round2
+    uint32_t* queue;     // [cap] point indices, scan s's from offset[s] on; their round-1 bound waits in d5
+    uint32_t* qcount;    // [scans][SO_MAX_ICP_ITERS] queue lengths, zeroed before every registration call
 };
 
 constexpr uint32_t kCoopMaxGrid = 32;     // k_knn_scan_coop serves scans of up to 32 x 256 queries (a decimated live scan is ~2 000)

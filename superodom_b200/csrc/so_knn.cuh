@@ -20,6 +20,7 @@
 // (scan_order_key), so the lanes of a warp walk the same or neighbouring cell rows.
 #pragma once
 #include "so_icp.cuh"
+#include "so_graph_rule.h"
 
 namespace so {
 
@@ -217,22 +218,25 @@ __device__ __forceinline__ void walk_octant(const BlockGrid& g, int nb, float cs
 // Recorded candidates per query before round 2 falls back to direct insertion.
 constexpr int kBufCap = 24;
 
-// s_buf: [kBufCap][blockDim.x] positions, column = this thread.  u_seed < 0: no seed.  `bound`: neighbours farther than this
-// (squared) are not wanted; tk must have been initialised with it.  Complete for d2 <= min(bound, (R*cs)^2).  On return tk.pos
-// holds positions in the sorted map.
+// Rounds 1 and 2 of the select search.  s_buf: [kBufCap][blockDim.x] positions, column = this thread.  u_seed < 0: no seed.
+// `bound`: neighbours farther than this (squared) are not wanted; tk must have been initialised with it.  Complete for
+// d2 <= min(bound, (R*cs)^2).  On return tk.pos holds positions in the sorted map.
 // OCT: round 1 over the 2x2x2 nearest cells (measured: -7 % on scans, whose lanes sit in different cells anyway) or over the 27
 // cells of ring 1 (dense query sets such as cfg5: lanes that share a cell then read the same rows; the octant splits them, +10 %).
+// Round 1 returns U; unless seeded it sets *anchor to the position of the nearest candidate it saw (0xFFFFFFFF: none).
 template <int K, bool OCT>
-__device__ __forceinline__ void knn_select(const BlockGrid& g, const MapView& m, const QueryCell& qc, float qx, float qy, float qz, float u_seed, float bound,
-                                           uint32_t* s_buf, TopK<K>& tk) {
+__device__ __forceinline__ float knn_bound(const BlockGrid& g, const MapView& m, const QueryCell& qc, float qx, float qy, float qz, float u_seed, float bound,
+                                           uint32_t* anchor) {
     float U;
     if (u_seed >= 0.f) U = u_seed * 1.000004f;
     else {
+        *anchor = 0xFFFFFFFFu;
         float a[K];                                                            // K smallest approx d2 so far, ascending
 #pragma unroll
         for (int j = 0; j < K; ++j) a[j] = bound;
-        auto net = [&](const float4 c, uint32_t) {
+        auto net = [&](const float4 c, uint32_t e) {
             const float d = approx_d2(c, qx, qy, qz);
+            if (d < a[0]) *anchor = e;
 #pragma unroll
             for (int j = K - 1; j > 0; --j) a[j] = fminf(a[j], fmaxf(a[j - 1], d));
             a[0] = fminf(a[0], d);
@@ -243,7 +247,12 @@ __device__ __forceinline__ void knn_select(const BlockGrid& g, const MapView& m,
         else walk_cube(g, m.nb, m.cs, qc, bound, 1, net);
         U = a[K - 1] * 1.000004f;
     }
-    U = fminf(U, bound * 1.000004f);
+    return fminf(U, bound * 1.000004f);
+}
+
+template <int K>
+__device__ __forceinline__ void knn_gather(const BlockGrid& g, const MapView& m, const QueryCell& qc, float qx, float qy, float qz, float U,
+                                           uint32_t* s_buf, TopK<K>& tk) {
     int cnt = 0;
     const int stride = blockDim.x;
     walk_cube(g, m.nb, m.cs, qc, U, m.R, [&](const float4 c, uint32_t e) {
@@ -256,6 +265,53 @@ __device__ __forceinline__ void knn_select(const BlockGrid& g, const MapView& m,
         const uint32_t e = s_buf[k * stride + threadIdx.x];
         const float4 c = g.load(e);
         tk.offer(exact_d2(c, qx, qy, qz), __float_as_uint(c.w), e);
+    }
+}
+
+template <int K, bool OCT>
+__device__ __forceinline__ void knn_select(const BlockGrid& g, const MapView& m, const QueryCell& qc, float qx, float qy, float qz, float u_seed, float bound,
+                                           uint32_t* s_buf, TopK<K>& tk) {
+    uint32_t anchor = 0xFFFFFFFFu;
+    const float U = knn_bound<K, OCT>(g, m, qc, qx, qy, qz, u_seed, bound, &anchor);
+    knn_gather<K>(g, m, qc, qx, qy, qz, U, s_buf, tk);
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// Neighbour graph (k_knn_scan): row a of MapView::graph holds the positions of the kGraphK nearest in-block points of map point a
+// (a excluded, (d2, id) order, exact_d2), radius[a] = 0.99999 sqrt(d2 of the last of them): every in-block point p with
+// |a - p| < radius[a] is in the row.  A block with at most kGraphK other points puts all of them in the row, radius +inf; a point
+// its own search does not return (more than kGraphK duplicates with smaller ids) gets radius 0 (never certifies).
+//
+// Certificate: a query q with round-1 bound U and an anchor a in its block.  Every point the select search could return lies within
+// sqrt(U) of q (U bounds the 5th distance, walk filter approx_d2 <= U), so within sqrt(U) + |q - a| of a; when that is below
+// radius[a], {a} + row a holds all of them, and ranking those few candidates gives exactly the select search's result: the same
+// top-5 in (d2, id) order over any candidate set between the true five and the block.  Error budget: approx_d2, exact_d2 and the
+// float square roots are within ~5e-7 of the true distances; the 0.99999 in radius is 20 times that.  A NaN or infinite term
+// fails the test (the comparison is false), so such queries take round 2.
+// ------------------------------------------------------------------------------------------------------------------
+// Anchor a certifies the query: then knn_graph_rank gives the select search's result.
+__device__ __forceinline__ bool graph_certified(const MapView& m, uint32_t a, float qx, float qy, float qz, float U) {
+    return graph_certifies(U, exact_d2(__ldg(&m.pts[a]), qx, qy, qz), __ldg(&m.graph_radius[a]));
+}
+
+// Ranks {a} + row a into tk (a certified anchor).
+template <int K>
+__device__ __forceinline__ void knn_graph_rank(const MapView& m, uint32_t a, float qx, float qy, float qz, float U, TopK<K>& tk) {
+    const float4 ca = __ldg(&m.pts[a]);
+    tk.offer(exact_d2(ca, qx, qy, qz), __float_as_uint(ca.w), a);
+    const uint4* row = m.graph + size_t(a) * (kGraphK / 4);
+    const float4 far = make_float4(3.0e18f, 3.0e18f, 3.0e18f, 0.f);
+    auto one = [&](const float4 c, uint32_t e) {
+        if (approx_d2(c, qx, qy, qz) <= U) tk.offer(exact_d2(c, qx, qy, qz), __float_as_uint(c.w), e);
+    };
+#pragma unroll 1
+    for (int j = 0; j < kGraphK / 4; ++j) {
+        const uint4 e = __ldg(row + j);                  // empty slots (0xFFFFFFFF) only in blocks of <= kGraphK points: a dummy that fails the filter
+        const float4 c0 = e.x != 0xFFFFFFFFu ? __ldg(&m.pts[e.x]) : far;
+        const float4 c1 = e.y != 0xFFFFFFFFu ? __ldg(&m.pts[e.y]) : far;
+        const float4 c2 = e.z != 0xFFFFFFFFu ? __ldg(&m.pts[e.z]) : far;
+        const float4 c3 = e.w != 0xFFFFFFFFu ? __ldg(&m.pts[e.w]) : far;
+        one(c0, e.x); one(c1, e.y); one(c2, e.z); one(c3, e.w);
     }
 }
 

@@ -112,6 +112,7 @@ void map_free(Ctx* c) {
     for (MapStore* ms : {&c->surf, &c->edge}) {
         cudaFree(ms->d_xyzi); cudaFree(ms->d_sorted); cudaFree(ms->d_block_slot); cudaFree(ms->d_block_count); cudaFree(ms->d_cell_start);
         cudaFree(ms->arc.d_pool); cudaFree(ms->arc.d_segs);
+        cudaFree(ms->d_graph); cudaFree(ms->d_graph_radius);
     }
     cudaFree(c->d_keys); cudaFree(c->d_keys_out); cudaFree(c->d_vals); cudaFree(c->d_vals_out); cudaFree(c->d_cub_tmp);
     cudaFree(c->d_map_scratch);
@@ -127,6 +128,77 @@ MapView map_view(const Ctx* c, const MapStore& ms) {
     m.inv_bound_d2 = 1.0 / double(m.bound_d2);
     m.plane_res = ms.res;
     m.R = map_rings(ms.res, ms.nb);
+    m.graph = nullptr; m.graph_radius = nullptr; m.graph_stats = nullptr;
+    return m;
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// Neighbour graph of the sorted cloud (so_knn.cuh): row t = the kGraphK nearest in-block points of point t, from the exact in-block
+// search for kGraphK + 1 neighbours with t itself dropped, and the radius below which the row is complete.  A point the search does
+// not return (more than kGraphK duplicates with smaller ids) or whose block lookup disagrees with its place in the index gets radius 0.
+// ------------------------------------------------------------------------------------------------------------------
+constexpr int kGraphThreads = 64;
+__global__ void __launch_bounds__(kGraphThreads) k_knn_graph(MapView m, uint32_t n, uint32_t* __restrict__ graph, float* __restrict__ radius) {
+    __shared__ uint32_t s_buf[kBufCap * kGraphThreads];
+    const uint32_t t = blockIdx.x * kGraphThreads + threadIdx.x;
+    if (t >= n) return;                                          // no CTA-wide synchronisation below
+    const float4 p = m.pts[t];
+    QueryCell qc;
+    locate(m, p.x, p.y, p.z, qc);
+    uint32_t* row = graph + size_t(t) * kGraphK;
+    int j = 0;
+    float r = 0.f;
+    if (qc.slot >= 0) {
+        const uint32_t cells = uint32_t(m.nb) * uint32_t(m.nb) * uint32_t(m.nb);
+        const uint32_t lo = m.cell_start[uint32_t(qc.slot) * cells], hi = m.cell_start[uint32_t(qc.slot) * cells + cells];
+        if (t >= lo && t < hi) {
+            TopK<kGraphK + 1> tk;
+            tk.init(FLT_MAX);
+            knn_search<kGraphK + 1>(BlockGrid(m, qc.slot), m, qc, p.x, p.y, p.z, 0.f, s_buf, tk);
+            bool self = false;
+            float last = 0.f;
+#pragma unroll
+            for (int i = 0; i < kGraphK + 1; ++i) {
+                // a block of at most kGraphK points also hands back the far-away dummies its walks pad spans with (for_span): entries
+                // whose position does not hold the point they name
+                const bool real = tk.id[i] != 0xFFFFFFFFu && tk.pos[i] >= lo && tk.pos[i] < hi && __float_as_uint(m.pts[tk.pos[i]].w) == tk.id[i] &&
+                                  exact_d2(m.pts[tk.pos[i]], p.x, p.y, p.z) == tk.d2[i];
+                const bool me = real && tk.pos[i] == t;
+                self |= me;
+                if (real && !me && j < kGraphK) { row[j++] = tk.pos[i]; last = tk.d2[i]; }
+            }
+            if (self) r = (hi - lo - 1u <= uint32_t(kGraphK)) ? INFINITY : kGraphRadiusScale * sqrtf(last);
+        }
+    }
+    for (; j < kGraphK; ++j) row[j] = 0xFFFFFFFFu;
+    radius[t] = r;
+}
+
+bool knn_graph_valid(const Ctx* c) {
+    const MapStore& ms = c->surf;
+    return c->knn_graph_mode >= 0 && !ms.dirty && ms.n > 0 && ms.graph_gen == ms.index_gen && ms.d_graph;
+}
+
+int knn_graph_prepare(Ctx* c, size_t queries) {
+    MapStore& ms = c->surf;
+    if (ms.dirty || knn_graph_valid(c) || !graph_build_due(c->knn_graph_mode, queries, ms.n)) return SO_OK;
+    int rc = grow_buffer(ms.d_graph, ms.graph_cap, size_t(ms.n) * kGraphK);
+    if (!rc) rc = grow_buffer(ms.d_graph_radius, ms.radius_cap, size_t(ms.n));
+    if (rc) return rc;
+    k_knn_graph<<<(ms.n + kGraphThreads - 1) / kGraphThreads, kGraphThreads, 0, c->stream>>>(map_view(c, ms), ms.n, ms.d_graph, ms.d_graph_radius);
+    c->launches++;
+    SO_CUDA_TRY(cudaGetLastError());
+    ms.graph_gen = ms.index_gen;
+    return SO_OK;
+}
+
+MapView search_view(const Ctx* c) {
+    MapView m = map_view(c, c->surf);
+    if (knn_graph_valid(c)) {
+        m.graph = reinterpret_cast<const uint4*>(c->surf.d_graph);
+        m.graph_radius = c->surf.d_graph_radius;
+        m.graph_stats = c->d_graph_stats;
+    }
     return m;
 }
 
@@ -445,6 +517,7 @@ static int index_cells(Ctx* c, MapStore& ms, uint32_t n_max, uint32_t slot_cap) 
     ms.n = h_info->n_out;
     ms.n_slots = int(h_info->n_slots);
     ms.dirty = h_info->error != 0;
+    ms.index_gen++;
     return SO_OK;
 }
 
@@ -485,6 +558,7 @@ static int set_empty_index(Ctx* c, MapStore& ms) {
     std::fill(ms.h_block_slot.begin(), ms.h_block_slot.end(), -1);
     ms.n_slots = 0;
     ms.dirty = false;
+    ms.index_gen++;
     return SO_OK;
 }
 
