@@ -236,6 +236,48 @@ int so_map_archive_info(so_ctx* ctx, int store, size_t* n_points, size_t* n_bloc
  * loaded with so_map_set_points, it is the next session's prior map. */
 int so_map_download_all(so_ctx* ctx, int store, float* out_xyzi, size_t cap_points, size_t* n_out);
 
+/* ---- keyframes: registered scans kept on the device, and the map rebuilt from them after a loop closure --------------------------
+ * No reference counterpart (the reference is an odometry front end).  What a loop-closing back end needs from the device: the scans
+ * with their poses, a submap built from chosen scans to register a kept scan against (the loop constraint: pose and cov), and the map
+ * rebuilt from every keyframe once the caller's pose graph has moved them.  The pose graph itself stays with the caller.  Off until
+ * so_keyframe_reserve; nothing else calls these, and no other call changes behaviour.
+ * so_keyframe_reserve: one pool of cap_points points for surf clouds and one for edge clouds, and room for cap_frames keyframes; again
+ * with other values to resize (contents kept); 0, 0 frees the store.  SO_ERR_ARG when only one of the two is 0 or when either is below
+ * what the store holds. */
+int so_keyframe_reserve(so_ctx* ctx, size_t cap_points, size_t cap_frames);
+/* Keep the scan of the last single-scan registration (and its edge cloud when it had one) as keyframe *id (0, 1, ... in call order),
+ * with pose.  Each cloud is kept exactly as so_map_add_registered_scan / so_map_add_registered_edges would place it before the world
+ * transform: in the sensor frame and, after APPROXIMATED / OPTIMIZED registration, compensated with pose as the insert would be.  The
+ * map is not touched.  SO_ERR_ARG, before any device work, without a store, for a non-finite pose, before the first registration or
+ * after one of an empty scan, and whenever so_map_add_registered_scan would fail (or so_map_add_registered_edges, when the
+ * registration had an edge cloud).  SO_ERR_CAPACITY
+ * with the store unchanged when a pool or the frame table is full. */
+int so_keyframe_add_registered(so_ctx* ctx, const double pose[7], int32_t* id);
+/* Keyframes held and the points of the surf and edge pools; any pointer may be NULL. */
+int so_keyframe_info(so_ctx* ctx, size_t* n_frames, size_t* n_points, size_t* n_edge_points);
+/* The keyframes' poses, [*n][7]; only cap are written.  A pose is the one the keyframe was added with, or the one the last
+ * so_map_from_keyframes of its own context (dst == src) rebuilt it at. */
+int so_keyframe_poses(so_ctx* ctx, double* out7, size_t cap, size_t* n);
+/* Keyframe id of store 0 (surf) or 1 (edge) as packed float4 {x,y,z,intensity}: in the sensor frame (pose7 NULL), or at pose7 by the
+ * device arithmetic of so_map_add_scan and so_map_from_keyframes (qrot in double, float store).  *n_out = its points; only cap_points
+ * are written.  SO_ERR_ARG for an id the store does not hold. */
+int so_keyframe_download(so_ctx* ctx, int32_t id, int store, const double pose7[7], float* out_xyzi, size_t cap_points, size_t* n_out);
+/* Replace the selected stores of dst (stores: 1 surf, 2 edge, 3 both) with the map of src's keyframes ids[0..n_ids), keyframe ids[i]
+ * at poses7[i].  dst == src is the rebuild after a pose-graph correction (the keyframes' poses become poses7); another context on the
+ * same device builds a loop-verification submap.  The result, under dst's origin and leaf (planeRes surf, lineRes edge):
+ *   - the union is the keyframes in ids order, each in its point order, each point transformed as so_keyframe_download(pose) does;
+ *   - every 50 m block of the union is filtered on its own, as an insert filters a touched block (pcl::VoxelGrid, centroids summed in
+ *     union order); the window's blocks make the window's cloud, block by block;
+ *   - with the block archive on, every block outside the window is filtered the same way and becomes dst's archive; with it off,
+ *     those blocks are dropped, as an insert drops them.
+ * One filter over the union, not a replay of inserts (which average centroids of centroids): rebuilding at unchanged poses gives a
+ * different, cleaner map than the live one.  The rebuilt stores hold their keyframes and nothing else: a prior map loaded with
+ * so_map_set_points, and points free-space clearing removed, are not kept.  The index is rebuilt as by any map change.
+ * SO_ERR_ARG, before any device work, for contexts on different devices, an id src does not hold, a non-finite pose or stores outside
+ * 1..3.  SO_ERR_CAPACITY, with both stores as they were, when the window's points exceed max_map_points, the off-window blocks exceed
+ * the archive, the window's blocks exceed the cell table, or 2^31 points or more are selected. */
+int so_map_from_keyframes(so_ctx* dst, so_ctx* src, const int32_t* ids, size_t n_ids, const double* poses7, int stores);
+
 /* ---- free-space clearing: take out the map points a scan sees through (moving objects) ---------------------------------------
  * No reference counterpart (LocalMap::addSurfPointCloud only adds points).  Off unless called; nothing else calls it.
  * Rule (DESIGN.md §2): the scan, in the frame of pose with the sensor at the pose's origin, is projected to a range image in FP64 --
@@ -374,6 +416,12 @@ int so_register_batch_edges(so_ctx* ctx, const void* surf_xyzi, const uint32_t* 
  * Used for the device-resident throughput figure; results are still copied back to host structs. */
 int so_register_batch_device(so_ctx* ctx, const void* d_scans_xyzi, const uint32_t* n_points, size_t n_scans,
                              const double* poses_in, const so_icp_opts* opts, so_icp_result* results);
+/* Keyframes ids[0..n) of src (surf clouds; see so_keyframe_add_registered) registered against dst's map from priors7[n][7], read on the
+ * device as so_register_batch_device reads device scans: mode NONE (a keyframe is already compensated), the map does not shift, dst's
+ * registered scan is untouched and a pose sink gets n rows.  results[i].pose and .cov give a loop factor.  dst and src may be the same
+ * context.  SO_ERR_ARG for contexts on different devices or an id src does not hold; SO_ERR_CAPACITY as so_register_batch_device. */
+int so_register_keyframes(so_ctx* dst, so_ctx* src, const int32_t* ids, size_t n, const double* priors7, const so_icp_opts* opts,
+                          so_icp_result* results);
 
 /* ---- within-scan motion compensation (LidarSlam.h:65-82 UndistortionMode; empty upstream, LidarSlam.cpp:382-400) ------------
  * A constant body-velocity model, re-estimated at the start of every ICP iteration from the current estimate T_cur:

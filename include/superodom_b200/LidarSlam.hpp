@@ -125,8 +125,11 @@ inline void point_layout(size_t* stride, size_t* ioff) {
     *ioff = size_t(reinterpret_cast<const char*>(&p.intensity) - reinterpret_cast<const char*>(&p));
 }
 
+class LidarSLAM;
+
 // ------------------------------------------------------------------------------------------------ LocalMap (LocalMap.h:123-766)
 class LocalMap {
+    friend class LidarSLAM;                    // alignKeyframes registers against another LocalMap's context
 public:
     static constexpr int laserCloudWidth = 21, laserCloudHeight = 21, laserCloudDepth = 11;
     static constexpr int laserCloudNum = laserCloudWidth * laserCloudHeight * laserCloudDepth;
@@ -220,6 +223,33 @@ public:
         return to_cloud<Cloud>(buf, n);
     }
 
+    // Shim only: keyframes (so_keyframe_*) for a loop-closing back end.  Room for `points` points in each of the surf and edge pools
+    // and for `frames` keyframes (0, 0 frees them); LidarSLAM::addKeyframe fills them.
+    void reserveKeyframes(size_t points, size_t frames) {
+        sync_resolution();
+        check(so_keyframe_reserve(ctx_->h, points, frames), "so_keyframe_reserve");
+    }
+    // The keyframes' poses: as added, or as the last rebuild (LidarSLAM::rebuildFromKeyframes) placed them
+    std::vector<Transformd> keyframePoses() const {
+        std::vector<Transformd> out;
+        if (!ctx_->h) return out;
+        size_t n = 0;
+        check(so_keyframe_poses(ctx_->h, nullptr, 0, &n), "so_keyframe_poses");
+        std::vector<double> p(7 * n);
+        check(so_keyframe_poses(ctx_->h, p.data(), n, &n), "so_keyframe_poses");
+        for (size_t i = 0; i < n; ++i) out.push_back(Transformd::from_pose7(p.data() + 7 * i));
+        return out;
+    }
+    // This map's stores (surf and edge) replaced by the map of src's keyframes ids, keyframe ids[i] at poses[i]
+    // (so_map_from_keyframes): a loop-verification submap, or with src == *this the rebuild after a pose-graph correction.  The map is
+    // then exactly its keyframes: a prior map loaded with loadPriorMap and free-space removals are not kept.
+    void buildFromKeyframes(const LocalMap& src, const std::vector<int32_t>& ids, const std::vector<Transformd>& poses) {
+        if (ids.size() != poses.size()) throw Error("buildFromKeyframes: one pose per keyframe id");
+        sync_resolution();
+        std::vector<double> p(7 * poses.size());
+        for (size_t i = 0; i < poses.size(); ++i) poses[i].to_pose7(p.data() + 7 * i);
+        check(so_map_from_keyframes(ctx_->h, src.ctx_->h, ids.data(), ids.size(), p.data(), 3), "so_map_from_keyframes");
+    }
     void sync_resolution() {
         ctx_->ensure(lineRes_, planeRes_);
         if (lineRes_ != pushed_line_ || planeRes_ != pushed_plane_) {
@@ -485,6 +515,42 @@ public:
     template <class CloudPtr>
     int globalLocalizeInWholeMap(const CloudPtr& planner_point, const Transformd& centre, so_global_opts opts) {
         return localizeInBox(planner_point, centre, opts, true);
+    }
+
+    // Shim only: loop closure (so_keyframe_*, so_register_keyframes, so_map_from_keyframes; INTEGRATION.md "Loop closure").
+    // addKeyframe keeps the scan the last Localization() registered, at T_w_lidar, and returns its id (localMap.reserveKeyframes first).
+    int32_t addKeyframe() {
+        double pose[7];
+        T_w_lidar.to_pose7(pose);
+        int32_t id = -1;
+        check(so_keyframe_add_registered(context.h, pose, &id), "so_keyframe_add_registered");
+        return id;
+    }
+    std::vector<Transformd> keyframePoses() const { return localMap.keyframePoses(); }
+    // The keyframes ids registered against `submap` from priors (mode NONE: a keyframe is already compensated), with this SLAM's ICP
+    // options: each result's pose and cov give a loop factor.  The live map and the registered scan are not touched.
+    std::vector<so_icp_result> alignKeyframes(LocalMap& submap, const std::vector<int32_t>& ids, const std::vector<Transformd>& priors) {
+        if (ids.size() != priors.size()) throw Error("alignKeyframes: one prior per keyframe id");
+        submap.sync_resolution();
+        so_icp_opts o{};
+        o.max_icp_iters = int32_t(LocalizationICPMaxIter);
+        o.max_surface_features = OptSet.max_surface_features;
+        o.lm_max_iterations = 4;
+        o.yaw_ratio = OptSet.yaw_ratio;
+        std::vector<double> p(7 * priors.size());
+        for (size_t i = 0; i < priors.size(); ++i) priors[i].to_pose7(p.data() + 7 * i);
+        std::vector<so_icp_result> out(ids.size());
+        check(so_register_keyframes(submap.ctx_->h, context.h, ids.data(), ids.size(), p.data(), &o, out.data()), "so_register_keyframes");
+        return out;
+    }
+    // The map rebuilt from every keyframe at the corrected poses (one per keyframe, in id order), both stores; T_w_lidar and
+    // last_T_w_lidar become the corrected pose of the last keyframe, so the next Localization() continues from the corrected map.
+    void rebuildFromKeyframes(const std::vector<Transformd>& corrected) {
+        std::vector<int32_t> ids(corrected.size());
+        for (size_t i = 0; i < ids.size(); ++i) ids[i] = int32_t(i);
+        localMap.buildFromKeyframes(localMap, ids, corrected);
+        if (!corrected.empty()) { T_w_lidar = corrected.back(); last_T_w_lidar = T_w_lidar; }
+        undistort_prev_pose = T_w_lidar;
     }
 
     // LidarSLAM::EstimateLidarUncertainty (LidarSlam.cpp:915-975)

@@ -27,6 +27,8 @@ EXPORTS = [
     "so_register_degeneracy", "so_register_batch_degeneracy", "so_degeneracy_analysis", "so_solve",
     "so_knn", "so_knn_device", "so_sampling_indices", "so_localize_global", "so_localize_scores", "so_localize_global_size", "so_localize_global_bnb", "so_localize_bnb_keys", "so_localize_bnb_bounds", "so_map_bounds", "so_map_bounds_all", "so_kernel_launches", "so_bytes_copied", "so_build_flags", "so_profile_enable", "so_profile_get",
     "so_knn_graph", "so_knn_graph_stats",
+    "so_keyframe_reserve", "so_keyframe_add_registered", "so_keyframe_info", "so_keyframe_poses", "so_keyframe_download", "so_map_from_keyframes",
+    "so_register_keyframes",
 ]
 
 
@@ -306,6 +308,13 @@ def load_library():
     L.so_profile_get.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int]
     L.so_knn_graph.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
     L.so_knn_graph_stats.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+    L.so_keyframe_reserve.argtypes = [C.c_void_p, C.c_size_t, C.c_size_t]
+    L.so_keyframe_add_registered.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+    L.so_keyframe_info.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.so_keyframe_poses.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
+    L.so_keyframe_download.argtypes = [C.c_void_p, C.c_int32, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
+    L.so_map_from_keyframes.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_int]
+    L.so_register_keyframes.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p]
     _lib = L
     return L
 
@@ -530,6 +539,60 @@ class Context:
             out = np.zeros((cap, 4), np.float32)
             self._chk(self.L.so_map_download_all(self.h, store, _p(out), cap, C.byref(n)), "so_map_download_all")
         return out[: n.value]
+
+    # ---- keyframes (off until keyframe_reserve): registered scans kept on the device, the map rebuilt from them
+    def keyframe_reserve(self, cap_points: int, cap_frames: int):
+        """Room for cap_points points in each of the surf and edge pools and for cap_frames keyframes; 0, 0 frees the store."""
+        self._chk(self.L.so_keyframe_reserve(self.h, int(cap_points), int(cap_frames)), "so_keyframe_reserve")
+
+    def keyframe_add_registered(self, pose7) -> int:
+        """Keep the scan (and edge cloud) of the last single-scan register*() as a keyframe at pose7 -> its id."""
+        pose = np.ascontiguousarray(pose7, dtype=np.float64)
+        i = C.c_int32()
+        self._chk(self.L.so_keyframe_add_registered(self.h, _p(pose), C.byref(i)), "so_keyframe_add_registered")
+        return i.value
+
+    def keyframe_info(self):
+        """-> (keyframes, surf pool points, edge pool points)"""
+        f, p, e = C.c_size_t(), C.c_size_t(), C.c_size_t()
+        self._chk(self.L.so_keyframe_info(self.h, C.byref(f), C.byref(p), C.byref(e)), "so_keyframe_info")
+        return f.value, p.value, e.value
+
+    def keyframe_poses(self) -> np.ndarray:
+        n = C.c_size_t()
+        self._chk(self.L.so_keyframe_poses(self.h, None, 0, C.byref(n)), "so_keyframe_poses")
+        out = np.zeros((n.value, 7), np.float64)
+        if n.value:
+            self._chk(self.L.so_keyframe_poses(self.h, _p(out), n.value, C.byref(n)), "so_keyframe_poses")
+        return out
+
+    def keyframe_download(self, kf_id: int, store: int = 0, pose7=None) -> np.ndarray:
+        """Keyframe kf_id of store 0 (surf) or 1 (edge): sensor frame, or at pose7 as the rebuild transforms it."""
+        pose = np.ascontiguousarray(pose7, dtype=np.float64) if pose7 is not None else None
+        n = C.c_size_t()
+        self._chk(self.L.so_keyframe_download(self.h, int(kf_id), int(store), _p(pose) if pose is not None else None, None, 0, C.byref(n)),
+                  "so_keyframe_download")
+        out = np.zeros((max(n.value, 1), 4), np.float32)
+        self._chk(self.L.so_keyframe_download(self.h, int(kf_id), int(store), _p(pose) if pose is not None else None, _p(out), n.value,
+                                              C.byref(n)), "so_keyframe_download")
+        return out[: n.value]
+
+    def map_from_keyframes(self, src: "Context", ids, poses, stores: int = 3):
+        """Replace the selected stores (1 surf, 2 edge, 3 both) with the map of src's keyframes ids at poses [n, 7]."""
+        ids = np.ascontiguousarray(ids, dtype=np.int32)
+        poses = np.ascontiguousarray(poses, dtype=np.float64).reshape(-1, 7)
+        assert len(ids) == len(poses)
+        self._chk(self.L.so_map_from_keyframes(self.h, src.h, _p(ids), len(ids), _p(poses), int(stores)), "so_map_from_keyframes")
+
+    def register_keyframes(self, src: "Context", ids, priors, max_icp_iters: int, max_surface_features: int = 0, **kw):
+        """src's keyframes ids registered against this context's map from priors [n, 7] -> [IcpResult]"""
+        ids = np.ascontiguousarray(ids, dtype=np.int32)
+        priors = np.ascontiguousarray(priors, dtype=np.float64).reshape(-1, 7)
+        assert len(ids) == len(priors)
+        o = self._opts(max_icp_iters, max_surface_features, **kw)
+        res = (IcpResult * len(ids))()
+        self._chk(self.L.so_register_keyframes(self.h, src.h, _p(ids), len(ids), _p(priors), C.byref(o), res), "so_register_keyframes")
+        return list(res)
 
     # ---- free-space clearing (off unless called)
     @staticmethod

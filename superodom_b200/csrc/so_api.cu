@@ -179,6 +179,7 @@ static void ctx_free(Ctx* c) {
     cudaFree(c->deg.d_st);
     features_free(c);
     free_space_free(c);
+    keyframes_free(c);
     if (c->ev_dec) cudaEventDestroy(c->ev_dec);
     if (c->ev0) cudaEventDestroy(c->ev0);
     if (c->ev1) cudaEventDestroy(c->ev1);
@@ -857,6 +858,20 @@ static RegisterRequest batch_request(const void* surf, const uint32_t* n_points,
     return q;
 }
 
+// dst[0..n) = the registered scan (Ctx::reg), still in d_scan, compensated for its motion as it was registered; with edges, its edge
+// cloud, still in d_escan (left by so_register, so_register_undistort_edges and so_register_optimized_edges).  The map inserts place it
+// at a store's tail, so_keyframe_add_registered at the keyframe pools' tails.
+int put_registered_scan(Ctx* c, bool edges, float4* dst, const double pose[7]) {
+    const RegisteredScan& r = c->reg;
+    SO_CUDA_TRY(cudaMemcpyAsync(dst, edges ? c->d_escan : c->d_scan, size_t(edges ? r.n_edge : r.n) * sizeof(float4),
+                                cudaMemcpyDeviceToDevice, c->stream));
+    switch (r.mode) {
+        case UndistortionMode::APPROXIMATED: return edges ? undistort_edge_tail(c, dst, r, pose) : undistort_tail(c, dst, r, pose);
+        case UndistortionMode::OPTIMIZED: return edges ? motion_edge_tail(c, dst, r) : motion_tail(c, dst, r);   // u(D_opt), whatever the pose
+        default: return SO_OK;
+    }
+}
+
 }  // namespace so
 
 // =================================================================================================== C ABI
@@ -987,20 +1002,6 @@ static int store_set_points(Ctx* c, MapStore& ms, const void* xyzi, size_t n, si
     ms.n = uint32_t(n);
     return map_rebuild(c, ms);
 }
-// ms tail = the registered scan (Ctx::reg), still in d_scan, compensated for its motion as it was registered; for the edge store, its
-// edge cloud, still in d_escan (left by so_register, so_register_undistort_edges and so_register_optimized_edges)
-static int put_registered_scan(Ctx* c, MapStore& ms, const double pose[7]) {
-    const RegisteredScan& r = c->reg;
-    const bool edges = &ms == &c->edge;
-    SO_CUDA_TRY(cudaMemcpyAsync(ms.d_xyzi + ms.n, edges ? c->d_escan : c->d_scan, size_t(edges ? r.n_edge : r.n) * sizeof(float4),
-                                cudaMemcpyDeviceToDevice, c->stream));
-    switch (r.mode) {
-        case UndistortionMode::APPROXIMATED: return edges ? undistort_edge_tail(c, ms, r, pose) : undistort_tail(c, ms, r, pose);
-        case UndistortionMode::OPTIMIZED: return edges ? motion_edge_tail(c, ms, r) : motion_tail(c, ms, r);   // u(D_opt), whatever the pose
-        default: return SO_OK;
-    }
-}
-
 // xyzi == nullptr with n != 0: the registered scan or its edge cloud (put_registered_scan)
 static int store_add(Ctx* c, MapStore& ms, const void* xyzi, size_t n, size_t stride, size_t ioff, const double* pose) {
     if (!c || stride < 12) return fail(SO_ERR_ARG, "bad args");
@@ -1011,7 +1012,7 @@ static int store_add(Ctx* c, MapStore& ms, const void* xyzi, size_t n, size_t st
     if (ms.dirty) { rc = map_rebuild(c, ms); if (rc) return rc; }           // pending origin / resolution change first: it may compact the cloud
     // ... or, with the block archive on, grow it by the blocks it restores: the new points must still fit behind it
     if (size_t(ms.n) + n > c->cfg.max_map_points) return fail(SO_ERR_CAPACITY, "map + new points exceed so_config.max_map_points");
-    rc = xyzi ? upload_cloud(c, xyzi, n, stride, ioff, ms.d_xyzi + ms.n) : put_registered_scan(c, ms, pose);
+    rc = xyzi ? upload_cloud(c, xyzi, n, stride, ioff, ms.d_xyzi + ms.n) : put_registered_scan(c, &ms == &c->edge, ms.d_xyzi + ms.n, pose);
     if (rc) return rc;
     if (pose) { rc = map_transform_tail(c, ms, uint32_t(n), pose); if (rc) return rc; }
     timed_launch_begin(c);
@@ -1095,7 +1096,7 @@ int so_map_clear_free_space_registered(so_ctx* ctx, int stores, const double pos
     if (rc) return rc;
     MapStore& ms = c->surf;
     if (size_t(ms.n) + c->reg.n > c->cfg.max_map_points) return fail(SO_ERR_CAPACITY, "map + registered scan exceed so_config.max_map_points");
-    rc = put_registered_scan(c, ms, pose);
+    rc = put_registered_scan(c, false, ms.d_xyzi + ms.n, pose);
     return rc ? rc : free_space_clear(c, stores, ms.d_xyzi + ms.n, c->reg.n, pose, *opts, result);
 }
 
@@ -1438,6 +1439,25 @@ int so_register_batch_device(so_ctx* ctx, const void* d_scans, const uint32_t* n
     int rc = check_batch(c, n_points, n_scans);
     if (rc) return rc;
     RegisterRequest q = batch_request(d_scans, n_points, n_scans, 16, 12, poses_in, opts, results);
+    q.src = Source::DEVICE;
+    return register_scans(c, q);
+}
+
+// Keyframes of src registered against dst's map as so_register_batch_device registers device scans: mode NONE (a keyframe is already
+// compensated), dst's registered-scan record untouched
+int so_register_keyframes(so_ctx* dst_ctx, so_ctx* src_ctx, const int32_t* ids, size_t n, const double* priors7, const so_icp_opts* opts,
+                          so_icp_result* results) {
+    Ctx* c = reinterpret_cast<Ctx*>(dst_ctx);
+    Ctx* s = reinterpret_cast<Ctx*>(src_ctx);
+    if (!c || !s || !ids || !priors7 || !opts || !results) return fail(SO_ERR_ARG, "bad args");
+    if (c->device != s->device) return fail(SO_ERR_ARG, "so_register_keyframes: the two contexts are on different devices");
+    SO_CUDA_TRY(cudaSetDevice(c->device));
+    const float4* scans = nullptr;
+    std::vector<uint32_t> n_points;
+    int rc = keyframe_scans(c, s, ids, n, &scans, &n_points);
+    if (!rc) rc = check_batch(c, n_points.data(), n);
+    if (rc) return rc;
+    RegisterRequest q = batch_request(scans, n_points.data(), n, 16, 12, priors7, opts, results);
     q.src = Source::DEVICE;
     return register_scans(c, q);
 }

@@ -122,6 +122,33 @@ struct BlockArchive {
     GatherSeg* d_segs = nullptr; size_t segs_cap = 0;   // segment lists of the gathers
 };
 
+// Keyframe store (so_keyframes.cu; so_keyframe_reserve): registered scans kept on the device with their poses, for a loop-closing back
+// end.  Per store (0 surf, 1 edge) one float4 pool holds the keyframes back to back in id order, each as put_registered_scan places
+// it (sensor frame, motion-compensated as registered).  cap_frames == 0: off, nothing allocated.
+struct KeyframeStore {
+    size_t cap_points = 0, cap_frames = 0;         // points per pool, keyframes
+    float4* d_pool[2] = {nullptr, nullptr};        // [cap_points] each
+    std::vector<uint64_t> off[2];                  // [frames + 1] first point of every keyframe, then the pool's tail
+    std::vector<double> poses;                     // [frames][7]
+    size_t frames() const { return poses.size() / 7; }
+};
+// One selected keyframe of so_map_from_keyframes: pool[src .. src + n) becomes union[start .. start + n), transformed by pose
+struct KfSeg { uint64_t src; uint32_t start, n; double pose[7]; };
+// Scratch of so_map_from_keyframes and so_register_keyframes (so_keyframes.cu), grown on demand: the union of the selected keyframes
+// in the world frame, its sort, and the filtered cloud of each store until both have passed their capacity checks
+struct KeyframeScratch {
+    KfSeg* d_segs = nullptr; size_t segs_cap = 0;
+    float4* d_raw = nullptr; size_t raw_cap = 0;
+    uint64_t* d_keys = nullptr; size_t keys_cap = 0;
+    uint64_t* d_keys_out = nullptr; size_t keys_out_cap = 0;
+    uint32_t* d_vals = nullptr; size_t vals_cap = 0;
+    uint32_t* d_vals_out = nullptr; size_t vals_out_cap = 0;
+    float4* d_out[2] = {nullptr, nullptr}; size_t out_cap[2] = {0, 0};
+    uint32_t* d_blk = nullptr; size_t blk_cap = 0;         // block of every filtered point, then the block runs
+    void* d_tmp = nullptr; size_t tmp_bytes = 0;
+    int32_t* d_ctl = nullptr; int32_t* h_ctl = nullptr;    // [8] world-block bounds and run count (pinned mirror)
+};
+
 // One per-block cloud family of the LocalMap (surf or edge): points in id order, the sorted hash grid, block tables.
 struct MapStore {
     float res = 0.4f;                              // planeRes_ (surf) / lineRes_ (edge): voxel leaf and gate / search radius
@@ -303,6 +330,10 @@ struct Ctx {
         struct FreeCounters* d_cnt = nullptr; struct FreeCounters* h_cnt = nullptr;   // counters of one call (pinned mirror)
     } fs;
 
+    // ---- keyframes (so_keyframe_*, so_map_from_keyframes, so_register_keyframes): allocated on first use ---------------------------
+    KeyframeStore kf;
+    KeyframeScratch kfs;
+
     // ---- instrumentation ----------------------------------------------------------------------------------------
     uint64_t launches = 0;
     uint64_t bytes_h2d = 0, bytes_d2h = 0;         // host<->device bytes moved by registration / k-NN calls
@@ -348,18 +379,18 @@ void launch_undistort(const BatchView& bv, float4* sorted, const float4* raw, co
 // and its times (indexed eoffset + i) into `out` at the same index, w kept
 void launch_undistort_edges(const BatchView& bv, const uint32_t* eoffset, float4* out, const float4* raw, const float* times,
                             const UndistortParams* par, uint32_t grid_e, uint32_t n_scans, cudaStream_t st);
-// ms tail = the registered scan r (APPROXIMATED): pInit at pose, in place
-int undistort_tail(Ctx* c, MapStore& ms, const RegisteredScan& r, const double pose[7]);
-// ms tail = the registered edge cloud r (APPROXIMATED): pInit at pose, in place
-int undistort_edge_tail(Ctx* c, MapStore& ms, const RegisteredScan& r, const double pose[7]);
+// dst[0..r.n) = the registered scan r (APPROXIMATED): pInit at pose, in place
+int undistort_tail(Ctx* c, float4* dst, const RegisteredScan& r, const double pose[7]);
+// dst[0..r.n_edge) = the registered edge cloud r (APPROXIMATED): pInit at pose, in place
+int undistort_edge_tail(Ctx* c, float4* dst, const RegisteredScan& r, const double pose[7]);
 // so_motion.cu
 void motion_free(Ctx* c);                                   // the buffers of Ctx::mot
 int motion_reserve(Ctx* c, size_t n_points);                // Ctx::mot's blocks and partials (max_batch), Ctx::und's times (n_points)
 int check_motion(const so_motion* m, const so_icp_opts* o); // argument errors of one so_motion and the options it registers with
 MotionState make_state(const so_motion& m);
 void fill_motion(const so_icp_result& icp, const MotionState& M, so_motion_result* out);   // out = icp + motion, pose_end = T * D
-int motion_tail(Ctx* c, MapStore& ms, const RegisteredScan& r);   // ms tail = the registered scan r (OPTIMIZED): u(r.D), in place
-int motion_edge_tail(Ctx* c, MapStore& ms, const RegisteredScan& r);   // ms tail = its edge cloud: u(r.D) with the edge times, in place
+int motion_tail(Ctx* c, float4* dst, const RegisteredScan& r);   // dst[0..r.n) = the registered scan r (OPTIMIZED): u(r.D), in place
+int motion_edge_tail(Ctx* c, float4* dst, const RegisteredScan& r);   // dst[0..r.n_edge) = its edge cloud: u(r.D) with the edge times, in place
 int motion_edge_reserve(Ctx* c);                             // Ctx::mot's edge partials
 // The edge cloud of an OPTIMIZED chunk: the edge map, the line buffers (eb.scan: where the warp puts float(u(D)) of the edge points,
 // eb.offset: the chunk's edge offsets), the raw edge points and their times, the edge partials and the CTAs covering the largest cloud
@@ -396,7 +427,28 @@ void free_space_free(Ctx* c);
 int free_space_clear(Ctx* c, int stores, const float4* d_pts, uint32_t n_pts, const double pose[7], const so_free_space& o,
                      so_free_space_result* out);
 // so_features.cu
-void features_free(Ctx* c);                                 // the buffers of Ctx::feat
+void features_free(Ctx* c);
+// so_api.cu: dst[0..n) = the registered scan (edges: its edge cloud) as the map inserts place it before the world transform
+int put_registered_scan(Ctx* c, bool edges, float4* dst, const double pose[7]);
+// so_keyframes.cu
+void keyframes_free(Ctx* c);
+// The surf clouds of src's keyframes ids[0..n) back to back on the device as registration input for dst, with their sizes: src's pool
+// in place when the ids are consecutive, else a gather into dst's scratch.  SO_ERR_ARG for an id src does not hold.
+int keyframe_scans(Ctx* dst, Ctx* src, const int32_t* ids, size_t n, const float4** scans, std::vector<uint32_t>* n_points);
+// so_map.cu: pts[0..n) at pose, in place, by k_transform_points (utils::TransformPoint: qrot in double, float store)
+void launch_transform(float4* pts, uint32_t n, const double pose[7], cudaStream_t st);
+// so_map.cu, so_map_from_keyframes in two steps so that two stores change together or not at all.  keyframe_map_filter: the map of the
+// union that segs[0..n_segs) (host, total points) cut from `pool`, filtered for store ms (0 surf, 1 edge) under c's origin and leaf into
+// the scratch c->kfs.d_out[store]; SO_ERR_CAPACITY when it does not fit ms, nothing changed either way.  keyframe_map_commit: ms
+// replaced by that map and its index built.
+struct KfBuild {
+    uint32_t n_win = 0, n_win_blocks = 0;          // window points and blocks
+    size_t n_arc = 0;                              // points of off-window blocks (archive on)
+    std::vector<GatherSeg> win;                    // filtered cloud -> window, block by block
+    std::vector<std::pair<uint64_t, GatherSeg>> arc;   // world key, filtered cloud -> archive pool
+};
+int keyframe_map_filter(Ctx* c, MapStore& ms, int store, const KfSeg* segs, uint32_t n_segs, uint32_t total, const float4* pool, KfBuild* b);
+int keyframe_map_commit(Ctx* c, MapStore& ms, int store, const KfBuild& b);                                 // the buffers of Ctx::feat
 // so_scan.cu
 struct DeskewParams {
     double start_time;                     // lidar_start_time

@@ -9,7 +9,9 @@
 // Every change to a store goes through one pipeline: an optional filter stage (voxel filter of the touched blocks, drop of
 // off-grid points; filter_stage) and one index stage (block counts, slots, cell table; count_blocks + index_cells).
 #include <algorithm>
+#include <climits>
 #include <cmath>
+#include <cstring>
 #include <set>
 
 #include <cub/cub.cuh>
@@ -245,21 +247,30 @@ int scan_sort(Ctx* c, size_t first, size_t n, int n_scans, int cell_bits, bool k
 }
 
 struct Pose7 { double v[7]; };
+// utils::TransformPoint (superodom_utils.h:116-127): double math, float store; w kept
+__device__ __forceinline__ float4 pose_point(const double* pose, float4 p) {
+    const double v[3] = {double(p.x), double(p.y), double(p.z)};
+    double o[3];
+    qrot(pose + 3, v, o);
+    p.x = float(o[0] + pose[0]); p.y = float(o[1] + pose[1]); p.z = float(o[2] + pose[2]);
+    return p;
+}
+
 __global__ void k_transform_points(float4* __restrict__ pts, uint32_t n, Pose7 pose) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    float4 p = pts[i];
-    const double v[3] = {double(p.x), double(p.y), double(p.z)};
-    double o[3];
-    qrot(pose.v + 3, v, o);                            // utils::TransformPoint (superodom_utils.h:116-127): double math, float store
-    p.x = float(o[0] + pose.v[0]); p.y = float(o[1] + pose.v[1]); p.z = float(o[2] + pose.v[2]);
-    pts[i] = p;
+    pts[i] = pose_point(pose.v, pts[i]);
+}
+
+void launch_transform(float4* pts, uint32_t n, const double pose[7], cudaStream_t st) {
+    if (!n) return;
+    Pose7 P;
+    for (int k = 0; k < 7; ++k) P.v[k] = pose[k];                            // by value in the launch: no staging copy, no wait
+    k_transform_points<<<(n + 255) / 256, 256, 0, st>>>(pts, n, P);
 }
 
 int map_transform_tail(Ctx* c, MapStore& ms, uint32_t n_new, const double pose[7]) {
-    Pose7 P;
-    for (int k = 0; k < 7; ++k) P.v[k] = pose[k];                            // by value in the launch: no staging copy, no wait
-    k_transform_points<<<(n_new + 255) / 256, 256, 0, c->stream>>>(ms.d_xyzi + ms.n, n_new, P);
+    launch_transform(ms.d_xyzi + ms.n, n_new, pose, c->stream);
     c->launches++;
     return SO_OK;
 }
@@ -338,12 +349,32 @@ __global__ void k_mark_touched_new(const float4* __restrict__ pts, uint32_t n_ne
     if (b >= 0) touched[b] = 1;
 }
 
+// Voxel of p inside world block w (grid block g = w + origin) as [vk][vj][vi], vb bits each.  PCL orders a block's output by the voxel
+// index relative to the block cloud's bounding box; subtracting any per-block constant keeps that order, so the index is taken relative
+// to the block's minimum corner (minus a 2-voxel guard for the float rounding of x * inv_leaf at the faces).
+__device__ __forceinline__ uint64_t block_voxel(const float4 p, int wx, int wy, int wz, float inv_leaf, int vb) {
+    const double il = double(inv_leaf);
+    const int64_t bx = int64_t(floor((double(wx) * kBlock - kHalfBlock) * il)) - 2;
+    const int64_t by = int64_t(floor((double(wy) * kBlock - kHalfBlock) * il)) - 2;
+    const int64_t bz = int64_t(floor((double(wz) * kBlock - kHalfBlock) * il)) - 2;
+    const int64_t vmax = (int64_t(1) << vb) - 1;
+    auto local = [vmax](int64_t v) { return uint64_t(v < 0 ? 0 : (v > vmax ? vmax : v)); };
+    const uint64_t vi = local(int64_t(floorf(__fmul_rn(p.x, inv_leaf))) - bx);      // pcl::VoxelGrid: floor(coord * inverse_leaf_size) in float
+    const uint64_t vj = local(int64_t(floorf(__fmul_rn(p.y, inv_leaf))) - by);
+    const uint64_t vk = local(int64_t(floorf(__fmul_rn(p.z, inv_leaf))) - bz);
+    return (vk << (2 * vb)) | (vj << vb) | vi;
+}
+
+// bits of a block-local voxel index: 50 m / leaf + 5 values
+static int voxel_bits(float inv_leaf) {
+    int vb = 1;
+    while (vb < 16 && double(1 << vb) < kBlock * double(inv_leaf) + 5.0) ++vb;
+    return vb;
+}
+
 // insert key of every point (old cloud followed by the new points), the block recomputed from the coordinates:
 // [class: 0 untouched block, 1 touched, 2 dropped][block 13 bits][vk][vj][vi], vb bits per block-local voxel index (50 m / leaf + 5
 // values: 8 bits at leaf 0.2) -- 39 key bits = 5 radix passes instead of the 8 of a full 64-bit key.
-// PCL orders a block's output by the voxel index relative to the block cloud's bounding box; subtracting any per-block constant
-// keeps that order, so the index is taken relative to the block's minimum corner (minus a 2-voxel guard for the float rounding of
-// x * inv_leaf at the faces).
 __global__ void k_insert_keys(const float4* __restrict__ raw, uint32_t n, float inv_leaf, int3 origin, const uint8_t* __restrict__ touched,
                               int vb, uint64_t* __restrict__ keys, uint32_t* __restrict__ vals) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -356,16 +387,7 @@ __global__ void k_insert_keys(const float4* __restrict__ raw, uint32_t n, float 
         if (!touched[b]) key = 0;                                         // untouched block: kept in place (stable sort)
         else {
             const int gx = b % kW, gy = (b / kW) % kH, gz = b / (kW * kH);
-            const double il = double(inv_leaf);
-            const int64_t bx = int64_t(floor((double(gx - origin.x) * kBlock - kHalfBlock) * il)) - 2;
-            const int64_t by = int64_t(floor((double(gy - origin.y) * kBlock - kHalfBlock) * il)) - 2;
-            const int64_t bz = int64_t(floor((double(gz - origin.z) * kBlock - kHalfBlock) * il)) - 2;
-            const int64_t vmax = (int64_t(1) << vb) - 1;
-            auto local = [vmax](int64_t v) { return uint64_t(v < 0 ? 0 : (v > vmax ? vmax : v)); };
-            const uint64_t vi = local(int64_t(floorf(__fmul_rn(p.x, inv_leaf))) - bx);      // pcl::VoxelGrid: floor(coord * inverse_leaf_size) in float
-            const uint64_t vj = local(int64_t(floorf(__fmul_rn(p.y, inv_leaf))) - by);
-            const uint64_t vk = local(int64_t(floorf(__fmul_rn(p.z, inv_leaf))) - bz);
-            key = (uint64_t(1) << cls_shift) | (uint64_t(b) << (3 * vb)) | (vk << (2 * vb)) | (vj << vb) | vi;
+            key = (uint64_t(1) << cls_shift) | (uint64_t(b) << (3 * vb)) | block_voxel(p, gx - origin.x, gy - origin.y, gz - origin.z, inv_leaf, vb);
         }
     }
     keys[i] = key;
@@ -383,8 +405,7 @@ static int filter_stage(Ctx* c, MapStore& ms, uint32_t n_new) {
     SO_CUDA_TRY(cudaMemsetAsync(d_touched, 0, kNumBlocks, st));
     if (n_new) k_mark_touched_new<<<(n_new + 255) / 256, 256, 0, st>>>(ms.d_xyzi + ms.n, n_new, origin, d_touched);
     const float inv_leaf = 1.0f / ms.res;                               // Eigen::Array4f::Ones() / leaf_size_
-    int vb = 1;                                                         // bits of a block-local voxel index: 50 m / leaf + 5 values
-    while (vb < 16 && double(1 << vb) < kBlock * double(inv_leaf) + 5.0) ++vb;
+    const int vb = voxel_bits(inv_leaf);
     const int cls_shift = 13 + 3 * vb;
     k_insert_keys<<<(total + 255) / 256, 256, 0, st>>>(ms.d_xyzi, total, inv_leaf, origin, d_touched, vb, c->d_keys, c->d_vals);
     size_t tmp = c->cub_tmp_bytes;
@@ -992,6 +1013,186 @@ int cloud_voxel_filter(Ctx* c, const float4* in, uint32_t n, float leaf, const V
 int scan_voxel_filter(Ctx* c, uint32_t n, float leaf, uint32_t* n_out) {
     const VoxelBufs b{c->d_skeys, c->d_skeys_out, c->d_svals, c->d_svals_out, c->d_sort_tmp, c->sort_tmp_bytes};
     return cloud_voxel_filter(c, c->d_scan, n, leaf, b, c->d_scan_sorted, n_out);
+}
+
+
+// ------------------------------------------------------------------------------------------------------------------
+// Map from keyframes (so_map_from_keyframes): ONE voxel filter over the union of the selected keyframes, each at its pose -- not a
+// replay of inserts.  Every block of the union is filtered on its own at the store's leaf, as the insert filters a touched block, with
+// the centroids summed in union order.  A thread per union point finds its keyframe in the segment table, transforms the point with
+// k_transform_points' arithmetic (pose_point) and bins it by world block; the sort key is [drop][block][vk][vj][vi], with the block
+// numbered in the box of the kept world blocks (z, y, x: world key order) and the voxel as the insert numbers it (block_voxel).  One
+// stable sort then orders the union by world block, by voxel, and by union order inside a voxel; voxel_reduce averages it.
+// Kept: the window's blocks, and with the archive on every block in the key range.
+// ------------------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ bool kf_block(const float4 p, int3 origin, int archive, int w[3]) {
+    if (!archive::world_axis(p.x, &w[0]) || !archive::world_axis(p.y, &w[1]) || !archive::world_axis(p.z, &w[2])) return false;
+    if (archive) return true;
+    const int gx = w[0] + origin.x, gy = w[1] + origin.y, gz = w[2] + origin.z;
+    return gx >= 0 && gx < kW && gy >= 0 && gy < kH && gz >= 0 && gz < kD;
+}
+
+// union point i -> raw[i] in the world frame; ctl[0..3) = min, ctl[3..6) = max world block of the kept points (warp-reduced atomics)
+__global__ void __launch_bounds__(256) k_kf_transform(const float4* __restrict__ pool, const KfSeg* __restrict__ segs, uint32_t n_segs,
+                                                      uint32_t total, int3 origin, int archive, float4* __restrict__ raw, int32_t* __restrict__ ctl) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    int w[3] = {0, 0, 0};
+    bool kept = false;
+    if (i < total) {
+        uint32_t lo = 0, hi = n_segs;                                  // the last segment starting at or before i: the one holding it
+        while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if (segs[mid].start <= i) lo = mid; else hi = mid; }
+        const KfSeg& s = segs[lo];
+        const float4 p = pose_point(s.pose, pool[s.src + (i - s.start)]);
+        raw[i] = p;
+        kept = kf_block(p, origin, archive, w);
+    }
+    for (int a = 0; a < 3; ++a) {                                      // every lane takes part: no early return above
+        const int mn = __reduce_min_sync(0xffffffffu, kept ? w[a] : INT_MAX);
+        const int mx = __reduce_max_sync(0xffffffffu, kept ? w[a] : INT_MIN);
+        if ((threadIdx.x & 31) == 0 && mn <= mx) { atomicMin(ctl + a, mn); atomicMax(ctl + 3 + a, mx); }
+    }
+}
+
+struct KfBox { int32_t lo[3]; uint32_t nx, ny; int32_t kb; };          // first block per axis, blocks along x and y; key bits below the drop bit
+
+__global__ void k_kf_keys(const float4* __restrict__ raw, uint32_t total, int3 origin, int archive, KfBox box, float inv_leaf, int vb,
+                          uint64_t* __restrict__ keys, uint32_t* __restrict__ vals) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= total) return;
+    const float4 p = raw[i];
+    int w[3];
+    uint64_t key = uint64_t(1) << box.kb;                              // dropped
+    if (kf_block(p, origin, archive, w)) {
+        const uint64_t b = (uint64_t(w[2] - box.lo[2]) * box.ny + uint64_t(w[1] - box.lo[1])) * box.nx + uint64_t(w[0] - box.lo[0]);
+        key = (b << (3 * vb)) | block_voxel(p, w[0], w[1], w[2], inv_leaf, vb);
+    }
+    keys[i] = key;
+    vals[i] = i;
+}
+
+// blk[rank[i]] = the block of the voxel starting at sorted position i (voxel_reduce's heads and ranks)
+__global__ void k_kf_voxel_blocks(const uint64_t* __restrict__ keys, const uint32_t* __restrict__ head, const uint32_t* __restrict__ rank, uint32_t total,
+                                  int shift, uint32_t* __restrict__ blk) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < total && head[i]) blk[rank[i]] = uint32_t(keys[i] >> shift);
+}
+
+int keyframe_map_filter(Ctx* c, MapStore& ms, int store, const KfSeg* segs, uint32_t n_segs, uint32_t total, const float4* pool, KfBuild* b) {
+    cudaStream_t st = c->stream;
+    KeyframeScratch& k = c->kfs;
+    *b = KfBuild{};
+    if (total == 0) return SO_OK;
+    const int archive_on = ms.arc.cap ? 1 : 0;
+    const int3 origin = make_int3(c->origin[0], c->origin[1], c->origin[2]);
+    int rc = grow_buffer(k.d_segs, k.segs_cap, n_segs);
+    if (!rc) rc = grow_buffer(k.d_raw, k.raw_cap, total);
+    if (!rc) rc = grow_buffer(k.d_keys, k.keys_cap, total);
+    if (!rc) rc = grow_buffer(k.d_keys_out, k.keys_out_cap, total);
+    if (!rc) rc = grow_buffer(k.d_vals, k.vals_cap, total);
+    if (!rc) rc = grow_buffer(k.d_vals_out, k.vals_out_cap, total);
+    if (!rc) rc = grow_buffer(k.d_out[store], k.out_cap[store], total);
+    if (!rc) rc = grow_buffer(k.d_blk, k.blk_cap, total);
+    if (!rc && !k.d_ctl) {
+        SO_CUDA_TRY(cudaMalloc(&k.d_ctl, 8 * sizeof(int32_t)));
+        SO_CUDA_TRY(cudaMallocHost(&k.h_ctl, 8 * sizeof(int32_t)));
+    }
+    if (rc) return rc;
+    {
+        size_t a = 0, s2 = 0, r = 0;
+        cub::DeviceRadixSort::SortPairs(nullptr, a, k.d_keys, k.d_keys_out, k.d_vals, k.d_vals_out, int(total), 0, 64);
+        cub::DeviceScan::ExclusiveSum(nullptr, s2, k.d_vals, k.d_vals, int(total));
+        cub::DeviceRunLengthEncode::Encode(nullptr, r, k.d_blk, k.d_vals, k.d_vals_out, k.d_ctl, int(total));
+        rc = grow_buffer(k.d_tmp, k.tmp_bytes, std::max({a, s2, r}) + 256);
+        if (rc) return rc;
+    }
+    // the box of the kept world blocks (one read-back)
+    const int32_t init[6] = {INT_MAX, INT_MAX, INT_MAX, INT_MIN, INT_MIN, INT_MIN};
+    std::memcpy(k.h_ctl, init, sizeof(init));
+    SO_CUDA_TRY(cudaMemcpyAsync(k.d_ctl, k.h_ctl, 6 * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    SO_CUDA_TRY(cudaMemcpyAsync(k.d_segs, segs, n_segs * sizeof(KfSeg), cudaMemcpyHostToDevice, st));
+    const uint32_t grid = (total + 255) / 256;
+    k_kf_transform<<<grid, 256, 0, st>>>(pool, k.d_segs, n_segs, total, origin, archive_on, k.d_raw, k.d_ctl);
+    SO_CUDA_TRY(cudaMemcpyAsync(k.h_ctl, k.d_ctl, 6 * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    SO_CUDA_TRY(cudaGetLastError());
+    SO_CUDA_TRY(cudaStreamSynchronize(st));
+    c->launches++;
+    int32_t lo[3], hi[3];
+    for (int a = 0; a < 3; ++a) { lo[a] = k.h_ctl[a]; hi[a] = k.h_ctl[3 + a]; }
+    if (lo[0] > hi[0]) return SO_OK;                                   // no point is kept: the store becomes empty
+    const float inv_leaf = 1.0f / ms.res;                              // Eigen::Array4f::Ones() / leaf_size_
+    const int vb = voxel_bits(inv_leaf);
+    const uint64_t nx = uint64_t(hi[0] - lo[0]) + 1, ny = uint64_t(hi[1] - lo[1]) + 1, nz = uint64_t(hi[2] - lo[2]) + 1;
+    int bb = 0;
+    while ((uint64_t(1) << bb) < nx * ny * nz) ++bb;
+    if (bb > 32 || 3 * vb + bb > 63) {
+        set_error("so_map_from_keyframes: the keyframes span too many 50 m blocks for the sort key at this leaf");
+        return SO_ERR_CAPACITY;
+    }
+    const KfBox box{{lo[0], lo[1], lo[2]}, uint32_t(nx), uint32_t(ny), 3 * vb + bb};
+    k_kf_keys<<<grid, 256, 0, st>>>(k.d_raw, total, origin, archive_on, box, inv_leaf, vb, k.d_keys, k.d_vals);
+    size_t tmp = k.tmp_bytes;
+    SO_CUDA_TRY(cub::DeviceRadixSort::SortPairs(k.d_tmp, tmp, k.d_keys, k.d_keys_out, k.d_vals, k.d_vals_out, int(total), 0, box.kb + 1, st));
+    c->launches += 6;
+    uint32_t* head = reinterpret_cast<uint32_t*>(k.d_keys);           // keys_in is free after the sort: 2 * total words
+    rc = voxel_reduce(c, k.d_raw, k.d_keys_out, k.d_vals_out, total, 0, uint64_t(1) << box.kb, head, k.d_tmp, k.tmp_bytes, k.d_out[store]);
+    if (rc) return rc;
+    k_kf_voxel_blocks<<<grid, 256, 0, st>>>(k.d_keys_out, head, head + total, total, 3 * vb, k.d_blk);
+    InsertInfo* h_info = c->h_map_info;
+    SO_CUDA_TRY(cudaMemcpyAsync(h_info, &c->d_map_scratch->info, sizeof(InsertInfo), cudaMemcpyDeviceToHost, st));
+    SO_CUDA_TRY(cudaGetLastError());
+    SO_CUDA_TRY(cudaStreamSynchronize(st));
+    const uint32_t n_out = h_info->n_out;
+    // the runs of blocks in the filtered cloud: the block directory, the only thing the host reads
+    uint32_t* run_blk = k.d_vals;                                      // free after the reduction
+    uint32_t* run_n = k.d_vals_out;
+    tmp = k.tmp_bytes;
+    SO_CUDA_TRY(cub::DeviceRunLengthEncode::Encode(k.d_tmp, tmp, k.d_blk, run_blk, run_n, k.d_ctl + 6, int(n_out), st));
+    SO_CUDA_TRY(cudaMemcpyAsync(k.h_ctl + 6, k.d_ctl + 6, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    SO_CUDA_TRY(cudaStreamSynchronize(st));
+    const uint32_t runs = uint32_t(k.h_ctl[6]);
+    std::vector<uint32_t> hb(runs), hn(runs);
+    SO_CUDA_TRY(cudaMemcpyAsync(hb.data(), run_blk, runs * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    SO_CUDA_TRY(cudaMemcpyAsync(hn.data(), run_n, runs * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    SO_CUDA_TRY(cudaStreamSynchronize(st));
+    c->launches += 3 + 5;
+    uint64_t at = 0, n_win = 0;
+    for (uint32_t r = 0; r < runs; ++r) {
+        const int w[3] = {int(hb[r] % uint32_t(nx)) + lo[0], int(hb[r] / uint32_t(nx) % uint32_t(ny)) + lo[1], int(hb[r] / uint32_t(nx * ny)) + lo[2]};
+        if (archive::in_window(w, c->origin)) { b->win.push_back(GatherSeg{at, n_win, hn[r], 0}); n_win += hn[r]; }
+        else { b->arc.emplace_back(archive::world_key(w[0], w[1], w[2]), GatherSeg{at, b->n_arc, hn[r], 0}); b->n_arc += hn[r]; }
+        at += hn[r];
+    }
+    b->n_win = uint32_t(n_win);
+    b->n_win_blocks = uint32_t(b->win.size());
+    // every check before the first change
+    if (n_win > c->cfg.max_map_points) { set_error("so_map_from_keyframes: the window's points exceed so_config.max_map_points"); return SO_ERR_CAPACITY; }
+    if (b->n_arc > ms.arc.cap) { set_error("so_map_from_keyframes: the blocks outside the window exceed the block archive (so_map_archive)"); return SO_ERR_CAPACITY; }
+    const size_t cells_per_slot = size_t(map_cells_per_block(ms.res));
+    if (b->n_win_blocks > (kMaxCells - 2) / (cells_per_slot * cells_per_slot * cells_per_slot)) {
+        set_error("map spans too many 50 m blocks for the dense cell table (n_slots * nb^3 >= 2^31)");
+        return SO_ERR_CAPACITY;
+    }
+    return SO_OK;
+}
+
+int keyframe_map_commit(Ctx* c, MapStore& ms, int store, const KfBuild& b) {
+    BlockArchive& a = ms.arc;
+    const float4* out = c->kfs.d_out[store];
+    int rc = seg_gather(c, a, b.win, out, ms.d_xyzi);
+    if (rc) return rc;
+    if (a.cap) {
+        std::vector<GatherSeg> segs;
+        segs.reserve(b.arc.size());
+        for (const auto& kv : b.arc) segs.push_back(kv.second);
+        SO_CUDA_TRY(cudaStreamSynchronize(c->stream));                 // the window's gather list has left the segment buffer
+        rc = seg_gather(c, a, segs, out, a.d_pool);
+        if (rc) return rc;
+        a.dir.clear();
+        for (const auto& kv : b.arc) a.dir[kv.first] = BlockArchive::Seg{kv.second.dst, kv.second.n};
+        a.used = a.live = b.n_arc;
+    }
+    ms.n = b.n_win;
+    return map_rebuild(c, ms);                                         // index stage; nothing is left to evict or restore
 }
 
 }  // namespace so

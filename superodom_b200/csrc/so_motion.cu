@@ -725,23 +725,23 @@ void launch_motion_solve(int phase, const BatchView& bv, const CorrBuf& cb, cons
     }
 }
 
-int motion_tail(Ctx* c, MapStore& ms, const RegisteredScan& r) {
+int motion_tail(Ctx* c, float4* dst, const RegisteredScan& r) {
     if (!r.n) return SO_OK;
     MotionD D;
     for (int k = 0; k < 7; ++k) D.v[k] = r.D[k];
     timed_launch_begin(c);
-    k_motion_cloud<<<(r.n + 255) / 256, 256, 0, c->stream>>>(ms.d_xyzi + ms.n, c->und.d_time, r.n, D, r.dt);
+    k_motion_cloud<<<(r.n + 255) / 256, 256, 0, c->stream>>>(dst, c->und.d_time, r.n, D, r.dt);
     timed_launch_end(c, 7);
     SO_CUDA_TRY(cudaGetLastError());
     return SO_OK;
 }
 
-int motion_edge_tail(Ctx* c, MapStore& ms, const RegisteredScan& r) {
+int motion_edge_tail(Ctx* c, float4* dst, const RegisteredScan& r) {
     if (!r.n_edge) return SO_OK;
     MotionD D;
     for (int k = 0; k < 7; ++k) D.v[k] = r.D[k];
     timed_launch_begin(c);
-    k_motion_cloud<<<(r.n_edge + 255) / 256, 256, 0, c->stream>>>(ms.d_xyzi + ms.n, c->und.d_etime, r.n_edge, D, r.dt);
+    k_motion_cloud<<<(r.n_edge + 255) / 256, 256, 0, c->stream>>>(dst, c->und.d_etime, r.n_edge, D, r.dt);
     timed_launch_end(c, 7);
     SO_CUDA_TRY(cudaGetLastError());
     return SO_OK;

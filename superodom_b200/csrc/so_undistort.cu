@@ -94,14 +94,14 @@ static void launch_undistort_cloud(Ctx* c, float4* pts, const float* times, uint
     timed_launch_end(c, 7);                                               // counts the launch
 }
 
-int undistort_tail(Ctx* c, MapStore& ms, const RegisteredScan& r, const double pose[7]) {
-    launch_undistort_cloud(c, ms.d_xyzi + ms.n, c->und.d_time, r.n, r.par, pose);
+int undistort_tail(Ctx* c, float4* dst, const RegisteredScan& r, const double pose[7]) {
+    launch_undistort_cloud(c, dst, c->und.d_time, r.n, r.par, pose);
     SO_CUDA_TRY(cudaGetLastError());
     return SO_OK;
 }
 
-int undistort_edge_tail(Ctx* c, MapStore& ms, const RegisteredScan& r, const double pose[7]) {
-    launch_undistort_cloud(c, ms.d_xyzi + ms.n, c->und.d_etime, r.n_edge, r.par, pose);
+int undistort_edge_tail(Ctx* c, float4* dst, const RegisteredScan& r, const double pose[7]) {
+    launch_undistort_cloud(c, dst, c->und.d_etime, r.n_edge, r.par, pose);
     SO_CUDA_TRY(cudaGetLastError());
     return SO_OK;
 }
