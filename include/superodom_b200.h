@@ -278,6 +278,55 @@ int so_keyframe_download(so_ctx* ctx, int32_t id, int store, const double pose7[
  * the archive, the window's blocks exceed the cell table, or 2^31 points or more are selected. */
 int so_map_from_keyframes(so_ctx* dst, so_ctx* src, const int32_t* ids, size_t n_ids, const double* poses7, int stores);
 
+/* ---- loop detection: which old keyframe a new one revisits (Scan Context, Kim & Kim, IROS 2018) ---------------------------------
+ * No reference counterpart.  Appearance-based, so it does not read the drifted positions of the keyframes: each keyframe is described
+ * by a polar max-height image of its surf cloud, and a query is compared with every eligible keyframe at every column shift.  The
+ * search is exhaustive (no ring-key prefilter); thresholding the distance is the caller's policy (DESIGN.md, "Loop detection").
+ * Descriptor of keyframe i, in FP64 without contractible multiply-adds (DESIGN.md gives the exact expression order):
+ *   - levelling: R = R(q_i) of its CURRENT pose (so_keyframe_poses), psi = atan2(R10, R00), L = Rz(-psi) R: roll and pitch come from
+ *     the pose, heading is left out; each finite point p of the sensor-frame surf cloud goes to v = L p;
+ *   - rho = hypot(vx, vy), points with rho >= max_range skipped; ring floor(rho / max_range * rings) (at most rings - 1);
+ *     az = atan2(vy, vx) in [-pi, pi), sector floor((az + pi) / (2 pi / sectors)), at most sectors - 1;
+ *   - cell value: the maximum of max(0, float(vz + height_offset)) over its points, 0 when empty (a cell whose maximum height lies
+ *     below -height_offset reads 0); column norms in FP64, summed in ring order.
+ * Distance of query a to candidate b at shift s: over query columns j with candidate column (j + s) mod sectors, pairs where both norms
+ * are non-zero, d = 1 - (sum of cosines in ascending j) / n_pairs, each dot summed in ring order in FP64; d = 1 with no pair.  The pair
+ * distance is the minimum over s, ties to the lowest s; yaw = s * 2 pi / sectors wrapped to (-pi, pi] is the query's heading minus the
+ * candidate's, in their levelled frames.
+ * Descriptors are cached per keyframe and computed lazily by the calls below: a descriptor is valid for the options and the pose it
+ * was computed with (the self-rebuild of so_map_from_keyframes marks the keyframes it moves stale; other options invalidate all).  No
+ * other call launches anything for them.  Both calls fail with SO_ERR_ARG, before any device work, without a keyframe store, for an id
+ * the store does not hold, and for options outside: rings 1..64, sectors 2..360 (the query image and its norms, at most 95 040 B, sit
+ * in shared memory), max_range finite and > 0, height_offset finite, exclude_recent >= 0. */
+typedef struct {
+    int32_t rings;            /* default 20 */
+    int32_t sectors;          /* default 60 */
+    double max_range;         /* metres, default 80 */
+    double height_offset;     /* the sensor's height above the ground, metres, default 2.0 */
+    int32_t exclude_recent;   /* keyframe id is eligible for query q when id < q - exclude_recent; default 30 */
+    int32_t pad_;
+} so_loop_opts;
+typedef struct {
+    int32_t query;            /* the query keyframe */
+    int32_t id;               /* the candidate keyframe; -1 in unused slots (fewer than k eligible) */
+    double distance;          /* in [0, 1] up to rounding; 1 without evidence */
+    int32_t shift;            /* best column shift s */
+    int32_t n_pairs;          /* column pairs that counted at that shift */
+    double yaw;               /* s * 2 pi / sectors wrapped to (-pi, pi]: query heading - candidate heading (radians) */
+} so_loop_candidate;
+typedef struct {
+    uint64_t n_described;     /* keyframes this call described (not found valid in the cache) */
+    double time_describe_ms;  /* device time of the describe stage (CUDA events), 0 when nothing was described */
+    double time_search_ms;    /* device time of the search and top-k stages (CUDA events) */
+} so_loop_stats;
+void so_loop_opts_defaults(so_loop_opts* opts);
+/* For each of queries[0..n): its k best eligible keyframes, out[i * k .. i * k + k), by distance ascending, then id ascending.  Every
+ * query is compared with every eligible keyframe at every shift.  stats may be NULL.  SO_ERR_ARG also for k outside 1..64. */
+int so_loop_candidates(so_ctx* ctx, const int32_t* queries, size_t n, const so_loop_opts* opts, int32_t k, so_loop_candidate* out,
+                       so_loop_stats* stats);
+/* The descriptors of keyframes ids[0..n) as the search sees them, out[n][rings][sectors] (described first where the cache holds none). */
+int so_keyframe_descriptors(so_ctx* ctx, const int32_t* ids, size_t n, const so_loop_opts* opts, float* out);
+
 /* ---- free-space clearing: take out the map points a scan sees through (moving objects) ---------------------------------------
  * No reference counterpart (LocalMap::addSurfPointCloud only adds points).  Off unless called; nothing else calls it.
  * Rule (DESIGN.md §2): the scan, in the frame of pose with the sensor at the pose's origin, is projected to a range image in FP64 --

@@ -543,6 +543,32 @@ public:
         check(so_register_keyframes(submap.ctx_->h, context.h, ids.data(), ids.size(), p.data(), &o, out.data()), "so_register_keyframes");
         return out;
     }
+    // Loop detection (so_loop_candidates with loopOpts): the k keyframes whose Scan Context descriptors are closest to keyframe id's,
+    // best first (id -1 in unused slots).  Thresholding the distance is the caller's policy (DESIGN.md, "Loop detection").
+    so_loop_opts loopOpts = defaultLoopOpts();
+    static so_loop_opts defaultLoopOpts() { so_loop_opts o{}; so_loop_opts_defaults(&o); return o; }
+    std::vector<so_loop_candidate> loopCandidates(int32_t id, int32_t k) {
+        std::vector<so_loop_candidate> out(size_t(k > 0 ? k : 0));
+        check(so_loop_candidates(context.h, &id, 1, &loopOpts, k, out.data(), nullptr), "so_loop_candidates");
+        return out;
+    }
+    // The alignment prior of a candidate for alignKeyframes, from keyframePoses(): the candidate keyframe's position, its heading
+    // plus c.yaw, and the query's roll and pitch (the query's orientation turned about the world z axis by psi_c + yaw - psi_q,
+    // psi = atan2(R10, R00) as the descriptor levels it)
+    Transformd loopPrior(const so_loop_candidate& c) const {
+        const std::vector<Transformd> p = keyframePoses();
+        if (c.id < 0 || size_t(c.id) >= p.size() || c.query < 0 || size_t(c.query) >= p.size()) throw Error("loopPrior: no such keyframe");
+        auto heading = [](const Quaterniond& q) {
+            const double n = std::sqrt(q.x() * q.x() + q.y() * q.y() + q.z() * q.z() + q.w() * q.w());
+            const double x = q.x() / n, y = q.y() / n, z = q.z() / n, w = q.w() / n;
+            return std::atan2(2 * (x * y + z * w), 1 - 2 * (y * y + z * z));
+        };
+        const Transformd& cand = p[size_t(c.id)];
+        const Transformd& query = p[size_t(c.query)];
+        const double turn = heading(cand.rot) + c.yaw - heading(query.rot);
+        const Quaterniond qz(std::cos(turn / 2), 0, 0, std::sin(turn / 2));
+        return Transformd(qz * query.rot, cand.pos);
+    }
     // The map rebuilt from every keyframe at the corrected poses (one per keyframe, in id order), both stores; T_w_lidar and
     // last_T_w_lidar become the corrected pose of the last keyframe, so the next Localization() continues from the corrected map.
     void rebuildFromKeyframes(const std::vector<Transformd>& corrected) {

@@ -29,6 +29,7 @@ EXPORTS = [
     "so_knn_graph", "so_knn_graph_stats",
     "so_keyframe_reserve", "so_keyframe_add_registered", "so_keyframe_info", "so_keyframe_poses", "so_keyframe_download", "so_map_from_keyframes",
     "so_register_keyframes",
+    "so_loop_opts_defaults", "so_loop_candidates", "so_keyframe_descriptors",
 ]
 
 
@@ -169,6 +170,32 @@ def free_space(**kw) -> FreeSpace:
     for k, v in kw.items():
         if not hasattr(o, k):
             raise TypeError(f"so_free_space has no field {k}")
+        setattr(o, k, v)
+    return o
+
+
+class LoopOpts(C.Structure):
+    """so_loop_opts: Scan Context geometry (rings, sectors, max_range m, height_offset m) and the search's exclude_recent."""
+    _fields_ = [("rings", C.c_int32), ("sectors", C.c_int32), ("max_range", C.c_double), ("height_offset", C.c_double),
+                ("exclude_recent", C.c_int32), ("pad_", C.c_int32)]
+
+
+class LoopStats(C.Structure):
+    _fields_ = [("n_described", C.c_uint64), ("time_describe_ms", C.c_double), ("time_search_ms", C.c_double)]
+
+
+# so_loop_candidate
+LOOP_CANDIDATE_DTYPE = np.dtype([("query", "<i4"), ("id", "<i4"), ("distance", "<f8"), ("shift", "<i4"), ("n_pairs", "<i4"),
+                                 ("yaw", "<f8")], align=True)
+
+
+def loop_opts(**kw) -> LoopOpts:
+    """so_loop_opts_defaults, then the given fields."""
+    o = LoopOpts()
+    load_library().so_loop_opts_defaults(C.byref(o))
+    for k, v in kw.items():
+        if not hasattr(o, k) or k == "pad_":
+            raise TypeError(f"so_loop_opts has no field {k}")
         setattr(o, k, v)
     return o
 
@@ -315,6 +342,10 @@ def load_library():
     L.so_keyframe_download.argtypes = [C.c_void_p, C.c_int32, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
     L.so_map_from_keyframes.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_int]
     L.so_register_keyframes.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.so_loop_opts_defaults.restype = None
+    L.so_loop_opts_defaults.argtypes = [C.c_void_p]
+    L.so_loop_candidates.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
+    L.so_keyframe_descriptors.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
     _lib = L
     return L
 
@@ -593,6 +624,28 @@ class Context:
         res = (IcpResult * len(ids))()
         self._chk(self.L.so_register_keyframes(self.h, src.h, _p(ids), len(ids), _p(priors), C.byref(o), res), "so_register_keyframes")
         return list(res)
+
+    # ---- loop detection over the keyframes (Scan Context; descriptors cached per keyframe, computed by these calls)
+    def loop_candidates(self, queries, k: int, opts: LoopOpts | None = None, stats: bool = False, **kw):
+        """For each query keyframe its k best eligible keyframes -> structured array [n, k] of LOOP_CANDIDATE_DTYPE (distance
+        ascending, then id; id -1 in unused slots); with stats=True also {n_described, time_describe_ms, time_search_ms}.  kw: fields
+        of so_loop_opts over the defaults."""
+        q = np.ascontiguousarray(np.atleast_1d(queries), dtype=np.int32)
+        o = opts if opts is not None else loop_opts(**kw)
+        out = np.zeros((len(q), max(int(k), 1)), LOOP_CANDIDATE_DTYPE)
+        st = LoopStats()
+        self._chk(self.L.so_loop_candidates(self.h, _p(q), len(q), C.byref(o), int(k), _p(out), C.byref(st)), "so_loop_candidates")
+        if stats:
+            return out, dict(n_described=st.n_described, time_describe_ms=st.time_describe_ms, time_search_ms=st.time_search_ms)
+        return out
+
+    def keyframe_descriptors(self, ids, opts: LoopOpts | None = None, **kw) -> np.ndarray:
+        """The Scan Context images of keyframes ids as the search sees them -> float32 [n, rings, sectors]."""
+        i = np.ascontiguousarray(np.atleast_1d(ids), dtype=np.int32)
+        o = opts if opts is not None else loop_opts(**kw)
+        out = np.zeros((len(i), max(o.rings, 1), max(o.sectors, 1)), np.float32)
+        self._chk(self.L.so_keyframe_descriptors(self.h, _p(i), len(i), C.byref(o), _p(out)), "so_keyframe_descriptors")
+        return out
 
     # ---- free-space clearing (off unless called)
     @staticmethod

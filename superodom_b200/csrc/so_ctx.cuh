@@ -131,6 +131,11 @@ struct KeyframeStore {
     std::vector<uint64_t> off[2];                  // [frames + 1] first point of every keyframe, then the pool's tail
     std::vector<double> poses;                     // [frames][7]
     size_t frames() const { return poses.size() / 7; }
+    // Scan Context descriptors (so_loop.cu), by keyframe id: [desc_frames][rings][sectors] images and [desc_frames][sectors] column
+    // norms for the options in desc_opts (rings == 0: no table); desc_ok[id] = 1 while id's descriptor is valid for them and its pose
+    float* d_desc = nullptr; double* d_desc_norm = nullptr; size_t desc_frames = 0;
+    so_loop_opts desc_opts{};
+    std::vector<uint8_t> desc_ok;
 };
 // One selected keyframe of so_map_from_keyframes: pool[src .. src + n) becomes union[start .. start + n), transformed by pose
 struct KfSeg { uint64_t src; uint32_t start, n; double pose[7]; };
@@ -147,6 +152,12 @@ struct KeyframeScratch {
     uint32_t* d_blk = nullptr; size_t blk_cap = 0;         // block of every filtered point, then the block runs
     void* d_tmp = nullptr; size_t tmp_bytes = 0;
     int32_t* d_ctl = nullptr; int32_t* h_ctl = nullptr;    // [8] world-block bounds and run count (pinned mirror)
+    // loop detection (so_loop.cu): keyframes to describe, the queries, one chunk's pair table and every query's top k
+    struct DescSeg* d_dsegs = nullptr; size_t dsegs_cap = 0;
+    int32_t* d_queries = nullptr; size_t queries_cap = 0;
+    struct LoopPair* d_pairs = nullptr; size_t pairs_cap = 0;
+    struct LoopPair* d_top = nullptr; size_t top_cap = 0;
+    cudaEvent_t ev_loop[4] = {};                            // describe start / end, search start / end
 };
 
 // One per-block cloud family of the LocalMap (surf or edge): points in id order, the sorted hash grid, block tables.
@@ -435,6 +446,10 @@ void keyframes_free(Ctx* c);
 // The surf clouds of src's keyframes ids[0..n) back to back on the device as registration input for dst, with their sizes: src's pool
 // in place when the ids are consecutive, else a gather into dst's scratch.  SO_ERR_ARG for an id src does not hold.
 int keyframe_scans(Ctx* dst, Ctx* src, const int32_t* ids, size_t n, const float4** scans, std::vector<uint32_t>* n_points);
+// so_loop.cu: the descriptor table at cap_frames keyframes (valid descriptors kept) into *desc / *norm, not yet the store's; NULLs
+// when there is no table.  Committed by the store after its pools; freed by loop_free
+int loop_table_alloc(const KeyframeStore& s, size_t cap_frames, float** desc, double** norm);
+void loop_free(Ctx* c);                                     // the scratch of loop detection in Ctx::kfs
 // so_map.cu: pts[0..n) at pose, in place, by k_transform_points (utils::TransformPoint: qrot in double, float store)
 void launch_transform(float4* pts, uint32_t n, const double pose[7], cudaStream_t st);
 // so_map.cu, so_map_from_keyframes in two steps so that two stores change together or not at all.  keyframe_map_filter: the map of the

@@ -10,7 +10,8 @@ namespace so {
 
 void keyframes_free(Ctx* c) {
     KeyframeStore& s = c->kf;
-    cudaFree(s.d_pool[0]); cudaFree(s.d_pool[1]);
+    cudaFree(s.d_pool[0]); cudaFree(s.d_pool[1]); cudaFree(s.d_desc); cudaFree(s.d_desc_norm);
+    loop_free(c);
     KeyframeScratch& k = c->kfs;
     cudaFree(k.d_segs); cudaFree(k.d_raw); cudaFree(k.d_keys); cudaFree(k.d_keys_out); cudaFree(k.d_vals); cudaFree(k.d_vals_out);
     cudaFree(k.d_out[0]); cudaFree(k.d_out[1]); cudaFree(k.d_blk); cudaFree(k.d_tmp); cudaFree(k.d_ctl);
@@ -24,27 +25,34 @@ static int keyframes_reserve(Ctx* c, size_t cap_points, size_t cap_frames) {
     KeyframeStore& s = c->kf;
     SO_CUDA_TRY(cudaStreamSynchronize(c->stream));
     if (cap_points == 0 && cap_frames == 0) {
-        cudaFree(s.d_pool[0]); cudaFree(s.d_pool[1]);
+        cudaFree(s.d_pool[0]); cudaFree(s.d_pool[1]); cudaFree(s.d_desc); cudaFree(s.d_desc_norm);
         s = KeyframeStore{};
         return SO_OK;
     }
     if (cap_frames < s.frames() || cap_points < held(s, 0) || cap_points < held(s, 1))
         return fail(SO_ERR_ARG, "so_keyframe_reserve: capacity below what the store holds");
+    float* desc = nullptr;
+    double* norm = nullptr;
+    if (cap_frames != s.desc_frames) { int rc = loop_table_alloc(s, cap_frames, &desc, &norm); if (rc) return rc; }
     float4* pool[2] = {nullptr, nullptr};
     if (cap_points != s.cap_points) {
         for (int k = 0; k < 2; ++k) {
             if (cudaMalloc(&pool[k], std::max<size_t>(cap_points, 1) * sizeof(float4)) != cudaSuccess) {
                 cudaGetLastError();
-                cudaFree(pool[0]);
+                cudaFree(pool[0]); cudaFree(desc); cudaFree(norm);
                 return fail(SO_ERR_CUDA, "so_keyframe_reserve: cudaMalloc of a keyframe pool failed");
             }
             if (held(s, k) && cudaMemcpy(pool[k], s.d_pool[k], held(s, k) * sizeof(float4), cudaMemcpyDeviceToDevice) != cudaSuccess) {
-                cudaFree(pool[0]); cudaFree(pool[1]);
+                cudaFree(pool[0]); cudaFree(pool[1]); cudaFree(desc); cudaFree(norm);
                 return fail(SO_ERR_CUDA, "so_keyframe_reserve: copy of the keyframes failed");
             }
         }
         for (int k = 0; k < 2; ++k) { cudaFree(s.d_pool[k]); s.d_pool[k] = pool[k]; }
         s.cap_points = cap_points;
+    }
+    if (desc) {                                                        // the descriptor table follows the frame table
+        cudaFree(s.d_desc); cudaFree(s.d_desc_norm);
+        s.d_desc = desc; s.d_desc_norm = norm; s.desc_frames = cap_frames;
     }
     for (int k = 0; k < 2; ++k) if (s.off[k].empty()) s.off[k].push_back(0);
     s.cap_frames = cap_frames;
@@ -201,7 +209,11 @@ int so_map_from_keyframes(so_ctx* dst_ctx, so_ctx* src_ctx, const int32_t* ids, 
         if (rc) return rc;
     }
     if (s == d)                                                        // the rebuild after a correction: the keyframes' poses move with it
-        for (size_t i = 0; i < n_ids; ++i) std::memcpy(d->kf.poses.data() + 7 * size_t(ids[i]), poses7 + 7 * i, 7 * sizeof(double));
+        for (size_t i = 0; i < n_ids; ++i) {                           // and the loop descriptors of those that moved go stale (host only)
+            double* p = d->kf.poses.data() + 7 * size_t(ids[i]);
+            if (std::memcmp(p, poses7 + 7 * i, 7 * sizeof(double)) && size_t(ids[i]) < d->kf.desc_ok.size()) d->kf.desc_ok[ids[i]] = 0;
+            std::memcpy(p, poses7 + 7 * i, 7 * sizeof(double));
+        }
     return SO_OK;
 }
 
