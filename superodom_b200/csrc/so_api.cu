@@ -97,60 +97,71 @@ int move_window(Ctx* c, const int32_t o[3]) {
 static int ctx_alloc(Ctx* c) {
     SO_CUDA_TRY(cudaSetDevice(c->device));
     SO_CUDA_TRY(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
-    SO_CUDA_TRY(cudaEventCreate(&c->ev0)); SO_CUDA_TRY(cudaEventCreate(&c->ev1));
-    SO_CUDA_TRY(cudaEventCreate(&c->evp0)); SO_CUDA_TRY(cudaEventCreate(&c->evp1));
+    int rc = c->ev0.create();
+    if (!rc) rc = c->ev1.create();
+    if (!rc) rc = c->evp0.create();
+    if (!rc) rc = c->evp1.create();
+    if (rc) return rc;
     SO_CUDA_TRY(cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking));
     SO_CUDA_TRY(cudaStreamCreateWithFlags(&c->aux_stream, cudaStreamNonBlocking));
-    SO_CUDA_TRY(cudaEventCreateWithFlags(&c->ev_fork, cudaEventDisableTiming));
-    SO_CUDA_TRY(cudaEventCreateWithFlags(&c->ev_join, cudaEventDisableTiming));
-    for (auto& e : c->ev_copy) SO_CUDA_TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    int rc = map_alloc(c);
+    rc = c->ev_fork.create(cudaEventDisableTiming);
+    if (!rc) rc = c->ev_join.create(cudaEventDisableTiming);
+    for (Event& e : c->ev_copy) if (!rc) rc = e.create(cudaEventDisableTiming);
+    if (!rc) rc = map_alloc(c);
     if (rc) return rc;
     c->max_batch = c->cfg.max_batch;
     c->scan_cap = size_t(c->cfg.max_scan_points) * c->max_batch;
     c->grid_x_cap = (c->cfg.max_scan_points + kThreads - 1) / kThreads;
-    SO_CUDA_TRY(cudaMalloc(&c->d_scan, c->scan_cap * sizeof(float4)));
-    SO_CUDA_TRY(cudaMalloc(&c->d_dec, size_t(kPrepareSmallCap) * sizeof(float4)));
-    SO_CUDA_TRY(cudaEventCreateWithFlags(&c->ev_dec, cudaEventDisableTiming));
-    SO_CUDA_TRY(cudaMalloc(&c->d_scan_sorted, c->scan_cap * sizeof(float4)));
-    SO_CUDA_TRY(cudaMalloc(&c->d_skeys, c->scan_cap * sizeof(uint64_t)));
-    SO_CUDA_TRY(cudaMalloc(&c->d_skeys_out, c->scan_cap * sizeof(uint64_t)));
-    SO_CUDA_TRY(cudaMalloc(&c->d_svals, c->scan_cap * sizeof(uint32_t)));
-    SO_CUDA_TRY(cudaMalloc(&c->d_svals_out, c->scan_cap * sizeof(uint32_t)));
-    SO_CUDA_TRY(cudaMalloc(&c->nn.pos, c->scan_cap * 5 * sizeof(uint32_t)));
-    SO_CUDA_TRY(cudaMalloc(&c->nn.d5, c->scan_cap * sizeof(float)));
-    SO_CUDA_TRY(cudaMalloc(&c->nn.pre, c->scan_cap));
-    c->nn.cap = c->scan_cap;
-    { int rc2 = scan_sort_alloc(c); if (rc2) return rc2; }
-    SO_CUDA_TRY(cudaMalloc(&c->d_offset, c->max_batch * sizeof(uint32_t)));
-    SO_CUDA_TRY(cudaMalloc(&c->d_state, c->max_batch * sizeof(IcpState)));
-    SO_CUDA_TRY(cudaMallocHost(&c->h_state, c->max_batch * sizeof(IcpState)));
-    SO_CUDA_TRY(cudaMallocHost(&c->h_offset, 2 * c->max_batch * sizeof(uint32_t)));      // [0, max_batch): scan offsets; then the edge clouds' offsets
+    rc = c->d_scan.reserve(c->scan_cap);
+    if (!rc) rc = c->d_dec.reserve(kPrepareSmallCap);
+    if (!rc) rc = c->ev_dec.create(cudaEventDisableTiming);
+    if (!rc) rc = c->d_scan_sorted.reserve(c->scan_cap);
+    if (!rc) rc = c->d_skeys.reserve(c->scan_cap);
+    if (!rc) rc = c->d_skeys_out.reserve(c->scan_cap);
+    if (!rc) rc = c->d_svals.reserve(c->scan_cap);
+    if (!rc) rc = c->d_svals_out.reserve(c->scan_cap);
+    if (!rc) rc = c->d_nn_pos.reserve(c->scan_cap * 5);
+    if (!rc) rc = c->d_nn_d5.reserve(c->scan_cap);
+    if (!rc) rc = c->d_nn_pre.reserve(c->scan_cap);
+    if (!rc) rc = scan_sort_alloc(c);
+    if (!rc) rc = c->d_offset.reserve(c->max_batch);
+    if (!rc) rc = c->d_state.reserve(c->max_batch);
+    if (!rc) rc = c->h_state.reserve(c->max_batch);
+    if (!rc) rc = c->h_offset.reserve(2 * size_t(c->max_batch));       // [0, max_batch): scan offsets; then the edge clouds' offsets
+    if (rc) return rc;
+    c->nn.pos = c->d_nn_pos; c->nn.d5 = c->d_nn_d5; c->nn.pre = c->d_nn_pre; c->nn.cap = c->scan_cap;
     c->h_eoffset = c->h_offset + c->max_batch;
     c->edge_cap = c->cfg.max_scan_points;
     c->edge_grid_cap = uint32_t((c->edge_cap + kThreads - 1) / kThreads);
-    SO_CUDA_TRY(cudaMalloc(&c->d_partials, size_t(c->max_batch) * (c->grid_x_cap + c->edge_grid_cap) * kAcc * sizeof(double)));
-    SO_CUDA_TRY(cudaMalloc(&c->d_escan, c->edge_cap * sizeof(float4)));
-    SO_CUDA_TRY(cudaMalloc(&c->d_eoffset, c->max_batch * sizeof(uint32_t)));
+    rc = c->d_partials.reserve(size_t(c->max_batch) * (c->grid_x_cap + c->edge_grid_cap) * kAcc);
+    if (!rc) rc = c->d_escan.reserve(c->edge_cap);
+    if (!rc) rc = c->d_eoffset.reserve(c->max_batch);
+    if (rc) return rc;
     SO_CUDA_TRY(cudaMemset(c->d_eoffset, 0, c->max_batch * sizeof(uint32_t)));
-    SO_CUDA_TRY(cudaMalloc(&c->ebuf.a, c->edge_cap * sizeof(double4)));
-    SO_CUDA_TRY(cudaMalloc(&c->ebuf.b, c->edge_cap * sizeof(double4)));
-    SO_CUDA_TRY(cudaMalloc(&c->ebuf.flags, c->edge_cap * sizeof(uchar4)));
-    SO_CUDA_TRY(cudaMalloc(&c->ebuf.nn, c->edge_cap * 10 * sizeof(uint32_t)));
-    SO_CUDA_TRY(cudaMalloc(&c->ebuf.selmask, c->edge_cap * sizeof(uint32_t)));
+    rc = c->d_ebuf_a.reserve(c->edge_cap);
+    if (!rc) rc = c->d_ebuf_b.reserve(c->edge_cap);
+    if (!rc) rc = c->d_ebuf_flags.reserve(c->edge_cap);
+    if (!rc) rc = c->d_ebuf_nn.reserve(c->edge_cap * 10);
+    if (!rc) rc = c->d_ebuf_selmask.reserve(c->edge_cap);
+    if (rc) return rc;
+    c->ebuf.a = c->d_ebuf_a; c->ebuf.b = c->d_ebuf_b; c->ebuf.flags = c->d_ebuf_flags; c->ebuf.nn = c->d_ebuf_nn; c->ebuf.selmask = c->d_ebuf_selmask;
     c->ebuf.scan = c->d_escan; c->ebuf.offset = c->d_eoffset;
-    SO_CUDA_TRY(cudaMalloc(&c->d_counters, c->max_batch * sizeof(uint32_t)));
-    SO_CUDA_TRY(cudaMalloc(&c->d_hist, c->max_batch * kHistStride * sizeof(int32_t)));
+    rc = c->d_counters.reserve(c->max_batch);
+    if (!rc) rc = c->d_hist.reserve(size_t(c->max_batch) * kHistStride);
+    if (rc) return rc;
     SO_CUDA_TRY(cudaMemset(c->d_counters, 0, c->max_batch * sizeof(uint32_t)));
     SO_CUDA_TRY(cudaMemset(c->d_hist, 0, c->max_batch * kHistStride * sizeof(int32_t)));
-    SO_CUDA_TRY(cudaMalloc(&c->corr.nd, c->scan_cap * sizeof(double4)));
-    SO_CUDA_TRY(cudaMalloc(&c->corr.w, c->scan_cap * sizeof(double)));
-    SO_CUDA_TRY(cudaMalloc(&c->corr.flags, c->scan_cap * sizeof(uchar4)));
-    SO_CUDA_TRY(cudaMalloc(&c->corr.nn, size_t(c->cfg.max_scan_points) * 5 * sizeof(uint32_t)));
-    SO_CUDA_TRY(cudaMalloc(&c->corr.nn_d2, size_t(c->cfg.max_scan_points) * 5 * sizeof(float)));
+    rc = c->d_corr_nd.reserve(c->scan_cap);
+    if (!rc) rc = c->d_corr_w.reserve(c->scan_cap);
+    if (!rc) rc = c->d_corr_flags.reserve(c->scan_cap);
+    if (!rc) rc = c->d_corr_nn.reserve(size_t(c->cfg.max_scan_points) * 5);
+    if (!rc) rc = c->d_corr_nn_d2.reserve(size_t(c->cfg.max_scan_points) * 5);
+    if (rc) return rc;
+    c->corr.nd = c->d_corr_nd; c->corr.w = c->d_corr_w; c->corr.flags = c->d_corr_flags; c->corr.nn = c->d_corr_nn; c->corr.nn_d2 = c->d_corr_nn_d2;
     return SO_OK;
 }
 
+// The buffers and events free themselves with the context; the streams and graph execs are freed here
 static void ctx_free(Ctx* c) {
     if (!c) return;
     cudaSetDevice(c->device);
@@ -158,44 +169,14 @@ static void ctx_free(Ctx* c) {
     for (auto& g : c->graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
     if (c->copy_stream) cudaStreamDestroy(c->copy_stream);
     if (c->aux_stream) cudaStreamDestroy(c->aux_stream);
-    if (c->ev_fork) cudaEventDestroy(c->ev_fork);
-    if (c->ev_join) cudaEventDestroy(c->ev_join);
-    for (auto& e : c->ev_copy) if (e) cudaEventDestroy(e);
-    map_free(c);
-    cudaFree(c->d_graph_stats);
-    cudaFree(c->d_scan_sorted); cudaFree(c->d_skeys); cudaFree(c->d_skeys_out); cudaFree(c->d_svals); cudaFree(c->d_svals_out);
-    cudaFree(c->d_sort_tmp); cudaFree(c->d_sort_tmp2); cudaFree(c->nn.pos); cudaFree(c->nn.d5); cudaFree(c->nn.pre); cudaFree(c->nn.queue); cudaFree(c->nn.qcount);
-    cudaFree(c->d_scan); cudaFree(c->d_offset); cudaFree(c->d_state); cudaFreeHost(c->h_state); cudaFreeHost(c->h_offset);
-    cudaFree(c->d_partials); cudaFree(c->d_counters); cudaFree(c->d_hist);
-    cudaFree(c->d_escan); cudaFree(c->d_eoffset); cudaFree(c->ebuf.a); cudaFree(c->ebuf.b); cudaFree(c->ebuf.flags); cudaFree(c->ebuf.nn); cudaFree(c->ebuf.selmask);
-    cudaFree(c->corr.nd); cudaFree(c->corr.w); cudaFree(c->corr.flags); cudaFree(c->corr.nn); cudaFree(c->corr.nn_d2);
-    cudaFree(c->d_q); cudaFree(c->d_knn_idx); cudaFree(c->d_knn_d2); cudaFree(c->d_inject);
-    cudaFree(c->d_qkeys); cudaFree(c->d_qkeys_out); cudaFree(c->d_qvals); cudaFree(c->d_qvals_out); cudaFree(c->d_qsort_tmp);
-    if (c->h_stage) cudaFreeHost(c->h_stage);
-    cudaFree(c->d_dec);
-    global_free(c);
-    undistort_free(c);
-    motion_free(c);
-    cudaFree(c->deg.d_st);
-    features_free(c);
-    free_space_free(c);
-    keyframes_free(c);
-    if (c->ev_dec) cudaEventDestroy(c->ev_dec);
-    if (c->ev0) cudaEventDestroy(c->ev0);
-    if (c->ev1) cudaEventDestroy(c->ev1);
-    if (c->evp0) cudaEventDestroy(c->evp0);
-    if (c->evp1) cudaEventDestroy(c->evp1);
     if (c->own_stream && c->stream) cudaStreamDestroy(c->stream);
     delete c;
 }
 
-static int ensure_stage(Ctx* c, size_t bytes) {
-    if (bytes <= c->h_stage_bytes) return SO_OK;
-    if (c->h_stage) { cudaDeviceSynchronize(); cudaFreeHost(c->h_stage); }      // no copy out of the old buffer may still be in flight
-    c->h_stage = nullptr; c->h_stage_bytes = 0;
-    SO_CUDA_TRY(cudaMallocHost(&c->h_stage, bytes));
-    c->h_stage_bytes = bytes;
-    return SO_OK;
+static int ensure_stage(Ctx* c, size_t n) {
+    if (n <= c->h_stage.cap()) return SO_OK;
+    if (c->h_stage) cudaDeviceSynchronize();           // no copy out of the old buffer may still be in flight
+    return c->h_stage.reserve(n);
 }
 
 // Copy a strided host cloud into device float4 {x,y,z,intensity}.  Packed float4 input goes straight through.
@@ -206,10 +187,10 @@ int upload_cloud(Ctx* c, const void* src, size_t n, size_t stride, size_t ioff, 
         c->bytes_h2d += n * sizeof(float4);
         return SO_OK;
     }
-    int rc = ensure_stage(c, n * sizeof(float4));
+    int rc = ensure_stage(c, n);
     if (rc) return rc;
     SO_CUDA_TRY(cudaStreamSynchronize(c->stream));     // staging buffer reuse
-    float4* h = static_cast<float4*>(c->h_stage);
+    float4* h = c->h_stage;
     const unsigned char* p = static_cast<const unsigned char*>(src);
     for (size_t i = 0; i < n; ++i, p += stride) {
         float xyz[3], it = 0.f;
@@ -250,7 +231,7 @@ static int run_deferred_upload(Ctx* c) {
     if (c->defer.stride == 16 && c->defer.ioff == 12) {
         SO_CUDA_TRY(cudaMemcpyAsync(c->d_scan, src, n * sizeof(float4), cudaMemcpyHostToDevice, c->copy_stream));
     } else {
-        float4* h = static_cast<float4*>(c->h_stage) + c->defer.stage_off;
+        float4* h = c->h_stage + c->defer.stage_off;
         const unsigned char* p = static_cast<const unsigned char*>(src);
         for (size_t i = 0; i < n; ++i, p += c->defer.stride) h[i] = read_point(p, c->defer.stride, c->defer.ioff);
         SO_CUDA_TRY(cudaMemcpyAsync(c->d_scan, h, n * sizeof(float4), cudaMemcpyHostToDevice, c->copy_stream));
@@ -292,9 +273,10 @@ void timed_launch_end(Ctx* c, int cls) {
 // per-scan, per-iteration queue lengths of the call's n_scans scans, zeroed.
 static int graph_queue_begin(Ctx* c, size_t n_scans) {
     if (!knn_graph_valid(c)) return SO_OK;
-    int rc = grow_buffer(c->nn.queue, c->queue_cap, c->scan_cap);
-    if (!rc) rc = grow_buffer(c->nn.qcount, c->qcount_cap, size_t(c->max_batch) * SO_MAX_ICP_ITERS);
+    int rc = c->d_nn_queue.reserve(c->scan_cap);
+    if (!rc) rc = c->d_nn_qcount.reserve(size_t(c->max_batch) * SO_MAX_ICP_ITERS);
     if (rc) return rc;
+    c->nn.queue = c->d_nn_queue; c->nn.qcount = c->d_nn_qcount;
     SO_CUDA_TRY(cudaMemsetAsync(c->nn.qcount, 0, n_scans * SO_MAX_ICP_ITERS * sizeof(uint32_t), c->stream));
     return SO_OK;
 }
@@ -680,7 +662,7 @@ static int register_core(Ctx* c, const RegisterRequest& q) {
             if (ch.grid_x == 0) continue;
             int rc = prepare_scans(c, d_scan, ch, st, true);
             bool was_loop = false;
-            if (!rc) rc = run_schedule(c, ch, o.max_icp_iters, o.lm_max_iterations, q.mode, q.inject ? c->d_inject : nullptr, q.inject_iters, st, &was_loop,
+            if (!rc) rc = run_schedule(c, ch, o.max_icp_iters, o.lm_max_iterations, q.mode, q.inject ? c->d_inject.get() : nullptr, q.inject_iters, st, &was_loop,
                                        q.degen ? c->deg.d_st + ch.first : nullptr);
             if (rc) {                                       // leave no work behind on the side streams before reporting the error
                 cudaStreamSynchronize(c->aux_stream);
@@ -731,9 +713,9 @@ static int upload_kept(Ctx* c, const RegisterRequest& q, size_t n_edge, uint32_t
     const bool packed = q.stride == 16 && q.ioff == 12;
     if (n_edge && !packed) SO_CUDA_TRY(cudaStreamSynchronize(c->stream));     // a strided edge cloud has to have left the staging buffer
     SO_CUDA_TRY(cudaEventSynchronize(c->ev_dec));                              // so has the previous call's deferred copy
-    int rc = ensure_stage(c, (size_t(kPrepareSmallCap) + (packed ? 0 : n)) * sizeof(float4));
+    int rc = ensure_stage(c, size_t(kPrepareSmallCap) + (packed ? 0 : n));
     if (rc) return rc;
-    float4* h = static_cast<float4*>(c->h_stage);
+    float4* h = c->h_stage;
     const unsigned char* p = static_cast<const unsigned char*>(q.scans);
     for (uint32_t j = 0; j < kept; ++j) h[j] = read_point(p + size_t(keep[j]) * q.stride, q.stride, q.ioff);
     SO_CUDA_TRY(cudaEventRecord(c->ev_copy[16], c->stream));                  // the whole-cloud copy must not overtake earlier readers of d_scan
@@ -757,10 +739,10 @@ int register_scans(Ctx* c, const RegisterRequest& q) {
     int rc = SO_OK;
     if (q.mode == UndistortionMode::APPROXIMATED) rc = undistort_reserve(c, total);
     if (q.mode == UndistortionMode::OPTIMIZED) rc = motion_reserve(c, total);
-    if (!rc && q.degen) rc = grow_buffer(c->deg.d_st, c->deg.st_cap, size_t(c->max_batch));
+    if (!rc && q.degen) rc = c->deg.d_st.reserve(c->max_batch);
     if (!rc && q.inject) {
         const size_t words = size_t(q.inject_iters) * total * 5;
-        rc = grow_buffer(c->d_inject, c->inject_cap, words);
+        rc = c->d_inject.reserve(words);
         if (!rc) SO_CUDA_TRY(cudaMemcpyAsync(c->d_inject, q.inject, words * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
     }
     const bool edge_times = q.mode != UndistortionMode::NONE && q.edge && total_e;    // so_register_undistort_edges / _optimized_edges
@@ -786,7 +768,7 @@ int register_scans(Ctx* c, const RegisterRequest& q) {
         if (total) SO_CUDA_TRY(cudaMemcpyAsync(c->d_scan, c->d_scan_sorted, total * sizeof(float4), cudaMemcpyDeviceToDevice, c->stream));
         // the filtered cloud's w (the VoxelGrid average of the time the extraction stored in intensity) is the time
         if (total && with_times)
-            SO_CUDA_TRY(cudaMemcpy2DAsync(c->und.d_time, sizeof(float), reinterpret_cast<const char*>(c->d_scan_sorted) + 12, sizeof(float4),
+            SO_CUDA_TRY(cudaMemcpy2DAsync(c->und.d_time, sizeof(float), reinterpret_cast<const char*>(c->d_scan_sorted.get()) + 12, sizeof(float4),
                                           sizeof(float), total, cudaMemcpyDeviceToDevice, c->stream));
     }
     if (!rc && host && with_times) rc = upload_times(c, q.scans, total, q.stride, q.toff, c->und.d_time);
@@ -988,9 +970,9 @@ int so_map_shift(so_ctx* ctx, const double t[3], int32_t out_ijk[3]) {
 
 static int store_set_points(Ctx* c, MapStore& ms, const void* xyzi, size_t n, size_t stride, size_t ioff) {
     if (!c || (!xyzi && n) || stride < 12) return fail(SO_ERR_ARG, "bad args");
-    if (n > c->cfg.max_map_points + ms.arc.cap) return fail(SO_ERR_CAPACITY, "map larger than so_config.max_map_points (plus the block archive)");
+    if (n > c->cfg.max_map_points + ms.arc.d_pool.cap()) return fail(SO_ERR_CAPACITY, "map larger than so_config.max_map_points (plus the block archive)");
     SO_CUDA_TRY(cudaSetDevice(c->device));
-    if (ms.arc.cap) {                                        // window and archive replaced together; the checks come before any change
+    if (ms.arc.d_pool) {                                          // window and archive replaced together; the checks come before any change
         std::vector<float4> pts(n);
         const unsigned char* p = static_cast<const unsigned char*>(xyzi);
         for (size_t i = 0; i < n; ++i) pts[i] = read_point(p + i * stride, stride, ioff);
@@ -1124,7 +1106,7 @@ int so_map_archive_info(so_ctx* ctx, int store, size_t* n_points, size_t* n_bloc
     const BlockArchive& a = (store ? c->edge : c->surf).arc;
     if (n_points) *n_points = a.live;
     if (n_blocks) *n_blocks = a.dir.size();
-    if (cap_points) *cap_points = a.cap;
+    if (cap_points) *cap_points = a.d_pool.cap();
     return SO_OK;
 }
 
@@ -1322,7 +1304,7 @@ int so_scan_deskew(so_ctx* ctx, void* points, size_t n, size_t stride, size_t ti
         hs[k] = sample_times[k];
         for (int j = 0; j < 7; ++j) hs[n_samples + 7 * k + j] = (imu_only && j < 3) ? 0.0 : sample_poses[7 * k + j];
     }
-    double* d_samples = reinterpret_cast<double*>(c->d_skeys);
+    double* d_samples = reinterpret_cast<double*>(c->d_skeys.get());
     SO_CUDA_TRY(cudaMemcpyAsync(d_samples, hs.data(), hs.size() * sizeof(double), cudaMemcpyHostToDevice, c->stream));
     count_h2d(c, hs.size() * sizeof(double));
     SO_CUDA_TRY(cudaMemsetAsync(c->d_svals, 0, 4, c->stream));
@@ -1331,14 +1313,14 @@ int so_scan_deskew(so_ctx* ctx, void* points, size_t n, size_t stride, size_t ti
     launch_deskew(c->d_scan, uint32_t(n), P, c->stream);
     c->launches++;
     timed_launch_end(c, 3);
-    rc = ensure_stage(c, n * sizeof(float4));
+    rc = ensure_stage(c, n);
     if (rc) return rc;
     uint32_t past = 0;
     SO_CUDA_TRY(cudaMemcpyAsync(c->h_stage, c->d_scan, n * sizeof(float4), cudaMemcpyDeviceToHost, c->stream));
     SO_CUDA_TRY(cudaMemcpyAsync(&past, c->d_svals, 4, cudaMemcpyDeviceToHost, c->stream));
     count_d2h(c, n * sizeof(float4) + 4);
     SO_CUDA_TRY(cudaStreamSynchronize(c->stream));                                 // also covers hs going out of scope
-    const float4* h = static_cast<const float4*>(c->h_stage);
+    const float4* h = c->h_stage;
     unsigned char* dst = static_cast<unsigned char*>(points);
     for (size_t i = 0; i < n; ++i, dst += stride) std::memcpy(dst, &h[i], 12);     // x, y, z only; every other field untouched
     if (n_past_end) *n_past_end = past;
@@ -1822,7 +1804,7 @@ int so_covariance(so_ctx* ctx, const double* H, int32_t n, so_icp_result* out) {
         SO_CUDA_TRY(cudaMemcpyAsync(c->d_state, c->h_state, sizeof(IcpState), cudaMemcpyHostToDevice, c->stream));
         launch_covariance(c->d_state, c->stream);
     } else {
-        { int rc = grow_buffer(c->mot.d_st, c->mot.st_cap, std::max<size_t>(c->max_batch, 1)); if (rc) return rc; }
+        { int rc = c->mot.d_st.reserve(std::max<size_t>(c->max_batch, 1)); if (rc) return rc; }
         MotionState M{};
         for (int i = 0; i < 12; ++i) for (int j = i; j < 12; ++j) M.H[i * 12 - (i * (i - 1)) / 2 + (j - i)] = H[i * 12 + j];
         SO_CUDA_TRY(cudaMemcpyAsync(c->d_state, c->h_state, sizeof(IcpState), cudaMemcpyHostToDevice, c->stream));
@@ -1846,7 +1828,7 @@ int so_degeneracy_analysis(so_ctx* ctx, const double* H, const so_degeneracy* d,
     if (!c || !H || !d || !out) return fail(SO_ERR_ARG, "bad args");
     { int rc = check_degeneracy(d, 1); if (rc) return rc; }
     SO_CUDA_TRY(cudaSetDevice(c->device));
-    { int rc = grow_buffer(c->deg.d_st, c->deg.st_cap, std::max<size_t>(c->max_batch, 1)); if (rc) return rc; }
+    { int rc = c->deg.d_st.reserve(std::max<size_t>(c->max_batch, 1)); if (rc) return rc; }
     IcpState& s = c->h_state[0];                              // the state of a preceding so_correspond* is replaced
     std::memset(&s, 0, sizeof(s));
     for (int i = 0; i < 6; ++i) for (int j = i; j < 6; ++j) s.H[tri(i, j)] = H[i * 6 + j];
@@ -1884,7 +1866,7 @@ int so_solve(so_ctx* ctx, const so_solve_row* rows, const so_solve_problem* pr, 
     }
     if (total && !rows) return fail(SO_ERR_ARG, "bad args");
     SO_CUDA_TRY(cudaSetDevice(c->device));
-    if (d) { int rc = grow_buffer(c->deg.d_st, c->deg.st_cap, size_t(c->max_batch)); if (rc) return rc; }
+    if (d) { int rc = c->deg.d_st.reserve(c->max_batch); if (rc) return rc; }
     c->prefiltered_n = SIZE_MAX;                                  // d_scan_sorted is overwritten
     std::vector<float4> sp(total);
     std::vector<double4> nd(total);
@@ -1930,7 +1912,7 @@ int so_solve(so_ctx* ctx, const so_solve_row* rows, const so_solve_problem* pr, 
     if (fused_lm(c, uint32_t(n_problems), UndistortionMode::NONE, d != nullptr)) bv.counters = c->d_counters;
     CorrBuf cb = c->corr;
     cb.nn = nullptr; cb.nn_d2 = nullptr;
-    DegenState* const ddg = d ? c->deg.d_st : nullptr;
+    DegenState* const ddg = d ? c->deg.d_st.get() : nullptr;
     const uint32_t nb = uint32_t(n_problems);
     timed_launch_begin(c);
     launch_first_eval(bv, cb, grid_x, nb, st, nullptr, nullptr, 0, ddg);
@@ -1992,9 +1974,9 @@ int so_knn(so_ctx* ctx, const float* q_xyz, size_t nq, size_t stride, int k, flo
     Ctx* c = reinterpret_cast<Ctx*>(ctx);
     if (!c || !q_xyz || !idx || !d2 || k < 1 || k > 8 || stride < 12) return fail(SO_ERR_ARG, "bad args");
     SO_CUDA_TRY(cudaSetDevice(c->device));
-    int rc = grow_buffer(c->d_q, c->q_cap, nq);
-    if (!rc) rc = grow_buffer(c->d_knn_idx, c->knn_idx_cap, nq * 8);
-    if (!rc) rc = grow_buffer(c->d_knn_d2, c->knn_d2_cap, nq * 8);
+    int rc = c->d_q.reserve(nq);
+    if (!rc) rc = c->d_knn_idx.reserve(nq * 8);
+    if (!rc) rc = c->d_knn_d2.reserve(nq * 8);
     if (rc) return rc;
     rc = upload_cloud(c, q_xyz, nq, stride, stride /* no intensity */, c->d_q);
     if (rc) return rc;
@@ -2104,12 +2086,14 @@ int so_knn_graph_stats(so_ctx* ctx, int on, uint64_t* counts) {
         }
         for (int i = 0; i < 2 * SO_MAX_ICP_ITERS; ++i) counts[i] = h[i];
     }
-    if (on && !c->d_graph_stats) SO_CUDA_TRY(cudaMalloc(&c->d_graph_stats, bytes));
-    if (on) SO_CUDA_TRY(cudaMemsetAsync(c->d_graph_stats, 0, bytes, c->stream));
+    if (on) {
+        int rc = c->d_graph_stats.reserve(2 * SO_MAX_ICP_ITERS);
+        if (rc) return rc;
+        SO_CUDA_TRY(cudaMemsetAsync(c->d_graph_stats, 0, bytes, c->stream));
+    }
     if (!on && c->d_graph_stats) {
         SO_CUDA_TRY(cudaStreamSynchronize(c->stream));
-        cudaFree(c->d_graph_stats);
-        c->d_graph_stats = nullptr;
+        c->d_graph_stats.reset();
     }
     return SO_OK;
 }

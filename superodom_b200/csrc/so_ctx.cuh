@@ -3,7 +3,7 @@
 #include <cstring>
 #include <map>
 #include <string>
-#include <type_traits>
+#include <utility>
 #include <vector>
 
 #include "so_icp.cuh"
@@ -21,20 +21,65 @@ namespace so {
 
 void set_error(const std::string& s);
 
-// Grow-only device buffer: when n elements (bytes for void) exceed cap, free the old buffer and allocate n; the contents are not
-// kept.  A failed allocation leaves cap at 0, so the next call retries.
-template <class T>
-int grow_buffer(T*& p, size_t& cap, size_t n) {
-    if (n <= cap) return SO_OK;
-    cudaFree(p);
-    p = nullptr;
-    cap = 0;
-    size_t bytes = n;
-    if constexpr (!std::is_void_v<T>) bytes *= sizeof(T);
-    SO_CUDA_TRY(cudaMalloc(&p, bytes));
-    cap = n;
-    return SO_OK;
-}
+// Owner of one device (Pinned = false: cudaMalloc) or pinned host (true: cudaMallocHost) allocation of T; freed by its destructor and
+// by move-assignment.  Grow-only: reserve(n) does nothing when n <= cap(), else frees the old allocation first (the contents are not
+// kept, so peak memory does not grow) and allocates n elements.  A failed allocation leaves the buffer empty, so the next call retries.
+// Converts to T* (and has ->), so kernel arguments, copies and pointer arithmetic take the buffer as they took the pointer.
+template <class T, bool Pinned>
+class Buffer {
+public:
+    Buffer() = default;
+    Buffer(const Buffer&) = delete;
+    Buffer& operator=(const Buffer&) = delete;
+    Buffer(Buffer&& o) noexcept : p_(std::exchange(o.p_, nullptr)), cap_(std::exchange(o.cap_, 0)) {}
+    Buffer& operator=(Buffer&& o) noexcept {
+        if (this != &o) { reset(); p_ = std::exchange(o.p_, nullptr); cap_ = std::exchange(o.cap_, 0); }
+        return *this;
+    }
+    ~Buffer() { reset(); }
+    int reserve(size_t n) {                        // the only member that needs T complete
+        if (n <= cap_) return SO_OK;
+        reset();
+        void* p = nullptr;
+        if constexpr (Pinned) SO_CUDA_TRY(cudaMallocHost(&p, n * sizeof(T)));
+        else SO_CUDA_TRY(cudaMalloc(&p, n * sizeof(T)));
+        p_ = static_cast<T*>(p);
+        cap_ = n;
+        return SO_OK;
+    }
+    void reset() {
+        if (p_) { if constexpr (Pinned) cudaFreeHost(p_); else cudaFree(p_); }
+        p_ = nullptr;
+        cap_ = 0;
+    }
+    T* get() const { return p_; }
+    size_t cap() const { return cap_; }
+    operator T*() const { return p_; }
+    T* operator->() const { return p_; }
+private:
+    T* p_ = nullptr;
+    size_t cap_ = 0;
+};
+template <class T> using DeviceBuffer = Buffer<T, false>;
+template <class T> using PinnedBuffer = Buffer<T, true>;
+
+// Owner of one CUDA event: create(flags) makes it (replacing any it held), the destructor destroys it
+class Event {
+public:
+    Event() = default;
+    Event(const Event&) = delete;
+    Event& operator=(const Event&) = delete;
+    ~Event() { if (e_) cudaEventDestroy(e_); }
+    int create(unsigned flags = cudaEventDefault) {
+        if (e_) cudaEventDestroy(e_);
+        e_ = nullptr;
+        SO_CUDA_TRY(cudaEventCreateWithFlags(&e_, flags));
+        return SO_OK;
+    }
+    operator cudaEvent_t() const { return e_; }
+private:
+    cudaEvent_t e_ = nullptr;
+};
 
 struct ProfileSlot { double ms = 0.0; uint64_t launches = 0; };
 constexpr int kMotionAcc = 91;                     // 78 (upper triangle of the 12x12 H) + 12 (g) + 1 (cost)
@@ -111,15 +156,14 @@ struct RegisterRequest {
 };
 
 // Block archive of one store (so_map_archive; so_archive.h): the clouds of blocks the window dropped, each kept as one segment of a
-// point pool in its in-block order, found through a directory sorted by world key.  cap == 0: off, nothing allocated.
+// point pool in its in-block order, found through a directory sorted by world key.  d_pool.cap() == 0: off, nothing allocated.
 struct GatherSeg { uint64_t src, dst; uint32_t n, pad; };      // one block cloud copied src[0..n) -> dst[0..n) (k_seg_gather)
 struct BlockArchive {
     struct Seg { uint64_t off; uint32_t n; };
-    size_t cap = 0;                                // points the pool holds
-    float4* d_pool = nullptr;                      // [cap]: segments in [0, used), holes where blocks were restored
+    DeviceBuffer<float4> d_pool;                   // [cap()]: segments in [0, used), holes where blocks were restored
     size_t used = 0, live = 0;                     // pool tail; points in live segments
     std::map<uint64_t, Seg> dir;                   // world key -> segment, key order (host: every origin change goes through the host)
-    GatherSeg* d_segs = nullptr; size_t segs_cap = 0;   // segment lists of the gathers
+    DeviceBuffer<GatherSeg> d_segs;                // segment lists of the gathers
 };
 
 // Keyframe store (so_keyframes.cu; so_keyframe_reserve): registered scans kept on the device with their poses, for a loop-closing back
@@ -127,13 +171,15 @@ struct BlockArchive {
 // it (sensor frame, motion-compensated as registered).  cap_frames == 0: off, nothing allocated.
 struct KeyframeStore {
     size_t cap_points = 0, cap_frames = 0;         // points per pool, keyframes
-    float4* d_pool[2] = {nullptr, nullptr};        // [cap_points] each
+    DeviceBuffer<float4> d_pool[2];                // [cap_points] each
     std::vector<uint64_t> off[2];                  // [frames + 1] first point of every keyframe, then the pool's tail
     std::vector<double> poses;                     // [frames][7]
     size_t frames() const { return poses.size() / 7; }
-    // Scan Context descriptors (so_loop.cu), by keyframe id: [desc_frames][rings][sectors] images and [desc_frames][sectors] column
-    // norms for the options in desc_opts (rings == 0: no table); desc_ok[id] = 1 while id's descriptor is valid for them and its pose
-    float* d_desc = nullptr; double* d_desc_norm = nullptr; size_t desc_frames = 0;
+    // Scan Context descriptors (so_loop.cu), by keyframe id: [cap_frames][rings][sectors] images and [cap_frames][sectors] column
+    // norms for the options in desc_opts (rings == 0: no table, else one of cap_frames keyframes); desc_ok[id] = 1 while id's
+    // descriptor is valid for them and its pose
+    DeviceBuffer<float> d_desc;
+    DeviceBuffer<double> d_desc_norm;
     so_loop_opts desc_opts{};
     std::vector<uint8_t> desc_ok;
 };
@@ -142,34 +188,31 @@ struct KfSeg { uint64_t src; uint32_t start, n; double pose[7]; };
 // Scratch of so_map_from_keyframes and so_register_keyframes (so_keyframes.cu), grown on demand: the union of the selected keyframes
 // in the world frame, its sort, and the filtered cloud of each store until both have passed their capacity checks
 struct KeyframeScratch {
-    KfSeg* d_segs = nullptr; size_t segs_cap = 0;
-    float4* d_raw = nullptr; size_t raw_cap = 0;
-    uint64_t* d_keys = nullptr; size_t keys_cap = 0;
-    uint64_t* d_keys_out = nullptr; size_t keys_out_cap = 0;
-    uint32_t* d_vals = nullptr; size_t vals_cap = 0;
-    uint32_t* d_vals_out = nullptr; size_t vals_out_cap = 0;
-    float4* d_out[2] = {nullptr, nullptr}; size_t out_cap[2] = {0, 0};
-    uint32_t* d_blk = nullptr; size_t blk_cap = 0;         // block of every filtered point, then the block runs
-    void* d_tmp = nullptr; size_t tmp_bytes = 0;
-    int32_t* d_ctl = nullptr; int32_t* h_ctl = nullptr;    // [8] world-block bounds and run count (pinned mirror)
+    DeviceBuffer<KfSeg> d_segs;
+    DeviceBuffer<float4> d_raw;
+    DeviceBuffer<uint64_t> d_keys, d_keys_out;
+    DeviceBuffer<uint32_t> d_vals, d_vals_out;
+    DeviceBuffer<float4> d_out[2];
+    DeviceBuffer<uint32_t> d_blk;                          // block of every filtered point, then the block runs
+    DeviceBuffer<unsigned char> d_tmp;
+    DeviceBuffer<int32_t> d_ctl;                           // [8] world-block bounds and run count
+    PinnedBuffer<int32_t> h_ctl;                           // its mirror
     // loop detection (so_loop.cu): keyframes to describe, the queries, one chunk's pair table and every query's top k
-    struct DescSeg* d_dsegs = nullptr; size_t dsegs_cap = 0;
-    int32_t* d_queries = nullptr; size_t queries_cap = 0;
-    struct LoopPair* d_pairs = nullptr; size_t pairs_cap = 0;
-    struct LoopPair* d_top = nullptr; size_t top_cap = 0;
-    cudaEvent_t ev_loop[4] = {};                            // describe start / end, search start / end
+    DeviceBuffer<struct DescSeg> d_dsegs;
+    DeviceBuffer<int32_t> d_queries;
+    DeviceBuffer<struct LoopPair> d_pairs, d_top;
+    Event ev_loop[4];                                      // describe start / end, search start / end
 };
 
 // One per-block cloud family of the LocalMap (surf or edge): points in id order, the sorted hash grid, block tables.
 struct MapStore {
     float res = 0.4f;                              // planeRes_ (surf) / lineRes_ (edge): voxel leaf and gate / search radius
     uint32_t n = 0;                                // points held (on-grid)
-    float4* d_xyzi = nullptr;                      // [max_map] id order, w = intensity
-    float4* d_sorted = nullptr;                    // [max_map] sorted by (slot, cell), w = bitcast(id)
-    int32_t* d_block_slot = nullptr;               // [4851]
-    int32_t* d_block_count = nullptr;              // [4851]
-    uint32_t* d_cell_start = nullptr;              // [cell_cap]
-    size_t cell_cap = 0;
+    DeviceBuffer<float4> d_xyzi;                   // [max_map] id order, w = intensity
+    DeviceBuffer<float4> d_sorted;                 // [max_map] sorted by (slot, cell), w = bitcast(id)
+    DeviceBuffer<int32_t> d_block_slot;            // [4851]
+    DeviceBuffer<int32_t> d_block_count;           // [4851]
+    DeviceBuffer<uint32_t> d_cell_start;
     std::vector<int32_t> h_block_count, h_block_slot;   // host mirrors
     int n_slots = 0;
     int nb = 64;                                   // cells per block axis
@@ -177,8 +220,8 @@ struct MapStore {
     uint64_t index_gen = 0;                        // bumped by every index build: a neighbour graph is valid for one index only
     // neighbour graph of the sorted cloud (surf store; knn_graph_prepare): kGraphK positions per point, AoS, and the radius below
     // which a row is complete.  Valid while graph_gen == index_gen and the store is clean.
-    uint32_t* d_graph = nullptr; size_t graph_cap = 0;      // [graph_cap][kGraphK]
-    float* d_graph_radius = nullptr; size_t radius_cap = 0;
+    DeviceBuffer<uint32_t> d_graph;                         // [points][kGraphK]
+    DeviceBuffer<float> d_graph_radius;
     uint64_t graph_gen = ~uint64_t(0);
     BlockArchive arc;
 };
@@ -193,64 +236,75 @@ struct Ctx {
     int32_t origin[3] = {kW / 2, kH / 2, kD / 2};  // LocalMap() ctor (LocalMap.h:141-144)
     MapStore surf, edge;                           // psurf_pc_ / pedge_pc_ of every MapBlock
     // scratch shared by both stores (builds are sequential on the context stream)
-    uint64_t* d_keys = nullptr;                    // [max_map] sort keys (in)
-    uint64_t* d_keys_out = nullptr;                // [max_map]
-    uint32_t* d_vals = nullptr;                    // [max_map] ids (in)
-    uint32_t* d_vals_out = nullptr;                // [max_map]
-    void* d_cub_tmp = nullptr;
-    size_t cub_tmp_bytes = 0;
-    struct MapScratch* d_map_scratch = nullptr;    // device-side bookkeeping of a store change or a scan pre-filter (so_map.cu)
-    struct InsertInfo* h_map_info = nullptr;       // pinned read-back target of its InsertInfo
+    DeviceBuffer<uint64_t> d_keys;                 // [max_map] sort keys (in)
+    DeviceBuffer<uint64_t> d_keys_out;             // [max_map]
+    DeviceBuffer<uint32_t> d_vals;                 // [max_map] ids (in)
+    DeviceBuffer<uint32_t> d_vals_out;             // [max_map]
+    DeviceBuffer<unsigned char> d_cub_tmp;
+    DeviceBuffer<struct MapScratch> d_map_scratch; // device-side bookkeeping of a store change or a scan pre-filter (so_map.cu)
+    PinnedBuffer<struct InsertInfo> h_map_info;    // read-back target of its InsertInfo
 
     // ---- scans / correspondences / optimiser state -------------------------------------------------------------
     uint32_t max_batch = 1;
     size_t scan_cap = 0;                           // points over the whole batch
     size_t prefiltered_n = SIZE_MAX;               // points so_scan_prefilter left in d_scan_sorted (SIZE_MAX: none / overwritten since)
     RegisteredScan reg;                            // what d_scan (and und.d_time) hold for so_map_add_registered_scan
-    float4* d_scan = nullptr;                      // upload target for host scans (original order)
-    float4* d_scan_sorted = nullptr;               // cell-ordered copy the kernels read; w = original index
-    uint64_t* d_skeys = nullptr; uint64_t* d_skeys_out = nullptr;   // scan sort keys (scan id << 32 | cell)
-    uint32_t* d_svals = nullptr; uint32_t* d_svals_out = nullptr;
-    void* d_sort_tmp = nullptr; size_t sort_tmp_bytes = 0;
-    void* d_sort_tmp2 = nullptr;                   // second radix-sort scratch: scan ordering of the chunks that run on aux_stream
-    NnBuf nn{};
-    size_t queue_cap = 0, qcount_cap = 0;         // nn.queue / nn.qcount (allocated with the first neighbour graph a search uses)
-    uint32_t* d_offset = nullptr;
-    IcpState* d_state = nullptr;
-    IcpState* h_state = nullptr;                   // pinned
-    uint32_t* h_offset = nullptr;                  // pinned
-    uint32_t* h_eoffset = nullptr;                 // second half of the same allocation
+    DeviceBuffer<float4> d_scan;                   // upload target for host scans (original order)
+    DeviceBuffer<float4> d_scan_sorted;            // cell-ordered copy the kernels read; w = original index
+    DeviceBuffer<uint64_t> d_skeys, d_skeys_out;   // scan sort keys (scan id << 32 | cell)
+    DeviceBuffer<uint32_t> d_svals, d_svals_out;
+    DeviceBuffer<unsigned char> d_sort_tmp;
+    DeviceBuffer<unsigned char> d_sort_tmp2;       // second radix-sort scratch: scan ordering of the chunks that run on aux_stream
+    NnBuf nn{};                                    // views of the five buffers below
+    DeviceBuffer<uint32_t> d_nn_pos;
+    DeviceBuffer<float> d_nn_d5;
+    DeviceBuffer<unsigned char> d_nn_pre;
+    DeviceBuffer<uint32_t> d_nn_queue, d_nn_qcount;   // allocated with the first neighbour graph a search uses
+    DeviceBuffer<uint32_t> d_offset;
+    DeviceBuffer<IcpState> d_state;
+    PinnedBuffer<IcpState> h_state;
+    PinnedBuffer<uint32_t> h_offset;
+    uint32_t* h_eoffset = nullptr;                 // second half of h_offset
     bool eoffset_dirty = false;                    // d_eoffset holds non-zero entries from the last batch
-    double* d_partials = nullptr;
-    uint32_t* d_counters = nullptr;
-    int32_t* d_hist = nullptr;
-    CorrBuf corr{};
+    DeviceBuffer<double> d_partials;
+    DeviceBuffer<uint32_t> d_counters;
+    DeviceBuffer<int32_t> d_hist;
+    CorrBuf corr{};                                // views of the five buffers below
+    DeviceBuffer<double4> d_corr_nd;
+    DeviceBuffer<double> d_corr_w;
+    DeviceBuffer<uchar4> d_corr_flags;
+    DeviceBuffer<uint32_t> d_corr_nn;
+    DeviceBuffer<float> d_corr_nn_d2;
     // edge / line branch (single-scan so_register only)
     size_t edge_cap = 0; uint32_t edge_grid_cap = 0;
-    float4* d_escan = nullptr; uint32_t* d_eoffset = nullptr; EdgeBuf ebuf{};
+    DeviceBuffer<float4> d_escan;
+    DeviceBuffer<uint32_t> d_eoffset;
+    EdgeBuf ebuf{};                                // views of d_escan, d_eoffset and the five buffers below
+    DeviceBuffer<double4> d_ebuf_a, d_ebuf_b;
+    DeviceBuffer<uchar4> d_ebuf_flags;
+    DeviceBuffer<uint32_t> d_ebuf_nn, d_ebuf_selmask;
     uint32_t grid_x_cap = 0;
     double* d_pose_sink = nullptr; size_t sink_cap = 0, sink_cursor = 0;   // so_set_pose_sink: device rows the batch calls append to
-    uint32_t* d_inject = nullptr; size_t inject_cap = 0;   // so_register_injected: caller-supplied neighbour ids [iters][n][5]
-    void* h_stage = nullptr;                       // pinned staging for strided host clouds
-    size_t h_stage_bytes = 0;
+    DeviceBuffer<uint32_t> d_inject;               // so_register_injected: caller-supplied neighbour ids [iters][n][5]
+    PinnedBuffer<float4> h_stage;                  // staging for strided host clouds
     // so_register of a DECIMATED scan (max_surface_features < n): only the points shouldProcessPoint keeps go up before the
     // registration is launched; the whole cloud (what so_map_add_registered_scan inserts) follows on the copy stream while it runs
-    float4* d_dec = nullptr;                       // [kPrepareSmallCap] the kept points, index order, w = intensity
+    DeviceBuffer<float4> d_dec;                    // [kPrepareSmallCap] the kept points, index order, w = intensity
     std::vector<uint32_t> dec_idx;                 // kept indices for (dec_n, dec_mf): the list depends on nothing else
     uint32_t dec_n = 0; int32_t dec_mf = 0;
-    cudaEvent_t ev_dec = nullptr;                  // the deferred upload of the whole cloud has landed in d_scan
+    Event ev_dec;                                  // the deferred upload of the whole cloud has landed in d_scan
     struct { const void* src = nullptr; size_t n = 0, stride = 0, ioff = 0, stage_off = 0; } defer;      // pending whole-cloud upload (src == nullptr: none)
     bool no_dec_upload = false;                    // SO_NO_DEC_UPLOAD: A/B aid, always upload the whole cloud first
     int knn_graph_mode = 0;                        // SO_KNN_GRAPH: test / A/B aid; 0 = built by the rule, 1 (on) = built for every search call,
                                                    // -1 (off) = never used
-    uint32_t* d_graph_stats = nullptr;             // so_knn_graph_stats: [SO_MAX_ICP_ITERS][2] counters while on, else nullptr
+    DeviceBuffer<uint32_t> d_graph_stats;          // so_knn_graph_stats: [SO_MAX_ICP_ITERS][2] counters while on, else empty
 
     // ---- k-NN scratch -------------------------------------------------------------------------------------------
-    float4* d_q = nullptr; uint32_t* d_knn_idx = nullptr; float* d_knn_d2 = nullptr;
-    size_t q_cap = 0, knn_idx_cap = 0, knn_d2_cap = 0;
-    uint32_t* d_qkeys = nullptr; uint32_t* d_qkeys_out = nullptr; uint32_t* d_qvals = nullptr; uint32_t* d_qvals_out = nullptr;   // cell ordering of so_knn* queries
-    size_t qkeys_cap = 0, qkeys_out_cap = 0, qvals_cap = 0, qvals_out_cap = 0;
-    void* d_qsort_tmp = nullptr; size_t qsort_tmp_bytes = 0;
+    DeviceBuffer<float4> d_q;
+    DeviceBuffer<uint32_t> d_knn_idx;
+    DeviceBuffer<float> d_knn_d2;
+    DeviceBuffer<uint32_t> d_qkeys, d_qkeys_out, d_qvals, d_qvals_out;   // cell ordering of so_knn* queries
+    DeviceBuffer<unsigned char> d_qsort_tmp;
 
     // ---- CUDA graph cache for the ICP schedule (one entry per batch chunk shape) ------------------------------------
     // Everything a captured schedule bakes into its kernel arguments: the chunk shape and both MapViews (pointers, origin, grid,
@@ -280,65 +334,67 @@ struct Ctx {
     bool no_cond_graph = false;                    // conditional nodes unavailable (or SO_NO_COND_GRAPH): unrolled schedule
     cudaStream_t aux_stream = nullptr;             // odd chunks of a batch run here, concurrently with the even ones on `stream`:
                                                    // one chunk's serial optimiser steps and kernel tails hide under the other's wide kernels
-    cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
+    Event ev_fork, ev_join;
     cudaStream_t copy_stream = nullptr;            // H2D of batch chunks overlaps the previous chunk's kernels
-    cudaEvent_t ev_copy[17] = {};           // [0..15]: per upload chunk; [16]: guard
+    Event ev_copy[17];                             // [0..15]: per upload chunk; [16]: guard
 
     // ---- global localization (so_localize_global*): allocated on first use, grown on demand ---------------------------
     struct Bnb {
-        float4* d_pts = nullptr;                                           // [kRelocMaxPoints] score points
-        double* d_q = nullptr; size_t q_cap = 0;                           // one quaternion per yaw
-        uint32_t* d_pyr = nullptr; size_t pyr_words = 0;                   // every level of the clipped pyramid, back to back
-        uint32_t* d_scratch = nullptr; size_t scratch_words = 0;           // raster / dilation ping-pong partner of level 0
-        int4* d_off = nullptr; size_t off_cap = 0;                         // [nyaw][n_pts] voxel offsets of the score points
-        uint64_t* d_nodes = nullptr;                                       // level buffers: [kBnbRoot] root chunk + [4C] per finer level
-        uint64_t* d_unsorted = nullptr;                                    // [kBnbRoot] scored nodes before the sort
-        uint64_t* d_merge[2] = {nullptr, nullptr};                         // [kBnbMerge] running top-P + new leaves, sorted copy
-        void* d_tmp = nullptr; size_t tmp_bytes = 0;                       // radix-sort scratch
-        struct BnbCtl* d_ctl = nullptr; struct BnbCtl* h_ctl = nullptr;    // K*, level counts and statistics (pinned mirror)
-        uint32_t* d_bounds = nullptr;                                      // [6] map bounding box (ordered float bits)
-        cudaEvent_t ev[4] = {};                                            // build start, build end / search start, search end, spare
+        DeviceBuffer<float4> d_pts;                                        // [kRelocMaxPoints] score points
+        DeviceBuffer<double> d_q;                                          // one quaternion per yaw
+        DeviceBuffer<uint32_t> d_pyr;                                      // every level of the clipped pyramid, back to back
+        DeviceBuffer<uint32_t> d_scratch;                                  // raster / dilation ping-pong partner of level 0
+        DeviceBuffer<int4> d_off;                                          // [nyaw][n_pts] voxel offsets of the score points
+        DeviceBuffer<uint64_t> d_nodes;                                    // level buffers: [kBnbRoot] root chunk + [4C] per finer level
+        DeviceBuffer<uint64_t> d_unsorted;                                 // [kBnbRoot] scored nodes before the sort
+        DeviceBuffer<uint64_t> d_merge[2];                                 // [kBnbMerge] running top-P + new leaves, sorted copy
+        DeviceBuffer<unsigned char> d_tmp;                                 // radix-sort scratch
+        DeviceBuffer<struct BnbCtl> d_ctl;                                 // K*, level counts and statistics
+        PinnedBuffer<struct BnbCtl> h_ctl;                                 // their mirror
+        DeviceBuffer<uint32_t> d_bounds;                                   // [6] map bounding box (ordered float bits)
+        Event ev[4];                                                       // build start, build end / search start, search end, spare
     } bnb;
     // ---- within-scan motion compensation (so_register_undistort*): allocated on first use, grown on demand ------------
     struct Und {
-        UndistortParams* d_par = nullptr; size_t par_cap = 0;              // [max_batch] per-scan parameters of the registration
-        float* d_time = nullptr; size_t time_cap = 0;                      // per-point times of the scans in d_scan (upload order)
-        float4* d_hook = nullptr; size_t hook_cap = 0;                     // so_undistort_points: the cloud and its times
-        float* d_hook_time = nullptr; size_t hook_time_cap = 0;
-        float* d_etime = nullptr; size_t etime_cap = 0;                    // [edge_cap] times of the edge cloud in d_escan
-        float4* d_ewarp = nullptr; size_t ewarp_cap = 0;                   // [edge_cap] its pInit at the current pose (EdgeBuf::scan)
+        DeviceBuffer<UndistortParams> d_par;                               // [max_batch] per-scan parameters of the registration
+        DeviceBuffer<float> d_time;                                        // per-point times of the scans in d_scan (upload order)
+        DeviceBuffer<float4> d_hook;                                       // so_undistort_points: the cloud and its times
+        DeviceBuffer<float> d_hook_time;
+        DeviceBuffer<float> d_etime;                                       // [edge_cap] times of the edge cloud in d_escan
+        DeviceBuffer<float4> d_ewarp;                                      // [edge_cap] its pInit at the current pose (EdgeBuf::scan)
     } und;
     // ---- within-scan motion estimated by the registration (so_register_optimized*): allocated on first use ------------------
     struct Mot {
-        MotionState* d_st = nullptr; size_t st_cap = 0;                    // [max_batch] per-scan motion blocks
-        double* d_partials = nullptr; size_t partials_cap = 0;             // [max_batch][stride][kMotionAcc] per-CTA sums
+        DeviceBuffer<MotionState> d_st;                                    // [max_batch] per-scan motion blocks
+        DeviceBuffer<double> d_partials;                                   // [max_batch][stride][kMotionAcc] per-CTA sums
         uint32_t stride = 0;                                               // CTAs per scan the partials are laid out for
-        double* d_epartials = nullptr; size_t epartials_cap = 0;           // the edge clouds' per-CTA sums (so_register_optimized_edges)
+        DeviceBuffer<double> d_epartials;                                  // the edge clouds' per-CTA sums (so_register_optimized_edges)
     } mot;
     // ---- degeneracy-aware registration (so_register_degeneracy*, so_degeneracy_analysis): allocated on first use --------------
     struct Deg {
-        DegenState* d_st = nullptr; size_t st_cap = 0;                     // [max_batch] per-scan analysis and solve columns
+        DeviceBuffer<DegenState> d_st;                                     // [max_batch] per-scan analysis and solve columns
     } deg;
     // ---- edge extraction (so_scan_extract_edges): allocated on first use, grown on demand; never touches the scan buffers ----
     struct Feat {
-        unsigned char* d_raw = nullptr; size_t raw_cap = 0;                // the caller's records as given
-        size_t cap = 0;                                                    // points every per-point buffer below holds
-        uint64_t* d_keys[2] = {nullptr, nullptr};                          // sort keys in / out: (ring, time), then (ring, sector, curvature)
-        uint32_t* d_vals[2] = {nullptr, nullptr};
-        float4* d_pts = nullptr;                                           // valid points in (ring, time, index) order, w = time
-        uint8_t* d_excl = nullptr; uint8_t* d_reach = nullptr;             // excluded marks; neighbour-mark reach of each candidate
-        uint32_t* d_sel = nullptr; uint32_t* d_rank = nullptr;             // accepted flags and their exclusive scan
-        float4* d_out = nullptr; float4* d_vout = nullptr;                 // edge cloud; after the voxel filter
-        void* d_tmp = nullptr; size_t tmp_bytes = 0;                       // radix-sort / scan scratch
-        uint32_t* d_ring = nullptr;                                        // [65536] first position, [65536] end, [65536] ring list, [4] control
+        DeviceBuffer<unsigned char> d_raw;                                 // the caller's records as given
+        // the per-point buffers, each of d_pts.cap() points
+        DeviceBuffer<uint64_t> d_keys[2];                                  // sort keys in / out: (ring, time), then (ring, sector, curvature)
+        DeviceBuffer<uint32_t> d_vals[2];
+        DeviceBuffer<float4> d_pts;                                        // valid points in (ring, time, index) order, w = time
+        DeviceBuffer<uint8_t> d_excl, d_reach;                             // excluded marks; neighbour-mark reach of each candidate
+        DeviceBuffer<uint32_t> d_sel, d_rank;                              // accepted flags and their exclusive scan
+        DeviceBuffer<float4> d_out, d_vout;                                // edge cloud; after the voxel filter
+        DeviceBuffer<unsigned char> d_tmp;                                 // radix-sort / scan scratch
+        DeviceBuffer<uint32_t> d_ring;                                     // [65536] first position, [65536] end, [65536] ring list, [4] control
     } feat;
 
     // ---- free-space clearing (so_map_clear_free_space*, so_free.cu): allocated on first use, grown on demand ---------------------
     struct FreeSpace {
-        uint32_t* d_img = nullptr; size_t img_cap = 0;                     // range image: float bits of the minimum range per pixel
-        float4* d_pts = nullptr; size_t pts_cap = 0;                       // the host form's cloud
-        uint8_t* d_keep = nullptr; size_t keep_cap = 0;                    // [2][max_map_points] keep flags of the surf and edge windows
-        struct FreeCounters* d_cnt = nullptr; struct FreeCounters* h_cnt = nullptr;   // counters of one call (pinned mirror)
+        DeviceBuffer<uint32_t> d_img;                                      // range image: float bits of the minimum range per pixel
+        DeviceBuffer<float4> d_pts;                                        // the host form's cloud
+        DeviceBuffer<uint8_t> d_keep;                                      // [2][max_map_points] keep flags of the surf and edge windows
+        DeviceBuffer<struct FreeCounters> d_cnt;                           // counters of one call
+        PinnedBuffer<struct FreeCounters> h_cnt;                           // their mirror
     } fs;
 
     // ---- keyframes (so_keyframe_*, so_map_from_keyframes, so_register_keyframes): allocated on first use ---------------------------
@@ -350,7 +406,7 @@ struct Ctx {
     uint64_t bytes_h2d = 0, bytes_d2h = 0;         // host<->device bytes moved by registration / k-NN calls
     bool profiling = false;
     ProfileSlot prof[9];
-    cudaEvent_t ev0 = nullptr, ev1 = nullptr, evp0 = nullptr, evp1 = nullptr;
+    Event ev0, ev1, evp0, evp1;
 };
 
 // so_api.cu
@@ -372,10 +428,7 @@ inline float4 read_point(const unsigned char* p, size_t stride, size_t ioff) {  
     if (ioff + 4 <= stride) std::memcpy(&it, p + ioff, 4);
     return make_float4(xyz[0], xyz[1], xyz[2], it);
 }
-// so_global.cu
-void global_free(Ctx* c);                                   // the search buffers and events of Ctx::bnb
 // so_undistort.cu
-void undistort_free(Ctx* c);                                // the buffers of Ctx::und
 int undistort_reserve(Ctx* c, size_t n_points);             // Ctx::und's parameters (max_batch) and times (n_points)
 int undistort_edge_reserve(Ctx* c);                         // Ctx::und's edge times and warped edge cloud (edge_cap, fixed once allocated)
 int check_undistort(const so_undistort* u);                 // argument errors of one so_undistort
@@ -395,7 +448,6 @@ int undistort_tail(Ctx* c, float4* dst, const RegisteredScan& r, const double po
 // dst[0..r.n_edge) = the registered edge cloud r (APPROXIMATED): pInit at pose, in place
 int undistort_edge_tail(Ctx* c, float4* dst, const RegisteredScan& r, const double pose[7]);
 // so_motion.cu
-void motion_free(Ctx* c);                                   // the buffers of Ctx::mot
 int motion_reserve(Ctx* c, size_t n_points);                // Ctx::mot's blocks and partials (max_batch), Ctx::und's times (n_points)
 int check_motion(const so_motion* m, const so_icp_opts* o); // argument errors of one so_motion and the options it registers with
 MotionState make_state(const so_motion& m);
@@ -419,7 +471,6 @@ void launch_motion_solve(int phase, const BatchView& bv, const CorrBuf& cb, cons
 void launch_covariance12(IcpState* st, const MotionState* ms, cudaStream_t stream);
 // so_map.cu
 int map_alloc(Ctx* c);
-void map_free(Ctx* c);
 int map_add_points(Ctx* c, MapStore& ms, uint32_t n_new);   // ms.d_xyzi[n .. n+n_new) holds the new points: voxel-filter touched blocks, index
 int map_transform_tail(Ctx* c, MapStore& ms, uint32_t n_new, const double pose[7]);   // sensor-frame tail points -> world frame
 int scan_voxel_filter(Ctx* c, uint32_t n, float leaf, uint32_t* n_out);   // d_scan -> d_scan_sorted (VoxelGrid on a scan)
@@ -433,23 +484,18 @@ void free_space_defaults(so_free_space* o);
 int free_space_check(const so_free_space* o, int stores, const double pose[7]);   // SO_ERR_ARG cases of so_map_clear_free_space*
 int free_space_prepare(Ctx* c, int stores);                 // rebuild the selected stores that are dirty
 int free_space_reserve_points(Ctx* c, size_t n);            // Ctx::fs.d_pts for a host cloud of n points
-void free_space_free(Ctx* c);
 // The range image of d_pts[0..n_pts) (sensor frame at pose), then every selected store carved against it; the stores are built
 int free_space_clear(Ctx* c, int stores, const float4* d_pts, uint32_t n_pts, const double pose[7], const so_free_space& o,
                      so_free_space_result* out);
-// so_features.cu
-void features_free(Ctx* c);
 // so_api.cu: dst[0..n) = the registered scan (edges: its edge cloud) as the map inserts place it before the world transform
 int put_registered_scan(Ctx* c, bool edges, float4* dst, const double pose[7]);
 // so_keyframes.cu
-void keyframes_free(Ctx* c);
 // The surf clouds of src's keyframes ids[0..n) back to back on the device as registration input for dst, with their sizes: src's pool
 // in place when the ids are consecutive, else a gather into dst's scratch.  SO_ERR_ARG for an id src does not hold.
 int keyframe_scans(Ctx* dst, Ctx* src, const int32_t* ids, size_t n, const float4** scans, std::vector<uint32_t>* n_points);
-// so_loop.cu: the descriptor table at cap_frames keyframes (valid descriptors kept) into *desc / *norm, not yet the store's; NULLs
-// when there is no table.  Committed by the store after its pools; freed by loop_free
-int loop_table_alloc(const KeyframeStore& s, size_t cap_frames, float** desc, double** norm);
-void loop_free(Ctx* c);                                     // the scratch of loop detection in Ctx::kfs
+// so_loop.cu: the descriptor table at cap_frames keyframes (valid descriptors kept) into *desc / *norm, not yet the store's; left
+// empty when there is no table.  Moved into the store after its pools
+int loop_table_alloc(const KeyframeStore& s, size_t cap_frames, DeviceBuffer<float>* desc, DeviceBuffer<double>* norm);
 // so_map.cu: pts[0..n) at pose, in place, by k_transform_points (utils::TransformPoint: qrot in double, float store)
 void launch_transform(float4* pts, uint32_t n, const double pose[7], cudaStream_t st);
 // so_map.cu, so_map_from_keyframes in two steps so that two stores change together or not at all.  keyframe_map_filter: the map of the
@@ -463,7 +509,7 @@ struct KfBuild {
     std::vector<std::pair<uint64_t, GatherSeg>> arc;   // world key, filtered cloud -> archive pool
 };
 int keyframe_map_filter(Ctx* c, MapStore& ms, int store, const KfSeg* segs, uint32_t n_segs, uint32_t total, const float4* pool, KfBuild* b);
-int keyframe_map_commit(Ctx* c, MapStore& ms, int store, const KfBuild& b);                                 // the buffers of Ctx::feat
+int keyframe_map_commit(Ctx* c, MapStore& ms, int store, const KfBuild& b);
 // so_scan.cu
 struct DeskewParams {
     double start_time;                     // lidar_start_time

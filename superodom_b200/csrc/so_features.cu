@@ -200,42 +200,33 @@ __global__ void __launch_bounds__(256) k_edge_scatter(const float4* __restrict__
     if (sel[p]) out[rank[p]] = pts[p];
 }
 
-void free_point_buffers(Ctx::Feat& F) {
-    for (void** p : {(void**)&F.d_keys[0], (void**)&F.d_keys[1], (void**)&F.d_vals[0], (void**)&F.d_vals[1], (void**)&F.d_pts, (void**)&F.d_excl,
-                     (void**)&F.d_reach, (void**)&F.d_sel, (void**)&F.d_rank, (void**)&F.d_out, (void**)&F.d_vout, &F.d_tmp}) {
-        cudaFree(*p);
-        *p = nullptr;
-    }
-    F.cap = 0;
-    F.tmp_bytes = 0;
-}
-
-// Every buffer for n points of raw_bytes of records; a failed allocation leaves cap at 0, so the next call retries
+// Every buffer for n points of raw_bytes of records
 int features_reserve(Ctx* c, size_t n, size_t raw_bytes) {
     Ctx::Feat& F = c->feat;
-    int rc = grow_buffer(F.d_raw, F.raw_cap, raw_bytes);
+    int rc = F.d_raw.reserve(raw_bytes);
+    if (!rc) rc = F.d_ring.reserve(3 * size_t(kRings) + 4);
     if (rc) return rc;
-    if (!F.d_ring) SO_CUDA_TRY(cudaMalloc(&F.d_ring, (3 * size_t(kRings) + 4) * sizeof(uint32_t)));
-    if (n <= F.cap) return SO_OK;
-    free_point_buffers(F);
-    for (int k = 0; k < 2; ++k) {
-        SO_CUDA_TRY(cudaMalloc(&F.d_keys[k], n * sizeof(uint64_t)));
-        SO_CUDA_TRY(cudaMalloc(&F.d_vals[k], n * sizeof(uint32_t)));
+    if (n > F.d_pts.cap()) {                       // the per-point buffers grow together: every old one goes before the first new one
+        for (int k = 0; k < 2; ++k) { F.d_keys[k].reset(); F.d_vals[k].reset(); }
+        F.d_pts.reset(); F.d_excl.reset(); F.d_reach.reset(); F.d_sel.reset(); F.d_rank.reset(); F.d_out.reset(); F.d_vout.reset();
+        F.d_tmp.reset();
     }
-    SO_CUDA_TRY(cudaMalloc(&F.d_pts, n * sizeof(float4)));
-    SO_CUDA_TRY(cudaMalloc(&F.d_excl, n));
-    SO_CUDA_TRY(cudaMalloc(&F.d_reach, n));
-    SO_CUDA_TRY(cudaMalloc(&F.d_sel, n * sizeof(uint32_t)));
-    SO_CUDA_TRY(cudaMalloc(&F.d_rank, n * sizeof(uint32_t)));
-    SO_CUDA_TRY(cudaMalloc(&F.d_out, n * sizeof(float4)));
-    SO_CUDA_TRY(cudaMalloc(&F.d_vout, n * sizeof(float4)));
+    for (int k = 0; k < 2 && !rc; ++k) {
+        rc = F.d_keys[k].reserve(n);
+        if (!rc) rc = F.d_vals[k].reserve(n);
+    }
+    if (!rc) rc = F.d_pts.reserve(n);
+    if (!rc) rc = F.d_excl.reserve(n);
+    if (!rc) rc = F.d_reach.reserve(n);
+    if (!rc) rc = F.d_sel.reserve(n);
+    if (!rc) rc = F.d_rank.reserve(n);
+    if (!rc) rc = F.d_out.reserve(n);
+    if (!rc) rc = F.d_vout.reserve(n);
+    if (rc) return rc;
     size_t a = 0, b = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, a, F.d_keys[0], F.d_keys[1], F.d_vals[0], F.d_vals[1], int(n), 0, 64);
-    cub::DeviceScan::ExclusiveSum(nullptr, b, F.d_sel, F.d_rank, int(n));
-    F.tmp_bytes = std::max(a, b) + 256;
-    SO_CUDA_TRY(cudaMalloc(&F.d_tmp, F.tmp_bytes));
-    F.cap = n;
-    return SO_OK;
+    cub::DeviceRadixSort::SortPairs(nullptr, a, F.d_keys[0].get(), F.d_keys[1].get(), F.d_vals[0].get(), F.d_vals[1].get(), int(n), 0, 64);
+    cub::DeviceScan::ExclusiveSum(nullptr, b, F.d_sel.get(), F.d_rank.get(), int(n));
+    return F.d_tmp.reserve(std::max(a, b) + 256);
 }
 
 // records already in F.d_raw -> F.d_out[0..*n_out) (then F.d_vout with a voxel leaf); *out_dev = the cloud to download
@@ -249,16 +240,16 @@ int extract_edges(Ctx* c, uint32_t n, uint32_t stride, uint32_t toff, uint32_t r
     SO_CUDA_TRY(cudaMemsetAsync(ctl, 0, 4 * sizeof(uint32_t), st));
     if (aligned) k_edge_keys<true><<<grid, 256, 0, st>>>(F.d_raw, n, stride, toff, roff, min_r2, F.d_keys[0], F.d_vals[0]);
     else k_edge_keys<false><<<grid, 256, 0, st>>>(F.d_raw, n, stride, toff, roff, min_r2, F.d_keys[0], F.d_vals[0]);
-    size_t tmp = F.tmp_bytes;
-    SO_CUDA_TRY(cub::DeviceRadixSort::SortPairs(F.d_tmp, tmp, F.d_keys[0], F.d_keys[1], F.d_vals[0], F.d_vals[1], int(n), 0, 49, st));
+    size_t tmp = F.d_tmp.cap();
+    SO_CUDA_TRY(cub::DeviceRadixSort::SortPairs(F.d_tmp, tmp, F.d_keys[0].get(), F.d_keys[1].get(), F.d_vals[0].get(), F.d_vals[1].get(), int(n), 0, 49, st));
     if (aligned) k_edge_rings<true><<<grid, 256, 0, st>>>(F.d_raw, n, stride, toff, F.d_keys[1], F.d_vals[1], F.d_pts, F.d_ring, F.d_excl, F.d_sel);
     else k_edge_rings<false><<<grid, 256, 0, st>>>(F.d_raw, n, stride, toff, F.d_keys[1], F.d_vals[1], F.d_pts, F.d_ring, F.d_excl, F.d_sel);
     k_edge_curv<<<grid, 256, 0, st>>>(F.d_pts, F.d_keys[1], n, F.d_ring, o.edge_threshold, F.d_excl, F.d_reach, F.d_keys[0], F.d_vals[0]);
-    tmp = F.tmp_bytes;
-    SO_CUDA_TRY(cub::DeviceRadixSort::SortPairs(F.d_tmp, tmp, F.d_keys[0], F.d_keys[1], F.d_vals[0], F.d_vals[1], int(n), 0, kCandBits + 1, st));
+    tmp = F.d_tmp.cap();
+    SO_CUDA_TRY(cub::DeviceRadixSort::SortPairs(F.d_tmp, tmp, F.d_keys[0].get(), F.d_keys[1].get(), F.d_vals[0].get(), F.d_vals[1].get(), int(n), 0, kCandBits + 1, st));
     k_edge_walk<<<kWalkBlocks, kWalkThreads, 0, st>>>(F.d_keys[1], F.d_vals[1], n, F.d_ring, F.d_excl, F.d_reach, F.d_sel, o.max_per_sector);
-    tmp = F.tmp_bytes;
-    SO_CUDA_TRY(cub::DeviceScan::ExclusiveSum(F.d_tmp, tmp, F.d_sel, F.d_rank, int(n), st));
+    tmp = F.d_tmp.cap();
+    SO_CUDA_TRY(cub::DeviceScan::ExclusiveSum(F.d_tmp, tmp, F.d_sel.get(), F.d_rank.get(), int(n), st));
     k_edge_scatter<<<grid, 256, 0, st>>>(F.d_pts, F.d_sel, F.d_rank, n, F.d_out, ctl + 1);
     c->launches += 7;            // five kernels, two sorts and a scan counted one each; timed_launch_end counts the eighth
     uint32_t m = 0;
@@ -268,7 +259,7 @@ int extract_edges(Ctx* c, uint32_t n, uint32_t stride, uint32_t toff, uint32_t r
     *out_dev = F.d_out;
     *n_out = m;
     if (o.voxel_leaf > 0.f && m) {
-        const VoxelBufs vb{F.d_keys[0], F.d_keys[1], F.d_vals[0], F.d_vals[1], F.d_tmp, F.tmp_bytes};
+        const VoxelBufs vb{F.d_keys[0], F.d_keys[1], F.d_vals[0], F.d_vals[1], F.d_tmp, F.d_tmp.cap()};
         const int rc = cloud_voxel_filter(c, F.d_out, m, o.voxel_leaf, vb, F.d_vout, n_out);
         if (rc) return rc;
         *out_dev = F.d_vout;
@@ -277,14 +268,6 @@ int extract_edges(Ctx* c, uint32_t n, uint32_t stride, uint32_t toff, uint32_t r
 }
 
 }  // namespace
-
-void features_free(Ctx* c) {
-    Ctx::Feat& F = c->feat;
-    free_point_buffers(F);
-    cudaFree(F.d_raw);
-    cudaFree(F.d_ring);
-    F = Ctx::Feat{};
-}
 
 }  // namespace so
 

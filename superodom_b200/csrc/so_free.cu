@@ -148,12 +148,7 @@ int free_space_prepare(Ctx* c, int stores) {
     return SO_OK;
 }
 
-int free_space_reserve_points(Ctx* c, size_t n) { return grow_buffer(c->fs.d_pts, c->fs.pts_cap, std::max<size_t>(n, 1)); }
-
-void free_space_free(Ctx* c) {
-    cudaFree(c->fs.d_img); cudaFree(c->fs.d_pts); cudaFree(c->fs.d_keep); cudaFree(c->fs.d_cnt);
-    if (c->fs.h_cnt) cudaFreeHost(c->fs.h_cnt);
-}
+int free_space_reserve_points(Ctx* c, size_t n) { return c->fs.d_pts.reserve(std::max<size_t>(n, 1)); }
 
 int free_space_clear(Ctx* c, int stores, const float4* d_pts, uint32_t n_pts, const double pose[7], const so_free_space& o,
                      so_free_space_result* out) {
@@ -177,13 +172,11 @@ int free_space_clear(Ctx* c, int stores, const float4* d_pts, uint32_t n_pts, co
         for (int k = 0; k < 3; ++k) P.t[k] = pose[k];
     }
     const size_t M = c->cfg.max_map_points;
-    int rc = grow_buffer(c->fs.d_img, c->fs.img_cap, size_t(g.W) * g.H);
-    if (!rc) rc = grow_buffer(c->fs.d_keep, c->fs.keep_cap, 2 * M);
+    int rc = c->fs.d_img.reserve(size_t(g.W) * g.H);
+    if (!rc) rc = c->fs.d_keep.reserve(2 * M);
+    if (!rc) rc = c->fs.d_cnt.reserve(1);
+    if (!rc) rc = c->fs.h_cnt.reserve(1);
     if (rc) return rc;
-    if (!c->fs.d_cnt) {
-        SO_CUDA_TRY(cudaMalloc(&c->fs.d_cnt, sizeof(FreeCounters)));
-        SO_CUDA_TRY(cudaMallocHost(&c->fs.h_cnt, sizeof(FreeCounters)));
-    }
     MapStore* ms[2] = {&c->surf, &c->edge};
     timed_launch_begin(c);
     SO_CUDA_TRY(cudaMemsetAsync(c->fs.d_img, 0xFF, size_t(g.W) * g.H * sizeof(uint32_t), st));

@@ -163,8 +163,9 @@ SO_NO_FP_CONTRACT static void yaw_quaternions(const GlobalPlan& P, const double 
 // Upload the score points and yaw quaternions on the context stream (the buffers allocated or grown on demand)
 static int global_upload(Ctx* c, const GlobalScan& S) {
     Ctx::Bnb& R = c->bnb;
-    if (!R.d_pts) SO_CUDA_TRY(cudaMalloc(&R.d_pts, size_t(kRelocMaxPoints) * sizeof(float4)));
-    { int rc = grow_buffer(R.d_q, R.q_cap, S.q.size()); if (rc) return rc; }
+    int rc = R.d_pts.reserve(kRelocMaxPoints);
+    if (!rc) rc = R.d_q.reserve(S.q.size());
+    if (rc) return rc;
     cudaStream_t st = c->stream;
     if (!S.pts.empty()) SO_CUDA_TRY(cudaMemcpyAsync(R.d_pts, S.pts.data(), S.pts.size() * sizeof(float4), cudaMemcpyHostToDevice, st));
     SO_CUDA_TRY(cudaMemcpyAsync(R.d_q, S.q.data(), S.q.size() * sizeof(double), cudaMemcpyHostToDevice, st));
@@ -190,7 +191,7 @@ static int global_check_args(Ctx* c, const void* xyzi, size_t n, size_t stride, 
     int rc = global_plan(gopts, P, bnb);
     if (rc) return rc;
     if (n > c->cfg.max_scan_points) return fail(SO_ERR_CAPACITY, "scan larger than so_config.max_scan_points");
-    P->whole = P->o.whole_map == 1 && c->surf.arc.cap != 0;        // archive off: the window is the whole map
+    P->whole = P->o.whole_map == 1 && c->surf.arc.d_pool.cap() != 0;        // archive off: the window is the whole map
     return SO_OK;
 }
 
@@ -340,18 +341,17 @@ static int bnb_check_table(const GlobalPlan& P, const GlobalScan& S) {
 
 static int bnb_alloc(Ctx* c) {
     Ctx::Bnb& B = c->bnb;
-    if (B.d_nodes) return SO_OK;
-    for (auto& e : B.ev) SO_CUDA_TRY(cudaEventCreate(&e));
-    SO_CUDA_TRY(cudaMalloc(&B.d_nodes, (size_t(kBnbRoot) + size_t(kBnbLevels - 2) * 4 * kBnbBatch) * sizeof(uint64_t)));
-    SO_CUDA_TRY(cudaMalloc(&B.d_unsorted, size_t(std::max(kBnbRoot, 4 * kBnbBatch)) * sizeof(uint64_t)));
-    SO_CUDA_TRY(cudaMalloc(&B.d_merge[0], size_t(kBnbMerge) * sizeof(uint64_t)));
-    SO_CUDA_TRY(cudaMalloc(&B.d_merge[1], size_t(kBnbMerge) * sizeof(uint64_t)));
-    B.tmp_bytes = std::max(bnb_sort_bytes(kBnbMerge), bnb_sort_bytes(kBnbRoot)) + 256;
-    SO_CUDA_TRY(cudaMalloc(&B.d_tmp, B.tmp_bytes));
-    SO_CUDA_TRY(cudaMalloc(&B.d_ctl, sizeof(BnbCtl)));
-    SO_CUDA_TRY(cudaMallocHost(&B.h_ctl, sizeof(BnbCtl)));
-    SO_CUDA_TRY(cudaMalloc(&B.d_bounds, 6 * sizeof(uint32_t)));
-    return SO_OK;
+    int rc = SO_OK;
+    for (Event& e : B.ev) if (!rc && !e) rc = e.create();
+    if (!rc) rc = B.d_nodes.reserve(size_t(kBnbRoot) + size_t(kBnbLevels - 2) * 4 * kBnbBatch);
+    if (!rc) rc = B.d_unsorted.reserve(size_t(std::max(kBnbRoot, 4 * kBnbBatch)));
+    if (!rc) rc = B.d_merge[0].reserve(kBnbMerge);
+    if (!rc) rc = B.d_merge[1].reserve(kBnbMerge);
+    if (!rc) rc = B.d_tmp.reserve(std::max(bnb_sort_bytes(kBnbMerge), bnb_sort_bytes(kBnbRoot)) + 256);
+    if (!rc) rc = B.d_ctl.reserve(1);
+    if (!rc) rc = B.h_ctl.reserve(1);
+    if (!rc) rc = B.d_bounds.reserve(6);
+    return rc;
 }
 
 static float float_from_order(uint32_t o) {
@@ -435,10 +435,10 @@ static int bnb_build(Ctx* c, const GlobalPlan& P, const GlobalScan& S, RelocGrid
     uint64_t words = 0;
     { int rc = bnb_layout(P, S.lo, mlo, mhi, n_map, &p, &words); if (rc) return rc; }
     const uint64_t w0 = p.off[1];                                   // level 0 words
-    { int rc = grow_buffer(B.d_pyr, B.pyr_words, words); if (rc) return rc; }
-    { int rc = grow_buffer(B.d_scratch, B.scratch_words, w0); if (rc) return rc; }
+    { int rc = B.d_pyr.reserve(words); if (rc) return rc; }
+    { int rc = B.d_scratch.reserve(w0); if (rc) return rc; }
     const size_t n_off = std::max<size_t>(1, size_t(g.nyaw) * S.pts.size());
-    { int rc = grow_buffer(B.d_off, B.off_cap, n_off); if (rc) return rc; }
+    { int rc = B.d_off.reserve(n_off); if (rc) return rc; }
     { int rc = global_upload(c, S); if (rc) return rc; }
     timed_launch_begin(c);
     SO_CUDA_TRY(cudaMemsetAsync(B.d_scratch, 0, w0 * sizeof(uint32_t), st));
@@ -496,7 +496,7 @@ static int bnb_search(Ctx* c, const RelocGrid& g, const BnbPyramid& p, int n_pts
         if (L == 0) {                                               // every level drained: the next chunk of the root
             const uint32_t nr = uint32_t(std::min<uint64_t>(kBnbRoot, root_n - r0));
             launch_bnb_score(g, p, B.d_pyr, B.d_off, n_pts, lmax, nullptr, r0, nr, B.d_ctl, B.d_unsorted, st);
-            { int rc = bnb_sort(B.d_tmp, B.tmp_bytes, B.d_unsorted, B.d_nodes + t.base[lmax], nr, st); if (rc) return rc; }
+            { int rc = bnb_sort(B.d_tmp, B.d_tmp.cap(), B.d_unsorted, B.d_nodes + t.base[lmax], nr, st); if (rc) return rc; }
             r0 += nr;
             t.head[lmax] = 0; t.cnt[lmax] = nr;
         } else {
@@ -505,12 +505,12 @@ static int bnb_search(Ctx* c, const RelocGrid& g, const BnbPyramid& p, int n_pts
             t.head[L] += take;
             if (L == 1) {                                           // leaves: merge into the running top P
                 launch_bnb_score(g, p, B.d_pyr, B.d_off, n_pts, 0, parents, 0, 4 * take, B.d_ctl, B.d_merge[0] + n_keys, st);
-                { int rc = bnb_sort(B.d_tmp, B.tmp_bytes, B.d_merge[0], B.d_merge[1], n_keys + 4 * take, st); if (rc) return rc; }
+                { int rc = bnb_sort(B.d_tmp, B.d_tmp.cap(), B.d_merge[0], B.d_merge[1], n_keys + 4 * take, st); if (rc) return rc; }
                 SO_CUDA_TRY(cudaMemcpyAsync(B.d_merge[0], B.d_merge[1], n_keys * sizeof(uint64_t), cudaMemcpyDeviceToDevice, st));
                 SO_CUDA_TRY(cudaMemcpyAsync(&B.d_ctl->kstar, B.d_merge[1] + n_keys - 1, sizeof(uint64_t), cudaMemcpyDeviceToDevice, st));
             } else {
                 launch_bnb_score(g, p, B.d_pyr, B.d_off, n_pts, L - 1, parents, 0, 4 * take, B.d_ctl, B.d_unsorted, st);
-                { int rc = bnb_sort(B.d_tmp, B.tmp_bytes, B.d_unsorted, B.d_nodes + t.base[L - 1], 4 * take, st); if (rc) return rc; }
+                { int rc = bnb_sort(B.d_tmp, B.d_tmp.cap(), B.d_unsorted, B.d_nodes + t.base[L - 1], 4 * take, st); if (rc) return rc; }
                 t.head[L - 1] = 0; t.cnt[L - 1] = 4 * take;
             }
         }
@@ -557,14 +557,6 @@ static int bnb_run(Ctx* c, const GlobalPlan& P, const GlobalScan& S, std::vector
         cudaEventElapsedTime(&ms, c->bnb.ev[2], c->bnb.ev[3]); stats->time_search_ms = ms;
     }
     return SO_OK;
-}
-
-void global_free(Ctx* c) {
-    cudaFree(c->bnb.d_pts); cudaFree(c->bnb.d_q);
-    cudaFree(c->bnb.d_pyr); cudaFree(c->bnb.d_scratch); cudaFree(c->bnb.d_off); cudaFree(c->bnb.d_nodes); cudaFree(c->bnb.d_unsorted);
-    cudaFree(c->bnb.d_merge[0]); cudaFree(c->bnb.d_merge[1]); cudaFree(c->bnb.d_tmp); cudaFree(c->bnb.d_ctl); cudaFree(c->bnb.d_bounds);
-    if (c->bnb.h_ctl) cudaFreeHost(c->bnb.h_ctl);
-    for (auto& e : c->bnb.ev) if (e) cudaEventDestroy(e);
 }
 
 // ---------------------------------------------------------------------------------------------- entry points

@@ -8,16 +8,6 @@
 
 namespace so {
 
-void keyframes_free(Ctx* c) {
-    KeyframeStore& s = c->kf;
-    cudaFree(s.d_pool[0]); cudaFree(s.d_pool[1]); cudaFree(s.d_desc); cudaFree(s.d_desc_norm);
-    loop_free(c);
-    KeyframeScratch& k = c->kfs;
-    cudaFree(k.d_segs); cudaFree(k.d_raw); cudaFree(k.d_keys); cudaFree(k.d_keys_out); cudaFree(k.d_vals); cudaFree(k.d_vals_out);
-    cudaFree(k.d_out[0]); cudaFree(k.d_out[1]); cudaFree(k.d_blk); cudaFree(k.d_tmp); cudaFree(k.d_ctl);
-    if (k.h_ctl) cudaFreeHost(k.h_ctl);
-}
-
 static size_t held(const KeyframeStore& s, int store) { return s.off[store].empty() ? 0 : size_t(s.off[store].back()); }
 
 // Both pools and the frame table at once: new pools are allocated and filled before the old ones go, so a failure changes nothing
@@ -25,34 +15,30 @@ static int keyframes_reserve(Ctx* c, size_t cap_points, size_t cap_frames) {
     KeyframeStore& s = c->kf;
     SO_CUDA_TRY(cudaStreamSynchronize(c->stream));
     if (cap_points == 0 && cap_frames == 0) {
-        cudaFree(s.d_pool[0]); cudaFree(s.d_pool[1]); cudaFree(s.d_desc); cudaFree(s.d_desc_norm);
         s = KeyframeStore{};
         return SO_OK;
     }
     if (cap_frames < s.frames() || cap_points < held(s, 0) || cap_points < held(s, 1))
         return fail(SO_ERR_ARG, "so_keyframe_reserve: capacity below what the store holds");
-    float* desc = nullptr;
-    double* norm = nullptr;
-    if (cap_frames != s.desc_frames) { int rc = loop_table_alloc(s, cap_frames, &desc, &norm); if (rc) return rc; }
-    float4* pool[2] = {nullptr, nullptr};
+    DeviceBuffer<float> desc;
+    DeviceBuffer<double> norm;
+    if (cap_frames != s.cap_frames) { int rc = loop_table_alloc(s, cap_frames, &desc, &norm); if (rc) return rc; }
     if (cap_points != s.cap_points) {
+        DeviceBuffer<float4> pool[2];
         for (int k = 0; k < 2; ++k) {
-            if (cudaMalloc(&pool[k], std::max<size_t>(cap_points, 1) * sizeof(float4)) != cudaSuccess) {
+            if (pool[k].reserve(std::max<size_t>(cap_points, 1))) {
                 cudaGetLastError();
-                cudaFree(pool[0]); cudaFree(desc); cudaFree(norm);
                 return fail(SO_ERR_CUDA, "so_keyframe_reserve: cudaMalloc of a keyframe pool failed");
             }
-            if (held(s, k) && cudaMemcpy(pool[k], s.d_pool[k], held(s, k) * sizeof(float4), cudaMemcpyDeviceToDevice) != cudaSuccess) {
-                cudaFree(pool[0]); cudaFree(pool[1]); cudaFree(desc); cudaFree(norm);
+            if (held(s, k) && cudaMemcpy(pool[k], s.d_pool[k], held(s, k) * sizeof(float4), cudaMemcpyDeviceToDevice) != cudaSuccess)
                 return fail(SO_ERR_CUDA, "so_keyframe_reserve: copy of the keyframes failed");
-            }
         }
-        for (int k = 0; k < 2; ++k) { cudaFree(s.d_pool[k]); s.d_pool[k] = pool[k]; }
+        for (int k = 0; k < 2; ++k) s.d_pool[k] = std::move(pool[k]);
         s.cap_points = cap_points;
     }
     if (desc) {                                                        // the descriptor table follows the frame table
-        cudaFree(s.d_desc); cudaFree(s.d_desc_norm);
-        s.d_desc = desc; s.d_desc_norm = norm; s.desc_frames = cap_frames;
+        s.d_desc = std::move(desc);
+        s.d_desc_norm = std::move(norm);
     }
     for (int k = 0; k < 2; ++k) if (s.off[k].empty()) s.off[k].push_back(0);
     s.cap_frames = cap_frames;
@@ -83,7 +69,7 @@ int keyframe_scans(Ctx* dst, Ctx* src, const int32_t* ids, size_t n, const float
     SO_CUDA_TRY(cudaStreamSynchronize(src->stream));                   // the keyframes have landed in src's pool
     if (consecutive) { *scans = s.d_pool[0] + (n ? s.off[0][ids[0]] : 0); return SO_OK; }
     KeyframeScratch& k = dst->kfs;
-    rc = grow_buffer(k.d_raw, k.raw_cap, std::max<size_t>(total, 1));
+    rc = k.d_raw.reserve(std::max<size_t>(total, 1));
     if (rc) return rc;
     size_t at = 0;
     for (size_t i = 0; i < n; ++i) {
@@ -164,7 +150,7 @@ int so_keyframe_download(so_ctx* ctx, int32_t id, int store, const double pose7[
     const float4* src = s.d_pool[store] + first;
     if (pose7) {                                                       // k_transform_points, as the rebuild transforms it
         KeyframeScratch& k = c->kfs;
-        int rc = grow_buffer(k.d_raw, k.raw_cap, n);
+        int rc = k.d_raw.reserve(n);
         if (rc) return rc;
         SO_CUDA_TRY(cudaMemcpyAsync(k.d_raw, src, n * sizeof(float4), cudaMemcpyDeviceToDevice, c->stream));
         launch_transform(k.d_raw, uint32_t(n), pose7, c->stream);

@@ -188,27 +188,21 @@ static bool same_descriptor(const so_loop_opts& a, const so_loop_opts& b) {
     return a.rings == b.rings && a.sectors == b.sectors && a.max_range == b.max_range && a.height_offset == b.height_offset;
 }
 
-int loop_table_alloc(const KeyframeStore& s, size_t cap_frames, float** desc, double** norm) {
-    *desc = nullptr; *norm = nullptr;
+int loop_table_alloc(const KeyframeStore& s, size_t cap_frames, DeviceBuffer<float>* desc, DeviceBuffer<double>* norm) {
     if (!s.desc_opts.rings || !cap_frames) return SO_OK;
-    const size_t cells = cells_of(s.desc_opts), sec = size_t(s.desc_opts.sectors), keep = std::min(s.frames(), s.desc_frames);
-    if (cudaMalloc(desc, cap_frames * cells * sizeof(float)) != cudaSuccess || cudaMalloc(norm, cap_frames * sec * sizeof(double)) != cudaSuccess) {
+    const size_t cells = cells_of(s.desc_opts), sec = size_t(s.desc_opts.sectors), keep = s.frames();   // a table holds cap_frames >= frames
+    DeviceBuffer<float> d;
+    DeviceBuffer<double> m;
+    if (d.reserve(cap_frames * cells) || m.reserve(cap_frames * sec)) {
         cudaGetLastError();
-        cudaFree(*desc); *desc = nullptr; *norm = nullptr;
         return fail(SO_ERR_CUDA, "so_keyframe_reserve: cudaMalloc of the loop descriptor table failed");
     }
-    if (keep && (cudaMemcpy(*desc, s.d_desc, keep * cells * sizeof(float), cudaMemcpyDeviceToDevice) != cudaSuccess ||
-                 cudaMemcpy(*norm, s.d_desc_norm, keep * sec * sizeof(double), cudaMemcpyDeviceToDevice) != cudaSuccess)) {
-        cudaFree(*desc); cudaFree(*norm); *desc = nullptr; *norm = nullptr;
+    if (keep && (cudaMemcpy(d, s.d_desc, keep * cells * sizeof(float), cudaMemcpyDeviceToDevice) != cudaSuccess ||
+                 cudaMemcpy(m, s.d_desc_norm, keep * sec * sizeof(double), cudaMemcpyDeviceToDevice) != cudaSuccess))
         return fail(SO_ERR_CUDA, "so_keyframe_reserve: copy of the loop descriptors failed");
-    }
+    *desc = std::move(d);
+    *norm = std::move(m);
     return SO_OK;
-}
-
-void loop_free(Ctx* c) {
-    KeyframeScratch& k = c->kfs;
-    cudaFree(k.d_dsegs); cudaFree(k.d_queries); cudaFree(k.d_pairs); cudaFree(k.d_top);
-    for (cudaEvent_t e : k.ev_loop) if (e) cudaEventDestroy(e);
 }
 
 // Levelling matrix L = Rz(-psi) R of a pose (row-major): R from the normalised quaternion, cos / sin psi as R00 / h and R10 / h with
@@ -234,7 +228,7 @@ static LoopGrid grid_of(const so_loop_opts& o) {
 }
 
 static int loop_events(Ctx* c) {
-    for (cudaEvent_t& e : c->kfs.ev_loop) if (!e) SO_CUDA_TRY(cudaEventCreate(&e));
+    for (Event& e : c->kfs.ev_loop) if (!e) { int rc = e.create(); if (rc) return rc; }
     return SO_OK;
 }
 
@@ -249,12 +243,11 @@ static int loop_describe(Ctx* c, const int32_t* ids, size_t n, const so_loop_opt
         s.desc_ok.assign(s.desc_ok.size(), 0);
         if (!s.desc_opts.rings || s.desc_opts.rings != o.rings || s.desc_opts.sectors != o.sectors) {
             SO_CUDA_TRY(cudaStreamSynchronize(c->stream));
-            cudaFree(s.d_desc); cudaFree(s.d_desc_norm);
-            s.d_desc = nullptr; s.d_desc_norm = nullptr; s.desc_frames = 0;
+            s.d_desc.reset(); s.d_desc_norm.reset();                  // at the new size, so the old table goes first
             s.desc_opts = so_loop_opts{};                             // no table until both allocations succeed
-            SO_CUDA_TRY(cudaMalloc(&s.d_desc, s.cap_frames * cells * sizeof(float)));
-            SO_CUDA_TRY(cudaMalloc(&s.d_desc_norm, s.cap_frames * size_t(o.sectors) * sizeof(double)));
-            s.desc_frames = s.cap_frames;
+            int rc = s.d_desc.reserve(s.cap_frames * cells);
+            if (!rc) rc = s.d_desc_norm.reserve(s.cap_frames * size_t(o.sectors));
+            if (rc) return rc;
         }
         s.desc_opts = o;
     }
@@ -272,7 +265,7 @@ static int loop_describe(Ctx* c, const int32_t* ids, size_t n, const so_loop_opt
     if (segs.empty()) return SO_OK;
     for (const DescSeg& g : segs) s.desc_ok[g.id] = 0;                // valid only once the kernel has run
     KeyframeScratch& k = c->kfs;
-    int rc = grow_buffer(k.d_dsegs, k.dsegs_cap, segs.size());
+    int rc = k.d_dsegs.reserve(segs.size());
     if (!rc) rc = loop_events(c);
     if (rc) return rc;
     SO_CUDA_TRY(cudaMemcpyAsync(k.d_dsegs, segs.data(), segs.size() * sizeof(DescSeg), cudaMemcpyHostToDevice, c->stream));
@@ -297,9 +290,9 @@ static int loop_search(Ctx* c, const int32_t* queries, size_t n, const so_loop_o
     auto eligible = [&](int32_t q) { return size_t(std::max(q - excl, 0)); };
     size_t max_m = 0;
     for (size_t i = 0; i < n; ++i) max_m = std::max(max_m, eligible(queries[i]));
-    int rc = grow_buffer(ks.d_queries, ks.queries_cap, std::max<size_t>(n, 1));
-    if (!rc) rc = grow_buffer(ks.d_pairs, ks.pairs_cap, std::max(kLoopPairCap, std::max<size_t>(max_m, 1)));
-    if (!rc) rc = grow_buffer(ks.d_top, ks.top_cap, std::max<size_t>(n * size_t(k), 1));
+    int rc = ks.d_queries.reserve(std::max<size_t>(n, 1));
+    if (!rc) rc = ks.d_pairs.reserve(std::max(kLoopPairCap, std::max<size_t>(max_m, 1)));
+    if (!rc) rc = ks.d_top.reserve(std::max<size_t>(n * size_t(k), 1));
     if (!rc) rc = loop_events(c);
     if (rc) return rc;
     SO_CUDA_TRY(cudaMemcpyAsync(ks.d_queries, queries, n * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
@@ -310,7 +303,7 @@ static int loop_search(Ctx* c, const int32_t* queries, size_t n, const so_loop_o
         size_t b = a, stride = 0;
         while (b < n && b - a < 65535) {
             const size_t st = std::max(stride, std::max<size_t>(eligible(queries[b]), 1));
-            if ((b - a + 1) * st > ks.pairs_cap) break;
+            if ((b - a + 1) * st > ks.d_pairs.cap()) break;
             stride = st; ++b;
         }
         const uint32_t nq = uint32_t(b - a), tiles = uint32_t((stride + kLoopTile - 1) / kLoopTile);

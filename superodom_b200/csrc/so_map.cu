@@ -77,10 +77,11 @@ __device__ __forceinline__ int grid_block(const float4 p, int3 origin) {
 
 static int store_alloc(Ctx* c, MapStore& ms) {
     const size_t M = c->cfg.max_map_points;
-    SO_CUDA_TRY(cudaMalloc(&ms.d_xyzi, M * sizeof(float4)));
-    SO_CUDA_TRY(cudaMalloc(&ms.d_sorted, M * sizeof(float4)));
-    SO_CUDA_TRY(cudaMalloc(&ms.d_block_slot, kNumBlocks * sizeof(int32_t)));
-    SO_CUDA_TRY(cudaMalloc(&ms.d_block_count, kNumBlocks * sizeof(int32_t)));
+    int rc = ms.d_xyzi.reserve(M);
+    if (!rc) rc = ms.d_sorted.reserve(M);
+    if (!rc) rc = ms.d_block_slot.reserve(kNumBlocks);
+    if (!rc) rc = ms.d_block_count.reserve(kNumBlocks);
+    if (rc) return rc;
     SO_CUDA_TRY(cudaMemset(ms.d_block_slot, 0xFF, kNumBlocks * sizeof(int32_t)));
     SO_CUDA_TRY(cudaMemset(ms.d_block_count, 0, kNumBlocks * sizeof(int32_t)));
     ms.h_block_count.assign(kNumBlocks, 0);
@@ -94,31 +95,20 @@ int map_alloc(Ctx* c) {
     if (rc) return rc;
     rc = store_alloc(c, c->edge);
     if (rc) return rc;
-    SO_CUDA_TRY(cudaMalloc(&c->d_keys, M * sizeof(uint64_t)));
-    SO_CUDA_TRY(cudaMalloc(&c->d_keys_out, M * sizeof(uint64_t)));
-    SO_CUDA_TRY(cudaMalloc(&c->d_vals, M * sizeof(uint32_t)));
-    SO_CUDA_TRY(cudaMalloc(&c->d_vals_out, M * sizeof(uint32_t)));
+    rc = c->d_keys.reserve(M);
+    if (!rc) rc = c->d_keys_out.reserve(M);
+    if (!rc) rc = c->d_vals.reserve(M);
+    if (!rc) rc = c->d_vals_out.reserve(M);
+    if (rc) return rc;
     // cub temp: the 64-bit filter sort (the 32-bit cell sort needs less) and the scan of its voxel heads at full capacity;
     // reserve_cells grows it for the scan of the cell table
     size_t a = 0, b = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, a, c->d_keys, c->d_keys_out, c->d_vals, c->d_vals_out, int(M), 0, 64);
+    cub::DeviceRadixSort::SortPairs(nullptr, a, c->d_keys.get(), c->d_keys_out.get(), c->d_vals.get(), c->d_vals_out.get(), int(M), 0, 64);
     cub::DeviceScan::ExclusiveSum(nullptr, b, (uint32_t*)nullptr, (uint32_t*)nullptr, int(M));
-    c->cub_tmp_bytes = std::max(a, b) + 256;
-    SO_CUDA_TRY(cudaMalloc(&c->d_cub_tmp, c->cub_tmp_bytes));
-    SO_CUDA_TRY(cudaMalloc(&c->d_map_scratch, sizeof(MapScratch)));
-    SO_CUDA_TRY(cudaMallocHost(&c->h_map_info, sizeof(InsertInfo)));
-    return SO_OK;
-}
-
-void map_free(Ctx* c) {
-    for (MapStore* ms : {&c->surf, &c->edge}) {
-        cudaFree(ms->d_xyzi); cudaFree(ms->d_sorted); cudaFree(ms->d_block_slot); cudaFree(ms->d_block_count); cudaFree(ms->d_cell_start);
-        cudaFree(ms->arc.d_pool); cudaFree(ms->arc.d_segs);
-        cudaFree(ms->d_graph); cudaFree(ms->d_graph_radius);
-    }
-    cudaFree(c->d_keys); cudaFree(c->d_keys_out); cudaFree(c->d_vals); cudaFree(c->d_vals_out); cudaFree(c->d_cub_tmp);
-    cudaFree(c->d_map_scratch);
-    if (c->h_map_info) cudaFreeHost(c->h_map_info);
+    rc = c->d_cub_tmp.reserve(std::max(a, b) + 256);
+    if (!rc) rc = c->d_map_scratch.reserve(1);
+    if (!rc) rc = c->h_map_info.reserve(1);
+    return rc;
 }
 
 MapView map_view(const Ctx* c, const MapStore& ms) {
@@ -184,8 +174,8 @@ bool knn_graph_valid(const Ctx* c) {
 int knn_graph_prepare(Ctx* c, size_t queries) {
     MapStore& ms = c->surf;
     if (ms.dirty || knn_graph_valid(c) || !graph_build_due(c->knn_graph_mode, queries, ms.n)) return SO_OK;
-    int rc = grow_buffer(ms.d_graph, ms.graph_cap, size_t(ms.n) * kGraphK);
-    if (!rc) rc = grow_buffer(ms.d_graph_radius, ms.radius_cap, size_t(ms.n));
+    int rc = ms.d_graph.reserve(size_t(ms.n) * kGraphK);
+    if (!rc) rc = ms.d_graph_radius.reserve(ms.n);
     if (rc) return rc;
     k_knn_graph<<<(ms.n + kGraphThreads - 1) / kGraphThreads, kGraphThreads, 0, c->stream>>>(map_view(c, ms), ms.n, ms.d_graph, ms.d_graph_radius);
     c->launches++;
@@ -197,7 +187,7 @@ int knn_graph_prepare(Ctx* c, size_t queries) {
 MapView search_view(const Ctx* c) {
     MapView m = map_view(c, c->surf);
     if (knn_graph_valid(c)) {
-        m.graph = reinterpret_cast<const uint4*>(c->surf.d_graph);
+        m.graph = reinterpret_cast<const uint4*>(c->surf.d_graph.get());
         m.graph_radius = c->surf.d_graph_radius;
         m.graph_stats = c->d_graph_stats;
     }
@@ -206,27 +196,26 @@ MapView search_view(const Ctx* c) {
 
 int scan_sort_alloc(Ctx* c) {
     size_t need = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, need, c->d_skeys, c->d_skeys_out, c->d_svals, c->d_svals_out, int(c->scan_cap), 0, 64);
-    c->sort_tmp_bytes = need + 256;
-    SO_CUDA_TRY(cudaMalloc(&c->d_sort_tmp, c->sort_tmp_bytes));
-    SO_CUDA_TRY(cudaMalloc(&c->d_sort_tmp2, c->sort_tmp_bytes));
-    return SO_OK;
+    cub::DeviceRadixSort::SortPairs(nullptr, need, c->d_skeys.get(), c->d_skeys_out.get(), c->d_svals.get(), c->d_svals_out.get(), int(c->scan_cap), 0, 64);
+    int rc = c->d_sort_tmp.reserve(need + 256);
+    if (!rc) rc = c->d_sort_tmp2.reserve(need + 256);
+    return rc;
 }
 
 int query_sort_reserve(Ctx* c, size_t n) {
-    int rc = grow_buffer(c->d_qkeys, c->qkeys_cap, n);
-    if (!rc) rc = grow_buffer(c->d_qkeys_out, c->qkeys_out_cap, n);
-    if (!rc) rc = grow_buffer(c->d_qvals, c->qvals_cap, n);
-    if (!rc) rc = grow_buffer(c->d_qvals_out, c->qvals_out_cap, n);
+    int rc = c->d_qkeys.reserve(n);
+    if (!rc) rc = c->d_qkeys_out.reserve(n);
+    if (!rc) rc = c->d_qvals.reserve(n);
+    if (!rc) rc = c->d_qvals_out.reserve(n);
     if (rc) return rc;
     size_t need = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, need, c->d_qkeys, c->d_qkeys_out, c->d_qvals, c->d_qvals_out, int(n), 0, 32);
-    return grow_buffer(c->d_qsort_tmp, c->qsort_tmp_bytes, need + 256);
+    cub::DeviceRadixSort::SortPairs(nullptr, need, c->d_qkeys.get(), c->d_qkeys_out.get(), c->d_qvals.get(), c->d_qvals_out.get(), int(n), 0, 32);
+    return c->d_qsort_tmp.reserve(need + 256);
 }
 
 int query_sort(Ctx* c, size_t n) {
-    size_t tmp = c->qsort_tmp_bytes;
-    SO_CUDA_TRY(cub::DeviceRadixSort::SortPairs(c->d_qsort_tmp, tmp, c->d_qkeys, c->d_qkeys_out, c->d_qvals, c->d_qvals_out, int(n), 0, 32, c->stream));
+    size_t tmp = c->d_qsort_tmp.cap();
+    SO_CUDA_TRY(cub::DeviceRadixSort::SortPairs(c->d_qsort_tmp, tmp, c->d_qkeys.get(), c->d_qkeys_out.get(), c->d_qvals.get(), c->d_qvals_out.get(), int(n), 0, 32, c->stream));
     c->launches += 5;
     return SO_OK;
 }
@@ -234,13 +223,13 @@ int query_sort(Ctx* c, size_t n) {
 int scan_sort(Ctx* c, size_t first, size_t n, int n_scans, int cell_bits, bool key32, cudaStream_t st) {
     int bits = cell_bits;
     while ((1 << (bits - cell_bits)) < n_scans) ++bits;
-    size_t tmp = c->sort_tmp_bytes;
+    size_t tmp = c->d_sort_tmp.cap();
     void* scratch = st == c->aux_stream ? c->d_sort_tmp2 : c->d_sort_tmp;
     if (key32)
-        SO_CUDA_TRY(cub::DeviceRadixSort::SortPairs(scratch, tmp, reinterpret_cast<uint32_t*>(c->d_skeys) + first, reinterpret_cast<uint32_t*>(c->d_skeys_out) + first,
+        SO_CUDA_TRY(cub::DeviceRadixSort::SortPairs(scratch, tmp, reinterpret_cast<uint32_t*>(c->d_skeys.get()) + first, reinterpret_cast<uint32_t*>(c->d_skeys_out.get()) + first,
                                                     c->d_svals + first, c->d_svals_out + first, int(n), 0, bits, st));
     else
-        SO_CUDA_TRY(cub::DeviceRadixSort::SortPairs(scratch, tmp, c->d_skeys + first, c->d_skeys_out + first,
+        SO_CUDA_TRY(cub::DeviceRadixSort::SortPairs(scratch, tmp, c->d_skeys.get() + first, c->d_skeys_out.get() + first,
                                                     c->d_svals + first, c->d_svals_out + first, int(n), 0, bits, st));
     c->launches += 5;
     return SO_OK;
@@ -408,12 +397,12 @@ static int filter_stage(Ctx* c, MapStore& ms, uint32_t n_new) {
     const int vb = voxel_bits(inv_leaf);
     const int cls_shift = 13 + 3 * vb;
     k_insert_keys<<<(total + 255) / 256, 256, 0, st>>>(ms.d_xyzi, total, inv_leaf, origin, d_touched, vb, c->d_keys, c->d_vals);
-    size_t tmp = c->cub_tmp_bytes;
-    SO_CUDA_TRY(cub::DeviceRadixSort::SortPairs(c->d_cub_tmp, tmp, c->d_keys, c->d_keys_out, c->d_vals, c->d_vals_out, int(total),
+    size_t tmp = c->d_cub_tmp.cap();
+    SO_CUDA_TRY(cub::DeviceRadixSort::SortPairs(c->d_cub_tmp, tmp, c->d_keys.get(), c->d_keys_out.get(), c->d_vals.get(), c->d_vals_out.get(), int(total),
                                                 n_new ? 0 : cls_shift, cls_shift + 2, st));
     c->launches += 8;
     const int rc = voxel_reduce(c, ms.d_xyzi, c->d_keys_out, c->d_vals_out, total, uint64_t(1) << cls_shift, uint64_t(2) << cls_shift,
-                                reinterpret_cast<uint32_t*>(c->d_keys), c->d_cub_tmp, c->cub_tmp_bytes, ms.d_sorted);   // keys_in is free after the sort
+                                reinterpret_cast<uint32_t*>(c->d_keys.get()), c->d_cub_tmp, c->d_cub_tmp.cap(), ms.d_sorted);   // keys_in is free after the sort
     std::swap(ms.d_xyzi, ms.d_sorted);                                  // d_xyzi: the new cloud in id order; d_sorted: free for the new index
     return rc;
 }
@@ -492,13 +481,13 @@ static int reserve_cells(Ctx* c, MapStore& ms, size_t slots, size_t spare) {
         set_error("map spans too many 50 m blocks for the dense cell table (n_slots * nb^3 >= 2^31)");
         return SO_ERR_CAPACITY;
     }
-    if (slots * cells_per_slot + 1 <= ms.cell_cap) return SO_OK;
+    if (slots * cells_per_slot + 1 <= ms.d_cell_start.cap()) return SO_OK;
     SO_CUDA_TRY(cudaStreamSynchronize(c->stream));
-    int rc = grow_buffer(ms.d_cell_start, ms.cell_cap, std::min(slots + spare, max_slots) * cells_per_slot + 1);
+    int rc = ms.d_cell_start.reserve(std::min(slots + spare, max_slots) * cells_per_slot + 1);
     if (rc) return rc;
     size_t need = 0;
-    cub::DeviceScan::ExclusiveSum(nullptr, need, ms.d_cell_start, ms.d_cell_start, int(ms.cell_cap));
-    return grow_buffer(c->d_cub_tmp, c->cub_tmp_bytes, need + 256);
+    cub::DeviceScan::ExclusiveSum(nullptr, need, ms.d_cell_start.get(), ms.d_cell_start.get(), int(ms.d_cell_start.cap()));
+    return c->d_cub_tmp.reserve(need + 256);
 }
 
 // block counts and slots of d_xyzi[0..info->n_out); more than slot_cap slots raise info->error
@@ -521,14 +510,14 @@ static int index_cells(Ctx* c, MapStore& ms, uint32_t n_max, uint32_t slot_cap) 
     const uint32_t grid = (n_max + 255) / 256;
     const size_t cells_used = size_t(slot_cap) * ms.nb * ms.nb * ms.nb + 1;
     SO_CUDA_TRY(cudaMemsetAsync(ms.d_cell_start, 0, cells_used * sizeof(uint32_t), st));
-    uint32_t* keys32 = reinterpret_cast<uint32_t*>(c->d_keys);
-    uint32_t* keys32_out = reinterpret_cast<uint32_t*>(c->d_keys_out);
+    uint32_t* keys32 = reinterpret_cast<uint32_t*>(c->d_keys.get());
+    uint32_t* keys32_out = reinterpret_cast<uint32_t*>(c->d_keys_out.get());
     k_cell_keys<<<grid, 256, 0, st>>>(ms.d_xyzi, n_max, d_info, map_view(c, ms), keys32, c->d_vals, ms.d_cell_start);
-    size_t tmp = c->cub_tmp_bytes;
-    SO_CUDA_TRY(cub::DeviceRadixSort::SortPairs(c->d_cub_tmp, tmp, keys32, keys32_out, c->d_vals, c->d_vals_out, int(n_max), 0, 32, st));
+    size_t tmp = c->d_cub_tmp.cap();
+    SO_CUDA_TRY(cub::DeviceRadixSort::SortPairs(c->d_cub_tmp, tmp, keys32, keys32_out, c->d_vals.get(), c->d_vals_out.get(), int(n_max), 0, 32, st));
     k_gather<<<grid, 256, 0, st>>>(ms.d_xyzi, c->d_vals_out, n_max, d_info, ms.d_sorted);
-    tmp = c->cub_tmp_bytes;
-    SO_CUDA_TRY(cub::DeviceScan::ExclusiveSum(c->d_cub_tmp, tmp, ms.d_cell_start, ms.d_cell_start, int(cells_used), st));
+    tmp = c->d_cub_tmp.cap();
+    SO_CUDA_TRY(cub::DeviceScan::ExclusiveSum(c->d_cub_tmp, tmp, ms.d_cell_start.get(), ms.d_cell_start.get(), int(cells_used), st));
     SO_CUDA_TRY(cudaMemcpyAsync(h_info, d_info, sizeof(InsertInfo), cudaMemcpyDeviceToHost, st));
     SO_CUDA_TRY(cudaMemcpyAsync(ms.h_block_count.data(), ms.d_block_count, kNumBlocks * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
     SO_CUDA_TRY(cudaMemcpyAsync(ms.h_block_slot.data(), ms.d_block_slot, kNumBlocks * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
@@ -551,12 +540,12 @@ static int set_empty_index(Ctx* c, MapStore& ms);
 int map_compact(Ctx* c, MapStore& ms, const uint8_t* keep, uint32_t n_keep, uint32_t* d_num_selected) {
     cudaStream_t st = c->stream;
     size_t need = 0;
-    cub::DeviceSelect::Flagged(nullptr, need, ms.d_xyzi, keep, ms.d_sorted, d_num_selected, int(ms.n));
-    int rc = grow_buffer(c->d_cub_tmp, c->cub_tmp_bytes, need + 256);
+    cub::DeviceSelect::Flagged(nullptr, need, ms.d_xyzi.get(), keep, ms.d_sorted.get(), d_num_selected, int(ms.n));
+    int rc = c->d_cub_tmp.reserve(need + 256);
     if (rc) return rc;
     ms.dirty = true;
-    size_t tmp = c->cub_tmp_bytes;
-    SO_CUDA_TRY(cub::DeviceSelect::Flagged(c->d_cub_tmp, tmp, ms.d_xyzi, keep, ms.d_sorted, d_num_selected, int(ms.n), st));
+    size_t tmp = c->d_cub_tmp.cap();
+    SO_CUDA_TRY(cub::DeviceSelect::Flagged(c->d_cub_tmp, tmp, ms.d_xyzi.get(), keep, ms.d_sorted.get(), d_num_selected, int(ms.n), st));
     c->launches += 2;
     std::swap(ms.d_xyzi, ms.d_sorted);                                  // d_xyzi: the kept cloud in id order; d_sorted: free for the index
     const uint32_t slots = uint32_t(ms.n_slots);
@@ -590,7 +579,7 @@ int map_rebuild(Ctx* c, MapStore& ms) {
     cudaStream_t st = c->stream;
     ms.nb = map_cells_per_block(ms.res);
     ms.dirty = true;
-    if (ms.arc.cap) return map_rebuild_archive(c, ms);
+    if (ms.arc.d_pool) return map_rebuild_archive(c, ms);
     if (ms.n == 0) return set_empty_index(c, ms);
     const uint32_t n = ms.n;
     InsertInfo* h_info = c->h_map_info;
@@ -674,7 +663,7 @@ __global__ void k_seg_gather(const float4* __restrict__ src, float4* __restrict_
 
 static int seg_gather(Ctx* c, BlockArchive& a, const std::vector<GatherSeg>& segs, const float4* src, float4* dst) {
     if (segs.empty()) return SO_OK;
-    int rc = grow_buffer(a.d_segs, a.segs_cap, segs.size());
+    int rc = a.d_segs.reserve(segs.size());
     if (rc) return rc;
     SO_CUDA_TRY(cudaMemcpyAsync(a.d_segs, segs.data(), segs.size() * sizeof(GatherSeg), cudaMemcpyHostToDevice, c->stream));
     k_seg_gather<<<unsigned(segs.size()), 256, 0, c->stream>>>(src, dst, a.d_segs);
@@ -708,17 +697,16 @@ int archive_set_cap(Ctx* c, size_t cap) {
     MapStore* stores[2] = {&c->surf, &c->edge};
     SO_CUDA_TRY(cudaStreamSynchronize(c->stream));
     if (cap == 0) {
-        for (MapStore* ms : stores) { cudaFree(ms->arc.d_pool); cudaFree(ms->arc.d_segs); ms->arc = BlockArchive{}; }
+        for (MapStore* ms : stores) ms->arc = BlockArchive{};
         return SO_OK;
     }
     for (MapStore* ms : stores)
         if (cap < ms->arc.live) { set_error("so_map_archive: capacity below the points the archive holds"); return SO_ERR_CAPACITY; }
-    float4* pool[2] = {nullptr, nullptr};
+    DeviceBuffer<float4> pool[2];
     for (int k = 0; k < 2; ++k) {
-        if (cap == stores[k]->arc.cap) continue;
-        if (cudaMalloc(&pool[k], cap * sizeof(float4)) != cudaSuccess) {
+        if (cap == stores[k]->arc.d_pool.cap()) continue;
+        if (pool[k].reserve(cap)) {
             cudaGetLastError();
-            cudaFree(pool[0]);
             set_error("so_map_archive: cudaMalloc of the archive pool failed");
             return SO_ERR_CUDA;
         }
@@ -728,13 +716,13 @@ int archive_set_cap(Ctx* c, size_t cap) {
     int rc = SO_OK;
     for (int k = 0; k < 2 && !rc; ++k) if (pool[k]) rc = repack(c, stores[k]->arc, pool[k], &packed[k], &moved[k]);
     if (!rc && cudaStreamSynchronize(c->stream) != cudaSuccess) rc = SO_ERR_CUDA;
-    if (rc) { cudaFree(pool[0]); cudaFree(pool[1]); return rc; }          // both directories as they were
+    if (rc) return rc;                                                   // both directories as they were
     for (int k = 0; k < 2; ++k) {
         if (!pool[k]) continue;
         BlockArchive& a = stores[k]->arc;
         apply_moves(moved[k]);
-        cudaFree(a.d_pool);
-        a.d_pool = pool[k]; a.cap = cap; a.used = packed[k];
+        a.d_pool = std::move(pool[k]);
+        a.used = packed[k];
     }
     return SO_OK;
 }
@@ -752,7 +740,7 @@ int archive_load(Ctx* c, MapStore& ms, const float4* pts, size_t n) {
         else off.emplace_back(key, uint32_t(i));
     }
     if (win.size() > c->cfg.max_map_points) { set_error("map points inside the window exceed so_config.max_map_points"); return SO_ERR_CAPACITY; }
-    if (off.size() > a.cap) { set_error("map points outside the window exceed the block archive (so_map_archive)"); return SO_ERR_CAPACITY; }
+    if (off.size() > a.d_pool.cap()) { set_error("map points outside the window exceed the block archive (so_map_archive)"); return SO_ERR_CAPACITY; }
     std::stable_sort(off.begin(), off.end(), [](const auto& x, const auto& y) { return x.first < y.first; });
     std::vector<float4> arc(off.size());
     for (size_t i = 0; i < off.size(); ++i) arc[i] = pts[off[i].second];
@@ -781,7 +769,7 @@ int archive_segments(Ctx* c, MapStore& ms, uint32_t* n_segs, uint32_t* max_n) {
     *n_segs = uint32_t(segs.size());
     *max_n = m;
     if (segs.empty()) return SO_OK;
-    int rc = grow_buffer(a.d_segs, a.segs_cap, segs.size());
+    int rc = a.d_segs.reserve(segs.size());
     if (rc) return rc;
     SO_CUDA_TRY(cudaMemcpyAsync(a.d_segs, segs.data(), segs.size() * sizeof(GatherSeg), cudaMemcpyHostToDevice, c->stream));
     return SO_OK;
@@ -839,15 +827,15 @@ static int map_rebuild_archive(Ctx* c, MapStore& ms) {
         const uint32_t m = n - n_kept;
         uint32_t* d_runs = &c->d_map_scratch->runs;
         size_t need = 0;
-        cub::DeviceRunLengthEncode::Encode(nullptr, need, c->d_keys_out, c->d_keys, c->d_vals, d_runs, int(m));
-        int rc = grow_buffer(c->d_cub_tmp, c->cub_tmp_bytes, need + 256);
+        cub::DeviceRunLengthEncode::Encode(nullptr, need, c->d_keys_out.get(), c->d_keys.get(), c->d_vals.get(), d_runs, int(m));
+        int rc = c->d_cub_tmp.reserve(need + 256);
         if (rc) return rc;
         k_evict_keys<<<(n + 255) / 256, 256, 0, st>>>(ms.d_xyzi, n, origin, c->d_keys, c->d_vals);
-        size_t tmp = c->cub_tmp_bytes;
-        SO_CUDA_TRY(cub::DeviceRadixSort::SortPairs(c->d_cub_tmp, tmp, c->d_keys, c->d_keys_out, c->d_vals, c->d_vals_out, int(n), 0,
+        size_t tmp = c->d_cub_tmp.cap();
+        SO_CUDA_TRY(cub::DeviceRadixSort::SortPairs(c->d_cub_tmp, tmp, c->d_keys.get(), c->d_keys_out.get(), c->d_vals.get(), c->d_vals_out.get(), int(n), 0,
                                                     kEvictShift + 2, st));
-        tmp = c->cub_tmp_bytes;           // run keys and counts into the sort's inputs, free now
-        SO_CUDA_TRY(cub::DeviceRunLengthEncode::Encode(c->d_cub_tmp, tmp, c->d_keys_out + n_kept, c->d_keys, c->d_vals, d_runs, int(m), st));
+        tmp = c->d_cub_tmp.cap();           // run keys and counts into the sort's inputs, free now
+        SO_CUDA_TRY(cub::DeviceRunLengthEncode::Encode(c->d_cub_tmp, tmp, c->d_keys_out.get() + n_kept, c->d_keys.get(), c->d_vals.get(), d_runs, int(m), st));
         uint32_t runs = 0;
         SO_CUDA_TRY(cudaMemcpyAsync(&h_info->pad, d_runs, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
         SO_CUDA_TRY(cudaGetLastError());
@@ -865,12 +853,12 @@ static int map_rebuild_archive(Ctx* c, MapStore& ms) {
         set_error("restoring archived blocks would exceed so_config.max_map_points");
         return SO_ERR_CAPACITY;
     }
-    if (a.live - n_back + n_evict > a.cap) { set_error("block archive full: grow it with so_map_archive"); return SO_ERR_CAPACITY; }
+    if (a.live - n_back + n_evict > a.d_pool.cap()) { set_error("block archive full: grow it with so_map_archive"); return SO_ERR_CAPACITY; }
     n_slots += uint32_t(back.size());                                   // restored blocks are not in the window's cloud
     if (n_kept + n_back) { int rc = reserve_cells(c, ms, n_slots, n_slots / 4); if (rc) return rc; }
-    const bool compact = a.used + n_evict > a.cap;
-    float4* scratch = nullptr;
-    if (compact) SO_CUDA_TRY(cudaMalloc(&scratch, std::max<size_t>(a.live - n_back, 1) * sizeof(float4)));
+    const bool compact = a.used + n_evict > a.d_pool.cap();
+    DeviceBuffer<float4> scratch;
+    if (compact) { int rc = scratch.reserve(std::max<size_t>(a.live - n_back, 1)); if (rc) return rc; }
     // restore: the blocks' clouds behind the window's points, then out of the directory
     float4* dst = n_kept < n ? ms.d_sorted : ms.d_xyzi;
     std::vector<GatherSeg> segs;
@@ -886,7 +874,7 @@ static int map_rebuild_archive(Ctx* c, MapStore& ms) {
         if (!rc && packed && cudaMemcpyAsync(a.d_pool, scratch, packed * sizeof(float4), cudaMemcpyDeviceToDevice, st) != cudaSuccess) rc = SO_ERR_CUDA;
         if (!rc && cudaStreamSynchronize(st) != cudaSuccess) rc = SO_ERR_CUDA;
     }
-    cudaFree(scratch);
+    scratch.reset();
     if (rc) return rc;            // the directory and the store still describe what they held: nothing restored, nothing lost
     if (compact) { apply_moves(moved); a.used = packed; }
     for (const auto& it : back) a.dir.erase(it);
@@ -1011,7 +999,7 @@ int cloud_voxel_filter(Ctx* c, const float4* in, uint32_t n, float leaf, const V
 }
 
 int scan_voxel_filter(Ctx* c, uint32_t n, float leaf, uint32_t* n_out) {
-    const VoxelBufs b{c->d_skeys, c->d_skeys_out, c->d_svals, c->d_svals_out, c->d_sort_tmp, c->sort_tmp_bytes};
+    const VoxelBufs b{c->d_skeys, c->d_skeys_out, c->d_svals, c->d_svals_out, c->d_sort_tmp, c->d_sort_tmp.cap()};
     return cloud_voxel_filter(c, c->d_scan, n, leaf, b, c->d_scan_sorted, n_out);
 }
 
@@ -1082,27 +1070,25 @@ int keyframe_map_filter(Ctx* c, MapStore& ms, int store, const KfSeg* segs, uint
     KeyframeScratch& k = c->kfs;
     *b = KfBuild{};
     if (total == 0) return SO_OK;
-    const int archive_on = ms.arc.cap ? 1 : 0;
+    const int archive_on = ms.arc.d_pool ? 1 : 0;
     const int3 origin = make_int3(c->origin[0], c->origin[1], c->origin[2]);
-    int rc = grow_buffer(k.d_segs, k.segs_cap, n_segs);
-    if (!rc) rc = grow_buffer(k.d_raw, k.raw_cap, total);
-    if (!rc) rc = grow_buffer(k.d_keys, k.keys_cap, total);
-    if (!rc) rc = grow_buffer(k.d_keys_out, k.keys_out_cap, total);
-    if (!rc) rc = grow_buffer(k.d_vals, k.vals_cap, total);
-    if (!rc) rc = grow_buffer(k.d_vals_out, k.vals_out_cap, total);
-    if (!rc) rc = grow_buffer(k.d_out[store], k.out_cap[store], total);
-    if (!rc) rc = grow_buffer(k.d_blk, k.blk_cap, total);
-    if (!rc && !k.d_ctl) {
-        SO_CUDA_TRY(cudaMalloc(&k.d_ctl, 8 * sizeof(int32_t)));
-        SO_CUDA_TRY(cudaMallocHost(&k.h_ctl, 8 * sizeof(int32_t)));
-    }
+    int rc = k.d_segs.reserve(n_segs);
+    if (!rc) rc = k.d_raw.reserve(total);
+    if (!rc) rc = k.d_keys.reserve(total);
+    if (!rc) rc = k.d_keys_out.reserve(total);
+    if (!rc) rc = k.d_vals.reserve(total);
+    if (!rc) rc = k.d_vals_out.reserve(total);
+    if (!rc) rc = k.d_out[store].reserve(total);
+    if (!rc) rc = k.d_blk.reserve(total);
+    if (!rc) rc = k.d_ctl.reserve(8);
+    if (!rc) rc = k.h_ctl.reserve(8);
     if (rc) return rc;
     {
         size_t a = 0, s2 = 0, r = 0;
-        cub::DeviceRadixSort::SortPairs(nullptr, a, k.d_keys, k.d_keys_out, k.d_vals, k.d_vals_out, int(total), 0, 64);
-        cub::DeviceScan::ExclusiveSum(nullptr, s2, k.d_vals, k.d_vals, int(total));
-        cub::DeviceRunLengthEncode::Encode(nullptr, r, k.d_blk, k.d_vals, k.d_vals_out, k.d_ctl, int(total));
-        rc = grow_buffer(k.d_tmp, k.tmp_bytes, std::max({a, s2, r}) + 256);
+        cub::DeviceRadixSort::SortPairs(nullptr, a, k.d_keys.get(), k.d_keys_out.get(), k.d_vals.get(), k.d_vals_out.get(), int(total), 0, 64);
+        cub::DeviceScan::ExclusiveSum(nullptr, s2, k.d_vals.get(), k.d_vals.get(), int(total));
+        cub::DeviceRunLengthEncode::Encode(nullptr, r, k.d_blk.get(), k.d_vals.get(), k.d_vals_out.get(), k.d_ctl.get(), int(total));
+        rc = k.d_tmp.reserve(std::max({a, s2, r}) + 256);
         if (rc) return rc;
     }
     // the box of the kept world blocks (one read-back)
@@ -1130,11 +1116,11 @@ int keyframe_map_filter(Ctx* c, MapStore& ms, int store, const KfSeg* segs, uint
     }
     const KfBox box{{lo[0], lo[1], lo[2]}, uint32_t(nx), uint32_t(ny), 3 * vb + bb};
     k_kf_keys<<<grid, 256, 0, st>>>(k.d_raw, total, origin, archive_on, box, inv_leaf, vb, k.d_keys, k.d_vals);
-    size_t tmp = k.tmp_bytes;
-    SO_CUDA_TRY(cub::DeviceRadixSort::SortPairs(k.d_tmp, tmp, k.d_keys, k.d_keys_out, k.d_vals, k.d_vals_out, int(total), 0, box.kb + 1, st));
+    size_t tmp = k.d_tmp.cap();
+    SO_CUDA_TRY(cub::DeviceRadixSort::SortPairs(k.d_tmp, tmp, k.d_keys.get(), k.d_keys_out.get(), k.d_vals.get(), k.d_vals_out.get(), int(total), 0, box.kb + 1, st));
     c->launches += 6;
-    uint32_t* head = reinterpret_cast<uint32_t*>(k.d_keys);           // keys_in is free after the sort: 2 * total words
-    rc = voxel_reduce(c, k.d_raw, k.d_keys_out, k.d_vals_out, total, 0, uint64_t(1) << box.kb, head, k.d_tmp, k.tmp_bytes, k.d_out[store]);
+    uint32_t* head = reinterpret_cast<uint32_t*>(k.d_keys.get());           // keys_in is free after the sort: 2 * total words
+    rc = voxel_reduce(c, k.d_raw, k.d_keys_out, k.d_vals_out, total, 0, uint64_t(1) << box.kb, head, k.d_tmp, k.d_tmp.cap(), k.d_out[store]);
     if (rc) return rc;
     k_kf_voxel_blocks<<<grid, 256, 0, st>>>(k.d_keys_out, head, head + total, total, 3 * vb, k.d_blk);
     InsertInfo* h_info = c->h_map_info;
@@ -1145,8 +1131,8 @@ int keyframe_map_filter(Ctx* c, MapStore& ms, int store, const KfSeg* segs, uint
     // the runs of blocks in the filtered cloud: the block directory, the only thing the host reads
     uint32_t* run_blk = k.d_vals;                                      // free after the reduction
     uint32_t* run_n = k.d_vals_out;
-    tmp = k.tmp_bytes;
-    SO_CUDA_TRY(cub::DeviceRunLengthEncode::Encode(k.d_tmp, tmp, k.d_blk, run_blk, run_n, k.d_ctl + 6, int(n_out), st));
+    tmp = k.d_tmp.cap();
+    SO_CUDA_TRY(cub::DeviceRunLengthEncode::Encode(k.d_tmp, tmp, k.d_blk.get(), run_blk, run_n, k.d_ctl.get() + 6, int(n_out), st));
     SO_CUDA_TRY(cudaMemcpyAsync(k.h_ctl + 6, k.d_ctl + 6, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
     SO_CUDA_TRY(cudaStreamSynchronize(st));
     const uint32_t runs = uint32_t(k.h_ctl[6]);
@@ -1166,7 +1152,7 @@ int keyframe_map_filter(Ctx* c, MapStore& ms, int store, const KfSeg* segs, uint
     b->n_win_blocks = uint32_t(b->win.size());
     // every check before the first change
     if (n_win > c->cfg.max_map_points) { set_error("so_map_from_keyframes: the window's points exceed so_config.max_map_points"); return SO_ERR_CAPACITY; }
-    if (b->n_arc > ms.arc.cap) { set_error("so_map_from_keyframes: the blocks outside the window exceed the block archive (so_map_archive)"); return SO_ERR_CAPACITY; }
+    if (b->n_arc > ms.arc.d_pool.cap()) { set_error("so_map_from_keyframes: the blocks outside the window exceed the block archive (so_map_archive)"); return SO_ERR_CAPACITY; }
     const size_t cells_per_slot = size_t(map_cells_per_block(ms.res));
     if (b->n_win_blocks > (kMaxCells - 2) / (cells_per_slot * cells_per_slot * cells_per_slot)) {
         set_error("map spans too many 50 m blocks for the dense cell table (n_slots * nb^3 >= 2^31)");
@@ -1180,7 +1166,7 @@ int keyframe_map_commit(Ctx* c, MapStore& ms, int store, const KfBuild& b) {
     const float4* out = c->kfs.d_out[store];
     int rc = seg_gather(c, a, b.win, out, ms.d_xyzi);
     if (rc) return rc;
-    if (a.cap) {
+    if (a.d_pool) {
         std::vector<GatherSeg> segs;
         segs.reserve(b.arc.size());
         for (const auto& kv : b.arc) segs.push_back(kv.second);

@@ -747,7 +747,6 @@ int motion_edge_tail(Ctx* c, float4* dst, const RegisteredScan& r) {
     return SO_OK;
 }
 
-void motion_free(Ctx* c) { cudaFree(c->mot.d_st); cudaFree(c->mot.d_partials); cudaFree(c->mot.d_epartials); }
 
 // ------------------------------------------------------------------------------------------------------------------ host side
 int check_motion(const so_motion* m, const so_icp_opts* o) {
@@ -775,16 +774,16 @@ MotionState make_state(const so_motion& m) {
 
 int motion_reserve(Ctx* c, size_t n_points) {
     c->mot.stride = eval_grid(c->grid_x_cap * kThreads);
-    int rc = grow_buffer(c->mot.d_st, c->mot.st_cap, size_t(c->max_batch));
-    if (!rc) rc = grow_buffer(c->mot.d_partials, c->mot.partials_cap, size_t(c->max_batch) * c->mot.stride * kMotionAcc);
-    if (!rc) rc = grow_buffer(c->und.d_time, c->und.time_cap, std::max<size_t>(n_points, 1));
+    int rc = c->mot.d_st.reserve(c->max_batch);
+    if (!rc) rc = c->mot.d_partials.reserve(size_t(c->max_batch) * c->mot.stride * kMotionAcc);
+    if (!rc) rc = c->und.d_time.reserve(std::max<size_t>(n_points, 1));
     return rc;
 }
 
 // The edge cloud's partials (edge_slot: at most the edge capacity's CTAs + max_batch slots), sized once, so that a captured schedule's
 // pointer stays valid
 int motion_edge_reserve(Ctx* c) {
-    return grow_buffer(c->mot.d_epartials, c->mot.epartials_cap, (size_t(c->edge_grid_cap) + c->max_batch) * kMotionAcc);
+    return c->mot.d_epartials.reserve((size_t(c->edge_grid_cap) + c->max_batch) * kMotionAcc);
 }
 
 // so_motion_result from the registration's result and the motion block: pose_end = T * D with T = pose_opt

@@ -135,8 +135,8 @@ int scan_extract_uniform(Ctx* c, uint32_t n, uint32_t skip, float block_range, i
     const uint32_t n_cand = (n - 2) / skip + 1;                 // i = 1, 1+skip, ... < n
     const uint32_t grid = (n_cand + 255) / 256;
     k_uniform_flags<<<grid, 256, 0, st>>>(c->d_scan, n_cand, skip, block_range * block_range, int_abs, c->d_svals);
-    size_t tmp = c->sort_tmp_bytes;
-    SO_CUDA_TRY(cub::DeviceScan::ExclusiveSum(c->d_sort_tmp, tmp, c->d_svals, c->d_svals_out, int(n_cand), st));
+    size_t tmp = c->d_sort_tmp.cap();
+    SO_CUDA_TRY(cub::DeviceScan::ExclusiveSum(c->d_sort_tmp, tmp, c->d_svals.get(), c->d_svals_out.get(), int(n_cand), st));
     uint32_t last_flag = 0, last_rank = 0;
     SO_CUDA_TRY(cudaMemcpyAsync(&last_flag, c->d_svals + n_cand - 1, 4, cudaMemcpyDeviceToHost, st));
     SO_CUDA_TRY(cudaMemcpyAsync(&last_rank, c->d_svals_out + n_cand - 1, 4, cudaMemcpyDeviceToHost, st));

@@ -106,10 +106,6 @@ int undistort_edge_tail(Ctx* c, float4* dst, const RegisteredScan& r, const doub
     return SO_OK;
 }
 
-void undistort_free(Ctx* c) {
-    cudaFree(c->und.d_par); cudaFree(c->und.d_time); cudaFree(c->und.d_hook); cudaFree(c->und.d_hook_time);
-    cudaFree(c->und.d_etime); cudaFree(c->und.d_ewarp);
-}
 
 // ------------------------------------------------------------------------------------------------------------------ host side
 bool finite_pose(const double p[7]) {
@@ -151,15 +147,15 @@ int upload_times(Ctx* c, const void* src, size_t n, size_t stride, size_t toff, 
 }
 
 int undistort_reserve(Ctx* c, size_t n_points) {
-    int rc = grow_buffer(c->und.d_par, c->und.par_cap, size_t(c->max_batch));
-    if (!rc) rc = grow_buffer(c->und.d_time, c->und.time_cap, std::max<size_t>(n_points, 1));
+    int rc = c->und.d_par.reserve(c->max_batch);
+    if (!rc) rc = c->und.d_time.reserve(std::max<size_t>(n_points, 1));
     return rc;
 }
 
 // Sized to the edge capacity on first use and never regrown, so that a captured schedule's pointer to d_ewarp stays valid
 int undistort_edge_reserve(Ctx* c) {
-    int rc = grow_buffer(c->und.d_etime, c->und.etime_cap, std::max<size_t>(c->edge_cap, 1));
-    if (!rc) rc = grow_buffer(c->und.d_ewarp, c->und.ewarp_cap, std::max<size_t>(c->edge_cap, 1));
+    int rc = c->und.d_etime.reserve(std::max<size_t>(c->edge_cap, 1));
+    if (!rc) rc = c->und.d_ewarp.reserve(std::max<size_t>(c->edge_cap, 1));
     return rc;
 }
 
@@ -178,8 +174,8 @@ int so_undistort_points(so_ctx* ctx, const void* xyzi, size_t n, size_t stride, 
     if (n > c->scan_cap) return fail(SO_ERR_CAPACITY, "cloud larger than the context's scan capacity");
     SO_CUDA_TRY(cudaSetDevice(c->device));
     if (n == 0) return SO_OK;
-    rc = grow_buffer(c->und.d_hook, c->und.hook_cap, n);
-    if (!rc) rc = grow_buffer(c->und.d_hook_time, c->und.hook_time_cap, n);
+    rc = c->und.d_hook.reserve(n);
+    if (!rc) rc = c->und.d_hook_time.reserve(n);
     if (!rc) rc = upload_cloud(c, xyzi, n, stride, ioff, c->und.d_hook);
     if (!rc) rc = upload_times(c, xyzi, n, stride, toff, c->und.d_hook_time);
     if (rc) return rc;
