@@ -1143,7 +1143,7 @@ int keyframe_map_filter(Ctx* c, MapStore& ms, int store, const KfSeg* segs, uint
     c->launches += 3 + 5;
     uint64_t at = 0, n_win = 0;
     for (uint32_t r = 0; r < runs; ++r) {
-        const int w[3] = {int(hb[r] % uint32_t(nx)) + lo[0], int(hb[r] / uint32_t(nx) % uint32_t(ny)) + lo[1], int(hb[r] / uint32_t(nx * ny)) + lo[2]};
+        const int w[3] = {int(hb[r] % nx) + lo[0], int(hb[r] / nx % ny) + lo[1], int(hb[r] / (nx * ny)) + lo[2]};   // nx * ny may be 2^32
         if (archive::in_window(w, c->origin)) { b->win.push_back(GatherSeg{at, n_win, hn[r], 0}); n_win += hn[r]; }
         else { b->arc.emplace_back(archive::world_key(w[0], w[1], w[2]), GatherSeg{at, b->n_arc, hn[r], 0}); b->n_arc += hn[r]; }
         at += hn[r];

@@ -14,7 +14,8 @@ bin of a ring or sector edge (the azimuth seam included, whose two sides are sec
 the lower image and put into every cell it may fall in in the upper one.
 
 The distance and the search loop in the device's fixed order (dot over rings, cosines over ascending query columns), so they are
-compared bit for bit.
+compared bit for bit.  `search` takes one pair at a time; `search_many` gives the same rows with the arithmetic vectorised over
+[candidates, shifts] (rings and columns still summed one at a time, in order), fast enough for thousands of keyframes.
 """
 from __future__ import annotations
 
@@ -163,4 +164,66 @@ def search(descs, queries, k: int, exclude_recent: int):
         best = [(b, d, s, n, yaw_of(s, Ns)) for d, b, s, n in rows[:k]]
         best += [(-1, 1.0, 0, 0, 0.0)] * (k - len(best))
         out.append(best)
+    return out
+
+
+def _norms_all(A):
+    """norms() of every image of A [frames, rings, sectors] float64, squares summed in ring order."""
+    acc = np.zeros((A.shape[0], A.shape[2]))
+    for r in range(A.shape[1]):
+        acc = acc + A[:, r] * A[:, r]
+    return np.sqrt(acc)
+
+
+def _row(A, nrm, q, m, k, Ns, chunk_elems=1 << 22):
+    """search()'s row of query q against candidates 0 .. m-1, vectorised over [candidates, shifts] in the same order of operations."""
+    if m == 0:
+        return [(-1, 1.0, 0, 0, 0.0)] * k
+    from numpy.lib.stride_tricks import sliding_window_view
+    Nr = A.shape[1]
+    na = nrm[q]
+    dq, sq, nq = np.empty(m), np.empty(m, np.int64), np.empty(m, np.int64)
+    step = max(1, chunk_elems // (Ns * Ns))
+    for c0 in range(0, m, step):
+        # the candidate's columns twice over: [.., s, j] of a window view is column (j + s) mod sectors, without a copy
+        B2 = np.concatenate([A[c0:min(c0 + step, m)]] * 2, 2)[..., :2 * Ns - 1]
+        nb2 = np.concatenate([nrm[c0:min(c0 + step, m)]] * 2, 1)[:, :2 * Ns - 1]
+        c = len(B2)
+        W = sliding_window_view(B2, Ns, axis=2)                             # [candidate, ring, s, j]
+        dot = np.zeros((c, Ns, Ns))                                         # [candidate, s, j]
+        prod = np.empty_like(dot)
+        for r in range(Nr):
+            np.multiply(A[q, r][None, None, :], W[:, r], out=prod)
+            np.add(dot, prod, out=dot)
+        nbc = sliding_window_view(nb2, Ns, axis=1)
+        valid = (na[None, None, :] != 0) & (nbc != 0)
+        with np.errstate(invalid="ignore", divide="ignore"):
+            cos = np.where(valid, dot / np.where(valid, na[None, None, :] * nbc, 1.0), 0.0)
+        acc = np.zeros((c, Ns))
+        for j in range(Ns):
+            acc = acc + cos[:, :, j]
+        n = valid.sum(2)
+        with np.errstate(invalid="ignore", divide="ignore"):
+            d = np.where(n > 0, 1.0 - acc / np.maximum(n, 1).astype(np.float64), 1.0)
+        s = np.argmin(d, 1)                                                 # the lowest shift of a tie
+        at = np.arange(c)
+        dq[c0:c0 + c], sq[c0:c0 + c], nq[c0:c0 + c] = d[at, s], s, n[at, s]
+    ids = np.arange(m)
+    order = np.lexsort((ids, dq))[:k]
+    best = [(int(b), float(dq[b]), int(sq[b]), int(nq[b]), yaw_of(int(sq[b]), Ns)) for b in order]
+    return best + [(-1, 1.0, 0, 0, 0.0)] * (k - len(best))
+
+
+def search_many(descs, queries, k: int, exclude_recent: int):
+    """search() for many candidates and queries: the same rows, bit for bit, with each distinct query's row computed once."""
+    A = np.asarray(descs, np.float32).astype(np.float64)
+    nrm = _norms_all(A)
+    Ns = A.shape[2]
+    rows = {}
+    out = []
+    for q in queries:
+        q = int(q)
+        if q not in rows:
+            rows[q] = _row(A, nrm, q, max(q - int(exclude_recent), 0), k, Ns)
+        out.append(list(rows[q]))
     return out

@@ -131,3 +131,33 @@ def test_search_order_and_padding():
     assert [t[0] for t in full].index(0) + 1 == [t[0] for t in full].index(2)    # the duplicate follows its twin
     assert [t[0] for t in out[1]][2:] == [-1, -1]                    # query 3, exclude 1: ids 0, 1 eligible
     assert [t[0] for t in out[2]] == [-1] * 4                        # query 1: none
+
+
+def _bits(rows):
+    return [[(i, np.float64(d).tobytes(), s, n, np.float64(y).tobytes()) for i, d, s, n, y in row] for row in rows]
+
+
+@pytest.mark.parametrize("rings,sectors", [(1, 2), (1, 31), (3, 32), (2, 33), (1, 65), (64, 2), (64, 33), (5, 65)])
+def test_search_many_equals_search(rings, sectors):
+    """search_many == search bit for bit (distances and yaws compared as bytes) on random images with crafted members: duplicates,
+    images periodic in the sectors (tied shifts), an all-zero image, a single-column image, and every exclude / k edge."""
+    rng = np.random.default_rng([rings, sectors])
+    n = 13
+    descs = np.where(rng.random((n, rings, sectors)) < 0.6, rng.uniform(0, 6, (n, rings, sectors)), 0).astype(np.float32)
+    descs[4] = descs[1]                                              # duplicates
+    descs[9] = descs[1]
+    tile = rng.uniform(0, 3, (rings, 2 if sectors % 2 == 0 else 1)).astype(np.float32)
+    descs[6] = np.tile(tile, (1, sectors // tile.shape[1]))          # periodic: the shifts of each period tie
+    descs[7] = 0                                                    # empty: distance 1.0, n_pairs 0 against everything
+    descs[11] = 0
+    descs[11][:, sectors // 2] = 2.5                                 # one occupied column
+    descs[12] = np.roll(descs[3], sectors - 1, axis=1)               # a turned copy: the shift wraps
+    queries = [12, 0, 7, 9, 12, 4, 11, 6, 1]
+    for k, exclude in ((1, 0), (3, 2), (5, 0), (13, 0), (16, 4), (2, 12), (4, 13)):
+        want = LD.search(descs, queries, k, exclude)
+        got = LD.search_many(descs, queries, k, exclude)
+        assert _bits(got) == _bits(want), (k, exclude)
+    # a tiny chunk size: the candidates split over several vectorised chunks give the same row
+    A = descs.astype(np.float64)
+    nrm = LD._norms_all(A)
+    assert _bits([LD._row(A, nrm, 12, 12, 13, sectors, chunk_elems=1)]) == _bits(LD.search(descs, [12], 13, 0))
