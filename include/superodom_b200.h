@@ -181,8 +181,8 @@ int so_map_add_scan(so_ctx* ctx, const void* xyzi, size_t n, size_t stride_bytes
  * so_register_optimized and their prefiltered forms, so_localize_global*), which is still in device memory: the live loop
  * Localization() -> transformAndAddToMap() (LidarSlam.cpp:155-171) without uploading the scan a second time.  Fails with SO_ERR_ARG,
  * before any device work, when a call that reuses the scan buffers ran in between: so_scan_prefilter, so_scan_deskew,
- * so_scan_extract_uniform, so_correspond, so_correspond_seeded, so_register_injected, the host batches so_register_batch*, so_evaluate_optimized (not
- * so_register_batch_device, the k-NN, the other map calls, so_undistort_points or so_correspond_edge).  SO_OK and nothing inserted
+ * so_scan_extract_uniform, so_correspond, so_correspond_seeded, so_register_injected, the host batches so_register_batch*, so_evaluate_optimized,
+ * so_solve_optimized (not so_register_batch_device, the k-NN, the other map calls, so_undistort_points, so_correspond_edge or so_solve).  SO_OK and nothing inserted
  * before the first registration. */
 int so_map_add_registered_scan(so_ctx* ctx, const double pose[7]);
 /* ... and transformAndAddToMap(cloud, world_cloud, true) for the edge cloud. */
@@ -628,6 +628,28 @@ typedef struct {
 } so_solve_result;
 int so_solve(so_ctx* ctx, const so_solve_row* rows, const so_solve_problem* problems, size_t n_problems, const so_degeneracy* d,
              so_solve_result* out);
+/* Test hook: the same for the two-block solve of so_register_optimized (T and the motion D over 12 tangent columns), by its kernels
+ * (k_motion_eval + k_motion_step) launched as one ICP iteration of a registration of n_problems scans launches them, without the warp,
+ * the neighbour search and the plane fit.  times[i] is the time of row i (alpha = time / dt, 0 when not finite); n_rows * info_k sets
+ * the motion prior's rows.  The solve runs with max_icp_iters = 1, so it ends with the covariance: cov is T's 6x6 block of the 12x12
+ * pseudo-inverse.  An empty problem ends with termination 6 and SO_STATUS_NO_CORRESPONDENCES.  Argument errors (those of so_solve,
+ * those of so_register_optimized's so_motion, a NULL times with rows) come before any device work.  Replaces the state a preceding
+ * so_correspond* left for so_evaluate, the scan buffer so_ordered_scans reads, and the scan and times so_map_add_registered_scan
+ * inserts, which then refuses until the next registration. */
+typedef struct {
+    uint32_t n_rows;
+    int32_t lm_max_iterations; /* <= 0: 4; at most 16 */
+    double pose[7];            /* T at the start */
+    double motion[7];          /* D at the start (its quaternion normalised); the prior's measurement is m.motion_prior */
+    so_motion m;
+} so_solve_optimized_problem;
+typedef struct {
+    so_solve_result solve;     /* pose = T; radius, decrease factor and gmax of the 12-column loop */
+    double motion[7];          /* D */
+    double cov[36];            /* T's block of the covariance (so_icp_result.cov) */
+} so_solve_optimized_result;
+int so_solve_optimized(so_ctx* ctx, const so_solve_row* rows, const float* times, const so_solve_optimized_problem* problems,
+                       size_t n_problems, so_solve_optimized_result* out);
 
 /* Sharded-replay plumbing (BASELINE cfg4; SURVEY 8e "K8"): a caller-owned DEVICE buffer of cap_rows x 8 doubles.  Every following
  * so_register / so_register_batch* call appends one row per scan, starting at first_row and advancing: {pose_opt[7] (the

@@ -111,6 +111,8 @@ def lib():
     L.orc_evaluate.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     L.orc_solve.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_float, C.c_int, C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]
     L.orc_covariance.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_float, C.c_void_p]
+    L.orc_solve_optimized.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p,
+                                      C.c_double, C.c_void_p, C.c_void_p, C.c_float, C.c_int, C.c_void_p, C.c_void_p]
     L.orc_register.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p]
     L.orc_set_nn_trace.argtypes = [C.c_void_p, C.c_size_t, C.c_int]
     L.orc_register_full.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -279,6 +281,23 @@ def solve(corr: np.ndarray, pose7, plane_res, lm_max_iterations=4, pose_prior=No
     L.orc_solve(_p(corr), corr.shape[0], _p(pose), C.c_float(plane_res), lm_max_iterations, None if meas is None else _p(meas),
                 C.c_float(vcf), None if unc is None else _p(unc), _p(summ), _p(costs))
     return pose, dict(successful=int(summ[0]), unsuccessful=int(summ[1]), iterations=int(summ[2]), termination=int(summ[3]),
+                      initial_cost=costs[0], final_cost=costs[1], radius=costs[2], decrease_factor=costs[3], gmax=costs[4])
+
+
+def solve_optimized(P, tau, N, D, W, T7, motion7, dt, D0, info, plane_res, lm_max_iterations=4):
+    """The two-block solve of so_register_optimized on given plane rows {p, tau, n, d, w} from (T7, motion7): the restatement's
+    trust-region loop over 12 columns with the motion prior rows (measurement D0, multiplier sqrt(n * info_k)).
+    -> (T, D, summary dict as solve's)."""
+    L = lib()
+    f64 = lambda a: np.ascontiguousarray(a, dtype=np.float64)         # noqa: E731
+    P, N, D, W, D0, info = f64(P), f64(N), f64(D), f64(W), f64(D0), f64(info)
+    tau = np.ascontiguousarray(tau, dtype=np.float32)
+    T, M = np.array(T7, dtype=np.float64), np.array(motion7, dtype=np.float64)
+    summ = np.zeros(4, np.int32)
+    costs = np.zeros(5)
+    L.orc_solve_optimized(_p(P), _p(tau), _p(N), _p(D), _p(W), len(P), _p(T), _p(M), float(dt), _p(D0), _p(info), C.c_float(plane_res),
+                          lm_max_iterations, _p(summ), _p(costs))
+    return T, M, dict(successful=int(summ[0]), unsuccessful=int(summ[1]), iterations=int(summ[2]), termination=int(summ[3]),
                       initial_cost=costs[0], final_cost=costs[1], radius=costs[2], decrease_factor=costs[3], gmax=costs[4])
 
 

@@ -796,6 +796,8 @@ struct Evaluator {
     double a2;                          // Tukey a^2, a = double(sqrtf(3*planeRes)) (LidarSlam.cpp:271)
     // TukeyLoss::Evaluate (ceres 2.0.0 loss_function.cc) wrapped by ScaledLoss(w)
     inline void rho(double s, double w, double r[3]) const { rho_a(s, w, a2, r); }
+    size_t rows() const { return blocks.size() + 3 * edges.size() + (prior.on ? 6 : 0); }
+    bool empty() const { return blocks.empty() && edges.empty() && !prior.on; }
     static inline void rho_a(double s, double w, double a2, double r[3]) {
         if (s <= a2) { const double v = 1.0 - s / a2, v2 = v * v; r[0] = a2 / 6.0 * (1.0 - v2 * v); r[1] = 0.5 * v2; r[2] = -1.0 / a2 * v; }
         else { r[0] = a2 / 6.0; r[1] = 0.0; r[2] = 0.0; }
@@ -870,38 +872,43 @@ struct SolveSummary {
 //              7 non-finite cost at the start (the reference aborts)
 
 // ceres::Solve with options {max_num_iterations=4, DENSE_QR} (LidarSlam.cpp:230-240), everything else default:
-// TrustRegionMinimizer::Minimize + LevenbergMarquardtStrategy + TrustRegionStepEvaluator(monotonic).
-static SolveSummary ceres_solve(const Evaluator& E, double params[7], int max_num_iterations = 4) {
+// TrustRegionMinimizer::Minimize + LevenbergMarquardtStrategy + TrustRegionStepEvaluator(monotonic).  NC tangent columns: NC / 6 pose7
+// blocks, each with PoseLocalParameterization (Plus block by block; x_norm, the step norm and the gradient max-norm over all of them).
+// E: rows(), empty(), cost(x) and full(x, ...) with a column-major rows() x NC Jacobian.
+template <int NC, class Eval>
+static SolveSummary ceres_solve_t(const Eval& E, double* params, int max_num_iterations) {
+    constexpr int NX = NC / 6 * 7;
     SolveSummary S;
-    if (E.blocks.empty() && E.edges.empty() && !E.prior.on) { S.termination = 6; return S; }
-    const size_t n = E.blocks.size() + 3 * E.edges.size() + (E.prior.on ? 6 : 0);      // residual rows
+    if (E.empty()) { S.termination = 6; return S; }
+    const size_t n = E.rows();      // residual rows
     const double function_tolerance = 1e-6, gradient_tolerance = 1e-10, parameter_tolerance = 1e-8;
     const double min_relative_decrease = 1e-3, min_lm_diagonal = 1e-6, max_lm_diagonal = 1e32;
     const double max_radius = 1e16, min_radius = 1e-32;
     const int max_consecutive_invalid = 5;
-    double x[7]; std::memcpy(x, params, sizeof(x));
-    double x_norm = 0; for (int i = 0; i < 7; ++i) x_norm += x[i] * x[i]; x_norm = std::sqrt(x_norm);
-    double x_cost; std::vector<double> res, J; double g[6];
-    double scale[6];
+    double x[NX]; std::memcpy(x, params, sizeof(x));
+    double x_norm = 0; for (int i = 0; i < NX; ++i) x_norm += x[i] * x[i]; x_norm = std::sqrt(x_norm);
+    double x_cost; std::vector<double> res, J; double g[NC];
+    double scale[NC];
+    auto plus = [](const double* xx, const double* d, double* out) { for (int b = 0; b < NC / 6; ++b) pose_plus(xx + 7 * b, d + 6 * b, out + 7 * b); };
     auto grad_max_norm = [&](const double* xx, const double* gg) {
-        double neg[6]; for (int j = 0; j < 6; ++j) neg[j] = -gg[j];
-        double xp[7]; pose_plus(xx, neg, xp);
-        double m = 0; for (int i = 0; i < 7; ++i) m = std::max(m, std::fabs(xx[i] - xp[i]));
+        double neg[NC]; for (int j = 0; j < NC; ++j) neg[j] = -gg[j];
+        double xp[NX]; plus(xx, neg, xp);
+        double m = 0; for (int i = 0; i < NX; ++i) m = std::max(m, std::fabs(xx[i] - xp[i]));
         return m;
     };
-    auto scale_columns = [&]() { for (int j = 0; j < 6; ++j) { double* c = &J[size_t(j) * n]; for (size_t i = 0; i < n; ++i) c[i] *= scale[j]; } };
+    auto scale_columns = [&]() { for (int j = 0; j < NC; ++j) { double* c = &J[size_t(j) * n]; for (size_t i = 0; i < n; ++i) c[i] *= scale[j]; } };
     // IterationZero
     E.full(x, &x_cost, res, J, g);
     // a non-finite loss weight (ScaledLoss(TukeyLoss, w), w = NaN) makes the cost NaN: Ceres 2.0 CHECK-fails in the Corrector of that
     // residual block (corrector.cc: neither rho'' <= 0 nor rho' > 0 holds) and ends the process; reported as termination 7
     if (!std::isfinite(x_cost)) { S.termination = 7; S.initial_cost = S.final_cost = x_cost; return S; }
-    for (int j = 0; j < 6; ++j) { double s = 0; const double* c = &J[size_t(j) * n]; for (size_t i = 0; i < n; ++i) s += c[i] * c[i]; scale[j] = 1.0 / (1.0 + std::sqrt(s)); }
+    for (int j = 0; j < NC; ++j) { double s = 0; const double* c = &J[size_t(j) * n]; for (size_t i = 0; i < n; ++i) s += c[i] * c[i]; scale[j] = 1.0 / (1.0 + std::sqrt(s)); }
     scale_columns();
     double gmax = grad_max_norm(x, g);
     S.initial_cost = x_cost;
-    double radius = 1e4, decrease_factor = 2.0; bool reuse_diagonal = false; double diagonal[6];
+    double radius = 1e4, decrease_factor = 2.0; bool reuse_diagonal = false; double diagonal[NC];
     int iteration = 0, consecutive_invalid = 0; bool step_successful = false;
-    double best[7]; std::memcpy(best, x, sizeof(x));
+    double best[NX]; std::memcpy(best, x, sizeof(x));
     std::vector<double> Aaug, baug;
     for (;;) {
         // FinalizeIterationAndCheckIfMinimizerCanContinue
@@ -911,29 +918,29 @@ static SolveSummary ceres_solve(const Evaluator& E, double params[7], int max_nu
         if (radius <= min_radius) { S.termination = 4; break; }
         ++iteration; step_successful = false;
         // LevenbergMarquardtStrategy::ComputeStep
-        if (!reuse_diagonal) for (int j = 0; j < 6; ++j) { double s = 0; const double* c = &J[size_t(j) * n]; for (size_t i = 0; i < n; ++i) s += c[i] * c[i]; diagonal[j] = std::min(std::max(s, min_lm_diagonal), max_lm_diagonal); }
-        double lm[6]; for (int j = 0; j < 6; ++j) lm[j] = std::sqrt(diagonal[j] / radius);
-        const int m = int(n) + 6;
-        Aaug.assign(size_t(m) * 6, 0.0); baug.assign(m, 0.0);
-        for (int j = 0; j < 6; ++j) { std::memcpy(&Aaug[size_t(j) * m], &J[size_t(j) * n], n * sizeof(double)); Aaug[size_t(j) * m + n + j] = lm[j]; }
+        if (!reuse_diagonal) for (int j = 0; j < NC; ++j) { double s = 0; const double* c = &J[size_t(j) * n]; for (size_t i = 0; i < n; ++i) s += c[i] * c[i]; diagonal[j] = std::min(std::max(s, min_lm_diagonal), max_lm_diagonal); }
+        double lm[NC]; for (int j = 0; j < NC; ++j) lm[j] = std::sqrt(diagonal[j] / radius);
+        const int m = int(n) + NC;
+        Aaug.assign(size_t(m) * NC, 0.0); baug.assign(m, 0.0);
+        for (int j = 0; j < NC; ++j) { std::memcpy(&Aaug[size_t(j) * m], &J[size_t(j) * n], n * sizeof(double)); Aaug[size_t(j) * m + n + j] = lm[j]; }
         std::memcpy(baug.data(), res.data(), n * sizeof(double));
-        double y[6]; householder_ls(m, 6, Aaug.data(), baug.data(), y, nullptr);
-        bool finite = true; for (int j = 0; j < 6; ++j) finite = finite && std::isfinite(y[j]);
+        double y[NC]; householder_ls(m, NC, Aaug.data(), baug.data(), y, nullptr);
+        bool finite = true; for (int j = 0; j < NC; ++j) finite = finite && std::isfinite(y[j]);
         reuse_diagonal = true;
-        double step[6]; for (int j = 0; j < 6; ++j) step[j] = -y[j];
+        double step[NC]; for (int j = 0; j < NC; ++j) step[j] = -y[j];
         // model_cost_change = -(J step)'(f + J step / 2)
         double mcc = 0.0;
-        if (finite) for (size_t i = 0; i < n; ++i) { double mr = 0; for (int j = 0; j < 6; ++j) mr += J[size_t(j) * n + i] * step[j]; mcc -= mr * (res[i] + mr / 2.0); }
+        if (finite) for (size_t i = 0; i < n; ++i) { double mr = 0; for (int j = 0; j < NC; ++j) mr += J[size_t(j) * n + i] * step[j]; mcc -= mr * (res[i] + mr / 2.0); }
         if (!finite || !(mcc > 0.0)) {   // HandleInvalidStep
             if (++consecutive_invalid >= max_consecutive_invalid) { S.termination = 5; break; }
             radius *= 0.5; reuse_diagonal = true; continue;
         }
         consecutive_invalid = 0;
-        double delta[6]; for (int j = 0; j < 6; ++j) delta[j] = step[j] * scale[j];
-        double cand[7]; pose_plus(x, delta, cand);
+        double delta[NC]; for (int j = 0; j < NC; ++j) delta[j] = step[j] * scale[j];
+        double cand[NX]; plus(x, delta, cand);
         const double cand_cost = E.cost(cand);
         // ParameterToleranceReached
-        double sn = 0; for (int i = 0; i < 7; ++i) sn += (x[i] - cand[i]) * (x[i] - cand[i]); sn = std::sqrt(sn);
+        double sn = 0; for (int i = 0; i < NX; ++i) sn += (x[i] - cand[i]) * (x[i] - cand[i]); sn = std::sqrt(sn);
         if (sn <= parameter_tolerance * (x_norm + parameter_tolerance)) { S.termination = 2; break; }
         // FunctionToleranceReached
         const double cost_change = x_cost - cand_cost;
@@ -941,7 +948,7 @@ static SolveSummary ceres_solve(const Evaluator& E, double params[7], int max_nu
         const double relative_decrease = cost_change / mcc;       // monotonic TrustRegionStepEvaluator
         if (relative_decrease > min_relative_decrease) {          // HandleSuccessfulStep
             std::memcpy(x, cand, sizeof(x));
-            x_norm = 0; for (int i = 0; i < 7; ++i) x_norm += x[i] * x[i]; x_norm = std::sqrt(x_norm);
+            x_norm = 0; for (int i = 0; i < NX; ++i) x_norm += x[i] * x[i]; x_norm = std::sqrt(x_norm);
             E.full(x, &x_cost, res, J, g); scale_columns();
             gmax = grad_max_norm(x, g);
             step_successful = true;
@@ -958,6 +965,130 @@ static SolveSummary ceres_solve(const Evaluator& E, double params[7], int max_nu
     std::memcpy(params, best, sizeof(best));
     return S;
 }
+static SolveSummary ceres_solve(const Evaluator& E, double params[7], int max_num_iterations = 4) { return ceres_solve_t<6>(E, params, max_num_iterations); }
+
+// The two-block problem of so_register_optimized (DESIGN.md section 3), for ceres_solve_t<12>: pose7 blocks T (the pose at tau = 0)
+// and D (the motion over dt).  Plane row i, alpha_i = tau_i / dt (0 for a non-finite tau_i):
+//   u_i = qrot(slerp(identity, q_D, alpha_i), p_i) + alpha_i t_D,   r_i = n_i . (qrot(q_T, u_i) + t_T) + d_i
+// under ScaledLoss(TukeyLoss(a), w_i) through the Corrector, as Evaluator's plane rows; then SE3AbsolutatePoseFactor on D (measurement
+// D0, row k times sqrt(n_rows * info_k), no loss).  Columns: T's translation and rotation, D's translation and rotation under
+// PoseLocalParameterization.  D's rotation columns are the exact derivative: a right perturbation delta of q_D moves
+// Log(q_D) = phi by J_r(phi)^-1 delta, so slerp's exp(alpha phi) by J_r(alpha phi) alpha J_r(phi)^-1 delta, and the row is
+//   alpha (p x b)^T J_r(alpha phi) J_r(phi)^-1,   b = R(q_alpha)^T R(q_T)^T n,   phi on the shortest path,
+// with J_r(v) = I - (1 - cos th) / th^2 [v]x + (th - sin th) / th^3 [v]x^2 and J_r(v)^-1 = I + [v]x / 2 + (1 / th^2 - (1 + cos th) /
+// (2 th sin th)) [v]x^2 (th = |v|) built as 3x3 matrices, their coefficients' Taylor series to th^4 below th = 1e-2.
+struct MotionEvaluator {
+    struct Row { double p[3], n[3], d, w, alpha; };
+    std::vector<Row> planes;
+    PosePrior prior;                    // on D, on always; sqrt_info = sqrt(n_rows * info)
+    double a2;
+    size_t rows() const { return planes.size() + 6; }
+    bool empty() const { return planes.empty(); }     // no correspondences: the registration's termination 6
+
+    static void mat_coeffs(double th, double* c1, double* c2, double* c3) {
+        const double t2 = th * th;
+        if (th < 1e-2) {
+            *c1 = 0.5 - t2 / 24.0 + t2 * t2 / 720.0;
+            *c2 = 1.0 / 6.0 - t2 / 120.0 + t2 * t2 / 5040.0;
+            *c3 = 1.0 / 12.0 + t2 / 720.0 + t2 * t2 / 30240.0;
+        } else {
+            *c1 = (1.0 - std::cos(th)) / t2;
+            *c2 = (th - std::sin(th)) / (t2 * th);
+            *c3 = 1.0 / t2 - (1.0 + std::cos(th)) / (2.0 * th * std::sin(th));
+        }
+    }
+    // I + a [v]x + b [v]x^2, row-major
+    static void jmat(const double v[3], double a, double b, double M[9]) {
+        const double K[9] = {0, -v[2], v[1], v[2], 0, -v[0], -v[1], v[0], 0};
+        for (int i = 0; i < 3; ++i)
+            for (int j = 0; j < 3; ++j) {
+                double k2 = 0.0;
+                for (int k = 0; k < 3; ++k) k2 += K[i * 3 + k] * K[k * 3 + j];
+                M[i * 3 + j] = (i == j ? 1.0 : 0.0) + a * K[i * 3 + j] + b * k2;
+            }
+    }
+    struct Setup { Quat qT, qD; double R[9], tT[3], tD[3], phi[3], th, Jinv[9]; bool linear; double s_theta, theta; };
+    static Setup setup(const double* x) {
+        Setup S;
+        S.qT = Quat{x[3], x[4], x[5], x[6]};
+        qtoR(S.qT, S.R);
+        S.qD = qnormalized(Quat{x[10], x[11], x[12], x[13]});
+        for (int k = 0; k < 3; ++k) { S.tT[k] = x[k]; S.tD[k] = x[7 + k]; }
+        const double absd = std::fabs(S.qD.w);                 // Eigen's slerp(identity, q_D, .): dot = q_D.w
+        S.linear = absd >= 1.0 - std::numeric_limits<double>::epsilon();
+        S.theta = S.linear ? 0.0 : std::acos(absd);
+        S.s_theta = std::sin(S.theta);
+        const Quat q = S.qD.w < 0.0 ? Quat{-S.qD.x, -S.qD.y, -S.qD.z, -S.qD.w} : S.qD;
+        const double vn = std::sqrt(q.x * q.x + q.y * q.y + q.z * q.z);
+        S.th = 2.0 * std::atan2(vn, q.w);
+        const double f = vn > 0.0 ? S.th / vn : 0.0;
+        S.phi[0] = f * q.x; S.phi[1] = f * q.y; S.phi[2] = f * q.z;
+        double c1, c2, c3;
+        mat_coeffs(S.th, &c1, &c2, &c3);
+        jmat(S.phi, 0.5, c3, S.Jinv);
+        return S;
+    }
+    static Quat slerp_alpha(const Setup& S, double al) {
+        double s0, s1;
+        if (S.linear) { s0 = 1.0 - al; s1 = al; }
+        else { s0 = std::sin((1.0 - al) * S.theta) / S.s_theta; s1 = std::sin(al * S.theta) / S.s_theta; }
+        if (S.qD.w < 0.0) s1 = -s1;
+        return Quat{s1 * S.qD.x, s1 * S.qD.y, s1 * S.qD.z, s0 + s1 * S.qD.w};
+    }
+    // residual of one row, with u and q_alpha for the Jacobian
+    static double residual(const Setup& S, const Row& r, double u[3], Quat* qa) {
+        *qa = slerp_alpha(S, r.alpha);
+        qrot(*qa, r.p, u);
+        for (int k = 0; k < 3; ++k) u[k] += r.alpha * S.tD[k];
+        double pw[3];
+        qrot(S.qT, u, pw);
+        return r.n[0] * (pw[0] + S.tT[0]) + r.n[1] * (pw[1] + S.tT[1]) + r.n[2] * (pw[2] + S.tT[2]) + r.d;
+    }
+    double cost(const double* x) const {
+        const Setup S = setup(x);
+        double c = 0.0;
+        for (const Row& r : planes) { double u[3], rr[3]; Quat qa; const double e = residual(S, r, u, &qa); Evaluator::rho_a(e * e, r.w, a2, rr); c += 0.5 * rr[0]; }
+        double rp[6], Jp[36]; prior.eval(x + 7, rp, Jp);
+        for (int i = 0; i < 6; ++i) c += 0.5 * rp[i] * rp[i];
+        return c;
+    }
+    void full(const double* x, double* cost_out, std::vector<double>& res, std::vector<double>& J, double g[12]) const {
+        const size_t np = planes.size(), n = rows();
+        res.assign(n, 0.0); J.assign(n * 12, 0.0);
+        for (int j = 0; j < 12; ++j) g[j] = 0.0;
+        const Setup S = setup(x);
+        double c = 0.0;
+        for (size_t i = 0; i < np; ++i) {
+            const Row& r = planes[i];
+            double u[3]; Quat qa;
+            const double e = residual(S, r, u, &qa);
+            const double a[3] = {S.R[0] * r.n[0] + S.R[3] * r.n[1] + S.R[6] * r.n[2], S.R[1] * r.n[0] + S.R[4] * r.n[1] + S.R[7] * r.n[2],
+                                 S.R[2] * r.n[0] + S.R[5] * r.n[1] + S.R[8] * r.n[2]};                      // R(q_T)^T n
+            double b[3];
+            qrot(qconj(qa), a, b);
+            const double w[3] = {r.p[1] * b[2] - r.p[2] * b[1], r.p[2] * b[0] - r.p[0] * b[2], r.p[0] * b[1] - r.p[1] * b[0]};     // p x b
+            const double v[3] = {r.alpha * S.phi[0], r.alpha * S.phi[1], r.alpha * S.phi[2]};
+            double c1, c2, c3, Jr[9], M[9];
+            mat_coeffs(std::fabs(r.alpha) * S.th, &c1, &c2, &c3);
+            jmat(v, -c1, c2, Jr);
+            for (int k = 0; k < 3; ++k) for (int l = 0; l < 3; ++l) { double t = 0.0; for (int m = 0; m < 3; ++m) t += Jr[k * 3 + m] * S.Jinv[m * 3 + l]; M[k * 3 + l] = t; }
+            double row[12] = {r.n[0], r.n[1], r.n[2], u[1] * a[2] - u[2] * a[1], u[2] * a[0] - u[0] * a[2], u[0] * a[1] - u[1] * a[0],
+                              r.alpha * a[0], r.alpha * a[1], r.alpha * a[2], 0, 0, 0};
+            for (int l = 0; l < 3; ++l) row[9 + l] = r.alpha * (w[0] * M[l] + w[1] * M[3 + l] + w[2] * M[6 + l]);
+            double rr[3]; Evaluator::rho_a(e * e, r.w, a2, rr);
+            c += 0.5 * rr[0];
+            const double sc = std::sqrt(rr[1]);
+            res[i] = e * sc;
+            for (int j = 0; j < 12; ++j) { J[size_t(j) * n + i] = row[j] * sc; g[j] += row[j] * sc * res[i]; }
+        }
+        double rp[6], Jp[36]; prior.eval(x + 7, rp, Jp);
+        for (int i = 0; i < 6; ++i) {
+            res[np + i] = rp[i]; c += 0.5 * rp[i] * rp[i];
+            for (int j = 0; j < 6; ++j) { J[size_t(6 + j) * n + np + i] = Jp[i * 6 + j]; g[6 + j] += Jp[i * 6 + j] * rp[i]; }
+        }
+        *cost_out = c;
+    }
+};
 
 // ceres::Covariance{apply_loss_function, DENSE_SVD, null_space_rank=-1} in tangent space (LidarSlam.cpp:854-871;
 // covariance_impl.cc ComputeCovarianceValuesUsingDenseSVD): V diag(1/s^2) V^T with s_i/s_0 < sqrt(1e-14) truncated.
@@ -1219,6 +1350,34 @@ int orc_solve(const orc_corr* corr, size_t n, double pose[7], float plane_res, i
     for (size_t i = 0; i < n; ++i) if (corr[i].status == orc::SUCCESS) E.blocks.push_back(&corr[i]);
     if (prior_meas) orc::set_pose_prior(E.prior, prior_meas, int(E.blocks.size()), visual_confidence_factor, prior_uncertainty);
     orc::SolveSummary S = orc::ceres_solve(E, pose, lm_max_iterations);
+    summary[0] = S.num_successful_steps; summary[1] = S.num_unsuccessful_steps; summary[2] = S.iterations; summary[3] = S.termination;
+    costs[0] = S.initial_cost; costs[1] = S.final_cost; costs[2] = S.radius; costs[3] = S.decrease_factor; costs[4] = S.gmax;
+    return 0;
+}
+
+// The two-block solve of so_register_optimized (MotionEvaluator) on n given rows {p, tau, n, d, w} from T and D (D's quaternion normalised
+// first); T and D are overwritten with the result.  summary and costs as orc_solve.
+int orc_solve_optimized(const double* p, const float* tau, const double* nrm, const double* d, const double* w, size_t n, double T[7],
+                        double D[7], double dt, const double D0[7], const double info[6], float plane_res, int lm_max_iterations,
+                        int32_t summary[4], double costs[5]) {
+    orc::MotionEvaluator E; const double a = double(std::sqrt(3 * plane_res)); E.a2 = a * a;
+    for (size_t i = 0; i < n; ++i) {
+        orc::MotionEvaluator::Row r;
+        for (int k = 0; k < 3; ++k) { r.p[k] = p[3 * i + k]; r.n[k] = nrm[3 * i + k]; }
+        r.d = d[i]; r.w = w[i];
+        r.alpha = std::isfinite(tau[i]) ? double(tau[i]) / dt : 0.0;
+        E.planes.push_back(r);
+    }
+    E.prior.on = true;
+    std::memcpy(E.prior.meas, D0, sizeof(E.prior.meas));
+    for (int k = 0; k < 6; ++k) E.prior.sqrt_info[k] = std::sqrt(double(n) * info[k]);
+    double x[14];
+    std::memcpy(x, T, 7 * sizeof(double));
+    const double qn = std::sqrt(D[3] * D[3] + D[4] * D[4] + D[5] * D[5] + D[6] * D[6]);
+    for (int k = 0; k < 7; ++k) x[7 + k] = k < 3 ? D[k] : D[k] / qn;
+    orc::SolveSummary S = orc::ceres_solve_t<12>(E, x, lm_max_iterations);
+    std::memcpy(T, x, 7 * sizeof(double));
+    std::memcpy(D, x + 7, 7 * sizeof(double));
     summary[0] = S.num_successful_steps; summary[1] = S.num_unsuccessful_steps; summary[2] = S.iterations; summary[3] = S.termination;
     costs[0] = S.initial_cost; costs[1] = S.final_cost; costs[2] = S.radius; costs[3] = S.decrease_factor; costs[4] = S.gmax;
     return 0;

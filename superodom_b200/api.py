@@ -24,7 +24,7 @@ EXPORTS = [
     "so_free_space_defaults", "so_map_clear_free_space", "so_map_clear_free_space_registered",
     "so_scan_prefilter", "so_scan_deskew", "so_scan_extract_uniform", "so_scan_extract_edges", "so_register", "so_register_prefiltered", "so_register_injected", "so_set_pose_sink", "so_register_batch", "so_register_batch_edges", "so_register_batch_device",
     "so_register_undistort", "so_register_undistort_edges", "so_register_prefiltered_undistort", "so_register_batch_undistort", "so_undistort_points", "so_register_optimized", "so_register_optimized_edges", "so_register_prefiltered_optimized", "so_register_batch_optimized", "so_evaluate_optimized", "so_evaluate_optimized_edges", "so_correspond", "so_correspond_seeded", "so_ordered_scans", "so_correspond_edge", "so_evaluate", "so_covariance",
-    "so_register_degeneracy", "so_register_batch_degeneracy", "so_degeneracy_analysis", "so_solve",
+    "so_register_degeneracy", "so_register_batch_degeneracy", "so_degeneracy_analysis", "so_solve", "so_solve_optimized",
     "so_knn", "so_knn_device", "so_sampling_indices", "so_localize_global", "so_localize_scores", "so_localize_global_size", "so_localize_global_bnb", "so_localize_bnb_keys", "so_localize_bnb_bounds", "so_map_bounds", "so_map_bounds_all", "so_kernel_launches", "so_bytes_copied", "so_build_flags", "so_profile_enable", "so_profile_get",
     "so_knn_graph", "so_knn_graph_stats",
     "so_keyframe_reserve", "so_keyframe_add_registered", "so_keyframe_info", "so_keyframe_poses", "so_keyframe_download", "so_map_from_keyframes",
@@ -220,6 +220,10 @@ SOLVE_RESULT_DTYPE = np.dtype([("pose", "<f8", 7), ("initial_cost", "<f8"), ("fi
                                ("successful", "<i4"), ("unsuccessful", "<i4"), ("termination", "<i4"), ("radius", "<f8"),
                                ("decrease_factor", "<f8"), ("gmax", "<f8"), ("n_flag_pos", "<i4"), ("n_flag_ori", "<i4"),
                                ("status", "<i4"), ("pad_", "<i4")], align=True)
+# so_solve_optimized's problems and results (rows: SOLVE_ROW_DTYPE, with one float32 time per row)
+SOLVE_OPTIMIZED_PROBLEM_DTYPE = np.dtype([("n_rows", "<u4"), ("lm_max_iterations", "<i4"), ("pose", "<f8", 7), ("motion", "<f8", 7),
+                                          ("dt", "<f8"), ("motion_prior", "<f8", 7), ("motion_info", "<f8", 6)], align=True)
+SOLVE_OPTIMIZED_RESULT_DTYPE = np.dtype([("solve", SOLVE_RESULT_DTYPE), ("motion", "<f8", 7), ("cov", "<f8", 36)], align=True)
 
 _lib = None
 
@@ -312,6 +316,7 @@ def load_library():
                                                C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     L.so_degeneracy_analysis.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     L.so_solve.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
+    L.so_solve_optimized.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
     L.so_knn.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_int, C.c_float, C.c_void_p, C.c_void_p]
     L.so_knn_device.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_float, C.c_void_p, C.c_void_p]
     L.so_sampling_indices.argtypes = [C.c_uint32, C.c_int32, C.c_void_p, C.c_size_t, C.c_void_p]
@@ -1072,6 +1077,19 @@ class Context:
         out = np.zeros(len(problems), SOLVE_RESULT_DTYPE)
         da = None if ds is None else (Degeneracy * len(problems))(*ds)
         self._chk(self.L.so_solve(self.h, _p(rows) if len(rows) else None, _p(problems), len(problems), da, _p(out)), "so_solve")
+        return out
+
+    def solve_optimized(self, rows: np.ndarray, times: np.ndarray, problems: np.ndarray) -> np.ndarray:
+        """The two-block solve of so_register_optimized per problem on given correspondences (so_solve_optimized): rows [sum n_rows] of
+        SOLVE_ROW_DTYPE and times [sum n_rows] float32, problem b's after problem b - 1's; problems [B] of
+        SOLVE_OPTIMIZED_PROBLEM_DTYPE.  -> [B] of SOLVE_OPTIMIZED_RESULT_DTYPE."""
+        rows = np.ascontiguousarray(rows, dtype=SOLVE_ROW_DTYPE)
+        times = np.ascontiguousarray(times, dtype=np.float32)
+        problems = np.ascontiguousarray(problems, dtype=SOLVE_OPTIMIZED_PROBLEM_DTYPE)
+        assert int(problems["n_rows"].sum()) == len(rows) == len(times)
+        out = np.zeros(len(problems), SOLVE_OPTIMIZED_RESULT_DTYPE)
+        self._chk(self.L.so_solve_optimized(self.h, _p(rows) if len(rows) else None, _p(times) if len(times) else None, _p(problems),
+                                            len(problems), _p(out)), "so_solve_optimized")
         return out
 
     # ---- global localization

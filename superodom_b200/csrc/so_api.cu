@@ -1847,52 +1847,40 @@ int so_degeneracy_analysis(so_ctx* ctx, const double* H, const so_degeneracy* d,
     return SO_OK;
 }
 
-// The buffers k_fit fills (scan point with its index in w, {n, d}, weight, flags, the accepted-row histogram) are written from the
-// caller's rows; then the first evaluation and lm_max evaluations run as one ICP iteration of a registration launches them.
-int so_solve(so_ctx* ctx, const so_solve_row* rows, const so_solve_problem* pr, size_t n_problems, const so_degeneracy* d, so_solve_result* out) {
-    Ctx* c = reinterpret_cast<Ctx*>(ctx);
-    if (!c || !pr || !out || n_problems == 0) return fail(SO_ERR_ARG, "bad args");
-    if (n_problems > size_t(c->max_batch)) return fail(SO_ERR_CAPACITY, "more problems than so_config.max_batch");
-    if (d) { int rc = check_degeneracy(d, n_problems); if (rc) return rc; }
+// so_solve / so_solve_optimized, once the caller has checked its arguments and initialised h_state[0..n_problems): the buffers k_fit
+// fills (scan point with its index in w, {n, d}, weight, flags, the accepted-row histogram) are written from the caller's rows; then the
+// first evaluation and lm evaluations run as one ICP iteration of a registration launches them.  ms (mode OPTIMIZED): the problems'
+// motion blocks, updated in place; the rows' raw points also go to d_scan and their times to und.d_time, where k_motion_eval reads them.
+// dg: the degeneracy-aware solve's states (so_solve), updated in place.
+static int solve_stage(Ctx* c, const so_solve_row* rows, const float* times, size_t n_problems, int lm, MotionState* ms, DegenState* dg,
+                       so_solve_result* out) {
     size_t total = 0;
     uint32_t max_n = 0;
-    int lm = 0;
-    for (size_t b = 0; b < n_problems; ++b) {
-        if (pr[b].n_rows > c->cfg.max_scan_points) return fail(SO_ERR_CAPACITY, "problem larger than so_config.max_scan_points");
-        if (pr[b].lm_max_iterations > 16) return fail(SO_ERR_ARG, "lm_max_iterations must be <= 16");
-        total += pr[b].n_rows;
-        max_n = std::max(max_n, pr[b].n_rows);
-        lm = std::max(lm, pr[b].lm_max_iterations <= 0 ? 4 : pr[b].lm_max_iterations);
-    }
-    if (total && !rows) return fail(SO_ERR_ARG, "bad args");
+    for (size_t b = 0; b < n_problems; ++b) { total += uint32_t(c->h_state[b].n_points); max_n = std::max(max_n, uint32_t(c->h_state[b].n_points)); }
     SO_CUDA_TRY(cudaSetDevice(c->device));
-    if (d) { int rc = c->deg.d_st.reserve(c->max_batch); if (rc) return rc; }
+    if (dg) { int rc = c->deg.d_st.reserve(c->max_batch); if (rc) return rc; }
+    if (ms) { int rc = motion_reserve(c, total); if (rc) return rc; }
     c->prefiltered_n = SIZE_MAX;                                  // d_scan_sorted is overwritten
-    std::vector<float4> sp(total);
+    if (ms) c->reg.valid = false;                                 // so are d_scan and the times
+    std::vector<float4> raw(ms ? total : 0), sp(total);
     std::vector<double4> nd(total);
     std::vector<double> w(total);
     std::vector<int32_t> hist(n_problems * kHistStride, 0);
-    std::vector<DegenState> dg(d ? n_problems : 0);
     uint32_t off = 0;
     for (size_t b = 0; b < n_problems; ++b) {
-        so_icp_opts o{};
-        o.max_icp_iters = 1; o.lm_max_iterations = pr[b].lm_max_iterations <= 0 ? 4 : pr[b].lm_max_iterations;
-        o.use_pose_prior = pr[b].use_pose_prior; o.visual_confidence_factor = pr[b].visual_confidence_factor;
-        for (int a = 0; a < 3; ++a) o.prior_uncertainty[a] = pr[b].prior_uncertainty[a];
-        init_state(c->h_state[b], pr[b].pose, pr[b].n_rows, o);
-        std::memcpy(c->h_state[b].x0, pr[b].x0, sizeof(c->h_state[b].x0));      // the prior's measurement, apart from the start
+        const uint32_t n = uint32_t(c->h_state[b].n_points);
         c->h_offset[b] = off;
-        for (uint32_t i = 0; i < pr[b].n_rows; ++i) {
+        for (uint32_t i = 0; i < n; ++i) {
             const so_solve_row& r = rows[off + i];
             float4 p = make_float4(r.p[0], r.p[1], r.p[2], 0.f);
+            if (ms) raw[off + i] = p;
             std::memcpy(&p.w, &i, 4);                             // the point's index inside its scan, as k_scan_gather writes it
             sp[off + i] = p;
             nd[off + i] = make_double4(r.n[0], r.n[1], r.n[2], r.d);
             w[off + i] = r.w;
         }
-        hist[b * kHistStride + 9] = int32_t(pr[b].n_rows);       // hist_rej[SUCCESS]: every row is accepted
-        if (d) dg[b] = degen_state(d[b]);
-        off += pr[b].n_rows;
+        hist[b * kHistStride + 9] = int32_t(n);                   // hist_rej[SUCCESS]: every row is accepted
+        off += n;
     }
     cudaStream_t st = c->stream;
     SO_CUDA_TRY(cudaMemcpyAsync(c->d_state, c->h_state, n_problems * sizeof(IcpState), cudaMemcpyHostToDevice, st));
@@ -1903,31 +1891,43 @@ int so_solve(so_ctx* ctx, const so_solve_row* rows, const so_solve_problem* pr, 
         SO_CUDA_TRY(cudaMemcpyAsync(c->corr.nd, nd.data(), total * sizeof(double4), cudaMemcpyHostToDevice, st));
         SO_CUDA_TRY(cudaMemcpyAsync(c->corr.w, w.data(), total * sizeof(double), cudaMemcpyHostToDevice, st));
         SO_CUDA_TRY(cudaMemsetAsync(c->corr.flags, 0, total * sizeof(uchar4), st));
+        if (ms) {
+            SO_CUDA_TRY(cudaMemcpyAsync(c->d_scan, raw.data(), total * sizeof(float4), cudaMemcpyHostToDevice, st));
+            SO_CUDA_TRY(cudaMemcpyAsync(c->und.d_time, times, total * sizeof(float), cudaMemcpyHostToDevice, st));
+        }
     }
-    if (d) SO_CUDA_TRY(cudaMemcpyAsync(c->deg.d_st, dg.data(), n_problems * sizeof(DegenState), cudaMemcpyHostToDevice, st));
+    if (dg) SO_CUDA_TRY(cudaMemcpyAsync(c->deg.d_st, dg, n_problems * sizeof(DegenState), cudaMemcpyHostToDevice, st));
+    if (ms) SO_CUDA_TRY(cudaMemcpyAsync(c->mot.d_st, ms, n_problems * sizeof(MotionState), cudaMemcpyHostToDevice, st));
     // the chunk's CTA count as register_core rounds it
     uint32_t grid_x = (max_n + kThreads - 1) / kThreads;
     if (grid_x) grid_x = std::min<uint32_t>(c->grid_x_cap, (grid_x + 15u) & ~15u);
     BatchView bv = batch_view(c, c->d_scan_sorted);
-    if (fused_lm(c, uint32_t(n_problems), UndistortionMode::NONE, d != nullptr)) bv.counters = c->d_counters;
+    const UndistortionMode mode = ms ? UndistortionMode::OPTIMIZED : UndistortionMode::NONE;
+    if (fused_lm(c, uint32_t(n_problems), mode, dg != nullptr)) bv.counters = c->d_counters;
     CorrBuf cb = c->corr;
     cb.nn = nullptr; cb.nn_d2 = nullptr;
-    DegenState* const ddg = d ? c->deg.d_st.get() : nullptr;
+    DegenState* const ddg = dg ? c->deg.d_st.get() : nullptr;
     const uint32_t nb = uint32_t(n_problems);
+    auto solve = [&](int phase) {                                  // run_schedule's solve(phase)
+        if (ms) launch_motion_solve(phase, bv, cb, c->d_scan, c->und.d_time, c->mot.d_st, 0, c->mot.d_partials, c->mot.stride, grid_x, nb, st, nullptr);
+        else if (phase == PH_CORR) launch_first_eval(bv, cb, grid_x, nb, st, nullptr, nullptr, 0, ddg);
+        else launch_evaluate(bv, cb, grid_x, nb, st, nullptr, 0, ddg);
+    };
     timed_launch_begin(c);
-    launch_first_eval(bv, cb, grid_x, nb, st, nullptr, nullptr, 0, ddg);
-    timed_launch_end(c, 4);
+    solve(PH_CORR);
+    timed_launch_end(c, ms ? 8 : 4);
     SO_CUDA_TRY(cudaGetLastError());
     std::vector<double> cost0(n_problems);                        // the cost IterationZero evaluated (the state's cost moves with the steps)
     SO_CUDA_TRY(cudaMemcpyAsync(c->h_state, c->d_state, n_problems * sizeof(IcpState), cudaMemcpyDeviceToHost, st));
     SO_CUDA_TRY(cudaStreamSynchronize(st));
     for (size_t b = 0; b < n_problems; ++b) cost0[b] = c->h_state[b].cost;
     for (int k = 0; k < lm; ++k) {
-        timed_launch_begin(c); launch_evaluate(bv, cb, grid_x, nb, st, nullptr, 0, ddg); timed_launch_end(c, 1);
+        timed_launch_begin(c); solve(PH_EVAL); timed_launch_end(c, ms ? 8 : 1);
     }
     SO_CUDA_TRY(cudaGetLastError());
     SO_CUDA_TRY(cudaMemcpyAsync(c->h_state, c->d_state, n_problems * sizeof(IcpState), cudaMemcpyDeviceToHost, st));
-    if (d) SO_CUDA_TRY(cudaMemcpyAsync(dg.data(), c->deg.d_st, n_problems * sizeof(DegenState), cudaMemcpyDeviceToHost, st));
+    if (dg) SO_CUDA_TRY(cudaMemcpyAsync(dg, c->deg.d_st, n_problems * sizeof(DegenState), cudaMemcpyDeviceToHost, st));
+    if (ms) SO_CUDA_TRY(cudaMemcpyAsync(ms, c->mot.d_st, n_problems * sizeof(MotionState), cudaMemcpyDeviceToHost, st));
     SO_CUDA_TRY(cudaStreamSynchronize(st));
     for (size_t b = 0; b < n_problems; ++b) {
         const IcpState& s = c->h_state[b];
@@ -1937,8 +1937,72 @@ int so_solve(so_ctx* ctx, const so_solve_row* rows, const so_solve_problem* pr, 
         r.initial_cost = cost0[b]; r.final_cost = s.cost;
         r.lm_iterations = s.lm_iter; r.successful = s.num_successful; r.unsuccessful = s.num_unsuccessful; r.termination = s.termination;
         r.radius = s.radius; r.decrease_factor = s.decrease_factor; r.gmax = s.gmax;
-        if (d) { r.n_flag_pos = dg[b].iter_n_flag_pos[0]; r.n_flag_ori = dg[b].iter_n_flag_ori[0]; }
+        if (dg) { r.n_flag_pos = dg[b].iter_n_flag_pos[0]; r.n_flag_ori = dg[b].iter_n_flag_ori[0]; }
         r.status = s.status;
+    }
+    return SO_OK;
+}
+
+int so_solve(so_ctx* ctx, const so_solve_row* rows, const so_solve_problem* pr, size_t n_problems, const so_degeneracy* d, so_solve_result* out) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c || !pr || !out || n_problems == 0) return fail(SO_ERR_ARG, "bad args");
+    if (n_problems > size_t(c->max_batch)) return fail(SO_ERR_CAPACITY, "more problems than so_config.max_batch");
+    if (d) { int rc = check_degeneracy(d, n_problems); if (rc) return rc; }
+    size_t total = 0;
+    int lm = 0;
+    for (size_t b = 0; b < n_problems; ++b) {
+        if (pr[b].n_rows > c->cfg.max_scan_points) return fail(SO_ERR_CAPACITY, "problem larger than so_config.max_scan_points");
+        if (pr[b].lm_max_iterations > 16) return fail(SO_ERR_ARG, "lm_max_iterations must be <= 16");
+        total += pr[b].n_rows;
+        lm = std::max(lm, pr[b].lm_max_iterations <= 0 ? 4 : pr[b].lm_max_iterations);
+    }
+    if (total && !rows) return fail(SO_ERR_ARG, "bad args");
+    std::vector<DegenState> dg(d ? n_problems : 0);
+    for (size_t b = 0; b < n_problems; ++b) {
+        so_icp_opts o{};
+        o.max_icp_iters = 1; o.lm_max_iterations = pr[b].lm_max_iterations <= 0 ? 4 : pr[b].lm_max_iterations;
+        o.use_pose_prior = pr[b].use_pose_prior; o.visual_confidence_factor = pr[b].visual_confidence_factor;
+        for (int a = 0; a < 3; ++a) o.prior_uncertainty[a] = pr[b].prior_uncertainty[a];
+        init_state(c->h_state[b], pr[b].pose, pr[b].n_rows, o);
+        std::memcpy(c->h_state[b].x0, pr[b].x0, sizeof(c->h_state[b].x0));      // the prior's measurement, apart from the start
+        if (d) dg[b] = degen_state(d[b]);
+    }
+    return solve_stage(c, rows, nullptr, n_problems, lm, nullptr, d ? dg.data() : nullptr, out);
+}
+
+// The two-block solve of so_register_optimized: each problem's motion block from its so_motion, with D and Dc at the start motion
+int so_solve_optimized(so_ctx* ctx, const so_solve_row* rows, const float* times, const so_solve_optimized_problem* pr, size_t n_problems,
+                       so_solve_optimized_result* out) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c || !pr || !out || n_problems == 0) return fail(SO_ERR_ARG, "bad args");
+    if (n_problems > size_t(c->max_batch)) return fail(SO_ERR_CAPACITY, "more problems than so_config.max_batch");
+    size_t total = 0;
+    int lm = 0;
+    std::vector<MotionState> ms(n_problems);
+    for (size_t b = 0; b < n_problems; ++b) {
+        if (pr[b].n_rows > c->cfg.max_scan_points) return fail(SO_ERR_CAPACITY, "problem larger than so_config.max_scan_points");
+        so_icp_opts o{};
+        o.max_icp_iters = 1; o.lm_max_iterations = pr[b].lm_max_iterations <= 0 ? 4 : pr[b].lm_max_iterations;
+        { int rc = check_motion(&pr[b].m, &o); if (rc) return rc; }
+        if (!finite_pose(pr[b].pose) || !finite_pose(pr[b].motion)) return fail(SO_ERR_ARG, "pose and motion must be finite with a non-zero quaternion");
+        total += pr[b].n_rows;
+        lm = std::max(lm, o.lm_max_iterations);
+        init_state(c->h_state[b], pr[b].pose, pr[b].n_rows, o);
+        ms[b] = make_state(pr[b].m);
+        const double* D = pr[b].motion;
+        const double n = std::sqrt(D[3] * D[3] + D[4] * D[4] + D[5] * D[5] + D[6] * D[6]);      // normalised as make_state normalises D0
+        for (int k = 0; k < 7; ++k) ms[b].D[k] = ms[b].Dc[k] = k < 3 ? D[k] : D[k] / n;
+    }
+    if (total && (!rows || !times)) return fail(SO_ERR_ARG, "bad args");
+    std::vector<so_solve_result> res(n_problems);
+    const int rc = solve_stage(c, rows, times, n_problems, lm, ms.data(), nullptr, res.data());
+    if (rc) return rc;
+    for (size_t b = 0; b < n_problems; ++b) {
+        so_solve_optimized_result& r = out[b];
+        std::memset(&r, 0, sizeof(r));
+        r.solve = res[b];
+        std::memcpy(r.motion, ms[b].D, sizeof(r.motion));
+        std::memcpy(r.cov, c->h_state[b].cov, sizeof(r.cov));
     }
     return SO_OK;
 }

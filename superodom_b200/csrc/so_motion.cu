@@ -707,19 +707,19 @@ void launch_motion_warp(const BatchView& bv, float4* sorted, const float4* raw, 
 void launch_motion_solve(int phase, const BatchView& bv, const CorrBuf& cb, const float4* raw, const float* times, MotionState* ms, uint32_t first,
                          double* partials, uint32_t stride, uint32_t grid_x, uint32_t n_scans, cudaStream_t st, const MotionEdges* me) {
     ms += first;
-    const uint32_t gx = eval_grid(grid_x * kThreads);
+    const uint32_t gx = grid_x ? eval_grid(grid_x * kThreads) : 0;       // 0: every scan is empty; k_motion_step still ends their solves
     const uint32_t ge = me ? me->grid_e : 0;
     const uint32_t* eoff = me ? me->eb.offset : nullptr;
     double* ep = me ? me->partials : nullptr;
     if (phase == PH_CORR) {
-        k_motion_eval<PH_CORR><<<dim3(gx, n_scans), kThreads, 0, st>>>(bv, cb, raw, times, ms, partials, stride);
+        if (gx) k_motion_eval<PH_CORR><<<dim3(gx, n_scans), kThreads, 0, st>>>(bv, cb, raw, times, ms, partials, stride);
         if (ge) {
             launch_edge_fit(me->map, bv, me->eb, ge, n_scans, st);
             k_motion_eval_edge<PH_CORR><<<dim3(ge, n_scans), kThreads, 0, st>>>(bv, me->eb, me->raw, me->times, ms, ep, first);
         }
         k_motion_step<PH_CORR><<<n_scans, 128, 0, st>>>(bv, ms, partials, stride, ep, eoff, first);
     } else {
-        k_motion_eval<PH_EVAL><<<dim3(gx, n_scans), kThreads, 0, st>>>(bv, cb, raw, times, ms, partials, stride);
+        if (gx) k_motion_eval<PH_EVAL><<<dim3(gx, n_scans), kThreads, 0, st>>>(bv, cb, raw, times, ms, partials, stride);
         if (ge) k_motion_eval_edge<PH_EVAL><<<dim3(ge, n_scans), kThreads, 0, st>>>(bv, me->eb, me->raw, me->times, ms, ep, first);
         k_motion_step<PH_EVAL><<<n_scans, 128, 0, st>>>(bv, ms, partials, stride, ep, eoff, first);
     }

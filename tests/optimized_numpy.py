@@ -1,8 +1,9 @@
 """numpy restatement of so_register_optimized's solve (so_motion.cu): the warp u(D), the plane rows over two pose7 blocks (T, D), their
-12-column Jacobian, the motion prior rows and the two-block trust-region loop.
+12-column Jacobian and the motion prior rows; the two-block trust-region loop is test_ceres_restatement.solve_full over the two pose7
+blocks (T, D).
 
 Written apart from the device code: rotation matrices instead of quaternion rotations, the D rotation columns as
-alpha (p x b)^T J_r(alpha phi) J_r(phi)^-1 with J_r built as 3x3 matrices, numpy's LAPACK least squares for the step.  The warp
+alpha (p x b)^T J_r(alpha phi) J_r(phi)^-1 with J_r(phi)^-1 a 3x3 matrix inverse, numpy's LAPACK least squares for the step.  The warp
 (float(u(D)), what every ICP iteration searches with) restates the device's bits through undistort_numpy."""
 from __future__ import annotations
 
@@ -11,8 +12,7 @@ import math
 import numpy as np
 
 import undistort_numpy as UN
-from test_ceres_restatement import (FUNCTION_TOL, GRADIENT_TOL, MAX_LM_DIAG, MAX_RADIUS, MIN_LM_DIAG, MIN_RADIUS, MIN_REL_DECREASE,
-                                    PARAMETER_TOL, _plus, _qmul, _rot)
+from test_ceres_restatement import _plus, _qmul, _rot, solve_full
 
 
 def warp_points(xyz_time: np.ndarray, D, dt: float) -> np.ndarray:
@@ -51,29 +51,32 @@ def _jr(v):
     return np.eye(3) - (1 - math.cos(th)) / th ** 2 * K + (th - math.sin(th)) / th ** 3 * K @ K
 
 
-def _slerp_R(q, a):
-    """R(slerp(identity, q, a)) with Eigen's branches (linear for |q.w| >= 1 - eps: not unit, as Eigen leaves it)"""
-    q = np.asarray(q, np.float64)
+def _slerp_coeffs(q, A):
+    """s0, s1 [n] of Eigen's slerp(identity, q, alpha) for unit q: linear for |q.w| >= 1 - eps (not unit then, as Eigen leaves it)"""
+    A = np.asarray(A, np.float64)
     ad = abs(q[3])
     if ad >= 1.0 - UN.EPS:
-        s0, s1 = 1.0 - a, a
+        s0, s1 = 1.0 - A, A.copy()
     else:
         th = math.acos(ad)
-        s0, s1 = math.sin((1 - a) * th) / math.sin(th), math.sin(a * th) / math.sin(th)
-    if q[3] < 0:
-        s1 = -s1
-    qa = np.array([s1 * q[0], s1 * q[1], s1 * q[2], s0 + s1 * q[3]])
-    x, y, z, w = qa                                                      # qrot of a possibly non-unit quaternion, as a matrix
-    return np.array([[w * w + x * x - y * y - z * z, 2 * (x * y - w * z), 2 * (x * z + w * y)],
-                     [2 * (x * y + w * z), w * w - x * x + y * y - z * z, 2 * (y * z - w * x)],
-                     [2 * (x * z - w * y), 2 * (y * z + w * x), w * w - x * x - y * y + z * z]])
+        s0, s1 = np.sin((1 - A) * th) / math.sin(th), np.sin(A * th) / math.sin(th)
+    return s0, (-s1 if q[3] < 0 else s1)
+
+
+def _slerp_Rs(q, A):
+    """R(slerp(identity, q, alpha)) [n, 3, 3] for every alpha: the rotation of a possibly non-unit quaternion, as a matrix"""
+    s0, s1 = _slerp_coeffs(np.asarray(q, np.float64), A)
+    x, y, z, w = s1 * q[0], s1 * q[1], s1 * q[2], s0 + s1 * q[3]
+    return np.stack([np.stack([w * w + x * x - y * y - z * z, 2 * (x * y - w * z), 2 * (x * z + w * y)], -1),
+                     np.stack([2 * (x * y + w * z), w * w - x * x + y * y - z * z, 2 * (y * z - w * x)], -1),
+                     np.stack([2 * (x * z - w * y), 2 * (y * z + w * x), w * w - x * x - y * y + z * z], -1)], -2)
 
 
 def warp_double(P, A, D):
     """u_i(D) in double [n, 3]"""
     D = np.asarray(D, np.float64)
     q = D[3:] / np.linalg.norm(D[3:])
-    return np.stack([_slerp_R(q, a) @ p for p, a in zip(P, A)]) + A[:, None] * D[:3]
+    return np.einsum("nij,nj->ni", _slerp_Rs(q, A), P) + A[:, None] * D[:3]
 
 
 def residuals(P, A, N, Dd, T, D):
@@ -86,16 +89,21 @@ def jacobian(P, A, N, T, D):
     q = np.asarray(D[3:], np.float64) / np.linalg.norm(D[3:])
     phi = _log_q(q)
     jinv = np.linalg.inv(_jr(phi))
-    U = warp_double(P, A, D)
-    out = np.zeros((len(P), 12))
-    for i, (p, a, n, u) in enumerate(zip(P, A, N, U)):
-        av = R.T @ n
-        b = _slerp_R(q, a).T @ av
-        out[i, :3] = n
-        out[i, 3:6] = np.cross(u, av)
-        out[i, 6:9] = a * av
-        out[i, 9:] = a * (np.cross(p, b) @ _jr(a * phi) @ jinv)
-    return out
+    Ra = _slerp_Rs(q, A)
+    U = np.einsum("nij,nj->ni", Ra, P) + A[:, None] * np.asarray(D[:3], np.float64)
+    av = N @ R                                                           # rows: R^T n
+    b = np.einsum("nji,nj->ni", Ra, av)                                  # R(q_alpha)^T R^T n
+    w = np.cross(P, b)
+    # w^T J_r(v), v = alpha phi: w^T [v]x = w x v, so w^T J_r(v) = w - c1 (w x v) + c2 (w x v) x v
+    V = A[:, None] * phi
+    th = np.abs(A) * np.linalg.norm(phi)
+    small = th < 1e-4
+    ths = np.where(small, 1.0, th)
+    c1 = np.where(small, 0.5, (1 - np.cos(ths)) / ths ** 2)
+    c2 = np.where(small, 1.0 / 6.0, (ths - np.sin(ths)) / ths ** 3)
+    wv = np.cross(w, V)
+    wj = w - c1[:, None] * wv + c2[:, None] * np.cross(wv, V)
+    return np.concatenate([N, np.cross(U, av), A[:, None] * av, A[:, None] * (wj @ jinv)], 1)
 
 
 class Problem:
@@ -140,68 +148,30 @@ class Problem:
         return (J * rho1[:, None]).T @ J, J.T @ (rho1 * r), 0.5 * rho0.sum()
 
 
+class _Stacked:
+    """A (T, D) problem as solve_full sees it: one vector of the two pose7 blocks"""
+
+    def __init__(self, prob):
+        self.prob = prob
+
+    def cost(self, x):
+        return self.prob.cost(x[:7], x[7:])
+
+    def linearise(self, x):
+        return self.prob.linearise(x[:7], x[7:])
+
+
+def solve_full2(prob, T0, D0, max_iterations=4):
+    """solve_full over (T, D) from T0 and D0 (its quaternion normalised): its dict, with x = [T, D]"""
+    D = np.array(D0, float)
+    D[3:] /= np.linalg.norm(D[3:])
+    return solve_full(_Stacked(prob), np.concatenate([np.asarray(T0, float), D]), max_iterations)
+
+
 def solve(prob, T0, D0, max_iterations=4):
     """-> (T, D, iterations, successful_steps, unsuccessful_steps, termination), the codes of so_icp_result.iter_lm_termination"""
-    T, D = np.array(T0, float), np.array(D0, float)
-    D[3:] /= np.linalg.norm(D[3:])
-    cost, res, J = prob.linearise(T, D)
-    scale = 1.0 / (1.0 + np.linalg.norm(J, axis=0))
-
-    def gmax_of(T, D, g):
-        return max(np.abs(T - _plus(T, -g[:6])).max(), np.abs(D - _plus(D, -g[6:])).max())
-    gmax = gmax_of(T, D, J.T @ res)
-    Js = J * scale
-    radius, decrease, reuse, diag = 1e4, 2.0, False, None
-    it = succ = unsucc = invalid = 0
-    step_ok = False
-    while True:
-        if step_ok:
-            succ += 1
-        else:
-            unsucc += 1
-        if it >= max_iterations:
-            return T, D, it, succ, unsucc, 0
-        if gmax <= GRADIENT_TOL:
-            return T, D, it, succ, unsucc, 1
-        if radius <= MIN_RADIUS:
-            return T, D, it, succ, unsucc, 4
-        it += 1
-        step_ok = False
-        if not reuse:
-            diag = np.clip((Js * Js).sum(0), MIN_LM_DIAG, MAX_LM_DIAG)
-        reuse = True
-        y = np.linalg.lstsq(np.concatenate([Js, np.diag(np.sqrt(diag / radius))]), np.concatenate([res, np.zeros(12)]), rcond=None)[0]
-        step = -y
-        mr = Js @ step
-        model_change = -(mr * (res + mr / 2.0)).sum()
-        if not (np.isfinite(step).all() and model_change > 0.0):
-            invalid += 1
-            if invalid >= 5:
-                return T, D, it, succ, unsucc, 5
-            radius *= 0.5
-            continue
-        invalid = 0
-        d = step * scale
-        Tc, Dc = _plus(T, d[:6]), _plus(D, d[6:])
-        cand_cost = prob.cost(Tc, Dc)
-        if math.sqrt(((T - Tc) ** 2).sum() + ((D - Dc) ** 2).sum()) <= PARAMETER_TOL * (math.sqrt((T * T).sum() + (D * D).sum()) + PARAMETER_TOL):
-            return T, D, it, succ, unsucc, 2
-        change = cost - cand_cost
-        if abs(change) <= FUNCTION_TOL * cost:
-            return T, D, it, succ, unsucc, 3
-        rel = change / model_change
-        if rel > MIN_REL_DECREASE:
-            T, D = Tc, Dc
-            cost, res, J = prob.linearise(T, D)
-            Js = J * scale
-            gmax = gmax_of(T, D, J.T @ res)
-            step_ok = True
-            radius = min(MAX_RADIUS, radius / max(1.0 / 3.0, 1.0 - (2.0 * rel - 1.0) ** 3))
-            decrease, reuse = 2.0, False
-        else:
-            radius /= decrease
-            decrease *= 2.0
-            reuse = True
+    r = solve_full2(prob, T0, D0, max_iterations)
+    return r["x"][:7], r["x"][7:], r["iterations"], r["successful"], r["unsuccessful"], r["termination"]
 
 
 def compose(T, D):

@@ -35,6 +35,10 @@ def _plus(x, d):              # PoseLocalParameterization::Plus (pose_local_para
     return np.concatenate([x[:3] + d[:3], q / np.linalg.norm(q)])
 
 
+def _plus_blocks(x, d):       # Plus of each pose7 block of x by its 6 tangent values in d
+    return np.concatenate([_plus(x[7 * k:7 * k + 7], d[6 * k:6 * k + 6]) for k in range(len(x) // 7)])
+
+
 class Problem:
     """n point-to-plane blocks {p, n, d, w} under ScaledLoss(TukeyLoss(a), w) (LidarSlam.cpp:268-274), and optionally the 6 rows of
     SE3AbsolutatePoseFactor (factor/SE3AbsolutatePoseFactor.cpp: [p - p_m ; 2 vec(q_m^* q)] times a diagonal sqrt-information, no
@@ -109,19 +113,21 @@ def _rel_margin(value, threshold):
 
 
 def solve_full(prob, x0, max_iterations=4, B=None):
-    """Ceres' trust-region LM on prob from x0; B (6 x m, optional): the solve on B's columns, local parameterisation x [+] B y
-    (Jacobian J B, Jacobi scaling and LM diagonal over the m columns, gradient max-norm through Plus(x, -B B^T g); x_norm and the
-    parameter / function tolerances ambient).  -> dict: x, iterations, successful, unsuccessful, termination (codes as
+    """Ceres' trust-region LM on prob from x0, a vector of k pose7 blocks (prob.linearise(x) gives the Jacobian over their 6k tangent
+    columns, block by block; Plus, the gradient max-norm, x_norm and the step norm run over all blocks); B (6k x m, optional): the
+    solve on B's columns, local parameterisation x [+] B y (Jacobian J B, Jacobi scaling and LM diagonal over the m columns, gradient
+    max-norm through Plus(x, -B B^T g); x_norm and the parameter / function tolerances ambient).  -> dict: x, iterations, successful, unsuccessful, termination (codes as
     oracle/so_oracle.cpp), initial_cost, final_cost, and the trust-region state the solve ends in (radius, decrease_factor, gmax);
     steps: 'a' accepted / 'r' rejected / 'i' invalid per LM iteration; margin: the smallest relative distance of any decision the
     solve took from its threshold (gradient, radius, parameter and function tolerances, step quality, model cost change);
-    radius_error: an estimate of the relative error of the final radius that rounding alone leaves.  A step is only known to about
+    radius_error: an estimate of the relative error of the final radius that rounding alone leaves; radius_error_normal: the same for a
+    solver that forms the normal equations (the device's Cholesky), whose step is known only to cond^2 x machine epsilon.  A step is only known to about
     cond x machine epsilon (cond: of the damped least-squares system it is solved from), and so is the model cost change; the cost
     change is a difference of sums rounded at the scale of the initial cost.  Both carry into the step quality rd, and every accepted
     step multiplies the radius by 1 / max(1/3, 1 - (2 rd - 1)^3), whose relative sensitivity to rd is summed over the steps."""
-    B = np.eye(6) if B is None else np.asarray(B, float)
-    m = B.shape[1]
     x = np.array(x0, float)
+    B = np.eye(6 * (len(x) // 7)) if B is None else np.asarray(B, float)
+    m = B.shape[1]
     cost, res, J = prob.linearise(x)
     initial_cost = cost
     Jr = J @ B
@@ -129,19 +135,19 @@ def solve_full(prob, x0, max_iterations=4, B=None):
     Js = Jr * scale
 
     def gmax_of(xx, JJ, rr):
-        return np.abs(xx - _plus(xx, -(B @ (B.T @ (JJ.T @ rr))))).max()
+        return np.abs(xx - _plus_blocks(xx, -(B @ (B.T @ (JJ.T @ rr))))).max()
     gmax = gmax_of(x, J, res)
     radius, decrease, reuse = 1e4, 2.0, False
     diag = None
     it = succ = unsucc = invalid = 0
     step_ok = False
     steps, margins = [], []
-    eps, radius_error = np.finfo(float).eps, 0.0
+    eps, radius_error, radius_error_normal = np.finfo(float).eps, 0.0, 0.0
 
     def done(term):
         return dict(x=x, iterations=it, successful=succ, unsuccessful=unsucc, termination=term, initial_cost=initial_cost,
                     final_cost=cost, radius=radius, decrease_factor=decrease, gmax=gmax, steps="".join(steps),
-                    margin=min(margins) if margins else np.inf, radius_error=radius_error)
+                    margin=min(margins) if margins else np.inf, radius_error=radius_error, radius_error_normal=radius_error_normal)
     while True:
         if step_ok:
             succ += 1
@@ -176,7 +182,7 @@ def solve_full(prob, x0, max_iterations=4, B=None):
             radius *= 0.5
             continue
         invalid = 0
-        cand = _plus(x, B @ (step * scale))
+        cand = _plus_blocks(x, B @ (step * scale))
         cand_cost = prob.cost(cand)
         sn, tol = np.linalg.norm(x - cand), PARAMETER_TOL * (np.linalg.norm(x) + PARAMETER_TOL)
         margins.append(_rel_margin(sn, tol))
@@ -193,6 +199,7 @@ def solve_full(prob, x0, max_iterations=4, B=None):
             t = 2.0 * rel - 1.0
             if 1.0 - t ** 3 > 1.0 / 3.0 and radius / (1.0 - t ** 3) < MAX_RADIUS:      # d ln(factor) / d ln(rd), 0 where capped
                 radius_error += abs(6.0 * t * t * rel / (1.0 - t ** 3)) * (cond * eps + eps * initial_cost / abs(change))
+                radius_error_normal += abs(6.0 * t * t * rel / (1.0 - t ** 3)) * (cond * cond * eps + eps * initial_cost / abs(change))
             x = cand
             cost, res, J = prob.linearise(x)
             Js = (J @ B) * scale

@@ -37,7 +37,22 @@ def _overwriting_calls(api, d):
         "so_register_batch_undistort": lambda c: c.register_batch_undistort(scan, [n], prior[None], [api.undistort(d["pose_prev"], 0.1)], 5, 2000),
         "so_register_batch_optimized": lambda c: c.register_batch_optimized(scan, [n], prior[None], [api.motion(0.1)], 5, 2000),
         "so_evaluate_optimized": lambda c: c.evaluate_optimized(scan, prior, IDENTITY, 0.1),
+        "so_solve_optimized": lambda c: c.solve_optimized(*_solve_rows(api, scan[:300], prior, optimized=True)),
     }
+
+
+def _solve_rows(api, scan, pose, optimized=False):
+    """one so_solve / so_solve_optimized problem whose rows are the scan's first points on the plane z = 0"""
+    n = len(scan)
+    rows = np.zeros(n, api.SOLVE_ROW_DTYPE)
+    rows["p"], rows["n"], rows["w"] = scan[:, :3], (0.0, 0.0, 1.0), 1.0
+    if not optimized:
+        pr = np.zeros(1, api.SOLVE_PROBLEM_DTYPE)
+        pr[0]["n_rows"], pr[0]["pose"] = n, pose
+        return rows, pr
+    pr = np.zeros(1, api.SOLVE_OPTIMIZED_PROBLEM_DTYPE)
+    pr[0]["n_rows"], pr[0]["pose"], pr[0]["motion"], pr[0]["dt"], pr[0]["motion_prior"] = n, pose, IDENTITY, 0.1, IDENTITY
+    return rows, np.linspace(0.0, 0.1, n, dtype=np.float32), pr
 
 
 def _leaving_calls(api, d):
@@ -66,6 +81,7 @@ def _leaving_calls(api, d):
         "so_map_add_scan_edge": lambda c: c.map_add_scan_edge(scan[:500], prior),
         "so_undistort_points": lambda c: c.undistort_points(scan, prior, api.undistort(d["pose_prev"], 0.1)),
         "so_correspond_edge": lambda c: c.correspond_edge(scan[:256], prior),
+        "so_solve": lambda c: c.solve(*_solve_rows(api, scan[:300], prior)),
     }
 
 
