@@ -110,7 +110,6 @@ struct MotionState {
     int32_t stage;             // so_evaluate_optimized: the first evaluation reports H, g, cost and ends the registration
     int32_t pad;
 };
-static_assert(sizeof(MotionState) % 8 == 0, "copied as 8-byte words");
 
 // The scan so_map_add_registered_scan inserts: d_scan[0..n) in upload order and, unless mode NONE, its times in und.d_time[0..n);
 // the edge cloud so_map_add_registered_edges inserts: d_escan[0..n_edge) and, unless mode NONE, its times in und.d_etime

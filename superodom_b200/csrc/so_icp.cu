@@ -21,6 +21,7 @@
 
 #include "so_icp.cuh"
 #include "so_knn.cuh"
+#include "so_trust_region.cuh"
 
 namespace so {
 
@@ -61,22 +62,9 @@ __device__ __forceinline__ void reduce_to_partials(double acc[kAcc], const Batch
 }
 
 // ------------------------------------------------------------------------------------------------------------------
-// Device-resident optimiser state machine (runs on one thread of the last CTA).
-// Restates ceres::Solve {max_num_iterations=4, DENSE_QR, defaults} of Ceres 2.0.0 as called at LidarSlam.cpp:230-240:
-// TrustRegionMinimizer::Minimize, LevenbergMarquardtStrategy::ComputeStep/StepAccepted/StepRejected and the monotonic
-// TrustRegionStepEvaluator, expressed on the robustified normal equations H = sum rho' J^T J, g = sum rho' J^T r
-// (the QR of [J;D] that DENSE_QR performs solves exactly (H + D^2) y = g).
+// Device-resident optimiser state machine (runs on one thread of the last CTA): the trust-region loop of so_trust_region.cuh
+// over the pose's six tangent columns.
 // ------------------------------------------------------------------------------------------------------------------
-__device__ __noinline__ double grad_max_norm(const double x[7], const double g[6]) {
-    // ||x - Plus(x, -g)||_inf  (TrustRegionMinimizer::EvaluateGradientAndJacobian)
-    double neg[6], xp[7];
-    _Pragma("unroll") for (int j = 0; j < 6; ++j) neg[j] = -g[j];
-    pose_plus(x, neg, xp);
-    double m = 0.0;
-    _Pragma("unroll") for (int i = 0; i < 7; ++i) m = fmax(m, fabs(x[i] - xp[i]));
-    return m;
-}
-
 // ceres::Covariance + EstimateRegistrationError at the end of a registration, on the 32 lanes of the CTA's first warp (S and sc in
 // shared memory).  The 6x6 cyclic Jacobi (at most 30 sweeps, convergence test of jacobi_eig, FP64 angles) takes its rotations in
 // ROUND-ROBIN order: five rounds of three pairs with disjoint indices -- (0,5)(1,4)(2,3) / (0,4)(3,5)(1,2) / (0,3)(2,4)(1,5) /
@@ -190,45 +178,7 @@ __device__ __noinline__ void covariance_and_errors_warp(IcpState& S, CovScratch&
         S.cov[e] = t;
     }
     __syncwarp();
-    // EstimateRegistrationError (LidarSlam.cpp:873-884): 3x3 eigen of the position (lane 0) / orientation (lane 1) blocks
-    if (lane < 2) {
-        double M[9], E[9], e[3];
-        const int o = lane * 3;
-#pragma unroll
-        for (int i = 0; i < 3; ++i)
-#pragma unroll
-            for (int j = 0; j < 3; ++j) M[i * 3 + j] = S.cov[(i + o) * 6 + (j + o)];
-        jacobi_eig<3, 20, true>(M, E, e);
-        // the block is positive semi-definite: below a cut direction its smallest eigenvalue is zero and comes out as +-rounding,
-        // read as 0 (the reference's sqrt of a negative rounding gives NaN; DESIGN.md section 3)
-        const double err = sqrt(e[2]), inv_cond = sqrt(fmax(e[0], 0.0)) / sqrt(e[2]);
-        if (lane == 0) { S.pos_err = err; S.pos_dir[0] = E[2]; S.pos_dir[1] = E[5]; S.pos_dir[2] = E[8]; S.pos_inv_cond = inv_cond; }
-        else { S.ori_err_deg = err / M_PI * 180.0; S.ori_dir[0] = E[2]; S.ori_dir[1] = E[5]; S.ori_dir[2] = E[8]; S.ori_inv_cond = inv_cond; }
-    }
-    __syncwarp();
-}
-
-// End of one ceres::Solve == end of one ICP iteration (LidarSlam.cpp:134-146).
-__device__ __noinline__ void end_solve(IcpState& st) {
-    const int it = st.icp_iter;
-    st.iter_n_surf[it] = st.n_ok - st.n_ok_edge;
-    st.iter_n_edge[it] = st.n_ok_edge;
-    rel_motion(st.x_iter_start, st.x, &st.iter_dtrans[it], &st.iter_drot[it]);      // recordIterationStats (:242-251)
-    st.iter_lm_steps[it] = st.lm_iter;
-    st.iter_lm_successful[it] = st.num_successful;
-    st.iter_lm_termination[it] = st.termination;
-    st.iter_cost[it] = st.cost;
-    st.n_iterations = it + 1;
-    if (st.n_ok == 0 && !st.use_prior) {          // reference: ceres::Covariance CHECK-fails on an empty problem; we stop with a status
-        st.status = SO_STATUS_NO_CORRESPONDENCES; st.phase = PH_DONE; return;
-    }
-    if (st.num_successful == 1 || it == st.max_icp_iters - 1) {      // (:141)
-        st.need_cov = 1;                          // lm_step_body: first warp of the CTA, right after this serial step
-        st.phase = PH_DONE;
-    } else {
-        st.icp_iter = it + 1;
-        st.phase = PH_CORR;
-    }
+    registration_errors(S, lane);
 }
 
 // Reduced system of a degeneracy-aware solve: Hr = B^T H B and gr = B^T g over the columns of B (zero beyond dg.m, so Hr and gr are
@@ -263,97 +213,6 @@ __device__ __noinline__ double grad_max_norm_red(const double x[7], const double
     double m = 0.0;
     _Pragma("unroll") for (int i = 0; i < 7; ++i) m = fmax(m, fabs(x[i] - xp[i]));
     return m;
-}
-
-// TrustRegionMinimizer loop from FinalizeIterationAndCheckIfMinimizerCanContinue up to the next cost evaluation.  RED: the solve on the
-// m columns of dg.B (local parameterisation x [+] B y): Jacobi scaling, LM diagonal and model cost change of the reduced system, which is
-// padded to 6 with identity rows and zero right-hand sides for chol6_solve.
-template <bool RED>
-__device__ __forceinline__ void lm_continue_t(IcpState& st, const DegenState* dg, bool step_successful) {
-    for (;;) {
-        if (step_successful) st.num_successful++; else st.num_unsuccessful++;
-        if (st.lm_iter >= st.lm_max_iterations) { st.termination = 0; end_solve(st); return; }
-        if (st.gmax <= 1e-10) { st.termination = 1; end_solve(st); return; }
-        if (st.radius <= 1e-32) { st.termination = 4; end_solve(st); return; }
-        st.lm_iter++;
-        step_successful = false;
-        // LevenbergMarquardtStrategy::ComputeStep on the Jacobi-scaled system
-        double Hs[36], gs[6];
-        if constexpr (RED) {
-            double Hr[36], gr[6];
-            reduced_system(st, *dg, Hr, gr);
-            _Pragma("unroll") for (int i = 0; i < 6; ++i) {
-                gs[i] = gr[i] * st.scale[i];
-                _Pragma("unroll") for (int j = 0; j < 6; ++j) Hs[i * 6 + j] = Hr[i * 6 + j] * st.scale[i] * st.scale[j];
-            }
-        } else {
-            _Pragma("unroll") for (int i = 0; i < 6; ++i) {
-                gs[i] = st.g[i] * st.scale[i];
-                _Pragma("unroll") for (int j = 0; j < 6; ++j) Hs[i * 6 + j] = st.H[i <= j ? tri(i, j) : tri(j, i)] * st.scale[i] * st.scale[j];
-            }
-        }
-        if (!st.reuse_diagonal)
-            _Pragma("unroll") for (int j = 0; j < 6; ++j) st.diag[j] = fmin(fmax(Hs[j * 6 + j], 1e-6), 1e32);
-        st.reuse_diagonal = 1;
-        double M[36], y[6];
-        _Pragma("unroll") for (int i = 0; i < 36; ++i) M[i] = Hs[i];
-        _Pragma("unroll") for (int j = 0; j < 6; ++j) M[j * 6 + j] += st.diag[j] / st.radius;       // lm_diagonal^2 = diagonal / radius
-        if constexpr (RED) _Pragma("unroll") for (int j = 0; j < 6; ++j) if (j >= dg->m) M[j * 6 + j] = 1.0;
-        bool valid = chol6_solve(M, gs, y);
-        double step[6], mcc = 0.0;
-        if (valid) {
-            _Pragma("unroll") for (int j = 0; j < 6; ++j) { step[j] = -y[j]; valid = valid && isfinite(step[j]); }
-            // model_cost_change = -(J step)'(f + J step / 2) = -step'gs - step'Hs step / 2
-            double sg = 0.0, sHs = 0.0;
-            _Pragma("unroll") for (int i = 0; i < 6; ++i) { sg += step[i] * gs[i]; double t = 0.0; _Pragma("unroll") for (int j = 0; j < 6; ++j) t += Hs[i * 6 + j] * step[j]; sHs += step[i] * t; }
-            mcc = -sg - 0.5 * sHs;
-        }
-        if (!valid || !(mcc > 0.0)) {           // HandleInvalidStep
-            if (++st.consecutive_invalid >= 5) { st.termination = 5; end_solve(st); return; }
-            st.radius *= 0.5; st.reuse_diagonal = 1;
-            continue;
-        }
-        st.consecutive_invalid = 0;
-        st.model_cost_change = mcc;
-        double delta[6];
-        _Pragma("unroll") for (int j = 0; j < 6; ++j) delta[j] = step[j] * st.scale[j];
-        if constexpr (RED) {                    // the ambient step B y
-            double d6[6];
-            _Pragma("unroll") for (int i = 0; i < 6; ++i) { double t = 0.0; _Pragma("unroll") for (int k = 0; k < 6; ++k) t += dg->B[i * 6 + k] * delta[k]; d6[i] = t; }
-            pose_plus(st.x, d6, st.cand);
-        } else {
-            pose_plus(st.x, delta, st.cand);
-        }
-        st.phase = PH_EVAL;
-        return;
-    }
-}
-__device__ __noinline__ void lm_continue(IcpState& st, bool step_successful) { lm_continue_t<false>(st, nullptr, step_successful); }
-__device__ __noinline__ void lm_continue_red(IcpState& st, const DegenState& dg, bool step_successful) { lm_continue_t<true>(st, &dg, step_successful); }
-
-// SE3AbsolutatePoseFactor (factor/SE3AbsolutatePoseFactor.cpp:9-51) added by addAbsolutePoseConstraints (LidarSlam.cpp:285-298):
-// residual [p - p_meas ; 2 vec(q_meas^* q)] times sqrt_information (diagonal here), no loss function; local Jacobian
-// [I 0; 0 (w I + [v]x)] of q_e = q_meas^* q (Utility::Qleft bottom-right block), T_meas = T_w_initial_guess.
-// Adds its J^T J, J^T r and 1/2 r^T r to the 28 reduced sums at pose x.
-__device__ __noinline__ void add_pose_prior(const IcpState& st, const double x[7], double a[kAcc]) {
-    const double qm[4] = {-st.x0[3], -st.x0[4], -st.x0[5], st.x0[6]};
-    double e[4];
-    qmul(qm, x + 3, e);
-    double r[6] = {x[0] - st.x0[0], x[1] - st.x0[1], x[2] - st.x0[2], 2.0 * e[0], 2.0 * e[1], 2.0 * e[2]};
-    double J[36];
-    _Pragma("unroll") for (int i = 0; i < 36; ++i) J[i] = 0.0;
-    J[0] = J[7] = J[14] = 1.0;
-    J[3 * 6 + 3] = e[3];  J[3 * 6 + 4] = -e[2]; J[3 * 6 + 5] = e[1];
-    J[4 * 6 + 3] = e[2];  J[4 * 6 + 4] = e[3];  J[4 * 6 + 5] = -e[0];
-    J[5 * 6 + 3] = -e[1]; J[5 * 6 + 4] = e[0];  J[5 * 6 + 5] = e[3];
-    _Pragma("unroll") for (int i = 0; i < 6; ++i) { r[i] *= st.prior_sqrt_info[i]; _Pragma("unroll") for (int j = 0; j < 6; ++j) J[i * 6 + j] *= st.prior_sqrt_info[i]; }
-    _Pragma("unroll") for (int i = 0; i < 6; ++i) {
-        _Pragma("unroll") for (int j = i; j < 6; ++j) { double t = 0.0; _Pragma("unroll") for (int k = 0; k < 6; ++k) t += J[k * 6 + i] * J[k * 6 + j]; a[tri(i, j)] += t; }
-        double t = 0.0; _Pragma("unroll") for (int k = 0; k < 6; ++k) t += J[k * 6 + i] * r[k];
-        a[21 + i] += t;
-    }
-    double sq = 0.0; _Pragma("unroll") for (int k = 0; k < 6; ++k) sq += r[k] * r[k];
-    a[27] += 0.5 * sq;
 }
 
 // Pseudo-inverse of a symmetric 3x3 with ceres::Covariance's cut rule (covariance_and_errors_warp): eigen-directions with
@@ -431,109 +290,126 @@ __device__ __noinline__ void degeneracy_analysis(const double Hu[21], DegenState
     dg.m = m;
 }
 
-// IterationZero of a new solve, fed by k_fit's reduction.  DEG: the degeneracy-aware solve -- the analysis on H at x_iter_start, then
-// the solve on B's columns when it has fewer than 6 (otherwise exactly the ambient solve).
-template <bool DEG>
-__device__ __forceinline__ void lm_begin_solve_t(IcpState& st, DegenState* dg, const double* acc_in, int n_ok) {
-    double acc[kAcc];
-    _Pragma("unroll") for (int k = 0; k < kAcc; ++k) acc[k] = acc_in[k];
-    if (st.use_prior) {
-        // information diagonal (LidarSlam.cpp:287-294); sqrt by Eigen's unblocked LLT: the first non-positive pivot and
-        // everything after it stay un-square-rooted
-        const double vcf = double(st.prior_vcf);
-        double info[6];
-        const int m1 = max(50, int(n_ok * 0.1)), m2 = max(10, int(n_ok * 0.01));
-        _Pragma("unroll") for (int a = 0; a < 3; ++a) info[a] = (1 - double(st.prior_unc[a])) * m1 * vcf;
-        info[3] = info[4] = m2 * vcf;
-        info[5] = max(5, int(n_ok * 0.001)) * 0;
-        bool failed = false;
-        _Pragma("unroll") for (int k = 0; k < 6; ++k) { if (!failed && info[k] <= 0.0) failed = true; st.prior_sqrt_info[k] = failed ? info[k] : sqrt(info[k]); }
-        add_pose_prior(st, st.x, acc);
-    }
-    _Pragma("unroll") for (int k = 0; k < 21; ++k) st.H[k] = acc[k];
-    _Pragma("unroll") for (int k = 0; k < 6; ++k) st.g[k] = acc[21 + k];
-    st.cost = acc[27];
-    st.n_ok = n_ok;
-    _Pragma("unroll") for (int i = 0; i < 7; ++i) st.x_iter_start[i] = st.x[i];
-    st.lm_iter = 0; st.num_successful = 0; st.num_unsuccessful = 0; st.consecutive_invalid = 0; st.termination = 0;
-    if (n_ok == 0 && !st.use_prior) { st.termination = 6; end_solve(st); return; }
-    if (!isfinite(st.cost)) {
-        // A row's loss weight is not finite (ScaledLoss(TukeyLoss, w) with w = NaN: a line fit on an exactly collinear neighbourhood,
-        // whose mean squared distance is rounding noise of either sign).  The reference CHECK-fails in ceres::Corrector here (Ceres
-        // 2.0 corrector.cc: neither rho'' <= 0 nor rho' > 0 holds for NaN) and ends the process; the registration stops with a status
-        // and the pose this ICP iteration started from (DESIGN.md section 3).
-        const int it = st.icp_iter;
-        st.iter_n_surf[it] = n_ok - st.n_ok_edge; st.iter_n_edge[it] = st.n_ok_edge; st.iter_cost[it] = st.cost;
-        st.n_iterations = it + 1;
-        st.status = SO_STATUS_INVALID_EVALUATION; st.phase = PH_DONE;
-        return;
-    }
-    bool red = false;
-    if constexpr (DEG) {
-        degeneracy_analysis(st.H, *dg);
-        dg->iter_n_flag_pos[st.icp_iter] = __popc(dg->flags_pos);
-        dg->iter_n_flag_ori[st.icp_iter] = __popc(dg->flags_ori);
-        red = dg->m < 6;
-    }
-    if (red) {
-        double Hr[36], gr[6];
-        reduced_system(st, *dg, Hr, gr);
-        _Pragma("unroll") for (int j = 0; j < 6; ++j) st.scale[j] = 1.0 / (1.0 + sqrt(Hr[j * 6 + j]));      // over B's columns
-    } else {
-        _Pragma("unroll") for (int j = 0; j < 6; ++j) st.scale[j] = 1.0 / (1.0 + sqrt(st.H[tri(j, j)]));      // jacobi_scaling at iteration 0
-    }
-    double xn = 0.0; _Pragma("unroll") for (int i = 0; i < 7; ++i) xn += st.x[i] * st.x[i];
-    st.x_norm = sqrt(xn);
-    st.gmax = red ? grad_max_norm_red(st.x, st.g, *dg) : grad_max_norm(st.x, st.g);
-    st.radius = 1e4; st.decrease_factor = 2.0; st.reuse_diagonal = 0;
-    if (red) lm_continue_red(st, *dg, false);
-    else lm_continue(st, false);
-}
-__device__ __noinline__ void lm_begin_solve(IcpState& st, const double* acc_in, int n_ok) { lm_begin_solve_t<false>(st, nullptr, acc_in, n_ok); }
-__device__ __noinline__ void lm_begin_solve_deg(IcpState& st, DegenState& dg, const double* acc_in, int n_ok) { lm_begin_solve_t<true>(st, &dg, acc_in, n_ok); }
+__device__ __noinline__ void lm_continue(IcpState& st, bool step_successful);
+__device__ __noinline__ void lm_continue_red(IcpState& st, const DegenState& dg, bool step_successful);
 
-// After the cost (and H, g) at the candidate are known.  RED: of a solve on B's columns.
-template <bool RED>
-__device__ __forceinline__ void lm_after_eval_t(IcpState& st, const DegenState* dg, const double* acc_in) {
-    double acc[kAcc];
-    _Pragma("unroll") for (int k = 0; k < kAcc; ++k) acc[k] = acc_in[k];
-    if (st.use_prior) add_pose_prior(st, st.cand, acc);
-    const double cand_cost = acc[27];
-    // ParameterToleranceReached
-    double sn = 0.0; _Pragma("unroll") for (int i = 0; i < 7; ++i) { const double d = st.x[i] - st.cand[i]; sn += d * d; }
-    sn = sqrt(sn);
-    if (sn <= 1e-8 * (st.x_norm + 1e-8)) { st.termination = 2; end_solve(st); return; }
-    // FunctionToleranceReached
-    const double cost_change = st.cost - cand_cost;
-    if (fabs(cost_change) <= 1e-6 * st.cost) { st.termination = 3; end_solve(st); return; }
-    const double rd = cost_change / st.model_cost_change;
-    if (rd > 1e-3) {        // HandleSuccessfulStep
-        _Pragma("unroll") for (int i = 0; i < 7; ++i) st.x[i] = st.cand[i];
-        double xn = 0.0; _Pragma("unroll") for (int i = 0; i < 7; ++i) xn += st.x[i] * st.x[i];
-        st.x_norm = sqrt(xn);
+// The SE3 prior of addAbsolutePoseConstraints (LidarSlam.cpp:285-298) on the pose x, T_meas = T_w_initial_guess
+__device__ __noinline__ void add_pose_prior(const IcpState& st, const double x[7], double a[kAcc]) {
+    add_se3_prior<6>(st.x0, st.prior_sqrt_info, x, a);
+}
+
+// The six-column solve on the pose (x [+] delta): H, g, scale and diag in IcpState; the prior rows on x when use_prior
+struct Ambient {
+    static constexpr int N = 6, kSums = kAcc;
+    static constexpr bool kAnyNonFinite = true;
+    IcpState& st;
+    __device__ __forceinline__ double* scale() const { return st.scale; }
+    __device__ __forceinline__ double* diag() const { return st.diag; }
+    __device__ __forceinline__ void take(const double* acc) const {
         _Pragma("unroll") for (int k = 0; k < 21; ++k) st.H[k] = acc[k];
         _Pragma("unroll") for (int k = 0; k < 6; ++k) st.g[k] = acc[21 + k];
-        st.cost = cand_cost;
-        if constexpr (RED) st.gmax = grad_max_norm_red(st.x, st.g, *dg);
-        else st.gmax = grad_max_norm(st.x, st.g);
-        const double t = 2.0 * rd - 1.0;
-        st.radius = st.radius / fmax(1.0 / 3.0, 1.0 - t * t * t);
-        st.radius = fmin(1e16, st.radius);
-        st.decrease_factor = 2.0; st.reuse_diagonal = 0;
-        if constexpr (RED) lm_continue_red(st, *dg, true);
-        else lm_continue(st, true);
-    } else {                // StepRejected
-        st.radius = st.radius / st.decrease_factor; st.decrease_factor *= 2.0; st.reuse_diagonal = 1;
-        if constexpr (RED) lm_continue_red(st, *dg, false);
-        else lm_continue(st, false);
     }
+    __device__ __forceinline__ void open_prior(double* acc, int n_ok) const {
+        if (st.use_prior) {
+            // information diagonal (LidarSlam.cpp:287-294); sqrt by Eigen's unblocked LLT: the first non-positive pivot and everything
+            // after it stay un-square-rooted
+            const double vcf = double(st.prior_vcf);
+            double info[6];
+            const int m1 = max(50, int(n_ok * 0.1)), m2 = max(10, int(n_ok * 0.01));
+            _Pragma("unroll") for (int a = 0; a < 3; ++a) info[a] = (1 - double(st.prior_unc[a])) * m1 * vcf;
+            info[3] = info[4] = m2 * vcf;
+            info[5] = max(5, int(n_ok * 0.001)) * 0;
+            bool failed = false;
+            _Pragma("unroll") for (int k = 0; k < 6; ++k) { if (!failed && info[k] <= 0.0) failed = true; st.prior_sqrt_info[k] = failed ? info[k] : sqrt(info[k]); }
+            add_pose_prior(st, st.x, acc);
+        }
+    }
+    __device__ __forceinline__ void prior_at_candidate(double* acc) const { if (st.use_prior) add_pose_prior(st, st.cand, acc); }
+    __device__ __forceinline__ void init_scale() const {
+        _Pragma("unroll") for (int j = 0; j < 6; ++j) st.scale[j] = 1.0 / (1.0 + sqrt(st.H[tri(j, j)]));
+    }
+    __device__ __forceinline__ void scaled_system(double* Hs, double* gs) const {
+        _Pragma("unroll") for (int i = 0; i < 6; ++i) {
+            gs[i] = st.g[i] * st.scale[i];
+            _Pragma("unroll") for (int j = 0; j < 6; ++j) Hs[i * 6 + j] = st.H[i <= j ? tri(i, j) : tri(j, i)] * st.scale[i] * st.scale[j];
+        }
+    }
+    __device__ __forceinline__ void pad(double*) const {}
+    __device__ __forceinline__ double x_norm2() const {
+        double xn = 0.0; _Pragma("unroll") for (int i = 0; i < 7; ++i) xn += st.x[i] * st.x[i];
+        return xn;
+    }
+    __device__ __forceinline__ double step_norm2() const {
+        double sn = 0.0; _Pragma("unroll") for (int i = 0; i < 7; ++i) { const double d = st.x[i] - st.cand[i]; sn += d * d; }
+        return sn;
+    }
+    __device__ __forceinline__ void accept() const { _Pragma("unroll") for (int i = 0; i < 7; ++i) st.x[i] = st.cand[i]; }
+    __device__ __forceinline__ double gmax() const { return grad_max_norm(st.x, st.g); }
+    __device__ __forceinline__ void candidate(const double* delta) const { pose_plus(st.x, delta, st.cand); }
+    __device__ __forceinline__ void next(bool step_successful) const { lm_continue(st, step_successful); }
+};
+
+// The degeneracy-aware solve on the m < 6 columns of dg.B (local parameterisation x [+] B y): Jacobi scaling, LM diagonal and model
+// cost change of the reduced system, which is padded to 6 with identity rows and zero right-hand sides for chol_solve<6>
+struct Reduced : Ambient {
+    const DegenState& dg;
+    __device__ __forceinline__ void init_scale() const {
+        double Hr[36], gr[6];
+        reduced_system(st, dg, Hr, gr);
+        _Pragma("unroll") for (int j = 0; j < 6; ++j) st.scale[j] = 1.0 / (1.0 + sqrt(Hr[j * 6 + j]));
+    }
+    __device__ __forceinline__ void scaled_system(double* Hs, double* gs) const {
+        double Hr[36], gr[6];
+        reduced_system(st, dg, Hr, gr);
+        _Pragma("unroll") for (int i = 0; i < 6; ++i) {
+            gs[i] = gr[i] * st.scale[i];
+            _Pragma("unroll") for (int j = 0; j < 6; ++j) Hs[i * 6 + j] = Hr[i * 6 + j] * st.scale[i] * st.scale[j];
+        }
+    }
+    __device__ __forceinline__ void pad(double* M) const { _Pragma("unroll") for (int j = 0; j < 6; ++j) if (j >= dg.m) M[j * 6 + j] = 1.0; }
+    __device__ __forceinline__ double gmax() const { return grad_max_norm_red(st.x, st.g, dg); }
+    __device__ __forceinline__ void candidate(const double* delta) const {      // the ambient step B y
+        double d6[6];
+        _Pragma("unroll") for (int i = 0; i < 6; ++i) { double t = 0.0; _Pragma("unroll") for (int k = 0; k < 6; ++k) t += dg.B[i * 6 + k] * delta[k]; d6[i] = t; }
+        pose_plus(st.x, d6, st.cand);
+    }
+    __device__ __forceinline__ void next(bool step_successful) const { lm_continue_red(st, dg, step_successful); }
+};
+
+// IterationZero's tail in the degeneracy-aware solve: on B's columns when the analysis left fewer than 6, else the ambient one
+struct DegStart : Ambient {
+    const DegenState& dg;
+    bool red;
+    __device__ __forceinline__ void init_scale() const { if (red) Reduced{{st}, dg}.init_scale(); else Ambient::init_scale(); }
+    __device__ __forceinline__ double gmax() const { return red ? grad_max_norm_red(st.x, st.g, dg) : grad_max_norm(st.x, st.g); }
+    __device__ __forceinline__ void next(bool step_successful) const { if (red) lm_continue_red(st, dg, step_successful); else lm_continue(st, step_successful); }
+};
+
+__device__ __noinline__ void lm_continue(IcpState& st, bool step_successful) { tr_continue(Ambient{st}, step_successful); }
+__device__ __noinline__ void lm_continue_red(IcpState& st, const DegenState& dg, bool step_successful) { tr_continue(Reduced{{st}, dg}, step_successful); }
+
+// IterationZero of a new solve, fed by k_fit's reduction
+__device__ __noinline__ void lm_begin_solve(IcpState& st, const double* acc_in, int n_ok) {
+    tr_begin_solve(Ambient{st}, acc_in, n_ok, [&] { tr_start(Ambient{st}); });
 }
-__device__ __noinline__ void lm_after_eval(IcpState& st, const double* acc_in) { lm_after_eval_t<false>(st, nullptr, acc_in); }
+// ... of the degeneracy-aware solve: the analysis on H at x_iter_start, then the solve on B's columns when it has fewer than 6
+// (otherwise exactly the ambient solve)
+__device__ __noinline__ void lm_begin_solve_deg(IcpState& st, DegenState& dg, const double* acc_in, int n_ok) {
+    tr_begin_solve(Ambient{st}, acc_in, n_ok, [&] {
+        degeneracy_analysis(st.H, dg);
+        dg.iter_n_flag_pos[st.icp_iter] = __popc(dg.flags_pos);
+        dg.iter_n_flag_ori[st.icp_iter] = __popc(dg.flags_ori);
+        tr_start(DegStart{{st}, dg, dg.m < 6});
+    });
+}
+
+// After the cost (and H, g) at the candidate are known
+__device__ __noinline__ void lm_after_eval(IcpState& st, const double* acc_in) { tr_after_eval(Ambient{st}, acc_in); }
 // the degeneracy-aware solve's: on B's columns when it has fewer than 6, else the ambient step (its own copy: a third caller of
 // lm_after_eval changes that function's code in the other kernels)
 __device__ __noinline__ void lm_after_eval_deg(IcpState& st, const DegenState& dg, const double* acc_in) {
-    if (dg.m < 6) lm_after_eval_t<true>(st, &dg, acc_in);
-    else lm_after_eval_t<false>(st, nullptr, acc_in);
+    if (dg.m < 6) tr_after_eval(Reduced{{st}, dg}, acc_in);
+    else tr_after_eval(Ambient{st}, acc_in);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -1643,19 +1519,12 @@ __device__ __forceinline__ void lm_step_body(const BatchView& bv, int s, uint32_
     // one working thread was a dependent L2 round trip (the step took 5-12 us, the covariance 40 us); the copy in and out is two
     // coalesced passes of the CTA.
     __shared__ IcpState s_st;
-    static_assert(sizeof(IcpState) % 8 == 0, "copied as 8-byte words");
-    {
-        const unsigned long long* src = reinterpret_cast<const unsigned long long*>(st);
-        unsigned long long* dst = reinterpret_cast<unsigned long long*>(&s_st);
-        for (uint32_t k = threadIdx.x; k < sizeof(IcpState) / 8; k += blockDim.x) dst[k] = src[k];
-    }
+    cta_copy(&s_st, st);
     DegenState* sdg = nullptr;                             // the DegenState's shared copy, the same way
     if constexpr (DEG) {
         __shared__ DegenState s_dg;
         sdg = &s_dg;
-        const unsigned long long* src = reinterpret_cast<const unsigned long long*>(dg + s);
-        unsigned long long* dst = reinterpret_cast<unsigned long long*>(&s_dg);
-        for (uint32_t k = threadIdx.x; k < sizeof(DegenState) / 8; k += blockDim.x) dst[k] = src[k];
+        cta_copy(sdg, dg + s);
     }
     __syncthreads();
     if (threadIdx.x < kAcc) s_sum[threadIdx.x] = (s_red[0][threadIdx.x] + s_red[1][threadIdx.x]) + (s_red[2][threadIdx.x] + s_red[3][threadIdx.x]);
@@ -1691,16 +1560,8 @@ __device__ __forceinline__ void lm_step_body(const BatchView& bv, int s, uint32_
         if (threadIdx.x < 32) covariance_and_errors_warp(s_st, s_cov);      // need_cov stays set: the state is re-initialised per registration
         __syncthreads();
     }
-    {
-        const unsigned long long* src = reinterpret_cast<const unsigned long long*>(&s_st);
-        unsigned long long* dst = reinterpret_cast<unsigned long long*>(st);
-        for (uint32_t k = threadIdx.x; k < sizeof(IcpState) / 8; k += blockDim.x) dst[k] = src[k];
-    }
-    if constexpr (DEG) {
-        const unsigned long long* src = reinterpret_cast<const unsigned long long*>(sdg);
-        unsigned long long* dst = reinterpret_cast<unsigned long long*>(dg + s);
-        for (uint32_t k = threadIdx.x; k < sizeof(DegenState) / 8; k += blockDim.x) dst[k] = src[k];
-    }
+    cta_copy(st, &s_st);
+    if constexpr (DEG) cta_copy(dg + s, sdg);
 }
 
 template <int AFTER>
@@ -1727,13 +1588,11 @@ void launch_degeneracy_analysis(const IcpState* st, DegenState* dg, cudaStream_t
 __global__ void __launch_bounds__(32) k_covariance(IcpState* st) {
     __shared__ IcpState s_st;
     __shared__ CovScratch s_cov;
-    unsigned long long* sh = reinterpret_cast<unsigned long long*>(&s_st);
-    unsigned long long* gl = reinterpret_cast<unsigned long long*>(st);
-    for (uint32_t k = threadIdx.x; k < sizeof(IcpState) / 8; k += blockDim.x) sh[k] = gl[k];
+    cta_copy(&s_st, st);
     __syncthreads();
     covariance_and_errors_warp(s_st, s_cov);
     __syncthreads();
-    for (uint32_t k = threadIdx.x; k < sizeof(IcpState) / 8; k += blockDim.x) gl[k] = sh[k];
+    cta_copy(st, &s_st);
 }
 
 void launch_covariance(IcpState* st, cudaStream_t stream) { k_covariance<<<1, 32, 0, stream>>>(st); }

@@ -20,11 +20,10 @@
 #include <cmath>
 #include <vector>
 
+#include "so_trust_region.cuh"
 #include "so_undistort.cuh"
 
 namespace so {
-
-__host__ __device__ inline int tri12(int i, int j) { return i * 12 - (i * (i - 1)) / 2 + (j - i); }
 
 // sh = {q_D[4] normalised, t_D[3], theta, 1 / sin(theta)} of a motion D, rounded as und_setup rounds
 __device__ __forceinline__ void motion_setup(const double D[7], double sh[9]) {
@@ -346,25 +345,19 @@ __global__ void __launch_bounds__(kThreads) k_motion_eval_edge(BatchView bv, Edg
 }
 
 // ------------------------------------------------------------------------------------------------------------------ step
-// The trust-region loop of so_icp.cu (lm_begin_solve / lm_continue / lm_after_eval / end_solve) over the 12 tangent columns of
-// (T, D): Jacobi scaling and the LM diagonal over 12 columns, x_norm and the step norm over the 14 ambient values, the gradient
-// max-norm through Plus of both blocks.  Runs on one thread, on shared-memory copies of the two states.
-__device__ __noinline__ void m_end_solve(IcpState& st) {
-    const int it = st.icp_iter;
-    st.iter_n_surf[it] = st.n_ok - st.n_ok_edge;
-    st.iter_n_edge[it] = st.n_ok_edge;
-    rel_motion(st.x_iter_start, st.x, &st.iter_dtrans[it], &st.iter_drot[it]);
-    st.iter_lm_steps[it] = st.lm_iter;
-    st.iter_lm_successful[it] = st.num_successful;
-    st.iter_lm_termination[it] = st.termination;
-    st.iter_cost[it] = st.cost;
-    st.n_iterations = it + 1;
-    if (st.n_ok == 0) { st.status = SO_STATUS_NO_CORRESPONDENCES; st.phase = PH_DONE; return; }     // the prior rows are zero then
-    if (st.num_successful == 1 || it == st.max_icp_iters - 1) { st.need_cov = 1; st.phase = PH_DONE; }
-    else { st.icp_iter = it + 1; st.phase = PH_CORR; }
+// The trust-region loop of so_trust_region.cuh over the 12 tangent columns of (T, D): Jacobi scaling and the LM diagonal over 12
+// columns, x_norm and the step norm over the 14 ambient values, the gradient max-norm through Plus of both blocks, the prior rows
+// on D.  Runs on one thread, on shared-memory copies of the two states.
+__device__ __noinline__ void lm_continue(IcpState& st, MotionState& M, bool step_successful);
+
+// SE3AbsolutatePoseFactor on D, multiplier sqrt(n_ok * info_k), measurement D0
+__device__ __noinline__ void add_motion_prior(const MotionState& M, const double D[7], double a[kMotionAcc]) {
+    add_se3_prior<12>(M.D0, M.sqrt_info, D, a);
 }
 
-__device__ __noinline__ double m_gmax(const IcpState& S, const MotionState& M) {
+// ||(x, D) - Plus((x, D), -g)||_inf over both blocks in one function (the larger of two grad_max_norm calls differs from it in the
+// last bits of some solves' gmax)
+__device__ __noinline__ double grad_max_norm(const IcpState& S, const MotionState& M) {
     double nt[6], nd[6], xp[7], dp[7];
     for (int j = 0; j < 6; ++j) { nt[j] = -M.g[j]; nd[j] = -M.g[6 + j]; }
     pose_plus(S.x, nt, xp);
@@ -374,153 +367,56 @@ __device__ __noinline__ double m_gmax(const IcpState& S, const MotionState& M) {
     return m;
 }
 
-// SE3AbsolutatePoseFactor on D (add_pose_prior's rows, columns 6..11)
-__device__ __noinline__ void m_add_prior(const MotionState& M, const double D[7], double a[kMotionAcc]) {
-    const double qm[4] = {-M.D0[3], -M.D0[4], -M.D0[5], M.D0[6]};
-    double e[4];
-    qmul(qm, D + 3, e);
-    double r[6] = {D[0] - M.D0[0], D[1] - M.D0[1], D[2] - M.D0[2], 2.0 * e[0], 2.0 * e[1], 2.0 * e[2]};
-    double J[36];
-    for (int i = 0; i < 36; ++i) J[i] = 0.0;
-    J[0] = J[7] = J[14] = 1.0;
-    J[3 * 6 + 3] = e[3];  J[3 * 6 + 4] = -e[2]; J[3 * 6 + 5] = e[1];
-    J[4 * 6 + 3] = e[2];  J[4 * 6 + 4] = e[3];  J[4 * 6 + 5] = -e[0];
-    J[5 * 6 + 3] = -e[1]; J[5 * 6 + 4] = e[0];  J[5 * 6 + 5] = e[3];
-    for (int i = 0; i < 6; ++i) { r[i] *= M.sqrt_info[i]; for (int j = 0; j < 6; ++j) J[i * 6 + j] *= M.sqrt_info[i]; }
-    for (int i = 0; i < 6; ++i) {
-        for (int j = i; j < 6; ++j) { double t = 0.0; for (int k = 0; k < 6; ++k) t += J[k * 6 + i] * J[k * 6 + j]; a[tri12(6 + i, 6 + j)] += t; }
-        double t = 0.0; for (int k = 0; k < 6; ++k) t += J[k * 6 + i] * r[k];
-        a[78 + 6 + i] += t;
+struct TwoBlock {
+    static constexpr int N = 12, kSums = kMotionAcc;
+    // only with line rows (n_ok_edge > 0) does a non-finite first cost stop the registration; so_solve_optimized's caller-given
+    // plane rows with a non-finite cost run the solve on
+    static constexpr bool kAnyNonFinite = false;
+    IcpState& st;
+    MotionState& M;
+    __device__ __forceinline__ double* scale() const { return M.scale; }
+    __device__ __forceinline__ double* diag() const { return M.diag; }
+    __device__ __forceinline__ void take(const double* acc) const {
+        for (int k = 0; k < 78; ++k) M.H[k] = acc[k];
+        for (int k = 0; k < 12; ++k) M.g[k] = acc[78 + k];
     }
-    double sq = 0.0; for (int k = 0; k < 6; ++k) sq += r[k] * r[k];
-    a[90] += 0.5 * sq;
-}
-
-// Cholesky solve of the SPD 12x12 M y = r (M full row-major, destroyed); false on a non-positive pivot
-__device__ __noinline__ bool chol12_solve(double* M, const double* r, double* y) {
-    double inv[12], z[12];
-#pragma unroll 1
-    for (int j = 0; j < 12; ++j) {
-        double s = M[j * 12 + j];
-        for (int k = 0; k < j; ++k) s -= M[j * 12 + k] * M[j * 12 + k];
-        if (!(s > 0.0)) return false;
-        const double il = rsqrt(s);
-        inv[j] = il;
-        M[j * 12 + j] = s * il;
-#pragma unroll 1
-        for (int i = j + 1; i < 12; ++i) {
-            double t = M[i * 12 + j];
-            for (int k = 0; k < j; ++k) t -= M[i * 12 + k] * M[j * 12 + k];
-            M[i * 12 + j] = t * il;
-        }
+    __device__ __forceinline__ void open_prior(double* acc, int n_ok) const {
+        for (int k = 0; k < 6; ++k) M.sqrt_info[k] = sqrt(double(n_ok) * M.info[k]);
+        add_motion_prior(M, M.D, acc);
     }
-#pragma unroll 1
-    for (int i = 0; i < 12; ++i) { double t = r[i]; for (int k = 0; k < i; ++k) t -= M[i * 12 + k] * z[k]; z[i] = t * inv[i]; }
-#pragma unroll 1
-    for (int i = 11; i >= 0; --i) { double t = z[i]; for (int k = i + 1; k < 12; ++k) t -= M[k * 12 + i] * y[k]; y[i] = t * inv[i]; }
-    return true;
-}
-
-__device__ __noinline__ void m_lm_continue(IcpState& st, MotionState& M, bool step_successful) {
-    for (;;) {
-        if (step_successful) st.num_successful++; else st.num_unsuccessful++;
-        if (st.lm_iter >= st.lm_max_iterations) { st.termination = 0; m_end_solve(st); return; }
-        if (st.gmax <= 1e-10) { st.termination = 1; m_end_solve(st); return; }
-        if (st.radius <= 1e-32) { st.termination = 4; m_end_solve(st); return; }
-        st.lm_iter++;
-        step_successful = false;
-        double Hs[144], gs[12], A[144], y[12];
+    __device__ __forceinline__ void prior_at_candidate(double* acc) const { add_motion_prior(M, M.Dc, acc); }
+    __device__ __forceinline__ void init_scale() const { for (int j = 0; j < 12; ++j) M.scale[j] = 1.0 / (1.0 + sqrt(M.H[tri12(j, j)])); }
+    __device__ __forceinline__ void scaled_system(double* Hs, double* gs) const {
         for (int i = 0; i < 12; ++i) {
             gs[i] = M.g[i] * M.scale[i];
             for (int j = 0; j < 12; ++j) Hs[i * 12 + j] = M.H[i <= j ? tri12(i, j) : tri12(j, i)] * M.scale[i] * M.scale[j];
         }
-        if (!st.reuse_diagonal) for (int j = 0; j < 12; ++j) M.diag[j] = fmin(fmax(Hs[j * 12 + j], 1e-6), 1e32);
-        st.reuse_diagonal = 1;
-        for (int i = 0; i < 144; ++i) A[i] = Hs[i];
-        for (int j = 0; j < 12; ++j) A[j * 12 + j] += M.diag[j] / st.radius;
-        bool valid = chol12_solve(A, gs, y);
-        double step[12], mcc = 0.0;
-        if (valid) {
-            double sg = 0.0, sHs = 0.0;
-            for (int j = 0; j < 12; ++j) { step[j] = -y[j]; valid = valid && isfinite(step[j]); }
-            for (int i = 0; i < 12; ++i) { sg += step[i] * gs[i]; double t = 0.0; for (int j = 0; j < 12; ++j) t += Hs[i * 12 + j] * step[j]; sHs += step[i] * t; }
-            mcc = -sg - 0.5 * sHs;
-        }
-        if (!valid || !(mcc > 0.0)) {
-            if (++st.consecutive_invalid >= 5) { st.termination = 5; m_end_solve(st); return; }
-            st.radius *= 0.5; st.reuse_diagonal = 1;
-            continue;
-        }
-        st.consecutive_invalid = 0;
-        st.model_cost_change = mcc;
-        double dT[6], dD[6];
-        for (int j = 0; j < 6; ++j) { dT[j] = step[j] * M.scale[j]; dD[j] = step[6 + j] * M.scale[6 + j]; }
-        pose_plus(st.x, dT, st.cand);
-        pose_plus(M.D, dD, M.Dc);
-        st.phase = PH_EVAL;
-        return;
     }
-}
-
-__device__ __noinline__ void m_begin_solve(IcpState& st, MotionState& M, const double* acc_in, int n_ok) {
-    double acc[kMotionAcc];
-    for (int k = 0; k < kMotionAcc; ++k) acc[k] = acc_in[k];
-    for (int k = 0; k < 6; ++k) M.sqrt_info[k] = sqrt(double(n_ok) * M.info[k]);
-    m_add_prior(M, M.D, acc);
-    for (int k = 0; k < 78; ++k) M.H[k] = acc[k];
-    for (int k = 0; k < 12; ++k) M.g[k] = acc[78 + k];
-    st.cost = acc[90];
-    st.n_ok = n_ok;
-    for (int i = 0; i < 7; ++i) st.x_iter_start[i] = st.x[i];
-    st.lm_iter = 0; st.num_successful = 0; st.num_unsuccessful = 0; st.consecutive_invalid = 0; st.termination = 0;
-    if (n_ok == 0) { st.termination = 6; m_end_solve(st); return; }
-    if (st.n_ok_edge > 0 && !isfinite(st.cost)) {
-        // a NaN-weighted line row: the rule of lm_begin_solve (so_icp.cu) -- the registration stops with a status and the pose this
-        // ICP iteration started from
-        const int it = st.icp_iter;
-        st.iter_n_surf[it] = n_ok - st.n_ok_edge; st.iter_n_edge[it] = st.n_ok_edge; st.iter_cost[it] = st.cost;
-        st.n_iterations = it + 1;
-        st.status = SO_STATUS_INVALID_EVALUATION; st.phase = PH_DONE;
-        return;
-    }
-    for (int j = 0; j < 12; ++j) M.scale[j] = 1.0 / (1.0 + sqrt(M.H[tri12(j, j)]));
-    double xn = 0.0;
-    for (int i = 0; i < 7; ++i) xn += st.x[i] * st.x[i] + M.D[i] * M.D[i];
-    st.x_norm = sqrt(xn);
-    st.gmax = m_gmax(st, M);
-    st.radius = 1e4; st.decrease_factor = 2.0; st.reuse_diagonal = 0;
-    m_lm_continue(st, M, false);
-}
-
-__device__ __noinline__ void m_after_eval(IcpState& st, MotionState& M, const double* acc_in) {
-    double acc[kMotionAcc];
-    for (int k = 0; k < kMotionAcc; ++k) acc[k] = acc_in[k];
-    m_add_prior(M, M.Dc, acc);
-    const double cand_cost = acc[90];
-    double sn = 0.0;
-    for (int i = 0; i < 7; ++i) { const double a = st.x[i] - st.cand[i], b = M.D[i] - M.Dc[i]; sn += a * a + b * b; }
-    sn = sqrt(sn);
-    if (sn <= 1e-8 * (st.x_norm + 1e-8)) { st.termination = 2; m_end_solve(st); return; }
-    const double cost_change = st.cost - cand_cost;
-    if (fabs(cost_change) <= 1e-6 * st.cost) { st.termination = 3; m_end_solve(st); return; }
-    const double rd = cost_change / st.model_cost_change;
-    if (rd > 1e-3) {
+    __device__ __forceinline__ void pad(double*) const {}
+    __device__ __forceinline__ double x_norm2() const {      // pairwise in i, as step_norm2
         double xn = 0.0;
-        for (int i = 0; i < 7; ++i) { st.x[i] = st.cand[i]; M.D[i] = M.Dc[i]; xn += st.x[i] * st.x[i] + M.D[i] * M.D[i]; }
-        st.x_norm = sqrt(xn);
-        for (int k = 0; k < 78; ++k) M.H[k] = acc[k];
-        for (int k = 0; k < 12; ++k) M.g[k] = acc[78 + k];
-        st.cost = cand_cost;
-        st.gmax = m_gmax(st, M);
-        const double t = 2.0 * rd - 1.0;
-        st.radius = fmin(1e16, st.radius / fmax(1.0 / 3.0, 1.0 - t * t * t));
-        st.decrease_factor = 2.0; st.reuse_diagonal = 0;
-        m_lm_continue(st, M, true);
-    } else {
-        st.radius = st.radius / st.decrease_factor; st.decrease_factor *= 2.0; st.reuse_diagonal = 1;
-        m_lm_continue(st, M, false);
+        for (int i = 0; i < 7; ++i) xn += st.x[i] * st.x[i] + M.D[i] * M.D[i];
+        return xn;
     }
+    __device__ __forceinline__ double step_norm2() const {
+        double sn = 0.0;
+        for (int i = 0; i < 7; ++i) { const double a = st.x[i] - st.cand[i], b = M.D[i] - M.Dc[i]; sn += a * a + b * b; }
+        return sn;
+    }
+    __device__ __forceinline__ void accept() const { for (int i = 0; i < 7; ++i) { st.x[i] = st.cand[i]; M.D[i] = M.Dc[i]; } }
+    __device__ __forceinline__ double gmax() const { return grad_max_norm(st, M); }
+    __device__ __forceinline__ void candidate(const double* delta) const {
+        pose_plus(st.x, delta, st.cand);
+        pose_plus(M.D, delta + 6, M.Dc);
+    }
+    __device__ __forceinline__ void next(bool step_successful) const { lm_continue(st, M, step_successful); }
+};
+
+__device__ __noinline__ void lm_continue(IcpState& st, MotionState& M, bool step_successful) { tr_continue(TwoBlock{st, M}, step_successful); }
+__device__ __noinline__ void lm_begin_solve(IcpState& st, MotionState& M, const double* acc_in, int n_ok) {
+    tr_begin_solve(TwoBlock{st, M}, acc_in, n_ok, [&] { tr_start(TwoBlock{st, M}); });
 }
+__device__ __noinline__ void lm_after_eval(IcpState& st, MotionState& M, const double* acc_in) { tr_after_eval(TwoBlock{st, M}, acc_in); }
 
 // ceres::Covariance{apply_loss_function, DENSE_SVD} over the 12 tangent columns on the CTA's first warp: cyclic Jacobi of H (each
 // rotation's angle on lane 0, the rows of H on lanes 0-11, of the eigenvectors on lanes 12-23, the 2x2 block on lane 24), the
@@ -603,16 +499,7 @@ __device__ __noinline__ void cov12_warp(IcpState& S, const MotionState& M, Cov12
         S.cov[e] = t;
     }
     __syncwarp();
-    if (lane < 2) {
-        double Mx[9], E[9], ev[3];
-        const int o = lane * 3;
-        for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) Mx[i * 3 + j] = S.cov[(i + o) * 6 + (j + o)];
-        jacobi_eig<3, 20, true>(Mx, E, ev);
-        const double err = sqrt(ev[2]), inv_cond = sqrt(fmax(ev[0], 0.0)) / sqrt(ev[2]);     // as covariance_and_errors_warp
-        if (lane == 0) { S.pos_err = err; S.pos_dir[0] = E[2]; S.pos_dir[1] = E[5]; S.pos_dir[2] = E[8]; S.pos_inv_cond = inv_cond; }
-        else { S.ori_err_deg = err / M_PI * 180.0; S.ori_dir[0] = E[2]; S.ori_dir[1] = E[5]; S.ori_dir[2] = E[8]; S.ori_inv_cond = inv_cond; }
-    }
-    __syncwarp();
+    registration_errors(S, lane);
 }
 
 // so_covariance (12 columns): cov12_warp on ms->H, in one 32-thread CTA and shared copies of both blocks as k_motion_step runs it
@@ -620,16 +507,12 @@ __global__ void __launch_bounds__(32) k_covariance12(IcpState* st, const MotionS
     __shared__ IcpState s_st;
     __shared__ MotionState s_m;
     __shared__ Cov12 s_cov;
-    unsigned long long* sh = reinterpret_cast<unsigned long long*>(&s_st);
-    unsigned long long* gl = reinterpret_cast<unsigned long long*>(st);
-    for (uint32_t k = threadIdx.x; k < sizeof(IcpState) / 8; k += blockDim.x) sh[k] = gl[k];
-    const unsigned long long* gm = reinterpret_cast<const unsigned long long*>(ms);
-    unsigned long long* sm = reinterpret_cast<unsigned long long*>(&s_m);
-    for (uint32_t k = threadIdx.x; k < sizeof(MotionState) / 8; k += blockDim.x) sm[k] = gm[k];
+    cta_copy(&s_st, st);
+    cta_copy(&s_m, ms);
     __syncthreads();
     cov12_warp(s_st, s_m, s_cov);
     __syncthreads();
-    for (uint32_t k = threadIdx.x; k < sizeof(IcpState) / 8; k += blockDim.x) gl[k] = sh[k];
+    cta_copy(st, &s_st);
 }
 
 void launch_covariance12(IcpState* st, const MotionState* ms, cudaStream_t stream) { k_covariance12<<<1, 32, 0, stream>>>(st, ms); }
@@ -643,14 +526,8 @@ __global__ void __launch_bounds__(128) k_motion_step(BatchView bv, MotionState* 
     __shared__ IcpState s_st;
     __shared__ MotionState s_m;
     __shared__ double s_sum[kMotionAcc];
-    {
-        const unsigned long long* a = reinterpret_cast<const unsigned long long*>(st);
-        unsigned long long* b = reinterpret_cast<unsigned long long*>(&s_st);
-        for (uint32_t k = threadIdx.x; k < sizeof(IcpState) / 8; k += blockDim.x) b[k] = a[k];
-        const unsigned long long* c = reinterpret_cast<const unsigned long long*>(ms + s);
-        unsigned long long* d = reinterpret_cast<unsigned long long*>(&s_m);
-        for (uint32_t k = threadIdx.x; k < sizeof(MotionState) / 8; k += blockDim.x) d[k] = c[k];
-    }
+    cta_copy(&s_st, st);
+    cta_copy(&s_m, ms + s);
     if (threadIdx.x < kMotionAcc) {                                      // the scan's CTAs in index order
         const uint32_t np = eval_ctas(uint32_t(st->n_points));
         const double* base = partials + size_t(s) * stride * kMotionAcc + threadIdx.x;
@@ -678,8 +555,8 @@ __global__ void __launch_bounds__(128) k_motion_step(BatchView bv, MotionState* 
                 for (int k = 0; k < 78; ++k) M.H[k] = s_sum[k];
                 for (int k = 0; k < 12; ++k) M.g[k] = s_sum[78 + k];
                 M.cost = s_sum[90]; S.n_ok = n_ok; S.n_iterations = 1; S.phase = PH_DONE;
-            } else m_begin_solve(S, M, s_sum, n_ok);
-        } else m_after_eval(S, M, s_sum);
+            } else lm_begin_solve(S, M, s_sum, n_ok);
+        } else lm_after_eval(S, M, s_sum);
     }
     __syncthreads();
     if (s_st.need_cov) {
@@ -687,14 +564,8 @@ __global__ void __launch_bounds__(128) k_motion_step(BatchView bv, MotionState* 
         if (threadIdx.x < 32) cov12_warp(s_st, s_m, s_cov);
         __syncthreads();
     }
-    {
-        const unsigned long long* a = reinterpret_cast<const unsigned long long*>(&s_st);
-        unsigned long long* b = reinterpret_cast<unsigned long long*>(st);
-        for (uint32_t k = threadIdx.x; k < sizeof(IcpState) / 8; k += blockDim.x) b[k] = a[k];
-        const unsigned long long* c = reinterpret_cast<const unsigned long long*>(&s_m);
-        unsigned long long* d = reinterpret_cast<unsigned long long*>(ms + s);
-        for (uint32_t k = threadIdx.x; k < sizeof(MotionState) / 8; k += blockDim.x) d[k] = c[k];
-    }
+    cta_copy(st, &s_st);
+    cta_copy(ms + s, &s_m);
 }
 
 void launch_motion_warp(const BatchView& bv, float4* sorted, const float4* raw, const float* times, const MotionState* ms, uint32_t first,

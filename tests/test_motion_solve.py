@@ -1,5 +1,5 @@
-"""The device's two-block solve of so_register_optimized (m_begin_solve / m_lm_continue / m_after_eval / chol12_solve / m_gmax in
-so_motion.cu, on one thread of k_motion_step, with k_motion_eval's partials summed in a fixed order and cov12_warp at the end) on given
+"""The device's two-block solve of so_register_optimized (so_trust_region.cuh's tr_begin_solve / tr_continue / tr_after_eval with
+chol_solve<12>, on so_motion.cu's TwoBlock policy, on one thread of k_motion_step, with k_motion_eval's partials summed in a fixed order and cov12_warp at the end) on given
 correspondences, through so_solve_optimized, against both restatements (optimized_numpy.solve_full2 and oracle.solve_optimized) on the
 families of tests/motion_solve_sets.py, and its batched forms against each other bit for bit.  Which exits stay unreached, and why, is
 argued in tests/test_motion_solve_cpu.py."""

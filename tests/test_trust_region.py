@@ -1,4 +1,5 @@
-"""The device's trust-region solve (lm_begin_solve_t / lm_continue_t / lm_after_eval_t in so_icp.cu) on given correspondences, through
+"""The device's trust-region solve (so_trust_region.cuh's tr_begin_solve / tr_continue / tr_after_eval on so_icp.cu's Ambient and
+Reduced policies) on given correspondences, through
 so_solve, against both restatements (tests/test_ceres_restatement.py, oracle/so_oracle.cpp; degeneracy_numpy.solve_reduced for the
 reduced solve) on the families of tests/trust_region_sets.py -- the ones that reject steps -- and its execution forms against each
 other bit for bit: the fused evaluation + step kernel (one problem), the split kernels (SO_NO_FUSED_LM, and batches of three or
