@@ -239,7 +239,7 @@ int so_map_download_all(so_ctx* ctx, int store, float* out_xyzi, size_t cap_poin
 /* ---- keyframes: registered scans kept on the device, and the map rebuilt from them after a loop closure --------------------------
  * No reference counterpart (the reference is an odometry front end).  What a loop-closing back end needs from the device: the scans
  * with their poses, a submap built from chosen scans to register a kept scan against (the loop constraint: pose and cov), and the map
- * rebuilt from every keyframe once the caller's pose graph has moved them.  The pose graph itself stays with the caller.  Off until
+ * rebuilt from every keyframe once a pose graph has moved them (so_pose_graph_solve below, or the caller's own).  Off until
  * so_keyframe_reserve; nothing else calls these, and no other call changes behaviour.
  * so_keyframe_reserve: one pool of cap_points points for surf clouds and one for edge clouds, and room for cap_frames keyframes; again
  * with other values to resize (contents kept); 0, 0 frees the store.  SO_ERR_ARG when only one of the two is 0 or when either is below
@@ -326,6 +326,47 @@ int so_loop_candidates(so_ctx* ctx, const int32_t* queries, size_t n, const so_l
                        so_loop_stats* stats);
 /* The descriptors of keyframes ids[0..n) as the search sees them, out[n][rings][sectors] (described first where the cache holds none). */
 int so_keyframe_descriptors(so_ctx* ctx, const int32_t* ids, size_t n, const so_loop_opts* opts, float* out);
+
+/* ---- pose graph: move the keyframes so that they agree with odometry and loop factors (sparse SE(3) least squares) -----------------
+ * No reference counterpart.  The Ceres problem a pose graph is written as, solved by the trust-region rules of the registration's
+ * solve (DESIGN.md section 3; "Pose graph" in section 4 states the definition in full):
+ *   - nodes k = 0 .. n-1, pose7 values, one parameter block each with PoseLocalParameterization's Plus; node `fixed` held constant
+ *     (it is not a parameter: norms, the gradient and the columns cover the free nodes only);
+ *   - edge (i, j, z, S, c): r = S [t_E ; Log(R_E)] with E = Z^-1 X_i^-1 X_j, Log's angle in [0, pi]; S is a 6x6 square-root
+ *     information matrix, row-major, order x, y, z, rx, ry, rz;
+ *   - cost 1/2 sum rho(|r|^2): rho(s) = s for c = 0, Cauchy rho(s) = c^2 log(1 + s / c^2) for c > 0, through Ceres' corrector;
+ *   - Jacobi scaling at iteration 0, LM diagonal [1e-6, 1e32], initial radius 1e4, tolerances 1e-10 (gradient), 1e-8 (parameter),
+ *     1e-6 (function), termination codes as so_icp_result.iter_lm_termination.
+ * Only the linear solve differs from Ceres' DENSE_QR: preconditioned conjugate gradients in FP64 with a block-tridiagonal
+ * preconditioner over the node order (exact for a graph of consecutive edges alone).  Results are bit-identical run to run. */
+typedef struct {
+    int32_t i, j;             /* nodes of the edge, i != j */
+    double z[7];              /* measured X_i^-1 X_j, pose7 */
+    double sqrt_info[36];     /* S, row-major */
+    double cauchy;            /* c: 0 for no loss, > 0 for CauchyLoss(c) */
+} so_pose_edge;
+typedef struct {
+    int32_t fixed;            /* the node held constant, default 0 */
+    int32_t max_iterations;   /* trust-region iterations, default 50 (Ceres' default); 0 evaluates the start only */
+} so_pose_graph_opts;
+typedef struct {
+    int32_t iterations, successful, unsuccessful, termination;   /* counted as Ceres counts them; termination codes as the registration's */
+    uint64_t pcg_iterations;  /* conjugate-gradient iterations over all trust-region steps */
+    double initial_cost, final_cost;
+    double gmax;              /* max-norm of the gradient through Plus at the solution */
+    double radius;            /* the trust-region radius the solve ends with */
+    double time_ms;           /* device time of the solve (CUDA events) */
+} so_pose_graph_result;
+void so_pose_graph_opts_defaults(so_pose_graph_opts* opts);
+/* Host-only: SO_ERR_ARG, with so_last_error naming the cause, for n_nodes < 2, an edge id out of range, i == j, a non-finite or
+ * zero-norm z quaternion, a non-finite z or S, c < 0 or non-finite, fixed out of range, max_iterations < 0, and a graph in which some
+ * node is not connected to `fixed`.  Duplicate edges are allowed. */
+int so_pose_graph_check(size_t n_nodes, const so_pose_edge* edges, size_t n_edges, const so_pose_graph_opts* opts);
+/* Solve from init7[n_nodes][7] (every pose finite with a non-zero quaternion; SO_ERR_ARG otherwise, and for every case of
+ * so_pose_graph_check, before any device work).  out7[n_nodes][7] gets the solution (the fixed node as given) and may alias init7;
+ * edge_weights (NULL or [n_edges]) gets each edge's rho' at it (1 without a loss).  opts NULL: the defaults.  result may be NULL. */
+int so_pose_graph_solve(so_ctx* ctx, const double* init7, size_t n_nodes, const so_pose_edge* edges, size_t n_edges,
+                        const so_pose_graph_opts* opts, double* out7, double* edge_weights, so_pose_graph_result* result);
 
 /* ---- free-space clearing: take out the map points a scan sees through (moving objects) ---------------------------------------
  * No reference counterpart (LocalMap::addSurfPointCloud only adds points).  Off unless called; nothing else calls it.

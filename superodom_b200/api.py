@@ -30,6 +30,7 @@ EXPORTS = [
     "so_keyframe_reserve", "so_keyframe_add_registered", "so_keyframe_info", "so_keyframe_poses", "so_keyframe_download", "so_map_from_keyframes",
     "so_register_keyframes",
     "so_loop_opts_defaults", "so_loop_candidates", "so_keyframe_descriptors",
+    "so_pose_graph_opts_defaults", "so_pose_graph_check", "so_pose_graph_solve",
 ]
 
 
@@ -200,6 +201,46 @@ def loop_opts(**kw) -> LoopOpts:
     return o
 
 
+# so_pose_edge, so_pose_graph_opts, so_pose_graph_result
+POSE_EDGE_DTYPE = np.dtype([("i", "<i4"), ("j", "<i4"), ("z", "<f8", 7), ("sqrt_info", "<f8", 36), ("cauchy", "<f8")], align=True)
+
+
+class PoseGraphOpts(C.Structure):
+    _fields_ = [("fixed", C.c_int32), ("max_iterations", C.c_int32)]
+
+
+class PoseGraphResult(C.Structure):
+    _fields_ = [("iterations", C.c_int32), ("successful", C.c_int32), ("unsuccessful", C.c_int32), ("termination", C.c_int32),
+                ("pcg_iterations", C.c_uint64), ("initial_cost", C.c_double), ("final_cost", C.c_double), ("gmax", C.c_double),
+                ("radius", C.c_double), ("time_ms", C.c_double)]
+
+
+def pose_edges(edges) -> np.ndarray:
+    """Edges as a POSE_EDGE_DTYPE array: given as one, or as tuples (i, j, z7, sqrt_info, cauchy=0), sqrt_info a 6x6 matrix or the
+    diagonal of one (6 values)."""
+    if isinstance(edges, np.ndarray) and edges.dtype == POSE_EDGE_DTYPE:
+        return np.ascontiguousarray(edges)
+    out = np.zeros(len(edges), POSE_EDGE_DTYPE)
+    for k, e in enumerate(edges):
+        s = np.asarray(e[3], np.float64)
+        out[k]["i"], out[k]["j"], out[k]["z"] = int(e[0]), int(e[1]), np.asarray(e[2], np.float64)
+        out[k]["sqrt_info"] = (np.diag(s) if s.shape == (6,) else s.reshape(6, 6)).ravel()
+        out[k]["cauchy"] = float(e[4]) if len(e) > 4 else 0.0
+    return out
+
+
+def pose_graph_check(n_nodes: int, edges, fixed: int = 0, max_iterations: int = 50):
+    """Host-only so_pose_graph_check: raises SuperOdomError with .code = SO_ERR_ARG (-1) and the cause for a graph the solve refuses."""
+    L = load_library()
+    e = pose_edges(edges)
+    o = PoseGraphOpts(int(fixed), int(max_iterations))
+    rc = L.so_pose_graph_check(int(n_nodes), _p(e) if len(e) else None, len(e), C.byref(o))
+    if rc < 0:
+        err = SuperOdomError(f"so_pose_graph_check failed ({rc}): " + L.so_last_error().decode())
+        err.code = rc
+        raise err
+
+
 class EdgeOpts(C.Structure):
     """so_edge_opts: zero fields take the defaults (min_range 0, edge_threshold 0.1, voxel_leaf 0 = no filter, max_per_sector 20)."""
     _fields_ = [("min_range", C.c_float), ("edge_threshold", C.c_float), ("voxel_leaf", C.c_float), ("max_per_sector", C.c_int32)]
@@ -351,6 +392,11 @@ def load_library():
     L.so_loop_opts_defaults.argtypes = [C.c_void_p]
     L.so_loop_candidates.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
     L.so_keyframe_descriptors.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
+    L.so_pose_graph_opts_defaults.restype = None
+    L.so_pose_graph_opts_defaults.argtypes = [C.c_void_p]
+    L.so_pose_graph_check.argtypes = [C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]
+    L.so_pose_graph_solve.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p,
+                                      C.c_void_p]
     _lib = L
     return L
 
@@ -651,6 +697,21 @@ class Context:
         out = np.zeros((len(i), max(o.rings, 1), max(o.sectors, 1)), np.float32)
         self._chk(self.L.so_keyframe_descriptors(self.h, _p(i), len(i), C.byref(o), _p(out)), "so_keyframe_descriptors")
         return out
+
+    # ---- pose graph (so_pose_graph_solve)
+    def pose_graph_solve(self, init, edges, fixed: int = 0, max_iterations: int = 50, weights: bool = False):
+        """The keyframe pose graph from init [n, 7] -> (poses [n, 7], result dict) and, with weights=True, each edge's final rho'.
+        edges: see pose_edges()."""
+        x = np.ascontiguousarray(init, dtype=np.float64).reshape(-1, 7)
+        e = pose_edges(edges)
+        out = np.zeros_like(x)
+        w = np.zeros(max(len(e), 1), np.float64) if weights else None
+        o = PoseGraphOpts(int(fixed), int(max_iterations))
+        r = PoseGraphResult()
+        self._chk(self.L.so_pose_graph_solve(self.h, _p(x), len(x), _p(e) if len(e) else None, len(e), C.byref(o), _p(out),
+                                             _p(w) if w is not None else None, C.byref(r)), "so_pose_graph_solve")
+        res = {k: getattr(r, k) for k, _ in PoseGraphResult._fields_}
+        return (out, res, w[:len(e)]) if weights else (out, res)
 
     # ---- free-space clearing (off unless called)
     @staticmethod

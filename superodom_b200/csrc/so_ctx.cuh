@@ -400,6 +400,25 @@ struct Ctx {
     KeyframeStore kf;
     KeyframeScratch kfs;
 
+    // ---- pose graph (so_pose_graph_solve, so_pose_graph.cu): allocated on first use, grown on demand ------------------------------
+    // Two linearisation sets: [cur] at the iterate, [1 - cur] at the candidate of the last trial (an accepted step swaps them)
+    struct Pg {
+        DeviceBuffer<so_pose_edge> d_edges;                                // [m]
+        DeviceBuffer<int32_t> d_inc;                                       // [n + 1] offsets, then [2m] incident edge ids, ascending per node
+        DeviceBuffer<double> d_x[2];                                       // [n][7]
+        DeviceBuffer<struct PgEdgeBlk> d_blk[2];                           // [m] per-edge Jacobian products
+        DeviceBuffer<double> d_ecost[2], d_w[2];                           // [m] 1/2 rho and rho' per edge
+        DeviceBuffer<double> d_H[2], d_C[2], d_g[2];                       // [n][36] node blocks, [n][36] chain blocks (k, k+1), [n][6]
+        DeviceBuffer<double> d_scale, d_diag, d_dd;                        // [6n] Jacobi scaling, LM diagonal, diag / radius
+        DeviceBuffer<double> d_vec;                                        // [6][6n] PCG vectors b, y, r, z, p, q
+        DeviceBuffer<double> d_crD, d_crL, d_crU, d_crB;                   // cyclic-reduction levels: [T][36] x 3, [T][6]
+        DeviceBuffer<double> d_red;                                        // [2][max_blocks] CTA partials of the trial's grid reductions
+        int max_blocks = 0;                                                // co-resident CTAs of k_pg_trial on the context's device
+        DeviceBuffer<struct PgCtl> d_ctl;
+        PinnedBuffer<struct PgCtl> h_ctl;
+        Event ev[2];
+    } pg;
+
     // ---- instrumentation ----------------------------------------------------------------------------------------
     uint64_t launches = 0;
     uint64_t bytes_h2d = 0, bytes_d2h = 0;         // host<->device bytes moved by registration / k-NN calls

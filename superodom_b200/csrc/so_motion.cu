@@ -90,22 +90,6 @@ __global__ void __launch_bounds__(256) k_motion_cloud(float4* __restrict__ pts, 
 }
 
 // ------------------------------------------------------------------------------------------------------------------ evaluation
-// Coefficients of J_r(v) = I - c1 [v]x + c2 [v]x^2 and J_r(v)^-1 = I + [v]x / 2 + c3 [v]x^2 at |v| = th.  Below th = 1e-2 their
-// Taylor series to th^4 (truncation < 3e-17, where the closed forms lose ~eps / th^2 to cancellation).
-__host__ __device__ inline void jr_coeffs(double th, double* c1, double* c2) {
-    if (th < 1e-2) {
-        const double t2 = th * th;
-        *c1 = 0.5 - t2 / 24.0 + t2 * t2 / 720.0;
-        *c2 = 1.0 / 6.0 - t2 / 120.0 + t2 * t2 / 5040.0;
-    } else {
-        *c1 = (1.0 - cos(th)) / (th * th);
-        *c2 = (th - sin(th)) / (th * th * th);
-    }
-}
-__host__ __device__ inline double jrinv_coeff(double th) {
-    if (th < 1e-2) { const double t2 = th * th; return 1.0 / 12.0 + t2 / 720.0 + t2 * t2 / 30240.0; }
-    return 1.0 / (th * th) - 1.0 / (2.0 * th * tan(0.5 * th));                // 1/th^2 - (1 + cos th) / (2 th sin th)
-}
 __device__ __forceinline__ void cross3(const double a[3], const double b[3], double o[3]) {
     o[0] = a[1] * b[2] - a[2] * b[1]; o[1] = a[2] * b[0] - a[0] * b[2]; o[2] = a[0] * b[1] - a[1] * b[0];
 }
