@@ -253,6 +253,15 @@ int so_keyframe_reserve(so_ctx* ctx, size_t cap_points, size_t cap_frames);
  * registration had an edge cloud).  SO_ERR_CAPACITY
  * with the store unchanged when a pool or the frame table is full. */
 int so_keyframe_add_registered(so_ctx* ctx, const double pose[7], int32_t* id);
+/* Append one keyframe from host clouds, as *id: surf_xyzi[n_surf] and edge_xyzi[n_edge] (either count may be 0), records of
+ * stride_bytes with x, y, z floats at 0 and the intensity float at intensity_offset (0 when it lies past the record), already in the
+ * sensor frame and already compensated, at pose.  The clouds are kept verbatim: so_keyframe_download(id, store, NULL) returns them bit
+ * for bit, so a session's keyframes saved through so_keyframe_poses and so_keyframe_download come back unchanged in another context.
+ * The registered scan, the map and every other keyframe's cached descriptor are not touched; the new keyframe is described lazily,
+ * as any other.  SO_ERR_ARG, before any device work, without a store, for a non-finite pose, a NULL cloud with a non-zero count or
+ * stride_bytes < 12; SO_ERR_CAPACITY with the store unchanged when a pool or the frame table is full. */
+int so_keyframe_import(so_ctx* ctx, const void* surf_xyzi, size_t n_surf, const void* edge_xyzi, size_t n_edge, size_t stride_bytes,
+                       size_t intensity_offset, const double pose[7], int32_t* id);
 /* Keyframes held and the points of the surf and edge pools; any pointer may be NULL. */
 int so_keyframe_info(so_ctx* ctx, size_t* n_frames, size_t* n_points, size_t* n_edge_points);
 /* The keyframes' poses, [*n][7]; only cap are written.  A pose is the one the keyframe was added with, or the one the last
@@ -324,6 +333,14 @@ void so_loop_opts_defaults(so_loop_opts* opts);
  * query is compared with every eligible keyframe at every shift.  stats may be NULL.  SO_ERR_ARG also for k outside 1..64. */
 int so_loop_candidates(so_ctx* ctx, const int32_t* queries, size_t n, const so_loop_opts* opts, int32_t k, so_loop_candidate* out,
                        so_loop_stats* stats);
+/* so_loop_candidates over the ids [id_begin, id_end) instead of the ids below q - exclude_recent: every keyframe of the range but the
+ * query itself is eligible, wherever the range lies relative to the query (a later session's query searching an earlier session's
+ * ids, imported before or after it started).  opts.exclude_recent is not used.  With the range [0, q - exclude_recent) the result is
+ * bit-identical to so_loop_candidates for query q.  A range that holds no eligible keyframe leaves every slot unused (id -1).
+ * SO_ERR_ARG, before any device work, as so_loop_candidates, and for id_begin < 0, id_end < id_begin or id_end past the keyframes
+ * the store holds. */
+int so_loop_candidates_range(so_ctx* ctx, const int32_t* queries, size_t n, const so_loop_opts* opts, int32_t id_begin, int32_t id_end,
+                             int32_t k, so_loop_candidate* out, so_loop_stats* stats);
 /* The descriptors of keyframes ids[0..n) as the search sees them, out[n][rings][sectors] (described first where the cache holds none). */
 int so_keyframe_descriptors(so_ctx* ctx, const int32_t* ids, size_t n, const so_loop_opts* opts, float* out);
 
@@ -367,6 +384,18 @@ int so_pose_graph_check(size_t n_nodes, const so_pose_edge* edges, size_t n_edge
  * edge_weights (NULL or [n_edges]) gets each edge's rho' at it (1 without a loss).  opts NULL: the defaults.  result may be NULL. */
 int so_pose_graph_solve(so_ctx* ctx, const double* init7, size_t n_nodes, const so_pose_edge* edges, size_t n_edges,
                         const so_pose_graph_opts* opts, double* out7, double* edge_weights, so_pose_graph_result* result);
+/* The same problem with every node k where constant[k] != 0 held constant (Ceres' SetParameterBlockConstant on each): norms, the
+ * gradient and the columns cover the free nodes only; opts->fixed is not used.  The multi-session merge holds an earlier session's
+ * keyframes constant while a later one is joined to them.  A mask with exactly one node set gives results bit-identical to
+ * so_pose_graph_solve with that node as `fixed`: poses, weights and every field of the result.  so_pose_graph_check_constant is
+ * so_pose_graph_check with the fixed-node rules replaced by: constant not NULL, at least one constant node, at least one free node
+ * unless max_iterations == 0, and every node connected to some constant node.  The solve fails with SO_ERR_ARG for every case of the
+ * check, and for a non-finite init, before any device work.  Constant nodes come back as given (their quaternion normalised). */
+int so_pose_graph_check_constant(size_t n_nodes, const so_pose_edge* edges, size_t n_edges, const uint8_t* constant,
+                                 const so_pose_graph_opts* opts);
+int so_pose_graph_solve_constant(so_ctx* ctx, const double* init7, size_t n_nodes, const so_pose_edge* edges, size_t n_edges,
+                                 const uint8_t* constant, const so_pose_graph_opts* opts, double* out7, double* edge_weights,
+                                 so_pose_graph_result* result);
 
 /* ---- free-space clearing: take out the map points a scan sees through (moving objects) ---------------------------------------
  * No reference counterpart (LocalMap::addSurfPointCloud only adds points).  Off unless called; nothing else calls it.

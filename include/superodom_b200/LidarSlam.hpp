@@ -31,6 +31,7 @@
 #include <vector>
 
 #include "../superodom_b200.h"
+#include "KeyframeIO.hpp"
 
 namespace super_odometry {
 namespace b200 {
@@ -249,6 +250,51 @@ public:
         std::vector<double> p(7 * poses.size());
         for (size_t i = 0; i < poses.size(); ++i) poses[i].to_pose7(p.data() + 7 * i);
         check(so_map_from_keyframes(ctx_->h, src.ctx_->h, ids.data(), ids.size(), p.data(), 3), "so_map_from_keyframes");
+    }
+    // Shim only: sessions (KeyframeIO.hpp; INTEGRATION.md "Sessions").  saveKeyframes writes every keyframe (pose, surf and edge
+    // clouds in the sensor frame) and the caller's graph edges to one file; loadKeyframes appends a saved session's keyframes to this
+    // map's store (so_keyframe_import) and returns the first new id, their count and the saved edges (node ids as saved: add `first`
+    // to place them in this store).  Neither call touches the map; the store must have room (reserveKeyframes).
+    struct LoadedKeyframes { int32_t first = 0; int32_t count = 0; std::vector<so_pose_edge> edges; };
+    void saveKeyframes(const std::string& path, const std::vector<so_pose_edge>& edges) {
+        sync_resolution();
+        KeyframeSession s;
+        size_t n = 0;
+        check(so_keyframe_poses(ctx_->h, nullptr, 0, &n), "so_keyframe_poses");
+        std::vector<double> p(7 * n);
+        check(so_keyframe_poses(ctx_->h, p.data(), n, &n), "so_keyframe_poses");
+        s.poses.resize(n); s.surf.resize(n); s.edge.resize(n);
+        for (size_t i = 0; i < n; ++i) {
+            std::memcpy(s.poses[i].data(), p.data() + 7 * i, 7 * sizeof(double));
+            for (int store = 0; store < 2; ++store) {
+                std::vector<float>& dst = store ? s.edge[i] : s.surf[i];
+                size_t m = 0;
+                check(so_keyframe_download(ctx_->h, int32_t(i), store, nullptr, nullptr, 0, &m), "so_keyframe_download");
+                dst.resize(4 * m);
+                if (m) check(so_keyframe_download(ctx_->h, int32_t(i), store, nullptr, dst.data(), m, &m), "so_keyframe_download");
+            }
+        }
+        s.edges = edges;
+        std::string err;
+        if (!writeKeyframeSession(path, s, &err)) throw Error(err);
+    }
+    LoadedKeyframes loadKeyframes(const std::string& path) {
+        sync_resolution();
+        KeyframeSession s;
+        std::string err;
+        if (!readKeyframeSession(path, &s, &err)) throw Error(err);
+        LoadedKeyframes out;
+        size_t have = 0;
+        check(so_keyframe_info(ctx_->h, &have, nullptr, nullptr), "so_keyframe_info");
+        out.first = int32_t(have);
+        for (size_t i = 0; i < s.poses.size(); ++i) {
+            int32_t id = -1;
+            check(so_keyframe_import(ctx_->h, s.surf[i].data(), s.surf[i].size() / 4, s.edge[i].data(), s.edge[i].size() / 4, 16, 12,
+                                     s.poses[i].data(), &id), "so_keyframe_import");
+            ++out.count;
+        }
+        out.edges = std::move(s.edges);
+        return out;
     }
     void sync_resolution() {
         ctx_->ensure(lineRes_, planeRes_);
@@ -568,6 +614,50 @@ public:
         const double turn = heading(cand.rot) + c.yaw - heading(query.rot);
         const Quaterniond qz(std::cos(turn / 2), 0, 0, std::sin(turn / 2));
         return Transformd(qz * query.rot, cand.pos);
+    }
+    // loopCandidates over the keyframes [begin, end) only (so_loop_candidates_range with loopOpts; its exclude_recent is not used):
+    // a live-session keyframe searched against an earlier session's ids, wherever they lie in the store
+    std::vector<so_loop_candidate> loopCandidatesIn(int32_t id, int32_t k, int32_t begin, int32_t end) {
+        std::vector<so_loop_candidate> out(size_t(k > 0 ? k : 0));
+        check(so_loop_candidates_range(context.h, &id, 1, &loopOpts, begin, end, k, out.data(), nullptr), "so_loop_candidates_range");
+        return out;
+    }
+    // The keyframe pose graph solved on the device (so_pose_graph_solve_constant): edges between keyframe ids, the keyframes where
+    // constant[id] != 0 held, started from `init` (one pose per keyframe) or, when it is empty, from keyframePoses().  A live session
+    // joined to an earlier one starts from its poses moved into the earlier frame by the loop result (INTEGRATION.md, "Sessions"):
+    // the solve is local and does not cross a large change of frame by itself.  The store's poses are not changed: pass `poses` to
+    // mergeKeyframes or rebuildFromKeyframes.
+    struct GraphSolution { std::vector<Transformd> poses; so_pose_graph_result result{}; std::vector<double> weights; };
+    GraphSolution optimizeKeyframes(const std::vector<so_pose_edge>& edges, const std::vector<uint8_t>& constant,
+                                    const so_pose_graph_opts& opts, const std::vector<Transformd>& init = {}) {
+        const std::vector<Transformd> est = init.empty() ? keyframePoses() : init;
+        if (constant.size() != est.size()) throw Error("optimizeKeyframes: one constant flag per keyframe");
+        std::vector<double> x(7 * est.size());
+        for (size_t i = 0; i < est.size(); ++i) est[i].to_pose7(x.data() + 7 * i);
+        GraphSolution out;
+        out.weights.resize(edges.size());
+        check(so_pose_graph_solve_constant(context.h, x.data(), est.size(), edges.data(), edges.size(), constant.data(), &opts, x.data(),
+                                           out.weights.data(), &out.result), "so_pose_graph_solve_constant");
+        for (size_t i = 0; i < est.size(); ++i) out.poses.push_back(Transformd::from_pose7(x.data() + 7 * i));
+        return out;
+    }
+    // The live session continues in the frame of `corrected` (one pose per keyframe, in id order; an earlier session's keyframes held
+    // constant in it): the change of frame C = corrected[live_id] * est[live_id]^-1 at the live session's newest keyframe live_id moves
+    // T_w_lidar, last_T_w_lidar and undistort_prev_pose; the window is re-centred at the new T_w_lidar; then both stores are rebuilt
+    // from every keyframe.  The window goes first: the corrected frame can lie far from the old one, and a rebuild under the old window
+    // would drop (or archive) the map around the sensor.
+    void mergeKeyframes(const std::vector<Transformd>& corrected, int32_t live_id) {
+        const std::vector<Transformd> est = keyframePoses();
+        if (corrected.size() != est.size()) throw Error("mergeKeyframes: one corrected pose per keyframe");
+        if (live_id < 0 || size_t(live_id) >= est.size()) throw Error("mergeKeyframes: no such keyframe");
+        const Transformd C = corrected[size_t(live_id)] * est[size_t(live_id)].inverse();
+        T_w_lidar = C * T_w_lidar;
+        last_T_w_lidar = C * last_T_w_lidar;
+        undistort_prev_pose = C * undistort_prev_pose;
+        localMap.setOrigin(T_w_lidar.pos);
+        std::vector<int32_t> ids(corrected.size());
+        for (size_t i = 0; i < ids.size(); ++i) ids[i] = int32_t(i);
+        localMap.buildFromKeyframes(localMap, ids, corrected);
     }
     // The map rebuilt from every keyframe at the corrected poses (one per keyframe, in id order), both stores; T_w_lidar and
     // last_T_w_lidar become the corrected pose of the last keyframe, so the next Localization() continues from the corrected map.

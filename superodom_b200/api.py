@@ -27,10 +27,10 @@ EXPORTS = [
     "so_register_degeneracy", "so_register_batch_degeneracy", "so_degeneracy_analysis", "so_solve", "so_solve_optimized",
     "so_knn", "so_knn_device", "so_sampling_indices", "so_localize_global", "so_localize_scores", "so_localize_global_size", "so_localize_global_bnb", "so_localize_bnb_keys", "so_localize_bnb_bounds", "so_map_bounds", "so_map_bounds_all", "so_kernel_launches", "so_bytes_copied", "so_build_flags", "so_profile_enable", "so_profile_get",
     "so_knn_graph", "so_knn_graph_stats",
-    "so_keyframe_reserve", "so_keyframe_add_registered", "so_keyframe_info", "so_keyframe_poses", "so_keyframe_download", "so_map_from_keyframes",
+    "so_keyframe_reserve", "so_keyframe_add_registered", "so_keyframe_import", "so_keyframe_info", "so_keyframe_poses", "so_keyframe_download", "so_map_from_keyframes",
     "so_register_keyframes",
-    "so_loop_opts_defaults", "so_loop_candidates", "so_keyframe_descriptors",
-    "so_pose_graph_opts_defaults", "so_pose_graph_check", "so_pose_graph_solve",
+    "so_loop_opts_defaults", "so_loop_candidates", "so_loop_candidates_range", "so_keyframe_descriptors",
+    "so_pose_graph_opts_defaults", "so_pose_graph_check", "so_pose_graph_solve", "so_pose_graph_check_constant", "so_pose_graph_solve_constant",
 ]
 
 
@@ -241,6 +241,22 @@ def pose_graph_check(n_nodes: int, edges, fixed: int = 0, max_iterations: int = 
         raise err
 
 
+def pose_graph_check_constant(n_nodes: int, edges, constant, max_iterations: int = 50):
+    """Host-only so_pose_graph_check_constant: as pose_graph_check, with the nodes where constant (a mask of n_nodes) is set held
+    constant in place of one fixed node."""
+    L = load_library()
+    e = pose_edges(edges)
+    m = np.ascontiguousarray(constant, dtype=np.uint8)
+    if m.shape != (int(n_nodes),):
+        raise ValueError(f"constant: a mask of {n_nodes} nodes, got shape {m.shape}")
+    o = PoseGraphOpts(0, int(max_iterations))
+    rc = L.so_pose_graph_check_constant(int(n_nodes), _p(e) if len(e) else None, len(e), _p(m), C.byref(o))
+    if rc < 0:
+        err = SuperOdomError(f"so_pose_graph_check_constant failed ({rc}): " + L.so_last_error().decode())
+        err.code = rc
+        raise err
+
+
 class EdgeOpts(C.Structure):
     """so_edge_opts: zero fields take the defaults (min_range 0, edge_threshold 0.1, voxel_leaf 0 = no filter, max_per_sector 20)."""
     _fields_ = [("min_range", C.c_float), ("edge_threshold", C.c_float), ("voxel_leaf", C.c_float), ("max_per_sector", C.c_int32)]
@@ -383,6 +399,8 @@ def load_library():
     L.so_knn_graph_stats.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
     L.so_keyframe_reserve.argtypes = [C.c_void_p, C.c_size_t, C.c_size_t]
     L.so_keyframe_add_registered.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+    L.so_keyframe_import.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p,
+                                     C.c_void_p]
     L.so_keyframe_info.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     L.so_keyframe_poses.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
     L.so_keyframe_download.argtypes = [C.c_void_p, C.c_int32, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
@@ -391,12 +409,17 @@ def load_library():
     L.so_loop_opts_defaults.restype = None
     L.so_loop_opts_defaults.argtypes = [C.c_void_p]
     L.so_loop_candidates.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
+    L.so_loop_candidates_range.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
+                                           C.c_void_p]
     L.so_keyframe_descriptors.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
     L.so_pose_graph_opts_defaults.restype = None
     L.so_pose_graph_opts_defaults.argtypes = [C.c_void_p]
     L.so_pose_graph_check.argtypes = [C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]
     L.so_pose_graph_solve.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_void_p]
+    L.so_pose_graph_check_constant.argtypes = [C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
+    L.so_pose_graph_solve_constant.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p,
+                                               C.c_void_p, C.c_void_p, C.c_void_p]
     _lib = L
     return L
 
@@ -634,6 +657,17 @@ class Context:
         self._chk(self.L.so_keyframe_add_registered(self.h, _p(pose), C.byref(i)), "so_keyframe_add_registered")
         return i.value
 
+    def keyframe_import(self, surf_xyzi: np.ndarray, pose7, edge_xyzi: np.ndarray | None = None) -> int:
+        """Append a keyframe from sensor-frame, already compensated clouds [n, 4] (x, y, z, intensity) at pose7 -> its id.  The clouds
+        are kept verbatim: keyframe_download(id, store) returns them bit for bit."""
+        pose = np.ascontiguousarray(pose7, dtype=np.float64)
+        a = np.ascontiguousarray(surf_xyzi, dtype=np.float32).reshape(-1, 4)
+        e = np.ascontiguousarray(edge_xyzi if edge_xyzi is not None else np.zeros((0, 4)), dtype=np.float32).reshape(-1, 4)
+        i = C.c_int32()
+        self._chk(self.L.so_keyframe_import(self.h, _p(a) if len(a) else None, len(a), _p(e) if len(e) else None, len(e), 16, 12, _p(pose),
+                                            C.byref(i)), "so_keyframe_import")
+        return i.value
+
     def keyframe_info(self):
         """-> (keyframes, surf pool points, edge pool points)"""
         f, p, e = C.c_size_t(), C.c_size_t(), C.c_size_t()
@@ -677,15 +711,21 @@ class Context:
         return list(res)
 
     # ---- loop detection over the keyframes (Scan Context; descriptors cached per keyframe, computed by these calls)
-    def loop_candidates(self, queries, k: int, opts: LoopOpts | None = None, stats: bool = False, **kw):
+    def loop_candidates(self, queries, k: int, opts: LoopOpts | None = None, stats: bool = False, ids=None, **kw):
         """For each query keyframe its k best eligible keyframes -> structured array [n, k] of LOOP_CANDIDATE_DTYPE (distance
         ascending, then id; id -1 in unused slots); with stats=True also {n_described, time_describe_ms, time_search_ms}.  kw: fields
-        of so_loop_opts over the defaults."""
+        of so_loop_opts over the defaults.  ids=(begin, end): the eligible keyframes are those of [begin, end) but the query
+        (so_loop_candidates_range; exclude_recent is not used), else those below query - exclude_recent."""
         q = np.ascontiguousarray(np.atleast_1d(queries), dtype=np.int32)
         o = opts if opts is not None else loop_opts(**kw)
         out = np.zeros((len(q), max(int(k), 1)), LOOP_CANDIDATE_DTYPE)
         st = LoopStats()
-        self._chk(self.L.so_loop_candidates(self.h, _p(q), len(q), C.byref(o), int(k), _p(out), C.byref(st)), "so_loop_candidates")
+        if ids is None:
+            self._chk(self.L.so_loop_candidates(self.h, _p(q), len(q), C.byref(o), int(k), _p(out), C.byref(st)), "so_loop_candidates")
+        else:
+            b, e = (int(v) for v in ids)
+            self._chk(self.L.so_loop_candidates_range(self.h, _p(q), len(q), C.byref(o), b, e, int(k), _p(out), C.byref(st)),
+                      "so_loop_candidates_range")
         if stats:
             return out, dict(n_described=st.n_described, time_describe_ms=st.time_describe_ms, time_search_ms=st.time_search_ms)
         return out
@@ -699,17 +739,25 @@ class Context:
         return out
 
     # ---- pose graph (so_pose_graph_solve)
-    def pose_graph_solve(self, init, edges, fixed: int = 0, max_iterations: int = 50, weights: bool = False):
+    def pose_graph_solve(self, init, edges, fixed: int = 0, max_iterations: int = 50, weights: bool = False, constant=None):
         """The keyframe pose graph from init [n, 7] -> (poses [n, 7], result dict) and, with weights=True, each edge's final rho'.
-        edges: see pose_edges()."""
+        edges: see pose_edges().  constant: a mask of n nodes held constant (so_pose_graph_solve_constant), in place of `fixed`."""
         x = np.ascontiguousarray(init, dtype=np.float64).reshape(-1, 7)
         e = pose_edges(edges)
         out = np.zeros_like(x)
         w = np.zeros(max(len(e), 1), np.float64) if weights else None
         o = PoseGraphOpts(int(fixed), int(max_iterations))
         r = PoseGraphResult()
-        self._chk(self.L.so_pose_graph_solve(self.h, _p(x), len(x), _p(e) if len(e) else None, len(e), C.byref(o), _p(out),
-                                             _p(w) if w is not None else None, C.byref(r)), "so_pose_graph_solve")
+        if constant is None:
+            self._chk(self.L.so_pose_graph_solve(self.h, _p(x), len(x), _p(e) if len(e) else None, len(e), C.byref(o), _p(out),
+                                                 _p(w) if w is not None else None, C.byref(r)), "so_pose_graph_solve")
+        else:
+            m = np.ascontiguousarray(constant, dtype=np.uint8)
+            if m.shape != (len(x),):
+                raise ValueError(f"constant: a mask of {len(x)} nodes, got shape {m.shape}")
+            self._chk(self.L.so_pose_graph_solve_constant(self.h, _p(x), len(x), _p(e) if len(e) else None, len(e), _p(m), C.byref(o),
+                                                          _p(out), _p(w) if w is not None else None, C.byref(r)),
+                      "so_pose_graph_solve_constant")
         res = {k: getattr(r, k) for k, _ in PoseGraphResult._fields_}
         return (out, res, w[:len(e)]) if weights else (out, res)
 

@@ -198,7 +198,7 @@ struct KeyframeScratch {
     PinnedBuffer<int32_t> h_ctl;                           // its mirror
     // loop detection (so_loop.cu): keyframes to describe, the queries, one chunk's pair table and every query's top k
     DeviceBuffer<struct DescSeg> d_dsegs;
-    DeviceBuffer<int32_t> d_queries;
+    DeviceBuffer<struct LoopQuery> d_queries;
     DeviceBuffer<struct LoopPair> d_pairs, d_top;
     Event ev_loop[4];                                      // describe start / end, search start / end
 };
@@ -405,6 +405,7 @@ struct Ctx {
     struct Pg {
         DeviceBuffer<so_pose_edge> d_edges;                                // [m]
         DeviceBuffer<int32_t> d_inc;                                       // [n + 1] offsets, then [2m] incident edge ids, ascending per node
+        DeviceBuffer<uint8_t> d_const;                                     // [n] 1: the node is held constant
         DeviceBuffer<double> d_x[2];                                       // [n][7]
         DeviceBuffer<struct PgEdgeBlk> d_blk[2];                           // [m] per-edge Jacobian products
         DeviceBuffer<double> d_ecost[2], d_w[2];                           // [m] 1/2 rho and rho' per edge

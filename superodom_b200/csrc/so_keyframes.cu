@@ -1,6 +1,6 @@
-// so_keyframes.cu -- keyframes for a loop-closing back end: registered scans kept on the device with their poses (so_keyframe_*), and
-// the map rebuilt from them at corrected poses (so_map_from_keyframes; its kernels are in so_map.cu).  The pose graph stays with the
-// caller.
+// so_keyframes.cu -- keyframes for a loop-closing back end: registered scans kept on the device with their poses (so_keyframe_*),
+// keyframes of an earlier session imported from the host (so_keyframe_import), and the map rebuilt from them at corrected poses
+// (so_map_from_keyframes; its kernels are in so_map.cu).
 #include <algorithm>
 #include <cstring>
 
@@ -113,6 +113,30 @@ int so_keyframe_add_registered(so_ctx* ctx, const double pose[7], int32_t* id) {
     for (int k = 0; k < 2; ++k)
         if (n[k]) { int rc = put_registered_scan(c, k == 1, s.d_pool[k] + held(s, k), pose); if (rc) return rc; }
     SO_CUDA_TRY(cudaGetLastError());
+    for (int k = 0; k < 2; ++k) s.off[k].push_back(s.off[k].back() + n[k]);
+    if (id) *id = int32_t(s.frames());
+    s.poses.insert(s.poses.end(), pose, pose + 7);
+    return SO_OK;
+}
+
+int so_keyframe_import(so_ctx* ctx, const void* surf_xyzi, size_t n_surf, const void* edge_xyzi, size_t n_edge, size_t stride_bytes,
+                       size_t intensity_offset, const double pose[7], int32_t* id) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c || !pose || (n_surf && !surf_xyzi) || (n_edge && !edge_xyzi)) return fail(SO_ERR_ARG, "bad args");
+    if (stride_bytes < 12) return fail(SO_ERR_ARG, "so_keyframe_import: stride_bytes must be >= 12");
+    KeyframeStore& s = c->kf;
+    if (!s.cap_frames) return fail(SO_ERR_ARG, "so_keyframe_import needs a keyframe store (so_keyframe_reserve)");
+    if (!finite_pose(pose)) return fail(SO_ERR_ARG, "so_keyframe_import: pose must be finite with a non-zero quaternion");
+    if (s.frames() >= s.cap_frames || n_surf > s.cap_points - held(s, 0) || n_edge > s.cap_points - held(s, 1))
+        return fail(SO_ERR_CAPACITY, "keyframe store full: grow it with so_keyframe_reserve");
+    SO_CUDA_TRY(cudaSetDevice(c->device));
+    const void* src[2] = {surf_xyzi, edge_xyzi};
+    const size_t n[2] = {n_surf, n_edge};
+    for (int k = 0; k < 2; ++k) {                                      // verbatim, as so_keyframe_download(id, k, NULL) returns them
+        int rc = upload_cloud(c, src[k], n[k], stride_bytes, intensity_offset, s.d_pool[k] + held(s, k));
+        if (rc) return rc;
+    }
+    SO_CUDA_TRY(cudaStreamSynchronize(c->stream));                    // the host clouds may go once this returns
     for (int k = 0; k < 2; ++k) s.off[k].push_back(s.off[k].back() + n[k]);
     if (id) *id = int32_t(s.frames());
     s.poses.insert(s.poses.end(), pose, pose + 7);

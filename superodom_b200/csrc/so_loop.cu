@@ -27,6 +27,7 @@ constexpr size_t kLoopPairCap = size_t(1) << 20;              // pair-table entr
 struct LoopGrid { int32_t rings, sectors; double max_range, h, sector_w; };
 struct DescSeg { uint64_t first; uint32_t n, id; double L[9]; };   // keyframe id: pool[first .. first + n), levelled by L (row-major)
 struct LoopPair { double d; int32_t id, shift, n_pairs, pad; };
+struct LoopQuery { int32_t q, lo, count; };                        // query q's candidates: ids [lo, lo + count) but q
 
 __device__ __forceinline__ double row3(const double* L, int r, double x, double y, double z) {
     return __dadd_rn(__dadd_rn(__dmul_rn(L[3 * r], x), __dmul_rn(L[3 * r + 1], y)), __dmul_rn(L[3 * r + 2], z));
@@ -67,15 +68,15 @@ __global__ void __launch_bounds__(kLoopDescThreads) k_loop_describe(const float4
     }
 }
 
-// pairs[qi * stride + b]: query queries[blockIdx.y] against candidate b, for every b < its eligible count
+// pairs[qi * stride + u]: query queries[blockIdx.y] against every candidate b of its range [lo, lo + count) but itself
 __global__ void __launch_bounds__(kLoopSearchThreads) k_loop_search(const float* __restrict__ desc, const double* __restrict__ norm,
-                                                                    const int32_t* __restrict__ queries, int32_t exclude, int rings,
-                                                                    int sectors, LoopPair* __restrict__ pairs, size_t stride) {
+                                                                    const LoopQuery* __restrict__ queries, int rings, int sectors,
+                                                                    LoopPair* __restrict__ pairs, size_t stride) {
     extern __shared__ double sm[];
     double* qn = sm;                                           // [sectors]
     float* qd = reinterpret_cast<float*>(sm + sectors);        // [rings][sectors]
-    const int32_t q = queries[blockIdx.y];
-    const int32_t m = max(q - exclude, 0);
+    const LoopQuery Q = queries[blockIdx.y];
+    const int32_t q = Q.q, m = Q.count;
     const int32_t first = blockIdx.x * kLoopTile;
     if (first >= m) return;
     const int cells = rings * sectors;
@@ -84,8 +85,10 @@ __global__ void __launch_bounds__(kLoopSearchThreads) k_loop_search(const float*
     __syncthreads();
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     for (int t = warp; t < kLoopTile; t += kLoopSearchThreads / 32) {
-        const int32_t b = first + t;
-        if (b >= m) break;
+        const int32_t u = first + t;
+        if (u >= m) break;
+        const int32_t b = Q.lo + u;
+        if (b == q) continue;                                  // k_loop_topk skips it
         const float* cd = desc + size_t(b) * cells;
         const double* cn = norm + size_t(b) * sectors;
         double best = HUGE_VAL;
@@ -111,19 +114,19 @@ __global__ void __launch_bounds__(kLoopSearchThreads) k_loop_search(const float*
             const int os = __shfl_xor_sync(0xffffffffu, best_s, o), on = __shfl_xor_sync(0xffffffffu, best_n, o);
             if (od < best || (od == best && os < best_s)) { best = od; best_s = os; best_n = on; }
         }
-        if (lane == 0) pairs[size_t(blockIdx.y) * stride + b] = LoopPair{best, b, best_s, best_n, 0};
+        if (lane == 0) pairs[size_t(blockIdx.y) * stride + u] = LoopPair{best, b, best_s, best_n, 0};
     }
 }
 
 __device__ __forceinline__ bool key_less(double d0, int32_t i0, double d1, int32_t i1) { return d0 < d1 || (d0 == d1 && i0 < i1); }
 
 // top[qi * k .. + k): the k smallest (distance, id) of the query's row, ascending; id -1 past the eligible count
-__global__ void __launch_bounds__(256) k_loop_topk(const LoopPair* __restrict__ pairs, size_t stride, const int32_t* __restrict__ queries,
-                                                   int32_t exclude, int k, LoopPair* __restrict__ top) {
+__global__ void __launch_bounds__(256) k_loop_topk(const LoopPair* __restrict__ pairs, size_t stride, const LoopQuery* __restrict__ queries,
+                                                   int k, LoopPair* __restrict__ top) {
     __shared__ double wd[8];
     __shared__ int32_t wi[8];
     __shared__ LoopPair last;
-    const int32_t m = max(queries[blockIdx.x] - exclude, 0);
+    const LoopQuery Q = queries[blockIdx.x];
     const LoopPair* row = pairs + size_t(blockIdx.x) * stride;
     LoopPair* out = top + size_t(blockIdx.x) * k;
     double ld = -HUGE_VAL;
@@ -131,8 +134,10 @@ __global__ void __launch_bounds__(256) k_loop_topk(const LoopPair* __restrict__ 
     for (int t = 0; t < k; ++t) {
         double bd = HUGE_VAL;
         int32_t bi = INT32_MAX;
-        for (int32_t b = threadIdx.x; b < m; b += blockDim.x) {
-            const double d = row[b].d;
+        for (int32_t j = threadIdx.x; j < Q.count; j += blockDim.x) {
+            const int32_t b = Q.lo + j;
+            if (b == Q.q) continue;
+            const double d = row[j].d;
             if (key_less(ld, li, d, b) && key_less(d, b, bd, bi)) { bd = d; bi = b; }
         }
         for (int o = 16; o; o >>= 1) {
@@ -145,7 +150,7 @@ __global__ void __launch_bounds__(256) k_loop_topk(const LoopPair* __restrict__ 
         if (threadIdx.x == 0) {
             for (int w = 1; w < int(blockDim.x >> 5); ++w)
                 if (key_less(wd[w], wi[w], bd, bi)) { bd = wd[w]; bi = wi[w]; }
-            last = bi == INT32_MAX ? LoopPair{1.0, -1, 0, 0, 0} : row[bi];
+            last = bi == INT32_MAX ? LoopPair{1.0, -1, 0, 0, 0} : row[bi - Q.lo];
             out[t] = last;
         }
         __syncthreads();
@@ -283,33 +288,33 @@ static int loop_describe(Ctx* c, const int32_t* ids, size_t n, const so_loop_opt
     return SO_OK;
 }
 
-static int loop_search(Ctx* c, const int32_t* queries, size_t n, const so_loop_opts& o, int k, so_loop_candidate* out, double* ms) {
+// Each query against its candidates qs[i] (LoopQuery); the pair table of a chunk of queries is as wide as its longest range
+static int loop_search(Ctx* c, const std::vector<LoopQuery>& qs, const so_loop_opts& o, int k, so_loop_candidate* out, double* ms) {
     KeyframeStore& s = c->kf;
     KeyframeScratch& ks = c->kfs;
-    const int excl = o.exclude_recent;
-    auto eligible = [&](int32_t q) { return size_t(std::max(q - excl, 0)); };
+    const size_t n = qs.size();
     size_t max_m = 0;
-    for (size_t i = 0; i < n; ++i) max_m = std::max(max_m, eligible(queries[i]));
+    for (const LoopQuery& q : qs) max_m = std::max(max_m, size_t(q.count));
     int rc = ks.d_queries.reserve(std::max<size_t>(n, 1));
     if (!rc) rc = ks.d_pairs.reserve(std::max(kLoopPairCap, std::max<size_t>(max_m, 1)));
     if (!rc) rc = ks.d_top.reserve(std::max<size_t>(n * size_t(k), 1));
     if (!rc) rc = loop_events(c);
     if (rc) return rc;
-    SO_CUDA_TRY(cudaMemcpyAsync(ks.d_queries, queries, n * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
+    SO_CUDA_TRY(cudaMemcpyAsync(ks.d_queries, qs.data(), n * sizeof(LoopQuery), cudaMemcpyHostToDevice, c->stream));
     const int smem = int(size_t(o.sectors) * sizeof(double) + cells_of(o) * sizeof(float));
     SO_CUDA_TRY(cudaFuncSetAttribute(k_loop_search, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     SO_CUDA_TRY(cudaEventRecord(ks.ev_loop[2], c->stream));
     for (size_t a = 0; a < n;) {                                      // query chunks whose pair table fits ks.d_pairs
         size_t b = a, stride = 0;
         while (b < n && b - a < 65535) {
-            const size_t st = std::max(stride, std::max<size_t>(eligible(queries[b]), 1));
+            const size_t st = std::max(stride, std::max<size_t>(size_t(qs[b].count), 1));
             if ((b - a + 1) * st > ks.d_pairs.cap()) break;
             stride = st; ++b;
         }
         const uint32_t nq = uint32_t(b - a), tiles = uint32_t((stride + kLoopTile - 1) / kLoopTile);
-        k_loop_search<<<dim3(tiles, nq), kLoopSearchThreads, smem, c->stream>>>(s.d_desc, s.d_desc_norm, ks.d_queries + a, excl,
-                                                                               o.rings, o.sectors, ks.d_pairs, stride);
-        k_loop_topk<<<nq, 256, 0, c->stream>>>(ks.d_pairs, stride, ks.d_queries + a, excl, k, ks.d_top + a * size_t(k));
+        k_loop_search<<<dim3(tiles, nq), kLoopSearchThreads, smem, c->stream>>>(s.d_desc, s.d_desc_norm, ks.d_queries + a, o.rings,
+                                                                               o.sectors, ks.d_pairs, stride);
+        k_loop_topk<<<nq, 256, 0, c->stream>>>(ks.d_pairs, stride, ks.d_queries + a, k, ks.d_top + a * size_t(k));
         c->launches += 2;
         a = b;
     }
@@ -323,7 +328,7 @@ static int loop_search(Ctx* c, const int32_t* queries, size_t n, const so_loop_o
     for (size_t i = 0; i < top.size(); ++i) {
         const LoopPair& p = top[i];
         so_loop_candidate& r = out[i];
-        r.query = queries[i / size_t(k)];
+        r.query = qs[i / size_t(k)].q;
         r.id = p.id;
         r.distance = p.d; r.shift = p.shift; r.n_pairs = p.n_pairs;
         double yaw = double(p.shift) * step;
@@ -353,12 +358,39 @@ int so_loop_candidates(so_ctx* ctx, const int32_t* queries, size_t n, const so_l
     SO_CUDA_TRY(cudaSetDevice(c->device));
     // every keyframe a query is compared with: the queries and ids 0 .. the largest eligible count
     int32_t top = 0;
-    for (size_t i = 0; i < n; ++i) top = std::max(top, queries[i] - opts->exclude_recent);
+    std::vector<LoopQuery> qs(n);
+    for (size_t i = 0; i < n; ++i) {
+        qs[i] = LoopQuery{queries[i], 0, std::max(queries[i] - opts->exclude_recent, 0)};
+        top = std::max(top, qs[i].count);
+    }
     std::vector<int32_t> need(queries, queries + n);
     for (int32_t i = 0; i < top; ++i) need.push_back(i);
     so_loop_stats st{};
     int rc = loop_describe(c, need.data(), need.size(), *opts, &st.n_described, &st.time_describe_ms);
-    if (!rc && n) rc = loop_search(c, queries, n, *opts, k, out, &st.time_search_ms);
+    if (!rc && n) rc = loop_search(c, qs, *opts, k, out, &st.time_search_ms);
+    if (rc) return rc;
+    if (stats) *stats = st;
+    return SO_OK;
+}
+
+int so_loop_candidates_range(so_ctx* ctx, const int32_t* queries, size_t n, const so_loop_opts* opts, int32_t id_begin, int32_t id_end,
+                             int32_t k, so_loop_candidate* out, so_loop_stats* stats) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c) return fail(SO_ERR_ARG, "null ctx");
+    { int rc = loop_check(c, opts); if (rc) return rc; }
+    if (k < 1 || k > kLoopMaxK) return fail(SO_ERR_ARG, "so_loop_candidates_range: k must be in 1..64");
+    if (n && !out) return fail(SO_ERR_ARG, "so_loop_candidates_range: NULL out");
+    if (id_begin < 0 || id_end < id_begin) return fail(SO_ERR_ARG, "so_loop_candidates_range: the range must have 0 <= id_begin <= id_end");
+    if (size_t(id_end) > c->kf.frames()) return fail(SO_ERR_ARG, "so_loop_candidates_range: id_end past the keyframes the store holds");
+    { int rc = check_loop_ids(c->kf, queries, n); if (rc) return rc; }
+    SO_CUDA_TRY(cudaSetDevice(c->device));
+    std::vector<LoopQuery> qs(n);
+    for (size_t i = 0; i < n; ++i) qs[i] = LoopQuery{queries[i], id_begin, id_end - id_begin};
+    std::vector<int32_t> need(queries, queries + n);
+    for (int32_t i = id_begin; i < id_end; ++i) need.push_back(i);
+    so_loop_stats st{};
+    int rc = loop_describe(c, need.data(), need.size(), *opts, &st.n_described, &st.time_describe_ms);
+    if (!rc && n) rc = loop_search(c, qs, *opts, k, out, &st.time_search_ms);
     if (rc) return rc;
     if (stats) *stats = st;
     return SO_OK;

@@ -156,14 +156,15 @@ __global__ void __launch_bounds__(128) k_pg_edges(const so_pose_edge* __restrict
 
 struct PgNodeArgs {
     const so_pose_edge* E; const int32_t* inc; const PgEdgeBlk* blk; const double* x;
-    double *H, *C, *g, *scale, *part;                                    // part: [n][2] gmax, |x_k|^2 (0 for the fixed node)
-    uint32_t n; int32_t fixed, init;
+    double *H, *C, *g, *scale, *part;                                    // part: [n][2] gmax, |x_k|^2 (0 for a constant node)
+    const uint8_t* constant;                                              // [n] 1: the node is held constant
+    uint32_t n; int32_t init;
 };
 
 __global__ void __launch_bounds__(128) k_pg_nodes(PgNodeArgs a) {
     const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= a.n) return;
-    const bool fixed = int32_t(k) == a.fixed, next_fixed = int32_t(k) + 1 == a.fixed;
+    const bool fixed = a.constant[k], next_fixed = k + 1 < a.n && a.constant[k + 1];
     double H[36], C[36], g[6];
     for (int t = 0; t < 36; ++t) { H[t] = 0.0; C[t] = 0.0; }
     for (int t = 0; t < 6; ++t) g[t] = 0.0;
@@ -248,7 +249,8 @@ struct PgTrialArgs {
     double *crD, *crL, *crU, *crB;
     double* red;                                                          // [2][gridDim.x] CTA partials of the grid reductions
     PgCtl* ctl;
-    uint32_t n; int32_t fixed, reuse_diagonal;
+    const uint8_t* constant;                                              // [n] 1: the node is held constant
+    uint32_t n; int32_t reuse_diagonal;
     double radius;
 };
 
@@ -273,7 +275,7 @@ __device__ __noinline__ double grid_reduce(double v, bool max, double* sh, doubl
 __device__ __noinline__ void pg_matvec(const PgTrialArgs& a, const double* p, double* q) {
     for (uint32_t k = gtid(); k < a.n; k += gstride()) {
         double y[6] = {0, 0, 0, 0, 0, 0}, sp[6];
-        if (int32_t(k) == a.fixed) { for (int t = 0; t < 6; ++t) q[6 * k + t] = p[6 * k + t]; continue; }
+        if (a.constant[k]) { for (int t = 0; t < 6; ++t) q[6 * k + t] = p[6 * k + t]; continue; }
         for (int t = 0; t < 6; ++t) sp[t] = a.scale[6 * k + t] * p[6 * k + t];
         mv6_add(a.H + 36 * size_t(k), sp, y, 1.0);
         if (k > 0) {
@@ -289,7 +291,7 @@ __device__ __noinline__ void pg_matvec(const PgTrialArgs& a, const double* p, do
             const int32_t i = a.E[e].i, j = a.E[e].j;
             if (i - j == 1 || j - i == 1) continue;                       // in the chain blocks
             const int32_t o = i == int32_t(k) ? j : i;
-            if (o == a.fixed) continue;
+            if (a.constant[o]) continue;
             for (int t = 0; t < 6; ++t) sp[t] = a.scale[6 * o + t] * p[6 * o + t];
             if (i == int32_t(k)) mv6_add(a.blk[e].aij, sp, y, 1.0);
             else mtv6_add(a.blk[e].aij, sp, y);
@@ -439,21 +441,22 @@ __global__ void __launch_bounds__(kTrialThreads) k_pg_trial(PgTrialArgs a) {
         const uint32_t k = i / 6, t = i % 6;
         if (!a.reuse_diagonal) {
             const double s = a.scale[i];
-            a.diag[i] = int32_t(k) == a.fixed ? 1.0 : fmin(fmax(s * s * a.H[36 * size_t(k) + t * 7], 1e-6), 1e32);
+            a.diag[i] = a.constant[k] ? 1.0 : fmin(fmax(s * s * a.H[36 * size_t(k) + t * 7], 1e-6), 1e32);
         }
         a.dd[i] = a.diag[i] / a.radius;
-        a.b[i] = int32_t(k) == a.fixed ? 0.0 : a.scale[i] * a.g[i];       // gs
+        a.b[i] = a.constant[k] ? 0.0 : a.scale[i] * a.g[i];               // gs
         a.y[i] = 0.0;
         a.r[i] = a.b[i];
     }
     gsync();
-    // level 0 of the preconditioner: the block-tridiagonal part of Hs + D^2 (identity row, zero coupling at the fixed node)
+    // level 0 of the preconditioner: the block-tridiagonal part of Hs + D^2 (identity row, zero coupling at a constant node; the
+    // chain blocks next to one are zero, k_pg_nodes leaves them so)
     for (uint32_t k = gtid(); k < n; k += gstride()) {
         const double* s = a.scale + 6 * size_t(k);
         double* D = a.crD + 36 * size_t(k);
         double* Lo = a.crL + 36 * size_t(k);
         double* Up = a.crU + 36 * size_t(k);
-        const bool fx = int32_t(k) == a.fixed;
+        const bool fx = a.constant[k];
         for (int r = 0; r < 6; ++r)
             for (int c = 0; c < 6; ++c) {
                 D[r * 6 + c] = fx ? (r == c ? 1.0 : 0.0) : s[r] * a.H[36 * size_t(k) + r * 6 + c] * s[c] + (r == c ? a.dd[6 * k + r] : 0.0);
@@ -506,7 +509,7 @@ __global__ void __launch_bounds__(kTrialThreads) k_pg_trial(PgTrialArgs a) {
     for (uint32_t k = gtid(); k < n; k += gstride()) {
         const double* xk = a.x + 7 * size_t(k);
         double* ck = a.xc + 7 * size_t(k);
-        if (int32_t(k) == a.fixed) { for (int t = 0; t < 7; ++t) ck[t] = xk[t]; continue; }
+        if (a.constant[k]) { for (int t = 0; t < 7; ++t) ck[t] = xk[t]; continue; }
         double d[6], o[7];
         for (int t = 0; t < 6; ++t) d[t] = -a.y[6 * k + t] * a.scale[6 * k + t];
         pose_plus(xk, d, o);
@@ -527,13 +530,14 @@ static bool finite_quat(const double* p) {
     return p[3] * p[3] + p[4] * p[4] + p[5] * p[5] + p[6] * p[6] > 0.0;
 }
 
-static int graph_check(size_t n, const so_pose_edge* edges, size_t m, const so_pose_graph_opts& o) {
+// Every rule but the constant set's; *comp gets each node's component (a root node id) when the graph passes
+static int graph_edges_check(size_t n, const so_pose_edge* edges, size_t m, int32_t max_iterations, std::vector<int32_t>* comp) {
     if (n < 2) return fail(SO_ERR_ARG, "so_pose_graph: at least two nodes");
     if (n >= (size_t(1) << 27) || m >= (size_t(1) << 28)) return fail(SO_ERR_ARG, "so_pose_graph: too many nodes or edges");
     if (m && !edges) return fail(SO_ERR_ARG, "so_pose_graph: NULL edges");
-    if (o.fixed < 0 || size_t(o.fixed) >= n) return fail(SO_ERR_ARG, "so_pose_graph: fixed node out of range");
-    if (o.max_iterations < 0) return fail(SO_ERR_ARG, "so_pose_graph: max_iterations < 0");
-    std::vector<int32_t> parent(n);
+    if (max_iterations < 0) return fail(SO_ERR_ARG, "so_pose_graph: max_iterations < 0");
+    std::vector<int32_t>& parent = *comp;
+    parent.resize(n);
     for (size_t k = 0; k < n; ++k) parent[k] = int32_t(k);
     auto root = [&](int32_t v) { while (parent[v] != v) { parent[v] = parent[parent[v]]; v = parent[v]; } return v; };
     for (size_t e = 0; e < m; ++e) {
@@ -547,9 +551,34 @@ static int graph_check(size_t n, const so_pose_edge* edges, size_t m, const so_p
         if (!std::isfinite(E.cauchy) || E.cauchy < 0.0) return fail(SO_ERR_ARG, "so_pose_graph: cauchy must be finite and >= 0" + at);
         parent[root(E.i)] = root(E.j);
     }
-    const int32_t rf = root(o.fixed);
+    for (size_t k = 0; k < n; ++k) parent[k] = root(int32_t(k));
+    return SO_OK;
+}
+
+static int graph_check(size_t n, const so_pose_edge* edges, size_t m, const so_pose_graph_opts& o) {
+    std::vector<int32_t> comp;
+    int rc = graph_edges_check(n, edges, m, o.max_iterations, &comp);
+    if (rc) return rc;
+    if (o.fixed < 0 || size_t(o.fixed) >= n) return fail(SO_ERR_ARG, "so_pose_graph: fixed node out of range");
     for (size_t k = 0; k < n; ++k)
-        if (root(int32_t(k)) != rf) return fail(SO_ERR_ARG, "so_pose_graph: node " + std::to_string(k) + " is not connected to the fixed node");
+        if (comp[k] != comp[o.fixed]) return fail(SO_ERR_ARG, "so_pose_graph: node " + std::to_string(k) + " is not connected to the fixed node");
+    return SO_OK;
+}
+
+// The constant set's rules: at least one constant node, one free node unless nothing is solved, and a constant node in every component
+static int graph_check_constant(size_t n, const so_pose_edge* edges, size_t m, const uint8_t* constant, int32_t max_iterations) {
+    if (!constant) return fail(SO_ERR_ARG, "so_pose_graph: NULL constant mask");
+    std::vector<int32_t> comp;
+    int rc = graph_edges_check(n, edges, m, max_iterations, &comp);
+    if (rc) return rc;
+    size_t held = 0;
+    std::vector<uint8_t> anchored(n, 0);
+    for (size_t k = 0; k < n; ++k)
+        if (constant[k]) { ++held; anchored[comp[k]] = 1; }
+    if (held == 0) return fail(SO_ERR_ARG, "so_pose_graph: no constant node");
+    if (held == n && max_iterations > 0) return fail(SO_ERR_ARG, "so_pose_graph: every node constant (no free node to solve for)");
+    for (size_t k = 0; k < n; ++k)
+        if (!anchored[comp[k]]) return fail(SO_ERR_ARG, "so_pose_graph: node " + std::to_string(k) + " is not connected to any constant node");
     return SO_OK;
 }
 
@@ -561,6 +590,7 @@ static int pg_reserve(Ctx* c, size_t n, size_t m) {
     for (size_t mm = n; ; mm = (mm + 1) / 2) { T += mm; if (mm == 1) break; }
     int rc = g.d_edges.reserve(m);
     if (!rc) rc = g.d_inc.reserve(n + 1 + 2 * m);
+    if (!rc) rc = g.d_const.reserve(n);
     for (int s = 0; s < 2 && !rc; ++s) {
         rc = g.d_x[s].reserve(7 * n);
         if (!rc) rc = g.d_blk[s].reserve(std::max<size_t>(m, 1));
@@ -596,17 +626,18 @@ static int pg_reserve(Ctx* c, size_t n, size_t m) {
 }
 
 // The linearisation of set s at d_x[s]: edges, nodes, the fixed-order reductions into ctl
-static void pg_linearise(Ctx* c, uint32_t n, uint32_t m, int32_t fixed, int s, bool init, double* part) {
+static void pg_linearise(Ctx* c, uint32_t n, uint32_t m, int s, bool init, double* part) {
     Ctx::Pg& g = c->pg;
     if (m) k_pg_edges<<<(m + 127) / 128, 128, 0, c->stream>>>(g.d_edges, m, g.d_x[s], g.d_blk[s], g.d_ecost[s], g.d_w[s]);
-    PgNodeArgs na{g.d_edges, g.d_inc, g.d_blk[s], g.d_x[s], g.d_H[s], g.d_C[s], g.d_g[s], g.d_scale, part, n, fixed, init ? 1 : 0};
+    PgNodeArgs na{g.d_edges, g.d_inc, g.d_blk[s], g.d_x[s], g.d_H[s], g.d_C[s], g.d_g[s], g.d_scale, part, g.d_const, n, init ? 1 : 0};
     k_pg_nodes<<<(n + 127) / 128, 128, 0, c->stream>>>(na);
     k_pg_reduce<<<1, kReduceThreads, 0, c->stream>>>(g.d_ecost[s], m, part, n, g.d_ctl, s);
     c->launches += m ? 3 : 2;
 }
 
-static int pg_solve(Ctx* c, const double* init7, uint32_t n, const so_pose_edge* edges, uint32_t m, const so_pose_graph_opts& o,
-                    double* out7, double* weights, so_pose_graph_result* res) {
+// The solve with the nodes constant[k] != 0 held constant (checked by graph_check_constant or, for one node, graph_check)
+static int pg_solve(Ctx* c, const double* init7, uint32_t n, const so_pose_edge* edges, uint32_t m, const uint8_t* constant,
+                    int32_t max_iterations, double* out7, double* weights, so_pose_graph_result* res) {
     Ctx::Pg& g = c->pg;
     int rc = pg_reserve(c, n, m);
     if (rc) return rc;
@@ -629,14 +660,17 @@ static int pg_solve(Ctx* c, const double* init7, uint32_t n, const so_pose_edge*
         std::vector<int32_t> at(inc.begin(), inc.begin() + n);
         for (uint32_t e = 0; e < m; ++e) { inc[n + 1 + at[E[e].i]++] = int32_t(e); inc[n + 1 + at[E[e].j]++] = int32_t(e); }
     }
+    std::vector<uint8_t> mask(n);
+    for (uint32_t k = 0; k < n; ++k) mask[k] = constant[k] ? 1 : 0;
     double* part = g.d_vec + 5 * 6 * size_t(n);                          // q's slot doubles as the node partials of a linearisation
     SO_CUDA_TRY(cudaEventRecord(g.ev[0], c->stream));
+    SO_CUDA_TRY(cudaMemcpyAsync(g.d_const, mask.data(), n, cudaMemcpyHostToDevice, c->stream));
     if (m) SO_CUDA_TRY(cudaMemcpyAsync(g.d_edges, E.data(), m * sizeof(so_pose_edge), cudaMemcpyHostToDevice, c->stream));
     SO_CUDA_TRY(cudaMemcpyAsync(g.d_inc, inc.data(), inc.size() * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
     SO_CUDA_TRY(cudaMemcpyAsync(g.d_x[0], x.data(), x.size() * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-    count_h2d(c, m * sizeof(so_pose_edge) + inc.size() * sizeof(int32_t) + x.size() * sizeof(double));
+    count_h2d(c, m * sizeof(so_pose_edge) + inc.size() * sizeof(int32_t) + x.size() * sizeof(double) + n);
     int cur = 0;
-    pg_linearise(c, n, m, o.fixed, cur, true, part);
+    pg_linearise(c, n, m, cur, true, part);
     SO_CUDA_TRY(cudaGetLastError());
     PgCtl& h = *g.h_ctl;
     SO_CUDA_TRY(cudaMemcpyAsync(g.h_ctl, g.d_ctl, sizeof(PgCtl), cudaMemcpyDeviceToHost, c->stream));
@@ -655,12 +689,12 @@ static int pg_solve(Ctx* c, const double* init7, uint32_t n, const so_pose_edge*
     const size_t len = 6 * size_t(n);
     ta.b = v; ta.y = v + len; ta.r = v + 2 * len; ta.z = v + 3 * len; ta.p = v + 4 * len; ta.q = v + 5 * len;
     ta.crD = g.d_crD; ta.crL = g.d_crL; ta.crU = g.d_crU; ta.crB = g.d_crB;
-    ta.ctl = g.d_ctl; ta.n = n; ta.fixed = o.fixed; ta.red = g.d_red;
+    ta.ctl = g.d_ctl; ta.constant = g.d_const; ta.n = n; ta.red = g.d_red;
     // one thread per node, at most the co-resident CTAs; a function of n and the device only, so the reductions' order is fixed
     const uint32_t blocks = std::max<uint32_t>(1, std::min<uint32_t>(uint32_t(g.max_blocks), (n + kTrialThreads - 1) / kTrialThreads));
     for (;;) {
         if (step_ok) r.successful++; else r.unsuccessful++;
-        if (r.iterations >= o.max_iterations) { term = 0; break; }
+        if (r.iterations >= max_iterations) { term = 0; break; }
         if (gmax <= 1e-10) { term = 1; break; }
         if (radius <= 1e-32) { term = 4; break; }
         r.iterations++;
@@ -675,7 +709,7 @@ static int pg_solve(Ctx* c, const double* init7, uint32_t n, const so_pose_edge*
             SO_CUDA_TRY(cudaLaunchCooperativeKernel((const void*)k_pg_trial, dim3(blocks), dim3(kTrialThreads), args, 0, c->stream));
         }
         c->launches++;
-        pg_linearise(c, n, m, o.fixed, 1 - cur, false, part);            // the candidate in full: an accepted step needs no second pass
+        pg_linearise(c, n, m, 1 - cur, false, part);            // the candidate in full: an accepted step needs no second pass
         SO_CUDA_TRY(cudaGetLastError());
         SO_CUDA_TRY(cudaMemcpyAsync(g.h_ctl, g.d_ctl, sizeof(PgCtl), cudaMemcpyDeviceToHost, c->stream));
         SO_CUDA_TRY(cudaStreamSynchronize(c->stream));
@@ -734,6 +768,12 @@ int so_pose_graph_check(size_t n_nodes, const so_pose_edge* edges, size_t n_edge
     return graph_check(n_nodes, edges, n_edges, o);
 }
 
+static int check_init(const double* init7, size_t n) {
+    for (size_t k = 0; k < n; ++k)
+        if (!finite_quat(init7 + 7 * k)) return fail(SO_ERR_ARG, "so_pose_graph_solve: init pose " + std::to_string(k) + " not finite or with a zero-norm quaternion");
+    return SO_OK;
+}
+
 int so_pose_graph_solve(so_ctx* ctx, const double* init7, size_t n_nodes, const so_pose_edge* edges, size_t n_edges,
                         const so_pose_graph_opts* opts, double* out7, double* edge_weights, so_pose_graph_result* result) {
     Ctx* c = reinterpret_cast<Ctx*>(ctx);
@@ -742,10 +782,33 @@ int so_pose_graph_solve(so_ctx* ctx, const double* init7, size_t n_nodes, const 
     pg_defaults(&o);
     if (opts) o = *opts;
     { int rc = graph_check(n_nodes, edges, n_edges, o); if (rc) return rc; }
-    for (size_t k = 0; k < n_nodes; ++k)
-        if (!finite_quat(init7 + 7 * k)) return fail(SO_ERR_ARG, "so_pose_graph_solve: init pose " + std::to_string(k) + " not finite or with a zero-norm quaternion");
+    { int rc = check_init(init7, n_nodes); if (rc) return rc; }
     SO_CUDA_TRY(cudaSetDevice(c->device));
-    return pg_solve(c, init7, uint32_t(n_nodes), edges, uint32_t(n_edges), o, out7, edge_weights, result);
+    std::vector<uint8_t> constant(n_nodes, 0);
+    constant[o.fixed] = 1;
+    return pg_solve(c, init7, uint32_t(n_nodes), edges, uint32_t(n_edges), constant.data(), o.max_iterations, out7, edge_weights, result);
+}
+
+int so_pose_graph_check_constant(size_t n_nodes, const so_pose_edge* edges, size_t n_edges, const uint8_t* constant,
+                                 const so_pose_graph_opts* opts) {
+    so_pose_graph_opts o;
+    pg_defaults(&o);
+    if (opts) o = *opts;
+    return graph_check_constant(n_nodes, edges, n_edges, constant, o.max_iterations);
+}
+
+int so_pose_graph_solve_constant(so_ctx* ctx, const double* init7, size_t n_nodes, const so_pose_edge* edges, size_t n_edges,
+                                 const uint8_t* constant, const so_pose_graph_opts* opts, double* out7, double* edge_weights,
+                                 so_pose_graph_result* result) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c || !init7 || !out7) return fail(SO_ERR_ARG, "so_pose_graph_solve_constant: NULL ctx, init7 or out7");
+    so_pose_graph_opts o;
+    pg_defaults(&o);
+    if (opts) o = *opts;
+    { int rc = graph_check_constant(n_nodes, edges, n_edges, constant, o.max_iterations); if (rc) return rc; }
+    { int rc = check_init(init7, n_nodes); if (rc) return rc; }
+    SO_CUDA_TRY(cudaSetDevice(c->device));
+    return pg_solve(c, init7, uint32_t(n_nodes), edges, uint32_t(n_edges), constant, o.max_iterations, out7, edge_weights, result);
 }
 
 }  // extern "C"
