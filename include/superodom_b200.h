@@ -360,7 +360,7 @@ typedef struct {
     int32_t i, j;             /* nodes of the edge, i != j */
     double z[7];              /* measured X_i^-1 X_j, pose7 */
     double sqrt_info[36];     /* S, row-major */
-    double cauchy;            /* c: 0 for no loss, > 0 for CauchyLoss(c) */
+    double cauchy;            /* c: 0 for no loss, > 0 for CauchyLoss(c) with c*c finite and normal (1.5e-154 <= c <= 1.3e154) */
 } so_pose_edge;
 typedef struct {
     int32_t fixed;            /* the node held constant, default 0 */

@@ -549,6 +549,12 @@ static int graph_edges_check(size_t n, const so_pose_edge* edges, size_t m, int3
         for (int k = 0; k < 36; ++k)
             if (!std::isfinite(E.sqrt_info[k])) return fail(SO_ERR_ARG, "so_pose_graph: sqrt_info not finite" + at);
         if (!std::isfinite(E.cauchy) || E.cauchy < 0.0) return fail(SO_ERR_ARG, "so_pose_graph: cauchy must be finite and >= 0" + at);
+        if (E.cauchy > 0.0) {                                             // k_pg_edges: b = c^2, 1 / b, b log(1 + s / b)
+            const double b = E.cauchy * E.cauchy;
+            if (!std::isfinite(b) || b < DBL_MIN)
+                return fail(SO_ERR_ARG, "so_pose_graph: cauchy out of range: its square " + std::string(std::isfinite(b) ? "is below DBL_MIN" : "overflows") +
+                                        ", so the loss would evaluate to NaN or inf (c > 0 must lie in about [1.5e-154, 1.3e154])" + at);
+        }
         parent[root(E.i)] = root(E.j);
     }
     for (size_t k = 0; k < n; ++k) parent[k] = root(int32_t(k));

@@ -3,7 +3,12 @@
 PoseGraph is a `prob` for test_ceres_restatement.solve_full over the free nodes' pose7 blocks (the fixed node is held inside the
 problem, so x_norm, the step norm and the gradient cover the free nodes only, as Ceres' reduced program does).  solve_sparse runs the
 same trust-region rules with the exact step from a sparse factorisation of the normal equations (scipy.sparse), for graphs too large
-for the dense restatement.  Edges are a POSE_EDGE_DTYPE array (superodom_b200.api)."""
+for the dense restatement; solve_chain the same with a banded factorisation, for graphs whose edges all join k and k +- 1.  Edges are
+a POSE_EDGE_DTYPE array (superodom_b200.api).
+
+The row helpers below (_rots, _qmul_rows, plus_blocks) are the row forms of test_ceres_restatement's _rot, _qmul and _plus with the
+same elementwise operations in the same order, so their results are bit-identical to the per-row calls
+(tests/test_pose_graph_edges_cpu.py)."""
 import numpy as np
 
 import test_ceres_restatement as CR
@@ -17,11 +22,28 @@ def _skew(v):
 
 
 def _rots(q):
-    return np.stack([CR._rot(r) for r in q])
+    """CR._rot of every row of q [m, 4] -> [m, 3, 3]"""
+    x, y, z, w = np.asarray(q, float).T
+    return np.stack([np.stack([1 - 2 * (y * y + z * z), 2 * (x * y - z * w), 2 * (x * z + y * w)], 1),
+                     np.stack([2 * (x * y + z * w), 1 - 2 * (x * x + z * z), 2 * (y * z - x * w)], 1),
+                     np.stack([2 * (x * z - y * w), 2 * (y * z + x * w), 1 - 2 * (x * x + y * y)], 1)], 1)
 
 
 def _qmul_rows(a, b):
-    return np.stack([CR._qmul(x, y) for x, y in zip(a, b)])
+    """CR._qmul of every row pair of a, b [m, 4] -> [m, 4]"""
+    ax, ay, az, aw = np.asarray(a, float).T
+    bx, by, bz, bw = np.asarray(b, float).T
+    return np.stack([aw * bx + ax * bw + ay * bz - az * by, aw * by - ax * bz + ay * bw + az * bx,
+                     aw * bz + ax * by - ay * bx + az * bw, aw * bw - ax * bx - ay * by - az * bz], 1)
+
+
+def plus_blocks(x, d):
+    """CR._plus_blocks: Plus of each pose7 block of x by its 6 tangent values in d.  np.vecdot runs the dot product np.linalg.norm
+    runs on one row, so the norms are the per-row ones bit for bit."""
+    X, D = np.asarray(x, float).reshape(-1, 7), np.asarray(d, float).reshape(-1, 6)
+    h = np.stack([D[:, 3] / 2, D[:, 4] / 2, D[:, 5] / 2, np.ones(len(D))], 1)
+    q = _qmul_rows(X[:, 3:], h)
+    return np.concatenate([X[:, :3] + D[:, :3], q / np.sqrt(np.vecdot(q, q))[:, None]], 1).ravel()
 
 
 def _jrinv_coeff(th):
@@ -136,20 +158,113 @@ class PoseGraph:
         return cost, res.ravel(), J
 
 
-def solve_sparse(prob, x0, max_iterations=50):
-    """solve_full's rules with the exact step from a sparse direct solve (scipy.sparse.linalg.spsolve) of
-    (Hs + D^2) y = gs.  -> dict as solve_full (margin over the same decisions; radius_error not estimated: 0)."""
-    import scipy.sparse as sp
-    import scipy.sparse.linalg as spl
-    x = np.array(x0, float)
-    cost, res, J = prob.sparse_jacobian(x)
-    initial_cost = cost
-    scale = 1.0 / (1.0 + np.sqrt(np.asarray(J.multiply(J).sum(0)).ravel()))
-    Sc = sp.diags(scale)
+class _SparseStep:
+    """The step of solve_sparse: the global Jacobian in scipy.sparse and a sparse direct solve (spsolve)."""
 
-    def gmax_of(xx, JJ, rr):
-        return np.abs(xx - CR._plus_blocks(xx, -(JJ.T @ rr))).max()
-    gmax = gmax_of(x, J, res)
+    def __init__(self, prob):
+        self.prob = prob
+
+    def linearise(self, x):
+        cost, self.res, self.J = self.prob.sparse_jacobian(x)
+        return cost, self.res
+
+    def column_norms2(self):
+        return np.asarray(self.J.multiply(self.J).sum(0)).ravel()
+
+    def gradient(self):
+        return self.J.T @ self.res
+
+    def system(self, scale):
+        """Hs = Js'Js and gs = Js'r of the scaled Jacobian Js = J diag(scale) -> the diagonal of Hs."""
+        import scipy.sparse as sp
+        self.Js = (self.J @ sp.diags(scale)).tocsc()
+        self.Hs = (self.Js.T @ self.Js).tocsc()
+        self.gs = self.Js.T @ self.res
+        return self.Hs.diagonal()
+
+    def solve(self, d):
+        """y of (Hs + diag(d)) y = gs"""
+        import scipy.sparse as sp
+        import scipy.sparse.linalg as spl
+        return spl.spsolve((self.Hs + sp.diags(d)).tocsc(), self.gs)
+
+    def model(self, step):
+        return self.Js @ step
+
+
+class _ChainStep:
+    """The step of solve_chain: per-edge blocks and a banded Cholesky solve (scipy.linalg.solveh_banded).  Every edge joins k and
+    k +- 1, so the free nodes' columns couple only to the next free node's and Hs + D^2 has 11 sub-diagonals; no global Jacobian is
+    formed, and a step costs O(n b^2)."""
+
+    def __init__(self, prob):
+        self.prob = prob
+        i, j = prob.E["i"].astype(np.int64), prob.E["j"].astype(np.int64)
+        assert (np.abs(i - j) == 1).all(), "solve_chain: an edge that does not join k and k +- 1"
+        self.ci, self.cj = prob.col[i], prob.col[j]                     # -1: a constant node
+        self.F = len(prob.free)
+        both = (self.ci >= 0) & (self.cj >= 0)
+        # edge-to-column sums as sparse products: P[c, e] = 1 where column block c is the edge's i (j) end; low[c], the block of
+        # rows c + 1 and columns c, takes the edges from c to c + 1 (fwd) and from c + 1 to c (rev)
+        self.Pi, self.Pj = self._scatter(self.ci, self.ci >= 0), self._scatter(self.cj, self.cj >= 0)
+        self.Pf, self.Pr = self._scatter(self.ci, both & (self.cj == self.ci + 1)), self._scatter(self.cj, both & (self.ci == self.cj + 1))
+
+    def _scatter(self, c, keep):
+        import scipy.sparse as sp
+        e = np.nonzero(keep)[0]
+        return sp.csr_matrix((np.ones(len(e)), (c[e], e)), shape=(self.F, len(c)))
+
+    def _sum(self, fi, fj, Pi=None, Pj=None):
+        """per free column block: the sum of fi over the edges' i ends and of fj over their j ends -> [F, ...]"""
+        Pi, Pj = (self.Pi, self.Pj) if Pi is None else (Pi, Pj)
+        m = len(fi)
+        return (Pi @ fi.reshape(m, -1) + Pj @ fj.reshape(m, -1)).reshape((self.F,) + fi.shape[1:])
+
+    def linearise(self, x):
+        cost, res, self.Ji, self.Jj = self.prob.blocks(x)
+        self.r = res
+        return cost, res.ravel()
+
+    def column_norms2(self):
+        return self._sum((self.Ji * self.Ji).sum(1), (self.Jj * self.Jj).sum(1)).ravel()
+
+    def gradient(self):
+        return self._sum(np.einsum("mki,mk->mi", self.Ji, self.r), np.einsum("mki,mk->mi", self.Jj, self.r)).ravel()
+
+    def system(self, scale):
+        s = np.vstack([scale.reshape(-1, 6), np.zeros((1, 6))])        # row -1: a constant node's columns are zero
+        self.Si, self.Sj = self.Ji * s[self.ci][:, None, :], self.Jj * s[self.cj][:, None, :]
+        tr = lambda A: np.transpose(A, (0, 2, 1))
+        D = self._sum(tr(self.Si) @ self.Si, tr(self.Sj) @ self.Sj)
+        self.gs = self._sum(np.einsum("mki,mk->mi", self.Si, self.r), np.einsum("mki,mk->mi", self.Sj, self.r)).ravel()
+        low = self._sum(tr(self.Sj) @ self.Si, tr(self.Si) @ self.Sj, self.Pf, self.Pr)
+        ab = np.zeros((12, 6 * self.F))                                 # lower band: ab[row - col, col]
+        for r in range(6):
+            for c in range(6):
+                if r >= c:
+                    ab[r - c, c::6] = D[:, r, c]
+                ab[6 + r - c, c:6 * (self.F - 1):6] = low[:-1, r, c]
+        self.ab = ab
+        return np.diagonal(D, axis1=1, axis2=2).ravel().copy()
+
+    def solve(self, d):
+        from scipy.linalg import solveh_banded
+        ab = self.ab.copy()
+        ab[0] += d
+        return solveh_banded(ab, self.gs, lower=True)
+
+    def model(self, step):
+        st = np.vstack([step.reshape(-1, 6), np.zeros((1, 6))])
+        return (np.einsum("mij,mj->mi", self.Si, st[self.ci]) + np.einsum("mij,mj->mi", self.Sj, st[self.cj])).ravel()
+
+
+def _solve_exact(lin, x0, max_iterations):
+    """solve_full's rules with the exact step of the linear algebra lin (_SparseStep or _ChainStep)."""
+    x = np.array(x0, float)
+    cost, res = lin.linearise(x)
+    initial_cost = cost
+    scale = 1.0 / (1.0 + np.sqrt(lin.column_norms2()))
+    gmax = np.abs(x - plus_blocks(x, -lin.gradient())).max()
     radius, decrease, reuse, diag = 1e4, 2.0, False, None
     it = succ = unsucc = invalid = 0
     step_ok, steps, margins = False, [], []
@@ -173,14 +288,12 @@ def solve_sparse(prob, x0, max_iterations=50):
             return done(4)
         it += 1
         step_ok = False
-        Js = (J @ Sc).tocsc()
-        Hs = (Js.T @ Js).tocsc()
-        gs = Js.T @ res
+        hs_diag = lin.system(scale)
         if not reuse:
-            diag = np.clip(Hs.diagonal(), CR.MIN_LM_DIAG, CR.MAX_LM_DIAG)
+            diag = np.clip(hs_diag, CR.MIN_LM_DIAG, CR.MAX_LM_DIAG)
         reuse = True
-        step = -spl.spsolve((Hs + sp.diags(diag / radius)).tocsc(), gs)
-        mr = Js @ step
+        step = -lin.solve(diag / radius)
+        mr = lin.model(step)
         model_change = -(mr * (res + mr / 2.0)).sum()
         if np.isfinite(step).all():
             margins.append(abs(model_change) / max(abs(mr * res).sum() + 0.5 * (mr * mr).sum(), np.finfo(float).tiny))
@@ -192,8 +305,8 @@ def solve_sparse(prob, x0, max_iterations=50):
             radius *= 0.5
             continue
         invalid = 0
-        cand = CR._plus_blocks(x, step * scale)
-        cand_cost = prob.cost(cand)
+        cand = plus_blocks(x, step * scale)
+        cand_cost = lin.prob.cost(cand)
         sn, tol = np.linalg.norm(x - cand), CR.PARAMETER_TOL * (np.linalg.norm(x) + CR.PARAMETER_TOL)
         margins.append(CR._rel_margin(sn, tol))
         if sn <= tol:
@@ -207,8 +320,8 @@ def solve_sparse(prob, x0, max_iterations=50):
         if rel > CR.MIN_REL_DECREASE:
             steps.append("a")
             x = cand
-            cost, res, J = prob.sparse_jacobian(x)
-            gmax = gmax_of(x, J, res)
+            cost, res = lin.linearise(x)
+            gmax = np.abs(x - plus_blocks(x, -lin.gradient())).max()
             step_ok = True
             radius = min(CR.MAX_RADIUS, radius / max(1.0 / 3.0, 1.0 - (2.0 * rel - 1.0) ** 3))
             decrease, reuse = 2.0, False
@@ -217,6 +330,18 @@ def solve_sparse(prob, x0, max_iterations=50):
             radius /= decrease
             decrease *= 2.0
             reuse = True
+
+
+def solve_sparse(prob, x0, max_iterations=50):
+    """solve_full's rules with the exact step from a sparse direct solve (scipy.sparse.linalg.spsolve) of
+    (Hs + D^2) y = gs.  -> dict as solve_full (margin over the same decisions; radius_error not estimated: 0)."""
+    return _solve_exact(_SparseStep(prob), x0, max_iterations)
+
+
+def solve_chain(prob, x0, max_iterations=50):
+    """solve_sparse for a graph whose edges all join k and k +- 1 (parallel and reversed edges, constant nodes anywhere), with the
+    exact step from the banded Cholesky factorisation of Hs + D^2 (11 sub-diagonals), assembled from the per-edge blocks."""
+    return _solve_exact(_ChainStep(prob), x0, max_iterations)
 
 
 # ------------------------------------------------------------------------------------------------------------------ problem families
@@ -250,11 +375,30 @@ def to_array(edges):
     return out
 
 
+def rotation(axis, angle):
+    """pose7 of a rotation by angle about axis"""
+    a = _unit(np.asarray(axis, float))
+    return np.r_[0.0, 0.0, 0.0, a * np.sin(angle / 2), np.cos(angle / 2)]
+
+
+def reversed_edge(e):
+    """(i, j, Z, S, c) stored as (j, i, Z^-1, S'): E' = Z X_j^-1 X_i = Z E^-1 Z^-1, whose residual is about -blkdiag(R_Z, R_Z) r, so
+    S' = S blkdiag(R_Z^T, R_Z^T) weighs it as S weighs r to first order (the references take any (i, j), exact or not)."""
+    i, j, z, S, c = e
+    Rt = CR._rot(z[3:]).T
+    B = np.zeros((6, 6))
+    B[:3, :3], B[3:, 3:] = Rt, Rt
+    return (j, i, inverse(z), S @ B, c)
+
+
 def drifted(rng, n, loops=0, step=1.0, noise=(0.02, 0.005), drift=(0.01, 0.003), sqrt_info=None, full_info=False, cauchy=0.0,
-            false_loops=0, dup=False, rank_def=False):
+            false_loops=0, dup=False, rank_def=False, reverse=0.0, both_ways=False, angles=None, max_span=None):
     """A random walk of n poses (truth), odometry edges measured with noise, `loops` revisit edges between random non-adjacent pairs
     measured from the truth, `false_loops` wrong Z between unrelated nodes, and the start: the odometry chained with drift.
-    -> (init [n, 7], edges list, truth)."""
+    dup: a second forward odometry edge at every third k; both_ways: a reversed one (reversed_edge of a second measurement) at every
+    third k; reverse: each edge stored reversed with this probability; angles: odometry edge k's measurement rotated by angles[k %
+    len(angles)] about a random axis, and the start chained from the true increments, so the start's residual rotations have these
+    angles (plus the drift); max_span: loop edges join nodes at most this far apart.  -> (init [n, 7], edges list, truth)."""
     truth = [np.r_[0, 0, 0, 0, 0, 0, 1.0]]
     for _ in range(n - 1):
         inc = np.r_[rng.normal(0, step, 3) * [1, 1, 0.2], _unit(np.r_[rng.normal(0, 0.15, 3), 1.0])]
@@ -277,12 +421,22 @@ def drifted(rng, n, loops=0, step=1.0, noise=(0.02, 0.005), drift=(0.01, 0.003),
     odo = []
     for k in range(n - 1):
         z = meas(k, k + 1, noise)
-        odo.append(z)
+        if angles is not None:
+            z = compose(z, rotation(rng.normal(size=3), angles[k % len(angles)]))
+            odo.append(compose(inverse(truth[k]), truth[k + 1]))
+        else:
+            odo.append(z)
         edges.append(edge(k, k + 1, z, info()))
         if dup and k % 3 == 0:
             edges.append(edge(k, k + 1, meas(k, k + 1, noise), info()))
+        if both_ways and k % 3 == 1:
+            edges.append(reversed_edge(edge(k, k + 1, meas(k, k + 1, noise), info())))
     for _ in range(loops):
-        i, j = sorted(rng.choice(n, 2, replace=False))
+        if max_span is None:
+            i, j = sorted(rng.choice(n, 2, replace=False))
+        else:
+            i = int(rng.integers(0, n - 2))
+            j = min(n - 1, i + int(rng.integers(2, max_span + 1)))
         if j - i < 2:
             j = min(n - 1, i + 2)
             if j - i < 2:
@@ -291,6 +445,9 @@ def drifted(rng, n, loops=0, step=1.0, noise=(0.02, 0.005), drift=(0.01, 0.003),
     for _ in range(false_loops):
         i, j = sorted(rng.choice(n, 2, replace=False))
         edges.append(edge(i, j, rand_pose(rng, 3.0, 0.3), info(), cauchy))
+    if reverse > 0.0:
+        flip = rng.random(len(edges)) < reverse
+        edges = [reversed_edge(e) if f else e for e, f in zip(edges, flip)]
     init = [truth[0]]
     for k in range(n - 1):
         d = np.r_[rng.normal(0, drift[0], 3), _unit(np.r_[rng.normal(0, drift[1] / 2, 3), 1.0])]
