@@ -281,7 +281,8 @@ int so_keyframe_download(so_ctx* ctx, int32_t id, int store, const double pose7[
  *     those blocks are dropped, as an insert drops them.
  * One filter over the union, not a replay of inserts (which average centroids of centroids): rebuilding at unchanged poses gives a
  * different, cleaner map than the live one.  The rebuilt stores hold their keyframes and nothing else: a prior map loaded with
- * so_map_set_points, and points free-space clearing removed, are not kept.  The index is rebuilt as by any map change.
+ * so_map_set_points, and points free-space clearing removed, are not kept (so_map_clear_free_space_keyframes clears the rebuilt map
+ * against the keyframes).  The index is rebuilt as by any map change.
  * SO_ERR_ARG, before any device work, for contexts on different devices, an id src does not hold, a non-finite pose or stores outside
  * 1..3.  SO_ERR_CAPACITY, with both stores as they were, when the window's points exceed max_map_points, the off-window blocks exceed
  * the archive, the window's blocks exceed the cell table, or 2^31 points or more are selected. */
@@ -439,6 +440,31 @@ int so_map_clear_free_space(so_ctx* ctx, int stores, const void* xyzi, size_t n,
  * or overwritten record (SO_ERR_ARG), and with SO_ERR_CAPACITY when the scan does not fit behind the surf window; SO_OK and nothing
  * removed before the first registration. */
 int so_map_clear_free_space_registered(so_ctx* ctx, int stores, const double pose[7], const so_free_space* opts, so_free_space_result* result);
+/* Clear dst's map against the surf clouds of src's keyframes ids[0..n_ids), keyframe ids[i] at poses7[i]: bit for bit what
+ *   for i in 0 .. n_ids-1: so_map_clear_free_space(dst, stores, <so_keyframe_download(src, ids[i], 0, NULL)>, poses7 + 7 i, opts)
+ * leaves -- the same points in both stores in the same order, the same index, the same n_removed -- with no host round trip.  One
+ * keyframe's decision on a map point reads only its own image and that point, so a point goes when any keyframe saw clearly past it,
+ * and each store that lost points is compacted once.  dst == src clears the map so_map_from_keyframes rebuilt, which brings back every
+ * point the live clearing had removed; dst != src (same device) clears another map, e.g. a prior map loaded with so_map_set_points,
+ * with a session's keyframes.  Duplicate ids are allowed.  Only the surf clouds are imaged; the window is carved, the block archive
+ * is not; a pending origin or resolution change is applied first; with nothing removed the stores are left bit for bit.  The
+ * keyframes are imaged in tiles of consecutive entries whose images fit 256 MiB (kFreeTileBytes, so_free_rule.h); the result does not
+ * depend on the tiling.  A keyframe is tested against a 50 m block only when its sensor position can lie within max_range of the block.
+ * SO_ERR_ARG before any device work, both stores as they were: every case of so_map_clear_free_space's options, stores outside 1..3,
+ * contexts on different devices, src without a keyframe store, NULL ids or poses7 with n_ids > 0, an id src does not hold, a pose that
+ * is not finite.  n_ids == 0 does nothing.  result may be NULL. */
+typedef struct {
+    uint64_t n_keyframes;           /* n_ids */
+    uint64_t n_image_points;        /* keyframe points that went into the images: the sum of the per-keyframe calls' counts */
+    uint64_t n_pixels_hit;          /* pixels with a return, summed over the keyframes' images */
+    uint64_t n_candidates;          /* map points with a fully observed neighbourhood in at least one keyframe, over the stores carved */
+    uint64_t n_removed;             /* map points removed, over the stores carved */
+    uint64_t n_after[2];            /* points in the surf and the edge window afterwards */
+    uint64_t n_tiles;               /* image tiles */
+    double time_ms;                 /* device time of the call (CUDA events) */
+} so_free_space_keyframes_result;
+int so_map_clear_free_space_keyframes(so_ctx* dst, so_ctx* src, const int32_t* ids, size_t n_ids, const double* poses7, int stores,
+                                      const so_free_space* opts, so_free_space_keyframes_result* result);
 
 /* ---- scan pre-filter (the step right before the path; SURVEY 8f row 2) ------------------------------------------ */
 /* replaces: laserMapping::adjustVoxelSize (src/LaserMapping/laserMapping.cpp:600-651) for the surf cloud: with

@@ -251,6 +251,21 @@ public:
         for (size_t i = 0; i < poses.size(); ++i) poses[i].to_pose7(p.data() + 7 * i);
         check(so_map_from_keyframes(ctx_->h, src.ctx_->h, ids.data(), ids.size(), p.data(), 3), "so_map_from_keyframes");
     }
+    // Shim only: this map cleared against the surf clouds of src's keyframes ids, keyframe ids[i] at poses[i]
+    // (so_map_clear_free_space_keyframes; stores: 1 surf, 2 edge, 3 both): the map clearFreeSpace of each keyframe in turn would leave,
+    // in one device call.  After buildFromKeyframes(*this, ...) it takes out again what the live clearing had removed; with another
+    // src it clears a prior map with a session's keyframes.
+    so_free_space_keyframes_result clearFreeSpaceFromKeyframes(const LocalMap& src, const std::vector<int32_t>& ids,
+                                                               const std::vector<Transformd>& poses, const so_free_space& opts, int stores = 3) {
+        if (ids.size() != poses.size()) throw Error("clearFreeSpaceFromKeyframes: one pose per keyframe id");
+        sync_resolution();
+        std::vector<double> p(7 * poses.size());
+        for (size_t i = 0; i < poses.size(); ++i) poses[i].to_pose7(p.data() + 7 * i);
+        so_free_space_keyframes_result r{};
+        check(so_map_clear_free_space_keyframes(ctx_->h, src.ctx_->h, ids.data(), ids.size(), p.data(), stores, &opts, &r),
+              "so_map_clear_free_space_keyframes");
+        return r;
+    }
     // Shim only: sessions (KeyframeIO.hpp; INTEGRATION.md "Sessions").  saveKeyframes writes every keyframe (pose, surf and edge
     // clouds in the sensor frame) and the caller's graph edges to one file; loadKeyframes appends a saved session's keyframes to this
     // map's store (so_keyframe_import) and returns the first new id, their count and the saved edges (node ids as saved: add `first`
@@ -659,6 +674,13 @@ public:
         for (size_t i = 0; i < ids.size(); ++i) ids[i] = int32_t(i);
         localMap.buildFromKeyframes(localMap, ids, corrected);
     }
+    // mergeKeyframes, then both stores cleared against every keyframe at its corrected pose (so_map_clear_free_space_keyframes with
+    // `clear`), so the merged map keeps out what either session's free-space clearing had removed.  last_keyframe_clear holds the result.
+    so_free_space_keyframes_result last_keyframe_clear{};
+    void mergeKeyframes(const std::vector<Transformd>& corrected, int32_t live_id, const so_free_space& clear) {
+        mergeKeyframes(corrected, live_id);
+        clearAllKeyframes(corrected, clear);
+    }
     // The map rebuilt from every keyframe at the corrected poses (one per keyframe, in id order), both stores; T_w_lidar and
     // last_T_w_lidar become the corrected pose of the last keyframe, so the next Localization() continues from the corrected map.
     void rebuildFromKeyframes(const std::vector<Transformd>& corrected) {
@@ -668,7 +690,22 @@ public:
         if (!corrected.empty()) { T_w_lidar = corrected.back(); last_T_w_lidar = T_w_lidar; }
         undistort_prev_pose = T_w_lidar;
     }
+    // rebuildFromKeyframes, then both stores cleared against every keyframe at its corrected pose (so_map_clear_free_space_keyframes
+    // with `clear`): with ClearFreeSpace on, the rebuilt map would otherwise bring back every point the live clearing removed.
+    // last_keyframe_clear holds the result.
+    void rebuildFromKeyframes(const std::vector<Transformd>& corrected, const so_free_space& clear) {
+        rebuildFromKeyframes(corrected);
+        clearAllKeyframes(corrected, clear);
+    }
 
+private:
+    void clearAllKeyframes(const std::vector<Transformd>& corrected, const so_free_space& clear) {
+        std::vector<int32_t> ids(corrected.size());
+        for (size_t i = 0; i < ids.size(); ++i) ids[i] = int32_t(i);
+        last_keyframe_clear = localMap.clearFreeSpaceFromKeyframes(localMap, ids, corrected, clear, 3);
+    }
+
+public:
     // LidarSLAM::EstimateLidarUncertainty (LidarSlam.cpp:915-975)
     void EstimateLidarUncertainty() {
         const auto& h = PlaneFeatureHistogramObs;

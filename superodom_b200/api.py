@@ -21,7 +21,7 @@ EXPORTS = [
     "so_map_set_resolution", "so_map_set_origin", "so_map_get_origin", "so_map_shift", "so_map_set_points",
     "so_map_set_edge_points", "so_map_add_surf", "so_map_add_edge", "so_map_add_scan", "so_map_add_registered_scan", "so_map_add_registered_edges", "so_map_add_scan_edge", "so_map_counts_5x5", "so_map_download", "so_map_size",
     "so_map_archive", "so_map_archive_info", "so_map_download_all",
-    "so_free_space_defaults", "so_map_clear_free_space", "so_map_clear_free_space_registered",
+    "so_free_space_defaults", "so_map_clear_free_space", "so_map_clear_free_space_registered", "so_map_clear_free_space_keyframes",
     "so_scan_prefilter", "so_scan_deskew", "so_scan_extract_uniform", "so_scan_extract_edges", "so_register", "so_register_prefiltered", "so_register_injected", "so_set_pose_sink", "so_register_batch", "so_register_batch_edges", "so_register_batch_device",
     "so_register_undistort", "so_register_undistort_edges", "so_register_prefiltered_undistort", "so_register_batch_undistort", "so_undistort_points", "so_register_optimized", "so_register_optimized_edges", "so_register_prefiltered_optimized", "so_register_batch_optimized", "so_evaluate_optimized", "so_evaluate_optimized_edges", "so_correspond", "so_correspond_seeded", "so_ordered_scans", "so_correspond_edge", "so_evaluate", "so_covariance",
     "so_register_degeneracy", "so_register_batch_degeneracy", "so_degeneracy_analysis", "so_solve", "so_solve_optimized",
@@ -162,6 +162,11 @@ class FreeSpace(C.Structure):
 class FreeSpaceResult(C.Structure):
     _fields_ = [("n_image_points", C.c_uint64), ("n_pixels_hit", C.c_uint64), ("n_candidates", C.c_uint64), ("n_removed", C.c_uint64),
                 ("n_after", C.c_uint64 * 2)]
+
+
+class FreeSpaceKeyframesResult(C.Structure):
+    _fields_ = [("n_keyframes", C.c_uint64), ("n_image_points", C.c_uint64), ("n_pixels_hit", C.c_uint64), ("n_candidates", C.c_uint64),
+                ("n_removed", C.c_uint64), ("n_after", C.c_uint64 * 2), ("n_tiles", C.c_uint64), ("time_ms", C.c_double)]
 
 
 def free_space(**kw) -> FreeSpace:
@@ -323,6 +328,8 @@ def load_library():
     L.so_map_clear_free_space.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p, C.c_void_p,
                                           C.c_void_p]
     L.so_map_clear_free_space_registered.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.so_map_clear_free_space_keyframes.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_int, C.c_void_p,
+                                                    C.c_void_p]
     L.so_scan_prefilter.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_int, C.c_void_p, C.c_void_p,
                                     C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
     L.so_scan_deskew.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_double, C.c_void_p, C.c_void_p, C.c_size_t,
@@ -786,6 +793,21 @@ class Context:
         self._chk(self.L.so_map_clear_free_space_registered(self.h, int(stores), _p(pose), C.byref(o), C.byref(r)),
                   "so_map_clear_free_space_registered")
         return self._free_result(r)
+
+    def map_clear_free_space_keyframes(self, src: "Context", ids, poses, opts: FreeSpace | None = None, stores: int = 1) -> dict:
+        """Clear this context's map against the surf clouds of src's keyframes ids at poses [n, 7], all at once: the map each
+        map_clear_free_space of a keyframe in turn leaves (src may be this context, e.g. after map_from_keyframes)."""
+        ids = np.ascontiguousarray(ids, dtype=np.int32).reshape(-1)
+        poses = np.ascontiguousarray(poses, dtype=np.float64).reshape(-1, 7)
+        if len(ids) != len(poses):
+            raise ValueError(f"map_clear_free_space_keyframes: {len(ids)} ids but {len(poses)} poses")
+        o = opts if opts is not None else free_space()
+        r = FreeSpaceKeyframesResult()
+        self._chk(self.L.so_map_clear_free_space_keyframes(self.h, src.h, _p(ids) if len(ids) else None, len(ids),
+                                                           _p(poses) if len(ids) else None, int(stores), C.byref(o), C.byref(r)),
+                  "so_map_clear_free_space_keyframes")
+        return dict(n_keyframes=r.n_keyframes, n_image_points=r.n_image_points, n_pixels_hit=r.n_pixels_hit, n_candidates=r.n_candidates,
+                    n_removed=r.n_removed, n_after=(r.n_after[0], r.n_after[1]), n_tiles=r.n_tiles, time_ms=r.time_ms)
 
     # ---- scan pre-filter
     def scan_prefilter(self, scan_xyzi: np.ndarray, line_res: float, plane_res: float, auto_voxel_size: bool = True, download: bool = True):

@@ -394,6 +394,14 @@ struct Ctx {
         DeviceBuffer<uint8_t> d_keep;                                      // [2][max_map_points] keep flags of the surf and edge windows
         DeviceBuffer<struct FreeCounters> d_cnt;                           // counters of one call
         PinnedBuffer<struct FreeCounters> h_cnt;                           // their mirror
+        // so_map_clear_free_space_keyframes: one tile's images in d_img, and for every selected keyframe its pool segment and pose
+        DeviceBuffer<struct KfImgSeg> d_kseg;
+        DeviceBuffer<struct FreePose> d_kpose;
+        DeviceBuffer<uint32_t> d_ccount, d_coff, d_clist;                  // per window block: candidate keyframes, offsets, the lists
+        DeviceBuffer<unsigned char> d_tmp;                                 // scan scratch
+        DeviceBuffer<struct FreeKfCounters> d_kcnt;                        // counters of one call
+        PinnedBuffer<struct FreeKfCounters> h_kcnt;                        // their mirror
+        Event ev[2];                                                       // start / end of the call's device work
     } fs;
 
     // ---- keyframes (so_keyframe_*, so_map_from_keyframes, so_register_keyframes): allocated on first use ---------------------------
@@ -506,6 +514,10 @@ int free_space_reserve_points(Ctx* c, size_t n);            // Ctx::fs.d_pts for
 // The range image of d_pts[0..n_pts) (sensor frame at pose), then every selected store carved against it; the stores are built
 int free_space_clear(Ctx* c, int stores, const float4* d_pts, uint32_t n_pts, const double pose[7], const so_free_space& o,
                      so_free_space_result* out);
+// The surf clouds of src's keyframes ids[0..n_ids) (n_ids > 0; ids and poses checked) imaged at poses7 and every selected store of c
+// carved against all of them: what so_map_clear_free_space of each keyframe in turn leaves; the stores are built
+int free_space_clear_keyframes(Ctx* c, Ctx* src, const int32_t* ids, size_t n_ids, const double* poses7, int stores, const so_free_space& o,
+                               so_free_space_keyframes_result* out);
 // so_api.cu: dst[0..n) = the registered scan (edges: its edge cloud) as the map inserts place it before the world transform
 int put_registered_scan(Ctx* c, bool edges, float4* dst, const double pose[7]);
 // so_keyframes.cu

@@ -227,4 +227,25 @@ int so_map_from_keyframes(so_ctx* dst_ctx, so_ctx* src_ctx, const int32_t* ids, 
     return SO_OK;
 }
 
+int so_map_clear_free_space_keyframes(so_ctx* dst_ctx, so_ctx* src_ctx, const int32_t* ids, size_t n_ids, const double* poses7, int stores,
+                                      const so_free_space* opts, so_free_space_keyframes_result* result) {
+    Ctx* d = reinterpret_cast<Ctx*>(dst_ctx);
+    Ctx* s = reinterpret_cast<Ctx*>(src_ctx);
+    if (!d || !s || (n_ids && (!ids || !poses7))) return fail(SO_ERR_ARG, "bad args");
+    static const double kIdentity[7] = {0, 0, 0, 0, 0, 0, 1};          // the options and stores alone: every pose is checked below
+    { int rc = free_space_check(opts, stores, kIdentity); if (rc) return rc; }
+    if (d->device != s->device) return fail(SO_ERR_ARG, "so_map_clear_free_space_keyframes: the two contexts are on different devices");
+    if (!s->kf.cap_frames) return fail(SO_ERR_ARG, "so_map_clear_free_space_keyframes needs a keyframe store in src (so_keyframe_reserve)");
+    { int rc = check_ids(s->kf, ids, n_ids); if (rc) return rc; }
+    for (size_t i = 0; i < n_ids; ++i)
+        if (!finite_pose(poses7 + 7 * i)) return fail(SO_ERR_ARG, "so_map_clear_free_space_keyframes: poses must be finite with a non-zero quaternion");
+    if (n_ids == 0) {
+        if (result) { *result = so_free_space_keyframes_result{}; result->n_after[0] = d->surf.n; result->n_after[1] = d->edge.n; }
+        return SO_OK;
+    }
+    SO_CUDA_TRY(cudaSetDevice(d->device));
+    int rc = free_space_prepare(d, stores);
+    return rc ? rc : free_space_clear_keyframes(d, s, ids, n_ids, poses7, stores, *opts, result);
+}
+
 }  // extern "C"
