@@ -466,6 +466,71 @@ typedef struct {
 int so_map_clear_free_space_keyframes(so_ctx* dst, so_ctx* src, const int32_t* ids, size_t n_ids, const double* poses7, int stores,
                                       const so_free_space* opts, so_free_space_keyframes_result* result);
 
+/* ---- loop verification: check a loop candidate before it becomes a pose-graph edge --------------------------------------------
+ * No reference counterpart.  A Scan Context match (so_loop_candidates) is appearance only, and look-alike places match closely
+ * (DESIGN.md §4, "Loop verification").  so_loop_verify builds each candidate's submap, aligns the query keyframe to it from the
+ * candidate's prior and scores the alignment with two tests that look-alike places fail in different ways: overlap (the query's points
+ * lie on the submap's surfaces) and visibility conflict (either side sees clearly through a surface the other one has).
+ * so_loop_prior (host only): the alignment prior of a candidate from the current poses of the candidate (cand7) and the query
+ * (query7) keyframes and its so_loop_candidate.yaw: the candidate's position, and the query's orientation turned about the world z
+ * axis by psi_cand + yaw - psi_query (psi = atan2(R10, R00), as the descriptor levels a keyframe), i.e. the candidate's heading plus
+ * yaw with the query's roll and pitch. */
+void so_loop_prior(const double cand7[7], const double query7[7], double yaw, double out7[7]);
+typedef struct {
+    int32_t half_window;      /* the submap is the candidate's ids +- half_window, 0..8; default 2 */
+    int32_t id_begin, id_end; /* the ids a submap may use: [id_begin, id_end) without the query; id_end < 0 (default -1): the ids
+                                 below query - exclude_recent, as so_loop_candidates selects them.  A range is for sessions. */
+    int32_t exclude_recent;   /* default 30 */
+    so_icp_opts icp;          /* the alignment; default max_icp_iters 20, max_surface_features 0 (the whole keyframe), lm 4 */
+    double inlier_dist;       /* metres: a query point is an inlier within this of the submap (d^2 <= float(inlier_dist^2)) */
+    so_free_space image;      /* the sensor's range-image options of the conflict tests (default: so_free_space_defaults, OS1-128) */
+    double min_overlap;       /* accepted only with overlap >= min_overlap */
+    double max_conflict;      /* ... and both conflict fractions <= max_conflict */
+} so_loop_verify_opts;
+typedef struct {
+    int32_t query, id;        /* the candidate as given */
+    int32_t skipped;          /* 1: an unused slot (id -1); nothing ran and every other field is 0 */
+    int32_t accepted;         /* 1: reg.status == 0, overlap >= min_overlap and both conflict fractions <= max_conflict */
+    so_icp_result reg;        /* the query aligned to the submap from so_loop_prior */
+    double rel7[7];           /* Z = X_id^-1 * reg.pose: the loop edge (id, query, Z) of so_pose_graph_solve */
+    int32_t n_submap_keyframes, pad_;
+    uint64_t n_submap_points; /* surf points of the submap (scratch's window) */
+    uint64_t n_query_points;  /* finite surf points of the query keyframe */
+    uint64_t n_inliers;       /* query points at reg.pose whose in-block nearest submap point lies within inlier_dist */
+    double overlap;           /* n_inliers / n_query_points (0 without points) */
+    double rmse;              /* sqrt(sum d^2 / n_inliers) over the inliers, metres (0 without inliers) */
+    uint64_t n_cand_query, n_conflict_query;   /* query points a submap keyframe's image observes / sees clearly past */
+    uint64_t n_cand_map, n_conflict_map;       /* submap points the query's image observes / sees clearly past */
+    double conflict_query;    /* n_conflict_query / n_cand_query (0 without candidates) */
+    double conflict_map;      /* n_conflict_map / n_cand_map (0 without candidates) */
+    double time_ms;           /* device time of this candidate (CUDA events on scratch's stream) */
+} so_loop_verify_result;
+/* The defaults above; inlier_dist, min_overlap and max_conflict as measured in DESIGN.md §4, "Loop verification". */
+void so_loop_verify_opts_defaults(so_loop_verify_opts* opts);
+/* Verify candidates c[0..n) (as so_loop_candidates / so_loop_candidates_range return them) of ctx's keyframes into out[0..n), one
+ * after another through the caller's scratch context (same device, not ctx), whose map is overwritten.  Per candidate (query q,
+ * id c; X_k the current pose of keyframe k):
+ *   1. submap ids: [c - w, c + w] intersected with the eligible ids, ascending; so_map_set_origin(scratch, X_c position), then
+ *      so_map_from_keyframes(scratch, ctx, ids, their X, 1);
+ *   2. so_register_keyframes(scratch, ctx, {q}, {so_loop_prior(X_c, X_q, c.yaw)}, &icp) -> reg: bit for bit this manual sequence;
+ *   3. overlap: the query's surf points at reg.pose, transformed as so_keyframe_download(reg.pose) transforms them; an inlier is a
+ *      finite point whose so_knn(k = 1, max_d2 = float(inlier_dist^2)) neighbour in scratch's surf store exists; sum d^2 in FP64 in
+ *      a fixed order (identical run to run);
+ *   4. conflicts, with the rule of so_map_clear_free_space: n_conflict_map / n_cand_map are n_removed / n_candidates of
+ *      so_map_clear_free_space(scratch, 1, <query's sensor-frame surf cloud>, reg.pose, image), counted, nothing removed;
+ *      n_conflict_query / n_cand_query are those of so_map_clear_free_space_keyframes(<a map of the finite points of step 3>, ctx,
+ *      submap ids, their X, 1, image);
+ *   5. accepted as so_loop_verify_result.accepted states.
+ * Each result equals a call with that candidate alone.  Nothing of ctx changes: its map, keyframes, poses, descriptors and
+ * registered scan.  A slot with id -1 comes back skipped with no device work.  SO_ERR_ARG before any device work: NULL arguments
+ * (c and out may be NULL with n = 0), scratch == ctx, contexts on different devices, ctx without a keyframe store, a query or id
+ * the store does not hold, id < -1, query == id, an id outside the eligible range, half_window outside 0..8, exclude_recent < 0,
+ * id_end >= 0 with id_begin < 0, id_end < id_begin or id_end past the keyframes, icp options so_register_keyframes refuses,
+ * inlier_dist not finite and positive, every case of so_map_clear_free_space's options, (2 half_window + 1) images over 256 MiB,
+ * min_overlap or max_conflict outside [0, 1].  Errors of the steps above are returned as they come, with out[0..i) filled. */
+int so_loop_verify(so_ctx* ctx, so_ctx* scratch, const so_loop_candidate* c, size_t n, const so_loop_verify_opts* opts,
+                   so_loop_verify_result* out);
+
 /* ---- scan pre-filter (the step right before the path; SURVEY 8f row 2) ------------------------------------------ */
 /* replaces: laserMapping::adjustVoxelSize (src/LaserMapping/laserMapping.cpp:600-651) for the surf cloud: with
  * auto_voxel_size, pick config_.lineRes/planeRes from the scan statistics (mean|x| * mean|y| * mean|z| < 25 -> 0.1/0.2,

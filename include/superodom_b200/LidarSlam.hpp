@@ -614,21 +614,30 @@ public:
         return out;
     }
     // The alignment prior of a candidate for alignKeyframes, from keyframePoses(): the candidate keyframe's position, its heading
-    // plus c.yaw, and the query's roll and pitch (the query's orientation turned about the world z axis by psi_c + yaw - psi_q,
-    // psi = atan2(R10, R00) as the descriptor levels it)
+    // plus c.yaw, and the query's roll and pitch (so_loop_prior)
     Transformd loopPrior(const so_loop_candidate& c) const {
         const std::vector<Transformd> p = keyframePoses();
         if (c.id < 0 || size_t(c.id) >= p.size() || c.query < 0 || size_t(c.query) >= p.size()) throw Error("loopPrior: no such keyframe");
-        auto heading = [](const Quaterniond& q) {
-            const double n = std::sqrt(q.x() * q.x() + q.y() * q.y() + q.z() * q.z() + q.w() * q.w());
-            const double x = q.x() / n, y = q.y() / n, z = q.z() / n, w = q.w() / n;
-            return std::atan2(2 * (x * y + z * w), 1 - 2 * (y * y + z * z));
-        };
-        const Transformd& cand = p[size_t(c.id)];
-        const Transformd& query = p[size_t(c.query)];
-        const double turn = heading(cand.rot) + c.yaw - heading(query.rot);
-        const Quaterniond qz(std::cos(turn / 2), 0, 0, std::sin(turn / 2));
-        return Transformd(qz * query.rot, cand.pos);
+        double cand[7], query[7], out[7];
+        p[size_t(c.id)].to_pose7(cand);
+        p[size_t(c.query)].to_pose7(query);
+        so_loop_prior(cand, query, c.yaw, out);
+        return Transformd::from_pose7(out);
+    }
+    // Loop verification (so_loop_verify with loopVerifyOpts): each candidate's submap built in `scratch` (its map is overwritten), the
+    // query aligned to it from loopPrior, and the alignment scored by overlap and visibility conflicts.  An accepted result's rel7 is
+    // the loop edge (id, query) for optimizeKeyframes.  Unused slots (id -1) come back skipped.
+    so_loop_verify_opts loopVerifyOpts = defaultLoopVerifyOpts();
+    static so_loop_verify_opts defaultLoopVerifyOpts() { so_loop_verify_opts o{}; so_loop_verify_opts_defaults(&o); return o; }
+    std::vector<so_loop_verify_result> verifyLoop(LocalMap& scratch, const std::vector<so_loop_candidate>& candidates,
+                                                  const so_loop_verify_opts& opts) {
+        scratch.sync_resolution();
+        std::vector<so_loop_verify_result> out(candidates.size());
+        check(so_loop_verify(context.h, scratch.ctx_->h, candidates.data(), candidates.size(), &opts, out.data()), "so_loop_verify");
+        return out;
+    }
+    std::vector<so_loop_verify_result> verifyLoop(LocalMap& scratch, const std::vector<so_loop_candidate>& candidates) {
+        return verifyLoop(scratch, candidates, loopVerifyOpts);
     }
     // loopCandidates over the keyframes [begin, end) only (so_loop_candidates_range with loopOpts; its exclude_recent is not used):
     // a live-session keyframe searched against an earlier session's ids, wherever they lie in the store

@@ -30,6 +30,7 @@ EXPORTS = [
     "so_keyframe_reserve", "so_keyframe_add_registered", "so_keyframe_import", "so_keyframe_info", "so_keyframe_poses", "so_keyframe_download", "so_map_from_keyframes",
     "so_register_keyframes",
     "so_loop_opts_defaults", "so_loop_candidates", "so_loop_candidates_range", "so_keyframe_descriptors",
+    "so_loop_prior", "so_loop_verify_opts_defaults", "so_loop_verify",
     "so_pose_graph_opts_defaults", "so_pose_graph_check", "so_pose_graph_solve", "so_pose_graph_check_constant", "so_pose_graph_solve_constant",
 ]
 
@@ -204,6 +205,49 @@ def loop_opts(**kw) -> LoopOpts:
             raise TypeError(f"so_loop_opts has no field {k}")
         setattr(o, k, v)
     return o
+
+
+class LoopVerifyOpts(C.Structure):
+    """so_loop_verify_opts: the submap (half_window, the eligible id range, exclude_recent), the alignment (icp), the overlap radius
+    (inlier_dist m), the range-image options of the conflict tests (image) and the decision thresholds."""
+    _fields_ = [("half_window", C.c_int32), ("id_begin", C.c_int32), ("id_end", C.c_int32), ("exclude_recent", C.c_int32),
+                ("icp", IcpOpts), ("inlier_dist", C.c_double), ("image", FreeSpace), ("min_overlap", C.c_double),
+                ("max_conflict", C.c_double)]
+
+
+class LoopVerifyResult(C.Structure):
+    _fields_ = [("query", C.c_int32), ("id", C.c_int32), ("skipped", C.c_int32), ("accepted", C.c_int32), ("reg", IcpResult),
+                ("rel7", C.c_double * 7), ("n_submap_keyframes", C.c_int32), ("pad_", C.c_int32), ("n_submap_points", C.c_uint64),
+                ("n_query_points", C.c_uint64), ("n_inliers", C.c_uint64), ("overlap", C.c_double), ("rmse", C.c_double),
+                ("n_cand_query", C.c_uint64), ("n_conflict_query", C.c_uint64), ("n_cand_map", C.c_uint64), ("n_conflict_map", C.c_uint64),
+                ("conflict_query", C.c_double), ("conflict_map", C.c_double), ("time_ms", C.c_double)]
+
+
+def loop_verify_opts(image: FreeSpace | dict | None = None, icp: dict | None = None, **kw) -> LoopVerifyOpts:
+    """so_loop_verify_opts_defaults, then the given fields; image: a FreeSpace or the fields of one over its defaults; icp: fields of
+    so_icp_opts over the defaults (max_icp_iters 20, max_surface_features 0, lm_max_iterations 4)."""
+    o = LoopVerifyOpts()
+    load_library().so_loop_verify_opts_defaults(C.byref(o))
+    if image is not None:
+        o.image = image if isinstance(image, FreeSpace) else free_space(**image)
+    for k, v in (icp or {}).items():
+        if not hasattr(o.icp, k):
+            raise TypeError(f"so_icp_opts has no field {k}")
+        setattr(o.icp, k, v)
+    for k, v in kw.items():
+        if not hasattr(o, k) or k in ("icp", "image"):
+            raise TypeError(f"so_loop_verify_opts has no field {k}")
+        setattr(o, k, v)
+    return o
+
+
+def loop_prior(cand7, query7, yaw: float) -> np.ndarray:
+    """Host-only so_loop_prior: the alignment prior of a loop candidate from the candidate's and the query's poses and its yaw."""
+    a = np.ascontiguousarray(cand7, dtype=np.float64)
+    b = np.ascontiguousarray(query7, dtype=np.float64)
+    out = np.zeros(7, np.float64)
+    load_library().so_loop_prior(_p(a), _p(b), float(yaw), _p(out))
+    return out
 
 
 # so_pose_edge, so_pose_graph_opts, so_pose_graph_result
@@ -419,6 +463,11 @@ def load_library():
     L.so_loop_candidates_range.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
                                            C.c_void_p]
     L.so_keyframe_descriptors.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
+    L.so_loop_prior.restype = None
+    L.so_loop_prior.argtypes = [C.c_void_p, C.c_void_p, C.c_double, C.c_void_p]
+    L.so_loop_verify_opts_defaults.restype = None
+    L.so_loop_verify_opts_defaults.argtypes = [C.c_void_p]
+    L.so_loop_verify.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
     L.so_pose_graph_opts_defaults.restype = None
     L.so_pose_graph_opts_defaults.argtypes = [C.c_void_p]
     L.so_pose_graph_check.argtypes = [C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]
@@ -744,6 +793,22 @@ class Context:
         out = np.zeros((len(i), max(o.rings, 1), max(o.sectors, 1)), np.float32)
         self._chk(self.L.so_keyframe_descriptors(self.h, _p(i), len(i), C.byref(o), _p(out)), "so_keyframe_descriptors")
         return out
+
+    # ---- loop verification (so_loop_verify)
+    def loop_prior(self, cand) -> np.ndarray:
+        """so_loop_prior of a candidate (a LOOP_CANDIDATE_DTYPE row) from this context's current keyframe poses."""
+        poses = self.keyframe_poses()
+        return loop_prior(poses[int(cand["id"])], poses[int(cand["query"])], float(cand["yaw"]))
+
+    def loop_verify(self, scratch: "Context", candidates, opts: LoopVerifyOpts | None = None, **kw) -> list:
+        """Verify loop candidates (LOOP_CANDIDATE_DTYPE, any shape; as loop_candidates returns them) of this context's keyframes
+        through the scratch context, whose map is overwritten -> [LoopVerifyResult] in the candidates' order.  kw: see
+        loop_verify_opts."""
+        c = np.ascontiguousarray(np.asarray(candidates, LOOP_CANDIDATE_DTYPE).reshape(-1))
+        o = opts if opts is not None else loop_verify_opts(**kw)
+        res = (LoopVerifyResult * max(len(c), 1))()
+        self._chk(self.L.so_loop_verify(self.h, scratch.h, _p(c) if len(c) else None, len(c), C.byref(o), res), "so_loop_verify")
+        return list(res)[: len(c)]
 
     # ---- pose graph (so_pose_graph_solve)
     def pose_graph_solve(self, init, edges, fixed: int = 0, max_iterations: int = 50, weights: bool = False, constant=None):

@@ -8,7 +8,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.environ.get("SO_LIB_OUT") or os.path.join(HERE, "libsuperodom_b200.so")
-SOURCES = ["so_icp.cu", "so_map.cu", "so_scan.cu", "so_reloc.cu", "so_global.cu", "so_undistort.cu", "so_motion.cu", "so_features.cu", "so_free.cu", "so_keyframes.cu", "so_loop.cu", "so_pose_graph.cu", "so_api.cu"]
+SOURCES = ["so_icp.cu", "so_map.cu", "so_scan.cu", "so_reloc.cu", "so_global.cu", "so_undistort.cu", "so_motion.cu", "so_features.cu", "so_free.cu", "so_keyframes.cu", "so_loop.cu", "so_pose_graph.cu", "so_verify.cu", "so_api.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 

@@ -408,6 +408,18 @@ struct Ctx {
     KeyframeStore kf;
     KeyframeScratch kfs;
 
+    // ---- loop verification (so_loop_verify, so_verify.cu), on the scratch context: allocated on first use, grown on demand -----------
+    struct Verify {
+        DeviceBuffer<float4> d_q;                                          // the query's surf points at the aligned pose
+        DeviceBuffer<uint32_t> d_img;                                      // the query's range image, then the submap keyframes' images
+        DeviceBuffer<struct KfImgSeg> d_kseg;                              // the submap keyframes' pool segments
+        DeviceBuffer<struct FreePose> d_kpose;                             // and their poses
+        DeviceBuffer<double> d_partials;                                   // per-CTA sums of d^2 over the inliers
+        DeviceBuffer<struct VerifyCounters> d_cnt;                         // counters of one candidate
+        PinnedBuffer<struct VerifyCounters> h_cnt;                         // their mirror
+        Event ev[2];                                                       // start / end of one candidate's device work
+    } ver;
+
     // ---- pose graph (so_pose_graph_solve, so_pose_graph.cu): allocated on first use, grown on demand ------------------------------
     // Two linearisation sets: [cur] at the iterate, [1 - cur] at the candidate of the last trial (an accepted step swaps them)
     struct Pg {

@@ -9,53 +9,10 @@
 
 #include <cub/cub.cuh>
 
-#include "so_ctx.cuh"
+#include "so_free.cuh"
 #include "so_free_rule.h"
 
 namespace so {
-
-constexpr uint32_t kUnknown = 0xFFFFFFFFu;     // pixel without a return: above the bits of every positive float (and of +inf)
-constexpr double kPiD = 3.141592653589793;
-
-// Image geometry and decision constants, all in double (angles in radians)
-struct FreeGrid {
-    double az_res, el_res, el_min, el_max;
-    int32_t W, H, d, pad;
-    double margin, margin_rel, min_range, max_range;
-};
-struct FreePose { double R[9]; double t[3]; };  // row-major R of the (normalised) pose quaternion; the map point goes to R^T (m - t)
-
-// Device counters of one call, read back once
-struct FreeCounters {
-    uint32_t image_points, pixels_hit;
-    uint32_t cand[2], removed[2];
-    uint32_t selected, pad;                     // cub::DeviceSelect's count (not read back: the host knows it)
-};
-
-// Pixel of a sensor-frame direction, or false when its elevation is outside [el_min, el_max).  Written without contractible
-// multiply-adds, so that a restatement in numpy takes the same roundings.
-__device__ __forceinline__ bool free_pixel(const FreeGrid& g, double x, double y, double z, int* row, int* col) {
-    double az = atan2(y, x);
-    if (az >= kPiD) az = __dsub_rn(az, 2.0 * kPiD);                  // [-pi, pi)
-    const double el = atan2(z, hypot(x, y));
-    if (!(el >= g.el_min && el < g.el_max)) return false;
-    const int r = int(floor(__ddiv_rn(__dsub_rn(el, g.el_min), g.el_res)));
-    if (r < 0 || r >= g.H) return false;
-    int c = int(floor(__ddiv_rn(__dadd_rn(az, kPiD), g.az_res)));
-    if (c > g.W - 1) c = g.W - 1;
-    *row = r; *col = c;
-    return true;
-}
-
-__device__ __forceinline__ double norm3(double x, double y, double z) {
-    return sqrt(__dadd_rn(__dadd_rn(__dmul_rn(x, x), __dmul_rn(y, y)), __dmul_rn(z, z)));
-}
-
-// warp-aggregated counter increment: one atomic per warp (every lane of the warp calls it)
-__device__ __forceinline__ void warp_count(uint32_t* ctr, bool flag) {
-    const unsigned b = __ballot_sync(0xffffffffu, flag);
-    if ((threadIdx.x & 31) == 0 && b) atomicAdd(ctr, uint32_t(__popc(b)));
-}
 
 __global__ void __launch_bounds__(256) k_range_image(const float4* __restrict__ pts, uint32_t n, FreeGrid g, uint32_t* __restrict__ img,
                                                      FreeCounters* __restrict__ cnt) {
@@ -77,38 +34,6 @@ __global__ void __launch_bounds__(256) k_range_image(const float4* __restrict__ 
     warp_count(&cnt->pixels_hit, first);
 }
 
-// The decision on map point p against one image: true when it is removed; *cand when its neighbourhood is fully observed.  The range
-// test comes before any pixel work.
-__device__ __forceinline__ bool free_decide(const FreeGrid& g, const FreePose& P, const float4 p, const uint32_t* __restrict__ img, bool* cand) {
-    const double dx = __dsub_rn(double(p.x), P.t[0]), dy = __dsub_rn(double(p.y), P.t[1]), dz = __dsub_rn(double(p.z), P.t[2]);
-    auto rt = [&](int a) {                                              // row a of R^T (m - t): column a of R
-        return __dadd_rn(__dadd_rn(__dmul_rn(dx, P.R[a]), __dmul_rn(dy, P.R[3 + a])), __dmul_rn(dz, P.R[6 + a]));
-    };
-    const double qx = rt(0), qy = rt(1), qz = rt(2);
-    const double rm = norm3(qx, qy, qz);
-    int row, col;
-    if (rm >= g.min_range && rm <= g.max_range && free_pixel(g, qx, qy, qz, &row, &col) && row - g.d >= 0 && row + g.d < g.H) {
-        uint32_t mn = kUnknown;
-        bool known = true;
-        for (int dr = -g.d; dr <= g.d && known; ++dr) {
-            const uint32_t* line = img + size_t(row + dr) * g.W;
-            for (int dc = -g.d; dc <= g.d; ++dc) {
-                int c = (col + dc) % g.W;
-                if (c < 0) c += g.W;
-                const uint32_t v = line[c];
-                if (v == kUnknown) { known = false; break; }
-                mn = min(mn, v);
-            }
-        }
-        if (known) {
-            *cand = true;
-            const double thr = __dadd_rn(rm, fmax(g.margin, __dmul_rn(g.margin_rel, rm)));
-            return double(__uint_as_float(mn)) > thr;
-        }
-    }
-    return false;
-}
-
 // keep[i] = 0 when window point i is removed
 __global__ void __launch_bounds__(256) k_free_mark(const float4* __restrict__ pts, uint32_t n, FreeGrid g, FreePose P,
                                                    const uint32_t* __restrict__ img, uint8_t* __restrict__ keep,
@@ -127,20 +52,9 @@ __global__ void __launch_bounds__(256) k_free_mark(const float4* __restrict__ pt
 // so_map_clear_free_space_keyframes: the clearing of every selected keyframe at once.  One keyframe's decision on a map point reads
 // only its own image and that point, so a point goes when any keyframe removes it.  Keyframes are imaged a tile at a time (kFreeTileBytes
 // of images), the keep flags carry from tile to tile, and each store that lost points is compacted once at the end.
-struct KfImgSeg { uint64_t src; uint32_t start, n; };      // tile entry j: pool[src .. src + n) are points start .. start + n of the tile
 struct FreeOrigin { int32_t o[3]; };
-struct FreeKfCounters {
-    unsigned long long image_points, pixels_hit;
-    unsigned long long cand[2], removed[2];
-    uint32_t selected, pad;                     // cub::DeviceSelect's count (not read back: the host knows it)
-};
 // keep flags of the keyframe form: 0 removed, 1 kept, 3 kept and a candidate of some keyframe already (counted once)
 constexpr uint8_t kKeep = 1, kKeepCand = 3;
-
-__device__ __forceinline__ void warp_count64(unsigned long long* ctr, bool flag) {
-    const unsigned b = __ballot_sync(0xffffffffu, flag);
-    if ((threadIdx.x & 31) == 0 && b) atomicAdd(ctr, (unsigned long long)__popc(b));
-}
 
 // The range images of one tile, one thread per keyframe point read in place from the pool; image j at imgs + j * W * H.  Each pixel
 // keeps its minimum as k_range_image keeps it.
@@ -266,7 +180,16 @@ int free_space_prepare(Ctx* c, int stores) {
 
 int free_space_reserve_points(Ctx* c, size_t n) { return c->fs.d_pts.reserve(std::max<size_t>(n, 1)); }
 
-static FreeGrid free_grid(const so_free_space& o) {
+void launch_range_image(const float4* pts, uint32_t n, const FreeGrid& g, uint32_t* img, FreeCounters* cnt, cudaStream_t st) {
+    if (n) k_range_image<<<(n + 255) / 256, 256, 0, st>>>(pts, n, g, img, cnt);
+}
+
+void launch_range_images(const float4* pool, const KfImgSeg* segs, uint32_t n_segs, uint32_t n, const FreeGrid& g, uint32_t* imgs,
+                         FreeKfCounters* cnt, cudaStream_t st) {
+    if (n) k_range_images<<<(n + 255) / 256, 256, 0, st>>>(pool, segs, n_segs, n, g, imgs, cnt);
+}
+
+FreeGrid free_grid(const so_free_space& o) {
     FreeGrid g{};
     g.az_res = double(o.az_res_deg) * (kPiD / 180.0); g.el_res = double(o.el_res_deg) * (kPiD / 180.0);
     g.el_min = double(o.el_min_deg) * (kPiD / 180.0); g.el_max = double(o.el_max_deg) * (kPiD / 180.0);
@@ -277,7 +200,7 @@ static FreeGrid free_grid(const so_free_space& o) {
     return g;
 }
 
-static FreePose free_pose(const double pose[7]) {
+FreePose free_pose(const double pose[7]) {
     FreePose P{};
     const double* q = pose + 3;
     const double nq = std::sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
