@@ -510,7 +510,8 @@ void so_loop_verify_opts_defaults(so_loop_verify_opts* opts);
 /* Verify candidates c[0..n) (as so_loop_candidates / so_loop_candidates_range return them) of ctx's keyframes into out[0..n), one
  * after another through the caller's scratch context (same device, not ctx), whose map is overwritten.  Per candidate (query q,
  * id c; X_k the current pose of keyframe k):
- *   1. submap ids: [c - w, c + w] intersected with the eligible ids, ascending; so_map_set_origin(scratch, X_c position), then
+ *   1. submap ids: [c - w, c + w] intersected with the eligible ids, ascending; scratch's edge store emptied
+ *      (so_map_set_edge_points(scratch, NULL, 0)), so_map_set_origin(scratch, X_c position), then
  *      so_map_from_keyframes(scratch, ctx, ids, their X, 1);
  *   2. so_register_keyframes(scratch, ctx, {q}, {so_loop_prior(X_c, X_q, c.yaw)}, &icp) -> reg: bit for bit this manual sequence;
  *   3. overlap: the query's surf points at reg.pose, transformed as so_keyframe_download(reg.pose) transforms them; an inlier is a

@@ -157,7 +157,10 @@ static int verify_one(Ctx* c, Ctx* s, const so_loop_candidate& cd, const so_loop
     SO_CUDA_TRY(cudaEventRecord(v.ev[0], st));
     so_ctx* hc = reinterpret_cast<so_ctx*>(c);
     so_ctx* hs = reinterpret_cast<so_ctx*>(s);
-    int rc = so_map_set_origin(hs, xc, nullptr);
+    // scratch's edge store emptied first: the submap is scratch's whole map, so nothing scratch held before enters a result
+    // (reg.map_edge_5x5 counted the edge points an earlier use left there)
+    int rc = (s->edge.n || s->edge.arc.d_pool) ? so_map_set_edge_points(hs, nullptr, 0, 16, 12) : SO_OK;
+    if (!rc) rc = so_map_set_origin(hs, xc, nullptr);
     if (!rc) rc = so_map_from_keyframes(hs, hc, ids.data(), ids.size(), poses.data(), 1);
     if (rc) return rc;
     // 2. the alignment from the candidate's prior
