@@ -1,8 +1,8 @@
 // so_pose_graph.cu -- sparse SE(3) pose-graph least squares on the device (so_pose_graph_solve), sm_90a, FP64.
 //
-// The problem and its trust-region rules: include/superodom_b200.h and DESIGN.md section 4, "Pose graph".  The rules are those of
-// so_trust_region.cuh (DESIGN.md section 3), restated here on the host: that loop runs on one thread over a dense system in shared
-// memory, this one over kernels and a control block read back once per trust-region trial.
+// The problem and its trust-region rules: include/superodom_b200.h and DESIGN.md section 4, "Pose graph".  The rules are those of the
+// registration's solve, shared with it through so_trust_region_rule.h: that loop runs on one thread over a dense system in shared
+// memory (so_trust_region.cuh), this one on the host over kernels and a control block read back once per trust-region trial.
 //   k_pg_edges     one thread per edge: E = Z^-1 X_i^-1 X_j, r, the Cauchy weight, the corrected Jacobians, the edge's blocks
 //                  A_ii, A_jj, A_ij, its gradient parts and 1/2 rho
 //   k_pg_nodes     one thread per node: its incident edges' blocks summed in incidence order (ascending edge id), the chain block
@@ -30,6 +30,12 @@ namespace cg = cooperative_groups;
 constexpr double kPcgTol = 1e-10;
 constexpr int kPcgMaxIter = 1000;
 constexpr int kTrialThreads = 256;
+
+// The trust-region state of pg_solve, with IcpState's member names for the rules of so_trust_region_rule.h
+struct PgTrState {
+    double radius, decrease_factor, x_norm, gmax, cost;
+    int32_t lm_iter, lm_max_iterations, num_successful, num_unsuccessful, reuse_diagonal, consecutive_invalid, termination;
+};
 
 struct PgEdgeBlk { double aii[36], ajj[36], aij[36], gi[6], gj[6]; };
 struct PgCtl {
@@ -441,7 +447,7 @@ __global__ void __launch_bounds__(kTrialThreads) k_pg_trial(PgTrialArgs a) {
         const uint32_t k = i / 6, t = i % 6;
         if (!a.reuse_diagonal) {
             const double s = a.scale[i];
-            a.diag[i] = a.constant[k] ? 1.0 : fmin(fmax(s * s * a.H[36 * size_t(k) + t * 7], 1e-6), 1e32);
+            a.diag[i] = a.constant[k] ? 1.0 : tr_lm_diagonal(s * s * a.H[36 * size_t(k) + t * 7]);
         }
         a.dd[i] = a.diag[i] / a.radius;
         a.b[i] = a.constant[k] ? 0.0 : a.scale[i] * a.g[i];               // gs
@@ -681,13 +687,14 @@ static int pg_solve(Ctx* c, const double* init7, uint32_t n, const so_pose_edge*
     PgCtl& h = *g.h_ctl;
     SO_CUDA_TRY(cudaMemcpyAsync(g.h_ctl, g.d_ctl, sizeof(PgCtl), cudaMemcpyDeviceToHost, c->stream));
     SO_CUDA_TRY(cudaStreamSynchronize(c->stream));
-    // TrustRegionMinimizer: the rules of so_trust_region.cuh (tr_start, tr_continue, tr_after_eval), restated over the kernels above
+    // TrustRegionMinimizer over the kernels above, in the exit order of so_trust_region.cuh's loop
+    PgTrState st{};
+    st.lm_max_iterations = max_iterations;
+    st.cost = h.cost[cur]; st.gmax = h.gmax[cur]; st.x_norm = std::sqrt(h.xnorm2[cur]);
+    tr_iteration_zero(st);
     so_pose_graph_result r{};
-    double cost = h.cost[cur], gmax = h.gmax[cur], x_norm = std::sqrt(h.xnorm2[cur]);
-    r.initial_cost = cost;
-    double radius = 1e4, decrease = 2.0;
-    bool reuse = false, step_ok = false;
-    int invalid = 0, term = 0;
+    r.initial_cost = st.cost;
+    bool step_ok = false;
     PgTrialArgs ta{};
     ta.E = g.d_edges; ta.inc = g.d_inc;
     ta.scale = g.d_scale; ta.diag = g.d_diag; ta.dd = g.d_dd;
@@ -699,17 +706,17 @@ static int pg_solve(Ctx* c, const double* init7, uint32_t n, const so_pose_edge*
     // one thread per node, at most the co-resident CTAs; a function of n and the device only, so the reductions' order is fixed
     const uint32_t blocks = std::max<uint32_t>(1, std::min<uint32_t>(uint32_t(g.max_blocks), (n + kTrialThreads - 1) / kTrialThreads));
     for (;;) {
-        if (step_ok) r.successful++; else r.unsuccessful++;
-        if (r.iterations >= max_iterations) { term = 0; break; }
-        if (gmax <= 1e-10) { term = 1; break; }
-        if (radius <= 1e-32) { term = 4; break; }
-        r.iterations++;
+        tr_count(st, step_ok);
+        if (tr_at_limit(st)) { st.termination = kTermIterations; break; }
+        if (tr_gradient_small(st)) { st.termination = kTermGradient; break; }
+        if (tr_radius_small(st)) { st.termination = kTermRadius; break; }
+        st.lm_iter++;
         step_ok = false;
         ta.blk = g.d_blk[cur]; ta.x = g.d_x[cur]; ta.H = g.d_H[cur]; ta.C = g.d_C[cur]; ta.g = g.d_g[cur];
         ta.xc = g.d_x[1 - cur];
-        ta.reuse_diagonal = reuse ? 1 : 0;
-        ta.radius = radius;
-        reuse = true;
+        ta.reuse_diagonal = st.reuse_diagonal;
+        ta.radius = st.radius;
+        st.reuse_diagonal = 1;
         {
             void* args[] = {&ta};
             SO_CUDA_TRY(cudaLaunchCooperativeKernel((const void*)k_pg_trial, dim3(blocks), dim3(kTrialThreads), args, 0, c->stream));
@@ -720,27 +727,23 @@ static int pg_solve(Ctx* c, const double* init7, uint32_t n, const so_pose_edge*
         SO_CUDA_TRY(cudaMemcpyAsync(g.h_ctl, g.d_ctl, sizeof(PgCtl), cudaMemcpyDeviceToHost, c->stream));
         SO_CUDA_TRY(cudaStreamSynchronize(c->stream));
         r.pcg_iterations += uint64_t(h.pcg_iters);
-        const double mcc = h.mcc;
-        if (!h.valid || !(mcc > 0.0)) {                                   // HandleInvalidStep
-            if (++invalid >= 5) { term = 5; break; }
-            radius *= 0.5;
+        if (!tr_step_valid(h.valid, h.mcc)) {                             // HandleInvalidStep
+            if (tr_invalid_step(st)) { st.termination = kTermInvalid; break; }
             continue;
         }
-        invalid = 0;
+        tr_valid_step(st);
         const double cand_cost = h.cost[1 - cur];
-        if (std::sqrt(h.step_norm2) <= 1e-8 * (x_norm + 1e-8)) { term = 2; break; }       // ParameterToleranceReached
-        const double change = cost - cand_cost;
-        if (std::fabs(change) <= 1e-6 * cost) { term = 3; break; }                          // FunctionToleranceReached
-        const double rd = change / mcc;
-        if (rd > 1e-3) {                                                  // HandleSuccessfulStep
+        if (tr_parameter_small(st, h.step_norm2)) { st.termination = kTermParameter; break; }
+        const double change = st.cost - cand_cost;
+        if (tr_function_small(st, change)) { st.termination = kTermFunction; break; }
+        const double rd = change / h.mcc;
+        if (tr_step_rejected(rd)) {                                       // StepRejected
+            tr_rejected(st);
+        } else {                                                          // HandleSuccessfulStep
             cur = 1 - cur;
-            cost = cand_cost; gmax = h.gmax[cur]; x_norm = std::sqrt(h.xnorm2[cur]);
-            const double t = 2.0 * rd - 1.0;
-            radius = std::fmin(1e16, radius / std::fmax(1.0 / 3.0, 1.0 - t * t * t));
-            decrease = 2.0; reuse = false;
+            st.cost = cand_cost; st.gmax = h.gmax[cur]; st.x_norm = std::sqrt(h.xnorm2[cur]);
+            tr_accepted(st, rd);
             step_ok = true;
-        } else {                                                          // StepRejected
-            radius = radius / decrease; decrease *= 2.0; reuse = true;
         }
     }
     SO_CUDA_TRY(cudaMemcpyAsync(x.data(), g.d_x[cur], x.size() * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
@@ -751,8 +754,8 @@ static int pg_solve(Ctx* c, const double* init7, uint32_t n, const so_pose_edge*
     float ms = 0.f;
     SO_CUDA_TRY(cudaEventElapsedTime(&ms, g.ev[0], g.ev[1]));
     std::memcpy(out7, x.data(), x.size() * sizeof(double));
-    r.termination = term;
-    r.final_cost = cost; r.gmax = gmax; r.radius = radius;
+    r.iterations = st.lm_iter; r.successful = st.num_successful; r.unsuccessful = st.num_unsuccessful; r.termination = st.termination;
+    r.final_cost = st.cost; r.gmax = st.gmax; r.radius = st.radius;
     r.time_ms = ms;
     if (res) *res = r;
     return SO_OK;

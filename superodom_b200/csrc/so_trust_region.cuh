@@ -5,8 +5,9 @@
 // TrustRegionMinimizer::Minimize, LevenbergMarquardtStrategy::ComputeStep/StepAccepted/StepRejected and the monotonic
 // TrustRegionStepEvaluator, expressed on the robustified normal equations H = sum rho' J^T J, g = sum rho' J^T r
 // (the QR of [J;D] that DENSE_QR performs solves exactly (H + D^2) y = g).  It runs on one thread of a step kernel, on shared-memory
-// copies of the scan's states.  The loop (tr_begin_solve / tr_start / tr_continue / tr_after_eval) owns the policy: exit order and
-// thresholds, step quality, radius rule, diagonal clamp, the ICP break rule (end_solve).  A parameter-block policy P supplies what
+// copies of the scan's states.  The loop (tr_begin_solve / tr_start / tr_continue / tr_after_eval) owns the control flow: the exit
+// order and the ICP break rule (end_solve); every threshold, the step quality, the radius rule and the diagonal clamp come from
+// so_trust_region_rule.h, which the pose graph's host loop shares.  A parameter-block policy P supplies what
 // differs between the forms (so_icp.cu: Ambient and Reduced, six columns, and DegStart;
 // so_motion.cu: TwoBlock, twelve):
 //   N, kSums                     tangent columns; reduced sums per evaluation (upper triangle of H, g, cost)
@@ -19,8 +20,12 @@
 //   open_prior(acc, n_ok) / prior_at_candidate(acc)  the prior rows at the iterate (solve start) and at the candidate
 //   next(ok)                     the policy's __noinline__ entry of tr_continue
 #include "so_internal.cuh"
+#include "so_trust_region_rule.h"
 
 namespace so {
+
+// The registration's own termination code beside so_trust_region_rule.h's 0-5: a solve without rows
+constexpr int kTermNoRows = 6;
 
 // Copy of a state between global and shared memory by the CTA's threads, as 8-byte words
 template <class T>
@@ -168,17 +173,17 @@ __device__ __forceinline__ void tr_continue(const P& p, bool step_successful) {
     constexpr int N = P::N;
     IcpState& st = p.st;
     for (;;) {
-        if (step_successful) st.num_successful++; else st.num_unsuccessful++;
-        if (st.lm_iter >= st.lm_max_iterations) { st.termination = 0; end_solve(st); return; }
-        if (st.gmax <= 1e-10) { st.termination = 1; end_solve(st); return; }
-        if (st.radius <= 1e-32) { st.termination = 4; end_solve(st); return; }
+        tr_count(st, step_successful);
+        if (tr_at_limit(st)) { st.termination = kTermIterations; end_solve(st); return; }
+        if (tr_gradient_small(st)) { st.termination = kTermGradient; end_solve(st); return; }
+        if (tr_radius_small(st)) { st.termination = kTermRadius; end_solve(st); return; }
         st.lm_iter++;
         step_successful = false;
         // LevenbergMarquardtStrategy::ComputeStep on the Jacobi-scaled system
         double Hs[N * N], gs[N];
         p.scaled_system(Hs, gs);
         if (!st.reuse_diagonal)
-            _Pragma("unroll") for (int j = 0; j < N; ++j) p.diag()[j] = fmin(fmax(Hs[j * N + j], 1e-6), 1e32);
+            _Pragma("unroll") for (int j = 0; j < N; ++j) p.diag()[j] = tr_lm_diagonal(Hs[j * N + j]);
         st.reuse_diagonal = 1;
         double M[N * N], y[N];
         _Pragma("unroll") for (int i = 0; i < N * N; ++i) M[i] = Hs[i];
@@ -193,12 +198,11 @@ __device__ __forceinline__ void tr_continue(const P& p, bool step_successful) {
             _Pragma("unroll") for (int i = 0; i < N; ++i) { sg += step[i] * gs[i]; double t = 0.0; _Pragma("unroll") for (int j = 0; j < N; ++j) t += Hs[i * N + j] * step[j]; sHs += step[i] * t; }
             mcc = -sg - 0.5 * sHs;
         }
-        if (!valid || !(mcc > 0.0)) {           // HandleInvalidStep
-            if (++st.consecutive_invalid >= 5) { st.termination = 5; end_solve(st); return; }
-            st.radius *= 0.5; st.reuse_diagonal = 1;
+        if (!tr_step_valid(valid, mcc)) {       // HandleInvalidStep
+            if (tr_invalid_step(st)) { st.termination = kTermInvalid; end_solve(st); return; }
             continue;
         }
-        st.consecutive_invalid = 0;
+        tr_valid_step(st);
         st.model_cost_change = mcc;
         double delta[N];
         _Pragma("unroll") for (int j = 0; j < N; ++j) delta[j] = step[j] * p.scale()[j];
@@ -220,7 +224,7 @@ __device__ __forceinline__ void tr_begin_solve(const P& p, const double* acc_in,
     st.n_ok = n_ok;
     _Pragma("unroll") for (int i = 0; i < 7; ++i) st.x_iter_start[i] = st.x[i];
     st.lm_iter = 0; st.num_successful = 0; st.num_unsuccessful = 0; st.consecutive_invalid = 0; st.termination = 0;
-    if (n_ok == 0 && !st.use_prior) { st.termination = 6; end_solve(st); return; }      // use_prior: see end_solve
+    if (n_ok == 0 && !st.use_prior) { st.termination = kTermNoRows; end_solve(st); return; }      // use_prior: see end_solve
     if ((P::kAnyNonFinite || st.n_ok_edge > 0) && !isfinite(st.cost)) {
         // A row's loss weight is not finite (ScaledLoss(TukeyLoss, w) with w = NaN: a line fit on an exactly collinear neighbourhood,
         // whose mean squared distance is rounding noise of either sign).  The reference CHECK-fails in ceres::Corrector here (Ceres
@@ -242,7 +246,7 @@ __device__ __forceinline__ void tr_start(const P& p) {
     p.init_scale();                                 // jacobi_scaling at iteration 0
     st.x_norm = sqrt(p.x_norm2());
     st.gmax = p.gmax();
-    st.radius = 1e4; st.decrease_factor = 2.0; st.reuse_diagonal = 0;
+    tr_iteration_zero(st);
     p.next(false);
 }
 
@@ -254,24 +258,21 @@ __device__ __forceinline__ void tr_after_eval(const P& p, const double* acc_in) 
     _Pragma("unroll") for (int k = 0; k < P::kSums; ++k) acc[k] = acc_in[k];
     p.prior_at_candidate(acc);
     const double cand_cost = acc[P::kSums - 1];
-    const double sn = sqrt(p.step_norm2());
-    if (sn <= 1e-8 * (st.x_norm + 1e-8)) { st.termination = 2; end_solve(st); return; }      // ParameterToleranceReached
+    if (tr_parameter_small(st, p.step_norm2())) { st.termination = kTermParameter; end_solve(st); return; }
     const double cost_change = st.cost - cand_cost;
-    if (fabs(cost_change) <= 1e-6 * st.cost) { st.termination = 3; end_solve(st); return; }  // FunctionToleranceReached
+    if (tr_function_small(st, cost_change)) { st.termination = kTermFunction; end_solve(st); return; }
     const double rd = cost_change / st.model_cost_change;
-    if (rd > 1e-3) {        // HandleSuccessfulStep
+    if (tr_step_rejected(rd)) {         // StepRejected
+        tr_rejected(st);
+        p.next(false);
+    } else {                            // HandleSuccessfulStep
         p.accept();
         st.x_norm = sqrt(p.x_norm2());
         p.take(acc);
         st.cost = cand_cost;
         st.gmax = p.gmax();
-        const double t = 2.0 * rd - 1.0;
-        st.radius = fmin(1e16, st.radius / fmax(1.0 / 3.0, 1.0 - t * t * t));
-        st.decrease_factor = 2.0; st.reuse_diagonal = 0;
+        tr_accepted(st, rd);
         p.next(true);
-    } else {                // StepRejected
-        st.radius = st.radius / st.decrease_factor; st.decrease_factor *= 2.0; st.reuse_diagonal = 1;
-        p.next(false);
     }
 }
 

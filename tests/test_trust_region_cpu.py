@@ -5,7 +5,7 @@ rejection, the radius recovering, the gradient-tolerance exit, and rejections wi
 Reusing the diagonal after a rejection and recomputing it there cannot be told apart: a rejected step leaves H and g as they were, so
 the recomputed diagonal is the same bits.  Only the recompute after an accepted step is observable.
 
-Two exits stay unreached, in every copy of the loop:
+Two exits stay unreached by every solve (tests/test_trust_region_rule_cpu.py reaches both on the rules themselves):
   * termination 4 (radius <= 1e-32): from 1e4 it takes 15 rejections in a row -- the radius falls by 2, 4, 8, ... -- so at least 16
     LM iterations, the device's cap.  Long before that the step is tiny and the parameter or function tolerance ends the solve:
     test_sixteen_iterations_do_not_reach_the_radius_floor runs the rejecting families at 16 iterations and finds no solve there.
@@ -13,8 +13,8 @@ Two exits stay unreached, in every copy of the loop:
     The damped system M = H + D / radius is positive definite (D >= 1e-6) for every finite input, so y = M^-1 g is finite, and the model
     cost change of the step -y is y'g - y'H y / 2 = y'H y / 2 + y'(D / radius) y, positive in exact arithmetic whenever g != 0; with
     g = 0 the gradient tolerance exits first.  Only rounding on a g at the edge of underflow could make it non-positive.
-Whether Ceres 2.0's LevenbergMarquardtStrategy::StepIsInvalid halves the radius (as all three copies do) or divides it by the decrease
-factor is not pinned: no copy of the loop can reach that branch to tell.
+Whether Ceres 2.0's LevenbergMarquardtStrategy::StepIsInvalid halves the radius (as so_trust_region_rule.h and every restatement do)
+or divides it by the decrease factor is not pinned: no solve can reach that branch to tell.
 """
 import numpy as np
 
