@@ -531,6 +531,8 @@ void so_loop_verify_opts_defaults(so_loop_verify_opts* opts);
  * min_overlap or max_conflict outside [0, 1].  Errors of the steps above are returned as they come, with out[0..i) filled. */
 int so_loop_verify(so_ctx* ctx, so_ctx* scratch, const so_loop_candidate* c, size_t n, const so_loop_verify_opts* opts,
                    so_loop_verify_result* out);
+/* The degeneracy-aware form, so_loop_verify_degeneracy, and the loop edge's information, so_loop_edge_information, follow
+ * so_register_keyframes_degeneracy under "degeneracy-aware registration" below. */
 
 /* ---- scan pre-filter (the step right before the path; SURVEY 8f row 2) ------------------------------------------ */
 /* replaces: laserMapping::adjustVoxelSize (src/LaserMapping/laserMapping.cpp:600-651) for the surf cloud: with
@@ -753,6 +755,31 @@ int so_register_degeneracy(so_ctx* ctx, const void* surf_xyzi, size_t n_surf, co
 int so_register_batch_degeneracy(so_ctx* ctx, const void* surf_xyzi, const uint32_t* n_points, const void* edge_xyzi, const uint32_t* n_edge,
                                  size_t n_scans, size_t stride_bytes, size_t intensity_offset, const double* poses_in, const so_degeneracy* d,
                                  const so_icp_opts* opts, so_degeneracy_result* results);
+/* ... of keyframes as so_register_keyframes (d[n]: one per keyframe), returning SO_OK as it does.  A single keyframe gives, bit for
+ * bit, what so_register_degeneracy gives on the cloud so_keyframe_download(src, id, 0, NULL) returns: pose, covariance, iteration
+ * counts, flags, *_info and *_axes.  Argument errors: those of so_register_keyframes and of so_register_degeneracy's d, before any
+ * device work. */
+int so_register_keyframes_degeneracy(so_ctx* dst, so_ctx* src, const int32_t* ids, size_t n, const double* priors7,
+                                     const so_degeneracy* d, const so_icp_opts* opts, so_degeneracy_result* results);
+/* so_loop_verify with the degeneracy-aware alignment (DESIGN.md §4, "Loop verification"): in a corridor, a tunnel or along a long
+ * wall the alignment has no information along some direction and stays at the prior there, which puts the query at the candidate's
+ * position; neither score sees it.  Steps 1, 3, 4 and 5 as so_loop_verify; step 2 is
+ *   so_register_keyframes_degeneracy(scratch, ctx, {q}, {so_loop_prior(X_c, X_q, c.yaw)}, d, &icp) -> deg[i], reg = deg[i].icp
+ * (one d for every candidate), so deg[i] holds the analysis of candidate i's last ICP iteration; a skipped slot gets a zeroed deg[i].
+ * The accept rule is so_loop_verify's.  With d->constrain = 0, or nothing flagged, every field of out equals so_loop_verify's bit
+ * for bit (the timings aside).  Build the loop edge's S with so_loop_edge_information(out[i].reg.pose, deg + i, S).  SO_ERR_ARG
+ * before any device work: every case of so_loop_verify, a NULL d (or deg with n > 0), and d values so_register_degeneracy refuses. */
+int so_loop_verify_degeneracy(so_ctx* ctx, so_ctx* scratch, const so_loop_candidate* c, size_t n, const so_loop_verify_opts* opts,
+                              const so_degeneracy* d, so_loop_verify_result* out, so_degeneracy_result* deg);
+/* Host only: the square-root information of the loop edge (id, query, Z = rel7) of a degeneracy-aware verification, without the
+ * directions its alignment left unconstrained: out = S (I - P), P = blockdiag(sum a_k a_k^T, sum b_k b_k^T) over the translation
+ * eigenvectors flagged in deg->flags_pos, a_k = R^T deg->pos_axes[k] (R the rotation of reg_pose7, the alignment's reg.pose), and the
+ * rotation ones flagged in deg->flags_ori, b_k = deg->ori_axes[k].  (The registration adds translation in the world frame and turns
+ * on the right; a step (dt, dtheta) at reg_pose7 moves the edge's residual by t_E = R^T dt, Log R_E = dtheta.)  S and out: 6x6
+ * row-major, order x, y, z, rx, ry, rz, as so_pose_edge.sqrt_info; out may alias S.  No flag set: out is a byte copy of S.  The pose
+ * graph leaves an unobserved direction to the other edges (DESIGN.md §4 "Pose graph").  SO_ERR_ARG, out untouched: a NULL
+ * argument, a non-finite pose, S or axis, a zero quaternion, flags outside 0..7. */
+int so_loop_edge_information(const double reg_pose7[7], const so_degeneracy_result* deg, const double S[36], double out[36]);
 /* Test hook: the analysis above on a given symmetric H (row-major 6x6, upper triangle read), by the device code a solve begins with,
  * in a one-thread launch.  Fills pos_info, pos_axes, ori_info, ori_axes and the flags; zeroes the rest.  Replaces the state a
  * preceding so_correspond* left for so_evaluate. */

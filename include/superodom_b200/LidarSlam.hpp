@@ -639,6 +639,35 @@ public:
     std::vector<so_loop_verify_result> verifyLoop(LocalMap& scratch, const std::vector<so_loop_candidate>& candidates) {
         return verifyLoop(scratch, candidates, loopVerifyOpts);
     }
+    // The same with the degeneracy-aware alignment (so_loop_verify_degeneracy): in a corridor or along a long wall the alignment is
+    // held along the directions it cannot measure, and `degeneracy[i]` says which; build candidate i's edge with loopEdge.
+    // DESIGN.md, "Loop verification", gives the recommended thresholds (translation 0.2, rotation 0.1).
+    struct VerifiedLoops { std::vector<so_loop_verify_result> results; std::vector<so_degeneracy_result> degeneracy; };
+    VerifiedLoops verifyLoop(LocalMap& scratch, const std::vector<so_loop_candidate>& candidates, const so_degeneracy& d,
+                             const so_loop_verify_opts& opts) {
+        scratch.sync_resolution();
+        VerifiedLoops out;
+        out.results.resize(candidates.size());
+        out.degeneracy.resize(candidates.size());
+        check(so_loop_verify_degeneracy(context.h, scratch.ctx_->h, candidates.data(), candidates.size(), &opts, &d, out.results.data(),
+                                        out.degeneracy.data()), "so_loop_verify_degeneracy");
+        return out;
+    }
+    VerifiedLoops verifyLoop(LocalMap& scratch, const std::vector<so_loop_candidate>& candidates, const so_degeneracy& d) {
+        return verifyLoop(scratch, candidates, d, loopVerifyOpts);
+    }
+    // The loop edge (v.id, v.query, Z = v.rel7) of an accepted degeneracy-aware verification for optimizeKeyframes: S (6x6 row-major,
+    // x, y, z, rx, ry, rz; from stated sigmas) without the directions the alignment left unconstrained (so_loop_edge_information), so
+    // the graph takes them from the other edges; `cauchy` as so_pose_edge.cauchy
+    static so_pose_edge loopEdge(const so_loop_verify_result& v, const so_degeneracy_result& deg, const double S[36], double cauchy) {
+        so_pose_edge e{};
+        e.i = v.id;
+        e.j = v.query;
+        for (int k = 0; k < 7; ++k) e.z[k] = v.rel7[k];
+        check(so_loop_edge_information(v.reg.pose, &deg, S, e.sqrt_info), "so_loop_edge_information");
+        e.cauchy = cauchy;
+        return e;
+    }
     // loopCandidates over the keyframes [begin, end) only (so_loop_candidates_range with loopOpts; its exclude_recent is not used):
     // a live-session keyframe searched against an earlier session's ids, wherever they lie in the store
     std::vector<so_loop_candidate> loopCandidatesIn(int32_t id, int32_t k, int32_t begin, int32_t end) {

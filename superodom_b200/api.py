@@ -28,9 +28,9 @@ EXPORTS = [
     "so_knn", "so_knn_device", "so_sampling_indices", "so_localize_global", "so_localize_scores", "so_localize_global_size", "so_localize_global_bnb", "so_localize_bnb_keys", "so_localize_bnb_bounds", "so_map_bounds", "so_map_bounds_all", "so_kernel_launches", "so_bytes_copied", "so_build_flags", "so_profile_enable", "so_profile_get",
     "so_knn_graph", "so_knn_graph_stats",
     "so_keyframe_reserve", "so_keyframe_add_registered", "so_keyframe_import", "so_keyframe_info", "so_keyframe_poses", "so_keyframe_download", "so_map_from_keyframes",
-    "so_register_keyframes",
+    "so_register_keyframes", "so_register_keyframes_degeneracy",
     "so_loop_opts_defaults", "so_loop_candidates", "so_loop_candidates_range", "so_keyframe_descriptors",
-    "so_loop_prior", "so_loop_verify_opts_defaults", "so_loop_verify",
+    "so_loop_prior", "so_loop_verify_opts_defaults", "so_loop_verify", "so_loop_verify_degeneracy", "so_loop_edge_information",
     "so_pose_graph_opts_defaults", "so_pose_graph_check", "so_pose_graph_solve", "so_pose_graph_check_constant", "so_pose_graph_solve_constant",
 ]
 
@@ -250,6 +250,25 @@ def loop_prior(cand7, query7, yaw: float) -> np.ndarray:
     return out
 
 
+def loop_edge_information(reg_pose, deg: DegeneracyResult, S) -> np.ndarray:
+    """Host-only so_loop_edge_information: the square-root information S [6, 6] (or its diagonal, 6 values) of a loop edge with the
+    directions deg flags (a loop_verify_degeneracy result) left out -> [6, 6].  Raises SuperOdomError (.code SO_ERR_ARG) as the C call
+    fails."""
+    L = load_library()
+    p = np.ascontiguousarray(reg_pose, dtype=np.float64)
+    s = np.asarray(S, np.float64)
+    s = np.ascontiguousarray(np.diag(s) if s.shape == (6,) else s.reshape(6, 6))
+    if p.shape != (7,):
+        raise ValueError(f"reg_pose: a pose7, got shape {p.shape}")
+    out = np.zeros((6, 6), np.float64)
+    rc = L.so_loop_edge_information(_p(p), C.byref(deg), _p(s), _p(out))
+    if rc < 0:
+        err = SuperOdomError(f"so_loop_edge_information failed ({rc}): " + L.so_last_error().decode())
+        err.code = rc
+        raise err
+    return out
+
+
 # so_pose_edge, so_pose_graph_opts, so_pose_graph_result
 POSE_EDGE_DTYPE = np.dtype([("i", "<i4"), ("j", "<i4"), ("z", "<f8", 7), ("sqrt_info", "<f8", 36), ("cauchy", "<f8")], align=True)
 
@@ -457,6 +476,8 @@ def load_library():
     L.so_keyframe_download.argtypes = [C.c_void_p, C.c_int32, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
     L.so_map_from_keyframes.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_int]
     L.so_register_keyframes.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.so_register_keyframes_degeneracy.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                   C.c_void_p]
     L.so_loop_opts_defaults.restype = None
     L.so_loop_opts_defaults.argtypes = [C.c_void_p]
     L.so_loop_candidates.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
@@ -468,6 +489,8 @@ def load_library():
     L.so_loop_verify_opts_defaults.restype = None
     L.so_loop_verify_opts_defaults.argtypes = [C.c_void_p]
     L.so_loop_verify.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
+    L.so_loop_verify_degeneracy.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.so_loop_edge_information.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     L.so_pose_graph_opts_defaults.restype = None
     L.so_pose_graph_opts_defaults.argtypes = [C.c_void_p]
     L.so_pose_graph_check.argtypes = [C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]
@@ -766,6 +789,20 @@ class Context:
         self._chk(self.L.so_register_keyframes(self.h, src.h, _p(ids), len(ids), _p(priors), C.byref(o), res), "so_register_keyframes")
         return list(res)
 
+    def register_keyframes_degeneracy(self, src: "Context", ids, priors, ds, max_icp_iters: int, max_surface_features: int = 0, **kw):
+        """register_keyframes with the degeneracy-aware solve; ds: one Degeneracy per keyframe, or one for all -> [DegeneracyResult]"""
+        ids = np.ascontiguousarray(ids, dtype=np.int32)
+        priors = np.ascontiguousarray(priors, dtype=np.float64).reshape(-1, 7)
+        assert len(ids) == len(priors)
+        ds = [ds] * len(ids) if isinstance(ds, Degeneracy) else list(ds)
+        assert len(ds) == len(ids)
+        da = (Degeneracy * max(len(ids), 1))(*ds)
+        o = self._opts(max_icp_iters, max_surface_features, **kw)
+        res = (DegeneracyResult * max(len(ids), 1))()
+        self._chk(self.L.so_register_keyframes_degeneracy(self.h, src.h, _p(ids), len(ids), _p(priors), da, C.byref(o), res),
+                  "so_register_keyframes_degeneracy")
+        return list(res)[: len(ids)]
+
     # ---- loop detection over the keyframes (Scan Context; descriptors cached per keyframe, computed by these calls)
     def loop_candidates(self, queries, k: int, opts: LoopOpts | None = None, stats: bool = False, ids=None, **kw):
         """For each query keyframe its k best eligible keyframes -> structured array [n, k] of LOOP_CANDIDATE_DTYPE (distance
@@ -809,6 +846,17 @@ class Context:
         res = (LoopVerifyResult * max(len(c), 1))()
         self._chk(self.L.so_loop_verify(self.h, scratch.h, _p(c) if len(c) else None, len(c), C.byref(o), res), "so_loop_verify")
         return list(res)[: len(c)]
+
+    def loop_verify_degeneracy(self, scratch: "Context", candidates, d: Degeneracy, opts: LoopVerifyOpts | None = None, **kw):
+        """loop_verify with the degeneracy-aware alignment (so_loop_verify_degeneracy; d: a Degeneracy, see degeneracy()) ->
+        ([LoopVerifyResult], [DegeneracyResult]); loop_edge_information(r.reg.pose, deg, S) gives the edge's square-root information."""
+        c = np.ascontiguousarray(np.asarray(candidates, LOOP_CANDIDATE_DTYPE).reshape(-1))
+        o = opts if opts is not None else loop_verify_opts(**kw)
+        res = (LoopVerifyResult * max(len(c), 1))()
+        deg = (DegeneracyResult * max(len(c), 1))()
+        self._chk(self.L.so_loop_verify_degeneracy(self.h, scratch.h, _p(c) if len(c) else None, len(c), C.byref(o), C.byref(d), res, deg),
+                  "so_loop_verify_degeneracy")
+        return list(res)[: len(c)], list(deg)[: len(c)]
 
     # ---- pose graph (so_pose_graph_solve)
     def pose_graph_solve(self, init, edges, fixed: int = 0, max_iterations: int = 50, weights: bool = False, constant=None):

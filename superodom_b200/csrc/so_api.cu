@@ -854,6 +854,16 @@ int put_registered_scan(Ctx* c, bool edges, float4* dst, const double pose[7]) {
     }
 }
 
+// so_degeneracy values of the degeneracy-aware entry points (so_register_degeneracy*, so_loop_verify_degeneracy, so_solve)
+int check_degeneracy(const so_degeneracy* d, size_t n) {
+    for (size_t s = 0; s < n; ++s) {
+        if (!(d[s].pos_threshold >= 0.0 && d[s].pos_threshold < 1.0) || !(d[s].ori_threshold >= 0.0 && d[s].ori_threshold < 1.0))
+            return fail(SO_ERR_ARG, "degeneracy thresholds must be in [0, 1)");
+        if (d[s].constrain != 0 && d[s].constrain != 1) return fail(SO_ERR_ARG, "so_degeneracy.constrain must be 0 or 1");
+    }
+    return SO_OK;
+}
+
 }  // namespace so
 
 // =================================================================================================== C ABI
@@ -1426,13 +1436,9 @@ int so_register_batch_device(so_ctx* ctx, const void* d_scans, const uint32_t* n
 }
 
 // Keyframes of src registered against dst's map as so_register_batch_device registers device scans: mode NONE (a keyframe is already
-// compensated), dst's registered-scan record untouched
-int so_register_keyframes(so_ctx* dst_ctx, so_ctx* src_ctx, const int32_t* ids, size_t n, const double* priors7, const so_icp_opts* opts,
-                          so_icp_result* results) {
-    Ctx* c = reinterpret_cast<Ctx*>(dst_ctx);
-    Ctx* s = reinterpret_cast<Ctx*>(src_ctx);
-    if (!c || !s || !ids || !priors7 || !opts || !results) return fail(SO_ERR_ARG, "bad args");
-    if (c->device != s->device) return fail(SO_ERR_ARG, "so_register_keyframes: the two contexts are on different devices");
+// compensated), dst's registered-scan record untouched.  degen: NULL, or one DegenState per keyframe (so_register_keyframes_degeneracy)
+static int register_keyframes(Ctx* c, Ctx* s, const int32_t* ids, size_t n, const double* priors7, const so_icp_opts* opts,
+                              so_icp_result* results, DegenState* degen) {
     SO_CUDA_TRY(cudaSetDevice(c->device));
     const float4* scans = nullptr;
     std::vector<uint32_t> n_points;
@@ -1441,18 +1447,20 @@ int so_register_keyframes(so_ctx* dst_ctx, so_ctx* src_ctx, const int32_t* ids, 
     if (rc) return rc;
     RegisterRequest q = batch_request(scans, n_points.data(), n, 16, 12, priors7, opts, results);
     q.src = Source::DEVICE;
+    q.degen = degen;
     return register_scans(c, q);
 }
 
-// ---- degeneracy-aware registration: so_register's schedule with k_lm_step_deg stepping the solves (DESIGN.md section 3)
-static int check_degeneracy(const so_degeneracy* d, size_t n) {
-    for (size_t s = 0; s < n; ++s) {
-        if (!(d[s].pos_threshold >= 0.0 && d[s].pos_threshold < 1.0) || !(d[s].ori_threshold >= 0.0 && d[s].ori_threshold < 1.0))
-            return fail(SO_ERR_ARG, "degeneracy thresholds must be in [0, 1)");
-        if (d[s].constrain != 0 && d[s].constrain != 1) return fail(SO_ERR_ARG, "so_degeneracy.constrain must be 0 or 1");
-    }
-    return SO_OK;
+int so_register_keyframes(so_ctx* dst_ctx, so_ctx* src_ctx, const int32_t* ids, size_t n, const double* priors7, const so_icp_opts* opts,
+                          so_icp_result* results) {
+    Ctx* c = reinterpret_cast<Ctx*>(dst_ctx);
+    Ctx* s = reinterpret_cast<Ctx*>(src_ctx);
+    if (!c || !s || !ids || !priors7 || !opts || !results) return fail(SO_ERR_ARG, "bad args");
+    if (c->device != s->device) return fail(SO_ERR_ARG, "so_register_keyframes: the two contexts are on different devices");
+    return register_keyframes(c, s, ids, n, priors7, opts, results, nullptr);
 }
+
+// ---- degeneracy-aware registration: so_register's schedule with k_lm_step_deg stepping the solves (DESIGN.md section 3)
 static DegenState degen_state(const so_degeneracy& d) {
     DegenState s{};
     s.pos_thr2 = d.pos_threshold * d.pos_threshold;
@@ -1510,6 +1518,24 @@ int so_register_batch_degeneracy(so_ctx* ctx, const void* surf, const uint32_t* 
     rc = register_scans(c, q);
     if (rc) return rc;
     for (size_t s = 0; s < n_scans; ++s) { results[s].icp = icp[s]; fill_degeneracy(S[s], results + s); }
+    return SO_OK;
+}
+
+// so_register_keyframes with the degeneracy-aware step, as so_register_batch_degeneracy adds it to so_register_batch
+int so_register_keyframes_degeneracy(so_ctx* dst_ctx, so_ctx* src_ctx, const int32_t* ids, size_t n, const double* priors7,
+                                     const so_degeneracy* d, const so_icp_opts* opts, so_degeneracy_result* results) {
+    Ctx* c = reinterpret_cast<Ctx*>(dst_ctx);
+    Ctx* s = reinterpret_cast<Ctx*>(src_ctx);
+    if (!c || !s || !ids || !priors7 || !d || !opts || !results) return fail(SO_ERR_ARG, "bad args");
+    if (c->device != s->device) return fail(SO_ERR_ARG, "so_register_keyframes_degeneracy: the two contexts are on different devices");
+    int rc = check_degeneracy(d, n);
+    if (rc) return rc;
+    std::vector<so_icp_result> icp(std::max<size_t>(n, 1));
+    std::vector<DegenState> S(std::max<size_t>(n, 1));
+    for (size_t k = 0; k < n; ++k) S[k] = degen_state(d[k]);
+    rc = register_keyframes(c, s, ids, n, priors7, opts, icp.data(), S.data());
+    if (rc) return rc;
+    for (size_t k = 0; k < n; ++k) { results[k].icp = icp[k]; fill_degeneracy(S[k], results + k); }
     return SO_OK;
 }
 

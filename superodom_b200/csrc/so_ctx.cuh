@@ -458,6 +458,7 @@ void count_d2h(Ctx* c, size_t b);
 void timed_launch_begin(Ctx* c);
 void timed_launch_end(Ctx* c, int cls);                     // counts one launch; profile class cls when profiling
 int icp_opts_check(const so_icp_opts& o);                   // max_icp_iters and lm_max_iterations in the supported range
+int check_degeneracy(const so_degeneracy* d, size_t n);     // d[0..n): thresholds in [0, 1), constrain 0 or 1
 // Serves one request: puts the scans, their times and the mode's parameters on the device, registers, reads the motion back, fills
 // results (time_total_ms included) and keeps the record of the scan left in d_scan.  The caller has checked the arguments.
 int register_scans(Ctx* c, const RegisterRequest& q);

@@ -5,6 +5,8 @@
 // so_register_keyframes), made on the caller's scratch context; the scores are new kernels: k_verify_overlap (the in-block 1-NN
 // of so_knn per query point, bounded by the inlier radius), and two counting passes of the free-space rule (so_free.cuh, k_verify_conflict)
 // -- the submap against the query's range image, the query against the submap keyframes' images.  Nothing is removed from either map.
+// so_loop_verify_degeneracy runs the same routine with so_register_keyframes_degeneracy as the alignment (DESIGN.md section 4,
+// "Loop verification"); so_loop_edge_information (so_verify_rule.h) drops the directions it held from the loop edge's information.
 #include <algorithm>
 #include <cmath>
 #include <vector>
@@ -134,10 +136,14 @@ static int verify_check(const Ctx* c, const so_loop_candidate* cands, size_t n, 
     return SO_OK;
 }
 
-static int verify_one(Ctx* c, Ctx* s, const so_loop_candidate& cd, const so_loop_verify_opts& o, so_loop_verify_result* out) {
+// One candidate.  d NULL: so_loop_verify; else so_loop_verify_degeneracy, whose alignment is the degeneracy-aware one and whose analysis
+// goes to *deg (zeroed for a skipped slot)
+static int verify_one(Ctx* c, Ctx* s, const so_loop_candidate& cd, const so_loop_verify_opts& o, const so_degeneracy* d,
+                      so_loop_verify_result* out, so_degeneracy_result* deg) {
     *out = so_loop_verify_result{};
     out->query = cd.query;
     out->id = cd.id;
+    if (d) *deg = so_degeneracy_result{};
     if (cd.id == -1) { out->skipped = 1; return SO_OK; }
     const KeyframeStore& kf = c->kf;
     const int32_t qid = cd.query, id = cd.id;
@@ -166,7 +172,12 @@ static int verify_one(Ctx* c, Ctx* s, const so_loop_candidate& cd, const so_loop
     // 2. the alignment from the candidate's prior
     double prior[7];
     loop_prior(xc, xq, cd.yaw, prior);
-    rc = so_register_keyframes(hs, hc, &qid, 1, prior, &o.icp, &out->reg);
+    if (d) {
+        rc = so_register_keyframes_degeneracy(hs, hc, &qid, 1, prior, d, &o.icp, deg);
+        out->reg = deg->icp;
+    } else {
+        rc = so_register_keyframes(hs, hc, &qid, 1, prior, &o.icp, &out->reg);
+    }
     if (rc < 0) return rc;
     rc = ensure_maps(s);
     if (rc) return rc;
@@ -250,6 +261,31 @@ static int verify_one(Ctx* c, Ctx* s, const so_loop_candidate& cd, const so_loop
     return SO_OK;
 }
 
+// so_loop_verify (d NULL) and so_loop_verify_degeneracy: the arguments checked before any device work, then one candidate at a time
+static int loop_verify(so_ctx* ctx, so_ctx* scratch, const so_loop_candidate* cands, size_t n, const so_loop_verify_opts* opts,
+                       const so_degeneracy* d, so_loop_verify_result* out, so_degeneracy_result* deg) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    Ctx* s = reinterpret_cast<Ctx*>(scratch);
+    if (!c || !s || !opts || (n && (!cands || !out))) return fail(SO_ERR_ARG, "bad args");
+    if (c == s) return fail(SO_ERR_ARG, "so_loop_verify: scratch must be another context than ctx");
+    if (c->device != s->device) return fail(SO_ERR_ARG, "so_loop_verify: the two contexts are on different devices");
+    if (!c->kf.cap_frames) return fail(SO_ERR_ARG, "so_loop_verify needs a keyframe store in ctx (so_keyframe_reserve)");
+    { int rc = verify_check(c, cands, n, *opts); if (rc) return rc; }
+    if (n == 0) return SO_OK;
+    bool any = false;
+    for (size_t i = 0; i < n; ++i) any |= cands[i].id != -1;
+    if (any) {
+        SO_CUDA_TRY(cudaSetDevice(s->device));
+        for (int k = 0; k < 2; ++k)
+            if (!s->ver.ev[k]) { int rc = s->ver.ev[k].create(); if (rc) return rc; }
+    }
+    for (size_t i = 0; i < n; ++i) {
+        int rc = verify_one(c, s, cands[i], *opts, d, out + i, d ? deg + i : nullptr);
+        if (rc) return rc;
+    }
+    return SO_OK;
+}
+
 }  // namespace so
 
 // =================================================================================================== C ABI
@@ -278,25 +314,20 @@ void so_loop_verify_opts_defaults(so_loop_verify_opts* o) {
 
 int so_loop_verify(so_ctx* ctx, so_ctx* scratch, const so_loop_candidate* cands, size_t n, const so_loop_verify_opts* opts,
                    so_loop_verify_result* out) {
-    Ctx* c = reinterpret_cast<Ctx*>(ctx);
-    Ctx* s = reinterpret_cast<Ctx*>(scratch);
-    if (!c || !s || !opts || (n && (!cands || !out))) return fail(SO_ERR_ARG, "bad args");
-    if (c == s) return fail(SO_ERR_ARG, "so_loop_verify: scratch must be another context than ctx");
-    if (c->device != s->device) return fail(SO_ERR_ARG, "so_loop_verify: the two contexts are on different devices");
-    if (!c->kf.cap_frames) return fail(SO_ERR_ARG, "so_loop_verify needs a keyframe store in ctx (so_keyframe_reserve)");
-    { int rc = verify_check(c, cands, n, *opts); if (rc) return rc; }
-    if (n == 0) return SO_OK;
-    bool any = false;
-    for (size_t i = 0; i < n; ++i) any |= cands[i].id != -1;
-    if (any) {
-        SO_CUDA_TRY(cudaSetDevice(s->device));
-        for (int k = 0; k < 2; ++k)
-            if (!s->ver.ev[k]) { int rc = s->ver.ev[k].create(); if (rc) return rc; }
-    }
-    for (size_t i = 0; i < n; ++i) {
-        int rc = verify_one(c, s, cands[i], *opts, out + i);
-        if (rc) return rc;
-    }
+    return loop_verify(ctx, scratch, cands, n, opts, nullptr, out, nullptr);
+}
+
+int so_loop_verify_degeneracy(so_ctx* ctx, so_ctx* scratch, const so_loop_candidate* cands, size_t n, const so_loop_verify_opts* opts,
+                              const so_degeneracy* d, so_loop_verify_result* out, so_degeneracy_result* deg) {
+    if (!d || (n && !deg)) return fail(SO_ERR_ARG, "bad args");
+    { int rc = check_degeneracy(d, 1); if (rc) return rc; }
+    return loop_verify(ctx, scratch, cands, n, opts, d, out, deg);
+}
+
+int so_loop_edge_information(const double reg_pose7[7], const so_degeneracy_result* deg, const double S[36], double out[36]) {
+    if (!reg_pose7 || !deg || !S || !out) return fail(SO_ERR_ARG, "bad args");
+    if (!loop_edge_information(reg_pose7, deg->flags_pos, deg->pos_axes, deg->flags_ori, deg->ori_axes, S, out))
+        return fail(SO_ERR_ARG, "so_loop_edge_information: a non-finite pose, axis or S, a zero quaternion, or flags outside 0..7");
     return SO_OK;
 }
 

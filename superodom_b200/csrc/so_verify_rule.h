@@ -1,5 +1,6 @@
 // so_verify_rule.h -- the host arithmetic of loop verification (so_loop_verify, so_verify.cu): the alignment prior of a candidate
-// (so_loop_prior), the relative pose a loop edge carries, the eligible submap ids and the accept rule.  Plain C++, so that a CPU test
+// (so_loop_prior), the relative pose a loop edge carries and its information without the unconstrained directions
+// (so_loop_edge_information), the eligible submap ids and the accept rule.  Plain C++, so that a CPU test
 // compiles it.
 #pragma once
 #include <cmath>
@@ -46,6 +47,57 @@ inline void loop_relative(const double x7[7], const double p7[7], double z7[7]) 
     for (int k = 0; k < 3; ++k) z7[k] = r[k];
     verify_qmul(xi, p7 + 3, r);
     for (int k = 0; k < 4; ++k) z7[3 + k] = r[k];
+}
+
+// The square-root information of a loop edge (id, query, Z = rel7) with the directions the alignment did not constrain left out:
+// out = S (I - P), P = blockdiag(sum a_k a_k^T, sum b_k b_k^T) over the translation eigenvectors flagged in flags_pos (a_k = R^T
+// pos_axes[k], R the rotation of reg_pose7, quaternion normalised first) and the rotation ones flagged in flags_ori (b_k = ori_axes[k]).
+// The registration adds translation in the world frame and turns on the right, and a registration step (dt, dtheta) at reg_pose7
+// moves the edge's residual [t_E; Log R_E] by t_E = R^T dt, Log R_E = dtheta: hence the R^T on the translation axes.
+// No flag set: out is S, copied.  false (out untouched) for a non-finite pose, S or axis, a zero quaternion, or flags outside 0..7.
+// out may alias S.  Products and sums in a fixed order (k, then the row, then the column), so that a CPU test restates them bit for
+// bit.
+inline bool loop_edge_information(const double pose7[7], int32_t flags_pos, const double pos_axes[9], int32_t flags_ori,
+                                  const double ori_axes[9], const double S[36], double out[36]) {
+    for (int k = 0; k < 7; ++k) if (!std::isfinite(pose7[k])) return false;
+    for (int k = 0; k < 36; ++k) if (!std::isfinite(S[k])) return false;
+    for (int k = 0; k < 9; ++k) if (!std::isfinite(pos_axes[k]) || !std::isfinite(ori_axes[k])) return false;
+    if (flags_pos < 0 || flags_pos > 7 || flags_ori < 0 || flags_ori > 7) return false;
+    const double n = std::sqrt(pose7[3] * pose7[3] + pose7[4] * pose7[4] + pose7[5] * pose7[5] + pose7[6] * pose7[6]);
+    if (!(n > 0.0)) return false;
+    if (!flags_pos && !flags_ori) {
+        for (int k = 0; k < 36; ++k) out[k] = S[k];
+        return true;
+    }
+    const double x = pose7[3] / n, y = pose7[4] / n, z = pose7[5] / n, w = pose7[6] / n;
+    const double R[9] = {1 - 2 * (y * y + z * z), 2 * (x * y - z * w),     2 * (x * z + y * w),
+                         2 * (x * y + z * w),     1 - 2 * (x * x + z * z), 2 * (y * z - x * w),
+                         2 * (x * z - y * w),     2 * (y * z + x * w),     1 - 2 * (x * x + y * y)};
+    double M[36] = {};                                                   // I - P
+    for (int i = 0; i < 6; ++i) M[7 * i] = 1.0;
+    for (int k = 0; k < 3; ++k) {
+        if (flags_pos >> k & 1) {
+            const double* u = pos_axes + 3 * k;
+            double a[3];
+            for (int i = 0; i < 3; ++i) a[i] = R[i] * u[0] + R[3 + i] * u[1] + R[6 + i] * u[2];    // R^T u
+            for (int i = 0; i < 3; ++i)
+                for (int j = 0; j < 3; ++j) M[6 * i + j] -= a[i] * a[j];
+        }
+        if (flags_ori >> k & 1) {
+            const double* b = ori_axes + 3 * k;
+            for (int i = 0; i < 3; ++i)
+                for (int j = 0; j < 3; ++j) M[6 * (3 + i) + 3 + j] -= b[i] * b[j];
+        }
+    }
+    double o[36];
+    for (int r = 0; r < 6; ++r)
+        for (int c = 0; c < 6; ++c) {
+            double v = 0.0;
+            for (int m = 0; m < 6; ++m) v += S[6 * r + m] * M[6 * m + c];
+            o[6 * r + c] = v;
+        }
+    for (int k = 0; k < 36; ++k) out[k] = o[k];
+    return true;
 }
 
 // The ids a submap of query may use: [begin, end) without the query itself; end < 0 selects [0, query - exclude_recent), the ids
