@@ -1049,8 +1049,8 @@ int so_bytes_copied(so_ctx* ctx, uint64_t* h2d, uint64_t* d2h, int reset);
  * k_lm_step (LM step), 2 k_knn (so_knn*), 3 scan ordering / map build / map insert / free-space clearing / scan preparation (pre-filter, deskew, uniform and edge extraction), 4 first evaluation of
  * a solve (k_evaluate + k_lm_step iteration zero), 5 k_fit (plane fit), 6 global localization search (map bounds, bitmap raster,
  * dilation, pyramid levels, offset table, traversal steps and dense scoring),
- * 7 k_undistort (within-scan motion compensation: per ICP iteration, and the undistorted map insert / so_undistort_points; the
- * per-iteration warp and the map insert of so_register_optimized*), 8 evaluation + trust-region step of so_register_optimized*.
+ * 7 the warp of within-scan motion compensation (k_warp_scan / k_warp_edges per ICP iteration, k_warp_cloud in the map insert
+ * and so_undistort_points; both so_register_undistort* and so_register_optimized*), 8 evaluation + trust-region step of so_register_optimized*.
  * Profiling mode serialises kernels; enable only for roofline runs. */
 /* Build-time switches of the loaded library.  Bit 0 (SO_BUILD_FUSED_MATCH, search and fit as one kernel) is reserved: this
  * library always runs them as two kernels and returns 0. */

@@ -104,6 +104,7 @@ def main():
                     t[m].append(res[0].time_total_ms)
         out[f"cfg2_batch{nb}_ms"] = {m: float(np.median(v)) for m, v in t.items()}
         if nb == 64:
+            # class 7 is the warp; its keys keep the kernel names of the first runs (k_undistort, k_motion_warp), so runs compare
             bctx.profile_enable(True)
             bctx.profile_get(7, reset=True)
             bctx.register_batch_undistort(flat, npts, priors, us, 20, 0, skip_map_checks=True)

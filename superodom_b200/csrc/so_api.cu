@@ -339,17 +339,29 @@ static bool fused_lm(const Ctx* c, uint32_t n_scans, UndistortionMode mode, bool
 // Kernels one ICP iteration of a captured schedule launches: the unrolled graph runs `iters` of them, the loop graph one per
 // iteration executed plus its k_loop_cond.  2: k_knn_scan + k_fit.
 static uint64_t iteration_launches(UndistortionMode mode, bool fused, uint32_t grid_e, int lm) {
-    if (mode == UndistortionMode::OPTIMIZED)                                                // warp, search + fit, (eval + step) x (1 + lm);
-        return 1 + 2 + 2 + 2 * uint64_t(lm) + (grid_e ? 1 + 2 + uint64_t(lm) : 0);       // edges: their warp, k_edge_fit + line rows, line rows x lm
-    const uint64_t head = mode == UndistortionMode::APPROXIMATED ? (grid_e ? 2 : 1) : 0;  // k_undistort (+ k_undistort_edges)
+    const uint64_t head = mode != UndistortionMode::NONE ? (grid_e ? 2 : 1) : 0;          // k_warp_scan (+ k_warp_edges)
     if (fused && !grid_e) return head + 2 + 1 + uint64_t(lm);
-    return head + 2 + 2 + 2 * uint64_t(lm) + (grid_e ? 1 + uint64_t(lm) : 0);
+    // (eval + step) x (1 + lm); edges: k_edge_fit, then the line rows x lm (OPTIMIZED: k_edge_fit + k_motion_eval_edge, then x lm)
+    return head + 2 + 2 + 2 * uint64_t(lm) + (grid_e ? 1 + uint64_t(lm) + (mode == UndistortionMode::OPTIMIZED ? 1 : 0) : 0);
+}
+
+// One solve phase of an ICP iteration for the chunk's scans (first: its first scan): PH_CORR opens a solve, PH_EVAL is one lm
+// evaluation.  OPTIMIZED: the two-block motion solve; otherwise the six-column one, stepped by k_lm_step_deg when dg is given.
+// me / eb: the edge map and the chunk's line buffers, read when grid_e > 0.
+static void launch_solve(const Ctx* c, UndistortionMode mode, int phase, const BatchView& bv, const CorrBuf& cb, uint32_t first, uint32_t grid_x,
+                         uint32_t n_scans, cudaStream_t st, const MapView* me, const EdgeBuf* eb, uint32_t grid_e, DegenState* dg) {
+    if (mode == UndistortionMode::OPTIMIZED) {
+        const MotionEdges med = grid_e ? MotionEdges{*me, *eb, c->d_escan, c->und.d_etime, c->mot.d_epartials, grid_e} : MotionEdges{};
+        launch_motion_solve(phase, bv, cb, c->d_scan, c->und.d_time, c->mot.d_st, first, c->mot.d_partials + size_t(first) * c->mot.stride * kMotionAcc,
+                            c->mot.stride, grid_x, n_scans, st, grid_e ? &med : nullptr);
+    } else if (phase == PH_CORR) launch_first_eval(bv, cb, grid_x, n_scans, st, me, eb, grid_e, dg);
+    else launch_evaluate(bv, cb, grid_x, n_scans, st, eb, grid_e, dg);
 }
 
 // One ICP iteration: [head, k_knn_scan, k_fit, first solve, lm solves].  Every kernel exits at once when its scan is not in the
 // matching phase, so a fixed schedule follows whatever path the device-side state machine takes.
-//   head         mode APPROXIMATED: k_undistort (the scans' pInit at the current pose) + k_undistort_edges when the chunk has an edge
-//                cloud; OPTIMIZED: k_motion_warp (u(D)) + k_motion_warp_edges likewise; NONE: none
+//   head         modes APPROXIMATED and OPTIMIZED: k_warp_scan (the scans warped by D, from the current pose or the motion block) +
+//                k_warp_edges when the chunk has an edge cloud; NONE: none
 //   first solve  k_evaluate<PH_CORR> (+ k_edge_fit) + k_lm_step; OPTIMIZED: k_motion_eval<PH_CORR> (+ k_edge_fit + k_motion_eval_edge)
 //                + k_motion_step
 //   lm solves    k_evaluate<PH_EVAL> (+ k_edge_evaluate) + k_lm_step; OPTIMIZED: k_motion_eval<PH_EVAL> (+ k_motion_eval_edge) + k_motion_step
@@ -375,22 +387,10 @@ static int run_schedule(Ctx* c, const Chunk& ch, int iters, int lm, Undistortion
     eb.nn = nullptr; eb.selmask = nullptr;
     *was_loop = false;
     const bool optimized = mode == UndistortionMode::OPTIMIZED;
-    const bool warp_edges = mode != UndistortionMode::NONE && grid_e;     // the line branch runs on the edge cloud's pInit / float(u(D))
+    const bool warp_edges = mode != UndistortionMode::NONE && grid_e;     // the line branch runs on the warped edge cloud
     if (warp_edges) eb.scan = c->und.d_ewarp;
-    double* const mot_partials = c->mot.d_partials ? c->mot.d_partials + size_t(ch.first) * c->mot.stride * kMotionAcc : nullptr;
-    const MotionEdges med{me, eb, c->d_escan, c->und.d_etime, c->mot.d_epartials, grid_e};
-    const MotionEdges* const mep = optimized && warp_edges ? &med : nullptr;
-    auto head = [&](cudaStream_t s) {
-        if (optimized) launch_motion_warp(bv, c->d_scan_sorted, c->d_scan, c->und.d_time, c->mot.d_st, ch.first, grid_x, n_scans, s, mep);
-        else launch_undistort(bv, c->d_scan_sorted, c->d_scan, c->und.d_time, c->und.d_par + ch.first, grid_x, n_scans, s);
-        if (warp_edges && !optimized)
-            launch_undistort_edges(bv, eb.offset, c->und.d_ewarp, c->d_escan, c->und.d_etime, c->und.d_par + ch.first, grid_e, n_scans, s);
-    };
-    auto solve = [&](int phase, cudaStream_t s) {
-        if (optimized) launch_motion_solve(phase, bv, cb, c->d_scan, c->und.d_time, c->mot.d_st, ch.first, mot_partials, c->mot.stride, grid_x, n_scans, s, mep);
-        else if (phase == PH_CORR) launch_first_eval(bv, cb, grid_x, n_scans, s, &me, &eb, grid_e, dg);
-        else launch_evaluate(bv, cb, grid_x, n_scans, s, &eb, grid_e, dg);
-    };
+    auto head = [&](cudaStream_t s) { launch_warp(c, mode, bv, eb.offset, ch.first, grid_x, grid_e, n_scans, s); };
+    auto solve = [&](int phase, cudaStream_t s) { launch_solve(c, mode, phase, bv, cb, ch.first, grid_x, n_scans, s, &me, &eb, grid_e, dg); };
     auto iteration = [&](cudaStream_t s) {
         if (mode != UndistortionMode::NONE) head(s);
         launch_match(mv, bv, cb, nn, grid_x, n_scans, s);
@@ -810,10 +810,12 @@ int register_scans(Ctx* c, const RegisterRequest& q) {
     }
     if (q.insertable) {
         c->reg = RegisteredScan{};
-        c->reg.n = uint32_t(total); c->reg.mode = q.mode;
+        c->reg.n = uint32_t(total); c->reg.warp.mode = q.mode;
         if (q.edge) c->reg.n_edge = uint32_t(total_e);
-        if (q.mode == UndistortionMode::APPROXIMATED) c->reg.par = q.und[0];
-        if (q.mode == UndistortionMode::OPTIMIZED) { std::memcpy(c->reg.D, q.motion[0].D, sizeof(c->reg.D)); c->reg.dt = q.motion[0].dt; }
+        if (q.mode == UndistortionMode::APPROXIMATED) c->reg.warp.par = q.und[0];
+        if (q.mode == UndistortionMode::OPTIMIZED) {
+            std::memcpy(c->reg.warp.motion.D, q.motion[0].D, sizeof(c->reg.warp.motion.D)); c->reg.warp.motion.dt = q.motion[0].dt;
+        }
     }
     return SO_OK;
 }
@@ -847,11 +849,7 @@ int put_registered_scan(Ctx* c, bool edges, float4* dst, const double pose[7]) {
     const RegisteredScan& r = c->reg;
     SO_CUDA_TRY(cudaMemcpyAsync(dst, edges ? c->d_escan : c->d_scan, size_t(edges ? r.n_edge : r.n) * sizeof(float4),
                                 cudaMemcpyDeviceToDevice, c->stream));
-    switch (r.mode) {
-        case UndistortionMode::APPROXIMATED: return edges ? undistort_edge_tail(c, dst, r, pose) : undistort_tail(c, dst, r, pose);
-        case UndistortionMode::OPTIMIZED: return edges ? motion_edge_tail(c, dst, r) : motion_tail(c, dst, r);   // u(D_opt), whatever the pose
-        default: return SO_OK;
-    }
+    return warp_cloud(c, dst, edges ? c->und.d_etime : c->und.d_time, edges ? r.n_edge : r.n, r.warp, pose);   // OPTIMIZED: u(D_opt), whatever the pose
 }
 
 // so_degeneracy values of the degeneracy-aware entry points (so_register_degeneracy*, so_loop_verify_degeneracy, so_solve)
@@ -1596,7 +1594,7 @@ int so_register_batch_undistort(so_ctx* ctx, const void* surf, const uint32_t* n
     }
     RegisterRequest q = batch_request(surf, n_points, n_scans, stride, ioff, poses_in, opts, results);
     q.toff = toff; q.und = P.data();
-    q.mode = any ? UndistortionMode::APPROXIMATED : UndistortionMode::NONE;   // mode 0 scans in an APPROXIMATED batch: k_undistort skips them
+    q.mode = any ? UndistortionMode::APPROXIMATED : UndistortionMode::NONE;   // mode 0 scans in an APPROXIMATED batch: the warp skips them
     return register_scans(c, q);
 }
 
@@ -1934,11 +1932,7 @@ static int solve_stage(Ctx* c, const so_solve_row* rows, const float* times, siz
     cb.nn = nullptr; cb.nn_d2 = nullptr;
     DegenState* const ddg = dg ? c->deg.d_st.get() : nullptr;
     const uint32_t nb = uint32_t(n_problems);
-    auto solve = [&](int phase) {                                  // run_schedule's solve(phase)
-        if (ms) launch_motion_solve(phase, bv, cb, c->d_scan, c->und.d_time, c->mot.d_st, 0, c->mot.d_partials, c->mot.stride, grid_x, nb, st, nullptr);
-        else if (phase == PH_CORR) launch_first_eval(bv, cb, grid_x, nb, st, nullptr, nullptr, 0, ddg);
-        else launch_evaluate(bv, cb, grid_x, nb, st, nullptr, 0, ddg);
-    };
+    auto solve = [&](int phase) { launch_solve(c, mode, phase, bv, cb, 0, grid_x, nb, st, nullptr, nullptr, 0, ddg); };
     timed_launch_begin(c);
     solve(PH_CORR);
     timed_launch_end(c, ms ? 8 : 4);

@@ -85,10 +85,11 @@ struct ProfileSlot { double ms = 0.0; uint64_t launches = 0; };
 constexpr int kMotionAcc = 91;                     // 78 (upper triangle of the 12x12 H) + 12 (g) + 1 (cost)
 
 // Within-scan motion compensation of a registration (the reference's UndistortionMode, LidarSlam.h:65-82): NONE, APPROXIMATED
-// (so_undistort.cu: k_undistort heads every ICP iteration), OPTIMIZED (so_motion.cu: the motion is a second parameter block).
+// (so_undistort.cu: the warp heads every ICP iteration, D from the previous and current pose), OPTIMIZED (so_motion.cu: the motion D
+// is a second parameter block; the same warp, D from that block).
 enum class UndistortionMode : int32_t { NONE = 0, APPROXIMATED = 1, OPTIMIZED = 2 };
 
-// Within-scan motion compensation of one scan (so_undistort, mode APPROXIMATED): everything k_undistort needs besides the
+// Within-scan motion compensation of one scan (so_undistort, mode APPROXIMATED): everything the warp needs besides the
 // current pose.  Kept out of IcpState so that the other kernels do not change.
 struct UndistortParams {
     double q_prev_conj[4];                         // conj(q_prev), xyzw
@@ -111,6 +112,17 @@ struct MotionState {
     int32_t pad;
 };
 
+// A motion D over dt, as a contiguous cloud is warped by it in mode OPTIMIZED
+struct MotionD { double D[7] = {0, 0, 0, 0, 0, 0, 1}, dt = 0; };
+
+// How a cloud is compensated for its motion (warp_cloud, so_undistort.cu): NONE not at all, APPROXIMATED by par at a pose given with
+// the cloud, OPTIMIZED by the motion the registration estimated, whatever the pose
+struct CloudWarp {
+    UndistortionMode mode = UndistortionMode::NONE;
+    UndistortParams par{};                         // APPROXIMATED
+    MotionD motion{};                              // OPTIMIZED
+};
+
 // The scan so_map_add_registered_scan inserts: d_scan[0..n) in upload order and, unless mode NONE, its times in und.d_time[0..n);
 // the edge cloud so_map_add_registered_edges inserts: d_escan[0..n_edge) and, unless mode NONE, its times in und.d_etime
 struct RegisteredScan {
@@ -118,9 +130,7 @@ struct RegisteredScan {
     bool edge_valid = true;                        // false: so_correspond_edge has overwritten d_escan since
     uint32_t n = 0;                                // 0: no scan registered yet, nothing to insert
     uint32_t n_edge = 0;                           // 0: the registration had no edge cloud, nothing to insert
-    UndistortionMode mode = UndistortionMode::NONE;
-    UndistortParams par{};                         // APPROXIMATED: the parameters it registered with
-    double D[7] = {0, 0, 0, 0, 0, 0, 1}, dt = 0;   // OPTIMIZED: the estimated motion D_opt and the time it spans
+    CloudWarp warp;                                // the compensation it registered with
 };
 
 // One registration call (register_scans, so_api.cu): where the scans come from, what they are, how they register, where the
@@ -475,36 +485,28 @@ int check_undistort(const so_undistort* u);                 // argument errors o
 UndistortParams make_params(const so_undistort& u);
 bool finite_pose(const double p[7]);                        // finite, with a non-zero quaternion
 int upload_times(Ctx* c, const void* src, size_t n, size_t stride, size_t toff, float* dst);   // the float at toff of every record -> dst
-// k_undistort: pInit of every active point of the chunk's scans (bv.st / bv.offset / par already offset to the chunk), from the
-// raw points in upload order (raw, times: indexed offset + original index) into the ordered copy `sorted`, w kept
-void launch_undistort(const BatchView& bv, float4* sorted, const float4* raw, const float* times, const UndistortParams* par,
-                      uint32_t grid_x, uint32_t n_scans, cudaStream_t st);
-// k_undistort_edges: pInit of every edge point of the chunk's scans (eoffset already offset to the chunk), from the raw edge cloud
-// and its times (indexed eoffset + i) into `out` at the same index, w kept
-void launch_undistort_edges(const BatchView& bv, const uint32_t* eoffset, float4* out, const float4* raw, const float* times,
-                            const UndistortParams* par, uint32_t grid_e, uint32_t n_scans, cudaStream_t st);
-// dst[0..r.n) = the registered scan r (APPROXIMATED): pInit at pose, in place
-int undistort_tail(Ctx* c, float4* dst, const RegisteredScan& r, const double pose[7]);
-// dst[0..r.n_edge) = the registered edge cloud r (APPROXIMATED): pInit at pose, in place
-int undistort_edge_tail(Ctx* c, float4* dst, const RegisteredScan& r, const double pose[7]);
+// The head of an ICP iteration of mode APPROXIMATED or OPTIMIZED (D from und.d_par or mot.d_st): every active point of the chunk's
+// scans (bv.st / bv.offset / eoffset already offset to the chunk, `first` its first scan) warped from the raw points in upload order
+// (d_scan, und.d_time: indexed offset + original index) into the ordered copy d_scan_sorted, w kept; with grid_e > 0 also every edge
+// point, from d_escan and und.d_etime into und.d_ewarp at the same index
+void launch_warp(const Ctx* c, UndistortionMode mode, const BatchView& bv, const uint32_t* eoffset, uint32_t first, uint32_t grid_x,
+                 uint32_t grid_e, uint32_t n_scans, cudaStream_t st);
+// pts[0..n) warped in place as w says, with their times[0..n) (APPROXIMATED: at pose); one launch of profile class 7 unless w.mode is
+// NONE or n is 0
+int warp_cloud(Ctx* c, float4* pts, const float* times, uint32_t n, const CloudWarp& w, const double pose[7]);
 // so_motion.cu
 int motion_reserve(Ctx* c, size_t n_points);                // Ctx::mot's blocks and partials (max_batch), Ctx::und's times (n_points)
 int check_motion(const so_motion* m, const so_icp_opts* o); // argument errors of one so_motion and the options it registers with
 MotionState make_state(const so_motion& m);
 void fill_motion(const so_icp_result& icp, const MotionState& M, so_motion_result* out);   // out = icp + motion, pose_end = T * D
-int motion_tail(Ctx* c, float4* dst, const RegisteredScan& r);   // dst[0..r.n) = the registered scan r (OPTIMIZED): u(r.D), in place
-int motion_edge_tail(Ctx* c, float4* dst, const RegisteredScan& r);   // dst[0..r.n_edge) = its edge cloud: u(r.D) with the edge times, in place
 int motion_edge_reserve(Ctx* c);                             // Ctx::mot's edge partials
-// The edge cloud of an OPTIMIZED chunk: the edge map, the line buffers (eb.scan: where the warp puts float(u(D)) of the edge points,
-// eb.offset: the chunk's edge offsets), the raw edge points and their times, the edge partials and the CTAs covering the largest cloud
+// The edge cloud of an OPTIMIZED chunk: the edge map, the line buffers (eb.scan: the warped edge points, eb.offset: the chunk's edge
+// offsets), the raw edge points and their times, the edge partials and the CTAs covering the largest cloud
 struct MotionEdges { MapView map; EdgeBuf eb; const float4* raw; const float* times; double* partials; uint32_t grid_e; };
-// One ICP iteration's kernels of mode OPTIMIZED for the chunk's scans (bv.st / bv.offset / partials already offset to the chunk, ms
-// the whole array and `first` the chunk's first scan): the warp u(D) into `sorted`, and one evaluation + trust-region step (phase
-// PH_CORR: the first of a solve)
-// me (optional): the chunk's edge clouds -- the warp also writes float(u(D)) of the edge points, the solve adds k_edge_fit (PH_CORR)
-// and the line rows (k_motion_eval_edge) to the sums k_motion_step reduces
-void launch_motion_warp(const BatchView& bv, float4* sorted, const float4* raw, const float* times, const MotionState* ms, uint32_t first,
-                        uint32_t grid_x, uint32_t n_scans, cudaStream_t st, const MotionEdges* me = nullptr);
+// One evaluation + trust-region step of mode OPTIMIZED for the chunk's scans (phase PH_CORR: the first of a solve; bv.st / bv.offset /
+// partials already offset to the chunk, ms the whole array and `first` the chunk's first scan)
+// me (optional): the chunk's edge clouds -- the solve adds k_edge_fit (PH_CORR) and the line rows (k_motion_eval_edge) to the sums
+// k_motion_step reduces
 void launch_motion_solve(int phase, const BatchView& bv, const CorrBuf& cb, const float4* raw, const float* times, MotionState* ms, uint32_t first,
                          double* partials, uint32_t stride, uint32_t grid_x, uint32_t n_scans, cudaStream_t st, const MotionEdges* me = nullptr);
 // so_covariance: cov12_warp on ms->H into st's covariance and error fields (device memory)

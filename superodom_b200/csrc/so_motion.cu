@@ -7,14 +7,13 @@
 //   u_i(D) = qrot(slerp(identity, q_D, alpha_i), p_i) + alpha_i * t_D          (und_point's formula with D from the state)
 //   r_i    = n_i . (R(q) u_i(D) + t) + d_i                                      under ScaledLoss(TukeyLoss), as so_register
 // plus six rows of SE3AbsolutatePoseFactor on D (measurement D0, multiplier sqrt(n_ok * info_k)).  Each ICP iteration rounds u(D) to
-// float and runs the unchanged search and fit at T on it (k_motion_warp -> d_scan_sorted); the solve evaluates u in double at the
-// candidate D.  Both blocks use PoseLocalParameterization; the D rotation columns are the exact derivative
+// float and runs the unchanged search and fit at T on it (so_undistort.cu's warp with D from the state -> d_scan_sorted); the solve
+// evaluates u in double at the candidate D.  Both blocks use PoseLocalParameterization; the D rotation columns are the exact derivative
 //   dr/d(dtheta_D) = alpha (p x b)^T J_r(alpha phi) J_r(phi)^-1,  b = R(q_alpha)^T R(q)^T n,  phi = Log(q_D) on the shortest path.
-//   k_motion_warp        float(u(D)) of every active point into the ordered scan (w kept), like k_undistort
 //   k_motion_eval<PH>    residual and 12-column row per correspondence, 91 per-CTA sums (78 + 12 + 1) through shared memory
 //   k_motion_step<PH>    fixed-order cross-CTA sum, then the 12-parameter trust-region step; the 12x12 covariance at the end
-//   k_motion_cloud       u(D_opt) of a contiguous cloud: the map insert after a single-scan registration
-// With an edge cloud (so_register_optimized_edges): k_motion_warp_edges writes float(u_e(D)) for k_edge_fit's search and fit at T, and
+// The map insert after a single-scan registration warps the cloud by u(D_opt) with the same warp.
+// With an edge cloud (so_register_optimized_edges): the warp writes float(u_e(D)) for k_edge_fit's search and fit at T, and
 //   k_motion_eval_edge<PH> adds the line rows' 91 per-CTA sums (three rows per line, motion_line_rows) into a partial buffer of their
 //   own, which k_motion_step adds after the planes' in the same fixed order
 #include <cmath>
@@ -24,70 +23,6 @@
 #include "so_undistort.cuh"
 
 namespace so {
-
-// sh = {q_D[4] normalised, t_D[3], theta, 1 / sin(theta)} of a motion D, rounded as und_setup rounds
-__device__ __forceinline__ void motion_setup(const double D[7], double sh[9]) {
-    const double n2 = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(D[3], D[3]), __dmul_rn(D[4], D[4])), __dmul_rn(D[5], D[5])), __dmul_rn(D[6], D[6]));
-    const double s = 1.0 / sqrt(n2);
-    for (int k = 0; k < 4; ++k) sh[k] = __dmul_rn(D[3 + k], s);
-    for (int k = 0; k < 3; ++k) sh[4 + k] = D[k];
-    und_angle(sh);
-}
-
-// ------------------------------------------------------------------------------------------------------------------ warp
-__global__ void __launch_bounds__(kThreads) k_motion_warp(BatchView bv, float4* __restrict__ sorted, const float4* __restrict__ raw,
-                                                          const float* __restrict__ times, const MotionState* __restrict__ ms) {
-    const int s = blockIdx.y;
-    const IcpState* st = bv.st + s;
-    if (st->phase != PH_CORR) return;
-    const uint32_t n = uint32_t(st->n_points);
-    if (blockIdx.x * kThreads >= n) return;
-    __shared__ double sh[9];
-    if (threadIdx.x == 0) motion_setup(ms[s].D, sh);
-    __syncthreads();
-    UndistortParams P{};
-    P.dt = ms[s].dt; P.on = 1; P.rotation = 1;
-    const uint32_t i = blockIdx.x * kThreads + threadIdx.x;
-    if (i >= n) return;
-    const size_t base = size_t(bv.offset[s]), gi = base + i;
-    const float w = sorted[gi].w;
-    const size_t src = base + __float_as_uint(w);                        // original index (scan ordering)
-    float4 o = und_point(P, sh, __ldg(&raw[src]), __ldg(&times[src]));
-    o.w = w;
-    sorted[gi] = o;
-}
-
-// The same warp for the edge cloud (so_register_optimized_edges): one thread per edge point, raw point, time and output at one index
-__global__ void __launch_bounds__(kThreads) k_motion_warp_edges(BatchView bv, const uint32_t* __restrict__ eoffset, float4* __restrict__ out,
-                                                                const float4* __restrict__ raw, const float* __restrict__ times,
-                                                                const MotionState* __restrict__ ms) {
-    const int s = blockIdx.y;
-    const IcpState* st = bv.st + s;
-    if (st->phase != PH_CORR) return;
-    const uint32_t n = uint32_t(st->n_edge);
-    if (blockIdx.x * kThreads >= n) return;
-    __shared__ double sh[9];
-    if (threadIdx.x == 0) motion_setup(ms[s].D, sh);
-    __syncthreads();
-    UndistortParams P{};
-    P.dt = ms[s].dt; P.on = 1; P.rotation = 1;
-    const uint32_t i = blockIdx.x * kThreads + threadIdx.x;
-    if (i >= n) return;
-    const size_t gi = size_t(eoffset[s]) + i;
-    out[gi] = und_point(P, sh, __ldg(&raw[gi]), __ldg(&times[gi]));
-}
-
-struct MotionD { double v[7]; };
-__global__ void __launch_bounds__(256) k_motion_cloud(float4* __restrict__ pts, const float* __restrict__ times, uint32_t n, MotionD D, double dt) {
-    __shared__ double sh[9];
-    if (threadIdx.x == 0) motion_setup(D.v, sh);
-    __syncthreads();
-    UndistortParams P{};
-    P.dt = dt; P.on = 1; P.rotation = 1;
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    pts[i] = und_point(P, sh, pts[i], times[i]);
-}
 
 // ------------------------------------------------------------------------------------------------------------------ evaluation
 __device__ __forceinline__ void cross3(const double a[3], const double b[3], double o[3]) {
@@ -552,13 +487,6 @@ __global__ void __launch_bounds__(128) k_motion_step(BatchView bv, MotionState* 
     cta_copy(ms + s, &s_m);
 }
 
-void launch_motion_warp(const BatchView& bv, float4* sorted, const float4* raw, const float* times, const MotionState* ms, uint32_t first,
-                        uint32_t grid_x, uint32_t n_scans, cudaStream_t st, const MotionEdges* me) {
-    k_motion_warp<<<dim3(grid_x, n_scans), kThreads, 0, st>>>(bv, sorted, raw, times, ms + first);
-    if (me && me->grid_e)
-        k_motion_warp_edges<<<dim3(me->grid_e, n_scans), kThreads, 0, st>>>(bv, me->eb.offset, const_cast<float4*>(me->eb.scan), me->raw, me->times, ms + first);
-}
-
 void launch_motion_solve(int phase, const BatchView& bv, const CorrBuf& cb, const float4* raw, const float* times, MotionState* ms, uint32_t first,
                          double* partials, uint32_t stride, uint32_t grid_x, uint32_t n_scans, cudaStream_t st, const MotionEdges* me) {
     ms += first;
@@ -578,28 +506,6 @@ void launch_motion_solve(int phase, const BatchView& bv, const CorrBuf& cb, cons
         if (ge) k_motion_eval_edge<PH_EVAL><<<dim3(ge, n_scans), kThreads, 0, st>>>(bv, me->eb, me->raw, me->times, ms, ep, first);
         k_motion_step<PH_EVAL><<<n_scans, 128, 0, st>>>(bv, ms, partials, stride, ep, eoff, first);
     }
-}
-
-int motion_tail(Ctx* c, float4* dst, const RegisteredScan& r) {
-    if (!r.n) return SO_OK;
-    MotionD D;
-    for (int k = 0; k < 7; ++k) D.v[k] = r.D[k];
-    timed_launch_begin(c);
-    k_motion_cloud<<<(r.n + 255) / 256, 256, 0, c->stream>>>(dst, c->und.d_time, r.n, D, r.dt);
-    timed_launch_end(c, 7);
-    SO_CUDA_TRY(cudaGetLastError());
-    return SO_OK;
-}
-
-int motion_edge_tail(Ctx* c, float4* dst, const RegisteredScan& r) {
-    if (!r.n_edge) return SO_OK;
-    MotionD D;
-    for (int k = 0; k < 7; ++k) D.v[k] = r.D[k];
-    timed_launch_begin(c);
-    k_motion_cloud<<<(r.n_edge + 255) / 256, 256, 0, c->stream>>>(dst, c->und.d_etime, r.n_edge, D, r.dt);
-    timed_launch_end(c, 7);
-    SO_CUDA_TRY(cudaGetLastError());
-    return SO_OK;
 }
 
 

@@ -1,6 +1,6 @@
-// so_undistort.cuh -- pInit of one point (so_undistort.cu, mode APPROXIMATED), shared with the per-iteration warp of mode OPTIMIZED
-// (so_motion.cu).  Every product and sum is rounded on its own (no FMA contraction), so that the numpy restatements in tests/ restate
-// the bits; only the FP64 acos / sin are the device's.
+// so_undistort.cuh -- the warp of one point by a scan's motion D over dt (so_undistort.cu): the per-scan setup of D for mode APPROXIMATED
+// (und_setup) and mode OPTIMIZED (motion_setup; so_motion.cu's solve reuses und_angle), then und_point.  Every product and sum is rounded
+// on its own (no FMA contraction), so that the numpy restatements in tests/ restate the bits; only the FP64 acos / sin are the device's.
 #pragma once
 #include "so_ctx.cuh"
 
@@ -40,6 +40,15 @@ __device__ __forceinline__ void und_setup(const UndistortParams& P, const double
     for (int k = 0; k < 4; ++k) sh[k] = __dmul_rn(q[k], s);
     const double d[3] = {__dsub_rn(x[0], P.t_prev[0]), __dsub_rn(x[1], P.t_prev[1]), __dsub_rn(x[2], P.t_prev[2])};
     qrot_rn(P.q_prev_conj, d, sh + 4);
+    und_angle(sh);
+}
+
+// sh = {q_D[4] normalised, t_D[3], theta, 1 / sin(theta)} of a motion D, rounded as und_setup rounds
+__device__ __forceinline__ void motion_setup(const double D[7], double sh[9]) {
+    const double n2 = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(D[3], D[3]), __dmul_rn(D[4], D[4])), __dmul_rn(D[5], D[5])), __dmul_rn(D[6], D[6]));
+    const double s = 1.0 / sqrt(n2);
+    for (int k = 0; k < 4; ++k) sh[k] = __dmul_rn(D[3 + k], s);
+    for (int k = 0; k < 3; ++k) sh[4 + k] = D[k];
     und_angle(sh);
 }
 
