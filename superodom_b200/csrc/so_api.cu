@@ -259,8 +259,8 @@ void count_h2d(Ctx* c, size_t b) { c->bytes_h2d += b; }
 void count_d2h(Ctx* c, size_t b) { c->bytes_d2h += b; }
 
 void timed_launch_begin(Ctx* c) { if (c->profiling) cudaEventRecord(c->evp0, c->stream); }
-void timed_launch_end(Ctx* c, int cls) {
-    c->launches++;
+void timed_launch_end(Ctx* c, int cls, uint32_t n) {
+    c->launches += n;
     if (!c->profiling) return;
     cudaEventRecord(c->evp1, c->stream);
     cudaEventSynchronize(c->evp1);
@@ -282,9 +282,36 @@ static int graph_queue_begin(Ctx* c, size_t n_scans) {
 }
 
 // A contiguous run of scans of the batch that is uploaded, ordered and registered together.
-// grid_in: CTAs covering the longest scan as uploaded (scan ordering); grid_x: CTAs covering the longest scan once it is reduced to the
-// points shouldProcessPoint keeps (the ICP kernels); small: every scan's survivors fit k_prepare_small
-struct Chunk { uint32_t first, count, pt_first, pt_count, grid_x, grid_e = 0, grid_in = 0; bool small = false; uint32_t max_kept = 0; };
+// grid_in: CTAs covering the longest scan as uploaded (scan ordering); small: every scan's survivors fit k_prepare_small.
+// grid_x, fused, coop: set by plan_chunk
+struct Chunk {
+    uint32_t first, count, pt_first, pt_count, grid_x = 0, grid_e = 0, grid_in = 0; bool small = false; uint32_t max_kept = 0;
+    bool fused = false, coop = false;
+};
+
+// The choices the ICP kernels of a chunk make, made once for the registration and the stage calls.  max_pts: the points of the
+// chunk's longest scan the ICP kernels cover; own_step: the solves keep a step kernel of their own (mode OPTIMIZED, the
+// degeneracy-aware step, the stage calls).
+//   grid_x  CTAs covering max_pts, rounded up to a bucket of 16 CTAs so that scans of slightly different sizes (live SLAM: every
+//           scan differs) share one captured graph; the kernels guard i < n_points and k_lm_step sums only the partial rows
+//           n_points implies
+//   fused   one or two scans in flight are launch-latency bound: the optimiser step is folded into the evaluation kernels
+//           (k_evaluate_lm, which launch_first_eval / launch_evaluate take when the chunk has no edge cloud)
+//   coop    the latency-bound search: a warp per query (k_knn_scan_coop)
+static void plan_chunk(const Ctx* c, Chunk& ch, uint32_t max_pts, bool own_step) {
+    const uint32_t g = (max_pts + kThreads - 1) / kThreads;
+    ch.grid_x = g ? std::min<uint32_t>(c->grid_x_cap, (g + 15u) & ~15u) : 0;
+    ch.fused = ch.count <= 2 && !c->profiling && !c->no_fused_lm && !own_step;
+    ch.coop = ch.count <= 2 && ch.grid_x <= kCoopMaxGrid && !c->no_coop_knn;
+}
+
+// The BatchView of the chunk's scans in `scan`, with the chunk's choices
+static BatchView chunk_view(const Ctx* c, const float4* scan, const Chunk& ch) {
+    BatchView bv = batch_view(c, scan, ch.first);
+    if (ch.fused) bv.counters = c->d_counters + ch.first;
+    bv.coop_knn = ch.coop;
+    return bv;
+}
 
 // Once per registration: order every scan by map cell at its prior pose (k_scan_keys -> radix sort -> k_scan_gather, or the one-CTA
 // k_prepare_small for small registrations).  compact: drop the points the decimation skips here, once, instead of in every kernel.
@@ -301,9 +328,7 @@ static int prepare_scans(Ctx* c, const float4* d_scan_in, const Chunk& ch, cudaS
     int cell_bits = 1, scan_bits = 0;
     while (cell_bits < 32 && (uint64_t(1) << cell_bits) <= n_cells) ++cell_bits;       // cells 0..n_cells-1 < mask = 2^cell_bits - 1
     if (compact && ch.small && !c->no_small_prepare) {
-        launch_prepare_small(mv, bv, c->d_scan_sorted, ch.count, cell_bits, ch.max_kept, st);
-        c->launches++;
-        timed_launch_end(c, 3);
+        timed_launch_end(c, 3, launch_prepare_small(mv, bv, c->d_scan_sorted, ch.count, cell_bits, ch.max_kept, st));
         SO_CUDA_TRY(cudaGetLastError());
         return SO_OK;
     }
@@ -316,87 +341,80 @@ static int prepare_scans(Ctx* c, const float4* d_scan_in, const Chunk& ch, cudaS
     const int extra = compact ? 1 : 0;
     const bool key32 = !c->force_key64 && cell_bits < 32 && cell_bits + extra + scan_bits <= 32;
     if (!key32) cell_bits = 32;
-    const uint32_t grid_in = ch.grid_in ? ch.grid_in : ch.grid_x;
-    launch_scan_keys(mv, bv, c->d_skeys, c->d_svals, grid_in, ch.count, cell_bits, key32, compact, st);
+    uint32_t n = launch_scan_keys(mv, bv, c->d_skeys, c->d_svals, ch.grid_in, ch.count, cell_bits, key32, compact, st);
     int rc = scan_sort(c, ch.pt_first, ch.pt_count, int(ch.count), cell_bits + extra, key32, st);
     if (rc) return rc;
-    launch_scan_gather(d_scan_in, c->d_svals_out, c->d_skeys_out, ch.pt_first, c->d_offset + ch.first, ch.pt_count,
-                       c->d_scan_sorted + ch.pt_first, cell_bits + extra, key32, st);
-    if (compact) { launch_scan_finish(bv, c->d_skeys_out, ch.pt_first, ch.pt_first, cell_bits, key32, ch.count, st); c->launches++; }
-    c->launches++;
-    timed_launch_end(c, 3);
+    n += launch_scan_gather(d_scan_in, c->d_svals_out, c->d_skeys_out, ch.pt_first, c->d_offset + ch.first, ch.pt_count,
+                            c->d_scan_sorted + ch.pt_first, cell_bits + extra, key32, st);
+    if (compact) n += launch_scan_finish(bv, c->d_skeys_out, ch.pt_first, ch.pt_first, cell_bits, key32, ch.count, st);
+    timed_launch_end(c, 3, n);
     SO_CUDA_TRY(cudaGetLastError());
     return SO_OK;
 }
 
-// One or two scans in flight are launch-latency bound: the optimiser step is folded into the evaluation kernels (k_evaluate_lm, which
-// launch_first_eval / launch_evaluate take when the chunk has no edge cloud).  Mode OPTIMIZED and the degeneracy-aware registration
-// have their own step kernels.
-static bool fused_lm(const Ctx* c, uint32_t n_scans, UndistortionMode mode, bool degen) {
-    return n_scans <= 2 && !c->profiling && !c->no_fused_lm && mode != UndistortionMode::OPTIMIZED && !degen;
-}
-
-// Kernels one ICP iteration of a captured schedule launches: the unrolled graph runs `iters` of them, the loop graph one per
-// iteration executed plus its k_loop_cond.  2: k_knn_scan + k_fit.
-static uint64_t iteration_launches(UndistortionMode mode, bool fused, uint32_t grid_e, int lm) {
-    const uint64_t head = mode != UndistortionMode::NONE ? (grid_e ? 2 : 1) : 0;          // k_warp_scan (+ k_warp_edges)
-    if (fused && !grid_e) return head + 2 + 1 + uint64_t(lm);
-    // (eval + step) x (1 + lm); edges: k_edge_fit, then the line rows x lm (OPTIMIZED: k_edge_fit + k_motion_eval_edge, then x lm)
-    return head + 2 + 2 + 2 * uint64_t(lm) + (grid_e ? 1 + uint64_t(lm) + (mode == UndistortionMode::OPTIMIZED ? 1 : 0) : 0);
-}
-
 // One solve phase of an ICP iteration for the chunk's scans (first: its first scan): PH_CORR opens a solve, PH_EVAL is one lm
 // evaluation.  OPTIMIZED: the two-block motion solve; otherwise the six-column one, stepped by k_lm_step_deg when dg is given.
-// me / eb: the edge map and the chunk's line buffers, read when grid_e > 0.
-static void launch_solve(const Ctx* c, UndistortionMode mode, int phase, const BatchView& bv, const CorrBuf& cb, uint32_t first, uint32_t grid_x,
-                         uint32_t n_scans, cudaStream_t st, const MapView* me, const EdgeBuf* eb, uint32_t grid_e, DegenState* dg) {
+// me / eb: the edge map and the chunk's line buffers, read when grid_e > 0.  Returns the kernels it enqueued.
+static uint32_t launch_solve(const Ctx* c, UndistortionMode mode, int phase, const BatchView& bv, const CorrBuf& cb, uint32_t first, uint32_t grid_x,
+                             uint32_t n_scans, cudaStream_t st, const MapView* me, const EdgeBuf* eb, uint32_t grid_e, DegenState* dg) {
     if (mode == UndistortionMode::OPTIMIZED) {
         const MotionEdges med = grid_e ? MotionEdges{*me, *eb, c->d_escan, c->und.d_etime, c->mot.d_epartials, grid_e} : MotionEdges{};
-        launch_motion_solve(phase, bv, cb, c->d_scan, c->und.d_time, c->mot.d_st, first, c->mot.d_partials + size_t(first) * c->mot.stride * kMotionAcc,
-                            c->mot.stride, grid_x, n_scans, st, grid_e ? &med : nullptr);
-    } else if (phase == PH_CORR) launch_first_eval(bv, cb, grid_x, n_scans, st, me, eb, grid_e, dg);
-    else launch_evaluate(bv, cb, grid_x, n_scans, st, eb, grid_e, dg);
+        return launch_motion_solve(phase, bv, cb, c->d_scan, c->und.d_time, c->mot.d_st, first, c->mot.d_partials + size_t(first) * c->mot.stride * kMotionAcc,
+                                   c->mot.stride, grid_x, n_scans, st, grid_e ? &med : nullptr);
+    }
+    if (phase == PH_CORR) return launch_first_eval(bv, cb, grid_x, n_scans, st, me, eb, grid_e, dg);
+    return launch_evaluate(bv, cb, grid_x, n_scans, st, eb, grid_e, dg);
 }
 
-// One ICP iteration: [head, k_knn_scan, k_fit, first solve, lm solves].  Every kernel exits at once when its scan is not in the
+// One ICP iteration: [head, search, k_fit, first solve, lm solves].  Every kernel exits at once when its scan is not in the
 // matching phase, so a fixed schedule follows whatever path the device-side state machine takes.
 //   head         modes APPROXIMATED and OPTIMIZED: k_warp_scan (the scans warped by D, from the current pose or the motion block) +
 //                k_warp_edges when the chunk has an edge cloud; NONE: none
+//   search       k_knn_scan (k_knn_scan_coop for a coop chunk; k_knn_scan<true> + k_knn_round2 with the neighbour graph), or
+//                k_knn_inject with injected neighbours
 //   first solve  k_evaluate<PH_CORR> (+ k_edge_fit) + k_lm_step; OPTIMIZED: k_motion_eval<PH_CORR> (+ k_edge_fit + k_motion_eval_edge)
 //                + k_motion_step
 //   lm solves    k_evaluate<PH_EVAL> (+ k_edge_evaluate) + k_lm_step; OPTIMIZED: k_motion_eval<PH_EVAL> (+ k_motion_eval_edge) + k_motion_step
 // Preferred form: a CUDA-graph WHILE node around ONE iteration (k_loop_cond ends the loop when every scan of the chunk is done);
-// fallback: the schedule unrolled `iters` times.  Sets *was_loop to whether the loop form ran.  Profiling or injected neighbours:
-// launched one kernel at a time instead.  dg: the chunk's DegenState array of a degeneracy-aware registration (k_lm_step_deg steps
-// its solves), else nullptr.
+// fallback: the schedule unrolled `iters` times.  Profiling or injected neighbours: launched one step at a time instead, each step
+// only when a scan of the chunk is in its phase.  dg: the chunk's DegenState array of a degeneracy-aware registration
+// (k_lm_step_deg steps its solves), else nullptr.
+// Counts the kernels it launched, except in the loop form, whose passes only the final states tell: *body_launches is then the
+// kernels one pass of the WHILE body launches, else 0.
 static int run_schedule(Ctx* c, const Chunk& ch, int iters, int lm, UndistortionMode mode, const uint32_t* d_inject, int inject_iters,
-                        cudaStream_t run_stream, bool* was_loop, DegenState* dg) {
+                        cudaStream_t run_stream, DegenState* dg, uint32_t* body_launches) {
     const MapView mv = search_view(c);
     NnBuf nn = c->nn;                                     // queue lengths: indexed by the scan's position inside the chunk
     if (nn.qcount) nn.qcount += size_t(ch.first) * SO_MAX_ICP_ITERS;
-    BatchView bv = batch_view(c, c->d_scan_sorted, ch.first);
+    const BatchView bv = chunk_view(c, c->d_scan_sorted, ch);
     CorrBuf cb = c->corr;
     cb.nn = nullptr; cb.nn_d2 = nullptr;
     const uint32_t grid_x = ch.grid_x, n_scans = ch.count, grid_e = ch.grid_e;
-    const bool fused = fused_lm(c, n_scans, mode, dg != nullptr);
-    if (fused) bv.counters = c->d_counters + ch.first;
-    bv.coop_knn = n_scans <= 2 && grid_x <= kCoopMaxGrid && !c->no_coop_knn;      // latency-bound search: a warp per query
     const MapView me = map_view(c, c->edge);
     EdgeBuf eb = c->ebuf;
     eb.offset = c->d_eoffset + ch.first;                  // like bv.offset: indexed by the scan's position inside the chunk
     eb.nn = nullptr; eb.selmask = nullptr;
-    *was_loop = false;
+    *body_launches = 0;
     const bool optimized = mode == UndistortionMode::OPTIMIZED;
     const bool warp_edges = mode != UndistortionMode::NONE && grid_e;     // the line branch runs on the warped edge cloud
     if (warp_edges) eb.scan = c->und.d_ewarp;
-    auto head = [&](cudaStream_t s) { launch_warp(c, mode, bv, eb.offset, ch.first, grid_x, grid_e, n_scans, s); };
-    auto solve = [&](int phase, cudaStream_t s) { launch_solve(c, mode, phase, bv, cb, ch.first, grid_x, n_scans, s, &me, &eb, grid_e, dg); };
-    auto iteration = [&](cudaStream_t s) {
-        if (mode != UndistortionMode::NONE) head(s);
-        launch_match(mv, bv, cb, nn, grid_x, n_scans, s);
-        solve(PH_CORR, s);
-        for (int k = 0; k < lm; ++k) solve(PH_EVAL, s);
+    // The iteration's steps in order, on c->stream: step(cls, phase, launch) with the step's profile class, the phase of the scans
+    // it serves, and launch() enqueueing it and returning its kernels.  Returns the sum of what step returned.
+    auto iteration = [&](auto&& step) -> uint32_t {
+        cudaStream_t s = c->stream;
+        uint32_t n = 0;
+        if (mode != UndistortionMode::NONE) n += step(7, PH_CORR, [&] { return launch_warp(c, mode, bv, eb.offset, ch.first, grid_x, grid_e, n_scans, s); });
+        n += step(0, PH_CORR, [&] {
+            return d_inject ? launch_inject(mv, c->surf.d_xyzi, c->surf.n, bv, c->nn, d_inject, inject_iters, grid_x, n_scans, s)
+                            : launch_match(mv, bv, cb, nn, grid_x, n_scans, s, 1);
+        });
+        n += step(5, PH_CORR, [&] { return launch_match(mv, bv, cb, nn, grid_x, n_scans, s, 2); });
+        n += step(optimized ? 8 : 4, PH_CORR, [&] { return launch_solve(c, mode, PH_CORR, bv, cb, ch.first, grid_x, n_scans, s, &me, &eb, grid_e, dg); });
+        for (int k = 0; k < lm; ++k)
+            n += step(optimized ? 8 : 1, PH_EVAL, [&] { return launch_solve(c, mode, PH_EVAL, bv, cb, ch.first, grid_x, n_scans, s, &me, &eb, grid_e, dg); });
+        return n;
     };
+    auto enqueue = [](int, int, auto&& launch) { return launch(); };
     if (c->profiling || d_inject) {
         // profiling mode: one launch at a time, timed with events, and only launches that have work (the host peeks
         // at the phases) so that the per-class average is the duration of a kernel that actually ran
@@ -407,21 +425,14 @@ static int run_schedule(Ctx* c, const Chunk& ch, int iters, int lm, Undistortion
             for (uint32_t s = 0; s < n_scans; ++s) if (peek[s].phase == ph) return true;
             return false;
         };
-        const uint64_t solve_extra = 1 + (grid_e ? 1 : 0);          // launches of a solve besides the one timed_launch_end counts
-        const uint64_t corr_extra = solve_extra + (optimized && grid_e ? 1 : 0);   // OPTIMIZED: k_edge_fit + k_motion_eval_edge
-        for (int it = 0; it < iters; ++it) {
-            if (any_in(PH_CORR)) {
-                if (mode != UndistortionMode::NONE) { timed_launch_begin(c); head(c->stream); c->launches += warp_edges ? 1 : 0; timed_launch_end(c, 7); }
-                timed_launch_begin(c);
-                if (d_inject) launch_inject(mv, c->surf.d_xyzi, c->surf.n, bv, c->nn, d_inject, inject_iters, grid_x, n_scans, c->stream);
-                else launch_match(mv, bv, cb, nn, grid_x, n_scans, c->stream, 1);                                               // k_knn_scan
-                timed_launch_end(c, 0);
-                timed_launch_begin(c); launch_match(mv, bv, cb, nn, grid_x, n_scans, c->stream, 2); timed_launch_end(c, 5);      // k_fit
-                timed_launch_begin(c); solve(PH_CORR, c->stream); c->launches += corr_extra; timed_launch_end(c, optimized ? 8 : 4);
-            }
-            for (int k = 0; k < lm; ++k)
-                if (any_in(PH_EVAL)) { timed_launch_begin(c); solve(PH_EVAL, c->stream); c->launches += solve_extra; timed_launch_end(c, optimized ? 8 : 1); }
-        }
+        auto timed = [&](int cls, int ph, auto&& launch) -> uint32_t {
+            if (!any_in(ph)) return 0;
+            timed_launch_begin(c);
+            const uint32_t n = launch();
+            timed_launch_end(c, cls, n);
+            return n;
+        };
+        for (int it = 0; it < iters; ++it) iteration(timed);
         SO_CUDA_TRY(cudaGetLastError());
         return SO_OK;
     }
@@ -459,8 +470,8 @@ static int run_schedule(Ctx* c, const Chunk& ch, int iters, int lm, Undistortion
                 cudaGraph_t body = p.conditional.phGraph_out[0];
                 ok = cudaStreamBeginCaptureToGraph(c->stream, body, nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal) == cudaSuccess;
                 if (ok) {
-                    iteration(c->stream);
-                    launch_loop_cond(bv, n_scans, handle, c->stream);
+                    slot->launches = iteration(enqueue);
+                    slot->launches += launch_loop_cond(bv, n_scans, handle, c->stream);
                     cudaGraph_t dummy = nullptr;
                     ok = cudaStreamEndCapture(c->stream, &dummy) == cudaSuccess;
                 }
@@ -473,7 +484,8 @@ static int run_schedule(Ctx* c, const Chunk& ch, int iters, int lm, Undistortion
         if (!slot->exec) {
             cudaGraph_t g = nullptr;
             SO_CUDA_TRY(cudaStreamBeginCapture(c->stream, cudaStreamCaptureModeThreadLocal));
-            for (int it = 0; it < iters; ++it) iteration(c->stream);
+            slot->launches = 0;
+            for (int it = 0; it < iters; ++it) slot->launches += iteration(enqueue);
             SO_CUDA_TRY(cudaStreamEndCapture(c->stream, &g));
             cudaError_t e = cudaGraphInstantiate(&slot->exec, g, 0);
             cudaGraphDestroy(g);
@@ -483,8 +495,8 @@ static int run_schedule(Ctx* c, const Chunk& ch, int iters, int lm, Undistortion
     }
     slot->used = ++c->graph_clock;
     SO_CUDA_TRY(cudaGraphLaunch(slot->exec, run_stream));
-    *was_loop = slot->is_loop;
-    if (!slot->is_loop) c->launches += uint64_t(iters) * iteration_launches(mode, fused, grid_e, lm);   // loop form: counted by register_core
+    if (slot->is_loop) *body_launches = slot->launches;
+    else c->launches += slot->launches;
     return SO_OK;
 }
 
@@ -587,7 +599,7 @@ static int register_core(Ctx* c, const RegisterRequest& q) {
     if (sink && c->sink_cursor + n_scans > c->sink_cap) return fail(SO_ERR_CAPACITY, "pose sink full (so_set_pose_sink)");
     if (!any && sink) {                                         // nothing to register: the rows are the priors
         SO_CUDA_TRY(cudaMemcpyAsync(c->d_state, c->h_state, n_scans * sizeof(IcpState), cudaMemcpyHostToDevice, c->stream));
-        launch_pack_poses(c->d_state, uint32_t(n_scans), sink + c->sink_cursor * 8, c->stream);
+        c->launches += launch_pack_poses(c->d_state, uint32_t(n_scans), sink + c->sink_cursor * 8, c->stream);
         SO_CUDA_TRY(cudaStreamSynchronize(c->stream));
     }
     if (any) {
@@ -618,7 +630,7 @@ static int register_core(Ctx* c, const RegisterRequest& q) {
         for (size_t k = 0; k < n_chunks; ++k) {
             const uint32_t f = bounds[k], e = bounds[k + 1];
             if (e == f) continue;
-            Chunk ch{f, e - f, c->h_offset[f], (e < n_scans ? c->h_offset[e] : off) - c->h_offset[f], 0};
+            Chunk ch{f, e - f, c->h_offset[f], (e < n_scans ? c->h_offset[e] : off) - c->h_offset[f]};
             uint32_t mx = 0, mx_in = 0;
             for (uint32_t s = f; s < e; ++s) if (c->h_state[s].phase == PH_CORR) {
                 mx_in = std::max(mx_in, n_points[s]);
@@ -629,10 +641,7 @@ static int register_core(Ctx* c, const RegisterRequest& q) {
             ch.grid_in = (mx_in + kThreads - 1) / kThreads;
             ch.small = mx <= kPrepareSmallCap && mx_in > 0;
             ch.max_kept = mx;
-            ch.grid_x = (mx + kThreads - 1) / kThreads;
-            // rounded up to a bucket of 16 CTAs so that scans of slightly different sizes (live SLAM: every scan differs) share one
-            // captured graph; the kernels guard i < n_points and k_lm_step sums only the partial rows n_points implies
-            if (ch.grid_x) ch.grid_x = std::min<uint32_t>(c->grid_x_cap, (ch.grid_x + 15u) & ~15u);
+            plan_chunk(c, ch, mx, q.mode == UndistortionMode::OPTIMIZED || q.degen);
             if (n_edge) for (uint32_t s = f; s < e; ++s) if (c->h_state[s].phase == PH_CORR) ch.grid_e = std::max(ch.grid_e, (n_edge[s] + kThreads - 1) / kThreads);
             chunks.push_back(ch);
         }
@@ -654,22 +663,20 @@ static int register_core(Ctx* c, const RegisterRequest& q) {
                 SO_CUDA_TRY(cudaEventRecord(c->ev_copy[k], c->copy_stream));
             }
         }
-        std::vector<char> loop_flags(chunks.size(), 0);
+        std::vector<uint32_t> body_launches(chunks.size(), 0);       // a later chunk's capture may evict this chunk's graph
         for (size_t k = 0; k < chunks.size(); ++k) {
             const Chunk& ch = chunks[k];
             cudaStream_t st = (two_streams && (k & 1)) ? c->aux_stream : c->stream;
             if (host_src) SO_CUDA_TRY(cudaStreamWaitEvent(st, c->ev_copy[k], 0));
             if (ch.grid_x == 0) continue;
             int rc = prepare_scans(c, d_scan, ch, st, true);
-            bool was_loop = false;
-            if (!rc) rc = run_schedule(c, ch, o.max_icp_iters, o.lm_max_iterations, q.mode, q.inject ? c->d_inject.get() : nullptr, q.inject_iters, st, &was_loop,
-                                       q.degen ? c->deg.d_st + ch.first : nullptr);
+            if (!rc) rc = run_schedule(c, ch, o.max_icp_iters, o.lm_max_iterations, q.mode, q.inject ? c->d_inject.get() : nullptr, q.inject_iters, st,
+                                       q.degen ? c->deg.d_st + ch.first : nullptr, &body_launches[k]);
             if (rc) {                                       // leave no work behind on the side streams before reporting the error
                 cudaStreamSynchronize(c->aux_stream);
                 cudaStreamSynchronize(c->copy_stream);
                 return rc;
             }
-            loop_flags[k] = was_loop;
         }
         if (two_streams) {
             SO_CUDA_TRY(cudaEventRecord(c->ev_join, c->aux_stream));
@@ -677,20 +684,16 @@ static int register_core(Ctx* c, const RegisterRequest& q) {
         }
         SO_CUDA_TRY(cudaEventRecord(c->ev1, c->stream));
         { int rc = run_deferred_upload(c); if (rc) return rc; }      // host-side staging of the whole cloud while the registration runs
-        if (sink) { launch_pack_poses(c->d_state, uint32_t(n_scans), sink + c->sink_cursor * 8, c->stream); c->launches++; }
+        if (sink) c->launches += launch_pack_poses(c->d_state, uint32_t(n_scans), sink + c->sink_cursor * 8, c->stream);
         SO_CUDA_TRY(cudaMemcpyAsync(c->h_state, c->d_state, n_scans * sizeof(IcpState), cudaMemcpyDeviceToHost, c->stream));
         count_d2h(c, n_scans * sizeof(IcpState));
         SO_CUDA_TRY(cudaStreamSynchronize(c->stream));
         float ms = 0.f;
         cudaEventElapsedTime(&ms, c->ev0, c->ev1);
-        for (size_t k = 0; k < chunks.size(); ++k) {
-            if (!loop_flags[k]) continue;
+        for (size_t k = 0; k < chunks.size(); ++k) {                // the loop form: the WHILE body ran once per iteration of the longest registration
             int max_it = 0;
             for (uint32_t s = chunks[k].first; s < chunks[k].first + chunks[k].count; ++s) max_it = std::max(max_it, int(c->h_state[s].n_iterations));
-            const bool fused = fused_lm(c, chunks[k].count, q.mode, q.degen != nullptr);
-            const bool coop = chunks[k].count <= 2 && chunks[k].grid_x <= kCoopMaxGrid && !c->no_coop_knn;
-            const uint64_t round2 = knn_graph_valid(c) && !coop ? 1 : 0;     // k_knn_round2
-            c->launches += uint64_t(max_it) * (iteration_launches(q.mode, fused, chunks[k].grid_e, o.lm_max_iterations) + 1 + round2);   // + k_loop_cond
+            c->launches += uint64_t(max_it) * body_launches[k];
         }
         for (size_t s = 0; s < n_scans; ++s) {
             if (results[s].status == SO_STATUS_NOT_ENOUGH_FEATURES || n_points[s] == 0) continue;
@@ -1007,7 +1010,7 @@ static int store_add(Ctx* c, MapStore& ms, const void* xyzi, size_t n, size_t st
     if (pose) { rc = map_transform_tail(c, ms, uint32_t(n), pose); if (rc) return rc; }
     timed_launch_begin(c);
     rc = map_add_points(c, ms, uint32_t(n));
-    timed_launch_end(c, 3);
+    timed_launch_end(c, 3, 1);
     return rc;
 }
 
@@ -1199,7 +1202,7 @@ int so_scan_prefilter(so_ctx* ctx, const void* xyzi, size_t n, size_t stride, si
     uint32_t m = 0;
     timed_launch_begin(c);
     rc = scan_voxel_filter(c, uint32_t(n), *plane_res, &m);
-    timed_launch_end(c, 3);
+    timed_launch_end(c, 3, 1);
     if (rc) return rc;
     *n_out = m;
     c->prefiltered_n = m;                                          // so_register_prefiltered: the filtered cloud stays in d_scan_sorted
@@ -1320,7 +1323,7 @@ int so_scan_deskew(so_ctx* ctx, void* points, size_t n, size_t stride, size_t ti
     timed_launch_begin(c);
     launch_deskew(c->d_scan, uint32_t(n), P, c->stream);
     c->launches++;
-    timed_launch_end(c, 3);
+    timed_launch_end(c, 3, 1);
     rc = ensure_stage(c, n);
     if (rc) return rc;
     uint32_t past = 0;
@@ -1349,7 +1352,7 @@ int so_scan_extract_uniform(so_ctx* ctx, const void* points, size_t n, size_t st
     uint32_t m = 0;
     timed_launch_begin(c);
     rc = scan_extract_uniform(c, uint32_t(n), uint32_t(skip_num), block_range, int_abs, &m);
-    timed_launch_end(c, 3);
+    timed_launch_end(c, 3, 1);
     if (rc) return rc;
     *n_out = m;
     const size_t ncopy = std::min<size_t>(m, cap);
@@ -1682,24 +1685,29 @@ static int correspond_stage(Ctx* c, const void* surf, size_t n, size_t stride, s
     c->h_offset[0] = 0;
     SO_CUDA_TRY(cudaMemcpyAsync(c->d_state, c->h_state, sizeof(IcpState), cudaMemcpyHostToDevice, c->stream));
     SO_CUDA_TRY(cudaMemcpyAsync(c->d_offset, c->h_offset, sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
-    const uint32_t grid_x = (uint32_t(n) + kThreads - 1) / kThreads;
-    const Chunk ch{0, 1, 0, uint32_t(n), grid_x};
+    Chunk ch{0, 1, 0, uint32_t(n)};
+    ch.grid_in = (uint32_t(n) + kThreads - 1) / kThreads;
+    plan_chunk(c, ch, uint32_t(n), true);                               // as a single small registration would search
     rc = prepare_scans(c, c->d_scan, ch, c->stream, false);              // stage API reports every point: decimation stays inside the kernels
     if (rc) return rc;
     rc = knn_graph_prepare(c, 0);                                       // a stage call builds the neighbour graph only when it is forced on
     if (!rc) rc = graph_queue_begin(c, 1);
     if (rc) return rc;
     const MapView mv = search_view(c);
-    BatchView bv = batch_view(c, c->d_scan_sorted);
-    bv.coop_knn = grid_x <= kCoopMaxGrid && !c->no_coop_knn;            // as a single small registration would search
-    timed_launch_begin(c); launch_correspond(mv, bv, c->corr, c->nn, grid_x, 1, c->stream); c->launches += 2 + 2; timed_launch_end(c, 0);
+    const BatchView bv = chunk_view(c, c->d_scan_sorted, ch);
+    auto correspond = [&] {
+        timed_launch_begin(c);
+        const uint32_t k = launch_match(mv, bv, c->corr, c->nn, ch.grid_x, 1, c->stream);
+        timed_launch_end(c, 0, k + launch_first_eval(bv, c->corr, ch.grid_x, 1, c->stream));
+    };
+    correspond();
     SO_CUDA_TRY(cudaGetLastError());
     if (pose_prev) {
         // iteration 1 at `pose`: same scan order, the neighbour records (pre, d5, pos) of iteration 0 are what seed_bound reads
         init_state(c->h_state[0], pose, uint32_t(n), o);
         c->h_state[0].icp_iter = 1;
         SO_CUDA_TRY(cudaMemcpyAsync(c->d_state, c->h_state, sizeof(IcpState), cudaMemcpyHostToDevice, c->stream));
-        timed_launch_begin(c); launch_correspond(mv, bv, c->corr, c->nn, grid_x, 1, c->stream); c->launches += 2 + 2; timed_launch_end(c, 0);
+        correspond();
         SO_CUDA_TRY(cudaGetLastError());
     }
     std::vector<double4> nd(n); std::vector<double> w(n); std::vector<uchar4> fl(n); std::vector<uint32_t> nn(n * 5); std::vector<float> d2(n * 5);
@@ -1770,9 +1778,8 @@ int so_correspond_edge(so_ctx* ctx, const void* edge, size_t n, size_t stride, s
     const MapView me = map_view(c, c->edge);
     const BatchView bv = batch_view(c, c->d_scan_sorted);
     timed_launch_begin(c);
-    launch_first_eval(bv, c->corr, 0, 1, c->stream, &me, &c->ebuf, grid_e);     // 0 plane CTAs: only the edge kernel + k_lm_step have work
-    c->launches += 2;
-    timed_launch_end(c, 4);
+    const uint32_t k = launch_first_eval(bv, c->corr, 0, 1, c->stream, &me, &c->ebuf, grid_e);     // 0 plane CTAs: only the edge kernel + k_lm_step have work
+    timed_launch_end(c, 4, k);
     SO_CUDA_TRY(cudaGetLastError());
     std::vector<double4> a(n), b(n); std::vector<uchar4> fl(n); std::vector<uint32_t> nn(n * 10), sel(n);
     SO_CUDA_TRY(cudaMemcpyAsync(a.data(), c->ebuf.a, n * sizeof(double4), cudaMemcpyDeviceToHost, c->stream));
@@ -1806,7 +1813,8 @@ int so_evaluate(so_ctx* ctx, const double pose[7], double H[36], double g[6], do
     SO_CUDA_TRY(cudaMemcpyAsync(c->d_state, c->h_state, sizeof(IcpState), cudaMemcpyHostToDevice, c->stream));
     const uint32_t grid_x = (n + kThreads - 1) / kThreads;
     const BatchView bv = batch_view(c, c->d_scan_sorted);
-    timed_launch_begin(c); launch_evaluate(bv, c->corr, grid_x, 1, c->stream, &c->ebuf, grid_e); c->launches++; timed_launch_end(c, 1);
+    timed_launch_begin(c);
+    timed_launch_end(c, 1, launch_evaluate(bv, c->corr, grid_x, 1, c->stream, &c->ebuf, grid_e));
     SO_CUDA_TRY(cudaGetLastError());
     SO_CUDA_TRY(cudaMemcpyAsync(c->h_state, c->d_state, sizeof(IcpState), cudaMemcpyDeviceToHost, c->stream));
     SO_CUDA_TRY(cudaStreamSynchronize(c->stream));
@@ -1823,20 +1831,20 @@ int so_covariance(so_ctx* ctx, const double* H, int32_t n, so_icp_result* out) {
     IcpState& s = c->h_state[0];                              // the state of a preceding so_correspond* is replaced
     std::memset(&s, 0, sizeof(s));
     timed_launch_begin(c);
+    uint32_t k = 0;
     if (n == 6) {
         for (int i = 0; i < 6; ++i) for (int j = i; j < 6; ++j) s.H[tri(i, j)] = H[i * 6 + j];
         SO_CUDA_TRY(cudaMemcpyAsync(c->d_state, c->h_state, sizeof(IcpState), cudaMemcpyHostToDevice, c->stream));
-        launch_covariance(c->d_state, c->stream);
+        k = launch_covariance(c->d_state, c->stream);
     } else {
         { int rc = c->mot.d_st.reserve(std::max<size_t>(c->max_batch, 1)); if (rc) return rc; }
         MotionState M{};
         for (int i = 0; i < 12; ++i) for (int j = i; j < 12; ++j) M.H[i * 12 - (i * (i - 1)) / 2 + (j - i)] = H[i * 12 + j];
         SO_CUDA_TRY(cudaMemcpyAsync(c->d_state, c->h_state, sizeof(IcpState), cudaMemcpyHostToDevice, c->stream));
         SO_CUDA_TRY(cudaMemcpyAsync(c->mot.d_st, &M, sizeof(MotionState), cudaMemcpyHostToDevice, c->stream));
-        launch_covariance12(c->d_state, c->mot.d_st, c->stream);
+        k = launch_covariance12(c->d_state, c->mot.d_st, c->stream);
     }
-    c->launches++;
-    timed_launch_end(c, 1);
+    timed_launch_end(c, 1, k);
     SO_CUDA_TRY(cudaGetLastError());
     SO_CUDA_TRY(cudaMemcpyAsync(c->h_state, c->d_state, sizeof(IcpState), cudaMemcpyDeviceToHost, c->stream));
     SO_CUDA_TRY(cudaStreamSynchronize(c->stream));
@@ -1860,9 +1868,7 @@ int so_degeneracy_analysis(so_ctx* ctx, const double* H, const so_degeneracy* d,
     timed_launch_begin(c);
     SO_CUDA_TRY(cudaMemcpyAsync(c->d_state, c->h_state, sizeof(IcpState), cudaMemcpyHostToDevice, c->stream));
     SO_CUDA_TRY(cudaMemcpyAsync(c->deg.d_st, &S, sizeof(DegenState), cudaMemcpyHostToDevice, c->stream));
-    launch_degeneracy_analysis(c->d_state, c->deg.d_st, c->stream);
-    c->launches++;
-    timed_launch_end(c, 1);
+    timed_launch_end(c, 1, launch_degeneracy_analysis(c->d_state, c->deg.d_st, c->stream));
     SO_CUDA_TRY(cudaGetLastError());
     SO_CUDA_TRY(cudaMemcpyAsync(&S, c->deg.d_st, sizeof(DegenState), cudaMemcpyDeviceToHost, c->stream));
     SO_CUDA_TRY(cudaStreamSynchronize(c->stream));
@@ -1922,27 +1928,23 @@ static int solve_stage(Ctx* c, const so_solve_row* rows, const float* times, siz
     }
     if (dg) SO_CUDA_TRY(cudaMemcpyAsync(c->deg.d_st, dg, n_problems * sizeof(DegenState), cudaMemcpyHostToDevice, st));
     if (ms) SO_CUDA_TRY(cudaMemcpyAsync(c->mot.d_st, ms, n_problems * sizeof(MotionState), cudaMemcpyHostToDevice, st));
-    // the chunk's CTA count as register_core rounds it
-    uint32_t grid_x = (max_n + kThreads - 1) / kThreads;
-    if (grid_x) grid_x = std::min<uint32_t>(c->grid_x_cap, (grid_x + 15u) & ~15u);
-    BatchView bv = batch_view(c, c->d_scan_sorted);
+    Chunk ch{0, uint32_t(n_problems), 0, uint32_t(total)};
+    plan_chunk(c, ch, max_n, ms || dg);
+    const BatchView bv = chunk_view(c, c->d_scan_sorted, ch);
     const UndistortionMode mode = ms ? UndistortionMode::OPTIMIZED : UndistortionMode::NONE;
-    if (fused_lm(c, uint32_t(n_problems), mode, dg != nullptr)) bv.counters = c->d_counters;
     CorrBuf cb = c->corr;
     cb.nn = nullptr; cb.nn_d2 = nullptr;
     DegenState* const ddg = dg ? c->deg.d_st.get() : nullptr;
-    const uint32_t nb = uint32_t(n_problems);
-    auto solve = [&](int phase) { launch_solve(c, mode, phase, bv, cb, 0, grid_x, nb, st, nullptr, nullptr, 0, ddg); };
+    auto solve = [&](int phase) { return launch_solve(c, mode, phase, bv, cb, 0, ch.grid_x, ch.count, st, nullptr, nullptr, 0, ddg); };
     timed_launch_begin(c);
-    solve(PH_CORR);
-    timed_launch_end(c, ms ? 8 : 4);
+    timed_launch_end(c, ms ? 8 : 4, solve(PH_CORR));
     SO_CUDA_TRY(cudaGetLastError());
     std::vector<double> cost0(n_problems);                        // the cost IterationZero evaluated (the state's cost moves with the steps)
     SO_CUDA_TRY(cudaMemcpyAsync(c->h_state, c->d_state, n_problems * sizeof(IcpState), cudaMemcpyDeviceToHost, st));
     SO_CUDA_TRY(cudaStreamSynchronize(st));
     for (size_t b = 0; b < n_problems; ++b) cost0[b] = c->h_state[b].cost;
     for (int k = 0; k < lm; ++k) {
-        timed_launch_begin(c); solve(PH_EVAL); timed_launch_end(c, ms ? 8 : 1);
+        timed_launch_begin(c); timed_launch_end(c, ms ? 8 : 1, solve(PH_EVAL));
     }
     SO_CUDA_TRY(cudaGetLastError());
     SO_CUDA_TRY(cudaMemcpyAsync(c->h_state, c->d_state, n_problems * sizeof(IcpState), cudaMemcpyDeviceToHost, st));
@@ -2049,7 +2051,7 @@ int so_knn_device(so_ctx* ctx, const void* d_q, size_t nq, int k, float max_d2, 
         c->launches++;
     }
     if (launch_knn(mv, static_cast<const float4*>(d_q), order, nq, k, max_d2, d_idx, d_d2, c->stream)) return fail(SO_ERR_ARG, "bad k");
-    timed_launch_end(c, 2);
+    timed_launch_end(c, 2, 1);
     SO_CUDA_TRY(cudaGetLastError());
     return SO_OK;
 }

@@ -330,6 +330,7 @@ struct Ctx {
     struct GraphSlot {
         cudaGraphExec_t exec = nullptr;
         GraphKey key{}; bool is_loop = false; uint64_t used = 0;
+        uint32_t launches = 0;                     // kernels one launch of the graph runs (loop form: one pass of the WHILE body), as captured
     };
     GraphSlot graphs[20];
     uint64_t graph_clock = 0;
@@ -466,7 +467,7 @@ int upload_cloud(Ctx* c, const void* src, size_t n, size_t stride, size_t ioff, 
 void count_h2d(Ctx* c, size_t b);
 void count_d2h(Ctx* c, size_t b);
 void timed_launch_begin(Ctx* c);
-void timed_launch_end(Ctx* c, int cls);                     // counts one launch; profile class cls when profiling
+void timed_launch_end(Ctx* c, int cls, uint32_t n);         // counts the group's n kernels; one timed launch of profile class cls when profiling
 int icp_opts_check(const so_icp_opts& o);                   // max_icp_iters and lm_max_iterations in the supported range
 int check_degeneracy(const so_degeneracy* d, size_t n);     // d[0..n): thresholds in [0, 1), constrain 0 or 1
 // Serves one request: puts the scans, their times and the mode's parameters on the device, registers, reads the motion back, fills
@@ -489,8 +490,8 @@ int upload_times(Ctx* c, const void* src, size_t n, size_t stride, size_t toff, 
 // scans (bv.st / bv.offset / eoffset already offset to the chunk, `first` its first scan) warped from the raw points in upload order
 // (d_scan, und.d_time: indexed offset + original index) into the ordered copy d_scan_sorted, w kept; with grid_e > 0 also every edge
 // point, from d_escan and und.d_etime into und.d_ewarp at the same index
-void launch_warp(const Ctx* c, UndistortionMode mode, const BatchView& bv, const uint32_t* eoffset, uint32_t first, uint32_t grid_x,
-                 uint32_t grid_e, uint32_t n_scans, cudaStream_t st);
+uint32_t launch_warp(const Ctx* c, UndistortionMode mode, const BatchView& bv, const uint32_t* eoffset, uint32_t first, uint32_t grid_x,
+                     uint32_t grid_e, uint32_t n_scans, cudaStream_t st);
 // pts[0..n) warped in place as w says, with their times[0..n) (APPROXIMATED: at pose); one launch of profile class 7 unless w.mode is
 // NONE or n is 0
 int warp_cloud(Ctx* c, float4* pts, const float* times, uint32_t n, const CloudWarp& w, const double pose[7]);
@@ -507,10 +508,10 @@ struct MotionEdges { MapView map; EdgeBuf eb; const float4* raw; const float* ti
 // partials already offset to the chunk, ms the whole array and `first` the chunk's first scan)
 // me (optional): the chunk's edge clouds -- the solve adds k_edge_fit (PH_CORR) and the line rows (k_motion_eval_edge) to the sums
 // k_motion_step reduces
-void launch_motion_solve(int phase, const BatchView& bv, const CorrBuf& cb, const float4* raw, const float* times, MotionState* ms, uint32_t first,
-                         double* partials, uint32_t stride, uint32_t grid_x, uint32_t n_scans, cudaStream_t st, const MotionEdges* me = nullptr);
+uint32_t launch_motion_solve(int phase, const BatchView& bv, const CorrBuf& cb, const float4* raw, const float* times, MotionState* ms, uint32_t first,
+                             double* partials, uint32_t stride, uint32_t grid_x, uint32_t n_scans, cudaStream_t st, const MotionEdges* me = nullptr);
 // so_covariance: cov12_warp on ms->H into st's covariance and error fields (device memory)
-void launch_covariance12(IcpState* st, const MotionState* ms, cudaStream_t stream);
+uint32_t launch_covariance12(IcpState* st, const MotionState* ms, cudaStream_t stream);
 // so_map.cu
 int map_alloc(Ctx* c);
 int map_add_points(Ctx* c, MapStore& ms, uint32_t n_new);   // ms.d_xyzi[n .. n+n_new) holds the new points: voxel-filter touched blocks, index

@@ -301,7 +301,7 @@ int so_scan_extract_edges(so_ctx* ctx, const void* points, size_t n, size_t stri
     uint32_t m = 0;
     timed_launch_begin(c);
     rc = extract_edges(c, uint32_t(n), uint32_t(stride), uint32_t(toff), uint32_t(roff), aligned, o, &out_dev, &m);
-    timed_launch_end(c, 3);
+    timed_launch_end(c, 3, 1);
     if (rc) return rc;
     *n_out = m;
     const size_t ncopy = std::min<size_t>(m, cap);

@@ -237,7 +237,7 @@ int free_space_clear(Ctx* c, int stores, const float4* d_pts, uint32_t n_pts, co
     }
     SO_CUDA_TRY(cudaMemcpyAsync(c->fs.h_cnt, c->fs.d_cnt, sizeof(FreeCounters), cudaMemcpyDeviceToHost, st));
     c->launches += 1;                                                   // the two memsets
-    timed_launch_end(c, 3);
+    timed_launch_end(c, 3, 1);
     SO_CUDA_TRY(cudaGetLastError());
     SO_CUDA_TRY(cudaStreamSynchronize(st));
     const FreeCounters h = *c->fs.h_cnt;
@@ -245,7 +245,7 @@ int free_space_clear(Ctx* c, int stores, const float4* d_pts, uint32_t n_pts, co
         if (!(stores & (1 << k)) || h.removed[k] == 0) continue;       // nothing removed: the store is not touched
         timed_launch_begin(c);
         rc = map_compact(c, *ms[k], c->fs.d_keep + k * M, ms[k]->n - h.removed[k], &c->fs.d_cnt->selected);
-        timed_launch_end(c, 3);
+        timed_launch_end(c, 3, 1);
         if (rc) return rc;
     }
     if (out) {

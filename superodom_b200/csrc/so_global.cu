@@ -380,7 +380,7 @@ static int map_bounds(Ctx* c, float lo[3], float hi[3], size_t* n, bool whole = 
         launch_seg_bounds(c->surf.arc.d_pool, c->surf.arc.d_segs, n_segs, max_n, c->bnb.d_bounds, st);
         c->launches += c->surf.n ? 1 : 0;                               // one launch is counted by timed_launch_end
     }
-    timed_launch_end(c, 6);
+    timed_launch_end(c, 6, 1);
     uint32_t h[6];
     SO_CUDA_TRY(cudaMemcpyAsync(h, c->bnb.d_bounds, sizeof(h), cudaMemcpyDeviceToHost, st));
     count_d2h(c, sizeof(h));
@@ -444,21 +444,21 @@ static int bnb_build(Ctx* c, const GlobalPlan& P, const GlobalScan& S, RelocGrid
     SO_CUDA_TRY(cudaMemsetAsync(B.d_scratch, 0, w0 * sizeof(uint32_t), st));
     launch_bnb_raster(c->surf.d_xyzi, c->surf.n, g, p, B.d_scratch, st);
     if (P.whole) { int rc = archive_raster(c, g, p, B.d_scratch); if (rc) return rc; }
-    timed_launch_end(c, 6);
+    timed_launch_end(c, 6, 1);
     SO_CUDA_TRY(cudaEventRecord(B.ev[1], st));
     RelocGrid gw{};                                                 // level 0 as k_reloc_dilate sees it: the window, same dilation
     gw.bx = p.wx; gw.by = p.wy; gw.bz = p.wz; gw.wpr = p.wpr[0];
     timed_launch_begin(c);
     launch_reloc_dilate(gw, P.o.dilate, B.d_scratch, B.d_pyr, st);  // ends in its second buffer: level 0
     c->launches += 2;
-    timed_launch_end(c, 6);
+    timed_launch_end(c, 6, 1);
     timed_launch_begin(c);
     launch_bnb_levels(p, B.d_pyr, st);
     c->launches += p.lmax > 0 ? p.lmax - 1 : 0;
-    timed_launch_end(c, 6);
+    timed_launch_end(c, 6, 1);
     timed_launch_begin(c);
     launch_bnb_offsets(B.d_pts, int(S.pts.size()), B.d_q, g, p, B.d_off, st);
-    timed_launch_end(c, 6);
+    timed_launch_end(c, 6, 1);
     SO_CUDA_TRY(cudaEventRecord(B.ev[2], st));
     SO_CUDA_TRY(cudaGetLastError());
     *g_out = g; *p_out = p; *pyr_words = words;
@@ -516,7 +516,7 @@ static int bnb_search(Ctx* c, const RelocGrid& g, const BnbPyramid& p, int n_pts
         }
         launch_bnb_trim(t, B.d_nodes, B.d_ctl, st);
         c->launches += 2;
-        timed_launch_end(c, 6);
+        timed_launch_end(c, 6, 1);
         SO_CUDA_TRY(cudaMemcpyAsync(B.h_ctl, B.d_ctl, sizeof(BnbCtl), cudaMemcpyDeviceToHost, st));
         count_d2h(c, sizeof(BnbCtl));
         SO_CUDA_TRY(cudaStreamSynchronize(st));
@@ -614,7 +614,7 @@ static int bnb_dense(Ctx* c, const GlobalPlan& P, const GlobalScan& S, int level
         const uint32_t nr = uint32_t(std::min<uint64_t>(kBnbRoot, total - r0));
         timed_launch_begin(c);
         launch_bnb_score(g, p, c->bnb.d_pyr, c->bnb.d_off, int(S.pts.size()), level, nullptr, r0, nr, c->bnb.d_ctl, c->bnb.d_unsorted, c->stream);
-        timed_launch_end(c, 6);
+        timed_launch_end(c, 6, 1);
         SO_CUDA_TRY(cudaMemcpyAsync(buf.data(), c->bnb.d_unsorted, nr * sizeof(uint64_t), cudaMemcpyDeviceToHost, c->stream));
         count_d2h(c, nr * sizeof(uint64_t));
         SO_CUDA_TRY(cudaStreamSynchronize(c->stream));

@@ -1581,7 +1581,7 @@ __global__ void __launch_bounds__(128) k_lm_step_deg(BatchView bv, uint32_t n_pa
 
 // so_degeneracy_analysis: degeneracy_analysis on st->H, one thread
 __global__ void k_degeneracy_analysis(const IcpState* __restrict__ st, DegenState* __restrict__ dg) { degeneracy_analysis(st->H, *dg); }
-void launch_degeneracy_analysis(const IcpState* st, DegenState* dg, cudaStream_t stream) { k_degeneracy_analysis<<<1, 1, 0, stream>>>(st, dg); }
+uint32_t launch_degeneracy_analysis(const IcpState* st, DegenState* dg, cudaStream_t stream) { k_degeneracy_analysis<<<1, 1, 0, stream>>>(st, dg); return 1; }
 
 // so_covariance (6 columns): the covariance step that ends a registration, on st->H, in one 32-thread CTA and a shared copy of the
 // state as lm_step_body runs it
@@ -1595,7 +1595,7 @@ __global__ void __launch_bounds__(32) k_covariance(IcpState* st) {
     cta_copy(st, &s_st);
 }
 
-void launch_covariance(IcpState* st, cudaStream_t stream) { k_covariance<<<1, 32, 0, stream>>>(st); }
+uint32_t launch_covariance(IcpState* st, cudaStream_t stream) { k_covariance<<<1, 32, 0, stream>>>(st); return 1; }
 
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -1686,77 +1686,87 @@ __global__ void k_pack_poses(const IcpState* __restrict__ st, uint32_t n_scans, 
 // host-side launchers
 // ------------------------------------------------------------------------------------------------------------------
 // keys: the 64-bit key buffer; with key32 it is used as an array of uint32_t (same point indexing)
-void launch_scan_keys(const MapView& m, const BatchView& bv, uint64_t* keys, uint32_t* vals, uint32_t grid_x, uint32_t n_scans, int cell_bits, bool key32,
-                      bool compact, cudaStream_t st) {
+uint32_t launch_scan_keys(const MapView& m, const BatchView& bv, uint64_t* keys, uint32_t* vals, uint32_t grid_x, uint32_t n_scans, int cell_bits, bool key32,
+                          bool compact, cudaStream_t st) {
     const dim3 g(grid_x, n_scans);
     uint32_t* k32 = reinterpret_cast<uint32_t*>(keys);
     if (key32) { if (compact) k_scan_keys<uint32_t, true><<<g, kThreads, 0, st>>>(m, bv, k32, vals, cell_bits); else k_scan_keys<uint32_t, false><<<g, kThreads, 0, st>>>(m, bv, k32, vals, cell_bits); }
     else { if (compact) k_scan_keys<uint64_t, true><<<g, kThreads, 0, st>>>(m, bv, keys, vals, cell_bits); else k_scan_keys<uint64_t, false><<<g, kThreads, 0, st>>>(m, bv, keys, vals, cell_bits); }
+    return 1;
 }
-void launch_scan_finish(const BatchView& bv, const uint64_t* sorted_keys, size_t first, uint32_t pt_first, int cell_bits, bool key32, uint32_t n_scans, cudaStream_t st) {
+uint32_t launch_scan_finish(const BatchView& bv, const uint64_t* sorted_keys, size_t first, uint32_t pt_first, int cell_bits, bool key32, uint32_t n_scans, cudaStream_t st) {
     if (key32) k_scan_finish<uint32_t><<<(n_scans + 63) / 64, 64, 0, st>>>(bv, reinterpret_cast<const uint32_t*>(sorted_keys) + first, pt_first, cell_bits, n_scans);
     else k_scan_finish<uint64_t><<<(n_scans + 63) / 64, 64, 0, st>>>(bv, sorted_keys + first, pt_first, cell_bits, n_scans);
+    return 1;
 }
-void launch_prepare_small(const MapView& m, const BatchView& bv, float4* out, uint32_t n_scans, int key_bits, uint32_t max_kept, cudaStream_t st) {
+uint32_t launch_prepare_small(const MapView& m, const BatchView& bv, float4* out, uint32_t n_scans, int key_bits, uint32_t max_kept, cudaStream_t st) {
     if (max_kept <= 2u * kSmallThreads) k_prepare_small<2><<<n_scans, kSmallThreads, 0, st>>>(m, bv, out, key_bits);
     else k_prepare_small<4><<<n_scans, kSmallThreads, 0, st>>>(m, bv, out, key_bits);
+    return 1;
 }
-void launch_scan_gather(const float4* in, const uint32_t* vals, const uint64_t* keys, size_t first, const uint32_t* offset, size_t total, float4* out,
-                        int cell_bits, bool key32, cudaStream_t st) {
+uint32_t launch_scan_gather(const float4* in, const uint32_t* vals, const uint64_t* keys, size_t first, const uint32_t* offset, size_t total, float4* out,
+                            int cell_bits, bool key32, cudaStream_t st) {
     const uint32_t grid = uint32_t((total + kThreads - 1) / kThreads);
     if (key32) k_scan_gather<uint32_t><<<grid, kThreads, 0, st>>>(in, vals + first, reinterpret_cast<const uint32_t*>(keys) + first, offset, total, out, cell_bits);
     else k_scan_gather<uint64_t><<<grid, kThreads, 0, st>>>(in, vals + first, keys + first, offset, total, out, cell_bits);
+    return 1;
 }
-// Correspondence stage of one ICP iteration = launch_match (search + fit of every scan point) + launch_first_eval (first
+// The correspondence stage of one ICP iteration is launch_match (search + fit of every scan point), then launch_first_eval (first
 // evaluation of the new solve, the edge kernel when an edge cloud is present, and the optimiser's iteration zero).
 // medge / eb / grid_e: edge branch (grid_e == 0: idle); k_lm_step sums the partials of both branches.
-void launch_match(const MapView& m, const BatchView& bv, const CorrBuf& cb, const NnBuf& nb, uint32_t grid_x, uint32_t n_scans, cudaStream_t st, int part) {
-    if (!grid_x) return;
+uint32_t launch_match(const MapView& m, const BatchView& bv, const CorrBuf& cb, const NnBuf& nb, uint32_t grid_x, uint32_t n_scans, cudaStream_t st, int part) {
+    if (!grid_x) return 0;
+    uint32_t n = 0;
     if (part != 2) {
-        if (bv.coop_knn) k_knn_scan_coop<<<dim3(grid_x * (kThreads / kCoopWarps), n_scans), kThreads, 0, st>>>(m, bv, nb);
+        if (bv.coop_knn) { k_knn_scan_coop<<<dim3(grid_x * (kThreads / kCoopWarps), n_scans), kThreads, 0, st>>>(m, bv, nb); n = 1; }
         else if (m.graph && nb.queue) {
             k_knn_scan<true><<<dim3(grid_x * (kThreads / kKnnThreads), n_scans), kKnnThreads, 0, st>>>(m, bv, nb);
             k_knn_round2<<<dim3(grid_x * (kThreads / kKnnThreads), n_scans), kKnnThreads, 0, st>>>(m, bv, nb);
-        } else k_knn_scan<false><<<dim3(grid_x * (kThreads / kKnnThreads), n_scans), kKnnThreads, 0, st>>>(m, bv, nb);
+            n = 2;
+        } else { k_knn_scan<false><<<dim3(grid_x * (kThreads / kKnnThreads), n_scans), kKnnThreads, 0, st>>>(m, bv, nb); n = 1; }
     }
     const uint32_t gf = (grid_x * kThreads + kFitPts * kFitThreads - 1) / (kFitPts * kFitThreads);
-    if (part != 1) k_fit<<<dim3(gf, n_scans), kFitThreads, 0, st>>>(m, bv, cb, nb);
+    if (part != 1) { k_fit<<<dim3(gf, n_scans), kFitThreads, 0, st>>>(m, bv, cb, nb); n++; }
+    return n;
 }
-void launch_inject(const MapView& m, const float4* by_id, uint32_t n_map, const BatchView& bv, const NnBuf& nb, const uint32_t* ids, int n_trace_iters,
-                   uint32_t grid_x, uint32_t n_scans, cudaStream_t st) {
-    if (grid_x) k_knn_inject<<<dim3(grid_x, n_scans), kThreads, 0, st>>>(m, by_id, n_map, bv, nb, ids, n_trace_iters);
+uint32_t launch_inject(const MapView& m, const float4* by_id, uint32_t n_map, const BatchView& bv, const NnBuf& nb, const uint32_t* ids, int n_trace_iters,
+                       uint32_t grid_x, uint32_t n_scans, cudaStream_t st) {
+    if (!grid_x) return 0;
+    k_knn_inject<<<dim3(grid_x, n_scans), kThreads, 0, st>>>(m, by_id, n_map, bv, nb, ids, n_trace_iters);
+    return 1;
 }
-void launch_first_eval(const BatchView& bv, const CorrBuf& cb, uint32_t grid_x, uint32_t n_scans, cudaStream_t st, const MapView* medge, const EdgeBuf* eb,
-                       uint32_t grid_e, DegenState* dg) {
+uint32_t launch_first_eval(const BatchView& bv, const CorrBuf& cb, uint32_t grid_x, uint32_t n_scans, cudaStream_t st, const MapView* medge, const EdgeBuf* eb,
+                           uint32_t grid_e, DegenState* dg) {
     const uint32_t gp = grid_x ? eval_grid(grid_x * kThreads) : 0;
-    if (bv.counters && gp && !grid_e && !dg) { k_evaluate_lm<PH_CORR><<<dim3(gp, n_scans), kThreads, 0, st>>>(bv, cb, bv.counters); return; }
+    if (bv.counters && gp && !grid_e && !dg) { k_evaluate_lm<PH_CORR><<<dim3(gp, n_scans), kThreads, 0, st>>>(bv, cb, bv.counters); return 1; }
     if (gp) k_evaluate<PH_CORR><<<dim3(gp, n_scans), kThreads, 0, st>>>(bv, cb);
     if (grid_e) k_edge_fit<<<dim3(grid_e, n_scans), kThreads, 0, st>>>(*medge, bv, *eb, bv.edge_partial_offset);
     if (dg) k_lm_step_deg<PH_CORR><<<n_scans, 128, 0, st>>>(bv, gp, bv.edge_partial_offset, dg);
     else k_lm_step<PH_CORR><<<n_scans, 128, 0, st>>>(bv, gp, bv.edge_partial_offset);
+    return (gp ? 1 : 0) + (grid_e ? 1 : 0) + 1;
 }
-void launch_edge_fit(const MapView& medge, const BatchView& bv, const EdgeBuf& eb, uint32_t grid_e, uint32_t n_scans, cudaStream_t st) {
-    if (grid_e) k_edge_fit<<<dim3(grid_e, n_scans), kThreads, 0, st>>>(medge, bv, eb, bv.edge_partial_offset);
+uint32_t launch_edge_fit(const MapView& medge, const BatchView& bv, const EdgeBuf& eb, uint32_t grid_e, uint32_t n_scans, cudaStream_t st) {
+    if (!grid_e) return 0;
+    k_edge_fit<<<dim3(grid_e, n_scans), kThreads, 0, st>>>(medge, bv, eb, bv.edge_partial_offset);
+    return 1;
 }
-void launch_correspond(const MapView& m, const BatchView& bv, const CorrBuf& cb, const NnBuf& nb, uint32_t grid_x, uint32_t n_scans, cudaStream_t st,
-                       const MapView* medge, const EdgeBuf* eb, uint32_t grid_e) {
-    launch_match(m, bv, cb, nb, grid_x, n_scans, st);
-    launch_first_eval(bv, cb, grid_x, n_scans, st, medge, eb, grid_e);
-}
-void launch_evaluate(const BatchView& bv, const CorrBuf& cb, uint32_t grid_x, uint32_t n_scans, cudaStream_t st, const EdgeBuf* eb, uint32_t grid_e,
-                     DegenState* dg) {
+uint32_t launch_evaluate(const BatchView& bv, const CorrBuf& cb, uint32_t grid_x, uint32_t n_scans, cudaStream_t st, const EdgeBuf* eb, uint32_t grid_e,
+                         DegenState* dg) {
     const uint32_t gx = grid_x ? eval_grid(grid_x * kThreads) : 0;
-    if (bv.counters && gx && !grid_e && !dg) { k_evaluate_lm<PH_EVAL><<<dim3(gx, n_scans), kThreads, 0, st>>>(bv, cb, bv.counters); return; }
+    if (bv.counters && gx && !grid_e && !dg) { k_evaluate_lm<PH_EVAL><<<dim3(gx, n_scans), kThreads, 0, st>>>(bv, cb, bv.counters); return 1; }
     if (gx) k_evaluate<PH_EVAL><<<dim3(gx, n_scans), kThreads, 0, st>>>(bv, cb);
     if (grid_e) k_edge_evaluate<<<dim3(grid_e, n_scans), kThreads, 0, st>>>(bv, *eb, bv.edge_partial_offset);
     if (dg) k_lm_step_deg<PH_EVAL><<<n_scans, 128, 0, st>>>(bv, gx, bv.edge_partial_offset, dg);
     else k_lm_step<PH_EVAL><<<n_scans, 128, 0, st>>>(bv, gx, bv.edge_partial_offset);
+    return (gx ? 1 : 0) + (grid_e ? 1 : 0) + 1;
 }
-void launch_loop_cond(const BatchView& bv, uint32_t n_scans, cudaGraphConditionalHandle handle, cudaStream_t st) {
+uint32_t launch_loop_cond(const BatchView& bv, uint32_t n_scans, cudaGraphConditionalHandle handle, cudaStream_t st) {
     k_loop_cond<<<1, 32, 0, st>>>(bv.st, n_scans, handle);
+    return 1;
 }
-void launch_pack_poses(const IcpState* st, uint32_t n_scans, double* rows, cudaStream_t stream) {
+uint32_t launch_pack_poses(const IcpState* st, uint32_t n_scans, double* rows, cudaStream_t stream) {
     k_pack_poses<<<(n_scans + 63) / 64, 64, 0, stream>>>(st, n_scans, rows);
+    return 1;
 }
 void launch_query_keys(const MapView& m, const float4* q, size_t nq, uint32_t* keys, uint32_t* vals, cudaStream_t st) {
     k_query_keys<<<uint32_t((nq + kThreads - 1) / kThreads), kThreads, 0, st>>>(m, q, nq, keys, vals);

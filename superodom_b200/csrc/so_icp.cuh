@@ -76,32 +76,31 @@ constexpr int kFitPts = 2;               // points per thread in k_fit
 constexpr int kFitThreads = 256;
 constexpr int kFitMinBlocks = 4;
 
-void launch_scan_keys(const MapView& m, const BatchView& bv, uint64_t* keys, uint32_t* vals, uint32_t grid_x, uint32_t n_scans, int cell_bits, bool key32,
-                      bool compact, cudaStream_t st);
-void launch_scan_finish(const BatchView& bv, const uint64_t* sorted_keys, size_t first, uint32_t pt_first, int cell_bits, bool key32, uint32_t n_scans, cudaStream_t st);
+// The launchers of the registration's kernels return the number of kernels they enqueued (Ctx::launches counts from that).
+uint32_t launch_scan_keys(const MapView& m, const BatchView& bv, uint64_t* keys, uint32_t* vals, uint32_t grid_x, uint32_t n_scans, int cell_bits, bool key32,
+                          bool compact, cudaStream_t st);
+uint32_t launch_scan_finish(const BatchView& bv, const uint64_t* sorted_keys, size_t first, uint32_t pt_first, int cell_bits, bool key32, uint32_t n_scans, cudaStream_t st);
 constexpr uint32_t kPrepareSmallCap = 4096;    // survivors k_prepare_small can order (one CTA per scan)
-void launch_prepare_small(const MapView& m, const BatchView& bv, float4* out, uint32_t n_scans, int key_bits, uint32_t max_kept, cudaStream_t st);
-void launch_scan_gather(const float4* in, const uint32_t* vals, const uint64_t* keys, size_t first, const uint32_t* offset, size_t total, float4* out,
-                        int cell_bits, bool key32, cudaStream_t st);
-// part: 0 = the whole stage; 1 = k_knn_scan alone, 2 = k_fit alone (profiling)
-void launch_match(const MapView& m, const BatchView& bv, const CorrBuf& cb, const NnBuf& nb, uint32_t grid_x, uint32_t n_scans, cudaStream_t st, int part = 0);
-void launch_inject(const MapView& m, const float4* by_id, uint32_t n_map, const BatchView& bv, const NnBuf& nb, const uint32_t* ids, int n_trace_iters,
-                   uint32_t grid_x, uint32_t n_scans, cudaStream_t st);
+uint32_t launch_prepare_small(const MapView& m, const BatchView& bv, float4* out, uint32_t n_scans, int key_bits, uint32_t max_kept, cudaStream_t st);
+uint32_t launch_scan_gather(const float4* in, const uint32_t* vals, const uint64_t* keys, size_t first, const uint32_t* offset, size_t total, float4* out,
+                            int cell_bits, bool key32, cudaStream_t st);
+// part: 0 = the whole stage; 1 = the search alone, 2 = k_fit alone
+uint32_t launch_match(const MapView& m, const BatchView& bv, const CorrBuf& cb, const NnBuf& nb, uint32_t grid_x, uint32_t n_scans, cudaStream_t st, int part = 0);
+uint32_t launch_inject(const MapView& m, const float4* by_id, uint32_t n_map, const BatchView& bv, const NnBuf& nb, const uint32_t* ids, int n_trace_iters,
+                       uint32_t grid_x, uint32_t n_scans, cudaStream_t st);
 // dg: the chunk's DegenState array of a degeneracy-aware registration (k_lm_step_deg in place of k_lm_step, no fused form)
-void launch_first_eval(const BatchView& bv, const CorrBuf& cb, uint32_t grid_x, uint32_t n_scans, cudaStream_t st, const MapView* medge = nullptr,
-                       const EdgeBuf* eb = nullptr, uint32_t grid_e = 0, DegenState* dg = nullptr);
+uint32_t launch_first_eval(const BatchView& bv, const CorrBuf& cb, uint32_t grid_x, uint32_t n_scans, cudaStream_t st, const MapView* medge = nullptr,
+                           const EdgeBuf* eb = nullptr, uint32_t grid_e = 0, DegenState* dg = nullptr);
 // k_edge_fit alone (mode OPTIMIZED: the line correspondences and histogram; its 6-column sums are not read there)
-void launch_edge_fit(const MapView& medge, const BatchView& bv, const EdgeBuf& eb, uint32_t grid_e, uint32_t n_scans, cudaStream_t st);
-void launch_correspond(const MapView& m, const BatchView& bv, const CorrBuf& cb, const NnBuf& nb, uint32_t grid_x, uint32_t n_scans, cudaStream_t st,
-                       const MapView* medge = nullptr, const EdgeBuf* eb = nullptr, uint32_t grid_e = 0);
-void launch_evaluate(const BatchView& bv, const CorrBuf& cb, uint32_t grid_x, uint32_t n_scans, cudaStream_t st, const EdgeBuf* eb = nullptr, uint32_t grid_e = 0,
-                     DegenState* dg = nullptr);
-void launch_loop_cond(const BatchView& bv, uint32_t n_scans, cudaGraphConditionalHandle handle, cudaStream_t st);
-void launch_pack_poses(const IcpState* st, uint32_t n_scans, double* rows, cudaStream_t stream);
+uint32_t launch_edge_fit(const MapView& medge, const BatchView& bv, const EdgeBuf& eb, uint32_t grid_e, uint32_t n_scans, cudaStream_t st);
+uint32_t launch_evaluate(const BatchView& bv, const CorrBuf& cb, uint32_t grid_x, uint32_t n_scans, cudaStream_t st, const EdgeBuf* eb = nullptr,
+                         uint32_t grid_e = 0, DegenState* dg = nullptr);
+uint32_t launch_loop_cond(const BatchView& bv, uint32_t n_scans, cudaGraphConditionalHandle handle, cudaStream_t st);
+uint32_t launch_pack_poses(const IcpState* st, uint32_t n_scans, double* rows, cudaStream_t stream);
 // so_covariance: covariance_and_errors_warp on st->H (one scan's state, device memory)
-void launch_covariance(IcpState* st, cudaStream_t stream);
+uint32_t launch_covariance(IcpState* st, cudaStream_t stream);
 // so_degeneracy_analysis: the analysis a degeneracy-aware solve begins with, on st->H, into *dg (device memory, thresholds set)
-void launch_degeneracy_analysis(const IcpState* st, DegenState* dg, cudaStream_t stream);
+uint32_t launch_degeneracy_analysis(const IcpState* st, DegenState* dg, cudaStream_t stream);
 void launch_query_keys(const MapView& m, const float4* q, size_t nq, uint32_t* keys, uint32_t* vals, cudaStream_t st);
 int launch_knn(const MapView& m, const float4* q, const uint32_t* order, size_t nq, int k, float max_d2, uint32_t* idx, float* d2, cudaStream_t st);
 

@@ -434,7 +434,7 @@ __global__ void __launch_bounds__(32) k_covariance12(IcpState* st, const MotionS
     cta_copy(st, &s_st);
 }
 
-void launch_covariance12(IcpState* st, const MotionState* ms, cudaStream_t stream) { k_covariance12<<<1, 32, 0, stream>>>(st, ms); }
+uint32_t launch_covariance12(IcpState* st, const MotionState* ms, cudaStream_t stream) { k_covariance12<<<1, 32, 0, stream>>>(st, ms); return 1; }
 
 template <int AFTER>
 __global__ void __launch_bounds__(128) k_motion_step(BatchView bv, MotionState* __restrict__ ms, const double* __restrict__ partials, uint32_t stride,
@@ -487,17 +487,18 @@ __global__ void __launch_bounds__(128) k_motion_step(BatchView bv, MotionState* 
     cta_copy(ms + s, &s_m);
 }
 
-void launch_motion_solve(int phase, const BatchView& bv, const CorrBuf& cb, const float4* raw, const float* times, MotionState* ms, uint32_t first,
-                         double* partials, uint32_t stride, uint32_t grid_x, uint32_t n_scans, cudaStream_t st, const MotionEdges* me) {
+uint32_t launch_motion_solve(int phase, const BatchView& bv, const CorrBuf& cb, const float4* raw, const float* times, MotionState* ms, uint32_t first,
+                             double* partials, uint32_t stride, uint32_t grid_x, uint32_t n_scans, cudaStream_t st, const MotionEdges* me) {
     ms += first;
     const uint32_t gx = grid_x ? eval_grid(grid_x * kThreads) : 0;       // 0: every scan is empty; k_motion_step still ends their solves
     const uint32_t ge = me ? me->grid_e : 0;
     const uint32_t* eoff = me ? me->eb.offset : nullptr;
     double* ep = me ? me->partials : nullptr;
+    uint32_t n = 1 + (gx ? 1 : 0) + (ge ? 1 : 0);                         // k_motion_step, k_motion_eval, k_motion_eval_edge
     if (phase == PH_CORR) {
         if (gx) k_motion_eval<PH_CORR><<<dim3(gx, n_scans), kThreads, 0, st>>>(bv, cb, raw, times, ms, partials, stride);
         if (ge) {
-            launch_edge_fit(me->map, bv, me->eb, ge, n_scans, st);
+            n += launch_edge_fit(me->map, bv, me->eb, ge, n_scans, st);
             k_motion_eval_edge<PH_CORR><<<dim3(ge, n_scans), kThreads, 0, st>>>(bv, me->eb, me->raw, me->times, ms, ep, first);
         }
         k_motion_step<PH_CORR><<<n_scans, 128, 0, st>>>(bv, ms, partials, stride, ep, eoff, first);
@@ -506,6 +507,7 @@ void launch_motion_solve(int phase, const BatchView& bv, const CorrBuf& cb, cons
         if (ge) k_motion_eval_edge<PH_EVAL><<<dim3(ge, n_scans), kThreads, 0, st>>>(bv, me->eb, me->raw, me->times, ms, ep, first);
         k_motion_step<PH_EVAL><<<n_scans, 128, 0, st>>>(bv, ms, partials, stride, ep, eoff, first);
     }
+    return n;
 }
 
 

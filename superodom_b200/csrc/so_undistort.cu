@@ -111,16 +111,18 @@ __global__ void __launch_bounds__(256) k_warp_cloud(float4* __restrict__ pts, co
 }
 
 template <class Src, class Rec>
-static void launch_warp_from(const Ctx* c, const BatchView& bv, const uint32_t* eoffset, const Rec* rec, uint32_t grid_x, uint32_t grid_e,
-                             uint32_t n_scans, cudaStream_t st) {
+static uint32_t launch_warp_from(const Ctx* c, const BatchView& bv, const uint32_t* eoffset, const Rec* rec, uint32_t grid_x, uint32_t grid_e,
+                                 uint32_t n_scans, cudaStream_t st) {
     k_warp_scan<Src><<<dim3(grid_x, n_scans), kThreads, 0, st>>>(bv, c->d_scan_sorted, c->d_scan, c->und.d_time, rec);
-    if (grid_e) k_warp_edges<Src><<<dim3(grid_e, n_scans), kThreads, 0, st>>>(bv, eoffset, c->und.d_ewarp, c->d_escan, c->und.d_etime, rec);
+    if (!grid_e) return 1;
+    k_warp_edges<Src><<<dim3(grid_e, n_scans), kThreads, 0, st>>>(bv, eoffset, c->und.d_ewarp, c->d_escan, c->und.d_etime, rec);
+    return 2;
 }
 
-void launch_warp(const Ctx* c, UndistortionMode mode, const BatchView& bv, const uint32_t* eoffset, uint32_t first, uint32_t grid_x,
-                 uint32_t grid_e, uint32_t n_scans, cudaStream_t st) {
-    if (mode == UndistortionMode::OPTIMIZED) launch_warp_from<FromMotion>(c, bv, eoffset, c->mot.d_st + first, grid_x, grid_e, n_scans, st);
-    else launch_warp_from<FromPose>(c, bv, eoffset, c->und.d_par + first, grid_x, grid_e, n_scans, st);
+uint32_t launch_warp(const Ctx* c, UndistortionMode mode, const BatchView& bv, const uint32_t* eoffset, uint32_t first, uint32_t grid_x,
+                     uint32_t grid_e, uint32_t n_scans, cudaStream_t st) {
+    if (mode == UndistortionMode::OPTIMIZED) return launch_warp_from<FromMotion>(c, bv, eoffset, c->mot.d_st + first, grid_x, grid_e, n_scans, st);
+    return launch_warp_from<FromPose>(c, bv, eoffset, c->und.d_par + first, grid_x, grid_e, n_scans, st);
 }
 
 int warp_cloud(Ctx* c, float4* pts, const float* times, uint32_t n, const CloudWarp& w, const double pose[7]) {
@@ -131,7 +133,7 @@ int warp_cloud(Ctx* c, float4* pts, const float* times, uint32_t n, const CloudW
     timed_launch_begin(c);
     if (w.mode == UndistortionMode::OPTIMIZED) k_warp_cloud<FromMotion><<<grid, 256, 0, c->stream>>>(pts, times, n, w.motion, x);
     else k_warp_cloud<FromPose><<<grid, 256, 0, c->stream>>>(pts, times, n, w.par, x);
-    timed_launch_end(c, 7);                                               // counts the launch
+    timed_launch_end(c, 7, 1);
     SO_CUDA_TRY(cudaGetLastError());
     return SO_OK;
 }
