@@ -151,13 +151,15 @@ static int ctx_alloc(Ctx* c) {
     if (rc) return rc;
     SO_CUDA_TRY(cudaMemset(c->d_counters, 0, c->max_batch * sizeof(uint32_t)));
     SO_CUDA_TRY(cudaMemset(c->d_hist, 0, c->max_batch * kHistStride * sizeof(int32_t)));
-    rc = c->d_corr_nd.reserve(c->scan_cap);
-    if (!rc) rc = c->d_corr_w.reserve(c->scan_cap);
+    const size_t slots = corr_tile_cap(c->scan_cap, c->max_batch) * kCorrTile;
+    rc = c->d_corr_x.reserve(slots * 4);
+    if (!rc) rc = c->d_corr_w.reserve(slots);
+    if (!rc) rc = c->d_corr_p.reserve(slots * 3);
     if (!rc) rc = c->d_corr_flags.reserve(c->scan_cap);
     if (!rc) rc = c->d_corr_nn.reserve(size_t(c->cfg.max_scan_points) * 5);
     if (!rc) rc = c->d_corr_nn_d2.reserve(size_t(c->cfg.max_scan_points) * 5);
     if (rc) return rc;
-    c->corr.nd = c->d_corr_nd; c->corr.w = c->d_corr_w; c->corr.flags = c->d_corr_flags; c->corr.nn = c->d_corr_nn; c->corr.nn_d2 = c->d_corr_nn_d2;
+    c->corr.x = c->d_corr_x; c->corr.w = c->d_corr_w; c->corr.p = c->d_corr_p; c->corr.flags = c->d_corr_flags; c->corr.nn = c->d_corr_nn; c->corr.nn_d2 = c->d_corr_nn_d2;
     return SO_OK;
 }
 
@@ -388,7 +390,7 @@ static int run_schedule(Ctx* c, const Chunk& ch, int iters, int lm, Undistortion
     if (nn.qcount) nn.qcount += size_t(ch.first) * SO_MAX_ICP_ITERS;
     const BatchView bv = chunk_view(c, c->d_scan_sorted, ch);
     CorrBuf cb = c->corr;
-    cb.nn = nullptr; cb.nn_d2 = nullptr;
+    cb.nn = nullptr; cb.nn_d2 = nullptr; cb.first = ch.first;
     const uint32_t grid_x = ch.grid_x, n_scans = ch.count, grid_e = ch.grid_e;
     const MapView me = map_view(c, c->edge);
     EdgeBuf eb = c->ebuf;
@@ -1710,9 +1712,9 @@ static int correspond_stage(Ctx* c, const void* surf, size_t n, size_t stride, s
         correspond();
         SO_CUDA_TRY(cudaGetLastError());
     }
-    std::vector<double4> nd(n); std::vector<double> w(n); std::vector<uchar4> fl(n); std::vector<uint32_t> nn(n * 5); std::vector<float> d2(n * 5);
+    std::vector<double> x(n * 3), w(n); std::vector<uchar4> fl(n); std::vector<uint32_t> nn(n * 5); std::vector<float> d2(n * 5);
     std::vector<float4> sorted(n);
-    SO_CUDA_TRY(cudaMemcpyAsync(nd.data(), c->corr.nd, n * sizeof(double4), cudaMemcpyDeviceToHost, c->stream));
+    SO_CUDA_TRY(cudaMemcpyAsync(x.data(), c->corr.x, n * 3 * sizeof(double), cudaMemcpyDeviceToHost, c->stream));     // scan 0 at offset 0: slot j
     SO_CUDA_TRY(cudaMemcpyAsync(w.data(), c->corr.w, n * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
     SO_CUDA_TRY(cudaMemcpyAsync(fl.data(), c->corr.flags, n * sizeof(uchar4), cudaMemcpyDeviceToHost, c->stream));
     SO_CUDA_TRY(cudaMemcpyAsync(nn.data(), c->corr.nn, n * 5 * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
@@ -1725,7 +1727,14 @@ static int correspond_stage(Ctx* c, const void* surf, size_t n, size_t stride, s
         std::memcpy(&orig, &sorted[j].w, 4);
         so_corr& r = corr[orig];
         std::memset(&r, 0, sizeof(r));
-        r.n[0] = nd[j].x; r.n[1] = nd[j].y; r.n[2] = nd[j].z; r.d = nd[j].w; r.w = w[j];
+        // plane_of_solution's steps as IEEE operations (every one correctly rounded, so the same bits); rejected points report 0
+        if (fl[j].x == SO_MATCH_SUCCESS) {
+            const double* xj = &x[j * 3];
+            const double nn = std::sqrt(std::fma(xj[2], xj[2], std::fma(xj[0], xj[0], xj[1] * xj[1])));
+            r.d = 1.0 / nn;
+            for (int k = 0; k < 3; ++k) r.n[k] = xj[k] / nn;
+        }
+        r.w = w[j];
         for (int k = 0; k < 5; ++k) { r.nn[k] = nn[j * 5 + k]; r.nn_d2[k] = d2[j * 5 + k]; }
         r.status = fl[j].x; r.obs[0] = fl[j].y; r.obs[1] = fl[j].z; r.obs[2] = fl[j].w;
     }
@@ -1893,21 +1902,25 @@ static int solve_stage(Ctx* c, const so_solve_row* rows, const float* times, siz
     c->prefiltered_n = SIZE_MAX;                                  // d_scan_sorted is overwritten
     if (ms) c->reg.valid = false;                                 // so are d_scan and the times
     std::vector<float4> raw(ms ? total : 0), sp(total);
-    std::vector<double4> nd(total);
-    std::vector<double> w(total);
+    // the record in its ND form ({n, d} per slot): slots of scan b from corr_first(b, offset) on; the gaps between scans are not read
+    const size_t slots = corr_first(uint32_t(n_problems), uint32_t(total));
+    std::vector<double> nd(slots * 4), w(slots);
+    std::vector<float> pr(slots * 3);
     std::vector<int32_t> hist(n_problems * kHistStride, 0);
     uint32_t off = 0;
     for (size_t b = 0; b < n_problems; ++b) {
         const uint32_t n = uint32_t(c->h_state[b].n_points);
         c->h_offset[b] = off;
+        const size_t r0 = corr_first(uint32_t(b), off);
         for (uint32_t i = 0; i < n; ++i) {
             const so_solve_row& r = rows[off + i];
             float4 p = make_float4(r.p[0], r.p[1], r.p[2], 0.f);
             if (ms) raw[off + i] = p;
             std::memcpy(&p.w, &i, 4);                             // the point's index inside its scan, as k_scan_gather writes it
             sp[off + i] = p;
-            nd[off + i] = make_double4(r.n[0], r.n[1], r.n[2], r.d);
-            w[off + i] = r.w;
+            for (int k = 0; k < 3; ++k) { nd[(r0 + i) * 4 + k] = r.n[k]; pr[(r0 + i) * 3 + k] = r.p[k]; }
+            nd[(r0 + i) * 4 + 3] = r.d;
+            w[r0 + i] = r.w;
         }
         hist[b * kHistStride + 9] = int32_t(n);                   // hist_rej[SUCCESS]: every row is accepted
         off += n;
@@ -1918,8 +1931,9 @@ static int solve_stage(Ctx* c, const so_solve_row* rows, const float* times, siz
     SO_CUDA_TRY(cudaMemcpyAsync(c->d_hist, hist.data(), hist.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
     if (total) {
         SO_CUDA_TRY(cudaMemcpyAsync(c->d_scan_sorted, sp.data(), total * sizeof(float4), cudaMemcpyHostToDevice, st));
-        SO_CUDA_TRY(cudaMemcpyAsync(c->corr.nd, nd.data(), total * sizeof(double4), cudaMemcpyHostToDevice, st));
-        SO_CUDA_TRY(cudaMemcpyAsync(c->corr.w, w.data(), total * sizeof(double), cudaMemcpyHostToDevice, st));
+        SO_CUDA_TRY(cudaMemcpyAsync(c->corr.x, nd.data(), slots * 4 * sizeof(double), cudaMemcpyHostToDevice, st));
+        SO_CUDA_TRY(cudaMemcpyAsync(c->corr.w, w.data(), slots * sizeof(double), cudaMemcpyHostToDevice, st));
+        SO_CUDA_TRY(cudaMemcpyAsync(c->corr.p, pr.data(), slots * 3 * sizeof(float), cudaMemcpyHostToDevice, st));
         SO_CUDA_TRY(cudaMemsetAsync(c->corr.flags, 0, total * sizeof(uchar4), st));
         if (ms) {
             SO_CUDA_TRY(cudaMemcpyAsync(c->d_scan, raw.data(), total * sizeof(float4), cudaMemcpyHostToDevice, st));
@@ -1933,7 +1947,7 @@ static int solve_stage(Ctx* c, const so_solve_row* rows, const float* times, siz
     const BatchView bv = chunk_view(c, c->d_scan_sorted, ch);
     const UndistortionMode mode = ms ? UndistortionMode::OPTIMIZED : UndistortionMode::NONE;
     CorrBuf cb = c->corr;
-    cb.nn = nullptr; cb.nn_d2 = nullptr;
+    cb.nn = nullptr; cb.nn_d2 = nullptr; cb.given = true;
     DegenState* const ddg = dg ? c->deg.d_st.get() : nullptr;
     auto solve = [&](int phase) { return launch_solve(c, mode, phase, bv, cb, 0, ch.grid_x, ch.count, st, nullptr, nullptr, 0, ddg); };
     timed_launch_begin(c);

@@ -278,9 +278,10 @@ struct Ctx {
     DeviceBuffer<double> d_partials;
     DeviceBuffer<uint32_t> d_counters;
     DeviceBuffer<int32_t> d_hist;
-    CorrBuf corr{};                                // views of the five buffers below
-    DeviceBuffer<double4> d_corr_nd;
-    DeviceBuffer<double> d_corr_w;
+    CorrBuf corr{};                                // views of the six buffers below
+    DeviceBuffer<double> d_corr_x;                 // record slots (so_corr_tiles.h) x 4: the QR solution or, for given rows, {n, d}
+    DeviceBuffer<double> d_corr_w;                 // record slots
+    DeviceBuffer<float> d_corr_p;                  // record slots x 3
     DeviceBuffer<uchar4> d_corr_flags;
     DeviceBuffer<uint32_t> d_corr_nn;
     DeviceBuffer<float> d_corr_nn_d2;

@@ -936,13 +936,14 @@ __device__ __forceinline__ double ld_shared_again(const double* p) {
 // pass widens each coordinate once and parks it in shared memory (nbd[(3 j + k) * kFitThreads], this thread's column), and the
 // later passes load it from there instead of re-reading and widening afresh (float -> double conversions run at a quarter of
 // the FP64 rate).
-__device__ __forceinline__ void fit_point(const MapView& m, const CorrBuf& cb, const NnBuf& nb, size_t gi, const float4 sp, const double* s_pose,
+__device__ __forceinline__ void fit_point(const MapView& m, const CorrBuf& cb, const NnBuf& nb, size_t gi, size_t ri, const float4 sp, const double* s_pose,
                                           int status, double* nbd, int* s_hist) {
     auto nbr_d = [&](int j, double& x, double& y, double& z) {
         x = ld_shared_again(nbd + (3 * j + 0) * kFitThreads); y = ld_shared_again(nbd + (3 * j + 1) * kFitThreads); z = ld_shared_again(nbd + (3 * j + 2) * kFitThreads);
     };
+    cb.p[ri * 3 + 0] = sp.x; cb.p[ri * 3 + 1] = sp.y; cb.p[ri * 3 + 2] = sp.z;
     int o0 = 0, o1 = 0, o2 = 0;
-    double nrm[3] = {0, 0, 0}, dpl = 0.0, wq = 0.0;
+    double xq[3] = {0, 0, 0}, wq = 0.0;
     if (status == SO_MATCH_SUCCESS) {
                     // ComputePointInitAndFinalPose (:382-400): pInit = double(p), pFinal = T_w_lidar * pInit
         const double pin[3] = {double(sp.x), double(sp.y), double(sp.z)};
@@ -1015,12 +1016,9 @@ __device__ __forceinline__ void fit_point(const MapView& m, const CorrBuf& cb, c
             }
             if (!(isfinite(x[0]) && isfinite(x[1]) && isfinite(x[2]))) status = SO_MATCH_INVALID_NUMERICAL;
             else {
-                // negative_OA_dot_norm = 1 / norm.norm(); norm.normalize()  (:812-816): square root and divisions as written there,
-                // because the planeRes/2 gate below reads both.  dd is RN(1/nn), so x / nn may be taken as div_rcp(x, nn, dd).
-                const double nn = sqrt(x[0] * x[0] + x[1] * x[1] + x[2] * x[2]);
-                const double dd = 1.0 / nn;
-#pragma unroll
-                for (int k = 0; k < 3; ++k) x[k] = div_rcp_ok(x[k], nn) ? div_rcp(x[k], nn, dd) : x[k] / nn;
+                // negative_OA_dot_norm and the normalised normal (:812-816), as every reader of the record decodes them from x
+                double pn[3], dd;
+                plane_of_solution(x[0], x[1], x[2], pn, dd);
                 const double maxd = double(m.plane_res) / 2.0;
                 double msum = 0.0;
                 bool ok = true;
@@ -1028,7 +1026,7 @@ __device__ __forceinline__ void fit_point(const MapView& m, const CorrBuf& cb, c
                 for (int j = 0; j < 5; ++j) {
                     double cx, cy, cz;
                     nbr_d(j, cx, cy, cz);
-                    const double dist = fabs(x[0] * cx + x[1] * cy + x[2] * cz + dd);
+                    const double dist = fabs(pn[0] * cx + pn[1] * cy + pn[2] * cz + dd);
                     if (ok && dist > maxd) ok = false;
                     msum += dist;
                 }
@@ -1074,7 +1072,7 @@ __device__ __forceinline__ void fit_point(const MapView& m, const CorrBuf& cb, c
                     if (trq[1] > tb) { t0 = 1; tb = trq[1]; }
                     if (trq[2] > tb) t0 = 2;
                     o0 = r0; o1 = r1; o2 = 6 + t0;
-                    nrm[0] = x[0]; nrm[1] = x[1]; nrm[2] = x[2]; dpl = dd;
+                    xq[0] = x[0]; xq[1] = x[1]; xq[2] = x[2];
                     // fitQualityCoeff = 1 - sqrt(meanDist / (3*planeRes_)) (:568); the map's inv_bound_d2 is RN(1 / bound_d2)
                     const double bd2 = double(m.bound_d2);
                     wq = 1.0 - sqrt(div_rcp_ok(mean_dist, bd2) ? div_rcp(mean_dist, bd2, m.inv_bound_d2) : mean_dist / bd2);
@@ -1094,8 +1092,8 @@ __device__ __forceinline__ void fit_point(const MapView& m, const CorrBuf& cb, c
         if (status == SO_MATCH_SUCCESS) { atomicAdd(&s_hist[o0], 1); atomicAdd(&s_hist[o1], 1); atomicAdd(&s_hist[o2], 1); }
         atomicAdd(&s_hist[9 + status], 1);
     }
-    cb.nd[gi] = make_double4(nrm[0], nrm[1], nrm[2], dpl);
-    cb.w[gi] = wq;
+    cb.x[ri * 3 + 0] = xq[0]; cb.x[ri * 3 + 1] = xq[1]; cb.x[ri * 3 + 2] = xq[2];
+    cb.w[ri] = wq;
     cb.flags[gi] = make_uchar4((unsigned char)status, (unsigned char)o0, (unsigned char)o1, (unsigned char)o2);
 }
 
@@ -1114,7 +1112,8 @@ __global__ void __launch_bounds__(kFitThreads, kFitMinBlocks) k_fit(MapView m, B
     for (int rr = 0; rr < kFitPts; ++rr) {          // kFitPts points per thread
         const uint32_t i = (blockIdx.x * kFitPts + rr) * kFitThreads + threadIdx.x;
         const size_t gi = size_t(bv.offset[s]) + i;
-        if (i < n) fit_point(m, cb, nb, gi, __ldg(&bv.scan[gi]), s_pose, int(nb.pre[gi]), s_nbd + threadIdx.x, s_hist);
+        if (i < n) fit_point(m, cb, nb, gi, corr_first(cb.first + s, bv.offset[s]) + i, __ldg(&bv.scan[gi]), s_pose, int(nb.pre[gi]),
+                             s_nbd + threadIdx.x, s_hist);
     }
     __syncthreads();
     if (threadIdx.x < 16 && s_hist[threadIdx.x]) atomicAdd(&bv.hist[s * kHistStride + threadIdx.x], s_hist[threadIdx.x]);
@@ -1124,8 +1123,9 @@ __global__ void __launch_bounds__(kFitThreads, kFitMinBlocks) k_fit(MapView m, B
 // k_evaluate: robustified normal equations at the candidate pose over the stored correspondences.
 // kEvalPts points per thread (strided by the CTA width, so loads stay coalesced) before the one warp/CTA reduction.
 // ------------------------------------------------------------------------------------------------------------------
-template <int PHASE>
+template <int PHASE, bool ND>
 __device__ __forceinline__ void evaluate_body(const BatchView& bv, const CorrBuf& cb, int s) {
+    constexpr int X = kCorrX<ND>;
     IcpState* st = bv.st + s;
     __shared__ double s_pose[7];
     __shared__ double s_R[9];
@@ -1135,42 +1135,42 @@ __device__ __forceinline__ void evaluate_body(const BatchView& bv, const CorrBuf
     if (threadIdx.x == 0) qtoR(s_pose + 3, s_R);
     __syncthreads();
     const uint32_t n = uint32_t(st->n_points);
-    const size_t base = size_t(bv.offset[s]);
+    const size_t base = corr_first(cb.first + s, bv.offset[s]);
     double acc[kAcc];
 #pragma unroll
     for (int k = 0; k < kAcc; ++k) acc[k] = 0.0;
     // Software-pipelined: the three loads of point r+1 are issued (unconditionally, so they do not chain behind the weight)
-    // before the FP64 work of point r, which keeps two points' worth of the 56 B/pt stream in flight per thread.
+    // before the FP64 work of point r, which keeps two points' worth of the record stream in flight per thread.
     const int pts = eval_pts(n);
     if (blockIdx.x >= eval_ctas(n)) return;                // the grid covers the largest scan of the chunk
     const uint32_t i0 = blockIdx.x * uint32_t(pts) * kThreads + threadIdx.x;
-    double w_n = 0.0;
-    double4 nd_n = make_double4(0.0, 0.0, 0.0, 0.0);
-    float4 sp_n = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (i0 < n) {
-        w_n = cb.w[base + i0];
-        nd_n = cb.nd[base + i0];
-        sp_n = __ldg(&bv.scan[base + i0]);
-    }
+    double w_n = 0.0, x_n[X] = {};
+    float p_n[3] = {0.f, 0.f, 0.f};
+    auto load = [&](uint32_t i) {
+        w_n = cb.w[base + i];
+#pragma unroll
+        for (int k = 0; k < X; ++k) x_n[k] = cb.x[(base + i) * X + k];
+#pragma unroll
+        for (int k = 0; k < 3; ++k) p_n[k] = cb.p[(base + i) * 3 + k];
+    };
+    if (i0 < n) load(i0);
 #pragma unroll 1
     for (int r = 0; r < pts; ++r) {
         const double w = w_n;
-        const double4 nd = nd_n;
-        const float4 sp = sp_n;
+        double xr[X];
+#pragma unroll
+        for (int k = 0; k < X; ++k) xr[k] = x_n[k];
+        const double pin[3] = {double(p_n[0]), double(p_n[1]), double(p_n[2])};
         const uint32_t inext = i0 + (r + 1) * kThreads;
         w_n = 0.0;
-        if (r + 1 < pts && inext < n) {
-            w_n = cb.w[base + inext];
-            nd_n = cb.nd[base + inext];
-            sp_n = __ldg(&bv.scan[base + inext]);
-        }
+        if (r + 1 < pts && inext < n) load(inext);
         if (w != 0.0) {
-            const double pin[3] = {double(sp.x), double(sp.y), double(sp.z)};
             double pw[3];
             qrot(s_pose + 3, pin, pw);
             pw[0] += s_pose[0]; pw[1] += s_pose[1]; pw[2] += s_pose[2];
-            const double nn[3] = {nd.x, nd.y, nd.z};
-            accumulate(acc, nn, nd.w, w, pin, pw, s_R, bv.tukey_a2);
+            double nn[3], d;
+            corr_plane<ND>(xr, nn, d);
+            accumulate(acc, nn, d, w, pin, pw, s_R, bv.tukey_a2);
         }
     }
     reduce_to_partials(acc, bv, s);
@@ -1203,24 +1203,26 @@ __device__ __forceinline__ void bulk_copy_g2s(void* dst_smem, const void* src_gl
                  : "memory");
 }
 
-// The same evaluation with the 56 B/point stream staged by the TMA engine.  A CTA's points are eval_pts(n) consecutive tiles of
-// kThreads points, and a tile is three contiguous spans (normals+offset 32 B/pt, scan point 16 B/pt, weight 8 B/pt): one elected
-// thread enqueues three cp.async.bulk copies per tile into a kEvalStages-deep shared-memory ring, each stage completing on its
-// own mbarrier; every thread then takes its own point from the stage (thread -> point mapping, arithmetic and reduction are
-// those of evaluate_body: results are bit-identical).  kEvalStages tiles (42 KB) are in flight per CTA whatever the threads are
-// doing, instead of the one software-prefetched point per thread that 124 registers x 2 CTAs per SM leave room for.
-// Falls back to generic loads for the ragged last tile of a scan and for scans whose first point is at an odd offset (the 8 B
-// weights of a tile must start 16 B-aligned for the bulk copy).
+// The same evaluation with the record staged by the TMA engine.  A CTA's points are eval_pts(n) consecutive tiles of kThreads points,
+// and a tile is three spans of the record (the QR solution 24 B/pt or {n, d} 32 B/pt, weight 8 B/pt, scan point 12 B/pt): one
+// elected thread enqueues three cp.async.bulk copies per tile into a kEvalStages-deep shared-memory ring, each stage completing on its
+// own mbarrier; every thread then takes its own point from the stage (thread -> point mapping, arithmetic and reduction are those of
+// evaluate_body: results are bit-identical).  kEvalStages tiles (33 KB) are in flight per CTA whatever the threads are doing, instead
+// of the one software-prefetched point per thread that 2 CTAs per SM leave room for.  Every scan's record starts on a tile of its own
+// (so_corr_tiles.h), so every span is 16 B-aligned and a scan's ragged last tile is copied whole: the slots past its last point are
+// the scan's own and are not read.
 constexpr int kEvalStages = 3;
-struct __align__(128) EvalStage { double4 nd[kThreads]; float4 sp[kThreads]; double w[kThreads]; };
-constexpr uint32_t kEvalStageBytes = uint32_t(sizeof(double4) + sizeof(float4) + sizeof(double)) * kThreads;
+template <bool ND>
+struct __align__(128) EvalStage { double x[kCorrX<ND> * kThreads]; double w[kThreads]; float p[3 * kThreads]; };
 
-template <int PHASE>
+template <int PHASE, bool ND>
 __device__ __forceinline__ void evaluate_body_tma(const BatchView& bv, const CorrBuf& cb, int s) {
+    constexpr int X = kCorrX<ND>;
+    constexpr uint32_t kStageBytes = uint32_t(X * sizeof(double) + sizeof(double) + 3 * sizeof(float)) * kThreads;
     IcpState* st = bv.st + s;
     __shared__ double s_pose[7];
     __shared__ double s_R[9];
-    __shared__ EvalStage s_stage[kEvalStages];
+    __shared__ EvalStage<ND> s_stage[kEvalStages];
     __shared__ unsigned long long s_bar[kEvalStages];
     const uint32_t n = uint32_t(st->n_points);
     const int pts = eval_pts(n);
@@ -1231,21 +1233,21 @@ __device__ __forceinline__ void evaluate_body_tma(const BatchView& bv, const Cor
         for (int k = 0; k < kEvalStages; ++k) mbar_init(&s_bar[k], 1);
     }
     __syncthreads();
-    const size_t base = size_t(bv.offset[s]);
+    const size_t base = corr_first(cb.first + s, bv.offset[s]);
     const uint32_t cta0 = blockIdx.x * uint32_t(pts) * kThreads;
-    // tiles [0, full) of this CTA are complete (kThreads points each); tile `full` may be ragged, later ones are empty
-    const int full = (base & 1) ? 0 : int(min(uint32_t(pts), (n - min(n, cta0)) / kThreads));
+    // tiles [0, tiles) of this CTA hold points (the last one may be ragged), later ones are empty
+    const int tiles = int(min(uint32_t(pts), (n - min(n, cta0) + kThreads - 1) / kThreads));
     auto issue = [&](int r) {                              // thread 0 only
-        EvalStage& sg = s_stage[r % kEvalStages];
+        EvalStage<ND>& sg = s_stage[r % kEvalStages];
         unsigned long long* bar = &s_bar[r % kEvalStages];
         const size_t g = base + cta0 + size_t(r) * kThreads;
-        mbar_arrive_expect_tx(bar, kEvalStageBytes);
-        bulk_copy_g2s(sg.nd, cb.nd + g, uint32_t(sizeof(double4)) * kThreads, bar);
-        bulk_copy_g2s(sg.sp, bv.scan + g, uint32_t(sizeof(float4)) * kThreads, bar);
+        mbar_arrive_expect_tx(bar, kStageBytes);
+        bulk_copy_g2s(sg.x, cb.x + g * X, uint32_t(X * sizeof(double)) * kThreads, bar);
         bulk_copy_g2s(sg.w, cb.w + g, uint32_t(sizeof(double)) * kThreads, bar);
+        bulk_copy_g2s(sg.p, cb.p + g * 3, uint32_t(3 * sizeof(float)) * kThreads, bar);
     };
     if (threadIdx.x == 0) {
-        for (int r = 0; r < kEvalStages && r < full; ++r) issue(r);
+        for (int r = 0; r < kEvalStages && r < tiles; ++r) issue(r);
         qtoR(s_pose + 3, s_R);
     }
     __syncthreads();
@@ -1253,49 +1255,39 @@ __device__ __forceinline__ void evaluate_body_tma(const BatchView& bv, const Cor
 #pragma unroll
     for (int k = 0; k < kAcc; ++k) acc[k] = 0.0;
 #pragma unroll 1
-    for (int r = 0; r < pts; ++r) {
+    for (int r = 0; r < tiles; ++r) {
         const uint32_t i = cta0 + uint32_t(r) * kThreads + threadIdx.x;
-        double w = 0.0;
-        double4 nd = make_double4(0.0, 0.0, 0.0, 0.0);
-        float4 sp = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (r < full) {                                    // CTA-uniform
-            const EvalStage& sg = s_stage[r % kEvalStages];
-            mbar_wait(&s_bar[r % kEvalStages], uint32_t(r / kEvalStages) & 1u);
-            w = sg.w[threadIdx.x];
-            nd = sg.nd[threadIdx.x];
-            sp = sg.sp[threadIdx.x];
-            __syncthreads();                               // every thread holds its point: the stage may be refilled
-            if (threadIdx.x == 0 && r + kEvalStages < full) {
-                // the stage was just read through the generic proxy and is rewritten through the async (TMA) proxy:
-                // the two are ordered only by a proxy fence
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                issue(r + kEvalStages);
-            }
-        } else {
-            if (cta0 + uint32_t(r) * kThreads >= n) break;
-            if (i < n) {
-                w = cb.w[base + i];
-                nd = cb.nd[base + i];
-                sp = __ldg(&bv.scan[base + i]);
-            }
+        const EvalStage<ND>& sg = s_stage[r % kEvalStages];
+        mbar_wait(&s_bar[r % kEvalStages], uint32_t(r / kEvalStages) & 1u);
+        const double w = i < n ? sg.w[threadIdx.x] : 0.0;
+        double xr[X];
+#pragma unroll
+        for (int k = 0; k < X; ++k) xr[k] = sg.x[threadIdx.x * X + k];
+        const double pin[3] = {double(sg.p[threadIdx.x * 3 + 0]), double(sg.p[threadIdx.x * 3 + 1]), double(sg.p[threadIdx.x * 3 + 2])};
+        __syncthreads();                                   // every thread holds its point: the stage may be refilled
+        if (threadIdx.x == 0 && r + kEvalStages < tiles) {
+            // the stage was just read through the generic proxy and is rewritten through the async (TMA) proxy:
+            // the two are ordered only by a proxy fence
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            issue(r + kEvalStages);
         }
         if (w != 0.0) {
-            const double pin[3] = {double(sp.x), double(sp.y), double(sp.z)};
             double pw[3];
             qrot(s_pose + 3, pin, pw);
             pw[0] += s_pose[0]; pw[1] += s_pose[1]; pw[2] += s_pose[2];
-            const double nn[3] = {nd.x, nd.y, nd.z};
-            accumulate(acc, nn, nd.w, w, pin, pw, s_R, bv.tukey_a2);
+            double nn[3], d;
+            corr_plane<ND>(xr, nn, d);
+            accumulate(acc, nn, d, w, pin, pw, s_R, bv.tukey_a2);
         }
     }
     reduce_to_partials(acc, bv, s);
 }
 
-template <int PHASE>
+template <int PHASE, bool ND>
 __global__ void __launch_bounds__(kThreads, 2) k_evaluate(BatchView bv, CorrBuf cb) {
     const int s = blockIdx.y;
     if (bv.st[s].phase != PHASE) return;
-    evaluate_body_tma<PHASE>(bv, cb, s);
+    evaluate_body_tma<PHASE, ND>(bv, cb, s);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -1604,11 +1596,11 @@ uint32_t launch_covariance(IcpState* st, cudaStream_t stream) { k_covariance<<<1
 // order as the two-kernel form, one launch less per cost evaluation: used when a registration is launch-latency bound (one or
 // two scans in flight, no edge cloud), where the ~190 registers of the serial step cost no occupancy that matters.
 // ------------------------------------------------------------------------------------------------------------------
-template <int PHASE>
+template <int PHASE, bool ND>
 __global__ void __launch_bounds__(kThreads, 1) k_evaluate_lm(BatchView bv, CorrBuf cb, uint32_t* __restrict__ counters) {
     const int s = blockIdx.y;
     if (bv.st[s].phase != PHASE) return;
-    evaluate_body<PHASE>(bv, cb, s);
+    evaluate_body<PHASE, ND>(bv, cb, s);
     __shared__ uint32_t s_ticket;
     __threadfence();
     __syncthreads();
@@ -1738,8 +1730,11 @@ uint32_t launch_inject(const MapView& m, const float4* by_id, uint32_t n_map, co
 uint32_t launch_first_eval(const BatchView& bv, const CorrBuf& cb, uint32_t grid_x, uint32_t n_scans, cudaStream_t st, const MapView* medge, const EdgeBuf* eb,
                            uint32_t grid_e, DegenState* dg) {
     const uint32_t gp = grid_x ? eval_grid(grid_x * kThreads) : 0;
-    if (bv.counters && gp && !grid_e && !dg) { k_evaluate_lm<PH_CORR><<<dim3(gp, n_scans), kThreads, 0, st>>>(bv, cb, bv.counters); return 1; }
-    if (gp) k_evaluate<PH_CORR><<<dim3(gp, n_scans), kThreads, 0, st>>>(bv, cb);
+    if (bv.counters && gp && !grid_e && !dg) {
+        (cb.given ? k_evaluate_lm<PH_CORR, true> : k_evaluate_lm<PH_CORR, false>)<<<dim3(gp, n_scans), kThreads, 0, st>>>(bv, cb, bv.counters);
+        return 1;
+    }
+    if (gp) (cb.given ? k_evaluate<PH_CORR, true> : k_evaluate<PH_CORR, false>)<<<dim3(gp, n_scans), kThreads, 0, st>>>(bv, cb);
     if (grid_e) k_edge_fit<<<dim3(grid_e, n_scans), kThreads, 0, st>>>(*medge, bv, *eb, bv.edge_partial_offset);
     if (dg) k_lm_step_deg<PH_CORR><<<n_scans, 128, 0, st>>>(bv, gp, bv.edge_partial_offset, dg);
     else k_lm_step<PH_CORR><<<n_scans, 128, 0, st>>>(bv, gp, bv.edge_partial_offset);
@@ -1753,8 +1748,11 @@ uint32_t launch_edge_fit(const MapView& medge, const BatchView& bv, const EdgeBu
 uint32_t launch_evaluate(const BatchView& bv, const CorrBuf& cb, uint32_t grid_x, uint32_t n_scans, cudaStream_t st, const EdgeBuf* eb, uint32_t grid_e,
                          DegenState* dg) {
     const uint32_t gx = grid_x ? eval_grid(grid_x * kThreads) : 0;
-    if (bv.counters && gx && !grid_e && !dg) { k_evaluate_lm<PH_EVAL><<<dim3(gx, n_scans), kThreads, 0, st>>>(bv, cb, bv.counters); return 1; }
-    if (gx) k_evaluate<PH_EVAL><<<dim3(gx, n_scans), kThreads, 0, st>>>(bv, cb);
+    if (bv.counters && gx && !grid_e && !dg) {
+        (cb.given ? k_evaluate_lm<PH_EVAL, true> : k_evaluate_lm<PH_EVAL, false>)<<<dim3(gx, n_scans), kThreads, 0, st>>>(bv, cb, bv.counters);
+        return 1;
+    }
+    if (gx) (cb.given ? k_evaluate<PH_EVAL, true> : k_evaluate<PH_EVAL, false>)<<<dim3(gx, n_scans), kThreads, 0, st>>>(bv, cb);
     if (grid_e) k_edge_evaluate<<<dim3(grid_e, n_scans), kThreads, 0, st>>>(bv, *eb, bv.edge_partial_offset);
     if (dg) k_lm_step_deg<PH_EVAL><<<n_scans, 128, 0, st>>>(bv, gx, bv.edge_partial_offset, dg);
     else k_lm_step<PH_EVAL><<<n_scans, 128, 0, st>>>(bv, gx, bv.edge_partial_offset);

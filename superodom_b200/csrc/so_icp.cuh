@@ -1,16 +1,48 @@
 // so_icp.cuh -- kernel-side views and host launchers shared by so_icp.cu / so_api.cu.
 #pragma once
+#include "so_corr_tiles.h"
 #include "so_internal.cuh"
 
 namespace so {
 
+// The solve's correspondence record: what every evaluation pass reads per point.  Its three arrays are indexed by record slot
+// (corr_first(first + s, offset[s]) + i for point i of scan s of the chunk, so_corr_tiles.h); flags, nn and nn_d2 by the point's
+// position in the scan buffer.  A fitted plane is kept as the QR solution x it comes from (24 B, plane_of_solution gives n and d),
+// not as {n, d} (32 B): the evaluation streams 44 B per point instead of 56.  Given rows (so_solve*) have no QR solution, so their
+// record holds {n.x, n.y, n.z, d} (the ND form of the evaluation kernels); x holds 4 doubles per slot so that both forms fit.
 struct CorrBuf {
-    double4* nd;        // {n.x,n.y,n.z,d}; all zero for rejected points
-    double* w;          // residualCoefficient (0 for rejected)
+    double* x;          // [3 per slot] QR solution x (ND form: [4 per slot] {n, d}); 0 for rejected points
+    double* w;          // [slot] residualCoefficient (0 for rejected)
+    float* p;           // [3 per slot] the scan point, as the scan buffer holds it
     uchar4* flags;      // {status, obs0, obs1, obs2}
     uint32_t* nn;       // optional [5 per point] neighbour ids (stage tests); may be null
     float* nn_d2;       // optional [5 per point]
+    uint32_t first = 0; // the chunk's first scan inside the batch
+    bool given = false; // the record holds {n, d} (so_solve*): the launchers take the ND form of the evaluation kernels
 };
+
+// The plane of a fit from its unnormalised QR solution x (A x = -1 over the neighbours): negative_OA_dot_norm = 1 / norm.norm();
+// norm.normalize() (LidarSlam.cpp:812-816).  k_fit gates on what this returns and every reader of the record decodes x with it, so
+// the rounding of each step is spelt out: |x|^2 as the compiler contracted the expression x0 x0 + x1 x1 + x2 x2 where the fit used
+// to compute it (x1 x1 rounded, then two FMAs), IEEE square root and reciprocal, and x / |x| as the division (div_rcp from the
+// reciprocal, which gives the same bits, where it is valid).
+__device__ __forceinline__ void plane_of_solution(double x0, double x1, double x2, double n[3], double& d) {
+    const double nn = __dsqrt_rn(__fma_rn(x2, x2, __fma_rn(x0, x0, __dmul_rn(x1, x1))));
+    d = __drcp_rn(nn);
+    n[0] = div_rcp_ok(x0, nn) ? div_rcp(x0, nn, d) : __ddiv_rn(x0, nn);
+    n[1] = div_rcp_ok(x1, nn) ? div_rcp(x1, nn, d) : __ddiv_rn(x1, nn);
+    n[2] = div_rcp_ok(x2, nn) ? div_rcp(x2, nn, d) : __ddiv_rn(x2, nn);
+}
+
+// Slots per record entry of the two forms: the QR solution, or {n, d} (given rows)
+template <bool ND> constexpr int kCorrX = ND ? 4 : 3;
+
+// n and d of the record entry at rec (kCorrX<ND> doubles)
+template <bool ND>
+__device__ __forceinline__ void corr_plane(const double* rec, double n[3], double& d) {
+    if (ND) { n[0] = rec[0]; n[1] = rec[1]; n[2] = rec[2]; d = rec[3]; }
+    else plane_of_solution(rec[0], rec[1], rec[2], n, d);
+}
 
 constexpr int kHistStride = 24;
 

@@ -160,7 +160,7 @@ constexpr int kRowStride = 14;
 // Tiles of kThreads points (the per-CTA layout of k_evaluate: eval_pts(n) tiles per CTA, eval_ctas(n) CTAs per scan): every thread
 // stages its row in shared memory, then thread e < 91 adds component e of the tile's 256 rows in index order.  One register
 // accumulator per thread instead of 91.
-template <int PHASE>
+template <int PHASE, bool ND>
 __global__ void __launch_bounds__(kThreads) k_motion_eval(BatchView bv, CorrBuf cb, const float4* __restrict__ raw, const float* __restrict__ times,
                                                           const MotionState* __restrict__ ms, double* __restrict__ partials, uint32_t stride) {
     const int s = blockIdx.y;
@@ -178,7 +178,7 @@ __global__ void __launch_bounds__(kThreads) k_motion_eval(BatchView bv, CorrBuf 
     else if (e < 90) { ei = e - 78; ej = 12; }
     else { ei = 13; ej = -1; }
     double acc = 0.0;
-    const size_t base = size_t(bv.offset[s]);
+    const size_t base = size_t(bv.offset[s]), rb = corr_first(cb.first + s, bv.offset[s]);
     __syncthreads();
 #pragma unroll 1
     for (int r = 0; r < pts; ++r) {
@@ -187,10 +187,10 @@ __global__ void __launch_bounds__(kThreads) k_motion_eval(BatchView bv, CorrBuf 
 #pragma unroll
         for (int k = 0; k < 14; ++k) row[k] = 0.0;
         if (i < n) {
-            const double wc = cb.w[base + i];
+            const double wc = cb.w[rb + i];
             if (wc != 0.0) {
-                const double4 nd4 = cb.nd[base + i];
-                const double nd[4] = {nd4.x, nd4.y, nd4.z, nd4.w};
+                double nd[4];
+                corr_plane<ND>(cb.x + (rb + i) * kCorrX<ND>, nd, nd[3]);
                 const size_t src = base + __float_as_uint(bv.scan[base + i].w);
                 motion_row(m, nd, wc, __ldg(&raw[src]), __ldg(&times[src]), bv.tukey_a2, row);
             }
@@ -496,14 +496,14 @@ uint32_t launch_motion_solve(int phase, const BatchView& bv, const CorrBuf& cb, 
     double* ep = me ? me->partials : nullptr;
     uint32_t n = 1 + (gx ? 1 : 0) + (ge ? 1 : 0);                         // k_motion_step, k_motion_eval, k_motion_eval_edge
     if (phase == PH_CORR) {
-        if (gx) k_motion_eval<PH_CORR><<<dim3(gx, n_scans), kThreads, 0, st>>>(bv, cb, raw, times, ms, partials, stride);
+        if (gx) (cb.given ? k_motion_eval<PH_CORR, true> : k_motion_eval<PH_CORR, false>)<<<dim3(gx, n_scans), kThreads, 0, st>>>(bv, cb, raw, times, ms, partials, stride);
         if (ge) {
             n += launch_edge_fit(me->map, bv, me->eb, ge, n_scans, st);
             k_motion_eval_edge<PH_CORR><<<dim3(ge, n_scans), kThreads, 0, st>>>(bv, me->eb, me->raw, me->times, ms, ep, first);
         }
         k_motion_step<PH_CORR><<<n_scans, 128, 0, st>>>(bv, ms, partials, stride, ep, eoff, first);
     } else {
-        if (gx) k_motion_eval<PH_EVAL><<<dim3(gx, n_scans), kThreads, 0, st>>>(bv, cb, raw, times, ms, partials, stride);
+        if (gx) (cb.given ? k_motion_eval<PH_EVAL, true> : k_motion_eval<PH_EVAL, false>)<<<dim3(gx, n_scans), kThreads, 0, st>>>(bv, cb, raw, times, ms, partials, stride);
         if (ge) k_motion_eval_edge<PH_EVAL><<<dim3(ge, n_scans), kThreads, 0, st>>>(bv, me->eb, me->raw, me->times, ms, ep, first);
         k_motion_step<PH_EVAL><<<n_scans, 128, 0, st>>>(bv, ms, partials, stride, ep, eoff, first);
     }
